@@ -41,7 +41,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class NvmlClockSampler:
@@ -93,7 +93,7 @@ def make_clock_sampler(gpu_index: int):
 
 
 class ClockSampler:
-    """Fallback: nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """Fallback: nvidia-smi clocks + throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -125,6 +125,30 @@ class ClockSampler:
         reasons = sorted({names[i] for r in self.rows if len(r) >= 9 for i in range(4) if r[5 + i].lower().startswith("active")})
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": reasons, "samples": len(sm)}
+
+
+def read_device(ptr: int, nbytes: int) -> np.ndarray:
+    """Copy `nbytes` of device memory at `ptr` (current device) to a host uint8 array."""
+    import ctypes as C
+
+    got = np.empty(nbytes, np.uint8)
+    cu = C.CDLL("libcuda.so.1")
+    cu.cuMemcpyDtoH_v2.argtypes = [C.c_void_p, C.c_uint64, C.c_size_t]
+    assert cu.cuMemcpyDtoH_v2(got.ctypes.data_as(C.c_void_p), C.c_uint64(ptr), got.size) == 0
+    return got
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """--dump-outputs: each array as <out_dir>/<name>.npy (float32 / float64), 64 MB at most in all."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT_BYTES, f"dump of {total} bytes exceeds {DUMP_LIMIT_BYTES}"
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def make_cloud(n: int):
@@ -197,7 +221,7 @@ def run_reference(args):
     if rank != 0:
         return 0
     world = int(os.environ.get("WORLD_SIZE", "1"))
-    value, ms, cores, desc, n_s, _ = cpu_reference_run(max(args.steps, 5) if args.steps < 50 else 5, min(args.warmup, 2), budget_s=150.0)
+    value, ms, cores, desc, n_s, _ = cpu_reference_run(args.steps, min(args.warmup, 2), budget_s=150.0)
     line = {
         "impl": "reference", "metric": METRIC, "value": round(value, 3), "unit": "Msplats/s", "n_gpus": args.gpus,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": round(ms, 3), "higher_is_better": True,
@@ -326,7 +350,7 @@ def run_cuda(args):
         if world > 1:
             sessions[k].gather_device(p.frame_device_ptr, all_frames[k].data_ptr() if all_frames[k] is not None else 0, frame_bytes)
 
-    # ---- device-resident throughput ("value"): inputs (768 MB cloud >> 126 MB L2) already in HBM
+    # ---- device-resident throughput ("value"): inputs (768 MB cloud >> 50 MB L2) already in HBM
     for p in plugins:
         p.render_view(handle, settings, view, fmt="rgba8_srgb", to_host=False)   # sizes every buffer
     # set-up, not warm-up: every context queues frames (and gathers) once so that lazily created state -- the second
@@ -355,6 +379,20 @@ def run_cuda(args):
     barrier()
     ms_total = max(e0.elapsed_time(ev) for ev in e1)     # device time from the first frame's start to the last frame's / gather's end
     clk = clocks.stop() if rank == 0 else None
+    # ---- what the timed path delivered in its last step (outside the timed region): the RGBA8 frame of the last step's
+    #      context, and on rank 0 of a multi-GPU run a fixed, seeded sample of the gathered frame stack
+    dumps = {}
+    if args.dump_outputs and rank == 0:
+        k_last = (args.steps - 1) % frames_in_flight
+        frame = read_device(plugins[k_last].frame_device_ptr, frame_bytes).reshape(HEIGHT, WIDTH, 4)
+        dumps["frame_rgba8"] = frame.astype(np.float32)
+        fs_last = plugins[k_last].frame_stats()
+        dumps["frame_stats"] = np.array([fs_last.n, fs_last.n_visible, fs_last.n_pairs, fs_last.rounds], np.float64)
+        if world > 1:
+            stack = all_frames[k_last].cpu().numpy().reshape(world * HEIGHT * WIDTH, 4)
+            pick = np.sort(np.random.default_rng(0).choice(len(stack), size=min(len(stack), 1 << 20), replace=False))
+            dumps["gathered_pixel_index"] = pick.astype(np.float64)
+            dumps["gathered_rgba8_sample"] = stack[pick].astype(np.float32)
     # ---- multi-GPU correctness on hardware: rank 0 re-renders every rank's view locally and compares it with the
     #      gathered frames, byte for byte (outside the timed region)
     gather_ok = None
@@ -375,15 +413,6 @@ def run_cuda(args):
     gather_ce = gather_direct = None
     peer_ready = False
     if world > 1:
-        import ctypes as C
-
-        def read_root(ptr, nbytes):
-            got = np.empty(nbytes, np.uint8)
-            cu = C.CDLL("libcuda.so.1")
-            cu.cuMemcpyDtoH_v2.argtypes = [C.c_void_p, C.c_uint64, C.c_size_t]
-            assert cu.cuMemcpyDtoH_v2(got.ctypes.data_as(C.c_void_p), C.c_uint64(ptr), got.size) == 0
-            return got
-
         def agree(ok: bool) -> bool:
             t_ = torch.tensor([1 if ok else 0], device="cuda", dtype=torch.int32)
             dist.all_reduce(t_, op=dist.ReduceOp.MIN)
@@ -433,7 +462,7 @@ def run_cuda(args):
             sig_ok = use_signal[0]
             if rank == 0 and sig_ok:
                 for k in range(frames_in_flight):
-                    words = read_root(sessions[k].peer_flags_ptr(), 4 * world).view(np.uint32)
+                    words = read_device(sessions[k].peer_flags_ptr(), 4 * world).view(np.uint32)
                     sig_ok = sig_ok and bool(np.all(words == np.uint32(sessions[k]._peer_seq & 0xFFFFFFFF)))
             use_signal[0] = agree(sig_ok)
             barrier()
@@ -457,7 +486,7 @@ def run_cuda(args):
             got = None
             if rank == 0 and use_signal[0]:
                 # read BEFORE any host barrier: the device-side wait alone has established that all frames are there
-                got = read_root(sessions[k_last]._peer_ptr.value, world * frame_bytes)
+                got = read_device(sessions[k_last]._peer_ptr.value, world * frame_bytes)
             barrier()
             leg_ms = max(c0.elapsed_time(ev) for ev in c1) / args.steps
             t_ = torch.tensor([leg_ms], device="cuda")
@@ -466,7 +495,7 @@ def run_cuda(args):
             leg_ok = None
             if rank == 0:
                 if got is None:
-                    got = read_root(sessions[k_last]._peer_ptr.value, world * frame_bytes)
+                    got = read_device(sessions[k_last]._peer_ptr.value, world * frame_bytes)
                 got = got.reshape(world, HEIGHT, WIDTH, 4)
                 leg_ok = True
                 for r in range(world):
@@ -588,26 +617,9 @@ def run_cuda(args):
                  "alg_bytes": int(front_bytes), "gbs": round(front_bytes / (front_us * 1e-6) / 1e9, 1),
                  "frac": round(front_bytes / (front_us * 1e-6) / 1e9 / peak, 4), "target": 0.70}
     dom = max(stages, key=lambda s: s["us"])
-    traffic_path = os.path.join(ROOT, "profiles", "traffic.json")
-    traffic = None
-    if os.path.exists(traffic_path):
-        traffic = json.load(open(traffic_path)).get(dom["stage"])
     roofline = {"kernel": dom["stage"], "bound": "hbm", "achieved": dom["gbs"], "peak": peak, "unit": "GB/s",
-                "frac": dom["frac"], "traffic": traffic, "traffic_source": "static: ncu dram__bytes of the committed capture under profiles/ (not measured in this run)",
-                "peak_source": peak_src,
-                "note": "dominant kernel by time; raster is bound by instruction issue, not by HBM -- see roofline.issue and stages[]"}
-    # the dominant kernel's OWN roofline: warp-instructions it executes per launch (ncu, profiles/traffic.json) against
-    # the SMs' issue rate (4 warp-instructions per SM cycle) at the SM clock sampled during the timed region
-    if traffic_path and os.path.exists(traffic_path):
-        wi = json.load(open(traffic_path)).get("warp_inst", {}).get(dom["stage"])
-        if wi:
-            sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
-            mhz = float((clk or {}).get("sm_mhz") or 1965.0)
-            peak_gi = sms * 4 * mhz * 1e6 / 1e9
-            ach_gi = wi / (dom["us"] * 1e-6) / 1e9
-            roofline["issue"] = {"warp_inst_per_launch": int(wi), "achieved": round(ach_gi, 1), "peak": round(peak_gi, 1),
-                                 "unit": "G warp-inst/s", "frac": round(ach_gi / peak_gi, 4),
-                                 "source": "ncu smsp__inst_executed.sum of the committed capture (profiles/), live CUDA-event time"}
+                "frac": dom["frac"], "peak_source": peak_src,
+                "note": "dominant kernel by time, algorithmic bytes; raster is bound by instruction issue, not by HBM -- see stages[]"}
 
     # ---- CPU baseline beside it + parity of the benchmarked frame (rank 0, N=1 only; outside the timed regions)
     cpu, parity = None, None
@@ -644,7 +656,7 @@ def run_cuda(args):
         "impl": "cuda", "metric": METRIC, "value": round(value, 1), "unit": "Msplats/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": round(ms_step, 4), "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32 (f16-packed inputs)", "data": "synthetic",
-        "config": bench_config(views, world, {"n_visible": nv, "n_pairs": I, "l2": "inputs larger than L2 (768 MB cloud vs 126 MB)",
+        "config": bench_config(views, world, {"n_visible": nv, "n_pairs": I, "l2": "inputs larger than L2 (768 MB cloud vs 50 MB)",
                                               "frames_in_flight": frames_in_flight, "rank0_numa_node": numa_node,
                                               "gather": None if world == 1 else
                                               f"{gather_name}: the fastest verified transport of this run (gather_nccl / gather_ce / gather_direct hold all three)",
@@ -663,6 +675,8 @@ def run_cuda(args):
         "raw_scale_1": raw, "clocks": clk,
     }
     print(json.dumps(line), flush=True)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dumps)
     for se in sessions:
         se.destroy()
     if dist is not None:
@@ -677,6 +691,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="cuda", choices=["cuda", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy (float32/float64)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":

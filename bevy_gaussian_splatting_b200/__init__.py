@@ -1,6 +1,6 @@
-"""bevy_gaussian_splatting_b200 -- B200-native forward splat path behind the reference's plugin surface.
+"""bevy_gaussian_splatting_b200 -- H100-native (sm_90a) forward splat path behind the reference's plugin surface.
 
-Product = `csrc/` (hand-written sm_100a kernels + the C ABI of include/bgs.h, built to libbgs.so).
+Product = `csrc/` (hand-written sm_90a kernels + the C ABI of include/bgs.h, built to libbgs.so).
 The Python modules here are the host-side mirror of the reference interface for this path
 (same names as mosure/bevy_gaussian_splatting: src/lib.rs:7-29 re-exports) used by tests and bench.
 """

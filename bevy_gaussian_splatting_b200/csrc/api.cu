@@ -1,7 +1,7 @@
 // api.cu -- the extern "C" boundary of libbgs (include/bgs.h): contexts, clouds, the per-view
 // frame (stage orchestration on one CUDA stream), parity/debug hooks, stage timing.
 //
-// No PyTorch, no wgpu, no CPU fallback: every stage is a hand-written sm_100a kernel.
+// No PyTorch, no wgpu, no CPU fallback: every stage is a hand-written sm_90a kernel.
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -77,14 +77,12 @@ struct bgs_cloud {
 
 struct bgs_context {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     int coop = 0;                 // device supports cooperative launch
     uint32_t kg_grid = 0, bin_grid = 0;   // co-resident grid sizes of the cooperative kernels (synchronous frames: latency)
     uint32_t kg_grid_async = 0, bin_grid_async = 0;   // ... of queued (BGS_FLAG_ASYNC) frames: 1 CTA per SM.  A latency-bound
                                           // cooperative grid holds its registers while it waits; with several frames in flight
                                           // a smaller grid leaves that room to the other frames' issue-bound blend
-                                          // (measured at C3, 3 contexts, 4 / 2 / 1 CTAs per SM: 0.346 / 0.319 / 0.311 ms per
-                                          // frame before, 0.283 -> 0.268 after the other changes, profiles/r2_experiments.md)
     int rs_per_sm = 0;                    // co-resident radix-sort CTAs per SM (radix.cu)
     int rs_per_sm_async = 1;              // ... the pair sort of queued frames may use (1: half an SM, two waves)
     uint32_t sort_epoch = 0;              // look-back status epoch: +1 per sort launch (status words never need clearing)
@@ -102,8 +100,7 @@ struct bgs_context {
                                       // frames an ESTIMATE of what one round would have emitted
     // chunked frames (saturation-aware binning): the visible set is binned / sorted / blended in front-to-back
     // rank rounds [frac[r], frac[r+1]) / 65536; once every tile has saturated the remaining rounds emit nothing
-    // (x8 schedule: the front of a heavy scene saturates the frame within a few hundred splats; measured on C2/C3
-    // at global_scale 1, profiles/r1_rounds.md)
+    // (x8 schedule: the front of a heavy scene saturates the frame within a few hundred splats)
     uint32_t chunk_frac[MAX_CHUNKS + 1] = {0, 16, 128, 1024, 8192, 65536, 65536, 65536, 65536};
     int chunk_count = 5;
     uint32_t chunk_pairs_hint[MAX_CHUNKS] = {};   // last chunked frame's pairs per round (pair sort tile size)
@@ -388,7 +385,7 @@ bgs_status bgs_context_create(int cuda_device, bgs_context** out) {
         c->chunk_count = k + 1;
     }
     if (e == cudaSuccess && !c->coop) {
-        snprintf(c->err, sizeof(c->err), "device %d cannot co-schedule the cooperative kernels (sm_100a B200 expected)", cuda_device);
+        snprintf(c->err, sizeof(c->err), "device %d cannot co-schedule the cooperative kernels (an sm_90a GPU such as the H100 is required)", cuda_device);
         fprintf(stderr, "libbgs: %s\n", c->err);
         e = cudaErrorNotSupported;
     }
@@ -736,7 +733,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     }
 
     // saturation-aware chunking: frames whose splats cover many tiles each (last frame: >= 32 pairs per visible splat
-    // and >= 2^24 pairs; measured crossover on B200: ~15-30 M pairs, profiles/r1_rounds.md) run binning / tile sort /
+    // and >= 2^24 pairs: below that, one round is cheaper than the extra launches) run binning / tile sort /
     // blend in front-to-back rank rounds; the rounds after every tile has saturated emit nothing.
     // Quad-uv records + cooperative binning only; BGS_FLAG_CHUNKS / _NO_CHUNKS force it.
     bool chunked = raster_mode == 0 && !want_aux && c->coop && num_tiles <= CHUNK_MAX_TILES && !(st->flags & BGS_FLAG_NO_CHUNKS) && c->chunk_count > 1;

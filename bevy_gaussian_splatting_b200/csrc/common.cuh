@@ -1,4 +1,4 @@
-// common.cuh -- shared device-side types and helpers of libbgs (sm_100a).
+// common.cuh -- shared device-side types and helpers of libbgs (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -2,7 +2,7 @@
 // exportable as an OS handle (POSIX file descriptor), which Vulkan -- and therefore wgpu-hal / Bevy's render device --
 // imports with VK_KHR_external_memory_fd as the memory of the view-target image / a buffer it copies from.
 //
-// Replaces, on the B200 path, the role of the render pass attachment the reference draws into
+// Replaces, on the CUDA path, the role of the render pass attachment the reference draws into
 // (src/render/mod.rs:1501-1569 binds pipelines that write the view target); here bgs_render writes it through a
 // CUDA device pointer.  Synchronisation: bgs_render (synchronous) or bgs_sync() returns after the frame is complete;
 // a timeline semaphore exported by Vulkan can be imported into CUDA by the host later (cudaImportExternalSemaphore) --

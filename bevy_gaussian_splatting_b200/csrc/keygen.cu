@@ -118,8 +118,7 @@ keygen_compact_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc
 //           (L2 / 32 B sectors, visible ones only), computes the key and writes (key, index, slot) at run + e --
 //           fully coalesced, in index order, so the stable LSD sort sees the reference's tie order.
 //           The depth sort's digit histograms are accumulated on the way (shared-memory atomics, visible keys only:
-//           at ~2 cycles per lane-atomic they are most of this phase's ~12 us -- measured with and without the
-//           position re-read, with thread-per-element and thread-per-word expansions, profiles/r2_experiments.md).
+//           at ~2 cycles per lane-atomic they are most of this phase's time, more than the position re-read).
 constexpr int KG_WORDS_PER_TILE = KG_TILE / 32;    // 64 mask words
 constexpr int KG_CHUNK_WORDS = 1024;               // phase 2 expands 1024 words (32 K gaussians) at a time
 

@@ -688,8 +688,8 @@ void launch_project(bool f16, bool blocked, const float4* pos, const void* sh, c
     static int use_ring = -1;
     if (use_ring < 0) { const char* e = getenv("BGS_PROJECT_RING"); use_ring = (e && atoi(e) > 0) ? 1 : 0; }
     if (blocked && use_ring && aux == nullptr) {
-        // (measured slower on B200 -- one UBLKCP per 128 B row sustains ~1 copy / 20 cycles / SM: 48 us vs 36 us for
-        // the per-thread gather at C3 -- kept behind BGS_PROJECT_RING=1 as the evidence, profiles/r2_experiments.md)
+        // (opt-in with BGS_PROJECT_RING=1: one bulk copy per 128 B row issues slowly enough that the per-thread gather
+        // below has been the faster default)
         // TMA ring over the gaussian-major blocks (`sh` carries the block array): a persistent grid of at most
         // ctas_per_sm CTAs per SM (2 when a depth sort shares the SMs, else the occupancy limit)
         static bool attr_set[64] = {};
@@ -714,7 +714,7 @@ void launch_project(bool f16, bool blocked, const float4* pos, const void* sh, c
     // head-room); the grid-stride loop keeps any n_vis correct.
     uint32_t blocks = (n_hint + 127) / 128;
     if (blocks > 65535u * 8u) blocks = 65535u * 8u;
-    if (blocks < 148u) blocks = 148u;
+    if (blocks < (uint32_t)sm_count) blocks = (uint32_t)sm_count;
     {   // tuning knob: cap the grid at BGS_PROJECT_CTAS CTAs per SM (grid-stride loop; smaller footprint beside other frames)
         static int cap = -1;
         if (cap < 0) { const char* e = getenv("BGS_PROJECT_CTAS"); cap = e ? atoi(e) : 0; }

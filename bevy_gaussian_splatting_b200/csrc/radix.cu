@@ -24,8 +24,8 @@
 
 namespace bgs {
 
-constexpr int RS_THREADS = 512;                   // fat CTAs, one (two for > 1.2 M entries) per SM: a single-wave sort has
-constexpr int RS_WARPS = RS_THREADS / 32;         // <= 148 (296) tiles, so the look-back walks (traffic ~ tiles^2 x 2 KB)
+constexpr int RS_THREADS = 512;                   // fat CTAs, one (two beyond 8 K entries x SMs) per SM: a single-wave sort has
+constexpr int RS_WARPS = RS_THREADS / 32;         // <= one (two) tiles per SM, so the look-back walks (traffic ~ tiles^2 x 2 KB)
                                                   // stay short; 512 x 64 registers leave half an SM to a concurrent kernel
 constexpr int RS_TABLE_WORDS = RS_WARPS * 256;    // one peer-mask table (all warps)
 #ifndef RS_MIN_CTAS
@@ -171,7 +171,7 @@ radix_coop_kernel(SortParams P) {
                     // small (latency-bound) sorts: peers via a per-warp mask table in shared memory (the tables alias
                     // s_vals / s_keys, unused until the scatter; even / odd items alternate tables so the clear of one
                     // item never races the next item's ORs): one ATOMS.OR per lane, conflicts only among lanes sharing
-                    // the digit.  Measured on B200 (C3): -8 us on the depth sort vs MATCH.ANY.
+                    // the digit.  Cheaper than MATCH.ANY when the sort is latency-bound.
                     uint32_t* mm = ((j & 1) ? s_keys : s_vals) + warp * 256;
                     atomicOr(&mm[d], 1u << lane);
                     __syncwarp();
@@ -180,7 +180,7 @@ radix_coop_kernel(SortParams P) {
                     __syncwarp();
                     if (lane == 31 - __clz(peers)) { mm[d] = 0u; s_whist[warp][d] = old + __popc(peers); }
                 } else {
-                    // large (throughput-bound) sorts: MATCH.ANY (the mask table loses there: 232 vs 190 us at 6 M entries)
+                    // large (throughput-bound) sorts: MATCH.ANY (the mask table's atomics cost more there than they save)
                     peers = __match_any_sync(0xffffffffu, d);
                     old = s_whist[warp][d];
                     __syncwarp();
@@ -256,7 +256,7 @@ radix_coop_kernel(SortParams P) {
             // 16-tile windows of predecessors; the windows of a round are combined in distance order through shared
             // memory.  In a single-wave sort every tile publishes its aggregate at about the same time and nobody but
             // tile 0 holds an inclusive prefix yet, so a tile walks all the way back: two windows per round halve that
-            // latency (a round ~0.45 us: C3 depth sort, tile 117 of 118: 5.0 -> ~2.5 us per pass).
+            // latency.
             if (tile != 0) {
                 uint32_t* s_part = s_binstart + 512;            // [2][256] window sums (after s_binstart, s_gbase)
                 uint32_t* s_fnd = s_part + 512;                 // [2][256] window ended at an inclusive prefix

@@ -621,8 +621,8 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
         else raster_kernel<2, true><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal);
         return;
     }
-    // measured on B200: the 2-pixels-per-thread variant wins when splats cover many tiles (C2 raw, scale 1:
-    // 131 -> 117 us) and loses when most splats are a few pixels (C3, scale 0.02: 178 -> 217 us)
+    // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
+    // pixels (more of its lanes then idle at the tile's splat boundaries)
     if (mode == 0 && large_footprints)
         raster2_kernel<false><<<grid, R2_THREADS, 0, stream>>>(recs, tile_entries, ranges, W, H, tiles_x, out, format,
                                                                nullptr, nullptr, nullptr, 1, 1);

@@ -2,7 +2,7 @@
 (src/io/codec.rs:4-18, src/io/gcloud/flexbuffers.rs:9-22) = the serde serialisation of `PlanarGaussian3d` into a
 FlexBuffer, uncompressed (src/io/loader.rs: `Some("gcloud") => PlanarGaussian3d::decode(bytes)`).
 
-The encoding itself lives in two crates that are NOT in /root/reference (`flexbuffers` 25.2 and the `Planar` derive
+The encoding itself lives in two crates that are NOT in the reference repository (`flexbuffers` 25.2 and the `Planar` derive
 of `bevy_interleave`), so this module restates the published FlexBuffers wire format (google/flatbuffers
 `flexbuffers.h`: values are read from the END of the buffer; offsets point backwards; vectors carry a length prefix and,
 when untyped, one packed-type byte per element; maps are a vector of values plus a sorted key vector) and serde's data

@@ -1,5 +1,5 @@
 /*
- * bgs.h -- C ABI of the B200-native forward splat path (libbgs.so).
+ * bgs.h -- C ABI of the H100-native (sm_90a) forward splat path (libbgs.so).
  *
  * Drop-in boundary for mosure/bevy_gaussian_splatting's per-view, per-frame GPU work.
  * One Rust render-world system calls bgs_render() in place of BOTH reference call sites:

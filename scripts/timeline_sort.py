@@ -13,7 +13,7 @@ lib = pl._lib; lib.bgs_debug_timeline_.argtypes = [C.c_void_p, C.c_void_p, C.POI
 lib.bgs_debug_timeline_(pl._ctx, buf.ctypes.data_as(C.c_void_p), C.byref(g))
 nt = int((buf[:, 0] != 0).sum())
 print("tiles stamped:", nt)
-t = buf[:nt, :6].astype(np.int64); t = (t - t[:, :1]) / 1965.0   # clock64 cycles -> us at 1.965 GHz, per-tile origin
+t = buf[:nt, :6].astype(np.int64); t = (t - t[:, :1]) / 1980.0   # clock64 cycles -> us at 1.98 GHz (H100 SXM max SM clock), per-tile origin
 names = ["tile start", "ranked", "scanned", "smem scatter", "post-lookback", "written"]
 for i, nm in enumerate(names):
     col = t[:, i]; print(f"{nm:14s} min {col.min():7.2f} median {np.median(col):7.2f} max {col.max():7.2f} us")

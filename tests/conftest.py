@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
 
 
 def _cuda_device_present() -> bool:
@@ -28,7 +28,7 @@ def pytest_collection_modifyitems(config, items):
     (the product itself still fails loudly: bgs_context_create returns BGS_ECUDA, there is no CPU path)."""
     if _cuda_device_present():
         return
-    skip = pytest.mark.skip(reason="no CUDA device on this box (run with -m gpu on the B200 box)")
+    skip = pytest.mark.skip(reason="no CUDA device on this machine (run with -m gpu on an H100)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

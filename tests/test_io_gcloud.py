@@ -195,8 +195,7 @@ def test_cpp_gcloud_reader_and_writer_interoperate_with_python(tmp_path):
 def test_damaged_files_are_errors_in_both_hosts(tmp_path):
     """Truncated, bit-flipped and tail-corrupted `.ply` / `.gcloud` files: the Python loaders raise ValueError, the C++ loader
     exits with its error code -- never a crash, a hang or an allocation sized by a corrupted count (the loaders of the
-    reference return io::Error, src/io/loader.rs:38-66).  A longer run of the same mutations under ASan / UBSan is logged
-    in profiles/r2_fuzz.txt."""
+    reference return io::Error, src/io/loader.rs:38-66)."""
     import io as pyio
     import os
     import subprocess

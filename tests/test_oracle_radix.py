@@ -1,6 +1,6 @@
 """Oracle pinned against the reference's own pure tests for the sort key / pass plan.
 
-Each test restates one test of /root/reference/tests/radix.rs (file:line in the docstring) against
+Each test restates one test of the reference's tests/radix.rs (file:line in the docstring) against
 the ORACLE's key formula and pass plan, plus the ABI-side mirror `ShaderDefines`.
 """
 import numpy as np
