@@ -4,7 +4,6 @@
 // No PyTorch, no wgpu, no CPU fallback: every stage is a hand-written sm_90a kernel.
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <algorithm>
 #include <mutex>
@@ -15,13 +14,12 @@
 
 namespace bgs {
 // keygen.cu
-void launch_keygen(const float4* pos, uint32_t n, const FrameConsts& fc, int sort_all, uint32_t* keys_out,
-                   uint32_t* ids_out, uint32_t* slots_out, uint32_t* status, FrameCounters* ctr, cudaStream_t stream);
-uint32_t keygen_num_tiles(uint32_t n);
+void launch_keygen_all(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* keys_out, uint32_t* ids_out,
+                       FrameCounters* ctr, cudaStream_t stream);
 int keygen_coop_blocks_per_sm();
 cudaError_t launch_keygen_coop(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* masks, uint32_t* keys_out,
                                uint32_t* ids_out, uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr,
-                               uint32_t* hist, int hist_passes, uint32_t grid, unsigned long long* tl, cudaStream_t stream);
+                               uint32_t* hist, int hist_passes, uint32_t grid, cudaStream_t stream);
 void launch_culled_flags(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* flags, cudaStream_t stream);
 // radix.cu
 uint32_t radix_num_tiles(uint32_t capacity);
@@ -29,28 +27,23 @@ int radix_coop_blocks_per_sm(int items);
 cudaError_t launch_radix_sort(uint32_t* keys0, uint32_t* vals0, uint32_t* keys1, uint32_t* vals1, const uint32_t* n_ptr,
                               uint32_t capacity, uint32_t n_hint, uint32_t* hist, int compute_hist, void* status,
                               size_t status_stride, uint32_t epoch, uint32_t* barrier, int passes, int shift0, uint2* ranges,
-                              int sm_count, int coop_per_sm, cudaStream_t stream, unsigned long long* tl);
+                              int sm_count, int coop_per_sm, cudaStream_t stream);
 // project.cu
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
                         FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream);
 void launch_repack(bool f16, const void* pos, const void* sh, const void* rot, const void* so, uint32_t n, void* blocks,
                    cudaStream_t stream);
-void launch_project(bool f16, bool blocked, const float4* pos, const void* sh, const void* rot, const void* so,
-                    const uint32_t* index_list, int by_slot, const FrameCounters* ctr, const FrameConsts& fc,
-                    SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, int ctas_per_sm, const float* cutoff_tab,
-                    float4* aux, cudaStream_t stream);
+void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+                    const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
+                    const float* cutoff_tab, float4* aux, cudaStream_t stream);
 void launch_cutoff_table(float* tab, cudaStream_t stream);
 // bin.cu
-void launch_bin_emit(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc, uint32_t* status, int tiles_x,
-                     uint32_t capacity, uint32_t* pair_keys, uint32_t* pair_vals, uint32_t n_upper, int sm_count,
-                     uint32_t* sticky_need, cudaStream_t stream);
-uint32_t bin_num_tiles(uint32_t n);
 int bin_coop_blocks_per_sm();
 cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
                                  uint32_t frac_a, uint32_t frac_b, uint32_t num_tiles_total, uint32_t* block_cnt,
                                  int tiles_x, uint32_t capacity, uint32_t* pair_keys, uint32_t* pair_vals,
-                                 uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, unsigned long long* timeline,
-                                 uint32_t grid, uint32_t* sticky_need, cudaStream_t stream);
+                                 uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, uint32_t grid,
+                                 uint32_t* sticky_need, cudaStream_t stream);
 // raster.cu
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
@@ -69,22 +62,17 @@ struct bgs_cloud {
     bool f16;
     bool cov;         // f16 layout whose second plane holds Covariance3dOpacityPacked128 records (precomputed Sigma3D)
     float4* pos;      // n * 16 B
-    void* sh;         // f32: n * 192 B; f16: n * 96 B
-    void* rot;        // f32: n * 16 B (w,x,y,z); f16: n * 16 B packed rotation+scale+opacity
-    void* so;         // f32: n * 16 B; f16: unused
-    void* blocks;     // gaussian-major copy (f16: n * 128 B, f32: n * 256 B); when set, sh/rot/so are freed
+    void* blocks;     // gaussian-major copy of every plane (f16: n * 128 B, f32: n * 256 B), what the projection gathers
 };
 
 struct bgs_context {
     int device = 0;
     int sm_count = 132;
-    int coop = 0;                 // device supports cooperative launch
     uint32_t kg_grid = 0, bin_grid = 0;   // co-resident grid sizes of the cooperative kernels (synchronous frames: latency)
     uint32_t kg_grid_async = 0, bin_grid_async = 0;   // ... of queued (BGS_FLAG_ASYNC) frames: 1 CTA per SM.  A latency-bound
                                           // cooperative grid holds its registers while it waits; with several frames in flight
                                           // a smaller grid leaves that room to the other frames' issue-bound blend
     int rs_per_sm = 0;                    // co-resident radix-sort CTAs per SM (radix.cu)
-    int rs_per_sm_async = 1;              // ... the pair sort of queued frames may use (1: half an SM, two waves)
     uint32_t sort_epoch = 0;              // look-back status epoch: +1 per sort launch (status words never need clearing)
     cudaStream_t stream = nullptr;    // render stream (high priority): everything but the projection
     cudaStream_t stream2 = nullptr;   // projection runs here, beside the depth sort
@@ -94,15 +82,9 @@ struct bgs_context {
     cudaEvent_t ev_front = nullptr, ev_rdone = nullptr;
     cudaEvent_t ev[6] = {};
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_p0 = nullptr, ev_p1 = nullptr;
-    unsigned long long* timeline = nullptr;   // BGS_TIMELINE=1: per-CTA phase stamps of bin_emit_coop (debug)
     uint32_t n_vis_hint = 0;          // last frame's visible count (sizes the projection grid)
     uint32_t n_pairs_hint = 0;        // last frame's pair count (picks the pair sort's tile size); on chunked
                                       // frames an ESTIMATE of what one round would have emitted
-    // chunked frames (saturation-aware binning): the visible set is binned / sorted / blended in front-to-back
-    // rank rounds [frac[r], frac[r+1]) / 65536; once every tile has saturated the remaining rounds emit nothing
-    // (x8 schedule: the front of a heavy scene saturates the frame within a few hundred splats)
-    uint32_t chunk_frac[MAX_CHUNKS + 1] = {0, 16, 128, 1024, 8192, 65536, 65536, 65536, 65536};
-    int chunk_count = 5;
     uint32_t chunk_pairs_hint[MAX_CHUNKS] = {};   // last chunked frame's pairs per round (pair sort tile size)
     bool chunk_hint_valid = false;
     float4* state = nullptr;          // per-pixel blend state between rounds (tile-major), tiles * 256 * 16 B
@@ -127,10 +109,10 @@ struct bgs_context {
     uint32_t cap_pairs = 0;
     uint32_t* pkeys[2] = {nullptr, nullptr};
     uint32_t* pvals[2] = {nullptr, nullptr};
-    // zeroed-per-frame arena: counters | hist | keygen status | bin status | ranges | done bytes
+    // zeroed-per-frame arena: counters | hist | keygen CTA counts | bin CTA counts | ranges | done bytes
     uint8_t* arena = nullptr;
     size_t arena_bytes = 0;
-    uint32_t arena_n = 0, arena_pairs = 0, arena_tiles = 0;
+    uint32_t arena_tiles = 0;
     // look-back status rows of the two sorts (64-bit epoch-tagged words, cleared once at allocation)
     void* status_depth = nullptr;      // [4][tiles(n)][256]
     void* status_pairs = nullptr;      // [4][tiles(cap_pairs)][256]
@@ -141,8 +123,8 @@ struct bgs_context {
     cudaEvent_t ev_done = nullptr;
     FrameCounters* ctr = nullptr;
     uint32_t* hist = nullptr;          // [8 + 4 * MAX_CHUNKS][256]: depth passes 0..3, pair passes 4..7 (round 0), 8 + 4r.. (round r)
-    uint32_t* status_keygen = nullptr;
-    uint32_t* status_bin = nullptr;
+    uint32_t* kg_block_cnt = nullptr;  // [kg_grid]: keygen_coop's per-CTA visible counts
+    uint32_t* bin_block_cnt = nullptr; // [bin_grid][3]: bin_emit_coop's per-CTA pair / medium / large counts
     uint2* ranges = nullptr;           // per tile (~start, end) into the sorted pair list (0, 0 = empty)
     // frame
     void* frame = nullptr;            // frames[0]
@@ -202,6 +184,14 @@ bgs_status fail(bgs_context* ctx, bgs_status st, const char* fmt, ...) {
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 constexpr uint32_t CHUNK_MAX_TILES = 65536;
+// chunked frames (saturation-aware binning): the visible set is binned / sorted / blended in front-to-back rank rounds
+// [CHUNK_FRAC[r], CHUNK_FRAC[r + 1]) / 65536; once every tile has saturated the remaining rounds emit nothing
+// (x8 schedule: the front of a heavy scene saturates the frame within a few hundred splats)
+constexpr uint32_t CHUNK_FRAC[MAX_CHUNKS + 1] = {0, 16, 128, 1024, 8192, 65536};
+// CTAs per SM of the cooperative key-gen and binning grids: synchronous frames (latency), queued (BGS_FLAG_ASYNC) frames
+constexpr int COOP_CTAS_PER_SM = 4, COOP_CTAS_PER_SM_ASYNC = 1;
+// radix-sort CTAs per SM the pair sort of queued frames may use (1: half an SM, two waves)
+constexpr int SORT_CTAS_PER_SM_ASYNC = 1;
 
 int pair_passes(uint32_t num_tiles) {
     int bits = 1;
@@ -245,17 +235,16 @@ bgs_status ensure_pair_scratch(bgs_context* c, uint32_t pairs) {
     return BGS_OK;
 }
 
-bgs_status ensure_arena(bgs_context* c, uint32_t n, uint32_t pairs, uint32_t tiles) {
-    if (c->arena && n <= c->arena_n && pairs <= c->arena_pairs && tiles <= c->arena_tiles) return BGS_OK;
-    n = n > c->arena_n ? n : c->arena_n;
-    pairs = pairs > c->arena_pairs ? pairs : c->arena_pairs;
+bgs_status ensure_arena(bgs_context* c, uint32_t tiles) {
+    if (c->arena && tiles <= c->arena_tiles) return BGS_OK;
     tiles = tiles > c->arena_tiles ? tiles : c->arena_tiles;
     cudaFree(c->arena); c->arena = nullptr;
     size_t off = 0;
     const size_t o_ctr = off; off = align_up(off + sizeof(FrameCounters), 256);
     const size_t o_hist = off; off = align_up(off + (8 + 4 * MAX_CHUNKS) * 256 * 4, 256);
-    const size_t o_skg = off; off = align_up(off + ((size_t)keygen_num_tiles(n) + 4096) * 4, 256);
-    const size_t o_sbin = off; off = align_up(off + ((size_t)bin_num_tiles(n) + 4096) * 4, 256);
+    // (the queued-frame grids are never larger than the synchronous ones)
+    const size_t o_kgc = off; off = align_up(off + (size_t)c->kg_grid * 4, 256);
+    const size_t o_binc = off; off = align_up(off + (size_t)c->bin_grid * 3 * 4, 256);
     // chunked frames (only for <= CHUNK_MAX_TILES tiles) use one ranges array per round + a done byte per tile; an
     // arena sized by a larger frame must still hold them for a later, smaller (chunkable) frame
     const size_t chunk_tiles = tiles <= CHUNK_MAX_TILES ? tiles : CHUNK_MAX_TILES;
@@ -266,11 +255,11 @@ bgs_status ensure_arena(bgs_context* c, uint32_t n, uint32_t pairs, uint32_t til
     c->arena_bytes = off;
     c->ctr = reinterpret_cast<FrameCounters*>(c->arena + o_ctr);
     c->hist = reinterpret_cast<uint32_t*>(c->arena + o_hist);
-    c->status_keygen = reinterpret_cast<uint32_t*>(c->arena + o_skg);
-    c->status_bin = reinterpret_cast<uint32_t*>(c->arena + o_sbin);
+    c->kg_block_cnt = reinterpret_cast<uint32_t*>(c->arena + o_kgc);
+    c->bin_block_cnt = reinterpret_cast<uint32_t*>(c->arena + o_binc);
     c->ranges = reinterpret_cast<uint2*>(c->arena + o_rng);
     c->tile_done = c->arena + o_done;
-    c->arena_n = n; c->arena_pairs = pairs; c->arena_tiles = tiles;
+    c->arena_tiles = tiles;
     return BGS_OK;
 }
 
@@ -354,37 +343,18 @@ bgs_status bgs_context_create(int cuda_device, bgs_context** out) {
     if (e == cudaSuccess) { launch_cutoff_table(c->cutoff_tab, c->stream); e = cudaStreamSynchronize(c->stream); }
     if (e == cudaSuccess) memset(c->h_sticky, 0, 16);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, cuda_device);
-    if (e == cudaSuccess && getenv("BGS_TIMELINE")) e = cudaMalloc(&c->timeline, 4096 * 8 * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&c->coop, cudaDevAttrCooperativeLaunch, cuda_device);
-    if (e == cudaSuccess && c->coop) {
+    int coop = 0;   // device supports cooperative launch
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, cuda_device);
+    if (e == cudaSuccess && coop) {
         const int kb = keygen_coop_blocks_per_sm(), bb = bin_coop_blocks_per_sm();
-        int lim = 4;   // CTAs per SM of the cooperative kernels (BGS_COOP_BLOCKS overrides; fewer leaves room for a
-        if (const char* e = getenv("BGS_COOP_BLOCKS")) lim = atoi(e) > 0 ? atoi(e) : 4;   // second context's kernels)
-        c->kg_grid = (uint32_t)(c->sm_count * (kb > lim ? lim : kb));
-        c->bin_grid = (uint32_t)(c->sm_count * (bb > lim ? lim : bb));
-        int lim_a = 1;
-        if (const char* e = getenv("BGS_COOP_BLOCKS_ASYNC")) lim_a = atoi(e) > 0 ? atoi(e) : 1;
-        if (lim_a > lim) lim_a = lim;
-        c->kg_grid_async = (uint32_t)(c->sm_count * (kb > lim_a ? lim_a : kb));
-        c->bin_grid_async = (uint32_t)(c->sm_count * (bb > lim_a ? lim_a : bb));
+        c->kg_grid = (uint32_t)(c->sm_count * std::min(kb, COOP_CTAS_PER_SM));
+        c->bin_grid = (uint32_t)(c->sm_count * std::min(bb, COOP_CTAS_PER_SM));
+        c->kg_grid_async = (uint32_t)(c->sm_count * std::min(kb, COOP_CTAS_PER_SM_ASYNC));
+        c->bin_grid_async = (uint32_t)(c->sm_count * std::min(bb, COOP_CTAS_PER_SM_ASYNC));
         c->rs_per_sm = radix_coop_blocks_per_sm(16);
-        if (const char* e = getenv("BGS_SORT_CTAS_ASYNC")) c->rs_per_sm_async = atoi(e) > 0 ? atoi(e) : 1;
-        if (c->rs_per_sm_async > c->rs_per_sm) c->rs_per_sm_async = c->rs_per_sm;
-        if (c->kg_grid == 0 || c->bin_grid == 0 || c->kg_grid > 4096 || c->bin_grid > 4096 || c->rs_per_sm == 0) c->coop = 0;
+        if (c->kg_grid == 0 || c->bin_grid == 0 || c->rs_per_sm == 0) coop = 0;
     }
-    if (const char* fr = getenv("BGS_CHUNK_FRACS")) {
-        // tuning knob: cumulative round boundaries out of 65536, e.g. "256,2048,16384" = 4 rounds
-        int k = 0;
-        uint32_t prev = 0;
-        while (*fr && k < MAX_CHUNKS - 1) {
-            const uint32_t v = (uint32_t)strtoul(fr, const_cast<char**>(&fr), 10);
-            if (v > prev && v < 65536u) { c->chunk_frac[++k] = v; prev = v; }
-            while (*fr == ',' || *fr == ' ') ++fr;
-        }
-        for (int j = k + 1; j <= MAX_CHUNKS; ++j) c->chunk_frac[j] = 65536u;
-        c->chunk_count = k + 1;
-    }
-    if (e == cudaSuccess && !c->coop) {
+    if (e == cudaSuccess && !coop) {
         snprintf(c->err, sizeof(c->err), "device %d cannot co-schedule the cooperative kernels (an sm_90a GPU such as the H100 is required)", cuda_device);
         fprintf(stderr, "libbgs: %s\n", c->err);
         e = cudaErrorNotSupported;
@@ -430,7 +400,6 @@ void bgs_context_destroy(bgs_context* c) {
     if (c->h_sticky) cudaFreeHost(c->h_sticky);
     cudaFree(c->d_sticky);
     cudaFree(c->cutoff_tab);
-    cudaFree(c->timeline);
     for (int i = 0; i < 6; ++i) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
     for (cudaEvent_t e : {c->ev_fork, c->ev_join, c->ev_p0, c->ev_p1, c->ev_done}) if (e) cudaEventDestroy(e);
     cudaFree(c->status_depth); cudaFree(c->status_pairs);
@@ -449,30 +418,25 @@ static bgs_status upload_common(bgs_context* ctx, uint32_t n, bool f16, const fl
     bgs_cloud* cl = new (std::nothrow) bgs_cloud();
     if (!cl) return BGS_ENOMEM;
     cl->ctx = ctx; cl->device = ctx->device; cl->n = n; cl->f16 = f16; cl->cov = false;
-    cl->pos = nullptr; cl->sh = nullptr; cl->rot = nullptr; cl->so = nullptr; cl->blocks = nullptr;
+    cl->pos = nullptr; cl->blocks = nullptr;
+    // the other planes go to device scratch, are repacked into the gaussian-major blocks the projection gathers, and
+    // are freed again
+    void* d_sh = nullptr; void* d_rot = nullptr; void* d_so = nullptr;
     const size_t sh_bytes = (size_t)n * (f16 ? 96 : 192);
     cudaError_t e = cudaMalloc(&cl->pos, (size_t)n * 16);
-    if (e == cudaSuccess) e = cudaMalloc(&cl->sh, sh_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&cl->rot, (size_t)n * 16);
-    if (e == cudaSuccess && !f16) e = cudaMalloc(&cl->so, (size_t)n * 16);
+    if (e == cudaSuccess) e = cudaMalloc(&d_sh, sh_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&d_rot, (size_t)n * 16);
+    if (e == cudaSuccess && !f16) e = cudaMalloc(&d_so, (size_t)n * 16);
     if (e == cudaSuccess) e = cudaMemcpyAsync(cl->pos, pos_vis, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(cl->sh, sh, sh_bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(cl->rot, rot, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess && !f16) e = cudaMemcpyAsync(cl->so, so, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
-    // gaussian-major blocks for the projection's gather (BGS_LAYOUT=planar keeps only the reference's planes)
-    const char* lay = getenv("BGS_LAYOUT");
-    if (e == cudaSuccess && !(lay && strcmp(lay, "planar") == 0)) {
-        e = cudaMalloc(&cl->blocks, (size_t)n * (f16 ? 128 : 256));
-        if (e == cudaSuccess) {
-            launch_repack(f16, cl->pos, cl->sh, cl->rot, cl->so, n, cl->blocks, ctx->stream);
-            e = cudaStreamSynchronize(ctx->stream);
-        }
-        if (e == cudaSuccess) {
-            cudaFree(cl->sh); cudaFree(cl->rot); cudaFree(cl->so);
-            cl->sh = cl->rot = cl->so = nullptr;
-        }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_sh, sh, sh_bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_rot, rot, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess && !f16) e = cudaMemcpyAsync(d_so, so, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMalloc(&cl->blocks, (size_t)n * (f16 ? 128 : 256));
+    if (e == cudaSuccess) {
+        launch_repack(f16, cl->pos, d_sh, d_rot, d_so, n, cl->blocks, ctx->stream);
+        e = cudaStreamSynchronize(ctx->stream);
     }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    cudaFree(d_sh); cudaFree(d_rot); cudaFree(d_so);
     if (e != cudaSuccess) {
         bgs_cloud_destroy(cl);
         return fail(ctx, e == cudaErrorMemoryAllocation ? BGS_ENOMEM : BGS_ECUDA, "cloud upload: %s", cudaGetErrorString(e));
@@ -523,7 +487,7 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
             c->clouds.erase(std::remove(c->clouds.begin(), c->clouds.end(), cl), c->clouds.end());
         }
     }
-    cudaFree(cl->pos); cudaFree(cl->sh); cudaFree(cl->rot); cudaFree(cl->so); cudaFree(cl->blocks);
+    cudaFree(cl->pos); cudaFree(cl->blocks);
     delete cl;
 }
 
@@ -561,7 +525,7 @@ static bgs_status finish_frame(bgs_context* c) {
         uint64_t got = 0;
         int full = 0;
         while (full < chunks && !c->h_ctr->chunk[full].skipped) got += c->h_ctr->chunk[full++].n_pairs_needed;
-        const uint64_t est = got * 65536ull / c->chunk_frac[full];
+        const uint64_t est = got * 65536ull / CHUNK_FRAC[full];
         c->n_pairs_hint = est > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)est;
         for (int r = 0; r < chunks; ++r) c->chunk_pairs_hint[r] = c->h_ctr->chunk[r].n_pairs;
         c->chunk_hint_valid = true;
@@ -735,12 +699,12 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     // saturation-aware chunking: frames whose splats cover many tiles each (last frame: >= 32 pairs per visible splat
     // and >= 2^24 pairs: below that, one round is cheaper than the extra launches) run binning / tile sort /
     // blend in front-to-back rank rounds; the rounds after every tile has saturated emit nothing.
-    // Quad-uv records + cooperative binning only; BGS_FLAG_CHUNKS / _NO_CHUNKS force it.
-    bool chunked = raster_mode == 0 && !want_aux && c->coop && num_tiles <= CHUNK_MAX_TILES && !(st->flags & BGS_FLAG_NO_CHUNKS) && c->chunk_count > 1;
+    // Quad-uv records only; BGS_FLAG_CHUNKS / _NO_CHUNKS force it.
+    bool chunked = raster_mode == 0 && !want_aux && num_tiles <= CHUNK_MAX_TILES && !(st->flags & BGS_FLAG_NO_CHUNKS);
     if (chunked && !(st->flags & BGS_FLAG_CHUNKS))
         chunked = c->n_vis_hint > 0 && c->n_pairs_hint >= (c->last_chunks > 1 ? 3u << 22 : 1u << 24) &&
                   (uint64_t)c->n_pairs_hint >= (c->last_chunks > 1 ? 24ull : 32ull) * c->n_vis_hint;   // (hysteresis)
-    const int rounds = chunked ? c->chunk_count : 1;
+    const int rounds = chunked ? MAX_CHUNKS : 1;
     if (chunked && c->cap_state_tiles < num_tiles) {
         cudaFree(c->state); c->state = nullptr; c->cap_state_tiles = 0;
         CU(c, cudaMalloc(&c->state, (size_t)num_tiles * 256 * sizeof(float4)));
@@ -748,29 +712,25 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     }
 
     for (int attempt = 0; attempt < 4; ++attempt) {
-        s = ensure_arena(c, n, c->cap_pairs, num_tiles);
+        s = ensure_arena(c, num_tiles);
         if (s != BGS_OK) return s;
         s = ensure_status(c, n, c->cap_pairs);
         if (s != BGS_OK) return s;
         cudaStream_t q = c->stream;
         uint32_t launches = 0;
-        CU(c, cudaMemsetAsync(c->arena, 0, c->arena_bytes, q));   // counters, histograms, ranges: ~0.6 MB
+        CU(c, cudaMemsetAsync(c->arena, 0, c->arena_bytes, q));   // counters, histograms, ranges: ~0.4 MB
         CU(c, cudaEventRecord(c->ev[0], q));
         // ---- stage 1: key-gen (+ stable compaction of the visible set)
         // compact mode: keys[0][slot], slot_ids[slot] = gaussian index, vals[0][slot] = slot (sort payload)
         // SORT_ALL    : keys[0][i], vals[0][i] = i (payload is the gaussian index itself)
         const bool by_slot = !sort_all;
-        bool hist_fused = false;   // the cooperative key-gen also produces the depth sort's digit histograms
-        if (!sort_all && c->coop) {
-            // cooperative: uncompacted keys go through keys[1] (scratch until the first sort pass overwrites it)
+        if (by_slot) {
+            // the cooperative key-gen also produces the depth sort's digit histograms
             // (keys[1] = visibility-mask scratch until the sort's first pass overwrites it)
-            CU(c, launch_keygen_coop(cloud->pos, n, fc, c->keys[1], c->keys[0], c->slot_ids, c->vals[0], c->status_keygen,
-                                     c->ctr, c->hist, depth_passes, (st->flags & BGS_FLAG_ASYNC) ? c->kg_grid_async : c->kg_grid,
-                                     (c->timeline && getenv("BGS_TIMELINE_KEYGEN")) ? c->timeline : nullptr, q));
-            hist_fused = true;
+            CU(c, launch_keygen_coop(cloud->pos, n, fc, c->keys[1], c->keys[0], c->slot_ids, c->vals[0], c->kg_block_cnt,
+                                     c->ctr, c->hist, depth_passes, (st->flags & BGS_FLAG_ASYNC) ? c->kg_grid_async : c->kg_grid, q));
         } else {
-            launch_keygen(cloud->pos, n, fc, sort_all ? 1 : 0, c->keys[0], sort_all ? c->vals[0] : c->slot_ids,
-                          sort_all ? c->slot_ids : c->vals[0], c->status_keygen, c->ctr, q);
+            launch_keygen_all(cloud->pos, n, fc, c->keys[0], c->vals[0], c->ctr, q);
         }
         ++launches;
         CU(c, cudaEventRecord(c->ev[1], q));
@@ -783,16 +743,15 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         // ---- stage 2: depth radix sort: all P = depth_bits / 8 digit places in ONE cooperative launch (enqueued before
         //      the projection so its one-CTA-per-SM grid becomes resident first; the projection fills the other half)
         CU(c, launch_radix_sort(c->keys[0], c->vals[0], c->keys[1], c->vals[1], &c->ctr->n_sort, n,
-                                sort_all ? n : (c->n_vis_hint ? c->n_vis_hint : n), c->hist, hist_fused ? 0 : 1, c->status_depth,
+                                sort_all ? n : (c->n_vis_hint ? c->n_vis_hint : n), c->hist, sort_all ? 1 : 0, c->status_depth,
                                 (size_t)radix_num_tiles(c->status_n) * 256, next_epoch(c), &c->ctr->barrier[1], depth_passes, 0,
-                                nullptr, c->sm_count, c->rs_per_sm, q,
-                                (c->timeline && getenv("BGS_TIMELINE_SORT")) ? c->timeline : nullptr));
+                                nullptr, c->sm_count, c->rs_per_sm, q));
         ++launches;
         if (overlap) {
             CU(c, cudaStreamWaitEvent(c->stream2, c->ev_fork, 0));
             CU(c, cudaEventRecord(c->ev_p0, c->stream2));
-            launch_project(cloud->f16, cloud->blocks != nullptr, cloud->pos, cloud->blocks ? cloud->blocks : cloud->sh, cloud->rot, cloud->so, c->slot_ids, 1, c->ctr, fc, c->recs,
-                           raster_mode == 2 ? c->extra : nullptr, n_hint < n ? n_hint : n, c->sm_count, 2, c->cutoff_tab, nullptr, c->stream2);
+            launch_project(cloud->f16, cloud->blocks, c->slot_ids, 1, c->ctr, fc, c->recs, raster_mode == 2 ? c->extra : nullptr,
+                           n_hint < n ? n_hint : n, c->sm_count, c->cutoff_tab, nullptr, c->stream2);
             ++launches;
             CU(c, cudaEventRecord(c->ev_p1, c->stream2));
             CU(c, cudaEventRecord(c->ev_join, c->stream2));
@@ -809,9 +768,8 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
                 ++launches;
             }
             CU(c, cudaEventRecord(c->ev_p0, q));
-            launch_project(cloud->f16, cloud->blocks != nullptr, cloud->pos, cloud->blocks ? cloud->blocks : cloud->sh, cloud->rot, cloud->so, by_slot ? c->slot_ids : c->vals[cur],
-                           by_slot ? 1 : 0, c->ctr, fc, c->recs,
-                           raster_mode == 2 ? c->extra : nullptr, n_hint < n ? n_hint : n, c->sm_count, 0, c->cutoff_tab,
+            launch_project(cloud->f16, cloud->blocks, by_slot ? c->slot_ids : c->vals[cur], by_slot ? 1 : 0, c->ctr, fc, c->recs,
+                           raster_mode == 2 ? c->extra : nullptr, n_hint < n ? n_hint : n, c->sm_count, c->cutoff_tab,
                            want_aux ? c->aux : nullptr, q);
             ++launches;
             CU(c, cudaEventRecord(c->ev_p1, q));
@@ -825,19 +783,14 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         int pcur = 0;
         for (int r = 0; r < rounds; ++r) {
             ChunkCounters* cc = &c->ctr->chunk[r];
-            const uint32_t fa = rounds > 1 ? c->chunk_frac[r] : 0u, fb = rounds > 1 ? c->chunk_frac[r + 1] : 65536u;
+            const uint32_t fa = rounds > 1 ? CHUNK_FRAC[r] : 0u, fb = rounds > 1 ? CHUNK_FRAC[r + 1] : 65536u;
             uint2* rng = c->ranges + (size_t)r * num_tiles;
             uint32_t* hist_r = c->hist + (size_t)(4 + 4 * r) * 256;
-            if (c->coop) {
-                // the depth sort's spare ping-pong buffers (N words each) hold the large-footprint queue
-                CU(c, launch_bin_emit_coop(c->recs, by_slot ? c->vals[cur] : nullptr, c->ctr, cc, fa, fb, num_tiles,
-                                           c->status_bin, tiles_x, c->cap_pairs, c->pkeys[0], c->pvals[0], c->keys[cur ^ 1],
-                                           c->vals[cur ^ 1], c->cap_n, (getenv("BGS_TIMELINE_SORT") || getenv("BGS_TIMELINE_KEYGEN")) ? nullptr : c->timeline,
-                                           (st->flags & BGS_FLAG_ASYNC) ? c->bin_grid_async : c->bin_grid, c->d_sticky, q));
-            } else {
-                launch_bin_emit(c->recs, by_slot ? c->vals[cur] : nullptr, c->ctr, cc, c->status_bin, tiles_x, c->cap_pairs,
-                                c->pkeys[0], c->pvals[0], n, c->sm_count, c->d_sticky, q);
-            }
+            // the depth sort's spare ping-pong buffers (N words each) hold the large-footprint queue
+            CU(c, launch_bin_emit_coop(c->recs, by_slot ? c->vals[cur] : nullptr, c->ctr, cc, fa, fb, num_tiles,
+                                       c->bin_block_cnt, tiles_x, c->cap_pairs, c->pkeys[0], c->pvals[0], c->keys[cur ^ 1],
+                                       c->vals[cur ^ 1], c->cap_n, (st->flags & BGS_FLAG_ASYNC) ? c->bin_grid_async : c->bin_grid,
+                                       c->d_sticky, q));
             ++launches;
             // stable tile-id sort of the pair list + per-tile ranges: histogram phase, both digit places and the range
             // build in ONE cooperative launch
@@ -845,8 +798,8 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
             if (rounds > 1) p_hint = c->chunk_hint_valid ? c->chunk_pairs_hint[r] : c->cap_pairs;
             if (p_hint > c->cap_pairs) p_hint = c->cap_pairs;
             CU(c, launch_radix_sort(c->pkeys[0], c->pvals[0], c->pkeys[1], c->pvals[1], &cc->n_pairs, c->cap_pairs, p_hint, hist_r, 1,
-                                    c->status_pairs, (size_t)radix_num_tiles(c->status_np) * 256, next_epoch(c), &cc->tile_ctr_sort[0],
-                                    tile_passes, 0, rng, c->sm_count, (st->flags & BGS_FLAG_ASYNC) ? c->rs_per_sm_async : c->rs_per_sm, q, nullptr));
+                                    c->status_pairs, (size_t)radix_num_tiles(c->status_np) * 256, next_epoch(c), &cc->sort_barrier,
+                                    tile_passes, 0, rng, c->sm_count, (st->flags & BGS_FLAG_ASYNC) ? SORT_CTAS_PER_SM_ASYNC : c->rs_per_sm, q));
             ++launches;
             pcur = tile_passes & 1;
             if (r + 1 == rounds) {
@@ -856,13 +809,12 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
             }
             if (rounds == 1) {
                 // the blend runs on the LOW-priority stream; the render stream resumes once it is done
-                static int split = -1;
-                if (split < 0) { const char* e = getenv("BGS_RASTER_PRIO"); split = (e && atoi(e) == 0) ? 0 : 1; }
-                cudaStream_t qr = split ? c->stream_r : q;
-                if (split) { CU(c, cudaEventRecord(c->ev_front, q)); CU(c, cudaStreamWaitEvent(qr, c->ev_front, 0)); }
+                CU(c, cudaEventRecord(c->ev_front, q));
+                CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
                 launch_raster(raster_mode, large_fp, c->recs, c->extra, c->pvals[pcur], rng, W, H, tiles_x, tiles_y, target, raster_format,
-                              want_aux ? c->aux : nullptr, tgt_depth, tgt_normal, qr);
-                if (split) { CU(c, cudaEventRecord(c->ev_rdone, qr)); CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0)); }
+                              want_aux ? c->aux : nullptr, tgt_depth, tgt_normal, c->stream_r);
+                CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
+                CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
             } else
                 launch_raster_round(c->recs, c->pvals[pcur], rng, W, H, tiles_x, tiles_y, target, raster_format, c->state,
                                     c->tile_done, &c->ctr->tiles_done, r == 0, r + 1 == rounds, q);
@@ -1049,14 +1001,6 @@ cudaStream_t bgs_internal_gather_begin_(bgs_context* c, const void* local_frame,
 void bgs_internal_gather_end_(bgs_context* c, int slot) {
     if (!c || slot < 0) return;
     if (cudaEventRecord(c->ev_copied[slot], c->stream_copy) == cudaSuccess) c->copy_pending[slot] = true;
-}
-
-// undocumented debug aid (not in bgs.h): copy the bin_emit_coop per-CTA timeline (grid x 8 u64 ns stamps)
-bgs_status bgs_debug_timeline_(bgs_context* c, unsigned long long* out, uint32_t* grid) {
-    if (!c || !out || !grid || !c->timeline) return BGS_EINVAL;
-    *grid = c->bin_grid;
-    CU(c, cudaMemcpy(out, c->timeline, (size_t)c->bin_grid * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    return BGS_OK;
 }
 
 const char* bgs_last_error(const bgs_context* c) { return c ? c->err : "null context"; }

@@ -2,127 +2,17 @@
 // reference, which rasterises one instanced quad per gaussian: src/render/mod.rs:1562-1566).
 //
 // For every visible splat in front-to-back rank order, emit one (tile id, rank) pair per 16x16
-// tile its conservative pixel bbox touches (payload = the splat's record index).  Pair offsets come from a single-pass chained scan
-// (decoupled look-back) over the per-splat tile counts, so pairs are emitted in rank order and
-// the stable tile-id radix sort that follows yields, per tile, a slice of the GLOBAL depth order.
-// range build: boundaries of equal tile ids in the sorted pair keys.
+// tile its conservative pixel bbox touches (payload = the splat's record index).  Pair offsets are an
+// exclusive scan of the per-splat tile counts in rank order, so the stable tile-id radix sort that
+// follows yields, per tile, a slice of the GLOBAL depth order.
 #include "common.cuh"
 
 namespace bgs {
 
 constexpr int BIN_THREADS = 256;
-constexpr int BIN_ITEMS = 4;
-constexpr int BIN_TILE = BIN_THREADS * BIN_ITEMS;
 constexpr int COOP_ITEMS = 8;        // cooperative kernel: up to 8 ranks per thread per round
 constexpr uint32_t BIN_TINY = 4u;   // footprints up to this many tiles: written by the owning thread
-constexpr uint32_t BIN_BIG = 128u;   // larger than this: global queue, drained by the whole grid   // splats touching more tiles than this are emitted by the whole block
-
-__global__ void __launch_bounds__(BIN_THREADS)
-bin_emit_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ perm, FrameCounters* __restrict__ ctr,
-                ChunkCounters* __restrict__ cc, uint32_t* __restrict__ status, int tiles_x, uint32_t capacity,
-                uint32_t* __restrict__ pair_keys, uint32_t* __restrict__ pair_vals, uint32_t* __restrict__ sticky_need) {
-    __shared__ uint32_t s_wtot[BIN_THREADS / 32];
-    __shared__ uint32_t s_base;
-    __shared__ uint32_t s_tile;
-    __shared__ uint32_t s_nbig;
-    __shared__ uint4 s_big[BIN_TILE];   // (rank, pair offset, bbox x, bbox y) of large-footprint splats
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    const uint32_t n_vis = ctr->n_vis;
-    const uint32_t num_tiles = (n_vis + BIN_TILE - 1) / BIN_TILE;
-    while (true) {
-        if (t == 0) { s_tile = atomicAdd(&cc->tile_ctr_bin, 1u); s_nbig = 0u; }
-        __syncthreads();
-        const uint32_t tile = s_tile;
-        if (tile >= num_tiles) break;
-        const uint32_t r0 = tile * BIN_TILE + t * BIN_ITEMS;   // blocked: 4 consecutive ranks per thread
-        uint32_t bx[BIN_ITEMS], by[BIN_ITEMS], cnt[BIN_ITEMS], ri[BIN_ITEMS];
-        uint32_t mine = 0u;
-#pragma unroll
-        for (int j = 0; j < BIN_ITEMS; ++j) {
-            const uint32_t r = r0 + j;
-            cnt[j] = 0u; ri[j] = 0u;
-            if (r < n_vis) {
-                ri[j] = perm ? __ldg(perm + (n_vis - 1u - r)) : r;   // rank -> record index
-                const uint2 b = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const char*>(recs + ri[j]) + 24));
-                bx[j] = b.x; by[j] = b.y;
-                const uint32_t xlo = b.x & 0xFFFFu, xhi = b.x >> 16, ylo = b.y & 0xFFFFu, yhi = b.y >> 16;
-                if (xlo <= xhi && ylo <= yhi)
-                    cnt[j] = ((xhi >> 4) - (xlo >> 4) + 1u) * ((yhi >> 4) - (ylo >> 4) + 1u);
-            }
-            mine += cnt[j];
-        }
-        uint32_t incl = mine;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += y;
-        }
-        if (lane == 31) s_wtot[warp] = incl;
-        __syncthreads();
-        if (warp == 0) {
-            uint32_t v = (lane < BIN_THREADS / 32) ? s_wtot[lane] : 0u;
-            uint32_t total = v;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-            // a frame needing >= 2^30 pairs cannot be represented in the status word: saturate
-            const uint32_t agg = total > LB_VMASK ? LB_VMASK : total;
-            const uint32_t base = warp_lookback(status, (int)tile, agg);
-            if (lane == 0) {
-                s_base = base;
-                if (tile == num_tiles - 1) {
-                    const uint32_t need = base + agg;
-                    cc->n_pairs_needed = need;
-                    cc->n_pairs = need < capacity ? need : capacity;
-                    atomicMax(sticky_need, need);   // survives the per-frame clear: bgs_sync sees every queued frame's need
-                }
-            }
-        }
-        __syncthreads();
-        uint32_t wprefix = 0u;
-        for (int w = 0; w < warp; ++w) wprefix += s_wtot[w];
-        uint32_t off = s_base + wprefix + incl - mine;
-#pragma unroll
-        for (int j = 0; j < BIN_ITEMS; ++j) {
-            if (cnt[j] == 0u) continue;
-            const uint32_t r = ri[j];
-            if (cnt[j] > BIN_BIG) {
-                // large footprint: hand it to the whole block (coalesced, parallel emission below)
-                const uint32_t q = atomicAdd(&s_nbig, 1u);
-                s_big[q] = make_uint4(r, off, bx[j], by[j]);
-            } else {
-                const uint32_t txlo = (bx[j] & 0xFFFFu) >> 4, txhi = (bx[j] >> 16) >> 4;
-                const uint32_t tylo = (by[j] & 0xFFFFu) >> 4, tyhi = (by[j] >> 16) >> 4;
-                uint32_t o = off;
-                for (uint32_t ty = tylo; ty <= tyhi; ++ty)
-                    for (uint32_t tx = txlo; tx <= txhi; ++tx) {
-                        if (o < capacity) {
-                            pair_keys[o] = ty * (uint32_t)tiles_x + tx;
-                            pair_vals[o] = r;
-                        }
-                        ++o;
-                    }
-            }
-            off += cnt[j];
-        }
-        __syncthreads();
-        const uint32_t nbig = s_nbig;
-        for (uint32_t q = 0; q < nbig; ++q) {
-            const uint4 b = s_big[q];
-            const uint32_t txlo = (b.z & 0xFFFFu) >> 4, txhi = (b.z >> 16) >> 4;
-            const uint32_t tylo = (b.w & 0xFFFFu) >> 4, tyhi = (b.w >> 16) >> 4;
-            const uint32_t w = txhi - txlo + 1u, total = w * (tyhi - tylo + 1u);
-            for (uint32_t i = t; i < total; i += BIN_THREADS) {
-                const uint32_t o = b.y + i;
-                if (o < capacity) {
-                    pair_keys[o] = (tylo + i / w) * (uint32_t)tiles_x + (txlo + i % w);
-                    pair_vals[o] = b.x;
-                }
-            }
-        }
-        __syncthreads();
-    }
-    // n_vis == 0: nothing was published; counters stay zero from the per-frame clear
-}
+constexpr uint32_t BIN_BIG = 128u;   // larger than this: global queue, drained by the whole grid
 
 // Cooperative variant (all CTAs co-resident).  Each CTA owns a contiguous range of front-to-back ranks.
 //   phase 1: per splat, the tiles its bbox touches; the CTA publishes THREE totals: pairs, medium-footprint splats,
@@ -158,8 +48,7 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
                      ChunkCounters* __restrict__ cc, uint32_t frac_a, uint32_t frac_b, uint32_t num_tiles_total,
                      uint32_t* __restrict__ block_cnt /* [grid][3] */, int tiles_x, uint32_t capacity, uint32_t* __restrict__ pair_keys,
                      uint32_t* __restrict__ pair_vals, uint32_t* __restrict__ q_rank, uint32_t* __restrict__ q_off,
-                     uint32_t q_cap, unsigned long long* __restrict__ tl, uint32_t* __restrict__ sticky_need) {
-    timeline_stamp(tl, 0);
+                     uint32_t q_cap, uint32_t* __restrict__ sticky_need) {
     __shared__ uint32_t s_wtot[3][BIN_THREADS / 32];
     __shared__ unsigned long long s_red64[3 * 8];
     __shared__ uint32_t s_tot[3];
@@ -231,9 +120,7 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
         s_tot[t] = tot;
         st_volatile(block_cnt + 3 * b + t, tot);
     }
-    timeline_stamp(tl, 1);
     grid_barrier(&cc->barrier, G);
-    timeline_stamp(tl, 2);
 
     // ---- phase 2 (pair sums saturate at 2^30 - 1: such a frame is rejected by the host)
     uint64_t pre[3];
@@ -307,9 +194,7 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
         run += ttotal; mrun += mtotal; brun += btotal;
         __syncthreads();
     }
-    timeline_stamp(tl, 3);
     grid_barrier(&cc->barrier, 2u * G);
-    timeline_stamp(tl, 4);
 
     // ---- phase 3a: medium footprints, 32 per warp: each lane fetches one splat's (record, offset, bbox)
     //      so the memory latency is paid once per 32 splats; then the warp writes them one after another
@@ -376,19 +261,7 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
             if (tx > txhi) { tx -= w; ++ty; }
         }
     }
-    timeline_stamp(tl, 5);
 }
-
-void launch_bin_emit(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc, uint32_t* status,
-                     int tiles_x, uint32_t capacity, uint32_t* pair_keys, uint32_t* pair_vals, uint32_t n_upper,
-                     int sm_count, uint32_t* sticky_need, cudaStream_t stream) {
-    uint32_t blocks = (n_upper + BIN_TILE - 1) / BIN_TILE;
-    const uint32_t cap_blocks = (uint32_t)sm_count * 4u;
-    if (blocks > cap_blocks) blocks = cap_blocks;
-    if (blocks == 0) blocks = 1;
-    bin_emit_kernel<<<blocks, BIN_THREADS, 0, stream>>>(recs, perm, ctr, cc, status, tiles_x, capacity, pair_keys, pair_vals, sticky_need);
-}
-uint32_t bin_num_tiles(uint32_t n) { return (n + BIN_TILE - 1) / BIN_TILE; }
 
 int bin_coop_blocks_per_sm() {
     int b = 0;
@@ -398,11 +271,10 @@ int bin_coop_blocks_per_sm() {
 cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
                                  uint32_t frac_a, uint32_t frac_b, uint32_t num_tiles_total, uint32_t* block_cnt,
                                  int tiles_x, uint32_t capacity, uint32_t* pair_keys, uint32_t* pair_vals,
-                                 uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, unsigned long long* timeline,
-                                 uint32_t grid, uint32_t* sticky_need, cudaStream_t stream) {
+                                 uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, uint32_t grid, uint32_t* sticky_need, cudaStream_t stream) {
     void* args[] = {(void*)&recs, (void*)&perm, (void*)&ctr, (void*)&cc, (void*)&frac_a, (void*)&frac_b, (void*)&num_tiles_total,
                     (void*)&block_cnt, (void*)&tiles_x, (void*)&capacity, (void*)&pair_keys,
-                    (void*)&pair_vals, (void*)&q_rank, (void*)&q_off, (void*)&q_cap, (void*)&timeline, (void*)&sticky_need};
+                    (void*)&pair_vals, (void*)&q_rank, (void*)&q_off, (void*)&q_cap, (void*)&sticky_need};
     return cudaLaunchCooperativeKernel((const void*)bin_emit_coop_kernel, dim3(grid), dim3(BIN_THREADS), args, 0, stream);
 }
 

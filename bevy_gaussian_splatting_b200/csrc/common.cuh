@@ -10,8 +10,8 @@ namespace bgs {
 constexpr int TILE_PX = 16;           // 16x16-pixel raster tiles (a7)
 constexpr float T_STOP = 1.0e-4f;     // a pixel stops once its transmittance drops below this
 
-// Look-back status word: bits 31:30 flag, bits 29:0 value (n and n_pairs are < 2^30).
-constexpr uint32_t LB_EMPTY = 0u, LB_AGG = 1u << 30, LB_INC = 2u << 30, LB_VMASK = (1u << 30) - 1u;
+// Saturation bound of the entry and pair counts (n and n_pairs are < 2^30).
+constexpr uint32_t LB_VMASK = (1u << 30) - 1u;
 
 // Per-frame constants handed to the kernels by value (column-major matrices, as Bevy).
 struct FrameConsts {
@@ -49,15 +49,14 @@ struct ChunkCounters {
     uint32_t n_pairs;           // (splat, tile) pairs emitted (clamped to capacity)
     uint32_t n_pairs_needed;    // pairs the round needs (may exceed capacity -> host regrows and redoes the frame)
     uint32_t barrier;           // grid barrier of bin_emit_coop (two uses per launch)
-    uint32_t big_count, big_head;   // queue of large footprints (grows from the back of the queue arrays)
-    uint32_t med_count, med_head;   // queue of medium footprints (grows from the front), drained 32 per warp
-    uint32_t tile_ctr_bin;      // tile tickets of the fallback (chained look-back) bin kernel
-    uint32_t tile_ctr_sort[4];  // tile tickets of the pair sort's passes
+    uint32_t big_count;         // queue of large footprints (grows from the back of the queue arrays)
+    uint32_t med_count;         // queue of medium footprints (grows from the front), drained 32 per warp
+    uint32_t sort_barrier;      // grid barrier of the pair sort
     uint32_t skipped;           // 1 = the round emitted nothing because every tile had already saturated
-    uint32_t pad[3];
+    uint32_t pad[9];
 };
 static_assert(sizeof(ChunkCounters) == 64, "ChunkCounters is 64 bytes");
-constexpr int MAX_CHUNKS = 8;
+constexpr int MAX_CHUNKS = 5;         // rounds of a chunked frame (api.cu: CHUNK_FRAC)
 
 // Device-resident per-frame counters (cleared at frame start).
 struct FrameCounters {
@@ -65,11 +64,10 @@ struct FrameCounters {
     uint32_t n_vis;             // in-frustum gaussians
     uint32_t tiles_done;        // tiles whose pixels have all saturated (chunked frames)
     uint32_t pad0;
-    uint32_t tile_ctr[8];       // dynamic tile tickets: [0] keygen (fallback kernel), [1..4] depth sort passes
     uint32_t culled_min_inv;    // RasterizeMode::Depth: max over culled of (0xFFFFFFFF - index); 0 = none culled
     uint32_t culled_max_p1;     //                       max over culled of (index + 1);          0 = none culled
     float depth_min, depth_max; //                       distances of sorted[N-1] / sorted[1] (gaussian.wgsl:329-349)
-    uint32_t barrier[4];        // grid barrier of keygen_coop: [0]
+    uint32_t barrier[2];        // grid barriers: [0] keygen_coop, [1] the depth sort
     ChunkCounters chunk[MAX_CHUNKS];
 };
 
@@ -77,42 +75,16 @@ struct FrameCounters {
 // ld/st.volatile would be SYSTEM scope)
 __device__ __forceinline__ uint32_t ld_volatile(const uint32_t* p) {
     uint32_t v;
-#ifdef BGS_SYS_SCOPE
-    asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-#else
     asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-#endif
     return v;
 }
 __device__ __forceinline__ void st_volatile(uint32_t* p, uint32_t v) {
-#ifdef BGS_SYS_SCOPE
-    asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-#else
     asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-#endif
 }
 __device__ __forceinline__ uint32_t lanemask_lt() {
     uint32_t m;
     asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
     return m;
-}
-__device__ __forceinline__ uint32_t lanemask_le() {
-    uint32_t m;
-    asm("mov.u32 %0, %%lanemask_le;" : "=r"(m));
-    return m;
-}
-
-// Optional per-CTA timeline (debug builds of a run: BGS_TIMELINE=1): %globaltimer stamps at phase boundaries.
-__device__ __forceinline__ void timeline_stamp(unsigned long long* tl, int slot) {
-    if (tl != nullptr && threadIdx.x == 0) {
-        unsigned long long t;
-#ifdef BGS_TIMELINE_CLOCK64
-        t = (unsigned long long)clock64();              // SM cycles: exact intra-CTA deltas
-#else
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-#endif
-        tl[(size_t)blockIdx.x * 8 + slot] = t;
-    }
 }
 
 // Grid-wide barrier for kernels launched with cudaLaunchCooperativeKernel (all CTAs co-resident).
@@ -143,38 +115,6 @@ __device__ __forceinline__ uint32_t block_sum_prefix(const uint32_t* counts, uin
     for (int w = 0; w < THREADS / 32; ++w) tot += s_red[w];
     __syncthreads();
     return tot;
-}
-
-// Decoupled look-back over single-word tile status, executed by ONE full warp.
-// Publishes this tile's aggregate, sums predecessors' aggregates back to the nearest inclusive
-// prefix, publishes the inclusive prefix, returns the exclusive prefix (same value on all lanes).
-__device__ __forceinline__ uint32_t warp_lookback(uint32_t* status, int tile, uint32_t aggregate) {
-    const int lane = threadIdx.x & 31;
-    if (tile == 0) {
-        if (lane == 0) st_volatile(status, LB_INC | aggregate);
-        return 0u;
-    }
-    if (lane == 0) st_volatile(status + tile, LB_AGG | aggregate);
-    uint32_t excl = 0u;
-    for (int base = tile - 1; base >= 0; base -= 32) {
-        const int idx = base - lane;
-        uint32_t w;
-        do {
-            w = (idx >= 0) ? ld_volatile(status + idx) : (LB_INC | 0u);
-        } while (__any_sync(0xffffffffu, (w >> 30) == 0u));
-        const uint32_t inc_mask = __ballot_sync(0xffffffffu, (w >> 30) == 2u);
-        uint32_t v = w & LB_VMASK;
-        if (inc_mask) {
-            const int first = __ffs(inc_mask) - 1;   // nearest predecessor holding an inclusive prefix
-            if (lane > first) v = 0u;
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        excl += v;
-        if (inc_mask) break;
-    }
-    if (lane == 0) st_volatile(status + tile, LB_INC | ((excl + aggregate) & LB_VMASK));
-    return excl;
 }
 
 }  // namespace bgs

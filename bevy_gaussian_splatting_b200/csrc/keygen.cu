@@ -3,9 +3,9 @@
 // Replaces radix_sort_a's key half (src/sort/radix.wgsl:86-106): key = 0xFFFFFFFF - bits(|Mp-cam|^2)
 // for in-frustum gaussians, 0xFFFFFFFF otherwise, shifted by 32 - depth_bits.  Instead of sorting
 // the culled (all-ones) keys with everything else, the visible (key, index) pairs are compacted
-// IN INDEX ORDER (single-pass chained scan with decoupled look-back), so the stable LSD sort that
-// follows sees the same tie order as the reference; the culled tail of the reference's
-// sorted_entry_buffer is "ascending index" and is reconstructed only by the debug hook.
+// IN INDEX ORDER (keygen_coop_kernel), so the stable LSD sort that follows sees the same tie order
+// as the reference; the culled tail of the reference's sorted_entry_buffer is "ascending index"
+// and is reconstructed only by the debug hook.  BGS_FLAG_SORT_ALL keeps every entry (keygen_all_kernel).
 //
 // HBM-bound streaming kernel: 16 B read per gaussian (coalesced float4), 8 B written per
 // visible gaussian.  Compiled with -fmad=false (see project_math.cuh).
@@ -17,94 +17,21 @@ constexpr int KG_THREADS = 256;
 constexpr int KG_ITEMS = 8;
 constexpr int KG_TILE = KG_THREADS * KG_ITEMS;
 
+// BGS_FLAG_SORT_ALL (reference-literal mode): every entry goes to the depth sort in index order, payload = the
+// gaussian index; only the visible ones are counted
 __global__ void __launch_bounds__(KG_THREADS)
-keygen_compact_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, int sort_all,
-                      uint32_t* __restrict__ keys_out, uint32_t* __restrict__ ids_out, uint32_t* __restrict__ slots_out,
-                      uint32_t* __restrict__ status, FrameCounters* __restrict__ ctr) {
-    __shared__ uint32_t s_cnt[KG_ITEMS * (KG_THREADS / 32)];
-    __shared__ uint32_t s_off[KG_ITEMS * (KG_THREADS / 32)];
-    __shared__ uint32_t s_base;
-    __shared__ int s_tile;
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    // dynamic tile ticket: look-back only ever waits on tiles that already started
-    if (t == 0) s_tile = (int)atomicAdd(&ctr->tile_ctr[0], 1u);
-    __syncthreads();
-    const int tile = s_tile;
-    const uint32_t tile_base = (uint32_t)tile * KG_TILE;
-
-    float4 p[KG_ITEMS];
-#pragma unroll
-    for (int j = 0; j < KG_ITEMS; ++j) {
-        const uint32_t i = tile_base + j * KG_THREADS + t;
-        p[j] = (i < n) ? __ldcs(pos + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+keygen_all_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, uint32_t* __restrict__ keys_out,
+                  uint32_t* __restrict__ ids_out, FrameCounters* __restrict__ ctr) {
+    const uint32_t i = blockIdx.x * KG_THREADS + threadIdx.x;
+    bool vis = false;
+    if (i < n) {
+        const float4 p = __ldcs(pos + i);
+        keys_out[i] = key_of_fast(fc, p.x, p.y, p.z, vis);
+        ids_out[i] = i;
     }
-    uint32_t key[KG_ITEMS];
-    uint32_t prefix[KG_ITEMS];   // rank among the visible items of (item j, this warp)
-    uint32_t vis_bits = 0;
-#pragma unroll
-    for (int j = 0; j < KG_ITEMS; ++j) {
-        const uint32_t i = tile_base + j * KG_THREADS + t;
-        bool kvis;
-        const uint32_t kkey = key_of_fast(fc, p[j].x, p[j].y, p[j].z, kvis);
-        const bool v = (i < n) && kvis;
-        key[j] = kkey;
-        if ((fc.rasterize_mode == BGS_RASTERIZE_DEPTH || fc.aux) && i < n && !kvis) {
-            atomicMax(&ctr->culled_min_inv, 0xFFFFFFFFu - i);
-            atomicMax(&ctr->culled_max_p1, i + 1u);
-        }
-        const uint32_t b = __ballot_sync(0xffffffffu, v);
-        prefix[j] = __popc(b & lanemask_lt());
-        if (v) vis_bits |= 1u << j;
-        if (lane == 0) s_cnt[j * (KG_THREADS / 32) + warp] = __popc(b);
-    }
-    __syncthreads();
-    if (sort_all) {
-        // reference-literal mode: every entry goes to the sort; just count the visible ones
-        if (warp == 0) {
-            uint32_t v = s_cnt[lane] + s_cnt[lane + 32];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-            if (lane == 0 && v) atomicAdd(&ctr->n_vis, v);
-            if (lane == 0 && tile == 0) ctr->n_sort = n;
-        }
-#pragma unroll
-        for (int j = 0; j < KG_ITEMS; ++j) {
-            const uint32_t i = tile_base + j * KG_THREADS + t;
-            if (i < n) { keys_out[i] = key[j]; ids_out[i] = i; }
-        }
-        return;
-    }
-    if (warp == 0) {
-        // 64 (item, warp) counts in index order: exclusive scan, two per lane
-        const uint32_t a = s_cnt[2 * lane], b = s_cnt[2 * lane + 1];
-        uint32_t incl = a + b;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t y = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += y;
-        }
-        const uint32_t excl = incl - (a + b);
-        s_off[2 * lane] = excl;
-        s_off[2 * lane + 1] = excl + a;
-        const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
-        const uint32_t base = warp_lookback(status, tile, total);
-        if (lane == 0) {
-            s_base = base;
-            // the last tile (in index order) knows the final count
-            if (tile_base + KG_TILE >= n) { ctr->n_vis = base + total; ctr->n_sort = base + total; }
-        }
-    }
-    __syncthreads();
-    const uint32_t base = s_base;
-#pragma unroll
-    for (int j = 0; j < KG_ITEMS; ++j) {
-        if (vis_bits & (1u << j)) {
-            const uint32_t dst = base + s_off[j * (KG_THREADS / 32) + warp] + prefix[j];
-            keys_out[dst] = key[j];
-            ids_out[dst] = tile_base + j * KG_THREADS + t;
-            slots_out[dst] = dst;
-        }
-    }
+    const int cnt = __syncthreads_count(vis);
+    if (threadIdx.x == 0 && cnt) atomicAdd(&ctr->n_vis, (uint32_t)cnt);
+    if (i == 0) ctr->n_sort = n;
 }
 
 // Cooperative variant (all CTAs co-resident, launched with cudaLaunchCooperativeKernel): each CTA owns a
@@ -126,8 +53,7 @@ __global__ void __launch_bounds__(KG_THREADS)
 keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, uint32_t* __restrict__ masks,
                    uint32_t* __restrict__ keys_out, uint32_t* __restrict__ ids_out, uint32_t* __restrict__ slots_out,
                    uint32_t* __restrict__ block_cnt, FrameCounters* __restrict__ ctr, uint32_t* __restrict__ hist,
-                   int hist_passes, unsigned long long* __restrict__ tl) {
-    timeline_stamp(tl, 0);
+                   int hist_passes) {
     __shared__ uint32_t s_hist[4 * 256];   // digit histograms of the visible keys (the depth sort's pre-pass, fused)
     __shared__ uint32_t s_red[KG_THREADS / 32];
     __shared__ uint32_t s_total;
@@ -179,15 +105,12 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
         s_total = tot;
         st_volatile(block_cnt + b, tot);
     }
-    timeline_stamp(tl, 1);
     grid_barrier(&ctr->barrier[0], G);
-    timeline_stamp(tl, 2);
 
     // ---- phase 2: exclusive prefix over CTAs, then ordered expansion of this CTA's mask words
     for (int i = t; i < hist_passes * 256; i += KG_THREADS) s_hist[i] = 0u;
     uint32_t run = block_sum_prefix<KG_THREADS>(block_cnt, b, s_red);
     if (b == G - 1 && t == 0) { ctr->n_vis = run + s_total; ctr->n_sort = run + s_total; }
-    timeline_stamp(tl, 3);
     const uint32_t w_begin = t0 * KG_WORDS_PER_TILE, w_end = t1 * KG_WORDS_PER_TILE;
     for (uint32_t wc = w_begin; wc < w_end; wc += KG_CHUNK_WORDS) {
         const uint32_t cw = min((uint32_t)KG_CHUNK_WORDS, w_end - wc);
@@ -246,12 +169,10 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
         run += chunk_total;
         __syncthreads();
     }
-    timeline_stamp(tl, 4);
     for (int i = t; i < hist_passes * 256; i += KG_THREADS) {
         const uint32_t c = s_hist[i];
         if (c) atomicAdd(&hist[i], c);
     }
-    timeline_stamp(tl, 5);
 }
 
 // Debug hook: rebuild the reference's full sorted_entry_buffer (sort/mod.rs:323-329) from the
@@ -265,12 +186,10 @@ __global__ void culled_flags_kernel(const float4* __restrict__ pos, uint32_t n, 
     flags[i] = key_of(fc, p.x, p.y, p.z).visible ? 0u : 1u;
 }
 
-void launch_keygen(const float4* pos, uint32_t n, const FrameConsts& fc, int sort_all, uint32_t* keys_out,
-                   uint32_t* ids_out, uint32_t* slots_out, uint32_t* status, FrameCounters* ctr, cudaStream_t stream) {
-    const uint32_t tiles = (n + KG_TILE - 1) / KG_TILE;
-    keygen_compact_kernel<<<tiles, KG_THREADS, 0, stream>>>(pos, n, fc, sort_all, keys_out, ids_out, slots_out, status, ctr);
+void launch_keygen_all(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* keys_out, uint32_t* ids_out,
+                       FrameCounters* ctr, cudaStream_t stream) {
+    keygen_all_kernel<<<(n + KG_THREADS - 1) / KG_THREADS, KG_THREADS, 0, stream>>>(pos, n, fc, keys_out, ids_out, ctr);
 }
-uint32_t keygen_num_tiles(uint32_t n) { return (n + KG_TILE - 1) / KG_TILE; }
 
 int keygen_coop_blocks_per_sm() {
     int b = 0;
@@ -279,10 +198,10 @@ int keygen_coop_blocks_per_sm() {
 }
 cudaError_t launch_keygen_coop(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* masks, uint32_t* keys_out,
                                uint32_t* ids_out, uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr,
-                               uint32_t* hist, int hist_passes, uint32_t grid, unsigned long long* tl, cudaStream_t stream) {
+                               uint32_t* hist, int hist_passes, uint32_t grid, cudaStream_t stream) {
     FrameConsts fcc = fc;
     void* args[] = {(void*)&pos, (void*)&n, (void*)&fcc, (void*)&masks, (void*)&keys_out, (void*)&ids_out,
-                    (void*)&slots_out, (void*)&block_cnt, (void*)&ctr, (void*)&hist, (void*)&hist_passes, (void*)&tl};
+                    (void*)&slots_out, (void*)&block_cnt, (void*)&ctr, (void*)&hist, (void*)&hist_passes};
     return cudaLaunchCooperativeKernel((const void*)keygen_coop_kernel, dim3(grid), dim3(KG_THREADS), args, 0, stream);
 }
 

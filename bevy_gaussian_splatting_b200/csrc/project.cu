@@ -3,13 +3,11 @@
 // its vertex stage: src/render/gaussian.wgsl:185-436).
 //
 // rank r (0 = nearest) -> gaussian id = sorted_ids[n_vis-1-r] (the sort is far->near like the
-// reference's, src/sort/radix.wgsl) -> gather the planar attributes (f32 240 B or f16 128 B per
-// gaussian) -> write one 48 B SplatRec at recs[r] (coalesced), which is all the tile stages read.
+// reference's, src/sort/radix.wgsl) -> gather the gaussian's block (f32 256 B or f16 128 B) ->
+// write one 48 B SplatRec at recs[r] (coalesced), which is all the tile stages read.
 //
 // Geometry (centre, OBB uv rows, pixel bbox) is bit-exact vs the oracle: compiled -fmad=false.
 #include <cuda_fp16.h>
-
-#include <cstdlib>
 
 #include "project_math.cuh"
 
@@ -57,16 +55,16 @@ __device__ __forceinline__ void make_bbox(float cx, float cy, float hx, float hy
     bx = pack_bbox(x0, x1); by = pack_bbox(y0, y1);
 }
 
-// Attribute fetch.  PLANAR: the reference's SoA planes as uploaded.  BLOCKED (default): a library-owned
-// gaussian-major copy made once at upload -- f16: 128 B = one cache line per gaussian (pos | rot/scale/opacity |
-// sh x 6), f32: 256 B (pos | rot | scale_opacity | sh x 12 | pad) -- so the random gather of a visible splat
-// touches exactly its own line(s) instead of 3-4 partially used ones (the planes stay planar for key-gen).
-template <bool F16, bool BLOCKED>
+// Attribute fetch from the library-owned gaussian-major copy made once at upload -- f16: 128 B = one cache line per
+// gaussian (pos | rot/scale/opacity | sh x 6), f32: 256 B (pos | rot | scale_opacity | sh x 12 | pad) -- so the random
+// gather of a visible splat touches exactly its own line(s) instead of 3-4 partially used ones of the reference's
+// planes (the position plane stays planar for key-gen).
+template <bool F16>
 struct Attr;
 template <>
-struct Attr<false, true> {
-    __device__ static float4 load(const float4*, const void* blocks, const void*, const void*, uint32_t id, float* sh,
-                                  float q[4], float so[4], bool need_sh, uint32_t* = nullptr) {
+struct Attr<false> {
+    __device__ static float4 load(const void* blocks, uint32_t id, float* sh, float q[4], float so[4], bool need_sh,
+                                  uint32_t* = nullptr) {
         const float4* b = reinterpret_cast<const float4*>(blocks) + (size_t)id * 16;
         const float4 p = __ldg(b), r = __ldg(b + 1), s = __ldg(b + 2);
         q[0] = r.x; q[1] = r.y; q[2] = r.z; q[3] = r.w;
@@ -82,11 +80,11 @@ struct Attr<false, true> {
     }
 };
 template <>
-struct Attr<true, true> {
+struct Attr<true> {
     __device__ static float lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu))); }
     __device__ static float hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
-    __device__ static float4 load(const float4*, const void* blocks, const void*, const void*, uint32_t id, float* sh,
-                                  float q[4], float so[4], bool need_sh, uint32_t* op_bits = nullptr) {
+    __device__ static float4 load(const void* blocks, uint32_t id, float* sh, float q[4], float so[4], bool need_sh,
+                                  uint32_t* op_bits = nullptr) {
         const uint4* b = reinterpret_cast<const uint4*>(blocks) + (size_t)id * 8;
         const uint4 pw = __ldg(b), w = __ldg(b + 1);
         if (op_bits) *op_bits = w.w & 0xFFFFu;
@@ -101,49 +99,6 @@ struct Attr<true, true> {
             }
         }
         return make_float4(__uint_as_float(pw.x), __uint_as_float(pw.y), __uint_as_float(pw.z), __uint_as_float(pw.w));
-    }
-};
-template <>
-struct Attr<false, false> {   // f32 planes: src/gaussian/f32.rs:53-175, planar.wgsl:334-364
-    __device__ static float4 load(const float4* pos, const void* sh_p, const void* rot_p, const void* so_p, uint32_t id,
-                                  float* sh, float q[4], float so[4], bool need_sh, uint32_t* = nullptr) {
-        const float4 p = __ldg(pos + id);
-        const float4 r = __ldg(reinterpret_cast<const float4*>(rot_p) + id);
-        const float4 s = __ldg(reinterpret_cast<const float4*>(so_p) + id);
-        q[0] = r.x; q[1] = r.y; q[2] = r.z; q[3] = r.w;
-        so[0] = s.x; so[1] = s.y; so[2] = s.z; so[3] = s.w;
-        if (need_sh) {
-            const float4* p = reinterpret_cast<const float4*>(sh_p) + (size_t)id * 12;
-#pragma unroll
-            for (int i = 0; i < 12; ++i) {
-                const float4 v = __ldg(p + i);
-                sh[4 * i] = v.x; sh[4 * i + 1] = v.y; sh[4 * i + 2] = v.z; sh[4 * i + 3] = v.w;
-            }
-        }
-        return p;
-    }
-};
-template <>
-struct Attr<true, false> {    // f16 planes: src/gaussian/f16.rs:30-56,244-263; planar.wgsl:117-176
-    __device__ static float lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu))); }
-    __device__ static float hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
-    __device__ static float4 load(const float4* pos, const void* sh_p, const void* rso_p, const void*, uint32_t id, float* sh,
-                                  float q[4], float so[4], bool need_sh, uint32_t* op_bits = nullptr) {
-        const float4 p = __ldg(pos + id);
-        const uint4 w = __ldg(reinterpret_cast<const uint4*>(rso_p) + id);
-        if (op_bits) *op_bits = w.w & 0xFFFFu;
-        q[0] = hi(w.x); q[1] = lo(w.x); q[2] = hi(w.y); q[3] = lo(w.y);
-        so[0] = hi(w.z); so[1] = lo(w.z); so[2] = hi(w.w); so[3] = lo(w.w);
-        if (need_sh) {
-            const uint4* p = reinterpret_cast<const uint4*>(sh_p) + (size_t)id * 6;
-#pragma unroll
-            for (int i = 0; i < 6; ++i) {
-                const uint4 v = __ldg(p + i);
-                sh[8 * i] = lo(v.x); sh[8 * i + 1] = hi(v.x); sh[8 * i + 2] = lo(v.y); sh[8 * i + 3] = hi(v.y);
-                sh[8 * i + 4] = lo(v.z); sh[8 * i + 5] = hi(v.z); sh[8 * i + 6] = lo(v.w); sh[8 * i + 7] = hi(v.w);
-            }
-        }
-        return p;
     }
 };
 
@@ -522,13 +477,10 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
     out[2] = make_float4(rec.r, rec.g, rec.b, rec.op);
 }
 
-#ifndef PROJ_MIN_CTAS
-#define PROJ_MIN_CTAS 6
-#endif
-template <bool F16, bool BLOCKED>
+constexpr int PROJ_MIN_CTAS = 6;
+template <bool F16>
 __global__ void __launch_bounds__(128, PROJ_MIN_CTAS)
-project_kernel(const float4* __restrict__ pos, const void* __restrict__ sh_p, const void* __restrict__ rot_p,
-               const void* __restrict__ so_p, const uint32_t* __restrict__ index_list, int by_slot,
+project_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
                const FrameCounters* __restrict__ ctr, FrameConsts fc, SplatRec* __restrict__ recs,
                float4* __restrict__ extra /* 4 x float4 per record, 2DGS + USE_AABB only */, const float* __restrict__ cutoff_tab,
                float4* __restrict__ aux /* 2 x float4 per record (depth rgb, normal rgb), bgs_render_aux only */) {
@@ -540,7 +492,7 @@ project_kernel(const float4* __restrict__ pos, const void* __restrict__ sh_p, co
         float sh[48], q[4], so[4];
         const bool need_sh = fc.rasterize_mode == BGS_RASTERIZE_COLOR;
         uint32_t op_bits = 0u;
-        const float4 p4 = Attr<F16, BLOCKED>::load(pos, sh_p, rot_p, so_p, id, sh, q, so, need_sh, &op_bits);
+        const float4 p4 = Attr<F16>::load(blocks, id, sh, q, so, need_sh, &op_bits);
         // f16 clouds: the adaptive cutoff of this 16-bit opacity comes from the per-context table (bit-identical)
         const float cutoff_pre = (F16 && fc.adaptive) ? __ldg(cutoff_tab + op_bits) : __uint_as_float(0x7FC00000u);
         project_one(fc, ctr, r, p4, q, so, cutoff_pre,
@@ -552,179 +504,21 @@ project_kernel(const float4* __restrict__ pos, const void* __restrict__ sh_p, co
     }
 }
 
-// ---- TMA ring variant (gaussian-major blocks): each warp streams batches of 32 gaussians through a ring of
-// shared-memory stages.  Every lane issues ONE bulk async copy (cp.async.bulk, SASS UBLKCP) of its gaussian's whole
-// block -- 128 B (f16) / 256 B (f32) -- tracked by the stage's mbarrier (expect_tx = bytes of the batch); the copies
-// of the next STAGES - 1 batches are in flight while the warp computes the current one from shared memory, so the
-// gather's latency hides behind the ~1000 instructions per gaussian regardless of the register budget.
-// Rows are padded by 16 B (144 / 272 B stride): lane l reading 16 B chunk c touches bank group (l + c) mod 8, so the
-// per-lane LDS.128 of a batch are conflict-free.
-constexpr int PR_THREADS = 128;
-constexpr int PR_WARPS = PR_THREADS / 32;
-template <bool F16> struct Ring {
-    static constexpr int ROW = F16 ? 128 : 256;
-    static constexpr int ROWP = ROW + 16;
-    static constexpr int STAGES = F16 ? 3 : 2;
-    static constexpr int WARP_BYTES = STAGES * 32 * ROWP;
-    static constexpr int SMEM = PR_WARPS * WARP_BYTES;
-};
-__device__ __forceinline__ void pr_mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void pr_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void pr_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void pr_mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ float h_lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu))); }
-__device__ __forceinline__ float h_hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
-
-template <bool F16>
-__global__ void __launch_bounds__(PR_THREADS, F16 ? 4 : 3)
-project_ring_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
-                    const FrameCounters* __restrict__ ctr, FrameConsts fc, SplatRec* __restrict__ recs,
-                    float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
-    using R = Ring<F16>;
-    extern __shared__ __align__(128) unsigned char s_ring[];
-    __shared__ __align__(8) unsigned long long s_bar[PR_WARPS][R::STAGES];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t n_vis = ctr->n_vis;
-    const uint32_t nb = (n_vis + 31u) >> 5;
-    const uint32_t wg = blockIdx.x * PR_WARPS + warp, nw = gridDim.x * PR_WARPS;
-    const uint32_t a_ring = (uint32_t)__cvta_generic_to_shared(s_ring) + (uint32_t)warp * R::WARP_BYTES;
-    const uint32_t a_bar = (uint32_t)__cvta_generic_to_shared(&s_bar[warp][0]);
-    if (lane == 0) {
-#pragma unroll
-        for (int s = 0; s < R::STAGES; ++s) pr_mbar_init(a_bar + 8u * s, 1u);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    auto issue = [&](uint32_t k) {
-        const uint32_t batch = wg + k * nw;
-        if (batch >= nb) return;                       // (warp-uniform)
-        const int s = (int)(k % R::STAGES);
-        const uint32_t r = batch * 32u + lane;
-        const bool valid = r < n_vis;
-        uint32_t id = 0u;
-        if (valid) id = by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r));
-        const uint32_t cnt = __popc(__ballot_sync(0xffffffffu, valid));
-        if (lane == 0) pr_mbar_expect_tx(a_bar + 8u * s, cnt * (uint32_t)R::ROW);
-        __syncwarp();
-        if (valid)
-            pr_bulk_g2s(a_ring + (uint32_t)(s * 32 + lane) * R::ROWP, reinterpret_cast<const char*>(blocks) + (size_t)id * R::ROW,
-                        (uint32_t)R::ROW, a_bar + 8u * s);
-    };
-#pragma unroll
-    for (int k = 0; k < R::STAGES; ++k) issue((uint32_t)k);
-
-    for (uint32_t k = 0;; ++k) {
-        const uint32_t batch = wg + k * nw;
-        if (batch >= nb) break;
-        const int s = (int)(k % R::STAGES);
-        pr_mbar_wait(a_bar + 8u * s, (k / R::STAGES) & 1u);
-        const uint32_t r = batch * 32u + lane;
-        if (r < n_vis) {
-            const uint4* row = reinterpret_cast<const uint4*>(s_ring + (size_t)warp * R::WARP_BYTES + (size_t)(s * 32 + lane) * R::ROWP);
-            float q[4], so[4];
-            float cutoff_pre = __uint_as_float(0x7FC00000u);
-            const uint4 pw = row[0];
-            const float4 p4 = make_float4(__uint_as_float(pw.x), __uint_as_float(pw.y), __uint_as_float(pw.z), __uint_as_float(pw.w));
-            if (F16) {
-                const uint4 w = row[1];
-                q[0] = h_hi(w.x); q[1] = h_lo(w.x); q[2] = h_hi(w.y); q[3] = h_lo(w.y);
-                so[0] = h_hi(w.z); so[1] = h_lo(w.z); so[2] = h_hi(w.w); so[3] = h_lo(w.w);
-                if (fc.adaptive) cutoff_pre = __ldg(cutoff_tab + (w.w & 0xFFFFu));
-            } else {
-                const uint4 a = row[1], b = row[2];
-                q[0] = __uint_as_float(a.x); q[1] = __uint_as_float(a.y); q[2] = __uint_as_float(a.z); q[3] = __uint_as_float(a.w);
-                so[0] = __uint_as_float(b.x); so[1] = __uint_as_float(b.y); so[2] = __uint_as_float(b.z); so[3] = __uint_as_float(b.w);
-            }
-            project_one(fc, ctr, r, p4, q, so, cutoff_pre,
-                        [&](float* sh) {
-                            if (F16) {
-#pragma unroll
-                                for (int i = 0; i < 6; ++i) {
-                                    const uint4 v = row[2 + i];
-                                    sh[8 * i] = h_lo(v.x); sh[8 * i + 1] = h_hi(v.x); sh[8 * i + 2] = h_lo(v.y); sh[8 * i + 3] = h_hi(v.y);
-                                    sh[8 * i + 4] = h_lo(v.z); sh[8 * i + 5] = h_hi(v.z); sh[8 * i + 6] = h_lo(v.w); sh[8 * i + 7] = h_hi(v.w);
-                                }
-                            } else {
-#pragma unroll
-                                for (int i = 0; i < 12; ++i) {
-                                    const uint4 v = row[3 + i];
-                                    sh[4 * i] = __uint_as_float(v.x); sh[4 * i + 1] = __uint_as_float(v.y);
-                                    sh[4 * i + 2] = __uint_as_float(v.z); sh[4 * i + 3] = __uint_as_float(v.w);
-                                }
-                            }
-                        },
-                        recs, extra, nullptr);
-        }
-        __syncwarp();                                  // every lane is done with the stage before it is refilled
-        issue(k + (uint32_t)R::STAGES);
-    }
-}
-
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
                         FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream) {
     depth_range_kernel<<<1, 32, 0, stream>>>(pos, n, sorted_payload, slot_ids, ctr, fc);
 }
 
-void launch_project(bool f16, bool blocked, const float4* pos, const void* sh, const void* rot, const void* so,
-                    const uint32_t* index_list, int by_slot, const FrameCounters* ctr, const FrameConsts& fc,
-                    SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, int ctas_per_sm, const float* cutoff_tab,
-                    float4* aux, cudaStream_t stream) {
-    static int use_ring = -1;
-    if (use_ring < 0) { const char* e = getenv("BGS_PROJECT_RING"); use_ring = (e && atoi(e) > 0) ? 1 : 0; }
-    if (blocked && use_ring && aux == nullptr) {
-        // (opt-in with BGS_PROJECT_RING=1: one bulk copy per 128 B row issues slowly enough that the per-thread gather
-        // below has been the faster default)
-        // TMA ring over the gaussian-major blocks (`sh` carries the block array): a persistent grid of at most
-        // ctas_per_sm CTAs per SM (2 when a depth sort shares the SMs, else the occupancy limit)
-        static bool attr_set[64] = {};
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-            cudaFuncSetAttribute(project_ring_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Ring<true>::SMEM);
-            cudaFuncSetAttribute(project_ring_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Ring<false>::SMEM);
-            if (dev >= 0 && dev < 64) attr_set[dev] = true;
-        }
-        const int occ = f16 ? 4 : 3;
-        if (ctas_per_sm <= 0 || ctas_per_sm > occ) ctas_per_sm = occ;
-        uint32_t blocks = (n_hint + PR_THREADS - 1) / PR_THREADS;
-        const uint32_t cap = (uint32_t)(sm_count * ctas_per_sm);
-        if (blocks > cap) blocks = cap;
-        if (blocks == 0) blocks = 1;
-        if (f16) project_ring_kernel<true><<<blocks, PR_THREADS, Ring<true>::SMEM, stream>>>(sh, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab);
-        else project_ring_kernel<false><<<blocks, PR_THREADS, Ring<false>::SMEM, stream>>>(sh, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab);
-        return;
-    }
-    // per-thread gather (gaussian-major blocks by default, the reference's planes with BGS_LAYOUT=planar).  Grid sized from a hint (last frame's visible count +
-    // head-room); the grid-stride loop keeps any n_vis correct.
-    uint32_t blocks = (n_hint + 127) / 128;
-    if (blocks > 65535u * 8u) blocks = 65535u * 8u;
-    if (blocks < (uint32_t)sm_count) blocks = (uint32_t)sm_count;
-    {   // tuning knob: cap the grid at BGS_PROJECT_CTAS CTAs per SM (grid-stride loop; smaller footprint beside other frames)
-        static int cap = -1;
-        if (cap < 0) { const char* e = getenv("BGS_PROJECT_CTAS"); cap = e ? atoi(e) : 0; }
-        if (cap > 0 && blocks > (uint32_t)(cap * sm_count)) blocks = (uint32_t)(cap * sm_count);
-    }
-    // blocked layout: `sh` carries the block array
-    if (f16 && blocked) project_kernel<true, true><<<blocks, 128, 0, stream>>>(pos, sh, rot, so, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
-    else if (f16) project_kernel<true, false><<<blocks, 128, 0, stream>>>(pos, sh, rot, so, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
-    else if (blocked) project_kernel<false, true><<<blocks, 128, 0, stream>>>(pos, sh, rot, so, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
-    else project_kernel<false, false><<<blocks, 128, 0, stream>>>(pos, sh, rot, so, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
+void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+                    const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
+                    const float* cutoff_tab, float4* aux, cudaStream_t stream) {
+    // per-thread gather.  Grid sized from a hint (last frame's visible count + head-room); the grid-stride loop keeps
+    // any n_vis correct.
+    uint32_t grid = (n_hint + 127) / 128;
+    if (grid > 65535u * 8u) grid = 65535u * 8u;
+    if (grid < (uint32_t)sm_count) grid = (uint32_t)sm_count;
+    if (f16) project_kernel<true><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
+    else project_kernel<false><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
 }
 
 }  // namespace bgs

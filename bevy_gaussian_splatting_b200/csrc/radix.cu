@@ -18,8 +18,6 @@
 //   pass over the sorted keys.
 //
 // HBM/L2-bound: per pass 8 B read + 8 B written per entry; histogram phase reads 4 B per entry.
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace bgs {
@@ -28,9 +26,7 @@ constexpr int RS_THREADS = 512;                   // fat CTAs, one (two beyond 8
 constexpr int RS_WARPS = RS_THREADS / 32;         // <= one (two) tiles per SM, so the look-back walks (traffic ~ tiles^2 x 2 KB)
                                                   // stay short; 512 x 64 registers leave half an SM to a concurrent kernel
 constexpr int RS_TABLE_WORDS = RS_WARPS * 256;    // one peer-mask table (all warps)
-#ifndef RS_MIN_CTAS
-#define RS_MIN_CTAS 2
-#endif
+constexpr int RS_MIN_CTAS = 2;                    // two co-resident CTAs per SM: caps the kernel at 64 registers
 constexpr int LB_BATCH = 16;                      // look-back loads in flight per thread
 
 // status word: [63:34] epoch, [33:32] flag (1 = tile aggregate, 2 = inclusive prefix), [31:0] value
@@ -42,9 +38,6 @@ __device__ __forceinline__ unsigned long long ld_status(const unsigned long long
 }
 __device__ __forceinline__ void st_status(unsigned long long* p, unsigned long long v) {
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ void stamp_clk(unsigned long long* tl, int slot) {   // debug: SM cycles, exact intra-CTA deltas
-    if (tl != nullptr && threadIdx.x == 0) tl[slot] = (unsigned long long)clock64();
 }
 
 struct SortParams {
@@ -60,8 +53,6 @@ struct SortParams {
     int shift0;                     // pass p sorts on bits [shift0 + 8p, shift0 + 8p + 8)
     int compute_hist;
     uint2* ranges;                  // non-null: the keys are tile ids; the last pass emits ranges[id] = (~start, end)
-    unsigned long long* tl;         // debug timeline (BGS_TIMELINE_SORT): per tile of pass tl_pass, 8 clock64 stamps
-    int tl_pass;
 };
 
 constexpr size_t radix_smem_bytes(int items) {
@@ -142,8 +133,6 @@ radix_coop_kernel(SortParams P) {
 
         for (uint32_t tile = blockIdx.x; tile < num_tiles; tile += G) {
             const uint32_t tile_base = tile * RS_TILE;
-            unsigned long long* tlt = (P.tl && p == P.tl_pass) ? P.tl + (size_t)(tile < 4096u ? tile : 4095u) * 8 : nullptr;
-            stamp_clk(tlt, 0);
             // warp-striped load: warp w owns [w*32*ITEMS, (w+1)*32*ITEMS) of the tile; item j = 32 consecutive entries
             uint32_t k[RS_ITEMS];
             const uint32_t my_base = tile_base + warp * (32 * RS_ITEMS) + lane;
@@ -189,7 +178,6 @@ radix_coop_kernel(SortParams P) {
                 }
                 rank[j] = old + __popc(peers & lanemask_lt());
             }
-            stamp_clk(tlt, 1);
             __syncthreads();
 
             const uint32_t tile_end = tile_base + RS_TILE;
@@ -238,7 +226,6 @@ radix_coop_kernel(SortParams P) {
                 }
             }
             __syncthreads();
-            stamp_clk(tlt, 2);
 
             // scatter into tile-sorted order in shared memory (the predecessors' words arrive meanwhile; the mask
             // tables aliasing s_keys / s_vals were last touched before the two barriers above)
@@ -250,7 +237,6 @@ radix_coop_kernel(SortParams P) {
                 s_keys[pos] = k[j];
                 s_vals[pos] = (i < n) ? __ldcg(vals_in + i) : 0u;
             }
-            stamp_clk(tlt, 3);
 
             // decoupled look-back: digit d = t & 255 is walked by TWO threads (halves h = t >> 8) that take alternate
             // 16-tile windows of predecessors; the windows of a round are combined in distance order through shared
@@ -296,7 +282,6 @@ radix_coop_kernel(SortParams P) {
             }
             if (t < 256) s_gbase[t] = excl - binstart;
             __syncthreads();
-            stamp_clk(tlt, 4);
 
             // coalesced write-out: consecutive positions of one digit land on consecutive addresses
             const uint32_t valid = RS_TILE - pad;
@@ -313,7 +298,6 @@ radix_coop_kernel(SortParams P) {
                     if (q == valid - 1u || s_keys[q + 1] != kk) atomicMax(&P.ranges[kk].y, dst + 1u);
                 }
             }
-            stamp_clk(tlt, 5);
             __syncthreads();
         }
         if (p + 1 < P.passes) {
@@ -364,13 +348,12 @@ int radix_coop_blocks_per_sm(int) {
 cudaError_t launch_radix_sort(uint32_t* keys0, uint32_t* vals0, uint32_t* keys1, uint32_t* vals1, const uint32_t* n_ptr,
                               uint32_t capacity, uint32_t n_hint, uint32_t* hist, int compute_hist, void* status,
                               size_t status_stride, uint32_t epoch, uint32_t* barrier, int passes, int shift0, uint2* ranges,
-                              int sm_count, int coop_per_sm, cudaStream_t stream, unsigned long long* tl) {
+                              int sm_count, int coop_per_sm, cudaStream_t stream) {
     SortParams P;
     P.keys[0] = keys0; P.keys[1] = keys1; P.vals[0] = vals0; P.vals[1] = vals1;
     P.n_ptr = n_ptr; P.hist = hist; P.status = reinterpret_cast<unsigned long long*>(status); P.status_stride = status_stride;
     P.epoch = epoch; P.barrier = barrier; P.passes = passes; P.shift0 = shift0; P.compute_hist = compute_hist;
-    P.ranges = ranges; P.tl = tl;
-    { const char* e = getenv("BGS_TIMELINE_SORT_PASS"); P.tl_pass = e ? atoi(e) : 1; }
+    P.ranges = ranges;
     if (n_hint > capacity) n_hint = capacity;
     // items per thread so that `waves` waves of tiles cover the expected count with ~3 % head-room (a frame that outgrows
     // it gives some CTAs one more tile: slower, never wrong).  One CTA per SM when the count allows, else two -- unless

@@ -14,8 +14,6 @@
 // Coverage maths uses explicit __fmul_rn/__fmaf_rn so u,v are bit-identical to the oracle.
 #include <cuda_fp16.h>
 
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace bgs {
@@ -626,13 +624,8 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
     if (mode == 0 && large_footprints)
         raster2_kernel<false><<<grid, R2_THREADS, 0, stream>>>(recs, tile_entries, ranges, W, H, tiles_x, out, format,
                                                                nullptr, nullptr, nullptr, 1, 1);
-    else if (mode == 0) {
-        // experiment knob: pad the CTA's shared memory so fewer raster CTAs fit per SM and kernels of another
-        // in-flight frame can co-run (BGS_RASTER_PAD = bytes of dynamic shared memory, default 0)
-        static int pad = -1;
-        if (pad < 0) { const char* e = getenv("BGS_RASTER_PAD"); pad = e ? atoi(e) : 0; }
-        raster_kernel<0, false><<<grid, RT_THREADS, pad, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr);
-    }
+    else if (mode == 0)
+        raster_kernel<0, false><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr);
     else if (mode == 1)
         raster_kernel<1, false><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr);
     else
