@@ -76,10 +76,12 @@ enum {
                                mod.rs:398-452) and a scene behind the splats.  Target = out_rgba when it is a device
                                pointer, else the context's frame (which keeps the previous call's result; frames
                                delivered to host memory are copied out after blending). */
-    BGS_FLAG_CHUNKS = 8u    /* always bin / tile-sort / blend in front-to-back rank rounds that stop emitting
-                               (splat, tile) pairs once every tile has saturated.  Same pixels, bit for bit.
-                               Without either flag the library picks rounds when the previous frame had
-                               >= 32 (splat, tile) pairs per visible splat and >= 2^24 pairs (USE_OBB records only). */
+    BGS_FLAG_CHUNKS = 8u    /* bin / tile-sort / blend in front-to-back rank rounds that stop emitting (splat, tile)
+                               pairs once every tile has saturated.  Same pixels, bit for bit.  Only USE_OBB frames from
+                               bgs_render (not USE_AABB ones, not bgs_render_aux) of at most 65536 tiles are ever split
+                               into rounds; other frames ignore the flag and run one round.  Without either flag the
+                               library picks rounds for such frames when the previous frame had >= 32 (splat, tile)
+                               pairs per visible splat and >= 2^24 pairs. */
 };
 typedef struct {
     uint32_t gaussian_mode;           /* BGS_GAUSSIAN_* */

@@ -1,0 +1,164 @@
+"""Which kernel path a frame takes, restated from libbgs's host code.
+
+libbgs picks launch geometries and kernel variants from a frame's size, the previous frame's counts (the hints),
+whether the frame is queued (BGS_FLAG_ASYNC) and how far the context's buffers have grown.  The results never depend
+on that choice, so a test that renders a frame cannot tell which path it ran.  The functions below restate each rule
+with the lines they mirror, so a test can assert that it reached the path it exists for: if the library's selection
+changes, those assertions fail instead of coverage moving silently.
+
+Constants are the ones in csrc/ (radix.cu, keygen.cu, bin.cu, api.cu).  Nothing here needs a GPU except
+`device_sm_count`.
+"""
+from __future__ import annotations
+
+from typing import NamedTuple
+
+RS_THREADS = 512                 # radix.cu:25
+RS_VARIANTS = (2, 4, 6, 8, 10, 12, 16)   # radix.cu:380-386: radix_coop_kernel<ITEMS, true>
+KG_TILE = 256 * 8                # keygen.cu:16-18: gaussians per key-gen tile
+KG_CHUNK_TILES = 1024 // 64      # keygen.cu:49-50: phase 2 expands 1024 mask words = 16 tiles per chunk
+BIN_SUBTILE_MAX = 256 * 8        # bin.cu:12-13: BIN_THREADS * COOP_ITEMS ranks per sub-tile
+BIN_TINY, BIN_BIG = 4, 128       # bin.cu:14-15: footprint classes (tiles)
+BIN_WARPS_PER_CTA = 256 // 32
+COOP_CTAS_PER_SM, COOP_CTAS_PER_SM_ASYNC = 4, 1   # api.cu:192
+SORT_CTAS_PER_SM_ASYNC = 1       # api.cu:194
+RADIX_CTAS_PER_SM = 2            # radix.cu:29,336: radix_coop_blocks_per_sm() of the 82 KB / 64-register kernel
+CHUNK_MAX_TILES = 65536          # api.cu:186
+TILE_PX = 16                     # common.cuh:10
+H100_SMS = 132
+
+
+class SortPath(NamedTuple):
+    items: int          # items per thread of the kernel that runs (its template ITEMS)
+    match_any: bool     # radix_coop_kernel<16, false>: MATCH.ANY ranking (else the peer-mask ranking)
+    grid: int           # CTAs
+    waves: int          # tiles per CTA the hint plans for
+
+
+def radix_status_rows(capacity: int) -> int:
+    """radix.cu:313-316 (radix_num_tiles): look-back status rows for a sort of up to `capacity` entries."""
+    return max(4096, capacity // (RS_THREADS * 16) + 1)
+
+
+def radix_sort_path(hint: int, capacity: int, sm_count: int = H100_SMS, ctas_per_sm: int = RADIX_CTAS_PER_SM,
+                    status_capacity: int | None = None) -> SortPath:
+    """radix.cu:357-387 (launch_radix_sort).  `capacity`: the sort's buffer capacity; `status_capacity`: what the
+    context's status rows were sized for (api.cu:268-284: the largest cloud / pair capacity seen, default `capacity`)."""
+    hint = min(hint, capacity)
+    want = hint + hint // 32 + 1024
+
+    def items_for(g):
+        per_wave = g * RS_THREADS * 16
+        waves = -(-want // per_wave)
+        return -(-want // (g * RS_THREADS * waves)), waves
+
+    grid = sm_count
+    items, waves = items_for(grid)
+    if waves > 1 and ctas_per_sm >= 2:
+        grid = 2 * sm_count
+        items, waves = items_for(grid)
+    if waves > 3:
+        items = 17
+    rows = radix_status_rows(capacity if status_capacity is None else status_capacity)
+    items = max(items, -(-capacity // (rows * RS_THREADS)))
+    for v in RS_VARIANTS:
+        if items <= v:
+            return SortPath(v, False, grid, waves)
+    return SortPath(16, True, grid, waves)
+
+
+def depth_sort_path(n: int, n_vis_hint: int, sort_all: bool, sm_count: int = H100_SMS, status_n: int | None = None) -> SortPath:
+    """api.cu:745-748: the depth sort of an n-gaussian cloud.  Its hint is n for SORT_ALL frames, else the previous
+    frame's visible count (n when there is none); it always runs with the synchronous CTAs per SM, queued or not."""
+    hint = n if sort_all or n_vis_hint == 0 else n_vis_hint
+    return radix_sort_path(hint, n, sm_count, RADIX_CTAS_PER_SM, status_n)
+
+
+def pair_sort_path(n_pairs_hint: int, cap_pairs: int, queued: bool, sm_count: int = H100_SMS) -> SortPath:
+    """api.cu:797-802: the tile-id sort of a one-round frame.  Its hint is the previous frame's pair count (the pair
+    capacity when there is none); queued frames run SORT_CTAS_PER_SM_ASYNC CTAs per SM."""
+    hint = n_pairs_hint if n_pairs_hint else cap_pairs
+    return radix_sort_path(min(hint, cap_pairs), cap_pairs, sm_count,
+                           SORT_CTAS_PER_SM_ASYNC if queued else RADIX_CTAS_PER_SM)
+
+
+def initial_pair_capacity(n: int) -> int:
+    """api.cu:672-676: the first frame of a context sizes the pair buffer to max(2^20, n)."""
+    return max(1 << 20, n)
+
+
+def grown_pair_capacity(cap_pairs: int, needed: int) -> int:
+    """api.cu:504-512: a frame that needed more pairs than the buffer holds grows it to needed * 1.25 + 1024."""
+    if needed <= cap_pairs:
+        return cap_pairs
+    return min(needed + needed // 4 + 1024, (1 << 30) - 1)
+
+
+def pair_passes(num_tiles: int) -> int:
+    """api.cu:196-200: digit passes of the tile-id sort."""
+    bits = 1
+    while (1 << bits) < num_tiles:
+        bits += 1
+    return (bits + 7) // 8
+
+
+def num_tiles(width: int, height: int) -> int:
+    return -(-width // TILE_PX) * -(-height // TILE_PX)
+
+
+def coop_grid(sm_count: int, ctas_per_sm_fit: int, queued: bool) -> int:
+    """api.cu:350-353: key-gen / binning grid.  `ctas_per_sm_fit`: the kernel's occupancy (cudaOccupancy...)."""
+    return sm_count * min(ctas_per_sm_fit, COOP_CTAS_PER_SM_ASYNC if queued else COOP_CTAS_PER_SM)
+
+
+def keygen_multi_chunk(n: int, grid: int) -> bool:
+    """keygen.cu:64-65,114-116: some CTA's phase 2 expands more than one 1024-word chunk (more than 16 tiles of 2048)."""
+    tiles = -(-n // KG_TILE)
+    return -(-tiles // grid) > KG_CHUNK_TILES
+
+
+def bin_multi_subtile(n_ranks: int, grid: int) -> bool:
+    """bin.cu:69-75: some CTA's rank range is longer than one sub-tile (`!single`): phase 2 reloads its bboxes."""
+    return n_ranks > 0 and -(-n_ranks // grid) > BIN_SUBTILE_MAX
+
+
+def footprint_class(tiles: int) -> str:
+    """bin.cu:166-192: who writes a splat's pairs."""
+    return "none" if tiles == 0 else ("tiny" if tiles <= BIN_TINY else ("medium" if tiles <= BIN_BIG else "large"))
+
+
+def large_split_parts(n_large: int, grid: int) -> int:
+    """bin.cu:235-237: into how many parts each large footprint is cut (1..16)."""
+    total_warps = grid * BIN_WARPS_PER_CTA
+    shift = 0
+    while shift < 4 and (n_large << (shift + 2)) <= total_warps:
+        shift += 1
+    return 1 << shift
+
+
+def large_footprint_raster(n_vis_hint: int, n_pairs_hint: int) -> bool:
+    """api.cu:782: raster2_kernel<false> instead of raster_kernel<0> (USE_OBB frames only)."""
+    return n_vis_hint > 0 and n_pairs_hint >= 8 * n_vis_hint
+
+
+def chunked(tiles: int, raster_mode: int = 0, aux: bool = False, flag: bool | None = None, n_vis_hint: int = 0,
+            n_pairs_hint: int = 0, last_rounds: int = 1) -> bool:
+    """api.cu:703-706: binning rounds.  `flag`: True = BGS_FLAG_CHUNKS, False = BGS_FLAG_NO_CHUNKS, None = neither.
+    Only USE_OBB colour frames of at most 65536 tiles are ever chunked, whatever the flag says."""
+    if raster_mode != 0 or aux or tiles > CHUNK_MAX_TILES or flag is False:
+        return False
+    if flag:
+        return True
+    return (n_vis_hint > 0 and n_pairs_hint >= ((3 << 22) if last_rounds > 1 else (1 << 24))
+            and n_pairs_hint >= (24 if last_rounds > 1 else 32) * n_vis_hint)
+
+
+def raster_lead(start: int) -> int:
+    """raster.cu:53: leading words a tile's first bulk copy skips (its slice start rounded down to 16 B)."""
+    return start & 3
+
+
+def device_sm_count(device: int = 0) -> int:
+    import torch
+
+    return torch.cuda.get_device_properties(device).multi_processor_count

@@ -24,10 +24,25 @@ def _uniform(s):
     return B.GaussianSplattingPlugin.cloud_uniform(s)
 
 
-def check_against_oracle(plugin, oracle, cloud, settings, view, f16=False, pixel_tol=PIXEL_TOL, ref_mode_too=False, cov=False):
+def render_frame(plugin, h, settings, view, asynchronous=False, out=None):
+    """One rgba32f frame.  `asynchronous`: enqueue it (BGS_FLAG_ASYNC), then `sync()`; a frame whose pair list outgrew
+    the buffer is rendered again, as the API asks."""
+    if not asynchronous:
+        return plugin.render_view(h, settings, view, fmt="rgba32f", out=out)
+    if out is None:
+        out = np.empty((view.height, view.width, 4), np.float32)
+    for _ in range(3):
+        plugin.render_view(h, settings, view, fmt="rgba32f", out=out, asynchronous=True)
+        if plugin.sync():
+            return out
+    raise AssertionError("a queued frame kept outgrowing the pair buffer")
+
+
+def check_against_oracle(plugin, oracle, cloud, settings, view, f16=False, pixel_tol=PIXEL_TOL, ref_mode_too=False, cov=False,
+                         asynchronous=False):
     h = plugin.add_cloud(cloud, f16=f16, precompute_covariance=cov)
     try:
-        img = plugin.render_view(h, settings, view, fmt="rgba32f")
+        img = render_frame(plugin, h, settings, view, asynchronous)
         oc = cloud.rounded_to_f16() if f16 else cloud
         if cov:      # row f3: the oracle reads the decoded Covariance3dOpacityPacked128 from the plane slots it occupies
             oc = cloud.precomputed_covariance().rounded_to_f16()
@@ -71,7 +86,7 @@ def check_against_oracle(plugin, oracle, cloud, settings, view, f16=False, pixel
             err_ref = float(np.abs(img - ref).max())
             assert err_ref <= pixel_tol, f"pixel L-inf {err_ref} vs the oracle's ref_mode"
         # the second frame picks kernel variants from the first frame's counts (sort tile size, raster variant)
-        img2 = plugin.render_view(h, settings, view, fmt="rgba32f")
+        img2 = render_frame(plugin, h, settings, view, asynchronous)
         err2 = float(np.abs(img2 - til["image"]).max())
         assert err2 <= pixel_tol, f"pixel L-inf {err2} on the hinted frame"
         if plugin.frame_stats().rounds == 1:   # (a multi-round frame keeps only its last round's ranges)
