@@ -20,6 +20,8 @@ KG_CHUNK_TILES = 1024 // 64      # keygen.cu:49-50: phase 2 expands 1024 mask wo
 BIN_SUBTILE_MAX = 256 * 8        # bin.cu:12-13: BIN_THREADS * COOP_ITEMS ranks per sub-tile
 BIN_TINY, BIN_BIG = 4, 128       # bin.cu:14-15: footprint classes (tiles)
 BIN_WARPS_PER_CTA = 256 // 32
+BIN_CTAS_PER_SM_FIT = 3          # bin.cu:266-270: bin_coop_blocks_per_sm() of the 74-register, 256-thread kernel
+                                 # (registers go in 256 per warp: 80 x 256 = 20 480 per CTA, 3 fit in 65 536)
 COOP_CTAS_PER_SM, COOP_CTAS_PER_SM_ASYNC = 4, 1   # api.cu:192
 SORT_CTAS_PER_SM_ASYNC = 1       # api.cu:194
 RADIX_CTAS_PER_SM = 2            # radix.cu:29,336: radix_coop_blocks_per_sm() of the 82 KB / 64-register kernel
@@ -122,6 +124,14 @@ def bin_multi_subtile(n_ranks: int, grid: int) -> bool:
     return n_ranks > 0 and -(-n_ranks // grid) > BIN_SUBTILE_MAX
 
 
+def bin_subtiles(n_ranks: int, grid: int) -> list[list[tuple[int, int]]]:
+    """bin.cu:69-75: each CTA's rank range [rlo, rhi), cut into sub-tiles of 256 * ipt ranks."""
+    ipt = min(max(-(-(-(-n_ranks // grid)) // 256), 1), 8)
+    sub = 256 * ipt
+    return [[(s, min(s + sub, (b + 1) * n_ranks // grid)) for s in range(b * n_ranks // grid, (b + 1) * n_ranks // grid, sub)]
+            for b in range(grid)]
+
+
 def footprint_class(tiles: int) -> str:
     """bin.cu:166-192: who writes a splat's pairs."""
     return "none" if tiles == 0 else ("tiny" if tiles <= BIN_TINY else ("medium" if tiles <= BIN_BIG else "large"))
@@ -134,6 +144,39 @@ def large_split_parts(n_large: int, grid: int) -> int:
     while shift < 4 and (n_large << (shift + 2)) <= total_warps:
         shift += 1
     return 1 << shift
+
+
+def bin_grid(sm_count: int, queued: bool) -> int:
+    """api.cu:349-353: binning CTAs.  Queued frames run one per SM; synchronous ones min(occupancy, 4) per SM."""
+    return coop_grid(sm_count, BIN_CTAS_PER_SM_FIT, queued)
+
+
+def medium_passes(n_med: int, grid: int) -> int:
+    """bin.cu:203-205: 32-splat batches of the medium queue the busiest warp (global warp 0) drains in phase 3a."""
+    batches = -(-n_med // 32)
+    return -(-batches // (grid * BIN_WARPS_PER_CTA))
+
+
+def large_tickets(n_large: int, grid: int) -> tuple[int, int]:
+    """bin.cu:234-239: (parts per large footprint, most tickets one warp takes); tickets are dealt round-robin over
+    every warp of the grid, so a warp takes a second one once there are more tickets than warps."""
+    parts = large_split_parts(n_large, grid)
+    return parts, -(-(n_large * parts) // (grid * BIN_WARPS_PER_CTA))
+
+
+def large_part_slices(total_all: int, parts: int) -> list[tuple[int, int]]:
+    """bin.cu:248-251: the pair slice [i0, end) of each part of a footprint of `total_all` tiles: `per` is the
+    per-part share rounded up to 32 pairs, so the trailing parts can be short or empty (end == i0)."""
+    per = ((-(-total_all // parts)) + 31) & ~31
+    return [(p * per, min(total_all, p * per + per)) if p * per < total_all else (p * per, p * per) for p in range(parts)]
+
+
+def footprint_rect(xlo: int, xhi: int, ylo: int, yhi: int) -> tuple[int, int, int, int]:
+    """bin.cu:92-93, 180-181: the (tx0, ty0, w, h) tile rectangle of a pixel bbox; (0, 0, 0, 0) when it is empty."""
+    if xlo > xhi or ylo > yhi:
+        return (0, 0, 0, 0)
+    tx0, ty0 = xlo // TILE_PX, ylo // TILE_PX
+    return (tx0, ty0, xhi // TILE_PX - tx0 + 1, yhi // TILE_PX - ty0 + 1)
 
 
 def large_footprint_raster(n_vis_hint: int, n_pairs_hint: int) -> bool:
