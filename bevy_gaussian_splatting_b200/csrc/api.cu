@@ -65,6 +65,35 @@ struct bgs_cloud {
     void* blocks;     // gaussian-major copy of every plane (f16: n * 128 B, f32: n * 256 B), what the projection gathers
 };
 
+// A grow-only device buffer.  grow() replaces a buffer smaller than `want` bytes by one of exactly `want` bytes, zeroed
+// on the render stream when asked; a failed grow leaves it empty.  Its owner (the context) releases it on destruction.
+namespace {
+template <class T>
+struct DevBuf {
+    T* p = nullptr;
+    size_t bytes = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
+    bgs_status grow(bgs_context* c, size_t want, bool zero);
+    void release() { cudaFree(p); p = nullptr; bytes = 0; }
+};
+}  // namespace
+
+// What the host knows of a frame it has enqueued: the context keeps the last one enqueued (`pend`) and, once its
+// counters are back, the last one completed (`last`, what the debug hooks read).
+struct FrameFacts {
+    const bgs_cloud* cloud = nullptr;   // (nulled if the cloud is destroyed meanwhile)
+    uint32_t n = 0;                     // gaussians in the cloud (a snapshot: the cloud may be gone by the time it is read)
+    FrameConsts fc = {};
+    bool sort_all = false;
+    bool by_slot = false;               // records indexed by compact slot (else by front-to-back rank)
+    int rounds = 1;                     // binning rounds
+    int tiles_x = 0, tiles_y = 0, W = 0, H = 0;
+    const void* target = nullptr;       // the device frame the blend wrote
+};
+
 struct bgs_context {
     int device = 0;
     int sm_count = 132;
@@ -79,81 +108,75 @@ struct bgs_context {
     cudaStream_t stream_r = nullptr;  // LOW priority: the tile blend of one-round frames.  With several contexts in flight the
                                       // latency-bound front of the next frame (high priority, cooperative grids) takes SMs as
                                       // the previous frame's short-lived raster CTAs retire, instead of queueing behind them
-    cudaEvent_t ev_front = nullptr, ev_rdone = nullptr;
-    cudaEvent_t ev[6] = {};
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_p0 = nullptr, ev_p1 = nullptr;
+    cudaStream_t stream_copy = nullptr;   // copy/comm stream: D2H copies and gathers of queued frames (default priority)
+    cudaEvent_t ev[6] = {};               // stage boundaries (timed)
+    cudaEvent_t ev_p0 = nullptr, ev_p1 = nullptr;   // the projection's own start / end (timed)
+    cudaEvent_t ev_front = nullptr, ev_rdone = nullptr, ev_fork = nullptr, ev_join = nullptr, ev_done = nullptr;
+    cudaEvent_t ev_raster[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
     uint32_t n_vis_hint = 0;          // last frame's visible count (sizes the projection grid)
     uint32_t n_pairs_hint = 0;        // last frame's pair count (picks the pair sort's tile size); on chunked
                                       // frames an ESTIMATE of what one round would have emitted
     uint32_t chunk_pairs_hint[MAX_CHUNKS] = {};   // last chunked frame's pairs per round (pair sort tile size)
     bool chunk_hint_valid = false;
-    float4* state = nullptr;          // per-pixel blend state between rounds (tile-major), tiles * 256 * 16 B
-    uint32_t cap_state_tiles = 0;
-    unsigned char* tile_done = nullptr;   // in the arena (cleared per frame)
-    int pend_chunks = 1, last_chunks = 1;
     char err[512] = {0};
 
-    // scratch sized by the cloud (grow-only)
+    // scratch sized by the cloud (grow-only; cap_n gaussians)
     uint32_t cap_n = 0;
-    uint32_t* keys[2] = {nullptr, nullptr};
-    uint32_t* vals[2] = {nullptr, nullptr};
-    uint32_t* slot_ids = nullptr;     // compact slot -> gaussian index (key-gen output, index order)
-    SplatRec* recs = nullptr;
-    float4* extra = nullptr;          // 4 x float4 per record: 2DGS + USE_AABB only (allocated on first use)
-    uint32_t cap_extra = 0;
-    float4* aux = nullptr;            // 2 x float4 per record: depth / normal colour sources (bgs_render_aux only)
-    uint32_t cap_aux = 0;
-    void* frame_aux[2] = {nullptr, nullptr};   // depth / normal frames when bgs_render_aux delivers to host memory
-    size_t frame_aux_bytes = 0;
-    // scratch sized by the pair capacity (grow-only)
+    DevBuf<uint32_t> keys[2], vals[2];
+    DevBuf<uint32_t> slot_ids;        // compact slot -> gaussian index (key-gen output, index order)
+    DevBuf<SplatRec> recs;
+    DevBuf<float4> extra;             // 4 x float4 per record: 2DGS + USE_AABB only (allocated on first use)
+    DevBuf<float4> aux;               // 2 x float4 per record: depth / normal colour sources (bgs_render_aux only)
+    DevBuf<void> frame_aux[2];        // depth / normal frames when bgs_render_aux delivers to host memory
+    // scratch sized by the pair capacity (grow-only; cap_pairs pairs)
     uint32_t cap_pairs = 0;
-    uint32_t* pkeys[2] = {nullptr, nullptr};
-    uint32_t* pvals[2] = {nullptr, nullptr};
+    DevBuf<uint32_t> pkeys[2], pvals[2];
+    DevBuf<float4> state;             // per-pixel blend state between rounds (tile-major), tiles * 256 * 16 B
     // zeroed-per-frame arena: counters | hist | keygen CTA counts | bin CTA counts | ranges | done bytes
-    uint8_t* arena = nullptr;
-    size_t arena_bytes = 0;
+    DevBuf<uint8_t> arena;
     uint32_t arena_tiles = 0;
     // look-back status rows of the two sorts (64-bit epoch-tagged words, cleared once at allocation)
-    void* status_depth = nullptr;      // [4][tiles(n)][256]
-    void* status_pairs = nullptr;      // [4][tiles(cap_pairs)][256]
+    DevBuf<void> status_depth;        // [4][tiles(status_n)][256]
+    DevBuf<void> status_pairs;        // [4][tiles(status_np)][256]
     uint32_t status_n = 0, status_np = 0;
     bool async_pending = false;        // a BGS_FLAG_ASYNC frame has been enqueued and not yet completed
-    const bgs_cloud* pend_cloud = nullptr; uint32_t pend_n = 0; FrameConsts pend_fc; bool pend_sort_all = false, pend_by_slot = false;
-    int pend_tiles_x = 0, pend_tiles_y = 0, pend_W = 0, pend_H = 0; const void* pend_target = nullptr;
-    cudaEvent_t ev_done = nullptr;
     FrameCounters* ctr = nullptr;
     uint32_t* hist = nullptr;          // [8 + 4 * MAX_CHUNKS][256]: depth passes 0..3, pair passes 4..7 (round 0), 8 + 4r.. (round r)
     uint32_t* kg_block_cnt = nullptr;  // [kg_grid]: keygen_coop's per-CTA visible counts
     uint32_t* bin_block_cnt = nullptr; // [bin_grid][3]: bin_emit_coop's per-CTA pair / medium / large counts
     uint2* ranges = nullptr;           // per tile (~start, end) into the sorted pair list (0, 0 = empty)
-    // frame
-    void* frame = nullptr;            // frames[0]
-    void* frame_alt = nullptr;        // frames[1]: async frames delivered to host memory alternate targets so
-    size_t frame_bytes = 0;           //            frame k's D2H copy (copy stream) overlaps frame k+1's kernels
+    unsigned char* tile_done = nullptr;   // per tile: saturated (chunked frames)
+    // async frames delivered to host memory alternate the two frames so frame k's D2H copy (copy stream) overlaps
+    // frame k+1's kernels
+    DevBuf<void> frames[2];
     int frame_toggle = 0;
-    cudaStream_t stream_copy = nullptr;
-    cudaEvent_t ev_raster[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
     bool copy_pending[2] = {false, false};
-    const void* last_frame = nullptr;
     FrameCounters* h_ctr = nullptr;    // pinned
+    float* cutoff_tab = nullptr;       // adaptive cutoff of every f16 opacity value (project.cu)
     // largest n_pairs_needed of ANY frame since the last bgs_sync / synchronous render (device word outside the
     // per-frame arena + its pinned copy): a queued async frame that overflowed the pair buffer is never missed
-    float* cutoff_tab = nullptr;       // adaptive cutoff of every f16 opacity value (project.cu)
     uint32_t* d_sticky = nullptr;
     uint32_t* h_sticky = nullptr;
     std::vector<bgs_cloud*> clouds;    // clouds uploaded through this context (their ctx is nulled on destroy)
 
-    // last-frame facts (for the debug hooks)
-    bool have_frame = false;
-    const bgs_cloud* last_cloud = nullptr;
-    FrameConsts last_fc;
-    bool last_sort_all = false;
-    bool last_by_slot = false;        // records indexed by compact slot (else by front-to-back rank)
+    FrameFacts pend, last;
+    bool have_frame = false;           // `last` is valid (for the debug hooks)
     int depth_result = 0, pair_result = 0;   // which ping-pong buffer holds the sorted result
     bgs_frame_stats stats = {};
     float stage_us[6] = {0, 0, 0, 0, 0, 0};
     bool stage_valid = false;
     uint32_t launches = 0;
+
+    // every stream with its priority (0 = highest, 1, 2 = lowest, -1 = the default) and every event with whether it is
+    // timed: bgs_context_create creates them, bgs_context_destroy destroys them
+    template <class F> void each_stream(F f) { f(stream, 0); f(stream2, 1); f(stream_r, 2); f(stream_copy, -1); }
+    template <class F> void each_event(F f) {
+        for (cudaEvent_t& e : ev) f(e, true);
+        f(ev_p0, true); f(ev_p1, true);
+        for (cudaEvent_t* e : {&ev_front, &ev_rdone, &ev_fork, &ev_join, &ev_done, &ev_raster[0], &ev_raster[1],
+                               &ev_copied[0], &ev_copied[1]})
+            f(*e, false);
+    }
 };
 
 namespace {
@@ -181,6 +204,29 @@ bgs_status fail(bgs_context* ctx, bgs_status st, const char* fmt, ...) {
                         cudaGetErrorString(e_));                                                        \
     } while (0)
 
+#define TRY(call)                     \
+    do {                              \
+        const bgs_status s_ = (call); \
+        if (s_ != BGS_OK) return s_;  \
+    } while (0)
+
+template <class T>
+bgs_status DevBuf<T>::grow(bgs_context* c, size_t want, bool zero) {
+    if (want <= bytes) return BGS_OK;
+    release();
+    void* np = nullptr;
+    cudaError_t e = cudaMalloc(&np, want);
+    if (e == cudaSuccess && zero) e = cudaMemsetAsync(np, 0, want, c->stream);
+    if (e != cudaSuccess) {
+        cudaFree(np);
+        return fail(c, e == cudaErrorMemoryAllocation ? BGS_ENOMEM : BGS_ECUDA, "allocating %zu bytes of device scratch: %s",
+                    want, cudaGetErrorString(e));
+    }
+    p = static_cast<T*>(np);
+    bytes = want;
+    return BGS_OK;
+}
+
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 constexpr uint32_t CHUNK_MAX_TILES = 65536;
@@ -201,44 +247,44 @@ int pair_passes(uint32_t num_tiles) {
 
 bgs_status ensure_cloud_scratch(bgs_context* c, uint32_t n) {
     if (n <= c->cap_n) return BGS_OK;
-    for (int i = 0; i < 2; ++i) {
-        cudaFree(c->keys[i]); cudaFree(c->vals[i]);
-        c->keys[i] = c->vals[i] = nullptr;
-    }
-    cudaFree(c->recs); c->recs = nullptr;
-    cudaFree(c->slot_ids); c->slot_ids = nullptr;
     c->cap_n = 0;
     for (int i = 0; i < 2; ++i) {
         // (>= 1024 words: keys[1] doubles as key-gen's visibility-mask scratch, one word per 32 gaussians rounded up to a tile)
-        CU(c, cudaMalloc(&c->keys[i], (size_t)(n < 1024u ? 1024u : n) * 4));
-        CU(c, cudaMalloc(&c->vals[i], (size_t)(n < 1024u ? 1024u : n) * 4));
+        TRY(c->keys[i].grow(c, (size_t)std::max(n, 1024u) * 4, false));
+        TRY(c->vals[i].grow(c, (size_t)std::max(n, 1024u) * 4, false));
     }
-    CU(c, cudaMalloc(&c->slot_ids, (size_t)n * 4));
-    CU(c, cudaMalloc(&c->recs, (size_t)n * sizeof(SplatRec)));
+    TRY(c->slot_ids.grow(c, (size_t)n * 4, false));
+    TRY(c->recs.grow(c, (size_t)n * sizeof(SplatRec), false));
     c->cap_n = n;
     return BGS_OK;
 }
 
 bgs_status ensure_pair_scratch(bgs_context* c, uint32_t pairs) {
     if (pairs <= c->cap_pairs) return BGS_OK;
-    for (int i = 0; i < 2; ++i) {
-        cudaFree(c->pkeys[i]); cudaFree(c->pvals[i]);
-        c->pkeys[i] = c->pvals[i] = nullptr;
-    }
     c->cap_pairs = 0;
     for (int i = 0; i < 2; ++i) {
         // +64 words: the raster's 16 B-granular bulk copies may read a few entries past the last pair
-        CU(c, cudaMalloc(&c->pkeys[i], ((size_t)pairs + 64) * 4));
-        CU(c, cudaMalloc(&c->pvals[i], ((size_t)pairs + 64) * 4));
+        TRY(c->pkeys[i].grow(c, ((size_t)pairs + 64) * 4, false));
+        TRY(c->pvals[i].grow(c, ((size_t)pairs + 64) * 4, false));
     }
     c->cap_pairs = pairs;
     return BGS_OK;
 }
 
+// A frame (one round) needed `needed` pairs: BGS_OK if they fit, else the pair buffer grows (x1.25 head-room) and the
+// frame must be rendered again (BGS_NOT_READY), or BGS_ENOMEM at the 2^30 limit.
+bgs_status grow_pairs(bgs_context* c, uint32_t needed) {
+    if (needed <= c->cap_pairs) return BGS_OK;
+    uint64_t want = (uint64_t)needed + needed / 4 + 1024;
+    if (want >= (1ull << 30)) want = (1ull << 30) - 1;
+    if (needed >= LB_VMASK || want <= c->cap_pairs) return fail(c, BGS_ENOMEM, "render: frame needs >= 2^30 (splat, tile) pairs");
+    TRY(ensure_pair_scratch(c, (uint32_t)want));
+    return BGS_NOT_READY;
+}
+
 bgs_status ensure_arena(bgs_context* c, uint32_t tiles) {
-    if (c->arena && tiles <= c->arena_tiles) return BGS_OK;
-    tiles = tiles > c->arena_tiles ? tiles : c->arena_tiles;
-    cudaFree(c->arena); c->arena = nullptr;
+    if (c->arena.p && tiles <= c->arena_tiles) return BGS_OK;
+    tiles = std::max(tiles, c->arena_tiles);
     size_t off = 0;
     const size_t o_ctr = off; off = align_up(off + sizeof(FrameCounters), 256);
     const size_t o_hist = off; off = align_up(off + (8 + 4 * MAX_CHUNKS) * 256 * 4, 256);
@@ -251,60 +297,131 @@ bgs_status ensure_arena(bgs_context* c, uint32_t tiles) {
     const size_t range_entries = chunk_tiles * MAX_CHUNKS > tiles ? chunk_tiles * MAX_CHUNKS : tiles;
     const size_t o_rng = off; off = align_up(off + range_entries * 8, 256);
     const size_t o_done = off; off = align_up(off + chunk_tiles, 256);
-    CU(c, cudaMalloc(&c->arena, off));
-    c->arena_bytes = off;
-    c->ctr = reinterpret_cast<FrameCounters*>(c->arena + o_ctr);
-    c->hist = reinterpret_cast<uint32_t*>(c->arena + o_hist);
-    c->kg_block_cnt = reinterpret_cast<uint32_t*>(c->arena + o_kgc);
-    c->bin_block_cnt = reinterpret_cast<uint32_t*>(c->arena + o_binc);
-    c->ranges = reinterpret_cast<uint2*>(c->arena + o_rng);
-    c->tile_done = c->arena + o_done;
+    TRY(c->arena.grow(c, off, false));
+    c->ctr = reinterpret_cast<FrameCounters*>(c->arena.p + o_ctr);
+    c->hist = reinterpret_cast<uint32_t*>(c->arena.p + o_hist);
+    c->kg_block_cnt = reinterpret_cast<uint32_t*>(c->arena.p + o_kgc);
+    c->bin_block_cnt = reinterpret_cast<uint32_t*>(c->arena.p + o_binc);
+    c->ranges = reinterpret_cast<uint2*>(c->arena.p + o_rng);
+    c->tile_done = c->arena.p + o_done;
     c->arena_tiles = tiles;
     return BGS_OK;
 }
 
-// look-back status rows of the sorts: 4 passes x tiles x 256 digits x 8 B, epoch-tagged (radix.cu), so they are
-// cleared exactly once -- here -- and never again
-bgs_status ensure_status(bgs_context* c, uint32_t n, uint32_t pairs) {
-    if (n > c->status_n) {
-        cudaFree(c->status_depth); c->status_depth = nullptr; c->status_n = 0;
-        const size_t bytes = (size_t)4 * radix_num_tiles(n) * 256 * 8;
-        CU(c, cudaMalloc(&c->status_depth, bytes));
-        CU(c, cudaMemsetAsync(c->status_depth, 0, bytes, c->stream));
-        c->status_n = n;
-    }
-    if (pairs > c->status_np) {
-        cudaFree(c->status_pairs); c->status_pairs = nullptr; c->status_np = 0;
-        const size_t bytes = (size_t)4 * radix_num_tiles(pairs) * 256 * 8;
-        CU(c, cudaMalloc(&c->status_pairs, bytes));
-        CU(c, cudaMemsetAsync(c->status_pairs, 0, bytes, c->stream));
-        c->status_np = pairs;
-    }
+// look-back status rows of a sort of up to `capacity` entries: 4 passes x tiles x 256 digits x 8 B, epoch-tagged
+// (radix.cu), so they are cleared exactly once -- when allocated -- and never again
+bgs_status ensure_status(bgs_context* c, DevBuf<void>& rows, uint32_t& rows_capacity, uint32_t capacity) {
+    if (capacity <= rows_capacity) return BGS_OK;
+    rows_capacity = 0;
+    TRY(rows.grow(c, (size_t)4 * radix_num_tiles(capacity) * 256 * 8, true));
+    rows_capacity = capacity;
     return BGS_OK;
 }
 
 uint32_t next_epoch(bgs_context* c) {
     if (++c->sort_epoch >= (1u << 30)) {     // (2^30 sorts later) start over from clean rows
-        if (c->status_depth) cudaMemsetAsync(c->status_depth, 0, (size_t)4 * radix_num_tiles(c->status_n) * 256 * 8, c->stream);
-        if (c->status_pairs) cudaMemsetAsync(c->status_pairs, 0, (size_t)4 * radix_num_tiles(c->status_np) * 256 * 8, c->stream);
+        for (DevBuf<void>* s : {&c->status_depth, &c->status_pairs})
+            if (s->p) cudaMemsetAsync(s->p, 0, s->bytes, c->stream);
         c->sort_epoch = 1;
     }
     return c->sort_epoch;
 }
 
-bgs_status ensure_frame(bgs_context* c, size_t bytes) {
-    if (bytes <= c->frame_bytes) return BGS_OK;
-    cudaFree(c->frame); cudaFree(c->frame_alt); c->frame = c->frame_alt = nullptr; c->frame_bytes = 0;
-    CU(c, cudaMalloc(&c->frame, bytes));
-    CU(c, cudaMalloc(&c->frame_alt, bytes));
-    CU(c, cudaMemsetAsync(c->frame, 0, bytes, c->stream));       // (BGS_FLAG_BLEND_OVER_TARGET reads the target)
-    CU(c, cudaMemsetAsync(c->frame_alt, 0, bytes, c->stream));
-    c->frame_bytes = bytes;
-    c->copy_pending[0] = c->copy_pending[1] = false;
-    return BGS_OK;
+size_t format_bpp(uint32_t f) { return f == BGS_FORMAT_RGBA32F ? 16 : (f == BGS_FORMAT_RGBA16F ? 8 : 4); }
+
+// Every choice a frame's launches depend on beyond the frame itself: made from the settings, the previous frame's
+// counts (the hints) and the context's grids and capacities.  plan_frame makes no CUDA call and changes nothing.
+struct FramePlan {
+    int raster_mode;        // 0 = quad-uv falloff (USE_OBB, 3DGS and 2DGS), 1 = 3DGS conic (USE_AABB), 2 = 2DGS ray-splat (USE_AABB)
+    int rounds;             // binning rounds: 1, or MAX_CHUNKS on a chunked frame
+    bool large_fp;          // blend variant for large footprints (results are identical)
+    bool by_slot;           // compact mode: records at recs[slot] (else SORT_ALL: by front-to-back rank)
+    bool depth_range;       // Depth colouring / aux frames: the projection needs sorted[1] / sorted[N-1]
+    bool overlap;           // the projection runs on the second stream beside the depth sort
+    int depth_passes, tile_passes;   // digit places of the depth sort and of the tile-id sort
+    uint32_t kg_grid, bin_grid;      // cooperative key-gen / binning CTAs
+    int pair_sort_per_sm;            // radix-sort CTAs per SM of the tile-id sort
+    uint32_t depth_hint;             // entries the depth sort plans for
+    uint32_t n_hint;                 // records the projection grid plans for
+    uint32_t pair_hint[MAX_CHUNKS];  // pairs each round's tile-id sort plans for
+};
+
+FramePlan plan_frame(const bgs_context* c, const bgs_settings* st, bool want_aux, uint32_t num_tiles, uint32_t n) {
+    FramePlan p;
+    const bool queued = (st->flags & BGS_FLAG_ASYNC) != 0;
+    p.raster_mode = !st->aabb ? 0 : (st->gaussian_mode == BGS_GAUSSIAN_3D ? 1 : 2);
+    // saturation-aware chunking: frames whose splats cover many tiles each (last frame: >= 32 pairs per visible splat
+    // and >= 2^24 pairs: below that, one round is cheaper than the extra launches) run binning / tile sort /
+    // blend in front-to-back rank rounds; the rounds after every tile has saturated emit nothing.
+    // Quad-uv records only; BGS_FLAG_CHUNKS / _NO_CHUNKS force it.
+    bool chunked = p.raster_mode == 0 && !want_aux && num_tiles <= CHUNK_MAX_TILES && !(st->flags & BGS_FLAG_NO_CHUNKS);
+    if (chunked && !(st->flags & BGS_FLAG_CHUNKS))
+        chunked = c->n_vis_hint > 0 && c->n_pairs_hint >= (c->last.rounds > 1 ? 3u << 22 : 1u << 24) &&
+                  (uint64_t)c->n_pairs_hint >= (c->last.rounds > 1 ? 24ull : 32ull) * c->n_vis_hint;   // (hysteresis)
+    p.rounds = chunked ? MAX_CHUNKS : 1;
+    // kernel variant picked from the previous frame's mean footprint (pairs per visible splat)
+    p.large_fp = c->n_vis_hint > 0 && (uint64_t)c->n_pairs_hint >= 8ull * c->n_vis_hint;
+    p.by_slot = !(st->flags & BGS_FLAG_SORT_ALL);
+    p.depth_range = st->rasterize_mode == BGS_RASTERIZE_DEPTH || want_aux;
+    p.overlap = p.by_slot && !p.depth_range;
+    p.depth_passes = (int)st->radix_sort_depth_bits / 8;
+    p.tile_passes = pair_passes(num_tiles);
+    p.kg_grid = queued ? c->kg_grid_async : c->kg_grid;
+    p.bin_grid = queued ? c->bin_grid_async : c->bin_grid;
+    p.pair_sort_per_sm = queued ? SORT_CTAS_PER_SM_ASYNC : c->rs_per_sm;
+    p.depth_hint = !p.by_slot ? n : (c->n_vis_hint ? c->n_vis_hint : n);
+    p.n_hint = std::min(c->n_vis_hint ? c->n_vis_hint + c->n_vis_hint / 4 + 1024 : n, n);
+    for (int r = 0; r < p.rounds; ++r) {
+        uint32_t h = c->n_pairs_hint ? c->n_pairs_hint : c->cap_pairs;
+        if (p.rounds > 1) h = c->chunk_hint_valid ? c->chunk_pairs_hint[r] : c->cap_pairs;
+        p.pair_hint[r] = std::min(h, c->cap_pairs);
+    }
+    return p;
 }
 
-size_t format_bpp(uint32_t f) { return f == BGS_FORMAT_RGBA32F ? 16 : (f == BGS_FORMAT_RGBA16F ? 8 : 4); }
+// Where a frame's pixels go.
+struct FrameOut {
+    void* rgba = nullptr;               // the blend's target (device): the caller's frame or one of the library's
+    void* depth = nullptr;              // bgs_render_aux's depth / normal targets (device)
+    void* normal = nullptr;
+    uint32_t raster_format = 0;         // output mode of the blend kernels: format | mode << 8 (raster.cu)
+    size_t bytes = 0;                   // of one frame
+    int slot = -1;                      // a queued frame in the library's own frames: which of the two (else -1)
+    void* host_rgba = nullptr;          // host frames the result is copied to
+    void* host_depth = nullptr;
+    void* host_normal = nullptr;
+};
+
+// the caller's device frames, or the library's own (grown on demand)
+bgs_status frame_out(bgs_context* c, const bgs_settings* st, uint32_t format, size_t bytes, void* out_rgba,
+                     int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal, FrameOut* o) {
+    const bool blend_over = (st->flags & BGS_FLAG_BLEND_OVER_TARGET) != 0;
+    o->raster_format = format | ((blend_over ? 2u : ((st->flags & BGS_FLAG_PREMULTIPLIED_OUT) ? 1u : 0u)) << 8);
+    o->bytes = bytes;
+    if (out_rgba && out_is_device_ptr) {
+        o->rgba = out_rgba;
+    } else {
+        for (int k = 0; k < 2; ++k) {
+            if (bytes <= c->frames[k].bytes) continue;
+            TRY(c->frames[k].grow(c, bytes, true));      // (BGS_FLAG_BLEND_OVER_TARGET reads the target)
+            c->copy_pending[k] = false;
+        }
+        // async frames rendered into the library's own buffers alternate two device frames, so whatever consumes
+        // frame k off the render stream (the D2H copy, the NCCL gather: both on the copy/comm stream) overlaps frame k+1
+        if (st->flags & BGS_FLAG_ASYNC) {
+            if (blend_over) o->slot = c->frame_toggle ^ 1;            // keep blending into the frame the previous call produced
+            else { o->slot = c->frame_toggle; c->frame_toggle ^= 1; }
+        }
+        o->rgba = c->frames[std::max(o->slot, 0)].p;
+        o->host_rgba = out_rgba;
+    }
+    if (!want_aux) return BGS_OK;
+    if (out_is_device_ptr) { o->depth = out_depth; o->normal = out_normal; return BGS_OK; }
+    for (int k = 0; k < 2; ++k) TRY(c->frame_aux[k].grow(c, bytes, true));
+    o->depth = c->frame_aux[0].p; o->normal = c->frame_aux[1].p;
+    o->host_depth = out_depth; o->host_normal = out_normal;
+    return BGS_OK;
+}
 
 }  // namespace
 
@@ -319,22 +436,13 @@ bgs_status bgs_context_create(int cuda_device, bgs_context** out) {
     cudaError_t e = cudaSetDevice(cuda_device);
     int prio_lo = 0, prio_hi = 0;
     if (e == cudaSuccess) e = cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_hi);
-    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->stream2, cudaStreamNonBlocking, (prio_lo + prio_hi) / 2);
-    if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&c->stream_r, cudaStreamNonBlocking, prio_lo);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_front, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_rdone, cudaEventDisableTiming);
-    for (int i = 0; i < 6 && e == cudaSuccess; ++i) e = cudaEventCreate(&c->ev[i]);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream_copy, cudaStreamNonBlocking);
-    for (int i = 0; i < 2 && e == cudaSuccess; ++i) {
-        e = cudaEventCreateWithFlags(&c->ev_raster[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_copied[i], cudaEventDisableTiming);
-    }
-    if (e == cudaSuccess) e = cudaEventCreate(&c->ev_p0);
-    if (e == cudaSuccess) e = cudaEventCreate(&c->ev_p1);
+    const int prio[3] = {prio_hi, (prio_lo + prio_hi) / 2, prio_lo};
+    c->each_stream([&](cudaStream_t& s, int rank) {
+        if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, rank < 0 ? 0 : prio[rank]);
+    });
+    c->each_event([&](cudaEvent_t& ev, bool timed) {
+        if (e == cudaSuccess) e = timed ? cudaEventCreate(&ev) : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+    });
     if (e == cudaSuccess) e = cudaMallocHost(&c->h_ctr, sizeof(FrameCounters));
     if (e == cudaSuccess) e = cudaMallocHost(&c->h_sticky, 16);
     if (e == cudaSuccess) e = cudaMalloc(&c->d_sticky, 16);
@@ -382,30 +490,14 @@ void bgs_context_destroy(bgs_context* c) {
         c->clouds.clear();
     }
     cudaSetDevice(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    if (c->stream2) cudaStreamSynchronize(c->stream2);
-    if (c->stream_r) { cudaStreamSynchronize(c->stream_r); cudaStreamDestroy(c->stream_r); }
-    if (c->ev_front) cudaEventDestroy(c->ev_front);
-    if (c->ev_rdone) cudaEventDestroy(c->ev_rdone);
-    if (c->stream_copy) { cudaStreamSynchronize(c->stream_copy); cudaStreamDestroy(c->stream_copy); }
-    for (int i = 0; i < 2; ++i) { if (c->ev_raster[i]) cudaEventDestroy(c->ev_raster[i]); if (c->ev_copied[i]) cudaEventDestroy(c->ev_copied[i]); }
-    cudaFree(c->frame_alt);
-    for (int i = 0; i < 2; ++i) {
-        cudaFree(c->keys[i]); cudaFree(c->vals[i]); cudaFree(c->pkeys[i]); cudaFree(c->pvals[i]);
-    }
-    cudaFree(c->state);
-    cudaFree(c->aux); cudaFree(c->frame_aux[0]); cudaFree(c->frame_aux[1]);
-    cudaFree(c->recs); cudaFree(c->extra); cudaFree(c->slot_ids); cudaFree(c->arena); cudaFree(c->frame);
+    c->each_stream([](cudaStream_t& s, int) { if (s) cudaStreamSynchronize(s); });
+    c->each_event([](cudaEvent_t& ev, bool) { if (ev) cudaEventDestroy(ev); });
+    c->each_stream([](cudaStream_t& s, int) { if (s) cudaStreamDestroy(s); });
     if (c->h_ctr) cudaFreeHost(c->h_ctr);
     if (c->h_sticky) cudaFreeHost(c->h_sticky);
     cudaFree(c->d_sticky);
     cudaFree(c->cutoff_tab);
-    for (int i = 0; i < 6; ++i) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
-    for (cudaEvent_t e : {c->ev_fork, c->ev_join, c->ev_p0, c->ev_p1, c->ev_done}) if (e) cudaEventDestroy(e);
-    cudaFree(c->status_depth); cudaFree(c->status_pairs);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    if (c->stream2) cudaStreamDestroy(c->stream2);
-    delete c;
+    delete c;   // (releases every DevBuf)
 }
 
 static bgs_status upload_common(bgs_context* ctx, uint32_t n, bool f16, const float* pos_vis, const void* sh,
@@ -474,15 +566,10 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
         // that still read the planes are drained first, the debug hooks lose their frame
         std::lock_guard<std::mutex> lk(g_registry_mu);
         for (bgs_context* c : g_contexts) {
-            if (c->pend_cloud == cl || c->last_cloud == cl) {
-                if (c->async_pending || c->pend_cloud == cl) {
-                    cudaStreamSynchronize(c->stream);
-                    cudaStreamSynchronize(c->stream2);
-                    cudaStreamSynchronize(c->stream_r);
-                    cudaStreamSynchronize(c->stream_copy);
-                }
-                if (c->pend_cloud == cl) { c->pend_cloud = nullptr; c->pend_n = 0; }
-                if (c->last_cloud == cl) { c->last_cloud = nullptr; c->have_frame = false; }
+            if (c->pend.cloud == cl || c->last.cloud == cl) {
+                if (c->async_pending || c->pend.cloud == cl) c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
+                if (c->pend.cloud == cl) { c->pend.cloud = nullptr; c->pend.n = 0; }
+                if (c->last.cloud == cl) { c->last.cloud = nullptr; c->have_frame = false; }
             }
             c->clouds.erase(std::remove(c->clouds.begin(), c->clouds.end(), cl), c->clouds.end());
         }
@@ -493,7 +580,7 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
 
 // Bookkeeping once a frame's counters are back on the host (sync render, or bgs_sync after async ones).
 static bgs_status finish_frame(bgs_context* c) {
-    const int chunks = c->pend_chunks;
+    const int chunks = c->pend.rounds;
     uint32_t needed = 0;
     uint64_t emitted = 0;
     for (int r = 0; r < chunks; ++r) {
@@ -501,24 +588,15 @@ static bgs_status finish_frame(bgs_context* c) {
         needed = cc.n_pairs_needed > needed ? cc.n_pairs_needed : needed;
         emitted += cc.n_pairs;
     }
-    if (needed > c->cap_pairs) {
-        // the pair list (of one round) did not fit: grow (x1.25 head-room); the caller redoes the frame
-        uint64_t want = (uint64_t)needed + needed / 4 + 1024;
-        if (want >= (1ull << 30)) want = (1ull << 30) - 1;
-        if (needed >= LB_VMASK || want <= c->cap_pairs)
-            return fail(c, BGS_ENOMEM, "render: frame needs >= 2^30 (splat, tile) pairs");
-        bgs_status s = ensure_pair_scratch(c, (uint32_t)want);
-        if (s != BGS_OK) return s;
-        return BGS_NOT_READY;
-    }
-    const uint32_t n = c->pend_n;   // (snapshot: the cloud may have been destroyed since the frame was queued)
+    TRY(grow_pairs(c, needed));   // (the pair list of one round did not fit: the caller redoes the frame)
+    c->last = c->pend;
+    c->have_frame = true;
     c->stage_valid = false;
-    c->stats.n = n; c->stats.n_visible = c->h_ctr->n_vis; c->stats.n_pairs = emitted;
+    c->stats.n = c->last.n; c->stats.n_visible = c->h_ctr->n_vis; c->stats.n_pairs = emitted;
     c->stats.rounds = (uint32_t)chunks; c->stats.tiles_saturated = c->h_ctr->tiles_done;
-    c->stats.tiles_x = (uint32_t)c->pend_tiles_x; c->stats.tiles_y = (uint32_t)c->pend_tiles_y;
-    c->stats.width = (uint32_t)c->pend_W; c->stats.height = (uint32_t)c->pend_H;
-    c->have_frame = true; c->last_cloud = c->pend_cloud; c->last_fc = c->pend_fc; c->last_sort_all = c->pend_sort_all;
-    c->last_by_slot = c->pend_by_slot; c->n_vis_hint = c->h_ctr->n_vis; c->last_chunks = chunks;
+    c->stats.tiles_x = (uint32_t)c->last.tiles_x; c->stats.tiles_y = (uint32_t)c->last.tiles_y;
+    c->stats.width = (uint32_t)c->last.W; c->stats.height = (uint32_t)c->last.H;
+    c->n_vis_hint = c->h_ctr->n_vis;
     if (chunks > 1) {
         // the rounds emitted in full, scaled up to the whole visible set (the nearest splats have the largest
         // footprints, so this errs towards staying chunked)
@@ -533,7 +611,6 @@ static bgs_status finish_frame(bgs_context* c) {
         c->n_pairs_hint = c->h_ctr->chunk[0].n_pairs;
         c->chunk_hint_valid = false;
     }
-    c->last_frame = c->pend_target;
     c->err[0] = 0;
     return BGS_OK;
 }
@@ -550,44 +627,21 @@ bgs_status bgs_sync(bgs_context* c) {
     // the sticky maximum covers EVERY frame queued since the last sync, not just the last one (whose counters are
     // in h_ctr): any of them that needed more pairs than the buffer holds was blended from a truncated list
     const uint32_t worst = c->h_sticky[0];
-    const bool earlier_overflow = worst > c->cap_pairs;
     c->h_sticky[0] = 0;
     CU(c, cudaMemsetAsync(c->d_sticky, 0, 4, c->stream));
     const bgs_status s = finish_frame(c);
     if (s == BGS_NOT_READY) return fail(c, BGS_NOT_READY, "an async frame outgrew the pair buffer (now grown): render the frames queued since the last bgs_sync again");
-    if (s == BGS_OK && earlier_overflow) {
-        uint64_t want = (uint64_t)worst + worst / 4 + 1024;
-        if (want >= (1ull << 30)) want = (1ull << 30) - 1;
-        if (worst >= LB_VMASK || want <= c->cap_pairs) return fail(c, BGS_ENOMEM, "render: frame needs >= 2^30 (splat, tile) pairs");
-        const bgs_status gs = ensure_pair_scratch(c, (uint32_t)want);
-        if (gs != BGS_OK) return gs;
+    if (s != BGS_OK) return s;
+    const bgs_status gs = grow_pairs(c, worst);
+    if (gs == BGS_NOT_READY) {
         c->have_frame = false;
         return fail(c, BGS_NOT_READY, "an earlier async frame (not the last one) outgrew the pair buffer (now grown): every frame queued since the last bgs_sync may be truncated, render them again");
     }
-    return s;
+    return gs;
 }
 
-static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                              const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr,
-                              bool want_aux, void* out_depth, void* out_normal);
-
-bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                      const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
-    return render_impl(c, cloud, view, uni, st, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr);
-}
-
-bgs_status bgs_render_aux(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                          const bgs_settings* st, void* out_rgba, void* out_depth, void* out_normal, uint32_t out_format,
-                          int out_is_device_ptr) {
-    if (c && (!out_rgba || !out_depth || !out_normal)) return fail(c, BGS_EINVAL, "render_aux: the three output frames are required");
-    if (c && st && (st->flags & BGS_FLAG_ASYNC)) return fail(c, BGS_EINVAL, "render_aux: BGS_FLAG_ASYNC is not supported");
-    return render_impl(c, cloud, view, uni, st, out_rgba, out_format, out_is_device_ptr, true, out_depth, out_normal);
-}
-
-static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                              const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr,
-                              bool want_aux, void* out_depth, void* out_normal) {
-    if (!c) return BGS_EINVAL;
+static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                               const bgs_settings* st, uint32_t out_format, bool want_aux) {
     // not-ready inputs map to the reference's silent skip-frame (radix.rs:645-658, mod.rs:1533-1539)
     if (!cloud || !view || !uni || !st) return fail(c, BGS_NOT_READY, "render: cloud/view/uniform/settings not ready");
     if (cloud->device != c->device)     // (cloud->ctx may be gone: clouds outlive the context that uploaded them)
@@ -604,21 +658,12 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         return fail(c, BGS_EINVAL, "render: a precomputed-covariance cloud has no rotation / scale: Gaussian3d with Color, Depth or Position only");
     const int W = (int)view->viewport[2], H = (int)view->viewport[3];
     if (W <= 0 || H <= 0 || W > 65535 || H > 65535) return fail(c, BGS_EINVAL, "render: viewport %dx%d out of range", W, H);
-    CU(c, cudaSetDevice(c->device));
-    if (c->async_pending && !(st->flags & BGS_FLAG_ASYNC)) {
-        // a synchronous render after queued frames completes them first; their failure (including an overflowed
-        // pair list = BGS_NOT_READY) is the caller's to see, so this frame is not rendered on top of it
-        const bgs_status ps = bgs_sync(c);
-        if (ps != BGS_OK) return ps;
-    }
+    return BGS_OK;
+}
 
-    const uint32_t n = cloud->n;
-    const int tiles_x = (W + TILE_PX - 1) / TILE_PX, tiles_y = (H + TILE_PX - 1) / TILE_PX;
-    const uint32_t num_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
-    const int depth_passes = (int)st->radix_sort_depth_bits / 8;
-    const int tile_passes = pair_passes(num_tiles);
-    const bool sort_all = (st->flags & BGS_FLAG_SORT_ALL) != 0;
-
+static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                                const bgs_settings* st, bool want_aux) {
+    const int W = (int)view->viewport[2], H = (int)view->viewport[3];
     FrameConsts fc;
     memcpy(fc.model, uni->transform, 64);
     memcpy(fc.view_from_world, view->view_from_world, 64);
@@ -631,260 +676,211 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     fc.key_shift = 32u - st->radix_sort_depth_bits;
     fc.gaussian_mode = st->gaussian_mode; fc.rasterize_mode = st->rasterize_mode; fc.aabb = st->aabb;
     fc.adaptive = st->opacity_adaptive_radius; fc.draw_mode = st->draw_mode;
-    fc.Wi = W; fc.Hi = H; fc.tiles_x = tiles_x; fc.tiles_y = tiles_y;
-    fc.n_cloud = n;
+    fc.Wi = W; fc.Hi = H; fc.tiles_x = (W + TILE_PX - 1) / TILE_PX; fc.tiles_y = (H + TILE_PX - 1) / TILE_PX;
+    fc.n_cloud = cloud->n;
     fc.aux = want_aux ? 1u : 0u;
     fc.cov_pre = cloud->cov ? 1u : 0u;
     memcpy(fc.aabb_min, uni->aabb_min, 12); memcpy(fc.aabb_max, uni->aabb_max, 12);
     static const float kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
     fc.model_identity = memcmp(uni->transform, kIdentity, 64) == 0 ? 1u : 0u;   // (-0.0 entries take the general path)
+    return fc;
+}
 
-    bgs_status s = ensure_cloud_scratch(c, n);
-    if (s != BGS_OK) return s;
-    // raster variant: 0 = quad-uv falloff (USE_OBB, 3DGS and 2DGS), 1 = 3DGS conic (USE_AABB), 2 = 2DGS ray-splat (USE_AABB)
-    const int raster_mode = !st->aabb ? 0 : (st->gaussian_mode == BGS_GAUSSIAN_3D ? 1 : 2);
-    if (raster_mode == 2 && c->cap_extra < c->cap_n) {
-        cudaFree(c->extra); c->extra = nullptr; c->cap_extra = 0;
-        CU(c, cudaMalloc(&c->extra, (size_t)c->cap_n * 64));
-        c->cap_extra = c->cap_n;
+// Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.
+static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const FramePlan& p,
+                                const FrameOut& o) {
+    const uint32_t n = cloud->n;
+    const uint32_t num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
+    cudaStream_t q = c->stream;
+    uint32_t launches = 0;
+    CU(c, cudaMemsetAsync(c->arena.p, 0, c->arena.bytes, q));   // counters, histograms, ranges: ~0.4 MB
+    CU(c, cudaEventRecord(c->ev[0], q));
+    // ---- stage 1: key-gen (+ stable compaction of the visible set)
+    // compact mode: keys[0][slot], slot_ids[slot] = gaussian index, vals[0][slot] = slot (sort payload)
+    // SORT_ALL    : keys[0][i], vals[0][i] = i (payload is the gaussian index itself)
+    if (p.by_slot) {
+        // the cooperative key-gen also produces the depth sort's digit histograms
+        // (keys[1] = visibility-mask scratch until the sort's first pass overwrites it)
+        CU(c, launch_keygen_coop(cloud->pos, n, fc, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt,
+                                 c->ctr, c->hist, p.depth_passes, p.kg_grid, q));
+    } else {
+        launch_keygen_all(cloud->pos, n, fc, c->keys[0].p, c->vals[0].p, c->ctr, q);
     }
-    void* tgt_depth = nullptr; void* tgt_normal = nullptr;
-    if (want_aux) {
-        if (c->cap_aux < c->cap_n) {
-            cudaFree(c->aux); c->aux = nullptr; c->cap_aux = 0;
-            CU(c, cudaMalloc(&c->aux, (size_t)c->cap_n * 32));
-            c->cap_aux = c->cap_n;
+    ++launches;
+    CU(c, cudaEventRecord(c->ev[1], q));
+    if (p.overlap) CU(c, cudaEventRecord(c->ev_fork, q));
+    // ---- stage 2: depth radix sort: all P = depth_bits / 8 digit places in ONE cooperative launch (enqueued before
+    //      the projection so its one-CTA-per-SM grid becomes resident first; the projection fills the other half)
+    CU(c, launch_radix_sort(c->keys[0].p, c->vals[0].p, c->keys[1].p, c->vals[1].p, &c->ctr->n_sort, n, p.depth_hint,
+                            c->hist, p.by_slot ? 0 : 1, c->status_depth.p, (size_t)radix_num_tiles(c->status_n) * 256,
+                            next_epoch(c), &c->ctr->barrier[1], p.depth_passes, 0, nullptr, c->sm_count, c->rs_per_sm, q));
+    ++launches;
+    const int cur = p.depth_passes & 1;
+    c->depth_result = cur;
+    CU(c, cudaEventRecord(c->ev[2], q));
+    // ---- stage 3: projection + colour.  Compact mode: in slot order on the second stream, concurrently with the depth
+    //      sort (it only needs slot_ids); records land at recs[slot].  After the sort: SORT_ALL (records by front-to-back
+    //      rank), or Depth colouring / aux frames (by slot), which need the depth range of the sorted set first
+    const cudaStream_t ps = p.overlap ? c->stream2 : q;
+    if (p.overlap) CU(c, cudaStreamWaitEvent(c->stream2, c->ev_fork, 0));
+    if (p.depth_range) {
+        launch_depth_range(cloud->pos, n, c->vals[cur].p, p.by_slot ? c->slot_ids.p : nullptr, c->ctr, fc, q);
+        ++launches;
+    }
+    CU(c, cudaEventRecord(c->ev_p0, ps));
+    launch_project(cloud->f16, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
+                   c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
+                   fc.aux ? c->aux.p : nullptr, ps);
+    ++launches;
+    CU(c, cudaEventRecord(c->ev_p1, ps));
+    if (p.overlap) {
+        CU(c, cudaEventRecord(c->ev_join, c->stream2));
+        CU(c, cudaStreamWaitEvent(q, c->ev_join, 0));
+    }
+    CU(c, cudaEventRecord(c->ev[3], q));
+    // ---- stage 4: tile binning -> stable tile-id sort -> ranges; stage 5: per-tile front-to-back blend.
+    //      One round normally; `rounds` front-to-back rank rounds on chunked frames, each resuming the pixels'
+    //      blend state, the last one writing the frame (identical pixels either way).
+    int pcur = 0;
+    for (int r = 0; r < p.rounds; ++r) {
+        ChunkCounters* cc = &c->ctr->chunk[r];
+        const uint32_t fa = p.rounds > 1 ? CHUNK_FRAC[r] : 0u, fb = p.rounds > 1 ? CHUNK_FRAC[r + 1] : 65536u;
+        uint2* rng = c->ranges + (size_t)r * num_tiles;
+        uint32_t* hist_r = c->hist + (size_t)(4 + 4 * r) * 256;
+        // the depth sort's spare ping-pong buffers (N words each) hold the large-footprint queue
+        CU(c, launch_bin_emit_coop(c->recs.p, p.by_slot ? c->vals[cur].p : nullptr, c->ctr, cc, fa, fb, num_tiles,
+                                   c->bin_block_cnt, fc.tiles_x, c->cap_pairs, c->pkeys[0].p, c->pvals[0].p,
+                                   c->keys[cur ^ 1].p, c->vals[cur ^ 1].p, c->cap_n, p.bin_grid, c->d_sticky, q));
+        ++launches;
+        // stable tile-id sort of the pair list + per-tile ranges: histogram phase, both digit places and the range
+        // build in ONE cooperative launch
+        CU(c, launch_radix_sort(c->pkeys[0].p, c->pvals[0].p, c->pkeys[1].p, c->pvals[1].p, &cc->n_pairs, c->cap_pairs,
+                                p.pair_hint[r], hist_r, 1, c->status_pairs.p, (size_t)radix_num_tiles(c->status_np) * 256,
+                                next_epoch(c), &cc->sort_barrier, p.tile_passes, 0, rng, c->sm_count, p.pair_sort_per_sm, q));
+        ++launches;
+        pcur = p.tile_passes & 1;
+        if (r + 1 == p.rounds) {
+            // (chunked frames: the earlier rounds' blends are accounted to stage 4)
+            CU(c, cudaEventRecord(c->ev[4], q));
+            if (o.slot >= 0 && c->copy_pending[o.slot]) CU(c, cudaStreamWaitEvent(q, c->ev_copied[o.slot], 0));   // target free again
         }
-        if (out_is_device_ptr) { tgt_depth = out_depth; tgt_normal = out_normal; }
-        else {
-            const size_t fb = (size_t)W * H * format_bpp(out_format);
-            if (fb > c->frame_aux_bytes) {
-                cudaFree(c->frame_aux[0]); cudaFree(c->frame_aux[1]); c->frame_aux[0] = c->frame_aux[1] = nullptr; c->frame_aux_bytes = 0;
-                CU(c, cudaMalloc(&c->frame_aux[0], fb));
-                CU(c, cudaMalloc(&c->frame_aux[1], fb));
-                CU(c, cudaMemsetAsync(c->frame_aux[0], 0, fb, c->stream));
-                CU(c, cudaMemsetAsync(c->frame_aux[1], 0, fb, c->stream));
-                c->frame_aux_bytes = fb;
-            }
-            tgt_depth = c->frame_aux[0]; tgt_normal = c->frame_aux[1];
+        if (p.rounds == 1) {
+            // the blend runs on the LOW-priority stream; the render stream resumes once it is done
+            CU(c, cudaEventRecord(c->ev_front, q));
+            CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
+            launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
+                          fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal, c->stream_r);
+            CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
+            CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
+        } else
+            launch_raster_round(c->recs.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x, fc.tiles_y, o.rgba, o.raster_format,
+                                c->state.p, c->tile_done, &c->ctr->tiles_done, r == 0, r + 1 == p.rounds, q);
+        ++launches;
+    }
+    c->pair_result = pcur;
+    CU(c, cudaEventRecord(c->ev[5], q));
+    CU(c, cudaEventRecord(c->ev_done, q));
+    CU(c, cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, q));
+    CU(c, cudaMemcpyAsync(c->h_sticky, c->d_sticky, 4, cudaMemcpyDeviceToHost, q));
+    if (o.slot >= 0) CU(c, cudaEventRecord(c->ev_raster[o.slot], q));
+    if (o.slot >= 0 && o.host_rgba) {
+        CU(c, cudaStreamWaitEvent(c->stream_copy, c->ev_raster[o.slot], 0));
+        CU(c, cudaMemcpyAsync(o.host_rgba, o.rgba, o.bytes, cudaMemcpyDeviceToHost, c->stream_copy));
+        CU(c, cudaEventRecord(c->ev_copied[o.slot], c->stream_copy));
+        c->copy_pending[o.slot] = true;
+    } else if (o.host_rgba) {
+        CU(c, cudaMemcpyAsync(o.host_rgba, o.rgba, o.bytes, cudaMemcpyDeviceToHost, q));
+        if (o.host_depth) {
+            CU(c, cudaMemcpyAsync(o.host_depth, o.depth, o.bytes, cudaMemcpyDeviceToHost, q));
+            CU(c, cudaMemcpyAsync(o.host_normal, o.normal, o.bytes, cudaMemcpyDeviceToHost, q));
         }
     }
-    if (c->cap_pairs == 0) {
-        uint32_t init = n < (1u << 20) ? (1u << 20) : n;   // first guess; grows on demand
-        s = ensure_pair_scratch(c, init);
-        if (s != BGS_OK) return s;
-    }
-    const size_t frame_bytes = (size_t)W * H * format_bpp(out_format);
-    void* target = c->frame;
-    if (out_rgba && out_is_device_ptr) target = out_rgba;
-    else {
-        s = ensure_frame(c, frame_bytes);
-        if (s != BGS_OK) return s;
-        target = c->frame;
-    }
-    // async frames rendered into the library's own buffers alternate two device frames, so whatever consumes
-    // frame k off the render stream (the D2H copy, the NCCL gather: both on the copy/comm stream) overlaps frame k+1
-    const bool async_own = (st->flags & BGS_FLAG_ASYNC) && !(out_rgba && out_is_device_ptr);
-    const bool async_host = async_own && out_rgba;
-    // output mode of the blend kernels: format | mode << 8 (raster.cu)
-    const bool blend_over = (st->flags & BGS_FLAG_BLEND_OVER_TARGET) != 0;
-    const uint32_t raster_format = out_format | ((blend_over ? 2u : ((st->flags & BGS_FLAG_PREMULTIPLIED_OUT) ? 1u : 0u)) << 8);
-    int fslot = 0;
-    if (async_own) {
-        if (blend_over) fslot = c->frame_toggle ^ 1;            // keep blending into the frame the previous call produced
-        else { fslot = c->frame_toggle; c->frame_toggle ^= 1; }
-        target = fslot ? c->frame_alt : c->frame;
-    }
+    c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, fc.tiles_x, fc.tiles_y, fc.Wi, fc.Hi, o.rgba};
+    c->launches = launches;
+    return BGS_OK;
+}
 
-    // saturation-aware chunking: frames whose splats cover many tiles each (last frame: >= 32 pairs per visible splat
-    // and >= 2^24 pairs: below that, one round is cheaper than the extra launches) run binning / tile sort /
-    // blend in front-to-back rank rounds; the rounds after every tile has saturated emit nothing.
-    // Quad-uv records only; BGS_FLAG_CHUNKS / _NO_CHUNKS force it.
-    bool chunked = raster_mode == 0 && !want_aux && num_tiles <= CHUNK_MAX_TILES && !(st->flags & BGS_FLAG_NO_CHUNKS);
-    if (chunked && !(st->flags & BGS_FLAG_CHUNKS))
-        chunked = c->n_vis_hint > 0 && c->n_pairs_hint >= (c->last_chunks > 1 ? 3u << 22 : 1u << 24) &&
-                  (uint64_t)c->n_pairs_hint >= (c->last_chunks > 1 ? 24ull : 32ull) * c->n_vis_hint;   // (hysteresis)
-    const int rounds = chunked ? MAX_CHUNKS : 1;
-    if (chunked && c->cap_state_tiles < num_tiles) {
-        cudaFree(c->state); c->state = nullptr; c->cap_state_tiles = 0;
-        CU(c, cudaMalloc(&c->state, (size_t)num_tiles * 256 * sizeof(float4)));
-        c->cap_state_tiles = num_tiles;
+static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                              const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr,
+                              bool want_aux, void* out_depth, void* out_normal) {
+    if (!c) return BGS_EINVAL;
+    TRY(check_render(c, cloud, view, uni, st, out_format, want_aux));
+    CU(c, cudaSetDevice(c->device));
+    if (c->async_pending && !(st->flags & BGS_FLAG_ASYNC)) {
+        // a synchronous render after queued frames completes them first; their failure (including an overflowed
+        // pair list = BGS_NOT_READY) is the caller's to see, so this frame is not rendered on top of it
+        TRY(bgs_sync(c));
     }
-
+    const FrameConsts fc = frame_consts(cloud, view, uni, st, want_aux);
+    const uint32_t n = cloud->n, num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
+    TRY(ensure_cloud_scratch(c, n));
+    if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
+    FrameOut o;
+    TRY(frame_out(c, st, out_format, (size_t)fc.Wi * fc.Hi * format_bpp(out_format), out_rgba, out_is_device_ptr, want_aux,
+                  out_depth, out_normal, &o));
     for (int attempt = 0; attempt < 4; ++attempt) {
-        s = ensure_arena(c, num_tiles);
-        if (s != BGS_OK) return s;
-        s = ensure_status(c, n, c->cap_pairs);
-        if (s != BGS_OK) return s;
-        cudaStream_t q = c->stream;
-        uint32_t launches = 0;
-        CU(c, cudaMemsetAsync(c->arena, 0, c->arena_bytes, q));   // counters, histograms, ranges: ~0.4 MB
-        CU(c, cudaEventRecord(c->ev[0], q));
-        // ---- stage 1: key-gen (+ stable compaction of the visible set)
-        // compact mode: keys[0][slot], slot_ids[slot] = gaussian index, vals[0][slot] = slot (sort payload)
-        // SORT_ALL    : keys[0][i], vals[0][i] = i (payload is the gaussian index itself)
-        const bool by_slot = !sort_all;
-        if (by_slot) {
-            // the cooperative key-gen also produces the depth sort's digit histograms
-            // (keys[1] = visibility-mask scratch until the sort's first pass overwrites it)
-            CU(c, launch_keygen_coop(cloud->pos, n, fc, c->keys[1], c->keys[0], c->slot_ids, c->vals[0], c->kg_block_cnt,
-                                     c->ctr, c->hist, depth_passes, (st->flags & BGS_FLAG_ASYNC) ? c->kg_grid_async : c->kg_grid, q));
-        } else {
-            launch_keygen_all(cloud->pos, n, fc, c->keys[0], c->vals[0], c->ctr, q);
-        }
-        ++launches;
-        CU(c, cudaEventRecord(c->ev[1], q));
-        // ---- stage 3 (compact mode): projection + colour in slot order on the second stream, concurrently
-        //      with the depth sort (it only needs slot_ids); records land at recs[slot]
-        const uint32_t n_hint = c->n_vis_hint ? c->n_vis_hint + c->n_vis_hint / 4 + 1024 : n;
-        // Depth colouring needs sorted[1] / sorted[N-1]: the projection then waits for the sort
-        const bool overlap = by_slot && st->rasterize_mode != BGS_RASTERIZE_DEPTH && !want_aux;
-        if (overlap) CU(c, cudaEventRecord(c->ev_fork, q));
-        // ---- stage 2: depth radix sort: all P = depth_bits / 8 digit places in ONE cooperative launch (enqueued before
-        //      the projection so its one-CTA-per-SM grid becomes resident first; the projection fills the other half)
-        CU(c, launch_radix_sort(c->keys[0], c->vals[0], c->keys[1], c->vals[1], &c->ctr->n_sort, n,
-                                sort_all ? n : (c->n_vis_hint ? c->n_vis_hint : n), c->hist, sort_all ? 1 : 0, c->status_depth,
-                                (size_t)radix_num_tiles(c->status_n) * 256, next_epoch(c), &c->ctr->barrier[1], depth_passes, 0,
-                                nullptr, c->sm_count, c->rs_per_sm, q));
-        ++launches;
-        if (overlap) {
-            CU(c, cudaStreamWaitEvent(c->stream2, c->ev_fork, 0));
-            CU(c, cudaEventRecord(c->ev_p0, c->stream2));
-            launch_project(cloud->f16, cloud->blocks, c->slot_ids, 1, c->ctr, fc, c->recs, raster_mode == 2 ? c->extra : nullptr,
-                           n_hint < n ? n_hint : n, c->sm_count, c->cutoff_tab, nullptr, c->stream2);
-            ++launches;
-            CU(c, cudaEventRecord(c->ev_p1, c->stream2));
-            CU(c, cudaEventRecord(c->ev_join, c->stream2));
-        }
-        const int cur = depth_passes & 1;
-        c->depth_result = cur;
-        CU(c, cudaEventRecord(c->ev[2], q));
-        if (overlap) {
-            CU(c, cudaStreamWaitEvent(q, c->ev_join, 0));
-        } else {
-            // ---- stage 3 after the sort: SORT_ALL (records by front-to-back rank) or Depth colouring (by slot)
-            if (st->rasterize_mode == BGS_RASTERIZE_DEPTH || want_aux) {
-                launch_depth_range(cloud->pos, n, c->vals[cur], by_slot ? c->slot_ids : nullptr, c->ctr, fc, q);
-                ++launches;
-            }
-            CU(c, cudaEventRecord(c->ev_p0, q));
-            launch_project(cloud->f16, cloud->blocks, by_slot ? c->slot_ids : c->vals[cur], by_slot ? 1 : 0, c->ctr, fc, c->recs,
-                           raster_mode == 2 ? c->extra : nullptr, n_hint < n ? n_hint : n, c->sm_count, c->cutoff_tab,
-                           want_aux ? c->aux : nullptr, q);
-            ++launches;
-            CU(c, cudaEventRecord(c->ev_p1, q));
-        }
-        CU(c, cudaEventRecord(c->ev[3], q));
-        // ---- stage 4: tile binning -> stable tile-id sort -> ranges; stage 5: per-tile front-to-back blend.
-        //      One round normally; `rounds` front-to-back rank rounds on chunked frames, each resuming the pixels'
-        //      blend state, the last one writing the frame (identical pixels either way).
-        // kernel variant picked from the previous frame's mean footprint (pairs per visible splat); results are identical
-        const bool large_fp = c->n_vis_hint > 0 && (uint64_t)c->n_pairs_hint >= 8ull * c->n_vis_hint;
-        int pcur = 0;
-        for (int r = 0; r < rounds; ++r) {
-            ChunkCounters* cc = &c->ctr->chunk[r];
-            const uint32_t fa = rounds > 1 ? CHUNK_FRAC[r] : 0u, fb = rounds > 1 ? CHUNK_FRAC[r + 1] : 65536u;
-            uint2* rng = c->ranges + (size_t)r * num_tiles;
-            uint32_t* hist_r = c->hist + (size_t)(4 + 4 * r) * 256;
-            // the depth sort's spare ping-pong buffers (N words each) hold the large-footprint queue
-            CU(c, launch_bin_emit_coop(c->recs, by_slot ? c->vals[cur] : nullptr, c->ctr, cc, fa, fb, num_tiles,
-                                       c->bin_block_cnt, tiles_x, c->cap_pairs, c->pkeys[0], c->pvals[0], c->keys[cur ^ 1],
-                                       c->vals[cur ^ 1], c->cap_n, (st->flags & BGS_FLAG_ASYNC) ? c->bin_grid_async : c->bin_grid,
-                                       c->d_sticky, q));
-            ++launches;
-            // stable tile-id sort of the pair list + per-tile ranges: histogram phase, both digit places and the range
-            // build in ONE cooperative launch
-            uint32_t p_hint = c->n_pairs_hint ? c->n_pairs_hint : c->cap_pairs;
-            if (rounds > 1) p_hint = c->chunk_hint_valid ? c->chunk_pairs_hint[r] : c->cap_pairs;
-            if (p_hint > c->cap_pairs) p_hint = c->cap_pairs;
-            CU(c, launch_radix_sort(c->pkeys[0], c->pvals[0], c->pkeys[1], c->pvals[1], &cc->n_pairs, c->cap_pairs, p_hint, hist_r, 1,
-                                    c->status_pairs, (size_t)radix_num_tiles(c->status_np) * 256, next_epoch(c), &cc->sort_barrier,
-                                    tile_passes, 0, rng, c->sm_count, (st->flags & BGS_FLAG_ASYNC) ? SORT_CTAS_PER_SM_ASYNC : c->rs_per_sm, q));
-            ++launches;
-            pcur = tile_passes & 1;
-            if (r + 1 == rounds) {
-                // (chunked frames: the earlier rounds' blends are accounted to stage 4)
-                CU(c, cudaEventRecord(c->ev[4], q));
-                if (async_own && c->copy_pending[fslot]) CU(c, cudaStreamWaitEvent(q, c->ev_copied[fslot], 0));   // target free again
-            }
-            if (rounds == 1) {
-                // the blend runs on the LOW-priority stream; the render stream resumes once it is done
-                CU(c, cudaEventRecord(c->ev_front, q));
-                CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
-                launch_raster(raster_mode, large_fp, c->recs, c->extra, c->pvals[pcur], rng, W, H, tiles_x, tiles_y, target, raster_format,
-                              want_aux ? c->aux : nullptr, tgt_depth, tgt_normal, c->stream_r);
-                CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
-                CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
-            } else
-                launch_raster_round(c->recs, c->pvals[pcur], rng, W, H, tiles_x, tiles_y, target, raster_format, c->state,
-                                    c->tile_done, &c->ctr->tiles_done, r == 0, r + 1 == rounds, q);
-            ++launches;
-        }
-        c->pair_result = pcur;
-        CU(c, cudaEventRecord(c->ev[5], q));
-        CU(c, cudaEventRecord(c->ev_done, q));
-        CU(c, cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, q));
-        CU(c, cudaMemcpyAsync(c->h_sticky, c->d_sticky, 4, cudaMemcpyDeviceToHost, q));
-        if (async_own) CU(c, cudaEventRecord(c->ev_raster[fslot], q));
-        if (async_host) {
-            CU(c, cudaStreamWaitEvent(c->stream_copy, c->ev_raster[fslot], 0));
-            CU(c, cudaMemcpyAsync(out_rgba, target, frame_bytes, cudaMemcpyDeviceToHost, c->stream_copy));
-            CU(c, cudaEventRecord(c->ev_copied[fslot], c->stream_copy));
-            c->copy_pending[fslot] = true;
-        } else if (out_rgba && !out_is_device_ptr) {
-            CU(c, cudaMemcpyAsync(out_rgba, target, frame_bytes, cudaMemcpyDeviceToHost, q));
-            if (want_aux) {
-                CU(c, cudaMemcpyAsync(out_depth, tgt_depth, frame_bytes, cudaMemcpyDeviceToHost, q));
-                CU(c, cudaMemcpyAsync(out_normal, tgt_normal, frame_bytes, cudaMemcpyDeviceToHost, q));
-            }
-        }
-        c->pend_cloud = cloud; c->pend_n = n; c->pend_fc = fc; c->pend_sort_all = sort_all; c->pend_by_slot = by_slot;
-        c->pend_chunks = rounds;
-        c->pend_tiles_x = tiles_x; c->pend_tiles_y = tiles_y; c->pend_W = W; c->pend_H = H; c->pend_target = target;
+        const FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
+        if (p.raster_mode == 2) TRY(c->extra.grow(c, (size_t)c->cap_n * 64, false));
+        if (want_aux) TRY(c->aux.grow(c, (size_t)c->cap_n * 32, false));
+        if (p.rounds > 1) TRY(c->state.grow(c, (size_t)num_tiles * 256 * sizeof(float4), false));
+        TRY(ensure_arena(c, num_tiles));
+        TRY(ensure_status(c, c->status_depth, c->status_n, n));
+        TRY(ensure_status(c, c->status_pairs, c->status_np, c->cap_pairs));
+        TRY(enqueue_frame(c, cloud, fc, p, o));
         if (st->flags & BGS_FLAG_ASYNC) {
-            c->launches = launches;
             c->async_pending = true;
             c->have_frame = false;     // hooks need bgs_sync() first
             return BGS_OK;
         }
-        CU(c, cudaStreamSynchronize(q));
+        CU(c, cudaStreamSynchronize(c->stream));
         CU(c, cudaGetLastError());
-        c->launches = launches;
         c->h_sticky[0] = 0;
-        CU(c, cudaMemsetAsync(c->d_sticky, 0, 4, q));   // synchronous frames report their own overflow right here
+        CU(c, cudaMemsetAsync(c->d_sticky, 0, 4, c->stream));   // synchronous frames report their own overflow right here
         const bgs_status fs = finish_frame(c);
-        if (fs == BGS_NOT_READY) continue;   // pair buffer grown: redo the frame
-        return fs;
+        if (fs != BGS_NOT_READY) return fs;   // (BGS_NOT_READY: pair buffer grown, redo the frame)
     }
     return fail(c, BGS_ENOMEM, "render: pair list kept overflowing");
 }
 
+bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                      const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    return render_impl(c, cloud, view, uni, st, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr);
+}
+
+bgs_status bgs_render_aux(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                          const bgs_settings* st, void* out_rgba, void* out_depth, void* out_normal, uint32_t out_format,
+                          int out_is_device_ptr) {
+    if (c && (!out_rgba || !out_depth || !out_normal)) return fail(c, BGS_EINVAL, "render_aux: the three output frames are required");
+    if (c && st && (st->flags & BGS_FLAG_ASYNC)) return fail(c, BGS_EINVAL, "render_aux: BGS_FLAG_ASYNC is not supported");
+    return render_impl(c, cloud, view, uni, st, out_rgba, out_format, out_is_device_ptr, true, out_depth, out_normal);
+}
+
 bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {
     if (!c || !out) return BGS_EINVAL;
-    if (!c->have_frame || !c->last_cloud) return fail(c, BGS_NOT_READY, "no frame rendered yet");
+    if (!c->have_frame || !c->last.cloud) return fail(c, BGS_NOT_READY, "no frame rendered yet");
     CU(c, cudaSetDevice(c->device));
-    const uint32_t n = c->last_cloud->n, n_vis = c->stats.n_visible;
-    const uint32_t n_sorted = c->last_sort_all ? n : n_vis;
+    const uint32_t n = c->last.cloud->n, n_vis = c->stats.n_visible;
+    const uint32_t n_sorted = c->last.sort_all ? n : n_vis;
     std::vector<uint32_t> k(n_sorted), v(n_sorted);
-    CU(c, cudaMemcpy(k.data(), c->keys[c->depth_result], (size_t)n_sorted * 4, cudaMemcpyDeviceToHost));
-    CU(c, cudaMemcpy(v.data(), c->vals[c->depth_result], (size_t)n_sorted * 4, cudaMemcpyDeviceToHost));
-    if (c->last_by_slot) {   // the sort's payload is the compact slot: map it to the gaussian index
+    CU(c, cudaMemcpy(k.data(), c->keys[c->depth_result].p, (size_t)n_sorted * 4, cudaMemcpyDeviceToHost));
+    CU(c, cudaMemcpy(v.data(), c->vals[c->depth_result].p, (size_t)n_sorted * 4, cudaMemcpyDeviceToHost));
+    if (c->last.by_slot) {   // the sort's payload is the compact slot: map it to the gaussian index
         std::vector<uint32_t> ids(n_sorted);
-        CU(c, cudaMemcpy(ids.data(), c->slot_ids, (size_t)n_sorted * 4, cudaMemcpyDeviceToHost));
+        CU(c, cudaMemcpy(ids.data(), c->slot_ids.p, (size_t)n_sorted * 4, cudaMemcpyDeviceToHost));
         for (uint32_t i = 0; i < n_sorted; ++i) v[i] = ids[v[i]];
     }
     for (uint32_t i = 0; i < n_sorted; ++i) { out[2 * i] = k[i]; out[2 * i + 1] = v[i]; }
-    if (!c->last_sort_all) {
+    if (!c->last.sort_all) {
         // culled tail: key = all-ones >> shift, indices ascending (what a stable sort leaves there)
         uint32_t* flags = nullptr;
         CU(c, cudaMalloc(&flags, (size_t)n * 4));
-        launch_culled_flags(c->last_cloud->pos, n, c->last_fc, flags, c->stream);
+        launch_culled_flags(c->last.cloud->pos, n, c->last.fc, flags, c->stream);
         std::vector<uint32_t> f(n);
         cudaError_t e = cudaMemcpyAsync(f.data(), flags, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         cudaFree(flags);
         if (e != cudaSuccess) return fail(c, BGS_ECUDA, "debug_sorted_entries: %s", cudaGetErrorString(e));
-        const uint32_t culled_key = 0xFFFFFFFFu >> c->last_fc.key_shift;
+        const uint32_t culled_key = 0xFFFFFFFFu >> c->last.fc.key_shift;
         uint32_t at = n_vis;
         for (uint32_t i = 0; i < n; ++i)
             if (f[i]) {
@@ -899,7 +895,7 @@ bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {
 bgs_status bgs_debug_tile_ranges(bgs_context* c, uint32_t* start_end) {
     if (!c || !start_end) return BGS_EINVAL;
     if (!c->have_frame) return fail(c, BGS_NOT_READY, "no frame rendered yet");
-    if (c->last_chunks > 1) return fail(c, BGS_NOT_READY, "the last frame was binned in %d rounds: set BGS_FLAG_NO_CHUNKS for the tile hooks", c->last_chunks);
+    if (c->last.rounds > 1) return fail(c, BGS_NOT_READY, "the last frame was binned in %d rounds: set BGS_FLAG_NO_CHUNKS for the tile hooks", c->last.rounds);
     CU(c, cudaSetDevice(c->device));
     const size_t tiles = (size_t)c->stats.tiles_x * c->stats.tiles_y;
     CU(c, cudaMemcpy(start_end, c->ranges, tiles * 8, cudaMemcpyDeviceToHost));
@@ -914,14 +910,14 @@ bgs_status bgs_debug_tile_ranges(bgs_context* c, uint32_t* start_end) {
 bgs_status bgs_debug_tile_entries(bgs_context* c, uint32_t* ranks, uint64_t capacity) {
     if (!c || !ranks) return BGS_EINVAL;
     if (!c->have_frame) return fail(c, BGS_NOT_READY, "no frame rendered yet");
-    if (c->last_chunks > 1) return fail(c, BGS_NOT_READY, "the last frame was binned in %d rounds: set BGS_FLAG_NO_CHUNKS for the tile hooks", c->last_chunks);
+    if (c->last.rounds > 1) return fail(c, BGS_NOT_READY, "the last frame was binned in %d rounds: set BGS_FLAG_NO_CHUNKS for the tile hooks", c->last.rounds);
     CU(c, cudaSetDevice(c->device));
     const uint64_t cnt = c->stats.n_pairs < capacity ? c->stats.n_pairs : capacity;
-    CU(c, cudaMemcpy(ranks, c->pvals[c->pair_result], (size_t)cnt * 4, cudaMemcpyDeviceToHost));
-    if (c->last_by_slot) {   // pair payload = record index = compact slot: convert to front-to-back rank
+    CU(c, cudaMemcpy(ranks, c->pvals[c->pair_result].p, (size_t)cnt * 4, cudaMemcpyDeviceToHost));
+    if (c->last.by_slot) {   // pair payload = record index = compact slot: convert to front-to-back rank
         const uint32_t n_vis = c->stats.n_visible;
         std::vector<uint32_t> perm(n_vis), inv(n_vis);
-        CU(c, cudaMemcpy(perm.data(), c->vals[c->depth_result], (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
+        CU(c, cudaMemcpy(perm.data(), c->vals[c->depth_result].p, (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
         for (uint32_t r = 0; r < n_vis; ++r) inv[perm[n_vis - 1 - r]] = r;
         for (uint64_t i = 0; i < cnt; ++i) ranks[i] = ranks[i] < n_vis ? inv[ranks[i]] : 0xFFFFFFFFu;
     }
@@ -934,21 +930,21 @@ bgs_status bgs_debug_projected(bgs_context* c, float* records, uint32_t* rank_to
     CU(c, cudaSetDevice(c->device));
     const uint32_t n_vis = c->stats.n_visible;
     std::vector<uint32_t> v(n_vis), ids;
-    CU(c, cudaMemcpy(v.data(), c->vals[c->depth_result], (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
-    if (c->last_by_slot) {
+    CU(c, cudaMemcpy(v.data(), c->vals[c->depth_result].p, (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
+    if (c->last.by_slot) {
         ids.resize(n_vis);
-        CU(c, cudaMemcpy(ids.data(), c->slot_ids, (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
+        CU(c, cudaMemcpy(ids.data(), c->slot_ids.p, (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
     }
     if (records) {
         std::vector<SplatRec> tmp(n_vis);
-        CU(c, cudaMemcpy(tmp.data(), c->recs, (size_t)n_vis * sizeof(SplatRec), cudaMemcpyDeviceToHost));
+        CU(c, cudaMemcpy(tmp.data(), c->recs.p, (size_t)n_vis * sizeof(SplatRec), cudaMemcpyDeviceToHost));
         for (uint32_t r = 0; r < n_vis; ++r) {
-            const uint32_t ri = c->last_by_slot ? v[n_vis - 1 - r] : r;   // rank -> record index
+            const uint32_t ri = c->last.by_slot ? v[n_vis - 1 - r] : r;   // rank -> record index
             memcpy(records + (size_t)r * 12, &tmp[ri], sizeof(SplatRec));
         }
     }
     if (rank_to_index)
-        for (uint32_t r = 0; r < n_vis; ++r) rank_to_index[r] = c->last_by_slot ? ids[v[n_vis - 1 - r]] : v[n_vis - 1 - r];
+        for (uint32_t r = 0; r < n_vis; ++r) rank_to_index[r] = c->last.by_slot ? ids[v[n_vis - 1 - r]] : v[n_vis - 1 - r];
     return BGS_OK;
 }
 
@@ -989,7 +985,7 @@ cudaStream_t bgs_internal_gather_begin_(bgs_context* c, const void* local_frame,
     *slot = -1;
     if (!c) return nullptr;
     for (int k = 0; k < 2; ++k) {
-        const void* f = k ? c->frame_alt : c->frame;
+        const void* f = c->frames[k].p;
         if (f && f == local_frame && c->async_pending) {
             if (cudaStreamWaitEvent(c->stream_copy, c->ev_raster[k], 0) != cudaSuccess) return c->stream;
             *slot = k;
@@ -1008,7 +1004,7 @@ void* bgs_context_stream(bgs_context* c) { return c ? (void*)c->stream : nullptr
 void* bgs_context_copy_stream(bgs_context* c) { return c ? (void*)c->stream_copy : nullptr; }
 const void* bgs_frame_device_ptr(bgs_context* c) {
     if (!c) return nullptr;
-    return c->have_frame ? c->last_frame : (c->async_pending ? c->pend_target : nullptr);
+    return c->have_frame ? c->last.target : (c->async_pending ? c->pend.target : nullptr);
 }
 uint32_t bgs_last_launch_count(const bgs_context* c) { return c ? c->launches : 0; }
 
