@@ -429,21 +429,27 @@ inline void depth_to_rgb(float depth, float dmin, float dmax, float rgb[3]) {
     rgb[2] = 1.0f - smooth(0.0f, 0.5f, nd);
 }
 
-// ---- fs_main (gaussian.wgsl:439-505) evaluated at pixel centre (fx, fy); returns coverage
-inline bool eval_alpha(const orc_splat& sp, const orc_settings& s, float fx, float fy, float* alpha) {
+// ---- fs_main (gaussian.wgsl:439-505) at pixel centre (fx, fy): the quantities the coverage decision turns on.
+// `fused` = false computes u, v with a separately rounded multiply and add (what a kernel without the explicit fma
+// would do); the decision is then `covered`, and `power` is filled only for covered pixels.
+struct Decision { float u, v, mx, my, Rq, power; bool covered; };
+inline Decision decide(const orc_splat& sp, const orc_settings& s, float fx, float fy, bool fused = true) {
+    Decision d{0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, false};
     const float dx = fx - sp.cx, dy = fy - sp.cy;
     float power;
     if (!s.aabb) {
         // USE_OBB: uv from the quad, power = -|uv|^2 / (2/9)
-        const float uu = std::fmaf(sp.uy, dy, sp.ux * dx);
-        const float vv = std::fmaf(sp.vy, dy, sp.vx * dx);
-        if (!(std::fabs(uu) <= 1.0f && std::fabs(vv) <= 1.0f)) return false;
+        d.u = fused ? std::fmaf(sp.uy, dy, sp.ux * dx) : sp.ux * dx + sp.uy * dy;
+        d.v = fused ? std::fmaf(sp.vy, dy, sp.vx * dx) : sp.vx * dx + sp.vy * dy;
+        const float uu = d.u, vv = d.v;
+        if (!(std::fabs(uu) <= 1.0f && std::fabs(vv) <= 1.0f)) return d;
         const float qd = std::fmaf(vv, vv, uu * uu);
         power = -4.5f * qd;
     } else {
         const float mx = dx + dx, my = -(dy + dy);      // quad-space offset in half-pixels (y up)
         const float Rq = sp.extra[3];
-        if (!(std::fabs(mx) <= Rq && std::fabs(my) <= Rq)) return false;
+        d.mx = mx; d.my = my; d.Rq = Rq;
+        if (!(std::fabs(mx) <= Rq && std::fabs(my) <= Rq)) return d;
         if (s.gaussian_mode == 1u) {
             const float ddx = -mx, ddy = -my;            // gaussian.wgsl:459-462
             const float t1 = (sp.extra[0] * ddx) * ddx, t2 = (sp.extra[2] * ddy) * ddy;
@@ -463,9 +469,21 @@ inline bool eval_alpha(const orc_splat& sp, const orc_settings& s, float fx, flo
             const float s2 = 2.0f * (ex * ex + ey * ey);
             power = -(0.5f * std::fmin(s3, s2));
         }
-        if (power > 0.0f) return false;                  // gaussian.wgsl:468-470
+        d.power = power;
+        if (power > 0.0f) return d;                      // gaussian.wgsl:468-470
     }
-    *alpha = std::fmin(std::exp(power) * sp.op, 0.999f);
+    d.power = power;
+    d.covered = true;
+    return d;
+}
+
+inline float alpha_of(const orc_splat& sp, float power) { return std::fmin(std::exp(power) * sp.op, 0.999f); }
+
+// returns coverage; *alpha = min(exp(power) * opacity, 0.999) where covered
+inline bool eval_alpha(const orc_splat& sp, const orc_settings& s, float fx, float fy, float* alpha) {
+    const Decision d = decide(sp, s, fx, fy);
+    if (!d.covered) return false;
+    *alpha = alpha_of(sp, d.power);
     return true;
 }
 
@@ -515,6 +533,28 @@ void build_frame(const Ctx& C, uint32_t n, const float* pos, const float* sh, co
                 F.splats[r].r = rgb[0]; F.splats[r].g = rgb[1]; F.splats[r].b = rgb[2];
             }
         }
+    }
+}
+
+// a7: per-tile slice of the global order: every splat whose pixel bbox touches the tile, in front-to-back rank
+// order.  count[t] .. count[t + 1] is tile t's slice of `entries` (ranks).
+void bin_tiles(const Frame& F, int TX, int TY, std::vector<uint64_t>& count, std::vector<uint32_t>& entries) {
+    const int NT = TX * TY;
+    count.assign((size_t)NT + 1, 0);
+    for (uint32_t r = 0; r < F.n_vis; ++r) {
+        const orc_splat& sp = F.splats[r];
+        if (sp.xlo > sp.xhi) continue;
+        for (int ty = sp.ylo / TILE; ty <= sp.yhi / TILE; ++ty)
+            for (int tx = sp.xlo / TILE; tx <= sp.xhi / TILE; ++tx) count[(size_t)ty * TX + tx + 1]++;
+    }
+    for (int t = 0; t < NT; ++t) count[t + 1] += count[t];
+    entries.resize(count[NT]);
+    std::vector<uint64_t> cur(count.begin(), count.end() - 1);
+    for (uint32_t r = 0; r < F.n_vis; ++r) {
+        const orc_splat& sp = F.splats[r];
+        if (sp.xlo > sp.xhi) continue;
+        for (int ty = sp.ylo / TILE; ty <= sp.yhi / TILE; ++ty)
+            for (int tx = sp.xlo / TILE; tx <= sp.xhi / TILE; ++tx) entries[cur[(size_t)ty * TX + tx]++] = r;
     }
 }
 
@@ -731,30 +771,13 @@ int orc_render_tiles(uint32_t n, const float* pos_vis, const float* sh, const fl
     const int W = C.Wi, H = C.Hi;
     const int TX = (W + TILE - 1) / TILE, TY = (H + TILE - 1) / TILE;
     const int NT = TX * TY;
-    // a7: per-tile slice of the global order: every splat whose pixel bbox touches the tile,
-    // in front-to-back rank order.
-    std::vector<uint64_t> count((size_t)NT + 1, 0);
-    for (uint32_t r = 0; r < F.n_vis; ++r) {
-        const orc_splat& sp = F.splats[r];
-        if (sp.xlo > sp.xhi) continue;
-        for (int ty = sp.ylo / TILE; ty <= sp.yhi / TILE; ++ty)
-            for (int tx = sp.xlo / TILE; tx <= sp.xhi / TILE; ++tx) count[(size_t)ty * TX + tx + 1]++;
-    }
-    for (int t = 0; t < NT; ++t) count[t + 1] += count[t];
+    std::vector<uint64_t> count;
+    std::vector<uint32_t> entries;
+    bin_tiles(F, TX, TY, count, entries);
     const uint64_t total = count[NT];
     if (n_pairs) *n_pairs = total;
     if (n_vis) *n_vis = F.n_vis;
     if (rank_to_id) std::memcpy(rank_to_id, F.rank_to_id.data(), (size_t)F.n_vis * 4);
-    std::vector<uint32_t> entries(total);
-    {
-        std::vector<uint64_t> cur(count.begin(), count.end() - 1);
-        for (uint32_t r = 0; r < F.n_vis; ++r) {
-            const orc_splat& sp = F.splats[r];
-            if (sp.xlo > sp.xhi) continue;
-            for (int ty = sp.ylo / TILE; ty <= sp.yhi / TILE; ++ty)
-                for (int tx = sp.xlo / TILE; tx <= sp.xhi / TILE; ++tx) entries[cur[(size_t)ty * TX + tx]++] = r;
-        }
-    }
     if (tile_ranges) for (int t = 0; t < NT; ++t) {
         // empty tiles report (0, 0), matching the CUDA range build
         const bool empty = count[t] == count[t + 1];
@@ -781,6 +804,87 @@ int orc_render_tiles(uint32_t n, const float* pos_vis, const float* sh, const fl
             }
             float* px = out + 4 * ((size_t)y * W + x);
             px[0] = cr; px[1] = cg; px[2] = cb; px[3] = 1.0f;   // over opaque black: alpha stays 1
+        }
+    }
+    return 0;
+}
+
+int orc_coverage_probe(uint32_t count, const orc_splat* splats, const orc_settings* s, const float* pixel_xy,
+                       orc_probe* out) {
+    if (!s) return 2;
+#pragma omp parallel for schedule(static)
+    for (int64_t j = 0; j < (int64_t)count; ++j) {
+        const orc_splat& sp = splats[j];
+        const float fx = pixel_xy[2 * j], fy = pixel_xy[2 * j + 1];
+        const Decision d = decide(sp, *s, fx, fy), du = decide(sp, *s, fx, fy, false);
+        orc_probe& o = out[j];
+        o.u = d.u; o.v = d.v; o.mx = d.mx; o.my = d.my; o.Rq = d.Rq; o.power = d.power;
+        o.covered = d.covered ? 1u : 0u;
+        o.covered_if_unfused = du.covered ? 1u : 0u;
+        o.alpha = d.covered ? alpha_of(sp, d.power) : 0.0f;
+    }
+    return 0;
+}
+
+int orc_blend_trace(uint32_t n, const float* pos_vis, const float* sh, const float* rot, const float* so,
+                    const orc_view* view, const orc_uniform* u, const orc_settings* s, orc_trace* out, int threads) {
+    Ctx C;
+    if (!make_ctx(C, view, u, s)) return 2;
+#ifdef _OPENMP
+    if (threads > 0) omp_set_num_threads(threads);
+#endif
+    Frame F;
+    build_frame(C, n, pos_vis, sh, rot, so, F);
+    const int W = C.Wi, H = C.Hi;
+    const int TX = (W + TILE - 1) / TILE, TY = (H + TILE - 1) / TILE;
+    std::vector<uint64_t> count;
+    std::vector<uint32_t> entries;
+    bin_tiles(F, TX, TY, count, entries);
+#pragma omp parallel for schedule(dynamic, 4)
+    for (int t = 0; t < TX * TY; ++t) {
+        const int tx = t % TX, ty = t / TX;
+        for (int ly = 0; ly < TILE; ++ly) for (int lx = 0; lx < TILE; ++lx) {
+            const int x = tx * TILE + lx, y = ty * TILE + ly;
+            if (x >= W || y >= H) continue;
+            orc_trace o;
+            std::memset(&o, 0, sizeof(o));
+            o.rank0 = o.rank1 = -1;
+            o.stop_margin = std::numeric_limits<double>::infinity();
+            float T = 1.0f;
+            double T64 = 1.0, c64[3] = {0.0, 0.0, 0.0};
+            for (uint64_t e = count[t]; e < count[t + 1]; ++e) {
+                const orc_splat& sp = F.splats[entries[e]];
+                const Decision d = decide(sp, *s, (float)x + 0.5f, (float)y + 0.5f);
+                if (!d.covered) continue;
+                // f32: exactly render_tiles' step
+                const float x32 = std::exp(d.power) * sp.op, a = std::fmin(x32, 0.999f);
+                // f64: the same decision and the same stop index, exp of the f32 power in double
+                const double a64 = std::fmin(std::exp((double)d.power) * (double)sp.op, 0.999);
+                const double w64 = a64 * T64;
+                o.w_power += w64 * std::fabs((double)d.power);
+                c64[0] += w64 * sp.r; c64[1] += w64 * sp.g; c64[2] += w64 * sp.b;
+                T64 *= 1.0 - a64;
+                if (o.n_blended == 0) o.rank0 = (int32_t)entries[e];
+                else if (o.n_blended == 1) o.rank1 = (int32_t)entries[e];
+                ++o.n_blended;
+                o.max_c = std::fmax(o.max_c, std::fmax(std::fabs(sp.r), std::fmax(std::fabs(sp.g), std::fabs(sp.b))));
+                o.max_power = std::fmax(o.max_power, std::fabs(d.power));
+                if (std::fabs(x32 - 0.999f) <= 1.0e-5f * 0.999f) o.flags |= ORC_TRACE_NEAR_CLAMP;
+                if (x32 < 0.999f) {
+                    o.flags |= ORC_TRACE_UNCLAMPED;
+                    o.t_sens += (double)a / (1.0 - (double)a);
+                    o.t_sens_power += (double)a / (1.0 - (double)a) * std::fabs((double)d.power);
+                }
+                T = T * (1.0f - a);
+                const double margin = std::fabs((double)T / (double)T_STOP - 1.0);
+                o.stop_margin = std::fmin(o.stop_margin, margin);
+                if (margin <= 1.0e-5) o.flags |= ORC_TRACE_NEAR_STOP;
+                if (T < T_STOP) break;
+            }
+            o.c64[0] = c64[0]; o.c64[1] = c64[1]; o.c64[2] = c64[2];
+            o.T64 = T64;
+            o.T = T;
+            out[(size_t)y * W + x] = o;
         }
     }
     return 0;

@@ -107,6 +107,46 @@ int orc_render_tiles(uint32_t n, const float* pos_vis, const float* sh, const fl
                      uint32_t* tile_entries, uint64_t cap, uint64_t* n_pairs, uint32_t* n_vis,
                      uint32_t* rank_to_id, int threads);
 
+/* Coverage probe: for each pair j, splat record splats[j] at the pixel centre (pixel_xy[2j], pixel_xy[2j+1]), the
+ * quantities fs_main's coverage decision turns on, exactly as render_tiles computes them.  u, v: USE_OBB quad uv
+ * (|u| <= 1 && |v| <= 1); mx, my, Rq: USE_AABB quad offset and half-side (|mx| <= Rq && |my| <= Rq); power: the
+ * exponent (covered pixels; USE_AABB also sets it when only power > 0 rejects).  covered_if_unfused: the decision with
+ * u, v from a separately rounded multiply and add instead of the fma. */
+typedef struct {
+    float u, v, mx, my, Rq, power, alpha;
+    uint32_t covered, covered_if_unfused;
+} orc_probe;
+int orc_coverage_probe(uint32_t count, const orc_splat* splats, const orc_settings* s, const float* pixel_xy,
+                       orc_probe* out);
+
+/* Blend trace: the tile_mode walk of render_tiles (same slices, same f32 coverage decisions, same f32 stop index),
+ * per pixel (row-major, W*H):
+ *   c64, T64: the colour and transmittance of that walk accumulated in float64, alpha = min(exp(power) * op, 0.999)
+ *             with exp taken in double of the f32 power -- the exact value of the blend the f32 walk performs;
+ *   T:        the f32 transmittance where the walk stopped; n_blended, rank0 / rank1 (first two blended ranks, -1 none);
+ *   max_c:    max |r|, |g|, |b| of the blended records; max_power: max |power| of the blended splats;
+ *   t_sens:   sum of a / (1 - a) over the blended alphas below the clamp: |dT / T| <= t_sens * (relative alpha error);
+ *   w_power, t_sens_power: sum of w64 |power| over the blended splats, sum of a / (1 - a) |power| over the unclamped
+ *             ones (for alpha errors that grow with |power|);
+ *   stop_margin: min over the T < T_STOP tests of |T / T_STOP - 1|;
+ *   flags:    NEAR_STOP (stop_margin <= 1e-5: a kernel computing T another way may stop one splat apart),
+ *             NEAR_CLAMP (a blended exp * op within 1e-5 relative of 0.999), UNCLAMPED (a blended exp * op < 0.999). */
+#define ORC_TRACE_NEAR_STOP 1u
+#define ORC_TRACE_NEAR_CLAMP 2u
+#define ORC_TRACE_UNCLAMPED 4u
+typedef struct {
+    double c64[3], T64, t_sens, stop_margin, w_power, t_sens_power;
+    float T;
+    uint32_t n_blended;
+    int32_t rank0, rank1;
+    uint32_t flags;
+    float max_c, max_power;
+    uint32_t pad;
+} orc_trace;
+int orc_blend_trace(uint32_t n, const float* pos_vis, const float* sh, const float* rot,
+                    const float* scale_opacity, const orc_view* view, const orc_uniform* u,
+                    const orc_settings* s, orc_trace* out, int threads);
+
 /* CPU-baseline model of the reference's native CPU sort (src/sort/rayon.rs:86-104):
  * key = bits(|p - cam|^2), parallel unstable sort, descending.  Returns seconds. */
 double orc_cpu_sort_model(uint32_t n, const float* pos_vis, const float* cam, int threads,

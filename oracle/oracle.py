@@ -168,6 +168,39 @@ def render_tiles(cloud, view, uniform, settings, want_image: bool = True, thread
                 rank_to_id=r2i)
 
 
+PROBE_DTYPE = np.dtype([("u", "f4"), ("v", "f4"), ("mx", "f4"), ("my", "f4"), ("Rq", "f4"), ("power", "f4"), ("alpha", "f4"),
+                        ("covered", "u4"), ("covered_if_unfused", "u4")])
+TRACE_DTYPE = np.dtype([("c64", "f8", (3,)), ("T64", "f8"), ("t_sens", "f8"), ("stop_margin", "f8"), ("w_power", "f8"),
+                        ("t_sens_power", "f8"), ("T", "f4"),
+                        ("n_blended", "u4"), ("rank0", "i4"), ("rank1", "i4"), ("flags", "u4"), ("max_c", "f4"),
+                        ("max_power", "f4"), ("pad", "u4")])
+assert TRACE_DTYPE.itemsize == 96
+TRACE_NEAR_STOP, TRACE_NEAR_CLAMP, TRACE_UNCLAMPED = 1, 2, 4
+
+
+def coverage_probe(splats: np.ndarray, settings, pixel_xy: np.ndarray) -> np.ndarray:
+    """`splats`: SPLAT_DTYPE records; `pixel_xy`: (len(splats), 2) pixel centres -> PROBE_DTYPE per pair."""
+    splats = np.ascontiguousarray(splats, SPLAT_DTYPE)
+    xy = np.ascontiguousarray(pixel_xy, np.float32).reshape(len(splats), 2)
+    out = np.zeros(len(splats), PROBE_DTYPE)
+    s = _conv(settings, orc_settings)
+    rc = load().orc_coverage_probe(C.c_uint32(len(splats)), _p(splats), C.byref(s), _p(xy), _p(out))
+    assert rc == 0
+    return out
+
+
+def blend_trace(cloud, view, uniform, settings, threads: int = 0) -> np.ndarray:
+    """-> (H, W) TRACE_DTYPE: render_tiles' walk per pixel, with its blend also evaluated in float64."""
+    v, u, s = _conv(view, orc_view), _conv(uniform, orc_uniform), _conv(settings, orc_settings)
+    W, H = int(v.viewport[2]), int(v.viewport[3])
+    out = np.zeros((H, W), TRACE_DTYPE)
+    rc = load().orc_blend_trace(C.c_uint32(len(cloud)), _p(cloud.position_visibility), _p(cloud.spherical_harmonic),
+                                _p(cloud.rotation), _p(cloud.scale_opacity), C.byref(v), C.byref(u), C.byref(s), _p(out),
+                                C.c_int(threads))
+    assert rc == 0
+    return out
+
+
 def cpu_sort_model(pos_vis: np.ndarray, cam, threads: int = 0) -> float:
     cam = np.asarray(cam, np.float32)
     return float(load().orc_cpu_sort_model(C.c_uint32(len(pos_vis)), _p(pos_vis), _p(cam), C.c_int(threads), None))

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import bevy_gaussian_splatting_b200 as B
+import blend_cases as BC
 
 pytestmark = pytest.mark.gpu
 
@@ -75,11 +76,26 @@ def check_against_oracle(plugin, oracle, cloud, settings, view, f16=False, pixel
         assert np.array_equal(bb[drawn, 0], (orec["xlo"][drawn].astype(np.uint32) | (orec["xhi"][drawn].astype(np.uint32) << 16)))
         assert np.array_equal(bb[drawn, 1], (orec["ylo"][drawn].astype(np.uint32) | (orec["yhi"][drawn].astype(np.uint32) << 16)))
         assert np.all((bb[~drawn, 0] & 0xFFFF) > (bb[~drawn, 0] >> 16))      # empty bbox where the oracle's is
+        dc = 1e-4                       # (Depth colours come from the frame pass: bounded by the record check's 1e-4)
         if drawn.any() and settings.rasterize_mode != B.RasterizeMode.Depth:   # orc_project leaves Depth colours to the frame pass
             col = np.stack([orec[k] for k in ("r", "g", "b", "op")], 1)
             assert np.abs(rec[drawn, 8:12] - col[drawn]).max() <= 1e-4
+            dc = float(np.abs(rec[drawn, 8:11] - col[drawn, :3]).max())
         err = float(np.abs(img - til["image"]).max())
         assert err <= pixel_tol, f"pixel L-inf {err}"
+        # per pixel: within the derived error bound of the float64 evaluation of the same walk (blend_cases.blend_bounds)
+        trace = oracle.blend_trace(oc, view.to_abi(), u, s_abi)
+        bound, _ = BC.frame_bounds(trace, bool(settings.aabb), "opaque", dc)
+        want = BC.expected_frame(trace, "opaque")
+
+        def check_bound(frame, which):
+            over = np.abs(frame.astype(np.float64) - want) - bound
+            if over.max() > 0:
+                y, x, c = np.unravel_index(int(over.argmax()), over.shape)
+                raise AssertionError(f"{which}: pixel (x={x}, y={y}) channel {c} exceeds its error bound {bound[y, x, c]:.3g} "
+                                     f"by {over[y, x, c]:.3g}")
+
+        check_bound(img, "first frame")
         if ref_mode_too:
             # the reference's own semantics (instanced quads blended back-to-front, no tiles, no early-out), directly
             ref = oracle.render_ref(oc, view.to_abi(), u, s_abi)
@@ -89,6 +105,7 @@ def check_against_oracle(plugin, oracle, cloud, settings, view, f16=False, pixel
         img2 = render_frame(plugin, h, settings, view, asynchronous)
         err2 = float(np.abs(img2 - til["image"]).max())
         assert err2 <= pixel_tol, f"pixel L-inf {err2} on the hinted frame"
+        check_bound(img2, "hinted frame")     # (raster2_kernel's frame where large_footprint_raster holds)
         if plugin.frame_stats().rounds == 1:   # (a multi-round frame keeps only its last round's ranges)
             assert np.array_equal(plugin.tile_ranges(), til["tile_ranges"])
         return img, til
