@@ -11,7 +11,7 @@
 // One CTA per tile, 256 threads = 8 warps, each warp owning an 8x4-pixel sub-rectangle so a
 // warp-uniform bbox test skips splats that cannot touch any of its 32 pixels.  The tile's slice
 // of the sorted pair list is staged through shared memory in chunks of 256 records.
-// Coverage maths uses explicit __fmul_rn/__fmaf_rn so u,v are bit-identical to the oracle.
+// Coverage maths (quad_uv) uses explicit __fmul_rn/__fmaf_rn so u,v are bit-identical to the oracle.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -22,10 +22,6 @@ constexpr int RT_THREADS = 256;
 constexpr int RT_CHUNK = 256;
 
 // ---- TMA (cp.async.bulk) staging of a tile's slice of the sorted pair list ------------------------------
-// The slice [range.x, range.y) of tile_entries is contiguous, so each 256-entry chunk is brought into shared
-// memory by ONE bulk async copy (UBLKCP) issued by one thread and tracked by an mbarrier; the next chunk's copy
-// is issued before the current chunk is rasterised (double buffer).  Bulk copies need 16 B alignment: the copy
-// starts at the slice address rounded down to 16 B and `lead` skips the extra leading entries.
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
@@ -47,14 +43,60 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 constexpr uint32_t ENT_WORDS = RT_CHUNK + 8;   // a chunk plus up to 3 leading + rounding words
 
-// issue the bulk copy of entries [base, base + cnt) into buffer `buf`; returns nothing (thread 0 only)
-__device__ __forceinline__ void issue_entries(const uint32_t* tile_entries, uint32_t base, uint32_t cnt, uint32_t a_ent,
-                                              uint32_t a_bar, int buf) {
-    const uint32_t lead = base & 3u;
-    const uint32_t bytes = ((lead + cnt) * 4u + 15u) & ~15u;
-    mbar_expect_tx(a_bar + 8u * buf, bytes);
-    tma_bulk_g2s(a_ent + (uint32_t)buf * ENT_WORDS * 4u, tile_entries + (base - lead), bytes, a_bar + 8u * buf);
-}
+// A tile's slice [range.x, range.y) of tile_entries, chunk by chunk: per chunk (loop index `chunk`, first entry `base`)
+// next(base), then entry(base, j); finish() after the loop.  A streamed slice (`tma`, the kernel's choice) comes into the
+// double buffer `ent` by ONE bulk async copy (UBLKCP) per chunk, issued by thread 0 and tracked by an mbarrier; chunk
+// k + 1's copy is in flight while chunk k is blended.  Bulk copies need 16 B alignment: a copy starts at the slice
+// address rounded down to 16 B and entry() skips the `base & 3` leading words.  Other slices are read from global memory.
+struct PairStream {
+    const uint32_t* entries;
+    uint32_t (*ent)[ENT_WORDS];
+    uint32_t a_ent, a_bar, end;
+    bool tma;
+    uint32_t issued = 0u, chunk = 0u;   // bulk copies issued; chunks [0, chunk) have been waited for
+
+    // collective when `tma`: initialises the barriers, then issues chunk 0's copy
+    __device__ __forceinline__ PairStream(const uint32_t* tile_entries, uint32_t (*s_ent)[ENT_WORDS], unsigned long long* s_bar,
+                                          uint2 range, bool use_tma)
+        : entries(tile_entries), ent(s_ent), a_ent((uint32_t)__cvta_generic_to_shared(s_ent)),
+          a_bar((uint32_t)__cvta_generic_to_shared(s_bar)), end(range.y), tma(use_tma) {
+        if (!tma) return;
+        if (threadIdx.x == 0) {
+            mbar_init(a_bar, 1u); mbar_init(a_bar + 8u, 1u);
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) issue(range.x, (uint32_t)RT_CHUNK, 0);
+        issued = 1u;
+    }
+    // bulk copy of entries [base, base + cnt) into buffer `buf` (thread 0 only)
+    __device__ __forceinline__ void issue(uint32_t base, uint32_t cnt, int buf) const {
+        const uint32_t lead = base & 3u;
+        const uint32_t bytes = ((lead + cnt) * 4u + 15u) & ~15u;
+        mbar_expect_tx(a_bar + 8u * buf, bytes);
+        tma_bulk_g2s(a_ent + (uint32_t)buf * ENT_WORDS * 4u, entries + (base - lead), bytes, a_bar + 8u * buf);
+    }
+    // chunk `chunk` starts at `base`: prefetch the NEXT chunk's entries (its buffer was last read two chunks ago, which
+    // the kernel's vote at the top of this chunk fenced), then wait for this one's
+    __device__ __forceinline__ void next(uint32_t base) {
+        const int buf = (int)(chunk & 1u);
+        if (tma) {
+            if (base + RT_CHUNK < end) {
+                if (threadIdx.x == 0) issue(base + RT_CHUNK, min((uint32_t)RT_CHUNK, end - base - RT_CHUNK), buf ^ 1);
+                ++issued;
+            }
+            mbar_wait(a_bar + 8u * buf, (chunk >> 1) & 1u);
+        }
+    }
+    template <class Index>   // int or uint32_t, as the caller's loop has it
+    __device__ __forceinline__ uint32_t entry(uint32_t base, Index j) const {
+        return tma ? ent[chunk & 1u][(base & 3u) + j] : __ldg(entries + base + j);
+    }
+    // an early exit (all pixels saturated) may leave one prefetch in flight: keep the CTA alive until it lands
+    __device__ __forceinline__ void finish() const {
+        if (threadIdx.x == 0 && issued > chunk) mbar_wait(a_bar + 8u * (chunk & 1u), (chunk >> 1) & 1u);
+    }
+};
 
 // CTA -> tile: rows are visited from the middle row outwards (mid, mid-1, mid+1, ...), so the tiles launched last --
 // the ones that form the kernel's tail -- are the top / bottom rows, usually the lightest.
@@ -91,6 +133,18 @@ __device__ __forceinline__ float4 read_pixel(const void* out, uint32_t fmt, size
     return make_float4(srgb_decode((float)(v & 255u) * (1.0f / 255.0f)), srgb_decode((float)((v >> 8) & 255u) * (1.0f / 255.0f)),
                        srgb_decode((float)((v >> 16) & 255u) * (1.0f / 255.0f)), (float)(v >> 24) * (1.0f / 255.0f));
 }
+// pixel encoders: RGBA16F, and sRGB8 with a linear alpha byte (or 255 when !with_alpha)
+__device__ __forceinline__ uint2 pack_rgba16f(float r, float g, float b, float a) {
+    const __half2 lo = __floats2half2_rn(r, g), hi = __floats2half2_rn(b, a);
+    return make_uint2(*reinterpret_cast<const uint32_t*>(&lo), *reinterpret_cast<const uint32_t*>(&hi));
+}
+__device__ __forceinline__ uint32_t pack_srgb8(float r, float g, float b, float a, bool with_alpha) {
+    const uint32_t r8 = (uint32_t)(linear_to_srgb(r) * 255.0f + 0.5f);
+    const uint32_t g8 = (uint32_t)(linear_to_srgb(g) * 255.0f + 0.5f);
+    const uint32_t b8 = (uint32_t)(linear_to_srgb(b) * 255.0f + 0.5f);
+    const uint32_t a8 = with_alpha ? (uint32_t)(fminf(fmaxf(a, 0.0f), 1.0f) * 255.0f + 0.5f) : 255u;
+    return r8 | (g8 << 8) | (b8 << 16) | (a8 << 24);
+}
 // one pixel's accumulated premultiplied colour (r, g, b) and remaining transmittance T -> the frame
 __device__ __forceinline__ void write_pixel(void* out, uint32_t format, size_t pix, float r, float g, float b, float T) {
     const uint32_t fmt = format & 0xFFu, mode = format >> 8;
@@ -105,17 +159,9 @@ __device__ __forceinline__ void write_pixel(void* out, uint32_t format, size_t p
     if (fmt == BGS_FORMAT_RGBA32F) {
         reinterpret_cast<float4*>(out)[pix] = make_float4(r, g, b, a);
     } else if (fmt == BGS_FORMAT_RGBA16F) {
-        const __half2 lo = __floats2half2_rn(r, g), hi = __floats2half2_rn(b, a);
-        uint2 o;
-        o.x = *reinterpret_cast<const uint32_t*>(&lo);
-        o.y = *reinterpret_cast<const uint32_t*>(&hi);
-        reinterpret_cast<uint2*>(out)[pix] = o;
+        reinterpret_cast<uint2*>(out)[pix] = pack_rgba16f(r, g, b, a);
     } else {
-        const uint32_t r8 = (uint32_t)(linear_to_srgb(r) * 255.0f + 0.5f);
-        const uint32_t g8 = (uint32_t)(linear_to_srgb(g) * 255.0f + 0.5f);
-        const uint32_t b8 = (uint32_t)(linear_to_srgb(b) * 255.0f + 0.5f);
-        const uint32_t a8 = mode ? (uint32_t)(fminf(fmaxf(a, 0.0f), 1.0f) * 255.0f + 0.5f) : 255u;
-        reinterpret_cast<uint32_t*>(out)[pix] = r8 | (g8 << 8) | (b8 << 16) | (a8 << 24);
+        reinterpret_cast<uint32_t*>(out)[pix] = pack_srgb8(r, g, b, a, mode != 0);
     }
 }
 
@@ -129,6 +175,44 @@ constexpr uint32_t SM_BYTES = SM_EXTRA;
 constexpr uint32_t SM_BYTES_2D = SM_EXTRA + 4 * RT_CHUNK * 16;
 // AUX (bgs_render_aux): 2 x float4 [256] after the mode's own arrays: depth rgb, normal rgb of the staged splats
 
+// a staged splat's uv and q2 records, as offsets from the shared address of its q0 record (what the candidate lists hold)
+constexpr uint32_t REC_UV = SM_UV - SM_Q0, REC_Q2 = SM_Q2 - SM_Q0;
+static_assert(REC_UV == RT_CHUNK * 16 && REC_Q2 == 2 * RT_CHUNK * 16, "q0, uv, q2 are consecutive float4 [RT_CHUNK] arrays");
+
+// loads from a shared address (volatile: they keep their order in the hot loops)
+__device__ __forceinline__ float4 lds4(uint32_t a) {
+    float4 r; asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(a)); return r;
+}
+__device__ __forceinline__ float2 lds2(uint32_t a) {
+    float2 r; asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(r.x), "=f"(r.y) : "r"(a)); return r;
+}
+__device__ __forceinline__ uint32_t lds_u16(uint32_t a) { uint32_t r; asm volatile("ld.shared.u16 %0, [%1];" : "=r"(r) : "r"(a)); return r; }
+__device__ __forceinline__ uint32_t lds_u32(uint32_t a) { uint32_t r; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(a)); return r; }
+
+// USE_OBB quad coordinates of the pixel centre (fx, fy) for q0 = (cx, cy, ux, uy), q1 = (vx, vy): u = ux dx + uy dy with
+// the fma on the dy term, v likewise.  The same rounding steps as decide() in oracle/bgs_oracle.cpp, so the coverage
+// test |u|, |v| <= 1 is bit-identical to the oracle's.
+__device__ __forceinline__ float2 quad_uv(float fx, float fy, float4 q0, float2 q1) {
+    const float dx = __fsub_rn(fx, q0.x), dy = __fsub_rn(fy, q0.y);
+    return make_float2(__fmaf_rn(q0.w, dy, __fmul_rn(q0.z, dx)), __fmaf_rn(q1.y, dy, __fmul_rn(q1.x, dx)));
+}
+
+// Each warp compacts the chunk's `cnt` staged splats to those `hit(j)` keeps, in order, into its u16 list as
+// `rec0 + j * 16` (the q0 record's address relative to rec0); returns the list's length.
+template <class Hit>
+__device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned short* list, uint32_t rec0, Hit hit) {
+    uint32_t nl = 0;
+    for (uint32_t j0 = 0; j0 < cnt; j0 += 32) {
+        const uint32_t j = j0 + (threadIdx.x & 31u);
+        bool h = false;
+        if (j < cnt) h = hit(j);
+        const uint32_t m = __ballot_sync(0xffffffffu, h);
+        if (h) list[nl + __popc(m & lanemask_lt())] = (unsigned short)(rec0 + j * 16u);
+        nl += __popc(m);
+    }
+    __syncwarp();
+    return nl;
+}
 
 // MODE 0: USE_OBB quad-uv falloff (3DGS, and 2DGS without aabb)   gaussian.wgsl:474-504
 // MODE 1: 3DGS USE_AABB conic falloff                              gaussian.wgsl:459-471
@@ -165,8 +249,6 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
     uint2 range = ranges[tile];
     range.x = ~range.x;                  // stored as (~start, end): the sort's last pass builds it with atomicMax (radix.cu)
 
-    const uint32_t a_ent = (uint32_t)__cvta_generic_to_shared(&s_ent[0][0]);
-    const uint32_t a_bar = (uint32_t)__cvta_generic_to_shared(&s_bar[0]);
     if (range.x >= range.y) {            // empty tile: nothing to stage (uniform across the CTA)
         // (blend-over mode leaves the target's pixels as they are)
         if (inside && !((format >> 8) & OUT_OVER)) {
@@ -178,36 +260,17 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
         }
         return;
     }
-    // tiles with more than one chunk stream their pair list through the TMA double buffer (the next chunk's
-    // copy overlaps this chunk's blending); single-chunk tiles read it directly (no barrier set-up on their path)
-    const bool use_tma = range.y - range.x > (uint32_t)RT_CHUNK;
-    uint32_t issued = 0u, chunk = 0u;
-    if (use_tma) {
-        if (t == 0) {
-            mbar_init(a_bar, 1u); mbar_init(a_bar + 8u, 1u);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (t == 0) issue_entries(tile_entries, range.x, (uint32_t)RT_CHUNK, a_ent, a_bar, 0);
-        issued = 1u;
-    }
+    // tiles with more than one chunk stream their pair list (the next chunk's copy overlaps this chunk's blending)
+    PairStream ps(tile_entries, s_ent, s_bar, range, range.y - range.x > (uint32_t)RT_CHUNK);
 
     float T = inside ? 1.0f : 0.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f;   // T < T_STOP <=> this pixel is done
     float dr = 0.0f, dg = 0.0f, db = 0.0f, nr = 0.0f, ng = 0.0f, nb = 0.0f;   // AUX: depth / normal frames
-    for (uint32_t base = range.x; base < range.y; base += RT_CHUNK, ++chunk) {
+    for (uint32_t base = range.x; base < range.y; base += RT_CHUNK, ++ps.chunk) {
         if (__syncthreads_count(T < T_STOP ? 0 : 1) == 0) break;   // also fences reuse of the staging buffers
         const uint32_t cnt = min((uint32_t)RT_CHUNK, range.y - base);
-        const int buf = (int)(chunk & 1u);
-        // prefetch the NEXT chunk's entries (its buffer was last read two iterations ago: the vote above fenced it)
-        if (use_tma) {
-            if (base + RT_CHUNK < range.y) {
-                if (t == 0) issue_entries(tile_entries, base + RT_CHUNK, min((uint32_t)RT_CHUNK, range.y - base - RT_CHUNK), a_ent, a_bar, buf ^ 1);
-                ++issued;
-            }
-            mbar_wait(a_bar + 8u * buf, (chunk >> 1) & 1u);
-        }
+        ps.next(base);
         if ((uint32_t)t < cnt) {
-            const uint32_t r = use_tma ? s_ent[buf][(base & 3u) + t] : __ldg(tile_entries + base + t);
+            const uint32_t r = ps.entry(base, t);
             const float4* rp = reinterpret_cast<const float4*>(recs + r);
             const float4 p0 = __ldg(rp), p1 = __ldg(rp + 1);
             s_q0[t] = p0;
@@ -236,33 +299,24 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
             }
         }
         __syncthreads();
-        // each warp compacts the chunk to the splats whose bbox touches its 8x4 pixels (order kept)
-        uint32_t nl = 0;
-        if (__any_sync(0xffffffffu, !(T < T_STOP))) {
-            for (uint32_t j0 = 0; j0 < cnt; j0 += 32) {
-                const uint32_t j = j0 + lane;
-                bool hit = false;
-                if (j < cnt) {
-                    const float4 q = s_uv[j];
-                    const uint32_t bx = __float_as_uint(q.z), by = __float_as_uint(q.w);
-                    hit = !((int)(bx >> 16) < wx0 || (int)(bx & 0xFFFFu) > wx0 + 7 || (int)(by >> 16) < wy0 ||
-                            (int)(by & 0xFFFFu) > wy0 + 3);
-                    if (MODE == 0 && hit) {
-                        // separating-axis test of the splat's quad against this warp's pixel centres
-                        // [wx0 + .5, wx0 + 7.5] x [wy0 + .5, wy0 + 3.5] (thresholds staged per splat above): the bbox
-                        // of a slanted quad passes many warps none of whose pixels it covers
-                        const float4 p = s_q0[j];
-                        const float2 th = s_thr[j];
-                        const float dxc = rcx - p.x, dyc = rcy - p.y;
-                        if (fabsf(p.z * dxc + p.w * dyc) > th.x || fabsf(q.x * dxc + q.y * dyc) > th.y) hit = false;
-                    }
-                }
-                const uint32_t m = __ballot_sync(0xffffffffu, hit);
-                if (hit) s_list[nl + __popc(m & lanemask_lt())] = (unsigned short)(a_base + j * 16u);   // shared address of q0[j]
-                nl += __popc(m);
+        // each warp's candidates: the splats whose bbox touches its 8x4 pixels, listed by shared address of q0[j]
+        const uint32_t nl = !__any_sync(0xffffffffu, !(T < T_STOP)) ? 0u : compact_candidates(cnt, s_list, a_base, [&](uint32_t j) {
+            const float4 q = s_uv[j];
+            const uint32_t bx = __float_as_uint(q.z), by = __float_as_uint(q.w);
+            // (`|`, not `||`: the four compares are one predicated test, not a chain of branches)
+            bool hit = !((int)(bx >> 16) < wx0 | (int)(bx & 0xFFFFu) > wx0 + 7 | (int)(by >> 16) < wy0 |
+                         (int)(by & 0xFFFFu) > wy0 + 3);
+            if (MODE == 0 && hit) {
+                // separating-axis test of the splat's quad against this warp's pixel centres
+                // [wx0 + .5, wx0 + 7.5] x [wy0 + .5, wy0 + 3.5] (thresholds staged per splat above): the bbox
+                // of a slanted quad passes many warps none of whose pixels it covers
+                const float4 p = s_q0[j];
+                const float2 th = s_thr[j];
+                const float dxc = rcx - p.x, dyc = rcy - p.y;
+                hit = !(fabsf(p.z * dxc + p.w * dyc) > th.x || fabsf(q.x * dxc + q.y * dyc) > th.y);
             }
-            __syncwarp();
-        }
+            return hit;
+        });
         if (MODE == 0 && !AUX) {
             // two candidates per iteration: one 32-bit load brings both list entries, the four record loads and both
             // coverage tests are independent (ILP), loop control is paid once; blending stays strictly in list order
@@ -271,88 +325,72 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
             // the warp anyway).  `lim` = 1 while the pixel is alive, -1 once it has stopped (T < T_STOP) or lies outside the
             // frame, so "covered" and "alive" are one comparison and a stopped pixel skips every later splat exactly as an
             // early exit would.
-            {
-                const uint32_t a_end = a_list + nl * 2u;
-                uint32_t a_it = a_list;
-                float lim = (T < T_STOP) ? -1.0f : 1.0f;
-                auto blend_if_covered = [&](uint32_t a_rec, float u, float v) {
-                    asm volatile(
-                        "{\n\t"
-                        ".reg .pred p, q;\n\t"
-                        ".reg .f32 au, av, x, y, z, o, qd, e, a, w, na;\n\t"
-                        "abs.f32 au, %5;\n\t"
-                        "abs.f32 av, %6;\n\t"
-                        "setp.le.f32 p, au, %4;\n\t"
-                        "setp.le.and.f32 p, av, %4, p;\n\t"
-                        // (the temporaries are computed unconditionally -- a predicated definition would keep their old values
-                        // alive across iterations -- only the four accumulations are predicated)
-                        "ld.shared.v4.f32 {x, y, z, o}, [%7+8192];\n\t"
-                        "mul.rn.f32 qd, %5, %5;\n\t"
-                        "fma.rn.f32 qd, %6, %6, qd;\n\t"
-                        "mul.rn.f32 qd, qd, 0fC0CFBF83;\n\t"             // -6.492127684f: exp(-4.5 qd) = 2^(qd * -4.5 log2 e)
-                        "ex2.approx.ftz.f32 e, qd;\n\t"
-                        "mul.rn.f32 a, e, o;\n\t"
-                        "min.f32 a, a, 0f3F7FBE77;\n\t"                 // 0.999f
-                        "mul.rn.f32 w, a, %0;\n\t"
-                        "neg.f32 na, a;\n\t"
-                        "@p fma.rn.f32 %1, w, x, %1;\n\t"
-                        "@p fma.rn.f32 %2, w, y, %2;\n\t"
-                        "@p fma.rn.f32 %3, w, z, %3;\n\t"
-                        "@p fma.rn.f32 %0, na, %0, %0;\n\t"
-                        "setp.lt.and.f32 q, %0, 0f38D1B717, p;\n\t"     // T < T_STOP (1e-4f) after a blend: the pixel stops
-                        "@q mov.f32 %4, 0fBF800000;\n\t"
-                        "}"
-                        : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb), "+f"(lim)
-                        : "f"(u), "f"(v), "r"(a_rec));
-                };
-                for (; a_it + 2u < a_end; a_it += 4u) {
-                    uint32_t two;
-                    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(two) : "r"(a_it));
-                    const uint32_t ra = two & 0xFFFFu, rb = two >> 16;
-                    float4 pa, pb; float2 sa, sb;
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(pa.x), "=f"(pa.y), "=f"(pa.z), "=f"(pa.w) : "r"(ra));
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(pb.x), "=f"(pb.y), "=f"(pb.z), "=f"(pb.w) : "r"(rb));
-                    asm volatile("ld.shared.v2.f32 {%0,%1}, [%2+4096];" : "=f"(sa.x), "=f"(sa.y) : "r"(ra));
-                    asm volatile("ld.shared.v2.f32 {%0,%1}, [%2+4096];" : "=f"(sb.x), "=f"(sb.y) : "r"(rb));
-                    const float dxa = __fsub_rn(fx, pa.x), dya = __fsub_rn(fy, pa.y);
-                    const float dxb = __fsub_rn(fx, pb.x), dyb = __fsub_rn(fy, pb.y);
-                    const float ua = __fmaf_rn(pa.w, dya, __fmul_rn(pa.z, dxa)), va = __fmaf_rn(sa.y, dya, __fmul_rn(sa.x, dxa));
-                    const float ub = __fmaf_rn(pb.w, dyb, __fmul_rn(pb.z, dxb)), vb = __fmaf_rn(sb.y, dyb, __fmul_rn(sb.x, dxb));
-                    blend_if_covered(ra, ua, va);
-                    blend_if_covered(rb, ub, vb);
-                }
-                if (a_it != a_end) {   // odd tail
-                    uint32_t ra;
-                    asm volatile("ld.shared.u16 %0, [%1];" : "=r"(ra) : "r"(a_it));
-                    float4 pa; float2 sa;
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(pa.x), "=f"(pa.y), "=f"(pa.z), "=f"(pa.w) : "r"(ra));
-                    asm volatile("ld.shared.v2.f32 {%0,%1}, [%2+4096];" : "=f"(sa.x), "=f"(sa.y) : "r"(ra));
-                    const float dxa = __fsub_rn(fx, pa.x), dya = __fsub_rn(fy, pa.y);
-                    const float ua = __fmaf_rn(pa.w, dya, __fmul_rn(pa.z, dxa)), va = __fmaf_rn(sa.y, dya, __fmul_rn(sa.x, dxa));
-                    blend_if_covered(ra, ua, va);
-                }
+            const uint32_t a_end = a_list + nl * 2u;
+            uint32_t a_it = a_list;
+            float lim = (T < T_STOP) ? -1.0f : 1.0f;
+            auto blend_if_covered = [&](uint32_t a_rec, float2 uv) {
+                asm volatile(
+                    "{\n\t"
+                    ".reg .pred p, q;\n\t"
+                    ".reg .f32 au, av, x, y, z, o, qd, e, a, w, na;\n\t"
+                    "abs.f32 au, %5;\n\t"
+                    "abs.f32 av, %6;\n\t"
+                    "setp.le.f32 p, au, %4;\n\t"
+                    "setp.le.and.f32 p, av, %4, p;\n\t"
+                    // (the temporaries are computed unconditionally -- a predicated definition would keep their old values
+                    // alive across iterations -- only the four accumulations are predicated)
+                    "ld.shared.v4.f32 {x, y, z, o}, [%7+%8];\n\t"
+                    "mul.rn.f32 qd, %5, %5;\n\t"
+                    "fma.rn.f32 qd, %6, %6, qd;\n\t"
+                    "mul.rn.f32 qd, qd, 0fC0CFBF83;\n\t"             // -6.492127684f: exp(-4.5 qd) = 2^(qd * -4.5 log2 e)
+                    "ex2.approx.ftz.f32 e, qd;\n\t"
+                    "mul.rn.f32 a, e, o;\n\t"
+                    "min.f32 a, a, 0f3F7FBE77;\n\t"                 // 0.999f
+                    "mul.rn.f32 w, a, %0;\n\t"
+                    "neg.f32 na, a;\n\t"
+                    "@p fma.rn.f32 %1, w, x, %1;\n\t"
+                    "@p fma.rn.f32 %2, w, y, %2;\n\t"
+                    "@p fma.rn.f32 %3, w, z, %3;\n\t"
+                    "@p fma.rn.f32 %0, na, %0, %0;\n\t"
+                    "setp.lt.and.f32 q, %0, 0f38D1B717, p;\n\t"     // T < T_STOP (1e-4f) after a blend: the pixel stops
+                    "@q mov.f32 %4, 0fBF800000;\n\t"
+                    "}"
+                    : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb), "+f"(lim)
+                    : "f"(uv.x), "f"(uv.y), "r"(a_rec), "n"(REC_Q2));
+            };
+            for (; a_it + 2u < a_end; a_it += 4u) {
+                const uint32_t two = lds_u32(a_it);
+                const uint32_t ra = two & 0xFFFFu, rb = two >> 16;
+                const float4 pa = lds4(ra), pb = lds4(rb);
+                const float2 sa = lds2(ra + REC_UV), sb = lds2(rb + REC_UV);
+                const float2 uva = quad_uv(fx, fy, pa, sa), uvb = quad_uv(fx, fy, pb, sb);
+                blend_if_covered(ra, uva);
+                blend_if_covered(rb, uvb);
+            }
+            if (a_it != a_end) {   // odd tail
+                const uint32_t ra = lds_u16(a_it);
+                const float4 pa = lds4(ra);
+                const float2 sa = lds2(ra + REC_UV);
+                blend_if_covered(ra, quad_uv(fx, fy, pa, sa));
             }
         } else if (!(T < T_STOP)) {
             const uint32_t a_end = a_list + nl * 2u;
             for (uint32_t a_it = a_list; a_it != a_end; a_it += 2u) {
-                uint32_t a_rec;
-                asm volatile("ld.shared.u16 %0, [%1];" : "=r"(a_rec) : "r"(a_it));
-                float4 q0; float2 q1;
-                asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(q0.x), "=f"(q0.y), "=f"(q0.z), "=f"(q0.w) : "r"(a_rec));
-                asm volatile("ld.shared.v2.f32 {%0,%1}, [%2+4096];" : "=f"(q1.x), "=f"(q1.y) : "r"(a_rec));
-                const float dx = __fsub_rn(fx, q0.x), dy = __fsub_rn(fy, q0.y);
-                float e, opac;
+                const uint32_t a_rec = lds_u16(a_it);
+                const float4 q0 = lds4(a_rec);
+                const float2 q1 = lds2(a_rec + REC_UV);
+                float e;
                 float4 q2;
                 if (MODE == 0) {
-                    const float u = __fmaf_rn(q0.w, dy, __fmul_rn(q0.z, dx));
-                    const float v = __fmaf_rn(q1.y, dy, __fmul_rn(q1.x, dx));
-                    if (!(fabsf(u) <= 1.0f && fabsf(v) <= 1.0f)) continue;
-                    const float qd = __fmaf_rn(v, v, __fmul_rn(u, u));
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4+8192];" : "=f"(q2.x), "=f"(q2.y), "=f"(q2.z), "=f"(q2.w) : "r"(a_rec));
+                    const float2 uv = quad_uv(fx, fy, q0, q1);
+                    if (!(fabsf(uv.x) <= 1.0f && fabsf(uv.y) <= 1.0f)) continue;
+                    const float qd = __fmaf_rn(uv.y, uv.y, __fmul_rn(uv.x, uv.x));
+                    q2 = lds4(a_rec + REC_Q2);
                     // exp(-4.5 qd) = 2^(qd * -4.5 log2 e); qd <= 2 so the argument stays >= -13 (no range fix-up)
                     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(qd * -6.492127684f));
                 } else {
                     // quad-space offset in half-pixels (x right, y up); the quad is the square |m| <= Rq
+                    const float dx = __fsub_rn(fx, q0.x), dy = __fsub_rn(fy, q0.y);
                     const float mx = __fadd_rn(dx, dx), my = -__fadd_rn(dy, dy);
                     const float Rq = q1.y;   // MODE 1: quad half-side in half-pixels
                     float power;
@@ -363,12 +401,11 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                         const float t1 = __fmul_rn(__fmul_rn(q0.z, ddx), ddx), t2 = __fmul_rn(__fmul_rn(q1.x, ddy), ddy);
                         power = __fadd_rn(__fmul_rn(-0.5f, __fadd_rn(t1, t2)), __fmul_rn(__fmul_rn(q0.w, ddx), ddy));
                     } else {
-                        float4 e0, e1, e2, e3;
-                        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(e0.x), "=f"(e0.y), "=f"(e0.z), "=f"(e0.w) : "r"(a_rec + SM_EXTRA));
+                        const float4 e0 = lds4(a_rec + SM_EXTRA);
                         if (!(fabsf(mx) <= e0.x && fabsf(my) <= e0.x)) continue;
-                        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(e1.x), "=f"(e1.y), "=f"(e1.z), "=f"(e1.w) : "r"(a_rec + SM_EXTRA + RT_CHUNK * 16));
-                        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(e2.x), "=f"(e2.y), "=f"(e2.z), "=f"(e2.w) : "r"(a_rec + SM_EXTRA + 2 * RT_CHUNK * 16));
-                        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(e3.x), "=f"(e3.y), "=f"(e3.z), "=f"(e3.w) : "r"(a_rec + SM_EXTRA + 3 * RT_CHUNK * 16));
+                        const float4 e1 = lds4(a_rec + SM_EXTRA + RT_CHUNK * 16);
+                        const float4 e2 = lds4(a_rec + SM_EXTRA + 2 * RT_CHUNK * 16);
+                        const float4 e3 = lds4(a_rec + SM_EXTRA + 3 * RT_CHUNK * 16);
                         // pixel_coord = uv * radius * (1, W/H) + mean   (gaussian.wgsl:441-447; uv * radius == m)
                         const float pcx = __fadd_rn(mx, e0.y), pcy = __fadd_rn(__fmul_rn(my, e0.w), e0.z);
                         // gaussian_2d.wgsl:134-156: hu = px*T2 - T0, hv = py*T2 - T1, p = hu x hv
@@ -386,17 +423,14 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                         power = -__fmul_rn(0.5f, fminf(s3, s2));
                     }
                     if (power > 0.0f) continue;                      // gaussian.wgsl:468-470
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4+8192];" : "=f"(q2.x), "=f"(q2.y), "=f"(q2.z), "=f"(q2.w) : "r"(a_rec));
+                    q2 = lds4(a_rec + REC_Q2);
                     e = __expf(power);
                 }
-                opac = q2.w;
-                const float a = fminf(e * opac, 0.999f);
+                const float a = fminf(e * q2.w, 0.999f);
                 const float w = a * T;
                 cr = fmaf(w, q2.x, cr); cg = fmaf(w, q2.y, cg); cb = fmaf(w, q2.z, cb);
                 if (AUX) {
-                    float4 ad, an;
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(ad.x), "=f"(ad.y), "=f"(ad.z), "=f"(ad.w) : "r"(a_rec + SM_AUX));
-                    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(an.x), "=f"(an.y), "=f"(an.z), "=f"(an.w) : "r"(a_rec + SM_AUX + RT_CHUNK * 16));
+                    const float4 ad = lds4(a_rec + SM_AUX), an = lds4(a_rec + SM_AUX + RT_CHUNK * 16);
                     dr = fmaf(w, ad.x, dr); dg = fmaf(w, ad.y, dg); db = fmaf(w, ad.z, db);
                     nr = fmaf(w, an.x, nr); ng = fmaf(w, an.y, ng); nb = fmaf(w, an.z, nb);
                 }
@@ -405,9 +439,7 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
             }
         }
     }
-    // an early exit (all pixels saturated) may leave one prefetch in flight: keep the CTA alive until it lands
-    if (t == 0 && issued > chunk)             // chunks [0, chunk) were waited for inside the loop
-        mbar_wait(a_bar + 8u * (chunk & 1u), (chunk >> 1) & 1u);
+    ps.finish();
     if (!inside) return;
     write_pixel(out, format, (size_t)py * W + px, cr, cg, cb, T);
     if (AUX) {
@@ -437,16 +469,12 @@ __device__ __forceinline__ void store_pixel2(void* out, uint32_t format, size_t 
         if (in1) o[1] = make_float4(r1, g1, b1, 1.0f);
     } else if (format == BGS_FORMAT_RGBA16F) {
         uint2* o = reinterpret_cast<uint2*>(out) + pix;
-        const __half2 l0 = __floats2half2_rn(r0, g0), h0 = __floats2half2_rn(b0, 1.0f);
-        const __half2 l1 = __floats2half2_rn(r1, g1), h1 = __floats2half2_rn(b1, 1.0f);
-        if (in0) o[0] = make_uint2(*reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&h0));
-        if (in1) o[1] = make_uint2(*reinterpret_cast<const uint32_t*>(&l1), *reinterpret_cast<const uint32_t*>(&h1));
+        const uint2 p0 = pack_rgba16f(r0, g0, b0, 1.0f), p1 = pack_rgba16f(r1, g1, b1, 1.0f);
+        if (in0) o[0] = p0;
+        if (in1) o[1] = p1;
     } else {
         uint32_t* o = reinterpret_cast<uint32_t*>(out) + pix;
-        const uint32_t p0 = (uint32_t)(linear_to_srgb(r0) * 255.0f + 0.5f) | ((uint32_t)(linear_to_srgb(g0) * 255.0f + 0.5f) << 8) |
-                            ((uint32_t)(linear_to_srgb(b0) * 255.0f + 0.5f) << 16) | 0xFF000000u;
-        const uint32_t p1 = (uint32_t)(linear_to_srgb(r1) * 255.0f + 0.5f) | ((uint32_t)(linear_to_srgb(g1) * 255.0f + 0.5f) << 8) |
-                            ((uint32_t)(linear_to_srgb(b1) * 255.0f + 0.5f) << 16) | 0xFF000000u;
+        const uint32_t p0 = pack_srgb8(r0, g0, b0, 1.0f, false), p1 = pack_srgb8(r1, g1, b1, 1.0f, false);
         if (in0 && in1 && (pix & 1) == 0) *reinterpret_cast<uint2*>(o) = make_uint2(p0, p1);
         else { if (in0) o[0] = p0; if (in1) o[1] = p1; }
     }
@@ -496,41 +524,20 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
             if (done) range.y = range.x;
         }
     }
-    // multi-chunk tiles (the norm on this path: heavy footprints put thousands of entries in a tile) stream their slice of
-    // the sorted pair list through the TMA double buffer, like raster_kernel: chunk k + 1's bulk copy (UBLKCP, mbarrier
-    // complete_tx) is in flight while chunk k is blended
+    // multi-chunk tiles (the norm on this path: heavy footprints put thousands of entries in a tile) stream their slice
+    // of the sorted pair list, like raster_kernel
     __shared__ __align__(16) uint32_t s_ent[2][ENT_WORDS];
     __shared__ __align__(8) unsigned long long s_bar[2];
-    const uint32_t a_ent = (uint32_t)__cvta_generic_to_shared(&s_ent[0][0]);
-    const uint32_t a_bar = (uint32_t)__cvta_generic_to_shared(&s_bar[0]);
-    const bool use_tma = range.y > range.x && range.y - range.x > (uint32_t)RT_CHUNK;
-    uint32_t issued = 0u, chunk = 0u;
-    if (use_tma) {
-        if (t == 0) {
-            mbar_init(a_bar, 1u); mbar_init(a_bar + 8u, 1u);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (t == 0) issue_entries(tile_entries, range.x, (uint32_t)RT_CHUNK, a_ent, a_bar, 0);
-        issued = 1u;
-    }
-    for (uint32_t base = range.x; base < range.y; base += RT_CHUNK, ++chunk) {
+    PairStream ps(tile_entries, s_ent, s_bar, range, range.y > range.x && range.y - range.x > (uint32_t)RT_CHUNK);
+    for (uint32_t base = range.x; base < range.y; base += RT_CHUNK, ++ps.chunk) {
         if (__syncthreads_count((lim0 > 0.f || lim1 > 0.f) ? 1 : 0) == 0) break;   // also fences smem reuse
         const uint32_t cnt = min((uint32_t)RT_CHUNK, range.y - base);
-        const int buf = (int)(chunk & 1u);
-        if (use_tma) {
-            // prefetch the NEXT chunk's entries (its buffer was last read two iterations ago: the vote above fenced it)
-            if (base + RT_CHUNK < range.y) {
-                if (t == 0) issue_entries(tile_entries, base + RT_CHUNK, min((uint32_t)RT_CHUNK, range.y - base - RT_CHUNK), a_ent, a_bar, buf ^ 1);
-                ++issued;
-            }
-            mbar_wait(a_bar + 8u * buf, (chunk >> 1) & 1u);
-        }
+        ps.next(base);
 #pragma unroll
         for (int k = 0; k < RT_CHUNK / R2_THREADS; ++k) {
             const uint32_t j = t + k * R2_THREADS;
             if (j < cnt) {
-                const uint32_t r = use_tma ? s_ent[buf][(base & 3u) + j] : __ldg(tile_entries + base + j);
+                const uint32_t r = ps.entry(base, j);
                 const float4* rp = reinterpret_cast<const float4*>(recs + r);
                 s_q0[j] = __ldg(rp);
                 s_uv[j] = __ldg(rp + 1);
@@ -538,43 +545,26 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
             }
         }
         __syncthreads();
-        // per-warp candidate list: splats whose bbox reaches this warp's rows (the x extent already meets the tile)
-        uint32_t nl = 0;
-        if (__any_sync(0xffffffffu, lim0 > 0.f || lim1 > 0.f)) {
-            for (uint32_t j0 = 0; j0 < cnt; j0 += 32) {
-                const uint32_t j = j0 + lane;
-                bool hit = false;
-                if (j < cnt) {
-                    const uint32_t by = __float_as_uint(s_uv[j].w);
-                    hit = !((int)(by >> 16) < wy0 || (int)(by & 0xFFFFu) > wy0 + 3);
-                }
-                const uint32_t m = __ballot_sync(0xffffffffu, hit);
-                if (hit) s_list[nl + __popc(m & lanemask_lt())] = (unsigned short)(j * 16u);
-                nl += __popc(m);
-            }
-            __syncwarp();
-        }
+        // per-warp candidate list: splats whose bbox reaches this warp's rows (the x extent already meets the tile),
+        // listed by offset of q0[j] from s_mem
+        const uint32_t nl = !__any_sync(0xffffffffu, lim0 > 0.f || lim1 > 0.f) ? 0u : compact_candidates(cnt, s_list, 0u, [&](uint32_t j) {
+            const uint32_t by = __float_as_uint(s_uv[j].w);
+            return !((int)(by >> 16) < wy0 || (int)(by & 0xFFFFu) > wy0 + 3);
+        });
         if (lim0 > 0.f || lim1 > 0.f) {
             const uint32_t a_end = a_list + nl * 2u;
             for (uint32_t a_it = a_list; a_it != a_end; a_it += 2u) {
-                uint32_t off;
-                asm volatile("ld.shared.u16 %0, [%1];" : "=r"(off) : "r"(a_it));
-                const uint32_t a_rec = a_base + off;
-                float4 q0; float2 q1;
-                asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(q0.x), "=f"(q0.y), "=f"(q0.z), "=f"(q0.w) : "r"(a_rec));
-                asm volatile("ld.shared.v2.f32 {%0,%1}, [%2+4096];" : "=f"(q1.x), "=f"(q1.y) : "r"(a_rec));
-                const float dy = __fsub_rn(fy, q0.y);
-                const float dxa = __fsub_rn(fx0, q0.x), dxb = __fsub_rn(fx1, q0.x);
-                const float ua = __fmaf_rn(q0.w, dy, __fmul_rn(q0.z, dxa)), va = __fmaf_rn(q1.y, dy, __fmul_rn(q1.x, dxa));
-                const float ub = __fmaf_rn(q0.w, dy, __fmul_rn(q0.z, dxb)), vb = __fmaf_rn(q1.y, dy, __fmul_rn(q1.x, dxb));
-                const bool ca = fabsf(ua) <= lim0 && fabsf(va) <= lim0;
-                const bool cb = fabsf(ub) <= lim1 && fabsf(vb) <= lim1;
+                const uint32_t a_rec = a_base + lds_u16(a_it);
+                const float4 q0 = lds4(a_rec);
+                const float2 q1 = lds2(a_rec + REC_UV);
+                const float2 uva = quad_uv(fx0, fy, q0, q1), uvb = quad_uv(fx1, fy, q0, q1);   // (dy is computed once)
+                const bool ca = fabsf(uva.x) <= lim0 && fabsf(uva.y) <= lim0;
+                const bool cb = fabsf(uvb.x) <= lim1 && fabsf(uvb.y) <= lim1;
                 if (!(ca || cb)) continue;
-                float4 q2;
-                asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4+8192];" : "=f"(q2.x), "=f"(q2.y), "=f"(q2.z), "=f"(q2.w) : "r"(a_rec));
+                const float4 q2 = lds4(a_rec + REC_Q2);
                 if (ca) {
                     float e;
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(__fmaf_rn(va, va, __fmul_rn(ua, ua)) * -6.492127684f));
+                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(__fmaf_rn(uva.y, uva.y, __fmul_rn(uva.x, uva.x)) * -6.492127684f));
                     const float a = fminf(e * q2.w, 0.999f);
                     const float w = a * T0;
                     r0 = fmaf(w, q2.x, r0); g0 = fmaf(w, q2.y, g0); b0 = fmaf(w, q2.z, b0);
@@ -583,7 +573,7 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
                 }
                 if (cb) {
                     float e;
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(__fmaf_rn(vb, vb, __fmul_rn(ub, ub)) * -6.492127684f));
+                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(__fmaf_rn(uvb.y, uvb.y, __fmul_rn(uvb.x, uvb.x)) * -6.492127684f));
                     const float a = fminf(e * q2.w, 0.999f);
                     const float w = a * T1;
                     r1 = fmaf(w, q2.x, r1); g1 = fmaf(w, q2.y, g1); b1 = fmaf(w, q2.z, b1);
@@ -594,8 +584,7 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
             }
         }
     }
-    // an early exit (all pixels saturated) may leave one prefetch in flight: keep the CTA alive until it lands
-    if (t == 0 && issued > chunk) mbar_wait(a_bar + 8u * (chunk & 1u), (chunk >> 1) & 1u);
+    ps.finish();
     if (CHUNKED && !last) {
         st[0] = make_float4(r0, g0, b0, T0);
         st[1] = make_float4(r1, g1, b1, T1);
@@ -613,23 +602,20 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
                    const float4* aux, void* out_depth, void* out_normal, cudaStream_t stream) {
     const int grid = tiles_x * tiles_y;
-    if (aux != nullptr) {          // colour + depth + normal in one pass (bgs_render_aux)
-        if (mode == 0) raster_kernel<0, true><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal);
-        else if (mode == 1) raster_kernel<1, true><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal);
-        else raster_kernel<2, true><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal);
-        return;
-    }
     // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
     // pixels (more of its lanes then idle at the tile's splat boundaries)
-    if (mode == 0 && large_footprints)
+    if (aux == nullptr && mode == 0 && large_footprints) {
         raster2_kernel<false><<<grid, R2_THREADS, 0, stream>>>(recs, tile_entries, ranges, W, H, tiles_x, out, format,
                                                                nullptr, nullptr, nullptr, 1, 1);
-    else if (mode == 0)
-        raster_kernel<0, false><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr);
-    else if (mode == 1)
-        raster_kernel<1, false><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr);
-    else
-        raster_kernel<2, false><<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr);
+        return;
+    }
+    // aux != nullptr: colour + depth + normal in one pass (bgs_render_aux)
+    static void (*const kernels[2][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*,
+                                       uint32_t, const float4*, void*, void*) = {
+        {raster_kernel<0, false>, raster_kernel<1, false>, raster_kernel<2, false>},
+        {raster_kernel<0, true>, raster_kernel<1, true>, raster_kernel<2, true>}};
+    kernels[aux != nullptr][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
+        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal);
 }
 
 // One front-to-back round of a chunked frame (quad-uv records only); see raster2_kernel.
