@@ -12,4 +12,4 @@ from .io import load_cloud, parse_ply_3d  # noqa: F401
 from .gcloud import decode_gcloud, encode_gcloud, read_gcloud, write_gcloud  # noqa: F401
 from .plugin import CloudTransform, GaussianSplattingPlugin, PlanarGaussian3dHandle  # noqa: F401
 from .settings import (CloudSettings, DrawMode, GaussianColorSpace, GaussianMode, RadixSortDepthBits,  # noqa: F401
-                       RasterizeMode, ShaderDefines, SortMode)
+                       RasterizeMode, ShaderDefines, SortMode, SparseSelect)

@@ -82,6 +82,9 @@ SYMBOLS = [
     ("bgs_cloud_upload_f16", C.c_int, [_P, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
     ("bgs_cloud_upload_f16_cov", C.c_int, [_P, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
     ("bgs_cloud_destroy", None, [_P]),
+    ("bgs_cloud_select_sparse", C.c_int, [_P, _P, C.c_float, C.c_uint32, C.POINTER(C.c_uint32)]),
+    ("bgs_cloud_visibility_get", C.c_int, [_P, _P, _P]),
+    ("bgs_cloud_visibility_set", C.c_int, [_P, _P, _P]),
     ("bgs_render", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P,
                              C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,

@@ -2,6 +2,7 @@
 // frame (stage orchestration on one CUDA stream), parity/debug hooks, stage timing.
 //
 // No PyTorch, no wgpu, no CPU fallback: every stage is a hand-written sm_90a kernel.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -51,6 +52,15 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
                          uint32_t* tiles_done, int first, int last, cudaStream_t stream);
+// select.cu
+uint32_t select_num_buckets(uint32_t n);
+int select_sort_passes(uint32_t n_buckets);
+void launch_select_keys(const float4* pos, uint32_t n, float radius, uint32_t n_buckets, uint32_t* keys, uint32_t* vals,
+                        uint32_t* n_sort, cudaStream_t stream);
+void launch_select_count(const float4* pos, const uint32_t* ids, const uint2* ranges, uint32_t n, float radius, uint32_t n_buckets,
+                         float r2, uint32_t threshold, float4* spos, float* pos_w, float* block_w, uint32_t block_stride,
+                         uint32_t* selected, cudaStream_t stream);
+void launch_select_fill(uint32_t n, float v, float* pos_w, float* block_w, uint32_t block_stride, cudaStream_t stream);
 }  // namespace bgs
 
 using namespace bgs;
@@ -139,6 +149,9 @@ struct bgs_context {
     DevBuf<void> status_depth;        // [4][tiles(status_n)][256]
     DevBuf<void> status_pairs;        // [4][tiles(status_np)][256]
     uint32_t status_n = 0, status_np = 0;
+    // bgs_cloud_select_sparse's own words, zeroed per call: sort count | sort barrier | selected | digit histograms |
+    // per-bucket ranges (the sort and the record buffer are the frame's, see bgs_cloud_select_sparse)
+    DevBuf<uint8_t> select_scratch;
     bool async_pending = false;        // a BGS_FLAG_ASYNC frame has been enqueued and not yet completed
     FrameCounters* ctr = nullptr;
     uint32_t* hist = nullptr;          // [8 + 4 * MAX_CHUNKS][256]: depth passes 0..3, pair passes 4..7 (round 0), 8 + 4r.. (round r)
@@ -156,7 +169,7 @@ struct bgs_context {
     // largest n_pairs_needed of ANY frame since the last bgs_sync / synchronous render (device word outside the
     // per-frame arena + its pinned copy): a queued async frame that overflowed the pair buffer is never missed
     uint32_t* d_sticky = nullptr;
-    uint32_t* h_sticky = nullptr;
+    uint32_t* h_sticky = nullptr;      // [0] the copy of *d_sticky, [1] bgs_cloud_select_sparse's selected count
     std::vector<bgs_cloud*> clouds;    // clouds uploaded through this context (their ctx is nulled on destroy)
 
     FrameFacts pend, last;
@@ -853,6 +866,96 @@ bgs_status bgs_render_aux(bgs_context* c, const bgs_cloud* cloud, const bgs_view
     if (c && (!out_rgba || !out_depth || !out_normal)) return fail(c, BGS_EINVAL, "render_aux: the three output frames are required");
     if (c && st && (st->flags & BGS_FLAG_ASYNC)) return fail(c, BGS_EINVAL, "render_aux: BGS_FLAG_ASYNC is not supported");
     return render_impl(c, cloud, view, uni, st, out_rgba, out_format, out_is_device_ptr, true, out_depth, out_normal);
+}
+
+// ---- selection edits of a resident cloud (select.cu).  The visibility lane lives twice on the device: the position
+// plane's .w (what key-gen streams) and the first 16 B of each gaussian-major block (what the projection reads): every
+// write updates both.
+
+// Before a selection writes a cloud: this context's queued frames are completed (their failure is returned, as a
+// synchronous render does), and so are the queued frames of every other context on the cloud's GPU, which may read it.
+static bgs_status quiesce_for_write(bgs_context* c, const bgs_cloud* cl) {
+    if (c->async_pending) TRY(bgs_sync(c));
+    std::lock_guard<std::mutex> lk(g_registry_mu);
+    for (bgs_context* o : g_contexts)
+        if (o != c && o->device == cl->device && o->async_pending)
+            o->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
+    return BGS_OK;
+}
+
+static size_t block_bytes(const bgs_cloud* cl) { return cl->f16 ? 128 : 256; }
+
+bgs_status bgs_cloud_select_sparse(bgs_context* c, bgs_cloud* cl, float radius, uint32_t threshold, uint32_t* out_selected) {
+    if (!c) return BGS_EINVAL;
+    if (!cl) return fail(c, BGS_EINVAL, "select_sparse: null cloud");
+    if (!(radius >= 0.0f) || std::isinf(radius)) return fail(c, BGS_EINVAL, "select_sparse: radius must be finite and >= 0");
+    if (cl->device != c->device) return fail(c, BGS_EINVAL, "select_sparse: cloud lives on another device");
+    CU(c, cudaSetDevice(c->device));
+    TRY(quiesce_for_write(c, cl));
+    const uint32_t n = cl->n;
+    const float r2 = radius * radius;
+    float* pos_w = reinterpret_cast<float*>(cl->pos) + 3;
+    float* block_w = reinterpret_cast<float*>(cl->blocks) + 3;
+    const uint32_t stride = (uint32_t)(block_bytes(cl) / 4);
+    cudaStream_t q = c->stream;
+    uint32_t selected = 0;
+    if (threshold == 0u || r2 == 0.0f) {
+        // no count can reach a threshold of 0; no distance is below a radius whose square is 0 (every count is 0)
+        selected = threshold == 0u ? 0u : n;
+        launch_select_fill(n, threshold == 0u ? 0.0f : 1.0f, pos_w, block_w, stride, q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaStreamSynchronize(q));
+    } else {
+        // the frame's scratch: key / value ping-pong buffers and depth-sort status rows (the sort), the record buffer
+        // (positions in bucket order).  The debug hooks lose the last frame; the hints the next frame plans from stay.
+        TRY(ensure_cloud_scratch(c, n));
+        TRY(ensure_status(c, c->status_depth, c->status_n, n));
+        const uint32_t nb = select_num_buckets(n);
+        const int passes = select_sort_passes(nb);
+        const size_t o_hist = 256, o_rng = o_hist + 4 * 256 * 4;
+        TRY(c->select_scratch.grow(c, o_rng + ((size_t)nb + 1) * sizeof(uint2), false));
+        c->have_frame = false;
+        uint32_t* words = reinterpret_cast<uint32_t*>(c->select_scratch.p);   // [0] sort count, [1] barrier, [2] selected
+        uint32_t* hist = reinterpret_cast<uint32_t*>(c->select_scratch.p + o_hist);
+        uint2* ranges = reinterpret_cast<uint2*>(c->select_scratch.p + o_rng);   // nb + 1: the sentinel key's too
+        CU(c, cudaMemsetAsync(c->select_scratch.p, 0, o_rng + ((size_t)nb + 1) * sizeof(uint2), q));
+        launch_select_keys(cl->pos, n, radius, nb, c->keys[0].p, c->vals[0].p, &words[0], q);
+        CU(c, cudaGetLastError());
+        CU(c, launch_radix_sort(c->keys[0].p, c->vals[0].p, c->keys[1].p, c->vals[1].p, &words[0], n, n, hist, 1,
+                                c->status_depth.p, (size_t)radix_num_tiles(c->status_n) * 256, next_epoch(c), &words[1], passes,
+                                0, ranges, c->sm_count, c->rs_per_sm, q));
+        launch_select_count(cl->pos, c->vals[passes & 1].p, ranges, n, radius, nb, r2, threshold,
+                            reinterpret_cast<float4*>(c->recs.p), pos_w, block_w, stride, &words[2], q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaMemcpyAsync(c->h_sticky + 1, &words[2], 4, cudaMemcpyDeviceToHost, q));
+        CU(c, cudaStreamSynchronize(q));
+        selected = c->h_sticky[1];
+    }
+    if (out_selected) *out_selected = selected;
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_visibility_get(bgs_context* c, const bgs_cloud* cl, float* out_vis) {
+    if (!c) return BGS_EINVAL;
+    if (!cl || !out_vis) return fail(c, BGS_EINVAL, "visibility_get: null cloud or array");
+    if (cl->device != c->device) return fail(c, BGS_EINVAL, "visibility_get: cloud lives on another device");
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaMemcpy2DAsync(out_vis, 4, reinterpret_cast<const char*>(cl->pos) + 12, 16, 4, cl->n, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_visibility_set(bgs_context* c, bgs_cloud* cl, const float* vis) {
+    if (!c) return BGS_EINVAL;
+    if (!cl || !vis) return fail(c, BGS_EINVAL, "visibility_set: null cloud or array");
+    if (cl->device != c->device) return fail(c, BGS_EINVAL, "visibility_set: cloud lives on another device");
+    CU(c, cudaSetDevice(c->device));
+    TRY(quiesce_for_write(c, cl));
+    CU(c, cudaMemcpy2DAsync(reinterpret_cast<char*>(cl->pos) + 12, 16, vis, 4, 4, cl->n, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpy2DAsync(reinterpret_cast<char*>(cl->blocks) + 12, block_bytes(cl), vis, 4, 4, cl->n, cudaMemcpyHostToDevice,
+                            c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
 }
 
 bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {

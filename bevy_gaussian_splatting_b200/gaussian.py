@@ -40,9 +40,17 @@ class PlanarGaussian3d:
     def __len__(self) -> int:
         return len(self.position_visibility)
 
-    def subset(self, n: int) -> "PlanarGaussian3d":
-        return PlanarGaussian3d(self.position_visibility[:n], self.spherical_harmonic[:n], self.rotation[:n],
-                                self.scale_opacity[:n])
+    def subset(self, n) -> "PlanarGaussian3d":
+        """An int: the first n gaussians.  An index array: those gaussians, in that order -- what the reference's
+        save_selection (src/query/select.rs:156-176) writes out for a selection."""
+        if np.ndim(n) == 0:
+            return PlanarGaussian3d(self.position_visibility[:n], self.spherical_harmonic[:n], self.rotation[:n],
+                                    self.scale_opacity[:n])
+        idx = np.asarray(n)
+        if idx.dtype.kind not in "iu":
+            raise TypeError("subset: indices must be integers")
+        return PlanarGaussian3d(self.position_visibility[idx], self.spherical_harmonic[idx], self.rotation[idx],
+                                self.scale_opacity[idx])
 
     # ---- f16 planar layout (src/gaussian/f16.rs:30-56,244-263; planar.wgsl:117-176) -----------------
     def compute_aabb(self) -> tuple[np.ndarray, np.ndarray]:

@@ -19,7 +19,7 @@ import numpy as np
 from . import abi
 from .camera import GaussianCamera, View
 from .gaussian import PlanarGaussian3d
-from .settings import CloudSettings
+from .settings import CloudSettings, SparseSelect
 
 
 def _ptr(a: np.ndarray):
@@ -184,6 +184,46 @@ class GaussianSplattingPlugin:
             return False
         self._check(st)
         return True
+
+    # -- selection: the visibility lane DrawMode::Selected / HighlightSelected read, edited in place (no re-upload)
+    def select_sparse(self, handle: PlanarGaussian3dHandle, query: SparseSelect | None = None) -> int:
+        """SparseSelect (src/query/sparse.rs:24-54) on the GPU: visibility 1 where fewer than `neighbor_threshold`
+        gaussians (itself included) lie within `radius`, else 0 (the exact rule: include/bgs.h).  Returns how many
+        were selected.  The debug hooks and frame stats are not ready again until the next render."""
+        q = query if query is not None else SparseSelect()
+        sel = C.c_uint32()
+        self._check(self._lib.bgs_cloud_select_sparse(self._ctx, handle._h, C.c_float(q.radius), C.c_uint32(q.neighbor_threshold),
+                                                      C.byref(sel)))
+        return int(sel.value)
+
+    def visibility(self, handle: PlanarGaussian3dHandle) -> np.ndarray:
+        """The visibility lane of every gaussian, (n,) float32."""
+        out = np.empty(handle.n, np.float32)
+        self._check(self._lib.bgs_cloud_visibility_get(self._ctx, handle._h, _ptr(out)))
+        return out
+
+    def set_visibility(self, handle: PlanarGaussian3dHandle, vis) -> None:
+        vis = np.ascontiguousarray(vis, np.float32)
+        if vis.shape != (handle.n,):
+            raise ValueError(f"visibility must have shape ({handle.n},)")
+        self._check(self._lib.bgs_cloud_visibility_set(self._ctx, handle._h, _ptr(vis)))
+
+    def apply_selection(self, handle: PlanarGaussian3dHandle, indices) -> None:
+        """src/query/select.rs:81-110: visibility 0 everywhere, 1 at `indices`."""
+        idx = np.asarray(indices).reshape(-1)
+        if idx.size and (idx.dtype.kind not in "iu" or idx.min() < 0 or idx.max() >= handle.n):
+            raise IndexError(f"selection indices must be integers in [0, {handle.n})")
+        vis = np.zeros(handle.n, np.float32)
+        vis[idx] = 1.0
+        self.set_visibility(handle, vis)
+
+    def invert_selection(self, handle: PlanarGaussian3dHandle) -> None:
+        """src/query/select.rs:116-150 on a 0/1 lane: visibility == 0.0 becomes 1, everything else 0."""
+        self.set_visibility(handle, (self.visibility(handle) == 0.0).astype(np.float32))
+
+    def selection(self, handle: PlanarGaussian3dHandle) -> np.ndarray:
+        """Indices of the selected gaussians: visibility >= 0.5, the ones DrawMode::Selected draws."""
+        return np.flatnonzero(self.visibility(handle) >= 0.5).astype(np.uint32)
 
     # -- parity / measurement hooks
     def frame_stats(self) -> abi.bgs_frame_stats:

@@ -73,6 +73,16 @@ class ShaderDefines:
 
 
 @dataclasses.dataclass
+class SparseSelect:
+    """src/query/sparse.rs:24-38, same field names and defaults: select the gaussians with fewer than
+    `neighbor_threshold` gaussians (themselves included) within `radius` -- the floater filter
+    (`GaussianSplattingPlugin.select_sparse`)."""
+
+    radius: float = 0.05
+    neighbor_threshold: int = 3
+
+
+@dataclasses.dataclass
 class CloudSettings:
     """src/gaussian/settings.rs:90-133, same field names and defaults."""
 

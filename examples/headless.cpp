@@ -2,9 +2,11 @@
 // examples/headless.rs (offscreen target, camera at (0, 1.5, 5), random cloud, one frame written to disk).
 //
 //   headless [count=100000] [width=1920] [height=1080] [global_scale=1.0] [out=headless_output/0.ppm]
-//            [--dump-cloud file] [--raw file]
+//            [--dump-cloud file] [--raw file] [--remove-floaters radius]
 // --dump-cloud writes the four f32 planes (n, then pos_vis, sh, rot, scale_opacity) so another host can
-// render the identical cloud; --raw writes the RGBA8 frame bytes.
+// render the identical cloud; --raw writes the RGBA8 frame bytes.  --remove-floaters selects the sparse gaussians
+// (SparseSelect with that radius), inverts the selection and draws only the rest (DrawMode::Selected), the
+// reference converter's floater filter (tools/ply_to_gcloud.rs:54-66) applied to the resident cloud.
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -17,11 +19,13 @@
 int main(int argc, char** argv) {
     size_t count = 100000; int W = 1920, H = 1080; float scale = 1.0f;
     std::string out = "headless_output/0.ppm", dump, raw;
+    float floater_radius = 0.0f;
     int pos = 0;
     for (int i = 1; i < argc; ++i) {
         const std::string a = argv[i];
         if (a == "--dump-cloud" && i + 1 < argc) { dump = argv[++i]; continue; }
         if (a == "--raw" && i + 1 < argc) { raw = argv[++i]; continue; }
+        if (a == "--remove-floaters" && i + 1 < argc) { floater_radius = (float)std::atof(argv[++i]); continue; }
         switch (pos++) {
             case 0: count = std::strtoull(a.c_str(), nullptr, 10); break;
             case 1: W = std::atoi(a.c_str()); break;
@@ -36,6 +40,14 @@ int main(int argc, char** argv) {
         bgs::PlanarGaussian3dHandle handle = plugin.add_cloud(cloud);
         bgs::CloudSettings settings;
         settings.global_scale = scale;
+        if (floater_radius > 0.0f) {
+            bgs::SparseSelect query;
+            query.radius = floater_radius;
+            const uint32_t sparse = plugin.select_sparse(handle, query);
+            plugin.invert_selection(handle);
+            settings.draw_mode = bgs::DrawMode::Selected;
+            std::printf("floaters: %u of %zu gaussians hidden\n", sparse, count);
+        }
         const bgs_view view = bgs::headless_view(W, H);
         std::vector<unsigned char> frame((size_t)W * H * 4);
         bool drawn = false;

@@ -131,6 +131,40 @@ bgs_status bgs_cloud_upload_f16_cov(bgs_context* ctx, uint32_t n, const float* p
                                     const uint32_t* cov3d_opacity, bgs_cloud** out);
 void bgs_cloud_destroy(bgs_cloud* cloud);
 
+/* Selection edits of a resident cloud: the visibility lane (pos_vis[4i + 3]) that DrawMode::Selected and
+ * HighlightSelected read, changed in place without a re-upload.  All three calls are synchronous.
+ *
+ * bgs_cloud_select_sparse: SparseSelect (src/query/sparse.rs:24-54).  Sets each gaussian's visibility to 1.0 when
+ * fewer than neighbor_threshold gaussians (itself included) lie within `radius` of it, else to 0.0.  Returns how many
+ * were set to 1 in *out_selected (may be NULL).  The rule, exactly:
+ *   - positions are the plane's x, y, z as uploaded (cloud-local: no model transform, no global_scale); every gaussian
+ *     takes part, whatever its current visibility;
+ *   - count_i = #{j : d2 < r2}, j == i included, d2 = ((dx*dx + dy*dy) + dz*dz), dx = x_j - x_i (likewise y, z),
+ *     r2 = radius*radius rounded to f32, every operation f32 round-to-nearest-even without FMA (the order of
+ *     `distance += diff * diff` from zero);
+ *   - gaussian i is selected iff count_i < neighbor_threshold.
+ *   So a non-finite position has a NaN d2 against everything, itself included: its count is 0.  radius == 0 counts
+ *   nothing (every gaussian is selected when neighbor_threshold > 0); neighbor_threshold == 0 selects nothing.
+ *   The reference delegates the comparison to the kd-tree 0.6.2 crate, absent here: `<` against `<=` and the
+ *   accumulation order are **unpinned**.
+ *   radius NaN, infinite or negative -> BGS_EINVAL.
+ *   Cost: a hashed uniform grid (cells just over `radius`), one radix sort, and a scan of the 27 neighbour cells that
+ *   stops once a count reaches neighbor_threshold.  A radius that puts most of the cloud into one cell (also: a radius
+ *   below max|coordinate| * 2^-40, where cell coordinates saturate) with a large threshold costs O(N x threshold).
+ *   It reuses the context's scratch (sort buffers and records): bgs_debug_* hooks, bgs_frame_stats_get and
+ *   bgs_stage_times_us return BGS_NOT_READY, and bgs_frame_device_ptr NULL, until the next render.  The next frame's
+ *   plan does not change (the hints it is planned from are kept).
+ * bgs_cloud_visibility_get / _set: the visibility lane of every gaussian, n floats to / from host memory (_set writes
+ *   the values as given: a 0/1 array built on the host covers Select, its inversion and any host-side labelling).
+ * The writers (select_sparse, visibility_set) first complete this context's queued (BGS_FLAG_ASYNC) frames, as a
+ * synchronous render does, returning their failure if there is one; and they wait for the queued frames of every
+ * other context on the cloud's GPU (which may read this cloud), as bgs_cloud_destroy does.
+ * A null cloud or array, or a cloud on another device than the context's -> BGS_EINVAL. */
+bgs_status bgs_cloud_select_sparse(bgs_context* ctx, bgs_cloud* cloud, float radius, uint32_t neighbor_threshold,
+                                   uint32_t* out_selected /* may be NULL */);
+bgs_status bgs_cloud_visibility_get(bgs_context* ctx, const bgs_cloud* cloud, float* out_vis);
+bgs_status bgs_cloud_visibility_set(bgs_context* ctx, bgs_cloud* cloud, const float* vis);
+
 /* One view of one cloud: key-gen -> depth radix sort -> projection + SH colour -> tile
  * binning -> per-tile front-to-back blend.  out_rgba is caller-owned (host pointer, or a
  * device pointer when out_is_device_ptr != 0); may be NULL to keep the frame on the device. */

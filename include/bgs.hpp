@@ -53,6 +53,11 @@ struct CloudSettings {   // src/gaussian/settings.rs:110-133 (defaults)
     }
 };
 
+struct SparseSelect {   // src/query/sparse.rs:24-38 (defaults): the floater filter
+    float radius = 0.05f;
+    uint32_t neighbor_threshold = 3;
+};
+
 struct ShaderDefines {   // src/render/mod.rs:698-760: the radix pass plan
     uint32_t radix_bits_per_digit, radix_digit_places, radix_key_shift, radix_base;
     static ShaderDefines for_radix_depth_bits(RadixSortDepthBits b) {
@@ -230,6 +235,45 @@ public:
         if (st == BGS_NOT_READY) return false;
         check(st);
         return true;
+    }
+    // Selection edits of a resident cloud: the visibility lane DrawMode::Selected / HighlightSelected read (bgs.h).
+    // select_sparse: SparseSelect (src/query/sparse.rs:24-54) on the GPU; returns how many were selected.
+    uint32_t select_sparse(PlanarGaussian3dHandle& cloud, const SparseSelect& query = {}) {
+        uint32_t selected = 0;
+        check(bgs_cloud_select_sparse(ctx_, cloud.get(), query.radius, query.neighbor_threshold, &selected));
+        return selected;
+    }
+    std::vector<float> visibility(const PlanarGaussian3dHandle& cloud) {
+        std::vector<float> v(cloud.len());
+        check(bgs_cloud_visibility_get(ctx_, cloud.get(), v.data()));
+        return v;
+    }
+    void set_visibility(PlanarGaussian3dHandle& cloud, const std::vector<float>& vis) {
+        if (vis.size() != cloud.len()) throw Error(BGS_EINVAL, "set_visibility: one value per gaussian");
+        check(bgs_cloud_visibility_set(ctx_, cloud.get(), vis.data()));
+    }
+    // src/query/select.rs:81-110: visibility 0 everywhere, 1 at `indices`
+    void apply_selection(PlanarGaussian3dHandle& cloud, const std::vector<uint32_t>& indices) {
+        std::vector<float> v(cloud.len(), 0.0f);
+        for (uint32_t i : indices) {
+            if (i >= cloud.len()) throw Error(BGS_EINVAL, "apply_selection: index out of range");
+            v[i] = 1.0f;
+        }
+        set_visibility(cloud, v);
+    }
+    // src/query/select.rs:116-150 on a 0/1 lane: visibility == 0 becomes 1, everything else 0
+    void invert_selection(PlanarGaussian3dHandle& cloud) {
+        std::vector<float> v = visibility(cloud);
+        for (float& x : v) x = x == 0.0f ? 1.0f : 0.0f;
+        set_visibility(cloud, v);
+    }
+    // indices with visibility >= 0.5: the gaussians DrawMode::Selected draws
+    std::vector<uint32_t> selection(const PlanarGaussian3dHandle& cloud) {
+        const std::vector<float> v = visibility(cloud);
+        std::vector<uint32_t> idx;
+        for (uint32_t i = 0; i < (uint32_t)v.size(); ++i)
+            if (v[i] >= 0.5f) idx.push_back(i);
+        return idx;
     }
     bgs_frame_stats frame_stats() { bgs_frame_stats fs{}; check(bgs_frame_stats_get(ctx_, &fs)); return fs; }
     bgs_context* context() const { return ctx_; }
