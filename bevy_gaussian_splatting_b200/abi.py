@@ -22,6 +22,7 @@ BGS_FLAG_NO_CHUNKS = 4
 BGS_FLAG_CHUNKS = 8
 BGS_FLAG_PREMULTIPLIED_OUT = 16
 BGS_FLAG_BLEND_OVER_TARGET = 32
+BGS_SELECT_REPLACE, BGS_SELECT_ADD = 0, 1
 
 
 class bgs_view(C.Structure):
@@ -85,6 +86,7 @@ SYMBOLS = [
     ("bgs_cloud_select_sparse", C.c_int, [_P, _P, C.c_float, C.c_uint32, C.POINTER(C.c_uint32)]),
     ("bgs_cloud_visibility_get", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_visibility_set", C.c_int, [_P, _P, _P]),
+    ("bgs_cloud_select_in_mesh", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32, _P, C.c_uint32, C.POINTER(C.c_uint32)]),
     ("bgs_render", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P,
                              C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,

@@ -61,6 +61,22 @@ void launch_select_count(const float4* pos, const uint32_t* ids, const uint2* ra
                          float r2, uint32_t threshold, float4* spos, float* pos_w, float* block_w, uint32_t block_stride,
                          uint32_t* selected, cudaStream_t stream);
 void launch_select_fill(uint32_t n, float v, float* pos_w, float* block_w, uint32_t block_stride, cudaStream_t stream);
+// mesh_select.cu
+size_t mesh_words_bytes();
+size_t mesh_rec_bytes();
+void launch_mesh_setup(const float* verts, const uint32_t* idx, uint32_t nt, void* bin_rec, void* bin_box, void* glob_rec, void* words,
+                       cudaStream_t stream);
+void launch_mesh_levels(const void* bin_box, const void* words_host, void* words, cudaStream_t stream);
+void mesh_pick_level(const void* words_host, int* level, uint64_t* pairs, uint32_t* cells);
+void launch_mesh_emit(const void* bin_box, const void* words_host, int level, uint32_t* keys, uint32_t* vals, void* words,
+                      cudaStream_t stream);
+uint32_t* mesh_words_pairs(void* words);
+uint32_t* mesh_words_barrier(void* words);
+uint32_t* mesh_words_inside(void* words);
+uint32_t mesh_words_n_bin(const void* words_host);
+void launch_mesh_count(const float4* pos, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
+                       const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, float* pos_w,
+                       float* block_w, uint32_t block_stride, void* words, cudaStream_t stream);
 }  // namespace bgs
 
 using namespace bgs;
@@ -152,6 +168,9 @@ struct bgs_context {
     // bgs_cloud_select_sparse's own words, zeroed per call: sort count | sort barrier | selected | digit histograms |
     // per-bucket ranges (the sort and the record buffer are the frame's, see bgs_cloud_select_sparse)
     DevBuf<uint8_t> select_scratch;
+    // bgs_cloud_select_in_mesh's own scratch (never the frame's): words | vertices | indices | binned records | binned
+    // boxes | global records, and the pair side: digit histograms | per-cell ranges | pair keys / values x 2
+    DevBuf<uint8_t> mesh_tri, mesh_pairs;
     bool async_pending = false;        // a BGS_FLAG_ASYNC frame has been enqueued and not yet completed
     FrameCounters* ctr = nullptr;
     uint32_t* hist = nullptr;          // [8 + 4 * MAX_CHUNKS][256]: depth passes 0..3, pair passes 4..7 (round 0), 8 + 4r.. (round r)
@@ -169,7 +188,7 @@ struct bgs_context {
     // largest n_pairs_needed of ANY frame since the last bgs_sync / synchronous render (device word outside the
     // per-frame arena + its pinned copy): a queued async frame that overflowed the pair buffer is never missed
     uint32_t* d_sticky = nullptr;
-    uint32_t* h_sticky = nullptr;      // [0] the copy of *d_sticky, [1] bgs_cloud_select_sparse's selected count
+    uint32_t* h_sticky = nullptr;      // [0] the copy of *d_sticky, [1] a selection's selected / inside count
     std::vector<bgs_cloud*> clouds;    // clouds uploaded through this context (their ctx is nulled on destroy)
 
     FrameFacts pend, last;
@@ -955,6 +974,87 @@ bgs_status bgs_cloud_visibility_set(bgs_context* c, bgs_cloud* cl, const float* 
     CU(c, cudaMemcpy2DAsync(reinterpret_cast<char*>(cl->blocks) + 12, block_bytes(cl), vis, 4, 4, cl->n, cudaMemcpyHostToDevice,
                             c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_select_in_mesh(bgs_context* c, bgs_cloud* cl, const float* vertices, uint32_t nv, const uint32_t* indices,
+                                    uint32_t nt, const float* mesh_from_cloud, uint32_t mode, uint32_t* out_inside) {
+    if (!c) return BGS_EINVAL;
+    if (!cl) return fail(c, BGS_EINVAL, "select_in_mesh: null cloud");
+    if (nt > 0 && (!vertices || !indices)) return fail(c, BGS_EINVAL, "select_in_mesh: null vertices or indices");
+    if (mode != BGS_SELECT_REPLACE && mode != BGS_SELECT_ADD) return fail(c, BGS_EINVAL, "select_in_mesh: unknown mode %u", mode);
+    if (cl->device != c->device) return fail(c, BGS_EINVAL, "select_in_mesh: cloud lives on another device");
+    for (size_t k = 0; k < (size_t)nt * 3; ++k)
+        if (indices[k] >= nv) return fail(c, BGS_EINVAL, "select_in_mesh: index %u of triangle %zu is >= %u vertices", indices[k], k / 3, nv);
+    if (nt >= (1u << 26)) return fail(c, BGS_ENOMEM, "select_in_mesh: more than 2^26 triangles");
+    static const float identity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    const float* M = mesh_from_cloud ? mesh_from_cloud : identity;
+    CU(c, cudaSetDevice(c->device));
+    TRY(quiesce_for_write(c, cl));
+    const uint32_t n = cl->n;
+    float* pos_w = reinterpret_cast<float*>(cl->pos) + 3;
+    float* block_w = reinterpret_cast<float*>(cl->blocks) + 3;
+    const uint32_t stride = (uint32_t)(block_bytes(cl) / 4);
+    cudaStream_t q = c->stream;
+
+    // triangle side: setup (records, classes, grid bounds)
+    const size_t o_v = 256, o_i = align_up(o_v + (size_t)nv * 12, 256), o_br = align_up(o_i + (size_t)nt * 12, 256);
+    const size_t o_bb = o_br + (size_t)nt * mesh_rec_bytes(), o_gr = o_bb + (size_t)nt * 32, tri_bytes = o_gr + (size_t)nt * mesh_rec_bytes();
+    TRY(c->mesh_tri.grow(c, tri_bytes, false));
+    uint8_t* tb = c->mesh_tri.p;
+    void* words = tb;
+    std::vector<unsigned long long> wh_buf((mesh_words_bytes() + 7) / 8);
+    void* wh = wh_buf.data();
+    CU(c, cudaMemsetAsync(words, 0, 256, q));
+    if (nt > 0) {
+        CU(c, cudaMemcpyAsync(tb + o_v, vertices, (size_t)nv * 12, cudaMemcpyHostToDevice, q));
+        CU(c, cudaMemcpyAsync(tb + o_i, indices, (size_t)nt * 12, cudaMemcpyHostToDevice, q));
+        launch_mesh_setup(reinterpret_cast<const float*>(tb + o_v), reinterpret_cast<const uint32_t*>(tb + o_i), nt, tb + o_br,
+                          tb + o_bb, tb + o_gr, words, q);
+        CU(c, cudaGetLastError());
+    }
+    CU(c, cudaMemcpyAsync(wh, words, mesh_words_bytes(), cudaMemcpyDeviceToHost, q));
+    CU(c, cudaStreamSynchronize(q));
+
+    // grid side: the level, the pairs, their sort by cell
+    int level = -1;
+    const uint32_t* cell_tri = nullptr;
+    const uint2* ranges = nullptr;
+    if (mesh_words_n_bin(wh) > 0) {
+        launch_mesh_levels(tb + o_bb, wh, words, q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaMemcpyAsync(wh, words, mesh_words_bytes(), cudaMemcpyDeviceToHost, q));
+        CU(c, cudaStreamSynchronize(q));
+        uint64_t pairs64 = 0;
+        uint32_t cells = 0;
+        mesh_pick_level(wh, &level, &pairs64, &cells);
+        const uint32_t pairs = (uint32_t)pairs64;
+        const size_t o_rng = 4 * 256 * 4, o_k0 = align_up(o_rng + (size_t)cells * 8, 256), pw = align_up((size_t)pairs * 4, 256);
+        TRY(c->mesh_pairs.grow(c, o_k0 + 4 * pw, false));
+        TRY(ensure_status(c, c->status_pairs, c->status_np, pairs));
+        uint8_t* pb = c->mesh_pairs.p;
+        uint32_t* k0 = reinterpret_cast<uint32_t*>(pb + o_k0);
+        uint32_t* v0 = reinterpret_cast<uint32_t*>(pb + o_k0 + pw);
+        uint32_t* k1 = reinterpret_cast<uint32_t*>(pb + o_k0 + 2 * pw);
+        uint32_t* v1 = reinterpret_cast<uint32_t*>(pb + o_k0 + 3 * pw);
+        uint2* rng = reinterpret_cast<uint2*>(pb + o_rng);
+        CU(c, cudaMemsetAsync(pb, 0, o_k0, q));
+        launch_mesh_emit(tb + o_bb, wh, level, k0, v0, words, q);
+        CU(c, cudaGetLastError());
+        const int passes = pair_passes(cells);
+        CU(c, launch_radix_sort(k0, v0, k1, v1, mesh_words_pairs(words), pairs, pairs, reinterpret_cast<uint32_t*>(pb), 1,
+                                c->status_pairs.p, (size_t)radix_num_tiles(c->status_np) * 256, next_epoch(c),
+                                mesh_words_barrier(words), passes, 0, rng, c->sm_count, c->rs_per_sm, q));
+        cell_tri = (passes & 1) ? v1 : v0;
+        ranges = rng;
+    }
+
+    // point side: the count and the lane
+    launch_mesh_count(cl->pos, n, M, tb + o_br, tb + o_gr, cell_tri, ranges, wh, level, mode, pos_w, block_w, stride, words, q);
+    CU(c, cudaGetLastError());
+    CU(c, cudaMemcpyAsync(c->h_sticky + 1, mesh_words_inside(words), 4, cudaMemcpyDeviceToHost, q));
+    CU(c, cudaStreamSynchronize(q));
+    if (out_inside) *out_inside = c->h_sticky[1];
     return BGS_OK;
 }
 

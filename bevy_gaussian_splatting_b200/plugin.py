@@ -196,6 +196,31 @@ class GaussianSplattingPlugin:
                                                       C.byref(sel)))
         return int(sel.value)
 
+    def select_in_mesh(self, handle: PlanarGaussian3dHandle, vertices, indices, mesh_from_cloud=None, mode: str = "replace") -> int:
+        """Point-in-mesh selection (src/query/raycast.rs:54-124) on the GPU: a gaussian is inside when the +x ray from
+        mesh_from_cloud * position hits an odd number of triangles (the exact rule: include/bgs.h).  vertices (nv, 3)
+        float32, indices (nt, 3) uint32, mesh_from_cloud a 4x4 (row-major numpy, i.e. M @ p; None = identity).
+        mode "replace": visibility 1 inside, 0 elsewhere; "add": 1 inside, the rest untouched.  Returns how many are inside."""
+        modes = {"replace": abi.BGS_SELECT_REPLACE, "add": abi.BGS_SELECT_ADD}
+        if mode not in modes:
+            raise ValueError(f"mode must be one of {sorted(modes)}")
+        v = np.ascontiguousarray(vertices, np.float32)
+        i = np.ascontiguousarray(indices, np.uint32)
+        if v.ndim != 2 or v.shape[1] != 3:
+            raise ValueError("vertices must have shape (nv, 3)")
+        if i.ndim != 2 or i.shape[1] != 3:
+            raise ValueError("indices must have shape (nt, 3)")
+        m = None
+        if mesh_from_cloud is not None:
+            m = np.asarray(mesh_from_cloud, np.float32)
+            if m.shape != (4, 4):
+                raise ValueError("mesh_from_cloud must be 4x4")
+            m = np.ascontiguousarray(m.T)                     # column-major for the C ABI
+        inside = C.c_uint32()
+        self._check(self._lib.bgs_cloud_select_in_mesh(self._ctx, handle._h, _ptr(v), len(v), _ptr(i), len(i),
+                                                       None if m is None else _ptr(m), modes[mode], C.byref(inside)))
+        return int(inside.value)
+
     def visibility(self, handle: PlanarGaussian3dHandle) -> np.ndarray:
         """The visibility lane of every gaussian, (n,) float32."""
         out = np.empty(handle.n, np.float32)

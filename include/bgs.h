@@ -156,7 +156,7 @@ void bgs_cloud_destroy(bgs_cloud* cloud);
  *   plan does not change (the hints it is planned from are kept).
  * bgs_cloud_visibility_get / _set: the visibility lane of every gaussian, n floats to / from host memory (_set writes
  *   the values as given: a 0/1 array built on the host covers Select, its inversion and any host-side labelling).
- * The writers (select_sparse, visibility_set) first complete this context's queued (BGS_FLAG_ASYNC) frames, as a
+ * The writers (select_sparse, select_in_mesh, visibility_set) first complete this context's queued (BGS_FLAG_ASYNC) frames, as a
  * synchronous render does, returning their failure if there is one; and they wait for the queued frames of every
  * other context on the cloud's GPU (which may read this cloud), as bgs_cloud_destroy does.
  * A null cloud or array, or a cloud on another device than the context's -> BGS_EINVAL. */
@@ -164,6 +164,41 @@ bgs_status bgs_cloud_select_sparse(bgs_context* ctx, bgs_cloud* cloud, float rad
                                    uint32_t* out_selected /* may be NULL */);
 bgs_status bgs_cloud_visibility_get(bgs_context* ctx, const bgs_cloud* cloud, float* out_vis);
 bgs_status bgs_cloud_visibility_set(bgs_context* ctx, bgs_cloud* cloud, const float* vis);
+
+/* bgs_cloud_select_in_mesh: point-in-mesh selection (src/query/raycast.rs:54-124, RaycastSelectionPlugin).  A
+ * gaussian is inside a triangle mesh iff the ray from its position along +x hits an odd number of its triangles.
+ * mode BGS_SELECT_REPLACE: visibility := inside ? 1.0 : 0.0.  BGS_SELECT_ADD: visibility := 1.0 where inside, left
+ * untouched elsewhere (the reference's sticky InsideMesh marker across several meshes; subtract is invert, ADD,
+ * invert).  *out_inside (may be NULL) = how many gaussians are inside.  The rule, exactly:
+ *   - q = mesh_from_cloud * (x, y, z, 1), (x, y, z) the plane's position as uploaded (cloud-local), mesh_from_cloud a
+ *     column-major 4x4 (NULL: identity; the reference's transform.to_matrix().inverse() is the caller's), each row
+ *     ((m_r0 x + m_r1 y) + m_r2 z) + m_r3; every gaussian takes part, whatever its current visibility;
+ *   - triangle k is (v[i[3k]], v[i[3k + 1]], v[i[3k + 2]]), vertices (nv, 3) f32, indices (nt, 3) u32;
+ *   - ray_intersects_triangle(q, dir = (1, 0, 0), tri) literally (raycast.rs:92-124): eps = 1e-6f; edge1 = v1 - v0,
+ *     edge2 = v2 - v0, h = dir x edge2, a = edge1 . h, miss if a > -eps && a < eps; f = 1 / a, s = q - v0,
+ *     u = f * (s . h), miss unless 0 <= u <= 1; q' = s x edge1, v = f * (dir . q'), miss if v < 0 || u + v > 1;
+ *     t = f * (edge2 . q'), hit iff t > eps.  dot = (x x' + y y') + z z', cross = (y z' - y' z, z x' - z' x,
+ *     x y' - x' y), the products with dir evaluated as written (0 * inf = NaN); every operation f32
+ *     round-to-nearest-even without FMA.  glam's operation order is assumed, not pinned: the glam crate is absent
+ *     here, so the order of its scalar Vec3 dot / cross / Mat4 transform is **unpinned**;
+ *   - inside iff the hit count is odd.
+ *   Consequences the rule keeps: a point on an edge shared by two triangles hits both (a ray through a shared edge
+ *   or vertex may flip parity); a triangle with |a| < 1e-6 (e.g. any whose yz extent is below ~1e-3: eps is
+ *   absolute) is never hit; an open or self-intersecting mesh gives whatever parity the rule gives; a non-finite
+ *   point or triangle is never hit.  nt == 0: nothing is inside.
+ *   Cost: a uniform grid over (y, z) binning the triangles, one radix sort of the (cell, triangle) pairs, and the
+ *   literal test of each gaussian against the triangles of its cell.  Slivers (edge^2 / |a| > 2^16), triangles with a
+ *   coordinate beyond 2^62 and gaussians with a coordinate of q beyond 2^62 are tested against everything instead.
+ *   Synchronous; the quiesce rules of the writers above.  It uses its own scratch, not the frame's: the bgs_debug_*
+ *   hooks, bgs_frame_stats_get and bgs_stage_times_us keep reporting the last frame, and the next frame's plan does
+ *   not change.
+ *   A null cloud, null vertices or indices with nt > 0, an index >= nv, an unknown mode, or a cloud on another device
+ *   -> BGS_EINVAL; a refused call changes nothing.  nt >= 2^26 -> BGS_ENOMEM. */
+enum { BGS_SELECT_REPLACE = 0u, BGS_SELECT_ADD = 1u };
+bgs_status bgs_cloud_select_in_mesh(bgs_context* ctx, bgs_cloud* cloud, const float* vertices /* nv * 3 */, uint32_t nv,
+                                    const uint32_t* indices /* nt * 3 */, uint32_t nt,
+                                    const float* mesh_from_cloud /* 16, column-major, may be NULL */, uint32_t mode,
+                                    uint32_t* out_inside /* may be NULL */);
 
 /* One view of one cloud: key-gen -> depth radix sort -> projection + SH colour -> tile
  * binning -> per-tile front-to-back blend.  out_rgba is caller-owned (host pointer, or a

@@ -243,6 +243,16 @@ public:
         check(bgs_cloud_select_sparse(ctx_, cloud.get(), query.radius, query.neighbor_threshold, &selected));
         return selected;
     }
+    // select_in_mesh: point-in-mesh selection (src/query/raycast.rs:54-124) on the GPU; vertices nv x 3, indices nt x 3,
+    // mesh_from_cloud column-major (nullptr = identity), mode BGS_SELECT_REPLACE / BGS_SELECT_ADD; returns how many are inside.
+    uint32_t select_in_mesh(PlanarGaussian3dHandle& cloud, const std::vector<float>& vertices, const std::vector<uint32_t>& indices,
+                            const float* mesh_from_cloud = nullptr, uint32_t mode = BGS_SELECT_REPLACE) {
+        if (vertices.size() % 3 || indices.size() % 3) throw Error(BGS_EINVAL, "select_in_mesh: vertices and indices come in threes");
+        uint32_t inside = 0;
+        check(bgs_cloud_select_in_mesh(ctx_, cloud.get(), vertices.data(), (uint32_t)(vertices.size() / 3), indices.data(),
+                                       (uint32_t)(indices.size() / 3), mesh_from_cloud, mode, &inside));
+        return inside;
+    }
     std::vector<float> visibility(const PlanarGaussian3dHandle& cloud) {
         std::vector<float> v(cloud.len());
         check(bgs_cloud_visibility_get(ctx_, cloud.get(), v.data()));

@@ -133,3 +133,276 @@ int orc_select_sparse_grid(uint32_t n, const float* pos, float radius, uint32_t 
 }
 
 }  // extern "C"
+
+// ---- point in mesh (src/query/raycast.rs:54-124) ----------------------------------------------------------------
+namespace {
+
+struct V3 {
+    float x, y, z;
+};
+V3 sub(V3 a, V3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
+// glam's scalar Vec3 order: dot = (x x' + y y') + z z', cross = (y z' - y' z, z x' - z' x, x y' - x' y)
+float dot(V3 a, V3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
+V3 cross(V3 a, V3 b) { return {a.y * b.z - b.y * a.z, a.z * b.x - b.z * a.x, a.x * b.y - b.x * a.y}; }
+constexpr float MS_EPS = 0.000001f;
+
+// raycast.rs:92-124, the definition
+bool ray_hits(V3 o, V3 v0, V3 v1, V3 v2) {
+    const V3 dir = {1.0f, 0.0f, 0.0f};
+    const V3 e1 = sub(v1, v0), e2 = sub(v2, v0);
+    const V3 h = cross(dir, e2);
+    const float a = dot(e1, h);
+    if (a > -MS_EPS && a < MS_EPS) return false;
+    const float f = 1.0f / a;
+    const V3 s = sub(o, v0);
+    const float u = f * dot(s, h);
+    if (!(u >= 0.0f && u <= 1.0f)) return false;
+    const V3 q = cross(s, e1);
+    const float v = f * dot(dir, q);
+    if (v < 0.0f || u + v > 1.0f) return false;
+    const float t = f * dot(e2, q);
+    return t > MS_EPS;
+}
+
+V3 xform(const float* m, const float* p) {   // column-major m, ((m_r0 x + m_r1 y) + m_r2 z) + m_r3
+    return {((m[0] * p[0] + m[4] * p[1]) + m[8] * p[2]) + m[12], ((m[1] * p[0] + m[5] * p[1]) + m[9] * p[2]) + m[13],
+            ((m[2] * p[0] + m[6] * p[1]) + m[10] * p[2]) + m[14]};
+}
+const float kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+V3 vert(const float* v, uint32_t i) { return {v[3 * (size_t)i], v[3 * (size_t)i + 1], v[3 * (size_t)i + 2]}; }
+bool bad_mesh(uint32_t nv, const float* verts, uint32_t nt, const uint32_t* idx) {
+    if (nt > 0 && (!verts || !idx)) return true;
+    for (size_t k = 0; k < (size_t)nt * 3; ++k)
+        if (idx[k] >= nv) return true;
+    return false;
+}
+uint32_t finish_mask(uint32_t n, const std::vector<uint32_t>& hits, uint8_t* mask) {
+    uint32_t in = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        mask[i] = hits[i] & 1u;
+        in += mask[i];
+    }
+    return in;
+}
+
+// ---- restated from bevy_gaussian_splatting_b200/csrc/mesh_select.cu (setup, classes, slack, grid ladder, cells) ----
+constexpr float MS_FAR = 4611686018427387904.0f;
+constexpr double MS_KAPPA_MAX = 65536.0;
+constexpr int MS_LEVELS = 13;
+constexpr uint32_t MS_MAX_DIM = 4096;
+bool ms_near(float x) { return std::fabs(x) < MS_FAR; }
+
+struct Rec {
+    V3 v0, e1, e2, h;
+    float f;
+};
+bool rec_hit(V3 o, const Rec& r) {
+    const V3 dir = {1.0f, 0.0f, 0.0f};
+    const V3 s = sub(o, r.v0);
+    const float u = r.f * dot(s, r.h);
+    if (!(u >= 0.0f && u <= 1.0f)) return false;
+    const V3 q = cross(s, r.e1);
+    const float v = r.f * dot(dir, q);
+    if (v < 0.0f || u + v > 1.0f) return false;
+    return r.f * dot(r.e2, q) > MS_EPS;
+}
+bool mesh_box(V3 v0, V3 v1, V3 v2, V3 e1, V3 e2, float a, double* box) {
+    if (!(ms_near(v0.x) && ms_near(v0.y) && ms_near(v0.z) && ms_near(v1.x) && ms_near(v1.y) && ms_near(v1.z) && ms_near(v2.x) &&
+          ms_near(v2.y) && ms_near(v2.z)))
+        return false;
+    const double E = std::fmax(std::fmax(std::fabs((double)e1.y), std::fabs((double)e1.z)),
+                               std::fmax(std::fabs((double)e2.y), std::fabs((double)e2.z)));
+    const double kappa = E * E / std::fabs((double)a);
+    if (!(kappa <= MS_KAPPA_MAX)) return false;
+    const double ylo = std::fmin(std::fmin((double)v0.y, (double)v1.y), (double)v2.y);
+    const double yhi = std::fmax(std::fmax((double)v0.y, (double)v1.y), (double)v2.y);
+    const double zlo = std::fmin(std::fmin((double)v0.z, (double)v1.z), (double)v2.z);
+    const double zhi = std::fmax(std::fmax((double)v0.z, (double)v1.z), (double)v2.z);
+    const double m = std::fmax(std::fmax(std::fabs(ylo), std::fabs(yhi)), std::fmax(std::fabs(zlo), std::fabs(zhi)));
+    const double slack = (kappa + 1.0) * E * (1.0 / 131072.0) + m * (1.0 / 1073741824.0) + 1e-30;
+    box[0] = ylo - slack;
+    box[1] = yhi + slack;
+    box[2] = zlo - slack;
+    box[3] = zhi + slack;
+    return true;
+}
+uint32_t mesh_cell(double p, double p0, double inv, uint32_t n) {
+    const double c = std::floor((p - p0) * inv);
+    return c < 0.0 ? 0u : (c >= (double)n ? n - 1u : (uint32_t)c);
+}
+struct Grid {
+    double y0, z0, inv_y, inv_z;
+    uint32_t ny, nz;
+};
+
+struct MeshPlan {
+    std::vector<Rec> bin, glob;
+    std::vector<double> box;   // 4 per binned record
+    double y0 = 0, y1 = 0, z0 = 0, z1 = 0;
+    std::vector<Grid> levels;
+    std::vector<uint64_t> level_pairs;
+    int level = -1;
+};
+
+MeshPlan plan_mesh(const float* verts, uint32_t nt, const uint32_t* idx) {
+    MeshPlan P;
+    for (uint32_t t = 0; t < nt; ++t) {
+        const V3 v0 = vert(verts, idx[3 * (size_t)t]), v1 = vert(verts, idx[3 * (size_t)t + 1]), v2 = vert(verts, idx[3 * (size_t)t + 2]);
+        const V3 e1 = sub(v1, v0), e2 = sub(v2, v0);
+        const V3 h = cross({1.0f, 0.0f, 0.0f}, e2);
+        const float a = dot(e1, h);
+        if ((a > -MS_EPS && a < MS_EPS) || !std::isfinite(a)) continue;
+        const Rec r = {v0, e1, e2, h, 1.0f / a};
+        double b[4];
+        if (mesh_box(v0, v1, v2, e1, e2, a, b)) {
+            P.bin.push_back(r);
+            P.box.insert(P.box.end(), b, b + 4);
+        } else {
+            P.glob.push_back(r);
+        }
+    }
+    const uint32_t nb = (uint32_t)P.bin.size();
+    if (nb == 0) return P;
+    P.y0 = P.z0 = INFINITY;
+    P.y1 = P.z1 = -INFINITY;
+    for (uint32_t b = 0; b < nb; ++b) {
+        P.y0 = std::fmin(P.y0, P.box[4 * b]);
+        P.y1 = std::fmax(P.y1, P.box[4 * b + 1]);
+        P.z0 = std::fmin(P.z0, P.box[4 * b + 2]);
+        P.z1 = std::fmax(P.z1, P.box[4 * b + 3]);
+    }
+    const double W = P.y1 - P.y0, H = P.z1 - P.z0;
+    const double side = std::sqrt(W * H / (2.0 * (double)nb));
+    auto dim = [&](double ext) {
+        const double d = std::ceil(ext / side);
+        return d >= (double)MS_MAX_DIM ? MS_MAX_DIM : (d >= 1.0 ? (uint32_t)d : 1u);
+    };
+    const uint32_t ny0 = side > 0.0 ? dim(W) : 1u, nz0 = side > 0.0 ? dim(H) : 1u;
+    for (int l = 0; l < MS_LEVELS; ++l) {
+        Grid g;
+        g.ny = ny0 >> l ? ny0 >> l : 1u;
+        g.nz = nz0 >> l ? nz0 >> l : 1u;
+        g.y0 = P.y0;
+        g.z0 = P.z0;
+        g.inv_y = (double)g.ny / W;
+        g.inv_z = (double)g.nz / H;
+        uint64_t pairs = 0;
+        for (uint32_t b = 0; b < nb; ++b) {
+            const double* x = &P.box[4 * (size_t)b];
+            pairs += (uint64_t)(mesh_cell(x[1], g.y0, g.inv_y, g.ny) - mesh_cell(x[0], g.y0, g.inv_y, g.ny) + 1u) *
+                     (mesh_cell(x[3], g.z0, g.inv_z, g.nz) - mesh_cell(x[2], g.z0, g.inv_z, g.nz) + 1u);
+        }
+        P.levels.push_back(g);
+        P.level_pairs.push_back(pairs);
+        if (g.ny == 1u && g.nz == 1u) break;
+    }
+    const uint64_t budget = (1ull << 24) + 4ull * nb;
+    int l = 0;
+    while (l + 1 < (int)P.levels.size() && P.level_pairs[l] > budget) ++l;
+    P.level = l;
+    return P;
+}
+
+}  // namespace
+
+extern "C" {
+
+int orc_select_in_mesh(uint32_t n, const float* pos_vis, uint32_t nv, const float* verts, uint32_t nt, const uint32_t* idx,
+                       const float* mesh_from_cloud, uint8_t* mask, uint32_t* out_inside, int threads) {
+    if (bad_mesh(nv, verts, nt, idx)) return -1;
+    const float* M = mesh_from_cloud ? mesh_from_cloud : kIdentity;
+    std::vector<uint32_t> hits(n, 0u);
+    if (threads > 0) omp_set_num_threads(threads);
+#pragma omp parallel for schedule(dynamic, 64)
+    for (long long i = 0; i < (long long)n; ++i) {
+        const V3 o = xform(M, pos_vis + 4 * i);
+        uint32_t c = 0;
+        for (uint32_t t = 0; t < nt; ++t)
+            c += ray_hits(o, vert(verts, idx[3 * (size_t)t]), vert(verts, idx[3 * (size_t)t + 1]), vert(verts, idx[3 * (size_t)t + 2]))
+                     ? 1u : 0u;
+        hits[i] = c;
+    }
+    const uint32_t in = finish_mask(n, hits, mask);
+    if (out_inside) *out_inside = in;
+    return 0;
+}
+
+int orc_select_in_mesh_grid(uint32_t n, const float* pos_vis, uint32_t nv, const float* verts, uint32_t nt, const uint32_t* idx,
+                            const float* mesh_from_cloud, uint8_t* mask, uint32_t* out_inside, int threads) {
+    if (bad_mesh(nv, verts, nt, idx)) return -1;
+    const float* M = mesh_from_cloud ? mesh_from_cloud : kIdentity;
+    const MeshPlan P = plan_mesh(verts, nt, idx);
+    const uint32_t nb = (uint32_t)P.bin.size();
+    // counting sort of the (cell, triangle) pairs by cell
+    Grid g{};
+    std::vector<uint32_t> start(1, 0u), tri;
+    if (P.level >= 0) {
+        g = P.levels[P.level];
+        const size_t cells = (size_t)g.ny * g.nz;
+        start.assign(cells + 1, 0u);
+        std::vector<uint32_t> keys, vals;
+        for (uint32_t b = 0; b < nb; ++b) {
+            const double* x = &P.box[4 * (size_t)b];
+            for (uint32_t z = mesh_cell(x[2], g.z0, g.inv_z, g.nz); z <= mesh_cell(x[3], g.z0, g.inv_z, g.nz); ++z)
+                for (uint32_t y = mesh_cell(x[0], g.y0, g.inv_y, g.ny); y <= mesh_cell(x[1], g.y0, g.inv_y, g.ny); ++y) {
+                    keys.push_back(z * g.ny + y);
+                    vals.push_back(b);
+                }
+        }
+        for (uint32_t k : keys) ++start[(size_t)k + 1];
+        for (size_t c = 0; c < cells; ++c) start[c + 1] += start[c];
+        tri.resize(keys.size());
+        std::vector<uint32_t> at(start.begin(), start.end() - 1);
+        for (size_t k = 0; k < keys.size(); ++k) tri[at[keys[k]]++] = vals[k];
+    }
+    std::vector<uint32_t> hits(n, 0u);
+    if (threads > 0) omp_set_num_threads(threads);
+#pragma omp parallel for schedule(dynamic, 256)
+    for (long long i = 0; i < (long long)n; ++i) {
+        const V3 q = xform(M, pos_vis + 4 * i);
+        uint32_t c = 0;
+        if (std::isfinite(q.x) && std::isfinite(q.y) && std::isfinite(q.z)) {
+            if (!(ms_near(q.x) && ms_near(q.y) && ms_near(q.z))) {
+                for (uint32_t b = 0; b < nb; ++b) c += rec_hit(q, P.bin[b]) ? 1u : 0u;
+            } else if (nb && (double)q.y >= P.y0 && (double)q.y <= P.y1 && (double)q.z >= P.z0 && (double)q.z <= P.z1) {
+                const size_t cell = (size_t)mesh_cell(q.z, g.z0, g.inv_z, g.nz) * g.ny + mesh_cell(q.y, g.y0, g.inv_y, g.ny);
+                for (uint32_t s = start[cell]; s < start[cell + 1]; ++s) c += rec_hit(q, P.bin[tri[s]]) ? 1u : 0u;
+            }
+            for (const Rec& r : P.glob) c += rec_hit(q, r) ? 1u : 0u;
+        }
+        hits[i] = c;
+    }
+    const uint32_t in = finish_mask(n, hits, mask);
+    if (out_inside) *out_inside = in;
+    return 0;
+}
+
+int orc_mesh_plan(uint32_t nv, const float* verts, uint32_t nt, const uint32_t* idx, uint32_t* out_counts, int32_t* out_level,
+                  uint64_t* out_pairs) {
+    if (bad_mesh(nv, verts, nt, idx)) return -1;
+    const MeshPlan P = plan_mesh(verts, nt, idx);
+    out_counts[0] = (uint32_t)P.bin.size();
+    out_counts[1] = (uint32_t)P.glob.size();
+    out_counts[2] = P.level >= 0 ? P.levels[P.level].ny : 0u;
+    out_counts[3] = P.level >= 0 ? P.levels[P.level].nz : 0u;
+    *out_level = P.level;
+    *out_pairs = P.level >= 0 ? P.level_pairs[P.level] : 0u;
+    return 0;
+}
+
+// The binned boxes (4 doubles each, ylo yhi zlo zhi) in triangle order, NaN rows for the dropped and global ones.
+int orc_mesh_boxes(uint32_t nv, const float* verts, uint32_t nt, const uint32_t* idx, double* out_box, int32_t* out_class) {
+    if (bad_mesh(nv, verts, nt, idx)) return -1;
+    for (uint32_t t = 0; t < nt; ++t) {
+        const V3 v0 = vert(verts, idx[3 * (size_t)t]), v1 = vert(verts, idx[3 * (size_t)t + 1]), v2 = vert(verts, idx[3 * (size_t)t + 2]);
+        const V3 e1 = sub(v1, v0), e2 = sub(v2, v0);
+        const float a = dot(e1, cross({1.0f, 0.0f, 0.0f}, e2));
+        double* b = out_box + 4 * (size_t)t;
+        b[0] = b[1] = b[2] = b[3] = NAN;
+        if ((a > -MS_EPS && a < MS_EPS) || !std::isfinite(a)) out_class[t] = 0;
+        else out_class[t] = mesh_box(v0, v1, v2, e1, e2, a, b) ? 1 : 2;
+    }
+    return 0;
+}
+
+}  // extern "C"

@@ -1,5 +1,5 @@
 /*
- * select_oracle.h -- CPU ORACLE of SparseSelect (src/query/sparse.rs:24-54).  TEST INFRASTRUCTURE ONLY: the product
+ * select_oracle.h -- CPU ORACLE of SparseSelect (src/query/sparse.rs:24-54) and of point-in-mesh selection.  TEST INFRASTRUCTURE ONLY: the product
  * (libbgs.so) never links, loads or calls it.  Built beside oracle/ (the render oracle) by __graft_entry__.build().
  *
  * The selection rule (include/bgs.h, bgs_cloud_select_sparse):
@@ -34,6 +34,26 @@ int orc_select_sparse_grid(uint32_t n, const float* pos_vis, float radius, uint3
 /* The grid's functions, per gaussian: the bucket (n_buckets for a non-finite position), and the three cell
  * coordinates.  Returns n_buckets. */
 uint32_t orc_select_buckets(uint32_t n, const float* pos_vis, float radius, uint32_t* out_bucket, int64_t* out_cell3);
+
+/* Point in mesh (include/bgs.h, bgs_cloud_select_in_mesh; src/query/raycast.rs:54-124): out_mask[i] = 1 iff the +x
+ * ray from mesh_from_cloud * (x, y, z, 1) (column-major, NULL = identity) hits an odd number of the nt triangles
+ * (vertices nv x 3 f32, indices nt x 3 u32), each decided by ray_intersects_triangle (raycast.rs:92-124) in glam's
+ * scalar Vec3 order, f32 without contraction.  PARITY STATUS: glam's operation order is **unpinned** (the crate is
+ * absent here).
+ *   orc_select_in_mesh       every (point, triangle) pair: the definition;
+ *   orc_select_in_mesh_grid  libbgs's mesh_select.cu restated (triangle setup and classes, slack, grid ladder and
+ *                            pair budget, cell function), so the CPU tests reach the cell boundaries the GPU does.
+ * Both return 0, or -1 for null arrays with nt > 0 or an index >= nv.  *out_inside (may be NULL) = popcount.
+ * orc_mesh_plan: out_counts = (binned, global, ny, nz) of the chosen level, *out_level (-1: no grid), *out_pairs.
+ * orc_mesh_boxes: per triangle, class 0 dropped / 1 binned / 2 global and the binned box (ylo, yhi, zlo, zhi). */
+int orc_select_in_mesh(uint32_t n, const float* pos_vis, uint32_t nv, const float* vertices, uint32_t nt, const uint32_t* indices,
+                       const float* mesh_from_cloud, uint8_t* out_mask, uint32_t* out_inside, int threads);
+int orc_select_in_mesh_grid(uint32_t n, const float* pos_vis, uint32_t nv, const float* vertices, uint32_t nt,
+                            const uint32_t* indices, const float* mesh_from_cloud, uint8_t* out_mask, uint32_t* out_inside,
+                            int threads);
+int orc_mesh_plan(uint32_t nv, const float* vertices, uint32_t nt, const uint32_t* indices, uint32_t* out_counts,
+                  int32_t* out_level, uint64_t* out_pairs);
+int orc_mesh_boxes(uint32_t nv, const float* vertices, uint32_t nt, const uint32_t* indices, double* out_box, int32_t* out_class);
 
 #ifdef __cplusplus
 }
