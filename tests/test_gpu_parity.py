@@ -8,6 +8,7 @@ import pytest
 
 import bevy_gaussian_splatting_b200 as B
 import blend_cases as BC
+import project_cases as PC
 
 pytestmark = pytest.mark.gpu
 
@@ -71,16 +72,27 @@ def check_against_oracle(plugin, oracle, cloud, settings, view, f16=False, pixel
                             orec["extra"][:, 3]], 1)
         else:
             geo = np.stack([orec[k] for k in ("cx", "cy", "ux", "uy", "vx", "vy")], 1)
-        assert np.array_equal(rec[drawn, :6].view(np.uint32), geo[drawn].view(np.uint32)), "projected geometry not bit-exact"
+        # (bit-exact with the sign of zero counted; NaN as a class: its payload is not part of the result)
+        assert PC.bits_agree(rec[drawn, :6], geo[drawn]).all(), "projected geometry not bit-exact"
         bb = rec[:, 6:8].view(np.uint32)
         assert np.array_equal(bb[drawn, 0], (orec["xlo"][drawn].astype(np.uint32) | (orec["xhi"][drawn].astype(np.uint32) << 16)))
         assert np.array_equal(bb[drawn, 1], (orec["ylo"][drawn].astype(np.uint32) | (orec["yhi"][drawn].astype(np.uint32) << 16)))
         assert np.all((bb[~drawn, 0] & 0xFFFF) > (bb[~drawn, 0] >> 16))      # empty bbox where the oracle's is
-        dc = 1e-4                       # (Depth colours come from the frame pass: bounded by the record check's 1e-4)
+        dc = 1e-4                       # (Depth colours come from the frame pass, tests/test_gpu_project.py restates them)
         if drawn.any() and settings.rasterize_mode != B.RasterizeMode.Depth:   # orc_project leaves Depth colours to the frame pass
-            col = np.stack([orec[k] for k in ("r", "g", "b", "op")], 1)
-            assert np.abs(rec[drawn, 8:12] - col[drawn]).max() <= 1e-4
-            dc = float(np.abs(rec[drawn, 8:11] - col[drawn, :3]).max())
+            col = np.stack([orec[k] for k in ("r", "g", "b")], 1)[drawn]
+            assert PC.bits_agree(rec[drawn, 11], orec["op"][drawn]).all(), "opacity differs"
+            if settings.rasterize_mode == B.RasterizeMode.Color:
+                # the derived per-record bound of the SH colour path (rsqrt.approx, fma accumulation, __powf)
+                bound = PC.colour_bound(oc, view, None, int(settings.color_space), ids[drawn])
+                lit = (settings.draw_mode == B.DrawMode.HighlightSelected) & (oc.position_visibility[ids[drawn], 3] > 0.5)
+                bound[lit] = 0.0
+            else:                       # Normal / Position: the same IEEE operations on both sides
+                bound = np.full(col.shape, 4 * PC.U) * np.maximum(1.0, np.abs(col))
+            assert PC.colours_agree(rec[drawn, 8:11], col, bound).all(), "record colour outside its bound"
+            with np.errstate(invalid="ignore"):
+                diff = np.abs(rec[drawn, 8:11].astype(np.float64) - col)
+            dc = float(np.max(np.where(np.isfinite(diff), diff, 0.0), initial=0.0))   # the measured record colour error
         err = float(np.abs(img - til["image"]).max())
         assert err <= pixel_tol, f"pixel L-inf {err}"
         # per pixel: within the derived error bound of the float64 evaluation of the same walk (blend_cases.blend_bounds)
