@@ -25,8 +25,10 @@ keygen_all_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, ui
     const uint32_t i = blockIdx.x * KG_THREADS + threadIdx.x;
     bool vis = false;
     if (i < n) {
-        const float4 p = __ldcs(pos + i);
-        keys_out[i] = key_of_fast(fc, p.x, p.y, p.z, vis);
+        float pw[4];
+        keygen_world_pos(fc, __ldcs(pos + i), pw);
+        vis = in_frustum_fast(fc, pw);
+        keys_out[i] = depth_key(fc, vis, cam_dist2(fc, pw));
         ids_out[i] = i;
     }
     const int cnt = __syncthreads_count(vis);
@@ -80,7 +82,12 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
 #pragma unroll
         for (int j = 0; j < KG_ITEMS; ++j) {
             const uint32_t i = wbase + j * 32 + lane;
-            const bool v = (i < n) && visible_fast(fc, p[j].x, p[j].y, p[j].z);
+            bool v = false;
+            if (i < n) {
+                float pw[4];
+                keygen_world_pos(fc, p[j], pw);
+                v = in_frustum_fast(fc, pw);
+            }
             const uint32_t bal = __ballot_sync(0xffffffffu, v);
             mine += __popc(bal);
             if (lane == j) myword = bal;
@@ -158,8 +165,9 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
             const uint32_t r = e - s_pref[lo];
             const uint32_t bit = __fns(s_mask[lo], 0u, (int)r + 1);
             const uint32_t i = (wc + lo) * 32u + bit;
-            const float4 p = __ldg(pos + i);
-            const uint32_t key = key_only(fc, p.x, p.y, p.z);
+            float pw[4];
+            keygen_world_pos(fc, __ldg(pos + i), pw);
+            const uint32_t key = depth_key(fc, true, cam_dist2(fc, pw));
             const uint32_t dst = run + e;
             keys_out[dst] = key;
             ids_out[dst] = i;          // compact slot -> gaussian index
@@ -183,7 +191,9 @@ __global__ void culled_flags_kernel(const float4* __restrict__ pos, uint32_t n, 
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float4 p = pos[i];
-    flags[i] = key_of(fc, p.x, p.y, p.z).visible ? 0u : 1u;
+    float pw[4], ndc[2];
+    mat4_point(fc.model, p.x, p.y, p.z, pw);
+    flags[i] = in_frustum(fc, pw, ndc) ? 0u : 1u;
 }
 
 void launch_keygen_all(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* keys_out, uint32_t* ids_out,

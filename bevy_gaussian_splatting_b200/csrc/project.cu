@@ -1,11 +1,18 @@
 // project.cu -- stage 3: per-gaussian 3D->2D covariance projection + SH-degree-3 colour, run
-// ONCE per visible gaussian in front-to-back rank order (the reference runs it 4x per gaussian in
-// its vertex stage: src/render/gaussian.wgsl:185-436).
+// ONCE per visible gaussian (the reference runs it 4x per gaussian in its vertex stage:
+// src/render/gaussian.wgsl:185-436).
 //
-// rank r (0 = nearest) -> gaussian id = sorted_ids[n_vis-1-r] (the sort is far->near like the
-// reference's, src/sort/radix.wgsl) -> gather the gaussian's block (f32 256 B or f16 128 B) ->
-// write one 48 B SplatRec at recs[r] (coalesced), which is all the tile stages read.
+// Record r of n_vis is the gaussian id the index list gives for r (project_kernel's `by_slot`):
+//  * compact frames (the default): r is a compact slot, id = slot_ids[r] (ascending gaussian index, as key-gen
+//    compacted them).  The projection runs beside the depth sort, whose payload is that slot: binning reads the
+//    record of rank k at recs[sorted slot of k];
+//  * BGS_FLAG_SORT_ALL: r is a front-to-back rank (0 = nearest), id = sorted_ids[n_vis-1-r] (the sort is far->near
+//    like the reference's, src/sort/radix.wgsl).
+// Either way: gather the gaussian's block (f32 256 B or f16 128 B) -> write one 48 B SplatRec at recs[r]
+// (coalesced), which is all the tile stages read.
 //
+// project_one is the vertex stage's dispatch: frustum and draw-mode test, cutoff, then the record of the splat's
+// geometry (3DGS USE_AABB conic, 3DGS USE_OBB, 2DGS surfel) and its colour source (SH, Depth, Normal, Position).
 // Geometry (centre, OBB uv rows, pixel bbox) is bit-exact vs the oracle: compiled -fmad=false.
 #include <cuda_fp16.h>
 
@@ -150,8 +157,7 @@ __global__ void depth_range_kernel(const float4* __restrict__ pos, uint32_t n, c
         const float4 p = pos[id];
         float pw[4];
         mat4_point(fc.model, p.x, p.y, p.z, pw);
-        const float d[3] = {pw[0] - fc.cam[0], pw[1] - fc.cam[1], pw[2] - fc.cam[2]};
-        return sqrtf(dot3(d, d));
+        return sqrtf(cam_dist2(fc, pw));
     };
     ctr->depth_min = dist(last);
     ctr->depth_max = dist(first);
@@ -170,79 +176,64 @@ __global__ void cutoff_table_kernel(float* __restrict__ tab) {
 }
 void launch_cutoff_table(float* tab, cudaStream_t stream) { cutoff_table_kernel<<<256, 256, 0, stream>>>(tab); }
 
-// One visible gaussian: projection + colour -> the 48 B record at recs[r] (+ the 2DGS extra record).
-// `load_sh(float sh[48])` fetches the SH coefficients (only called for RasterizeMode::Color); `cutoff_pre` is the
-// tabulated adaptive cutoff, or NaN to evaluate it here.
-template <class ShLoader>
-__device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCounters* __restrict__ ctr, uint32_t r, float4 p4,
-                                            const float q[4], const float so[4], float cutoff_pre, ShLoader load_sh,
-                                            SplatRec* __restrict__ recs, float4* __restrict__ extra, float4* __restrict__ aux) {
-    SplatRec rec;
-    rec.ux = 0.f; rec.uy = 0.f; rec.vx = 0.f; rec.vy = 0.f;
-    rec.bx = BBOX_EMPTY; rec.by = BBOX_EMPTY;
-    rec.r = 0.f; rec.g = 0.f; rec.b = 0.f;
+// gaussian.wgsl:228-232: the quad's extent in standard deviations; with OPACITY_ADAPTIVE_RADIUS, f16 clouds read it
+// from the table of their 16-bit opacity
+template <bool F16>
+__device__ __forceinline__ float splat_cutoff(const FrameConsts& fc, float opacity, const float* __restrict__ cutoff_tab,
+                                              uint32_t op_bits) {
+    if (!fc.adaptive) return 3.0f;
+    if constexpr (F16) return __ldg(cutoff_tab + op_bits);
+    else return adaptive_cutoff(opacity);
+}
 
-    const KeyOut k = key_of(fc, p4.x, p4.y, p4.z);
-    const float W = fc.W, H = fc.H;
-    const float hw = 0.5f * W, hh = 0.5f * H;
-    const float cx = k.ndc[0] * hw + hw;
-    const float cy = hh - k.ndc[1] * hh;
-    rec.cx = cx; rec.cy = cy;
-    const float opacity = so[3];
-    rec.op = opacity * fc.global_opacity;
-    const bool drawn = k.visible && !(fc.draw_mode == BGS_DRAW_SELECTED && p4.w < 0.5f);
+// helpers.wgsl:137-158 as (row, col); the quaternion is NOT normalised
+__device__ __forceinline__ void rotation_rows(const float q[4], float Rm[3][3]) {
+    const float qr = q[0], x = q[1], y = q[2], z = q[3];
+    Rm[0][0] = 1.0f - 2.0f * (y * y + z * z);
+    Rm[1][0] = 2.0f * (x * y - qr * z);
+    Rm[2][0] = 2.0f * (x * z + qr * y);
+    Rm[0][1] = 2.0f * (x * y + qr * z);
+    Rm[1][1] = 1.0f - 2.0f * (x * x + z * z);
+    Rm[2][1] = 2.0f * (y * z - qr * x);
+    Rm[0][2] = 2.0f * (x * z - qr * y);
+    Rm[1][2] = 2.0f * (y * z + qr * x);
+    Rm[2][2] = 1.0f - 2.0f * (x * x + y * y);
+}
 
-    float A[3][3];
-#pragma unroll
-    for (int rr = 0; rr < 3; ++rr)
-#pragma unroll
-        for (int cc = 0; cc < 3; ++cc) A[rr][cc] = fc.model[cc * 4 + rr];
-    // helpers.wgsl:137-158 as (row, col); the quaternion is NOT normalised
-    float Rm[3][3];
-    {
-        const float qr = q[0], x = q[1], y = q[2], z = q[3];
-        Rm[0][0] = 1.0f - 2.0f * (y * y + z * z);
-        Rm[1][0] = 2.0f * (x * y - qr * z);
-        Rm[2][0] = 2.0f * (x * z + qr * y);
-        Rm[0][1] = 2.0f * (x * y + qr * z);
-        Rm[1][1] = 1.0f - 2.0f * (x * x + z * z);
-        Rm[2][1] = 2.0f * (y * z - qr * x);
-        Rm[0][2] = 2.0f * (x * z - qr * y);
-        Rm[1][2] = 2.0f * (y * z + qr * x);
-        Rm[2][2] = 1.0f - 2.0f * (x * x + y * y);
+// gaussian_3d.wgsl:49-72: the world-space covariance T Sigma T^t, Sigma = M^t M, M = S R, T = the model 3x3, as its six
+// entries (WGSL [col][row] order)
+__device__ __forceinline__ void sigma3d(const FrameConsts& fc, const float A[3][3], const float Rm[3][3], const float sc[3],
+                                        const float q[4], const float so[4], float c3[6]) {
+    if (fc.cov_pre) {
+        // PRECOMPUTE_COVARIANCE_3D (gaussian_3d.wgsl:78-79, planar.wgsl:133-152): the decoded record goes straight into
+        // cov2d -- no global_scale, no model 3x3.  It arrives in the plane slots it occupies: q = c0..c3, so = c4, c5,
+        // opacity, opacity
+        c3[0] = q[0]; c3[1] = q[1]; c3[2] = q[2]; c3[3] = q[3]; c3[4] = so[0]; c3[5] = so[1];
+        return;
     }
-    const float sc[3] = {so[0] * fc.global_scale, so[1] * fc.global_scale, so[2] * fc.global_scale};
-
-    if (drawn) {
-        float cutoff = 3.0f;
-        if (fc.adaptive) {   // gaussian.wgsl:228-232
-            cutoff = cutoff_pre == cutoff_pre ? cutoff_pre : adaptive_cutoff(opacity);
-        }
-        if (fc.gaussian_mode == BGS_GAUSSIAN_3D) {
-        // gaussian_3d.wgsl:49-72
-        float M[3][3], Sg[3][3], X[3][3], TS[3][3];
+    float M[3][3], Sg[3][3], X[3][3], TS[3][3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) M[i][j] = sc[i] * Rm[i][j];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) Sg[i][j] = (M[0][i] * M[0][j] + M[1][i] * M[1][j]) + M[2][i] * M[2][j];
+    // identity model: T Sigma T^t == Sigma bit for bit as long as every entry of Sigma is finite and NON-ZERO
+    // (x*1 + y*0 + z*0 then only ever adds +-0 to a non-zero value); zero entries (axis-aligned splats) keep
+    // the multiply so that even the sign of a zero matches the oracle
+    const float mn = fminf(fminf(fminf(fabsf(Sg[0][0]), fabsf(Sg[0][1])), fminf(fabsf(Sg[0][2]), fabsf(Sg[1][1]))),
+                           fminf(fabsf(Sg[1][2]), fabsf(Sg[2][2])));
+    const float mx = fmaxf(fmaxf(fmaxf(fabsf(Sg[0][0]), fabsf(Sg[0][1])), fmaxf(fabsf(Sg[0][2]), fabsf(Sg[1][1]))),
+                           fmaxf(fabsf(Sg[1][2]), fabsf(Sg[2][2])));
+    if (fc.model_identity && mn > 0.0f && mx < __uint_as_float(0x7F800000u) && Sg[0][0] == Sg[0][0] &&
+        Sg[0][1] == Sg[0][1] && Sg[0][2] == Sg[0][2] && Sg[1][1] == Sg[1][1] && Sg[1][2] == Sg[1][2] && Sg[2][2] == Sg[2][2]) {
 #pragma unroll
         for (int i = 0; i < 3; ++i)
 #pragma unroll
-            for (int j = 0; j < 3; ++j) M[i][j] = sc[i] * Rm[i][j];
-#pragma unroll
-        for (int i = 0; i < 3; ++i)
-#pragma unroll
-            for (int j = 0; j < 3; ++j) Sg[i][j] = (M[0][i] * M[0][j] + M[1][i] * M[1][j]) + M[2][i] * M[2][j];
-        // identity model: T Sigma T^t == Sigma bit for bit as long as every entry of Sigma is finite and NON-ZERO
-        // (x*1 + y*0 + z*0 then only ever adds +-0 to a non-zero value); zero entries (axis-aligned splats) keep
-        // the multiply so that even the sign of a zero matches the oracle
-        const float mn = fminf(fminf(fminf(fabsf(Sg[0][0]), fabsf(Sg[0][1])), fminf(fabsf(Sg[0][2]), fabsf(Sg[1][1]))),
-                               fminf(fabsf(Sg[1][2]), fabsf(Sg[2][2])));
-        const float mx = fmaxf(fmaxf(fmaxf(fabsf(Sg[0][0]), fabsf(Sg[0][1])), fmaxf(fabsf(Sg[0][2]), fabsf(Sg[1][1]))),
-                               fmaxf(fabsf(Sg[1][2]), fabsf(Sg[2][2])));
-        if (fc.model_identity && mn > 0.0f && mx < __uint_as_float(0x7F800000u) && Sg[0][0] == Sg[0][0] &&
-            Sg[0][1] == Sg[0][1] && Sg[0][2] == Sg[0][2] && Sg[1][1] == Sg[1][1] && Sg[1][2] == Sg[1][2] && Sg[2][2] == Sg[2][2]) {
-#pragma unroll
-            for (int i = 0; i < 3; ++i)
-#pragma unroll
-                for (int j = 0; j < 3; ++j) TS[i][j] = Sg[i][j];
-        } else {
+            for (int j = 0; j < 3; ++j) TS[i][j] = Sg[i][j];
+    } else {
 #pragma unroll
         for (int i = 0; i < 3; ++i)
 #pragma unroll
@@ -251,230 +242,291 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
         for (int i = 0; i < 3; ++i)
 #pragma unroll
             for (int j = 0; j < 3; ++j) TS[i][j] = (X[i][0] * A[j][0] + X[i][1] * A[j][1]) + X[i][2] * A[j][2];
-        }
-        float c3[6] = {TS[0][0], TS[1][0], TS[2][0], TS[1][1], TS[2][1], TS[2][2]};
-        if (fc.cov_pre) {
-            // PRECOMPUTE_COVARIANCE_3D (gaussian_3d.wgsl:78-79, planar.wgsl:133-152): the decoded record goes straight into
-            // cov2d -- no global_scale, no model 3x3.  It arrives in the plane slots it occupies: q = c0..c3, so = c4, c5,
-            // opacity, opacity
-            c3[0] = q[0]; c3[1] = q[1]; c3[2] = q[2]; c3[3] = q[3]; c3[4] = so[0]; c3[5] = so[1];
-        }
-        const float Vrk[3][3] = {{c3[0], c3[1], c3[2]}, {c3[1], c3[3], c3[4]}, {c3[2], c3[4], c3[5]}};
-        // helpers.wgsl:8-47
-        float tv[4];
-        mat4_point(fc.view_from_world, k.pw[0], k.pw[1], k.pw[2], tv);
-        const float fx = fc.p00 * W, fy = fc.p11 * H;
-        const float sz = 1.0f / (tv[2] * tv[2]);
-        const float J00 = fx / tv[2], J20 = -(fx * tv[0]) * sz;
-        const float J11 = -fy / tv[2], J21 = (fy * tv[1]) * sz;
-        float Tm[3][2];
+    }
+    c3[0] = TS[0][0]; c3[1] = TS[1][0]; c3[2] = TS[2][0]; c3[3] = TS[1][1]; c3[4] = TS[2][1]; c3[5] = TS[2][2];
+}
+
+// helpers.wgsl:8-67: the screen-space covariance [a b; b c] (+0.3 on the diagonal) of the splat at pw, its determinant
+// and its eigenvalues mid +- term (l1 = the larger)
+struct Cov2d {
+    float a, b, c, det, mid, term, l1;
+};
+__device__ __forceinline__ Cov2d cov2d(const FrameConsts& fc, const float pw[3], const float c3[6]) {
+    const float Vrk[3][3] = {{c3[0], c3[1], c3[2]}, {c3[1], c3[3], c3[4]}, {c3[2], c3[4], c3[5]}};
+    float tv[4];
+    mat4_point(fc.view_from_world, pw[0], pw[1], pw[2], tv);
+    const float fx = fc.p00 * fc.W, fy = fc.p11 * fc.H;
+    const float sz = 1.0f / (tv[2] * tv[2]);
+    const float J00 = fx / tv[2], J20 = -(fx * tv[0]) * sz;
+    const float J11 = -fy / tv[2], J21 = (fy * tv[1]) * sz;
+    float Tm[3][2];
 #pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            const float v0 = fc.view_from_world[i * 4 + 0], v1 = fc.view_from_world[i * 4 + 1],
-                        v2 = fc.view_from_world[i * 4 + 2];
-            Tm[i][0] = v0 * J00 + v2 * J20;
-            Tm[i][1] = v1 * J11 + v2 * J21;
+    for (int i = 0; i < 3; ++i) {
+        const float v0 = fc.view_from_world[i * 4 + 0], v1 = fc.view_from_world[i * 4 + 1],
+                    v2 = fc.view_from_world[i * 4 + 2];
+        Tm[i][0] = v0 * J00 + v2 * J20;
+        Tm[i][1] = v1 * J11 + v2 * J21;
+    }
+    float Y[3][2];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int b = 0; b < 2; ++b) Y[i][b] = (Vrk[i][0] * Tm[0][b] + Vrk[i][1] * Tm[1][b]) + Vrk[i][2] * Tm[2][b];
+    Cov2d v;
+    v.a = ((Tm[0][0] * Y[0][0] + Tm[1][0] * Y[1][0]) + Tm[2][0] * Y[2][0]) + 0.3f;
+    v.b = (Tm[0][1] * Y[0][0] + Tm[1][1] * Y[1][0]) + Tm[2][1] * Y[2][0];
+    v.c = ((Tm[0][1] * Y[0][1] + Tm[1][1] * Y[1][1]) + Tm[2][1] * Y[2][1]) + 0.3f;
+    v.det = v.a * v.c - v.b * v.b;
+    v.mid = 0.5f * (v.a + v.c);
+    v.term = sqrtf(fmaxf(0.0f, v.mid * v.mid - v.det));
+    v.l1 = v.mid + v.term;
+    return v;
+}
+
+// helpers.wgsl:69-79 + gaussian.wgsl:299-309 (USE_AABB): a square of half-side cutoff * sqrt(l1) and the conic
+// record: ux, uy, vx = conic.x, .y, .z; vy = the quad's half-side (half-pixels)
+__device__ __forceinline__ void aabb_record(const FrameConsts& fc, const Cov2d& v, float cutoff, SplatRec& rec) {
+    const float l2 = fmaxf(v.mid - v.term, 0.0f);
+    const float Rq = cutoff * fmaxf(sqrtf(v.l1), sqrtf(l2));
+    const float dinv = 1.0f / v.det;
+    rec.ux = v.c * dinv; rec.uy = -v.b * dinv; rec.vx = v.a * dinv; rec.vy = Rq;
+    const float h = 0.5f * Rq;
+    make_bbox(rec.cx, rec.cy, h, h, fc.Wi, fc.Hi, rec.bx, rec.by);
+}
+
+// helpers.wgsl:81-119 (USE_OBB): the rows of the pixel-offset -> quad-uv map along the eigenvectors, scaled by
+// cutoff * the axis lengths; no bbox when the map is NaN (b = 0 and a = c)
+__device__ __forceinline__ void obb_record(const FrameConsts& fc, const Cov2d& v, float cutoff, SplatRec& rec) {
+    const float a = v.a, b = v.b, c = v.c;
+    const float aa = (a - c) * (a - c);
+    const float bb = sqrtf(aa + (4.0f * b) * b);
+    const float major = sqrtf(((a + c) + bb) * 0.5f);
+    const float minor = sqrtf(((a + c) - bb) * 0.5f);
+    const float Bx = cutoff * major, By = cutoff * minor;
+    const float evx = -b, evy = v.l1 - a;
+    const float el = sqrtf(evx * evx + evy * evy);
+    const float e1x = evx / el, e1y = evy / el;
+    const float e2x = e1y, e2y = -e1x;
+    rec.ux = (2.0f * e1x) / Bx; rec.uy = (-2.0f * e1y) / Bx;
+    rec.vx = (2.0f * e2x) / By; rec.vy = (-2.0f * e2y) / By;
+    const float hx = 0.5f * (fabsf(e1x) * Bx + fabsf(e2x) * By);
+    const float hy = 0.5f * (fabsf(e1y) * Bx + fabsf(e2y) * By);
+    if (rec.ux == rec.ux && rec.uy == rec.uy && rec.vx == rec.vx && rec.vy == rec.vy)
+        make_bbox(rec.cx, rec.cy, hx, hy, fc.Wi, fc.Hi, rec.bx, rec.by);
+}
+
+// 2DGS surfel: gaussian_2d.wgsl:77-132 (homography) + :49-75 (quad).  The record is an OBB one with e1 = (1, 0),
+// e2 = (0, 1); with USE_AABB the blend evaluates the ray-splat intersection from the homography rows in extra[4 r..]
+__device__ __forceinline__ void surfel_record(const FrameConsts& fc, const float A[3][3], const float Rm[3][3],
+                                              const float sc[3], const float pw[3], float cutoff, uint32_t r,
+                                              float4* __restrict__ extra, SplatRec& rec) {
+    const float W = fc.W, H = fc.H;
+    float L[3][2];   // first two columns of A * R_std * S, R_std = transpose(Rm)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+        const float rc[3] = {Rm[j][0] * sc[j], Rm[j][1] * sc[j], Rm[j][2] * sc[j]};
+#pragma unroll
+        for (int i = 0; i < 3; ++i) L[i][j] = (A[i][0] * rc[0] + A[i][1] * rc[1]) + A[i][2] * rc[2];
+    }
+    float G[3][4];
+    mat4_dir(fc.clip_from_world, L[0][0], L[1][0], L[2][0], G[0]);
+    mat4_dir(fc.clip_from_world, L[0][1], L[1][1], L[2][1], G[1]);
+    mat4_point(fc.clip_from_world, pw[0], pw[1], pw[2], G[2]);
+    const float fxk = fc.p00 * W / 2.0f, fyk = fc.p11 * H / 2.0f;     // helpers.wgsl:122-135
+    const float cxk = (W - 1.0f) / 2.0f, cyk = (H - 1.0f) / 2.0f;
+    float T0[3], T1[3], T2[3];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        T0[j] = fxk * G[j][0] + cxk * G[j][3];
+        T1[j] = fyk * G[j][1] + cyk * G[j][3];
+        T2[j] = G[j][3];
+    }
+    const float c2 = cutoff * cutoff;
+    const float test[3] = {c2, c2, -1.0f};
+    const float tt[3] = {test[0] * T2[0], test[1] * T2[1], test[2] * T2[2]};
+    const float d = dot3(tt, T2);
+    if (fabsf(d) < 1.0e-4f) return;
+    const float inv = 1.0f / d;
+    const float f[3] = {inv * test[0], inv * test[1], inv * test[2]};
+    const float t02[3] = {T0[0] * T2[0], T0[1] * T2[1], T0[2] * T2[2]};
+    const float t12[3] = {T1[0] * T2[0], T1[1] * T2[1], T1[2] * T2[2]};
+    const float mean0 = dot3(f, t02), mean1 = dot3(f, t12);
+    const float f0[3] = {f[0] * T0[0], f[1] * T0[1], f[2] * T0[2]};
+    const float f1[3] = {f[0] * T1[0], f[1] * T1[1], f[2] * T1[2]};
+    const float ex = mean0 * mean0 - dot3(f0, T0);
+    const float ey = mean1 * mean1 - dot3(f1, T1);
+    if (ex < 1.0e-4f || ey < 1.0e-4f) return;
+    const float Rq = fmaxf(fmaxf(sqrtf(ex), sqrtf(ey)), cutoff * 0.707106f);
+    rec.ux = 2.0f / Rq; rec.uy = 0.0f; rec.vx = 0.0f; rec.vy = -2.0f / Rq;
+    const float h = 0.5f * Rq;
+    if (Rq == Rq) make_bbox(rec.cx, rec.cy, h, h, fc.Wi, fc.Hi, rec.bx, rec.by);
+    if (fc.aabb && extra != nullptr) {
+        float4* e = extra + (size_t)r * 4;
+        e[0] = make_float4(Rq, mean0, mean1, W / H);
+        e[1] = make_float4(T0[0], T0[1], T0[2], 0.0f);
+        e[2] = make_float4(T1[0], T1[1], T1[2], 0.0f);
+        e[3] = make_float4(T2[0], T2[1], T2[2], 0.0f);
+    }
+}
+
+// RasterizeMode::Color: gaussian.wgsl:166-183,406-416 + spherical_harmonics.wgsl:34-68, the SH-3 colour seen along
+// the camera ray in the splat's model frame
+__device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3][3], const float pw[3], const float sh[48],
+                                          float rgb[3]) {
+    const float dlt[3] = {pw[0] - fc.cam[0], pw[1] - fc.cam[1], pw[2] - fc.cam[2]};
+    float dw[3], loc[3], dl[3];
+    normalize3(dlt, dw);
+    if (fc.model_identity) {     // the normalised model columns are the unit axes
+        loc[0] = dw[0]; loc[1] = dw[1]; loc[2] = dw[2];
+    } else {
+#pragma unroll
+        for (int cc = 0; cc < 3; ++cc) {
+            const float col[3] = {A[0][cc], A[1][cc], A[2][cc]};
+            float bn[3];
+            normalize3(col, bn);
+            loc[cc] = dot3(bn, dw);
         }
-        float Y[3][2];
+    }
+    normalize3(loc, dl);
+    const float x = dl[0], y = dl[1], z = dl[2];
+    const float xx = x * x, yy = y * y, zz = z * z;
+    float basis[16];   // (the SH constants are folded in below: 16 multiplies instead of 48)
+    basis[0] = 1.0f;
+    basis[1] = y; basis[2] = z; basis[3] = x;
+    basis[4] = x * y; basis[5] = y * z; basis[6] = (2.0f * zz - xx) - yy;
+    basis[7] = x * z; basis[8] = xx - yy;
+    basis[9] = y * (3.0f * xx - yy);
+    basis[10] = (x * y) * z;
+    basis[11] = y * ((4.0f * zz - xx) - yy);
+    basis[12] = z * ((2.0f * zz - 3.0f * xx) - 3.0f * yy);
+    basis[13] = x * ((4.0f * zz - xx) - yy);
+    basis[14] = z * (xx - yy);
+    basis[15] = x * (xx - 3.0f * yy);
 #pragma unroll
-        for (int i = 0; i < 3; ++i)
+    for (int kk = 0; kk < 16; ++kk) basis[kk] *= c_shc[kk];
 #pragma unroll
-            for (int b = 0; b < 2; ++b) Y[i][b] = (Vrk[i][0] * Tm[0][b] + Vrk[i][1] * Tm[1][b]) + Vrk[i][2] * Tm[2][b];
-        const float a = ((Tm[0][0] * Y[0][0] + Tm[1][0] * Y[1][0]) + Tm[2][0] * Y[2][0]) + 0.3f;
-        const float b = (Tm[0][1] * Y[0][0] + Tm[1][1] * Y[1][0]) + Tm[2][1] * Y[2][0];
-        const float c = ((Tm[0][1] * Y[0][1] + Tm[1][1] * Y[1][1]) + Tm[2][1] * Y[2][1]) + 0.3f;
-        // helpers.wgsl:49-67
-        const float det = a * c - b * b;
-        const float mid = 0.5f * (a + c);
-        const float disc = fmaxf(0.0f, mid * mid - det);
-        const float term = sqrtf(disc);
-        const float l1 = mid + term;
-        if (fc.aabb) {
-            // helpers.wgsl:69-79 + gaussian.wgsl:299-309: square of half-side cutoff*sqrt(l1), conic
-            // record (USE_AABB): ux,uy,vx = conic.x,.y,.z; vy = quad half-side (half-pixels)
-            const float l2 = fmaxf(mid - term, 0.0f);
-            const float Rq = cutoff * fmaxf(sqrtf(l1), sqrtf(l2));
-            const float dinv = 1.0f / det;
-            rec.ux = c * dinv; rec.uy = -b * dinv; rec.vx = a * dinv; rec.vy = Rq;
-            const float h = 0.5f * Rq;
-            make_bbox(cx, cy, h, h, fc.Wi, fc.Hi, rec.bx, rec.by);
+    for (int cc = 0; cc < 3; ++cc) {
+        float acc = 0.5f;
+#pragma unroll
+        for (int kk = 0; kk < 16; ++kk) acc = fmaf(sh[3 * kk + cc], basis[kk], acc);   // colour: FMA is fine
+        rgb[cc] = acc;
+    }
+    if (fc.color_space == 0u) {
+#pragma unroll
+        for (int cc = 0; cc < 3; ++cc) rgb[cc] = srgb_to_linear(rgb[cc]);
+    }
+}
+
+// RasterizeMode::Depth: material/depth.wgsl:3-11 over depth_range_kernel's [depth_min, depth_max]
+__device__ __forceinline__ void depth_colour(const FrameConsts& fc, const FrameCounters* __restrict__ ctr,
+                                             const float pw[3], float rgb[3]) {
+    if (fc.n_cloud < 2u) return;   // the reference reads sorted[1]: undefined for a 1-gaussian cloud (oracle: black)
+    const float depth = sqrtf(cam_dist2(fc, pw));
+    const float dmin = ctr->depth_min, dmax = ctr->depth_max;
+    float nd = (depth - dmin) / (dmax - dmin);
+    nd = fminf(fmaxf(nd, 0.0f), 1.0f);   // fmin/fmax ignore a NaN operand, like the oracle's
+    float t1 = (nd - 0.5f) / (1.0f - 0.5f); t1 = fminf(fmaxf(t1, 0.0f), 1.0f);
+    float t2 = (nd - 0.0f) / (0.5f - 0.0f); t2 = fminf(fmaxf(t2, 0.0f), 1.0f);
+    rgb[0] = t1 * t1 * (3.0f - 2.0f * t1);
+    rgb[1] = 1.0f - fabsf(nd - 0.5f) * 2.0f;
+    rgb[2] = 1.0f - t2 * t2 * (3.0f - 2.0f * t2);
+}
+
+// RasterizeMode::Normal: gaussian.wgsl:350-368, the view-space direction of the splat's third scaled axis
+__device__ __forceinline__ void normal_colour(const FrameConsts& fc, const float A[3][3], const float Rm[3][3],
+                                              const float sc[3], float rgb[3]) {
+    float SR[3], Ln[3], wn[4];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) SR[i] = sc[i] * Rm[i][2];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) Ln[i] = (A[i][0] * SR[0] + A[i][1] * SR[1]) + A[i][2] * SR[2];
+    mat4_dir(fc.view_from_world, Ln[0], Ln[1], Ln[2], wn);
+    const float l = sqrtf(((wn[0] * wn[0] + wn[1] * wn[1]) + wn[2] * wn[2]) + wn[3] * wn[3]);
+#pragma unroll
+    for (int cc = 0; cc < 3; ++cc) rgb[cc] = 0.5f * (wn[cc] / l + 1.0f);
+}
+
+// RasterizeMode::Position: gaussian.wgsl:375-376, (transformed_position - min) / (max - min)
+__device__ __forceinline__ void position_colour(const FrameConsts& fc, const float pw[3], float rgb[3]) {
+#pragma unroll
+    for (int cc = 0; cc < 3; ++cc) rgb[cc] = (pw[cc] - fc.aabb_min[cc]) / (fc.aabb_max[cc] - fc.aabb_min[cc]);
+}
+
+// DrawMode::HighlightSelected (gaussian.wgsl:423-427): a selected splat is drawn opaque and green in every colour source
+__device__ __forceinline__ void highlight_selected(SplatRec& rec, float drgb[3], float nrgb[3]) {
+    rec.r = 0.3f; rec.g = 1.0f; rec.b = 0.1f; rec.op = 1.0f;
+    drgb[0] = nrgb[0] = 0.3f; drgb[1] = nrgb[1] = 1.0f; drgb[2] = nrgb[2] = 0.1f;
+}
+
+// the 48 B record, three 16 B stores
+__device__ __forceinline__ void store_rec(SplatRec* __restrict__ dst, const SplatRec& rec) {
+    float4* out = reinterpret_cast<float4*>(dst);
+    out[0] = make_float4(rec.cx, rec.cy, rec.ux, rec.uy);
+    out[1] = make_float4(rec.vx, rec.vy, __uint_as_float(rec.bx), __uint_as_float(rec.by));
+    out[2] = make_float4(rec.r, rec.g, rec.b, rec.op);
+}
+
+// One entry of the index list -> the 48 B record at recs[r] (+ the 2DGS extra record and the aux colours).  An
+// undrawn gaussian (outside the frustum, or unselected under DrawMode::Selected) gets an empty bbox and no colour.
+template <bool F16>
+__device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCounters* __restrict__ ctr, uint32_t r,
+                                            float4 p4, const float q[4], const float so[4], const float sh[48],
+                                            const float* __restrict__ cutoff_tab, uint32_t op_bits,
+                                            SplatRec* __restrict__ recs, float4* __restrict__ extra,
+                                            float4* __restrict__ aux) {
+    SplatRec rec;
+    rec.ux = 0.f; rec.uy = 0.f; rec.vx = 0.f; rec.vy = 0.f;
+    rec.bx = BBOX_EMPTY; rec.by = BBOX_EMPTY;
+    rec.r = 0.f; rec.g = 0.f; rec.b = 0.f;
+    // the full model multiply, even for an identity model: keygen_world_pos's shortcut would turn a -0 into +0 here
+    float pw[4], ndc[2];
+    mat4_point(fc.model, p4.x, p4.y, p4.z, pw);
+    const bool visible = in_frustum(fc, pw, ndc);   // gaussian.wgsl:209-210 (SORT_ALL lists hold culled gaussians too)
+    const float hw = 0.5f * fc.W, hh = 0.5f * fc.H;
+    rec.cx = ndc[0] * hw + hw;
+    rec.cy = hh - ndc[1] * hh;
+    const float opacity = so[3];
+    rec.op = opacity * fc.global_opacity;
+    if (visible && !(fc.draw_mode == BGS_DRAW_SELECTED && p4.w < 0.5f)) {   // gaussian.wgsl:203-205 (DrawMode::Selected)
+        const float cutoff = splat_cutoff<F16>(fc, opacity, cutoff_tab, op_bits);
+        float A[3][3], Rm[3][3];   // the model 3x3 and the rotation, (row, col)
+#pragma unroll
+        for (int rr = 0; rr < 3; ++rr)
+#pragma unroll
+            for (int cc = 0; cc < 3; ++cc) A[rr][cc] = fc.model[cc * 4 + rr];
+        rotation_rows(q, Rm);
+        const float sc[3] = {so[0] * fc.global_scale, so[1] * fc.global_scale, so[2] * fc.global_scale};
+
+        if (fc.gaussian_mode == BGS_GAUSSIAN_3D) {
+            float c3[6];
+            sigma3d(fc, A, Rm, sc, q, so, c3);
+            const Cov2d v = cov2d(fc, pw, c3);
+            if (fc.aabb) aabb_record(fc, v, cutoff, rec);
+            else obb_record(fc, v, cutoff, rec);
         } else {
-        // helpers.wgsl:81-119 (USE_OBB)
-        const float aa = (a - c) * (a - c);
-        const float bb = sqrtf(aa + (4.0f * b) * b);
-        const float major = sqrtf(((a + c) + bb) * 0.5f);
-        const float minor = sqrtf(((a + c) - bb) * 0.5f);
-        const float Bx = cutoff * major, By = cutoff * minor;
-        const float evx = -b, evy = l1 - a;
-        const float el = sqrtf(evx * evx + evy * evy);
-        const float e1x = evx / el, e1y = evy / el;
-        const float e2x = e1y, e2y = -e1x;
-        rec.ux = (2.0f * e1x) / Bx; rec.uy = (-2.0f * e1y) / Bx;
-        rec.vx = (2.0f * e2x) / By; rec.vy = (-2.0f * e2y) / By;
-        const float hx = 0.5f * (fabsf(e1x) * Bx + fabsf(e2x) * By);
-        const float hy = 0.5f * (fabsf(e1y) * Bx + fabsf(e2y) * By);
-        if (rec.ux == rec.ux && rec.uy == rec.uy && rec.vx == rec.vx && rec.vy == rec.vy)
-            make_bbox(cx, cy, hx, hy, fc.Wi, fc.Hi, rec.bx, rec.by);
-        }
-        } else {
-            // ---- 2DGS surfel: gaussian_2d.wgsl:77-132 (homography) + :49-75 (quad)
-            float L[3][2];   // first two columns of A * R_std * S, R_std = transpose(Rm)
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                const float rc[3] = {Rm[j][0] * sc[j], Rm[j][1] * sc[j], Rm[j][2] * sc[j]};
-#pragma unroll
-                for (int i = 0; i < 3; ++i) L[i][j] = (A[i][0] * rc[0] + A[i][1] * rc[1]) + A[i][2] * rc[2];
-            }
-            float G[3][4];
-            mat4_dir(fc.clip_from_world, L[0][0], L[1][0], L[2][0], G[0]);
-            mat4_dir(fc.clip_from_world, L[0][1], L[1][1], L[2][1], G[1]);
-            mat4_point(fc.clip_from_world, k.pw[0], k.pw[1], k.pw[2], G[2]);
-            const float fxk = fc.p00 * W / 2.0f, fyk = fc.p11 * H / 2.0f;     // helpers.wgsl:122-135
-            const float cxk = (W - 1.0f) / 2.0f, cyk = (H - 1.0f) / 2.0f;
-            float T0[3], T1[3], T2[3];
-#pragma unroll
-            for (int j = 0; j < 3; ++j) {
-                T0[j] = fxk * G[j][0] + cxk * G[j][3];
-                T1[j] = fyk * G[j][1] + cyk * G[j][3];
-                T2[j] = G[j][3];
-            }
-            const float c2 = cutoff * cutoff;
-            const float test[3] = {c2, c2, -1.0f};
-            const float tt[3] = {test[0] * T2[0], test[1] * T2[1], test[2] * T2[2]};
-            const float d = dot3(tt, T2);
-            float Rq = 0.0f, mean0 = 0.0f, mean1 = 0.0f;
-            bool ok = !(fabsf(d) < 1.0e-4f);
-            if (ok) {
-                const float inv = 1.0f / d;
-                const float f[3] = {inv * test[0], inv * test[1], inv * test[2]};
-                const float t02[3] = {T0[0] * T2[0], T0[1] * T2[1], T0[2] * T2[2]};
-                const float t12[3] = {T1[0] * T2[0], T1[1] * T2[1], T1[2] * T2[2]};
-                mean0 = dot3(f, t02); mean1 = dot3(f, t12);
-                const float f0[3] = {f[0] * T0[0], f[1] * T0[1], f[2] * T0[2]};
-                const float f1[3] = {f[0] * T1[0], f[1] * T1[1], f[2] * T1[2]};
-                const float ex = mean0 * mean0 - dot3(f0, T0);
-                const float ey = mean1 * mean1 - dot3(f1, T1);
-                if (ex < 1.0e-4f || ey < 1.0e-4f) ok = false;
-                else Rq = fmaxf(fmaxf(sqrtf(ex), sqrtf(ey)), cutoff * 0.707106f);
-            }
-            if (ok) {
-                rec.ux = 2.0f / Rq; rec.uy = 0.0f; rec.vx = 0.0f; rec.vy = -2.0f / Rq;   // OBB branch: e1=(1,0), e2=(0,1)
-                const float h = 0.5f * Rq;
-                if (Rq == Rq) make_bbox(cx, cy, h, h, fc.Wi, fc.Hi, rec.bx, rec.by);
-                if (fc.aabb && extra != nullptr) {
-                    float4* e = extra + (size_t)r * 4;
-                    e[0] = make_float4(Rq, mean0, mean1, W / H);
-                    e[1] = make_float4(T0[0], T0[1], T0[2], 0.0f);
-                    e[2] = make_float4(T1[0], T1[1], T1[2], 0.0f);
-                    e[3] = make_float4(T2[0], T2[1], T2[2], 0.0f);
-                }
-            }
+            surfel_record(fc, A, Rm, sc, pw, cutoff, r, extra, rec);
         }
 
-        // colour source
-        float rgb[3] = {0.f, 0.f, 0.f};
-        if (fc.rasterize_mode == BGS_RASTERIZE_COLOR) {
-            float sh[48];
-            load_sh(sh);
-            // gaussian.wgsl:166-183,406-416
-            const float dlt[3] = {k.pw[0] - fc.cam[0], k.pw[1] - fc.cam[1], k.pw[2] - fc.cam[2]};
-            float dw[3], loc[3], dl[3];
-            normalize3(dlt, dw);
-            if (fc.model_identity) {     // the normalised model columns are the unit axes
-                loc[0] = dw[0]; loc[1] = dw[1]; loc[2] = dw[2];
-            } else {
-#pragma unroll
-                for (int cc = 0; cc < 3; ++cc) {
-                    const float col[3] = {A[0][cc], A[1][cc], A[2][cc]};
-                    float bn[3];
-                    normalize3(col, bn);
-                    loc[cc] = dot3(bn, dw);
-                }
-            }
-            normalize3(loc, dl);
-            // spherical_harmonics.wgsl:34-68
-            const float x = dl[0], y = dl[1], z = dl[2];
-            const float xx = x * x, yy = y * y, zz = z * z;
-            float basis[16];   // (the SH constants are folded in below: 16 multiplies instead of 48)
-            basis[0] = 1.0f;
-            basis[1] = y; basis[2] = z; basis[3] = x;
-            basis[4] = x * y; basis[5] = y * z; basis[6] = (2.0f * zz - xx) - yy;
-            basis[7] = x * z; basis[8] = xx - yy;
-            basis[9] = y * (3.0f * xx - yy);
-            basis[10] = (x * y) * z;
-            basis[11] = y * ((4.0f * zz - xx) - yy);
-            basis[12] = z * ((2.0f * zz - 3.0f * xx) - 3.0f * yy);
-            basis[13] = x * ((4.0f * zz - xx) - yy);
-            basis[14] = z * (xx - yy);
-            basis[15] = x * (xx - 3.0f * yy);
-#pragma unroll
-            for (int kk = 0; kk < 16; ++kk) basis[kk] *= c_shc[kk];
-#pragma unroll
-            for (int cc = 0; cc < 3; ++cc) {
-                float acc = 0.5f;
-#pragma unroll
-                for (int kk = 0; kk < 16; ++kk) acc = fmaf(sh[3 * kk + cc], basis[kk], acc);   // colour: FMA is fine
-                rgb[cc] = acc;
-            }
-            if (fc.color_space == 0u) {
-#pragma unroll
-                for (int cc = 0; cc < 3; ++cc) rgb[cc] = srgb_to_linear(rgb[cc]);
-            }
-        }
-        // aux outputs (bgs_render_aux, config C4): the Depth and Normal colour sources ride along with the main one, so one
-        // pass yields what three single-mode frames would (the geometry and alpha of a splat do not depend on the mode)
-        float drgb[3] = {0.f, 0.f, 0.f}, nrgb[3] = {0.f, 0.f, 0.f};
-        if (fc.rasterize_mode == BGS_RASTERIZE_DEPTH || fc.aux) {
-            float* rgb = drgb;
-            // material/depth.wgsl:3-11
-            const float dlt[3] = {k.pw[0] - fc.cam[0], k.pw[1] - fc.cam[1], k.pw[2] - fc.cam[2]};
-            const float depth = sqrtf(dot3(dlt, dlt));
-            const float dmin = ctr->depth_min, dmax = ctr->depth_max;
-            if (fc.n_cloud >= 2u) {   // the reference reads sorted[1]: undefined for a 1-gaussian cloud (oracle: black)
-            float nd = (depth - dmin) / (dmax - dmin);
-            nd = fminf(fmaxf(nd, 0.0f), 1.0f);   // fmin/fmax ignore a NaN operand, like the oracle's
-            float t1 = (nd - 0.5f) / (1.0f - 0.5f); t1 = fminf(fmaxf(t1, 0.0f), 1.0f);
-            float t2 = (nd - 0.0f) / (0.5f - 0.0f); t2 = fminf(fmaxf(t2, 0.0f), 1.0f);
-            rgb[0] = t1 * t1 * (3.0f - 2.0f * t1);
-            rgb[1] = 1.0f - fabsf(nd - 0.5f) * 2.0f;
-            rgb[2] = 1.0f - t2 * t2 * (3.0f - 2.0f * t2);
-            }
-        }
-        if (fc.rasterize_mode == BGS_RASTERIZE_POSITION) {
-            // gaussian.wgsl:375-376: (transformed_position - min) / (max - min)
-#pragma unroll
-            for (int cc = 0; cc < 3; ++cc) rgb[cc] = (k.pw[cc] - fc.aabb_min[cc]) / (fc.aabb_max[cc] - fc.aabb_min[cc]);
-        }
-        if (fc.rasterize_mode == BGS_RASTERIZE_NORMAL || fc.aux) {
-            float* rgb = nrgb;
-            // gaussian.wgsl:350-368
-            float SR[3], Ln[3], wn[4];
-#pragma unroll
-            for (int i = 0; i < 3; ++i) SR[i] = sc[i] * Rm[i][2];
-#pragma unroll
-            for (int i = 0; i < 3; ++i) Ln[i] = (A[i][0] * SR[0] + A[i][1] * SR[1]) + A[i][2] * SR[2];
-            mat4_dir(fc.view_from_world, Ln[0], Ln[1], Ln[2], wn);
-            const float l = sqrtf(((wn[0] * wn[0] + wn[1] * wn[1]) + wn[2] * wn[2]) + wn[3] * wn[3]);
-#pragma unroll
-            for (int cc = 0; cc < 3; ++cc) rgb[cc] = 0.5f * (wn[cc] / l + 1.0f);
-        }
-        if (fc.rasterize_mode == BGS_RASTERIZE_DEPTH) { rgb[0] = drgb[0]; rgb[1] = drgb[1]; rgb[2] = drgb[2]; }
-        if (fc.rasterize_mode == BGS_RASTERIZE_NORMAL) { rgb[0] = nrgb[0]; rgb[1] = nrgb[1]; rgb[2] = nrgb[2]; }
-        rec.r = rgb[0]; rec.g = rgb[1]; rec.b = rgb[2];
-        if (fc.draw_mode == BGS_DRAW_HIGHLIGHT_SELECTED && p4.w > 0.5f) {   // gaussian.wgsl:423-427
-            rec.r = 0.3f; rec.g = 1.0f; rec.b = 0.1f; rec.op = 1.0f;
-            drgb[0] = nrgb[0] = 0.3f; drgb[1] = nrgb[1] = 1.0f; drgb[2] = nrgb[2] = 0.1f;
-        }
+        // colour source.  The Depth and Normal ones also ride along with the main one as the aux outputs
+        // (bgs_render_aux, config C4): one pass yields what three single-mode frames would (the geometry and alpha of
+        // a splat do not depend on the mode)
+        const uint32_t mode = fc.rasterize_mode;
+        float rgb[3] = {0.f, 0.f, 0.f}, drgb[3] = {0.f, 0.f, 0.f}, nrgb[3] = {0.f, 0.f, 0.f};
+        if (mode == BGS_RASTERIZE_COLOR) sh_colour(fc, A, pw, sh, rgb);
+        if (mode == BGS_RASTERIZE_POSITION) position_colour(fc, pw, rgb);
+        if (mode == BGS_RASTERIZE_DEPTH || fc.aux) depth_colour(fc, ctr, pw, drgb);
+        if (mode == BGS_RASTERIZE_NORMAL || fc.aux) normal_colour(fc, A, Rm, sc, nrgb);
+        const bool depth = mode == BGS_RASTERIZE_DEPTH, normal = mode == BGS_RASTERIZE_NORMAL;
+        rec.r = depth ? drgb[0] : normal ? nrgb[0] : rgb[0];
+        rec.g = depth ? drgb[1] : normal ? nrgb[1] : rgb[1];
+        rec.b = depth ? drgb[2] : normal ? nrgb[2] : rgb[2];
+        if (fc.draw_mode == BGS_DRAW_HIGHLIGHT_SELECTED && p4.w > 0.5f) highlight_selected(rec, drgb, nrgb);
         if (fc.aux && aux != nullptr) {
             aux[(size_t)r * 2] = make_float4(drgb[0], drgb[1], drgb[2], 0.0f);
             aux[(size_t)r * 2 + 1] = make_float4(nrgb[0], nrgb[1], nrgb[2], 0.0f);
         }
     }
-    // 48 B record, three 16 B stores
-    float4* out = reinterpret_cast<float4*>(recs + r);
-    out[0] = make_float4(rec.cx, rec.cy, rec.ux, rec.uy);
-    out[1] = make_float4(rec.vx, rec.vy, __uint_as_float(rec.bx), __uint_as_float(rec.by));
-    out[2] = make_float4(rec.r, rec.g, rec.b, rec.op);
+    store_rec(recs + r, rec);
 }
 
 constexpr int PROJ_MIN_CTAS = 6;
@@ -493,14 +545,7 @@ project_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ ind
         const bool need_sh = fc.rasterize_mode == BGS_RASTERIZE_COLOR;
         uint32_t op_bits = 0u;
         const float4 p4 = Attr<F16>::load(blocks, id, sh, q, so, need_sh, &op_bits);
-        // f16 clouds: the adaptive cutoff of this 16-bit opacity comes from the per-context table (bit-identical)
-        const float cutoff_pre = (F16 && fc.adaptive) ? __ldg(cutoff_tab + op_bits) : __uint_as_float(0x7FC00000u);
-        project_one(fc, ctr, r, p4, q, so, cutoff_pre,
-                    [&](float* out) {
-#pragma unroll
-                        for (int i = 0; i < 48; ++i) out[i] = sh[i];
-                    },
-                    recs, extra, aux);
+        project_one<F16>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux);
     }
 }
 

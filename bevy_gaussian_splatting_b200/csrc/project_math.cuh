@@ -21,80 +21,32 @@ __device__ __forceinline__ void mat4_dir(const float* m, float x, float y, float
     for (int r = 0; r < 4; ++r) out[r] = (m[0 + r] * x + m[4 + r] * y) + m[8 + r] * z;
 }
 
-struct KeyOut {
-    uint32_t key;
-    bool visible;
-    float pw[3];
-    float ndc[2];
-    float d2;
-};
+// Key-gen's world position (radix.wgsl:89-90): M * (p, 1), skipping the multiply under an identity model matrix (the
+// common case) when p is finite, where x*1 + y*0 + z*0 + 0 == x bit for bit -- except that a -0 coordinate comes out
+// +0.  The sign of that zero changes no key and no visibility decision, but it does reach the projection's records,
+// so the projection keeps the full multiply.
+__device__ __forceinline__ void keygen_world_pos(const FrameConsts& c, float4 p, float pw[4]) {
+    if (c.model_identity && (fabsf(p.x) + fabsf(p.y)) + fabsf(p.z) < __uint_as_float(0x7F800000u)) {
+        pw[0] = p.x; pw[1] = p.y; pw[2] = p.z; pw[3] = 1.0f;
+    } else {
+        mat4_point(c.model, p.x, p.y, p.z, pw);
+    }
+}
 
-// radix.wgsl:86-101 (key) + transform.wgsl:5-14 (world_to_clip, in_frustum).
-__device__ __forceinline__ KeyOut key_of(const FrameConsts& c, float px, float py, float pz) {
-    KeyOut k;
-    float pw[4];
-    mat4_point(c.model, px, py, pz, pw);
-    k.pw[0] = pw[0]; k.pw[1] = pw[1]; k.pw[2] = pw[2];
+// transform.wgsl:5-14, literal: world_to_clip (three IEEE divisions by w + 1e-9) and in_frustum.
+__device__ __forceinline__ bool in_frustum(const FrameConsts& c, const float pw[3], float ndc[2]) {
     float cl[4];
     mat4_point(c.clip_from_world, pw[0], pw[1], pw[2], cl);
     const float den = cl[3] + 0.000000001f;
     const float nx = cl[0] / den, ny = cl[1] / den, nz = cl[2] / den;
-    k.ndc[0] = nx; k.ndc[1] = ny;
-    k.visible = fabsf(nx) < 1.1f && fabsf(ny) < 1.1f && fabsf(nz - 0.5f) < 0.5f;
-    const float dx = pw[0] - c.cam[0], dy = pw[1] - c.cam[1], dz = pw[2] - c.cam[2];
-    k.d2 = (dx * dx + dy * dy) + dz * dz;
-    uint32_t key = 0xFFFFFFFFu;
-    if (k.visible) key = 0xFFFFFFFFu - __float_as_uint(k.d2);
-    k.key = key >> c.key_shift;
-    return k;
+    ndc[0] = nx; ndc[1] = ny;
+    return fabsf(nx) < 1.1f && fabsf(ny) < 1.1f && fabsf(nz - 0.5f) < 0.5f;
 }
 
-// Key-gen's version of key_of: the SAME key and the SAME visibility decision, cheaper.
-//  * identity model matrix (the common case): M*(p,1) == p bit for bit when p is finite (x*1 + y*0 + z*0 + 0), so
-//    the multiply is skipped for finite positions;
-//  * the three IEEE divisions of world_to_clip only feed the frustum test here: one approximate reciprocal
-//    (|error| < 4e-7 relative) decides every gaussian whose ndc is not within 1e-4 of a frustum bound; the few that
-//    are fall back to the exact divisions.  Denominators outside [1e-30, 1e30] (rcp.approx flushes) also fall back.
-__device__ __forceinline__ uint32_t key_of_fast(const FrameConsts& c, float px, float py, float pz, bool& visible) {
-    float pw[4];
-    if (c.model_identity && (fabsf(px) + fabsf(py)) + fabsf(pz) < __uint_as_float(0x7F800000u)) {
-        pw[0] = px; pw[1] = py; pw[2] = pz;
-    } else {
-        mat4_point(c.model, px, py, pz, pw);
-    }
-    float cl[4];
-    mat4_point(c.clip_from_world, pw[0], pw[1], pw[2], cl);
-    const float den = cl[3] + 0.000000001f;
-    float rc;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(den));
-    const float ax = fabsf(cl[0] * rc), ay = fabsf(cl[1] * rc), z = cl[2] * rc;
-    const float ad = fabsf(den);
-    const bool sure_in = ax < 1.0999f && ay < 1.0999f && z > 1e-6f && z < 0.9999f;
-    const bool sure_out = ax > 1.1001f || ay > 1.1001f || z < -1e-6f || z > 1.0001f;
-    const bool den_ok = ad > 1e-30f && ad < 1e30f;
-    bool vis;
-    if (den_ok && (sure_in || sure_out)) {
-        vis = sure_in;
-    } else {
-        const float nx = cl[0] / den, ny = cl[1] / den, nz = cl[2] / den;
-        vis = fabsf(nx) < 1.1f && fabsf(ny) < 1.1f && fabsf(nz - 0.5f) < 0.5f;
-    }
-    visible = vis;
-    const float dx = pw[0] - c.cam[0], dy = pw[1] - c.cam[1], dz = pw[2] - c.cam[2];
-    const float d2 = (dx * dx + dy * dy) + dz * dz;
-    uint32_t key = 0xFFFFFFFFu;
-    if (vis) key = 0xFFFFFFFFu - __float_as_uint(d2);
-    return key >> c.key_shift;
-}
-
-// The visibility decision of key_of_fast alone (key-gen phase 1: one bit per gaussian, no key).
-__device__ __forceinline__ bool visible_fast(const FrameConsts& c, float px, float py, float pz) {
-    float pw[4];
-    if (c.model_identity && (fabsf(px) + fabsf(py)) + fabsf(pz) < __uint_as_float(0x7F800000u)) {
-        pw[0] = px; pw[1] = py; pw[2] = pz;
-    } else {
-        mat4_point(c.model, px, py, pz, pw);
-    }
+// in_frustum's decision, cheaper, for key-gen (which needs no ndc): one approximate reciprocal (|error| < 4e-7
+// relative) decides every gaussian whose ndc is not within 1e-4 of a frustum bound; the few that are fall back to
+// the exact divisions.  Denominators outside [1e-30, 1e30] (rcp.approx flushes) also fall back.
+__device__ __forceinline__ bool in_frustum_fast(const FrameConsts& c, const float pw[3]) {
     float cl[4];
     mat4_point(c.clip_from_world, pw[0], pw[1], pw[2], cl);
     const float den = cl[3] + 0.000000001f;
@@ -106,21 +58,21 @@ __device__ __forceinline__ bool visible_fast(const FrameConsts& c, float px, flo
     const bool sure_out = ax > 1.1001f || ay > 1.1001f || z < -1e-6f || z > 1.0001f;
     const bool den_ok = ad > 1e-30f && ad < 1e30f;
     if (den_ok && (sure_in || sure_out)) return sure_in;
-    const float nx = cl[0] / den, ny = cl[1] / den, nz = cl[2] / den;
-    return fabsf(nx) < 1.1f && fabsf(ny) < 1.1f && fabsf(nz - 0.5f) < 0.5f;
+    float ndc[2];
+    return in_frustum(c, pw, ndc);
 }
 
-// The key of a gaussian already known to be visible (key-gen phase 2): same pw, same d2 as key_of.
-__device__ __forceinline__ uint32_t key_only(const FrameConsts& c, float px, float py, float pz) {
-    float pw[4];
-    if (c.model_identity && (fabsf(px) + fabsf(py)) + fabsf(pz) < __uint_as_float(0x7F800000u)) {
-        pw[0] = px; pw[1] = py; pw[2] = pz;
-    } else {
-        mat4_point(c.model, px, py, pz, pw);
-    }
+// |pw - cam|^2 (radix.wgsl:92-93): what the depth key encodes; its square root is the Depth colour source's depth.
+__device__ __forceinline__ float cam_dist2(const FrameConsts& c, const float pw[3]) {
     const float dx = pw[0] - c.cam[0], dy = pw[1] - c.cam[1], dz = pw[2] - c.cam[2];
-    const float d2 = (dx * dx + dy * dy) + dz * dz;
-    return (0xFFFFFFFFu - __float_as_uint(d2)) >> c.key_shift;
+    return (dx * dx + dy * dy) + dz * dz;
+}
+
+// radix.wgsl:94-99: the depth key, far first; a culled gaussian's is all ones.
+__device__ __forceinline__ uint32_t depth_key(const FrameConsts& c, bool visible, float d2) {
+    uint32_t key = 0xFFFFFFFFu;
+    if (visible) key = 0xFFFFFFFFu - __float_as_uint(d2);
+    return key >> c.key_shift;
 }
 
 // Fixed-series natural log in f64 (the policy replacement for WGSL log(), gaussian.wgsl:229):

@@ -1,7 +1,7 @@
-"""The projection (project.cu) and key-gen (project_math.cuh) on the constructions of `project_cases.py`, against the
-oracle: sorted keys and permutation bit-exact, n_visible equal, every record's drawn / undrawn decision equal, drawn
-geometry and bboxes bit-exact (sign of zero counted, NaN compared as a class), colours within the per-record bound
-`project_cases.colour_bound`, Depth colours from the literal sorted[1] / sorted[N-1] range."""
+"""The projection (project.cu) and key-gen (keygen.cu over project_math.cuh) on the constructions of
+`project_cases.py`, against the oracle: sorted keys and permutation bit-exact, n_visible equal, every record's drawn /
+undrawn decision equal, drawn geometry and bboxes bit-exact (sign of zero counted, NaN compared as a class), colours
+within the per-record bound `project_cases.colour_bound`, Depth colours from the literal sorted[1] / sorted[N-1] range."""
 import numpy as np
 import pytest
 
