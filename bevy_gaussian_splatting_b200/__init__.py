@@ -10,6 +10,8 @@ from .gaussian import (PlanarGaussian3d, random_gaussians_3d, random_gaussians_3
                        SH_COEFF_COUNT)
 from .io import load_cloud, parse_ply_3d  # noqa: F401
 from .gcloud import decode_gcloud, encode_gcloud, read_gcloud, write_gcloud  # noqa: F401
-from .plugin import CloudTransform, GaussianSplattingPlugin, PlanarGaussian3dHandle  # noqa: F401
+from .particles import (PARTICLE_BEHAVIOR_DTYPE, PARTICLE_INACTIVE, ParticleBehaviors,  # noqa: F401
+                        random_particle_behaviors)
+from .plugin import CloudTransform, GaussianSplattingPlugin, ParticleBehaviorsHandle, PlanarGaussian3dHandle  # noqa: F401
 from .settings import (CloudSettings, DrawMode, GaussianColorSpace, GaussianMode, RadixSortDepthBits,  # noqa: F401
                        RasterizeMode, ShaderDefines, SortMode, SparseSelect)

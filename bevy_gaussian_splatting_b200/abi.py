@@ -74,6 +74,16 @@ class bgs_frame_stats(C.Structure):
     ]
 
 
+class bgs_particle_behavior(C.Structure):
+    """ParticleBehavior (src/morph/particle.rs:349-358), 64 B; the numpy twin is gaussian.PARTICLE_BEHAVIOR_DTYPE."""
+    _fields_ = [
+        ("indices", C.c_uint32 * 4),
+        ("velocity", C.c_float * 4),
+        ("acceleration", C.c_float * 4),
+        ("jerk", C.c_float * 4),
+    ]
+
+
 # every symbol include/bgs.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = [
@@ -87,6 +97,11 @@ SYMBOLS = [
     ("bgs_cloud_visibility_get", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_visibility_set", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_select_in_mesh", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32, _P, C.c_uint32, C.POINTER(C.c_uint32)]),
+    ("bgs_particles_create", C.c_int, [_P, _P, C.c_uint32, C.POINTER(_P)]),
+    ("bgs_particles_get", C.c_int, [_P, _P, _P]),
+    ("bgs_particles_destroy", None, [_P]),
+    ("bgs_cloud_particles_step", C.c_int, [_P, _P, _P, C.c_float]),
+    ("bgs_cloud_positions_get", C.c_int, [_P, _P, _P]),
     ("bgs_render", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P,
                              C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,

@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstring>
 #include <algorithm>
+#include <atomic>
 #include <mutex>
 #include <new>
 #include <vector>
@@ -77,6 +78,9 @@ uint32_t mesh_words_n_bin(const void* words_host);
 void launch_mesh_count(const float4* pos, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
                        const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, float* pos_w,
                        float* block_w, uint32_t block_stride, void* words, cudaStream_t stream);
+// particles.cu
+void launch_particle_step(void* behaviors, uint32_t count, float dt, float4* pos, void* blocks, uint32_t block_stride,
+                          cudaStream_t stream);
 }  // namespace bgs
 
 using namespace bgs;
@@ -89,6 +93,20 @@ struct bgs_cloud {
     bool cov;         // f16 layout whose second plane holds Covariance3dOpacityPacked128 records (precomputed Sigma3D)
     float4* pos;      // n * 16 B
     void* blocks;     // gaussian-major copy of every plane (f16: n * 128 B, f32: n * 256 B), what the projection gathers
+    // enqueued writes (particle steps): ev_write marks the last one, on whichever context's stream it was queued; every
+    // later reader or writer waits for it on the device.  Created by the first step; `stepped` is set once it exists,
+    // so a cloud that is never stepped costs its frames nothing
+    cudaEvent_t ev_write = nullptr;
+    std::atomic<bool> stepped{false};
+};
+
+// A ParticleBehaviors asset resident on one GPU: count 64 B records (bgs_particle_behavior), read and written by the step
+struct bgs_particles {
+    int device;
+    uint32_t count;
+    int64_t max_index;            // largest active gaussian index (-1: none is active)
+    void* d = nullptr;            // count * 64 B
+    cudaEvent_t ev_write = nullptr;   // the last step of these behaviours (recorded on the stepping context's stream)
 };
 
 // A grow-only device buffer.  grow() replaces a buffer smaller than `want` bytes by one of exactly `want` bytes, zeroed
@@ -172,6 +190,7 @@ struct bgs_context {
     // boxes | global records, and the pair side: digit histograms | per-cell ranges | pair keys / values x 2
     DevBuf<uint8_t> mesh_tri, mesh_pairs;
     bool async_pending = false;        // a BGS_FLAG_ASYNC frame has been enqueued and not yet completed
+    bool step_pending = false;         // a particle step has been enqueued since the last bgs_sync
     FrameCounters* ctr = nullptr;
     uint32_t* hist = nullptr;          // [8 + 4 * MAX_CHUNKS][256]: depth passes 0..3, pair passes 4..7 (round 0), 8 + 4r.. (round r)
     uint32_t* kg_block_cnt = nullptr;  // [kg_grid]: keygen_coop's per-CTA visible counts
@@ -606,6 +625,10 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
             c->clouds.erase(std::remove(c->clouds.begin(), c->clouds.end(), cl), c->clouds.end());
         }
     }
+    if (cl->ev_write) {   // particle steps still queued on any context write the planes
+        cudaEventSynchronize(cl->ev_write);
+        cudaEventDestroy(cl->ev_write);
+    }
     cudaFree(cl->pos); cudaFree(cl->blocks);
     delete cl;
 }
@@ -649,8 +672,14 @@ static bgs_status finish_frame(bgs_context* c) {
 
 bgs_status bgs_sync(bgs_context* c) {
     if (!c) return BGS_EINVAL;
-    if (!c->async_pending) return BGS_OK;
+    if (!c->async_pending && !c->step_pending) return BGS_OK;
     CU(c, cudaSetDevice(c->device));
+    c->step_pending = false;
+    if (!c->async_pending) {   // only particle steps were queued: no frame to account for
+        CU(c, cudaStreamSynchronize(c->stream));
+        CU(c, cudaGetLastError());
+        return BGS_OK;
+    }
     CU(c, cudaStreamSynchronize(c->stream));
     CU(c, cudaStreamSynchronize(c->stream_copy));
     c->copy_pending[0] = c->copy_pending[1] = false;
@@ -725,6 +754,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     const uint32_t num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     cudaStream_t q = c->stream;
     uint32_t launches = 0;
+    // a stepped cloud: the frame reads the positions of every step enqueued before it, on any context
+    if (cloud->stepped.load(std::memory_order_acquire)) CU(c, cudaStreamWaitEvent(q, cloud->ev_write, 0));
     CU(c, cudaMemsetAsync(c->arena.p, 0, c->arena.bytes, q));   // counters, histograms, ranges: ~0.4 MB
     CU(c, cudaEventRecord(c->ev[0], q));
     // ---- stage 1: key-gen (+ stable compaction of the visible set)
@@ -891,10 +922,18 @@ bgs_status bgs_render_aux(bgs_context* c, const bgs_cloud* cloud, const bgs_view
 // plane's .w (what key-gen streams) and the first 16 B of each gaussian-major block (what the projection reads): every
 // write updates both.
 
+// The particle steps enqueued on any context before a call that reads or writes the cloud on this context's stream.
+static bgs_status wait_cloud_steps(bgs_context* c, const bgs_cloud* cl) {
+    if (cl->stepped.load(std::memory_order_acquire)) CU(c, cudaStreamWaitEvent(c->stream, cl->ev_write, 0));
+    return BGS_OK;
+}
+
 // Before a selection writes a cloud: this context's queued frames are completed (their failure is returned, as a
 // synchronous render does), and so are the queued frames of every other context on the cloud's GPU, which may read it.
+// Particle steps queued on any context come first on the device (the writer runs on this context's stream).
 static bgs_status quiesce_for_write(bgs_context* c, const bgs_cloud* cl) {
     if (c->async_pending) TRY(bgs_sync(c));
+    TRY(wait_cloud_steps(c, cl));
     std::lock_guard<std::mutex> lk(g_registry_mu);
     for (bgs_context* o : g_contexts)
         if (o != c && o->device == cl->device && o->async_pending)
@@ -959,6 +998,7 @@ bgs_status bgs_cloud_visibility_get(bgs_context* c, const bgs_cloud* cl, float* 
     if (!cl || !out_vis) return fail(c, BGS_EINVAL, "visibility_get: null cloud or array");
     if (cl->device != c->device) return fail(c, BGS_EINVAL, "visibility_get: cloud lives on another device");
     CU(c, cudaSetDevice(c->device));
+    TRY(wait_cloud_steps(c, cl));
     CU(c, cudaMemcpy2DAsync(out_vis, 4, reinterpret_cast<const char*>(cl->pos) + 12, 16, 4, cl->n, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return BGS_OK;
@@ -1055,6 +1095,103 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* c, bgs_cloud* cl, const float* 
     CU(c, cudaMemcpyAsync(c->h_sticky + 1, mesh_words_inside(words), 4, cudaMemcpyDeviceToHost, q));
     CU(c, cudaStreamSynchronize(q));
     if (out_inside) *out_inside = c->h_sticky[1];
+    return BGS_OK;
+}
+
+// ---- particle behaviours (particles.cu).  The step is enqueued, never drained: it waits on the device for whatever
+// may still read the positions (the queued frames of every context on the GPU: each context's ev_done marks its last
+// frame; earlier steps of the cloud and of the behaviours), and marks itself on the cloud and the behaviours for
+// whatever comes after.
+
+bgs_status bgs_particles_create(bgs_context* c, const bgs_particle_behavior* behaviors, uint32_t count, bgs_particles** out) {
+    if (!c || !out) return BGS_EINVAL;
+    *out = nullptr;
+    if (!behaviors) return fail(c, BGS_EINVAL, "particles_create: null behaviours");
+    if (count == 0 || count >= (1u << 30)) return fail(c, BGS_EINVAL, "particles_create: count must be in [1, 2^30)");
+    static_assert(sizeof(bgs_particle_behavior) == 64, "ParticleBehavior is 64 B");
+    std::vector<uint32_t> active;
+    active.reserve(count);
+    for (uint32_t i = 0; i < count; ++i)
+        if (behaviors[i].indices[0] < 0x80000000u) active.push_back(behaviors[i].indices[0]);
+    std::sort(active.begin(), active.end());
+    const auto dup = std::adjacent_find(active.begin(), active.end());
+    if (dup != active.end()) return fail(c, BGS_EINVAL, "particles_create: two active behaviours name gaussian %u", *dup);
+    CU(c, cudaSetDevice(c->device));
+    bgs_particles* p = new (std::nothrow) bgs_particles();
+    if (!p) return BGS_ENOMEM;
+    p->device = c->device;
+    p->count = count;
+    p->max_index = active.empty() ? -1 : (int64_t)active.back();
+    cudaError_t e = cudaMalloc(&p->d, (size_t)count * 64);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_write, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(p->d, behaviors, (size_t)count * 64, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) {
+        bgs_particles_destroy(p);
+        return fail(c, e == cudaErrorMemoryAllocation ? BGS_ENOMEM : BGS_ECUDA, "particles_create: %s", cudaGetErrorString(e));
+    }
+    *out = p;
+    return BGS_OK;
+}
+
+bgs_status bgs_particles_get(bgs_context* c, const bgs_particles* p, bgs_particle_behavior* out) {
+    if (!c) return BGS_EINVAL;
+    if (!p || !out) return fail(c, BGS_EINVAL, "particles_get: null behaviours or array");
+    if (p->device != c->device) return fail(c, BGS_EINVAL, "particles_get: behaviours live on another device");
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaStreamWaitEvent(c->stream, p->ev_write, 0));   // every step of these behaviours, on any context
+    CU(c, cudaMemcpyAsync(out, p->d, (size_t)p->count * 64, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
+}
+
+void bgs_particles_destroy(bgs_particles* p) {
+    if (!p) return;
+    cudaSetDevice(p->device);
+    if (p->ev_write) {   // steps still queued on any context read and write the records
+        cudaEventSynchronize(p->ev_write);
+        cudaEventDestroy(p->ev_write);
+    }
+    cudaFree(p->d);
+    delete p;
+}
+
+bgs_status bgs_cloud_particles_step(bgs_context* c, bgs_cloud* cl, bgs_particles* p, float delta_time) {
+    if (!c) return BGS_EINVAL;
+    if (!cl || !p) return fail(c, BGS_EINVAL, "particles_step: null cloud or behaviours");
+    if (!std::isfinite(delta_time)) return fail(c, BGS_EINVAL, "particles_step: delta_time must be finite");
+    if (cl->device != c->device || p->device != c->device)
+        return fail(c, BGS_EINVAL, "particles_step: cloud or behaviours live on another device");
+    if (p->max_index >= (int64_t)cl->n)
+        return fail(c, BGS_EINVAL, "particles_step: behaviour names gaussian %lld of a cloud of %u", (long long)p->max_index, cl->n);
+    CU(c, cudaSetDevice(c->device));
+    cudaStream_t q = c->stream;
+    {
+        // (under the registry lock: another context's step of the same cloud or behaviours waits and records in turn)
+        std::lock_guard<std::mutex> lk(g_registry_mu);
+        if (!cl->ev_write) CU(c, cudaEventCreateWithFlags(&cl->ev_write, cudaEventDisableTiming));
+        for (bgs_context* o : g_contexts)
+            if (o != c && o->device == c->device) CU(c, cudaStreamWaitEvent(q, o->ev_done, 0));
+        if (cl->stepped.load(std::memory_order_relaxed)) CU(c, cudaStreamWaitEvent(q, cl->ev_write, 0));
+        CU(c, cudaStreamWaitEvent(q, p->ev_write, 0));
+        launch_particle_step(p->d, p->count, delta_time, cl->pos, cl->blocks, (uint32_t)(block_bytes(cl) / 16), q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaEventRecord(cl->ev_write, q));
+        CU(c, cudaEventRecord(p->ev_write, q));
+        cl->stepped.store(true, std::memory_order_release);
+    }
+    c->step_pending = true;
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_positions_get(bgs_context* c, const bgs_cloud* cl, float* out_pos_vis) {
+    if (!c) return BGS_EINVAL;
+    if (!cl || !out_pos_vis) return fail(c, BGS_EINVAL, "positions_get: null cloud or array");
+    if (cl->device != c->device) return fail(c, BGS_EINVAL, "positions_get: cloud lives on another device");
+    CU(c, cudaSetDevice(c->device));
+    TRY(wait_cloud_steps(c, cl));
+    CU(c, cudaMemcpyAsync(out_pos_vis, cl->pos, (size_t)cl->n * 16, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
     return BGS_OK;
 }
 

@@ -19,6 +19,7 @@ import numpy as np
 from . import abi
 from .camera import GaussianCamera, View
 from .gaussian import PlanarGaussian3d
+from .particles import PARTICLE_BEHAVIOR_DTYPE, as_particle_behaviors
 from .settings import CloudSettings, SparseSelect
 
 
@@ -67,6 +68,35 @@ class PlanarGaussian3dHandle:
     def destroy(self):
         if self._h:
             self._lib.bgs_cloud_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
+class ParticleBehaviorsHandle:
+    """A `ParticleBehaviors` asset resident in HBM (`bgs_particles`): what the reference attaches to a cloud entity."""
+
+    def __init__(self, plugin: "GaussianSplattingPlugin", behaviors):
+        b = as_particle_behaviors(behaviors)
+        self._plugin = plugin
+        self._lib = plugin._lib
+        self.count = len(b)
+        self._h = C.c_void_p()
+        plugin._check(self._lib.bgs_particles_create(plugin._ctx, _ptr(b), self.count, C.byref(self._h)))
+
+    def get(self) -> np.ndarray:
+        """The current records (velocity and acceleration advanced by every step queued so far)."""
+        out = np.empty(self.count, PARTICLE_BEHAVIOR_DTYPE)
+        self._plugin._check(self._lib.bgs_particles_get(self._plugin._ctx, self._h, _ptr(out)))
+        return out
+
+    def destroy(self):
+        if self._h:
+            self._lib.bgs_particles_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -249,6 +279,22 @@ class GaussianSplattingPlugin:
     def selection(self, handle: PlanarGaussian3dHandle) -> np.ndarray:
         """Indices of the selected gaussians: visibility >= 0.5, the ones DrawMode::Selected draws."""
         return np.flatnonzero(self.visibility(handle) >= 0.5).astype(np.uint32)
+
+    # -- particle behaviours (src/morph/particle.rs): an enqueued per-frame edit of the positions (the rule: include/bgs.h)
+    def add_particles(self, behaviors) -> ParticleBehaviorsHandle:
+        """Upload a ParticleBehaviors array (PARTICLE_BEHAVIOR_DTYPE records).  Duplicate active indices are refused."""
+        return ParticleBehaviorsHandle(self, behaviors)
+
+    def step_particles(self, handle: PlanarGaussian3dHandle, particles: ParticleBehaviorsHandle, delta_time: float) -> None:
+        """One step of every behaviour over `delta_time` seconds, enqueued on this context: frames rendered before it
+        (on any context) see the old positions, everything after it the new ones.  `sync()` completes it."""
+        self._check(self._lib.bgs_cloud_particles_step(self._ctx, handle._h, particles._h, C.c_float(delta_time)))
+
+    def positions(self, handle: PlanarGaussian3dHandle) -> np.ndarray:
+        """The position plane, (n, 4) float32 (x, y, z, visibility), after every step queued on the cloud."""
+        out = np.empty((handle.n, 4), np.float32)
+        self._check(self._lib.bgs_cloud_positions_get(self._ctx, handle._h, _ptr(out)))
+        return out
 
     # -- parity / measurement hooks
     def frame_stats(self) -> abi.bgs_frame_stats:

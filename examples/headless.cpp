@@ -3,10 +3,14 @@
 //
 //   headless [count=100000] [width=1920] [height=1080] [global_scale=1.0] [out=headless_output/0.ppm]
 //            [--dump-cloud file] [--raw file] [--remove-floaters radius]
+//            [--particles N --steps K --dt S [--dump-particles file]]
 // --dump-cloud writes the four f32 planes (n, then pos_vis, sh, rot, scale_opacity) so another host can
 // render the identical cloud; --raw writes the RGBA8 frame bytes.  --remove-floaters selects the sparse gaussians
 // (SparseSelect with that radius), inverts the selection and draws only the rest (DrawMode::Selected), the
 // reference converter's floater filter (tools/ply_to_gcloud.rs:54-66) applied to the resident cloud.
+// --particles attaches random_particle_behaviors(N, 0) to the cloud and enqueues K steps of S seconds before the frames
+// (the reference's morph_particles feature, stepped once per frame); --dump-particles writes N (u64), the behaviours
+// before and after the steps (N * 64 B each) and the position plane after them (count * 16 B).
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -20,12 +24,18 @@ int main(int argc, char** argv) {
     size_t count = 100000; int W = 1920, H = 1080; float scale = 1.0f;
     std::string out = "headless_output/0.ppm", dump, raw;
     float floater_radius = 0.0f;
+    size_t n_particles = 0; int steps = 0; float dt = 1.0f / 60.0f;
+    std::string dump_particles;
     int pos = 0;
     for (int i = 1; i < argc; ++i) {
         const std::string a = argv[i];
         if (a == "--dump-cloud" && i + 1 < argc) { dump = argv[++i]; continue; }
         if (a == "--raw" && i + 1 < argc) { raw = argv[++i]; continue; }
         if (a == "--remove-floaters" && i + 1 < argc) { floater_radius = (float)std::atof(argv[++i]); continue; }
+        if (a == "--particles" && i + 1 < argc) { n_particles = std::strtoull(argv[++i], nullptr, 10); continue; }
+        if (a == "--steps" && i + 1 < argc) { steps = std::atoi(argv[++i]); continue; }
+        if (a == "--dt" && i + 1 < argc) { dt = (float)std::atof(argv[++i]); continue; }
+        if (a == "--dump-particles" && i + 1 < argc) { dump_particles = argv[++i]; continue; }
         switch (pos++) {
             case 0: count = std::strtoull(a.c_str(), nullptr, 10); break;
             case 1: W = std::atoi(a.c_str()); break;
@@ -47,6 +57,22 @@ int main(int argc, char** argv) {
             plugin.invert_selection(handle);
             settings.draw_mode = bgs::DrawMode::Selected;
             std::printf("floaters: %u of %zu gaussians hidden\n", sparse, count);
+        }
+        if (n_particles > 0) {
+            const bgs::ParticleBehaviors behaviors = bgs::random_particle_behaviors(n_particles, 0);
+            bgs::ParticleBehaviorsHandle particles = plugin.add_particles(behaviors);
+            for (int k = 0; k < steps; ++k) plugin.step_particles(handle, particles, dt);
+            const bgs::ParticleBehaviors after = plugin.particles(particles);
+            const std::vector<float> moved = plugin.positions(handle);
+            std::printf("particles: %zu behaviours, %d steps of %g s\n", n_particles, steps, (double)dt);
+            if (!dump_particles.empty()) {
+                std::ofstream f(dump_particles, std::ios::binary);
+                const uint64_t n = n_particles;
+                f.write((const char*)&n, 8);
+                f.write((const char*)behaviors.data(), n * 64);
+                f.write((const char*)after.data(), n * 64);
+                f.write((const char*)moved.data(), moved.size() * 4);
+            }
         }
         const bgs_view view = bgs::headless_view(W, H);
         std::vector<unsigned char> frame((size_t)W * H * 4);

@@ -200,6 +200,61 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* ctx, bgs_cloud* cloud, const fl
                                     const float* mesh_from_cloud /* 16, column-major, may be NULL */, uint32_t mode,
                                     uint32_t* out_inside /* may be NULL */);
 
+/* Particle behaviours (src/morph/particle.rs, particle.wgsl; the reference's `morph_particles` feature): a
+ * ParticleBehaviors asset moves the gaussians it names every frame, in place, without a re-upload.
+ *
+ * bgs_particle_behavior is ParticleBehavior (particle.rs:349-358), 64 B.  indices[0] = the gaussian's index; a value
+ * >= 2^31 (negative read as i32, as the shader reads it) marks the behaviour inactive; indices[1..3] are carried and
+ * unused.
+ * bgs_particles_create: uploads `count` behaviours (count in [1, 2^30)); two active behaviours naming the same gaussian
+ *   -> BGS_EINVAL.  bgs_particles_get copies the current records back (count of them); bgs_particles_destroy releases
+ *   them (steps still queued on any context complete first).
+ * bgs_cloud_particles_step: one step of every behaviour over delta_time dt (particle.wgsl:36-52).  The rule, exactly:
+ *   for each active behaviour, with p = pos_vis[indices[0]] (all four lanes: the visibility lane .w moves too),
+ *   C6 = (float)(1.0 / 6.0) and every operation f32 round-to-nearest-even without FMA, per lane:
+ *     dp = ((v*dt) + (((0.5f*a)*dt)*dt)) + ((((C6*j)*dt)*dt)*dt)
+ *     dv = (a*dt) + (((0.5f*j)*dt)*dt)
+ *     da = j*dt
+ *   pos_vis[indices[0]] := p + dp, velocity := v + dv, acceleration := a + da; jerk and indices are never written.
+ *   Inactive behaviours write nothing; gaussians no active behaviour names are untouched; non-finite values propagate
+ *   as the arithmetic gives them.  Both device copies of the position (the plane key-gen streams, the block the
+ *   projection reads) get the same four floats.  dt may be negative or zero.
+ *   dt NaN or infinite, a behaviour naming a gaussian >= the cloud's n, a null argument, or a cloud or behaviours on
+ *   another device than the context's -> BGS_EINVAL; a refused call changes nothing.
+ * Ordering.  The step is ENQUEUED on the context's render stream (one kernel) and returns: no host synchronisation.
+ *   Over every context on the cloud's GPU: a frame (or any call) enqueued before the step, on any context, reads the
+ *   positions from before it; every call after it, on any context, observes it -- bgs_render, bgs_render_aux, the
+ *   selection calls, bgs_cloud_visibility_get / _set, bgs_cloud_positions_get and further steps.  Steps of one
+ *   bgs_particles, or of one cloud, run in call order whatever context queued them.  bgs_cloud_destroy and
+ *   bgs_particles_destroy wait for steps queued on any context.  bgs_sync(ctx) completes ctx's queued steps; a fault
+ *   of a step is reported by the next synchronising call on that context.  Frames of a cloud that was never stepped
+ *   run exactly as before (no added wait, no added launch).
+ * bgs_cloud_positions_get: the position plane, n * 4 floats (x, y, z, visibility), after every step queued on the cloud.
+ * Where this port deliberately differs from the reference:
+ *   1. Out-of-bounds dispatch: the shader indexes gid.x * 32 + gid.y with @workgroup_size(32, 32) over ceil(count / 32)
+ *      workgroups, ~32x more invocations than behaviours; the extra ones read past the array, and under robust-access
+ *      clamping the last behaviour is applied many times in one frame, racing with itself.  Here each behaviour is
+ *      applied exactly once per step.
+ *   2. Indices past the cloud and duplicate indices (particle_count may exceed the cloud, viewer.rs:407-438; two
+ *      behaviours on one gaussian race) are refused with BGS_EINVAL.
+ *   3. The reference runs the pass once per camera view (particle.rs:272-323: two cameras move the particles twice a
+ *      frame), unordered against the sort (sort/radix.rs:97-118).  Here the caller steps explicitly, and a frame sees
+ *      exactly the steps enqueued before it.
+ *   4. The entity's Aabb is not updated, as in the reference (gaussian/cloud.rs:43): RasterizeMode::Position keeps
+ *      the uniform's aabb_min / aabb_max as the caller passes them. */
+typedef struct bgs_particles bgs_particles; /* opaque, library-owned: a ParticleBehaviors asset resident on one GPU */
+typedef struct {
+    uint32_t indices[4]; /* [0] = gaussian index; >= 2^31 (i32 < 0) = inactive; [1..3] carried, unused */
+    float velocity[4];
+    float acceleration[4];
+    float jerk[4];
+} bgs_particle_behavior;
+bgs_status bgs_particles_create(bgs_context* ctx, const bgs_particle_behavior* behaviors, uint32_t count, bgs_particles** out);
+bgs_status bgs_particles_get(bgs_context* ctx, const bgs_particles* particles, bgs_particle_behavior* out /* count */);
+void bgs_particles_destroy(bgs_particles* particles);
+bgs_status bgs_cloud_particles_step(bgs_context* ctx, bgs_cloud* cloud, bgs_particles* particles, float delta_time);
+bgs_status bgs_cloud_positions_get(bgs_context* ctx, const bgs_cloud* cloud, float* out_pos_vis /* n * 4 */);
+
 /* One view of one cloud: key-gen -> depth radix sort -> projection + SH colour -> tile
  * binning -> per-tile front-to-back blend.  out_rgba is caller-owned (host pointer, or a
  * device pointer when out_is_device_ptr != 0); may be NULL to keep the frame on the device. */

@@ -7,6 +7,7 @@
 //   PlanarGaussian3d                 src/gaussian/formats/planar_3d.rs:28-54 (struct of four planes)
 //   random_gaussians_3d_seeded       src/gaussian/formats/planar_3d.rs:120-191 (distributions + field order)
 //   GaussianCamera                   src/camera.rs:6-9
+//   ParticleBehaviors                src/morph/particle.rs:349-410 (random_particle_behaviors: distributions)
 //   GaussianSplattingPlugin          src/lib.rs:48-80 -- here: owns the bgs_context of one GPU; render_view() is
 //                                    run_radix_sort (src/sort/radix.rs:616-756) + DrawGaussians
 //                                    (src/render/mod.rs:986-992) for one view
@@ -110,6 +111,27 @@ inline PlanarGaussian3d random_gaussians_3d_seeded(size_t n, uint64_t seed) {
     return c;
 }
 
+// random_particle_behaviors (particle.rs:374-410): behaviour i moves gaussian i; velocity U(-1, 1), acceleration
+// U(-0.01, 0.01), jerk U(-1e-4, 1e-4) in all four lanes.  The same splitmix64 stream as above, seeded.
+using ParticleBehaviors = std::vector<bgs_particle_behavior>;
+inline ParticleBehaviors random_particle_behaviors(size_t n, uint64_t seed) {
+    ParticleBehaviors b(n);
+    uint64_t ctr = seed * 0x9E3779B97F4A7C15ull + 0x7654321ull;
+    auto uni = [&ctr]() {
+        uint64_t z = (ctr += 0x9E3779B97F4A7C15ull);
+        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull; z = (z ^ (z >> 27)) * 0x94D049BB133111EBull; z ^= z >> 31;
+        return (float)(z >> 40) * (1.0f / 16777216.0f);   // [0, 1)
+    };
+    for (size_t i = 0; i < n; ++i) {
+        b[i].indices[0] = (uint32_t)i;
+        b[i].indices[1] = b[i].indices[2] = b[i].indices[3] = 0;
+        for (int k = 0; k < 4; ++k) b[i].acceleration[k] = (uni() * 2.0f - 1.0f) * 0.01f;
+        for (int k = 0; k < 4; ++k) b[i].jerk[k] = (uni() * 2.0f - 1.0f) * 1e-4f;
+        for (int k = 0; k < 4; ++k) b[i].velocity[k] = uni() * 2.0f - 1.0f;
+    }
+    return b;
+}
+
 struct GaussianCamera { bool warmup = false; };   // src/camera.rs:6-9
 
 // Column-major 4x4 helpers (Bevy/glam conventions).
@@ -180,6 +202,21 @@ private:
     bgs_cloud* h_ = nullptr;
     uint32_t n_ = 0;
     float aabb_min_[3] = {0, 0, 0}, aabb_max_[3] = {1, 1, 1};
+};
+
+class ParticleBehaviorsHandle {   // a ParticleBehaviors asset resident in HBM (bgs_particles)
+public:
+    ParticleBehaviorsHandle() = default;
+    ParticleBehaviorsHandle(const ParticleBehaviorsHandle&) = delete;
+    ParticleBehaviorsHandle& operator=(const ParticleBehaviorsHandle&) = delete;
+    ParticleBehaviorsHandle(ParticleBehaviorsHandle&& o) noexcept : h_(o.h_), count_(o.count_) { o.h_ = nullptr; }
+    ~ParticleBehaviorsHandle() { if (h_) bgs_particles_destroy(h_); }
+    bgs_particles* get() const { return h_; }
+    uint32_t len() const { return count_; }
+private:
+    friend class GaussianSplattingPlugin;
+    bgs_particles* h_ = nullptr;
+    uint32_t count_ = 0;
 };
 
 class GaussianSplattingPlugin {
@@ -284,6 +321,33 @@ public:
         for (uint32_t i = 0; i < (uint32_t)v.size(); ++i)
             if (v[i] >= 0.5f) idx.push_back(i);
         return idx;
+    }
+    // Particle behaviours (src/morph/particle.rs; the rule and its ordering: bgs.h).  step_particles only enqueues the
+    // step: frames rendered before it (on any context) see the old positions, everything after it the new ones.
+    ParticleBehaviorsHandle add_particles(const ParticleBehaviors& behaviors) {
+        ParticleBehaviorsHandle h;
+        h.count_ = (uint32_t)behaviors.size();
+        check(bgs_particles_create(ctx_, behaviors.data(), h.count_, &h.h_));
+        return h;
+    }
+    ParticleBehaviors particles(const ParticleBehaviorsHandle& p) {
+        ParticleBehaviors b(p.len());
+        check(bgs_particles_get(ctx_, p.get(), b.data()));
+        return b;
+    }
+    void step_particles(PlanarGaussian3dHandle& cloud, ParticleBehaviorsHandle& p, float delta_time) {
+        check(bgs_cloud_particles_step(ctx_, cloud.get(), p.get(), delta_time));
+    }
+    std::vector<float> positions(const PlanarGaussian3dHandle& cloud) {   // n * 4: x, y, z, visibility
+        std::vector<float> v((size_t)cloud.len() * 4);
+        check(bgs_cloud_positions_get(ctx_, cloud.get(), v.data()));
+        return v;
+    }
+    bool sync() {   // complete the queued frames and steps; false: the last queued frame must be rendered again
+        const bgs_status st = bgs_sync(ctx_);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
     }
     bgs_frame_stats frame_stats() { bgs_frame_stats fs{}; check(bgs_frame_stats_get(ctx_, &fs)); return fs; }
     bgs_context* context() const { return ctx_; }
