@@ -97,6 +97,9 @@ SYMBOLS = [
     ("bgs_cloud_visibility_get", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_visibility_set", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_select_in_mesh", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32, _P, C.c_uint32, C.POINTER(C.c_uint32)]),
+    ("bgs_cloud_subset", C.c_int, [_P, _P, _P, C.c_uint32, C.POINTER(_P), C.POINTER(C.c_uint32)]),
+    ("bgs_cloud_download_f32", C.c_int, [_P, _P, _P, _P, _P, _P]),
+    ("bgs_cloud_download_f16", C.c_int, [_P, _P, _P, _P, _P]),
     ("bgs_particles_create", C.c_int, [_P, _P, C.c_uint32, C.POINTER(_P)]),
     ("bgs_particles_get", C.c_int, [_P, _P, _P]),
     ("bgs_particles_destroy", None, [_P]),

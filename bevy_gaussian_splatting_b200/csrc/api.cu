@@ -81,6 +81,14 @@ void launch_mesh_count(const float4* pos, uint32_t n, const float* mesh_from_clo
 // particles.cu
 void launch_particle_step(void* behaviors, uint32_t count, float dt, float4* pos, void* blocks, uint32_t block_stride,
                           cudaStream_t stream);
+// subset.cu
+uint32_t subset_num_ctas(uint32_t n);
+void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t* cta_cnt, uint32_t* total, cudaStream_t stream);
+void launch_subset_scatter(bool f16, const void* pos, const void* blocks, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
+                           void* out_pos, void* out_blocks, cudaStream_t stream);
+void launch_subset_gather(bool f16, const void* pos, const void* blocks, const uint32_t* idx, uint32_t k, void* out_pos,
+                          void* out_blocks, cudaStream_t stream);
+void launch_unpack(bool f16, const void* blocks, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream);
 }  // namespace bgs
 
 using namespace bgs;
@@ -208,6 +216,9 @@ struct bgs_context {
     // per-frame arena + its pinned copy): a queued async frame that overflowed the pair buffer is never missed
     uint32_t* d_sticky = nullptr;
     uint32_t* h_sticky = nullptr;      // [0] the copy of *d_sticky, [1] a selection's selected / inside count
+    // bgs_cloud_download_*'s two pinned bounce buffers (2 x 30 MB, allocated by the first download, kept until the
+    // context goes): one chunk's planes each, so the host's copy of one chunk overlaps the device-to-host copy of the next
+    uint8_t* h_bounce = nullptr;
     std::vector<bgs_cloud*> clouds;    // clouds uploaded through this context (their ctx is nulled on destroy)
 
     FrameFacts pend, last;
@@ -546,6 +557,7 @@ void bgs_context_destroy(bgs_context* c) {
     c->each_stream([](cudaStream_t& s, int) { if (s) cudaStreamDestroy(s); });
     if (c->h_ctr) cudaFreeHost(c->h_ctr);
     if (c->h_sticky) cudaFreeHost(c->h_sticky);
+    if (c->h_bounce) cudaFreeHost(c->h_bounce);
     cudaFree(c->d_sticky);
     cudaFree(c->cutoff_tab);
     delete c;   // (releases every DevBuf)
@@ -1193,6 +1205,157 @@ bgs_status bgs_cloud_positions_get(bgs_context* c, const bgs_cloud* cl, float* o
     CU(c, cudaMemcpyAsync(out_pos_vis, cl->pos, (size_t)cl->n * 16, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return BGS_OK;
+}
+
+// ---- subset and download (subset.cu).  Both only read the source cloud, after every particle step queued on it (on
+// the device, like visibility_get); neither drains another context's frames.  Their scratch is their own, allocated and
+// released on the render stream within the call (stream-ordered: no device-wide synchronisation), so the frame's
+// buffers, the debug hooks and the next frame's plan are untouched.
+
+// Device scratch of one call, released on the stream when it goes out of scope.
+namespace {
+struct StreamScratch {
+    void* p = nullptr;
+    cudaStream_t q;
+    explicit StreamScratch(cudaStream_t s) : q(s) {}
+    StreamScratch(const StreamScratch&) = delete;
+    StreamScratch& operator=(const StreamScratch&) = delete;
+    ~StreamScratch() { if (p) cudaFreeAsync(p, q); }
+    cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes, q); }
+};
+}  // namespace
+
+bgs_status bgs_cloud_subset(bgs_context* c, const bgs_cloud* cl, const uint32_t* indices, uint32_t k, bgs_cloud** out,
+                            uint32_t* out_n) {
+    if (!c) return BGS_EINVAL;
+    if (out) *out = nullptr;
+    if (!cl || !out) return fail(c, BGS_EINVAL, "subset: null cloud or out");
+    if (cl->device != c->device) return fail(c, BGS_EINVAL, "subset: cloud lives on another device");
+    if (!indices && k != 0) return fail(c, BGS_EINVAL, "subset: selection mode (indices == NULL) takes k == 0");
+    if (indices && (k == 0 || k >= (1u << 30))) return fail(c, BGS_EINVAL, "subset: k must be in [1, 2^30)");
+    for (uint32_t j = 0; indices && j < k; ++j)
+        if (indices[j] >= cl->n) return fail(c, BGS_EINVAL, "subset: index %u at %u is >= the cloud's %u gaussians", indices[j], j, cl->n);
+    CU(c, cudaSetDevice(c->device));
+    TRY(wait_cloud_steps(c, cl));
+    cudaStream_t q = c->stream;
+    const uint32_t n = cl->n;
+    StreamScratch scratch(q);
+    // selection mode: mask words | CTA counts (-> offsets) | the total
+    const size_t o_cnt = align_up((size_t)(n + 31) / 32 * 4, 256), o_tot = align_up(o_cnt + (size_t)subset_num_ctas(n) * 4, 256);
+    uint32_t kept = k;
+    if (!indices) {
+        CU(c, scratch.alloc(o_tot + 4));
+        uint8_t* s = static_cast<uint8_t*>(scratch.p);
+        launch_subset_count(cl->pos, n, reinterpret_cast<uint32_t*>(s), reinterpret_cast<uint32_t*>(s + o_cnt),
+                            reinterpret_cast<uint32_t*>(s + o_tot), q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaMemcpyAsync(c->h_sticky + 1, s + o_tot, 4, cudaMemcpyDeviceToHost, q));
+        CU(c, cudaStreamSynchronize(q));
+        kept = c->h_sticky[1];
+        if (kept == 0) {
+            if (out_n) *out_n = 0;
+            return BGS_OK;
+        }
+    } else {
+        CU(c, scratch.alloc((size_t)k * 4));
+        CU(c, cudaMemcpyAsync(scratch.p, indices, (size_t)k * 4, cudaMemcpyHostToDevice, q));
+    }
+    bgs_cloud* nc = new (std::nothrow) bgs_cloud();
+    if (!nc) return fail(c, BGS_ENOMEM, "subset: out of host memory");
+    nc->ctx = c; nc->device = c->device; nc->n = kept; nc->f16 = cl->f16; nc->cov = cl->cov;
+    nc->pos = nullptr; nc->blocks = nullptr;
+    cudaError_t e = cudaMalloc(&nc->pos, (size_t)kept * 16);
+    if (e == cudaSuccess) e = cudaMalloc(&nc->blocks, (size_t)kept * block_bytes(cl));
+    if (e == cudaSuccess) {
+        if (!indices) {
+            const uint8_t* s = static_cast<const uint8_t*>(scratch.p);
+            launch_subset_scatter(cl->f16, cl->pos, cl->blocks, n, reinterpret_cast<const uint32_t*>(s),
+                                  reinterpret_cast<const uint32_t*>(s + o_cnt), nc->pos, nc->blocks, q);
+        } else {
+            launch_subset_gather(cl->f16, cl->pos, cl->blocks, static_cast<const uint32_t*>(scratch.p), k, nc->pos, nc->blocks, q);
+        }
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+    if (e != cudaSuccess) {
+        cudaFree(nc->pos); cudaFree(nc->blocks);
+        delete nc;
+        return fail(c, e == cudaErrorMemoryAllocation ? BGS_ENOMEM : BGS_ECUDA, "subset: %s", cudaGetErrorString(e));
+    }
+    {
+        std::lock_guard<std::mutex> lk(g_registry_mu);
+        c->clouds.push_back(nc);
+    }
+    *out = nc;
+    if (out_n) *out_n = kept;
+    return BGS_OK;
+}
+
+// gaussians per chunk of a download: the device staging arrays hold one chunk (f32: 28 MB), each of the context's two
+// pinned bounce buffers one chunk's four planes (f32: 30 MB)
+constexpr uint32_t DOWNLOAD_CHUNK = 1u << 17;
+constexpr size_t DOWNLOAD_BOUNCE_BYTES = (size_t)DOWNLOAD_CHUNK * (16 + 192 + 16 + 16);
+
+// Per chunk: unpack into device staging, copy the chunk's position plane and the staged planes to a pinned bounce
+// buffer, and -- while the next chunk goes the same way into the other bounce buffer -- copy it into the caller's arrays.
+static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, bool f16, float* pos_vis, void* sh, void* rot, void* so) {
+    if (!c) return BGS_EINVAL;
+    if (!cl || !pos_vis || !sh || !rot || (!f16 && !so)) return fail(c, BGS_EINVAL, "download: null cloud or plane pointer");
+    if (cl->device != c->device) return fail(c, BGS_EINVAL, "download: cloud lives on another device");
+    if (cl->f16 != f16) return fail(c, BGS_EINVAL, "download: the cloud is in the %s layout", cl->f16 ? "f16" : "f32");
+    CU(c, cudaSetDevice(c->device));
+    TRY(wait_cloud_steps(c, cl));
+    cudaStream_t q = c->stream;
+    const uint32_t n = cl->n, m_max = std::min(n, DOWNLOAD_CHUNK);
+    const size_t sh_b = f16 ? 96 : 192, so_b = f16 ? 0 : 16;
+    const size_t plane_b[4] = {16, sh_b, 16, so_b};          // pos | sh | rot | so, per gaussian
+    // (sized once for the largest chunk of either layout: it never grows)
+    if (!c->h_bounce) CU(c, cudaMallocHost(&c->h_bounce, 2 * DOWNLOAD_BOUNCE_BYTES));
+    const size_t chunk_b = DOWNLOAD_BOUNCE_BYTES;
+    StreamScratch staging(q);   // sh | rot | so of one chunk
+    CU(c, staging.alloc((size_t)m_max * (sh_b + 16 + so_b)));
+    uint8_t* st = static_cast<uint8_t*>(staging.p);
+    uint8_t* st_rot = st + (size_t)m_max * sh_b;
+    uint8_t* st_so = st_rot + (size_t)m_max * 16;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 2; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
+    for (cudaEvent_t& e : ev) CU(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    uint8_t* dst[4] = {reinterpret_cast<uint8_t*>(pos_vis), static_cast<uint8_t*>(sh), static_cast<uint8_t*>(rot), static_cast<uint8_t*>(so)};
+    const uint32_t chunks = (n + m_max - 1) / m_max;
+    // enqueue chunk i into bounce buffer i & 1
+    auto enqueue = [&](uint32_t i) -> bgs_status {
+        const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
+        uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
+        launch_unpack(f16, cl->blocks, lo, m, st, st_rot, st_so, q);
+        CU(c, cudaGetLastError());
+        const uint8_t* src[4] = {reinterpret_cast<const uint8_t*>(cl->pos) + (size_t)lo * 16, st, st_rot, st_so};
+        for (int p = 0; p < 4; ++p) {
+            if (plane_b[p]) CU(c, cudaMemcpyAsync(hb, src[p], (size_t)m * plane_b[p], cudaMemcpyDeviceToHost, q));
+            hb += (size_t)m * plane_b[p];
+        }
+        CU(c, cudaEventRecord(ev[i & 1], q));
+        return BGS_OK;
+    };
+    TRY(enqueue(0));
+    for (uint32_t i = 0; i < chunks; ++i) {
+        if (i + 1 < chunks) TRY(enqueue(i + 1));
+        CU(c, cudaEventSynchronize(ev[i & 1]));
+        const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
+        const uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
+        for (int p = 0; p < 4; ++p) {
+            if (plane_b[p]) memcpy(dst[p] + (size_t)lo * plane_b[p], hb, (size_t)m * plane_b[p]);
+            hb += (size_t)m * plane_b[p];
+        }
+    }
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_download_f32(bgs_context* c, const bgs_cloud* cl, float* pos_vis, float* sh, float* rot_wxyz, float* scale_opacity) {
+    return download_common(c, cl, false, pos_vis, sh, rot_wxyz, scale_opacity);
+}
+
+bgs_status bgs_cloud_download_f16(bgs_context* c, const bgs_cloud* cl, float* pos_vis, uint32_t* sh_packed, uint32_t* second_plane) {
+    return download_common(c, cl, true, pos_vis, sh_packed, second_plane, nullptr);
 }
 
 bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {

@@ -57,15 +57,23 @@ class PlanarGaussian3d:
         """The entity `Aabb` as the render world sees it: `compute_aabb` (src/gaussian/interface.rs:22-66: positions
         +- 0.1) -> `Aabb {center, half_extents}` (src/gaussian/cloud.rs:45-62) -> `aabb.min()` / `aabb.max()`
         (center -+ half_extents, src/render/mod.rs:1070-1071), every step in f32 like glam."""
-        p = self.position_visibility[:, :3]
-        off = np.float32(0.1)
-        # (min over (p - 0.1) == min(p) - 0.1: f32 subtraction of a constant is monotone)
-        lo = (p.min(0) - off).astype(np.float32) if len(p) else np.full(3, np.inf, np.float32)
-        hi = (p.max(0) + off).astype(np.float32) if len(p) else np.full(3, -np.inf, np.float32)
-        two = np.float32(2.0)
-        center = ((lo + hi).astype(np.float32) / two).astype(np.float32)
-        half = ((hi - lo).astype(np.float32) / two).astype(np.float32)
-        return (center - half).astype(np.float32), (center + half).astype(np.float32)
+        return compute_aabb(self.position_visibility)
+
+    @staticmethod
+    def from_f16(pos_vis, sh_packed, rot_scale_opacity) -> "PlanarGaussian3d":
+        """The exact inverse of `pack_f16`: each half widened to f32 (pack_f16 of the result gives the same words back for
+        every non-NaN half; a NaN half stays NaN).  For a precomputed-covariance record the result holds the covariance in
+        the slots `precomputed_covariance()` uses."""
+        def halves(w, shift):
+            return ((np.asarray(w, np.uint32) >> np.uint32(shift)) & np.uint32(0xFFFF)).astype(np.uint16).view(np.float16).astype(np.float32)
+
+        shp = np.asarray(sh_packed, np.uint32).reshape(-1, HALF_SH_COEFF_COUNT)
+        w = np.asarray(rot_scale_opacity, np.uint32).reshape(-1, 4)
+        sh = np.empty((len(shp), SH_COEFF_COUNT), np.float32)
+        sh[:, 0::2], sh[:, 1::2] = halves(shp, 0), halves(shp, 16)     # even coefficient in the low half
+        rot = np.stack([halves(w[:, 0], 16), halves(w[:, 0], 0), halves(w[:, 1], 16), halves(w[:, 1], 0)], axis=1)
+        so = np.stack([halves(w[:, 2], 16), halves(w[:, 2], 0), halves(w[:, 3], 16), halves(w[:, 3], 0)], axis=1)
+        return PlanarGaussian3d(np.asarray(pos_vis, np.float32).reshape(-1, 4), sh, rot, so)
 
     def pack_f16(self) -> tuple[np.ndarray, np.ndarray]:
         """-> (sh_packed (n,24) u32, rot_scale_opacity (n,4) u32); pack(upper, lower) = upper<<16 | lower."""
@@ -106,6 +114,19 @@ class PlanarGaussian3d:
 
         return PlanarGaussian3d(self.position_visibility, rt(self.spherical_harmonic), rt(self.rotation),
                                 rt(self.scale_opacity))
+
+
+def compute_aabb(position_visibility: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
+    """`PlanarGaussian3d.compute_aabb` of an (n, 4) position plane."""
+    p = np.asarray(position_visibility, np.float32)[:, :3]
+    off = np.float32(0.1)
+    # (min over (p - 0.1) == min(p) - 0.1: f32 subtraction of a constant is monotone)
+    lo = (p.min(0) - off).astype(np.float32) if len(p) else np.full(3, np.inf, np.float32)
+    hi = (p.max(0) + off).astype(np.float32) if len(p) else np.full(3, -np.inf, np.float32)
+    two = np.float32(2.0)
+    center = ((lo + hi).astype(np.float32) / two).astype(np.float32)
+    half = ((hi - lo).astype(np.float32) / two).astype(np.float32)
+    return (center - half).astype(np.float32), (center + half).astype(np.float32)
 
 
 def random_gaussians_3d_seeded(n: int, seed: int = 0, chunk: int = 1 << 18) -> PlanarGaussian3d:

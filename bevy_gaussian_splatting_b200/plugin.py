@@ -13,12 +13,13 @@ from __future__ import annotations
 
 import ctypes as C
 import dataclasses
+import os
 
 import numpy as np
 
 from . import abi
 from .camera import GaussianCamera, View
-from .gaussian import PlanarGaussian3d
+from .gaussian import PlanarGaussian3d, compute_aabb
 from .particles import PARTICLE_BEHAVIOR_DTYPE, as_particle_behaviors
 from .settings import CloudSettings, SparseSelect
 
@@ -64,6 +65,20 @@ class PlanarGaussian3dHandle:
                                                 _ptr(cloud.spherical_harmonic), _ptr(cloud.rotation),
                                                 _ptr(cloud.scale_opacity), C.byref(self._h))
         plugin._check(st)
+
+    @classmethod
+    def _adopt(cls, plugin: "GaussianSplattingPlugin", h: C.c_void_p, n: int, f16: bool,
+               precompute_covariance: bool) -> "PlanarGaussian3dHandle":
+        """A handle owning a `bgs_cloud*` the library made (bgs_cloud_subset); its Aabb is computed from the positions,
+        as `calculate_bounds` would compute it for the cloud once saved and loaded."""
+        self = cls.__new__(cls)
+        PlanarGaussian3dHandle._next_serial += 1
+        self.serial = PlanarGaussian3dHandle._next_serial
+        self._plugin, self._lib = plugin, plugin._lib
+        self.n, self.f16, self.precompute_covariance = n, f16, precompute_covariance
+        self._h = h
+        self.aabb = compute_aabb(plugin.positions(self))
+        return self
 
     def destroy(self):
         if self._h:
@@ -279,6 +294,65 @@ class GaussianSplattingPlugin:
     def selection(self, handle: PlanarGaussian3dHandle) -> np.ndarray:
         """Indices of the selected gaussians: visibility >= 0.5, the ones DrawMode::Selected draws."""
         return np.flatnonzero(self.visibility(handle) >= 0.5).astype(np.uint32)
+
+    # -- keeping a selection as its own cloud, reading clouds back (src/query/select.rs:156-176; the rule: include/bgs.h)
+    def subset(self, handle: PlanarGaussian3dHandle, indices=None) -> PlanarGaussian3dHandle | None:
+        """A new resident cloud of `handle`'s gaussians, in its layout.  indices None: the selected ones, visibility
+        !(w < 0.5) -- the set DrawMode::Selected draws, NaN included (unlike `selection()`) -- in index order; None when
+        nothing is selected.  Otherwise gaussian j of the result is gaussian indices[j] (order kept, repeats allowed)."""
+        out, n = C.c_void_p(), C.c_uint32()
+        if indices is None:
+            self._check(self._lib.bgs_cloud_subset(self._ctx, handle._h, None, 0, C.byref(out), C.byref(n)))
+        else:
+            idx = np.asarray(indices).reshape(-1)
+            if idx.dtype.kind not in "iu" or (idx.size and (idx.min() < 0 or idx.max() >= 1 << 32)):
+                raise IndexError("subset: indices must be non-negative integers")
+            idx = np.ascontiguousarray(idx, np.uint32)
+            self._check(self._lib.bgs_cloud_subset(self._ctx, handle._h, _ptr(idx), idx.size, C.byref(out), C.byref(n)))
+        if not out:
+            return None
+        return PlanarGaussian3dHandle._adopt(self, out, int(n.value), handle.f16, handle.precompute_covariance)
+
+    def download_planes(self, handle: PlanarGaussian3dHandle) -> tuple[np.ndarray, ...]:
+        """The cloud's planes as the matching upload call takes them: f32 (pos_vis, sh, rotation, scale_opacity); f16
+        and precomputed-covariance clouds (pos_vis, sh_packed, second plane words)."""
+        pos = np.empty((handle.n, 4), np.float32)
+        if handle.f16 or handle.precompute_covariance:
+            sh, second = np.empty((handle.n, 24), np.uint32), np.empty((handle.n, 4), np.uint32)
+            self._check(self._lib.bgs_cloud_download_f16(self._ctx, handle._h, _ptr(pos), _ptr(sh), _ptr(second)))
+            return pos, sh, second
+        sh, rot, so = np.empty((handle.n, 48), np.float32), np.empty((handle.n, 4), np.float32), np.empty((handle.n, 4), np.float32)
+        self._check(self._lib.bgs_cloud_download_f32(self._ctx, handle._h, _ptr(pos), _ptr(sh), _ptr(rot), _ptr(so)))
+        return pos, sh, rot, so
+
+    def download(self, handle: PlanarGaussian3dHandle) -> PlanarGaussian3d:
+        """The cloud as a host PlanarGaussian3d: f16 planes widened to f32 (`PlanarGaussian3d.from_f16`); a
+        precomputed-covariance cloud holds its covariance in the slots `precomputed_covariance()` uses."""
+        planes = self.download_planes(handle)
+        return PlanarGaussian3d.from_f16(*planes) if len(planes) == 3 else PlanarGaussian3d(*planes)
+
+    def save_selection(self, handle: PlanarGaussian3dHandle, path) -> int:
+        """The reference's save_selection (src/query/select.rs:156-176): the selected gaussians (`subset(handle)`)
+        written to `path` as .gcloud or .ply by its extension.  Returns how many were written.  A precomputed-covariance
+        cloud raises ValueError (its rotation and scale are gone, and the file holds those).  Nothing selected raises
+        ValueError and writes nothing, where the reference would write an empty cloud."""
+        from .gcloud import write_gcloud
+        from .io import write_ply_3d
+
+        ext = os.path.splitext(str(path))[1].lower()
+        writers = {".gcloud": write_gcloud, ".ply": write_ply_3d}
+        if ext not in writers:
+            raise ValueError("save_selection: only .ply and .gcloud supported")
+        if handle.precompute_covariance:
+            raise ValueError("save_selection: a precomputed-covariance cloud has no rotation and scale to save")
+        sub = self.subset(handle)
+        if sub is None:
+            raise ValueError("save_selection: nothing is selected")
+        try:
+            writers[ext](path, self.download(sub))
+            return sub.n
+        finally:
+            sub.destroy()
 
     # -- particle behaviours (src/morph/particle.rs): an enqueued per-frame edit of the positions (the rule: include/bgs.h)
     def add_particles(self, behaviors) -> ParticleBehaviorsHandle:

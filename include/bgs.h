@@ -200,6 +200,44 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* ctx, bgs_cloud* cloud, const fl
                                     const float* mesh_from_cloud /* 16, column-major, may be NULL */, uint32_t mode,
                                     uint32_t* out_inside /* may be NULL */);
 
+/* Keeping a selection as its own cloud, and reading a cloud back (the reference's save_selection,
+ * src/query/select.rs:156-176: cloud.subset(indices), then write_to_file).
+ *
+ * bgs_cloud_subset: a new resident cloud holding some of `cloud`'s gaussians, on the same device and in the same layout
+ * (f32 / f16 / f16 precomputed covariance).  The rule, exactly:
+ *   - selection mode (indices == NULL; k must be 0): gaussian i is kept iff !(w_i < 0.5f), w_i its visibility lane as
+ *     it is now (after every selection edit, and every particle step enqueued on any context, before the call).  That is
+ *     the set DrawMode::Selected draws: 0.5 is kept, nextafterf(0.5f, 0) is not; NaN and +inf are kept; -0, +0, -inf and
+ *     subnormals are dropped.  (The hosts' selection() helpers use w >= 0.5, which drops NaN; they are unchanged.)  The
+ *     kept gaussians stay in ascending index order.  Nothing kept: BGS_OK with *out = NULL and *out_n = 0 (a cloud
+ *     still holds at least one gaussian, as at upload).
+ *   - index mode (indices != NULL): the reference's subset(indices) literally: gaussian j of the result is gaussian
+ *     indices[j] of the source; order is kept, repeats are allowed.  k must be in [1, 2^30); an index >= the cloud's n
+ *     -> BGS_EINVAL, checked on the host before anything is allocated.
+ *   - every byte of both device copies is copied unchanged (the position plane and the gaussian-major block), and the
+ *     covariance flag is carried over.  The new cloud is registered with ctx like an uploaded one and released with
+ *     bgs_cloud_destroy; it outlives its source and ctx.  It has never been stepped: its frames add no wait.
+ *   Selection mode reads one number back (the kept count, which sizes the new planes).  Device memory beyond the new
+ *   cloud: one mask word per 32 gaussians and one count per 256 (selection mode), or the k indices (index mode).
+ * bgs_cloud_download_f32 / _f16: the planes exactly as the matching upload call takes them.  pos_vis comes from the
+ *   position plane, the other planes from the blocks; a cloud that was never edited gives back the upload's arrays bit
+ *   for bit.  For f16 clouds second_plane is the packed rotation-scale-opacity words, or the Covariance3dOpacityPacked128
+ *   words of a precomputed-covariance cloud.  The planes go in chunks of 2^17 gaussians through device staging
+ *   and two pinned host buffers the context keeps (2 x 30 MB, from its first download on).  The call of the other
+ *   layout -> BGS_EINVAL.
+ * Ordering: both calls only read the source and are synchronous.  They wait on the device for the particle steps
+ * queued on the cloud (as bgs_cloud_visibility_get does) and do not drain other contexts' queued frames.  Their
+ * scratch is their own: the bgs_debug_* hooks, bgs_frame_stats_get and bgs_stage_times_us keep reporting the last
+ * frame, and the next frame's plan does not change.
+ * A null ctx, cloud, out or plane pointer, a cloud on another device, or indices == NULL with k != 0 -> BGS_EINVAL;
+ * an allocation failure -> BGS_ENOMEM.  A refused call creates and changes nothing (*out stays NULL). */
+bgs_status bgs_cloud_subset(bgs_context* ctx, const bgs_cloud* cloud, const uint32_t* indices /* k, may be NULL */, uint32_t k,
+                            bgs_cloud** out, uint32_t* out_n /* may be NULL */);
+bgs_status bgs_cloud_download_f32(bgs_context* ctx, const bgs_cloud* cloud, float* pos_vis /* n*4 */, float* sh /* n*48 */,
+                                  float* rot_wxyz /* n*4 */, float* scale_opacity /* n*4 */);
+bgs_status bgs_cloud_download_f16(bgs_context* ctx, const bgs_cloud* cloud, float* pos_vis /* n*4 */,
+                                  uint32_t* sh_packed /* n*24 */, uint32_t* second_plane /* n*4 */);
+
 /* Particle behaviours (src/morph/particle.rs, particle.wgsl; the reference's `morph_particles` feature): a
  * ParticleBehaviors asset moves the gaussians it names every frame, in place, without a re-upload.
  *

@@ -322,6 +322,32 @@ public:
             if (v[i] >= 0.5f) idx.push_back(i);
         return idx;
     }
+    // Keeping a selection as its own cloud (src/query/select.rs:156-176; the rule: bgs.h).  indices nullptr: the gaussians
+    // DrawMode::Selected draws (visibility !(w < 0.5), NaN included), in index order -- an empty handle (get() == nullptr,
+    // len() == 0) when none is; else gaussian j of the result is gaussian (*indices)[j].  The Aabb is the new cloud's own.
+    PlanarGaussian3dHandle subset(const PlanarGaussian3dHandle& cloud, const std::vector<uint32_t>* indices = nullptr) {
+        PlanarGaussian3dHandle h;
+        if (indices) check(bgs_cloud_subset(ctx_, cloud.get(), indices->data(), (uint32_t)indices->size(), &h.h_, &h.n_));
+        else check(bgs_cloud_subset(ctx_, cloud.get(), nullptr, 0, &h.h_, &h.n_));
+        if (h.h_) {
+            PlanarGaussian3d p;
+            p.position_visibility = positions(h);
+            p.compute_aabb(h.aabb_min_, h.aabb_max_);
+        }
+        return h;
+    }
+    // The cloud's four planes (bgs_cloud_download_f32: this host uploads f32 clouds only).
+    PlanarGaussian3d download(const PlanarGaussian3dHandle& cloud) {
+        const size_t n = cloud.len();
+        PlanarGaussian3d c;
+        c.position_visibility.resize(n * 4); c.spherical_harmonic.resize(n * 48); c.rotation.resize(n * 4); c.scale_opacity.resize(n * 4);
+        check(bgs_cloud_download_f32(ctx_, cloud.get(), c.position_visibility.data(), c.spherical_harmonic.data(), c.rotation.data(),
+                                     c.scale_opacity.data()));
+        return c;
+    }
+    // The reference's save_selection: the selected gaussians written to `path` as .gcloud (bgs::io::encode_gcloud, defined
+    // in bgs_io.hpp).  Returns how many were written; nothing selected throws Error(BGS_EINVAL) and writes nothing.
+    uint32_t save_selection(const PlanarGaussian3dHandle& cloud, const std::string& path);
     // Particle behaviours (src/morph/particle.rs; the rule and its ordering: bgs.h).  step_particles only enqueues the
     // step: frames rendered before it (on any context) see the old positions, everything after it the new ones.
     ParticleBehaviorsHandle add_particles(const ParticleBehaviors& behaviors) {
@@ -358,3 +384,5 @@ private:
 };
 
 }  // namespace bgs
+
+#include "bgs_io.hpp"   // GaussianSplattingPlugin::save_selection

@@ -433,4 +433,15 @@ inline PlanarGaussian3d load_cloud(const std::string& path) {
 }
 
 }  // namespace io
+
+// src/query/select.rs:156-176: cloud.subset(selected), then write_to_file (declared in bgs.hpp)
+inline uint32_t GaussianSplattingPlugin::save_selection(const PlanarGaussian3dHandle& cloud, const std::string& path) {
+    const PlanarGaussian3dHandle sub = subset(cloud);
+    if (!sub.get()) throw Error(BGS_EINVAL, "save_selection: nothing is selected");
+    const std::vector<unsigned char> bytes = io::encode_gcloud(download(sub));
+    std::ofstream f(path, std::ios::binary);
+    if (!f.write(reinterpret_cast<const char*>(bytes.data()), (std::streamsize)bytes.size()))
+        throw std::runtime_error("save_selection: cannot write " + path);
+    return sub.len();
+}
 }  // namespace bgs
