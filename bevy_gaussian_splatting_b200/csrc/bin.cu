@@ -6,6 +6,7 @@
 // exclusive scan of the per-splat tile counts in rank order, so the stable tile-id radix sort that
 // follows yields, per tile, a slice of the GLOBAL depth order.
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 

@@ -1,0 +1,482 @@
+// cloud.cu -- the extern "C" calls of libbgs (include/bgs.h) on a resident cloud: upload and destroy, selection edits,
+// particle behaviours, positions and visibility read-back, subset and download.  None of them is part of a frame; the
+// order in which they and the frames reach a cloud is host.cuh's.
+#include <cmath>
+#include <cstring>
+#include <algorithm>
+#include <new>
+#include <vector>
+
+#include "host.cuh"
+
+namespace {
+
+size_t block_bytes(const bgs_cloud* cl) { return cl->f16 ? 128 : 256; }
+
+// Releases a cloud that a call failed to finish, and reports why.
+bgs_status drop_cloud(bgs_context* c, const char* call, bgs_cloud* cl, cudaError_t e) {
+    bgs_cloud_destroy(cl);
+    return fail(c, status_of(e), "%s: %s", call, cudaGetErrorString(e));
+}
+
+// A new cloud of n gaussians in the given layout on the context's device, its planes allocated but not yet written.
+bgs_status new_cloud(bgs_context* c, const char* call, uint32_t n, bool f16, bool cov, bgs_cloud** out) {
+    bgs_cloud* cl = new (std::nothrow) bgs_cloud();
+    if (!cl) return fail(c, BGS_ENOMEM, "%s: out of host memory", call);
+    cl->device = c->device; cl->n = n; cl->f16 = f16; cl->cov = cov;
+    cudaError_t e = cudaMalloc(&cl->pos, (size_t)n * 16);
+    if (e == cudaSuccess) e = cudaMalloc(&cl->blocks, (size_t)n * block_bytes(cl));
+    if (e != cudaSuccess) return drop_cloud(c, call, cl, e);
+    *out = cl;
+    return BGS_OK;
+}
+
+// One device word read back: copied to the context's own pinned word on the render stream, which is then drained.
+bgs_status read_word(bgs_context* c, const uint32_t* word, uint32_t* out) {
+    CU(c, cudaMemcpyAsync(c->h_word, word, 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    *out = *c->h_word;
+    return BGS_OK;
+}
+
+// Device scratch of one call, released on the stream when it goes out of scope.
+struct StreamScratch {
+    void* p = nullptr;
+    cudaStream_t q;
+    explicit StreamScratch(cudaStream_t s) : q(s) {}
+    StreamScratch(const StreamScratch&) = delete;
+    StreamScratch& operator=(const StreamScratch&) = delete;
+    ~StreamScratch() { if (p) cudaFreeAsync(p, q); }
+    cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes, q); }
+};
+
+// gaussians per chunk of a download: the device staging arrays hold one chunk (f32: 28 MB), each of the context's two
+// pinned bounce buffers one chunk's four planes (f32: 30 MB)
+constexpr uint32_t DOWNLOAD_CHUNK = 1u << 17;
+constexpr size_t DOWNLOAD_BOUNCE_BYTES = (size_t)DOWNLOAD_CHUNK * (16 + 192 + 16 + 16);
+
+}  // namespace
+
+extern "C" {
+
+static bgs_status upload_common(bgs_context* ctx, uint32_t n, bool f16, bool cov, const float* pos_vis, const void* sh,
+                                const void* rot, const void* so, bgs_cloud** out) {
+    if (!ctx || !out) return BGS_EINVAL;
+    *out = nullptr;
+    if (!pos_vis || !sh || !rot || (!f16 && !so)) return fail(ctx, BGS_EINVAL, "cloud upload: null plane pointer");
+    if (n == 0 || n >= (1u << 30)) return fail(ctx, BGS_EINVAL, "cloud upload: n must be in [1, 2^30)");
+    CU(ctx, cudaSetDevice(ctx->device));
+    bgs_cloud* cl = nullptr;
+    TRY(new_cloud(ctx, "cloud upload", n, f16, cov, &cl));
+    // the other planes go to device scratch, are repacked into the gaussian-major blocks the projection gathers, and
+    // are freed again
+    void* d_sh = nullptr; void* d_rot = nullptr; void* d_so = nullptr;
+    const size_t sh_bytes = (size_t)n * (f16 ? 96 : 192);
+    cudaError_t e = cudaMalloc(&d_sh, sh_bytes);
+    if (e == cudaSuccess) e = cudaMalloc(&d_rot, (size_t)n * 16);
+    if (e == cudaSuccess && !f16) e = cudaMalloc(&d_so, (size_t)n * 16);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(cl->pos, pos_vis, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_sh, sh, sh_bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_rot, rot, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess && !f16) e = cudaMemcpyAsync(d_so, so, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) {
+        launch_repack(f16, cl->pos, d_sh, d_rot, d_so, n, cl->blocks, ctx->stream);
+        e = cudaStreamSynchronize(ctx->stream);
+    }
+    cudaFree(d_sh); cudaFree(d_rot); cudaFree(d_so);
+    if (e != cudaSuccess) return drop_cloud(ctx, "cloud upload", cl, e);
+    *out = cl;
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_upload_f32(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh,
+                                const float* rot_wxyz, const float* scale_opacity, bgs_cloud** out) {
+    return upload_common(ctx, n, false, false, pos_vis, sh, rot_wxyz, scale_opacity, out);
+}
+
+bgs_status bgs_cloud_upload_f16(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
+                                const uint32_t* rot_scale_opacity, bgs_cloud** out) {
+    return upload_common(ctx, n, true, false, pos_vis, sh_packed, rot_scale_opacity, nullptr, out);
+}
+
+bgs_status bgs_cloud_upload_f16_cov(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
+                                    const uint32_t* cov3d_opacity, bgs_cloud** out) {
+    return upload_common(ctx, n, true, true, pos_vis, sh_packed, cov3d_opacity, nullptr, out);
+}
+
+void bgs_cloud_destroy(bgs_cloud* cl) {
+    if (!cl) return;
+    cudaSetDevice(cl->device);
+    {
+        // every live context (clouds are shared by the contexts of one GPU) drops its references: queued frames
+        // that still read the planes are drained first, the debug hooks lose their frame
+        std::lock_guard<std::mutex> lk(g_registry_mu);
+        for (bgs_context* c : g_contexts) {
+            if (c->pend.cloud == cl || c->last.cloud == cl) {
+                if (c->async_pending || c->pend.cloud == cl) c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
+                if (c->pend.cloud == cl) { c->pend.cloud = nullptr; c->pend.n = 0; }
+                if (c->last.cloud == cl) { c->last.cloud = nullptr; c->have_frame = false; }
+            }
+        }
+    }
+    if (cl->ev_write) {   // particle steps still queued on any context write the planes
+        cudaEventSynchronize(cl->ev_write);
+        cudaEventDestroy(cl->ev_write);
+    }
+    cudaFree(cl->pos); cudaFree(cl->blocks);
+    delete cl;
+}
+
+// ---- selection edits of a resident cloud (select.cu).  The visibility lane lives twice on the device: the position
+// plane's .w (what key-gen streams) and the first 16 B of each gaussian-major block (what the projection reads): every
+// write updates both.
+
+bgs_status bgs_cloud_select_sparse(bgs_context* c, bgs_cloud* cl, float radius, uint32_t threshold, uint32_t* out_selected) {
+    if (!cl) return fail(c, BGS_EINVAL, "select_sparse: null cloud");
+    if (!(radius >= 0.0f) || std::isinf(radius)) return fail(c, BGS_EINVAL, "select_sparse: radius must be finite and >= 0");
+    TRY(enter_call(c, "select_sparse", cl->device));
+    TRY(before_cloud_write(c, cl));
+    const uint32_t n = cl->n;
+    const float r2 = radius * radius;
+    float* pos_w = reinterpret_cast<float*>(cl->pos) + 3;
+    float* block_w = reinterpret_cast<float*>(cl->blocks) + 3;
+    const uint32_t stride = (uint32_t)(block_bytes(cl) / 4);
+    cudaStream_t q = c->stream;
+    uint32_t selected = 0;
+    if (threshold == 0u || r2 == 0.0f) {
+        // no count can reach a threshold of 0; no distance is below a radius whose square is 0 (every count is 0)
+        selected = threshold == 0u ? 0u : n;
+        launch_select_fill(n, threshold == 0u ? 0.0f : 1.0f, pos_w, block_w, stride, q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaStreamSynchronize(q));
+    } else {
+        // the frame's scratch: key / value ping-pong buffers and depth-sort status rows (the sort), the record buffer
+        // (positions in bucket order).  The debug hooks lose the last frame; the hints the next frame plans from stay.
+        TRY(ensure_cloud_scratch(c, n));
+        TRY(ensure_status(c, c->status_depth, c->status_n, n));
+        const uint32_t nb = select_num_buckets(n);
+        const int passes = select_sort_passes(nb);
+        Layout l;
+        const size_t o_words = l.add(3 * 4), o_hist = l.add(4 * 256 * 4);
+        const size_t o_rng = l.add(((size_t)nb + 1) * sizeof(uint2));   // nb + 1: the sentinel key's too
+        TRY(c->select_scratch.grow(c, l.end, false));
+        c->have_frame = false;
+        uint32_t* words = reinterpret_cast<uint32_t*>(c->select_scratch.p + o_words);   // [0] sort count, [1] barrier, [2] selected
+        uint32_t* hist = reinterpret_cast<uint32_t*>(c->select_scratch.p + o_hist);
+        uint2* ranges = reinterpret_cast<uint2*>(c->select_scratch.p + o_rng);
+        CU(c, cudaMemsetAsync(c->select_scratch.p, 0, l.end, q));
+        launch_select_keys(cl->pos, n, radius, nb, c->keys[0].p, c->vals[0].p, &words[0], q);
+        CU(c, cudaGetLastError());
+        CU(c, launch_radix_sort(c->keys[0].p, c->vals[0].p, c->keys[1].p, c->vals[1].p, &words[0], n, n, hist, 1,
+                                c->status_depth.p, (size_t)radix_num_tiles(c->status_n) * 256, next_epoch(c), &words[1], passes,
+                                0, ranges, c->sm_count, c->rs_per_sm, q));
+        launch_select_count(cl->pos, c->vals[passes & 1].p, ranges, n, radius, nb, r2, threshold,
+                            reinterpret_cast<float4*>(c->recs.p), pos_w, block_w, stride, &words[2], q);
+        CU(c, cudaGetLastError());
+        TRY(read_word(c, &words[2], &selected));
+    }
+    if (out_selected) *out_selected = selected;
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_visibility_get(bgs_context* c, const bgs_cloud* cl, float* out_vis) {
+    if (!cl || !out_vis) return fail(c, BGS_EINVAL, "visibility_get: null cloud or array");
+    TRY(enter_call(c, "visibility_get", cl->device));
+    TRY(before_cloud_read(c, cl));
+    CU(c, cudaMemcpy2DAsync(out_vis, 4, reinterpret_cast<const char*>(cl->pos) + 12, 16, 4, cl->n, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_visibility_set(bgs_context* c, bgs_cloud* cl, const float* vis) {
+    if (!cl || !vis) return fail(c, BGS_EINVAL, "visibility_set: null cloud or array");
+    TRY(enter_call(c, "visibility_set", cl->device));
+    TRY(before_cloud_write(c, cl));
+    CU(c, cudaMemcpy2DAsync(reinterpret_cast<char*>(cl->pos) + 12, 16, vis, 4, 4, cl->n, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpy2DAsync(reinterpret_cast<char*>(cl->blocks) + 12, block_bytes(cl), vis, 4, 4, cl->n, cudaMemcpyHostToDevice,
+                            c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_select_in_mesh(bgs_context* c, bgs_cloud* cl, const float* vertices, uint32_t nv, const uint32_t* indices,
+                                    uint32_t nt, const float* mesh_from_cloud, uint32_t mode, uint32_t* out_inside) {
+    if (!cl) return fail(c, BGS_EINVAL, "select_in_mesh: null cloud");
+    if (nt > 0 && (!vertices || !indices)) return fail(c, BGS_EINVAL, "select_in_mesh: null vertices or indices");
+    if (mode != BGS_SELECT_REPLACE && mode != BGS_SELECT_ADD) return fail(c, BGS_EINVAL, "select_in_mesh: unknown mode %u", mode);
+    TRY(enter_call(c, "select_in_mesh", cl->device));
+    for (size_t k = 0; k < (size_t)nt * 3; ++k)
+        if (indices[k] >= nv) return fail(c, BGS_EINVAL, "select_in_mesh: index %u of triangle %zu is >= %u vertices", indices[k], k / 3, nv);
+    if (nt >= (1u << 26)) return fail(c, BGS_ENOMEM, "select_in_mesh: more than 2^26 triangles");
+    static const float identity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    const float* M = mesh_from_cloud ? mesh_from_cloud : identity;
+    TRY(before_cloud_write(c, cl));
+    const uint32_t n = cl->n;
+    float* pos_w = reinterpret_cast<float*>(cl->pos) + 3;
+    float* block_w = reinterpret_cast<float*>(cl->blocks) + 3;
+    const uint32_t stride = (uint32_t)(block_bytes(cl) / 4);
+    cudaStream_t q = c->stream;
+
+    // triangle side: setup (records, classes, grid bounds)
+    Layout lt;
+    const size_t o_w = lt.add(256);   // (mesh_words_bytes() <= 256)
+    const size_t o_v = lt.add((size_t)nv * 12), o_i = lt.add((size_t)nt * 12);
+    const size_t o_br = lt.add((size_t)nt * (2 * mesh_rec_bytes() + 32));   // binned records | binned boxes | global records
+    const size_t o_bb = o_br + (size_t)nt * mesh_rec_bytes(), o_gr = o_bb + (size_t)nt * 32;
+    TRY(c->mesh_tri.grow(c, lt.end, false));
+    uint8_t* tb = c->mesh_tri.p;
+    void* words = tb + o_w;
+    std::vector<unsigned long long> wh_buf((mesh_words_bytes() + 7) / 8);
+    void* wh = wh_buf.data();
+    CU(c, cudaMemsetAsync(words, 0, 256, q));
+    if (nt > 0) {
+        CU(c, cudaMemcpyAsync(tb + o_v, vertices, (size_t)nv * 12, cudaMemcpyHostToDevice, q));
+        CU(c, cudaMemcpyAsync(tb + o_i, indices, (size_t)nt * 12, cudaMemcpyHostToDevice, q));
+        launch_mesh_setup(reinterpret_cast<const float*>(tb + o_v), reinterpret_cast<const uint32_t*>(tb + o_i), nt, tb + o_br,
+                          tb + o_bb, tb + o_gr, words, q);
+        CU(c, cudaGetLastError());
+    }
+    CU(c, cudaMemcpyAsync(wh, words, mesh_words_bytes(), cudaMemcpyDeviceToHost, q));
+    CU(c, cudaStreamSynchronize(q));
+
+    // grid side: the level, the pairs, their sort by cell
+    int level = -1;
+    const uint32_t* cell_tri = nullptr;
+    const uint2* ranges = nullptr;
+    if (mesh_words_n_bin(wh) > 0) {
+        launch_mesh_levels(tb + o_bb, wh, words, q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaMemcpyAsync(wh, words, mesh_words_bytes(), cudaMemcpyDeviceToHost, q));
+        CU(c, cudaStreamSynchronize(q));
+        uint64_t pairs64 = 0;
+        uint32_t cells = 0;
+        mesh_pick_level(wh, &level, &pairs64, &cells);
+        const uint32_t pairs = (uint32_t)pairs64;
+        Layout lp;
+        const size_t o_hist = lp.add(4 * 256 * 4), o_rng = lp.add((size_t)cells * 8);
+        const size_t o_k0 = lp.add((size_t)pairs * 4), o_v0 = lp.add((size_t)pairs * 4);
+        const size_t o_k1 = lp.add((size_t)pairs * 4), o_v1 = lp.add((size_t)pairs * 4);
+        TRY(c->mesh_pairs.grow(c, lp.padded(), false));
+        TRY(ensure_status(c, c->status_pairs, c->status_np, pairs));
+        uint8_t* pb = c->mesh_pairs.p;
+        uint32_t* k0 = reinterpret_cast<uint32_t*>(pb + o_k0);
+        uint32_t* v0 = reinterpret_cast<uint32_t*>(pb + o_v0);
+        uint32_t* k1 = reinterpret_cast<uint32_t*>(pb + o_k1);
+        uint32_t* v1 = reinterpret_cast<uint32_t*>(pb + o_v1);
+        uint2* rng = reinterpret_cast<uint2*>(pb + o_rng);
+        CU(c, cudaMemsetAsync(pb, 0, o_k0, q));   // histograms and ranges
+        launch_mesh_emit(tb + o_bb, wh, level, k0, v0, words, q);
+        CU(c, cudaGetLastError());
+        const int passes = pair_passes(cells);
+        CU(c, launch_radix_sort(k0, v0, k1, v1, mesh_words_pairs(words), pairs, pairs, reinterpret_cast<uint32_t*>(pb + o_hist), 1,
+                                c->status_pairs.p, (size_t)radix_num_tiles(c->status_np) * 256, next_epoch(c),
+                                mesh_words_barrier(words), passes, 0, rng, c->sm_count, c->rs_per_sm, q));
+        cell_tri = (passes & 1) ? v1 : v0;
+        ranges = rng;
+    }
+
+    // point side: the count and the lane
+    launch_mesh_count(cl->pos, n, M, tb + o_br, tb + o_gr, cell_tri, ranges, wh, level, mode, pos_w, block_w, stride, words, q);
+    CU(c, cudaGetLastError());
+    uint32_t inside = 0;
+    TRY(read_word(c, mesh_words_inside(words), &inside));
+    if (out_inside) *out_inside = inside;
+    return BGS_OK;
+}
+
+// ---- particle behaviours (particles.cu).  The step is a queued write (host.cuh: queue_cloud_write), never drained;
+// it also orders itself after the behaviours' earlier steps and marks itself on them.
+
+bgs_status bgs_particles_create(bgs_context* c, const bgs_particle_behavior* behaviors, uint32_t count, bgs_particles** out) {
+    if (!c || !out) return BGS_EINVAL;
+    *out = nullptr;
+    if (!behaviors) return fail(c, BGS_EINVAL, "particles_create: null behaviours");
+    if (count == 0 || count >= (1u << 30)) return fail(c, BGS_EINVAL, "particles_create: count must be in [1, 2^30)");
+    static_assert(sizeof(bgs_particle_behavior) == 64, "ParticleBehavior is 64 B");
+    std::vector<uint32_t> active;
+    active.reserve(count);
+    for (uint32_t i = 0; i < count; ++i)
+        if (behaviors[i].indices[0] < 0x80000000u) active.push_back(behaviors[i].indices[0]);
+    std::sort(active.begin(), active.end());
+    const auto dup = std::adjacent_find(active.begin(), active.end());
+    if (dup != active.end()) return fail(c, BGS_EINVAL, "particles_create: two active behaviours name gaussian %u", *dup);
+    CU(c, cudaSetDevice(c->device));
+    bgs_particles* p = new (std::nothrow) bgs_particles();
+    if (!p) return BGS_ENOMEM;
+    p->device = c->device;
+    p->count = count;
+    p->max_index = active.empty() ? -1 : (int64_t)active.back();
+    cudaError_t e = cudaMalloc(&p->d, (size_t)count * 64);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_write, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(p->d, behaviors, (size_t)count * 64, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) {
+        bgs_particles_destroy(p);
+        return fail(c, status_of(e), "particles_create: %s", cudaGetErrorString(e));
+    }
+    *out = p;
+    return BGS_OK;
+}
+
+bgs_status bgs_particles_get(bgs_context* c, const bgs_particles* p, bgs_particle_behavior* out) {
+    if (!p || !out) return fail(c, BGS_EINVAL, "particles_get: null behaviours or array");
+    TRY(enter_call(c, "particles_get", p->device, "behaviours live"));
+    CU(c, cudaStreamWaitEvent(c->stream, p->ev_write, 0));   // every step of these behaviours, on any context
+    CU(c, cudaMemcpyAsync(out, p->d, (size_t)p->count * 64, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
+}
+
+void bgs_particles_destroy(bgs_particles* p) {
+    if (!p) return;
+    cudaSetDevice(p->device);
+    if (p->ev_write) {   // steps still queued on any context read and write the records
+        cudaEventSynchronize(p->ev_write);
+        cudaEventDestroy(p->ev_write);
+    }
+    cudaFree(p->d);
+    delete p;
+}
+
+bgs_status bgs_cloud_particles_step(bgs_context* c, bgs_cloud* cl, bgs_particles* p, float delta_time) {
+    if (!cl || !p) return fail(c, BGS_EINVAL, "particles_step: null cloud or behaviours");
+    if (!std::isfinite(delta_time)) return fail(c, BGS_EINVAL, "particles_step: delta_time must be finite");
+    // (-1: the two are on different devices, so neither can be the context's)
+    TRY(enter_call(c, "particles_step", cl->device == p->device ? cl->device : -1, "cloud or behaviours live"));
+    if (p->max_index >= (int64_t)cl->n)
+        return fail(c, BGS_EINVAL, "particles_step: behaviour names gaussian %lld of a cloud of %u", (long long)p->max_index, cl->n);
+    TRY(queue_cloud_write(c, cl, [&](cudaStream_t q) {
+        CU(c, cudaStreamWaitEvent(q, p->ev_write, 0));
+        launch_particle_step(p->d, p->count, delta_time, cl->pos, cl->blocks, (uint32_t)(block_bytes(cl) / 16), q);
+        CU(c, cudaGetLastError());
+        CU(c, cudaEventRecord(p->ev_write, q));
+        return BGS_OK;
+    }));
+    c->step_pending = true;
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_positions_get(bgs_context* c, const bgs_cloud* cl, float* out_pos_vis) {
+    if (!cl || !out_pos_vis) return fail(c, BGS_EINVAL, "positions_get: null cloud or array");
+    TRY(enter_call(c, "positions_get", cl->device));
+    TRY(before_cloud_read(c, cl));
+    CU(c, cudaMemcpyAsync(out_pos_vis, cl->pos, (size_t)cl->n * 16, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return BGS_OK;
+}
+
+// ---- subset and download (subset.cu).  Both only read the source cloud (before_cloud_read), so neither drains another
+// context's frames.  Their scratch is their own, allocated and released on the render stream within the call
+// (stream-ordered: no device-wide synchronisation), so the frame's buffers, the debug hooks and the next frame's plan
+// are untouched.
+
+bgs_status bgs_cloud_subset(bgs_context* c, const bgs_cloud* cl, const uint32_t* indices, uint32_t k, bgs_cloud** out,
+                            uint32_t* out_n) {
+    if (out) *out = nullptr;
+    if (!cl || !out) return fail(c, BGS_EINVAL, "subset: null cloud or out");
+    TRY(enter_call(c, "subset", cl->device));
+    if (!indices && k != 0) return fail(c, BGS_EINVAL, "subset: selection mode (indices == NULL) takes k == 0");
+    if (indices && (k == 0 || k >= (1u << 30))) return fail(c, BGS_EINVAL, "subset: k must be in [1, 2^30)");
+    for (uint32_t j = 0; indices && j < k; ++j)
+        if (indices[j] >= cl->n) return fail(c, BGS_EINVAL, "subset: index %u at %u is >= the cloud's %u gaussians", indices[j], j, cl->n);
+    TRY(before_cloud_read(c, cl));
+    cudaStream_t q = c->stream;
+    const uint32_t n = cl->n;
+    StreamScratch scratch(q);
+    // selection mode: mask words | CTA counts (-> offsets) | the total
+    Layout l;
+    const size_t o_mask = l.add((size_t)(n + 31) / 32 * 4), o_cnt = l.add((size_t)subset_num_ctas(n) * 4), o_tot = l.add(4);
+    uint32_t kept = k;
+    if (!indices) {
+        CU(c, scratch.alloc(l.end));
+        uint8_t* s = static_cast<uint8_t*>(scratch.p);
+        launch_subset_count(cl->pos, n, reinterpret_cast<uint32_t*>(s + o_mask), reinterpret_cast<uint32_t*>(s + o_cnt),
+                            reinterpret_cast<uint32_t*>(s + o_tot), q);
+        CU(c, cudaGetLastError());
+        TRY(read_word(c, reinterpret_cast<const uint32_t*>(s + o_tot), &kept));
+        if (kept == 0) {
+            if (out_n) *out_n = 0;
+            return BGS_OK;
+        }
+    } else {
+        CU(c, scratch.alloc((size_t)k * 4));
+        CU(c, cudaMemcpyAsync(scratch.p, indices, (size_t)k * 4, cudaMemcpyHostToDevice, q));
+    }
+    bgs_cloud* nc = nullptr;
+    TRY(new_cloud(c, "subset", kept, cl->f16, cl->cov, &nc));
+    if (!indices) {
+        const uint8_t* s = static_cast<const uint8_t*>(scratch.p);
+        launch_subset_scatter(cl->f16, cl->pos, cl->blocks, n, reinterpret_cast<const uint32_t*>(s + o_mask),
+                              reinterpret_cast<const uint32_t*>(s + o_cnt), nc->pos, nc->blocks, q);
+    } else {
+        launch_subset_gather(cl->f16, cl->pos, cl->blocks, static_cast<const uint32_t*>(scratch.p), k, nc->pos, nc->blocks, q);
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+    if (e != cudaSuccess) return drop_cloud(c, "subset", nc, e);
+    *out = nc;
+    if (out_n) *out_n = kept;
+    return BGS_OK;
+}
+
+// Per chunk: unpack into device staging, copy the chunk's position plane and the staged planes to a pinned bounce
+// buffer, and -- while the next chunk goes the same way into the other bounce buffer -- copy it into the caller's arrays.
+static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, bool f16, float* pos_vis, void* sh, void* rot, void* so) {
+    if (!cl || !pos_vis || !sh || !rot || (!f16 && !so)) return fail(c, BGS_EINVAL, "download: null cloud or plane pointer");
+    TRY(enter_call(c, "download", cl->device));
+    if (cl->f16 != f16) return fail(c, BGS_EINVAL, "download: the cloud is in the %s layout", cl->f16 ? "f16" : "f32");
+    TRY(before_cloud_read(c, cl));
+    cudaStream_t q = c->stream;
+    const uint32_t n = cl->n, m_max = std::min(n, DOWNLOAD_CHUNK);
+    const size_t sh_b = f16 ? 96 : 192, so_b = f16 ? 0 : 16;
+    const size_t plane_b[4] = {16, sh_b, 16, so_b};          // pos | sh | rot | so, per gaussian
+    // (sized once for the largest chunk of either layout: it never grows)
+    if (!c->h_bounce) CU(c, cudaMallocHost(&c->h_bounce, 2 * DOWNLOAD_BOUNCE_BYTES));
+    const size_t chunk_b = DOWNLOAD_BOUNCE_BYTES;
+    StreamScratch staging(q);   // sh | rot | so of one chunk
+    CU(c, staging.alloc((size_t)m_max * (sh_b + 16 + so_b)));
+    uint8_t* st = static_cast<uint8_t*>(staging.p);
+    uint8_t* st_rot = st + (size_t)m_max * sh_b;
+    uint8_t* st_so = st_rot + (size_t)m_max * 16;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 2; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
+    for (cudaEvent_t& e : ev) CU(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    uint8_t* dst[4] = {reinterpret_cast<uint8_t*>(pos_vis), static_cast<uint8_t*>(sh), static_cast<uint8_t*>(rot), static_cast<uint8_t*>(so)};
+    const uint32_t chunks = (n + m_max - 1) / m_max;
+    // enqueue chunk i into bounce buffer i & 1
+    auto enqueue = [&](uint32_t i) -> bgs_status {
+        const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
+        uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
+        launch_unpack(f16, cl->blocks, lo, m, st, st_rot, st_so, q);
+        CU(c, cudaGetLastError());
+        const uint8_t* src[4] = {reinterpret_cast<const uint8_t*>(cl->pos) + (size_t)lo * 16, st, st_rot, st_so};
+        for (int p = 0; p < 4; ++p) {
+            if (plane_b[p]) CU(c, cudaMemcpyAsync(hb, src[p], (size_t)m * plane_b[p], cudaMemcpyDeviceToHost, q));
+            hb += (size_t)m * plane_b[p];
+        }
+        CU(c, cudaEventRecord(ev[i & 1], q));
+        return BGS_OK;
+    };
+    TRY(enqueue(0));
+    for (uint32_t i = 0; i < chunks; ++i) {
+        if (i + 1 < chunks) TRY(enqueue(i + 1));
+        CU(c, cudaEventSynchronize(ev[i & 1]));
+        const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
+        const uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
+        for (int p = 0; p < 4; ++p) {
+            if (plane_b[p]) memcpy(dst[p] + (size_t)lo * plane_b[p], hb, (size_t)m * plane_b[p]);
+            hb += (size_t)m * plane_b[p];
+        }
+    }
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_download_f32(bgs_context* c, const bgs_cloud* cl, float* pos_vis, float* sh, float* rot_wxyz, float* scale_opacity) {
+    return download_common(c, cl, false, pos_vis, sh, rot_wxyz, scale_opacity);
+}
+
+bgs_status bgs_cloud_download_f16(bgs_context* c, const bgs_cloud* cl, float* pos_vis, uint32_t* sh_packed, uint32_t* second_plane) {
+    return download_common(c, cl, true, pos_vis, sh_packed, second_plane, nullptr);
+}
+
+}  // extern "C"

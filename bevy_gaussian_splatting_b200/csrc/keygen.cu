@@ -10,6 +10,7 @@
 // HBM-bound streaming kernel: 16 B read per gaussian (coalesced float4), 8 B written per
 // visible gaussian.  Compiled with -fmad=false (see project_math.cuh).
 #include "project_math.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 

@@ -1,0 +1,81 @@
+// launch.cuh -- the host entry points of libbgs's kernels: one declaration each, included by the .cu file that defines
+// it and by the host code that calls it (api.cu, cloud.cu), so a signature that drifts fails to compile.
+#pragma once
+#include "common.cuh"
+
+namespace bgs {
+// keygen.cu
+void launch_keygen_all(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* keys_out, uint32_t* ids_out,
+                       FrameCounters* ctr, cudaStream_t stream);
+int keygen_coop_blocks_per_sm();
+cudaError_t launch_keygen_coop(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* masks, uint32_t* keys_out,
+                               uint32_t* ids_out, uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr,
+                               uint32_t* hist, int hist_passes, uint32_t grid, cudaStream_t stream);
+void launch_culled_flags(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* flags, cudaStream_t stream);
+// radix.cu
+uint32_t radix_num_tiles(uint32_t capacity);
+int radix_coop_blocks_per_sm(int items);
+cudaError_t launch_radix_sort(uint32_t* keys0, uint32_t* vals0, uint32_t* keys1, uint32_t* vals1, const uint32_t* n_ptr,
+                              uint32_t capacity, uint32_t n_hint, uint32_t* hist, int compute_hist, void* status,
+                              size_t status_stride, uint32_t epoch, uint32_t* barrier, int passes, int shift0, uint2* ranges,
+                              int sm_count, int coop_per_sm, cudaStream_t stream);
+// project.cu
+void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
+                        FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream);
+void launch_repack(bool f16, const void* pos, const void* sh, const void* rot, const void* so, uint32_t n, void* blocks,
+                   cudaStream_t stream);
+void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+                    const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
+                    const float* cutoff_tab, float4* aux, cudaStream_t stream);
+void launch_cutoff_table(float* tab, cudaStream_t stream);
+// bin.cu
+int bin_coop_blocks_per_sm();
+cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
+                                 uint32_t frac_a, uint32_t frac_b, uint32_t num_tiles_total, uint32_t* block_cnt,
+                                 int tiles_x, uint32_t capacity, uint32_t* pair_keys, uint32_t* pair_vals,
+                                 uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, uint32_t grid,
+                                 uint32_t* sticky_need, cudaStream_t stream);
+// raster.cu
+void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
+                   const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
+                   const float4* aux, void* out_depth, void* out_normal, cudaStream_t stream);
+void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
+                         int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
+                         uint32_t* tiles_done, int first, int last, cudaStream_t stream);
+// select.cu
+uint32_t select_num_buckets(uint32_t n);
+int select_sort_passes(uint32_t n_buckets);
+void launch_select_keys(const float4* pos, uint32_t n, float radius, uint32_t n_buckets, uint32_t* keys, uint32_t* vals,
+                        uint32_t* n_sort, cudaStream_t stream);
+void launch_select_count(const float4* pos, const uint32_t* ids, const uint2* ranges, uint32_t n, float radius, uint32_t n_buckets,
+                         float r2, uint32_t threshold, float4* spos, float* pos_w, float* block_w, uint32_t block_stride,
+                         uint32_t* selected, cudaStream_t stream);
+void launch_select_fill(uint32_t n, float v, float* pos_w, float* block_w, uint32_t block_stride, cudaStream_t stream);
+// mesh_select.cu
+size_t mesh_words_bytes();
+size_t mesh_rec_bytes();
+void launch_mesh_setup(const float* verts, const uint32_t* idx, uint32_t nt, void* bin_rec, void* bin_box, void* glob_rec, void* words,
+                       cudaStream_t stream);
+void launch_mesh_levels(const void* bin_box, const void* words_host, void* words, cudaStream_t stream);
+void mesh_pick_level(const void* words_host, int* level, uint64_t* pairs, uint32_t* cells);
+void launch_mesh_emit(const void* bin_box, const void* words_host, int level, uint32_t* keys, uint32_t* vals, void* words,
+                      cudaStream_t stream);
+uint32_t* mesh_words_pairs(void* words);
+uint32_t* mesh_words_barrier(void* words);
+uint32_t* mesh_words_inside(void* words);
+uint32_t mesh_words_n_bin(const void* words_host);
+void launch_mesh_count(const float4* pos, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
+                       const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, float* pos_w,
+                       float* block_w, uint32_t block_stride, void* words, cudaStream_t stream);
+// particles.cu
+void launch_particle_step(void* behaviors, uint32_t count, float dt, float4* pos, void* blocks, uint32_t block_stride,
+                          cudaStream_t stream);
+// subset.cu
+uint32_t subset_num_ctas(uint32_t n);
+void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t* cta_cnt, uint32_t* total, cudaStream_t stream);
+void launch_subset_scatter(bool f16, const void* pos, const void* blocks, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
+                           void* out_pos, void* out_blocks, cudaStream_t stream);
+void launch_subset_gather(bool f16, const void* pos, const void* blocks, const uint32_t* idx, uint32_t k, void* out_pos,
+                          void* out_blocks, cudaStream_t stream);
+void launch_unpack(bool f16, const void* blocks, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream);
+}  // namespace bgs

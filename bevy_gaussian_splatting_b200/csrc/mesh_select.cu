@@ -23,6 +23,7 @@
 // Cost: O(T) setup and pair emission, one radix sort of the pairs, and a count of O(N x (triangles per cell +
 // global triangles)).  A closed mesh covers its yz silhouette about twice, so a cell holds a few triangles.
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 
@@ -320,7 +321,7 @@ static MeshLevels mesh_plan_levels(const unsigned long long bound[4], uint32_t n
 }
 
 // The pair budget: 2^24 + 4 per binned triangle (the 1 x 1 level, n_bin pairs, always fits).
-uint64_t mesh_pair_budget(uint32_t n_bin) { return (1ull << 24) + 4ull * n_bin; }
+static uint64_t mesh_pair_budget(uint32_t n_bin) { return (1ull << 24) + 4ull * n_bin; }
 
 // Level counts for the ladder of a setup whose words are back on the host (`words_host`).
 void launch_mesh_levels(const void* bin_box, const void* words_host, void* words, cudaStream_t stream) {

@@ -11,6 +11,7 @@
 // FMA (explicit __fmul_rn / __fadd_rn; the file is also built with -fmad=false).  1.0 / 6.0 is WGSL's abstract
 // constant, rounded to f32 once.  particle_oracle/particle_oracle.cpp restates it (test infrastructure).
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 

@@ -17,6 +17,7 @@
 #include <cuda_fp16.h>
 
 #include "project_math.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 

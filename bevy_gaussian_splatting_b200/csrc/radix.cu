@@ -19,6 +19,7 @@
 //
 // HBM/L2-bound: per pass 8 B read + 8 B written per entry; histogram phase reads 4 B per entry.
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 

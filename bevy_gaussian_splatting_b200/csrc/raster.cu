@@ -15,6 +15,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 

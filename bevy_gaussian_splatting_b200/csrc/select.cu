@@ -18,6 +18,7 @@
 // Worst case: a radius that puts most of the cloud into one cell (or one clamped cell, see cell_coord) with a large
 // threshold is O(N x threshold).
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 

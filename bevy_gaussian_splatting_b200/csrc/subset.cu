@@ -15,6 +15,7 @@
 // Index mode: subset_gather_kernel copies gaussian indices[j] to j, CH threads per gaussian.
 // Download: unpack_kernel is repack_kernel's inverse over one chunk of gaussians, into planar staging arrays.
 #include "common.cuh"
+#include "launch.cuh"
 
 namespace bgs {
 
