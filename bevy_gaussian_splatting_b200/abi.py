@@ -105,6 +105,7 @@ SYMBOLS = [
     ("bgs_particles_destroy", None, [_P]),
     ("bgs_cloud_particles_step", C.c_int, [_P, _P, _P, C.c_float]),
     ("bgs_cloud_positions_get", C.c_int, [_P, _P, _P]),
+    ("bgs_cloud_interpolate", C.c_int, [_P, _P, _P, _P, C.c_float, C.c_float, C.c_float]),
     ("bgs_render", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P,
                              C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,

@@ -341,16 +341,18 @@ static bgs_status finish_frame(bgs_context* c) {
 
 bgs_status bgs_sync(bgs_context* c) {
     if (!c) return BGS_EINVAL;
-    if (!c->async_pending && !c->step_pending) return BGS_OK;
+    if (!c->async_pending && !c->step_pending && !c->reads_pending.load(std::memory_order_relaxed)) return BGS_OK;
     CU(c, cudaSetDevice(c->device));
     c->step_pending = false;
-    if (!c->async_pending) {   // only particle steps were queued: no frame to account for
+    if (!c->async_pending) {   // only particle steps or interpolations were queued: no frame to account for
         CU(c, cudaStreamSynchronize(c->stream));
+        c->reads_pending.store(false, std::memory_order_relaxed);
         CU(c, cudaGetLastError());
         return BGS_OK;
     }
     CU(c, cudaStreamSynchronize(c->stream));
     CU(c, cudaStreamSynchronize(c->stream_copy));
+    c->reads_pending.store(false, std::memory_order_relaxed);
     c->copy_pending[0] = c->copy_pending[1] = false;
     CU(c, cudaGetLastError());
     c->async_pending = false;

@@ -1,6 +1,6 @@
 // cloud.cu -- the extern "C" calls of libbgs (include/bgs.h) on a resident cloud: upload and destroy, selection edits,
-// particle behaviours, positions and visibility read-back, subset and download.  None of them is part of a frame; the
-// order in which they and the frames reach a cloud is host.cuh's.
+// particle behaviours, positions and visibility read-back, interpolation, subset and download.  None of them is part of
+// a frame; the order in which they and the frames reach a cloud is host.cuh's.
 #include <cmath>
 #include <cstring>
 #include <algorithm>
@@ -109,9 +109,12 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
     cudaSetDevice(cl->device);
     {
         // every live context (clouds are shared by the contexts of one GPU) drops its references: queued frames
-        // that still read the planes are drained first, the debug hooks lose their frame
+        // that still read the planes are drained first, the debug hooks lose their frame.  Contexts with queued
+        // interpolations (which may read this cloud) are drained too.
         std::lock_guard<std::mutex> lk(g_registry_mu);
         for (bgs_context* c : g_contexts) {
+            if (c->device == cl->device && c->reads_pending.load(std::memory_order_relaxed))
+                c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
             if (c->pend.cloud == cl || c->last.cloud == cl) {
                 if (c->async_pending || c->pend.cloud == cl) c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
                 if (c->pend.cloud == cl) { c->pend.cloud = nullptr; c->pend.n = 0; }
@@ -363,6 +366,41 @@ bgs_status bgs_cloud_positions_get(bgs_context* c, const bgs_cloud* cl, float* o
     CU(c, cudaMemcpyAsync(out_pos_vis, cl->pos, (size_t)cl->n * 16, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return BGS_OK;
+}
+
+// ---- interpolation (interpolate.cu).  A queued write of `out` that reads `lhs` and `rhs` (host.cuh:
+// queue_cloud_write_reading), never drained.
+
+// interpolate.wgsl:51-57 in f32: false (t untouched) for non-finite inputs or a NaN factor
+static bool interpolation_factor(float time, float time_start, float time_stop, float* t) {
+    if (!std::isfinite(time) || !std::isfinite(time_start) || !std::isfinite(time_stop)) return false;
+    const float d = time_stop - time_start;
+    float f;
+    if (std::fabs(d) < 1e-6f) f = time >= time_stop ? 1.0f : 0.0f;
+    else f = std::min(std::max((time - time_start) / d, 0.0f), 1.0f);
+    if (std::isnan(f)) return false;   // (std::max / std::min would pass NaN through; it is caught here)
+    *t = f;
+    return true;
+}
+
+bgs_status bgs_cloud_interpolate(bgs_context* c, bgs_cloud* out, const bgs_cloud* lhs, const bgs_cloud* rhs, float time,
+                                 float time_start, float time_stop) {
+    if (!out || !lhs || !rhs) return fail(c, BGS_EINVAL, "interpolate: null cloud");
+    // (-1: the three are not on one device, so not all are on the context's)
+    TRY(enter_call(c, "interpolate", lhs->device == out->device && rhs->device == out->device ? out->device : -1, "clouds live"));
+    if (lhs->n != out->n || rhs->n != out->n)
+        return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out hold %u, %u and %u gaussians", lhs->n, rhs->n, out->n);
+    if (lhs->f16 != out->f16 || rhs->f16 != out->f16 || lhs->cov != out->cov || rhs->cov != out->cov)
+        return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out are not in one layout");
+    if (out == lhs || out == rhs) return fail(c, BGS_EINVAL, "interpolate: out is lhs or rhs");
+    float t = 0.0f;
+    if (!interpolation_factor(time, time_start, time_stop, &t))
+        return fail(c, BGS_EINVAL, "interpolate: time %g, time_start %g, time_stop %g give no factor", time, time_start, time_stop);
+    return queue_cloud_write_reading(c, out, lhs, rhs, [&](cudaStream_t q) {
+        launch_interpolate(out->f16, out->cov, lhs->blocks, rhs->blocks, out->n, t, out->blocks, out->pos, q);
+        CU(c, cudaGetLastError());
+        return BGS_OK;
+    });
 }
 
 // ---- subset and download (subset.cu).  Both only read the source cloud (before_cloud_read), so neither drains another

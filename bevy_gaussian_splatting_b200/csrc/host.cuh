@@ -126,6 +126,10 @@ struct bgs_context {
     DevBuf<uint8_t> mesh_tri, mesh_pairs;
     bool async_pending = false;        // a BGS_FLAG_ASYNC frame has been enqueued and not yet completed
     bool step_pending = false;         // a particle step has been enqueued since the last bgs_sync
+    // an interpolation (a queued write that reads other clouds) has been enqueued since the last bgs_sync: ev_done
+    // marks it, and the synchronous writers and bgs_cloud_destroy drain this context (set and read under the registry
+    // lock; cleared by bgs_sync)
+    std::atomic<bool> reads_pending{false};
     FrameCounters* ctr = nullptr;
     uint32_t* hist = nullptr;          // [8 + 4 * MAX_CHUNKS][256]: depth passes 0..3, pair passes 4..7 (round 0), 8 + 4r.. (round r)
     uint32_t* kg_block_cnt = nullptr;  // [kg_grid]: keygen_coop's per-CTA visible counts
@@ -223,6 +227,9 @@ inline bgs_status enter_call(bgs_context* c, const char* call, int device, const
 // bgs_sync (whose failure is returned).  Queued write (the step): on the device, after every frame queued on any
 // context of the GPU (each context's ev_done marks its last) and every earlier step of the cloud, under the registry
 // lock so another context's write waits and records in turn; it then marks itself on the cloud's ev_write.
+// Queued write that reads other clouds (the interpolation): the queued write's order, after the read order of each
+// input; it then re-records the context's ev_done and sets reads_pending, so that a later queued write of an input waits
+// for it on the device and a later synchronous write or destroy of an input drains it on the host.
 
 inline bgs_status before_cloud_read(bgs_context* c, const bgs_cloud* cl) {
     if (cl->stepped.load(std::memory_order_acquire)) CU(c, cudaStreamWaitEvent(c->stream, cl->ev_write, 0));
@@ -234,7 +241,7 @@ inline bgs_status before_cloud_write(bgs_context* c, const bgs_cloud* cl) {
     TRY(before_cloud_read(c, cl));
     std::lock_guard<std::mutex> lk(g_registry_mu);
     for (bgs_context* o : g_contexts)
-        if (o != c && o->device == cl->device && o->async_pending)
+        if (o != c && o->device == cl->device && (o->async_pending || o->reads_pending.load(std::memory_order_relaxed)))
             o->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
     return BGS_OK;
 }
@@ -252,6 +259,19 @@ bgs_status queue_cloud_write(bgs_context* c, bgs_cloud* cl, Write write) {
     CU(c, cudaEventRecord(cl->ev_write, q));
     cl->stepped.store(true, std::memory_order_release);
     return BGS_OK;
+}
+
+// `write(stream)` enqueues the write of `cl`, which reads `in0` and `in1`
+template <class Write>
+bgs_status queue_cloud_write_reading(bgs_context* c, bgs_cloud* cl, const bgs_cloud* in0, const bgs_cloud* in1, Write write) {
+    return queue_cloud_write(c, cl, [&](cudaStream_t q) {
+        TRY(before_cloud_read(c, in0));
+        if (in1 != in0) TRY(before_cloud_read(c, in1));
+        TRY(write(q));
+        CU(c, cudaEventRecord(c->ev_done, q));
+        c->reads_pending.store(true, std::memory_order_relaxed);
+        return BGS_OK;
+    });
 }
 
 // ---- frame scratch (api.cu) that the selections borrow

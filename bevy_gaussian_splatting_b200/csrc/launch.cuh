@@ -78,4 +78,7 @@ void launch_subset_scatter(bool f16, const void* pos, const void* blocks, uint32
 void launch_subset_gather(bool f16, const void* pos, const void* blocks, const uint32_t* idx, uint32_t k, void* out_pos,
                           void* out_blocks, cudaStream_t stream);
 void launch_unpack(bool f16, const void* blocks, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream);
+// interpolate.cu
+void launch_interpolate(bool f16, bool cov, const void* lhs_blocks, const void* rhs_blocks, uint32_t n, float t,
+                        void* out_blocks, float4* out_pos, cudaStream_t stream);
 }  // namespace bgs

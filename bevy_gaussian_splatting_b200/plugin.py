@@ -370,6 +370,16 @@ class GaussianSplattingPlugin:
         self._check(self._lib.bgs_cloud_positions_get(self._ctx, handle._h, _ptr(out)))
         return out
 
+    # -- interpolation (src/morph/interpolate.rs): an enqueued per-frame blend of two clouds (the rule: include/bgs.h)
+    def interpolate(self, out: PlanarGaussian3dHandle, lhs: PlanarGaussian3dHandle, rhs: PlanarGaussian3dHandle,
+                    settings: CloudSettings) -> None:
+        """`out` := the blend of `lhs` and `rhs` at `settings.time` between `settings.time_start` and `time_stop`,
+        enqueued on this context: frames rendered before it (on any context) see the old `out`, everything after it the
+        blend.  The three clouds hold the same number of gaussians in one layout; make `out` once as
+        `subset(lhs, np.arange(lhs.n))`.  `sync()` completes it."""
+        self._check(self._lib.bgs_cloud_interpolate(self._ctx, out._h, lhs._h, rhs._h, C.c_float(settings.time),
+                                                    C.c_float(settings.time_start), C.c_float(settings.time_stop)))
+
     # -- parity / measurement hooks
     def frame_stats(self) -> abi.bgs_frame_stats:
         fs = abi.bgs_frame_stats()

@@ -104,6 +104,10 @@ class CloudSettings:
     # this repo's extension: front-to-back binning rounds (BGS_FLAG_CHUNKS): None = library's choice from the last
     # frame's footprint statistics, True = always, False = never (the tile debug hooks need a one-round frame)
     binning_rounds: Optional[bool] = None
+    # the interpolation window (settings.rs:106-107, 128-129): `GaussianSplattingPlugin.interpolate` blends at
+    # (time - time_start) / (time_stop - time_start).  Last, so positional construction keeps its meaning
+    time_start: float = 0.0
+    time_stop: float = 1.0
 
     def to_abi(self) -> abi.bgs_settings:
         if self.visualize_bounding_box:

@@ -3,7 +3,7 @@
 //
 //   headless [count=100000] [width=1920] [height=1080] [global_scale=1.0] [out=headless_output/0.ppm]
 //            [--dump-cloud file] [--raw file] [--remove-floaters radius]
-//            [--particles N --steps K --dt S [--dump-particles file]]
+//            [--particles N --steps K --dt S [--dump-particles file]] [--interpolate SEED --time T]
 // --dump-cloud writes the four f32 planes (n, then pos_vis, sh, rot, scale_opacity) so another host can
 // render the identical cloud; --raw writes the RGBA8 frame bytes.  --remove-floaters selects the sparse gaussians
 // (SparseSelect with that radius), inverts the selection and draws only the rest (DrawMode::Selected), the
@@ -11,6 +11,11 @@
 // --particles attaches random_particle_behaviors(N, 0) to the cloud and enqueues K steps of S seconds before the frames
 // (the reference's morph_particles feature, stepped once per frame); --dump-particles writes N (u64), the behaviours
 // before and after the steps (N * 64 B each) and the position plane after them (count * 16 B).
+// --interpolate blends the cloud (lhs) with random_gaussians_3d_seeded(count, SEED) (rhs) at time T of the window
+// [0, 1] into a third cloud, made as the subset of every gaussian of lhs, and draws that one (the reference's
+// GaussianInterpolate { lhs, rhs }); --dump-cloud then writes rhs's four planes after lhs's.
+#include <memory>
+#include <numeric>
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -26,6 +31,7 @@ int main(int argc, char** argv) {
     float floater_radius = 0.0f;
     size_t n_particles = 0; int steps = 0; float dt = 1.0f / 60.0f;
     std::string dump_particles;
+    long interp_seed = -1; float interp_time = 0.0f;
     int pos = 0;
     for (int i = 1; i < argc; ++i) {
         const std::string a = argv[i];
@@ -36,6 +42,8 @@ int main(int argc, char** argv) {
         if (a == "--steps" && i + 1 < argc) { steps = std::atoi(argv[++i]); continue; }
         if (a == "--dt" && i + 1 < argc) { dt = (float)std::atof(argv[++i]); continue; }
         if (a == "--dump-particles" && i + 1 < argc) { dump_particles = argv[++i]; continue; }
+        if (a == "--interpolate" && i + 1 < argc) { interp_seed = std::atol(argv[++i]); continue; }
+        if (a == "--time" && i + 1 < argc) { interp_time = (float)std::atof(argv[++i]); continue; }
         switch (pos++) {
             case 0: count = std::strtoull(a.c_str(), nullptr, 10); break;
             case 1: W = std::atoi(a.c_str()); break;
@@ -74,10 +82,24 @@ int main(int argc, char** argv) {
                 f.write((const char*)moved.data(), moved.size() * 4);
             }
         }
+        bgs::PlanarGaussian3d rhs_cloud;
+        std::unique_ptr<bgs::PlanarGaussian3dHandle> blended;
+        if (interp_seed >= 0) {
+            rhs_cloud = bgs::random_gaussians_3d_seeded(count, (uint64_t)interp_seed);
+            bgs::PlanarGaussian3dHandle rhs = plugin.add_cloud(rhs_cloud);
+            std::vector<uint32_t> all(count);
+            std::iota(all.begin(), all.end(), 0u);
+            blended.reset(new bgs::PlanarGaussian3dHandle(plugin.subset(handle, &all)));
+            bgs::CloudSettings window = settings;
+            window.time = interp_time; window.time_start = 0.0f; window.time_stop = 1.0f;
+            plugin.interpolate(*blended, handle, rhs, window);
+            std::printf("interpolated: seed %ld at time %g\n", interp_seed, (double)interp_time);
+        }
+        const bgs::PlanarGaussian3dHandle& drawn_cloud = blended ? *blended : handle;
         const bgs_view view = bgs::headless_view(W, H);
         std::vector<unsigned char> frame((size_t)W * H * 4);
         bool drawn = false;
-        for (int f = 0; f < 3; ++f) drawn = plugin.render_view(handle, settings, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);
+        for (int f = 0; f < 3; ++f) drawn = plugin.render_view(drawn_cloud, settings, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);
         const bgs_frame_stats fs = plugin.frame_stats();
         float us[6];
         bgs_stage_times_us(plugin.context(), us);
@@ -91,6 +113,12 @@ int main(int argc, char** argv) {
             f.write((const char*)cloud.spherical_harmonic.data(), n * 192);
             f.write((const char*)cloud.rotation.data(), n * 16);
             f.write((const char*)cloud.scale_opacity.data(), n * 16);
+            if (interp_seed >= 0) {
+                f.write((const char*)rhs_cloud.position_visibility.data(), n * 16);
+                f.write((const char*)rhs_cloud.spherical_harmonic.data(), n * 192);
+                f.write((const char*)rhs_cloud.rotation.data(), n * 16);
+                f.write((const char*)rhs_cloud.scale_opacity.data(), n * 16);
+            }
         }
         if (!raw.empty()) { std::ofstream f(raw, std::ios::binary); f.write((const char*)frame.data(), frame.size()); }
         const size_t slash = out.find_last_of('/');

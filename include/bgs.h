@@ -293,6 +293,50 @@ void bgs_particles_destroy(bgs_particles* particles);
 bgs_status bgs_cloud_particles_step(bgs_context* ctx, bgs_cloud* cloud, bgs_particles* particles, float delta_time);
 bgs_status bgs_cloud_positions_get(bgs_context* ctx, const bgs_cloud* cloud, float* out_pos_vis /* n * 4 */);
 
+/* Interpolation (src/morph/interpolate.rs, interpolate.wgsl:51-119; the reference's GaussianInterpolate { lhs, rhs }):
+ * `out` := the blend of two clouds at a time between time_start and time_stop (CloudSettings.time / time_start /
+ * time_stop of the output entity, defaults 0 / 0 / 1), without a re-upload.  The output cloud is made once, e.g. as
+ * bgs_cloud_subset(lhs, [0, n)), the device form of the reference's "clone lhs".
+ * bgs_cloud_interpolate.  The rule, exactly:
+ *   - the factor t (interpolate.wgsl:51-57), computed once on the host in f32: d = time_stop - time_start; if
+ *     |d| < 1e-6f, t = (time >= time_stop) ? 1 : 0; otherwise t = min(max((time - time_start) / d, 0), 1), where a
+ *     quotient of -0 stays -0 (time == time_start with d < 0; WGSL does not pin the sign of a zero max);
+ *   - every lane of gaussian i is mix(a, b, t) = a*(1-t) + b*t, a from lhs, b from rhs, 1-t rounded once; every
+ *     operation f32 round-to-nearest-even without FMA, subnormals kept.  The lanes: position xyz and visibility (both
+ *     device copies: the position plane and the block), the 48 SH coefficients, scale xyz and opacity, or for the
+ *     precomputed-covariance layout the six covariance entries and opacity;
+ *   - the rotation is normalize_quaternion(mix(q_l, q_r, t)) (:59-65): l2 = ((q0*q0 + q1*q1) + q2*q2) + q3*q3 in
+ *     storage lane order (w, x, y, z); if l2 <= 0 the lanes are (0, 0, 0, 1), i.e. w = 0, z = 1 (a half-turn about z:
+ *     it renders like the identity, and is what a download returns), which also covers q and -q at t = 0.5 and
+ *     components whose squares underflow; otherwise each lane is q_k / sqrt(l2), IEEE division and square root.  NaN
+ *     and overflow propagate as that arithmetic gives them;
+ *   - f16 layouts: each half is widened exactly, blended as above in f32 and narrowed with round-to-nearest-even
+ *     (past the f16 range: +-inf), in the lane map of the upload (planar.wgsl:264-331 against :116-176), except that
+ *     the covariance record's fourth word is pack2x16float(vec2(0.0, opacity)): its low half is +0 whatever the inputs
+ *     held.  The reference's f16 path is never compiled and the rounding of its pack2x16float is the implementation's:
+ *     both are **unpinned**, as for the rest of f16.
+ *   Note that mix(a, a, t) need not equal a; lhs == rhs is allowed.
+ * Ordering.  The call is ENQUEUED on the context's render stream (one kernel) and returns: no host synchronisation.
+ *   `out` is written as a particle step writes a cloud: after every frame queued on any context of the GPU and every
+ *   earlier queued write of `out`; frames and reads of `out` on any context see exactly the interpolations enqueued
+ *   before them.  lhs and rhs are read after every queued write of them enqueued before the call (particle steps,
+ *   interpolations into them), on any context.  A later write of lhs or rhs -- a particle step, an interpolation into
+ *   them, bgs_cloud_visibility_set, the selection calls -- or bgs_cloud_destroy waits for the interpolation.  bgs_sync(ctx)
+ *   completes ctx's queued interpolations; a fault is reported by the next synchronising call on that context.  A
+ *   context that never interpolates issues the same launches and waits as before.
+ * Where this port deliberately differs from the reference:
+ *   1. lhs, rhs and out must hold the same n in the same layout (f32 / f16 / f16 precomputed covariance).  The reference
+ *      sizes the output as a clone of lhs and indexes rhs unguarded.
+ *   2. out may not be lhs or rhs (in the reference it is always a separate asset).
+ *   3. The caller interpolates explicitly, once; the reference runs the pass once per camera view
+ *      (interpolate.rs:388-475), with the same inputs and so the same result.
+ *   4. The entity's Aabb is not updated, as for the particle step: RasterizeMode::Position reads the caller's.
+ * A null argument, a cloud on another device than the context's, a mismatch of n or layout, out == lhs or rhs, a
+ * time, time_start or time_stop that is not finite, or a NaN factor (e.g. (3e38 - -3e38) / inf) -> BGS_EINVAL; a
+ * refused call changes and enqueues nothing. */
+bgs_status bgs_cloud_interpolate(bgs_context* ctx, bgs_cloud* out, const bgs_cloud* lhs, const bgs_cloud* rhs, float time,
+                                 float time_start, float time_stop);
+
 /* One view of one cloud: key-gen -> depth radix sort -> projection + SH colour -> tile
  * binning -> per-tile front-to-back blend.  out_rgba is caller-owned (host pointer, or a
  * device pointer when out_is_device_ptr != 0); may be NULL to keep the frame on the device. */

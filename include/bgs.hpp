@@ -40,6 +40,8 @@ struct CloudSettings {   // src/gaussian/settings.rs:110-133 (defaults)
     RasterizeMode rasterize_mode = RasterizeMode::Color;
     GaussianColorSpace color_space = GaussianColorSpace::SrgbRec709Display;
     float time = 0.0f;
+    float time_start = 0.0f;   // the interpolation window (GaussianSplattingPlugin::interpolate)
+    float time_stop = 1.0f;
     // this repo's extension: front-to-back binning rounds (BGS_FLAG_CHUNKS): -1 = the library's choice from the last
     // frame's footprint statistics, 1 = always, 0 = never (the tile debug hooks need a one-round frame)
     int binning_rounds = -1;
@@ -363,6 +365,13 @@ public:
     }
     void step_particles(PlanarGaussian3dHandle& cloud, ParticleBehaviorsHandle& p, float delta_time) {
         check(bgs_cloud_particles_step(ctx_, cloud.get(), p.get(), delta_time));
+    }
+    // Interpolation (src/morph/interpolate.rs; the rule and its ordering: bgs.h): out := the blend of lhs and rhs at
+    // settings.time between settings.time_start and time_stop, enqueued like a particle step.  The three clouds hold the
+    // same number of gaussians in one layout; make `out` once as subset(lhs, &indices 0 .. n-1).
+    void interpolate(PlanarGaussian3dHandle& out, const PlanarGaussian3dHandle& lhs, const PlanarGaussian3dHandle& rhs,
+                     const CloudSettings& settings) {
+        check(bgs_cloud_interpolate(ctx_, out.get(), lhs.get(), rhs.get(), settings.time, settings.time_start, settings.time_stop));
     }
     std::vector<float> positions(const PlanarGaussian3dHandle& cloud) {   // n * 4: x, y, z, visibility
         std::vector<float> v((size_t)cloud.len() * 4);
