@@ -199,6 +199,13 @@ bgs_status frame_out(bgs_context* c, const bgs_settings* st, uint32_t format, si
     const bool blend_over = (st->flags & BGS_FLAG_BLEND_OVER_TARGET) != 0;
     o->raster_format = format | ((blend_over ? 2u : ((st->flags & BGS_FLAG_PREMULTIPLIED_OUT) ? 1u : 0u)) << 8);
     o->bytes = bytes;
+    // device targets are written with pixel-sized vector stores (and read so in blend-over mode): each must be aligned to
+    // one pixel, 4 / 8 / 16 bytes
+    const size_t bpp = format_bpp(format);
+    if (out_is_device_ptr)
+        for (const void* t : {out_rgba, want_aux ? out_depth : nullptr, want_aux ? out_normal : nullptr})
+            if (reinterpret_cast<uintptr_t>(t) % bpp != 0)
+                return fail(c, BGS_EINVAL, "render: device target %p is not aligned to its %zu-byte pixels", t, bpp);
     if (out_rgba && out_is_device_ptr) {
         o->rgba = out_rgba;
     } else {
@@ -209,11 +216,14 @@ bgs_status frame_out(bgs_context* c, const bgs_settings* st, uint32_t format, si
         }
         // async frames rendered into the library's own buffers alternate two device frames, so whatever consumes
         // frame k off the render stream (the D2H copy, the NCCL gather: both on the copy/comm stream) overlaps frame k+1
-        if (st->flags & BGS_FLAG_ASYNC) {
-            if (blend_over) o->slot = c->frame_toggle ^ 1;            // keep blending into the frame the previous call produced
-            else { o->slot = c->frame_toggle; c->frame_toggle ^= 1; }
-        }
-        o->rgba = c->frames[std::max(o->slot, 0)].p;
+        // (blend-over, queued or not, keeps blending into the frame the previous call produced; synchronous calls that do
+        // not blend over use frame 0)
+        int k = 0;
+        if (blend_over) k = c->frame_last;
+        else if (st->flags & BGS_FLAG_ASYNC) { k = c->frame_toggle; c->frame_toggle ^= 1; }
+        c->frame_last = k;
+        if (st->flags & BGS_FLAG_ASYNC) o->slot = k;
+        o->rgba = c->frames[k].p;
         o->host_rgba = out_rgba;
     }
     if (!want_aux) return BGS_OK;
@@ -501,12 +511,13 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaEventRecord(c->ev_front, q));
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
             launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
-                          fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal, c->stream_r);
+                          fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal, &c->ctr->truncated,
+                          c->stream_r);
             CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
             CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
         } else
             launch_raster_round(c->recs.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x, fc.tiles_y, o.rgba, o.raster_format,
-                                c->state.p, c->tile_done, &c->ctr->tiles_done, r == 0, r + 1 == p.rounds, q);
+                                c->state.p, c->tile_done, &c->ctr->tiles_done, &c->ctr->truncated, r == 0, r + 1 == p.rounds, q);
         ++launches;
     }
     c->pair_result = pcur;

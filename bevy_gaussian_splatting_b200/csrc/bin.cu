@@ -134,6 +134,7 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
         cc->med_count = (uint32_t)(pre[1] + s_tot[1]);
         cc->big_count = (uint32_t)(pre[2] + s_tot[2]);
         atomicMax(sticky_need, need);
+        if (need > capacity) ctr->truncated = 1u;
     }
     uint32_t run = pre[0] > LB_VMASK ? LB_VMASK : (uint32_t)pre[0];
     uint32_t mrun = (uint32_t)pre[1], brun = (uint32_t)pre[2];

@@ -63,7 +63,7 @@ struct FrameCounters {
     uint32_t n_sort;            // entries the depth sort runs over (n_vis, or N with SORT_ALL)
     uint32_t n_vis;             // in-frustum gaussians
     uint32_t tiles_done;        // tiles whose pixels have all saturated (chunked frames)
-    uint32_t pad0;
+    uint32_t truncated;         // some round needed more pairs than the buffer holds: the blend leaves the target as it was
     uint32_t culled_min_inv;    // RasterizeMode::Depth: max over culled of (0xFFFFFFFF - index); 0 = none culled
     uint32_t culled_max_p1;     //                       max over culled of (index + 1);          0 = none culled
     float depth_min, depth_max; //                       distances of sorted[N-1] / sorted[1] (gaussian.wgsl:329-349)

@@ -139,7 +139,8 @@ struct bgs_context {
     // async frames delivered to host memory alternate the two frames so frame k's D2H copy (copy stream) overlaps
     // frame k+1's kernels
     DevBuf<void> frames[2];
-    int frame_toggle = 0;
+    int frame_toggle = 0;              // the frame the next queued call that does not blend over takes
+    int frame_last = 0;                // the frame the last call rendering into the library's frames wrote (blend-over's target)
     bool copy_pending[2] = {false, false};
     FrameCounters* h_ctr = nullptr;    // pinned
     float* cutoff_tab = nullptr;       // adaptive cutoff of every f16 opacity value (project.cu)

@@ -38,10 +38,10 @@ cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, Fra
 // raster.cu
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
-                   const float4* aux, void* out_depth, void* out_normal, cudaStream_t stream);
+                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, cudaStream_t stream);
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
-                         uint32_t* tiles_done, int first, int last, cudaStream_t stream);
+                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, cudaStream_t stream);
 // select.cu
 uint32_t select_num_buckets(uint32_t n);
 int select_sort_passes(uint32_t n_buckets);

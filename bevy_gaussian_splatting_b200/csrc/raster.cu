@@ -224,7 +224,8 @@ template <int MODE, bool AUX>
 __global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : 5)
 raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
               const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
-              const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal) {
+              const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
+              const uint32_t* __restrict__ truncated) {
     __shared__ __align__(16) unsigned char s_mem[(MODE == 2 ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0)];
     constexpr uint32_t SM_AUX = MODE == 2 ? SM_BYTES_2D : SM_BYTES;
     __shared__ __align__(16) uint32_t s_ent[2][ENT_WORDS];    // TMA destination: the tile's pair-list chunks
@@ -248,6 +249,10 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
     const float rcx = (float)wx0 + 4.0f, rcy = (float)wy0 + 2.0f;   // centre of the warp's pixel centres
     const float tcx = (float)(tile_x * TILE_PX) + 8.0f, tcy = (float)(tile_y * TILE_PX) + 8.0f;   // tile centre
     uint2 range = ranges[tile];
+    // a pair list cut short by the buffer's capacity: the frame is rendered again after the buffer grows, so this attempt
+    // leaves every target as it was (blend-over must not composite the layer twice).  (Loaded beside the range, and not
+    // kept live through the blend: the register budget of raster_kernel<0> has no room for it.)
+    if (*truncated) return;
     range.x = ~range.x;                  // stored as (~start, end): the sort's last pass builds it with atomicMax (radix.cu)
 
     if (range.x >= range.y) {            // empty tile: nothing to stage (uniform across the CTA)
@@ -476,7 +481,8 @@ __device__ __forceinline__ void store_pixel2(void* out, uint32_t format, size_t 
     } else {
         uint32_t* o = reinterpret_cast<uint32_t*>(out) + pix;
         const uint32_t p0 = pack_srgb8(r0, g0, b0, 1.0f, false), p1 = pack_srgb8(r1, g1, b1, 1.0f, false);
-        if (in0 && in1 && (pix & 1) == 0) *reinterpret_cast<uint2*>(o) = make_uint2(p0, p1);
+        // one 8-byte store where the address allows it (targets are only required to be 4-byte aligned)
+        if (in0 && in1 && (reinterpret_cast<uintptr_t>(o) & 7u) == 0) *reinterpret_cast<uint2*>(o) = make_uint2(p0, p1);
         else { if (in0) o[0] = p0; if (in1) o[1] = p1; }
     }
 }
@@ -485,7 +491,8 @@ template <bool CHUNKED>
 __global__ void __launch_bounds__(R2_THREADS)
 raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges,
                int W, int H, int tiles_x, void* __restrict__ out, uint32_t format, float4* __restrict__ state,
-               unsigned char* __restrict__ tile_done, uint32_t* __restrict__ tiles_done, int first, int last) {
+               unsigned char* __restrict__ tile_done, uint32_t* __restrict__ tiles_done, const uint32_t* __restrict__ truncated,
+               int first, int last) {
     __shared__ __align__(16) unsigned char s_mem[R2_BYTES];
     float4* s_q0 = reinterpret_cast<float4*>(s_mem + SM_Q0);
     float4* s_uv = reinterpret_cast<float4*>(s_mem + SM_UV);
@@ -502,6 +509,7 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
     const bool in0 = px0 < W && py < H, in1 = px0 + 1 < W && py < H;
     const float fx0 = (float)px0 + 0.5f, fx1 = (float)px0 + 1.5f, fy = (float)py + 0.5f;
     uint2 range = ranges[tile];
+    if (*truncated) return;              // (as raster_kernel; on a chunked frame the word also covers the earlier rounds)
     range.x = ~range.x;                  // stored as (~start, end), (0, 0) = empty (radix.cu)
 
     // T < T_STOP <=> pixel done; lim = 1 while alive, -1 once done (folds the "alive" test into |u| <= lim)
@@ -601,30 +609,30 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
 
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
-                   const float4* aux, void* out_depth, void* out_normal, cudaStream_t stream) {
+                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, cudaStream_t stream) {
     const int grid = tiles_x * tiles_y;
     // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
     // pixels (more of its lanes then idle at the tile's splat boundaries)
     if (aux == nullptr && mode == 0 && large_footprints) {
         raster2_kernel<false><<<grid, R2_THREADS, 0, stream>>>(recs, tile_entries, ranges, W, H, tiles_x, out, format,
-                                                               nullptr, nullptr, nullptr, 1, 1);
+                                                               nullptr, nullptr, nullptr, truncated, 1, 1);
         return;
     }
     // aux != nullptr: colour + depth + normal in one pass (bgs_render_aux)
     static void (*const kernels[2][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*,
-                                       uint32_t, const float4*, void*, void*) = {
+                                       uint32_t, const float4*, void*, void*, const uint32_t*) = {
         {raster_kernel<0, false>, raster_kernel<1, false>, raster_kernel<2, false>},
         {raster_kernel<0, true>, raster_kernel<1, true>, raster_kernel<2, true>}};
     kernels[aux != nullptr][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
-        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal);
+        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated);
 }
 
 // One front-to-back round of a chunked frame (quad-uv records only); see raster2_kernel.
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
-                         uint32_t* tiles_done, int first, int last, cudaStream_t stream) {
+                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, cudaStream_t stream) {
     raster2_kernel<true><<<tiles_x * tiles_y, R2_THREADS, 0, stream>>>(recs, tile_entries, ranges, W, H, tiles_x, out, format,
-                                                                       state, tile_done, tiles_done, first, last);
+                                                                       state, tile_done, tiles_done, truncated, first, last);
 }
 
 }  // namespace bgs

@@ -212,13 +212,15 @@ class GaussianSplattingPlugin:
         return outs
 
     def render_view_to_device(self, handle: PlanarGaussian3dHandle, settings: CloudSettings, view: View, device_ptr: int,
-                              transform: CloudTransform | None = None, fmt: str = "rgba8_srgb", asynchronous: bool = False) -> None:
+                              transform: CloudTransform | None = None, fmt: str = "rgba8_srgb", asynchronous: bool = False,
+                              premultiplied: bool = False, blend_over: bool = False) -> None:
         """Render straight into caller-owned device memory: an exported frame target (`bgs_frame_export_create`), or
         another GPU's memory mapped into this process (`bgs_peer_buffer_open`) -- the blend kernel's pixel stores then
-        travel over NVLink themselves."""
+        travel over NVLink themselves.  The target must be aligned to one pixel (4 / 8 / 16 bytes).  `premultiplied` /
+        `blend_over` as in `render_view`; blend-over reads what `device_ptr` holds."""
         code, _, _ = self.FORMATS[fmt]
         v = view.to_abi()
-        u, s = self._uniform_and_settings(handle, settings, transform, asynchronous)
+        u, s = self._uniform_and_settings(handle, settings, transform, asynchronous, premultiplied, blend_over)
         self._check(self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.c_void_p(device_ptr), code, 1))
 
     def sync(self) -> bool:

@@ -74,8 +74,14 @@ enum {
                                channels -- the reference's PREMULTIPLIED_ALPHA_BLENDING on the view target
                                (render/mod.rs:944-948): several clouds per view (one bgs_render each, far cloud first,
                                mod.rs:398-452) and a scene behind the splats.  Target = out_rgba when it is a device
-                               pointer, else the context's frame (which keeps the previous call's result; frames
-                               delivered to host memory are copied out after blending). */
+                               pointer, else the context's frame that the previous call rendering into the context's
+                               frames wrote, synchronous or queued (frames delivered to host memory are copied out
+                               after blending).  A pixel no splat blends keeps its bytes, except that -0.0 becomes +0.0
+                               in RGBA16F / RGBA32F targets (and a NaN may come back as another NaN).  A frame whose
+                               (splat, tile) pair list outgrew the buffer (BGS_NOT_READY) leaves the target as it was:
+                               a synchronous call renders such a frame again by itself and composites it once; after a
+                               queued one, bgs_sync's BGS_NOT_READY means the overflowed frames did not touch their
+                               targets, so rendering them again composites each once. */
     BGS_FLAG_CHUNKS = 8u    /* bin / tile-sort / blend in front-to-back rank rounds that stop emitting (splat, tile)
                                pairs once every tile has saturated.  Same pixels, bit for bit.  Only USE_OBB frames from
                                bgs_render (not USE_AABB ones, not bgs_render_aux) of at most 65536 tiles are ever split
@@ -339,7 +345,9 @@ bgs_status bgs_cloud_interpolate(bgs_context* ctx, bgs_cloud* out, const bgs_clo
 
 /* One view of one cloud: key-gen -> depth radix sort -> projection + SH colour -> tile
  * binning -> per-tile front-to-back blend.  out_rgba is caller-owned (host pointer, or a
- * device pointer when out_is_device_ptr != 0); may be NULL to keep the frame on the device. */
+ * device pointer when out_is_device_ptr != 0); may be NULL to keep the frame on the device.
+ * A device target must be aligned to one pixel: 4 bytes for RGBA8, 8 for RGBA16F, 16 for RGBA32F
+ * (bgs_render_aux: each of its three targets); else BGS_EINVAL, nothing enqueued or written. */
 bgs_status bgs_render(bgs_context* ctx, const bgs_cloud* cloud, const bgs_view* view,
                       const bgs_cloud_uniform* uniform, const bgs_settings* settings, void* out_rgba,
                       uint32_t out_format, int out_is_device_ptr);
@@ -355,8 +363,9 @@ bgs_status bgs_render_aux(bgs_context* ctx, const bgs_cloud* cloud, const bgs_vi
                           void* out_depth, void* out_normal, uint32_t out_format, int out_is_device_ptr);
 
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
- * BGS_NOT_READY: the last frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
- * lot); the buffer has been grown -- render that frame again.  A no-op after a synchronous render. */
+ * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
+ * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target
+ * as it was (see BGS_FLAG_BLEND_OVER_TARGET).  A no-op after a synchronous render. */
 bgs_status bgs_sync(bgs_context* ctx);
 
 /* Parity / debug hooks (valid after a completed bgs_render on this context). */

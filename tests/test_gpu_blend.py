@@ -31,6 +31,7 @@ import pytest
 import bevy_gaussian_splatting_b200 as B
 import blend_cases as BC
 import kernel_paths as KP
+import output_cases as OC
 
 pytestmark = pytest.mark.gpu
 
@@ -133,9 +134,17 @@ def assert_coverage_map(name, got, oracle_img, trace, out_mode, classes=None):
 
 
 def assert_quantised(got, trace, aabb, out_mode, fmt, dc, dst=None):
-    """RGBA16F / RGBA8-sRGB: the format's rounding of some value inside each pixel's interval [want - b, want + b]."""
+    """RGBA16F / RGBA8-sRGB: the format's rounding of some value inside each pixel's interval [want - b, want + b].
+    `dst` (over): the target in the frame's format; an RGBA8 one is blended as the kernel decodes it, which is the
+    float64 decode within `srgb_decode_err` (colour) and 2 U (alpha), each scaled by T."""
+    derr = 0.0
+    if dst is not None and dst.dtype == np.uint8:
+        T = trace["T64"][..., None]
+        derr = np.concatenate([OC.srgb_decode_err(dst[..., :3]), 2 * BC.U * dst[..., 3:] / 255.0], -1) * T
+        dst = np.concatenate([OC.srgb_decode64(dst[..., :3] / 255.0), dst[..., 3:] / 255.0], -1)
     want = BC.expected_frame(trace, out_mode, dst)
     b, _ = BC.frame_bounds(trace, aabb, out_mode, dc, dst)
+    b = b + derr
     lo, hi = want - b, want + b
     if fmt == "rgba16f":
         def q(x):
@@ -238,10 +247,11 @@ def test_blend_variant_vs_oracle(oracle, variant):
                 if sat:
                     assert_coverage_map(name + "/" + out_mode, got, oimg, trace, out_mode, classes)
                 assert_within_bound(name, got, trace, aabb, out_mode, dc, dst, classes)
-                if out_mode != "over" and not variant.endswith("aux") and variant != "r0aux":
+                if not variant.endswith("aux") and variant != "r0aux":
                     for fmt in ("rgba16f", "rgba8_srgb"):
-                        q = run_path(p, h, s, view, variant, out_mode, fmt)
-                        assert_quantised(q, trace, aabb, out_mode, fmt, dc)
+                        dq = seeded_target(view, 7, fmt) if out_mode == "over" else None
+                        q = run_path(p, h, s, view, variant, out_mode, fmt, dst=dq)
+                        assert_quantised(q, trace, aabb, out_mode, fmt, dc, dst=dq)
                 h.destroy()
             finally:
                 p.destroy()
