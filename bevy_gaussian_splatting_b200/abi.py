@@ -60,6 +60,14 @@ class bgs_settings(C.Structure):
     ]
 
 
+class bgs_render_extras(C.Structure):
+    _fields_ = [
+        ("previous_clip_from_world", C.c_float * 16),
+        ("delta_time", C.c_float),
+        ("num_classes", C.c_uint32),
+    ]
+
+
 class bgs_frame_stats(C.Structure):
     _fields_ = [
         ("n", C.c_uint32),
@@ -108,6 +116,8 @@ SYMBOLS = [
     ("bgs_cloud_interpolate", C.c_int, [_P, _P, _P, _P, C.c_float, C.c_float, C.c_float]),
     ("bgs_render", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P,
                              C.c_uint32, C.c_int]),
+    ("bgs_render_ex", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings),
+                                C.POINTER(bgs_render_extras), _P, C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,
                                  C.c_uint32, C.c_int]),
     ("bgs_sync", C.c_int, [_P]),

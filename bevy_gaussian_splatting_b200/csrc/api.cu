@@ -2,6 +2,7 @@
 // one CUDA stream), parity/debug hooks, stage timing.  The calls on a resident cloud are in cloud.cu.
 //
 // No PyTorch, no wgpu, no CPU fallback: every stage is a hand-written sm_90a kernel.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -383,7 +384,7 @@ bgs_status bgs_sync(bgs_context* c) {
 }
 
 static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                               const bgs_settings* st, uint32_t out_format, bool want_aux) {
+                               const bgs_settings* st, const bgs_render_extras* ex, uint32_t out_format, bool want_aux) {
     // not-ready inputs map to the reference's silent skip-frame (radix.rs:645-658, mod.rs:1533-1539)
     if (!cloud || !view || !uni || !st) return fail(c, BGS_NOT_READY, "render: cloud/view/uniform/settings not ready");
     TRY(enter_call(c, "render", cloud->device));   // (contexts of one GPU may share clouds)
@@ -392,8 +393,20 @@ static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs
         return fail(c, BGS_EINVAL, "render: radix_sort_depth_bits must be 16, 24 or 32");
     if (st->gaussian_mode != BGS_GAUSSIAN_3D && st->gaussian_mode != BGS_GAUSSIAN_2D)
         return fail(c, BGS_EINVAL, "render: gaussian_mode %u not supported (Gaussian4d is out of scope)", st->gaussian_mode);
-    if (st->rasterize_mode > BGS_RASTERIZE_POSITION)
-        return fail(c, BGS_EINVAL, "render: rasterize_mode %u not supported (Color, Depth, Normal, Position are)", st->rasterize_mode);
+    if (st->rasterize_mode > BGS_RASTERIZE_OPTICAL_FLOW)
+        return fail(c, BGS_EINVAL, "render: rasterize_mode %u not supported (Velocity needs Gaussian4d, out of scope)", st->rasterize_mode);
+    if (st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION && want_aux)
+        return fail(c, BGS_EINVAL, "render_aux: Classification and OpticalFlow frames take extras: use bgs_render_ex");
+    if (st->rasterize_mode == BGS_RASTERIZE_CLASSIFICATION && ex && ex->num_classes == 0)
+        return fail(c, BGS_EINVAL, "render: Classification with num_classes = 0");
+    if (st->rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW) {
+        if (!ex) return fail(c, BGS_EINVAL, "render: OpticalFlow needs the previous view (bgs_render_ex extras)");
+        if (!(std::isfinite(ex->delta_time) && ex->delta_time > 0.0f))
+            return fail(c, BGS_EINVAL, "render: OpticalFlow delta_time %g is not finite and > 0", (double)ex->delta_time);
+        for (int i = 0; i < 16; ++i)
+            if (!std::isfinite(ex->previous_clip_from_world[i]))
+                return fail(c, BGS_EINVAL, "render: previous_clip_from_world[%d] is not finite", i);
+    }
     if (st->draw_mode > BGS_DRAW_HIGHLIGHT_SELECTED) return fail(c, BGS_EINVAL, "render: bad draw_mode");
     if (cloud->cov && (st->gaussian_mode != BGS_GAUSSIAN_3D || st->rasterize_mode == BGS_RASTERIZE_NORMAL || want_aux))
         return fail(c, BGS_EINVAL, "render: a precomputed-covariance cloud has no rotation / scale: Gaussian3d with Color, Depth or Position only");
@@ -428,8 +441,8 @@ static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, co
 }
 
 // Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.
-static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const FramePlan& p,
-                                const FrameOut& o) {
+static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const ModeConsts* modes,
+                                const FramePlan& p, const FrameOut& o) {
     const uint32_t n = cloud->n;
     const uint32_t num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     cudaStream_t q = c->stream;
@@ -472,7 +485,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaEventRecord(c->ev_p0, ps));
     launch_project(cloud->f16, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
                    c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
-                   fc.aux ? c->aux.p : nullptr, ps);
+                   fc.aux ? c->aux.p : nullptr, modes, ps);
     ++launches;
     CU(c, cudaEventRecord(c->ev_p1, ps));
     if (p.overlap) {
@@ -544,16 +557,21 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
 }
 
 static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                              const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr,
-                              bool want_aux, void* out_depth, void* out_normal) {
+                              const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
+                              int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal) {
     if (!c) return BGS_EINVAL;
-    TRY(check_render(c, cloud, view, uni, st, out_format, want_aux));
+    TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux));
     if (c->async_pending && !(st->flags & BGS_FLAG_ASYNC)) {
         // a synchronous render after queued frames completes them first; their failure (including an overflowed
         // pair list = BGS_NOT_READY) is the caller's to see, so this frame is not rendered on top of it
         TRY(bgs_sync(c));
     }
     const FrameConsts fc = frame_consts(cloud, view, uni, st, want_aux);
+    // Classification / OpticalFlow: project_modes_kernel with the extras (NULL extras: num_classes = 1)
+    ModeConsts mc = {};
+    mc.num_classes = ex ? ex->num_classes : 1u;
+    if (ex) { memcpy(mc.prev_clip_from_world, ex->previous_clip_from_world, 64); mc.delta_time = ex->delta_time; }
+    const ModeConsts* modes = st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION ? &mc : nullptr;
     const uint32_t n = cloud->n, num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
@@ -568,7 +586,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         TRY(ensure_arena(c, num_tiles));
         TRY(ensure_status(c, c->status_depth, c->status_n, n));
         TRY(ensure_status(c, c->status_pairs, c->status_np, c->cap_pairs));
-        TRY(enqueue_frame(c, cloud, fc, p, o));
+        TRY(enqueue_frame(c, cloud, fc, modes, p, o));
         if (st->flags & BGS_FLAG_ASYNC) {
             c->async_pending = true;
             c->have_frame = false;     // hooks need bgs_sync() first
@@ -584,9 +602,15 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     return fail(c, BGS_ENOMEM, "render: pair list kept overflowing");
 }
 
+bgs_status bgs_render_ex(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                         const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
+                         int out_is_device_ptr) {
+    return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr);
+}
+
 bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                       const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
-    return render_impl(c, cloud, view, uni, st, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr);
+    return bgs_render_ex(c, cloud, view, uni, st, nullptr, out_rgba, out_format, out_is_device_ptr);
 }
 
 bgs_status bgs_render_aux(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
@@ -594,7 +618,7 @@ bgs_status bgs_render_aux(bgs_context* c, const bgs_cloud* cloud, const bgs_view
                           int out_is_device_ptr) {
     if (c && (!out_rgba || !out_depth || !out_normal)) return fail(c, BGS_EINVAL, "render_aux: the three output frames are required");
     if (c && st && (st->flags & BGS_FLAG_ASYNC)) return fail(c, BGS_EINVAL, "render_aux: BGS_FLAG_ASYNC is not supported");
-    return render_impl(c, cloud, view, uni, st, out_rgba, out_format, out_is_device_ptr, true, out_depth, out_normal);
+    return render_impl(c, cloud, view, uni, st, nullptr, out_rgba, out_format, out_is_device_ptr, true, out_depth, out_normal);
 }
 
 bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {

@@ -33,6 +33,14 @@ struct FrameConsts {
     uint32_t aux;               // bgs_render_aux: the projection also emits the Depth and Normal colour sources
 };
 
+// bgs_render_extras as the Classification / OpticalFlow projection reads it.  Only project_modes_kernel takes it (as an
+// argument of its own), so the arguments and code of every other kernel stay what they were.
+struct ModeConsts {
+    float prev_clip_from_world[16];   // the view's clip_from_world of the previous frame (column-major)
+    float delta_time;                 // > 0, finite
+    uint32_t num_classes;             // > 0
+};
+
 // Projected splat record, 48 B, stored by front-to-back rank.
 struct __align__(16) SplatRec {
     float cx, cy, ux, uy;       // centre (px), first row of the pixel-offset -> uv map

@@ -26,7 +26,8 @@ void launch_repack(bool f16, const void* pos, const void* sh, const void* rot, c
                    cudaStream_t stream);
 void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
-                    const float* cutoff_tab, float4* aux, cudaStream_t stream);
+                    const float* cutoff_tab, float4* aux, const ModeConsts* modes /* null: project_kernel */,
+                    cudaStream_t stream);
 void launch_cutoff_table(float* tab, cudaStream_t stream);
 // bin.cu
 int bin_coop_blocks_per_sm();

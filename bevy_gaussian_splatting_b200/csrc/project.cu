@@ -453,6 +453,74 @@ __device__ __forceinline__ void position_colour(const FrameConsts& fc, const flo
     for (int cc = 0; cc < 3; ++cc) rgb[cc] = (pw[cc] - fc.aabb_min[cc]) / (fc.aabb_max[cc] - fc.aabb_min[cc]);
 }
 
+// bevy_render::maths' FRAC_PI_3 and PI_2, rounded to f32
+constexpr float FRAC_PI_3_F = 1.0471975512f;
+constexpr float PI_2_F = 6.28318530718f;
+
+// bevy_render::color_operations::hsv_to_rgb: k = (vec3(5, 3, 1) + h / FRAC_PI_3) % 6.0 with WGSL's f32 remainder
+// x - y * trunc(x / y), then rgb = v - v * s * max(0, min(k, min(4 - k, 1))); every step rounded, in this order
+__device__ __forceinline__ void hsv_to_rgb(float h, float s, float v, float rgb[3]) {
+    const float hk = h / FRAC_PI_3_F, vs = v * s;
+    const float base[3] = {5.0f, 3.0f, 1.0f};
+#pragma unroll
+    for (int cc = 0; cc < 3; ++cc) {
+        const float x = base[cc] + hk;
+        const float k = x - 6.0f * truncf(x / 6.0f);
+        rgb[cc] = v - vs * fmaxf(0.0f, fminf(k, fminf(4.0f - k, 1.0f)));
+    }
+}
+
+// Fixed-series atan2 in f64 (the policy replacement for WGSL atan2, optical_flow.wgsl), shared with the oracle:
+// t = min(|x|, |y|) / max(|x|, |y|) in [0, 1]; above tan(pi/8), atan t = pi/4 + atan((t - 1) / (t + 1)); atan u =
+// u P(u^2) by 22 odd terms (|u| <= tan(pi/8): remainder < 3e-18); then the octant and quadrant by |y| > |x| and the
+// signs of x and y (IEEE atan2's values at zeros and infinities), rounded to f32.
+__device__ __forceinline__ float det_atan2(float yf, float xf) {
+    if (yf != yf || xf != xf) return __uint_as_float(0x7FC00000u);
+    const double ay = fabs((double)yf), ax = fabs((double)xf);
+    const bool steep = ay > ax;
+    double t;
+    if (ax == ay) t = ax == 0.0 ? 0.0 : 1.0;           // 0 / 0 and inf / inf
+    else t = steep ? __ddiv_rn(ax, ay) : __ddiv_rn(ay, ax);
+    double base = 0.0, u = t;
+    if (t > 0.41421356237309503) { base = 0.7853981633974483; u = __ddiv_rn(__dsub_rn(t, 1.0), __dadd_rn(t, 1.0)); }
+    const double z = __dmul_rn(u, u);
+    double p = -1.0 / 43.0;
+#pragma unroll
+    for (int k = 20; k >= 0; --k) p = __dadd_rn(__dmul_rn(p, z), (k & 1 ? -1.0 : 1.0) / (double)(2 * k + 1));
+    double r = __dadd_rn(base, __dmul_rn(u, p));
+    if (steep) r = __dsub_rn(1.5707963267948966, r);
+    if (__float_as_uint(xf) >> 31) r = __dsub_rn(3.141592653589793, r);
+    if (__float_as_uint(yf) >> 31) r = -r;
+    return (float)r;   // cvt.rn.f32.f64
+}
+
+// RasterizeMode::Classification (gaussian.wgsl:315-328, material/classification.wgsl:9-27): rgb holds the Color-mode
+// colour (sRGB decode included); a visibility lane >= 2 mixes it half and half with the hue of class vis - 2
+__device__ __forceinline__ void class_colour(const ModeConsts& mc, float vis, float rgb[3]) {
+    if (vis < 2.0f) return;   // (a NaN lane takes the hue path, as in the reference)
+    const float hue = ((vis - 2.0f) / (float)mc.num_classes) * 6.283185307f;
+    float h[3];
+    hsv_to_rgb(hue, 1.0f, 1.0f, h);
+#pragma unroll
+    for (int cc = 0; cc < 3; ++cc) rgb[cc] = rgb[cc] * (1.0f - 0.5f) + h[cc] * 0.5f;   // mix(sh, hue, 0.5)
+}
+
+// RasterizeMode::OpticalFlow (gaussian.wgsl:201,369-375, material/optical_flow.wgsl:16-53): the screen motion of the
+// transformed position pw between the previous and this clip_from_world, per second, as hue = direction and
+// saturation = speed (clamped to 1)
+__device__ __forceinline__ void flow_colour(const FrameConsts& fc, const ModeConsts& mc, const float pw[3], float rgb[3]) {
+    float c[4], cp[4];
+    mat4_point(fc.clip_from_world, pw[0], pw[1], pw[2], c);
+    mat4_point(mc.prev_clip_from_world, pw[0], pw[1], pw[2], cp);
+    const float mvx = (c[0] / c[3] - cp[0] / cp[3]) * 0.5f;
+    const float mvy = (c[1] / c[3] - cp[1] / cp[3]) * -0.5f;
+    const float fx = mvx / mc.delta_time, fy = mvy / mc.delta_time;
+    const float radius = sqrtf(fx * fx + fy * fy);
+    float angle = det_atan2(fy, fx);
+    if (angle < 0.0f) angle = angle + PI_2_F;
+    hsv_to_rgb(angle, fminf(fmaxf(radius, 0.0f), 1.0f), 1.0f, rgb);
+}
+
 // DrawMode::HighlightSelected (gaussian.wgsl:423-427): a selected splat is drawn opaque and green in every colour source
 __device__ __forceinline__ void highlight_selected(SplatRec& rec, float drgb[3], float nrgb[3]) {
     rec.r = 0.3f; rec.g = 1.0f; rec.b = 0.1f; rec.op = 1.0f;
@@ -469,12 +537,13 @@ __device__ __forceinline__ void store_rec(SplatRec* __restrict__ dst, const Spla
 
 // One entry of the index list -> the 48 B record at recs[r] (+ the 2DGS extra record and the aux colours).  An
 // undrawn gaussian (outside the frustum, or unselected under DrawMode::Selected) gets an empty bbox and no colour.
-template <bool F16>
+// MODES2: the Classification / OpticalFlow colour sources (project_modes_kernel) instead of the four others.
+template <bool F16, bool MODES2>
 __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCounters* __restrict__ ctr, uint32_t r,
                                             float4 p4, const float q[4], const float so[4], const float sh[48],
                                             const float* __restrict__ cutoff_tab, uint32_t op_bits,
                                             SplatRec* __restrict__ recs, float4* __restrict__ extra,
-                                            float4* __restrict__ aux) {
+                                            float4* __restrict__ aux, const ModeConsts& mc) {
     SplatRec rec;
     rec.ux = 0.f; rec.uy = 0.f; rec.vx = 0.f; rec.vy = 0.f;
     rec.bx = BBOX_EMPTY; rec.by = BBOX_EMPTY;
@@ -513,14 +582,24 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
         // a splat do not depend on the mode)
         const uint32_t mode = fc.rasterize_mode;
         float rgb[3] = {0.f, 0.f, 0.f}, drgb[3] = {0.f, 0.f, 0.f}, nrgb[3] = {0.f, 0.f, 0.f};
-        if (mode == BGS_RASTERIZE_COLOR) sh_colour(fc, A, pw, sh, rgb);
-        if (mode == BGS_RASTERIZE_POSITION) position_colour(fc, pw, rgb);
-        if (mode == BGS_RASTERIZE_DEPTH || fc.aux) depth_colour(fc, ctr, pw, drgb);
-        if (mode == BGS_RASTERIZE_NORMAL || fc.aux) normal_colour(fc, A, Rm, sc, nrgb);
-        const bool depth = mode == BGS_RASTERIZE_DEPTH, normal = mode == BGS_RASTERIZE_NORMAL;
-        rec.r = depth ? drgb[0] : normal ? nrgb[0] : rgb[0];
-        rec.g = depth ? drgb[1] : normal ? nrgb[1] : rgb[1];
-        rec.b = depth ? drgb[2] : normal ? nrgb[2] : rgb[2];
+        if constexpr (MODES2) {
+            if (mode == BGS_RASTERIZE_CLASSIFICATION) {
+                sh_colour(fc, A, pw, sh, rgb);
+                class_colour(mc, p4.w, rgb);
+            } else {
+                flow_colour(fc, mc, pw, rgb);
+            }
+            rec.r = rgb[0]; rec.g = rgb[1]; rec.b = rgb[2];
+        } else {
+            if (mode == BGS_RASTERIZE_COLOR) sh_colour(fc, A, pw, sh, rgb);
+            if (mode == BGS_RASTERIZE_POSITION) position_colour(fc, pw, rgb);
+            if (mode == BGS_RASTERIZE_DEPTH || fc.aux) depth_colour(fc, ctr, pw, drgb);
+            if (mode == BGS_RASTERIZE_NORMAL || fc.aux) normal_colour(fc, A, Rm, sc, nrgb);
+            const bool depth = mode == BGS_RASTERIZE_DEPTH, normal = mode == BGS_RASTERIZE_NORMAL;
+            rec.r = depth ? drgb[0] : normal ? nrgb[0] : rgb[0];
+            rec.g = depth ? drgb[1] : normal ? nrgb[1] : rgb[1];
+            rec.b = depth ? drgb[2] : normal ? nrgb[2] : rgb[2];
+        }
         if (fc.draw_mode == BGS_DRAW_HIGHLIGHT_SELECTED && p4.w > 0.5f) highlight_selected(rec, drgb, nrgb);
         if (fc.aux && aux != nullptr) {
             aux[(size_t)r * 2] = make_float4(drgb[0], drgb[1], drgb[2], 0.0f);
@@ -546,7 +625,25 @@ project_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ ind
         const bool need_sh = fc.rasterize_mode == BGS_RASTERIZE_COLOR;
         uint32_t op_bits = 0u;
         const float4 p4 = Attr<F16>::load(blocks, id, sh, q, so, need_sh, &op_bits);
-        project_one<F16>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux);
+        project_one<F16, false>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, ModeConsts{});
+    }
+}
+
+// project_kernel for RasterizeMode::Classification / OpticalFlow (bgs_render_ex): the same records but for r, g, b.  A
+// kernel of its own, so that project_kernel's mode branch (and its 80-register budget) stays as it is.
+template <bool F16>
+__global__ void __launch_bounds__(128, PROJ_MIN_CTAS)
+project_modes_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
+                     const FrameCounters* __restrict__ ctr, FrameConsts fc, ModeConsts mc, SplatRec* __restrict__ recs,
+                     float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
+    const uint32_t n_vis = ctr->n_vis;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_vis; r += gridDim.x * blockDim.x) {
+        const uint32_t id = by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r));
+        float sh[48], q[4], so[4];
+        const bool need_sh = fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION;   // OpticalFlow reads the position only
+        uint32_t op_bits = 0u;
+        const float4 p4 = Attr<F16>::load(blocks, id, sh, q, so, need_sh, &op_bits);
+        project_one<F16, true>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, nullptr, mc);
     }
 }
 
@@ -557,12 +654,17 @@ void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_pa
 
 void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
-                    const float* cutoff_tab, float4* aux, cudaStream_t stream) {
+                    const float* cutoff_tab, float4* aux, const ModeConsts* modes, cudaStream_t stream) {
     // per-thread gather.  Grid sized from a hint (last frame's visible count + head-room); the grid-stride loop keeps
     // any n_vis correct.
     uint32_t grid = (n_hint + 127) / 128;
     if (grid > 65535u * 8u) grid = 65535u * 8u;
     if (grid < (uint32_t)sm_count) grid = (uint32_t)sm_count;
+    if (modes) {   // Classification / OpticalFlow (no aux outputs)
+        if (f16) project_modes_kernel<true><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
+        else project_modes_kernel<false><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
+        return;
+    }
     if (f16) project_kernel<true><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
     else project_kernel<false><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
 }

@@ -162,31 +162,44 @@ class GaussianSplattingPlugin:
     def render_view(self, handle: PlanarGaussian3dHandle, settings: CloudSettings, view: View,
                     camera: GaussianCamera | None = None, transform: CloudTransform | None = None,
                     fmt: str = "rgba32f", out: np.ndarray | None = None, to_host: bool = True,
-                    asynchronous: bool = False, premultiplied: bool = False, blend_over: bool = False):
+                    asynchronous: bool = False, premultiplied: bool = False, blend_over: bool = False,
+                    previous_view: View | None = None, delta_time: float | None = None):
         """Returns the (H, W, 4) frame (host) or None when `to_host` is False / the camera is warming up.
         `asynchronous`: only enqueue the frame (BGS_FLAG_ASYNC); call `sync()` before reading anything.
         `premultiplied`: the splat layer alone, (C, 1 - T) (BGS_FLAG_PREMULTIPLIED_OUT).  `blend_over`: blend over what
         the context's frame already holds -- the previous call's result (BGS_FLAG_BLEND_OVER_TARGET): one call per
-        cloud, far cloud first, like the reference's Transparent3d items (render/mod.rs:398-452, :944-948)."""
+        cloud, far cloud first, like the reference's Transparent3d items (render/mod.rs:398-452, :944-948).
+        `previous_view` / `delta_time`: RasterizeMode.OpticalFlow's camera of the previous frame and the seconds since
+        it (the other modes ignore them); RasterizeMode.Classification reads `settings.num_classes`."""
         if camera is not None and camera.warmup:   # queue_gaussians skips warm-up cameras (render/mod.rs:361-371)
             return None
         code, dtype, ch = self.FORMATS[fmt]
         v = view.to_abi()
-        u, s = self._uniform_and_settings(handle, settings, transform, asynchronous, premultiplied, blend_over)
+        u, s, ex = self._call_args(handle, settings, transform, asynchronous, premultiplied, blend_over, previous_view, delta_time)
         if to_host:
             if out is None:
                 out = np.empty((view.height, view.width, ch), dtype)
             assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
-            st = self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), _ptr(out), code, 0)
+        target = _ptr(out) if to_host else None
+        if ex is None:
+            st = self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), target, code, 0)
         else:
-            st = self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), None, code, 0)
+            st = self._lib.bgs_render_ex(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.byref(ex), target, code, 0)
         self._check(st)
         return out if to_host else None
 
     def _uniform_and_settings(self, handle, settings, transform, asynchronous=False, premultiplied=False, blend_over=False):
-        """The two ABI structs of a call; cached while (settings, transform, cloud, flags) repeat from frame to frame."""
+        """The uniform and settings structs of a call (see `_call_args`)."""
+        return self._call_args(handle, settings, transform, asynchronous, premultiplied, blend_over)[:2]
+
+    def _call_args(self, handle, settings, transform, asynchronous=False, premultiplied=False, blend_over=False,
+                   previous_view=None, delta_time=None):
+        """The uniform, settings and extras of a call; cached while (settings, transform, cloud, flags, extras) repeat
+        from frame to frame.  The extras are None -- bgs_render, i.e. bgs_render_ex's NULL -- when they would say what NULL
+        says: no previous view and num_classes = 1."""
+        prev = None if previous_view is None else bytes(previous_view.to_abi().clip_from_world)
         key = (dataclasses.astuple(settings), None if transform is None else transform.matrix.tobytes(), asynchronous, handle.serial,
-               premultiplied, blend_over)
+               premultiplied, blend_over, prev, delta_time)
         if getattr(self, "_us_cache", (None,))[0] != key:
             s_ = settings.to_abi()
             if asynchronous:
@@ -195,8 +208,14 @@ class GaussianSplattingPlugin:
                 s_.flags |= abi.BGS_FLAG_PREMULTIPLIED_OUT
             if blend_over:
                 s_.flags |= abi.BGS_FLAG_BLEND_OVER_TARGET
-            self._us_cache = (key, self.cloud_uniform(settings, transform, handle.aabb), s_)
-        return self._us_cache[1], self._us_cache[2]
+            ex = None
+            if prev is not None or settings.num_classes != 1:
+                ex = abi.bgs_render_extras(num_classes=int(settings.num_classes))
+                if prev is not None:
+                    ex.previous_clip_from_world[:] = previous_view.to_abi().clip_from_world[:]
+                    ex.delta_time = float(delta_time) if delta_time is not None else 0.0
+            self._us_cache = (key, self.cloud_uniform(settings, transform, handle.aabb), s_, ex)
+        return self._us_cache[1], self._us_cache[2], self._us_cache[3]
 
     def render_view_aux(self, handle: PlanarGaussian3dHandle, settings: CloudSettings, view: View,
                         transform: CloudTransform | None = None, fmt: str = "rgba32f"):
@@ -213,15 +232,20 @@ class GaussianSplattingPlugin:
 
     def render_view_to_device(self, handle: PlanarGaussian3dHandle, settings: CloudSettings, view: View, device_ptr: int,
                               transform: CloudTransform | None = None, fmt: str = "rgba8_srgb", asynchronous: bool = False,
-                              premultiplied: bool = False, blend_over: bool = False) -> None:
+                              premultiplied: bool = False, blend_over: bool = False, previous_view: View | None = None,
+                              delta_time: float | None = None) -> None:
         """Render straight into caller-owned device memory: an exported frame target (`bgs_frame_export_create`), or
         another GPU's memory mapped into this process (`bgs_peer_buffer_open`) -- the blend kernel's pixel stores then
         travel over NVLink themselves.  The target must be aligned to one pixel (4 / 8 / 16 bytes).  `premultiplied` /
-        `blend_over` as in `render_view`; blend-over reads what `device_ptr` holds."""
+        `blend_over`, `previous_view` and `delta_time` as in `render_view`; blend-over reads what `device_ptr` holds."""
         code, _, _ = self.FORMATS[fmt]
         v = view.to_abi()
-        u, s = self._uniform_and_settings(handle, settings, transform, asynchronous, premultiplied, blend_over)
-        self._check(self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.c_void_p(device_ptr), code, 1))
+        u, s, ex = self._call_args(handle, settings, transform, asynchronous, premultiplied, blend_over, previous_view, delta_time)
+        if ex is None:
+            self._check(self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.c_void_p(device_ptr), code, 1))
+        else:
+            self._check(self._lib.bgs_render_ex(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.byref(ex),
+                                                C.c_void_p(device_ptr), code, 1))
 
     def sync(self) -> bool:
         """Complete the frames enqueued with `asynchronous=True`.  False = the last frame must be rendered again

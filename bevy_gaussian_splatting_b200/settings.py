@@ -24,11 +24,13 @@ class GaussianMode(enum.IntEnum):  # settings.rs:17-22 (Gaussian4d is out of sco
     Gaussian3d = 1
 
 
-class RasterizeMode(enum.IntEnum):  # settings.rs:38-48 (Color/Depth/Normal/Position are on the path)
+class RasterizeMode(enum.IntEnum):  # settings.rs:38-48 (all but Velocity, which needs Gaussian4d, are on the path)
     Color = 0
     Depth = 1
     Normal = 2
     Position = 3
+    Classification = 4   # the hue of class vis - 2 from the visibility lane, CloudSettings.num_classes hues
+    OpticalFlow = 5      # camera motion since the previous view (render_view's previous_view / delta_time)
 
 
 class RadixSortDepthBits(enum.IntEnum):  # settings.rs:50-77

@@ -4,6 +4,7 @@
 //   headless [count=100000] [width=1920] [height=1080] [global_scale=1.0] [out=headless_output/0.ppm]
 //            [--dump-cloud file] [--raw file] [--remove-floaters radius]
 //            [--particles N --steps K --dt S [--dump-particles file]] [--interpolate SEED --time T]
+//            [--rasterize classification|optical-flow] [--num-classes K] [--prev-view dx,dy,dz]
 // --dump-cloud writes the four f32 planes (n, then pos_vis, sh, rot, scale_opacity) so another host can
 // render the identical cloud; --raw writes the RGBA8 frame bytes.  --remove-floaters selects the sparse gaussians
 // (SparseSelect with that radius), inverts the selection and draws only the rest (DrawMode::Selected), the
@@ -14,6 +15,9 @@
 // --interpolate blends the cloud (lhs) with random_gaussians_3d_seeded(count, SEED) (rhs) at time T of the window
 // [0, 1] into a third cloud, made as the subset of every gaussian of lhs, and draws that one (the reference's
 // GaussianInterpolate { lhs, rhs }); --dump-cloud then writes rhs's four planes after lhs's.
+// --rasterize picks RasterizeMode::Classification (labels: gaussian i gets visibility 2 + i % K, --num-classes K, default
+// 3) or OpticalFlow (the previous frame's camera is the headless camera moved by --prev-view, default 0.05,0,0, at
+// 1/60 s); the previous view's clip_from_world is printed as 16 hex words ("prev_clip: ...").
 #include <memory>
 #include <numeric>
 #include <cstdio>
@@ -32,6 +36,7 @@ int main(int argc, char** argv) {
     size_t n_particles = 0; int steps = 0; float dt = 1.0f / 60.0f;
     std::string dump_particles;
     long interp_seed = -1; float interp_time = 0.0f;
+    std::string rasterize = "color"; uint32_t num_classes = 3; float prev_off[3] = {0.05f, 0.0f, 0.0f};
     int pos = 0;
     for (int i = 1; i < argc; ++i) {
         const std::string a = argv[i];
@@ -44,6 +49,12 @@ int main(int argc, char** argv) {
         if (a == "--dump-particles" && i + 1 < argc) { dump_particles = argv[++i]; continue; }
         if (a == "--interpolate" && i + 1 < argc) { interp_seed = std::atol(argv[++i]); continue; }
         if (a == "--time" && i + 1 < argc) { interp_time = (float)std::atof(argv[++i]); continue; }
+        if (a == "--rasterize" && i + 1 < argc) { rasterize = argv[++i]; continue; }
+        if (a == "--num-classes" && i + 1 < argc) { num_classes = (uint32_t)std::strtoul(argv[++i], nullptr, 10); continue; }
+        if (a == "--prev-view" && i + 1 < argc) {
+            if (std::sscanf(argv[++i], "%f,%f,%f", &prev_off[0], &prev_off[1], &prev_off[2]) != 3) return 1;
+            continue;
+        }
         switch (pos++) {
             case 0: count = std::strtoull(a.c_str(), nullptr, 10); break;
             case 1: W = std::atoi(a.c_str()); break;
@@ -97,9 +108,36 @@ int main(int argc, char** argv) {
         }
         const bgs::PlanarGaussian3dHandle& drawn_cloud = blended ? *blended : handle;
         const bgs_view view = bgs::headless_view(W, H);
+        const float prev_eye[3] = {prev_off[0], 1.5f + prev_off[1], 5.0f + prev_off[2]};
+        const bgs_view prev_view = bgs::make_view(bgs::view_from_translation(prev_eye[0], prev_eye[1], prev_eye[2]),
+                                                  bgs::perspective_infinite_reverse_rh(3.14159265358979323846f / 4.0f,
+                                                                                       (float)W / (float)H, 0.1f),
+                                                  prev_eye, W, H);
+        if (rasterize == "classification") {
+            settings.rasterize_mode = bgs::RasterizeMode::Classification;
+            settings.num_classes = num_classes;
+            std::vector<float> labels(count);
+            for (size_t i = 0; i < count; ++i) labels[i] = 2.0f + (float)(i % num_classes);
+            bgs_cloud_visibility_set(plugin.context(), drawn_cloud.get(), labels.data());
+        } else if (rasterize == "optical-flow") {
+            settings.rasterize_mode = bgs::RasterizeMode::OpticalFlow;
+            std::printf("prev_clip:");
+            for (int k = 0; k < 16; ++k) {
+                uint32_t w;
+                std::memcpy(&w, &prev_view.clip_from_world[k], 4);
+                std::printf(" %08x", w);
+            }
+            std::printf("\n");
+        } else if (rasterize != "color") {
+            std::fprintf(stderr, "headless: --rasterize %s (color, classification or optical-flow)\n", rasterize.c_str());
+            return 1;
+        }
         std::vector<unsigned char> frame((size_t)W * H * 4);
         bool drawn = false;
-        for (int f = 0; f < 3; ++f) drawn = plugin.render_view(drawn_cloud, settings, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);
+        for (int f = 0; f < 3; ++f)
+            drawn = settings.rasterize_mode == bgs::RasterizeMode::OpticalFlow
+                        ? plugin.render_view(drawn_cloud, settings, view, prev_view, 1.0f / 60.0f, frame.data(), BGS_FORMAT_RGBA8_SRGB)
+                        : plugin.render_view(drawn_cloud, settings, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);
         const bgs_frame_stats fs = plugin.frame_stats();
         float us[6];
         bgs_stage_times_us(plugin.context(), us);

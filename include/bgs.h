@@ -58,7 +58,10 @@ typedef struct {
 
 /* CloudSettings / CloudPipelineKey (src/gaussian/settings.rs:90-133, render/mod.rs:898-909). */
 enum { BGS_GAUSSIAN_2D = 0, BGS_GAUSSIAN_3D = 1 };
-enum { BGS_RASTERIZE_COLOR = 0, BGS_RASTERIZE_DEPTH = 1, BGS_RASTERIZE_NORMAL = 2, BGS_RASTERIZE_POSITION = 3 };
+enum {
+    BGS_RASTERIZE_COLOR = 0, BGS_RASTERIZE_DEPTH = 1, BGS_RASTERIZE_NORMAL = 2, BGS_RASTERIZE_POSITION = 3,
+    BGS_RASTERIZE_CLASSIFICATION = 4, BGS_RASTERIZE_OPTICAL_FLOW = 5   /* bgs_render_ex; Velocity (6) is out of scope */
+};
 enum { BGS_DRAW_ALL = 0, BGS_DRAW_SELECTED = 1, BGS_DRAW_HIGHLIGHT_SELECTED = 2 };
 enum {
     BGS_FLAG_SORT_ALL = 1u, /* sort all N entries like the reference (culled keyed 0xFFFFFFFF)
@@ -361,6 +364,52 @@ bgs_status bgs_render(bgs_context* ctx, const bgs_cloud* cloud, const bgs_view* 
 bgs_status bgs_render_aux(bgs_context* ctx, const bgs_cloud* cloud, const bgs_view* view,
                           const bgs_cloud_uniform* uniform, const bgs_settings* settings, void* out_rgba,
                           void* out_depth, void* out_normal, uint32_t out_format, int out_is_device_ptr);
+
+/* What a frame needs beyond bgs_render's arguments for RasterizeMode::Classification and OpticalFlow. */
+typedef struct {
+    float previous_clip_from_world[16]; /* OpticalFlow: this view's clip_from_world of the previous frame
+                                           (PreviousViewUniforms.clip_from_world), column-major */
+    float delta_time;                   /* OpticalFlow: seconds since that frame (Bevy's globals.delta_time) */
+    uint32_t num_classes;               /* Classification: CloudSettings.num_classes (CloudUniform.num_classes) */
+} bgs_render_extras;
+
+/* bgs_render with extras: the one call that renders RasterizeMode::Classification and OpticalFlow.  bgs_render is this
+ * call with extras == NULL, which means num_classes = 1 and no previous view; the four other modes ignore extras.
+ * Both modes change only the colour a splat gets in the vertex stage (gaussian.wgsl:312-421): geometry, opacity,
+ * coverage, sort order and blending are those of Color mode, and so are every geometry, layout, draw mode, output format
+ * and flag they accept.
+ *
+ * The rule, exactly (f32, every step rounded, in the order written):
+ *   Classification (gaussian.wgsl:315-328, material/classification.wgsl:9-27): sh = the Color-mode colour (the SH-3
+ *     evaluation along the camera ray, sRGB -> linear decoded when color_space == 0: the decode is part of get_color,
+ *     planar.wgsl:92-96, so it applies to sh and not to the hue); vis = the gaussian's visibility lane.  vis < 2: sh.
+ *     Else hue = ((vis - 2) / f32(num_classes)) * 6.283185307 and the colour is mix(sh, hsv_to_rgb(hue, 1, 1), 0.5) =
+ *     sh * (1 - 0.5) + rgb * 0.5.  vis is not floored (fractional labels give in-between hues) and a NaN vis takes the
+ *     hue path, as in the reference.  An app labels gaussian i with class k by writing 2 + k into its visibility lane
+ *     (bgs_cloud_visibility_set).
+ *   OpticalFlow (gaussian.wgsl:201,369-375, material/optical_flow.wgsl:16-53): p = the transformed position (model * pos);
+ *     the reference's previous position is the same p, so the colour shows camera motion only (particles and
+ *     interpolation do not show).  c = clip_from_world (p, 1), c' = previous_clip_from_world (p, 1);
+ *     mv = (c.xy / c.w - c'.xy / c'.w) * (0.5, -0.5); flow = mv / delta_time; radius = sqrt(flow.x^2 + flow.y^2);
+ *     angle = atan2(flow.y, flow.x), + PI_2 when angle < 0; rgb = hsv_to_rgb(angle, clamp(radius, 0, 1), 1).
+ *   hsv_to_rgb(h, s, v) (bevy_render::color_operations): k = (vec3(5, 3, 1) + h / FRAC_PI_3) % 6 with WGSL's f32
+ *     remainder x - 6 * trunc(x / 6) (not fmodf); rgb = v - v * s * max(0, min(k, min(4 - k, 1))).  FRAC_PI_3 =
+ *     1.0471975512 and PI_2 = 6.28318530718 (bevy_render::maths) rounded to f32.  The formula and the constants are
+ *     restated from Bevy's source and its cited formula (Wikipedia, "HSV to RGB alternative"): parity unpinned, as f16
+ *     rounding is.
+ *   FP policy: min / max / clamp ignore a NaN operand (fminf / fmaxf); atan2 is a fixed f64 series rounded to f32
+ *     (IEEE atan2's values at zeros and infinities: atan2(+-0, +0) = +-0, atan2(+-0, -0) = +-pi), so OpticalFlow colours
+ *     are bit-exact against the oracle; Classification keeps Color mode's tolerance on sh, halved by the mix.
+ *   DrawMode::HighlightSelected still paints every gaussian with vis > 0.5 green, labelled ones included
+ *     (gaussian.wgsl:423-427); DrawMode::Selected still drops vis < 0.5.
+ * Where this port deliberately differs from the reference (each BGS_EINVAL; a refused call changes and enqueues nothing):
+ *   1. Classification with num_classes == 0 (the reference divides by zero).
+ *   2. OpticalFlow without extras, with a delta_time that is not finite and > 0, or with a non-finite entry of
+ *      previous_clip_from_world.
+ *   3. Either mode through bgs_render_aux, which takes no extras. */
+bgs_status bgs_render_ex(bgs_context* ctx, const bgs_cloud* cloud, const bgs_view* view,
+                         const bgs_cloud_uniform* uniform, const bgs_settings* settings,
+                         const bgs_render_extras* extras, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
 
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a

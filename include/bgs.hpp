@@ -25,7 +25,7 @@ namespace bgs {
 
 enum class DrawMode : uint32_t { All = 0, Selected = 1, HighlightSelected = 2 };
 enum class GaussianMode : uint32_t { Gaussian2d = 0, Gaussian3d = 1 };
-enum class RasterizeMode : uint32_t { Color = 0, Depth = 1, Normal = 2, Position = 3 };
+enum class RasterizeMode : uint32_t { Color = 0, Depth = 1, Normal = 2, Position = 3, Classification = 4, OpticalFlow = 5 };
 enum class RadixSortDepthBits : uint32_t { Bits16 = 16, Bits24 = 24, Bits32 = 32 };
 enum class GaussianColorSpace : uint32_t { SrgbRec709Display = 0, LinRec709Display = 1 };
 
@@ -39,6 +39,7 @@ struct CloudSettings {   // src/gaussian/settings.rs:110-133 (defaults)
     GaussianMode gaussian_mode = GaussianMode::Gaussian3d;
     RasterizeMode rasterize_mode = RasterizeMode::Color;
     GaussianColorSpace color_space = GaussianColorSpace::SrgbRec709Display;
+    uint32_t num_classes = 1;   // RasterizeMode::Classification's hue count (CloudUniform.num_classes)
     float time = 0.0f;
     float time_start = 0.0f;   // the interpolation window (GaussianSplattingPlugin::interpolate)
     float time_stop = 1.0f;
@@ -259,7 +260,28 @@ public:
         bgs_cloud_uniform u = cloud_uniform(settings);
         std::memcpy(u.aabb_min, cloud.aabb_min(), 12); std::memcpy(u.aabb_max, cloud.aabb_max(), 12);
         const bgs_settings s = settings.to_abi(extra_flags);
-        const bgs_status st = bgs_render(ctx_, cloud.get(), &view, &u, &s, out_rgba, format, out_is_device ? 1 : 0);
+        bgs_render_extras ex{};   // Classification's num_classes; no previous view (OpticalFlow takes the overload below)
+        ex.num_classes = settings.num_classes;
+        const bgs_status st = bgs_render_ex(ctx_, cloud.get(), &view, &u, &s,
+                                            settings.rasterize_mode == RasterizeMode::OpticalFlow ? nullptr : &ex, out_rgba,
+                                            format, out_is_device ? 1 : 0);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
+    // RasterizeMode::OpticalFlow needs the view's previous frame: its clip_from_world and the seconds since
+    // (bgs_render_ex); RasterizeMode::Classification reads settings.num_classes.
+    bool render_view(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view,
+                     const bgs_view& previous_view, float delta_time, void* out_rgba, uint32_t format = BGS_FORMAT_RGBA8_SRGB,
+                     bool out_is_device = false, uint32_t extra_flags = 0) {
+        bgs_cloud_uniform u = cloud_uniform(settings);
+        std::memcpy(u.aabb_min, cloud.aabb_min(), 12); std::memcpy(u.aabb_max, cloud.aabb_max(), 12);
+        const bgs_settings s = settings.to_abi(extra_flags);
+        bgs_render_extras ex{};
+        std::memcpy(ex.previous_clip_from_world, previous_view.clip_from_world, 64);
+        ex.delta_time = delta_time;
+        ex.num_classes = settings.num_classes;
+        const bgs_status st = bgs_render_ex(ctx_, cloud.get(), &view, &u, &s, &ex, out_rgba, format, out_is_device ? 1 : 0);
         if (st == BGS_NOT_READY) return false;
         check(st);
         return true;
