@@ -63,24 +63,56 @@ __device__ __forceinline__ void make_bbox(float cx, float cy, float hx, float hy
     bx = pack_bbox(x0, x1); by = pack_bbox(y0, y1);
 }
 
-// Attribute fetch from the library-owned gaussian-major copy made once at upload -- f16: 128 B = one cache line per
+// Attributes live in the library-owned gaussian-major copy made once at upload -- f16: 128 B = one cache line per
 // gaussian (pos | rot/scale/opacity | sh x 6), f32: 256 B (pos | rot | scale_opacity | sh x 12 | pad) -- so the random
 // gather of a visible splat touches exactly its own line(s) instead of 3-4 partially used ones of the reference's
 // planes (the position plane stays planar for key-gen).
+//
+// A warp gathers the blocks of 32 consecutive entries of the index list into its own shared-memory stage with
+// coalesced 16 B asynchronous copies (cp.async.cg: no staging registers, L1 bypassed, every line is used once): a
+// lane's copy k moves piece (32 k + lane) % NP of entry (32 k + lane) / NP, so NP consecutive lanes read one block
+// front to back.  NP = CH (the whole block) when the colour source reads the SH coefficients, else GEO pieces:
+// position, rotation, scale and opacity (f32: plus the first SH piece, which shares scale_opacity's 32 B sector).
+// Piece p of entry g sits at 16 B unit g * CH + (p ^ (g & 7)): the eight lanes of a quarter warp that read the same
+// piece of their own entries hit eight different 16 B bank groups, and so do the copies' stores.
+__device__ __forceinline__ void cp_async16(uint4* dst_shared, const uint4* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_shared)), "l"(src)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+template <int CH, int NP>
+__device__ __forceinline__ void gather_blocks(const uint4* __restrict__ blocks, uint32_t id, uint32_t n_valid,
+                                              uint4* stage, int lane) {
+    static_assert(32 % NP == 0 && NP <= CH, "NP lanes per block");
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+        const int g = (32 * k + lane) / NP, p = lane % NP;
+        const uint32_t gid = __shfl_sync(0xFFFFFFFFu, id, g);
+        if ((uint32_t)g < n_valid) cp_async16(stage + g * CH + (p ^ (g & 7)), blocks + (size_t)gid * CH + p);
+    }
+}
+
+// entry g's attributes out of a stage
 template <bool F16>
 struct Attr;
 template <>
 struct Attr<false> {
-    __device__ static float4 load(const void* blocks, uint32_t id, float* sh, float q[4], float so[4], bool need_sh,
-                                  uint32_t* = nullptr) {
-        const float4* b = reinterpret_cast<const float4*>(blocks) + (size_t)id * 16;
-        const float4 p = __ldg(b), r = __ldg(b + 1), s = __ldg(b + 2);
+    static constexpr int CH = 16, GEO = 4;
+    __device__ static float4 load(const uint4* stage, int g, float* sh, float q[4], float so[4], bool need_sh, uint32_t&) {
+        auto piece = [&](int p) {
+            const uint4 v = stage[g * CH + (p ^ (g & 7))];
+            return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
+        };
+        const float4 p = piece(0), r = piece(1), s = piece(2);
         q[0] = r.x; q[1] = r.y; q[2] = r.z; q[3] = r.w;
         so[0] = s.x; so[1] = s.y; so[2] = s.z; so[3] = s.w;
         if (need_sh) {
 #pragma unroll
             for (int i = 0; i < 12; ++i) {
-                const float4 v = __ldg(b + 3 + i);
+                const float4 v = piece(3 + i);
                 sh[4 * i] = v.x; sh[4 * i + 1] = v.y; sh[4 * i + 2] = v.z; sh[4 * i + 3] = v.w;
             }
         }
@@ -89,19 +121,20 @@ struct Attr<false> {
 };
 template <>
 struct Attr<true> {
+    static constexpr int CH = 8, GEO = 2;
     __device__ static float lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu))); }
     __device__ static float hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
-    __device__ static float4 load(const void* blocks, uint32_t id, float* sh, float q[4], float so[4], bool need_sh,
-                                  uint32_t* op_bits = nullptr) {
-        const uint4* b = reinterpret_cast<const uint4*>(blocks) + (size_t)id * 8;
-        const uint4 pw = __ldg(b), w = __ldg(b + 1);
-        if (op_bits) *op_bits = w.w & 0xFFFFu;
+    __device__ static float4 load(const uint4* stage, int g, float* sh, float q[4], float so[4], bool need_sh,
+                                  uint32_t& op_bits) {
+        auto piece = [&](int p) { return stage[g * CH + (p ^ (g & 7))]; };
+        const uint4 pw = piece(0), w = piece(1);
+        op_bits = w.w & 0xFFFFu;
         q[0] = hi(w.x); q[1] = lo(w.x); q[2] = hi(w.y); q[3] = lo(w.y);
         so[0] = hi(w.z); so[1] = lo(w.z); so[2] = hi(w.w); so[3] = lo(w.w);
         if (need_sh) {
 #pragma unroll
             for (int i = 0; i < 6; ++i) {
-                const uint4 v = __ldg(b + 2 + i);
+                const uint4 v = piece(2 + i);
                 sh[8 * i] = lo(v.x); sh[8 * i + 1] = hi(v.x); sh[8 * i + 2] = lo(v.y); sh[8 * i + 3] = hi(v.y);
                 sh[8 * i + 4] = lo(v.z); sh[8 * i + 5] = hi(v.z); sh[8 * i + 6] = lo(v.w); sh[8 * i + 7] = hi(v.w);
             }
@@ -609,42 +642,76 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
     store_rec(recs + r, rec);
 }
 
-constexpr int PROJ_MIN_CTAS = 6;
+// 128 threads at up to 128 registers (no spills).  Beside the depth sort an SM has shared memory for one such CTA, so
+// a tighter register bound buys no occupancy there, and with several frames in flight fewer, fatter CTAs measured
+// faster than 6 or 8 per SM (DESIGN.md section 9).
+constexpr int PROJ_THREADS = 128, PROJ_WARPS = PROJ_THREADS / 32, PROJ_MIN_CTAS = 4;
+
+// The projection loop of both kernels.  Record r of n_vis is entry r of the index list:
+//   by_slot: r is a compact slot (ascending gaussian index; runs concurrently with the depth sort)
+//   else   : r is a front-to-back rank, the list is the far->near sorted index list
+// The grid is persistent and each warp strides over groups of 32 entries with two groups in flight: once the lanes
+// hold group i's attributes in registers, the copies of group i + 1 start filling the warp's stage and the list
+// entries of group i + 2 are on their way into a register, so both dependent memory latencies sit under project_one.
+template <bool F16, bool MODES2>
+__device__ __forceinline__ void project_groups(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list,
+                                               int by_slot, const FrameCounters* __restrict__ ctr, const FrameConsts& fc,
+                                               bool need_sh, SplatRec* __restrict__ recs, float4* __restrict__ extra,
+                                               const float* __restrict__ cutoff_tab, float4* __restrict__ aux,
+                                               const ModeConsts& mc) {
+    constexpr int CH = Attr<F16>::CH;
+    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * CH];   // f16 16 KB, f32 32 KB
+    const int lane = threadIdx.x & 31;
+    uint4* const stage = s_stages[threadIdx.x >> 5];
+    const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
+    auto list_id = [&](uint32_t r) {
+        return r < n_vis ? (by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r))) : 0u;
+    };
+    auto gather = [&](uint32_t r0, uint32_t id) {   // one commit group per call, empty past the list's end
+        const uint32_t n_valid = r0 < n_vis ? n_vis - r0 : 0u;
+        const uint4* b = reinterpret_cast<const uint4*>(blocks);
+        if (need_sh) gather_blocks<CH, CH>(b, id, n_valid, stage, lane);
+        else gather_blocks<CH, Attr<F16>::GEO>(b, id, n_valid, stage, lane);
+        cp_async_commit();
+    };
+    uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
+    gather(r0, list_id(r0 + lane));
+    uint32_t id_next = list_id(r0 + stride + lane);
+    for (; r0 < n_vis; r0 += stride) {
+        cp_async_wait<0>();
+        __syncwarp();   // every lane's copies of this group have landed
+        const uint32_t r = r0 + lane;
+        float sh[48], q[4], so[4];
+        uint32_t op_bits = 0u;
+        float4 p4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (r < n_vis) p4 = Attr<F16>::load(stage, lane, sh, q, so, need_sh, op_bits);
+        __syncwarp();   // the stage is read out before the next group's copies overwrite it
+        gather(r0 + stride, id_next);
+        id_next = list_id(r0 + 2u * stride + lane);
+        if (r < n_vis) project_one<F16, MODES2>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc);
+    }
+}
+
 template <bool F16>
-__global__ void __launch_bounds__(128, PROJ_MIN_CTAS)
+__global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
                const FrameCounters* __restrict__ ctr, FrameConsts fc, SplatRec* __restrict__ recs,
                float4* __restrict__ extra /* 4 x float4 per record, 2DGS + USE_AABB only */, const float* __restrict__ cutoff_tab,
                float4* __restrict__ aux /* 2 x float4 per record (depth rgb, normal rgb), bgs_render_aux only */) {
-    const uint32_t n_vis = ctr->n_vis;
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_vis; r += gridDim.x * blockDim.x) {
-        // by_slot: r is a compact slot (ascending gaussian index; runs concurrently with the depth sort)
-        // else   : r is a front-to-back rank, the list is the far->near sorted index list
-        const uint32_t id = by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r));
-        float sh[48], q[4], so[4];
-        const bool need_sh = fc.rasterize_mode == BGS_RASTERIZE_COLOR;
-        uint32_t op_bits = 0u;
-        const float4 p4 = Attr<F16>::load(blocks, id, sh, q, so, need_sh, &op_bits);
-        project_one<F16, false>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, ModeConsts{});
-    }
+    project_groups<F16, false>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs, extra,
+                               cutoff_tab, aux, ModeConsts{});
 }
 
 // project_kernel for RasterizeMode::Classification / OpticalFlow (bgs_render_ex): the same records but for r, g, b.  A
-// kernel of its own, so that project_kernel's mode branch (and its 80-register budget) stays as it is.
+// kernel of its own, so that project_kernel's mode branch (and its register budget) stays as it is.
 template <bool F16>
-__global__ void __launch_bounds__(128, PROJ_MIN_CTAS)
+__global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_modes_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
                      const FrameCounters* __restrict__ ctr, FrameConsts fc, ModeConsts mc, SplatRec* __restrict__ recs,
                      float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
-    const uint32_t n_vis = ctr->n_vis;
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_vis; r += gridDim.x * blockDim.x) {
-        const uint32_t id = by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r));
-        float sh[48], q[4], so[4];
-        const bool need_sh = fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION;   // OpticalFlow reads the position only
-        uint32_t op_bits = 0u;
-        const float4 p4 = Attr<F16>::load(blocks, id, sh, q, so, need_sh, &op_bits);
-        project_one<F16, true>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, nullptr, mc);
-    }
+    // OpticalFlow reads the position only
+    project_groups<F16, true>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs,
+                              extra, cutoff_tab, nullptr, mc);
 }
 
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
@@ -655,18 +722,18 @@ void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_pa
 void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes, cudaStream_t stream) {
-    // per-thread gather.  Grid sized from a hint (last frame's visible count + head-room); the grid-stride loop keeps
-    // any n_vis correct.
-    uint32_t grid = (n_hint + 127) / 128;
-    if (grid > 65535u * 8u) grid = 65535u * 8u;
-    if (grid < (uint32_t)sm_count) grid = (uint32_t)sm_count;
+    // a persistent grid: as many CTAs as the launch bound lets the SMs hold, fewer when the hint (last frame's visible
+    // count + head-room) has less than one group of 32 entries for each warp; the loop strides, so any n_vis is correct
+    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
+    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
+    if (grid < 1u) grid = 1u;
     if (modes) {   // Classification / OpticalFlow (no aux outputs)
-        if (f16) project_modes_kernel<true><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
-        else project_modes_kernel<false><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
+        if (f16) project_modes_kernel<true><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
+        else project_modes_kernel<false><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
         return;
     }
-    if (f16) project_kernel<true><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
-    else project_kernel<false><<<grid, 128, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
+    if (f16) project_kernel<true><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
+    else project_kernel<false><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
 }
 
 }  // namespace bgs
