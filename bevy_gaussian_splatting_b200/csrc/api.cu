@@ -408,7 +408,7 @@ static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs
                 return fail(c, BGS_EINVAL, "render: previous_clip_from_world[%d] is not finite", i);
     }
     if (st->draw_mode > BGS_DRAW_HIGHLIGHT_SELECTED) return fail(c, BGS_EINVAL, "render: bad draw_mode");
-    if (cloud->cov && (st->gaussian_mode != BGS_GAUSSIAN_3D || st->rasterize_mode == BGS_RASTERIZE_NORMAL || want_aux))
+    if (cloud->layout == CloudLayout::F16Cov && (st->gaussian_mode != BGS_GAUSSIAN_3D || st->rasterize_mode == BGS_RASTERIZE_NORMAL || want_aux))
         return fail(c, BGS_EINVAL, "render: a precomputed-covariance cloud has no rotation / scale: Gaussian3d with Color, Depth or Position only");
     const int W = (int)view->viewport[2], H = (int)view->viewport[3];
     if (W <= 0 || H <= 0 || W > 65535 || H > 65535) return fail(c, BGS_EINVAL, "render: viewport %dx%d out of range", W, H);
@@ -433,7 +433,7 @@ static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, co
     fc.Wi = W; fc.Hi = H; fc.tiles_x = (W + TILE_PX - 1) / TILE_PX; fc.tiles_y = (H + TILE_PX - 1) / TILE_PX;
     fc.n_cloud = cloud->n;
     fc.aux = want_aux ? 1u : 0u;
-    fc.cov_pre = cloud->cov ? 1u : 0u;
+    fc.cov_pre = cloud->layout == CloudLayout::F16Cov ? 1u : 0u;
     memcpy(fc.aabb_min, uni->aabb_min, 12); memcpy(fc.aabb_max, uni->aabb_max, 12);
     static const float kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
     fc.model_identity = memcmp(uni->transform, kIdentity, 64) == 0 ? 1u : 0u;   // (-0.0 entries take the general path)
@@ -483,7 +483,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
         ++launches;
     }
     CU(c, cudaEventRecord(c->ev_p0, ps));
-    launch_project(cloud->f16, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
+    launch_project(cloud->layout, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
                    c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
                    fc.aux ? c->aux.p : nullptr, modes, ps);
     ++launches;

@@ -11,8 +11,6 @@
 
 namespace {
 
-size_t block_bytes(const bgs_cloud* cl) { return cl->f16 ? 128 : 256; }
-
 // Releases a cloud that a call failed to finish, and reports why.
 bgs_status drop_cloud(bgs_context* c, const char* call, bgs_cloud* cl, cudaError_t e) {
     bgs_cloud_destroy(cl);
@@ -20,12 +18,12 @@ bgs_status drop_cloud(bgs_context* c, const char* call, bgs_cloud* cl, cudaError
 }
 
 // A new cloud of n gaussians in the given layout on the context's device, its planes allocated but not yet written.
-bgs_status new_cloud(bgs_context* c, const char* call, uint32_t n, bool f16, bool cov, bgs_cloud** out) {
+bgs_status new_cloud(bgs_context* c, const char* call, uint32_t n, CloudLayout layout, bgs_cloud** out) {
     bgs_cloud* cl = new (std::nothrow) bgs_cloud();
     if (!cl) return fail(c, BGS_ENOMEM, "%s: out of host memory", call);
-    cl->device = c->device; cl->n = n; cl->f16 = f16; cl->cov = cov;
-    cudaError_t e = cudaMalloc(&cl->pos, (size_t)n * 16);
-    if (e == cudaSuccess) e = cudaMalloc(&cl->blocks, (size_t)n * block_bytes(cl));
+    cl->device = c->device; cl->n = n; cl->layout = layout;
+    cudaError_t e = cudaMalloc(&cl->pos, (size_t)n * plane_bytes(layout, PLANE_POS));
+    if (e == cudaSuccess) e = cudaMalloc(&cl->blocks, (size_t)n * block_bytes(layout));
     if (e != cudaSuccess) return drop_cloud(c, call, cl, e);
     *out = cl;
     return BGS_OK;
@@ -53,37 +51,38 @@ struct StreamScratch {
 // gaussians per chunk of a download: the device staging arrays hold one chunk (f32: 28 MB), each of the context's two
 // pinned bounce buffers one chunk's four planes (f32: 30 MB)
 constexpr uint32_t DOWNLOAD_CHUNK = 1u << 17;
-constexpr size_t DOWNLOAD_BOUNCE_BYTES = (size_t)DOWNLOAD_CHUNK * (16 + 192 + 16 + 16);
+constexpr size_t DOWNLOAD_BOUNCE_BYTES = (size_t)DOWNLOAD_CHUNK * planar_bytes(CloudLayout::F32);
 
 }  // namespace
 
 extern "C" {
 
-static bgs_status upload_common(bgs_context* ctx, uint32_t n, bool f16, bool cov, const float* pos_vis, const void* sh,
+static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout, const float* pos_vis, const void* sh,
                                 const void* rot, const void* so, bgs_cloud** out) {
     if (!ctx || !out) return BGS_EINVAL;
     *out = nullptr;
-    if (!pos_vis || !sh || !rot || (!f16 && !so)) return fail(ctx, BGS_EINVAL, "cloud upload: null plane pointer");
+    const void* src[PLANES] = {pos_vis, sh, rot, so};
+    for (int p = 0; p < PLANES; ++p)
+        if (plane_bytes(layout, p) && !src[p]) return fail(ctx, BGS_EINVAL, "cloud upload: null plane pointer");
     if (n == 0 || n >= (1u << 30)) return fail(ctx, BGS_EINVAL, "cloud upload: n must be in [1, 2^30)");
     CU(ctx, cudaSetDevice(ctx->device));
     bgs_cloud* cl = nullptr;
-    TRY(new_cloud(ctx, "cloud upload", n, f16, cov, &cl));
-    // the other planes go to device scratch, are repacked into the gaussian-major blocks the projection gathers, and
-    // are freed again
-    void* d_sh = nullptr; void* d_rot = nullptr; void* d_so = nullptr;
-    const size_t sh_bytes = (size_t)n * (f16 ? 96 : 192);
-    cudaError_t e = cudaMalloc(&d_sh, sh_bytes);
-    if (e == cudaSuccess) e = cudaMalloc(&d_rot, (size_t)n * 16);
-    if (e == cudaSuccess && !f16) e = cudaMalloc(&d_so, (size_t)n * 16);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(cl->pos, pos_vis, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_sh, sh, sh_bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_rot, rot, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess && !f16) e = cudaMemcpyAsync(d_so, so, (size_t)n * 16, cudaMemcpyHostToDevice, ctx->stream);
+    TRY(new_cloud(ctx, "cloud upload", n, layout, &cl));
+    // the position plane is the cloud's own; the other planes go to device scratch, are repacked into the
+    // gaussian-major blocks the projection gathers, and are freed again
+    void* d[PLANES] = {cl->pos, nullptr, nullptr, nullptr};
+    cudaError_t e = cudaSuccess;
+    for (int p = 0; p < PLANES && e == cudaSuccess; ++p) {
+        const size_t bytes = (size_t)n * plane_bytes(layout, p);
+        if (bytes == 0) continue;
+        if (p != PLANE_POS) e = cudaMalloc(&d[p], bytes);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d[p], src[p], bytes, cudaMemcpyHostToDevice, ctx->stream);
+    }
     if (e == cudaSuccess) {
-        launch_repack(f16, cl->pos, d_sh, d_rot, d_so, n, cl->blocks, ctx->stream);
+        launch_repack(layout, d[PLANE_SH], d[PLANE_ROT], d[PLANE_SO], n, cl->view(), ctx->stream);
         e = cudaStreamSynchronize(ctx->stream);
     }
-    cudaFree(d_sh); cudaFree(d_rot); cudaFree(d_so);
+    for (int p = PLANE_SH; p < PLANES; ++p) cudaFree(d[p]);
     if (e != cudaSuccess) return drop_cloud(ctx, "cloud upload", cl, e);
     *out = cl;
     return BGS_OK;
@@ -91,17 +90,17 @@ static bgs_status upload_common(bgs_context* ctx, uint32_t n, bool f16, bool cov
 
 bgs_status bgs_cloud_upload_f32(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh,
                                 const float* rot_wxyz, const float* scale_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, false, false, pos_vis, sh, rot_wxyz, scale_opacity, out);
+    return upload_common(ctx, n, CloudLayout::F32, pos_vis, sh, rot_wxyz, scale_opacity, out);
 }
 
 bgs_status bgs_cloud_upload_f16(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
                                 const uint32_t* rot_scale_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, true, false, pos_vis, sh_packed, rot_scale_opacity, nullptr, out);
+    return upload_common(ctx, n, CloudLayout::F16, pos_vis, sh_packed, rot_scale_opacity, nullptr, out);
 }
 
 bgs_status bgs_cloud_upload_f16_cov(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
                                     const uint32_t* cov3d_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, true, true, pos_vis, sh_packed, cov3d_opacity, nullptr, out);
+    return upload_common(ctx, n, CloudLayout::F16Cov, pos_vis, sh_packed, cov3d_opacity, nullptr, out);
 }
 
 void bgs_cloud_destroy(bgs_cloud* cl) {
@@ -130,9 +129,8 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
     delete cl;
 }
 
-// ---- selection edits of a resident cloud (select.cu).  The visibility lane lives twice on the device: the position
-// plane's .w (what key-gen streams) and the first 16 B of each gaussian-major block (what the projection reads): every
-// write updates both.
+// ---- selection edits of a resident cloud (select.cu).  The visibility lane lives in both of the cloud's copies
+// (cloud_layout.cuh): every write updates both.
 
 bgs_status bgs_cloud_select_sparse(bgs_context* c, bgs_cloud* cl, float radius, uint32_t threshold, uint32_t* out_selected) {
     if (!cl) return fail(c, BGS_EINVAL, "select_sparse: null cloud");
@@ -141,15 +139,12 @@ bgs_status bgs_cloud_select_sparse(bgs_context* c, bgs_cloud* cl, float radius, 
     TRY(before_cloud_write(c, cl));
     const uint32_t n = cl->n;
     const float r2 = radius * radius;
-    float* pos_w = reinterpret_cast<float*>(cl->pos) + 3;
-    float* block_w = reinterpret_cast<float*>(cl->blocks) + 3;
-    const uint32_t stride = (uint32_t)(block_bytes(cl) / 4);
     cudaStream_t q = c->stream;
     uint32_t selected = 0;
     if (threshold == 0u || r2 == 0.0f) {
         // no count can reach a threshold of 0; no distance is below a radius whose square is 0 (every count is 0)
         selected = threshold == 0u ? 0u : n;
-        launch_select_fill(n, threshold == 0u ? 0.0f : 1.0f, pos_w, block_w, stride, q);
+        launch_select_fill(cl->view(), n, threshold == 0u ? 0.0f : 1.0f, q);
         CU(c, cudaGetLastError());
         CU(c, cudaStreamSynchronize(q));
     } else {
@@ -173,8 +168,8 @@ bgs_status bgs_cloud_select_sparse(bgs_context* c, bgs_cloud* cl, float radius, 
         CU(c, launch_radix_sort(c->keys[0].p, c->vals[0].p, c->keys[1].p, c->vals[1].p, &words[0], n, n, hist, 1,
                                 c->status_depth.p, (size_t)radix_num_tiles(c->status_n) * 256, next_epoch(c), &words[1], passes,
                                 0, ranges, c->sm_count, c->rs_per_sm, q));
-        launch_select_count(cl->pos, c->vals[passes & 1].p, ranges, n, radius, nb, r2, threshold,
-                            reinterpret_cast<float4*>(c->recs.p), pos_w, block_w, stride, &words[2], q);
+        launch_select_count(cl->view(), c->vals[passes & 1].p, ranges, n, radius, nb, r2, threshold,
+                            reinterpret_cast<float4*>(c->recs.p), &words[2], q);
         CU(c, cudaGetLastError());
         TRY(read_word(c, &words[2], &selected));
     }
@@ -186,7 +181,7 @@ bgs_status bgs_cloud_visibility_get(bgs_context* c, const bgs_cloud* cl, float* 
     if (!cl || !out_vis) return fail(c, BGS_EINVAL, "visibility_get: null cloud or array");
     TRY(enter_call(c, "visibility_get", cl->device));
     TRY(before_cloud_read(c, cl));
-    CU(c, cudaMemcpy2DAsync(out_vis, 4, reinterpret_cast<const char*>(cl->pos) + 12, 16, 4, cl->n, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemcpy2DAsync(out_vis, 4, &cl->pos->w, sizeof(float4), 4, cl->n, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return BGS_OK;
 }
@@ -195,9 +190,10 @@ bgs_status bgs_cloud_visibility_set(bgs_context* c, bgs_cloud* cl, const float* 
     if (!cl || !vis) return fail(c, BGS_EINVAL, "visibility_set: null cloud or array");
     TRY(enter_call(c, "visibility_set", cl->device));
     TRY(before_cloud_write(c, cl));
-    CU(c, cudaMemcpy2DAsync(reinterpret_cast<char*>(cl->pos) + 12, 16, vis, 4, 4, cl->n, cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemcpy2DAsync(reinterpret_cast<char*>(cl->blocks) + 12, block_bytes(cl), vis, 4, 4, cl->n, cudaMemcpyHostToDevice,
-                            c->stream));
+    const CloudView v = cl->view();
+    CU(c, cudaMemcpy2DAsync(&v.pos->w, sizeof(float4), vis, 4, 4, cl->n, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpy2DAsync(&reinterpret_cast<float4*>(v.blocks)[POS_CHUNK].w, block_bytes(cl->layout), vis, 4, 4, cl->n,
+                            cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return BGS_OK;
 }
@@ -215,9 +211,6 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* c, bgs_cloud* cl, const float* 
     const float* M = mesh_from_cloud ? mesh_from_cloud : identity;
     TRY(before_cloud_write(c, cl));
     const uint32_t n = cl->n;
-    float* pos_w = reinterpret_cast<float*>(cl->pos) + 3;
-    float* block_w = reinterpret_cast<float*>(cl->blocks) + 3;
-    const uint32_t stride = (uint32_t)(block_bytes(cl) / 4);
     cudaStream_t q = c->stream;
 
     // triangle side: setup (records, classes, grid bounds)
@@ -279,7 +272,7 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* c, bgs_cloud* cl, const float* 
     }
 
     // point side: the count and the lane
-    launch_mesh_count(cl->pos, n, M, tb + o_br, tb + o_gr, cell_tri, ranges, wh, level, mode, pos_w, block_w, stride, words, q);
+    launch_mesh_count(cl->view(), n, M, tb + o_br, tb + o_gr, cell_tri, ranges, wh, level, mode, words, q);
     CU(c, cudaGetLastError());
     uint32_t inside = 0;
     TRY(read_word(c, mesh_words_inside(words), &inside));
@@ -350,7 +343,7 @@ bgs_status bgs_cloud_particles_step(bgs_context* c, bgs_cloud* cl, bgs_particles
         return fail(c, BGS_EINVAL, "particles_step: behaviour names gaussian %lld of a cloud of %u", (long long)p->max_index, cl->n);
     TRY(queue_cloud_write(c, cl, [&](cudaStream_t q) {
         CU(c, cudaStreamWaitEvent(q, p->ev_write, 0));
-        launch_particle_step(p->d, p->count, delta_time, cl->pos, cl->blocks, (uint32_t)(block_bytes(cl) / 16), q);
+        launch_particle_step(p->d, p->count, delta_time, cl->view(), q);
         CU(c, cudaGetLastError());
         CU(c, cudaEventRecord(p->ev_write, q));
         return BGS_OK;
@@ -390,14 +383,14 @@ bgs_status bgs_cloud_interpolate(bgs_context* c, bgs_cloud* out, const bgs_cloud
     TRY(enter_call(c, "interpolate", lhs->device == out->device && rhs->device == out->device ? out->device : -1, "clouds live"));
     if (lhs->n != out->n || rhs->n != out->n)
         return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out hold %u, %u and %u gaussians", lhs->n, rhs->n, out->n);
-    if (lhs->f16 != out->f16 || rhs->f16 != out->f16 || lhs->cov != out->cov || rhs->cov != out->cov)
+    if (lhs->layout != out->layout || rhs->layout != out->layout)
         return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out are not in one layout");
     if (out == lhs || out == rhs) return fail(c, BGS_EINVAL, "interpolate: out is lhs or rhs");
     float t = 0.0f;
     if (!interpolation_factor(time, time_start, time_stop, &t))
         return fail(c, BGS_EINVAL, "interpolate: time %g, time_start %g, time_stop %g give no factor", time, time_start, time_stop);
     return queue_cloud_write_reading(c, out, lhs, rhs, [&](cudaStream_t q) {
-        launch_interpolate(out->f16, out->cov, lhs->blocks, rhs->blocks, out->n, t, out->blocks, out->pos, q);
+        launch_interpolate(out->layout, lhs->view(), rhs->view(), out->n, t, out->view(), q);
         CU(c, cudaGetLastError());
         return BGS_OK;
     });
@@ -441,13 +434,13 @@ bgs_status bgs_cloud_subset(bgs_context* c, const bgs_cloud* cl, const uint32_t*
         CU(c, cudaMemcpyAsync(scratch.p, indices, (size_t)k * 4, cudaMemcpyHostToDevice, q));
     }
     bgs_cloud* nc = nullptr;
-    TRY(new_cloud(c, "subset", kept, cl->f16, cl->cov, &nc));
+    TRY(new_cloud(c, "subset", kept, cl->layout, &nc));
     if (!indices) {
         const uint8_t* s = static_cast<const uint8_t*>(scratch.p);
-        launch_subset_scatter(cl->f16, cl->pos, cl->blocks, n, reinterpret_cast<const uint32_t*>(s + o_mask),
-                              reinterpret_cast<const uint32_t*>(s + o_cnt), nc->pos, nc->blocks, q);
+        launch_subset_scatter(cl->layout, cl->view(), n, reinterpret_cast<const uint32_t*>(s + o_mask),
+                              reinterpret_cast<const uint32_t*>(s + o_cnt), nc->view(), q);
     } else {
-        launch_subset_gather(cl->f16, cl->pos, cl->blocks, static_cast<const uint32_t*>(scratch.p), k, nc->pos, nc->blocks, q);
+        launch_subset_gather(cl->layout, cl->view(), static_cast<const uint32_t*>(scratch.p), k, nc->view(), q);
     }
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(q);
@@ -462,35 +455,34 @@ bgs_status bgs_cloud_subset(bgs_context* c, const bgs_cloud* cl, const uint32_t*
 static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, bool f16, float* pos_vis, void* sh, void* rot, void* so) {
     if (!cl || !pos_vis || !sh || !rot || (!f16 && !so)) return fail(c, BGS_EINVAL, "download: null cloud or plane pointer");
     TRY(enter_call(c, "download", cl->device));
-    if (cl->f16 != f16) return fail(c, BGS_EINVAL, "download: the cloud is in the %s layout", cl->f16 ? "f16" : "f32");
+    const CloudLayout l = cl->layout;
+    if (is_f16(l) != f16) return fail(c, BGS_EINVAL, "download: the cloud is in the %s layout", is_f16(l) ? "f16" : "f32");
     TRY(before_cloud_read(c, cl));
     cudaStream_t q = c->stream;
     const uint32_t n = cl->n, m_max = std::min(n, DOWNLOAD_CHUNK);
-    const size_t sh_b = f16 ? 96 : 192, so_b = f16 ? 0 : 16;
-    const size_t plane_b[4] = {16, sh_b, 16, so_b};          // pos | sh | rot | so, per gaussian
     // (sized once for the largest chunk of either layout: it never grows)
     if (!c->h_bounce) CU(c, cudaMallocHost(&c->h_bounce, 2 * DOWNLOAD_BOUNCE_BYTES));
     const size_t chunk_b = DOWNLOAD_BOUNCE_BYTES;
     StreamScratch staging(q);   // sh | rot | so of one chunk
-    CU(c, staging.alloc((size_t)m_max * (sh_b + 16 + so_b)));
-    uint8_t* st = static_cast<uint8_t*>(staging.p);
-    uint8_t* st_rot = st + (size_t)m_max * sh_b;
-    uint8_t* st_so = st_rot + (size_t)m_max * 16;
+    CU(c, staging.alloc((size_t)m_max * (planar_bytes(l) - plane_bytes(l, PLANE_POS))));
+    uint8_t* st[PLANES] = {nullptr, static_cast<uint8_t*>(staging.p)};
+    for (int p = PLANE_SH + 1; p < PLANES; ++p) st[p] = st[p - 1] + (size_t)m_max * plane_bytes(l, p - 1);
     cudaEvent_t ev[2] = {nullptr, nullptr};
     struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 2; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
     for (cudaEvent_t& e : ev) CU(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    uint8_t* dst[4] = {reinterpret_cast<uint8_t*>(pos_vis), static_cast<uint8_t*>(sh), static_cast<uint8_t*>(rot), static_cast<uint8_t*>(so)};
+    uint8_t* dst[PLANES] = {reinterpret_cast<uint8_t*>(pos_vis), static_cast<uint8_t*>(sh), static_cast<uint8_t*>(rot), static_cast<uint8_t*>(so)};
     const uint32_t chunks = (n + m_max - 1) / m_max;
     // enqueue chunk i into bounce buffer i & 1
     auto enqueue = [&](uint32_t i) -> bgs_status {
         const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
         uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
-        launch_unpack(f16, cl->blocks, lo, m, st, st_rot, st_so, q);
+        launch_unpack(l, cl->view(), lo, m, st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO], q);
         CU(c, cudaGetLastError());
-        const uint8_t* src[4] = {reinterpret_cast<const uint8_t*>(cl->pos) + (size_t)lo * 16, st, st_rot, st_so};
-        for (int p = 0; p < 4; ++p) {
-            if (plane_b[p]) CU(c, cudaMemcpyAsync(hb, src[p], (size_t)m * plane_b[p], cudaMemcpyDeviceToHost, q));
-            hb += (size_t)m * plane_b[p];
+        const uint8_t* src[PLANES] = {reinterpret_cast<const uint8_t*>(cl->pos + lo), st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO]};
+        for (int p = 0; p < PLANES; ++p) {
+            const size_t bytes = (size_t)m * plane_bytes(l, p);
+            if (bytes) CU(c, cudaMemcpyAsync(hb, src[p], bytes, cudaMemcpyDeviceToHost, q));
+            hb += bytes;
         }
         CU(c, cudaEventRecord(ev[i & 1], q));
         return BGS_OK;
@@ -501,9 +493,10 @@ static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, bool f16,
         CU(c, cudaEventSynchronize(ev[i & 1]));
         const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
         const uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
-        for (int p = 0; p < 4; ++p) {
-            if (plane_b[p]) memcpy(dst[p] + (size_t)lo * plane_b[p], hb, (size_t)m * plane_b[p]);
-            hb += (size_t)m * plane_b[p];
+        for (int p = 0; p < PLANES; ++p) {
+            const size_t b = plane_bytes(l, p);
+            if (b) memcpy(dst[p] + (size_t)lo * b, hb, (size_t)m * b);
+            hb += (size_t)m * b;
         }
     }
     return BGS_OK;

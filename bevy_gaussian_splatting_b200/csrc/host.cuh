@@ -40,15 +40,15 @@ using namespace bgs;
 struct bgs_cloud {
     int device;       // the CUDA device the planes live on
     uint32_t n;
-    bool f16;
-    bool cov;         // f16 layout whose second plane holds Covariance3dOpacityPacked128 records (precomputed Sigma3D)
-    float4* pos = nullptr;      // n * 16 B
-    void* blocks = nullptr;     // gaussian-major copy of every plane (f16: n * 128 B, f32: n * 256 B), what the projection gathers
+    CloudLayout layout;
+    float4* pos = nullptr;      // the position plane and the gaussian-major blocks (cloud_layout.cuh)
+    void* blocks = nullptr;
     // enqueued writes (particle steps): ev_write marks the last one, on whichever context's stream it was queued; every
     // later reader or writer waits for it on the device.  Created by the first step; `stepped` is set once it exists,
     // so a cloud that is never stepped costs its frames nothing
     cudaEvent_t ev_write = nullptr;
     std::atomic<bool> stepped{false};
+    CloudView view() const { return {pos, static_cast<uint4*>(blocks), chunks(layout)}; }
 };
 
 // A ParticleBehaviors asset resident on one GPU: count 64 B records (bgs_particle_behavior), read and written by the step

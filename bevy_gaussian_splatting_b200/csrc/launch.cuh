@@ -1,7 +1,7 @@
 // launch.cuh -- the host entry points of libbgs's kernels: one declaration each, included by the .cu file that defines
 // it and by the host code that calls it (api.cu, cloud.cu), so a signature that drifts fails to compile.
 #pragma once
-#include "common.cuh"
+#include "cloud_layout.cuh"
 
 namespace bgs {
 // keygen.cu
@@ -22,9 +22,9 @@ cudaError_t launch_radix_sort(uint32_t* keys0, uint32_t* vals0, uint32_t* keys1,
 // project.cu
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
                         FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream);
-void launch_repack(bool f16, const void* pos, const void* sh, const void* rot, const void* so, uint32_t n, void* blocks,
+void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, uint32_t n, CloudView cloud,
                    cudaStream_t stream);
-void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+void launch_project(CloudLayout layout, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes /* null: project_kernel */,
                     cudaStream_t stream);
@@ -48,10 +48,9 @@ uint32_t select_num_buckets(uint32_t n);
 int select_sort_passes(uint32_t n_buckets);
 void launch_select_keys(const float4* pos, uint32_t n, float radius, uint32_t n_buckets, uint32_t* keys, uint32_t* vals,
                         uint32_t* n_sort, cudaStream_t stream);
-void launch_select_count(const float4* pos, const uint32_t* ids, const uint2* ranges, uint32_t n, float radius, uint32_t n_buckets,
-                         float r2, uint32_t threshold, float4* spos, float* pos_w, float* block_w, uint32_t block_stride,
-                         uint32_t* selected, cudaStream_t stream);
-void launch_select_fill(uint32_t n, float v, float* pos_w, float* block_w, uint32_t block_stride, cudaStream_t stream);
+void launch_select_count(CloudView cloud, const uint32_t* ids, const uint2* ranges, uint32_t n, float radius, uint32_t n_buckets,
+                         float r2, uint32_t threshold, float4* spos, uint32_t* selected, cudaStream_t stream);
+void launch_select_fill(CloudView cloud, uint32_t n, float v, cudaStream_t stream);
 // mesh_select.cu
 size_t mesh_words_bytes();
 size_t mesh_rec_bytes();
@@ -65,21 +64,18 @@ uint32_t* mesh_words_pairs(void* words);
 uint32_t* mesh_words_barrier(void* words);
 uint32_t* mesh_words_inside(void* words);
 uint32_t mesh_words_n_bin(const void* words_host);
-void launch_mesh_count(const float4* pos, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
-                       const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, float* pos_w,
-                       float* block_w, uint32_t block_stride, void* words, cudaStream_t stream);
+void launch_mesh_count(CloudView cloud, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
+                       const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, void* words,
+                       cudaStream_t stream);
 // particles.cu
-void launch_particle_step(void* behaviors, uint32_t count, float dt, float4* pos, void* blocks, uint32_t block_stride,
-                          cudaStream_t stream);
+void launch_particle_step(void* behaviors, uint32_t count, float dt, CloudView cloud, cudaStream_t stream);
 // subset.cu
 uint32_t subset_num_ctas(uint32_t n);
 void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t* cta_cnt, uint32_t* total, cudaStream_t stream);
-void launch_subset_scatter(bool f16, const void* pos, const void* blocks, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
-                           void* out_pos, void* out_blocks, cudaStream_t stream);
-void launch_subset_gather(bool f16, const void* pos, const void* blocks, const uint32_t* idx, uint32_t k, void* out_pos,
-                          void* out_blocks, cudaStream_t stream);
-void launch_unpack(bool f16, const void* blocks, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream);
+void launch_subset_scatter(CloudLayout layout, CloudView src, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
+                           CloudView dst, cudaStream_t stream);
+void launch_subset_gather(CloudLayout layout, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst, cudaStream_t stream);
+void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream);
 // interpolate.cu
-void launch_interpolate(bool f16, bool cov, const void* lhs_blocks, const void* rhs_blocks, uint32_t n, float t,
-                        void* out_blocks, float4* out_pos, cudaStream_t stream);
+void launch_interpolate(CloudLayout layout, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream);
 }  // namespace bgs

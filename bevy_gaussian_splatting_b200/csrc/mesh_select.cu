@@ -233,17 +233,16 @@ struct MeshXform {
 };
 
 // One thread per gaussian.  mode 0 (replace): lane = inside ? 1 : 0; mode 1 (add): lane = 1 where inside, else untouched.
-__global__ void __launch_bounds__(MS_THREADS) mesh_count_kernel(const float4* __restrict__ pos, uint32_t n, MeshXform M,
+__global__ void __launch_bounds__(MS_THREADS) mesh_count_kernel(CloudView cloud, uint32_t n, MeshXform M,
                                                                 const MeshRec* __restrict__ bin_rec, uint32_t n_bin,
                                                                 const MeshRec* __restrict__ glob_rec, uint32_t n_glob,
                                                                 const uint32_t* __restrict__ cell_tri, const uint2* __restrict__ ranges,
                                                                 MeshGrid g, double y1, double z1, uint32_t mode,
-                                                                float* __restrict__ pos_w, float* __restrict__ block_w,
-                                                                uint32_t block_stride, uint32_t* __restrict__ inside_count) {
+                                                                uint32_t* __restrict__ inside_count) {
     const uint32_t i = blockIdx.x * MS_THREADS + threadIdx.x;
     bool inside = false;
     if (i < n) {
-        const float4 p = __ldg(pos + i);
+        const float4 p = __ldg(cloud.pos + i);
         const float* m = M.m;
         // q = M (x, y, z, 1): ((m_r0 x + m_r1 y) + m_r2 z) + m_r3 per row r
         float3 q;
@@ -263,11 +262,7 @@ __global__ void __launch_bounds__(MS_THREADS) mesh_count_kernel(const float4* __
             for (uint32_t b = 0; b < n_glob; ++b) hits += ms_hit(q, glob_rec[b]) ? 1u : 0u;
         }
         inside = (hits & 1u) != 0u;
-        if (mode == 0u || inside) {
-            const float v = inside ? 1.0f : 0.0f;
-            pos_w[(size_t)i * 4] = v;
-            block_w[(size_t)i * block_stride] = v;
-        }
+        if (mode == 0u || inside) cloud.store_visibility(i, inside ? 1.0f : 0.0f);
     }
     const uint32_t ballot = __ballot_sync(0xffffffffu, inside);
     if ((threadIdx.x & 31) == 0 && ballot) atomicAdd(inside_count, (uint32_t)__popc(ballot));
@@ -356,9 +351,9 @@ uint32_t* mesh_words_inside(void* words) { return &static_cast<MeshWords*>(words
 uint32_t mesh_words_n_bin(const void* words_host) { return static_cast<const MeshWords*>(words_host)->n_bin; }
 
 // level < 0: no binned triangle (no grid)
-void launch_mesh_count(const float4* pos, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
-                       const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, float* pos_w,
-                       float* block_w, uint32_t block_stride, void* words, cudaStream_t stream) {
+void launch_mesh_count(CloudView cloud, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
+                       const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, void* words,
+                       cudaStream_t stream) {
     if (n == 0) return;
     const MeshWords* wh = static_cast<const MeshWords*>(words_host);
     MeshXform M;
@@ -370,10 +365,9 @@ void launch_mesh_count(const float4* pos, uint32_t n, const float* mesh_from_clo
         y1 = ms_unkey(wh->bound[1]);
         z1 = ms_unkey(wh->bound[3]);
     }
-    mesh_count_kernel<<<ms_grid(n), MS_THREADS, 0, stream>>>(pos, n, M, static_cast<const MeshRec*>(bin_rec), level >= 0 ? wh->n_bin : 0u,
+    mesh_count_kernel<<<ms_grid(n), MS_THREADS, 0, stream>>>(cloud, n, M, static_cast<const MeshRec*>(bin_rec), level >= 0 ? wh->n_bin : 0u,
                                                              static_cast<const MeshRec*>(glob_rec), wh->n_glob, cell_tri, ranges, g, y1,
-                                                             z1, mode, pos_w, block_w, block_stride,
-                                                             &static_cast<MeshWords*>(words)->inside);
+                                                             z1, mode, &static_cast<MeshWords*>(words)->inside);
 }
 
 }  // namespace bgs

@@ -8,14 +8,12 @@
 //    record of rank k at recs[sorted slot of k];
 //  * BGS_FLAG_SORT_ALL: r is a front-to-back rank (0 = nearest), id = sorted_ids[n_vis-1-r] (the sort is far->near
 //    like the reference's, src/sort/radix.wgsl).
-// Either way: gather the gaussian's block (f32 256 B or f16 128 B) -> write one 48 B SplatRec at recs[r]
+// Either way: gather the gaussian's block (cloud_layout.cuh) -> write one 48 B SplatRec at recs[r]
 // (coalesced), which is all the tile stages read.
 //
 // project_one is the vertex stage's dispatch: frustum and draw-mode test, cutoff, then the record of the splat's
 // geometry (3DGS USE_AABB conic, 3DGS USE_OBB, 2DGS surfel) and its colour source (SH, Depth, Normal, Position).
 // Geometry (centre, OBB uv rows, pixel bbox) is bit-exact vs the oracle: compiled -fmad=false.
-#include <cuda_fp16.h>
-
 #include "project_math.cuh"
 #include "launch.cuh"
 
@@ -63,10 +61,8 @@ __device__ __forceinline__ void make_bbox(float cx, float cy, float hx, float hy
     bx = pack_bbox(x0, x1); by = pack_bbox(y0, y1);
 }
 
-// Attributes live in the library-owned gaussian-major copy made once at upload -- f16: 128 B = one cache line per
-// gaussian (pos | rot/scale/opacity | sh x 6), f32: 256 B (pos | rot | scale_opacity | sh x 12 | pad) -- so the random
-// gather of a visible splat touches exactly its own line(s) instead of 3-4 partially used ones of the reference's
-// planes (the position plane stays planar for key-gen).
+// Attributes come from the cloud's gaussian-major blocks (cloud_layout.cuh), so the random gather of a visible splat
+// touches exactly its own line(s) instead of 3-4 partially used ones of the reference's planes.
 //
 // A warp gathers the blocks of 32 consecutive entries of the index list into its own shared-memory stage with
 // coalesced 16 B asynchronous copies (cp.async.cg: no staging registers, L1 bypassed, every line is used once): a
@@ -95,24 +91,25 @@ __device__ __forceinline__ void gather_blocks(const uint4* __restrict__ blocks, 
     }
 }
 
-// entry g's attributes out of a stage
+// entry g's attributes out of a stage (the covariance layout's record arrives in q and so as its lanes fall)
 template <bool F16>
 struct Attr;
 template <>
 struct Attr<false> {
-    static constexpr int CH = 16, GEO = 4;
+    static constexpr CloudLayout L = CloudLayout::F32;
+    static constexpr int CH = chunks(L), GEO = 4;
     __device__ static float4 load(const uint4* stage, int g, float* sh, float q[4], float so[4], bool need_sh, uint32_t&) {
         auto piece = [&](int p) {
             const uint4 v = stage[g * CH + (p ^ (g & 7))];
             return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
         };
-        const float4 p = piece(0), r = piece(1), s = piece(2);
+        const float4 p = piece(POS_CHUNK), r = piece(SECOND_CHUNK), s = piece(SO_CHUNK);
         q[0] = r.x; q[1] = r.y; q[2] = r.z; q[3] = r.w;
         so[0] = s.x; so[1] = s.y; so[2] = s.z; so[3] = s.w;
         if (need_sh) {
 #pragma unroll
-            for (int i = 0; i < 12; ++i) {
-                const float4 v = piece(3 + i);
+            for (int i = 0; i < (int)sh_chunks(L); ++i) {
+                const float4 v = piece(sh_first(L) + i);
                 sh[4 * i] = v.x; sh[4 * i + 1] = v.y; sh[4 * i + 2] = v.z; sh[4 * i + 3] = v.w;
             }
         }
@@ -121,22 +118,21 @@ struct Attr<false> {
 };
 template <>
 struct Attr<true> {
-    static constexpr int CH = 8, GEO = 2;
-    __device__ static float lo(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu))); }
-    __device__ static float hi(uint32_t w) { return __half2float(__ushort_as_half((unsigned short)(w >> 16))); }
+    static constexpr CloudLayout L = CloudLayout::F16;
+    static constexpr int CH = chunks(L), GEO = 2;
     __device__ static float4 load(const uint4* stage, int g, float* sh, float q[4], float so[4], bool need_sh,
                                   uint32_t& op_bits) {
         auto piece = [&](int p) { return stage[g * CH + (p ^ (g & 7))]; };
-        const uint4 pw = piece(0), w = piece(1);
+        const uint4 pw = piece(POS_CHUNK), w = piece(SECOND_CHUNK);
         op_bits = w.w & 0xFFFFu;
-        q[0] = hi(w.x); q[1] = lo(w.x); q[2] = hi(w.y); q[3] = lo(w.y);
-        so[0] = hi(w.z); so[1] = lo(w.z); so[2] = hi(w.w); so[3] = lo(w.w);
+        second_lanes(w.x, w.y, q);
+        second_lanes(w.z, w.w, so);
         if (need_sh) {
 #pragma unroll
-            for (int i = 0; i < 6; ++i) {
-                const uint4 v = piece(2 + i);
-                sh[8 * i] = lo(v.x); sh[8 * i + 1] = hi(v.x); sh[8 * i + 2] = lo(v.y); sh[8 * i + 3] = hi(v.y);
-                sh[8 * i + 4] = lo(v.z); sh[8 * i + 5] = hi(v.z); sh[8 * i + 6] = lo(v.w); sh[8 * i + 7] = hi(v.w);
+            for (int i = 0; i < (int)sh_chunks(L); ++i) {
+                const uint4 v = piece(sh_first(L) + i);
+                sh[8 * i] = half_lo(v.x); sh[8 * i + 1] = half_hi(v.x); sh[8 * i + 2] = half_lo(v.y); sh[8 * i + 3] = half_hi(v.y);
+                sh[8 * i + 4] = half_lo(v.z); sh[8 * i + 5] = half_hi(v.z); sh[8 * i + 6] = half_lo(v.w); sh[8 * i + 7] = half_hi(v.w);
             }
         }
         return make_float4(__uint_as_float(pw.x), __uint_as_float(pw.y), __uint_as_float(pw.z), __uint_as_float(pw.w));
@@ -144,30 +140,19 @@ struct Attr<true> {
 };
 
 // upload-time repack of the planes into gaussian-major blocks (one thread per 16 B chunk; coalesced both ways)
-template <bool F16>
-__global__ void repack_kernel(const uint4* __restrict__ pos, const uint4* __restrict__ sh, const uint4* __restrict__ rot,
-                              const uint4* __restrict__ so, uint32_t n, uint4* __restrict__ blocks) {
-    constexpr uint32_t CH = F16 ? 8u : 16u;          // 16 B chunks per block
-    constexpr uint32_t SHC = F16 ? 6u : 12u;         // sh chunks per gaussian
+template <CloudLayout L>
+__global__ void repack_kernel(CloudPlanes<const uint4> planes, uint32_t n, uint4* __restrict__ blocks) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (size_t)n * CH) return;
-    const uint32_t id = (uint32_t)(i / CH), c = (uint32_t)(i % CH);
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (c == 0) v = pos[id];
-    else if (c == 1) v = rot[id];                    // f16: packed rotation + scale + opacity
-    else if (!F16 && c == 2) v = so[id];
-    else {
-        const uint32_t k = c - (F16 ? 2u : 3u);
-        if (k < SHC) v = sh[(size_t)id * SHC + k];
-    }
-    blocks[i] = v;
+    if (i >= (size_t)n * chunks(L)) return;
+    const uint4* src = planes.unit<L>((uint32_t)(i % chunks(L)), i / chunks(L));
+    blocks[i] = src ? __ldg(src) : make_uint4(0u, 0u, 0u, 0u);
 }
-void launch_repack(bool f16, const void* pos, const void* sh, const void* rot, const void* so, uint32_t n, void* blocks,
+void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, uint32_t n, CloudView cloud,
                    cudaStream_t stream) {
-    const size_t total = (size_t)n * (f16 ? 8 : 16);
-    const uint32_t grid = (uint32_t)((total + 255) / 256);
-    if (f16) repack_kernel<true><<<grid, 256, 0, stream>>>((const uint4*)pos, (const uint4*)sh, (const uint4*)rot, (const uint4*)so, n, (uint4*)blocks);
-    else repack_kernel<false><<<grid, 256, 0, stream>>>((const uint4*)pos, (const uint4*)sh, (const uint4*)rot, (const uint4*)so, n, (uint4*)blocks);
+    const CloudPlanes<const uint4> planes{reinterpret_cast<const uint4*>(cloud.pos), static_cast<const uint4*>(sh),
+                                          static_cast<const uint4*>(rot), static_cast<const uint4*>(so)};
+    const uint32_t grid = (uint32_t)(((size_t)n * cloud.chunks + 255) / 256);
+    with_layout(layout, [&](auto L) { repack_kernel<decltype(L)::value><<<grid, 256, 0, stream>>>(planes, n, cloud.blocks); });
 }
 
 // RasterizeMode::Depth (gaussian.wgsl:329-349): min distance from sorted[N-1], max from sorted[1] of the
@@ -719,7 +704,7 @@ void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_pa
     depth_range_kernel<<<1, 32, 0, stream>>>(pos, n, sorted_payload, slot_ids, ctr, fc);
 }
 
-void launch_project(bool f16, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+void launch_project(CloudLayout layout, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes, cudaStream_t stream) {
     // a persistent grid: as many CTAs as the launch bound lets the SMs hold, fewer when the hint (last frame's visible
@@ -727,6 +712,7 @@ void launch_project(bool f16, const void* blocks, const uint32_t* index_list, in
     uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
     if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
     if (grid < 1u) grid = 1u;
+    const bool f16 = is_f16(layout);
     if (modes) {   // Classification / OpticalFlow (no aux outputs)
         if (f16) project_modes_kernel<true><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
         else project_modes_kernel<false><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);

@@ -11,7 +11,7 @@
 //   3. select_gather_kernel: positions in bucket order, so each bucket's scan reads contiguous memory;
 //   4. select_count_kernel: one thread per sorted entry (neighbouring threads share cells) scans the distinct
 //      buckets of its 27 neighbour cells with the exact f32 test, stops once the count reaches the threshold,
-//      and writes the visibility into both device copies (position plane .w, gaussian-major block .w).
+//      and writes the visibility into both of the cloud's copies of it.
 // Hash collisions only add distance tests; the dedupe of the 27 buckets keeps a bucket from being counted twice.
 //
 // Cost: O(N) for keys and sort; the count is O(N x min(threshold, neighbours in 27 cells)), plus the collisions.
@@ -76,8 +76,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_gather_kernel(const float4
 __global__ void __launch_bounds__(SEL_THREADS) select_count_kernel(const float4* __restrict__ spos, const uint32_t* __restrict__ ids,
                                                                    const uint2* __restrict__ ranges, uint32_t n, double cell,
                                                                    uint32_t bucket_mask, float r2, uint32_t threshold,
-                                                                   float* __restrict__ pos_w, float* __restrict__ block_w,
-                                                                   uint32_t block_stride, uint32_t* __restrict__ selected) {
+                                                                   CloudView cloud, uint32_t* __restrict__ selected) {
     const uint32_t t = blockIdx.x * SEL_THREADS + threadIdx.x;
     bool sel = false;
     if (t < n) {
@@ -108,22 +107,16 @@ __global__ void __launch_bounds__(SEL_THREADS) select_count_kernel(const float4*
             }
         }
         sel = cnt < threshold;
-        const uint32_t i = ids[t];
-        const float v = sel ? 1.0f : 0.0f;
-        pos_w[(size_t)i * 4] = v;
-        block_w[(size_t)i * block_stride] = v;
+        cloud.store_visibility(ids[t], sel ? 1.0f : 0.0f);
     }
     const uint32_t ballot = __ballot_sync(0xffffffffu, sel);
     if ((threadIdx.x & 31) == 0 && ballot) atomicAdd(selected, (uint32_t)__popc(ballot));
 }
 
 // Every visibility set to `v` (threshold 0, or a radius whose square rounds to 0: no count can matter).
-__global__ void __launch_bounds__(SEL_THREADS) select_fill_kernel(uint32_t n, float v, float* __restrict__ pos_w,
-                                                                  float* __restrict__ block_w, uint32_t block_stride) {
+__global__ void __launch_bounds__(SEL_THREADS) select_fill_kernel(CloudView cloud, uint32_t n, float v) {
     const uint32_t i = blockIdx.x * SEL_THREADS + threadIdx.x;
-    if (i >= n) return;
-    pos_w[(size_t)i * 4] = v;
-    block_w[(size_t)i * block_stride] = v;
+    if (i < n) cloud.store_visibility(i, v);
 }
 
 // ---- host side -----------------------------------------------------------------------------------------------------
@@ -147,16 +140,15 @@ void launch_select_keys(const float4* pos, uint32_t n, float radius, uint32_t n_
     select_keys_kernel<<<sel_grid(n), SEL_THREADS, 0, stream>>>(pos, n, sel_cell_size(radius), n_buckets, keys, vals, n_sort);
 }
 
-void launch_select_count(const float4* pos, const uint32_t* ids, const uint2* ranges, uint32_t n, float radius, uint32_t n_buckets,
-                         float r2, uint32_t threshold, float4* spos, float* pos_w, float* block_w, uint32_t block_stride,
-                         uint32_t* selected, cudaStream_t stream) {
-    select_gather_kernel<<<sel_grid(n), SEL_THREADS, 0, stream>>>(pos, ids, n, spos);
+void launch_select_count(CloudView cloud, const uint32_t* ids, const uint2* ranges, uint32_t n, float radius, uint32_t n_buckets,
+                         float r2, uint32_t threshold, float4* spos, uint32_t* selected, cudaStream_t stream) {
+    select_gather_kernel<<<sel_grid(n), SEL_THREADS, 0, stream>>>(cloud.pos, ids, n, spos);
     select_count_kernel<<<sel_grid(n), SEL_THREADS, 0, stream>>>(spos, ids, ranges, n, sel_cell_size(radius), n_buckets - 1u, r2,
-                                                                 threshold, pos_w, block_w, block_stride, selected);
+                                                                 threshold, cloud, selected);
 }
 
-void launch_select_fill(uint32_t n, float v, float* pos_w, float* block_w, uint32_t block_stride, cudaStream_t stream) {
-    select_fill_kernel<<<sel_grid(n), SEL_THREADS, 0, stream>>>(n, v, pos_w, block_w, block_stride);
+void launch_select_fill(CloudView cloud, uint32_t n, float v, cudaStream_t stream) {
+    select_fill_kernel<<<sel_grid(n), SEL_THREADS, 0, stream>>>(cloud, n, v);
 }
 
 }  // namespace bgs

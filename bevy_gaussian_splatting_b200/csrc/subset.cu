@@ -1,9 +1,7 @@
 // subset.cu -- a resident cloud's gaussians copied into a new resident cloud (the reference's `cloud.subset(indices)`,
 // src/query/select.rs:156-176), and a resident cloud read back into the planar arrays its upload call takes.
 //
-// Both device copies of a gaussian move unchanged: its 16 B of the position plane and its gaussian-major block
-// (project.cu's repack_kernel: f16 layouts 128 B = pos | rot-scale-opacity or covariance record | 6 sh chunks, f32
-// 256 B = pos | rot | scale-opacity | 12 sh chunks | pad).
+// Both device copies of a gaussian (cloud_layout.cuh) move unchanged.
 //
 // Selection mode (kept iff !(visibility < 0.5f), the set DrawMode::Selected draws):
 //   1. subset_count_kernel: one thread per gaussian reads its position (16 B, coalesced); each warp ballots the
@@ -11,7 +9,7 @@
 //   2. subset_scan_kernel: one CTA turns the CTA counts into exclusive offsets and writes the total;
 //   3. (host: the total is read back and the new planes are allocated)
 //   4. subset_scatter_kernel: each warp walks its mask word; the kept gaussians' blocks are copied as 16 B chunks by
-//      CH lanes each (f16: 8 lanes = one 128 B line, f32: 16 lanes = two), in ascending index order.
+//      CH lanes each (one lane per chunk), in ascending index order.
 // Index mode: subset_gather_kernel copies gaussian indices[j] to j, CH threads per gaussian.
 // Download: unpack_kernel is repack_kernel's inverse over one chunk of gaussians, into planar staging arrays.
 #include "common.cuh"
@@ -77,19 +75,15 @@ __global__ void __launch_bounds__(1024) subset_scan_kernel(uint32_t* __restrict_
     if (threadIdx.x == 0) *total = carry;
 }
 
-// One 16 B chunk c of gaussian src's block (and, for c == 0, its position) to slot dst of the new cloud.
+// One 16 B chunk c of gaussian s's block (CH chunks) to gaussian d of the new cloud (the position chunk to both copies).
 template <uint32_t CH>
-__device__ __forceinline__ void subset_copy(const uint4* __restrict__ pos, const uint4* __restrict__ blocks, uint32_t src,
-                                            uint32_t dst, uint32_t c, uint4* __restrict__ out_pos, uint4* __restrict__ out_blocks) {
-    out_blocks[(size_t)dst * CH + c] = __ldg(blocks + (size_t)src * CH + c);
-    if (c == 0) out_pos[dst] = __ldg(pos + src);
+__device__ __forceinline__ void subset_copy(const CloudView& src, uint32_t s, uint32_t d, uint32_t c, const CloudView& dst) {
+    dst.store_chunk(d, c, __ldg(src.blocks + (size_t)s * CH + c));
 }
 
 template <uint32_t CH>
-__global__ void __launch_bounds__(SUBSET_THREADS) subset_scatter_kernel(const uint4* __restrict__ pos, const uint4* __restrict__ blocks,
-                                                                        uint32_t n_words, const uint32_t* __restrict__ mask,
-                                                                        const uint32_t* __restrict__ cta_off,
-                                                                        uint4* __restrict__ out_pos, uint4* __restrict__ out_blocks) {
+__global__ void __launch_bounds__(SUBSET_THREADS) subset_scatter_kernel(CloudView src, uint32_t n_words, const uint32_t* __restrict__ mask,
+                                                                        const uint32_t* __restrict__ cta_off, CloudView dst) {
     constexpr uint32_t G = 32u / CH;   // gaussians per warp pass
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const uint32_t word = blockIdx.x * SUBSET_WORDS_PER_CTA + warp;
@@ -101,37 +95,28 @@ __global__ void __launch_bounds__(SUBSET_THREADS) subset_scatter_kernel(const ui
     const uint32_t k = __popc(m), c = lane % CH;
     for (uint32_t j0 = 0; j0 < k; j0 += G) {
         const uint32_t j = j0 + lane / CH;
-        if (j < k) subset_copy<CH>(pos, blocks, word * 32u + __fns(m, 0, (int)j + 1), base + j, c, out_pos, out_blocks);
+        if (j < k) subset_copy<CH>(src, word * 32u + __fns(m, 0, (int)j + 1), base + j, c, dst);
     }
 }
 
 template <uint32_t CH>
-__global__ void __launch_bounds__(SUBSET_THREADS) subset_gather_kernel(const uint4* __restrict__ pos, const uint4* __restrict__ blocks,
-                                                                       const uint32_t* __restrict__ idx, uint32_t k,
-                                                                       uint4* __restrict__ out_pos, uint4* __restrict__ out_blocks) {
+__global__ void __launch_bounds__(SUBSET_THREADS) subset_gather_kernel(CloudView src, const uint32_t* __restrict__ idx, uint32_t k,
+                                                                       CloudView dst) {
     const size_t t = (size_t)blockIdx.x * SUBSET_THREADS + threadIdx.x;
     if (t >= (size_t)k * CH) return;
     const uint32_t j = (uint32_t)(t / CH), c = (uint32_t)(t % CH);
-    subset_copy<CH>(pos, blocks, __ldg(idx + j), j, c, out_pos, out_blocks);
+    subset_copy<CH>(src, __ldg(idx + j), j, c, dst);
 }
 
-// repack_kernel's inverse over gaussians [lo, lo + m): block chunk c of gaussian lo + j goes to sh[j * SHC + k], rot[j]
-// or so[j] (the position chunk and the f32 pad are skipped: the position plane is read back directly).
-template <bool F16>
+// repack_kernel's inverse over gaussians [lo, lo + m): block chunk c of gaussian lo + j goes back to its unit of
+// gaussian j in the planes (planes.pos is null: the position plane is read back directly).
+template <CloudLayout L>
 __global__ void __launch_bounds__(SUBSET_THREADS) unpack_kernel(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
-                                                                uint4* __restrict__ sh, uint4* __restrict__ rot, uint4* __restrict__ so) {
-    constexpr uint32_t CH = F16 ? 8u : 16u, SHC = F16 ? 6u : 12u;
+                                                                CloudPlanes<uint4> planes) {
     const size_t t = (size_t)blockIdx.x * SUBSET_THREADS + threadIdx.x;
-    if (t >= (size_t)m * CH) return;
-    const uint32_t j = (uint32_t)(t / CH), c = (uint32_t)(t % CH);
-    if (c == 0) return;
-    const uint4 v = __ldg(blocks + (size_t)lo * CH + t);
-    if (c == 1) rot[j] = v;
-    else if (!F16 && c == 2) so[j] = v;
-    else {
-        const uint32_t k = c - (F16 ? 2u : 3u);
-        if (k < SHC) sh[(size_t)j * SHC + k] = v;
-    }
+    if (t >= (size_t)m * chunks(L)) return;
+    uint4* dst = planes.unit<L>((uint32_t)(t % chunks(L)), t / chunks(L));
+    if (dst) *dst = __ldg(blocks + (size_t)lo * chunks(L) + t);
 }
 
 uint32_t subset_num_ctas(uint32_t n) { return (n + SUBSET_THREADS - 1) / SUBSET_THREADS; }
@@ -142,30 +127,30 @@ void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t
     subset_scan_kernel<<<1, 1024, 0, stream>>>(cta_cnt, g, total);
 }
 
-void launch_subset_scatter(bool f16, const void* pos, const void* blocks, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
-                           void* out_pos, void* out_blocks, cudaStream_t stream) {
+// (the copies depend on the layout only through the block's size: both f16 layouts run the same kernels)
+void launch_subset_scatter(CloudLayout layout, CloudView src, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
+                           CloudView dst, cudaStream_t stream) {
     const uint32_t g = subset_num_ctas(n), words = (n + 31) / 32;
-    if (f16) subset_scatter_kernel<8><<<g, SUBSET_THREADS, 0, stream>>>((const uint4*)pos, (const uint4*)blocks, words, mask, cta_off,
-                                                                         (uint4*)out_pos, (uint4*)out_blocks);
-    else subset_scatter_kernel<16><<<g, SUBSET_THREADS, 0, stream>>>((const uint4*)pos, (const uint4*)blocks, words, mask, cta_off,
-                                                                      (uint4*)out_pos, (uint4*)out_blocks);
+    with_layout(layout, [&](auto L) {
+        subset_scatter_kernel<chunks(decltype(L)::value)><<<g, SUBSET_THREADS, 0, stream>>>(src, words, mask, cta_off, dst);
+    });
 }
 
-void launch_subset_gather(bool f16, const void* pos, const void* blocks, const uint32_t* idx, uint32_t k, void* out_pos,
-                          void* out_blocks, cudaStream_t stream) {
-    const size_t total = (size_t)k * (f16 ? 8 : 16);
-    const uint32_t grid = (uint32_t)((total + SUBSET_THREADS - 1) / SUBSET_THREADS);
-    if (f16) subset_gather_kernel<8><<<grid, SUBSET_THREADS, 0, stream>>>((const uint4*)pos, (const uint4*)blocks, idx, k,
-                                                                           (uint4*)out_pos, (uint4*)out_blocks);
-    else subset_gather_kernel<16><<<grid, SUBSET_THREADS, 0, stream>>>((const uint4*)pos, (const uint4*)blocks, idx, k,
-                                                                        (uint4*)out_pos, (uint4*)out_blocks);
+static uint32_t chunk_grid(uint32_t n, uint32_t chunks) {
+    return (uint32_t)(((size_t)n * chunks + SUBSET_THREADS - 1) / SUBSET_THREADS);
 }
 
-void launch_unpack(bool f16, const void* blocks, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream) {
-    const size_t total = (size_t)m * (f16 ? 8 : 16);
-    const uint32_t grid = (uint32_t)((total + SUBSET_THREADS - 1) / SUBSET_THREADS);
-    if (f16) unpack_kernel<true><<<grid, SUBSET_THREADS, 0, stream>>>((const uint4*)blocks, lo, m, (uint4*)sh, (uint4*)rot, (uint4*)so);
-    else unpack_kernel<false><<<grid, SUBSET_THREADS, 0, stream>>>((const uint4*)blocks, lo, m, (uint4*)sh, (uint4*)rot, (uint4*)so);
+void launch_subset_gather(CloudLayout layout, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst, cudaStream_t stream) {
+    with_layout(layout, [&](auto L) {
+        subset_gather_kernel<chunks(decltype(L)::value)><<<chunk_grid(k, src.chunks), SUBSET_THREADS, 0, stream>>>(src, idx, k, dst);
+    });
+}
+
+void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream) {
+    const CloudPlanes<uint4> planes{nullptr, static_cast<uint4*>(sh), static_cast<uint4*>(rot), static_cast<uint4*>(so)};
+    with_layout(layout, [&](auto L) {
+        unpack_kernel<decltype(L)::value><<<chunk_grid(m, cloud.chunks), SUBSET_THREADS, 0, stream>>>(cloud.blocks, lo, m, planes);
+    });
 }
 
 }  // namespace bgs
