@@ -68,6 +68,14 @@ class bgs_render_extras(C.Structure):
     ]
 
 
+class bgs_scene_depth(C.Structure):
+    """The scene's Depth32Float depth buffer a frame is depth-tested against (bgs_render_depth_test)."""
+    _fields_ = [
+        ("depth", C.c_void_p),
+        ("pitch_bytes", C.c_uint64),
+    ]
+
+
 class bgs_frame_stats(C.Structure):
     _fields_ = [
         ("n", C.c_uint32),
@@ -118,6 +126,8 @@ SYMBOLS = [
                              C.c_uint32, C.c_int]),
     ("bgs_render_ex", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings),
                                 C.POINTER(bgs_render_extras), _P, C.c_uint32, C.c_int]),
+    ("bgs_render_depth_test", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings),
+                                        C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,
                                  C.c_uint32, C.c_int]),
     ("bgs_sync", C.c_int, [_P]),
@@ -125,6 +135,7 @@ SYMBOLS = [
     ("bgs_debug_tile_ranges", C.c_int, [_P, _P]),
     ("bgs_debug_tile_entries", C.c_int, [_P, _P, C.c_uint64]),
     ("bgs_debug_projected", C.c_int, [_P, _P, _P]),
+    ("bgs_debug_splat_depths", C.c_int, [_P, _P]),
     ("bgs_frame_stats_get", C.c_int, [_P, C.POINTER(bgs_frame_stats)]),
     ("bgs_stage_times_us", C.c_int, [_P, C.POINTER(C.c_float * 6)]),
     ("bgs_last_error", C.c_char_p, [_P]),

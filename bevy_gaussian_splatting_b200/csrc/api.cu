@@ -442,7 +442,7 @@ static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, co
 
 // Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.
 static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const ModeConsts* modes,
-                                const FramePlan& p, const FrameOut& o) {
+                                const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd) {
     const uint32_t n = cloud->n;
     const uint32_t num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     cudaStream_t q = c->stream;
@@ -488,6 +488,14 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
                    fc.aux ? c->aux.p : nullptr, modes, ps);
     ++launches;
     CU(c, cudaEventRecord(c->ev_p1, ps));
+    // depth-tested frames: the splat depths, indexed like the records (the projection's index list)
+    ZTestArgs zt;
+    if (zd) {
+        launch_splat_depth(cloud->pos, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
+                           c->splat_depth.p, p.n_hint, c->sm_count, ps);
+        ++launches;
+        zt.splat_d = c->splat_depth.p; zt.scene = zd->depth; zt.pitch = (size_t)zd->pitch_bytes;
+    }
     if (p.overlap) {
         CU(c, cudaEventRecord(c->ev_join, c->stream2));
         CU(c, cudaStreamWaitEvent(q, c->ev_join, 0));
@@ -525,12 +533,13 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
             launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
                           fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal, &c->ctr->truncated,
-                          c->stream_r);
+                          zt, c->stream_r);
             CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
             CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
         } else
             launch_raster_round(c->recs.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x, fc.tiles_y, o.rgba, o.raster_format,
-                                c->state.p, c->tile_done, &c->ctr->tiles_done, &c->ctr->truncated, r == 0, r + 1 == p.rounds, q);
+                                c->state.p, c->tile_done, &c->ctr->tiles_done, &c->ctr->truncated, r == 0, r + 1 == p.rounds, zt,
+                                q);
         ++launches;
     }
     c->pair_result = pcur;
@@ -551,16 +560,37 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaMemcpyAsync(o.host_normal, o.normal, o.bytes, cudaMemcpyDeviceToHost, q));
         }
     }
-    c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, fc.tiles_x, fc.tiles_y, fc.Wi, fc.Hi, o.rgba};
+    c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, fc.tiles_x, fc.tiles_y, fc.Wi, fc.Hi, o.rgba, zd != nullptr};
     c->launches = launches;
+    return BGS_OK;
+}
+
+// bgs_render_depth_test's refusals (include/bgs.h): the buffer must be 4-byte aligned device memory of the context's GPU
+// with a pitch that holds a row of the viewport
+static bgs_status check_scene_depth(bgs_context* c, const bgs_scene_depth* zd, const bgs_view* view) {
+    const uint64_t W = (uint64_t)view->viewport[2];
+    if (!zd->depth) return fail(c, BGS_EINVAL, "render_depth_test: depth->depth is NULL");
+    if (zd->pitch_bytes % 4 != 0 || zd->pitch_bytes < 4 * W)
+        return fail(c, BGS_EINVAL, "render_depth_test: pitch %llu is not a multiple of 4 of at least 4 w = %llu",
+                    (unsigned long long)zd->pitch_bytes, (unsigned long long)(4 * W));
+    if (reinterpret_cast<uintptr_t>(zd->depth) % 4 != 0)
+        return fail(c, BGS_EINVAL, "render_depth_test: depth buffer %p is not 4-byte aligned", (const void*)zd->depth);
+    cudaPointerAttributes a = {};
+    const cudaError_t e = cudaPointerGetAttributes(&a, zd->depth);
+    if (e != cudaSuccess) cudaGetLastError();   // (an unknown pointer: clear the error, refuse below)
+    if (e != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != c->device)
+        return fail(c, BGS_EINVAL, "render_depth_test: depth buffer %p is not device memory of device %d", (const void*)zd->depth,
+                    c->device);
     return BGS_OK;
 }
 
 static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                               const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
-                              int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal) {
+                              int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal,
+                              const bgs_scene_depth* zd = nullptr) {
     if (!c) return BGS_EINVAL;
     TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux));
+    if (zd) TRY(check_scene_depth(c, zd, view));
     if (c->async_pending && !(st->flags & BGS_FLAG_ASYNC)) {
         // a synchronous render after queued frames completes them first; their failure (including an overflowed
         // pair list = BGS_NOT_READY) is the caller's to see, so this frame is not rendered on top of it
@@ -582,11 +612,12 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         const FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
         if (p.raster_mode == 2) TRY(c->extra.grow(c, (size_t)c->cap_n * 64, false));
         if (want_aux) TRY(c->aux.grow(c, (size_t)c->cap_n * 32, false));
+        if (zd) TRY(c->splat_depth.grow(c, (size_t)c->cap_n * 4, false));
         if (p.rounds > 1) TRY(c->state.grow(c, (size_t)num_tiles * 256 * sizeof(float4), false));
         TRY(ensure_arena(c, num_tiles));
         TRY(ensure_status(c, c->status_depth, c->status_n, n));
         TRY(ensure_status(c, c->status_pairs, c->status_np, c->cap_pairs));
-        TRY(enqueue_frame(c, cloud, fc, modes, p, o));
+        TRY(enqueue_frame(c, cloud, fc, modes, p, o, zd));
         if (st->flags & BGS_FLAG_ASYNC) {
             c->async_pending = true;
             c->have_frame = false;     // hooks need bgs_sync() first
@@ -606,6 +637,12 @@ bgs_status bgs_render_ex(bgs_context* c, const bgs_cloud* cloud, const bgs_view*
                          const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
                          int out_is_device_ptr) {
     return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr);
+}
+
+bgs_status bgs_render_depth_test(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                                 const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                                 void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth);
 }
 
 bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
@@ -711,6 +748,20 @@ bgs_status bgs_debug_projected(bgs_context* c, float* records, uint32_t* rank_to
     }
     if (rank_to_index)
         for (uint32_t r = 0; r < n_vis; ++r) rank_to_index[r] = c->last.by_slot ? ids[v[n_vis - 1 - r]] : v[n_vis - 1 - r];
+    return BGS_OK;
+}
+
+bgs_status bgs_debug_splat_depths(bgs_context* c, float* out) {
+    if (!c || !out) return BGS_EINVAL;
+    if (!c->have_frame || !c->last.depth_tested) return fail(c, BGS_NOT_READY, "no depth-tested frame rendered yet");
+    CU(c, cudaSetDevice(c->device));
+    const uint32_t n_vis = c->stats.n_visible;
+    std::vector<float> d(n_vis);
+    CU(c, cudaMemcpy(d.data(), c->splat_depth.p, (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
+    if (!c->last.by_slot) { std::copy(d.begin(), d.end(), out); return BGS_OK; }
+    std::vector<uint32_t> v(n_vis);   // compact frames: rank r's record is at the slot the sort put at n_vis - 1 - r
+    CU(c, cudaMemcpy(v.data(), c->vals[c->depth_result].p, (size_t)n_vis * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t r = 0; r < n_vis; ++r) out[r] = d[v[n_vis - 1 - r]];
     return BGS_OK;
 }
 

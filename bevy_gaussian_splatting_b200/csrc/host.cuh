@@ -71,6 +71,7 @@ struct FrameFacts {
     int rounds = 1;                     // binning rounds
     int tiles_x = 0, tiles_y = 0, W = 0, H = 0;
     const void* target = nullptr;       // the device frame the blend wrote
+    bool depth_tested = false;          // bgs_render_depth_test with a depth buffer: splat_depth holds the splats' d
 };
 
 struct bgs_context {
@@ -106,6 +107,7 @@ struct bgs_context {
     DevBuf<SplatRec> recs;
     DevBuf<float4> extra;             // 4 x float4 per record: 2DGS + USE_AABB only (allocated on first use)
     DevBuf<float4> aux;               // 2 x float4 per record: depth / normal colour sources (bgs_render_aux only)
+    DevBuf<float> splat_depth;        // 1 float per record: the splat depths d of depth-tested frames (allocated on first use)
     DevBuf<void> frame_aux[2];        // depth / normal frames when bgs_render_aux delivers to host memory
     // scratch sized by the pair capacity (grow-only; cap_pairs pairs)
     uint32_t cap_pairs = 0;

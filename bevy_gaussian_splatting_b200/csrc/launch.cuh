@@ -36,13 +36,24 @@ cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, Fra
                                  int tiles_x, uint32_t capacity, uint32_t* pair_keys, uint32_t* pair_vals,
                                  uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, uint32_t grid,
                                  uint32_t* sticky_need, cudaStream_t stream);
-// raster.cu
+// scene_depth.cu
+void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+                        const FrameConsts& fc, float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
+// raster.cu.  ZTestArgs: a depth-tested frame's splat depths (indexed like the records) and the scene's depth buffer
+// (bgs_scene_depth); scene == nullptr blends without the test.
+struct ZTestArgs {
+    const float* splat_d = nullptr;
+    const float* scene = nullptr;
+    size_t pitch = 0;
+};
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
-                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, cudaStream_t stream);
+                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
+                   cudaStream_t stream);
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
-                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, cudaStream_t stream);
+                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,
+                         cudaStream_t stream);
 // select.cu
 uint32_t select_num_buckets(uint32_t n);
 int select_sort_passes(uint32_t n_buckets);

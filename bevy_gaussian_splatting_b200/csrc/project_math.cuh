@@ -33,14 +33,30 @@ __device__ __forceinline__ void keygen_world_pos(const FrameConsts& c, float4 p,
     }
 }
 
-// transform.wgsl:5-14, literal: world_to_clip (three IEEE divisions by w + 1e-9) and in_frustum.
-__device__ __forceinline__ bool in_frustum(const FrameConsts& c, const float pw[3], float ndc[2]) {
+// transform.wgsl:5-8, literal: world_to_clip, clip_from_world (p, 1) with every lane divided (IEEE) by w + 1e-9.
+// (Callers that read only some lanes leave the other divisions to dead-code elimination.)
+__device__ __forceinline__ void world_to_clip(const FrameConsts& c, const float pw[3], float out[4]) {
     float cl[4];
     mat4_point(c.clip_from_world, pw[0], pw[1], pw[2], cl);
     const float den = cl[3] + 0.000000001f;
-    const float nx = cl[0] / den, ny = cl[1] / den, nz = cl[2] / den;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) out[i] = cl[i] / den;
+}
+
+// transform.wgsl:10-14, literal: in_frustum of world_to_clip's x, y, z.
+__device__ __forceinline__ bool in_frustum(const FrameConsts& c, const float pw[3], float ndc[2]) {
+    float h[4];
+    world_to_clip(c, pw, h);
+    const float nx = h[0], ny = h[1], nz = h[2];
     ndc[0] = nx; ndc[1] = ny;
     return fabsf(nx) < 1.1f && fabsf(ny) < 1.1f && fabsf(nz - 0.5f) < 0.5f;
+}
+
+// bgs_render_depth_test's splat depth (include/bgs.h): world_to_clip's z over its w.
+__device__ __forceinline__ float splat_depth(const FrameConsts& c, const float pw[3]) {
+    float h[4];
+    world_to_clip(c, pw, h);
+    return h[2] / h[3];
 }
 
 // in_frustum's decision, cheaper, for key-gen (which needs no ndc): one approximate reciprocal (|error| < 4e-7

@@ -175,6 +175,10 @@ constexpr uint32_t SM_EXTRA = SM_LIST + (RT_THREADS / 32) * RT_CHUNK * 2;   // M
 constexpr uint32_t SM_BYTES = SM_EXTRA;
 constexpr uint32_t SM_BYTES_2D = SM_EXTRA + 4 * RT_CHUNK * 16;
 // AUX (bgs_render_aux): 2 x float4 [256] after the mode's own arrays: depth rgb, normal rgb of the staged splats
+// ZTEST (bgs_render_depth_test): float [256] at a 16 B stride after the mode's own arrays: the staged splats' depths d,
+// at the same offset from a splat's q0 record for every splat (what the candidate lists hold), so the blend loops reach
+// d with one load from the record address
+constexpr uint32_t ZT_BYTES = RT_CHUNK * 16;
 
 // a staged splat's uv and q2 records, as offsets from the shared address of its q0 record (what the candidate lists hold)
 constexpr uint32_t REC_UV = SM_UV - SM_Q0, REC_Q2 = SM_Q2 - SM_Q0;
@@ -198,6 +202,21 @@ __device__ __forceinline__ float2 quad_uv(float fx, float fy, float4 q0, float2 
     return make_float2(__fmaf_rn(q0.w, dy, __fmul_rn(q0.z, dx)), __fmaf_rn(q1.y, dy, __fmul_rn(q1.x, dx)));
 }
 
+// bgs_render_depth_test: the scene depth of pixel (px, py), row pitch in bytes; pixels outside the frame are never read
+// and get NaN, which the warp's minimum ignores and which blends nothing (those pixels are stopped from the start)
+__device__ __forceinline__ float scene_depth_at(const float* scene, size_t pitch, int px, int py, bool inside) {
+    return inside ? __ldg(reinterpret_cast<const float*>(reinterpret_cast<const char*>(scene) + (size_t)py * pitch) + px)
+                  : __uint_as_float(0x7FC00000u);
+}
+// the minimum over the warp's pixels, NaN ignored (fminf): a splat whose d is below it fails d >= scene at every pixel of
+// the warp's rectangle, so the candidate compaction may drop it without changing any decision
+__device__ __forceinline__ float warp_min_depth(float z) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) z = fminf(z, __shfl_xor_sync(0xffffffffu, z, o));
+    return z;
+}
+__device__ __forceinline__ float lds_f32(uint32_t a) { float r; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(a)); return r; }
+
 // Each warp compacts the chunk's `cnt` staged splats to those `hit(j)` keeps, in order, into its u16 list as
 // `rec0 + j * 16` (the q0 record's address relative to rec0); returns the list's length.
 template <class Hit>
@@ -220,14 +239,20 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // MODE 2: 2DGS USE_AABB ray-splat intersection                     gaussian.wgsl:441-458, gaussian_2d.wgsl:134-156
 // AUX: the same pass also blends the splats' Depth and Normal colour sources (aux records, 2 x float4 per splat) into two
 // more frames with the very same alphas: config C4's colour + depth + normal outputs cost one pass, not three.
-template <int MODE, bool AUX>
+// ZTEST (MODE 0, 1, 2 without AUX): bgs_render_depth_test.  A pair blends only where its coverage decision holds and
+// d >= the pixel's scene depth; the warp's candidates leave out the splats below the scene everywhere in its rectangle.
+template <int MODE, bool AUX, bool ZTEST = false>
 __global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : 5)
 raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
               const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
               const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
-              const uint32_t* __restrict__ truncated) {
-    __shared__ __align__(16) unsigned char s_mem[(MODE == 2 ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0)];
+              const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
+              size_t pitch) {
+    static_assert(!(AUX && ZTEST), "bgs_render_aux takes no depth buffer");
+    __shared__ __align__(16) unsigned char s_mem[(MODE == 2 ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0) +
+                                                 (ZTEST ? ZT_BYTES : 0)];
     constexpr uint32_t SM_AUX = MODE == 2 ? SM_BYTES_2D : SM_BYTES;
+    constexpr uint32_t REC_D = SM_AUX;   // ZTEST: d of the splat whose q0 record is at a, at a + REC_D
     __shared__ __align__(16) uint32_t s_ent[2][ENT_WORDS];    // TMA destination: the tile's pair-list chunks
     __shared__ __align__(8) unsigned long long s_bar[2];
     __shared__ __align__(8) float2 s_thr[MODE == 0 ? RT_CHUNK : 1];   // MODE 0: per staged splat cull thresholds (u, v)
@@ -268,6 +293,11 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
     }
     // tiles with more than one chunk stream their pair list (the next chunk's copy overlaps this chunk's blending)
     PairStream ps(tile_entries, s_ent, s_bar, range, range.y - range.x > (uint32_t)RT_CHUNK);
+    float zs = 0.0f, zmin = 0.0f;   // ZTEST: this pixel's scene depth, the minimum over the warp's pixels
+    if (ZTEST) {
+        zs = scene_depth_at(scene, pitch, px, py, inside);
+        zmin = warp_min_depth(zs);
+    }
 
     float T = inside ? 1.0f : 0.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f;   // T < T_STOP <=> this pixel is done
     float dr = 0.0f, dg = 0.0f, db = 0.0f, nr = 0.0f, ng = 0.0f, nb = 0.0f;   // AUX: depth / normal frames
@@ -303,6 +333,7 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                 s_ax[t] = __ldg(aux + (size_t)r * 2);
                 s_ax[RT_CHUNK + t] = __ldg(aux + (size_t)r * 2 + 1);
             }
+            if (ZTEST) reinterpret_cast<float*>(s_mem + REC_D)[4 * t] = __ldg(splat_d + r);
         }
         __syncthreads();
         // each warp's candidates: the splats whose bbox touches its 8x4 pixels, listed by shared address of q0[j]
@@ -321,6 +352,7 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                 const float dxc = rcx - p.x, dyc = rcy - p.y;
                 hit = !(fabsf(p.z * dxc + p.w * dyc) > th.x || fabsf(q.x * dxc + q.y * dyc) > th.y);
             }
+            if (ZTEST && hit) hit = !(reinterpret_cast<const float*>(s_mem + REC_D)[4 * j] < zmin);
             return hit;
         });
         if (MODE == 0 && !AUX) {
@@ -334,36 +366,51 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
             const uint32_t a_end = a_list + nl * 2u;
             uint32_t a_it = a_list;
             float lim = (T < T_STOP) ? -1.0f : 1.0f;
-            auto blend_if_covered = [&](uint32_t a_rec, float2 uv) {
-                asm volatile(
-                    "{\n\t"
-                    ".reg .pred p, q;\n\t"
-                    ".reg .f32 au, av, x, y, z, o, qd, e, a, w, na;\n\t"
-                    "abs.f32 au, %5;\n\t"
-                    "abs.f32 av, %6;\n\t"
-                    "setp.le.f32 p, au, %4;\n\t"
+            // ZTEST: one more load and one more `setp ... .and`: the pair blends only where d >= the scene depth (%9)
+#define BLEND_COVER_                                                                                                    \
+                    "{\n\t"                                                                                             \
+                    ".reg .pred p, q;\n\t"                                                                              \
+                    ".reg .f32 au, av, x, y, z, o, qd, e, a, w, na;\n\t"                                                \
+                    "abs.f32 au, %5;\n\t"                                                                               \
+                    "abs.f32 av, %6;\n\t"                                                                               \
+                    "setp.le.f32 p, au, %4;\n\t"                                                                        \
                     "setp.le.and.f32 p, av, %4, p;\n\t"
+#define BLEND_ZTEST_                                                                                                    \
+                    ".reg .f32 dz;\n\t"                                                                                \
+                    "ld.shared.f32 dz, [%7+%10];\n\t"                                                                   \
+                    "setp.ge.and.f32 p, dz, %9, p;\n\t"
                     // (the temporaries are computed unconditionally -- a predicated definition would keep their old values
                     // alive across iterations -- only the four accumulations are predicated)
-                    "ld.shared.v4.f32 {x, y, z, o}, [%7+%8];\n\t"
-                    "mul.rn.f32 qd, %5, %5;\n\t"
-                    "fma.rn.f32 qd, %6, %6, qd;\n\t"
-                    "mul.rn.f32 qd, qd, 0fC0CFBF83;\n\t"             // -6.492127684f: exp(-4.5 qd) = 2^(qd * -4.5 log2 e)
-                    "ex2.approx.ftz.f32 e, qd;\n\t"
-                    "mul.rn.f32 a, e, o;\n\t"
-                    "min.f32 a, a, 0f3F7FBE77;\n\t"                 // 0.999f
-                    "mul.rn.f32 w, a, %0;\n\t"
-                    "neg.f32 na, a;\n\t"
-                    "@p fma.rn.f32 %1, w, x, %1;\n\t"
-                    "@p fma.rn.f32 %2, w, y, %2;\n\t"
-                    "@p fma.rn.f32 %3, w, z, %3;\n\t"
-                    "@p fma.rn.f32 %0, na, %0, %0;\n\t"
-                    "setp.lt.and.f32 q, %0, 0f38D1B717, p;\n\t"     // T < T_STOP (1e-4f) after a blend: the pixel stops
-                    "@q mov.f32 %4, 0fBF800000;\n\t"
+#define BLEND_ACCUMULATE_                                                                                               \
+                    "ld.shared.v4.f32 {x, y, z, o}, [%7+%8];\n\t"                                                       \
+                    "mul.rn.f32 qd, %5, %5;\n\t"                                                                        \
+                    "fma.rn.f32 qd, %6, %6, qd;\n\t"                                                                    \
+                    "mul.rn.f32 qd, qd, 0fC0CFBF83;\n\t"     /* -6.492127684f: exp(-4.5 qd) = 2^(qd * -4.5 log2 e) */  \
+                    "ex2.approx.ftz.f32 e, qd;\n\t"                                                                     \
+                    "mul.rn.f32 a, e, o;\n\t"                                                                           \
+                    "min.f32 a, a, 0f3F7FBE77;\n\t"          /* 0.999f */                                               \
+                    "mul.rn.f32 w, a, %0;\n\t"                                                                          \
+                    "neg.f32 na, a;\n\t"                                                                                \
+                    "@p fma.rn.f32 %1, w, x, %1;\n\t"                                                                   \
+                    "@p fma.rn.f32 %2, w, y, %2;\n\t"                                                                   \
+                    "@p fma.rn.f32 %3, w, z, %3;\n\t"                                                                   \
+                    "@p fma.rn.f32 %0, na, %0, %0;\n\t"                                                                 \
+                    "setp.lt.and.f32 q, %0, 0f38D1B717, p;\n\t"   /* T < T_STOP (1e-4f) after a blend: the pixel stops */ \
+                    "@q mov.f32 %4, 0fBF800000;\n\t"                                                                    \
                     "}"
-                    : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb), "+f"(lim)
-                    : "f"(uv.x), "f"(uv.y), "r"(a_rec), "n"(REC_Q2));
+            auto blend_if_covered = [&](uint32_t a_rec, float2 uv) {
+                if constexpr (ZTEST)
+                    asm volatile(BLEND_COVER_ BLEND_ZTEST_ BLEND_ACCUMULATE_
+                                 : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb), "+f"(lim)
+                                 : "f"(uv.x), "f"(uv.y), "r"(a_rec), "n"(REC_Q2), "f"(zs), "n"(REC_D));
+                else
+                    asm volatile(BLEND_COVER_ BLEND_ACCUMULATE_
+                                 : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb), "+f"(lim)
+                                 : "f"(uv.x), "f"(uv.y), "r"(a_rec), "n"(REC_Q2));
             };
+#undef BLEND_COVER_
+#undef BLEND_ZTEST_
+#undef BLEND_ACCUMULATE_
             for (; a_it + 2u < a_end; a_it += 4u) {
                 const uint32_t two = lds_u32(a_it);
                 const uint32_t ra = two & 0xFFFFu, rb = two >> 16;
@@ -385,11 +432,13 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                 const uint32_t a_rec = lds_u16(a_it);
                 const float4 q0 = lds4(a_rec);
                 const float2 q1 = lds2(a_rec + REC_UV);
+                // ZTEST: the depth test joins each mode's coverage test (d >= scene; a NaN on either side fails)
+                auto depth_ok = [&]() { return !ZTEST || lds_f32(a_rec + REC_D) >= zs; };
                 float e;
                 float4 q2;
                 if (MODE == 0) {
                     const float2 uv = quad_uv(fx, fy, q0, q1);
-                    if (!(fabsf(uv.x) <= 1.0f && fabsf(uv.y) <= 1.0f)) continue;
+                    if (!(fabsf(uv.x) <= 1.0f && fabsf(uv.y) <= 1.0f && depth_ok())) continue;
                     const float qd = __fmaf_rn(uv.y, uv.y, __fmul_rn(uv.x, uv.x));
                     q2 = lds4(a_rec + REC_Q2);
                     // exp(-4.5 qd) = 2^(qd * -4.5 log2 e); qd <= 2 so the argument stays >= -13 (no range fix-up)
@@ -401,14 +450,14 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                     const float Rq = q1.y;   // MODE 1: quad half-side in half-pixels
                     float power;
                     if (MODE == 1) {
-                        if (!(fabsf(mx) <= Rq && fabsf(my) <= Rq)) continue;
+                        if (!(fabsf(mx) <= Rq && fabsf(my) <= Rq && depth_ok())) continue;
                         // q0.z, q0.w, q1.x = conic x, y, z;  d = -m  (gaussian.wgsl:459-462)
                         const float ddx = -mx, ddy = -my;
                         const float t1 = __fmul_rn(__fmul_rn(q0.z, ddx), ddx), t2 = __fmul_rn(__fmul_rn(q1.x, ddy), ddy);
                         power = __fadd_rn(__fmul_rn(-0.5f, __fadd_rn(t1, t2)), __fmul_rn(__fmul_rn(q0.w, ddx), ddy));
                     } else {
                         const float4 e0 = lds4(a_rec + SM_EXTRA);
-                        if (!(fabsf(mx) <= e0.x && fabsf(my) <= e0.x)) continue;
+                        if (!(fabsf(mx) <= e0.x && fabsf(my) <= e0.x && depth_ok())) continue;
                         const float4 e1 = lds4(a_rec + SM_EXTRA + RT_CHUNK * 16);
                         const float4 e2 = lds4(a_rec + SM_EXTRA + 2 * RT_CHUNK * 16);
                         const float4 e3 = lds4(a_rec + SM_EXTRA + 3 * RT_CHUNK * 16);
@@ -487,13 +536,16 @@ __device__ __forceinline__ void store_pixel2(void* out, uint32_t format, size_t 
     }
 }
 
-template <bool CHUNKED>
+// ZTEST: bgs_render_depth_test, as raster_kernel's (each pixel of the pair has its own scene depth; the warp's rectangle
+// for the candidate cull is its 16x4 pixels)
+template <bool CHUNKED, bool ZTEST = false>
 __global__ void __launch_bounds__(R2_THREADS)
 raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges,
                int W, int H, int tiles_x, void* __restrict__ out, uint32_t format, float4* __restrict__ state,
                unsigned char* __restrict__ tile_done, uint32_t* __restrict__ tiles_done, const uint32_t* __restrict__ truncated,
-               int first, int last) {
-    __shared__ __align__(16) unsigned char s_mem[R2_BYTES];
+               int first, int last, const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch) {
+    __shared__ __align__(16) unsigned char s_mem[R2_BYTES + (ZTEST ? ZT_BYTES : 0)];
+    constexpr uint32_t REC_D = R2_BYTES;   // ZTEST: d of the splat whose q0 record is at a, at a + REC_D
     float4* s_q0 = reinterpret_cast<float4*>(s_mem + SM_Q0);
     float4* s_uv = reinterpret_cast<float4*>(s_mem + SM_UV);
     float4* s_q2 = reinterpret_cast<float4*>(s_mem + SM_Q2);
@@ -533,6 +585,13 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
             if (done) range.y = range.x;
         }
     }
+    // ZTEST: the scene depths of the two pixels (read again by every round of a chunked frame), the warp's minimum
+    float zs0 = 0.0f, zs1 = 0.0f, zmin = 0.0f;
+    if (ZTEST) {
+        zs0 = scene_depth_at(scene, pitch, px0, py, in0);
+        zs1 = scene_depth_at(scene, pitch, px0 + 1, py, in1);
+        zmin = warp_min_depth(fminf(zs0, zs1));
+    }
     // multi-chunk tiles (the norm on this path: heavy footprints put thousands of entries in a tile) stream their slice
     // of the sorted pair list, like raster_kernel
     __shared__ __align__(16) uint32_t s_ent[2][ENT_WORDS];
@@ -551,6 +610,7 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
                 s_q0[j] = __ldg(rp);
                 s_uv[j] = __ldg(rp + 1);
                 s_q2[j] = __ldg(rp + 2);
+                if (ZTEST) reinterpret_cast<float*>(s_mem + REC_D)[4 * j] = __ldg(splat_d + r);
             }
         }
         __syncthreads();
@@ -558,7 +618,8 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
         // listed by offset of q0[j] from s_mem
         const uint32_t nl = !__any_sync(0xffffffffu, lim0 > 0.f || lim1 > 0.f) ? 0u : compact_candidates(cnt, s_list, 0u, [&](uint32_t j) {
             const uint32_t by = __float_as_uint(s_uv[j].w);
-            return !((int)(by >> 16) < wy0 || (int)(by & 0xFFFFu) > wy0 + 3);
+            const bool hit = !((int)(by >> 16) < wy0 || (int)(by & 0xFFFFu) > wy0 + 3);
+            return ZTEST ? hit && !(reinterpret_cast<const float*>(s_mem + REC_D)[4 * j] < zmin) : hit;
         });
         if (lim0 > 0.f || lim1 > 0.f) {
             const uint32_t a_end = a_list + nl * 2u;
@@ -567,8 +628,13 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
                 const float4 q0 = lds4(a_rec);
                 const float2 q1 = lds2(a_rec + REC_UV);
                 const float2 uva = quad_uv(fx0, fy, q0, q1), uvb = quad_uv(fx1, fy, q0, q1);   // (dy is computed once)
-                const bool ca = fabsf(uva.x) <= lim0 && fabsf(uva.y) <= lim0;
-                const bool cb = fabsf(uvb.x) <= lim1 && fabsf(uvb.y) <= lim1;
+                bool ca = fabsf(uva.x) <= lim0 && fabsf(uva.y) <= lim0;
+                bool cb = fabsf(uvb.x) <= lim1 && fabsf(uvb.y) <= lim1;
+                if (ZTEST) {
+                    const float d = lds_f32(a_rec + REC_D);
+                    ca = ca && d >= zs0;
+                    cb = cb && d >= zs1;
+                }
                 if (!(ca || cb)) continue;
                 const float4 q2 = lds4(a_rec + REC_Q2);
                 if (ca) {
@@ -609,30 +675,38 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
 
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
-                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, cudaStream_t stream) {
+                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
+                   cudaStream_t stream) {
     const int grid = tiles_x * tiles_y;
+    const bool ztest = zt.scene != nullptr;   // (bgs_render_aux frames never carry a depth buffer)
     // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
     // pixels (more of its lanes then idle at the tile's splat boundaries)
     if (aux == nullptr && mode == 0 && large_footprints) {
-        raster2_kernel<false><<<grid, R2_THREADS, 0, stream>>>(recs, tile_entries, ranges, W, H, tiles_x, out, format,
-                                                               nullptr, nullptr, nullptr, truncated, 1, 1);
+        (ztest ? raster2_kernel<false, true> : raster2_kernel<false, false>)<<<grid, R2_THREADS, 0, stream>>>(
+            recs, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr, truncated, 1, 1, zt.splat_d,
+            zt.scene, zt.pitch);
         return;
     }
     // aux != nullptr: colour + depth + normal in one pass (bgs_render_aux)
-    static void (*const kernels[2][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*,
-                                       uint32_t, const float4*, void*, void*, const uint32_t*) = {
+    static void (*const kernels[3][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*,
+                                       uint32_t, const float4*, void*, void*, const uint32_t*, const float*, const float*,
+                                       size_t) = {
         {raster_kernel<0, false>, raster_kernel<1, false>, raster_kernel<2, false>},
-        {raster_kernel<0, true>, raster_kernel<1, true>, raster_kernel<2, true>}};
-    kernels[aux != nullptr][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
-        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated);
+        {raster_kernel<0, true>, raster_kernel<1, true>, raster_kernel<2, true>},
+        {raster_kernel<0, false, true>, raster_kernel<1, false, true>, raster_kernel<2, false, true>}};
+    kernels[ztest ? 2 : aux != nullptr][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
+        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated, zt.splat_d,
+        zt.scene, zt.pitch);
 }
 
 // One front-to-back round of a chunked frame (quad-uv records only); see raster2_kernel.
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
-                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, cudaStream_t stream) {
-    raster2_kernel<true><<<tiles_x * tiles_y, R2_THREADS, 0, stream>>>(recs, tile_entries, ranges, W, H, tiles_x, out, format,
-                                                                       state, tile_done, tiles_done, truncated, first, last);
+                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,
+                         cudaStream_t stream) {
+    (zt.scene ? raster2_kernel<true, true> : raster2_kernel<true, false>)<<<tiles_x * tiles_y, R2_THREADS, 0, stream>>>(
+        recs, tile_entries, ranges, W, H, tiles_x, out, format, state, tile_done, tiles_done, truncated, first, last,
+        zt.splat_d, zt.scene, zt.pitch);
 }
 
 }  // namespace bgs

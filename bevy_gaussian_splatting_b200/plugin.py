@@ -28,6 +28,50 @@ def _ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def scene_depth_arg(scene_depth, width: int, height: int) -> tuple[abi.bgs_scene_depth | None, int | None]:
+    """(`bgs_scene_depth`, producer stream) for any object with `__cuda_array_interface__` (a torch CUDA tensor, a CuPy
+    array, ...): float32, shape (height, width), rows contiguous, the row stride taken from the interface.  The producer
+    stream is the interface's (v3) "stream" entry, None when it names none.  None -> (None, None)."""
+    if scene_depth is None:
+        return None, None
+    cai = getattr(scene_depth, "__cuda_array_interface__", None)
+    if cai is None:
+        raise TypeError("scene_depth must expose __cuda_array_interface__ (device memory)")
+    if np.dtype(cai["typestr"]) != np.dtype("<f4"):
+        raise TypeError(f"scene_depth must be float32, not {cai['typestr']}")
+    if tuple(cai["shape"]) != (height, width):
+        raise ValueError(f"scene_depth must have shape ({height}, {width}), not {tuple(cai['shape'])}")
+    strides = cai.get("strides")
+    pitch = 4 * width
+    if strides is not None:
+        if strides[1] != 4 and width > 1:
+            raise ValueError("scene_depth rows must be contiguous")
+        pitch = int(strides[0])
+    return abi.bgs_scene_depth(depth=int(cai["data"][0]), pitch_bytes=pitch), cai.get("stream")
+
+
+_cuda_driver = None
+
+
+def _stream_wait(consumer: int, producer: int) -> None:
+    """Order `consumer` (a CUstream) after the work queued so far on `producer` (a CUstream, or the interface's 1 / 2 for
+    the legacy / per-thread default stream, which are also the driver's handles for them): one event, recorded on the
+    producer and waited for on the device, as __cuda_array_interface__ v3 asks of a consumer."""
+    global _cuda_driver
+    if _cuda_driver is None:
+        _cuda_driver = C.CDLL("libcuda.so.1")
+    cu, ev = _cuda_driver, C.c_void_p()
+    for call in (lambda: cu.cuEventCreate(C.byref(ev), C.c_uint(2)),        # CU_EVENT_DISABLE_TIMING
+                 lambda: cu.cuEventRecord(ev, C.c_void_p(producer)),
+                 lambda: cu.cuStreamWaitEvent(C.c_void_p(consumer), ev, C.c_uint(0))):
+        rc = call()
+        if rc != 0:
+            if ev.value:
+                cu.cuEventDestroy_v2(ev)
+            raise RuntimeError(f"scene_depth: ordering after the producer's stream failed (CUDA driver error {rc})")
+    cu.cuEventDestroy_v2(ev)   # (released once the wait has been satisfied)
+
+
 @dataclasses.dataclass
 class CloudTransform:
     """GlobalTransform of the cloud entity -> CloudUniform.transform (render/mod.rs:1056-1072)."""
@@ -163,8 +207,12 @@ class GaussianSplattingPlugin:
                     camera: GaussianCamera | None = None, transform: CloudTransform | None = None,
                     fmt: str = "rgba32f", out: np.ndarray | None = None, to_host: bool = True,
                     asynchronous: bool = False, premultiplied: bool = False, blend_over: bool = False,
-                    previous_view: View | None = None, delta_time: float | None = None):
+                    previous_view: View | None = None, delta_time: float | None = None, scene_depth=None):
         """Returns the (H, W, 4) frame (host) or None when `to_host` is False / the camera is warming up.
+        `scene_depth`: the view's Depth32Float depth buffer on this GPU (see `scene_depth_arg`); splats behind it are
+        hidden, as the reference's GreaterEqual depth test hides them (bgs_render_depth_test).  When its interface names
+        a stream (v3), the frame waits on the device for the work queued there; without one the buffer must be complete
+        when the call is made.  It must stay unchanged until an asynchronous frame completes.
         `asynchronous`: only enqueue the frame (BGS_FLAG_ASYNC); call `sync()` before reading anything.
         `premultiplied`: the splat layer alone, (C, 1 - T) (BGS_FLAG_PREMULTIPLIED_OUT).  `blend_over`: blend over what
         the context's frame already holds -- the previous call's result (BGS_FLAG_BLEND_OVER_TARGET): one call per
@@ -181,12 +229,24 @@ class GaussianSplattingPlugin:
                 out = np.empty((view.height, view.width, ch), dtype)
             assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
         target = _ptr(out) if to_host else None
-        if ex is None:
+        zd = self._scene_depth(scene_depth, view)
+        if zd is not None:
+            st = self._lib.bgs_render_depth_test(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s),
+                                                 None if ex is None else C.byref(ex), C.byref(zd), target, code, 0)
+        elif ex is None:
             st = self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), target, code, 0)
         else:
             st = self._lib.bgs_render_ex(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.byref(ex), target, code, 0)
         self._check(st)
         return out if to_host else None
+
+    def _scene_depth(self, scene_depth, view):
+        """The call's bgs_scene_depth; a buffer whose interface names its producer's stream is read only after the work
+        queued on that stream so far (every launch of a frame is ordered after the context's stream)."""
+        zd, producer = scene_depth_arg(scene_depth, view.width, view.height)
+        if producer is not None:
+            _stream_wait(self.stream_ptr, int(producer))
+        return zd
 
     def _uniform_and_settings(self, handle, settings, transform, asynchronous=False, premultiplied=False, blend_over=False):
         """The uniform and settings structs of a call (see `_call_args`)."""
@@ -233,15 +293,21 @@ class GaussianSplattingPlugin:
     def render_view_to_device(self, handle: PlanarGaussian3dHandle, settings: CloudSettings, view: View, device_ptr: int,
                               transform: CloudTransform | None = None, fmt: str = "rgba8_srgb", asynchronous: bool = False,
                               premultiplied: bool = False, blend_over: bool = False, previous_view: View | None = None,
-                              delta_time: float | None = None) -> None:
+                              delta_time: float | None = None, scene_depth=None) -> None:
         """Render straight into caller-owned device memory: an exported frame target (`bgs_frame_export_create`), or
         another GPU's memory mapped into this process (`bgs_peer_buffer_open`) -- the blend kernel's pixel stores then
         travel over NVLink themselves.  The target must be aligned to one pixel (4 / 8 / 16 bytes).  `premultiplied` /
-        `blend_over`, `previous_view` and `delta_time` as in `render_view`; blend-over reads what `device_ptr` holds."""
+        `blend_over`, `previous_view`, `delta_time` and `scene_depth` as in `render_view`; blend-over reads what
+        `device_ptr` holds."""
         code, _, _ = self.FORMATS[fmt]
         v = view.to_abi()
         u, s, ex = self._call_args(handle, settings, transform, asynchronous, premultiplied, blend_over, previous_view, delta_time)
-        if ex is None:
+        zd = self._scene_depth(scene_depth, view)
+        if zd is not None:
+            self._check(self._lib.bgs_render_depth_test(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s),
+                                                        None if ex is None else C.byref(ex), C.byref(zd),
+                                                        C.c_void_p(device_ptr), code, 1))
+        elif ex is None:
             self._check(self._lib.bgs_render(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.c_void_p(device_ptr), code, 1))
         else:
             self._check(self._lib.bgs_render_ex(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.byref(ex),
@@ -443,6 +509,14 @@ class GaussianSplattingPlugin:
         if fs.n_visible:
             self._check(self._lib.bgs_debug_projected(self._ctx, _ptr(rec), _ptr(ids)))
         return rec, ids
+
+    def splat_depths(self) -> np.ndarray:
+        """The last depth-tested frame's splat depths d, (n_visible,) float32 in front-to-back rank order."""
+        fs = self.frame_stats()
+        out = np.empty((fs.n_visible,), np.float32)
+        if fs.n_visible:
+            self._check(self._lib.bgs_debug_splat_depths(self._ctx, _ptr(out)))
+        return out
 
     @property
     def stream_ptr(self) -> int:

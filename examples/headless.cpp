@@ -26,6 +26,7 @@
 #include <iostream>
 #include <string>
 #include <sys/stat.h>
+#include <dlfcn.h>
 
 #include "../include/bgs.hpp"
 
@@ -37,6 +38,7 @@ int main(int argc, char** argv) {
     std::string dump_particles;
     long interp_seed = -1; float interp_time = 0.0f;
     std::string rasterize = "color"; uint32_t num_classes = 3; float prev_off[3] = {0.05f, 0.0f, 0.0f};
+    float depth_plane = -1.0f;   // --depth-plane Z: render depth-tested against a half-frame plane at reverse-Z depth Z
     int pos = 0;
     for (int i = 1; i < argc; ++i) {
         const std::string a = argv[i];
@@ -50,6 +52,7 @@ int main(int argc, char** argv) {
         if (a == "--interpolate" && i + 1 < argc) { interp_seed = std::atol(argv[++i]); continue; }
         if (a == "--time" && i + 1 < argc) { interp_time = (float)std::atof(argv[++i]); continue; }
         if (a == "--rasterize" && i + 1 < argc) { rasterize = argv[++i]; continue; }
+        if (a == "--depth-plane" && i + 1 < argc) { depth_plane = (float)std::atof(argv[++i]); continue; }
         if (a == "--num-classes" && i + 1 < argc) { num_classes = (uint32_t)std::strtoul(argv[++i], nullptr, 10); continue; }
         if (a == "--prev-view" && i + 1 < argc) {
             if (std::sscanf(argv[++i], "%f,%f,%f", &prev_off[0], &prev_off[1], &prev_off[2]) != 3) return 1;
@@ -134,7 +137,33 @@ int main(int argc, char** argv) {
         }
         std::vector<unsigned char> frame((size_t)W * H * 4);
         bool drawn = false;
-        for (int f = 0; f < 3; ++f)
+        if (depth_plane >= 0.0f) {
+            // the scene's depth buffer: the left half of the frame at depth_plane, the rest cleared (reverse-Z 0), rows
+            // padded to 256 bytes as wgpu's copy_texture_to_buffer pads them; device memory through the CUDA driver
+            // (libbgs's context is current on this thread)
+            using Alloc = int (*)(unsigned long long*, size_t);
+            using HtoD = int (*)(unsigned long long, const void*, size_t);
+            using Free = int (*)(unsigned long long);
+            void* cu = dlopen("libcuda.so.1", RTLD_NOW);
+            if (!cu) { std::fprintf(stderr, "headless: libcuda.so.1 not found\n"); return 1; }
+            const Alloc mem_alloc = (Alloc)dlsym(cu, "cuMemAlloc_v2");
+            const HtoD htod = (HtoD)dlsym(cu, "cuMemcpyHtoD_v2");
+            const Free mem_free = (Free)dlsym(cu, "cuMemFree_v2");
+            const size_t pitch = ((size_t)W * 4 + 255) / 256 * 256;
+            std::vector<float> z(pitch / 4 * H, 0.0f);
+            for (int y = 0; y < H; ++y)
+                for (int x = 0; x < W / 2; ++x) z[(size_t)y * (pitch / 4) + x] = depth_plane;
+            unsigned long long d = 0;
+            if (mem_alloc(&d, pitch * H) != 0 || htod(d, z.data(), pitch * H) != 0) {
+                std::fprintf(stderr, "headless: could not place the depth buffer\n");
+                return 1;
+            }
+            for (int f = 0; f < 3; ++f)
+                drawn = plugin.render_view_depth_test(drawn_cloud, settings, view, reinterpret_cast<const float*>(d), pitch,
+                                                      frame.data(), BGS_FORMAT_RGBA8_SRGB);
+            mem_free(d);
+        }
+        for (int f = 0; f < 3 && depth_plane < 0.0f; ++f)
             drawn = settings.rasterize_mode == bgs::RasterizeMode::OpticalFlow
                         ? plugin.render_view(drawn_cloud, settings, view, prev_view, 1.0f / 60.0f, frame.data(), BGS_FORMAT_RGBA8_SRGB)
                         : plugin.render_view(drawn_cloud, settings, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);

@@ -411,6 +411,46 @@ bgs_status bgs_render_ex(bgs_context* ctx, const bgs_cloud* cloud, const bgs_vie
                          const bgs_cloud_uniform* uniform, const bgs_settings* settings,
                          const bgs_render_extras* extras, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
 
+/* The scene's depth buffer a frame is depth-tested against (the view's Depth32Float depth texture, reverse-Z). */
+typedef struct {
+    const float* depth;    /* device memory on the context's GPU: the viewport's w x h Depth32Float values,
+                              row-major, pixel (0, 0) at the viewport's top-left */
+    uint64_t pitch_bytes;  /* bytes from one row to the next: a multiple of 4, >= 4 w (wgpu's copy_texture_to_buffer
+                              pads rows to 256 bytes) */
+} bgs_scene_depth;
+
+/* bgs_render_ex with the reference's depth test: splats are drawn in the transparent pass against the view's depth
+ * buffer with depth_compare GreaterEqual and depth writes off (render/mod.rs:959-974), so opaque geometry drawn earlier
+ * hides the splats behind it.  depth == NULL makes the call exactly bgs_render_ex.  Every geometry, layout, RasterizeMode,
+ * draw mode, format, output mode and flag bgs_render_ex accepts is accepted here.
+ *
+ * The rule, exactly (f32, round to nearest even, IEEE division, no contraction):
+ *   Splat depth.  Each splat has one depth d = pz / pw, where p = model * pos as the projection computes it,
+ *     h = clip_from_world * (p, 1), pz = h.z / (h.w + 1e-9) and pw = h.w / (h.w + 1e-9): the z and w lanes of
+ *     world_to_clip (transform.wgsl:5-8).  The reference emits (projected.xy + bb.xy, projected.zw) for all four quad
+ *     vertices (gaussian.wgsl:429-433), so its fragment depth is constant over the quad; 2DGS surfels use the same d.
+ *     Fixed-function depth interpolation may differ from this d in the last ulp: parity unpinned, as f16 rounding is.
+ *   The test.  A (pixel, splat) pair blends iff the coverage decision of bgs_render_ex holds and d >= scene[pixel].  The
+ *     compare is IEEE: a NaN scene depth or +inf hides every splat, and -0 == +0.  A hidden pair leaves T and the colour
+ *     unchanged, and later splats at that pixel continue.  A cleared reverse-Z buffer (0.0) hides nothing drawn with
+ *     h.w >= 0 (every drawn splat has pz > 0); a splat drawn with h.w in (-1e-9, 0) -- possible only when the frustum
+ *     test passes with |h.x|, |h.y|, h.z all below 1.1e-9, e.g. a clip matrix scaled to tiny values -- has pw < 0 and
+ *     d < 0, and a zero buffer hides it.
+ *   Unchanged stages.  Key-gen, the depth sort, the projection records, binning, the pair list, the tile ranges and
+ *     entries and bgs_frame_stats are those of the same frame without a depth buffer; only pixels change.
+ *   The buffer.  Only read, never written (the reference does not write depth either).  A queued frame
+ *     (BGS_FLAG_ASYNC) reads it in its blend kernel, so it must stay unchanged until that frame completes, the same
+ *     contract a device target has.
+ * Known difference, left as it is: a splat with h.w below about 0.03 can have pz / pw > 1.  The reference's clipper
+ *   (unclipped_depth: false) drops it; this port draws it, with or without a depth buffer.
+ * Refused with BGS_EINVAL, nothing enqueued or written: a NULL depth->depth; a pitch that is not a multiple of 4 or is
+ *   below 4 w; a pointer that is not 4-byte aligned; a pointer that is not device memory of the context's GPU.
+ * bgs_render_aux takes no depth buffer. */
+bgs_status bgs_render_depth_test(bgs_context* ctx, const bgs_cloud* cloud, const bgs_view* view,
+                                 const bgs_cloud_uniform* uniform, const bgs_settings* settings,
+                                 const bgs_render_extras* extras, const bgs_scene_depth* depth, void* out_rgba,
+                                 uint32_t out_format, int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target
@@ -428,6 +468,9 @@ bgs_status bgs_debug_tile_entries(bgs_context* ctx, uint32_t* ranks, uint64_t ca
 /* n_visible records of 12 floats: cx, cy, ux, uy, vx, vy, bbox(2 words), r, g, b, opacity;
  * and n_visible gaussian indices (front-to-back rank -> index). */
 bgs_status bgs_debug_projected(bgs_context* ctx, float* records, uint32_t* rank_to_index);
+/* n_visible floats: each splat's depth d (bgs_render_depth_test's rule) in front-to-back rank order, the order of
+ * bgs_debug_projected.  Valid after a completed depth-tested frame (else BGS_NOT_READY). */
+bgs_status bgs_debug_splat_depths(bgs_context* ctx, float* out);
 bgs_status bgs_frame_stats_get(bgs_context* ctx, bgs_frame_stats* out);
 
 /* Last frame's stage times (CUDA events on the context stream), microseconds:

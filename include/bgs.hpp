@@ -286,6 +286,27 @@ public:
         check(st);
         return true;
     }
+    // render_view depth-tested against the scene's depth buffer (bgs_render_depth_test: the reference's GreaterEqual test,
+    // no depth writes): `depth` is the view's w x h Depth32Float buffer in device memory of this context's GPU, rows
+    // `pitch_bytes` apart.  A queued frame reads it until it completes.
+    bool render_view_depth_test(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view,
+                                const float* depth, uint64_t pitch_bytes, void* out_rgba,
+                                uint32_t format = BGS_FORMAT_RGBA8_SRGB, const GaussianCamera& camera = {},
+                                bool out_is_device = false, uint32_t extra_flags = 0) {
+        if (camera.warmup) return false;
+        bgs_cloud_uniform u = cloud_uniform(settings);
+        std::memcpy(u.aabb_min, cloud.aabb_min(), 12); std::memcpy(u.aabb_max, cloud.aabb_max(), 12);
+        const bgs_settings s = settings.to_abi(extra_flags);
+        bgs_render_extras ex{};
+        ex.num_classes = settings.num_classes;
+        const bgs_scene_depth zd{depth, pitch_bytes};
+        const bgs_status st = bgs_render_depth_test(ctx_, cloud.get(), &view, &u, &s,
+                                                    settings.rasterize_mode == RasterizeMode::OpticalFlow ? nullptr : &ex,
+                                                    &zd, out_rgba, format, out_is_device ? 1 : 0);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
     // Colour + depth + normal frames of one view in one pass (BASELINE.json config 4; bgs_render_aux).
     bool render_view_aux(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view, void* out_rgba,
                          void* out_depth, void* out_normal, uint32_t format = BGS_FORMAT_RGBA8_SRGB, bool out_is_device = false) {
