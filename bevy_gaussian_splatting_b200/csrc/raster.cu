@@ -192,7 +192,6 @@ __device__ __forceinline__ float2 lds2(uint32_t a) {
     float2 r; asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(r.x), "=f"(r.y) : "r"(a)); return r;
 }
 __device__ __forceinline__ uint32_t lds_u16(uint32_t a) { uint32_t r; asm volatile("ld.shared.u16 %0, [%1];" : "=r"(r) : "r"(a)); return r; }
-__device__ __forceinline__ uint32_t lds_u32(uint32_t a) { uint32_t r; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(a)); return r; }
 
 // USE_OBB quad coordinates of the pixel centre (fx, fy) for q0 = (cx, cy, ux, uy), q1 = (vx, vy): u = ux dx + uy dy with
 // the fma on the dy term, v likewise.  The same rounding steps as decide() in oracle/bgs_oracle.cpp, so the coverage
@@ -356,35 +355,35 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
             return hit;
         });
         if (MODE == 0 && !AUX) {
-            // two candidates per iteration: one 32-bit load brings both list entries, the four record loads and both
-            // coverage tests are independent (ILP), loop control is paid once; blending stays strictly in list order
-            // The blend is PREDICATED, not branched: 14 predicated instructions per candidate instead of a divergent block
+            // four candidates per iteration, so loop control is paid once per four; each list entry is its own 16-bit
+            // load (cheaper than unpacking a 32-bit pair); blending stays strictly in list order.
+            // The blend is PREDICATED, not branched: 15 SASS instructions per candidate instead of a divergent block
             // with its BSSY / BRA / BREAK / BSYNC bookkeeping (~23 issue slots; 98 % of the candidates cover some pixel of
-            // the warp anyway).  `lim` = 1 while the pixel is alive, -1 once it has stopped (T < T_STOP) or lies outside the
-            // frame, so "covered" and "alive" are one comparison and a stopped pixel skips every later splat exactly as an
-            // early exit would.
-            const uint32_t a_end = a_list + nl * 2u;
+            // the warp anyway).  A candidate blends where it covers the pixel and T >= T_STOP: a stopped pixel (and one
+            // outside the frame, T = 0) skips every later splat exactly as an early exit would, and the stop costs one
+            // `setp ... .and` of the T the previous blend left, instead of a stop flag updated after every blend.
+            const uint32_t a_end = a_list + nl * 2u, a_end4 = a_end - 6u;   // (no wrap: a_list >= SM_LIST)
             uint32_t a_it = a_list;
-            float lim = (T < T_STOP) ? -1.0f : 1.0f;
-            // ZTEST: one more load and one more `setp ... .and`: the pair blends only where d >= the scene depth (%9)
+            // ZTEST: one more load and one more `setp ... .and`: the pair blends only where d >= the scene depth (%8)
 #define BLEND_COVER_                                                                                                    \
                     "{\n\t"                                                                                             \
-                    ".reg .pred p, q;\n\t"                                                                              \
+                    ".reg .pred p;\n\t"                                                                                 \
                     ".reg .f32 au, av, x, y, z, o, qd, e, a, w, na;\n\t"                                                \
-                    "abs.f32 au, %5;\n\t"                                                                               \
-                    "abs.f32 av, %6;\n\t"                                                                               \
-                    "setp.le.f32 p, au, %4;\n\t"                                                                        \
-                    "setp.le.and.f32 p, av, %4, p;\n\t"
+                    "abs.f32 au, %4;\n\t"                                                                               \
+                    "abs.f32 av, %5;\n\t"                                                                               \
+                    "setp.le.f32 p, au, 0f3F800000;\n\t"                                                                \
+                    "setp.le.and.f32 p, av, 0f3F800000, p;\n\t"                                                         \
+                    "setp.ge.and.f32 p, %0, 0f38D1B717, p;\n\t"   /* alive: T >= T_STOP (1e-4f) */
 #define BLEND_ZTEST_                                                                                                    \
                     ".reg .f32 dz;\n\t"                                                                                \
-                    "ld.shared.f32 dz, [%7+%10];\n\t"                                                                   \
-                    "setp.ge.and.f32 p, dz, %9, p;\n\t"
+                    "ld.shared.f32 dz, [%6+%9];\n\t"                                                                    \
+                    "setp.ge.and.f32 p, dz, %8, p;\n\t"
                     // (the temporaries are computed unconditionally -- a predicated definition would keep their old values
                     // alive across iterations -- only the four accumulations are predicated)
 #define BLEND_ACCUMULATE_                                                                                               \
-                    "ld.shared.v4.f32 {x, y, z, o}, [%7+%8];\n\t"                                                       \
-                    "mul.rn.f32 qd, %5, %5;\n\t"                                                                        \
-                    "fma.rn.f32 qd, %6, %6, qd;\n\t"                                                                    \
+                    "ld.shared.v4.f32 {x, y, z, o}, [%6+%7];\n\t"                                                       \
+                    "mul.rn.f32 qd, %4, %4;\n\t"                                                                        \
+                    "fma.rn.f32 qd, %5, %5, qd;\n\t"                                                                    \
                     "mul.rn.f32 qd, qd, 0fC0CFBF83;\n\t"     /* -6.492127684f: exp(-4.5 qd) = 2^(qd * -4.5 log2 e) */  \
                     "ex2.approx.ftz.f32 e, qd;\n\t"                                                                     \
                     "mul.rn.f32 a, e, o;\n\t"                                                                           \
@@ -395,36 +394,31 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                     "@p fma.rn.f32 %2, w, y, %2;\n\t"                                                                   \
                     "@p fma.rn.f32 %3, w, z, %3;\n\t"                                                                   \
                     "@p fma.rn.f32 %0, na, %0, %0;\n\t"                                                                 \
-                    "setp.lt.and.f32 q, %0, 0f38D1B717, p;\n\t"   /* T < T_STOP (1e-4f) after a blend: the pixel stops */ \
-                    "@q mov.f32 %4, 0fBF800000;\n\t"                                                                    \
                     "}"
             auto blend_if_covered = [&](uint32_t a_rec, float2 uv) {
                 if constexpr (ZTEST)
                     asm volatile(BLEND_COVER_ BLEND_ZTEST_ BLEND_ACCUMULATE_
-                                 : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb), "+f"(lim)
+                                 : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb)
                                  : "f"(uv.x), "f"(uv.y), "r"(a_rec), "n"(REC_Q2), "f"(zs), "n"(REC_D));
                 else
                     asm volatile(BLEND_COVER_ BLEND_ACCUMULATE_
-                                 : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb), "+f"(lim)
+                                 : "+f"(T), "+f"(cr), "+f"(cg), "+f"(cb)
                                  : "f"(uv.x), "f"(uv.y), "r"(a_rec), "n"(REC_Q2));
             };
 #undef BLEND_COVER_
 #undef BLEND_ZTEST_
 #undef BLEND_ACCUMULATE_
-            for (; a_it + 2u < a_end; a_it += 4u) {
-                const uint32_t two = lds_u32(a_it);
-                const uint32_t ra = two & 0xFFFFu, rb = two >> 16;
-                const float4 pa = lds4(ra), pb = lds4(rb);
-                const float2 sa = lds2(ra + REC_UV), sb = lds2(rb + REC_UV);
-                const float2 uva = quad_uv(fx, fy, pa, sa), uvb = quad_uv(fx, fy, pb, sb);
-                blend_if_covered(ra, uva);
-                blend_if_covered(rb, uvb);
+            for (; a_it < a_end4; a_it += 8u) {
+                const uint32_t ra = lds_u16(a_it), rb = lds_u16(a_it + 2u), rc = lds_u16(a_it + 4u), rd = lds_u16(a_it + 6u);
+                blend_if_covered(ra, quad_uv(fx, fy, lds4(ra), lds2(ra + REC_UV)));
+                blend_if_covered(rb, quad_uv(fx, fy, lds4(rb), lds2(rb + REC_UV)));
+                blend_if_covered(rc, quad_uv(fx, fy, lds4(rc), lds2(rc + REC_UV)));
+                blend_if_covered(rd, quad_uv(fx, fy, lds4(rd), lds2(rd + REC_UV)));
             }
-            if (a_it != a_end) {   // odd tail
+#pragma unroll 1
+            for (; a_it != a_end; a_it += 2u) {   // the last nl % 4
                 const uint32_t ra = lds_u16(a_it);
-                const float4 pa = lds4(ra);
-                const float2 sa = lds2(ra + REC_UV);
-                blend_if_covered(ra, quad_uv(fx, fy, pa, sa));
+                blend_if_covered(ra, quad_uv(fx, fy, lds4(ra), lds2(ra + REC_UV)));
             }
         } else if (!(T < T_STOP)) {
             const uint32_t a_end = a_list + nl * 2u;
