@@ -6,12 +6,13 @@ The Python modules here are the host-side mirror of the reference interface for 
 """
 from .abi import BgsError  # noqa: F401
 from .camera import GaussianCamera, View, headless_view, orbit_view, perspective_view  # noqa: F401
-from .gaussian import (PlanarGaussian3d, random_gaussians_3d, random_gaussians_3d_seeded,  # noqa: F401
-                       SH_COEFF_COUNT)
-from .io import load_cloud, parse_ply_3d  # noqa: F401
+from .gaussian import (PlanarGaussian3d, PlanarGaussian4d, random_gaussians_3d, random_gaussians_3d_seeded,  # noqa: F401
+                       random_gaussians_4d_seeded, SH_COEFF_COUNT, SH_4D_COEFF_COUNT)
+from .io import load_cloud, parse_ply_3d, parse_ply_4d, write_ply_4d  # noqa: F401
 from .gcloud import decode_gcloud, encode_gcloud, read_gcloud, write_gcloud  # noqa: F401
 from .particles import (PARTICLE_BEHAVIOR_DTYPE, PARTICLE_INACTIVE, ParticleBehaviors,  # noqa: F401
                         random_particle_behaviors)
-from .plugin import CloudTransform, GaussianSplattingPlugin, ParticleBehaviorsHandle, PlanarGaussian3dHandle  # noqa: F401
-from .settings import (CloudSettings, DrawMode, GaussianColorSpace, GaussianMode, RadixSortDepthBits,  # noqa: F401
-                       RasterizeMode, ShaderDefines, SortMode, SparseSelect)
+from .plugin import (CloudTransform, GaussianSplattingPlugin, ParticleBehaviorsHandle, PlanarGaussian3dHandle,  # noqa: F401
+                     PlanarGaussian4dHandle)
+from .settings import (CloudSettings, DrawMode, GaussianColorSpace, GaussianMode, PlaybackMode,  # noqa: F401
+                       RadixSortDepthBits, RasterizeMode, ShaderDefines, SortMode, SparseSelect, playback_update)

@@ -116,6 +116,8 @@ SYMBOLS = [
     ("bgs_cloud_subset", C.c_int, [_P, _P, _P, C.c_uint32, C.POINTER(_P), C.POINTER(C.c_uint32)]),
     ("bgs_cloud_download_f32", C.c_int, [_P, _P, _P, _P, _P, _P]),
     ("bgs_cloud_download_f16", C.c_int, [_P, _P, _P, _P, _P]),
+    ("bgs_cloud_upload_4d", C.c_int, [_P, C.c_uint32, _P, _P, _P, _P, _P, C.POINTER(_P)]),
+    ("bgs_cloud_download_4d", C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
     ("bgs_particles_create", C.c_int, [_P, _P, C.c_uint32, C.POINTER(_P)]),
     ("bgs_particles_get", C.c_int, [_P, _P, _P]),
     ("bgs_particles_destroy", None, [_P]),
@@ -128,6 +130,9 @@ SYMBOLS = [
                                 C.POINTER(bgs_render_extras), _P, C.c_uint32, C.c_int]),
     ("bgs_render_depth_test", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings),
                                         C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
+    ("bgs_render_4d", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings),
+                                C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int, C.c_float,
+                                C.c_float]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,
                                  C.c_uint32, C.c_int]),
     ("bgs_sync", C.c_int, [_P]),

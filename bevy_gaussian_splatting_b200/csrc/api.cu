@@ -151,7 +151,7 @@ struct FramePlan {
 FramePlan plan_frame(const bgs_context* c, const bgs_settings* st, bool want_aux, uint32_t num_tiles, uint32_t n) {
     FramePlan p;
     const bool queued = (st->flags & BGS_FLAG_ASYNC) != 0;
-    p.raster_mode = !st->aabb ? 0 : (st->gaussian_mode == BGS_GAUSSIAN_3D ? 1 : 2);
+    p.raster_mode = !st->aabb ? 0 : (st->gaussian_mode == BGS_GAUSSIAN_2D ? 2 : 1);   // (4D records are 3DGS conics)
     // saturation-aware chunking: frames whose splats cover many tiles each (last frame: >= 32 pairs per visible splat
     // and >= 2^24 pairs: below that, one round is cheaper than the extra launches) run binning / tile sort /
     // blend in front-to-back rank rounds; the rounds after every tile has saturated emit nothing.
@@ -384,17 +384,27 @@ bgs_status bgs_sync(bgs_context* c) {
 }
 
 static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                               const bgs_settings* st, const bgs_render_extras* ex, uint32_t out_format, bool want_aux) {
+                               const bgs_settings* st, const bgs_render_extras* ex, uint32_t out_format, bool want_aux,
+                               bool temporal) {
     // not-ready inputs map to the reference's silent skip-frame (radix.rs:645-658, mod.rs:1533-1539)
     if (!cloud || !view || !uni || !st) return fail(c, BGS_NOT_READY, "render: cloud/view/uniform/settings not ready");
     TRY(enter_call(c, "render", cloud->device));   // (contexts of one GPU may share clouds)
     if (out_format > BGS_FORMAT_RGBA32F) return fail(c, BGS_EINVAL, "render: unknown out_format %u", out_format);
     if (st->radix_sort_depth_bits != 16 && st->radix_sort_depth_bits != 24 && st->radix_sort_depth_bits != 32)
         return fail(c, BGS_EINVAL, "render: radix_sort_depth_bits must be 16, 24 or 32");
-    if (st->gaussian_mode != BGS_GAUSSIAN_3D && st->gaussian_mode != BGS_GAUSSIAN_2D)
-        return fail(c, BGS_EINVAL, "render: gaussian_mode %u not supported (Gaussian4d is out of scope)", st->gaussian_mode);
-    if (st->rasterize_mode > BGS_RASTERIZE_OPTICAL_FLOW)
-        return fail(c, BGS_EINVAL, "render: rasterize_mode %u not supported (Velocity needs Gaussian4d, out of scope)", st->rasterize_mode);
+    if (temporal) {
+        if (!is_4d(cloud->layout)) return fail(c, BGS_EINVAL, "render_4d: the cloud is not a Gaussian4d cloud (bgs_cloud_upload_4d)");
+        if (st->gaussian_mode != BGS_GAUSSIAN_4D)
+            return fail(c, BGS_EINVAL, "render_4d: gaussian_mode %u is not BGS_GAUSSIAN_4D", st->gaussian_mode);
+        if (st->rasterize_mode > BGS_RASTERIZE_VELOCITY || st->rasterize_mode == BGS_RASTERIZE_NORMAL)
+            return fail(c, BGS_EINVAL, "render_4d: rasterize_mode %u not supported (Normal has no 4D rotation)", st->rasterize_mode);
+    } else {
+        if (is_4d(cloud->layout)) return fail(c, BGS_EINVAL, "render: a Gaussian4d cloud renders through bgs_render_4d");
+        if (st->gaussian_mode != BGS_GAUSSIAN_3D && st->gaussian_mode != BGS_GAUSSIAN_2D)
+            return fail(c, BGS_EINVAL, "render: gaussian_mode %u not supported here (Gaussian4d: bgs_render_4d)", st->gaussian_mode);
+        if (st->rasterize_mode > BGS_RASTERIZE_OPTICAL_FLOW)
+            return fail(c, BGS_EINVAL, "render: rasterize_mode %u not supported here (Velocity: bgs_render_4d)", st->rasterize_mode);
+    }
     if (st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION && want_aux)
         return fail(c, BGS_EINVAL, "render_aux: Classification and OpticalFlow frames take extras: use bgs_render_ex");
     if (st->rasterize_mode == BGS_RASTERIZE_CLASSIFICATION && ex && ex->num_classes == 0)
@@ -442,7 +452,7 @@ static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, co
 
 // Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.
 static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const ModeConsts* modes,
-                                const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd) {
+                                const TemporalConsts* tc, const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd) {
     const uint32_t n = cloud->n;
     const uint32_t num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     cudaStream_t q = c->stream;
@@ -483,19 +493,24 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
         ++launches;
     }
     CU(c, cudaEventRecord(c->ev_p0, ps));
-    launch_project(cloud->layout, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
-                   c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
-                   fc.aux ? c->aux.p : nullptr, modes, ps);
+    if (tc) {   // Gaussian4d: the projection also writes the depth-tested frame's splat depths, from the moved positions
+        launch_project_4d(cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
+                          modes ? *modes : ModeConsts{}, *tc, c->recs.p, zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
+    } else {
+        launch_project(cloud->layout, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
+                       c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
+                       fc.aux ? c->aux.p : nullptr, modes, ps);
+    }
     ++launches;
     CU(c, cudaEventRecord(c->ev_p1, ps));
     // depth-tested frames: the splat depths, indexed like the records (the projection's index list)
     ZTestArgs zt;
-    if (zd) {
+    if (zd && !tc) {
         launch_splat_depth(cloud->pos, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
                            c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
-        zt.splat_d = c->splat_depth.p; zt.scene = zd->depth; zt.pitch = (size_t)zd->pitch_bytes;
     }
+    if (zd) { zt.splat_d = c->splat_depth.p; zt.scene = zd->depth; zt.pitch = (size_t)zd->pitch_bytes; }
     if (p.overlap) {
         CU(c, cudaEventRecord(c->ev_join, c->stream2));
         CU(c, cudaStreamWaitEvent(q, c->ev_join, 0));
@@ -587,9 +602,9 @@ static bgs_status check_scene_depth(bgs_context* c, const bgs_scene_depth* zd, c
 static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                               const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
                               int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal,
-                              const bgs_scene_depth* zd = nullptr) {
+                              const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr) {
     if (!c) return BGS_EINVAL;
-    TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux));
+    TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));
     if (zd) TRY(check_scene_depth(c, zd, view));
     if (c->async_pending && !(st->flags & BGS_FLAG_ASYNC)) {
         // a synchronous render after queued frames completes them first; their failure (including an overflowed
@@ -617,7 +632,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         TRY(ensure_arena(c, num_tiles));
         TRY(ensure_status(c, c->status_depth, c->status_n, n));
         TRY(ensure_status(c, c->status_pairs, c->status_np, c->cap_pairs));
-        TRY(enqueue_frame(c, cloud, fc, modes, p, o, zd));
+        TRY(enqueue_frame(c, cloud, fc, modes, tc, p, o, zd));
         if (st->flags & BGS_FLAG_ASYNC) {
             c->async_pending = true;
             c->have_frame = false;     // hooks need bgs_sync() first
@@ -643,6 +658,23 @@ bgs_status bgs_render_depth_test(bgs_context* c, const bgs_cloud* cloud, const b
                                  const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
     return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth);
+}
+
+bgs_status bgs_render_4d(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                         const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba,
+                         uint32_t out_format, int out_is_device_ptr, float time_start, float time_stop) {
+    if (!c) return BGS_EINVAL;
+    TemporalConsts tc = {};
+    if (uni) {
+        if (!std::isfinite(uni->time) || !std::isfinite(time_start) || !std::isfinite(time_stop) || time_stop == time_start)
+            return fail(c, BGS_EINVAL, "render_4d: time %g, time_start %g, time_stop %g: all finite and time_stop != time_start",
+                        (double)uni->time, (double)time_start, (double)time_stop);
+        tc.duration = time_stop - time_start;
+        if (!std::isfinite(tc.duration)) return fail(c, BGS_EINVAL, "render_4d: time_stop - time_start overflows");
+        tc.time = uni->time;
+        tc.time_future = uni->time + 1.0e-3f;
+    }
+    return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth, &tc);
 }
 
 bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,

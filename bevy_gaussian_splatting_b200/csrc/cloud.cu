@@ -49,19 +49,24 @@ struct StreamScratch {
 };
 
 // gaussians per chunk of a download: the device staging arrays hold one chunk (f32: 28 MB), each of the context's two
-// pinned bounce buffers one chunk's four planes (f32: 30 MB)
+// pinned bounce buffers one chunk's planes (f32: 30 MB).  4D gaussians are wider: their chunks hold as many gaussians
+// as fit the same bounce buffers
 constexpr uint32_t DOWNLOAD_CHUNK = 1u << 17;
 constexpr size_t DOWNLOAD_BOUNCE_BYTES = (size_t)DOWNLOAD_CHUNK * planar_bytes(CloudLayout::F32);
+static_assert(planar_bytes(CloudLayout::F32) >= planar_bytes(CloudLayout::F16), "the f32 chunk is the largest 3D one");
+
+// the family of download call a layout answers to (0: _f32, 1: _f16, both f16 layouts; 2: _4d)
+int download_family(CloudLayout l) { return is_4d(l) ? 2 : is_f16(l) ? 1 : 0; }
 
 }  // namespace
 
 extern "C" {
 
 static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout, const float* pos_vis, const void* sh,
-                                const void* rot, const void* so, bgs_cloud** out) {
+                                const void* rot, const void* so, const void* tt, bgs_cloud** out) {
     if (!ctx || !out) return BGS_EINVAL;
     *out = nullptr;
-    const void* src[PLANES] = {pos_vis, sh, rot, so};
+    const void* src[PLANES] = {pos_vis, sh, rot, so, tt};
     for (int p = 0; p < PLANES; ++p)
         if (plane_bytes(layout, p) && !src[p]) return fail(ctx, BGS_EINVAL, "cloud upload: null plane pointer");
     if (n == 0 || n >= (1u << 30)) return fail(ctx, BGS_EINVAL, "cloud upload: n must be in [1, 2^30)");
@@ -70,7 +75,7 @@ static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout
     TRY(new_cloud(ctx, "cloud upload", n, layout, &cl));
     // the position plane is the cloud's own; the other planes go to device scratch, are repacked into the
     // gaussian-major blocks the projection gathers, and are freed again
-    void* d[PLANES] = {cl->pos, nullptr, nullptr, nullptr};
+    void* d[PLANES] = {cl->pos, nullptr, nullptr, nullptr, nullptr};
     cudaError_t e = cudaSuccess;
     for (int p = 0; p < PLANES && e == cudaSuccess; ++p) {
         const size_t bytes = (size_t)n * plane_bytes(layout, p);
@@ -79,7 +84,7 @@ static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout
         if (e == cudaSuccess) e = cudaMemcpyAsync(d[p], src[p], bytes, cudaMemcpyHostToDevice, ctx->stream);
     }
     if (e == cudaSuccess) {
-        launch_repack(layout, d[PLANE_SH], d[PLANE_ROT], d[PLANE_SO], n, cl->view(), ctx->stream);
+        launch_repack(layout, d[PLANE_SH], d[PLANE_ROT], d[PLANE_SO], d[PLANE_TT], n, cl->view(), ctx->stream);
         e = cudaStreamSynchronize(ctx->stream);
     }
     for (int p = PLANE_SH; p < PLANES; ++p) cudaFree(d[p]);
@@ -90,17 +95,22 @@ static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout
 
 bgs_status bgs_cloud_upload_f32(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh,
                                 const float* rot_wxyz, const float* scale_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, CloudLayout::F32, pos_vis, sh, rot_wxyz, scale_opacity, out);
+    return upload_common(ctx, n, CloudLayout::F32, pos_vis, sh, rot_wxyz, scale_opacity, nullptr, out);
 }
 
 bgs_status bgs_cloud_upload_f16(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
                                 const uint32_t* rot_scale_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, CloudLayout::F16, pos_vis, sh_packed, rot_scale_opacity, nullptr, out);
+    return upload_common(ctx, n, CloudLayout::F16, pos_vis, sh_packed, rot_scale_opacity, nullptr, nullptr, out);
 }
 
 bgs_status bgs_cloud_upload_f16_cov(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
                                     const uint32_t* cov3d_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, CloudLayout::F16Cov, pos_vis, sh_packed, cov3d_opacity, nullptr, out);
+    return upload_common(ctx, n, CloudLayout::F16Cov, pos_vis, sh_packed, cov3d_opacity, nullptr, nullptr, out);
+}
+
+bgs_status bgs_cloud_upload_4d(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh, const float* rotations,
+                               const float* scale_opacity, const float* timestamp_timescale, bgs_cloud** out) {
+    return upload_common(ctx, n, CloudLayout::F32x4D, pos_vis, sh, rotations, scale_opacity, timestamp_timescale, out);
 }
 
 void bgs_cloud_destroy(bgs_cloud* cl) {
@@ -385,6 +395,7 @@ bgs_status bgs_cloud_interpolate(bgs_context* c, bgs_cloud* out, const bgs_cloud
         return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out hold %u, %u and %u gaussians", lhs->n, rhs->n, out->n);
     if (lhs->layout != out->layout || rhs->layout != out->layout)
         return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out are not in one layout");
+    if (is_4d(out->layout)) return fail(c, BGS_EINVAL, "interpolate: Gaussian4d clouds are not interpolated");
     if (out == lhs || out == rhs) return fail(c, BGS_EINVAL, "interpolate: out is lhs or rhs");
     float t = 0.0f;
     if (!interpolation_factor(time, time_start, time_stop, &t))
@@ -452,33 +463,38 @@ bgs_status bgs_cloud_subset(bgs_context* c, const bgs_cloud* cl, const uint32_t*
 
 // Per chunk: unpack into device staging, copy the chunk's position plane and the staged planes to a pinned bounce
 // buffer, and -- while the next chunk goes the same way into the other bounce buffer -- copy it into the caller's arrays.
-static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, bool f16, float* pos_vis, void* sh, void* rot, void* so) {
-    if (!cl || !pos_vis || !sh || !rot || (!f16 && !so)) return fail(c, BGS_EINVAL, "download: null cloud or plane pointer");
+static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, int family, float* pos_vis, void* sh, void* rot, void* so,
+                                  void* tt) {
+    if (!cl || !pos_vis || !sh || !rot || (family != 1 && !so) || (family == 2 && !tt))
+        return fail(c, BGS_EINVAL, "download: null cloud or plane pointer");
     TRY(enter_call(c, "download", cl->device));
     const CloudLayout l = cl->layout;
-    if (is_f16(l) != f16) return fail(c, BGS_EINVAL, "download: the cloud is in the %s layout", is_f16(l) ? "f16" : "f32");
+    static const char* const kFamily[3] = {"f32", "f16", "4D"};
+    if (download_family(l) != family) return fail(c, BGS_EINVAL, "download: the cloud is in the %s layout", kFamily[download_family(l)]);
     TRY(before_cloud_read(c, cl));
     cudaStream_t q = c->stream;
-    const uint32_t n = cl->n, m_max = std::min(n, DOWNLOAD_CHUNK);
+    const uint32_t n = cl->n, m_max = std::min<uint32_t>(n, (uint32_t)(DOWNLOAD_BOUNCE_BYTES / planar_bytes(l)));
     // (sized once for the largest chunk of either layout: it never grows)
     if (!c->h_bounce) CU(c, cudaMallocHost(&c->h_bounce, 2 * DOWNLOAD_BOUNCE_BYTES));
     const size_t chunk_b = DOWNLOAD_BOUNCE_BYTES;
-    StreamScratch staging(q);   // sh | rot | so of one chunk
+    StreamScratch staging(q);   // sh | rot | so | tt of one chunk
     CU(c, staging.alloc((size_t)m_max * (planar_bytes(l) - plane_bytes(l, PLANE_POS))));
     uint8_t* st[PLANES] = {nullptr, static_cast<uint8_t*>(staging.p)};
     for (int p = PLANE_SH + 1; p < PLANES; ++p) st[p] = st[p - 1] + (size_t)m_max * plane_bytes(l, p - 1);
     cudaEvent_t ev[2] = {nullptr, nullptr};
     struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 2; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
     for (cudaEvent_t& e : ev) CU(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    uint8_t* dst[PLANES] = {reinterpret_cast<uint8_t*>(pos_vis), static_cast<uint8_t*>(sh), static_cast<uint8_t*>(rot), static_cast<uint8_t*>(so)};
+    uint8_t* dst[PLANES] = {reinterpret_cast<uint8_t*>(pos_vis), static_cast<uint8_t*>(sh), static_cast<uint8_t*>(rot),
+                            static_cast<uint8_t*>(so), static_cast<uint8_t*>(tt)};
     const uint32_t chunks = (n + m_max - 1) / m_max;
     // enqueue chunk i into bounce buffer i & 1
     auto enqueue = [&](uint32_t i) -> bgs_status {
         const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
         uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
-        launch_unpack(l, cl->view(), lo, m, st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO], q);
+        launch_unpack(l, cl->view(), lo, m, st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO], st[PLANE_TT], q);
         CU(c, cudaGetLastError());
-        const uint8_t* src[PLANES] = {reinterpret_cast<const uint8_t*>(cl->pos + lo), st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO]};
+        const uint8_t* src[PLANES] = {reinterpret_cast<const uint8_t*>(cl->pos + lo), st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO],
+                                      st[PLANE_TT]};
         for (int p = 0; p < PLANES; ++p) {
             const size_t bytes = (size_t)m * plane_bytes(l, p);
             if (bytes) CU(c, cudaMemcpyAsync(hb, src[p], bytes, cudaMemcpyDeviceToHost, q));
@@ -503,11 +519,16 @@ static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, bool f16,
 }
 
 bgs_status bgs_cloud_download_f32(bgs_context* c, const bgs_cloud* cl, float* pos_vis, float* sh, float* rot_wxyz, float* scale_opacity) {
-    return download_common(c, cl, false, pos_vis, sh, rot_wxyz, scale_opacity);
+    return download_common(c, cl, 0, pos_vis, sh, rot_wxyz, scale_opacity, nullptr);
 }
 
 bgs_status bgs_cloud_download_f16(bgs_context* c, const bgs_cloud* cl, float* pos_vis, uint32_t* sh_packed, uint32_t* second_plane) {
-    return download_common(c, cl, true, pos_vis, sh_packed, second_plane, nullptr);
+    return download_common(c, cl, 1, pos_vis, sh_packed, second_plane, nullptr, nullptr);
+}
+
+bgs_status bgs_cloud_download_4d(bgs_context* c, const bgs_cloud* cl, float* pos_vis, float* sh, float* rotations,
+                                 float* scale_opacity, float* timestamp_timescale) {
+    return download_common(c, cl, 2, pos_vis, sh, rotations, scale_opacity, timestamp_timescale);
 }
 
 }  // extern "C"

@@ -41,6 +41,13 @@ struct ModeConsts {
     uint32_t num_classes;             // > 0
 };
 
+// bgs_render_4d's time, as the Gaussian4d projection (project_4d_kernel, an argument of its own) reads it
+struct TemporalConsts {
+    float time;          // bgs_cloud_uniform.time
+    float time_future;   // time + 1e-3f: RasterizeMode::Velocity's second conditioning
+    float duration;      // time_stop - time_start (finite, non-zero): the time terms' theta = dt / duration
+};
+
 // Projected splat record, 48 B, stored by front-to-back rank.
 struct __align__(16) SplatRec {
     float cx, cy, ux, uy;       // centre (px), first row of the pixel-offset -> uv map

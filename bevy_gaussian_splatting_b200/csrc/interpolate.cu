@@ -89,8 +89,9 @@ __global__ void __launch_bounds__(INTERP_THREADS) interpolate_kernel(const uint4
 void launch_interpolate(CloudLayout layout, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream) {
     const size_t n_chunks = (size_t)n * out.chunks;
     const uint32_t grid = (uint32_t)((n_chunks + INTERP_THREADS - 1) / INTERP_THREADS);
-    with_layout(layout, [&](auto L) {
-        interpolate_kernel<decltype(L)::value><<<grid, INTERP_THREADS, 0, stream>>>(lhs.blocks, rhs.blocks, n_chunks, t, out);
+    with_layout(layout, [&](auto L) {   // (bgs_cloud_interpolate refuses 4D clouds)
+        if constexpr (!is_4d(decltype(L)::value))
+            interpolate_kernel<decltype(L)::value><<<grid, INTERP_THREADS, 0, stream>>>(lhs.blocks, rhs.blocks, n_chunks, t, out);
     });
 }
 

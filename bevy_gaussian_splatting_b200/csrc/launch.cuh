@@ -22,13 +22,18 @@ cudaError_t launch_radix_sort(uint32_t* keys0, uint32_t* vals0, uint32_t* keys1,
 // project.cu
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
                         FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream);
-void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, uint32_t n, CloudView cloud,
-                   cudaStream_t stream);
+void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, const void* tt /* 4D only */,
+                   uint32_t n, CloudView cloud, cudaStream_t stream);
 void launch_project(CloudLayout layout, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes /* null: project_kernel */,
                     cudaStream_t stream);
 void launch_cutoff_table(float* tab, cudaStream_t stream);
+// Gaussian4d clouds (bgs_render_4d): records as launch_project's, and the splat depths of depth-tested frames (depths
+// non-null) from the moved positions
+void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+                       const FrameConsts& fc, const ModeConsts& mc, const TemporalConsts& tc, SplatRec* recs, float* depths,
+                       uint32_t n_hint, int sm_count, cudaStream_t stream);
 // bin.cu
 int bin_coop_blocks_per_sm();
 cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
@@ -86,7 +91,8 @@ void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t
 void launch_subset_scatter(CloudLayout layout, CloudView src, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
                            CloudView dst, cudaStream_t stream);
 void launch_subset_gather(CloudLayout layout, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst, cudaStream_t stream);
-void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream);
+void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so,
+                   void* tt /* 4D only */, cudaStream_t stream);
 // interpolate.cu
 void launch_interpolate(CloudLayout layout, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream);
 }  // namespace bgs

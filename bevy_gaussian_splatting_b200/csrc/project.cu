@@ -141,18 +141,33 @@ struct Attr<true> {
 
 // upload-time repack of the planes into gaussian-major blocks (one thread per 16 B chunk; coalesced both ways)
 template <CloudLayout L>
-__global__ void repack_kernel(CloudPlanes<const uint4> planes, uint32_t n, uint4* __restrict__ blocks) {
+__device__ __forceinline__ void repack_chunk(const CloudPlanes<const uint4>& planes, uint32_t n, uint4* __restrict__ blocks,
+                                             const uint4* __restrict__ tt) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)n * chunks(L)) return;
-    const uint4* src = planes.unit<L>((uint32_t)(i % chunks(L)), i / chunks(L));
+    const uint4* src = planes.unit<L>((uint32_t)(i % chunks(L)), i / chunks(L), tt);
     blocks[i] = src ? __ldg(src) : make_uint4(0u, 0u, 0u, 0u);
 }
-void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, uint32_t n, CloudView cloud,
-                   cudaStream_t stream) {
+template <CloudLayout L>
+__global__ void repack_kernel(CloudPlanes<const uint4> planes, uint32_t n, uint4* __restrict__ blocks) {
+    repack_chunk<L>(planes, n, blocks, nullptr);
+}
+// the 4D layout's, which also reads the timestamp-timescale plane
+__global__ void repack_4d_kernel(CloudPlanes<const uint4> planes, uint32_t n, uint4* __restrict__ blocks,
+                                 const uint4* __restrict__ tt) {
+    repack_chunk<CloudLayout::F32x4D>(planes, n, blocks, tt);
+}
+void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, const void* tt, uint32_t n,
+                   CloudView cloud, cudaStream_t stream) {
     const CloudPlanes<const uint4> planes{reinterpret_cast<const uint4*>(cloud.pos), static_cast<const uint4*>(sh),
                                           static_cast<const uint4*>(rot), static_cast<const uint4*>(so)};
     const uint32_t grid = (uint32_t)(((size_t)n * cloud.chunks + 255) / 256);
-    with_layout(layout, [&](auto L) { repack_kernel<decltype(L)::value><<<grid, 256, 0, stream>>>(planes, n, cloud.blocks); });
+    with_layout(layout, [&](auto L) {
+        if constexpr (is_4d(decltype(L)::value))
+            repack_4d_kernel<<<grid, 256, 0, stream>>>(planes, n, cloud.blocks, static_cast<const uint4*>(tt));
+        else
+            repack_kernel<decltype(L)::value><<<grid, 256, 0, stream>>>(planes, n, cloud.blocks);
+    });
 }
 
 // RasterizeMode::Depth (gaussian.wgsl:329-349): min distance from sorted[N-1], max from sorted[1] of the
@@ -388,10 +403,9 @@ __device__ __forceinline__ void surfel_record(const FrameConsts& fc, const float
     }
 }
 
-// RasterizeMode::Color: gaussian.wgsl:166-183,406-416 + spherical_harmonics.wgsl:34-68, the SH-3 colour seen along
-// the camera ray in the splat's model frame
-__device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3][3], const float pw[3], const float sh[48],
-                                          float rgb[3]) {
+// The SH-3 basis of the camera ray in the splat's model frame (gaussian.wgsl:166-183,406-416, spherical_harmonics.wgsl:
+// 34-68), the SH constants folded in (16 multiplies instead of 48)
+__device__ __forceinline__ void sh_basis(const FrameConsts& fc, const float A[3][3], const float pw[3], float basis[16]) {
     const float dlt[3] = {pw[0] - fc.cam[0], pw[1] - fc.cam[1], pw[2] - fc.cam[2]};
     float dw[3], loc[3], dl[3];
     normalize3(dlt, dw);
@@ -409,7 +423,6 @@ __device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3
     normalize3(loc, dl);
     const float x = dl[0], y = dl[1], z = dl[2];
     const float xx = x * x, yy = y * y, zz = z * z;
-    float basis[16];   // (the SH constants are folded in below: 16 multiplies instead of 48)
     basis[0] = 1.0f;
     basis[1] = y; basis[2] = z; basis[3] = x;
     basis[4] = x * y; basis[5] = y * z; basis[6] = (2.0f * zz - xx) - yy;
@@ -423,6 +436,13 @@ __device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3
     basis[15] = x * (xx - 3.0f * yy);
 #pragma unroll
     for (int kk = 0; kk < 16; ++kk) basis[kk] *= c_shc[kk];
+}
+
+// RasterizeMode::Color: the SH-3 colour seen along the camera ray in the splat's model frame
+__device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3][3], const float pw[3], const float sh[48],
+                                          float rgb[3]) {
+    float basis[16];
+    sh_basis(fc, A, pw, basis);
 #pragma unroll
     for (int cc = 0; cc < 3; ++cc) {
         float acc = 0.5f;
@@ -523,13 +543,14 @@ __device__ __forceinline__ void class_colour(const ModeConsts& mc, float vis, fl
     for (int cc = 0; cc < 3; ++cc) rgb[cc] = rgb[cc] * (1.0f - 0.5f) + h[cc] * 0.5f;   // mix(sh, hue, 0.5)
 }
 
-// RasterizeMode::OpticalFlow (gaussian.wgsl:201,369-375, material/optical_flow.wgsl:16-53): the screen motion of the
-// transformed position pw between the previous and this clip_from_world, per second, as hue = direction and
-// saturation = speed (clamped to 1)
-__device__ __forceinline__ void flow_colour(const FrameConsts& fc, const ModeConsts& mc, const float pw[3], float rgb[3]) {
+// RasterizeMode::OpticalFlow (gaussian.wgsl:201,369-375, material/optical_flow.wgsl:16-53): the screen motion between
+// pw_prev under the previous and pw under this clip_from_world, per second, as hue = direction and saturation = speed
+// (clamped to 1).  3D splats pass their transformed position as both; a 4D splat its moved and its unmoved one
+__device__ __forceinline__ void flow_colour_from(const FrameConsts& fc, const ModeConsts& mc, const float pw[3],
+                                                 const float pw_prev[3], float rgb[3]) {
     float c[4], cp[4];
     mat4_point(fc.clip_from_world, pw[0], pw[1], pw[2], c);
-    mat4_point(mc.prev_clip_from_world, pw[0], pw[1], pw[2], cp);
+    mat4_point(mc.prev_clip_from_world, pw_prev[0], pw_prev[1], pw_prev[2], cp);
     const float mvx = (c[0] / c[3] - cp[0] / cp[3]) * 0.5f;
     const float mvy = (c[1] / c[3] - cp[1] / cp[3]) * -0.5f;
     const float fx = mvx / mc.delta_time, fy = mvy / mc.delta_time;
@@ -537,6 +558,9 @@ __device__ __forceinline__ void flow_colour(const FrameConsts& fc, const ModeCon
     float angle = det_atan2(fy, fx);
     if (angle < 0.0f) angle = angle + PI_2_F;
     hsv_to_rgb(angle, fminf(fmaxf(radius, 0.0f), 1.0f), 1.0f, rgb);
+}
+__device__ __forceinline__ void flow_colour(const FrameConsts& fc, const ModeConsts& mc, const float pw[3], float rgb[3]) {
+    flow_colour_from(fc, mc, pw, pw, rgb);
 }
 
 // DrawMode::HighlightSelected (gaussian.wgsl:423-427): a selected splat is drawn opaque and green in every colour source
@@ -697,6 +721,225 @@ project_modes_kernel(const void* __restrict__ blocks, const uint32_t* __restrict
     // OpticalFlow reads the position only
     project_groups<F16, true>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs,
                               extra, cutoff_tab, nullptr, mc);
+}
+
+// ---- Gaussian4d (bgs_render_4d; the rule is include/bgs.h's).  Matrices [col][row], as WGSL indexes them.
+
+// gaussian_4d.wgsl:37-130: Sigma of the 4D gaussian conditioned on time t
+struct Cond4d {
+    float c3[6];       // the conditioned 3D covariance, WGSL [0][0], [0][1], [0][2], [1][1], [1][2], [2][2]
+    float dm[3];       // delta_mean
+    float marginal;    // marginal_t
+    bool mask;         // marginal_t > 0.05 (false for NaN)
+};
+__device__ __forceinline__ Cond4d condition_4d(float gs, const float ql[4], const float qr[4], const float so[4], float timestamp,
+                                               float timescale, float t) {
+    Cond4d g;
+    const float dt = t - timestamp;
+    const float sd[4] = {gs * so[0], gs * so[1], gs * so[2], timescale};
+    const float w = ql[0], x = ql[1], y = ql[2], z = ql[3];
+    const float wr = qr[0], xr = qr[1], yr = qr[2], zr = qr[3];
+    const float Ml[4][4] = {{w, -x, -y, -z}, {x, w, -z, y}, {y, z, w, -x}, {z, -y, x, w}};
+    const float Mr[4][4] = {{wr, -xr, -yr, -zr}, {xr, wr, zr, -yr}, {yr, -zr, wr, xr}, {zr, yr, -xr, wr}};
+    float M[4][4];   // M = (M_r * M_l) * S: R[c][r] = sum_k M_r[k][r] M_l[c][k], then column c times S[c][c]
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+            M[c][r] = (((Mr[0][r] * Ml[c][0] + Mr[1][r] * Ml[c][1]) + Mr[2][r] * Ml[c][2]) + Mr[3][r] * Ml[c][3]) * sd[c];
+    // Sigma = transpose(M) * M: Sigma[c][r] = sum_k M[r][k] M[c][k]
+    auto sig = [&](int c, int r) {
+        return ((M[r][0] * M[c][0] + M[r][1] * M[c][1]) + M[r][2] * M[c][2]) + M[r][3] * M[c][3];
+    };
+    const float cov_t = sig(3, 3);
+    g.marginal = det_exp(((-0.5f * dt) * dt) / cov_t);
+    g.mask = g.marginal > 0.05f;
+#pragma unroll
+    for (int i = 0; i < 6; ++i) g.c3[i] = 0.0f;
+    g.dm[0] = g.dm[1] = g.dm[2] = 0.0f;
+    if (!g.mask) return g;
+    const float c12[3] = {sig(0, 3), sig(1, 3), sig(2, 3)};
+    auto cond = [&](int c, int r) { return sig(c, r) - (c12[c] * c12[r]) / cov_t; };
+    g.c3[0] = cond(0, 0); g.c3[1] = cond(0, 1); g.c3[2] = cond(0, 2);
+    g.c3[3] = cond(1, 1); g.c3[4] = cond(1, 2); g.c3[5] = cond(2, 2);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) g.dm[i] = (c12[i] / cov_t) * dt;
+    return g;
+}
+
+// spherindrical_harmonics.wgsl:11-126: the SH-3 colour plus cos(2 pi theta) and cos(4 pi theta) times the second and
+// third 48 coefficients, theta = dt / duration.  The coefficients stream from the block (gaussian-major, 36 chunks from
+// sh) a chunk at a time: only drawn splats of the colour sources that read them ever fetch them.
+constexpr float PI_F = 3.14159274f;   // radians(180.0) in f32
+__device__ __forceinline__ void spherindrical_colour(const FrameConsts& fc, const TemporalConsts& tc, const float A[3][3],
+                                                     const float pw[3], float dt, const uint4* __restrict__ sh, float rgb[3]) {
+    float basis[16];
+    sh_basis(fc, A, pw, basis);
+    float acc[3][3];   // [section][channel]: the SH-3 colour (from 0.5), then the two time sums (from 0)
+#pragma unroll
+    for (int t = 0; t < 3; ++t) { acc[t][0] = t ? 0.0f : 0.5f; acc[t][1] = acc[t][0]; acc[t][2] = acc[t][0]; }
+#pragma unroll
+    for (int q = 0; q < 36; ++q) {
+        const uint4 v = __ldg(sh + q);
+        const float f[4] = {__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w)};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int j = 4 * q + e, t = j / 48, k = (j % 48) / 3, cc = j % 3;
+            acc[t][cc] = fmaf(f[e], basis[k], acc[t][cc]);   // colour: FMA is fine
+        }
+    }
+    const float theta = dt / tc.duration;
+    const float t1 = det_cos((2.0f * PI_F) * theta), t2 = det_cos((4.0f * PI_F) * theta);
+#pragma unroll
+    for (int cc = 0; cc < 3; ++cc) {
+        rgb[cc] = (acc[0][cc] + t1 * acc[1][cc]) + t2 * acc[2][cc];
+        if (fc.color_space == 0u) rgb[cc] = srgb_to_linear(rgb[cc]);
+    }
+}
+
+// RasterizeMode::Velocity (gaussian.wgsl:378-405): the splat's velocity in the local frame by a forward difference of
+// 1e-3; opacity 0 (and rgb 0: the reference's NaN) below 1 % of the magnitude scale
+__device__ __forceinline__ void velocity_colour(const Cond4d& now, const Cond4d& fut, float rgb[3], float& opacity) {
+    float v[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) v[i] = ((fut.mask ? fut.dm[i] : 0.0f) - now.dm[i]) / 1.0e-3f;
+    const float len = sqrtf((v[0] * v[0] + v[1] * v[1]) + v[2] * v[2]);
+    const float scaled = fminf(fmaxf((len - 1.0f) / (2.0f - 1.0f), 0.0f), 1.0f);
+    if (scaled < 1.0e-2f) {
+        opacity = 0.0f;
+        rgb[0] = rgb[1] = rgb[2] = 0.0f;
+        return;
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) rgb[i] = (0.5f * (v[i] / len + 1.0f)) * scaled;
+}
+
+// One entry of the index list of a 4D cloud -> its record at recs[r] (and, on depth-tested frames, its splat depth).
+// Undrawn (outside the frustum at the base position, unselected under DrawMode::Selected, masked by time, or outside
+// the frustum at the moved position): the base position's centre, the stored opacity, an empty bbox and no colour.
+__device__ __forceinline__ void project_one_4d(const FrameConsts& fc, const ModeConsts& mc, const TemporalConsts& tc,
+                                               const FrameCounters* __restrict__ ctr, uint32_t r, float4 p4, const float ql[4],
+                                               const float qr[4], const float so[4], const float tt[4],
+                                               const uint4* __restrict__ sh, SplatRec* __restrict__ recs,
+                                               float* __restrict__ depths) {
+    SplatRec rec;
+    rec.ux = 0.f; rec.uy = 0.f; rec.vx = 0.f; rec.vy = 0.f;
+    rec.bx = BBOX_EMPTY; rec.by = BBOX_EMPTY;
+    rec.r = 0.f; rec.g = 0.f; rec.b = 0.f;
+    float pw[4], ndc[2];
+    mat4_point(fc.model, p4.x, p4.y, p4.z, pw);
+    const bool visible = in_frustum(fc, pw, ndc);   // every depth width culls on the base position (include/bgs.h)
+    const float hw = 0.5f * fc.W, hh = 0.5f * fc.H;
+    rec.cx = ndc[0] * hw + hw;
+    rec.cy = hh - ndc[1] * hh;
+    const float opacity = so[3];
+    rec.op = opacity * fc.global_opacity;
+    float pm[4] = {pw[0], pw[1], pw[2], pw[3]};   // the position the record's centre comes from
+    if (visible && !(fc.draw_mode == BGS_DRAW_SELECTED && p4.w < 0.5f)) {
+        const float cutoff = splat_cutoff<false>(fc, opacity, nullptr, 0u);   // from the stored opacity
+        const Cond4d g = condition_4d(fc.global_scale, ql, qr, so, tt[0], tt[1], tc.time);
+        float nm[2];
+        if (g.mask) mat4_point(fc.model, p4.x + g.dm[0], p4.y + g.dm[1], p4.z + g.dm[2], pm);
+        if (g.mask && in_frustum(fc, pm, nm)) {
+            rec.cx = nm[0] * hw + hw;
+            rec.cy = hh - nm[1] * hh;
+            float op = opacity * g.marginal;
+            const Cov2d v = cov2d(fc, pm, g.c3);   // (the model 3x3 does not touch cov3d)
+            if (fc.aabb) aabb_record(fc, v, cutoff, rec);
+            else obb_record(fc, v, cutoff, rec);
+            float A[3][3];
+#pragma unroll
+            for (int rr = 0; rr < 3; ++rr)
+#pragma unroll
+                for (int cc = 0; cc < 3; ++cc) A[rr][cc] = fc.model[cc * 4 + rr];
+            const uint32_t mode = fc.rasterize_mode;
+            float rgb[3] = {0.f, 0.f, 0.f};
+            if (mode == BGS_RASTERIZE_COLOR || mode == BGS_RASTERIZE_CLASSIFICATION) {
+                spherindrical_colour(fc, tc, A, pm, tc.time - tt[0], sh, rgb);
+                if (mode == BGS_RASTERIZE_CLASSIFICATION) class_colour(mc, p4.w, rgb);
+            } else if (mode == BGS_RASTERIZE_DEPTH) {
+                depth_colour(fc, ctr, pm, rgb);
+            } else if (mode == BGS_RASTERIZE_POSITION) {
+                position_colour(fc, pm, rgb);
+            } else if (mode == BGS_RASTERIZE_OPTICAL_FLOW) {
+                flow_colour_from(fc, mc, pm, pw, rgb);   // the previous position is the unmoved one (gaussian.wgsl:201)
+            } else {
+                const Cond4d fut = condition_4d(fc.global_scale, ql, qr, so, tt[0], tt[1], tc.time_future);
+                velocity_colour(g, fut, rgb, op);
+            }
+            rec.r = rgb[0]; rec.g = rgb[1]; rec.b = rgb[2];
+            rec.op = op * fc.global_opacity;
+            float unused[3];
+            if (fc.draw_mode == BGS_DRAW_HIGHLIGHT_SELECTED && p4.w > 0.5f) highlight_selected(rec, unused, unused);
+        } else {
+            pm[0] = pw[0]; pm[1] = pw[1]; pm[2] = pw[2];
+        }
+    }
+    store_rec(recs + r, rec);
+    if (depths) depths[r] = splat_depth(fc, pm);
+}
+
+// The 4D block is 768 B: a warp stages only each entry's first 128 B line (position, both rotations, scale-opacity,
+// timestamp-timescale; 4 KB per warp) with the coalesced copies of project_groups, piece p of entry g at
+// g * GEO4 + (p ^ (g & 7)).  The coefficients stay in global memory until a drawn splat's colour needs them.
+constexpr int CH4 = (int)chunks(CloudLayout::F32x4D), GEO4 = 8;
+__global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
+project_4d_kernel(const uint4* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
+                  const FrameCounters* __restrict__ ctr, FrameConsts fc, ModeConsts mc, TemporalConsts tc,
+                  SplatRec* __restrict__ recs, float* __restrict__ depths /* depth-tested frames only */) {
+    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * GEO4];
+    const int lane = threadIdx.x & 31;
+    uint4* const stage = s_stages[threadIdx.x >> 5];
+    const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
+    auto list_id = [&](uint32_t r) {
+        return r < n_vis ? (by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r))) : 0u;
+    };
+    auto gather = [&](uint32_t r0, uint32_t id) {   // one commit group per call, empty past the list's end
+        const uint32_t n_valid = r0 < n_vis ? n_vis - r0 : 0u;
+#pragma unroll
+        for (int k = 0; k < GEO4; ++k) {
+            const int g = (32 * k + lane) / GEO4, p = lane % GEO4;
+            const uint32_t gid = __shfl_sync(0xFFFFFFFFu, id, g);
+            if ((uint32_t)g < n_valid) cp_async16(stage + g * GEO4 + (p ^ (g & 7)), blocks + (size_t)gid * CH4 + p);
+        }
+        cp_async_commit();
+    };
+    uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
+    uint32_t id = list_id(r0 + lane);
+    gather(r0, id);
+    uint32_t id_next = list_id(r0 + stride + lane);
+    for (; r0 < n_vis; r0 += stride) {
+        cp_async_wait<0>();
+        __syncwarp();
+        const uint32_t r = r0 + lane;
+        auto piece = [&](int p) {
+            const uint4 v = stage[lane * GEO4 + (p ^ (lane & 7))];
+            return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
+        };
+        const float4 p4 = piece(POS_CHUNK), a = piece(SECOND_CHUNK), b = piece(ROT_R_CHUNK), c = piece(SO_4D_CHUNK),
+                     d = piece(TT_CHUNK);
+        __syncwarp();   // the stage is read out before the next group's copies overwrite it
+        const uint32_t my_id = id;
+        gather(r0 + stride, id_next);
+        id = id_next;
+        id_next = list_id(r0 + 2u * stride + lane);
+        if (r < n_vis) {
+            const float ql[4] = {a.x, a.y, a.z, a.w}, qr[4] = {b.x, b.y, b.z, b.w}, so[4] = {c.x, c.y, c.z, c.w},
+                        tt[4] = {d.x, d.y, d.z, d.w};
+            project_one_4d(fc, mc, tc, ctr, r, p4, ql, qr, so, tt, blocks + (size_t)my_id * CH4 + sh_first(CloudLayout::F32x4D),
+                           recs, depths);
+        }
+    }
+}
+
+void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+                       const FrameConsts& fc, const ModeConsts& mc, const TemporalConsts& tc, SplatRec* recs, float* depths,
+                       uint32_t n_hint, int sm_count, cudaStream_t stream) {
+    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
+    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
+    if (grid < 1u) grid = 1u;
+    project_4d_kernel<<<grid, PROJ_THREADS, 0, stream>>>(static_cast<const uint4*>(blocks), index_list, by_slot, ctr, fc, mc, tc,
+                                                         recs, depths);
 }
 
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,

@@ -122,4 +122,45 @@ __device__ __forceinline__ float det_ln(float xf) {
     return (float)r;   // cvt.rn.f32.f64
 }
 
+// Fixed-series exp in f64 (the policy replacement for WGSL exp, gaussian_4d.wgsl's marginal_t), shared with the oracle:
+// x = k ln2 + r, k = rint(x / ln2), r = x - k ln2 (|r| <= 0.35); e^r by its Taylor polynomial to degree 16 (remainder
+// < 1e-20), coefficients 1 / j! built by repeated division; times 2^k exactly; rounded to f32.  Below -110 the f32
+// result is 0, above 89 it is +inf.
+__device__ __forceinline__ float det_exp(float xf) {
+    if (xf != xf) return xf;
+    if (xf < -110.0f) return 0.0f;
+    if (xf > 89.0f) return __uint_as_float(0x7F800000u);
+    const double x = (double)xf;
+    const double k = rint(__dmul_rn(x, 1.4426950408889634));
+    const double r = __dsub_rn(x, __dmul_rn(k, 0.6931471805599453));
+    double c[17];
+    c[0] = 1.0;
+#pragma unroll
+    for (int j = 1; j <= 16; ++j) c[j] = c[j - 1] / (double)j;   // (folded by the compiler, IEEE)
+    double p = c[16];
+#pragma unroll
+    for (int j = 15; j >= 0; --j) p = __dadd_rn(__dmul_rn(p, r), c[j]);
+    const double scale = __longlong_as_double((long long)((unsigned long long)((int)k + 1023) << 52));
+    return (float)__dmul_rn(p, scale);   // cvt.rn.f32.f64
+}
+
+// Fixed-series cos in f64 (the policy replacement for WGSL cos, spherindrical_harmonics.wgsl's time terms), shared with
+// the oracle: r = x - k 2pi, k = rint(x / 2pi) (|r| <= pi + rounding); cos r = P(r^2) by its Taylor polynomial to degree
+// 36 (remainder < 1e-24), coefficients (-1)^j / (2j)! built by repeated division; rounded to f32.  Not finite: NaN.
+__device__ __forceinline__ float det_cos(float xf) {
+    if (!(fabsf(xf) < __uint_as_float(0x7F800000u))) return __uint_as_float(0x7FC00000u);
+    const double x = (double)xf;
+    const double k = rint(__dmul_rn(x, 0.15915494309189535));
+    const double r = __dsub_rn(x, __dmul_rn(k, 6.283185307179586));
+    const double z = __dmul_rn(r, r);
+    double c[19];
+    c[0] = 1.0;
+#pragma unroll
+    for (int j = 1; j <= 18; ++j) c[j] = -c[j - 1] / (double)((2 * j - 1) * (2 * j));   // (folded, IEEE)
+    double p = c[18];
+#pragma unroll
+    for (int j = 17; j >= 0; --j) p = __dadd_rn(__dmul_rn(p, z), c[j]);
+    return (float)p;
+}
+
 }  // namespace bgs

@@ -92,10 +92,16 @@ __global__ void __launch_bounds__(SUBSET_THREADS) subset_scatter_kernel(CloudVie
     const uint32_t before = lane < warp ? __popc(mask[blockIdx.x * SUBSET_WORDS_PER_CTA + lane]) : 0u;
     const uint32_t base = cta_off[blockIdx.x] + __reduce_add_sync(0xFFFFFFFFu, before);
     const uint32_t m = mask[word];
-    const uint32_t k = __popc(m), c = lane % CH;
-    for (uint32_t j0 = 0; j0 < k; j0 += G) {
-        const uint32_t j = j0 + lane / CH;
-        if (j < k) subset_copy<CH>(src, word * 32u + __fns(m, 0, (int)j + 1), base + j, c, dst);
+    const uint32_t k = __popc(m);
+    if constexpr (G == 0) {   // (a block wider than a warp, the 4D layout's: the warp copies one gaussian at a time)
+        for (uint32_t j = 0; j < k; ++j)
+            for (uint32_t c = lane; c < CH; c += 32u) subset_copy<CH>(src, word * 32u + __fns(m, 0, (int)j + 1), base + j, c, dst);
+    } else {
+        const uint32_t c = lane % CH;
+        for (uint32_t j0 = 0; j0 < k; j0 += G) {
+            const uint32_t j = j0 + lane / CH;
+            if (j < k) subset_copy<CH>(src, word * 32u + __fns(m, 0, (int)j + 1), base + j, c, dst);
+        }
     }
 }
 
@@ -111,12 +117,22 @@ __global__ void __launch_bounds__(SUBSET_THREADS) subset_gather_kernel(CloudView
 // repack_kernel's inverse over gaussians [lo, lo + m): block chunk c of gaussian lo + j goes back to its unit of
 // gaussian j in the planes (planes.pos is null: the position plane is read back directly).
 template <CloudLayout L>
-__global__ void __launch_bounds__(SUBSET_THREADS) unpack_kernel(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
-                                                                CloudPlanes<uint4> planes) {
+__device__ __forceinline__ void unpack_chunk(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
+                                             const CloudPlanes<uint4>& planes, uint4* __restrict__ tt) {
     const size_t t = (size_t)blockIdx.x * SUBSET_THREADS + threadIdx.x;
     if (t >= (size_t)m * chunks(L)) return;
-    uint4* dst = planes.unit<L>((uint32_t)(t % chunks(L)), t / chunks(L));
+    uint4* dst = planes.unit<L>((uint32_t)(t % chunks(L)), t / chunks(L), tt);
     if (dst) *dst = __ldg(blocks + (size_t)lo * chunks(L) + t);
+}
+template <CloudLayout L>
+__global__ void __launch_bounds__(SUBSET_THREADS) unpack_kernel(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
+                                                                CloudPlanes<uint4> planes) {
+    unpack_chunk<L>(blocks, lo, m, planes, nullptr);
+}
+// the 4D layout's, which also writes the timestamp-timescale plane
+__global__ void __launch_bounds__(SUBSET_THREADS) unpack_4d_kernel(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
+                                                                   CloudPlanes<uint4> planes, uint4* __restrict__ tt) {
+    unpack_chunk<CloudLayout::F32x4D>(blocks, lo, m, planes, tt);
 }
 
 uint32_t subset_num_ctas(uint32_t n) { return (n + SUBSET_THREADS - 1) / SUBSET_THREADS; }
@@ -127,7 +143,8 @@ void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t
     subset_scan_kernel<<<1, 1024, 0, stream>>>(cta_cnt, g, total);
 }
 
-// (the copies depend on the layout only through the block's size: both f16 layouts run the same kernels)
+// (the copies depend on the layout only through the block's size: both f16 layouts run the same kernels, and the 4D
+// layout's 48-chunk blocks a warp-wide variant of the scatter)
 void launch_subset_scatter(CloudLayout layout, CloudView src, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
                            CloudView dst, cudaStream_t stream) {
     const uint32_t g = subset_num_ctas(n), words = (n + 31) / 32;
@@ -146,10 +163,15 @@ void launch_subset_gather(CloudLayout layout, CloudView src, const uint32_t* idx
     });
 }
 
-void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, cudaStream_t stream) {
+void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, void* tt,
+                   cudaStream_t stream) {
     const CloudPlanes<uint4> planes{nullptr, static_cast<uint4*>(sh), static_cast<uint4*>(rot), static_cast<uint4*>(so)};
+    const uint32_t grid = chunk_grid(m, cloud.chunks);
     with_layout(layout, [&](auto L) {
-        unpack_kernel<decltype(L)::value><<<chunk_grid(m, cloud.chunks), SUBSET_THREADS, 0, stream>>>(cloud.blocks, lo, m, planes);
+        if constexpr (is_4d(decltype(L)::value))
+            unpack_4d_kernel<<<grid, SUBSET_THREADS, 0, stream>>>(cloud.blocks, lo, m, planes, static_cast<uint4*>(tt));
+        else
+            unpack_kernel<decltype(L)::value><<<grid, SUBSET_THREADS, 0, stream>>>(cloud.blocks, lo, m, planes);
     });
 }
 

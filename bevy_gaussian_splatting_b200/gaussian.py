@@ -153,6 +153,66 @@ def random_gaussians_3d(n: int) -> PlanarGaussian3d:
     return random_gaussians_3d_seeded(n, 0)
 
 
+SH_4D_COEFF_COUNT = 144  # src/material/spherindrical_harmonics.rs: SH-3 colour times time degree 2
+
+
+@dataclasses.dataclass
+class PlanarGaussian4d:
+    """src/gaussian/formats/planar_4d.rs:38-51: the five planes `bgs_cloud_upload_4d` borrows."""
+    position_visibility: np.ndarray     # (n, 4) f32: x, y, z, visibility
+    spherindrical_harmonic: np.ndarray  # (n, 144) f32: SH-3 colour (0..47), cos(2 pi t) set (48..95), cos(4 pi t) set
+    isotropic_rotations: np.ndarray     # (n, 8) f32: rotation (w, x, y, z), rotation_r (w, x, y, z); not normalised
+    scale_opacity: np.ndarray           # (n, 4) f32: sx, sy, sz, opacity
+    timestamp_timescale: np.ndarray     # (n, 4) f32: timestamp, timescale, pad, pad
+
+    def __post_init__(self):
+        for name, width in (("position_visibility", 4), ("spherindrical_harmonic", SH_4D_COEFF_COUNT),
+                            ("isotropic_rotations", 8), ("scale_opacity", 4), ("timestamp_timescale", 4)):
+            a = np.ascontiguousarray(getattr(self, name), dtype=np.float32)
+            if a.ndim != 2 or a.shape[1] != width:
+                raise ValueError(f"{name} must have shape (n, {width})")
+            setattr(self, name, a)
+        n = len(self.position_visibility)
+        if not all(len(getattr(self, f.name)) == n for f in dataclasses.fields(self)):
+            raise ValueError("planes disagree on n")
+
+    def __len__(self) -> int:
+        return len(self.position_visibility)
+
+    def planes(self) -> tuple[np.ndarray, ...]:
+        return tuple(getattr(self, f.name) for f in dataclasses.fields(self))
+
+    def subset(self, n) -> "PlanarGaussian4d":
+        """An int: the first n gaussians.  An index array: those gaussians, in that order."""
+        idx = slice(0, n) if np.ndim(n) == 0 else np.asarray(n)
+        return PlanarGaussian4d(*(a[idx] for a in self.planes()))
+
+    def compute_aabb(self) -> tuple[np.ndarray, np.ndarray]:
+        return compute_aabb(self.position_visibility)
+
+
+def random_gaussians_4d_seeded(n: int, seed: int = 0, chunk: int = 1 << 16) -> PlanarGaussian4d:
+    """planar_4d.rs:244-289 (distributions + field order: 144 coefficients U(-1,1); both rotations 8xU(-1,1),
+    unnormalised; position 3xU(-20,20), visibility 1; scale 3xU(0,1), opacity U(0,0.8); timestamp U(0,1), timescale
+    U(-1,1), pads 0), Philox stream, deterministic in (n, seed)."""
+    rng = np.random.Generator(np.random.Philox(seed))
+    planes = (np.empty((n, 4), np.float32), np.empty((n, SH_4D_COEFF_COUNT), np.float32), np.empty((n, 8), np.float32),
+              np.empty((n, 4), np.float32), np.zeros((n, 4), np.float32))
+    pos, sh, rot, so, tt = planes
+    for lo in range(0, n, chunk):
+        hi = min(n, lo + chunk)
+        u = rng.random((chunk, 163), dtype=np.float32)[: hi - lo]  # always draw whole chunks: stream is n-independent
+        sh[lo:hi] = u[:, 0:144] * 2.0 - 1.0
+        rot[lo:hi] = u[:, 144:152] * 2.0 - 1.0
+        pos[lo:hi, 0:3] = u[:, 152:155] * 40.0 - 20.0
+        pos[lo:hi, 3] = 1.0
+        so[lo:hi, 0:3] = u[:, 155:158]
+        so[lo:hi, 3] = u[:, 158] * 0.8
+        tt[lo:hi, 0] = u[:, 159]
+        tt[lo:hi, 1] = u[:, 160] * 2.0 - 1.0
+    return PlanarGaussian4d(*planes)
+
+
 def test_model(seed: int = 0) -> PlanarGaussian3d:
     """planar_3d.rs:193-251: 8 corner gaussians at (+-0.5)^3 + a repeat of the first, shuffled SH."""
     rng = np.random.Generator(np.random.Philox(seed))

@@ -18,7 +18,7 @@ import os
 
 import numpy as np
 
-from .gaussian import PlanarGaussian3d, SH_COEFF_COUNT
+from .gaussian import PlanarGaussian3d, PlanarGaussian4d, SH_COEFF_COUNT, SH_4D_COEFF_COUNT
 
 MAX_SIZE_VARIANCE = 4.0
 SH_CHANNELS = 3
@@ -171,10 +171,100 @@ def write_ply_3d(path, cloud: PlanarGaussian3d, n: int | None = None) -> None:
         f.write(arr.tobytes())
 
 
-def load_cloud(path) -> PlanarGaussian3d:
-    """`Gaussian3dLoader::load` (src/io/loader.rs:24-70): `.ply` -> parse_ply_3d, `.gcloud` -> CloudCodec::decode,
-    anything else is an error ("only .ply and .gcloud supported")."""
+# ply.rs:134-182: the float properties of a Gaussian4d vertex -> (plane, column)
+PLY4D_PROPERTIES = {"x": (0, 0), "y": (0, 1), "z": (0, 2), "visibility": (0, 3), "t": (4, 0), "st": (4, 1),
+                    "sx": (3, 0), "sy": (3, 1), "sz": (3, 2), "opacity": (3, 3),
+                    "rot_x": (2, 0), "rot_y": (2, 1), "rot_z": (2, 2), "rot_w": (2, 3),
+                    "rot_r_x": (2, 4), "rot_r_y": (2, 5), "rot_r_z": (2, 6), "rot_r_w": (2, 7)}
+PLY4D_REQUIRED = ["x", "y", "z", "t", "st", "sx", "sy", "sz", "opacity", "rot_x", "rot_y", "rot_z", "rot_w",
+                  "rot_r_x", "rot_r_y", "rot_r_z", "rot_r_w"]
+
+
+def parse_ply_4d(source) -> PlanarGaussian4d:
+    """ply.rs:134-247, `parse_ply_4d`: float properties only (others are ignored, as the reference's match ignores
+    them); feat_{r,g,b}_{i} -> coefficient 3 i + channel (ignored past 144); the required properties above or
+    ValueError; both quaternions divided by their norms, lanes in the file's rot_x, rot_y, rot_z, rot_w order (lane 0,
+    read by the shader as w, is rot_x); padded with default gaussians (visibility 1, all else 0) by 32 - (n % 32)."""
+    if isinstance(source, (str, os.PathLike)):
+        with open(source, "rb") as fh:
+            return parse_ply_4d(fh.read())
+    try:
+        return _parse_ply_4d(source)
+    except (TypeError, IndexError, KeyError, UnicodeDecodeError, OverflowError, MemoryError) as e:
+        raise ValueError(f"malformed ply4d: {type(e).__name__}: {e}") from e
+
+
+def _parse_ply_4d(source) -> PlanarGaussian4d:
+    f = io.BytesIO(source) if isinstance(source, (bytes, bytearray)) else source
+    fmt, elements = _read_header(f)
+    if fmt != "binary_little_endian":
+        raise ValueError(f"only binary_little_endian PLY is supported, got {fmt}")
+    planes = [np.zeros((0, w), np.float32) for w in (4, SH_4D_COEFF_COUNT, 8, 4, 4)]
+    for el in elements:
+        if any(isinstance(t, tuple) for _, t in el["props"]):
+            raise ValueError("list properties are not supported")
+        dt = np.dtype([(name, "<" + t) for name, t in el["props"]])
+        data = np.frombuffer(f.read(dt.itemsize * el["count"]), dt, count=el["count"])
+        if el["name"] != "vertex":
+            continue
+        names = [name for name, _ in el["props"]]
+        if any(r not in names for r in PLY4D_REQUIRED):
+            raise ValueError("missing required properties")
+        n = el["count"]
+        planes = [np.zeros((n, w), np.float32) for w in (4, SH_4D_COEFF_COUNT, 8, 4, 4)]
+        planes[0][:, 3] = 1.0
+        for name, t in el["props"]:
+            if t != "f4":
+                continue
+            if name in PLY4D_PROPERTIES:
+                k, c = PLY4D_PROPERTIES[name]
+                planes[k][:, c] = data[name]
+            elif name.startswith("feat_"):
+                channel = "rgb".index(name[5])
+                idx = int(name[7:]) * 3 + channel
+                if idx < SH_4D_COEFF_COUNT:
+                    planes[1][:, idx] = data[name]
+    rot = planes[2]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        for lo in (0, 4):
+            q = rot[:, lo:lo + 4]
+            norm = np.sqrt(np.sum(q * q, axis=1, dtype=np.float32), dtype=np.float32)
+            rot[:, lo:lo + 4] = (q / norm[:, None]).astype(np.float32)
+    pad = 32 - (len(rot) % 32)
+    out = []
+    for k, a in enumerate(planes):
+        z = np.zeros((pad, a.shape[1]), np.float32)
+        if k == 0:
+            z[:, 3] = 1.0
+        out.append(np.concatenate([a, z]))
+    return PlanarGaussian4d(*out)
+
+
+def write_ply_4d(path, cloud: PlanarGaussian4d, n: int | None = None) -> None:
+    """The first n gaussians of `cloud` as a binary .ply4d `parse_ply_4d` reads back (every property float)."""
+    n = len(cloud) if n is None else n
+    props = list(PLY4D_PROPERTIES) + [f"feat_{'rgb'[i % 3]}_{i // 3}" for i in range(SH_4D_COEFF_COUNT)]
+    arr = np.zeros(n, np.dtype([(p, "<f4") for p in props]))
+    planes = cloud.planes()
+    for name, (k, c) in PLY4D_PROPERTIES.items():
+        arr[name] = planes[k][:n, c]
+    for i in range(SH_4D_COEFF_COUNT):
+        arr[f"feat_{'rgb'[i % 3]}_{i // 3}"] = planes[1][:n, i]
+    with open(path, "wb") as f:
+        f.write(("ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % n).encode())
+        for p in props:
+            f.write(f"property float {p}\n".encode())
+        f.write(b"end_header\n")
+        f.write(arr.tobytes())
+
+
+def load_cloud(path) -> PlanarGaussian3d | PlanarGaussian4d:
+    """`Gaussian3dLoader::load` (src/io/loader.rs:24-70): `.ply` -> parse_ply_3d, `.gcloud` -> CloudCodec::decode;
+    `Gaussian4dLoader::load` (loader.rs:69-115): `.ply4d` -> parse_ply_4d (`.gc4d` is not read here); anything else is
+    an error."""
     ext = os.path.splitext(str(path))[1].lower()
+    if ext == ".ply4d":
+        return parse_ply_4d(path)
     if ext == ".ply":
         return parse_ply_3d(path)
     if ext == ".gcloud":

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import abi
 from .camera import GaussianCamera, View
-from .gaussian import PlanarGaussian3d, compute_aabb
+from .gaussian import PlanarGaussian3d, PlanarGaussian4d, compute_aabb
 from .particles import PARTICLE_BEHAVIOR_DTYPE, as_particle_behaviors
 from .settings import CloudSettings, SparseSelect
 
@@ -136,6 +136,22 @@ class PlanarGaussian3dHandle:
             pass
 
 
+class PlanarGaussian4dHandle(PlanarGaussian3dHandle):
+    """A Gaussian4d cloud resident in HBM (`bgs_cloud_upload_4d`); `render_view` draws it through `bgs_render_4d` at
+    `settings.time` in the window [settings.time_start, settings.time_stop]."""
+
+    temporal = True
+
+    def __init__(self, plugin: "GaussianSplattingPlugin", cloud: PlanarGaussian4d):
+        PlanarGaussian3dHandle._next_serial += 1
+        self.serial = PlanarGaussian3dHandle._next_serial
+        self._plugin, self._lib = plugin, plugin._lib
+        self.n, self.f16, self.precompute_covariance = len(cloud), False, False
+        self.aabb = cloud.compute_aabb()
+        self._h = C.c_void_p()
+        plugin._check(self._lib.bgs_cloud_upload_4d(plugin._ctx, self.n, *(_ptr(a) for a in cloud.planes()), C.byref(self._h)))
+
+
 class ParticleBehaviorsHandle:
     """A `ParticleBehaviors` asset resident in HBM (`bgs_particles`): what the reference attaches to a cloud entity."""
 
@@ -180,7 +196,13 @@ class GaussianSplattingPlugin:
         self.device = cuda_device
 
     # -- resources
-    def add_cloud(self, cloud: PlanarGaussian3d, f16: bool = False, precompute_covariance: bool = False) -> PlanarGaussian3dHandle:
+    def add_cloud(self, cloud: PlanarGaussian3d | PlanarGaussian4d, f16: bool = False,
+                  precompute_covariance: bool = False) -> PlanarGaussian3dHandle:
+        """A PlanarGaussian4d cloud gives a PlanarGaussian4dHandle (f32 only: the reference has no f16 4D layout)."""
+        if isinstance(cloud, PlanarGaussian4d):
+            if f16 or precompute_covariance:
+                raise ValueError("add_cloud: a Gaussian4d cloud is stored in f32 only")
+            return PlanarGaussian4dHandle(self, cloud)
         return PlanarGaussian3dHandle(self, cloud, f16, precompute_covariance)
 
     def _check(self, st: int):
@@ -230,7 +252,9 @@ class GaussianSplattingPlugin:
             assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
         target = _ptr(out) if to_host else None
         zd = self._scene_depth(scene_depth, view)
-        if zd is not None:
+        if getattr(handle, "temporal", False):
+            st = self._render_4d(handle, v, u, s, ex, zd, settings, target, code, 0)
+        elif zd is not None:
             st = self._lib.bgs_render_depth_test(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s),
                                                  None if ex is None else C.byref(ex), C.byref(zd), target, code, 0)
         elif ex is None:
@@ -239,6 +263,11 @@ class GaussianSplattingPlugin:
             st = self._lib.bgs_render_ex(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.byref(ex), target, code, 0)
         self._check(st)
         return out if to_host else None
+
+    def _render_4d(self, handle, v, u, s, ex, zd, settings, target, code, is_device):
+        return self._lib.bgs_render_4d(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), None if ex is None else C.byref(ex),
+                                       None if zd is None else C.byref(zd), target, code, is_device, float(settings.time_start),
+                                       float(settings.time_stop))
 
     def _scene_depth(self, scene_depth, view):
         """The call's bgs_scene_depth; a buffer whose interface names its producer's stream is read only after the work
@@ -303,7 +332,9 @@ class GaussianSplattingPlugin:
         v = view.to_abi()
         u, s, ex = self._call_args(handle, settings, transform, asynchronous, premultiplied, blend_over, previous_view, delta_time)
         zd = self._scene_depth(scene_depth, view)
-        if zd is not None:
+        if getattr(handle, "temporal", False):
+            self._check(self._render_4d(handle, v, u, s, ex, zd, settings, C.c_void_p(device_ptr), code, 1))
+        elif zd is not None:
             self._check(self._lib.bgs_render_depth_test(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s),
                                                         None if ex is None else C.byref(ex), C.byref(zd),
                                                         C.c_void_p(device_ptr), code, 1))
@@ -403,12 +434,17 @@ class GaussianSplattingPlugin:
             self._check(self._lib.bgs_cloud_subset(self._ctx, handle._h, _ptr(idx), idx.size, C.byref(out), C.byref(n)))
         if not out:
             return None
-        return PlanarGaussian3dHandle._adopt(self, out, int(n.value), handle.f16, handle.precompute_covariance)
+        return type(handle)._adopt(self, out, int(n.value), handle.f16, handle.precompute_covariance)
 
     def download_planes(self, handle: PlanarGaussian3dHandle) -> tuple[np.ndarray, ...]:
         """The cloud's planes as the matching upload call takes them: f32 (pos_vis, sh, rotation, scale_opacity); f16
         and precomputed-covariance clouds (pos_vis, sh_packed, second plane words)."""
         pos = np.empty((handle.n, 4), np.float32)
+        if getattr(handle, "temporal", False):   # (pos_vis, sh, rotations, scale_opacity, timestamp_timescale)
+            planes = (pos, np.empty((handle.n, 144), np.float32), np.empty((handle.n, 8), np.float32),
+                      np.empty((handle.n, 4), np.float32), np.empty((handle.n, 4), np.float32))
+            self._check(self._lib.bgs_cloud_download_4d(self._ctx, handle._h, *(_ptr(a) for a in planes)))
+            return planes
         if handle.f16 or handle.precompute_covariance:
             sh, second = np.empty((handle.n, 24), np.uint32), np.empty((handle.n, 4), np.uint32)
             self._check(self._lib.bgs_cloud_download_f16(self._ctx, handle._h, _ptr(pos), _ptr(sh), _ptr(second)))
@@ -421,6 +457,8 @@ class GaussianSplattingPlugin:
         """The cloud as a host PlanarGaussian3d: f16 planes widened to f32 (`PlanarGaussian3d.from_f16`); a
         precomputed-covariance cloud holds its covariance in the slots `precomputed_covariance()` uses."""
         planes = self.download_planes(handle)
+        if len(planes) == 5:
+            return PlanarGaussian4d(*planes)
         return PlanarGaussian3d.from_f16(*planes) if len(planes) == 3 else PlanarGaussian3d(*planes)
 
     def save_selection(self, handle: PlanarGaussian3dHandle, path) -> int:

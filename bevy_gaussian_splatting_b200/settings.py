@@ -10,6 +10,8 @@ import dataclasses
 import enum
 from typing import Optional
 
+import numpy as np
+
 from . import abi
 
 
@@ -19,18 +21,20 @@ class DrawMode(enum.IntEnum):  # settings.rs:6-12
     HighlightSelected = 2
 
 
-class GaussianMode(enum.IntEnum):  # settings.rs:17-22 (Gaussian4d is out of scope, SURVEY §2 row 14)
+class GaussianMode(enum.IntEnum):  # settings.rs:17-22
     Gaussian2d = 0
     Gaussian3d = 1
+    Gaussian4d = 2       # PlanarGaussian4d clouds, through bgs_render_4d
 
 
-class RasterizeMode(enum.IntEnum):  # settings.rs:38-48 (all but Velocity, which needs Gaussian4d, are on the path)
+class RasterizeMode(enum.IntEnum):  # settings.rs:38-48
     Color = 0
     Depth = 1
     Normal = 2
     Position = 3
     Classification = 4   # the hue of class vis - 2 from the visibility lane, CloudSettings.num_classes hues
     OpticalFlow = 5      # camera motion since the previous view (render_view's previous_view / delta_time)
+    Velocity = 6         # Gaussian4d only: each splat's velocity at CloudSettings.time
 
 
 class RadixSortDepthBits(enum.IntEnum):  # settings.rs:50-77
@@ -45,6 +49,13 @@ class RadixSortDepthBits(enum.IntEnum):  # settings.rs:50-77
 class GaussianColorSpace(enum.IntEnum):  # settings.rs:79-84
     SrgbRec709Display = 0
     LinRec709Display = 1
+
+
+class PlaybackMode(enum.IntEnum):  # settings.rs:24-36
+    Loop = 0
+    Once = 1
+    Sin = 2
+    Still = 3
 
 
 class SortMode(enum.IntEnum):  # src/sort/mod.rs:46-74; only Radix exists here (no CPU fallback)
@@ -110,6 +121,9 @@ class CloudSettings:
     # (time - time_start) / (time_stop - time_start).  Last, so positional construction keeps its meaning
     time_start: float = 0.0
     time_stop: float = 1.0
+    # playback of a Gaussian4d cloud (settings.rs:110-111): how `playback_update` advances `time`
+    time_scale: float = 1.0
+    playback_mode: PlaybackMode = PlaybackMode.Still
 
     def to_abi(self) -> abi.bgs_settings:
         if self.visualize_bounding_box:
@@ -126,3 +140,24 @@ class CloudSettings:
             | (0 if self.binning_rounds is None else (abi.BGS_FLAG_CHUNKS if self.binning_rounds else abi.BGS_FLAG_NO_CHUNKS)),
             reserved=0,
         )
+
+
+def playback_update(settings: CloudSettings, delta_secs: float, elapsed_secs: float) -> None:
+    """settings.rs:145-191, the reference's playback_update for one cloud, in f32 as there: nothing when time_scale is
+    0 or the mode is Still, or in Once mode once time >= time_stop; Loop and Once add delta_secs * time_scale (Loop
+    then wraps to time_start past time_stop; Once is not clamped); Sin sets time = time_start + (time_stop -
+    time_start) * (sin(time_scale * elapsed_secs * 2 * PI) + 1) / 2.  np.sin of an f32 stands for Rust's f32 sin."""
+    f = np.float32
+    time, start, stop, scale = f(settings.time), f(settings.time_start), f(settings.time_stop), f(settings.time_scale)
+    mode = PlaybackMode(settings.playback_mode)
+    if scale == 0 or mode == PlaybackMode.Still or (mode == PlaybackMode.Once and time >= stop):
+        return
+    if mode in (PlaybackMode.Loop, PlaybackMode.Once):
+        time = f(time + f(f(delta_secs) * scale))
+        if mode == PlaybackMode.Loop and time > stop:
+            time = start
+    else:
+        theta = f(scale * f(elapsed_secs))
+        y = np.sin(f(f(theta * f(2.0)) * f(np.pi)), dtype=np.float32)
+        time = f(start + f(f(f(stop - start) * f(y + f(1.0))) / f(2.0)))
+    settings.time = float(time)

@@ -57,10 +57,11 @@ typedef struct {
 } bgs_cloud_uniform;
 
 /* CloudSettings / CloudPipelineKey (src/gaussian/settings.rs:90-133, render/mod.rs:898-909). */
-enum { BGS_GAUSSIAN_2D = 0, BGS_GAUSSIAN_3D = 1 };
+enum { BGS_GAUSSIAN_2D = 0, BGS_GAUSSIAN_3D = 1, BGS_GAUSSIAN_4D = 2 /* bgs_render_4d only */ };
 enum {
     BGS_RASTERIZE_COLOR = 0, BGS_RASTERIZE_DEPTH = 1, BGS_RASTERIZE_NORMAL = 2, BGS_RASTERIZE_POSITION = 3,
-    BGS_RASTERIZE_CLASSIFICATION = 4, BGS_RASTERIZE_OPTICAL_FLOW = 5   /* bgs_render_ex; Velocity (6) is out of scope */
+    BGS_RASTERIZE_CLASSIFICATION = 4, BGS_RASTERIZE_OPTICAL_FLOW = 5,   /* bgs_render_ex */
+    BGS_RASTERIZE_VELOCITY = 6                                           /* bgs_render_4d only */
 };
 enum { BGS_DRAW_ALL = 0, BGS_DRAW_SELECTED = 1, BGS_DRAW_HIGHLIGHT_SELECTED = 2 };
 enum {
@@ -246,6 +247,23 @@ bgs_status bgs_cloud_download_f32(bgs_context* ctx, const bgs_cloud* cloud, floa
                                   float* rot_wxyz /* n*4 */, float* scale_opacity /* n*4 */);
 bgs_status bgs_cloud_download_f16(bgs_context* ctx, const bgs_cloud* cloud, float* pos_vis /* n*4 */,
                                   uint32_t* sh_packed /* n*24 */, uint32_t* second_plane /* n*4 */);
+
+/* Gaussian4d clouds (planar_4d.rs:38-51, f32.rs:110-123,195-205; f32 only, as in the reference).  Per gaussian:
+ *   pos_vis n*4 (x, y, z, visibility); sh n*144 (the SH-3 colour times time degree 2: coefficients 0..47 as
+ *   bgs_cloud_upload_f32's, 48..95 the cos(2 pi theta) set, 96..143 the cos(4 pi theta) set, each interleaved RGB x 16);
+ *   rotations n*8 (rotation then rotation_r, each (w, x, y, z) in storage order, used exactly as given: not normalised);
+ *   scale_opacity n*4 (linear scale xyz, linear opacity); timestamp_timescale n*4 (timestamp, timescale, pad, pad).
+ * The cloud is stored as 768 B gaussian-major blocks beside the position plane.  bgs_cloud_download_4d returns the
+ * planes as uploaded, bit for bit for a cloud that was never edited (pads included).  bgs_cloud_subset,
+ * bgs_cloud_select_sparse, bgs_cloud_select_in_mesh, bgs_cloud_visibility_get / _set, bgs_cloud_positions_get and
+ * bgs_cloud_particles_step work on a 4D cloud as on a 3D one: they read and write the base position and visibility only.
+ * The download call of another layout, bgs_cloud_interpolate of 4D clouds, bgs_render, bgs_render_ex,
+ * bgs_render_depth_test and bgs_render_aux of a 4D cloud -> BGS_EINVAL. */
+bgs_status bgs_cloud_upload_4d(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh, const float* rotations,
+                               const float* scale_opacity, const float* timestamp_timescale, bgs_cloud** out);
+bgs_status bgs_cloud_download_4d(bgs_context* ctx, const bgs_cloud* cloud, float* pos_vis /* n*4 */, float* sh /* n*144 */,
+                                 float* rotations /* n*8 */, float* scale_opacity /* n*4 */,
+                                 float* timestamp_timescale /* n*4 */);
 
 /* Particle behaviours (src/morph/particle.rs, particle.wgsl; the reference's `morph_particles` feature): a
  * ParticleBehaviors asset moves the gaussians it names every frame, in place, without a re-upload.
@@ -450,6 +468,63 @@ bgs_status bgs_render_depth_test(bgs_context* ctx, const bgs_cloud* cloud, const
                                  const bgs_cloud_uniform* uniform, const bgs_settings* settings,
                                  const bgs_render_extras* extras, const bgs_scene_depth* depth, void* out_rgba,
                                  uint32_t out_format, int out_is_device_ptr);
+
+/* A Gaussian4d cloud (bgs_cloud_upload_4d) at time uniform->time: the reference's GaussianMode::Gaussian4d
+ * (gaussian.wgsl:191-311, gaussian_4d.wgsl:37-130, spherindrical_harmonics.wgsl:11-126).  Arguments as
+ * bgs_render_depth_test's (extras and depth may be NULL), plus the playback window time_start / time_stop
+ * (CloudSettings.time_start / time_stop).  settings->gaussian_mode must be BGS_GAUSSIAN_4D; rasterize_mode Color, Depth,
+ * Position, Classification, OpticalFlow or Velocity; every draw mode, format, output mode and flag of
+ * bgs_render_depth_test is accepted.  Key-gen and the depth sort are those of a 3D cloud of the same base positions (the
+ * key does not depend on time); binning, the blend and the depth test are unchanged; records have the 3D format.
+ *
+ * The rule, exactly (f32, round to nearest even, IEEE division and sqrt, no contraction, in the order written; matrices
+ * [col][row] as WGSL indexes them, mat4x4(a, b, c, d, ...) filling columns):
+ *   1. Drawn only if the base position p0 = model * (pos, 1) passes the frustum test (every depth width: difference 1
+ *      below) and not (DrawMode::Selected and vis < 0.5).
+ *   2. cutoff from the stored opacity (gaussian.wgsl:229-235), before the time modifier.
+ *   3. S = diag(gs*sx, gs*sy, gs*sz, timescale), gs = global_scale.  With (w, x, y, z) = rotation and (wr, xr, yr, zr) =
+ *      rotation_r as stored (lane 0 is w; not normalised): M_l = mat4x4(w,-x,-y,-z, x,w,-z,y, y,z,w,-x, z,-y,x,w),
+ *      M_r = mat4x4(wr,-xr,-yr,-zr, xr,wr,zr,-yr, yr,-zr,wr,xr, zr,yr,-xr,wr).  R = M_r * M_l: R[c][r] =
+ *      ((M_r[0][r] M_l[c][0] + M_r[1][r] M_l[c][1]) + M_r[2][r] M_l[c][2]) + M_r[3][r] M_l[c][3].  M = R * S:
+ *      M[c][r] = R[c][r] * S[c][c] (the zero products of the diagonal are not added).  Sigma = transpose(M) * M:
+ *      Sigma[c][r] = ((M[r][0] M[c][0] + M[r][1] M[c][1]) + M[r][2] M[c][2]) + M[r][3] M[c][3].
+ *   4. dt = time - timestamp; cov_t = Sigma[3][3]; marginal_t = exp(((-0.5 * dt) * dt) / cov_t), exp the fixed f64
+ *      series of csrc/project_math.cuh (det_exp: range reduction by ln 2, Taylor to degree 16, rounded to f32; 0 below
+ *      -110, +inf above 89).  Not drawn unless marginal_t > 0.05 (a NaN, e.g. from cov_t == 0 with dt == 0, is not).
+ *   5. c12 = (Sigma[0][3], Sigma[1][3], Sigma[2][3]); cov3d[c][r] = Sigma[c][r] - (c12[c] * c12[r]) / cov_t, passed to
+ *      cov2d as (cov3d[0][0], [0][1], [0][2], [1][1], [1][2], [2][2]); delta_mean[i] = (c12[i] / cov_t) * dt.
+ *   6. p = model * (pos + delta_mean, 1); not drawn unless p passes the frustum test; opacity = stored opacity *
+ *      marginal_t.  The record is that of bgs_render's projection at p with cov3d (OBB or AABB; the model 3x3 does not
+ *      touch cov3d, global_scale enters through S only), opacity * global_opacity, centre from p.
+ *   7. Colour: Color = spherindrical_harmonics_lookup(dir, dt, sh): the SH-3 colour of bgs_render along the camera ray
+ *      to p in the model frame, + cos(2 pi theta) * (sum_k basis_k sh[48 + 3k + c]) + cos(4 pi theta) * (sum_k basis_k
+ *      sh[96 + 3k + c]), theta = dt / (time_stop - time_start), 2 pi and 4 pi the f32 multiples of radians(180.0), cos the
+ *      fixed f64 series det_cos (reduction by 2 pi, Taylor to degree 36, rounded to f32); then the sRGB decode when
+ *      color_space == 0.  Classification = that colour, then bgs_render_ex's class hue.  Depth = bgs_render's depth
+ *      colour of |p - cam| between the distances of sorted entries 1 and count - 1, which hold base positions.
+ *      Position = from p.  OpticalFlow = bgs_render_ex's rule with the current clip of p and the previous clip of the
+ *      unmoved p0 (gaussian.wgsl:201).  Velocity (gaussian.wgsl:378-405): f = the conditioning at time + 1e-3 (its
+ *      delta_mean 0 when its mask fails); v = (f.delta_mean - delta_mean) / 1e-3 in the local frame;
+ *      scaled = clamp((|v| - 1) / (2 - 1), 0, 1), |v| = sqrt((vx*vx + vy*vy) + vz*vz); scaled < 1e-2: opacity 0 and rgb
+ *      0 (difference 2); else rgb = (0.5 * (v / |v| + 1)) * scaled.
+ *   8. DrawMode::HighlightSelected overrides colour and opacity of vis > 0.5 splats, as in bgs_render.
+ *   9. The depth-test depth d is bgs_render_depth_test's of p.
+ *   An undrawn record keeps the base position's centre and the stored opacity, with an empty bbox and no colour.
+ *   FP policy: geometry, bbox, the draw decision, opacity, Velocity, OpticalFlow, Depth and Position colours are
+ *   bit-exact against the oracle (temporal_oracle/); the SH-based colours are compared under a bound (FMA sums,
+ *   approximate rsqrt and pow).
+ * Where this port deliberately differs from the reference (BGS_EINVAL items: nothing enqueued or written):
+ *   1. The reference drops base-culled gaussians by their key only at 32 depth bits; at 16 and 24 bits it skips the base
+ *      frustum test for 4D and draws a base-culled gaussian whose moved position is in view, sorted as the farthest.
+ *      Here every depth width culls on the base position, as the reference does at 32 bits.
+ *   2. When Velocity sets opacity to 0, rgb is 0 too; the reference blends normalize(0) * 0 = NaN whenever v == 0.
+ *   3. time_start == time_stop, time_stop - time_start not finite, or any of time, time_start, time_stop not finite
+ *      -> BGS_EINVAL (the reference divides by zero).
+ *   4. RasterizeMode::Normal (the reference calls get_rotation, which its 4D layout does not define), a cloud that is not
+ *      4D, gaussian_mode != BGS_GAUSSIAN_4D -> BGS_EINVAL; bgs_render_aux and bgs_cloud_interpolate take no 4D cloud. */
+bgs_status bgs_render_4d(bgs_context* ctx, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uniform,
+                         const bgs_settings* settings, const bgs_render_extras* extras, const bgs_scene_depth* depth,
+                         void* out_rgba, uint32_t out_format, int out_is_device_ptr, float time_start, float time_stop);
 
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a

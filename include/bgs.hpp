@@ -24,8 +24,10 @@
 namespace bgs {
 
 enum class DrawMode : uint32_t { All = 0, Selected = 1, HighlightSelected = 2 };
-enum class GaussianMode : uint32_t { Gaussian2d = 0, Gaussian3d = 1 };
-enum class RasterizeMode : uint32_t { Color = 0, Depth = 1, Normal = 2, Position = 3, Classification = 4, OpticalFlow = 5 };
+enum class GaussianMode : uint32_t { Gaussian2d = 0, Gaussian3d = 1, Gaussian4d = 2 };
+enum class RasterizeMode : uint32_t {
+    Color = 0, Depth = 1, Normal = 2, Position = 3, Classification = 4, OpticalFlow = 5, Velocity = 6 /* Gaussian4d only */
+};
 enum class RadixSortDepthBits : uint32_t { Bits16 = 16, Bits24 = 24, Bits32 = 32 };
 enum class GaussianColorSpace : uint32_t { SrgbRec709Display = 0, LinRec709Display = 1 };
 
@@ -41,7 +43,7 @@ struct CloudSettings {   // src/gaussian/settings.rs:110-133 (defaults)
     GaussianColorSpace color_space = GaussianColorSpace::SrgbRec709Display;
     uint32_t num_classes = 1;   // RasterizeMode::Classification's hue count (CloudUniform.num_classes)
     float time = 0.0f;
-    float time_start = 0.0f;   // the interpolation window (GaussianSplattingPlugin::interpolate)
+    float time_start = 0.0f;   // the interpolation window (GaussianSplattingPlugin::interpolate), a 4D cloud's playback window
     float time_stop = 1.0f;
     // this repo's extension: front-to-back binning rounds (BGS_FLAG_CHUNKS): -1 = the library's choice from the last
     // frame's footprint statistics, 1 = always, 0 = never (the tile debug hooks need a one-round frame)
@@ -69,6 +71,15 @@ struct ShaderDefines {   // src/render/mod.rs:698-760: the radix pass plan
         return {8u, bits / 8u, 32u - bits, 256u};
     }
     uint32_t radix_initial_parity() const { return radix_digit_places % 2u; }
+};
+
+struct PlanarGaussian4d {   // five planes, binding order (planar_4d.rs:38-51); bgs_cloud_upload_4d's
+    std::vector<float> position_visibility;     // n*4
+    std::vector<float> spherindrical_harmonic;  // n*144: SH-3 colour, cos(2 pi t) set, cos(4 pi t) set
+    std::vector<float> isotropic_rotations;     // n*8: rotation (w, x, y, z), rotation_r (w, x, y, z)
+    std::vector<float> scale_opacity;           // n*4
+    std::vector<float> timestamp_timescale;     // n*4: timestamp, timescale, pad, pad
+    size_t len() const { return position_visibility.size() / 4; }
 };
 
 struct PlanarGaussian3d {   // four planes, binding order (planar_3d.rs:45-54)
@@ -207,6 +218,10 @@ private:
     float aabb_min_[3] = {0, 0, 0}, aabb_max_[3] = {1, 1, 1};
 };
 
+// a Gaussian4d cloud resident in HBM (bgs_cloud_upload_4d): rendered by render_view_4d.  The calls on a cloud's
+// positions and visibility take it through get() as they take a 3D one
+class PlanarGaussian4dHandle : public PlanarGaussian3dHandle {};
+
 class ParticleBehaviorsHandle {   // a ParticleBehaviors asset resident in HBM (bgs_particles)
 public:
     ParticleBehaviorsHandle() = default;
@@ -238,6 +253,22 @@ public:
         c.compute_aabb(h.aabb_min_, h.aabb_max_);
         check(bgs_cloud_upload_f32(ctx_, h.n_, c.position_visibility.data(), c.spherical_harmonic.data(), c.rotation.data(),
                                    c.scale_opacity.data(), &h.h_));
+        return h;
+    }
+    PlanarGaussian4dHandle add_cloud(const PlanarGaussian4d& c) {
+        PlanarGaussian4dHandle h;
+        h.n_ = (uint32_t)c.len();
+        for (int k = 0; k < 3; ++k) {   // the Aabb as PlanarGaussian3d::compute_aabb makes it, from the positions
+            float lo = INFINITY, hi = -INFINITY;
+            for (size_t i = 0; i < c.len(); ++i) {
+                lo = std::fmin(lo, c.position_visibility[4 * i + k]); hi = std::fmax(hi, c.position_visibility[4 * i + k]);
+            }
+            lo -= 0.1f; hi += 0.1f;
+            const float center = (lo + hi) / 2.0f, half = (hi - lo) / 2.0f;
+            h.aabb_min_[k] = center - half; h.aabb_max_[k] = center + half;
+        }
+        check(bgs_cloud_upload_4d(ctx_, h.n_, c.position_visibility.data(), c.spherindrical_harmonic.data(),
+                                  c.isotropic_rotations.data(), c.scale_opacity.data(), c.timestamp_timescale.data(), &h.h_));
         return h;
     }
     static bgs_cloud_uniform cloud_uniform(const CloudSettings& s, const Mat4& transform = Mat4::identity()) {
@@ -282,6 +313,31 @@ public:
         ex.delta_time = delta_time;
         ex.num_classes = settings.num_classes;
         const bgs_status st = bgs_render_ex(ctx_, cloud.get(), &view, &u, &s, &ex, out_rgba, format, out_is_device ? 1 : 0);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
+    // A Gaussian4d cloud at settings.time in [settings.time_start, settings.time_stop] (bgs_render_4d; settings.gaussian_mode
+    // must be Gaussian4d).  `previous_view` / `delta_time`: OpticalFlow's (nullptr otherwise); `depth` / `pitch_bytes`: the
+    // scene's depth buffer as render_view_depth_test takes it (nullptr: no depth test).
+    bool render_view_4d(const PlanarGaussian4dHandle& cloud, const CloudSettings& settings, const bgs_view& view, void* out_rgba,
+                        uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr, float delta_time = 0.0f,
+                        const float* depth = nullptr, uint64_t pitch_bytes = 0, bool out_is_device = false,
+                        uint32_t extra_flags = 0) {
+        bgs_cloud_uniform u = cloud_uniform(settings);
+        std::memcpy(u.aabb_min, cloud.aabb_min(), 12); std::memcpy(u.aabb_max, cloud.aabb_max(), 12);
+        const bgs_settings s = settings.to_abi(extra_flags);
+        bgs_render_extras ex{};
+        ex.num_classes = settings.num_classes;
+        if (previous_view) {
+            std::memcpy(ex.previous_clip_from_world, previous_view->clip_from_world, 64);
+            ex.delta_time = delta_time;
+        }
+        bgs_scene_depth zd{depth, pitch_bytes};
+        const bgs_status st = bgs_render_4d(ctx_, cloud.get(), &view, &u, &s,
+                                            settings.rasterize_mode == RasterizeMode::OpticalFlow && !previous_view ? nullptr : &ex,
+                                            depth ? &zd : nullptr, out_rgba, format, out_is_device ? 1 : 0, settings.time_start,
+                                            settings.time_stop);
         if (st == BGS_NOT_READY) return false;
         check(st);
         return true;
