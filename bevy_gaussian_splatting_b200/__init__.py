@@ -7,7 +7,7 @@ The Python modules here are the host-side mirror of the reference interface for 
 from .abi import BgsError  # noqa: F401
 from .camera import GaussianCamera, View, headless_view, orbit_view, perspective_view  # noqa: F401
 from .gaussian import (PlanarGaussian3d, PlanarGaussian4d, random_gaussians_3d, random_gaussians_3d_seeded,  # noqa: F401
-                       random_gaussians_4d_seeded, SH_COEFF_COUNT, SH_4D_COEFF_COUNT)
+                       random_gaussians_4d_seeded, SH_COEFF_COUNT, SH_4D_COEFF_COUNT, SH_WIDTHS)
 from .io import load_cloud, parse_ply_3d, parse_ply_4d, write_ply_4d  # noqa: F401
 from .gcloud import decode_gcloud, encode_gcloud, read_gcloud, write_gcloud  # noqa: F401
 from .particles import (PARTICLE_BEHAVIOR_DTYPE, PARTICLE_INACTIVE, ParticleBehaviors,  # noqa: F401

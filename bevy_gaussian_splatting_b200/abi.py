@@ -108,6 +108,12 @@ SYMBOLS = [
     ("bgs_cloud_upload_f32", C.c_int, [_P, C.c_uint32, _P, _P, _P, _P, C.POINTER(_P)]),
     ("bgs_cloud_upload_f16", C.c_int, [_P, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
     ("bgs_cloud_upload_f16_cov", C.c_int, [_P, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
+    ("bgs_cloud_upload_f32_sh", C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P, _P, C.POINTER(_P)]),
+    ("bgs_cloud_upload_f16_sh", C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
+    ("bgs_cloud_upload_f16_cov_sh", C.c_int, [_P, C.c_uint32, C.c_uint32, _P, _P, _P, C.POINTER(_P)]),
+    ("bgs_cloud_download_f32_sh", C.c_int, [_P, _P, _P, _P, _P, _P]),
+    ("bgs_cloud_download_f16_sh", C.c_int, [_P, _P, _P, _P, _P]),
+    ("bgs_cloud_sh_degree", C.c_int, [_P, C.POINTER(C.c_uint32)]),
     ("bgs_cloud_destroy", None, [_P]),
     ("bgs_cloud_select_sparse", C.c_int, [_P, _P, C.c_float, C.c_uint32, C.POINTER(C.c_uint32)]),
     ("bgs_cloud_visibility_get", C.c_int, [_P, _P, _P]),

@@ -497,8 +497,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
         launch_project_4d(cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
                           modes ? *modes : ModeConsts{}, *tc, c->recs.p, zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
     } else {
-        launch_project(cloud->layout, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
-                       c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
+        launch_project(cloud->layout, cloud->sh_degree, cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p,
+                       p.by_slot ? 1 : 0, c->ctr, fc, c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
                        fc.aux ? c->aux.p : nullptr, modes, ps);
     }
     ++launches;

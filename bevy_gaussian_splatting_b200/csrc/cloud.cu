@@ -17,13 +17,14 @@ bgs_status drop_cloud(bgs_context* c, const char* call, bgs_cloud* cl, cudaError
     return fail(c, status_of(e), "%s: %s", call, cudaGetErrorString(e));
 }
 
-// A new cloud of n gaussians in the given layout on the context's device, its planes allocated but not yet written.
-bgs_status new_cloud(bgs_context* c, const char* call, uint32_t n, CloudLayout layout, bgs_cloud** out) {
+// A new cloud of n gaussians in the given layout and SH degree on the context's device, its planes allocated but not
+// yet written.
+bgs_status new_cloud(bgs_context* c, const char* call, uint32_t n, CloudLayout layout, uint32_t sh_degree, bgs_cloud** out) {
     bgs_cloud* cl = new (std::nothrow) bgs_cloud();
     if (!cl) return fail(c, BGS_ENOMEM, "%s: out of host memory", call);
-    cl->device = c->device; cl->n = n; cl->layout = layout;
-    cudaError_t e = cudaMalloc(&cl->pos, (size_t)n * plane_bytes(layout, PLANE_POS));
-    if (e == cudaSuccess) e = cudaMalloc(&cl->blocks, (size_t)n * block_bytes(layout));
+    cl->device = c->device; cl->n = n; cl->layout = layout; cl->sh_degree = sh_degree;
+    cudaError_t e = cudaMalloc(&cl->pos, (size_t)n * plane_bytes(layout, sh_degree, PLANE_POS));
+    if (e == cudaSuccess) e = cudaMalloc(&cl->blocks, (size_t)n * block_bytes(layout, sh_degree));
     if (e != cudaSuccess) return drop_cloud(c, call, cl, e);
     *out = cl;
     return BGS_OK;
@@ -52,39 +53,50 @@ struct StreamScratch {
 // pinned bounce buffers one chunk's planes (f32: 30 MB).  4D gaussians are wider: their chunks hold as many gaussians
 // as fit the same bounce buffers
 constexpr uint32_t DOWNLOAD_CHUNK = 1u << 17;
-constexpr size_t DOWNLOAD_BOUNCE_BYTES = (size_t)DOWNLOAD_CHUNK * planar_bytes(CloudLayout::F32);
-static_assert(planar_bytes(CloudLayout::F32) >= planar_bytes(CloudLayout::F16), "the f32 chunk is the largest 3D one");
+constexpr size_t DOWNLOAD_BOUNCE_BYTES = (size_t)DOWNLOAD_CHUNK * planar_bytes(CloudLayout::F32, SH_DEGREE_MAX);
+static_assert(planar_bytes(CloudLayout::F32, SH_DEGREE_MAX) >= planar_bytes(CloudLayout::F16, SH_DEGREE_MAX),
+              "the f32 chunk is the largest 3D one");
 
 // the family of download call a layout answers to (0: _f32, 1: _f16, both f16 layouts; 2: _4d)
 int download_family(CloudLayout l) { return is_4d(l) ? 2 : is_f16(l) ? 1 : 0; }
+
+// n rows of `width` bytes between arrays of pitch src_pitch and dst_pitch (one contiguous copy when both are `width`)
+cudaError_t copy_rows(void* dst, size_t dst_pitch, const void* src, size_t src_pitch, size_t width, size_t n,
+                      cudaMemcpyKind kind, cudaStream_t q) {
+    if (dst_pitch == width && src_pitch == width) return cudaMemcpyAsync(dst, src, n * width, kind, q);
+    return cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, width, n, kind, q);
+}
 
 }  // namespace
 
 extern "C" {
 
-static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout, const float* pos_vis, const void* sh,
-                                const void* rot, const void* so, const void* tt, bgs_cloud** out) {
+static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout, uint32_t sh_degree, const float* pos_vis,
+                                const void* sh, const void* rot, const void* so, const void* tt, bgs_cloud** out) {
     if (!ctx || !out) return BGS_EINVAL;
     *out = nullptr;
+    if (sh_degree > SH_DEGREE_MAX) return fail(ctx, BGS_EINVAL, "cloud upload: sh_degree %u is not in [0, 3]", sh_degree);
     const void* src[PLANES] = {pos_vis, sh, rot, so, tt};
     for (int p = 0; p < PLANES; ++p)
-        if (plane_bytes(layout, p) && !src[p]) return fail(ctx, BGS_EINVAL, "cloud upload: null plane pointer");
+        if (plane_bytes(layout, sh_degree, p) && !src[p]) return fail(ctx, BGS_EINVAL, "cloud upload: null plane pointer");
     if (n == 0 || n >= (1u << 30)) return fail(ctx, BGS_EINVAL, "cloud upload: n must be in [1, 2^30)");
     CU(ctx, cudaSetDevice(ctx->device));
     bgs_cloud* cl = nullptr;
-    TRY(new_cloud(ctx, "cloud upload", n, layout, &cl));
-    // the position plane is the cloud's own; the other planes go to device scratch, are repacked into the
-    // gaussian-major blocks the projection gathers, and are freed again
+    TRY(new_cloud(ctx, "cloud upload", n, layout, sh_degree, &cl));
+    // the position plane is the cloud's own; the other planes go to device scratch (the SH plane at whole chunks per
+    // gaussian, the rest of each last chunk zero), are repacked into the gaussian-major blocks the projection gathers,
+    // and are freed again
     void* d[PLANES] = {cl->pos, nullptr, nullptr, nullptr, nullptr};
     cudaError_t e = cudaSuccess;
     for (int p = 0; p < PLANES && e == cudaSuccess; ++p) {
-        const size_t bytes = (size_t)n * plane_bytes(layout, p);
-        if (bytes == 0) continue;
-        if (p != PLANE_POS) e = cudaMalloc(&d[p], bytes);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d[p], src[p], bytes, cudaMemcpyHostToDevice, ctx->stream);
+        const size_t width = plane_bytes(layout, sh_degree, p), staged = staged_bytes(layout, sh_degree, p);
+        if (width == 0) continue;
+        if (p != PLANE_POS) e = cudaMalloc(&d[p], (size_t)n * staged);
+        if (e == cudaSuccess && staged != width) e = cudaMemsetAsync(d[p], 0, (size_t)n * staged, ctx->stream);
+        if (e == cudaSuccess) e = copy_rows(d[p], staged, src[p], width, width, n, cudaMemcpyHostToDevice, ctx->stream);
     }
     if (e == cudaSuccess) {
-        launch_repack(layout, d[PLANE_SH], d[PLANE_ROT], d[PLANE_SO], d[PLANE_TT], n, cl->view(), ctx->stream);
+        launch_repack(layout, sh_degree, d[PLANE_SH], d[PLANE_ROT], d[PLANE_SO], d[PLANE_TT], n, cl->view(), ctx->stream);
         e = cudaStreamSynchronize(ctx->stream);
     }
     for (int p = PLANE_SH; p < PLANES; ++p) cudaFree(d[p]);
@@ -95,22 +107,44 @@ static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout
 
 bgs_status bgs_cloud_upload_f32(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh,
                                 const float* rot_wxyz, const float* scale_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, CloudLayout::F32, pos_vis, sh, rot_wxyz, scale_opacity, nullptr, out);
+    return upload_common(ctx, n, CloudLayout::F32, SH_DEGREE_MAX, pos_vis, sh, rot_wxyz, scale_opacity, nullptr, out);
+}
+
+bgs_status bgs_cloud_upload_f32_sh(bgs_context* ctx, uint32_t n, uint32_t sh_degree, const float* pos_vis, const float* sh,
+                                   const float* rot_wxyz, const float* scale_opacity, bgs_cloud** out) {
+    return upload_common(ctx, n, CloudLayout::F32, sh_degree, pos_vis, sh, rot_wxyz, scale_opacity, nullptr, out);
 }
 
 bgs_status bgs_cloud_upload_f16(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
                                 const uint32_t* rot_scale_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, CloudLayout::F16, pos_vis, sh_packed, rot_scale_opacity, nullptr, nullptr, out);
+    return upload_common(ctx, n, CloudLayout::F16, SH_DEGREE_MAX, pos_vis, sh_packed, rot_scale_opacity, nullptr, nullptr, out);
+}
+
+bgs_status bgs_cloud_upload_f16_sh(bgs_context* ctx, uint32_t n, uint32_t sh_degree, const float* pos_vis,
+                                   const uint32_t* sh_packed, const uint32_t* rot_scale_opacity, bgs_cloud** out) {
+    return upload_common(ctx, n, CloudLayout::F16, sh_degree, pos_vis, sh_packed, rot_scale_opacity, nullptr, nullptr, out);
 }
 
 bgs_status bgs_cloud_upload_f16_cov(bgs_context* ctx, uint32_t n, const float* pos_vis, const uint32_t* sh_packed,
                                     const uint32_t* cov3d_opacity, bgs_cloud** out) {
-    return upload_common(ctx, n, CloudLayout::F16Cov, pos_vis, sh_packed, cov3d_opacity, nullptr, nullptr, out);
+    return upload_common(ctx, n, CloudLayout::F16Cov, SH_DEGREE_MAX, pos_vis, sh_packed, cov3d_opacity, nullptr, nullptr, out);
+}
+
+bgs_status bgs_cloud_upload_f16_cov_sh(bgs_context* ctx, uint32_t n, uint32_t sh_degree, const float* pos_vis,
+                                       const uint32_t* sh_packed, const uint32_t* cov3d_opacity, bgs_cloud** out) {
+    return upload_common(ctx, n, CloudLayout::F16Cov, sh_degree, pos_vis, sh_packed, cov3d_opacity, nullptr, nullptr, out);
 }
 
 bgs_status bgs_cloud_upload_4d(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh, const float* rotations,
                                const float* scale_opacity, const float* timestamp_timescale, bgs_cloud** out) {
-    return upload_common(ctx, n, CloudLayout::F32x4D, pos_vis, sh, rotations, scale_opacity, timestamp_timescale, out);
+    return upload_common(ctx, n, CloudLayout::F32x4D, SH_DEGREE_MAX, pos_vis, sh, rotations, scale_opacity, timestamp_timescale,
+                         out);
+}
+
+bgs_status bgs_cloud_sh_degree(const bgs_cloud* cl, uint32_t* out) {
+    if (!cl || !out) return BGS_EINVAL;
+    *out = cl->sh_degree;
+    return BGS_OK;
 }
 
 void bgs_cloud_destroy(bgs_cloud* cl) {
@@ -202,7 +236,8 @@ bgs_status bgs_cloud_visibility_set(bgs_context* c, bgs_cloud* cl, const float* 
     TRY(before_cloud_write(c, cl));
     const CloudView v = cl->view();
     CU(c, cudaMemcpy2DAsync(&v.pos->w, sizeof(float4), vis, 4, 4, cl->n, cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemcpy2DAsync(&reinterpret_cast<float4*>(v.blocks)[POS_CHUNK].w, block_bytes(cl->layout), vis, 4, 4, cl->n,
+    CU(c, cudaMemcpy2DAsync(&reinterpret_cast<float4*>(v.blocks)[POS_CHUNK].w, block_bytes(cl->layout, cl->sh_degree), vis, 4, 4,
+                            cl->n,
                             cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return BGS_OK;
@@ -395,13 +430,16 @@ bgs_status bgs_cloud_interpolate(bgs_context* c, bgs_cloud* out, const bgs_cloud
         return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out hold %u, %u and %u gaussians", lhs->n, rhs->n, out->n);
     if (lhs->layout != out->layout || rhs->layout != out->layout)
         return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out are not in one layout");
+    if (lhs->sh_degree != out->sh_degree || rhs->sh_degree != out->sh_degree)
+        return fail(c, BGS_EINVAL, "interpolate: lhs, rhs and out have SH degrees %u, %u and %u", lhs->sh_degree, rhs->sh_degree,
+                    out->sh_degree);
     if (is_4d(out->layout)) return fail(c, BGS_EINVAL, "interpolate: Gaussian4d clouds are not interpolated");
     if (out == lhs || out == rhs) return fail(c, BGS_EINVAL, "interpolate: out is lhs or rhs");
     float t = 0.0f;
     if (!interpolation_factor(time, time_start, time_stop, &t))
         return fail(c, BGS_EINVAL, "interpolate: time %g, time_start %g, time_stop %g give no factor", time, time_start, time_stop);
     return queue_cloud_write_reading(c, out, lhs, rhs, [&](cudaStream_t q) {
-        launch_interpolate(out->layout, lhs->view(), rhs->view(), out->n, t, out->view(), q);
+        launch_interpolate(out->layout, out->sh_degree, lhs->view(), rhs->view(), out->n, t, out->view(), q);
         CU(c, cudaGetLastError());
         return BGS_OK;
     });
@@ -445,13 +483,13 @@ bgs_status bgs_cloud_subset(bgs_context* c, const bgs_cloud* cl, const uint32_t*
         CU(c, cudaMemcpyAsync(scratch.p, indices, (size_t)k * 4, cudaMemcpyHostToDevice, q));
     }
     bgs_cloud* nc = nullptr;
-    TRY(new_cloud(c, "subset", kept, cl->layout, &nc));
+    TRY(new_cloud(c, "subset", kept, cl->layout, cl->sh_degree, &nc));
     if (!indices) {
         const uint8_t* s = static_cast<const uint8_t*>(scratch.p);
-        launch_subset_scatter(cl->layout, cl->view(), n, reinterpret_cast<const uint32_t*>(s + o_mask),
+        launch_subset_scatter(cl->layout, cl->sh_degree, cl->view(), n, reinterpret_cast<const uint32_t*>(s + o_mask),
                               reinterpret_cast<const uint32_t*>(s + o_cnt), nc->view(), q);
     } else {
-        launch_subset_gather(cl->layout, cl->view(), static_cast<const uint32_t*>(scratch.p), k, nc->view(), q);
+        launch_subset_gather(cl->layout, cl->sh_degree, cl->view(), static_cast<const uint32_t*>(scratch.p), k, nc->view(), q);
     }
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(q);
@@ -463,24 +501,30 @@ bgs_status bgs_cloud_subset(bgs_context* c, const bgs_cloud* cl, const uint32_t*
 
 // Per chunk: unpack into device staging, copy the chunk's position plane and the staged planes to a pinned bounce
 // buffer, and -- while the next chunk goes the same way into the other bounce buffer -- copy it into the caller's arrays.
-static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, int family, float* pos_vis, void* sh, void* rot, void* so,
-                                  void* tt) {
+// any_degree: a call of the _sh family, which takes the SH plane at the cloud's degree; the others take degree 3 only.
+static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, int family, bool any_degree, float* pos_vis, void* sh,
+                                  void* rot, void* so, void* tt) {
     if (!cl || !pos_vis || !sh || !rot || (family != 1 && !so) || (family == 2 && !tt))
         return fail(c, BGS_EINVAL, "download: null cloud or plane pointer");
     TRY(enter_call(c, "download", cl->device));
     const CloudLayout l = cl->layout;
+    const uint32_t d = cl->sh_degree;
     static const char* const kFamily[3] = {"f32", "f16", "4D"};
     if (download_family(l) != family) return fail(c, BGS_EINVAL, "download: the cloud is in the %s layout", kFamily[download_family(l)]);
+    if (!any_degree && d != SH_DEGREE_MAX)
+        return fail(c, BGS_EINVAL, "download: the cloud has SH degree %u (bgs_cloud_download_%s_sh reads it)", d, kFamily[family]);
     TRY(before_cloud_read(c, cl));
     cudaStream_t q = c->stream;
-    const uint32_t n = cl->n, m_max = std::min<uint32_t>(n, (uint32_t)(DOWNLOAD_BOUNCE_BYTES / planar_bytes(l)));
+    const uint32_t n = cl->n, m_max = std::min<uint32_t>(n, (uint32_t)(DOWNLOAD_BOUNCE_BYTES / planar_bytes(l, d)));
     // (sized once for the largest chunk of either layout: it never grows)
     if (!c->h_bounce) CU(c, cudaMallocHost(&c->h_bounce, 2 * DOWNLOAD_BOUNCE_BYTES));
     const size_t chunk_b = DOWNLOAD_BOUNCE_BYTES;
-    StreamScratch staging(q);   // sh | rot | so | tt of one chunk
-    CU(c, staging.alloc((size_t)m_max * (planar_bytes(l) - plane_bytes(l, PLANE_POS))));
+    StreamScratch staging(q);   // sh | rot | so | tt of one chunk, the SH plane at whole chunks per gaussian
+    size_t staged_total = 0;
+    for (int p = PLANE_SH; p < PLANES; ++p) staged_total += staged_bytes(l, d, p);
+    CU(c, staging.alloc((size_t)m_max * staged_total));
     uint8_t* st[PLANES] = {nullptr, static_cast<uint8_t*>(staging.p)};
-    for (int p = PLANE_SH + 1; p < PLANES; ++p) st[p] = st[p - 1] + (size_t)m_max * plane_bytes(l, p - 1);
+    for (int p = PLANE_SH + 1; p < PLANES; ++p) st[p] = st[p - 1] + (size_t)m_max * staged_bytes(l, d, p - 1);
     cudaEvent_t ev[2] = {nullptr, nullptr};
     struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 2; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
     for (cudaEvent_t& e : ev) CU(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -491,14 +535,15 @@ static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, int famil
     auto enqueue = [&](uint32_t i) -> bgs_status {
         const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
         uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
-        launch_unpack(l, cl->view(), lo, m, st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO], st[PLANE_TT], q);
+        launch_unpack(l, d, cl->view(), lo, m, st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO], st[PLANE_TT], q);
         CU(c, cudaGetLastError());
         const uint8_t* src[PLANES] = {reinterpret_cast<const uint8_t*>(cl->pos + lo), st[PLANE_SH], st[PLANE_ROT], st[PLANE_SO],
                                       st[PLANE_TT]};
         for (int p = 0; p < PLANES; ++p) {
-            const size_t bytes = (size_t)m * plane_bytes(l, p);
-            if (bytes) CU(c, cudaMemcpyAsync(hb, src[p], bytes, cudaMemcpyDeviceToHost, q));
-            hb += bytes;
+            const size_t width = plane_bytes(l, d, p);
+            if (width) CU(c, copy_rows(hb, width, src[p], p == PLANE_POS ? width : staged_bytes(l, d, p), width, m,
+                                       cudaMemcpyDeviceToHost, q));
+            hb += (size_t)m * width;
         }
         CU(c, cudaEventRecord(ev[i & 1], q));
         return BGS_OK;
@@ -510,7 +555,7 @@ static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, int famil
         const uint32_t lo = i * m_max, m = std::min(m_max, n - lo);
         const uint8_t* hb = c->h_bounce + (i & 1) * chunk_b;
         for (int p = 0; p < PLANES; ++p) {
-            const size_t b = plane_bytes(l, p);
+            const size_t b = plane_bytes(l, d, p);
             if (b) memcpy(dst[p] + (size_t)lo * b, hb, (size_t)m * b);
             hb += (size_t)m * b;
         }
@@ -519,16 +564,26 @@ static bgs_status download_common(bgs_context* c, const bgs_cloud* cl, int famil
 }
 
 bgs_status bgs_cloud_download_f32(bgs_context* c, const bgs_cloud* cl, float* pos_vis, float* sh, float* rot_wxyz, float* scale_opacity) {
-    return download_common(c, cl, 0, pos_vis, sh, rot_wxyz, scale_opacity, nullptr);
+    return download_common(c, cl, 0, false, pos_vis, sh, rot_wxyz, scale_opacity, nullptr);
 }
 
 bgs_status bgs_cloud_download_f16(bgs_context* c, const bgs_cloud* cl, float* pos_vis, uint32_t* sh_packed, uint32_t* second_plane) {
-    return download_common(c, cl, 1, pos_vis, sh_packed, second_plane, nullptr, nullptr);
+    return download_common(c, cl, 1, false, pos_vis, sh_packed, second_plane, nullptr, nullptr);
+}
+
+bgs_status bgs_cloud_download_f32_sh(bgs_context* c, const bgs_cloud* cl, float* pos_vis, float* sh, float* rot_wxyz,
+                                     float* scale_opacity) {
+    return download_common(c, cl, 0, true, pos_vis, sh, rot_wxyz, scale_opacity, nullptr);
+}
+
+bgs_status bgs_cloud_download_f16_sh(bgs_context* c, const bgs_cloud* cl, float* pos_vis, uint32_t* sh_packed,
+                                     uint32_t* second_plane) {
+    return download_common(c, cl, 1, true, pos_vis, sh_packed, second_plane, nullptr, nullptr);
 }
 
 bgs_status bgs_cloud_download_4d(bgs_context* c, const bgs_cloud* cl, float* pos_vis, float* sh, float* rotations,
                                  float* scale_opacity, float* timestamp_timescale) {
-    return download_common(c, cl, 2, pos_vis, sh, rotations, scale_opacity, timestamp_timescale);
+    return download_common(c, cl, 2, false, pos_vis, sh, rotations, scale_opacity, timestamp_timescale);
 }
 
 }  // extern "C"

@@ -41,6 +41,7 @@ struct bgs_cloud {
     int device;       // the CUDA device the planes live on
     uint32_t n;
     CloudLayout layout;
+    uint32_t sh_degree;         // 0..3 (include/bgs.h); 3 for every cloud of the calls without _sh, 4D clouds included
     float4* pos = nullptr;      // the position plane and the gaussian-major blocks (cloud_layout.cuh)
     void* blocks = nullptr;
     // enqueued writes (particle steps): ev_write marks the last one, on whichever context's stream it was queued; every
@@ -48,7 +49,7 @@ struct bgs_cloud {
     // so a cloud that is never stepped costs its frames nothing
     cudaEvent_t ev_write = nullptr;
     std::atomic<bool> stepped{false};
-    CloudView view() const { return {pos, static_cast<uint4*>(blocks), chunks(layout)}; }
+    CloudView view() const { return {pos, static_cast<uint4*>(blocks), chunks(layout, sh_degree)}; }
 };
 
 // A ParticleBehaviors asset resident on one GPU: count 64 B records (bgs_particle_behavior), read and written by the step

@@ -4,7 +4,8 @@
 //
 // One thread per 16 B chunk of the output block (cloud_layout.cuh).  Each chunk is blended from the same chunk of the
 // two input blocks and is self-contained: no lane reads another chunk.  The position chunk's thread also stores the
-// position plane; the f32 pad chunk is not written.
+// position plane; the pad chunks are not written.  Every SH chunk is blended whole: at SH degrees below 3 that includes
+// the padding lanes and, in f16, the zero words that fill the last chunk (mix(0, 0, t) = 0).
 //
 // Arithmetic: mix(a, b, t) = a*(1-t) + b*t (WGSL's definition, 1-t rounded once), the normalisation
 // q / sqrt(((q0*q0 + q1*q1) + q2*q2) + q3*q3) in storage lane order (w, x, y, z) with (0, 0, 0, 1) when that sum is
@@ -59,14 +60,14 @@ __device__ __forceinline__ uint4 mix_covariance(uint4 a, uint4 b, float t, float
                       pack_halves(mix_lane(half_hi(a.w), half_hi(b.w), t, omt), 0.0f));
 }
 
-template <CloudLayout L>
+template <CloudLayout L, uint32_t D>
 __global__ void __launch_bounds__(INTERP_THREADS) interpolate_kernel(const uint4* __restrict__ lhs, const uint4* __restrict__ rhs,
                                                                      size_t n_chunks, float t, CloudView out) {
-    constexpr uint32_t CH = chunks(L);
+    constexpr uint32_t CH = chunks(L, D);
     const size_t i = (size_t)blockIdx.x * INTERP_THREADS + threadIdx.x;
     if (i >= n_chunks) return;
     const uint32_t c = (uint32_t)(i % CH);
-    if (is_pad(L, c)) return;
+    if (is_pad(L, D, c)) return;
     const float omt = __fsub_rn(1.0f, t);
     const uint4 a = __ldg(lhs + i), b = __ldg(rhs + i);
     uint4 r;
@@ -86,12 +87,13 @@ __global__ void __launch_bounds__(INTERP_THREADS) interpolate_kernel(const uint4
     out.store_chunk(i / CH, c, r);
 }
 
-void launch_interpolate(CloudLayout layout, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream) {
+void launch_interpolate(CloudLayout layout, uint32_t sh_degree, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out,
+                        cudaStream_t stream) {
     const size_t n_chunks = (size_t)n * out.chunks;
     const uint32_t grid = (uint32_t)((n_chunks + INTERP_THREADS - 1) / INTERP_THREADS);
-    with_layout(layout, [&](auto L) {   // (bgs_cloud_interpolate refuses 4D clouds)
+    with_layout_degree(layout, sh_degree, [&](auto L, auto D) {   // (bgs_cloud_interpolate refuses 4D clouds)
         if constexpr (!is_4d(decltype(L)::value))
-            interpolate_kernel<decltype(L)::value><<<grid, INTERP_THREADS, 0, stream>>>(lhs.blocks, rhs.blocks, n_chunks, t, out);
+            interpolate_kernel<decltype(L)::value, decltype(D)::value><<<grid, INTERP_THREADS, 0, stream>>>(lhs.blocks, rhs.blocks, n_chunks, t, out);
     });
 }
 

@@ -22,9 +22,9 @@ cudaError_t launch_radix_sort(uint32_t* keys0, uint32_t* vals0, uint32_t* keys1,
 // project.cu
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
                         FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream);
-void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, const void* tt /* 4D only */,
+void launch_repack(CloudLayout layout, uint32_t sh_degree, const void* sh /* staged: staged_bytes per gaussian */, const void* rot, const void* so, const void* tt /* 4D only */,
                    uint32_t n, CloudView cloud, cudaStream_t stream);
-void launch_project(CloudLayout layout, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+void launch_project(CloudLayout layout, uint32_t sh_degree, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes /* null: project_kernel */,
                     cudaStream_t stream);
@@ -88,11 +88,11 @@ void launch_particle_step(void* behaviors, uint32_t count, float dt, CloudView c
 // subset.cu
 uint32_t subset_num_ctas(uint32_t n);
 void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t* cta_cnt, uint32_t* total, cudaStream_t stream);
-void launch_subset_scatter(CloudLayout layout, CloudView src, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
+void launch_subset_scatter(CloudLayout layout, uint32_t sh_degree, CloudView src, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
                            CloudView dst, cudaStream_t stream);
-void launch_subset_gather(CloudLayout layout, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst, cudaStream_t stream);
-void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so,
+void launch_subset_gather(CloudLayout layout, uint32_t sh_degree, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst, cudaStream_t stream);
+void launch_unpack(CloudLayout layout, uint32_t sh_degree, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so,
                    void* tt /* 4D only */, cudaStream_t stream);
 // interpolate.cu
-void launch_interpolate(CloudLayout layout, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream);
+void launch_interpolate(CloudLayout layout, uint32_t sh_degree, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream);
 }  // namespace bgs

@@ -1,4 +1,4 @@
-// project.cu -- stage 3: per-gaussian 3D->2D covariance projection + SH-degree-3 colour, run
+// project.cu -- stage 3: per-gaussian 3D->2D covariance projection + SH colour (degree 0..3), run
 // ONCE per visible gaussian (the reference runs it 4x per gaussian in its vertex stage:
 // src/render/gaussian.wgsl:185-436).
 //
@@ -69,8 +69,8 @@ __device__ __forceinline__ void make_bbox(float cx, float cy, float hx, float hy
 // lane's copy k moves piece (32 k + lane) % NP of entry (32 k + lane) / NP, so NP consecutive lanes read one block
 // front to back.  NP = CH (the whole block) when the colour source reads the SH coefficients, else GEO pieces:
 // position, rotation, scale and opacity (f32: plus the first SH piece, which shares scale_opacity's 32 B sector).
-// Piece p of entry g sits at 16 B unit g * CH + (p ^ (g & 7)): the eight lanes of a quarter warp that read the same
-// piece of their own entries hit eight different 16 B bank groups, and so do the copies' stores.
+// Piece p of entry g sits at 16 B unit g * CH + slot(p, g) (stage_slot): the eight lanes of a quarter warp that read
+// the same piece of their own entries hit eight different 16 B bank groups, and so do the copies' stores.
 __device__ __forceinline__ void cp_async16(uint4* dst_shared, const uint4* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_shared)), "l"(src)
                  : "memory");
@@ -78,6 +78,17 @@ __device__ __forceinline__ void cp_async16(uint4* dst_shared, const uint4* src) 
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// Blocks of 8 or more chunks: p ^ (g & 7) (a permutation of each aligned group of 8 pieces).  4-chunk blocks: two
+// entries share a 128 B row of banks, so p ^ ((g >> 1) & 3) -- entries g of one quarter warp take the 8 combinations of
+// (g & 1, (g >> 1) & 3), hence 8 bank groups; a copy round's 8 lanes move pieces 0..3 of an even and the next odd entry,
+// the 8 units of one row.
+template <int CH>
+__device__ __forceinline__ int stage_slot(int p, int g) {
+    static_assert(CH % 8 == 0 || CH == 4, "blocks of 4 or a multiple of 8 chunks");
+    if constexpr (CH == 4) return p ^ ((g >> 1) & 3);
+    else return p ^ (g & 7);
+}
 
 template <int CH, int NP>
 __device__ __forceinline__ void gather_blocks(const uint4* __restrict__ blocks, uint32_t id, uint32_t n_valid,
@@ -87,20 +98,21 @@ __device__ __forceinline__ void gather_blocks(const uint4* __restrict__ blocks, 
     for (int k = 0; k < NP; ++k) {
         const int g = (32 * k + lane) / NP, p = lane % NP;
         const uint32_t gid = __shfl_sync(0xFFFFFFFFu, id, g);
-        if ((uint32_t)g < n_valid) cp_async16(stage + g * CH + (p ^ (g & 7)), blocks + (size_t)gid * CH + p);
+        if ((uint32_t)g < n_valid) cp_async16(stage + g * CH + stage_slot<CH>(p, g), blocks + (size_t)gid * CH + p);
     }
 }
 
-// entry g's attributes out of a stage (the covariance layout's record arrives in q and so as its lanes fall)
-template <bool F16>
+// entry g's attributes out of a stage, the S_d SH floats into sh (the covariance layout's record arrives in q and so as
+// its lanes fall)
+template <bool F16, uint32_t D>
 struct Attr;
-template <>
-struct Attr<false> {
+template <uint32_t D>
+struct Attr<false, D> {
     static constexpr CloudLayout L = CloudLayout::F32;
-    static constexpr int CH = chunks(L), GEO = 4;
+    static constexpr int CH = chunks(L, D), GEO = 4;
     __device__ static float4 load(const uint4* stage, int g, float* sh, float q[4], float so[4], bool need_sh, uint32_t&) {
         auto piece = [&](int p) {
-            const uint4 v = stage[g * CH + (p ^ (g & 7))];
+            const uint4 v = stage[g * CH + stage_slot<CH>(p, g)];
             return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
         };
         const float4 p = piece(POS_CHUNK), r = piece(SECOND_CHUNK), s = piece(SO_CHUNK);
@@ -108,7 +120,7 @@ struct Attr<false> {
         so[0] = s.x; so[1] = s.y; so[2] = s.z; so[3] = s.w;
         if (need_sh) {
 #pragma unroll
-            for (int i = 0; i < (int)sh_chunks(L); ++i) {
+            for (int i = 0; i < (int)sh_chunks(L, D); ++i) {
                 const float4 v = piece(sh_first(L) + i);
                 sh[4 * i] = v.x; sh[4 * i + 1] = v.y; sh[4 * i + 2] = v.z; sh[4 * i + 3] = v.w;
             }
@@ -116,23 +128,29 @@ struct Attr<false> {
         return p;
     }
 };
-template <>
-struct Attr<true> {
+template <uint32_t D>
+struct Attr<true, D> {
     static constexpr CloudLayout L = CloudLayout::F16;
-    static constexpr int CH = chunks(L), GEO = 2;
+    static constexpr int CH = chunks(L, D), GEO = 2;
+    static constexpr int FULL = (int)sh_floats(D) / 8;   // SH chunks of 4 words; below degree 3 a last one of 2 words
     __device__ static float4 load(const uint4* stage, int g, float* sh, float q[4], float so[4], bool need_sh,
                                   uint32_t& op_bits) {
-        auto piece = [&](int p) { return stage[g * CH + (p ^ (g & 7))]; };
+        auto piece = [&](int p) { return stage[g * CH + stage_slot<CH>(p, g)]; };
         const uint4 pw = piece(POS_CHUNK), w = piece(SECOND_CHUNK);
         op_bits = w.w & 0xFFFFu;
         second_lanes(w.x, w.y, q);
         second_lanes(w.z, w.w, so);
         if (need_sh) {
 #pragma unroll
-            for (int i = 0; i < (int)sh_chunks(L); ++i) {
+            for (int i = 0; i < FULL; ++i) {
                 const uint4 v = piece(sh_first(L) + i);
                 sh[8 * i] = half_lo(v.x); sh[8 * i + 1] = half_hi(v.x); sh[8 * i + 2] = half_lo(v.y); sh[8 * i + 3] = half_hi(v.y);
                 sh[8 * i + 4] = half_lo(v.z); sh[8 * i + 5] = half_hi(v.z); sh[8 * i + 6] = half_lo(v.w); sh[8 * i + 7] = half_hi(v.w);
+            }
+            if constexpr (sh_floats(D) % 8 != 0) {
+                const uint4 v = piece(sh_first(L) + FULL);
+                sh[8 * FULL] = half_lo(v.x); sh[8 * FULL + 1] = half_hi(v.x);
+                sh[8 * FULL + 2] = half_lo(v.y); sh[8 * FULL + 3] = half_hi(v.y);
             }
         }
         return make_float4(__uint_as_float(pw.x), __uint_as_float(pw.y), __uint_as_float(pw.z), __uint_as_float(pw.w));
@@ -140,33 +158,34 @@ struct Attr<true> {
 };
 
 // upload-time repack of the planes into gaussian-major blocks (one thread per 16 B chunk; coalesced both ways)
-template <CloudLayout L>
+template <CloudLayout L, uint32_t D>
 __device__ __forceinline__ void repack_chunk(const CloudPlanes<const uint4>& planes, uint32_t n, uint4* __restrict__ blocks,
                                              const uint4* __restrict__ tt) {
+    constexpr uint32_t CH = chunks(L, D);
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (size_t)n * chunks(L)) return;
-    const uint4* src = planes.unit<L>((uint32_t)(i % chunks(L)), i / chunks(L), tt);
+    if (i >= (size_t)n * CH) return;
+    const uint4* src = planes.unit<L, D>((uint32_t)(i % CH), i / CH, tt);
     blocks[i] = src ? __ldg(src) : make_uint4(0u, 0u, 0u, 0u);
 }
-template <CloudLayout L>
+template <CloudLayout L, uint32_t D>
 __global__ void repack_kernel(CloudPlanes<const uint4> planes, uint32_t n, uint4* __restrict__ blocks) {
-    repack_chunk<L>(planes, n, blocks, nullptr);
+    repack_chunk<L, D>(planes, n, blocks, nullptr);
 }
 // the 4D layout's, which also reads the timestamp-timescale plane
 __global__ void repack_4d_kernel(CloudPlanes<const uint4> planes, uint32_t n, uint4* __restrict__ blocks,
                                  const uint4* __restrict__ tt) {
-    repack_chunk<CloudLayout::F32x4D>(planes, n, blocks, tt);
+    repack_chunk<CloudLayout::F32x4D, SH_DEGREE_MAX>(planes, n, blocks, tt);
 }
-void launch_repack(CloudLayout layout, const void* sh, const void* rot, const void* so, const void* tt, uint32_t n,
-                   CloudView cloud, cudaStream_t stream) {
+void launch_repack(CloudLayout layout, uint32_t sh_degree, const void* sh, const void* rot, const void* so, const void* tt,
+                   uint32_t n, CloudView cloud, cudaStream_t stream) {
     const CloudPlanes<const uint4> planes{reinterpret_cast<const uint4*>(cloud.pos), static_cast<const uint4*>(sh),
                                           static_cast<const uint4*>(rot), static_cast<const uint4*>(so)};
     const uint32_t grid = (uint32_t)(((size_t)n * cloud.chunks + 255) / 256);
-    with_layout(layout, [&](auto L) {
+    with_layout_degree(layout, sh_degree, [&](auto L, auto D) {
         if constexpr (is_4d(decltype(L)::value))
             repack_4d_kernel<<<grid, 256, 0, stream>>>(planes, n, cloud.blocks, static_cast<const uint4*>(tt));
         else
-            repack_kernel<decltype(L)::value><<<grid, 256, 0, stream>>>(planes, n, cloud.blocks);
+            repack_kernel<decltype(L)::value, decltype(D)::value><<<grid, 256, 0, stream>>>(planes, n, cloud.blocks);
     });
 }
 
@@ -438,8 +457,10 @@ __device__ __forceinline__ void sh_basis(const FrameConsts& fc, const float A[3]
     for (int kk = 0; kk < 16; ++kk) basis[kk] *= c_shc[kk];
 }
 
-// RasterizeMode::Color: the SH-3 colour seen along the camera ray in the splat's model frame
-__device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3][3], const float pw[3], const float sh[48],
+// RasterizeMode::Color: the SH colour seen along the camera ray in the splat's model frame, over the K_d bands of degree
+// D (spherical_harmonics.wgsl:34-68 keeps the bands its SH_COEFF_COUNT holds); sh holds S_d floats
+template <uint32_t D>
+__device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3][3], const float pw[3], const float* sh,
                                           float rgb[3]) {
     float basis[16];
     sh_basis(fc, A, pw, basis);
@@ -447,7 +468,7 @@ __device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3
     for (int cc = 0; cc < 3; ++cc) {
         float acc = 0.5f;
 #pragma unroll
-        for (int kk = 0; kk < 16; ++kk) acc = fmaf(sh[3 * kk + cc], basis[kk], acc);   // colour: FMA is fine
+        for (int kk = 0; kk < (int)sh_bands(D); ++kk) acc = fmaf(sh[3 * kk + cc], basis[kk], acc);   // colour: FMA is fine
         rgb[cc] = acc;
     }
     if (fc.color_space == 0u) {
@@ -580,9 +601,9 @@ __device__ __forceinline__ void store_rec(SplatRec* __restrict__ dst, const Spla
 // One entry of the index list -> the 48 B record at recs[r] (+ the 2DGS extra record and the aux colours).  An
 // undrawn gaussian (outside the frustum, or unselected under DrawMode::Selected) gets an empty bbox and no colour.
 // MODES2: the Classification / OpticalFlow colour sources (project_modes_kernel) instead of the four others.
-template <bool F16, bool MODES2>
+template <bool F16, uint32_t D, bool MODES2>
 __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCounters* __restrict__ ctr, uint32_t r,
-                                            float4 p4, const float q[4], const float so[4], const float sh[48],
+                                            float4 p4, const float q[4], const float so[4], const float* sh,
                                             const float* __restrict__ cutoff_tab, uint32_t op_bits,
                                             SplatRec* __restrict__ recs, float4* __restrict__ extra,
                                             float4* __restrict__ aux, const ModeConsts& mc) {
@@ -626,14 +647,14 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
         float rgb[3] = {0.f, 0.f, 0.f}, drgb[3] = {0.f, 0.f, 0.f}, nrgb[3] = {0.f, 0.f, 0.f};
         if constexpr (MODES2) {
             if (mode == BGS_RASTERIZE_CLASSIFICATION) {
-                sh_colour(fc, A, pw, sh, rgb);
+                sh_colour<D>(fc, A, pw, sh, rgb);
                 class_colour(mc, p4.w, rgb);
             } else {
                 flow_colour(fc, mc, pw, rgb);
             }
             rec.r = rgb[0]; rec.g = rgb[1]; rec.b = rgb[2];
         } else {
-            if (mode == BGS_RASTERIZE_COLOR) sh_colour(fc, A, pw, sh, rgb);
+            if (mode == BGS_RASTERIZE_COLOR) sh_colour<D>(fc, A, pw, sh, rgb);
             if (mode == BGS_RASTERIZE_POSITION) position_colour(fc, pw, rgb);
             if (mode == BGS_RASTERIZE_DEPTH || fc.aux) depth_colour(fc, ctr, pw, drgb);
             if (mode == BGS_RASTERIZE_NORMAL || fc.aux) normal_colour(fc, A, Rm, sc, nrgb);
@@ -662,14 +683,15 @@ constexpr int PROJ_THREADS = 128, PROJ_WARPS = PROJ_THREADS / 32, PROJ_MIN_CTAS 
 // The grid is persistent and each warp strides over groups of 32 entries with two groups in flight: once the lanes
 // hold group i's attributes in registers, the copies of group i + 1 start filling the warp's stage and the list
 // entries of group i + 2 are on their way into a register, so both dependent memory latencies sit under project_one.
-template <bool F16, bool MODES2>
+template <bool F16, uint32_t D, bool MODES2>
 __device__ __forceinline__ void project_groups(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list,
                                                int by_slot, const FrameCounters* __restrict__ ctr, const FrameConsts& fc,
                                                bool need_sh, SplatRec* __restrict__ recs, float4* __restrict__ extra,
                                                const float* __restrict__ cutoff_tab, float4* __restrict__ aux,
                                                const ModeConsts& mc) {
-    constexpr int CH = Attr<F16>::CH;
-    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * CH];   // f16 16 KB, f32 32 KB
+    using A = Attr<F16, D>;
+    constexpr int CH = A::CH;
+    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * CH];   // degree 3: f16 16 KB, f32 32 KB
     const int lane = threadIdx.x & 31;
     uint4* const stage = s_stages[threadIdx.x >> 5];
     const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
@@ -680,7 +702,7 @@ __device__ __forceinline__ void project_groups(const void* __restrict__ blocks, 
         const uint32_t n_valid = r0 < n_vis ? n_vis - r0 : 0u;
         const uint4* b = reinterpret_cast<const uint4*>(blocks);
         if (need_sh) gather_blocks<CH, CH>(b, id, n_valid, stage, lane);
-        else gather_blocks<CH, Attr<F16>::GEO>(b, id, n_valid, stage, lane);
+        else gather_blocks<CH, A::GEO>(b, id, n_valid, stage, lane);
         cp_async_commit();
     };
     uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
@@ -690,36 +712,36 @@ __device__ __forceinline__ void project_groups(const void* __restrict__ blocks, 
         cp_async_wait<0>();
         __syncwarp();   // every lane's copies of this group have landed
         const uint32_t r = r0 + lane;
-        float sh[48], q[4], so[4];
+        float sh[sh_floats(D)], q[4], so[4];
         uint32_t op_bits = 0u;
         float4 p4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (r < n_vis) p4 = Attr<F16>::load(stage, lane, sh, q, so, need_sh, op_bits);
+        if (r < n_vis) p4 = A::load(stage, lane, sh, q, so, need_sh, op_bits);
         __syncwarp();   // the stage is read out before the next group's copies overwrite it
         gather(r0 + stride, id_next);
         id_next = list_id(r0 + 2u * stride + lane);
-        if (r < n_vis) project_one<F16, MODES2>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc);
+        if (r < n_vis) project_one<F16, D, MODES2>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc);
     }
 }
 
-template <bool F16>
+template <bool F16, uint32_t D>
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
                const FrameCounters* __restrict__ ctr, FrameConsts fc, SplatRec* __restrict__ recs,
                float4* __restrict__ extra /* 4 x float4 per record, 2DGS + USE_AABB only */, const float* __restrict__ cutoff_tab,
                float4* __restrict__ aux /* 2 x float4 per record (depth rgb, normal rgb), bgs_render_aux only */) {
-    project_groups<F16, false>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs, extra,
+    project_groups<F16, D, false>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs, extra,
                                cutoff_tab, aux, ModeConsts{});
 }
 
 // project_kernel for RasterizeMode::Classification / OpticalFlow (bgs_render_ex): the same records but for r, g, b.  A
 // kernel of its own, so that project_kernel's mode branch (and its register budget) stays as it is.
-template <bool F16>
+template <bool F16, uint32_t D>
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_modes_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
                      const FrameCounters* __restrict__ ctr, FrameConsts fc, ModeConsts mc, SplatRec* __restrict__ recs,
                      float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
     // OpticalFlow reads the position only
-    project_groups<F16, true>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs,
+    project_groups<F16, D, true>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs,
                               extra, cutoff_tab, nullptr, mc);
 }
 
@@ -882,7 +904,7 @@ __device__ __forceinline__ void project_one_4d(const FrameConsts& fc, const Mode
 // The 4D block is 768 B: a warp stages only each entry's first 128 B line (position, both rotations, scale-opacity,
 // timestamp-timescale; 4 KB per warp) with the coalesced copies of project_groups, piece p of entry g at
 // g * GEO4 + (p ^ (g & 7)).  The coefficients stay in global memory until a drawn splat's colour needs them.
-constexpr int CH4 = (int)chunks(CloudLayout::F32x4D), GEO4 = 8;
+constexpr int CH4 = (int)chunks(CloudLayout::F32x4D, SH_DEGREE_MAX), GEO4 = 8;
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_4d_kernel(const uint4* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
                   const FrameCounters* __restrict__ ctr, FrameConsts fc, ModeConsts mc, TemporalConsts tc,
@@ -947,7 +969,7 @@ void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_pa
     depth_range_kernel<<<1, 32, 0, stream>>>(pos, n, sorted_payload, slot_ids, ctr, fc);
 }
 
-void launch_project(CloudLayout layout, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
+void launch_project(CloudLayout layout, uint32_t sh_degree, const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                     const FrameConsts& fc, SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count,
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes, cudaStream_t stream) {
     // a persistent grid: as many CTAs as the launch bound lets the SMs hold, fewer when the hint (last frame's visible
@@ -955,14 +977,19 @@ void launch_project(CloudLayout layout, const void* blocks, const uint32_t* inde
     uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
     if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
     if (grid < 1u) grid = 1u;
-    const bool f16 = is_f16(layout);
-    if (modes) {   // Classification / OpticalFlow (no aux outputs)
-        if (f16) project_modes_kernel<true><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
-        else project_modes_kernel<false><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes, recs, extra, cutoff_tab);
-        return;
-    }
-    if (f16) project_kernel<true><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
-    else project_kernel<false><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra, cutoff_tab, aux);
+    // (both f16 layouts run the F16 kernels: the covariance record differs only in fc.cov_pre)
+    with_layout_degree(layout, sh_degree, [&](auto L, auto Dt) {
+        constexpr CloudLayout Lv = decltype(L)::value;
+        constexpr uint32_t D = decltype(Dt)::value;
+        if constexpr (!is_4d(Lv)) {
+            if (modes)   // Classification / OpticalFlow (no aux outputs)
+                project_modes_kernel<is_f16(Lv), D><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, *modes,
+                                                                                      recs, extra, cutoff_tab);
+            else
+                project_kernel<is_f16(Lv), D><<<grid, PROJ_THREADS, 0, stream>>>(blocks, index_list, by_slot, ctr, fc, recs, extra,
+                                                                                cutoff_tab, aux);
+        }
+    });
 }
 
 }  // namespace bgs

@@ -116,23 +116,24 @@ __global__ void __launch_bounds__(SUBSET_THREADS) subset_gather_kernel(CloudView
 
 // repack_kernel's inverse over gaussians [lo, lo + m): block chunk c of gaussian lo + j goes back to its unit of
 // gaussian j in the planes (planes.pos is null: the position plane is read back directly).
-template <CloudLayout L>
+template <CloudLayout L, uint32_t D>
 __device__ __forceinline__ void unpack_chunk(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
                                              const CloudPlanes<uint4>& planes, uint4* __restrict__ tt) {
+    constexpr uint32_t CH = chunks(L, D);
     const size_t t = (size_t)blockIdx.x * SUBSET_THREADS + threadIdx.x;
-    if (t >= (size_t)m * chunks(L)) return;
-    uint4* dst = planes.unit<L>((uint32_t)(t % chunks(L)), t / chunks(L), tt);
-    if (dst) *dst = __ldg(blocks + (size_t)lo * chunks(L) + t);
+    if (t >= (size_t)m * CH) return;
+    uint4* dst = planes.unit<L, D>((uint32_t)(t % CH), t / CH, tt);
+    if (dst) *dst = __ldg(blocks + (size_t)lo * CH + t);
 }
-template <CloudLayout L>
+template <CloudLayout L, uint32_t D>
 __global__ void __launch_bounds__(SUBSET_THREADS) unpack_kernel(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
                                                                 CloudPlanes<uint4> planes) {
-    unpack_chunk<L>(blocks, lo, m, planes, nullptr);
+    unpack_chunk<L, D>(blocks, lo, m, planes, nullptr);
 }
 // the 4D layout's, which also writes the timestamp-timescale plane
 __global__ void __launch_bounds__(SUBSET_THREADS) unpack_4d_kernel(const uint4* __restrict__ blocks, uint32_t lo, uint32_t m,
                                                                    CloudPlanes<uint4> planes, uint4* __restrict__ tt) {
-    unpack_chunk<CloudLayout::F32x4D>(blocks, lo, m, planes, tt);
+    unpack_chunk<CloudLayout::F32x4D, SH_DEGREE_MAX>(blocks, lo, m, planes, tt);
 }
 
 uint32_t subset_num_ctas(uint32_t n) { return (n + SUBSET_THREADS - 1) / SUBSET_THREADS; }
@@ -143,13 +144,14 @@ void launch_subset_count(const float4* pos, uint32_t n, uint32_t* mask, uint32_t
     subset_scan_kernel<<<1, 1024, 0, stream>>>(cta_cnt, g, total);
 }
 
-// (the copies depend on the layout only through the block's size: both f16 layouts run the same kernels, and the 4D
-// layout's 48-chunk blocks a warp-wide variant of the scatter)
-void launch_subset_scatter(CloudLayout layout, CloudView src, uint32_t n, const uint32_t* mask, const uint32_t* cta_off,
-                           CloudView dst, cudaStream_t stream) {
+// (the copies depend on the layout and the SH degree only through the block's size: blocks of one size run the same
+// kernels, and the 4D layout's 48-chunk blocks a warp-wide variant of the scatter)
+void launch_subset_scatter(CloudLayout layout, uint32_t sh_degree, CloudView src, uint32_t n, const uint32_t* mask,
+                           const uint32_t* cta_off, CloudView dst, cudaStream_t stream) {
     const uint32_t g = subset_num_ctas(n), words = (n + 31) / 32;
-    with_layout(layout, [&](auto L) {
-        subset_scatter_kernel<chunks(decltype(L)::value)><<<g, SUBSET_THREADS, 0, stream>>>(src, words, mask, cta_off, dst);
+    with_layout_degree(layout, sh_degree, [&](auto L, auto D) {
+        subset_scatter_kernel<chunks(decltype(L)::value, decltype(D)::value)><<<g, SUBSET_THREADS, 0, stream>>>(src, words, mask,
+                                                                                                             cta_off, dst);
     });
 }
 
@@ -157,21 +159,23 @@ static uint32_t chunk_grid(uint32_t n, uint32_t chunks) {
     return (uint32_t)(((size_t)n * chunks + SUBSET_THREADS - 1) / SUBSET_THREADS);
 }
 
-void launch_subset_gather(CloudLayout layout, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst, cudaStream_t stream) {
-    with_layout(layout, [&](auto L) {
-        subset_gather_kernel<chunks(decltype(L)::value)><<<chunk_grid(k, src.chunks), SUBSET_THREADS, 0, stream>>>(src, idx, k, dst);
+void launch_subset_gather(CloudLayout layout, uint32_t sh_degree, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst,
+                          cudaStream_t stream) {
+    with_layout_degree(layout, sh_degree, [&](auto L, auto D) {
+        subset_gather_kernel<chunks(decltype(L)::value, decltype(D)::value)><<<chunk_grid(k, src.chunks), SUBSET_THREADS, 0, stream>>>(
+            src, idx, k, dst);
     });
 }
 
-void launch_unpack(CloudLayout layout, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so, void* tt,
-                   cudaStream_t stream) {
+void launch_unpack(CloudLayout layout, uint32_t sh_degree, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot,
+                   void* so, void* tt, cudaStream_t stream) {
     const CloudPlanes<uint4> planes{nullptr, static_cast<uint4*>(sh), static_cast<uint4*>(rot), static_cast<uint4*>(so)};
     const uint32_t grid = chunk_grid(m, cloud.chunks);
-    with_layout(layout, [&](auto L) {
+    with_layout_degree(layout, sh_degree, [&](auto L, auto D) {
         if constexpr (is_4d(decltype(L)::value))
             unpack_4d_kernel<<<grid, SUBSET_THREADS, 0, stream>>>(cloud.blocks, lo, m, planes, static_cast<uint4*>(tt));
         else
-            unpack_kernel<decltype(L)::value><<<grid, SUBSET_THREADS, 0, stream>>>(cloud.blocks, lo, m, planes);
+            unpack_kernel<decltype(L)::value, decltype(D)::value><<<grid, SUBSET_THREADS, 0, stream>>>(cloud.blocks, lo, m, planes);
     });
 }
 

@@ -17,18 +17,37 @@ import numpy as np
 
 SH_COEFF_COUNT = 48  # src/material/spherical_harmonics.rs:46-47 (sh3 default)
 HALF_SH_COEFF_COUNT = 24
+# SH degree d (the reference's sh0 .. sh3 features; include/bgs.h): K_d = (d + 1)^2 coefficients per channel, S_d =
+# pad4(3 K_d) floats per gaussian, coefficient k of channel c at sh[3k + c]; lanes 3 K_d .. S_d - 1 are padding
+SH_WIDTHS = (4, 12, 28, 48)
+
+
+def sh_bands(sh_degree: int) -> int:
+    """K_d: coefficients per channel at degree d."""
+    return (sh_degree + 1) ** 2
+
+
+def sh_degree_of_width(width: int) -> int:
+    """The degree whose SH plane is `width` floats (4, 12, 28 or 48); any other width raises ValueError."""
+    if width not in SH_WIDTHS:
+        raise ValueError(f"an SH plane holds 4, 12, 28 or 48 floats per gaussian (degree 0..3), not {width}")
+    return SH_WIDTHS.index(width)
 
 
 @dataclasses.dataclass
 class PlanarGaussian3d:
     position_visibility: np.ndarray  # (n, 4) f32: x, y, z, visibility      f32.rs:53-56
-    spherical_harmonic: np.ndarray   # (n, 48) f32: sh[3k + c]              spherical_harmonics.rs:114-120
+    spherical_harmonic: np.ndarray   # (n, S_d) f32: sh[3k + c], S_d = 4, 12, 28 or 48 spherical_harmonics.rs:114-120
     rotation: np.ndarray             # (n, 4) f32: w, x, y, z               f32.rs:95-97
     scale_opacity: np.ndarray        # (n, 4) f32: sx, sy, sz, opacity      f32.rs:172-175
 
     def __post_init__(self):
-        for name, width in (("position_visibility", 4), ("spherical_harmonic", SH_COEFF_COUNT), ("rotation", 4),
-                            ("scale_opacity", 4)):
+        sh = np.ascontiguousarray(self.spherical_harmonic, dtype=np.float32)
+        if sh.ndim != 2:
+            raise ValueError("spherical_harmonic must have shape (n, S_d)")
+        sh_degree_of_width(sh.shape[1])
+        self.spherical_harmonic = sh
+        for name, width in (("position_visibility", 4), ("rotation", 4), ("scale_opacity", 4)):
             a = np.ascontiguousarray(getattr(self, name), dtype=np.float32)
             if a.ndim != 2 or a.shape[1] != width:
                 raise ValueError(f"{name} must have shape (n, {width})")
@@ -39,6 +58,23 @@ class PlanarGaussian3d:
 
     def __len__(self) -> int:
         return len(self.position_visibility)
+
+    @property
+    def sh_degree(self) -> int:
+        """0..3, from the SH plane's width (4, 12, 28, 48)."""
+        return sh_degree_of_width(self.spherical_harmonic.shape[1])
+
+    def with_sh_degree(self, sh_degree: int) -> "PlanarGaussian3d":
+        """The cloud at another degree: the coefficients of the bands both degrees hold are kept, the others (and every
+        padding lane) are zero.  Truncating drops the higher bands; zero-padding to degree 3 gives a cloud that renders
+        exactly like this one."""
+        if sh_degree not in range(4):
+            raise ValueError(f"sh_degree must be 0..3, not {sh_degree}")
+        width = SH_WIDTHS[sh_degree]
+        keep = 3 * min(sh_bands(sh_degree), sh_bands(self.sh_degree))
+        sh = np.zeros((len(self), width), np.float32)
+        sh[:, :keep] = self.spherical_harmonic[:, :keep]
+        return PlanarGaussian3d(self.position_visibility, sh, self.rotation, self.scale_opacity)
 
     def subset(self, n) -> "PlanarGaussian3d":
         """An int: the first n gaussians.  An index array: those gaussians, in that order -- what the reference's
@@ -60,23 +96,30 @@ class PlanarGaussian3d:
         return compute_aabb(self.position_visibility)
 
     @staticmethod
-    def from_f16(pos_vis, sh_packed, rot_scale_opacity) -> "PlanarGaussian3d":
+    def from_f16(pos_vis, sh_packed, rot_scale_opacity, sh_degree: int | None = None) -> "PlanarGaussian3d":
         """The exact inverse of `pack_f16`: each half widened to f32 (pack_f16 of the result gives the same words back for
         every non-NaN half; a NaN half stays NaN).  For a precomputed-covariance record the result holds the covariance in
-        the slots `precomputed_covariance()` uses."""
+        the slots `precomputed_covariance()` uses.  sh_degree None: the degree of a 2-D sh_packed's width (S_d / 2
+        words), 3 for a flat one."""
         def halves(w, shift):
             return ((np.asarray(w, np.uint32) >> np.uint32(shift)) & np.uint32(0xFFFF)).astype(np.uint16).view(np.float16).astype(np.float32)
 
-        shp = np.asarray(sh_packed, np.uint32).reshape(-1, HALF_SH_COEFF_COUNT)
+        shp = np.asarray(sh_packed, np.uint32)
+        if sh_degree is None:
+            sh_degree = sh_degree_of_width(2 * shp.shape[1]) if shp.ndim == 2 else 3
+        if sh_degree not in range(4):
+            raise ValueError(f"sh_degree must be 0..3, not {sh_degree}")
+        width = SH_WIDTHS[sh_degree]
+        shp = shp.reshape(-1, width // 2)
         w = np.asarray(rot_scale_opacity, np.uint32).reshape(-1, 4)
-        sh = np.empty((len(shp), SH_COEFF_COUNT), np.float32)
+        sh = np.empty((len(shp), width), np.float32)
         sh[:, 0::2], sh[:, 1::2] = halves(shp, 0), halves(shp, 16)     # even coefficient in the low half
         rot = np.stack([halves(w[:, 0], 16), halves(w[:, 0], 0), halves(w[:, 1], 16), halves(w[:, 1], 0)], axis=1)
         so = np.stack([halves(w[:, 2], 16), halves(w[:, 2], 0), halves(w[:, 3], 16), halves(w[:, 3], 0)], axis=1)
         return PlanarGaussian3d(np.asarray(pos_vis, np.float32).reshape(-1, 4), sh, rot, so)
 
     def pack_f16(self) -> tuple[np.ndarray, np.ndarray]:
-        """-> (sh_packed (n,24) u32, rot_scale_opacity (n,4) u32); pack(upper, lower) = upper<<16 | lower."""
+        """-> (sh_packed (n, S_d / 2) u32, rot_scale_opacity (n,4) u32); pack(upper, lower) = upper<<16 | lower."""
         def bits(a):
             return np.ascontiguousarray(a, dtype=np.float32).astype(np.float16).view(np.uint16).astype(np.uint32)
 
@@ -129,8 +172,9 @@ def compute_aabb(position_visibility: np.ndarray) -> tuple[np.ndarray, np.ndarra
     return (center - half).astype(np.float32), (center + half).astype(np.float32)
 
 
-def random_gaussians_3d_seeded(n: int, seed: int = 0, chunk: int = 1 << 18) -> PlanarGaussian3d:
-    """planar_3d.rs:182-191 (distributions + field order), Philox stream, deterministic in (n, seed)."""
+def random_gaussians_3d_seeded(n: int, seed: int = 0, chunk: int = 1 << 18, sh_degree: int = 3) -> PlanarGaussian3d:
+    """planar_3d.rs:182-191 (distributions + field order), Philox stream, deterministic in (n, seed).  sh_degree < 3:
+    the same cloud through `with_sh_degree` (the lower bands of the same draws, padding lanes zero)."""
     rng = np.random.Generator(np.random.Philox(seed))
     pos = np.empty((n, 4), np.float32)
     sh = np.empty((n, SH_COEFF_COUNT), np.float32)
@@ -145,7 +189,8 @@ def random_gaussians_3d_seeded(n: int, seed: int = 0, chunk: int = 1 << 18) -> P
         so[lo:hi, 0:3] = u[:, 7:10]
         so[lo:hi, 3] = u[:, 10] * 0.8
         sh[lo:hi] = u[:, 11:59] * 2.0 - 1.0
-    return PlanarGaussian3d(pos, sh, rot, so)
+    cloud = PlanarGaussian3d(pos, sh, rot, so)
+    return cloud if sh_degree == 3 else cloud.with_sh_degree(sh_degree)
 
 
 def random_gaussians_3d(n: int) -> PlanarGaussian3d:

@@ -28,7 +28,7 @@ import struct
 
 import numpy as np
 
-from .gaussian import PlanarGaussian3d
+from .gaussian import SH_WIDTHS, PlanarGaussian3d
 
 # FlexBuffers value types (flexbuffers.h, enum Type)
 FBT_NULL, FBT_INT, FBT_UINT, FBT_FLOAT, FBT_KEY, FBT_STRING = 0, 1, 2, 3, 4, 5
@@ -272,10 +272,41 @@ class Builder:
 _PLANES = (
     # plane of PlanarGaussian3d, [(field, first column, width)] of its element struct
     (b"position_visibility", "position_visibility", ((b"position", 0, 3), (b"visibility", 3, 1))),
-    (b"spherical_harmonic", "spherical_harmonic", ((b"coefficients", 0, 48),)),
+    (b"spherical_harmonic", "spherical_harmonic", ((b"coefficients", 0, 48),)),   # (S_d at degree d: _sh_fields)
     (b"rotation", "rotation", ((b"rotation", 0, 4),)),
     (b"scale_opacity", "scale_opacity", ((b"scale", 0, 3), (b"opacity", 3, 1))),
 )
+
+
+def _sh_fields(width: int):
+    """The SH plane's fields for an S_d-tuple (the reference's sh_d build serialises [f32; S_d])."""
+    return ((b"coefficients", 0, width),)
+
+
+def _cloud_planes(cloud: PlanarGaussian3d):
+    """_PLANES with the SH plane at the cloud's width."""
+    return tuple((key, attr, _sh_fields(cloud.spherical_harmonic.shape[1]) if attr == "spherical_harmonic" else fields)
+                 for key, attr, fields in _PLANES)
+
+
+def _sh_width(pr: "Ref") -> int:
+    """The S_d of an SH plane, from its first element's coefficient tuple (4, 12, 28 or 48; 48 for an empty plane or an
+    element that leaves the field to its default).  Any other length raises FlexBufferError."""
+    if len(pr) == 0:
+        return 48
+    e = pr[0]
+    if e.type == FBT_MAP:
+        v = e.as_dict().get(b"coefficients")
+    elif e.is_vector():
+        v = e[0] if len(e) else None
+    else:
+        raise FlexBufferError("plane element is not a struct")
+    if v is None:
+        return 48
+    w = len(v.as_float_array())
+    if w not in SH_WIDTHS:
+        raise FlexBufferError(f"coefficients has {w} elements, expected 4, 12, 28 or 48 (SH degree 0..3)")
+    return w
 
 
 def _encode_plane(b: Builder, arr: np.ndarray, fields):
@@ -359,7 +390,7 @@ def encode_gcloud_elementwise(cloud: PlanarGaussian3d) -> bytes:
     interleaved with their vectors): a differently laid out but equivalent FlexBuffer, used to exercise the generic reader."""
     b = Builder()
     planes = {}
-    for key, attr, fields in _PLANES:
+    for key, attr, fields in _cloud_planes(cloud):
         arr = np.ascontiguousarray(getattr(cloud, attr), np.float32)
         elems = []
         for row in arr:
@@ -375,7 +406,7 @@ def encode_gcloud(cloud: PlanarGaussian3d) -> bytes:
     """`PlanarGaussian3d::encode` (src/io/gcloud/flexbuffers.rs:9-16)."""
     b = Builder()
     planes = {}
-    for key, attr, fields in _PLANES:
+    for key, attr, fields in _cloud_planes(cloud):
         planes[key] = _encode_plane(b, np.ascontiguousarray(getattr(cloud, attr), np.float32), fields)
     return b.finish(*b.map(planes))
 
@@ -471,6 +502,8 @@ def _decode_gcloud(data) -> PlanarGaussian3d:
         n_ref = n if n_ref is None else n_ref
         if n != n_ref:
             raise FlexBufferError("planes differ in length")
+        if key == b"spherical_harmonic":   # the degree the file was written at, from its tuple length
+            fields = _sh_fields(_sh_width(pr))
         width = sum(w for _, _, w in fields)
         arr = _decode_plane_fast(pr, fields, width)
         if arr is None:

@@ -6,6 +6,9 @@ Restates src/io/ply.rs:23-132 of the reference, including its quirks:
   * rotation normalised (w, x, y, z = rot_0..3)              ply.rs:118-124
   * f_rest_i -> channel = i / 16 (not i / 15), coefficient = (i % 15) + 1, interleaved index
     coefficient * 3 + channel, ignored when >= 48            ply.rs:49-69 (later properties overwrite earlier)
+    At SH degree d (the reference's sh_d build; K_d = (d + 1)^2, S_d = 4, 12, 28, 48): channel = i / K_d, coefficient
+    = 1 if K_d == 1 else (i % (K_d - 1)) + 1, kept when coefficient * 3 + channel < S_d -- so sh0 stores f_rest_0 in
+    padding lane 3.
   * the cloud is padded with default gaussians by 32 - (n % 32) entries -- a full 32 when n is already
     a multiple of 32                                          ply.rs:127-129
 `.gcloud` (flexbuffers serde, src/io/gcloud/flexbuffers.rs:9-22) lives in `gcloud.py`; `load_cloud` below is the
@@ -18,11 +21,10 @@ import os
 
 import numpy as np
 
-from .gaussian import PlanarGaussian3d, PlanarGaussian4d, SH_COEFF_COUNT, SH_4D_COEFF_COUNT
+from .gaussian import PlanarGaussian3d, PlanarGaussian4d, SH_4D_COEFF_COUNT, SH_WIDTHS, sh_bands
 
 MAX_SIZE_VARIANCE = 4.0
 SH_CHANNELS = 3
-SH_COEFF_COUNT_PER_CHANNEL = 16
 REQUIRED = ["x", "y", "z", "f_dc_0", "f_dc_1", "f_dc_2", "scale_0", "scale_1", "opacity", "rot_0", "rot_1", "rot_2", "rot_3"]
 _PLY_TYPES = {"float": "f4", "float32": "f4", "double": "f8", "float64": "f8", "uchar": "u1", "uint8": "u1", "char": "i1",
               "int8": "i1", "short": "i2", "int16": "i2", "ushort": "u2", "uint16": "u2", "int": "i4", "int32": "i4",
@@ -57,19 +59,23 @@ def _read_header(f):
     return fmt, elements
 
 
-def parse_ply_3d(source) -> PlanarGaussian3d:
-    """`source`: path, bytes or binary file object.  A malformed file raises ValueError (ply.rs returns io::Error)."""
+def parse_ply_3d(source, sh_degree: int = 3) -> PlanarGaussian3d:
+    """`source`: path, bytes or binary file object.  A malformed file raises ValueError (ply.rs returns io::Error).
+    `sh_degree`: the SH degree of the cloud made (the reference's sh0 .. sh3 builds), f_rest_ placed by its rule."""
+    if sh_degree not in range(4):
+        raise ValueError(f"sh_degree must be 0..3, not {sh_degree}")
     if isinstance(source, (str, os.PathLike)):
         with open(source, "rb") as fh:
-            return parse_ply_3d(fh.read())
+            return parse_ply_3d(fh.read(), sh_degree)
     try:
         with np.errstate(over="ignore", invalid="ignore"):
-            return _parse_ply_3d(source)
+            return _parse_ply_3d(source, sh_degree)
     except (TypeError, IndexError, KeyError, UnicodeDecodeError, OverflowError, MemoryError) as e:
         raise ValueError(f"malformed ply: {type(e).__name__}: {e}") from e
 
 
-def _parse_ply_3d(source) -> PlanarGaussian3d:
+def _parse_ply_3d(source, sh_degree: int) -> PlanarGaussian3d:
+    width, bands = SH_WIDTHS[sh_degree], sh_bands(sh_degree)
     f = io.BytesIO(source) if isinstance(source, (bytes, bytearray)) else source
     fmt, elements = _read_header(f)
     vertex = None
@@ -103,11 +109,11 @@ def _parse_ply_3d(source) -> PlanarGaussian3d:
                 else:
                     f.read(np.dtype([(p, end + t) for p, t in el["props"]]).itemsize * el["count"])
     if vertex is None:
-        return PlanarGaussian3d(np.zeros((0, 4), np.float32), np.zeros((0, 48), np.float32), np.zeros((0, 4), np.float32),
+        return PlanarGaussian3d(np.zeros((0, 4), np.float32), np.zeros((0, width), np.float32), np.zeros((0, 4), np.float32),
                                 np.zeros((0, 4), np.float32))
     n = len(vertex["x"])
     pos = np.zeros((n, 4), np.float32); pos[:, 3] = 1.0                # PositionVisibility::default: visibility 1
-    sh = np.zeros((n, SH_COEFF_COUNT), np.float32)
+    sh = np.zeros((n, width), np.float32)
     rot = np.zeros((n, 4), np.float32)
     so = np.zeros((n, 4), np.float32)
     for key, v in vertex.items():                                      # header order, like set_property calls
@@ -126,10 +132,10 @@ def _parse_ply_3d(source) -> PlanarGaussian3d:
             rot[:, int(key[-1])] = v
         elif key.startswith("f_rest_"):
             i = int(key[7:])
-            channel = i // SH_COEFF_COUNT_PER_CHANNEL
-            coefficient = (i % (SH_COEFF_COUNT_PER_CHANNEL - 1)) + 1
+            channel = i // bands
+            coefficient = 1 if bands == 1 else (i % (bands - 1)) + 1
             idx = coefficient * SH_CHANNELS + channel
-            if idx < SH_COEFF_COUNT:
+            if idx < width:
                 sh[:, idx] = v
     mean = (so[:, 0] + so[:, 1] + so[:, 2]) / np.float32(3.0)
     for i in range(3):
@@ -147,16 +153,18 @@ def _parse_ply_3d(source) -> PlanarGaussian3d:
 
 
 def write_ply_3d(path, cloud: PlanarGaussian3d, n: int | None = None) -> None:
-    """Test helper: the inverse transformation (logit opacity, log scale, INRIA property order)."""
+    """Test helper: the inverse transformation (logit opacity, log scale, INRIA property order).  A degree-d cloud
+    writes 3 (K_d - 1) f_rest_ properties, channel-major (none at degree 0); its padding lanes are not written."""
     n = len(cloud) if n is None else n
-    props = ["x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2"] + [f"f_rest_{i}" for i in range(45)] + \
+    rest = sh_bands(cloud.sh_degree) - 1   # coefficients per channel beyond the DC term
+    props = ["x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2"] + [f"f_rest_{i}" for i in range(3 * rest)] + \
             ["opacity", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3"]
     arr = np.zeros(n, np.dtype([(p, "<f4") for p in props]))
     arr["x"], arr["y"], arr["z"] = cloud.position_visibility[:n, 0], cloud.position_visibility[:n, 1], cloud.position_visibility[:n, 2]
     for c in range(3):
         arr[f"f_dc_{c}"] = cloud.spherical_harmonic[:n, c]
-    for i in range(45):   # INRIA planar order: channel-major, 15 coefficients each
-        arr[f"f_rest_{i}"] = cloud.spherical_harmonic[:n, ((i % 15) + 1) * 3 + i // 15]
+    for i in range(3 * rest):   # INRIA planar order: channel-major, K_d - 1 coefficients each
+        arr[f"f_rest_{i}"] = cloud.spherical_harmonic[:n, ((i % rest) + 1) * 3 + i // rest]
     o = np.clip(cloud.scale_opacity[:n, 3].astype(np.float64), 1e-6, 1 - 1e-6)
     arr["opacity"] = np.log(o / (1 - o)).astype(np.float32)
     for c in range(3):

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import abi
 from .camera import GaussianCamera, View
-from .gaussian import PlanarGaussian3d, PlanarGaussian4d, compute_aabb
+from .gaussian import SH_WIDTHS, PlanarGaussian3d, PlanarGaussian4d, compute_aabb
 from .particles import PARTICLE_BEHAVIOR_DTYPE, as_particle_behaviors
 from .settings import CloudSettings, SparseSelect
 
@@ -92,22 +92,24 @@ class PlanarGaussian3dHandle:
         self._lib = plugin._lib
         self.n = len(cloud)
         self.f16 = f16
+        self.sh_degree = cloud.sh_degree        # stored at the cloud's own SH width (the _sh upload calls)
         self.aabb = cloud.compute_aabb()        # the entity's Aabb (calculate_bounds, src/gaussian/cloud.rs:45-62)
         self._h = C.c_void_p()
         self.precompute_covariance = precompute_covariance
+        d = self.sh_degree
         if precompute_covariance:
             # the reference's `precompute_covariance_3d` feature: Covariance3dOpacityPacked128 in the second plane
             sh_p, cov_op = cloud.precomputed_covariance().pack_f16()
-            st = self._lib.bgs_cloud_upload_f16_cov(plugin._ctx, self.n, _ptr(cloud.position_visibility), _ptr(sh_p),
-                                                    _ptr(cov_op), C.byref(self._h))
+            st = self._lib.bgs_cloud_upload_f16_cov_sh(plugin._ctx, self.n, d, _ptr(cloud.position_visibility), _ptr(sh_p),
+                                                       _ptr(cov_op), C.byref(self._h))
         elif f16:
             sh_p, rso = cloud.pack_f16()
-            st = self._lib.bgs_cloud_upload_f16(plugin._ctx, self.n, _ptr(cloud.position_visibility), _ptr(sh_p),
-                                                _ptr(rso), C.byref(self._h))
+            st = self._lib.bgs_cloud_upload_f16_sh(plugin._ctx, self.n, d, _ptr(cloud.position_visibility), _ptr(sh_p),
+                                                   _ptr(rso), C.byref(self._h))
         else:
-            st = self._lib.bgs_cloud_upload_f32(plugin._ctx, self.n, _ptr(cloud.position_visibility),
-                                                _ptr(cloud.spherical_harmonic), _ptr(cloud.rotation),
-                                                _ptr(cloud.scale_opacity), C.byref(self._h))
+            st = self._lib.bgs_cloud_upload_f32_sh(plugin._ctx, self.n, d, _ptr(cloud.position_visibility),
+                                                   _ptr(cloud.spherical_harmonic), _ptr(cloud.rotation),
+                                                   _ptr(cloud.scale_opacity), C.byref(self._h))
         plugin._check(st)
 
     @classmethod
@@ -121,6 +123,9 @@ class PlanarGaussian3dHandle:
         self._plugin, self._lib = plugin, plugin._lib
         self.n, self.f16, self.precompute_covariance = n, f16, precompute_covariance
         self._h = h
+        d = C.c_uint32()
+        plugin._check(plugin._lib.bgs_cloud_sh_degree(h, C.byref(d)))
+        self.sh_degree = int(d.value)
         self.aabb = compute_aabb(plugin.positions(self))
         return self
 
@@ -147,6 +152,7 @@ class PlanarGaussian4dHandle(PlanarGaussian3dHandle):
         self.serial = PlanarGaussian3dHandle._next_serial
         self._plugin, self._lib = plugin, plugin._lib
         self.n, self.f16, self.precompute_covariance = len(cloud), False, False
+        self.sh_degree = 3                      # the spatial degree of the spherindrical colour
         self.aabb = cloud.compute_aabb()
         self._h = C.c_void_p()
         plugin._check(self._lib.bgs_cloud_upload_4d(plugin._ctx, self.n, *(_ptr(a) for a in cloud.planes()), C.byref(self._h)))
@@ -437,20 +443,21 @@ class GaussianSplattingPlugin:
         return type(handle)._adopt(self, out, int(n.value), handle.f16, handle.precompute_covariance)
 
     def download_planes(self, handle: PlanarGaussian3dHandle) -> tuple[np.ndarray, ...]:
-        """The cloud's planes as the matching upload call takes them: f32 (pos_vis, sh, rotation, scale_opacity); f16
-        and precomputed-covariance clouds (pos_vis, sh_packed, second plane words)."""
+        """The cloud's planes as the matching upload call takes them: f32 (pos_vis, sh (n, S_d), rotation,
+        scale_opacity); f16 and precomputed-covariance clouds (pos_vis, sh_packed (n, S_d / 2), second plane words)."""
         pos = np.empty((handle.n, 4), np.float32)
         if getattr(handle, "temporal", False):   # (pos_vis, sh, rotations, scale_opacity, timestamp_timescale)
             planes = (pos, np.empty((handle.n, 144), np.float32), np.empty((handle.n, 8), np.float32),
                       np.empty((handle.n, 4), np.float32), np.empty((handle.n, 4), np.float32))
             self._check(self._lib.bgs_cloud_download_4d(self._ctx, handle._h, *(_ptr(a) for a in planes)))
             return planes
+        width = SH_WIDTHS[handle.sh_degree]
         if handle.f16 or handle.precompute_covariance:
-            sh, second = np.empty((handle.n, 24), np.uint32), np.empty((handle.n, 4), np.uint32)
-            self._check(self._lib.bgs_cloud_download_f16(self._ctx, handle._h, _ptr(pos), _ptr(sh), _ptr(second)))
+            sh, second = np.empty((handle.n, width // 2), np.uint32), np.empty((handle.n, 4), np.uint32)
+            self._check(self._lib.bgs_cloud_download_f16_sh(self._ctx, handle._h, _ptr(pos), _ptr(sh), _ptr(second)))
             return pos, sh, second
-        sh, rot, so = np.empty((handle.n, 48), np.float32), np.empty((handle.n, 4), np.float32), np.empty((handle.n, 4), np.float32)
-        self._check(self._lib.bgs_cloud_download_f32(self._ctx, handle._h, _ptr(pos), _ptr(sh), _ptr(rot), _ptr(so)))
+        sh, rot, so = np.empty((handle.n, width), np.float32), np.empty((handle.n, 4), np.float32), np.empty((handle.n, 4), np.float32)
+        self._check(self._lib.bgs_cloud_download_f32_sh(self._ctx, handle._h, _ptr(pos), _ptr(sh), _ptr(rot), _ptr(so)))
         return pos, sh, rot, so
 
     def download(self, handle: PlanarGaussian3dHandle) -> PlanarGaussian3d:

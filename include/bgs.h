@@ -141,6 +141,44 @@ bgs_status bgs_cloud_upload_f16_cov(bgs_context* ctx, uint32_t n, const float* p
                                     const uint32_t* cov3d_opacity, bgs_cloud** out);
 void bgs_cloud_destroy(bgs_cloud* cloud);
 
+/* Spherical-harmonic degree (the reference's build features sh0 .. sh3, src/material/spherical_harmonics.rs:41-87,
+ * chosen here per cloud at upload).  The calls above store degree 3.  The rule, for d in {0, 1, 2, 3}:
+ *   - K_d = (d + 1)^2 coefficients per channel; the SH plane holds S_d = pad4(3 K_d) floats per gaussian: 4, 12, 28, 48.
+ *     Coefficient k of channel c is sh[3k + c] for k < K_d; lanes 3 K_d .. S_d - 1 are padding (lane 3 at degree 0,
+ *     lane 27 at degree 2; degrees 1 and 3 have none).
+ *   - f16 layouts hold S_d / 2 words per gaussian: 2, 6, 14, 24; the even coefficient in the low half.
+ *   - colour = 0.5 + sum over k < K_d of shc[k] * basis_k(dir) * sh[3k + c] (the bands spherical_harmonics.wgsl:34-68
+ *     keeps for SH_COEFF_COUNT > 11 / > 26 / > 47), then the sRGB decode as at degree 3.  Padding lanes are stored,
+ *     downloaded, subset and interpolated, and never evaluated.  A degree-d cloud therefore renders exactly like the
+ *     same cloud with its coefficients zero-padded to 48 (an FMA with a zero coefficient and a finite basis is exact).
+ *   - Degree 3 is exactly the storage and the kernels of the calls above.
+ * bgs_cloud_upload_f32_sh / _f16_sh / _f16_cov_sh take the arguments of the call without _sh plus sh_degree, and the SH
+ * plane at the degree's width.  bgs_cloud_download_f32_sh / _f16_sh give the planes back at the cloud's width, bit for
+ * bit as uploaded, padding lanes included; the downloads without _sh refuse a cloud of degree < 3.  Every other call
+ * takes a cloud of any degree with unchanged semantics: the render calls in every geometry, mode, format and flag,
+ * bgs_cloud_subset (the new cloud keeps the degree), selection, visibility, positions, particle steps, and
+ * bgs_cloud_interpolate (over all S_d lanes or S_d / 2 words; lhs, rhs and out must share the degree).
+ * bgs_cloud_sh_degree: the cloud's degree (3 for clouds of the calls without _sh, and for Gaussian4d clouds, whose
+ * spatial degree it is).
+ * sh_degree > 3, a null out for bgs_cloud_sh_degree, an _sh download of a cloud of the other precision or of a 4D
+ * cloud, or an interpolation of clouds of different degrees -> BGS_EINVAL, with nothing allocated or enqueued.
+ * Block sizes per gaussian (resident, besides the 16 B position plane): f32 64 / 128 / 256 / 256 B and f16 64 / 64 /
+ * 128 / 128 B for degrees 0 / 1 / 2 / 3. */
+bgs_status bgs_cloud_upload_f32_sh(bgs_context* ctx, uint32_t n, uint32_t sh_degree, const float* pos_vis,
+                                   const float* sh /* n * S_d */, const float* rot_wxyz, const float* scale_opacity,
+                                   bgs_cloud** out);
+bgs_status bgs_cloud_upload_f16_sh(bgs_context* ctx, uint32_t n, uint32_t sh_degree, const float* pos_vis,
+                                   const uint32_t* sh_packed /* n * S_d / 2 */, const uint32_t* rot_scale_opacity,
+                                   bgs_cloud** out);
+bgs_status bgs_cloud_upload_f16_cov_sh(bgs_context* ctx, uint32_t n, uint32_t sh_degree, const float* pos_vis,
+                                       const uint32_t* sh_packed /* n * S_d / 2 */, const uint32_t* cov3d_opacity,
+                                       bgs_cloud** out);
+bgs_status bgs_cloud_download_f32_sh(bgs_context* ctx, const bgs_cloud* cloud, float* pos_vis /* n*4 */,
+                                     float* sh /* n * S_d */, float* rot_wxyz /* n*4 */, float* scale_opacity /* n*4 */);
+bgs_status bgs_cloud_download_f16_sh(bgs_context* ctx, const bgs_cloud* cloud, float* pos_vis /* n*4 */,
+                                     uint32_t* sh_packed /* n * S_d / 2 */, uint32_t* second_plane /* n*4 */);
+bgs_status bgs_cloud_sh_degree(const bgs_cloud* cloud, uint32_t* out);
+
 /* Selection edits of a resident cloud: the visibility lane (pos_vis[4i + 3]) that DrawMode::Selected and
  * HighlightSelected read, changed in place without a re-upload.  All three calls are synchronous.
  *
@@ -234,7 +272,7 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* ctx, bgs_cloud* cloud, const fl
  *   for bit.  For f16 clouds second_plane is the packed rotation-scale-opacity words, or the Covariance3dOpacityPacked128
  *   words of a precomputed-covariance cloud.  The planes go in chunks of 2^17 gaussians through device staging
  *   and two pinned host buffers the context keeps (2 x 30 MB, from its first download on).  The call of the other
- *   layout -> BGS_EINVAL.
+ *   layout, or of a cloud of SH degree < 3 (bgs_cloud_download_f32_sh / _f16_sh read those) -> BGS_EINVAL.
  * Ordering: both calls only read the source and are synchronous.  They wait on the device for the particle steps
  * queued on the cloud (as bgs_cloud_visibility_get does) and do not drain other contexts' queued frames.  Their
  * scratch is their own: the bgs_debug_* hooks, bgs_frame_stats_get and bgs_stage_times_us keep reporting the last
@@ -330,7 +368,7 @@ bgs_status bgs_cloud_positions_get(bgs_context* ctx, const bgs_cloud* cloud, flo
  *     quotient of -0 stays -0 (time == time_start with d < 0; WGSL does not pin the sign of a zero max);
  *   - every lane of gaussian i is mix(a, b, t) = a*(1-t) + b*t, a from lhs, b from rhs, 1-t rounded once; every
  *     operation f32 round-to-nearest-even without FMA, subnormals kept.  The lanes: position xyz and visibility (both
- *     device copies: the position plane and the block), the 48 SH coefficients, scale xyz and opacity, or for the
+ *     device copies: the position plane and the block), the S_d SH lanes (48 at degree 3), scale xyz and opacity, or for the
  *     precomputed-covariance layout the six covariance entries and opacity;
  *   - the rotation is normalize_quaternion(mix(q_l, q_r, t)) (:59-65): l2 = ((q0*q0 + q1*q1) + q2*q2) + q3*q3 in
  *     storage lane order (w, x, y, z); if l2 <= 0 the lanes are (0, 0, 0, 1), i.e. w = 0, z = 1 (a half-turn about z:
@@ -352,13 +390,13 @@ bgs_status bgs_cloud_positions_get(bgs_context* ctx, const bgs_cloud* cloud, flo
  *   completes ctx's queued interpolations; a fault is reported by the next synchronising call on that context.  A
  *   context that never interpolates issues the same launches and waits as before.
  * Where this port deliberately differs from the reference:
- *   1. lhs, rhs and out must hold the same n in the same layout (f32 / f16 / f16 precomputed covariance).  The reference
- *      sizes the output as a clone of lhs and indexes rhs unguarded.
+ *   1. lhs, rhs and out must hold the same n in the same layout (f32 / f16 / f16 precomputed covariance) and SH
+ *      degree.  The reference sizes the output as a clone of lhs and indexes rhs unguarded.
  *   2. out may not be lhs or rhs (in the reference it is always a separate asset).
  *   3. The caller interpolates explicitly, once; the reference runs the pass once per camera view
  *      (interpolate.rs:388-475), with the same inputs and so the same result.
  *   4. The entity's Aabb is not updated, as for the particle step: RasterizeMode::Position reads the caller's.
- * A null argument, a cloud on another device than the context's, a mismatch of n or layout, out == lhs or rhs, a
+ * A null argument, a cloud on another device than the context's, a mismatch of n, layout or SH degree, out == lhs or rhs, a
  * time, time_start or time_stop that is not finite, or a NaN factor (e.g. (3e38 - -3e38) / inf) -> BGS_EINVAL; a
  * refused call changes and enqueues nothing. */
 bgs_status bgs_cloud_interpolate(bgs_context* ctx, bgs_cloud* out, const bgs_cloud* lhs, const bgs_cloud* rhs, float time,

@@ -82,11 +82,15 @@ struct PlanarGaussian4d {   // five planes, binding order (planar_4d.rs:38-51); 
     size_t len() const { return position_visibility.size() / 4; }
 };
 
+// SH degree d (bgs.h): S_d floats per gaussian in the SH plane
+inline size_t sh_width(uint32_t sh_degree) { return sh_degree == 0 ? 4 : sh_degree == 1 ? 12 : sh_degree == 2 ? 28 : 48; }
+
 struct PlanarGaussian3d {   // four planes, binding order (planar_3d.rs:45-54)
     std::vector<float> position_visibility;   // n*4
-    std::vector<float> spherical_harmonic;    // n*48, sh[3k + c]
+    std::vector<float> spherical_harmonic;    // n*S_d, sh[3k + c] (S_d = sh_width(sh_degree))
     std::vector<float> rotation;              // n*4, (w, x, y, z)
     std::vector<float> scale_opacity;         // n*4
+    uint32_t sh_degree = 3;                   // 0..3
     size_t len() const { return position_visibility.size() / 4; }
     // the entity Aabb's min()/max(): compute_aabb (interface.rs:22-66, positions +- 0.1) -> Aabb {center, half_extents}
     // (cloud.rs:45-62) -> center -+ half_extents (render/mod.rs:1070-1071), all in f32
@@ -247,12 +251,14 @@ public:
     GaussianSplattingPlugin& operator=(const GaussianSplattingPlugin&) = delete;
     ~GaussianSplattingPlugin() { bgs_context_destroy(ctx_); }
 
-    PlanarGaussian3dHandle add_cloud(const PlanarGaussian3d& c) {   // asset prepare
+    PlanarGaussian3dHandle add_cloud(const PlanarGaussian3d& c) {   // asset prepare, at the cloud's SH degree
+        if (c.sh_degree > 3 || c.spherical_harmonic.size() != c.len() * sh_width(c.sh_degree))
+            throw Error(BGS_EINVAL, "add_cloud: spherical_harmonic must hold sh_width(sh_degree) floats per gaussian");
         PlanarGaussian3dHandle h;
         h.n_ = (uint32_t)c.len();
         c.compute_aabb(h.aabb_min_, h.aabb_max_);
-        check(bgs_cloud_upload_f32(ctx_, h.n_, c.position_visibility.data(), c.spherical_harmonic.data(), c.rotation.data(),
-                                   c.scale_opacity.data(), &h.h_));
+        check(bgs_cloud_upload_f32_sh(ctx_, h.n_, c.sh_degree, c.position_visibility.data(), c.spherical_harmonic.data(),
+                                      c.rotation.data(), c.scale_opacity.data(), &h.h_));
         return h;
     }
     PlanarGaussian4dHandle add_cloud(const PlanarGaussian4d& c) {
@@ -437,13 +443,15 @@ public:
         }
         return h;
     }
-    // The cloud's four planes (bgs_cloud_download_f32: this host uploads f32 clouds only).
+    // The cloud's four planes at its SH degree (bgs_cloud_download_f32_sh: this host uploads f32 clouds only).
     PlanarGaussian3d download(const PlanarGaussian3dHandle& cloud) {
         const size_t n = cloud.len();
         PlanarGaussian3d c;
-        c.position_visibility.resize(n * 4); c.spherical_harmonic.resize(n * 48); c.rotation.resize(n * 4); c.scale_opacity.resize(n * 4);
-        check(bgs_cloud_download_f32(ctx_, cloud.get(), c.position_visibility.data(), c.spherical_harmonic.data(), c.rotation.data(),
-                                     c.scale_opacity.data()));
+        check(bgs_cloud_sh_degree(cloud.get(), &c.sh_degree));
+        c.position_visibility.resize(n * 4); c.spherical_harmonic.resize(n * sh_width(c.sh_degree)); c.rotation.resize(n * 4);
+        c.scale_opacity.resize(n * 4);
+        check(bgs_cloud_download_f32_sh(ctx_, cloud.get(), c.position_visibility.data(), c.spherical_harmonic.data(),
+                                        c.rotation.data(), c.scale_opacity.data()));
         return c;
     }
     // The reference's save_selection: the selected gaussians written to `path` as .gcloud (bgs::io::encode_gcloud, defined

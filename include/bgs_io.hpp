@@ -6,6 +6,8 @@
 //     * opacity = sigmoid(raw)                                          ply.rs:40-42
 //     * f_rest_i -> channel i / 16 (not / 15), coefficient (i % 15) + 1, interleaved index coefficient * 3 + channel,
 //       dropped when >= 48; later properties overwrite earlier ones       ply.rs:49-69
+//       (at SH degree d, the reference's sh_d build: K = (d + 1)^2, channel i / K, coefficient 1 if K == 1 else
+//       (i % (K - 1)) + 1, dropped when coefficient * 3 + channel >= S_d)
 //     * scale_i = exp(clamp(raw_i, mean(raw) -+ 4))                      ply.rs:103-116
 //     * rotation normalised                                              ply.rs:118-124
 //     * padded with default gaussians by 32 - (n % 32) entries           ply.rs:127-129
@@ -54,8 +56,10 @@ inline float load_f32(const unsigned char* p, bool big_endian) {
 }
 }  // namespace detail
 
-inline PlanarGaussian3d parse_ply_3d(std::istream& in) {
+inline PlanarGaussian3d parse_ply_3d(std::istream& in, uint32_t sh_degree = 3) {
     using namespace detail;
+    if (sh_degree > 3) throw std::runtime_error("ply: sh_degree must be 0..3");
+    const size_t S = sh_width(sh_degree), K = (size_t)(sh_degree + 1) * (sh_degree + 1);
     std::string line;
     if (!std::getline(in, line) || line.substr(0, 3) != "ply") throw std::runtime_error("not a PLY file");
     std::string format;
@@ -147,10 +151,11 @@ inline PlanarGaussian3d parse_ply_3d(std::istream& in) {
         }
     }
     PlanarGaussian3d out;
+    out.sh_degree = sh_degree;
     if (!have_vertex) return out;
     const size_t pad = 32 - (n % 32), total = n + pad;
     out.position_visibility.assign(total * 4, 0.0f);
-    out.spherical_harmonic.assign(total * 48, 0.0f);
+    out.spherical_harmonic.assign(total * S, 0.0f);
     out.rotation.assign(total * 4, 0.0f);
     out.scale_opacity.assign(total * 4, 0.0f);
     for (size_t i = 0; i < total; ++i) out.position_visibility[4 * i + 3] = 1.0f;   // PositionVisibility::default
@@ -162,9 +167,9 @@ inline PlanarGaussian3d parse_ply_3d(std::istream& in) {
         else if (key == "y") put(out.position_visibility, 4, 1);
         else if (key == "z") put(out.position_visibility, 4, 2);
         else if (key == "visibility") put(out.position_visibility, 4, 3);
-        else if (key == "f_dc_0") put(out.spherical_harmonic, 48, 0);
-        else if (key == "f_dc_1") put(out.spherical_harmonic, 48, 1);
-        else if (key == "f_dc_2") put(out.spherical_harmonic, 48, 2);
+        else if (key == "f_dc_0") put(out.spherical_harmonic, S, 0);
+        else if (key == "f_dc_1") put(out.spherical_harmonic, S, 1);
+        else if (key == "f_dc_2") put(out.spherical_harmonic, S, 2);
         else if (key == "scale_0") put(out.scale_opacity, 4, 0);
         else if (key == "scale_1") put(out.scale_opacity, 4, 1);
         else if (key == "scale_2") put(out.scale_opacity, 4, 2);
@@ -180,8 +185,8 @@ inline PlanarGaussian3d parse_ply_3d(std::istream& in) {
             for (const char* q = dig; *q; ++q)
                 if (*q < '0' || *q > '9') throw std::runtime_error("ply: bad property name " + key);
             const unsigned long i = std::strtoul(dig, nullptr, 10);
-            const unsigned long channel = i / 16, coefficient = (i % 15) + 1, idx = coefficient * 3 + channel;
-            if (idx < 48) put(out.spherical_harmonic, 48, (size_t)idx);
+            const unsigned long channel = i / K, coefficient = K == 1 ? 1 : (i % (K - 1)) + 1, idx = coefficient * 3 + channel;
+            if (idx < S) put(out.spherical_harmonic, S, (size_t)idx);
         }
     }
     for (size_t i = 0; i < n; ++i) {
@@ -322,9 +327,16 @@ struct Builder {
 inline PlanarGaussian3d decode_gcloud(const unsigned char* data, size_t len) {
     const flex::Ref r = flex::root(data, len);
     PlanarGaussian3d out;
+    // the SH degree the file was written at, from the first coefficient tuple's length (4, 12, 28 or 48)
+    const flex::Ref shv = r.get("spherical_harmonic");
+    if (shv.is_vector() && shv.size() > 0) {
+        const size_t w = shv.at(0).get("coefficients").size();
+        out.sh_degree = w == 4 ? 0 : w == 12 ? 1 : w == 28 ? 2 : w == 48 ? 3 : 4;
+        if (out.sh_degree > 3) throw std::runtime_error("gcloud: coefficients hold 4, 12, 28 or 48 floats (SH degree 0..3)");
+    }
     struct Plane { const char* name; std::vector<float>* dst; const char* f0; size_t w0; const char* f1; };
     const Plane planes[4] = {{"position_visibility", &out.position_visibility, "position", 3, "visibility"},
-                             {"spherical_harmonic", &out.spherical_harmonic, "coefficients", 48, nullptr},
+                             {"spherical_harmonic", &out.spherical_harmonic, "coefficients", sh_width(out.sh_degree), nullptr},
                              {"rotation", &out.rotation, "rotation", 4, nullptr},
                              {"scale_opacity", &out.scale_opacity, "scale", 3, "opacity"}};
     size_t n = 0;
@@ -346,17 +358,18 @@ inline PlanarGaussian3d decode_gcloud(const unsigned char* data, size_t len) {
 inline PlanarGaussian3d decode_gcloud(const std::vector<unsigned char>& bytes) { return decode_gcloud(bytes.data(), bytes.size()); }
 
 // CloudCodec::encode (src/io/gcloud/flexbuffers.rs:9-16): struct -> map keyed by field name (keys sorted), Vec / array ->
-// vector; 2..4 floats use the fixed-length typed vector, 48 a length-prefixed VECTOR_FLOAT.
+// vector; 2..4 floats use the fixed-length typed vector, more a length-prefixed VECTOR_FLOAT.  The SH tuple is the
+// cloud's S_d.
 inline std::vector<unsigned char> encode_gcloud(const PlanarGaussian3d& c) {
     using namespace flex;
     Builder b;
-    const size_t n = c.len();
+    const size_t n = c.len(), S = sh_width(c.sh_degree);
     struct Field { const char* name; size_t col, w; };
     struct Plane { const char* name; const std::vector<float>* src; size_t stride; std::vector<Field> fields; };   // fields sorted by name
     const Plane planes[4] = {{"position_visibility", &c.position_visibility, 4, {{"position", 0, 3}, {"visibility", 3, 1}}},
                              {"rotation", &c.rotation, 4, {{"rotation", 0, 4}}},
                              {"scale_opacity", &c.scale_opacity, 4, {{"opacity", 3, 1}, {"scale", 0, 3}}},
-                             {"spherical_harmonic", &c.spherical_harmonic, 48, {{"coefficients", 0, 48}}}};     // (sorted by name)
+                             {"spherical_harmonic", &c.spherical_harmonic, S, {{"coefficients", 0, S}}}};     // (sorted by name)
     size_t plane_pos[4]; unsigned plane_type[4];
     // gcloud.py encodes the planes in struct order (position_visibility, spherical_harmonic, rotation, scale_opacity)
     const int order[4] = {0, 3, 1, 2};
