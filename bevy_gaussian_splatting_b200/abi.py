@@ -22,6 +22,7 @@ BGS_FLAG_NO_CHUNKS = 4
 BGS_FLAG_CHUNKS = 8
 BGS_FLAG_PREMULTIPLIED_OUT = 16
 BGS_FLAG_BLEND_OVER_TARGET = 32
+BGS_SCENE_MAX_CLOUDS = 64
 BGS_SELECT_REPLACE, BGS_SELECT_ADD = 0, 1
 
 
@@ -139,6 +140,8 @@ SYMBOLS = [
     ("bgs_render_4d", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings),
                                 C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int, C.c_float,
                                 C.c_float]),
+    ("bgs_render_scene", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
+                                   C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,
                                  C.c_uint32, C.c_int]),
     ("bgs_sync", C.c_int, [_P]),

@@ -273,7 +273,8 @@ bgs_status bgs_context_create(int cuda_device, bgs_context** out) {
         c->kg_grid_async = (uint32_t)(c->sm_count * std::min(kb, COOP_CTAS_PER_SM_ASYNC));
         c->bin_grid_async = (uint32_t)(c->sm_count * std::min(bb, COOP_CTAS_PER_SM_ASYNC));
         c->rs_per_sm = radix_coop_blocks_per_sm(16);
-        if (c->kg_grid == 0 || c->bin_grid == 0 || c->rs_per_sm == 0) coop = 0;
+        c->kg_scene_per_sm = (uint32_t)keygen_scene_blocks_per_sm();
+        if (c->kg_grid == 0 || c->bin_grid == 0 || c->rs_per_sm == 0 || c->kg_scene_per_sm == 0) coop = 0;
     }
     if (e == cudaSuccess && !coop) {
         snprintf(c->err, sizeof(c->err), "device %d cannot co-schedule the cooperative kernels (an sm_90a GPU such as the H100 is required)", cuda_device);
@@ -450,20 +451,32 @@ static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, co
     return fc;
 }
 
-// Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.
+// Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.  A scene frame
+// (bgs_render_scene) runs key-gen, the depth range, the projection and the splat depths over its segment table; `cloud`
+// is then its first cloud and fc its first segment's.
 static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const ModeConsts* modes,
-                                const TemporalConsts* tc, const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd) {
-    const uint32_t n = cloud->n;
+                                const TemporalConsts* tc, const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd,
+                                const std::shared_ptr<const SceneFacts>& scene) {
+    const uint32_t n = scene ? scene->tab.n_total : cloud->n;
     const uint32_t num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     cudaStream_t q = c->stream;
     uint32_t launches = 0;
-    TRY(before_cloud_read(c, cloud));
+    if (scene) {
+        const std::vector<const bgs_cloud*>& cl = scene->clouds;
+        for (size_t j = 0; j < cl.size(); ++j)
+            if (std::find(cl.begin(), cl.begin() + j, cl[j]) == cl.begin() + j) TRY(before_cloud_read(c, cl[j]));
+    } else {
+        TRY(before_cloud_read(c, cloud));
+    }
     CU(c, cudaMemsetAsync(c->arena.p, 0, c->arena.bytes, q));   // counters, histograms, ranges: ~0.4 MB
     CU(c, cudaEventRecord(c->ev[0], q));
     // ---- stage 1: key-gen (+ stable compaction of the visible set)
     // compact mode: keys[0][slot], slot_ids[slot] = gaussian index, vals[0][slot] = slot (sort payload)
     // SORT_ALL    : keys[0][i], vals[0][i] = i (payload is the gaussian index itself)
-    if (p.by_slot) {
+    if (scene) {   // (scenes are compact frames)
+        CU(c, launch_keygen_scene(scene->tab, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt, c->ctr,
+                                  c->hist, p.depth_passes, std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
+    } else if (p.by_slot) {
         // the cooperative key-gen also produces the depth sort's digit histograms
         // (keys[1] = visibility-mask scratch until the sort's first pass overwrites it)
         CU(c, launch_keygen_coop(cloud->pos, n, fc, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt,
@@ -489,11 +502,18 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     const cudaStream_t ps = p.overlap ? c->stream2 : q;
     if (p.overlap) CU(c, cudaStreamWaitEvent(c->stream2, c->ev_fork, 0));
     if (p.depth_range) {
-        launch_depth_range(cloud->pos, n, c->vals[cur].p, p.by_slot ? c->slot_ids.p : nullptr, c->ctr, fc, q);
+        if (scene) launch_depth_range_scene(scene->tab, c->vals[cur].p, c->slot_ids.p, c->ctr, q);
+        else launch_depth_range(cloud->pos, n, c->vals[cur].p, p.by_slot ? c->slot_ids.p : nullptr, c->ctr, fc, q);
         ++launches;
     }
     CU(c, cudaEventRecord(c->ev_p0, ps));
-    if (tc) {   // Gaussian4d: the projection also writes the depth-tested frame's splat depths, from the moved positions
+    if (scene) {   // one launch per projection kernel the scene's clouds need
+        for (const uint32_t g : scene->groups) {
+            launch_project_scene(scene->tab, g, c->slot_ids.p, c->ctr, c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint,
+                                 c->sm_count, c->cutoff_tab, modes, ps);
+            ++launches;
+        }
+    } else if (tc) {   // Gaussian4d: the projection also writes the depth-tested frame's splat depths, from the moved positions
         launch_project_4d(cloud->blocks, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
                           modes ? *modes : ModeConsts{}, *tc, c->recs.p, zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
     } else {
@@ -501,11 +521,14 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
                        p.by_slot ? 1 : 0, c->ctr, fc, c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab,
                        fc.aux ? c->aux.p : nullptr, modes, ps);
     }
-    ++launches;
+    if (!scene) ++launches;
     CU(c, cudaEventRecord(c->ev_p1, ps));
     // depth-tested frames: the splat depths, indexed like the records (the projection's index list)
     ZTestArgs zt;
-    if (zd && !tc) {
+    if (zd && scene) {
+        launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
+        ++launches;
+    } else if (zd && !tc) {
         launch_splat_depth(cloud->pos, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
                            c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
@@ -575,7 +598,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaMemcpyAsync(o.host_normal, o.normal, o.bytes, cudaMemcpyDeviceToHost, q));
         }
     }
-    c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, fc.tiles_x, fc.tiles_y, fc.Wi, fc.Hi, o.rgba, zd != nullptr};
+    c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, fc.tiles_x, fc.tiles_y, fc.Wi, fc.Hi, o.rgba, zd != nullptr, scene};
     c->launches = launches;
     return BGS_OK;
 }
@@ -602,7 +625,8 @@ static bgs_status check_scene_depth(bgs_context* c, const bgs_scene_depth* zd, c
 static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                               const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
                               int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal,
-                              const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr) {
+                              const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr,
+                              const std::shared_ptr<const SceneFacts>& scene = nullptr) {
     if (!c) return BGS_EINVAL;
     TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));
     if (zd) TRY(check_scene_depth(c, zd, view));
@@ -611,13 +635,13 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         // pair list = BGS_NOT_READY) is the caller's to see, so this frame is not rendered on top of it
         TRY(bgs_sync(c));
     }
-    const FrameConsts fc = frame_consts(cloud, view, uni, st, want_aux);
+    const FrameConsts fc = scene ? scene->tab.seg[0].fc : frame_consts(cloud, view, uni, st, want_aux);
     // Classification / OpticalFlow: project_modes_kernel with the extras (NULL extras: num_classes = 1)
     ModeConsts mc = {};
     mc.num_classes = ex ? ex->num_classes : 1u;
     if (ex) { memcpy(mc.prev_clip_from_world, ex->previous_clip_from_world, 64); mc.delta_time = ex->delta_time; }
     const ModeConsts* modes = st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION ? &mc : nullptr;
-    const uint32_t n = cloud->n, num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
+    const uint32_t n = scene ? scene->tab.n_total : cloud->n, num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
     FrameOut o;
@@ -632,7 +656,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         TRY(ensure_arena(c, num_tiles));
         TRY(ensure_status(c, c->status_depth, c->status_n, n));
         TRY(ensure_status(c, c->status_pairs, c->status_np, c->cap_pairs));
-        TRY(enqueue_frame(c, cloud, fc, modes, tc, p, o, zd));
+        TRY(enqueue_frame(c, cloud, fc, modes, tc, p, o, zd, scene));
         if (st->flags & BGS_FLAG_ASYNC) {
             c->async_pending = true;
             c->have_frame = false;     // hooks need bgs_sync() first
@@ -677,6 +701,45 @@ bgs_status bgs_render_4d(bgs_context* c, const bgs_cloud* cloud, const bgs_view*
     return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth, &tc);
 }
 
+bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis, uint32_t k,
+                            const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                            void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    if (!c) return BGS_EINVAL;
+    if (!clouds || !unis || !view || !st) return fail(c, BGS_NOT_READY, "render_scene: clouds/uniforms/view/settings not ready");
+    if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "render_scene: k = %u is not in 1..%d", k, BGS_SCENE_MAX_CLOUDS);
+    if (st->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "render_scene: BGS_FLAG_SORT_ALL is not supported");
+    uint64_t total = 0;
+    for (uint32_t j = 0; j < k; ++j) {
+        if (!clouds[j]) return fail(c, BGS_EINVAL, "render_scene: clouds[%u] is NULL", j);
+        TRY(check_render(c, clouds[j], view, &unis[j], st, ex, out_format, false, false));   // (refuses 4D clouds, other devices)
+        total += clouds[j]->n;
+    }
+    if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "render_scene: N = %llu gaussians, must be < 2^30", (unsigned long long)total);
+    if (depth) TRY(check_scene_depth(c, depth, view));
+    auto scene = std::make_shared<SceneFacts>();
+    SceneTable& tab = scene->tab;
+    memset(&tab, 0, sizeof(tab));
+    tab.k = k;
+    tab.n_total = (uint32_t)total;
+    uint32_t offset = 0;
+    for (uint32_t j = 0; j < k; ++j) {
+        const bgs_cloud* cl = clouds[j];
+        SceneSeg& sg = tab.seg[j];
+        sg.fc = frame_consts(cl, view, &unis[j], st, false);
+        sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
+        sg.pos = cl->pos;
+        sg.blocks = cl->blocks;
+        sg.offset = offset;
+        sg.n = cl->n;
+        sg.group = project_group(cl->layout, cl->sh_degree);
+        offset += cl->n;
+        scene->clouds.push_back(cl);
+        if (std::find(scene->groups.begin(), scene->groups.end(), sg.group) == scene->groups.end()) scene->groups.push_back(sg.group);
+    }
+    return render_impl(c, clouds[0], view, &unis[0], st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth,
+                       nullptr, scene);
+}
+
 bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                       const bgs_settings* st, void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
     return bgs_render_ex(c, cloud, view, uni, st, nullptr, out_rgba, out_format, out_is_device_ptr);
@@ -694,7 +757,7 @@ bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {
     if (!c || !out) return BGS_EINVAL;
     if (!c->have_frame || !c->last.cloud) return fail(c, BGS_NOT_READY, "no frame rendered yet");
     CU(c, cudaSetDevice(c->device));
-    const uint32_t n = c->last.cloud->n, n_vis = c->stats.n_visible;
+    const uint32_t n = c->last.n, n_vis = c->stats.n_visible;
     const uint32_t n_sorted = c->last.sort_all ? n : n_vis;
     std::vector<uint32_t> k(n_sorted), v(n_sorted);
     CU(c, cudaMemcpy(k.data(), c->keys[c->depth_result].p, (size_t)n_sorted * 4, cudaMemcpyDeviceToHost));
@@ -709,7 +772,8 @@ bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {
         // culled tail: key = all-ones >> shift, indices ascending (what a stable sort leaves there)
         uint32_t* flags = nullptr;
         CU(c, cudaMalloc(&flags, (size_t)n * 4));
-        launch_culled_flags(c->last.cloud->pos, n, c->last.fc, flags, c->stream);
+        if (c->last.scene) launch_culled_flags_scene(c->last.scene->tab, flags, c->stream);
+        else launch_culled_flags(c->last.cloud->pos, n, c->last.fc, flags, c->stream);
         std::vector<uint32_t> f(n);
         cudaError_t e = cudaMemcpyAsync(f.data(), flags, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);

@@ -158,10 +158,10 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
         for (bgs_context* c : g_contexts) {
             if (c->device == cl->device && c->reads_pending.load(std::memory_order_relaxed))
                 c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
-            if (c->pend.cloud == cl || c->last.cloud == cl) {
-                if (c->async_pending || c->pend.cloud == cl) c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
-                if (c->pend.cloud == cl) { c->pend.cloud = nullptr; c->pend.n = 0; }
-                if (c->last.cloud == cl) { c->last.cloud = nullptr; c->have_frame = false; }
+            if (c->pend.reads(cl) || c->last.reads(cl)) {
+                if (c->async_pending || c->pend.reads(cl)) c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
+                if (c->pend.reads(cl)) { c->pend.forget(); c->pend.n = 0; }
+                if (c->last.reads(cl)) { c->last.forget(); c->have_frame = false; }
             }
         }
     }

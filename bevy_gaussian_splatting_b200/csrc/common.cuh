@@ -33,6 +33,37 @@ struct FrameConsts {
     uint32_t aux;               // bgs_render_aux: the projection also emits the Depth and Normal colour sources
 };
 
+// bgs_render_scene's segment table.  Segment j holds cloud j's gaussians at global indices [offset, offset + n); its
+// FrameConsts carry the frame-wide values and cloud j's uniform and layout (n_cloud is the scene's N).  The scene
+// kernels take it by value: 64 segments are ~22 KB of kernel parameters (CUDA >= 12.1 allows 32 KB on sm_90), so a
+// queued frame's table lives in its own launches and no later frame can overwrite it.
+struct SceneSeg {
+    FrameConsts fc;
+    const float4* pos;          // the cloud's position plane and blocks (cloud_layout.cuh)
+    const void* blocks;
+    uint32_t offset, n;
+    uint32_t group;             // the projection launch the segment belongs to (api.cu: one per kernel instantiation)
+};
+struct SceneTable {
+    uint32_t k;                 // segments, 1 .. BGS_SCENE_MAX_CLOUDS
+    uint32_t n_total;           // N = sum of n
+    SceneSeg seg[BGS_SCENE_MAX_CLOUDS];
+    // the segment of global index g < N: the last j with offset <= g (empty segments share their successor's offset)
+    __device__ __forceinline__ uint32_t find(uint32_t g) const {
+        uint32_t lo = 0u, hi = k;
+        while (hi - lo > 1u) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (seg[mid].offset <= g) lo = mid; else hi = mid;
+        }
+        return lo;
+    }
+    // find() for a g that only grows from one call to the next (j: the previous answer)
+    __device__ __forceinline__ uint32_t advance(uint32_t j, uint32_t g) const {
+        while (j + 1u < k && seg[j + 1u].offset <= g) ++j;
+        return j;
+    }
+};
+
 // bgs_render_extras as the Classification / OpticalFlow projection reads it.  Only project_modes_kernel takes it (as an
 // argument of its own), so the arguments and code of every other kernel stay what they were.
 struct ModeConsts {

@@ -3,6 +3,7 @@
 // the order of a cloud's accesses, and the frame scratch that the selections borrow.
 #pragma once
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -61,11 +62,19 @@ struct bgs_particles {
     cudaEvent_t ev_write = nullptr;   // the last step of these behaviours (recorded on the stepping context's stream)
 };
 
+// A bgs_render_scene frame: its segment table (what its kernels and the culled-flags hook read), the clouds it lists
+// (clouds[j] is segment j's; a cloud may be listed more than once) and its distinct projection groups
+struct SceneFacts {
+    SceneTable tab;
+    std::vector<const bgs_cloud*> clouds;
+    std::vector<uint32_t> groups;
+};
+
 // What the host knows of a frame it has enqueued: the context keeps the last one enqueued (`pend`) and, once its
 // counters are back, the last one completed (`last`, what the debug hooks read).
 struct FrameFacts {
-    const bgs_cloud* cloud = nullptr;   // (nulled if the cloud is destroyed meanwhile)
-    uint32_t n = 0;                     // gaussians in the cloud (a snapshot: the cloud may be gone by the time it is read)
+    const bgs_cloud* cloud = nullptr;   // (nulled if the cloud is destroyed meanwhile; a scene frame's first cloud)
+    uint32_t n = 0;                     // gaussians in the cloud, or the scene's N (a snapshot: the cloud may be gone by the time it is read)
     FrameConsts fc = {};
     bool sort_all = false;
     bool by_slot = false;               // records indexed by compact slot (else by front-to-back rank)
@@ -73,6 +82,15 @@ struct FrameFacts {
     int tiles_x = 0, tiles_y = 0, W = 0, H = 0;
     const void* target = nullptr;       // the device frame the blend wrote
     bool depth_tested = false;          // bgs_render_depth_test with a depth buffer: splat_depth holds the splats' d
+    std::shared_ptr<const SceneFacts> scene;   // bgs_render_scene frames only (nulled with `cloud`)
+    bool reads(const bgs_cloud* cl) const {
+        if (cloud == cl) return true;
+        if (scene)
+            for (const bgs_cloud* s : scene->clouds)
+                if (s == cl) return true;
+        return false;
+    }
+    void forget() { cloud = nullptr; scene.reset(); }
 };
 
 struct bgs_context {
@@ -83,6 +101,7 @@ struct bgs_context {
                                           // cooperative grid holds its registers while it waits; with several frames in flight
                                           // a smaller grid leaves that room to the other frames' issue-bound blend
     int rs_per_sm = 0;                    // co-resident radix-sort CTAs per SM (radix.cu)
+    uint32_t kg_scene_per_sm = 0;         // co-resident CTAs per SM of bgs_render_scene's key-gen (keygen.cu)
     uint32_t sort_epoch = 0;              // look-back status epoch: +1 per sort launch (status words never need clearing)
     cudaStream_t stream = nullptr;    // render stream (high priority): everything but the projection
     cudaStream_t stream2 = nullptr;   // projection runs here, beside the depth sort

@@ -52,11 +52,31 @@ keygen_all_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, ui
 constexpr int KG_WORDS_PER_TILE = KG_TILE / 32;    // 64 mask words
 constexpr int KG_CHUNK_WORDS = 1024;               // phase 2 expands 1024 words (32 K gaussians) at a time
 
-__global__ void __launch_bounds__(KG_THREADS)
-keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, uint32_t* __restrict__ masks,
-                   uint32_t* __restrict__ keys_out, uint32_t* __restrict__ ids_out, uint32_t* __restrict__ slots_out,
-                   uint32_t* __restrict__ block_cnt, FrameCounters* __restrict__ ctr, uint32_t* __restrict__ hist,
-                   int hist_passes) {
+//
+// The positions come from a Src: one cloud (OneCloud) or a scene's segment table (SceneSrc), where global index i is
+// gaussian i - offset of its segment and keyed with that segment's FrameConsts.  Src::first / advance give the segment of
+// an index that only grows within a thread (both phases walk their indices upwards).
+struct OneCloud {
+    const float4* pos;
+    const FrameConsts& f;
+    __device__ __forceinline__ uint32_t first(uint32_t) const { return 0u; }
+    __device__ __forceinline__ uint32_t advance(uint32_t j, uint32_t) const { return j; }
+    __device__ __forceinline__ const FrameConsts& fc(uint32_t) const { return f; }
+    __device__ __forceinline__ const float4* at(uint32_t, uint32_t i) const { return pos + i; }
+};
+struct SceneSrc {
+    const SceneTable& t;
+    __device__ __forceinline__ uint32_t first(uint32_t i) const { return t.find(i < t.n_total ? i : t.n_total - 1u); }
+    __device__ __forceinline__ uint32_t advance(uint32_t j, uint32_t i) const { return t.advance(j, i); }
+    __device__ __forceinline__ const FrameConsts& fc(uint32_t j) const { return t.seg[j].fc; }
+    __device__ __forceinline__ const float4* at(uint32_t j, uint32_t i) const { return t.seg[j].pos + (i - t.seg[j].offset); }
+};
+
+template <class Src>
+__device__ __forceinline__ void keygen_coop_body(const Src& src, uint32_t n, const FrameConsts& fc, uint32_t* __restrict__ masks,
+                                                 uint32_t* __restrict__ keys_out, uint32_t* __restrict__ ids_out,
+                                                 uint32_t* __restrict__ slots_out, uint32_t* __restrict__ block_cnt,
+                                                 FrameCounters* __restrict__ ctr, uint32_t* __restrict__ hist, int hist_passes) {
     __shared__ uint32_t s_hist[4 * 256];   // digit histograms of the visible keys (the depth sort's pre-pass, fused)
     __shared__ uint32_t s_red[KG_THREADS / 32];
     __shared__ uint32_t s_total;
@@ -70,24 +90,28 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
     // ---- phase 1: one visibility bit per gaussian of this CTA's range, visible count
     uint32_t mine = 0u;                      // (warp-uniform: every lane counts its warp's ballots)
     uint32_t cmin_inv = 0u, cmax_p1 = 0u;   // Depth mode only: extremes of the culled indices
+    uint32_t sj = src.first(t0 * KG_TILE + warp * (32 * KG_ITEMS) + lane);
     for (uint32_t tile = t0; tile < t1; ++tile) {
         // warp w covers 256 consecutive gaussians of the tile, item j = 32 consecutive ones (coalesced 512 B loads)
         const uint32_t wbase = tile * KG_TILE + warp * (32 * KG_ITEMS);
         float4 p[KG_ITEMS];
+        const uint32_t sj0 = sj;   // (the second loop walks the segments again from here)
 #pragma unroll
         for (int j = 0; j < KG_ITEMS; ++j) {
             const uint32_t i = wbase + j * 32 + lane;
-            p[j] = (i < n) ? __ldcs(pos + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+            if (i < n) sj = src.advance(sj, i);
+            p[j] = (i < n) ? __ldcs(src.at(sj, i)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        uint32_t myword = 0u;
+        uint32_t myword = 0u, sk = sj0;
 #pragma unroll
         for (int j = 0; j < KG_ITEMS; ++j) {
             const uint32_t i = wbase + j * 32 + lane;
             bool v = false;
             if (i < n) {
+                sk = src.advance(sk, i);
                 float pw[4];
-                keygen_world_pos(fc, p[j], pw);
-                v = in_frustum_fast(fc, pw);
+                keygen_world_pos(src.fc(sk), p[j], pw);
+                v = in_frustum_fast(src.fc(sk), pw);
             }
             const uint32_t bal = __ballot_sync(0xffffffffu, v);
             mine += __popc(bal);
@@ -120,6 +144,7 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
     uint32_t run = block_sum_prefix<KG_THREADS>(block_cnt, b, s_red);
     if (b == G - 1 && t == 0) { ctr->n_vis = run + s_total; ctr->n_sort = run + s_total; }
     const uint32_t w_begin = t0 * KG_WORDS_PER_TILE, w_end = t1 * KG_WORDS_PER_TILE;
+    uint32_t ej = src.first(t0 * KG_TILE);
     for (uint32_t wc = w_begin; wc < w_end; wc += KG_CHUNK_WORDS) {
         const uint32_t cw = min((uint32_t)KG_CHUNK_WORDS, w_end - wc);
         // each thread owns 4 consecutive words of the chunk: local prefix, then a block scan of the per-thread sums
@@ -166,9 +191,11 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
             const uint32_t r = e - s_pref[lo];
             const uint32_t bit = __fns(s_mask[lo], 0u, (int)r + 1);
             const uint32_t i = (wc + lo) * 32u + bit;
+            ej = src.advance(ej, i);
+            const FrameConsts& fi = src.fc(ej);
             float pw[4];
-            keygen_world_pos(fc, __ldg(pos + i), pw);
-            const uint32_t key = depth_key(fc, true, cam_dist2(fc, pw));
+            keygen_world_pos(fi, __ldg(src.at(ej, i)), pw);
+            const uint32_t key = depth_key(fi, true, cam_dist2(fi, pw));
             const uint32_t dst = run + e;
             keys_out[dst] = key;
             ids_out[dst] = i;          // compact slot -> gaussian index
@@ -184,6 +211,24 @@ keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, u
     }
 }
 
+__global__ void __launch_bounds__(KG_THREADS)
+keygen_coop_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, uint32_t* __restrict__ masks,
+                   uint32_t* __restrict__ keys_out, uint32_t* __restrict__ ids_out, uint32_t* __restrict__ slots_out,
+                   uint32_t* __restrict__ block_cnt, FrameCounters* __restrict__ ctr, uint32_t* __restrict__ hist,
+                   int hist_passes) {
+    keygen_coop_body(OneCloud{pos, fc}, n, fc, masks, keys_out, ids_out, slots_out, block_cnt, ctr, hist, hist_passes);
+}
+
+// bgs_render_scene: the same over the N global indices of a segment table (ids_out holds global indices).  fc of
+// segment 0 carries the frame-wide values.
+__global__ void __launch_bounds__(KG_THREADS)
+keygen_scene_kernel(SceneTable tab, uint32_t* __restrict__ masks, uint32_t* __restrict__ keys_out,
+                    uint32_t* __restrict__ ids_out, uint32_t* __restrict__ slots_out, uint32_t* __restrict__ block_cnt,
+                    FrameCounters* __restrict__ ctr, uint32_t* __restrict__ hist, int hist_passes) {
+    keygen_coop_body(SceneSrc{tab}, tab.n_total, tab.seg[0].fc, masks, keys_out, ids_out, slots_out, block_cnt, ctr, hist,
+                     hist_passes);
+}
+
 // Debug hook: rebuild the reference's full sorted_entry_buffer (sort/mod.rs:323-329) from the
 // compacted result: [0, n_vis) = sorted visible entries, then every culled index ascending
 // with key 0xFFFFFFFF >> shift.  Single block per call chunk; not on the hot path.
@@ -195,6 +240,16 @@ __global__ void culled_flags_kernel(const float4* __restrict__ pos, uint32_t n, 
     float pw[4], ndc[2];
     mat4_point(fc.model, p.x, p.y, p.z, pw);
     flags[i] = in_frustum(fc, pw, ndc) ? 0u : 1u;
+}
+
+__global__ void culled_flags_scene_kernel(SceneTable tab, uint32_t* __restrict__ flags) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= tab.n_total) return;
+    const SceneSeg& s = tab.seg[tab.find(i)];
+    const float4 p = s.pos[i - s.offset];
+    float pw[4], ndc[2];
+    mat4_point(s.fc.model, p.x, p.y, p.z, pw);
+    flags[i] = in_frustum(s.fc, pw, ndc) ? 0u : 1u;
 }
 
 void launch_keygen_all(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* keys_out, uint32_t* ids_out,
@@ -218,6 +273,23 @@ cudaError_t launch_keygen_coop(const float4* pos, uint32_t n, const FrameConsts&
 
 void launch_culled_flags(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* flags, cudaStream_t stream) {
     culled_flags_kernel<<<(n + 255) / 256, 256, 0, stream>>>(pos, n, fc, flags);
+}
+
+int keygen_scene_blocks_per_sm() {
+    int b = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, keygen_scene_kernel, KG_THREADS, 0) != cudaSuccess) return 0;
+    return b;
+}
+cudaError_t launch_keygen_scene(const SceneTable& tab, uint32_t* masks, uint32_t* keys_out, uint32_t* ids_out,
+                                uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr, uint32_t* hist, int hist_passes,
+                                uint32_t grid, cudaStream_t stream) {
+    void* args[] = {(void*)&tab, (void*)&masks, (void*)&keys_out, (void*)&ids_out, (void*)&slots_out, (void*)&block_cnt,
+                    (void*)&ctr, (void*)&hist, (void*)&hist_passes};
+    return cudaLaunchCooperativeKernel((const void*)keygen_scene_kernel, dim3(grid), dim3(KG_THREADS), args, 0, stream);
+}
+
+void launch_culled_flags_scene(const SceneTable& tab, uint32_t* flags, cudaStream_t stream) {
+    culled_flags_scene_kernel<<<(tab.n_total + 255) / 256, 256, 0, stream>>>(tab, flags);
 }
 
 }  // namespace bgs

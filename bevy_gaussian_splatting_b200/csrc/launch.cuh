@@ -12,6 +12,12 @@ cudaError_t launch_keygen_coop(const float4* pos, uint32_t n, const FrameConsts&
                                uint32_t* ids_out, uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr,
                                uint32_t* hist, int hist_passes, uint32_t grid, cudaStream_t stream);
 void launch_culled_flags(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* flags, cudaStream_t stream);
+// bgs_render_scene's key-gen (one cooperative launch over the segment table's N global indices) and debug flags
+int keygen_scene_blocks_per_sm();
+cudaError_t launch_keygen_scene(const SceneTable& tab, uint32_t* masks, uint32_t* keys_out, uint32_t* ids_out,
+                                uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr, uint32_t* hist, int hist_passes,
+                                uint32_t grid, cudaStream_t stream);
+void launch_culled_flags_scene(const SceneTable& tab, uint32_t* flags, cudaStream_t stream);
 // radix.cu
 uint32_t radix_num_tiles(uint32_t capacity);
 int radix_coop_blocks_per_sm(int items);
@@ -29,6 +35,13 @@ void launch_project(CloudLayout layout, uint32_t sh_degree, const void* blocks, 
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes /* null: project_kernel */,
                     cudaStream_t stream);
 void launch_cutoff_table(float* tab, cudaStream_t stream);
+// bgs_render_scene: the projection of the segments whose project_group is `group` (one launch), and the depth range
+uint32_t project_group(CloudLayout layout, uint32_t sh_degree);
+void launch_project_scene(const SceneTable& tab, uint32_t group, const uint32_t* slot_ids, const FrameCounters* ctr,
+                          SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
+                          const ModeConsts* modes /* null: project_scene_kernel */, cudaStream_t stream);
+void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payload, const uint32_t* slot_ids, FrameCounters* ctr,
+                              cudaStream_t stream);
 // Gaussian4d clouds (bgs_render_4d): records as launch_project's, and the splat depths of depth-tested frames (depths
 // non-null) from the moved positions
 void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
@@ -44,6 +57,8 @@ cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, Fra
 // scene_depth.cu
 void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                         const FrameConsts& fc, float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
+void launch_splat_depth_scene(const SceneTable& tab, const uint32_t* slot_ids, const FrameCounters* ctr, float* depths,
+                              uint32_t n_hint, int sm_count, cudaStream_t stream);
 // raster.cu.  ZTestArgs: a depth-tested frame's splat depths (indexed like the records) and the scene's depth buffer
 // (bgs_scene_depth); scene == nullptr blends without the test.
 struct ZTestArgs {

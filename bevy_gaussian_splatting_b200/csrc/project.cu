@@ -745,6 +745,137 @@ project_modes_kernel(const void* __restrict__ blocks, const uint32_t* __restrict
                               extra, cutoff_tab, nullptr, mc);
 }
 
+// ---- bgs_render_scene: the projection over a segment table (common.cuh).  Record r is compact slot r, whose global
+// index slot_ids[r] lies in segment j: its block is gaussian slot_ids[r] - offset of cloud j's blocks, and project_one
+// runs with segment j's FrameConsts, so the record is the one a frame of cloud j alone would write.  One launch per
+// kernel instantiation (`group`): its warps stride over every slot and project those whose cloud is in the group.
+template <int CH, int NP>
+__device__ __forceinline__ void gather_block_ptrs(const uint4* block /* this lane's entry; null: none */, uint4* stage, int lane) {
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+        const int g = (32 * k + lane) / NP, p = lane % NP;
+        const uint4* src = reinterpret_cast<const uint4*>(
+            __shfl_sync(0xFFFFFFFFu, (unsigned long long)reinterpret_cast<uintptr_t>(block), g));
+        if (src) cp_async16(stage + g * CH + stage_slot<CH>(p, g), src + p);
+    }
+}
+
+template <bool F16, uint32_t D, bool MODES2>
+__device__ __forceinline__ void project_scene_groups(const SceneTable& tab, uint32_t group, const uint32_t* __restrict__ slot_ids,
+                                                     const FrameCounters* __restrict__ ctr, bool need_sh,
+                                                     SplatRec* __restrict__ recs, float4* __restrict__ extra,
+                                                     const float* __restrict__ cutoff_tab, const ModeConsts& mc) {
+    using A = Attr<F16, D>;
+    constexpr int CH = A::CH;
+    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * CH];
+    const int lane = threadIdx.x & 31;
+    uint4* const stage = s_stages[threadIdx.x >> 5];
+    const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
+    constexpr uint32_t NONE = 0xFFFFFFFFu;
+    auto list_id = [&](uint32_t r) { return r < n_vis ? __ldg(slot_ids + r) : NONE; };   // slot r's global index
+    // global index g's block, null when there is none or its cloud is another launch's
+    auto block_of = [&](uint32_t g) -> const uint4* {
+        if (g == NONE) return nullptr;
+        const SceneSeg& s = tab.seg[tab.find(g)];
+        if (s.group != group) return nullptr;
+        return static_cast<const uint4*>(s.blocks) + (size_t)(g - s.offset) * CH;
+    };
+    auto gather = [&](uint32_t g) {   // one commit group per call
+        const uint4* block = block_of(g);
+        if (need_sh) gather_block_ptrs<CH, CH>(block, stage, lane);
+        else gather_block_ptrs<CH, A::GEO>(block, stage, lane);
+        cp_async_commit();
+    };
+    uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
+    uint32_t g_cur = list_id(r0 + lane);
+    gather(g_cur);
+    uint32_t g_next = list_id(r0 + stride + lane);
+    for (; r0 < n_vis; r0 += stride) {
+        cp_async_wait<0>();
+        __syncwarp();   // every lane's copies of this group have landed
+        const uint32_t r = r0 + lane;
+        const uint32_t j = g_cur == NONE ? 0u : tab.find(g_cur);
+        const bool mine = g_cur != NONE && tab.seg[j].group == group;
+        float sh[sh_floats(D)], q[4], so[4];
+        uint32_t op_bits = 0u;
+        float4 p4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (mine) p4 = A::load(stage, lane, sh, q, so, need_sh, op_bits);
+        __syncwarp();   // the stage is read out before the next group's copies overwrite it
+        gather(g_next);
+        g_cur = g_next;
+        g_next = list_id(r0 + 2u * stride + lane);
+        if (mine) project_one<F16, D, MODES2>(tab.seg[j].fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, nullptr, mc);
+    }
+}
+
+// (the f32 blocks of degree 2 and 3 hold 48 SH floats in registers beside the segment's constants: 3 CTAs per SM keeps
+// them from spilling)
+template <bool F16, uint32_t D>
+constexpr int scene_min_ctas() { return !F16 && D >= 2 ? 3 : PROJ_MIN_CTAS; }
+
+template <bool F16, uint32_t D>
+__global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
+project_scene_kernel(SceneTable tab, uint32_t group, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                     SplatRec* __restrict__ recs, float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
+    project_scene_groups<F16, D, false>(tab, group, slot_ids, ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs,
+                                        extra, cutoff_tab, ModeConsts{});
+}
+template <bool F16, uint32_t D>
+__global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
+project_modes_scene_kernel(SceneTable tab, uint32_t group, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
+                           const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs, float4* __restrict__ extra,
+                           const float* __restrict__ cutoff_tab) {
+    project_scene_groups<F16, D, true>(tab, group, slot_ids, ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION,
+                                       recs, extra, cutoff_tab, mc);
+}
+
+// depth_range_kernel over a segment table (compact frames only: bgs_render_scene refuses SORT_ALL)
+__global__ void depth_range_scene_kernel(SceneTable tab, const uint32_t* __restrict__ sorted_payload,
+                                         const uint32_t* __restrict__ slot_ids, FrameCounters* __restrict__ ctr) {
+    const uint32_t n = tab.n_total;
+    if (threadIdx.x != 0 || blockIdx.x != 0 || n < 2u) return;
+    const uint32_t n_vis = ctr->n_vis;
+    const uint32_t cmin = 0xFFFFFFFFu - ctr->culled_min_inv, cmax = ctr->culled_max_p1 - 1u;
+    const uint32_t first = n_vis >= 2u ? slot_ids[sorted_payload[1]] : cmin;
+    const uint32_t last = (n - n_vis) >= 1u ? cmax : slot_ids[sorted_payload[n - 1u]];
+    auto dist = [&](uint32_t g) {
+        const SceneSeg& s = tab.seg[tab.find(g)];
+        const float4 p = s.pos[g - s.offset];
+        float pw[4];
+        mat4_point(s.fc.model, p.x, p.y, p.z, pw);
+        return sqrtf(cam_dist2(s.fc, pw));
+    };
+    ctr->depth_min = dist(last);
+    ctr->depth_max = dist(first);
+}
+
+void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payload, const uint32_t* slot_ids, FrameCounters* ctr,
+                              cudaStream_t stream) {
+    depth_range_scene_kernel<<<1, 32, 0, stream>>>(tab, sorted_payload, slot_ids, ctr);
+}
+
+uint32_t project_group(CloudLayout layout, uint32_t sh_degree) { return (is_f16(layout) ? 1u : 0u) | sh_degree << 1; }
+
+void launch_project_scene(const SceneTable& tab, uint32_t group, const uint32_t* slot_ids, const FrameCounters* ctr,
+                          SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
+                          const ModeConsts* modes, cudaStream_t stream) {
+    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
+    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
+    if (grid < 1u) grid = 1u;
+    with_layout_degree(group & 1u ? CloudLayout::F16 : CloudLayout::F32, group >> 1, [&](auto L, auto Dt) {
+        constexpr CloudLayout Lv = decltype(L)::value;
+        constexpr uint32_t D = decltype(Dt)::value;
+        if constexpr (!is_4d(Lv)) {
+            if (modes)
+                project_modes_scene_kernel<is_f16(Lv), D><<<grid, PROJ_THREADS, 0, stream>>>(tab, group, *modes, slot_ids, ctr, recs,
+                                                                                            extra, cutoff_tab);
+            else
+                project_scene_kernel<is_f16(Lv), D><<<grid, PROJ_THREADS, 0, stream>>>(tab, group, slot_ids, ctr, recs, extra,
+                                                                                      cutoff_tab);
+        }
+    });
+}
+
 // ---- Gaussian4d (bgs_render_4d; the rule is include/bgs.h's).  Matrices [col][row], as WGSL indexes them.
 
 // gaussian_4d.wgsl:37-130: Sigma of the 4D gaussian conditioned on time t

@@ -24,6 +24,21 @@ splat_depth_kernel(const float4* __restrict__ pos, const uint32_t* __restrict__ 
     }
 }
 
+// bgs_render_scene: record r is compact slot r, its global index in segment j (common.cuh)
+__global__ void __launch_bounds__(SD_THREADS)
+splat_depth_scene_kernel(SceneTable tab, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                         float* __restrict__ depths) {
+    const uint32_t n_vis = ctr->n_vis;
+    for (uint32_t r = blockIdx.x * SD_THREADS + threadIdx.x; r < n_vis; r += gridDim.x * SD_THREADS) {
+        const uint32_t g = __ldg(slot_ids + r);
+        const SceneSeg& s = tab.seg[tab.find(g)];
+        const float4 p = __ldg(s.pos + (g - s.offset));
+        float pw[4];
+        mat4_point(s.fc.model, p.x, p.y, p.z, pw);
+        depths[r] = splat_depth(s.fc, pw);
+    }
+}
+
 void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                         const FrameConsts& fc, float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream) {
     // grid-stride over the visible count, which only the device knows: sized by the hint, at most 8 CTAs per SM
@@ -31,6 +46,14 @@ void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_sl
     if (grid > (uint32_t)(8 * sm_count)) grid = (uint32_t)(8 * sm_count);
     if (grid < 1u) grid = 1u;
     splat_depth_kernel<<<grid, SD_THREADS, 0, stream>>>(pos, index_list, by_slot, ctr, fc, depths);
+}
+
+void launch_splat_depth_scene(const SceneTable& tab, const uint32_t* slot_ids, const FrameCounters* ctr, float* depths,
+                              uint32_t n_hint, int sm_count, cudaStream_t stream) {
+    uint32_t grid = (n_hint + SD_THREADS - 1) / SD_THREADS;
+    if (grid > (uint32_t)(8 * sm_count)) grid = (uint32_t)(8 * sm_count);
+    if (grid < 1u) grid = 1u;
+    splat_depth_scene_kernel<<<grid, SD_THREADS, 0, stream>>>(tab, slot_ids, ctr, depths);
 }
 
 }  // namespace bgs

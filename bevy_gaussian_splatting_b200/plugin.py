@@ -187,6 +187,31 @@ class ParticleBehaviorsHandle:
             pass
 
 
+# CloudSettings fields a bgs_render_scene call takes from each entity (into its bgs_cloud_uniform); every other field is
+# the frame's and must agree across the entities
+SCENE_PER_ENTITY_FIELDS = frozenset({"global_opacity", "global_scale", "color_space"})
+
+
+def check_scene_entities(entities) -> CloudSettings:
+    """`entities`: a sequence of (handle, CloudSettings, transform or None), one bgs_render_scene call's clouds.  Returns
+    the settings the frame-wide values come from (the first entity's); raises ValueError when there are none, too many,
+    or two entities disagree on a frame-wide field (anything but global_opacity, global_scale and color_space)."""
+    entities = list(entities)
+    if not entities:
+        raise ValueError("render_scene: no entities")
+    if len(entities) > abi.BGS_SCENE_MAX_CLOUDS:
+        raise ValueError(f"render_scene: {len(entities)} entities, at most {abi.BGS_SCENE_MAX_CLOUDS}")
+    first = entities[0][1]
+    for j, (_, st, _) in enumerate(entities[1:], 1):
+        for f in dataclasses.fields(first):
+            if f.name in SCENE_PER_ENTITY_FIELDS:
+                continue
+            a, b = getattr(first, f.name), getattr(st, f.name)
+            if a != b:
+                raise ValueError(f"render_scene: entity {j} has {f.name} = {b!r}, entity 0 {a!r}: frame-wide fields must agree")
+    return first
+
+
 class GaussianSplattingPlugin:
     """Owns one `bgs_context` (one GPU).  `render_view` = run_radix_sort + DrawGaussians for one view."""
 
@@ -269,6 +294,32 @@ class GaussianSplattingPlugin:
             st = self._lib.bgs_render_ex(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), C.byref(ex), target, code, 0)
         self._check(st)
         return out if to_host else None
+
+    def render_scene(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None, previous_view: View | None = None,
+                     delta_time: float | None = None, asynchronous: bool = False, premultiplied: bool = False,
+                     blend_over: bool = False, out: np.ndarray | None = None) -> np.ndarray:
+        """Every entity of one view in ONE frame (`bgs_render_scene`): `entities` is a sequence of (handle, CloudSettings,
+        CloudTransform or None), the Bevy world's cloud entities.  Their splats share one depth sort, so clouds that
+        interpenetrate are blended splat by splat instead of one painted over the other.  Each entity's global_opacity,
+        global_scale, color_space, transform and handle.aabb go to its own uniform; every other settings field is the
+        frame's and must agree across entities (`check_scene_entities`, ValueError before any call).  The other arguments
+        are `render_view`'s.  Returns the (H, W, 4) host frame."""
+        settings = check_scene_entities(entities)
+        entities = list(entities)
+        code, dtype, ch = self.FORMATS[fmt]
+        v = view.to_abi()
+        _, s, ex = self._call_args(entities[0][0], settings, entities[0][2], asynchronous, premultiplied, blend_over,
+                                   previous_view, delta_time)
+        k = len(entities)
+        clouds = (C.c_void_p * k)(*[h._h.value for h, _, _ in entities])
+        unis = (abi.bgs_cloud_uniform * k)(*[self.cloud_uniform(st, tr, h.aabb) for h, st, tr in entities])
+        if out is None:
+            out = np.empty((view.height, view.width, ch), dtype)
+        assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
+        zd = self._scene_depth(scene_depth, view)
+        self._check(self._lib.bgs_render_scene(self._ctx, clouds, unis, k, C.byref(v), C.byref(s), None if ex is None else C.byref(ex),
+                                               None if zd is None else C.byref(zd), _ptr(out), code, 0))
+        return out
 
     def _render_4d(self, handle, v, u, s, ex, zd, settings, target, code, is_device):
         return self._lib.bgs_render_4d(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), None if ex is None else C.byref(ex),

@@ -564,6 +564,48 @@ bgs_status bgs_render_4d(bgs_context* ctx, const bgs_cloud* cloud, const bgs_vie
                          const bgs_settings* settings, const bgs_render_extras* extras, const bgs_scene_depth* depth,
                          void* out_rgba, uint32_t out_format, int out_is_device_ptr, float time_start, float time_stop);
 
+/* Several resident clouds in one view, rendered as one depth-sorted set: the k clouds clouds[0..k), cloud j with its own
+ * uniforms[j], into one frame as if their gaussians were one cloud.  Arguments otherwise as bgs_render_depth_test's
+ * (extras and depth may be NULL).  The reference draws each cloud entity as its own transparent item, sorted by entity
+ * distance (render/mod.rs:398-452), so one cloud is painted wholly over another even where they interpenetrate; here
+ * the clouds' splats share one depth sort, one binning and one blend.
+ *
+ * The rule, exactly:
+ *   Index space.  Cloud j contributes its n_j gaussians at global indices o_j + i, o_j = n_0 + ... + n_{j-1};
+ *     N = n_0 + ... + n_{k-1}.  The same cloud may be listed more than once (instancing): each listing is its own segment.
+ *   Per-cloud values.  Everything a bgs_cloud_uniform carries (transform, global_opacity, global_scale, color_space,
+ *     aabb_min / max) and the cloud's layout and SH degree come from the gaussian's own cloud j.  gaussian_mode,
+ *     rasterize_mode, aabb, opacity_adaptive_radius, draw_mode, radix_sort_depth_bits, flags, num_classes and the depth
+ *     buffer are the frame's.
+ *   Key.  The key of global index g = o_j + i is the key bgs_render computes for gaussian i of cloud j with uniforms[j].
+ *     The depth sort is stable and ascending over (key, g).
+ *   Projected record.  The record of g is, bit for bit, the record bgs_render_depth_test with cloud j and uniforms[j]
+ *     writes for i; so are its splat depth under a depth buffer, its OpticalFlow colour (p = M_j * pos) and its Position
+ *     colour (cloud j's aabb).
+ *   Depth mode.  The range is the sorted[1] / sorted[N-1] rule applied to the joint sorted entry list of N entries
+ *     (culled tail in ascending global index); each entry's distance is taken from its own cloud's transformed position.
+ *   Everything else is unchanged.  Binning, tile ranges and slices, chunked rounds, the blend, the depth test,
+ *     PREMULTIPLIED_OUT, BLEND_OVER_TARGET, ASYNC and the pair-overflow re-render work on the joint record set exactly as
+ *     for one cloud.  So k == 1 is exactly bgs_render_depth_test, and a cloud split into contiguous subsets (bgs_cloud_subset
+ *     in index mode), each listed with the uniform of the whole, renders bit-identically to the whole cloud: pixels,
+ *     sorted entries, tile ranges and slices, records, frame stats and launch count.  Clouds whose depth intervals do not
+ *     overlap match the reference's far-first blend-over composite up to the rounding of the reassociated "over".
+ *   Ordering.  Each listed cloud is read after every write queued on it before the call (particle steps, interpolations),
+ *     on any context.  A queued frame's targets and depth buffer follow bgs_render_depth_test's contract.
+ *   Debug hooks.  bgs_debug_sorted_entries, _tile_ranges, _tile_entries, _projected, _splat_depths, bgs_frame_stats_get
+ *     (n = N) and bgs_stage_times_us report the frame in the global index space.
+ * Launches: one key-gen over the whole scene, and one projection per distinct projection kernel among the clouds (f32
+ *   or f16 storage, SH degree; the f16 and f16-covariance layouts share one), so a scene of clouds of one layout and
+ *   degree costs the launches of one cloud.
+ * Refused with BGS_EINVAL, nothing enqueued or written: k == 0 or k > BGS_SCENE_MAX_CLOUDS; a NULL entry in clouds; a
+ *   Gaussian4d cloud; a cloud on another device; N >= 2^30; BGS_FLAG_SORT_ALL (the reference-literal order belongs to
+ *   one draw, and a scene is several); any refusal bgs_render_depth_test makes for one of the clouds with its uniform.
+ *   NULL clouds, uniforms, view or settings -> BGS_NOT_READY, as for bgs_render. */
+#define BGS_SCENE_MAX_CLOUDS 64
+bgs_status bgs_render_scene(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms, uint32_t k,
+                            const bgs_view* view, const bgs_settings* settings, const bgs_render_extras* extras,
+                            const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target

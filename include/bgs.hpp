@@ -369,6 +369,44 @@ public:
         check(st);
         return true;
     }
+    // One cloud entity of a scene frame: its resident cloud, settings and transform
+    struct SceneEntity {
+        const PlanarGaussian3dHandle* cloud;
+        CloudSettings settings;
+        Mat4 transform = Mat4::identity();
+    };
+    // Every cloud entity of one view in one frame (bgs_render_scene): their splats share one depth sort, so clouds that
+    // interpenetrate blend splat by splat.  Each entity's global_opacity, global_scale, color_space, transform and aabb
+    // go to its own uniform; the other settings are the frame's, taken from entities[0].  `depth` / `pitch_bytes` as render_view_depth_test's (nullptr: no depth test).
+    bool render_scene(const std::vector<SceneEntity>& entities, const bgs_view& view, void* out_rgba,
+                      uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr, float delta_time = 0.0f,
+                      const float* depth = nullptr, uint64_t pitch_bytes = 0, bool out_is_device = false,
+                      uint32_t extra_flags = 0) {
+        if (entities.empty()) check(BGS_EINVAL);
+        std::vector<const bgs_cloud*> clouds;
+        std::vector<bgs_cloud_uniform> unis;
+        for (const SceneEntity& e : entities) {
+            bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
+            std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
+            clouds.push_back(e.cloud->get());
+            unis.push_back(u);
+        }
+        const CloudSettings& settings = entities[0].settings;
+        const bgs_settings s = settings.to_abi(extra_flags);
+        bgs_render_extras ex{};
+        ex.num_classes = settings.num_classes;
+        if (previous_view) {
+            std::memcpy(ex.previous_clip_from_world, previous_view->clip_from_world, 64);
+            ex.delta_time = delta_time;
+        }
+        const bgs_scene_depth zd{depth, pitch_bytes};
+        const bgs_status st = bgs_render_scene(ctx_, clouds.data(), unis.data(), (uint32_t)clouds.size(), &view, &s,
+                                               settings.rasterize_mode == RasterizeMode::OpticalFlow && !previous_view ? nullptr : &ex,
+                                               depth ? &zd : nullptr, out_rgba, format, out_is_device ? 1 : 0);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
     // Colour + depth + normal frames of one view in one pass (BASELINE.json config 4; bgs_render_aux).
     bool render_view_aux(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view, void* out_rgba,
                          void* out_depth, void* out_normal, uint32_t format = BGS_FORMAT_RGBA8_SRGB, bool out_is_device = false) {
