@@ -77,6 +77,14 @@ class bgs_scene_depth(C.Structure):
     ]
 
 
+class bgs_time_window(C.Structure):
+    """CloudSettings.time_start / time_stop of one entity of a bgs_render_scene_4d call."""
+    _fields_ = [
+        ("time_start", C.c_float),
+        ("time_stop", C.c_float),
+    ]
+
+
 class bgs_frame_stats(C.Structure):
     _fields_ = [
         ("n", C.c_uint32),
@@ -142,6 +150,9 @@ SYMBOLS = [
                                 C.c_float]),
     ("bgs_render_scene", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
                                    C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
+    ("bgs_render_scene_4d", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_time_window), C.c_uint32,
+                                      C.POINTER(bgs_view), C.POINTER(bgs_settings), C.POINTER(bgs_render_extras),
+                                      C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,
                                  C.c_uint32, C.c_int]),
     ("bgs_sync", C.c_int, [_P]),

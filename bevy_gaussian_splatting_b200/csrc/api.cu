@@ -507,10 +507,17 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
         ++launches;
     }
     CU(c, cudaEventRecord(c->ev_p0, ps));
+    bool scene_3d = false;   // a scene lists a non-4D cloud (whose splat depths splat_depth_scene writes)
     if (scene) {   // one launch per projection kernel the scene's clouds need
         for (const uint32_t g : scene->groups) {
-            launch_project_scene(scene->tab, g, c->slot_ids.p, c->ctr, c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr, p.n_hint,
-                                 c->sm_count, c->cutoff_tab, modes, ps);
+            if (g == PROJECT_GROUP_4D) {   // (also writes the 4D segments' splat depths, from the moved positions)
+                launch_project_4d_scene(scene->tab, scene->times, c->slot_ids.p, c->ctr, modes ? *modes : ModeConsts{}, c->recs.p,
+                                        zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
+            } else {
+                launch_project_scene(scene->tab, g, c->slot_ids.p, c->ctr, c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr,
+                                     p.n_hint, c->sm_count, c->cutoff_tab, modes, ps);
+                scene_3d = true;
+            }
             ++launches;
         }
     } else if (tc) {   // Gaussian4d: the projection also writes the depth-tested frame's splat depths, from the moved positions
@@ -525,10 +532,10 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaEventRecord(c->ev_p1, ps));
     // depth-tested frames: the splat depths, indexed like the records (the projection's index list)
     ZTestArgs zt;
-    if (zd && scene) {
+    if (zd && scene_3d) {
         launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
-    } else if (zd && !tc) {
+    } else if (zd && !tc && !scene) {
         launch_splat_depth(cloud->pos, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
                            c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
@@ -628,7 +635,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
                               const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr,
                               const std::shared_ptr<const SceneFacts>& scene = nullptr) {
     if (!c) return BGS_EINVAL;
-    TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));
+    if (!scene) TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));   // (scenes: per cloud, before)
     if (zd) TRY(check_scene_depth(c, zd, view));
     if (c->async_pending && !(st->flags & BGS_FLAG_ASYNC)) {
         // a synchronous render after queued frames completes them first; their failure (including an overflowed
@@ -684,39 +691,67 @@ bgs_status bgs_render_depth_test(bgs_context* c, const bgs_cloud* cloud, const b
     return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth);
 }
 
+// bgs_render_4d's time refusals (include/bgs.h): time and window finite, time_stop != time_start, and a window length
+// that does not overflow
+static bgs_status temporal_consts(bgs_context* c, const char* call, float time, float time_start, float time_stop,
+                                  TemporalConsts& tc) {
+    if (!std::isfinite(time) || !std::isfinite(time_start) || !std::isfinite(time_stop) || time_stop == time_start)
+        return fail(c, BGS_EINVAL, "%s: time %g, time_start %g, time_stop %g: all finite and time_stop != time_start", call,
+                    (double)time, (double)time_start, (double)time_stop);
+    tc.duration = time_stop - time_start;
+    if (!std::isfinite(tc.duration)) return fail(c, BGS_EINVAL, "%s: time_stop - time_start overflows", call);
+    tc.time = time;
+    tc.time_future = time + 1.0e-3f;
+    return BGS_OK;
+}
+
 bgs_status bgs_render_4d(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                          const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba,
                          uint32_t out_format, int out_is_device_ptr, float time_start, float time_stop) {
     if (!c) return BGS_EINVAL;
     TemporalConsts tc = {};
-    if (uni) {
-        if (!std::isfinite(uni->time) || !std::isfinite(time_start) || !std::isfinite(time_stop) || time_stop == time_start)
-            return fail(c, BGS_EINVAL, "render_4d: time %g, time_start %g, time_stop %g: all finite and time_stop != time_start",
-                        (double)uni->time, (double)time_start, (double)time_stop);
-        tc.duration = time_stop - time_start;
-        if (!std::isfinite(tc.duration)) return fail(c, BGS_EINVAL, "render_4d: time_stop - time_start overflows");
-        tc.time = uni->time;
-        tc.time_future = uni->time + 1.0e-3f;
-    }
+    if (uni) TRY(temporal_consts(c, "render_4d", uni->time, time_start, time_stop, tc));
     return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth, &tc);
 }
 
-bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis, uint32_t k,
-                            const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
-                            void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+// bgs_render_scene, and bgs_render_scene_4d (with_4d: Gaussian4d clouds are projected at uniforms[j].time in windows[j];
+// with none listed the two calls are one and windows is not read)
+static bgs_status render_scene_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
+                                    const bgs_cloud_uniform* unis, const bgs_time_window* windows, uint32_t k,
+                                    const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex,
+                                    const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
     if (!c) return BGS_EINVAL;
-    if (!clouds || !unis || !view || !st) return fail(c, BGS_NOT_READY, "render_scene: clouds/uniforms/view/settings not ready");
-    if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "render_scene: k = %u is not in 1..%d", k, BGS_SCENE_MAX_CLOUDS);
-    if (st->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "render_scene: BGS_FLAG_SORT_ALL is not supported");
+    if (!clouds || !unis || !view || !st) return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/view/settings not ready", call);
+    if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "%s: k = %u is not in 1..%d", call, k, BGS_SCENE_MAX_CLOUDS);
+    if (st->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
+    bool any_4d = false;
+    for (uint32_t j = 0; j < k; ++j) {
+        if (!clouds[j]) return fail(c, BGS_EINVAL, "%s: clouds[%u] is NULL", call, j);
+        any_4d = any_4d || (with_4d && is_4d(clouds[j]->layout));
+    }
+    // a scene with 4D clouds: those are checked as bgs_render_4d frames (gaussian_mode read as Gaussian4d), the others
+    // against the frame's settings, a Velocity frame's as a Color one (they are drawn as nothing, include/bgs.h)
+    bgs_settings s4 = *st, s3 = *st;
+    if (any_4d) {
+        if (!windows) return fail(c, BGS_EINVAL, "%s: windows is NULL with a Gaussian4d cloud listed", call);
+        if (st->gaussian_mode == BGS_GAUSSIAN_2D && st->aabb)
+            return fail(c, BGS_EINVAL, "%s: BGS_GAUSSIAN_2D with aabb = 1 takes no Gaussian4d cloud (its blend reads a surfel record for every splat)", call);
+        s4.gaussian_mode = BGS_GAUSSIAN_4D;
+        if (s3.rasterize_mode == BGS_RASTERIZE_VELOCITY) s3.rasterize_mode = BGS_RASTERIZE_COLOR;
+    }
+    auto scene = std::make_shared<SceneFacts>();
     uint64_t total = 0;
     for (uint32_t j = 0; j < k; ++j) {
-        if (!clouds[j]) return fail(c, BGS_EINVAL, "render_scene: clouds[%u] is NULL", j);
-        TRY(check_render(c, clouds[j], view, &unis[j], st, ex, out_format, false, false));   // (refuses 4D clouds, other devices)
+        const bool is4 = any_4d && is_4d(clouds[j]->layout);
+        if (any_4d && !is4 && st->gaussian_mode == BGS_GAUSSIAN_4D)
+            return fail(c, BGS_EINVAL, "%s: gaussian_mode BGS_GAUSSIAN_4D with clouds[%u], which is not a Gaussian4d cloud", call, j);
+        // (without 4D clouds: bgs_render_depth_test's check, which refuses 4D clouds and other devices)
+        TRY(check_render(c, clouds[j], view, &unis[j], is4 ? &s4 : &s3, ex, out_format, false, is4));
+        if (is4) TRY(temporal_consts(c, call, unis[j].time, windows[j].time_start, windows[j].time_stop, scene->times.t[j]));
         total += clouds[j]->n;
     }
-    if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "render_scene: N = %llu gaussians, must be < 2^30", (unsigned long long)total);
+    if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "%s: N = %llu gaussians, must be < 2^30", call, (unsigned long long)total);
     if (depth) TRY(check_scene_depth(c, depth, view));
-    auto scene = std::make_shared<SceneFacts>();
     SceneTable& tab = scene->tab;
     memset(&tab, 0, sizeof(tab));
     tab.k = k;
@@ -725,7 +760,7 @@ bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, cons
     for (uint32_t j = 0; j < k; ++j) {
         const bgs_cloud* cl = clouds[j];
         SceneSeg& sg = tab.seg[j];
-        sg.fc = frame_consts(cl, view, &unis[j], st, false);
+        sg.fc = frame_consts(cl, view, &unis[j], any_4d && is_4d(cl->layout) ? &s4 : st, false);
         sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
         sg.pos = cl->pos;
         sg.blocks = cl->blocks;
@@ -738,6 +773,21 @@ bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, cons
     }
     return render_impl(c, clouds[0], view, &unis[0], st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth,
                        nullptr, scene);
+}
+
+bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis, uint32_t k,
+                            const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                            void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    return render_scene_impl(c, "render_scene", false, clouds, unis, nullptr, k, view, st, ex, depth, out_rgba, out_format,
+                             out_is_device_ptr);
+}
+
+bgs_status bgs_render_scene_4d(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                               const bgs_time_window* windows, uint32_t k, const bgs_view* view, const bgs_settings* st,
+                               const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
+                               int out_is_device_ptr) {
+    return render_scene_impl(c, "render_scene_4d", true, clouds, unis, windows, k, view, st, ex, depth, out_rgba, out_format,
+                             out_is_device_ptr);
 }
 
 bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,

@@ -64,6 +64,11 @@ struct SceneTable {
     }
 };
 
+// The projection group of Gaussian4d segments (bgs_render_scene_4d): project_group gives the 3D layouts 0 .. 7 (f16 bit,
+// SH degree << 1), so 4D segments never fall into a 3D launch, and splat_depth_scene leaves their depths to the 4D
+// projection, which takes them from the moved positions.
+constexpr uint32_t PROJECT_GROUP_4D = 8u;
+
 // bgs_render_extras as the Classification / OpticalFlow projection reads it.  Only project_modes_kernel takes it (as an
 // argument of its own), so the arguments and code of every other kernel stay what they were.
 struct ModeConsts {
@@ -77,6 +82,12 @@ struct TemporalConsts {
     float time;          // bgs_cloud_uniform.time
     float time_future;   // time + 1e-3f: RasterizeMode::Velocity's second conditioning
     float duration;      // time_stop - time_start (finite, non-zero): the time terms' theta = dt / duration
+};
+
+// bgs_render_scene_4d's per-segment times (t[j] is segment j's; only 4D segments read theirs).  An argument of
+// project_4d_scene_kernel alone (768 B beside the ~22 KB segment table), so the other scene kernels keep theirs.
+struct SceneTimes {
+    TemporalConsts t[BGS_SCENE_MAX_CLOUDS];
 };
 
 // Projected splat record, 48 B, stored by front-to-back rank.

@@ -63,9 +63,11 @@ struct bgs_particles {
 };
 
 // A bgs_render_scene frame: its segment table (what its kernels and the culled-flags hook read), the clouds it lists
-// (clouds[j] is segment j's; a cloud may be listed more than once) and its distinct projection groups
+// (clouds[j] is segment j's; a cloud may be listed more than once) and its distinct projection groups.  A
+// bgs_render_scene_4d frame also carries its 4D segments' times (PROJECT_GROUP_4D among the groups).
 struct SceneFacts {
     SceneTable tab;
+    SceneTimes times = {};
     std::vector<const bgs_cloud*> clouds;
     std::vector<uint32_t> groups;
 };

@@ -47,6 +47,11 @@ void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payl
 void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                        const FrameConsts& fc, const ModeConsts& mc, const TemporalConsts& tc, SplatRec* recs, float* depths,
                        uint32_t n_hint, int sm_count, cudaStream_t stream);
+// bgs_render_scene_4d: the projection of every segment in PROJECT_GROUP_4D (one launch), each at its own times, and their
+// splat depths from the moved positions (depths non-null)
+void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const uint32_t* slot_ids, const FrameCounters* ctr,
+                             const ModeConsts& mc, SplatRec* recs, float* depths, uint32_t n_hint, int sm_count,
+                             cudaStream_t stream);
 // bin.cu
 int bin_coop_blocks_per_sm();
 cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,

@@ -601,12 +601,14 @@ __device__ __forceinline__ void store_rec(SplatRec* __restrict__ dst, const Spla
 // One entry of the index list -> the 48 B record at recs[r] (+ the 2DGS extra record and the aux colours).  An
 // undrawn gaussian (outside the frustum, or unselected under DrawMode::Selected) gets an empty bbox and no colour.
 // MODES2: the Classification / OpticalFlow colour sources (project_modes_kernel) instead of the four others.
+// no_source: the frame has no colour source for this gaussian (a 3D or 2D one in a bgs_render_scene_4d Velocity frame:
+// the reference builds no pipeline for it), so it stays undrawn.  Only the scene kernels pass it.
 template <bool F16, uint32_t D, bool MODES2>
 __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCounters* __restrict__ ctr, uint32_t r,
                                             float4 p4, const float q[4], const float so[4], const float* sh,
                                             const float* __restrict__ cutoff_tab, uint32_t op_bits,
                                             SplatRec* __restrict__ recs, float4* __restrict__ extra,
-                                            float4* __restrict__ aux, const ModeConsts& mc) {
+                                            float4* __restrict__ aux, const ModeConsts& mc, bool no_source = false) {
     SplatRec rec;
     rec.ux = 0.f; rec.uy = 0.f; rec.vx = 0.f; rec.vy = 0.f;
     rec.bx = BBOX_EMPTY; rec.by = BBOX_EMPTY;
@@ -620,7 +622,7 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
     rec.cy = hh - ndc[1] * hh;
     const float opacity = so[3];
     rec.op = opacity * fc.global_opacity;
-    if (visible && !(fc.draw_mode == BGS_DRAW_SELECTED && p4.w < 0.5f)) {   // gaussian.wgsl:203-205 (DrawMode::Selected)
+    if (visible && !no_source && !(fc.draw_mode == BGS_DRAW_SELECTED && p4.w < 0.5f)) {   // gaussian.wgsl:203-205 (DrawMode::Selected)
         const float cutoff = splat_cutoff<F16>(fc, opacity, cutoff_tab, op_bits);
         float A[3][3], Rm[3][3];   // the model 3x3 and the rotation, (row, col)
 #pragma unroll
@@ -804,7 +806,9 @@ __device__ __forceinline__ void project_scene_groups(const SceneTable& tab, uint
         gather(g_next);
         g_cur = g_next;
         g_next = list_id(r0 + 2u * stride + lane);
-        if (mine) project_one<F16, D, MODES2>(tab.seg[j].fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, nullptr, mc);
+        if (mine)
+            project_one<F16, D, MODES2>(tab.seg[j].fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, nullptr, mc,
+                                        MODES2 && tab.seg[j].fc.rasterize_mode == BGS_RASTERIZE_VELOCITY);
     }
 }
 
@@ -854,7 +858,10 @@ void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payl
     depth_range_scene_kernel<<<1, 32, 0, stream>>>(tab, sorted_payload, slot_ids, ctr);
 }
 
-uint32_t project_group(CloudLayout layout, uint32_t sh_degree) { return (is_f16(layout) ? 1u : 0u) | sh_degree << 1; }
+uint32_t project_group(CloudLayout layout, uint32_t sh_degree) {
+    if (is_4d(layout)) return PROJECT_GROUP_4D;   // (launch_project_4d_scene)
+    return (is_f16(layout) ? 1u : 0u) | sh_degree << 1;
+}
 
 void launch_project_scene(const SceneTable& tab, uint32_t group, const uint32_t* slot_ids, const FrameCounters* ctr,
                           SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
@@ -1093,6 +1100,75 @@ void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_sl
     if (grid < 1u) grid = 1u;
     project_4d_kernel<<<grid, PROJ_THREADS, 0, stream>>>(static_cast<const uint4*>(blocks), index_list, by_slot, ctr, fc, mc, tc,
                                                          recs, depths);
+}
+
+// ---- bgs_render_scene_4d: project_4d_kernel over a segment table.  Record r is compact slot r; its global index lies in
+// segment j, and only the segments of PROJECT_GROUP_4D are this launch's (the 3D ones are launch_project_scene's).  Each
+// lane stages its own entry's first 128 B line from its own cloud's blocks (gather_block_ptrs), then project_one_4d runs
+// with segment j's FrameConsts and times, so the record and splat depth are those bgs_render_4d writes for that cloud.
+__global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
+project_4d_scene_kernel(SceneTable tab, SceneTimes times, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
+                        const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs,
+                        float* __restrict__ depths /* depth-tested frames only */) {
+    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * GEO4];
+    const int lane = threadIdx.x & 31;
+    uint4* const stage = s_stages[threadIdx.x >> 5];
+    const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
+    constexpr uint32_t NONE = 0xFFFFFFFFu;
+    auto list_id = [&](uint32_t r) { return r < n_vis ? __ldg(slot_ids + r) : NONE; };   // slot r's global index
+    // global index g's block, null when there is none or its cloud is not a 4D one
+    auto block_of = [&](uint32_t g) -> const uint4* {
+        if (g == NONE) return nullptr;
+        const SceneSeg& s = tab.seg[tab.find(g)];
+        if (s.group != PROJECT_GROUP_4D) return nullptr;
+        return static_cast<const uint4*>(s.blocks) + (size_t)(g - s.offset) * CH4;
+    };
+    auto gather = [&](uint32_t g) {   // one commit group per call
+        gather_block_ptrs<GEO4, GEO4>(block_of(g), stage, lane);   // (slot p ^ (g & 7), as project_4d_kernel's)
+        cp_async_commit();
+    };
+    uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
+    uint32_t g_cur = list_id(r0 + lane);
+    gather(g_cur);
+    uint32_t g_next = list_id(r0 + stride + lane);
+    for (; r0 < n_vis; r0 += stride) {
+        cp_async_wait<0>();
+        __syncwarp();   // every lane's copies of this group have landed
+        const uint32_t r = r0 + lane;
+        const uint32_t j = g_cur == NONE ? 0u : tab.find(g_cur);
+        const bool mine = g_cur != NONE && tab.seg[j].group == PROJECT_GROUP_4D;
+        auto piece = [&](int p) {
+            const uint4 v = stage[lane * GEO4 + (p ^ (lane & 7))];
+            return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
+        };
+        const float4 p4 = piece(POS_CHUNK), a = piece(SECOND_CHUNK), b = piece(ROT_R_CHUNK), c = piece(SO_4D_CHUNK),
+                     d = piece(TT_CHUNK);
+        __syncwarp();   // the stage is read out before the next group's copies overwrite it
+        const uint32_t g_mine = g_cur;
+        gather(g_next);
+        g_cur = g_next;
+        g_next = list_id(r0 + 2u * stride + lane);
+        if (mine) {
+            const SceneSeg& s = tab.seg[j];
+            const float ql[4] = {a.x, a.y, a.z, a.w}, qr[4] = {b.x, b.y, b.z, b.w}, so[4] = {c.x, c.y, c.z, c.w},
+                        tt[4] = {d.x, d.y, d.z, d.w};
+            const uint4* sh = static_cast<const uint4*>(s.blocks) + (size_t)(g_mine - s.offset) * CH4 + sh_first(CloudLayout::F32x4D);
+            project_one_4d(s.fc, mc, times.t[j], ctr, r, p4, ql, qr, so, tt, sh, recs, depths);
+        }
+    }
+}
+// sm_90 takes up to 32764 B of kernel parameters (CUDA >= 12.1): the table (~22 KB), the times (768 B), the extras and
+// four pointers
+static_assert(sizeof(SceneTable) + sizeof(SceneTimes) + sizeof(ModeConsts) + 4 * sizeof(void*) + 16 <= 32764,
+              "project_4d_scene_kernel's parameters exceed the sm_90 limit");
+
+void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const uint32_t* slot_ids, const FrameCounters* ctr,
+                             const ModeConsts& mc, SplatRec* recs, float* depths, uint32_t n_hint, int sm_count,
+                             cudaStream_t stream) {
+    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
+    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
+    if (grid < 1u) grid = 1u;
+    project_4d_scene_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, times, mc, slot_ids, ctr, recs, depths);
 }
 
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,

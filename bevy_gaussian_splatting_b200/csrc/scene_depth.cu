@@ -24,7 +24,8 @@ splat_depth_kernel(const float4* __restrict__ pos, const uint32_t* __restrict__ 
     }
 }
 
-// bgs_render_scene: record r is compact slot r, its global index in segment j (common.cuh)
+// bgs_render_scene: record r is compact slot r, its global index in segment j (common.cuh).  Gaussian4d segments
+// (bgs_render_scene_4d) are skipped: their projection writes their depths from the moved positions.
 __global__ void __launch_bounds__(SD_THREADS)
 splat_depth_scene_kernel(SceneTable tab, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
                          float* __restrict__ depths) {
@@ -32,6 +33,7 @@ splat_depth_scene_kernel(SceneTable tab, const uint32_t* __restrict__ slot_ids, 
     for (uint32_t r = blockIdx.x * SD_THREADS + threadIdx.x; r < n_vis; r += gridDim.x * SD_THREADS) {
         const uint32_t g = __ldg(slot_ids + r);
         const SceneSeg& s = tab.seg[tab.find(g)];
+        if (s.group == PROJECT_GROUP_4D) continue;
         const float4 p = __ldg(s.pos + (g - s.offset));
         float pw[4];
         mat4_point(s.fc.model, p.x, p.y, p.z, pw);

@@ -21,7 +21,7 @@ from . import abi
 from .camera import GaussianCamera, View
 from .gaussian import SH_WIDTHS, PlanarGaussian3d, PlanarGaussian4d, compute_aabb
 from .particles import PARTICLE_BEHAVIOR_DTYPE, as_particle_behaviors
-from .settings import CloudSettings, SparseSelect
+from .settings import CloudSettings, GaussianMode, SparseSelect
 
 
 def _ptr(a: np.ndarray):
@@ -212,6 +212,52 @@ def check_scene_entities(entities) -> CloudSettings:
     return first
 
 
+# bgs_render_scene_4d also takes each entity's time and window, and its playback settings are its own
+SCENE_4D_PER_ENTITY_FIELDS = SCENE_PER_ENTITY_FIELDS | {"time", "time_start", "time_stop", "time_scale", "playback_mode",
+                                                        "gaussian_mode"}
+
+
+def is_4d_handle(handle) -> bool:
+    return bool(getattr(handle, "temporal", False))
+
+
+def check_scene_entities_4d(entities) -> CloudSettings:
+    """`check_scene_entities` for an entity list with Gaussian4d clouds (one bgs_render_scene_4d call).  time, time_start,
+    time_stop, time_scale and playback_mode are per entity too.  A 4D entity's gaussian_mode must be Gaussian4d; the other
+    entities' must agree and be Gaussian2d or Gaussian3d, and Gaussian2d with aabb takes no 4D entity.  Returns the
+    frame's settings: the first entity's, with gaussian_mode the non-4D entities' (Gaussian4d when every entity is 4D).
+    Raises ValueError on any disagreement."""
+    entities = list(entities)
+    if not entities:
+        raise ValueError("render_scene: no entities")
+    if len(entities) > abi.BGS_SCENE_MAX_CLOUDS:
+        raise ValueError(f"render_scene: {len(entities)} entities, at most {abi.BGS_SCENE_MAX_CLOUDS}")
+    first = entities[0][1]
+    for j, (_, st, _) in enumerate(entities[1:], 1):
+        for f in dataclasses.fields(first):
+            if f.name in SCENE_4D_PER_ENTITY_FIELDS:
+                continue
+            a, b = getattr(first, f.name), getattr(st, f.name)
+            if a != b:
+                raise ValueError(f"render_scene: entity {j} has {f.name} = {b!r}, entity 0 {a!r}: frame-wide fields must agree")
+    others = set()
+    for j, (h, st, _) in enumerate(entities):
+        gm = GaussianMode(st.gaussian_mode)
+        if is_4d_handle(h):
+            if gm != GaussianMode.Gaussian4d:
+                raise ValueError(f"render_scene: entity {j} is a Gaussian4d cloud with gaussian_mode {gm.name}")
+        elif gm == GaussianMode.Gaussian4d:
+            raise ValueError(f"render_scene: entity {j} is not a Gaussian4d cloud but has gaussian_mode Gaussian4d")
+        else:
+            others.add(gm)
+    if len(others) > 1:
+        raise ValueError(f"render_scene: the non-4D entities disagree on gaussian_mode ({sorted(m.name for m in others)})")
+    mode = others.pop() if others else GaussianMode.Gaussian4d
+    if mode == GaussianMode.Gaussian2d and first.aabb and any(is_4d_handle(h) for h, _, _ in entities):
+        raise ValueError("render_scene: Gaussian2d with aabb takes no Gaussian4d entity (its blend reads surfel records)")
+    return dataclasses.replace(first, gaussian_mode=mode)
+
+
 class GaussianSplattingPlugin:
     """Owns one `bgs_context` (one GPU).  `render_view` = run_radix_sort + DrawGaussians for one view."""
 
@@ -303,9 +349,13 @@ class GaussianSplattingPlugin:
         interpenetrate are blended splat by splat instead of one painted over the other.  Each entity's global_opacity,
         global_scale, color_space, transform and handle.aabb go to its own uniform; every other settings field is the
         frame's and must agree across entities (`check_scene_entities`, ValueError before any call).  The other arguments
-        are `render_view`'s.  Returns the (H, W, 4) host frame."""
-        settings = check_scene_entities(entities)
+        are `render_view`'s.  Returns the (H, W, 4) host frame.
+        A list with a PlanarGaussian4dHandle goes to `bgs_render_scene_4d`: each entity's time, time_start, time_stop,
+        time_scale and playback_mode are its own, a 4D entity's gaussian_mode is Gaussian4d and the others' must agree
+        (`check_scene_entities_4d`)."""
         entities = list(entities)
+        temporal = any(is_4d_handle(h) for h, _, _ in entities)
+        settings = check_scene_entities_4d(entities) if temporal else check_scene_entities(entities)
         code, dtype, ch = self.FORMATS[fmt]
         v = view.to_abi()
         _, s, ex = self._call_args(entities[0][0], settings, entities[0][2], asynchronous, premultiplied, blend_over,
@@ -317,6 +367,12 @@ class GaussianSplattingPlugin:
             out = np.empty((view.height, view.width, ch), dtype)
         assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
         zd = self._scene_depth(scene_depth, view)
+        if temporal:
+            windows = (abi.bgs_time_window * k)(*[abi.bgs_time_window(float(st.time_start), float(st.time_stop)) for _, st, _ in entities])
+            self._check(self._lib.bgs_render_scene_4d(self._ctx, clouds, unis, windows, k, C.byref(v), C.byref(s),
+                                                      None if ex is None else C.byref(ex), None if zd is None else C.byref(zd),
+                                                      _ptr(out), code, 0))
+            return out
         self._check(self._lib.bgs_render_scene(self._ctx, clouds, unis, k, C.byref(v), C.byref(s), None if ex is None else C.byref(ex),
                                                None if zd is None else C.byref(zd), _ptr(out), code, 0))
         return out

@@ -606,6 +606,45 @@ bgs_status bgs_render_scene(bgs_context* ctx, const bgs_cloud* const* clouds, co
                             const bgs_view* view, const bgs_settings* settings, const bgs_render_extras* extras,
                             const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
 
+/* bgs_render_scene with Gaussian4d clouds among the k: a dynamic 4D capture inside a static 3D scan, or one 4D capture
+ * shown several times at staggered times, rendered as one depth-sorted set.  windows[j] is entity j's
+ * CloudSettings.time_start / time_stop; it is read for Gaussian4d clouds only.  The reference draws each entity as its
+ * own transparent item, so a performer is painted wholly over or under the room around it.
+ *
+ * The rule, exactly:
+ *   Index space, keys, sort, binning, blend, depth test, flags, debug hooks, ordering: bgs_render_scene's.  A 4D cloud's
+ *     key is bgs_render_4d's, the 3D key of its base position; every depth width culls on the base position.
+ *   Per-cloud time.  A Gaussian4d cloud j is conditioned at uniforms[j].time in windows[j] (time_future = time + 1e-3f,
+ *     duration = time_stop - time_start).  The same 4D cloud may be listed more than once, at different times.
+ *   Record of a 4D gaussian: bit for bit the record bgs_render_4d writes for it with cloud j, uniforms[j] and windows[j];
+ *     so are its splat depth under a depth buffer (from the moved position), its Position, OpticalFlow, Classification
+ *     and Velocity colours, its Depth colour (the range from the joint sorted list, as in bgs_render_scene) and its
+ *     undrawn record (masked by time, or moved out of the frustum).
+ *   Record of any other gaussian: bgs_render_scene's.  In a Velocity frame it is keyed, sorted and counted in n_visible
+ *     but undrawn (empty bbox, no colour): the reference's Velocity source conditions a 4D covariance, so a 3D entity
+ *     has no pipeline in that mode and draws nothing.
+ *   gaussian_mode.  4D clouds render as Gaussian4d; settings->gaussian_mode is the other clouds' (2D or 3D), and may be
+ *     BGS_GAUSSIAN_4D only when every listed cloud is a Gaussian4d one.
+ *   So with no 4D cloud listed the call is exactly bgs_render_scene (windows is not read and may be NULL), and a 4D cloud
+ *   split into contiguous subsets, each listed with the uniform and window of the whole, renders exactly like
+ *   bgs_render_4d of the whole: pixels, sorted entries, tile ranges and slices, records, splat depths, frame stats and
+ *   launch count.
+ * Launches: bgs_render_scene's for the non-4D clouds, plus one projection covering every 4D cloud.  The splat-depth
+ *   launch runs only when a non-4D cloud is listed (the 4D projection writes its own), so an all-4D scene costs what
+ *   bgs_render_4d costs.
+ * Refused with BGS_EINVAL, nothing enqueued or written: every refusal of bgs_render_scene but the 4D one; every refusal
+ *   of bgs_render_4d for a 4D cloud with its uniform and window (non-finite time or window, time_stop == time_start, an
+ *   overflowing window, RasterizeMode::Normal, ...); windows == NULL with a 4D cloud listed; BGS_GAUSSIAN_4D with a
+ *   non-4D cloud; BGS_GAUSSIAN_2D with aabb = 1 and a 4D cloud (that blend reads a surfel record for every splat; under
+ *   OBB 2D and 4D records share one blend).  NULL clouds, uniforms, view or settings -> BGS_NOT_READY. */
+typedef struct {
+    float time_start, time_stop;   /* CloudSettings.time_start / time_stop of one entity */
+} bgs_time_window;
+bgs_status bgs_render_scene_4d(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                               const bgs_time_window* windows /* k; read for Gaussian4d clouds only */, uint32_t k,
+                               const bgs_view* view, const bgs_settings* settings, const bgs_render_extras* extras,
+                               const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target

@@ -207,7 +207,7 @@ public:
     PlanarGaussian3dHandle() = default;
     PlanarGaussian3dHandle(const PlanarGaussian3dHandle&) = delete;
     PlanarGaussian3dHandle& operator=(const PlanarGaussian3dHandle&) = delete;
-    PlanarGaussian3dHandle(PlanarGaussian3dHandle&& o) noexcept : h_(o.h_), n_(o.n_) {
+    PlanarGaussian3dHandle(PlanarGaussian3dHandle&& o) noexcept : h_(o.h_), n_(o.n_), temporal_(o.temporal_) {
         std::memcpy(aabb_min_, o.aabb_min_, 12); std::memcpy(aabb_max_, o.aabb_max_, 12); o.h_ = nullptr;
     }
     const float* aabb_min() const { return aabb_min_; }
@@ -215,15 +215,17 @@ public:
     ~PlanarGaussian3dHandle() { if (h_) bgs_cloud_destroy(h_); }
     bgs_cloud* get() const { return h_; }
     uint32_t len() const { return n_; }
+    bool temporal() const { return temporal_; }   // a Gaussian4d cloud (PlanarGaussian4dHandle)
 private:
     friend class GaussianSplattingPlugin;
     bgs_cloud* h_ = nullptr;
     uint32_t n_ = 0;
+    bool temporal_ = false;
     float aabb_min_[3] = {0, 0, 0}, aabb_max_[3] = {1, 1, 1};
 };
 
-// a Gaussian4d cloud resident in HBM (bgs_cloud_upload_4d): rendered by render_view_4d.  The calls on a cloud's
-// positions and visibility take it through get() as they take a 3D one
+// a Gaussian4d cloud resident in HBM (bgs_cloud_upload_4d): rendered by render_view_4d, or by render_scene among other
+// entities.  The calls on a cloud's positions and visibility take it through get() as they take a 3D one
 class PlanarGaussian4dHandle : public PlanarGaussian3dHandle {};
 
 class ParticleBehaviorsHandle {   // a ParticleBehaviors asset resident in HBM (bgs_particles)
@@ -264,6 +266,7 @@ public:
     PlanarGaussian4dHandle add_cloud(const PlanarGaussian4d& c) {
         PlanarGaussian4dHandle h;
         h.n_ = (uint32_t)c.len();
+        h.temporal_ = true;
         for (int k = 0; k < 3; ++k) {   // the Aabb as PlanarGaussian3d::compute_aabb makes it, from the positions
             float lo = INFINITY, hi = -INFINITY;
             for (size_t i = 0; i < c.len(); ++i) {
@@ -378,6 +381,9 @@ public:
     // Every cloud entity of one view in one frame (bgs_render_scene): their splats share one depth sort, so clouds that
     // interpenetrate blend splat by splat.  Each entity's global_opacity, global_scale, color_space, transform and aabb
     // go to its own uniform; the other settings are the frame's, taken from entities[0].  `depth` / `pitch_bytes` as render_view_depth_test's (nullptr: no depth test).
+    // With a Gaussian4d entity (a PlanarGaussian4dHandle) the frame is bgs_render_scene_4d's: each entity's time and
+    // [time_start, time_stop] are its own too, a 4D entity's gaussian_mode is Gaussian4d, and the frame's gaussian_mode is
+    // the first non-4D entity's (Gaussian4d when every entity is 4D).
     bool render_scene(const std::vector<SceneEntity>& entities, const bgs_view& view, void* out_rgba,
                       uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr, float delta_time = 0.0f,
                       const float* depth = nullptr, uint64_t pitch_bytes = 0, bool out_is_device = false,
@@ -385,13 +391,21 @@ public:
         if (entities.empty()) check(BGS_EINVAL);
         std::vector<const bgs_cloud*> clouds;
         std::vector<bgs_cloud_uniform> unis;
+        std::vector<bgs_time_window> windows;
+        bool temporal = false;
+        CloudSettings settings = entities[0].settings;
+        settings.gaussian_mode = GaussianMode::Gaussian4d;
         for (const SceneEntity& e : entities) {
             bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
             std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
             clouds.push_back(e.cloud->get());
             unis.push_back(u);
+            windows.push_back({e.settings.time_start, e.settings.time_stop});
+            temporal = temporal || e.cloud->temporal();
         }
-        const CloudSettings& settings = entities[0].settings;
+        for (auto it = entities.rbegin(); it != entities.rend(); ++it)   // (the first non-4D entity's mode)
+            if (!it->cloud->temporal()) settings.gaussian_mode = it->settings.gaussian_mode;
+        if (!temporal) settings = entities[0].settings;
         const bgs_settings s = settings.to_abi(extra_flags);
         bgs_render_extras ex{};
         ex.num_classes = settings.num_classes;
@@ -400,9 +414,12 @@ public:
             ex.delta_time = delta_time;
         }
         const bgs_scene_depth zd{depth, pitch_bytes};
-        const bgs_status st = bgs_render_scene(ctx_, clouds.data(), unis.data(), (uint32_t)clouds.size(), &view, &s,
-                                               settings.rasterize_mode == RasterizeMode::OpticalFlow && !previous_view ? nullptr : &ex,
-                                               depth ? &zd : nullptr, out_rgba, format, out_is_device ? 1 : 0);
+        const bgs_render_extras* exp = settings.rasterize_mode == RasterizeMode::OpticalFlow && !previous_view ? nullptr : &ex;
+        const bgs_status st =
+            temporal ? bgs_render_scene_4d(ctx_, clouds.data(), unis.data(), windows.data(), (uint32_t)clouds.size(), &view, &s, exp,
+                                           depth ? &zd : nullptr, out_rgba, format, out_is_device ? 1 : 0)
+                     : bgs_render_scene(ctx_, clouds.data(), unis.data(), (uint32_t)clouds.size(), &view, &s, exp,
+                                        depth ? &zd : nullptr, out_rgba, format, out_is_device ? 1 : 0);
         if (st == BGS_NOT_READY) return false;
         check(st);
         return true;
