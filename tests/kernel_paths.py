@@ -205,6 +205,69 @@ def raster_lead(start: int) -> int:
     return start & 3
 
 
+PROJ_THREADS, PROJ_MIN_CTAS = 128, 4   # project.cu:680: projection CTA size and the launch bound's CTAs per SM
+PROJ_WARPS = PROJ_THREADS // 32
+SD_THREADS, SD_CTAS_PER_SM = 256, 8    # scene_depth.cu:12,46-48: splat-depth CTA size and its cap per SM
+
+
+def projection_hint(prev_n_vis: int, n: int) -> int:
+    """api.cu:175 (plan_frame n_hint): records the projection grid plans for.  The previous completed frame's visible
+    count plus a quarter and 1024, at most n; n on a context's first frame (no visible count yet)."""
+    return min(prev_n_vis + prev_n_vis // 4 + 1024, n) if prev_n_vis else n
+
+
+def project_grid(n_hint: int, sm_count: int = H100_SMS) -> int:
+    """project.cu:869-871, 1098-1100, 1168-1170, 1184-1186 (launch_project_scene, launch_project_4d,
+    launch_project_4d_scene, launch_project): ceil(n_hint / 128) CTAs, at most 4 per SM, at least 1."""
+    return max(1, min(-(-n_hint // PROJ_THREADS), PROJ_MIN_CTAS * sm_count))
+
+
+def project_passes(n_vis: int, grid: int, warp: int = 0) -> int:
+    """project.cu:710-713 (and 791-795, 1067-1071, 1130-1134): grid-stride passes of global warp `warp`.  Warp w
+    projects slots [w * 32 + p * stride, + 32) in pass p, stride = grid * 128; warp 0 takes the most passes, the last
+    warp of the grid the fewest."""
+    r0 = warp * 32
+    return 0 if r0 >= n_vis else -(-(n_vis - r0) // (grid * PROJ_THREADS))
+
+
+def project_min_passes(n_vis: int, grid: int) -> int:
+    """The passes of the grid's last warp: every warp of the launch strides at least this often."""
+    return project_passes(n_vis, grid, grid * PROJ_WARPS - 1)
+
+
+def project_warp_slots(n_vis: int, grid: int, warp: int, p: int) -> range:
+    """The slots (records) global warp `warp` projects in pass p."""
+    r0 = warp * 32 + p * grid * PROJ_THREADS
+    return range(min(r0, n_vis), min(r0 + 32, n_vis))
+
+
+def splat_depth_grid(n_hint: int, sm_count: int = H100_SMS) -> int:
+    """scene_depth.cu:46-49, 55-57 (launch_splat_depth, launch_splat_depth_scene): ceil(n_hint / 256) CTAs, at most 8
+    per SM, at least 1."""
+    return max(1, min(-(-n_hint // SD_THREADS), SD_CTAS_PER_SM * sm_count))
+
+
+def splat_depth_passes(n_vis: int, grid: int) -> int:
+    """scene_depth.cu:18, 33: grid-stride passes of thread 0 (the most any thread takes)."""
+    return -(-n_vis // (grid * SD_THREADS))
+
+
+def scene_keygen_grid(queued: bool, sm_count: int = H100_SMS, kg_ctas_per_sm_fit: int = COOP_CTAS_PER_SM,
+                      scene_ctas_per_sm_fit: int = COOP_CTAS_PER_SM) -> int:
+    """api.cu:271-276, 478 (bgs_context_create kg_grid / kg_grid_async, enqueue_frame): keygen_scene_kernel's CTAs, the
+    single-cloud key-gen grid capped by the scene kernel's own occupancy (`scene_ctas_per_sm_fit`, kg_scene_per_sm).
+    Queued frames run exactly sm_count CTAs (both occupancies are at least 1); a synchronous frame at most 4 per SM,
+    whatever the occupancies are."""
+    return min(coop_grid(sm_count, kg_ctas_per_sm_fit, queued), sm_count * scene_ctas_per_sm_fit)
+
+
+def keygen_cta_tiles(n: int, grid: int) -> list[tuple[int, int]]:
+    """keygen.cu:87-88: the [t0, t1) range of 2048-gaussian tiles each key-gen CTA owns (phase 1 walks them in order,
+    phase 2 expands their mask words in chunks of KG_CHUNK_TILES tiles)."""
+    tiles = -(-n // KG_TILE)
+    return [(b * tiles // grid, (b + 1) * tiles // grid) for b in range(grid)]
+
+
 def device_sm_count(device: int = 0) -> int:
     import torch
 
