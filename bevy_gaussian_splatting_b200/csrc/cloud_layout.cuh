@@ -16,7 +16,7 @@
 //                   d 0:  64 B: position | rotation | scale-opacity | 1 SH chunk
 //      f32 4D,      768 B: position | rotation | rotation_r | scale-opacity | timestamp-timescale | 36 SH chunks | 7 pad
 //    Blocks are 4, 8, 16 or 48 chunks, so a whole number of them fills a 128 B line and a warp's 32 lanes copy a block
-//    in whole rounds (project.cu: gather_blocks).  (f32 d 2 would fit 160 B, but a 10-chunk block breaks both.)
+//    in whole rounds (entry_src.cuh: Src::copy).  (f32 d 2 would fit 160 B, but a 10-chunk block breaks both.)
 //    (4D: the five geometry chunks and the first three SH chunks fill the first 128 B line, the only one the projection
 //    stages; the coefficients are fetched only for drawn splats of the colour sources that read them)
 //    The f16 second record is the packed rotation-scale-opacity words or, in the covariance layout, the

@@ -10,6 +10,7 @@
 // HBM-bound streaming kernel: 16 B read per gaussian (coalesced float4), 8 B written per
 // visible gaussian.  Compiled with -fmad=false (see project_math.cuh).
 #include "project_math.cuh"
+#include "entry_src.cuh"
 #include "launch.cuh"
 
 namespace bgs {
@@ -52,26 +53,8 @@ keygen_all_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc, ui
 constexpr int KG_WORDS_PER_TILE = KG_TILE / 32;    // 64 mask words
 constexpr int KG_CHUNK_WORDS = 1024;               // phase 2 expands 1024 words (32 K gaussians) at a time
 
-//
-// The positions come from a Src: one cloud (OneCloud) or a scene's segment table (SceneSrc), where global index i is
-// gaussian i - offset of its segment and keyed with that segment's FrameConsts.  Src::first / advance give the segment of
-// an index that only grows within a thread (both phases walk their indices upwards).
-struct OneCloud {
-    const float4* pos;
-    const FrameConsts& f;
-    __device__ __forceinline__ uint32_t first(uint32_t) const { return 0u; }
-    __device__ __forceinline__ uint32_t advance(uint32_t j, uint32_t) const { return j; }
-    __device__ __forceinline__ const FrameConsts& fc(uint32_t) const { return f; }
-    __device__ __forceinline__ const float4* at(uint32_t, uint32_t i) const { return pos + i; }
-};
-struct SceneSrc {
-    const SceneTable& t;
-    __device__ __forceinline__ uint32_t first(uint32_t i) const { return t.find(i < t.n_total ? i : t.n_total - 1u); }
-    __device__ __forceinline__ uint32_t advance(uint32_t j, uint32_t i) const { return t.advance(j, i); }
-    __device__ __forceinline__ const FrameConsts& fc(uint32_t j) const { return t.seg[j].fc; }
-    __device__ __forceinline__ const float4* at(uint32_t j, uint32_t i) const { return t.seg[j].pos + (i - t.seg[j].offset); }
-};
-
+// The positions come from a Src (entry_src.cuh): one cloud or a scene's segment table.  Both phases walk their indices
+// upwards, so a thread finds its first index's segment once and advances from there.
 template <class Src>
 __device__ __forceinline__ void keygen_coop_body(const Src& src, uint32_t n, const FrameConsts& fc, uint32_t* __restrict__ masks,
                                                  uint32_t* __restrict__ keys_out, uint32_t* __restrict__ ids_out,
@@ -90,7 +73,7 @@ __device__ __forceinline__ void keygen_coop_body(const Src& src, uint32_t n, con
     // ---- phase 1: one visibility bit per gaussian of this CTA's range, visible count
     uint32_t mine = 0u;                      // (warp-uniform: every lane counts its warp's ballots)
     uint32_t cmin_inv = 0u, cmax_p1 = 0u;   // Depth mode only: extremes of the culled indices
-    uint32_t sj = src.first(t0 * KG_TILE + warp * (32 * KG_ITEMS) + lane);
+    uint32_t sj = src.seg(t0 * KG_TILE + warp * (32 * KG_ITEMS) + lane);
     for (uint32_t tile = t0; tile < t1; ++tile) {
         // warp w covers 256 consecutive gaussians of the tile, item j = 32 consecutive ones (coalesced 512 B loads)
         const uint32_t wbase = tile * KG_TILE + warp * (32 * KG_ITEMS);
@@ -100,7 +83,7 @@ __device__ __forceinline__ void keygen_coop_body(const Src& src, uint32_t n, con
         for (int j = 0; j < KG_ITEMS; ++j) {
             const uint32_t i = wbase + j * 32 + lane;
             if (i < n) sj = src.advance(sj, i);
-            p[j] = (i < n) ? __ldcs(src.at(sj, i)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            p[j] = (i < n) ? __ldcs(src.pos_at(sj, i)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
         uint32_t myword = 0u, sk = sj0;
 #pragma unroll
@@ -144,7 +127,7 @@ __device__ __forceinline__ void keygen_coop_body(const Src& src, uint32_t n, con
     uint32_t run = block_sum_prefix<KG_THREADS>(block_cnt, b, s_red);
     if (b == G - 1 && t == 0) { ctr->n_vis = run + s_total; ctr->n_sort = run + s_total; }
     const uint32_t w_begin = t0 * KG_WORDS_PER_TILE, w_end = t1 * KG_WORDS_PER_TILE;
-    uint32_t ej = src.first(t0 * KG_TILE);
+    uint32_t ej = src.seg(t0 * KG_TILE);
     for (uint32_t wc = w_begin; wc < w_end; wc += KG_CHUNK_WORDS) {
         const uint32_t cw = min((uint32_t)KG_CHUNK_WORDS, w_end - wc);
         // each thread owns 4 consecutive words of the chunk: local prefix, then a block scan of the per-thread sums
@@ -194,7 +177,7 @@ __device__ __forceinline__ void keygen_coop_body(const Src& src, uint32_t n, con
             ej = src.advance(ej, i);
             const FrameConsts& fi = src.fc(ej);
             float pw[4];
-            keygen_world_pos(fi, __ldg(src.at(ej, i)), pw);
+            keygen_world_pos(fi, __ldg(src.pos_at(ej, i)), pw);
             const uint32_t key = depth_key(fi, true, cam_dist2(fi, pw));
             const uint32_t dst = run + e;
             keys_out[dst] = key;
@@ -232,24 +215,25 @@ keygen_scene_kernel(SceneTable tab, uint32_t* __restrict__ masks, uint32_t* __re
 // Debug hook: rebuild the reference's full sorted_entry_buffer (sort/mod.rs:323-329) from the
 // compacted result: [0, n_vis) = sorted visible entries, then every culled index ascending
 // with key 0xFFFFFFFF >> shift.  Single block per call chunk; not on the hot path.
-__global__ void culled_flags_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc,
-                                    uint32_t* __restrict__ flags) {
+template <class Src>
+__device__ __forceinline__ void culled_flags_body(const Src& src, uint32_t n, uint32_t* __restrict__ flags) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float4 p = pos[i];
+    const uint32_t j = src.seg(i);
+    const FrameConsts& fc = src.fc(j);
+    const float4 p = *src.pos_at(j, i);
     float pw[4], ndc[2];
     mat4_point(fc.model, p.x, p.y, p.z, pw);
     flags[i] = in_frustum(fc, pw, ndc) ? 0u : 1u;
 }
 
+__global__ void culled_flags_kernel(const float4* __restrict__ pos, uint32_t n, FrameConsts fc,
+                                    uint32_t* __restrict__ flags) {
+    culled_flags_body(OneCloud{pos, fc}, n, flags);
+}
+
 __global__ void culled_flags_scene_kernel(SceneTable tab, uint32_t* __restrict__ flags) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= tab.n_total) return;
-    const SceneSeg& s = tab.seg[tab.find(i)];
-    const float4 p = s.pos[i - s.offset];
-    float pw[4], ndc[2];
-    mat4_point(s.fc.model, p.x, p.y, p.z, pw);
-    flags[i] = in_frustum(s.fc, pw, ndc) ? 0u : 1u;
+    culled_flags_body(SceneSrc{tab}, tab.n_total, flags);
 }
 
 void launch_keygen_all(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* keys_out, uint32_t* ids_out,

@@ -15,6 +15,7 @@
 // geometry (3DGS USE_AABB conic, 3DGS USE_OBB, 2DGS surfel) and its colour source (SH, Depth, Normal, Position).
 // Geometry (centre, OBB uv rows, pixel bbox) is bit-exact vs the oracle: compiled -fmad=false.
 #include "project_math.cuh"
+#include "entry_src.cuh"
 #include "launch.cuh"
 
 namespace bgs {
@@ -65,42 +66,11 @@ __device__ __forceinline__ void make_bbox(float cx, float cy, float hx, float hy
 // touches exactly its own line(s) instead of 3-4 partially used ones of the reference's planes.
 //
 // A warp gathers the blocks of 32 consecutive entries of the index list into its own shared-memory stage with
-// coalesced 16 B asynchronous copies (cp.async.cg: no staging registers, L1 bypassed, every line is used once): a
-// lane's copy k moves piece (32 k + lane) % NP of entry (32 k + lane) / NP, so NP consecutive lanes read one block
-// front to back.  NP = CH (the whole block) when the colour source reads the SH coefficients, else GEO pieces:
-// position, rotation, scale and opacity (f32: plus the first SH piece, which shares scale_opacity's 32 B sector).
-// Piece p of entry g sits at 16 B unit g * CH + slot(p, g) (stage_slot): the eight lanes of a quarter warp that read
-// the same piece of their own entries hit eight different 16 B bank groups, and so do the copies' stores.
-__device__ __forceinline__ void cp_async16(uint4* dst_shared, const uint4* src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst_shared)), "l"(src)
-                 : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-// Blocks of 8 or more chunks: p ^ (g & 7) (a permutation of each aligned group of 8 pieces).  4-chunk blocks: two
-// entries share a 128 B row of banks, so p ^ ((g >> 1) & 3) -- entries g of one quarter warp take the 8 combinations of
-// (g & 1, (g >> 1) & 3), hence 8 bank groups; a copy round's 8 lanes move pieces 0..3 of an even and the next odd entry,
-// the 8 units of one row.
-template <int CH>
-__device__ __forceinline__ int stage_slot(int p, int g) {
-    static_assert(CH % 8 == 0 || CH == 4, "blocks of 4 or a multiple of 8 chunks");
-    if constexpr (CH == 4) return p ^ ((g >> 1) & 3);
-    else return p ^ (g & 7);
-}
-
-template <int CH, int NP>
-__device__ __forceinline__ void gather_blocks(const uint4* __restrict__ blocks, uint32_t id, uint32_t n_valid,
-                                              uint4* stage, int lane) {
-    static_assert(32 % NP == 0 && NP <= CH, "NP lanes per block");
-#pragma unroll
-    for (int k = 0; k < NP; ++k) {
-        const int g = (32 * k + lane) / NP, p = lane % NP;
-        const uint32_t gid = __shfl_sync(0xFFFFFFFFu, id, g);
-        if ((uint32_t)g < n_valid) cp_async16(stage + g * CH + stage_slot<CH>(p, g), blocks + (size_t)gid * CH + p);
-    }
-}
+// coalesced 16 B asynchronous copies (cp.async.cg: no staging registers, L1 bypassed, every line is used once; the
+// source's copy, entry_src.cuh).  NP = CH (the whole block) when the colour source reads the SH coefficients, else GEO
+// pieces: position, rotation, scale and opacity (f32: plus the first SH piece, which shares scale_opacity's 32 B
+// sector).  Piece p of entry g sits at 16 B unit g * CH + stage_slot<CH>(p, g): the eight lanes of a quarter warp that
+// read the same piece of their own entries hit eight different 16 B bank groups, and so do the copies' stores.
 
 // entry g's attributes out of a stage, the S_d SH floats into sh (the covariance layout's record arrives in q and so as
 // its lanes fall)
@@ -192,9 +162,9 @@ void launch_repack(CloudLayout layout, uint32_t sh_degree, const void* sh, const
 // RasterizeMode::Depth (gaussian.wgsl:329-349): min distance from sorted[N-1], max from sorted[1] of the
 // reference's FULL sorted buffer (culled entries keyed all-ones sit at its end, in index order) -- literal,
 // including the [1] (not [0]) and the fact that the "nearest" entry is a culled gaussian whenever one exists.
-__global__ void depth_range_kernel(const float4* __restrict__ pos, uint32_t n, const uint32_t* __restrict__ sorted_payload,
-                                   const uint32_t* __restrict__ slot_ids /* null: payload is the gaussian index */,
-                                   FrameCounters* __restrict__ ctr, FrameConsts fc) {
+template <class Src>
+__device__ __forceinline__ void depth_range_body(const Src& src, uint32_t n, const uint32_t* __restrict__ sorted_payload,
+                                                 const uint32_t* __restrict__ slot_ids, FrameCounters* __restrict__ ctr) {
     if (threadIdx.x != 0 || blockIdx.x != 0 || n < 2u) return;
     const uint32_t n_vis = ctr->n_vis, n_sorted = ctr->n_sort;
     auto id_at = [&](uint32_t i) { const uint32_t p = sorted_payload[i]; return slot_ids ? slot_ids[p] : p; };
@@ -207,13 +177,28 @@ __global__ void depth_range_kernel(const float4* __restrict__ pos, uint32_t n, c
         last = (n - n_vis) >= 1u ? cmax : id_at(n - 1u);
     }
     auto dist = [&](uint32_t id) {
-        const float4 p = pos[id];
+        const uint32_t j = src.seg(id);
+        const FrameConsts& fc = src.fc(j);
+        const float4 p = *src.pos_at(j, id);
         float pw[4];
         mat4_point(fc.model, p.x, p.y, p.z, pw);
         return sqrtf(cam_dist2(fc, pw));
     };
     ctr->depth_min = dist(last);
     ctr->depth_max = dist(first);
+}
+
+__global__ void depth_range_kernel(const float4* __restrict__ pos, uint32_t n, const uint32_t* __restrict__ sorted_payload,
+                                   const uint32_t* __restrict__ slot_ids /* null: payload is the gaussian index */,
+                                   FrameCounters* __restrict__ ctr, FrameConsts fc) {
+    depth_range_body(OneCloud{pos, fc}, n, sorted_payload, slot_ids, ctr);
+}
+
+// bgs_render_scene (compact frames only: it refuses SORT_ALL); the SORT_ALL branch takes the compact one's ends when
+// every gaussian is visible
+__global__ void depth_range_scene_kernel(SceneTable tab, const uint32_t* __restrict__ sorted_payload,
+                                         const uint32_t* __restrict__ slot_ids, FrameCounters* __restrict__ ctr) {
+    depth_range_body(SceneSrc{tab}, tab.n_total, sorted_payload, slot_ids, ctr);
 }
 
 // gaussian.wgsl:228-232: cutoff = sqrt(max(9 + 2 ln(opacity), 1e-6)) (fixed-series ln, see project_math.cuh)
@@ -679,51 +664,76 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
 // faster than 6 or 8 per SM (DESIGN.md section 9).
 constexpr int PROJ_THREADS = 128, PROJ_WARPS = PROJ_THREADS / 32, PROJ_MIN_CTAS = 4;
 
-// The projection loop of both kernels.  Record r of n_vis is entry r of the index list:
-//   by_slot: r is a compact slot (ascending gaussian index; runs concurrently with the depth sort)
-//   else   : r is a front-to-back rank, the list is the far->near sorted index list
+// The projection loop of every projection kernel.  Record r of n_vis is entry r of the source's list (entry_src.cuh):
+//   one cloud, by_slot: r is a compact slot (ascending gaussian index; runs concurrently with the depth sort)
+//   one cloud, else   : r is a front-to-back rank, the list is the far->near sorted index list
+//   a scene           : r is a compact slot, its entry a global index; the launch projects the entries whose segment
+//                       Src::mine covers, each with its segment's constants
 // The grid is persistent and each warp strides over groups of 32 entries with two groups in flight: once the lanes
 // hold group i's attributes in registers, the copies of group i + 1 start filling the warp's stage and the list
 // entries of group i + 2 are on their way into a register, so both dependent memory latencies sit under project_one.
-template <bool F16, uint32_t D, bool MODES2>
-__device__ __forceinline__ void project_groups(const void* __restrict__ blocks, const uint32_t* __restrict__ index_list,
-                                               int by_slot, const FrameCounters* __restrict__ ctr, const FrameConsts& fc,
-                                               bool need_sh, SplatRec* __restrict__ recs, float4* __restrict__ extra,
-                                               const float* __restrict__ cutoff_tab, float4* __restrict__ aux,
-                                               const ModeConsts& mc) {
-    using A = Attr<F16, D>;
-    constexpr int CH = A::CH;
-    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * CH];   // degree 3: f16 16 KB, f32 32 KB
+// Geo is the splat geometry: chunks per entry in the stage (SCH) and in the block (BCH), the pieces copied when the
+// colour source does not read the SH coefficients (GEO), read (an entry's position, q, so and EXT more floats out of
+// the stage) and project (its record).  The registers are plain arrays of this loop: gathered into a struct, they
+// change how ptxas allocates the benchmarked project_kernel.
+template <class Src, class Geo>
+__device__ __forceinline__ void project_loop(const Src& src, const Geo& geo, const FrameCounters* __restrict__ ctr,
+                                             const ModeConsts& mc) {
+    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * Geo::SCH];   // 3D degree 3: f16 16 KB, f32 32 KB; 4D 16 KB
     const int lane = threadIdx.x & 31;
     uint4* const stage = s_stages[threadIdx.x >> 5];
     const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
-    auto list_id = [&](uint32_t r) {
-        return r < n_vis ? (by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r))) : 0u;
-    };
-    auto gather = [&](uint32_t r0, uint32_t id) {   // one commit group per call, empty past the list's end
+    auto gather = [&](uint32_t r0, uint32_t e) {   // one commit group per call, empty past the list's end
         const uint32_t n_valid = r0 < n_vis ? n_vis - r0 : 0u;
-        const uint4* b = reinterpret_cast<const uint4*>(blocks);
-        if (need_sh) gather_blocks<CH, CH>(b, id, n_valid, stage, lane);
-        else gather_blocks<CH, A::GEO>(b, id, n_valid, stage, lane);
+        if (geo.need_sh) src.template copy<Geo::SCH, Geo::SCH, Geo::BCH>(e, n_valid, stage, lane);
+        else src.template copy<Geo::SCH, Geo::GEO, Geo::BCH>(e, n_valid, stage, lane);
         cp_async_commit();
     };
     uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
-    gather(r0, list_id(r0 + lane));
-    uint32_t id_next = list_id(r0 + stride + lane);
+    uint32_t e = src.entry(r0 + lane, n_vis);
+    gather(r0, e);
+    uint32_t e_next = src.entry(r0 + stride + lane, n_vis);
     for (; r0 < n_vis; r0 += stride) {
         cp_async_wait<0>();
         __syncwarp();   // every lane's copies of this group have landed
-        const uint32_t r = r0 + lane;
-        float sh[sh_floats(D)], q[4], so[4];
+        const uint32_t r = r0 + lane, j = src.seg(e);
+        const bool mine = r < n_vis && (!Src::SEGMENTED || src.mine(j));
+        float ext[Geo::EXT], q[4], so[4];
         uint32_t op_bits = 0u;
         float4 p4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (r < n_vis) p4 = A::load(stage, lane, sh, q, so, need_sh, op_bits);
+        if (mine) p4 = geo.read(stage, lane, ext, q, so, op_bits);
         __syncwarp();   // the stage is read out before the next group's copies overwrite it
-        gather(r0 + stride, id_next);
-        id_next = list_id(r0 + 2u * stride + lane);
-        if (r < n_vis) project_one<F16, D, MODES2>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc);
+        const uint32_t e_mine = e;
+        gather(r0 + stride, e_next);
+        e = e_next;
+        e_next = src.entry(r0 + 2u * stride + lane, n_vis);
+        if (mine) geo.project(src, j, e_mine, r, p4, q, so, ext, op_bits, mc);
     }
 }
+
+// The 3D and 2D splats: Attr<F16, D>'s blocks and project_one's record.  MODES2: project_modes_kernel's colour sources.
+template <bool F16, uint32_t D, bool MODES2>
+struct Geo3d {
+    using A = Attr<F16, D>;
+    static constexpr int SCH = A::CH, BCH = A::CH, GEO = A::GEO, EXT = sh_floats(D);
+    const FrameCounters* ctr;
+    bool need_sh;   // the colour source reads the SH coefficients
+    SplatRec* recs;
+    float4* extra;
+    const float* cutoff_tab;
+    float4* aux;
+
+    __device__ __forceinline__ float4 read(const uint4* stage, int lane, float* sh, float q[4], float so[4], uint32_t& op_bits) const {
+        return A::load(stage, lane, sh, q, so, need_sh, op_bits);
+    }
+    template <class Src>
+    __device__ __forceinline__ void project(const Src& src, uint32_t j, uint32_t, uint32_t r, float4 p4, const float q[4],
+                                            const float so[4], const float* sh, uint32_t op_bits, const ModeConsts& mc) const {
+        const FrameConsts& fc = src.fc(j);
+        project_one<F16, D, MODES2>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc,
+                                    MODES2 && Src::SEGMENTED && fc.rasterize_mode == BGS_RASTERIZE_VELOCITY);
+    }
+};
 
 template <bool F16, uint32_t D>
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
@@ -731,8 +741,9 @@ project_kernel(const void* __restrict__ blocks, const uint32_t* __restrict__ ind
                const FrameCounters* __restrict__ ctr, FrameConsts fc, SplatRec* __restrict__ recs,
                float4* __restrict__ extra /* 4 x float4 per record, 2DGS + USE_AABB only */, const float* __restrict__ cutoff_tab,
                float4* __restrict__ aux /* 2 x float4 per record (depth rgb, normal rgb), bgs_render_aux only */) {
-    project_groups<F16, D, false>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs, extra,
-                               cutoff_tab, aux, ModeConsts{});
+    project_loop(OneCloud{nullptr, fc, static_cast<const uint4*>(blocks), index_list, by_slot},
+                 Geo3d<F16, D, false>{ctr, fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs, extra, cutoff_tab, aux},
+                 ctr, ModeConsts{});
 }
 
 // project_kernel for RasterizeMode::Classification / OpticalFlow (bgs_render_ex): the same records but for r, g, b.  A
@@ -743,74 +754,15 @@ project_modes_kernel(const void* __restrict__ blocks, const uint32_t* __restrict
                      const FrameCounters* __restrict__ ctr, FrameConsts fc, ModeConsts mc, SplatRec* __restrict__ recs,
                      float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
     // OpticalFlow reads the position only
-    project_groups<F16, D, true>(blocks, index_list, by_slot, ctr, fc, fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs,
-                              extra, cutoff_tab, nullptr, mc);
+    project_loop(OneCloud{nullptr, fc, static_cast<const uint4*>(blocks), index_list, by_slot},
+                 Geo3d<F16, D, true>{ctr, fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs, extra, cutoff_tab, nullptr},
+                 ctr, mc);
 }
 
 // ---- bgs_render_scene: the projection over a segment table (common.cuh).  Record r is compact slot r, whose global
 // index slot_ids[r] lies in segment j: its block is gaussian slot_ids[r] - offset of cloud j's blocks, and project_one
 // runs with segment j's FrameConsts, so the record is the one a frame of cloud j alone would write.  One launch per
 // kernel instantiation (`group`): its warps stride over every slot and project those whose cloud is in the group.
-template <int CH, int NP>
-__device__ __forceinline__ void gather_block_ptrs(const uint4* block /* this lane's entry; null: none */, uint4* stage, int lane) {
-#pragma unroll
-    for (int k = 0; k < NP; ++k) {
-        const int g = (32 * k + lane) / NP, p = lane % NP;
-        const uint4* src = reinterpret_cast<const uint4*>(
-            __shfl_sync(0xFFFFFFFFu, (unsigned long long)reinterpret_cast<uintptr_t>(block), g));
-        if (src) cp_async16(stage + g * CH + stage_slot<CH>(p, g), src + p);
-    }
-}
-
-template <bool F16, uint32_t D, bool MODES2>
-__device__ __forceinline__ void project_scene_groups(const SceneTable& tab, uint32_t group, const uint32_t* __restrict__ slot_ids,
-                                                     const FrameCounters* __restrict__ ctr, bool need_sh,
-                                                     SplatRec* __restrict__ recs, float4* __restrict__ extra,
-                                                     const float* __restrict__ cutoff_tab, const ModeConsts& mc) {
-    using A = Attr<F16, D>;
-    constexpr int CH = A::CH;
-    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * CH];
-    const int lane = threadIdx.x & 31;
-    uint4* const stage = s_stages[threadIdx.x >> 5];
-    const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
-    constexpr uint32_t NONE = 0xFFFFFFFFu;
-    auto list_id = [&](uint32_t r) { return r < n_vis ? __ldg(slot_ids + r) : NONE; };   // slot r's global index
-    // global index g's block, null when there is none or its cloud is another launch's
-    auto block_of = [&](uint32_t g) -> const uint4* {
-        if (g == NONE) return nullptr;
-        const SceneSeg& s = tab.seg[tab.find(g)];
-        if (s.group != group) return nullptr;
-        return static_cast<const uint4*>(s.blocks) + (size_t)(g - s.offset) * CH;
-    };
-    auto gather = [&](uint32_t g) {   // one commit group per call
-        const uint4* block = block_of(g);
-        if (need_sh) gather_block_ptrs<CH, CH>(block, stage, lane);
-        else gather_block_ptrs<CH, A::GEO>(block, stage, lane);
-        cp_async_commit();
-    };
-    uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
-    uint32_t g_cur = list_id(r0 + lane);
-    gather(g_cur);
-    uint32_t g_next = list_id(r0 + stride + lane);
-    for (; r0 < n_vis; r0 += stride) {
-        cp_async_wait<0>();
-        __syncwarp();   // every lane's copies of this group have landed
-        const uint32_t r = r0 + lane;
-        const uint32_t j = g_cur == NONE ? 0u : tab.find(g_cur);
-        const bool mine = g_cur != NONE && tab.seg[j].group == group;
-        float sh[sh_floats(D)], q[4], so[4];
-        uint32_t op_bits = 0u;
-        float4 p4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (mine) p4 = A::load(stage, lane, sh, q, so, need_sh, op_bits);
-        __syncwarp();   // the stage is read out before the next group's copies overwrite it
-        gather(g_next);
-        g_cur = g_next;
-        g_next = list_id(r0 + 2u * stride + lane);
-        if (mine)
-            project_one<F16, D, MODES2>(tab.seg[j].fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, nullptr, mc,
-                                        MODES2 && tab.seg[j].fc.rasterize_mode == BGS_RASTERIZE_VELOCITY);
-    }
-}
 
 // (the f32 blocks of degree 2 and 3 hold 48 SH floats in registers beside the segment's constants: 3 CTAs per SM keeps
 // them from spilling)
@@ -821,36 +773,19 @@ template <bool F16, uint32_t D>
 __global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
 project_scene_kernel(SceneTable tab, uint32_t group, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
                      SplatRec* __restrict__ recs, float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
-    project_scene_groups<F16, D, false>(tab, group, slot_ids, ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs,
-                                        extra, cutoff_tab, ModeConsts{});
+    project_loop(SceneSrc{tab, 1u << group, slot_ids},
+                 Geo3d<F16, D, false>{ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs, extra, cutoff_tab, nullptr},
+                 ctr, ModeConsts{});
 }
 template <bool F16, uint32_t D>
 __global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
 project_modes_scene_kernel(SceneTable tab, uint32_t group, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
                            const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs, float4* __restrict__ extra,
                            const float* __restrict__ cutoff_tab) {
-    project_scene_groups<F16, D, true>(tab, group, slot_ids, ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION,
-                                       recs, extra, cutoff_tab, mc);
-}
-
-// depth_range_kernel over a segment table (compact frames only: bgs_render_scene refuses SORT_ALL)
-__global__ void depth_range_scene_kernel(SceneTable tab, const uint32_t* __restrict__ sorted_payload,
-                                         const uint32_t* __restrict__ slot_ids, FrameCounters* __restrict__ ctr) {
-    const uint32_t n = tab.n_total;
-    if (threadIdx.x != 0 || blockIdx.x != 0 || n < 2u) return;
-    const uint32_t n_vis = ctr->n_vis;
-    const uint32_t cmin = 0xFFFFFFFFu - ctr->culled_min_inv, cmax = ctr->culled_max_p1 - 1u;
-    const uint32_t first = n_vis >= 2u ? slot_ids[sorted_payload[1]] : cmin;
-    const uint32_t last = (n - n_vis) >= 1u ? cmax : slot_ids[sorted_payload[n - 1u]];
-    auto dist = [&](uint32_t g) {
-        const SceneSeg& s = tab.seg[tab.find(g)];
-        const float4 p = s.pos[g - s.offset];
-        float pw[4];
-        mat4_point(s.fc.model, p.x, p.y, p.z, pw);
-        return sqrtf(cam_dist2(s.fc, pw));
-    };
-    ctr->depth_min = dist(last);
-    ctr->depth_max = dist(first);
+    project_loop(SceneSrc{tab, 1u << group, slot_ids},
+                 Geo3d<F16, D, true>{ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs, extra, cutoff_tab,
+                                     nullptr},
+                 ctr, mc);
 }
 
 void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payload, const uint32_t* slot_ids, FrameCounters* ctr,
@@ -866,9 +801,7 @@ uint32_t project_group(CloudLayout layout, uint32_t sh_degree) {
 void launch_project_scene(const SceneTable& tab, uint32_t group, const uint32_t* slot_ids, const FrameCounters* ctr,
                           SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
                           const ModeConsts* modes, cudaStream_t stream) {
-    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
-    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
-    if (grid < 1u) grid = 1u;
+    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     with_layout_degree(group & 1u ? CloudLayout::F16 : CloudLayout::F32, group >> 1, [&](auto L, auto Dt) {
         constexpr CloudLayout Lv = decltype(L)::value;
         constexpr uint32_t D = decltype(Dt)::value;
@@ -882,7 +815,6 @@ void launch_project_scene(const SceneTable& tab, uint32_t group, const uint32_t*
         }
     });
 }
-
 // ---- Gaussian4d (bgs_render_4d; the rule is include/bgs.h's).  Matrices [col][row], as WGSL indexes them.
 
 // gaussian_4d.wgsl:37-130: Sigma of the 4D gaussian conditioned on time t
@@ -1040,122 +972,58 @@ __device__ __forceinline__ void project_one_4d(const FrameConsts& fc, const Mode
 }
 
 // The 4D block is 768 B: a warp stages only each entry's first 128 B line (position, both rotations, scale-opacity,
-// timestamp-timescale; 4 KB per warp) with the coalesced copies of project_groups, piece p of entry g at
-// g * GEO4 + (p ^ (g & 7)).  The coefficients stay in global memory until a drawn splat's colour needs them.
+// timestamp-timescale; 4 KB per warp), piece p of entry g at g * GEO4 + stage_slot<GEO4>(p, g).  The coefficients stay
+// in global memory until a drawn splat's colour needs them.
 constexpr int CH4 = (int)chunks(CloudLayout::F32x4D, SH_DEGREE_MAX), GEO4 = 8;
+struct Geo4d {
+    static constexpr int SCH = GEO4, BCH = CH4, GEO = GEO4, EXT = 8;
+    static constexpr bool need_sh = false;
+    const FrameCounters* ctr;
+    SplatRec* recs;
+    float* depths;   // depth-tested frames only
+
+    // q: rotation, so: scale-opacity, ext: rotation_r, then timestamp-timescale
+    __device__ __forceinline__ float4 read(const uint4* stage, int lane, float ext[8], float q[4], float so[4], uint32_t&) const {
+        auto piece = [&](int p, float* out) {
+            const uint4 v = stage[lane * GEO4 + stage_slot<GEO4>(p, lane)];
+            out[0] = __uint_as_float(v.x); out[1] = __uint_as_float(v.y); out[2] = __uint_as_float(v.z); out[3] = __uint_as_float(v.w);
+        };
+        float p4[4];
+        piece(POS_CHUNK, p4); piece(SECOND_CHUNK, q); piece(ROT_R_CHUNK, ext); piece(SO_4D_CHUNK, so); piece(TT_CHUNK, ext + 4);
+        return make_float4(p4[0], p4[1], p4[2], p4[3]);
+    }
+    template <class Src>
+    __device__ __forceinline__ void project(const Src& src, uint32_t j, uint32_t e, uint32_t r, float4 p4, const float q[4],
+                                            const float so[4], const float ext[8], uint32_t, const ModeConsts& mc) const {
+        project_one_4d(src.fc(j), mc, src.tc(j), ctr, r, p4, q, ext, so, ext + 4,
+                       src.template block_at<CH4>(j, e) + sh_first(CloudLayout::F32x4D), recs, depths);
+    }
+};
+
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_4d_kernel(const uint4* __restrict__ blocks, const uint32_t* __restrict__ index_list, int by_slot,
                   const FrameCounters* __restrict__ ctr, FrameConsts fc, ModeConsts mc, TemporalConsts tc,
                   SplatRec* __restrict__ recs, float* __restrict__ depths /* depth-tested frames only */) {
-    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * GEO4];
-    const int lane = threadIdx.x & 31;
-    uint4* const stage = s_stages[threadIdx.x >> 5];
-    const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
-    auto list_id = [&](uint32_t r) {
-        return r < n_vis ? (by_slot ? __ldg(index_list + r) : __ldg(index_list + (n_vis - 1u - r))) : 0u;
-    };
-    auto gather = [&](uint32_t r0, uint32_t id) {   // one commit group per call, empty past the list's end
-        const uint32_t n_valid = r0 < n_vis ? n_vis - r0 : 0u;
-#pragma unroll
-        for (int k = 0; k < GEO4; ++k) {
-            const int g = (32 * k + lane) / GEO4, p = lane % GEO4;
-            const uint32_t gid = __shfl_sync(0xFFFFFFFFu, id, g);
-            if ((uint32_t)g < n_valid) cp_async16(stage + g * GEO4 + (p ^ (g & 7)), blocks + (size_t)gid * CH4 + p);
-        }
-        cp_async_commit();
-    };
-    uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
-    uint32_t id = list_id(r0 + lane);
-    gather(r0, id);
-    uint32_t id_next = list_id(r0 + stride + lane);
-    for (; r0 < n_vis; r0 += stride) {
-        cp_async_wait<0>();
-        __syncwarp();
-        const uint32_t r = r0 + lane;
-        auto piece = [&](int p) {
-            const uint4 v = stage[lane * GEO4 + (p ^ (lane & 7))];
-            return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
-        };
-        const float4 p4 = piece(POS_CHUNK), a = piece(SECOND_CHUNK), b = piece(ROT_R_CHUNK), c = piece(SO_4D_CHUNK),
-                     d = piece(TT_CHUNK);
-        __syncwarp();   // the stage is read out before the next group's copies overwrite it
-        const uint32_t my_id = id;
-        gather(r0 + stride, id_next);
-        id = id_next;
-        id_next = list_id(r0 + 2u * stride + lane);
-        if (r < n_vis) {
-            const float ql[4] = {a.x, a.y, a.z, a.w}, qr[4] = {b.x, b.y, b.z, b.w}, so[4] = {c.x, c.y, c.z, c.w},
-                        tt[4] = {d.x, d.y, d.z, d.w};
-            project_one_4d(fc, mc, tc, ctr, r, p4, ql, qr, so, tt, blocks + (size_t)my_id * CH4 + sh_first(CloudLayout::F32x4D),
-                           recs, depths);
-        }
-    }
+    project_loop(OneCloud{nullptr, fc, blocks, index_list, by_slot, &tc}, Geo4d{ctr, recs, depths}, ctr, mc);
 }
 
 void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                        const FrameConsts& fc, const ModeConsts& mc, const TemporalConsts& tc, SplatRec* recs, float* depths,
                        uint32_t n_hint, int sm_count, cudaStream_t stream) {
-    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
-    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
-    if (grid < 1u) grid = 1u;
+    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     project_4d_kernel<<<grid, PROJ_THREADS, 0, stream>>>(static_cast<const uint4*>(blocks), index_list, by_slot, ctr, fc, mc, tc,
                                                          recs, depths);
 }
 
 // ---- bgs_render_scene_4d: project_4d_kernel over a segment table.  Record r is compact slot r; its global index lies in
 // segment j, and only the segments of PROJECT_GROUP_4D are this launch's (the 3D ones are launch_project_scene's).  Each
-// lane stages its own entry's first 128 B line from its own cloud's blocks (gather_block_ptrs), then project_one_4d runs
-// with segment j's FrameConsts and times, so the record and splat depth are those bgs_render_4d writes for that cloud.
+// lane stages its own entry's first 128 B line from its own cloud's blocks, then project_one_4d runs with segment j's
+// FrameConsts and times, so the record and splat depth are those bgs_render_4d writes for that cloud.
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_4d_scene_kernel(SceneTable tab, SceneTimes times, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
                         const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs,
                         float* __restrict__ depths /* depth-tested frames only */) {
-    __shared__ __align__(16) uint4 s_stages[PROJ_WARPS][32 * GEO4];
-    const int lane = threadIdx.x & 31;
-    uint4* const stage = s_stages[threadIdx.x >> 5];
-    const uint32_t n_vis = ctr->n_vis, stride = gridDim.x * PROJ_THREADS;
-    constexpr uint32_t NONE = 0xFFFFFFFFu;
-    auto list_id = [&](uint32_t r) { return r < n_vis ? __ldg(slot_ids + r) : NONE; };   // slot r's global index
-    // global index g's block, null when there is none or its cloud is not a 4D one
-    auto block_of = [&](uint32_t g) -> const uint4* {
-        if (g == NONE) return nullptr;
-        const SceneSeg& s = tab.seg[tab.find(g)];
-        if (s.group != PROJECT_GROUP_4D) return nullptr;
-        return static_cast<const uint4*>(s.blocks) + (size_t)(g - s.offset) * CH4;
-    };
-    auto gather = [&](uint32_t g) {   // one commit group per call
-        gather_block_ptrs<GEO4, GEO4>(block_of(g), stage, lane);   // (slot p ^ (g & 7), as project_4d_kernel's)
-        cp_async_commit();
-    };
-    uint32_t r0 = (blockIdx.x * PROJ_WARPS + (threadIdx.x >> 5)) * 32u;
-    uint32_t g_cur = list_id(r0 + lane);
-    gather(g_cur);
-    uint32_t g_next = list_id(r0 + stride + lane);
-    for (; r0 < n_vis; r0 += stride) {
-        cp_async_wait<0>();
-        __syncwarp();   // every lane's copies of this group have landed
-        const uint32_t r = r0 + lane;
-        const uint32_t j = g_cur == NONE ? 0u : tab.find(g_cur);
-        const bool mine = g_cur != NONE && tab.seg[j].group == PROJECT_GROUP_4D;
-        auto piece = [&](int p) {
-            const uint4 v = stage[lane * GEO4 + (p ^ (lane & 7))];
-            return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
-        };
-        const float4 p4 = piece(POS_CHUNK), a = piece(SECOND_CHUNK), b = piece(ROT_R_CHUNK), c = piece(SO_4D_CHUNK),
-                     d = piece(TT_CHUNK);
-        __syncwarp();   // the stage is read out before the next group's copies overwrite it
-        const uint32_t g_mine = g_cur;
-        gather(g_next);
-        g_cur = g_next;
-        g_next = list_id(r0 + 2u * stride + lane);
-        if (mine) {
-            const SceneSeg& s = tab.seg[j];
-            const float ql[4] = {a.x, a.y, a.z, a.w}, qr[4] = {b.x, b.y, b.z, b.w}, so[4] = {c.x, c.y, c.z, c.w},
-                        tt[4] = {d.x, d.y, d.z, d.w};
-            const uint4* sh = static_cast<const uint4*>(s.blocks) + (size_t)(g_mine - s.offset) * CH4 + sh_first(CloudLayout::F32x4D);
-            project_one_4d(s.fc, mc, times.t[j], ctr, r, p4, ql, qr, so, tt, sh, recs, depths);
-        }
-    }
+    project_loop(SceneSrc{tab, 1u << PROJECT_GROUP_4D, slot_ids, &times}, Geo4d{ctr, recs, depths}, ctr, mc);
 }
 // sm_90 takes up to 32764 B of kernel parameters (CUDA >= 12.1): the table (~22 KB), the times (768 B), the extras and
 // four pointers
@@ -1165,12 +1033,9 @@ static_assert(sizeof(SceneTable) + sizeof(SceneTimes) + sizeof(ModeConsts) + 4 *
 void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const uint32_t* slot_ids, const FrameCounters* ctr,
                              const ModeConsts& mc, SplatRec* recs, float* depths, uint32_t n_hint, int sm_count,
                              cudaStream_t stream) {
-    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
-    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
-    if (grid < 1u) grid = 1u;
+    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     project_4d_scene_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, times, mc, slot_ids, ctr, recs, depths);
 }
-
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
                         FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream) {
     depth_range_kernel<<<1, 32, 0, stream>>>(pos, n, sorted_payload, slot_ids, ctr, fc);
@@ -1181,9 +1046,7 @@ void launch_project(CloudLayout layout, uint32_t sh_degree, const void* blocks, 
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes, cudaStream_t stream) {
     // a persistent grid: as many CTAs as the launch bound lets the SMs hold, fewer when the hint (last frame's visible
     // count + head-room) has less than one group of 32 entries for each warp; the loop strides, so any n_vis is correct
-    uint32_t grid = (n_hint + PROJ_THREADS - 1) / PROJ_THREADS;
-    if (grid > (uint32_t)(PROJ_MIN_CTAS * sm_count)) grid = (uint32_t)(PROJ_MIN_CTAS * sm_count);
-    if (grid < 1u) grid = 1u;
+    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     // (both f16 layouts run the F16 kernels: the covariance record differs only in fc.cov_pre)
     with_layout_degree(layout, sh_degree, [&](auto L, auto Dt) {
         constexpr CloudLayout Lv = decltype(L)::value;
