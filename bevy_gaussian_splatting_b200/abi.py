@@ -85,6 +85,19 @@ class bgs_time_window(C.Structure):
     ]
 
 
+class bgs_entity_settings(C.Structure):
+    """One entity's own CloudSettings in a bgs_render_entities call."""
+    _fields_ = [
+        ("gaussian_mode", C.c_uint32),
+        ("rasterize_mode", C.c_uint32),
+        ("aabb", C.c_uint32),
+        ("opacity_adaptive_radius", C.c_uint32),
+        ("draw_mode", C.c_uint32),
+        ("num_classes", C.c_uint32),
+        ("window", bgs_time_window),
+    ]
+
+
 class bgs_frame_stats(C.Structure):
     _fields_ = [
         ("n", C.c_uint32),
@@ -151,6 +164,9 @@ SYMBOLS = [
     ("bgs_render_scene", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
                                    C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
     ("bgs_render_scene_4d", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_time_window), C.c_uint32,
+                                      C.POINTER(bgs_view), C.POINTER(bgs_settings), C.POINTER(bgs_render_extras),
+                                      C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
+    ("bgs_render_entities", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), C.c_uint32,
                                       C.POINTER(bgs_view), C.POINTER(bgs_settings), C.POINTER(bgs_render_extras),
                                       C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,

@@ -473,7 +473,13 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     // ---- stage 1: key-gen (+ stable compaction of the visible set)
     // compact mode: keys[0][slot], slot_ids[slot] = gaussian index, vals[0][slot] = slot (sort payload)
     // SORT_ALL    : keys[0][i], vals[0][i] = i (payload is the gaussian index itself)
-    if (scene) {   // (scenes are compact frames)
+    if (scene && scene->entities && p.depth_range && scene->tab.seg[0].fc.rasterize_mode != BGS_RASTERIZE_DEPTH) {
+        // (key-gen gathers the culled ends for the Depth range when segment 0 is in Depth mode: some other entity is)
+        SceneTable kt = scene->tab;
+        kt.seg[0].fc.rasterize_mode = BGS_RASTERIZE_DEPTH;
+        CU(c, launch_keygen_scene(kt, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt, c->ctr, c->hist,
+                                  p.depth_passes, std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
+    } else if (scene) {   // (scenes are compact frames)
         CU(c, launch_keygen_scene(scene->tab, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt, c->ctr,
                                   c->hist, p.depth_passes, std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
     } else if (p.by_slot) {
@@ -508,7 +514,22 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     }
     CU(c, cudaEventRecord(c->ev_p0, ps));
     bool scene_3d = false;   // a scene lists a non-4D cloud (whose splat depths splat_depth_scene writes)
-    if (scene) {   // one launch per projection kernel the scene's clouds need
+    if (scene && scene->entities) {   // entities that disagree: each segment with its own settings and num_classes
+        const ModeConsts mc = modes ? *modes : ModeConsts{};
+        for (size_t i = 0; i < scene->groups.size(); ++i) {
+            const uint32_t g = scene->groups[i];
+            if (g == PROJECT_GROUP_4D) {
+                launch_project_4d_entities(scene->tab, scene->times, scene->classes, mc, c->slot_ids.p, c->ctr, c->recs.p,
+                                           zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
+            } else {
+                launch_project_entities(scene->tab, g, scene->need_sh[i] != 0, scene->classes, mc, c->slot_ids.p, c->ctr,
+                                        c->recs.p, (p.raster_mode == 2 || p.raster_mode == 4) ? c->extra.p : nullptr, p.n_hint,
+                                        c->sm_count, c->cutoff_tab, ps);
+                scene_3d = true;
+            }
+            ++launches;
+        }
+    } else if (scene) {   // one launch per projection kernel the scene's clouds need
         for (const uint32_t g : scene->groups) {
             if (g == PROJECT_GROUP_4D) {   // (also writes the 4D segments' splat depths, from the moved positions)
                 launch_project_4d_scene(scene->tab, scene->times, c->slot_ids.p, c->ctr, modes ? *modes : ModeConsts{}, c->recs.p,
@@ -532,7 +553,15 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaEventRecord(c->ev_p1, ps));
     // depth-tested frames: the splat depths, indexed like the records (the projection's index list)
     ZTestArgs zt;
-    if (zd && scene_3d) {
+    if (zd && scene_3d && scene->entities) {
+        // (the splat-depth launch covers the 3D groups 0 .. 7: an entity frame's Classification / OpticalFlow /
+        // Velocity segments, groups 16 .. 23, are read as the plain group of their layout)
+        SceneTable dt = scene->tab;
+        for (uint32_t j = 0; j < dt.k; ++j)
+            if (dt.seg[j].group != PROJECT_GROUP_4D) dt.seg[j].group &= ~ENTITY_MODES;
+        launch_splat_depth_scene(dt, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
+        ++launches;
+    } else if (zd && scene_3d) {
         launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
     } else if (zd && !tc && !scene) {
@@ -546,6 +575,10 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
         CU(c, cudaStreamWaitEvent(q, c->ev_join, 0));
     }
     CU(c, cudaEventRecord(c->ev[3], q));
+    if (p.raster_mode >= 3) {   // a mixed-geometry frame: each record's blend kind, for the blend
+        launch_segment_kinds(scene->kinds, c->slot_ids.p, c->ctr, c->kinds.p, p.n_hint, c->sm_count, q);
+        ++launches;
+    }
     // ---- stage 4: tile binning -> stable tile-id sort -> ranges; stage 5: per-tile front-to-back blend.
     //      One round normally; `rounds` front-to-back rank rounds on chunked frames, each resuming the pixels'
     //      blend state, the last one writing the frame (identical pixels either way).
@@ -578,7 +611,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
             launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
                           fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal, &c->ctr->truncated,
-                          zt, c->stream_r);
+                          zt, c->stream_r, c->kinds.p);
             CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
             CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
         } else
@@ -647,7 +680,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     ModeConsts mc = {};
     mc.num_classes = ex ? ex->num_classes : 1u;
     if (ex) { memcpy(mc.prev_clip_from_world, ex->previous_clip_from_world, 64); mc.delta_time = ex->delta_time; }
-    const ModeConsts* modes = st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION ? &mc : nullptr;
+    const ModeConsts* modes = st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION || (scene && scene->entities) ? &mc : nullptr;
     const uint32_t n = scene ? scene->tab.n_total : cloud->n, num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
@@ -655,8 +688,10 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     TRY(frame_out(c, st, out_format, (size_t)fc.Wi * fc.Hi * format_bpp(out_format), out_rgba, out_is_device_ptr, want_aux,
                   out_depth, out_normal, &o));
     for (int attempt = 0; attempt < 4; ++attempt) {
-        const FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
-        if (p.raster_mode == 2) TRY(c->extra.grow(c, (size_t)c->cap_n * 64, false));
+        FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
+        if (scene && scene->entities) p.raster_mode = scene->raster_mode;   // (st plans it as an aabb frame: one round)
+        if (p.raster_mode == 2 || p.raster_mode == 4) TRY(c->extra.grow(c, (size_t)c->cap_n * 64, false));
+        if (p.raster_mode >= 3) TRY(c->kinds.grow(c, (size_t)c->cap_n, false));
         if (want_aux) TRY(c->aux.grow(c, (size_t)c->cap_n * 32, false));
         if (zd) TRY(c->splat_depth.grow(c, (size_t)c->cap_n * 4, false));
         if (p.rounds > 1) TRY(c->state.grow(c, (size_t)num_tiles * 256 * sizeof(float4), false));
@@ -788,6 +823,108 @@ bgs_status bgs_render_scene_4d(bgs_context* c, const bgs_cloud* const* clouds, c
                                int out_is_device_ptr) {
     return render_scene_impl(c, "render_scene_4d", true, clouds, unis, windows, k, view, st, ex, depth, out_rgba, out_format,
                              out_is_device_ptr);
+}
+
+// the blend kind of an entity's records (raster.cu): 0 = quad-uv, 1 = conic (3DGS and 4D with aabb), 2 = surfel
+static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.gaussian_mode == BGS_GAUSSIAN_2D ? 2 : 1); }
+
+bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                               const bgs_entity_settings* ents, uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                               const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
+                               int out_is_device_ptr) {
+    const char* call = "render_entities";
+    if (!c) return BGS_EINVAL;
+    if (!clouds || !unis || !ents || !view || !frame)
+        return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/entities/view/settings not ready", call);
+    if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "%s: k = %u is not in 1..%d", call, k, BGS_SCENE_MAX_CLOUDS);
+    if (frame->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
+    for (uint32_t j = 0; j < k; ++j)
+        if (!clouds[j]) return fail(c, BGS_EINVAL, "%s: clouds[%u] is NULL", call, j);
+    // entity j as its single-cloud call: its settings with the frame's sort bits and flags, its num_classes and window
+    std::vector<bgs_settings> st(k);
+    std::vector<bgs_render_extras> exs(k);
+    std::vector<bgs_time_window> windows(k);
+    SceneTimes times = {};
+    bool agree = true, any_3d = false, any_depth = false;
+    uint32_t gm3 = 0, kinds = 0;
+    uint64_t total = 0;
+    for (uint32_t j = 0; j < k; ++j) {
+        const bgs_entity_settings& e = ents[j];
+        const bool is4 = is_4d(clouds[j]->layout);
+        bgs_settings& s = st[j];
+        s = *frame;
+        s.gaussian_mode = e.gaussian_mode; s.rasterize_mode = e.rasterize_mode; s.aabb = e.aabb;
+        s.opacity_adaptive_radius = e.opacity_adaptive_radius; s.draw_mode = e.draw_mode;
+        exs[j] = ex ? *ex : bgs_render_extras{};
+        exs[j].num_classes = e.num_classes;
+        windows[j] = e.window;
+        bgs_settings chk = s;   // (a non-4D entity in Velocity is undrawn, and checked as a Color one, as in scenes)
+        if (!is4 && chk.rasterize_mode == BGS_RASTERIZE_VELOCITY) chk.rasterize_mode = BGS_RASTERIZE_COLOR;
+        TRY(check_render(c, clouds[j], view, &unis[j], &chk, ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &exs[j] : nullptr,
+                         out_format, false, is4));
+        if (is4) TRY(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, times.t[j]));
+        const bgs_entity_settings& e0 = ents[0];
+        agree = agree && e.rasterize_mode == e0.rasterize_mode && e.aabb == e0.aabb &&
+                e.opacity_adaptive_radius == e0.opacity_adaptive_radius && e.draw_mode == e0.draw_mode &&
+                (e.rasterize_mode != BGS_RASTERIZE_CLASSIFICATION || e.num_classes == e0.num_classes) &&
+                blend_kind(e) == blend_kind(e0) && (is4 || !any_3d || e.gaussian_mode == gm3);
+        if (!is4) { any_3d = true; gm3 = e.gaussian_mode; }
+        any_depth = any_depth || e.rasterize_mode == BGS_RASTERIZE_DEPTH;
+        kinds |= 1u << blend_kind(e);
+        total += clouds[j]->n;
+    }
+    if (agree) {   // one frame's settings: exactly bgs_render_scene_4d
+        bgs_settings s = st[0];
+        s.gaussian_mode = any_3d ? gm3 : (uint32_t)BGS_GAUSSIAN_4D;
+        const bool need_ex = ex || ents[0].rasterize_mode == BGS_RASTERIZE_CLASSIFICATION;
+        return render_scene_impl(c, call, true, clouds, unis, windows.data(), k, view, &s, need_ex ? &exs[0] : nullptr, depth,
+                                 out_rgba, out_format, out_is_device_ptr);
+    }
+    if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "%s: N = %llu gaussians, must be < 2^30", call, (unsigned long long)total);
+    if (depth) TRY(check_scene_depth(c, depth, view));
+    auto scene = std::make_shared<SceneFacts>();
+    scene->entities = true;
+    scene->times = times;
+    SceneTable& tab = scene->tab;
+    memset(&tab, 0, sizeof(tab));
+    tab.k = k;
+    tab.n_total = (uint32_t)total;
+    scene->kinds.k = k;
+    uint32_t offset = 0;
+    for (uint32_t j = 0; j < k; ++j) {
+        const bgs_cloud* cl = clouds[j];
+        const uint32_t rm = st[j].rasterize_mode;
+        SceneSeg& sg = tab.seg[j];
+        sg.fc = frame_consts(cl, view, &unis[j], &st[j], false);
+        sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
+        sg.pos = cl->pos;
+        sg.blocks = cl->blocks;
+        sg.offset = offset;
+        sg.n = cl->n;
+        // the plain colour kernel, or the Classification / OpticalFlow one (which leaves a 3D Velocity record undrawn)
+        sg.group = project_group(cl->layout, cl->sh_degree);
+        if (sg.group != PROJECT_GROUP_4D && rm >= BGS_RASTERIZE_CLASSIFICATION) sg.group |= ENTITY_MODES;
+        const bool sh = rm == ((sg.group & ENTITY_MODES) ? BGS_RASTERIZE_CLASSIFICATION : BGS_RASTERIZE_COLOR);
+        const size_t gi = std::find(scene->groups.begin(), scene->groups.end(), sg.group) - scene->groups.begin();
+        if (gi == scene->groups.size()) { scene->groups.push_back(sg.group); scene->need_sh.push_back(0u); }
+        if (sh) scene->need_sh[gi] = 1u;
+        scene->classes.n[j] = ents[j].num_classes;
+        scene->kinds.offset[j] = offset;
+        scene->kinds.kind[j] = (uint32_t)blend_kind(ents[j]);
+        offset += cl->n;
+        scene->clouds.push_back(cl);
+    }
+    // one kind: its own blend; several: the mixed one (with the surfel records when some entity has them)
+    scene->raster_mode = __builtin_popcount(kinds) > 1 ? ((kinds & 4u) ? 4 : 3) : __builtin_ctz(kinds);
+    // the frame as render_impl plans it: its flags and sort bits, the Depth range when some entity is in Depth mode, and
+    // the blend kind (an aabb frame when it is not quad-uv: one round)
+    bgs_settings sf = *frame;
+    sf.rasterize_mode = any_depth ? BGS_RASTERIZE_DEPTH : BGS_RASTERIZE_COLOR;
+    sf.aabb = scene->raster_mode != 0;
+    sf.gaussian_mode = scene->raster_mode == 2 ? BGS_GAUSSIAN_2D : BGS_GAUSSIAN_3D;
+    sf.draw_mode = BGS_DRAW_ALL;
+    return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr,
+                       depth, nullptr, scene);
 }
 
 bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,

@@ -68,6 +68,8 @@ struct SceneTable {
 // SH degree << 1), so 4D segments never fall into a 3D launch, and splat_depth_scene leaves their depths to the 4D
 // projection, which takes them from the moved positions.
 constexpr uint32_t PROJECT_GROUP_4D = 8u;
+// bgs_render_entities: a 3D group's bit for the Classification / OpticalFlow / Velocity colour kernel (groups 16 .. 23)
+constexpr uint32_t ENTITY_MODES = 16u;
 
 // bgs_render_extras as the Classification / OpticalFlow projection reads it.  Only project_modes_kernel takes it (as an
 // argument of its own), so the arguments and code of every other kernel stay what they were.
@@ -88,6 +90,20 @@ struct TemporalConsts {
 // project_4d_scene_kernel alone (768 B beside the ~22 KB segment table), so the other scene kernels keep theirs.
 struct SceneTimes {
     TemporalConsts t[BGS_SCENE_MAX_CLOUDS];
+};
+
+// bgs_render_entities' per-segment num_classes (n[j] is segment j's).  An argument of the entity projection kernels alone,
+// as SceneTimes is, so FrameConsts -- and the parameters of every single-cloud kernel -- stay as they are.
+struct SceneClasses {
+    uint32_t n[BGS_SCENE_MAX_CLOUDS];
+};
+
+// The blend kind of each segment of a mixed-geometry frame (bgs_render_entities): 0 = quad-uv (OBB), 1 = conic (3DGS / 4D
+// with aabb), 2 = surfel (2DGS with aabb); raster.cu's class launch tags each compact slot with its segment's kind.
+struct SegmentKinds {
+    uint32_t k;
+    uint32_t offset[BGS_SCENE_MAX_CLOUDS];
+    uint32_t kind[BGS_SCENE_MAX_CLOUDS];
 };
 
 // Projected splat record, 48 B, stored by front-to-back rank.

@@ -70,6 +70,15 @@ struct SceneFacts {
     SceneTimes times = {};
     std::vector<const bgs_cloud*> clouds;
     std::vector<uint32_t> groups;
+    // bgs_render_entities frames whose entities disagree: each group's launch (project_group, plus ENTITY_MODES for the
+    // Classification / OpticalFlow / Velocity colour kernel) with whether one of its segments reads the SH coefficients,
+    // the segments' num_classes, and the blend (raster.cu's mode: 0..2 when every splat has one kind, else 3 / 4 with
+    // `kinds`)
+    bool entities = false;
+    std::vector<uint32_t> need_sh;   // per entry of groups
+    SceneClasses classes = {};
+    int raster_mode = 0;
+    SegmentKinds kinds = {};
 };
 
 // What the host knows of a frame it has enqueued: the context keeps the last one enqueued (`pend`) and, once its
@@ -130,6 +139,7 @@ struct bgs_context {
     DevBuf<float4> extra;             // 4 x float4 per record: 2DGS + USE_AABB only (allocated on first use)
     DevBuf<float4> aux;               // 2 x float4 per record: depth / normal colour sources (bgs_render_aux only)
     DevBuf<float> splat_depth;        // 1 float per record: the splat depths d of depth-tested frames (allocated on first use)
+    DevBuf<unsigned char> kinds;      // 1 byte per record: the blend kind of a mixed-geometry frame's splats (first use)
     DevBuf<void> frame_aux[2];        // depth / normal frames when bgs_render_aux delivers to host memory
     // scratch sized by the pair capacity (grow-only; cap_pairs pairs)
     uint32_t cap_pairs = 0;

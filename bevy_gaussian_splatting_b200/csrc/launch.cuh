@@ -52,6 +52,15 @@ void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_sl
 void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const uint32_t* slot_ids, const FrameCounters* ctr,
                              const ModeConsts& mc, SplatRec* recs, float* depths, uint32_t n_hint, int sm_count,
                              cudaStream_t stream);
+// bgs_render_entities frames whose entities disagree: the projection of the segments of one group (project_group, |
+// ENTITY_MODES for the Classification / OpticalFlow / Velocity kernel), each with its own settings and num_classes;
+// need_sh: some segment of the group reads the SH coefficients.  And the 4D segments' (PROJECT_GROUP_4D).
+void launch_project_entities(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
+                             const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
+                             float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream);
+void launch_project_4d_entities(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
+                                const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
+                                float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
 // bin.cu
 int bin_coop_blocks_per_sm();
 cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
@@ -71,10 +80,15 @@ struct ZTestArgs {
     const float* scene = nullptr;
     size_t pitch = 0;
 };
+// mode 0..2: one blend kind for every splat; 3 / 4 (bgs_render_entities): mixed kinds, read from `kinds` (one byte per
+// record), 4 when some splat is a surfel
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
                    const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
-                   cudaStream_t stream);
+                   cudaStream_t stream, const unsigned char* kinds = nullptr);
+// a mixed-geometry frame's blend kind of each compact slot (records n_vis of ctr), from its segment's
+void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
+                          uint32_t n_hint, int sm_count, cudaStream_t stream);
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
                          uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,

@@ -1036,6 +1036,63 @@ void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, con
     const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     project_4d_scene_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, times, mc, slot_ids, ctr, recs, depths);
 }
+// ---- bgs_render_entities frames whose entities disagree.  The scene kernels above take the colour kernel's SH need and
+// num_classes from the frame; here each segment's FrameConsts carries its own entity's settings, the launch is told
+// whether any of its segments reads the SH coefficients, and project_one sees its segment's num_classes.
+template <class G>
+struct EntityGeo : G {
+    const SceneClasses& classes;
+    template <class Src>
+    __device__ __forceinline__ void project(const Src& src, uint32_t j, uint32_t e, uint32_t r, float4 p4, const float q[4],
+                                            const float so[4], const float* ext, uint32_t op_bits, const ModeConsts& mc) const {
+        ModeConsts m = mc;
+        m.num_classes = classes.n[j];
+        G::project(src, j, e, r, p4, q, so, ext, op_bits, m);
+    }
+};
+
+template <bool F16, uint32_t D, bool MODES2>
+__global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
+project_entities_kernel(SceneTable tab, uint32_t group, uint32_t need_sh, SceneClasses classes, ModeConsts mc,
+                        const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs,
+                        float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
+    project_loop(SceneSrc{tab, 1u << group, slot_ids},
+                 EntityGeo<Geo3d<F16, D, MODES2>>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, nullptr}, classes}, ctr, mc);
+}
+
+__global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
+project_4d_entities_kernel(SceneTable tab, SceneTimes times, SceneClasses classes, ModeConsts mc,
+                           const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                           SplatRec* __restrict__ recs, float* __restrict__ depths /* depth-tested frames only */) {
+    project_loop(SceneSrc{tab, 1u << PROJECT_GROUP_4D, slot_ids, &times}, EntityGeo<Geo4d>{{ctr, recs, depths}, classes}, ctr, mc);
+}
+static_assert(sizeof(SceneTable) + sizeof(SceneTimes) + sizeof(SceneClasses) + sizeof(ModeConsts) + 4 * sizeof(void*) + 16 <= 32764,
+              "project_4d_entities_kernel's parameters exceed the sm_90 limit");
+
+void launch_project_entities(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
+                             const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
+                             float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream) {
+    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
+    const uint32_t g = group & ~ENTITY_MODES;
+    with_layout_degree(g & 1u ? CloudLayout::F16 : CloudLayout::F32, g >> 1, [&](auto L, auto Dt) {
+        constexpr CloudLayout Lv = decltype(L)::value;
+        constexpr uint32_t D = decltype(Dt)::value;
+        if constexpr (!is_4d(Lv)) {
+            auto* kernel = (group & ENTITY_MODES) ? project_entities_kernel<is_f16(Lv), D, true>
+                                                  : project_entities_kernel<is_f16(Lv), D, false>;
+            kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, group, need_sh ? 1u : 0u, classes, mc, slot_ids, ctr, recs, extra,
+                                                      cutoff_tab);
+        }
+    });
+}
+
+void launch_project_4d_entities(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
+                                const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
+                                float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream) {
+    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
+    project_4d_entities_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, times, classes, mc, slot_ids, ctr, recs, depths);
+}
+
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,
                         FrameCounters* ctr, const FrameConsts& fc, cudaStream_t stream) {
     depth_range_kernel<<<1, 32, 0, stream>>>(pos, n, sorted_payload, slot_ids, ctr, fc);

@@ -240,21 +240,29 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // more frames with the very same alphas: config C4's colour + depth + normal outputs cost one pass, not three.
 // ZTEST (MODE 0, 1, 2 without AUX): bgs_render_depth_test.  A pair blends only where its coverage decision holds and
 // d >= the pixel's scene depth; the warp's candidates leave out the splats below the scene everywhere in its rectangle.
-template <int MODE, bool AUX, bool ZTEST = false>
-__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : 5)
-raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
-              const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
-              const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
-              const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
-              size_t pitch) {
+// MODE 3 / 4 (bgs_render_entities): mixed kinds, each splat tested by its own: kinds[r] (raster_kinds_kernel) is record r's
+// 0 = quad-uv, 1 = conic, 2 = surfel; MODE 4 when some splat is a surfel (the only one that stages the surfel records).
+// Warp candidates: bbox for every kind, and the separating-axis test of MODE 0 for the quad-uv splats.
+template <int MODE, bool AUX, bool ZTEST>
+__device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
+                                            const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
+                                            int H, int tiles_x, void* __restrict__ out, uint32_t format,
+                                            const float4* __restrict__ aux, void* __restrict__ out_depth,
+                                            void* __restrict__ out_normal, const uint32_t* __restrict__ truncated,
+                                            const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
+                                            const unsigned char* __restrict__ kinds) {
     static_assert(!(AUX && ZTEST), "bgs_render_aux takes no depth buffer");
-    __shared__ __align__(16) unsigned char s_mem[(MODE == 2 ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0) +
+    constexpr bool MIXED = MODE >= 3, SURF = MODE == 2 || MODE == 4;
+    static_assert(!(AUX && MIXED), "bgs_render_aux renders one cloud");
+    __shared__ __align__(16) unsigned char s_mem[(SURF ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0) +
                                                  (ZTEST ? ZT_BYTES : 0)];
-    constexpr uint32_t SM_AUX = MODE == 2 ? SM_BYTES_2D : SM_BYTES;
+    constexpr uint32_t SM_AUX = SURF ? SM_BYTES_2D : SM_BYTES;
     constexpr uint32_t REC_D = SM_AUX;   // ZTEST: d of the splat whose q0 record is at a, at a + REC_D
     __shared__ __align__(16) uint32_t s_ent[2][ENT_WORDS];    // TMA destination: the tile's pair-list chunks
     __shared__ __align__(8) unsigned long long s_bar[2];
-    __shared__ __align__(8) float2 s_thr[MODE == 0 ? RT_CHUNK : 1];   // MODE 0: per staged splat cull thresholds (u, v)
+    // MODE 0 and mixed: per staged splat cull thresholds (u, v) (quad-uv splats only)
+    __shared__ __align__(8) float2 s_thr[MODE == 0 || MIXED ? RT_CHUNK : 1];
+    __shared__ unsigned char s_kind[MIXED ? RT_CHUNK : 1];   // mixed: the staged splats' kinds
     float4* s_q0 = reinterpret_cast<float4*>(s_mem + SM_Q0);
     float4* s_uv = reinterpret_cast<float4*>(s_mem + SM_UV);
     float4* s_q2 = reinterpret_cast<float4*>(s_mem + SM_Q2);
@@ -311,7 +319,9 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
             s_q0[t] = p0;
             s_uv[t] = p1;
             s_q2[t] = __ldg(rp + 2);
-            if (MODE == 0) {
+            const int kind = MIXED ? (int)__ldg(kinds + r) : MODE;
+            if (MIXED) s_kind[t] = (unsigned char)kind;
+            if (kind == 0) {
                 // thresholds of the per-warp separating-axis cull below, once per splat: the quad |u| <= 1, |v| <= 1
                 // misses a warp rectangle (pixel centres within +-3.5 x +-1.5 of its centre) when |u(centre)| exceeds
                 // 1 + |ux| 3.5 + |uy| 1.5 (same for v).  Slack: 1e-5 of the largest magnitude the terms of u can take
@@ -321,7 +331,7 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                 const float um = fabsf(p0.z) * ax + fabsf(p0.w) * ay + ur, vm = fabsf(p1.x) * ax + fabsf(p1.y) * ay + vr;
                 s_thr[t] = make_float2(ur + 1.0f + 1e-5f * um, vr + 1.0f + 1e-5f * vm);
             }
-            if (MODE == 2) {
+            if (SURF && kind == 2) {
                 float4* s_ex = reinterpret_cast<float4*>(s_mem + SM_EXTRA);
                 const float4* ep = extra + (size_t)r * 4;
 #pragma unroll
@@ -342,7 +352,7 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
             // (`|`, not `||`: the four compares are one predicated test, not a chain of branches)
             bool hit = !((int)(bx >> 16) < wx0 | (int)(bx & 0xFFFFu) > wx0 + 7 | (int)(by >> 16) < wy0 |
                          (int)(by & 0xFFFFu) > wy0 + 3);
-            if (MODE == 0 && hit) {
+            if ((MODE == 0 || (MIXED && s_kind[j] == 0)) && hit) {
                 // separating-axis test of the splat's quad against this warp's pixel centres
                 // [wx0 + .5, wx0 + 7.5] x [wy0 + .5, wy0 + 3.5] (thresholds staged per splat above): the bbox
                 // of a slanted quad passes many warps none of whose pixels it covers
@@ -430,7 +440,8 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                 auto depth_ok = [&]() { return !ZTEST || lds_f32(a_rec + REC_D) >= zs; };
                 float e;
                 float4 q2;
-                if (MODE == 0) {
+                const int kind = MIXED ? (int)s_kind[(a_rec - a_base) >> 4] : MODE;
+                if (kind == 0) {
                     const float2 uv = quad_uv(fx, fy, q0, q1);
                     if (!(fabsf(uv.x) <= 1.0f && fabsf(uv.y) <= 1.0f && depth_ok())) continue;
                     const float qd = __fmaf_rn(uv.y, uv.y, __fmul_rn(uv.x, uv.x));
@@ -443,7 +454,7 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
                     const float mx = __fadd_rn(dx, dx), my = -__fadd_rn(dy, dy);
                     const float Rq = q1.y;   // MODE 1: quad half-side in half-pixels
                     float power;
-                    if (MODE == 1) {
+                    if (kind == 1 || !SURF) {
                         if (!(fabsf(mx) <= Rq && fabsf(my) <= Rq && depth_ok())) continue;
                         // q0.z, q0.w, q1.x = conic x, y, z;  d = -m  (gaussian.wgsl:459-462)
                         const float ddx = -mx, ddy = -my;
@@ -495,6 +506,51 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
         write_pixel(out_depth, format, (size_t)py * W + px, dr, dg, db, T);
         write_pixel(out_normal, format, (size_t)py * W + px, nr, ng, nb, T);
     }
+}
+
+template <int MODE, bool AUX, bool ZTEST = false>
+__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : 5)
+raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
+              const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
+              const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
+              const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
+              size_t pitch) {
+    raster_body<MODE, AUX, ZTEST>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal,
+                                  truncated, splat_d, scene, pitch, nullptr);
+}
+
+// bgs_render_entities' blend of mixed kinds (MODE 3, or 4 with surfels).  (At 5 CTAs per SM the depth-tested variant
+// spills: 4 leave it 64 registers.)
+template <int MODE, bool ZTEST>
+__global__ void __launch_bounds__(RT_THREADS, ZTEST ? 4 : 5)
+raster_mixed_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
+                    const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
+                    const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
+                    size_t pitch, const unsigned char* __restrict__ kinds) {
+    raster_body<MODE, false, ZTEST>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr,
+                                    truncated, splat_d, scene, pitch, kinds);
+}
+
+// the kind of each compact slot r < n_vis: its global index's segment's
+__global__ void raster_kinds_kernel(SegmentKinds sk, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                                    unsigned char* __restrict__ out) {
+    const uint32_t n_vis = ctr->n_vis;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_vis; r += gridDim.x * blockDim.x) {
+        const uint32_t g = __ldg(slot_ids + r);
+        uint32_t lo = 0u, hi = sk.k;   // the last j with offset <= g (SceneTable::find)
+        while (hi - lo > 1u) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (sk.offset[mid] <= g) lo = mid; else hi = mid;
+        }
+        out[r] = (unsigned char)sk.kind[lo];
+    }
+}
+
+void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
+                          uint32_t n_hint, int sm_count, cudaStream_t stream) {
+    uint32_t grid = (n_hint + 255) / 256;
+    grid = grid < 1u ? 1u : (grid > (uint32_t)(8 * sm_count) ? (uint32_t)(8 * sm_count) : grid);
+    raster_kinds_kernel<<<grid, 256, 0, stream>>>(kinds, slot_ids, ctr, out);
 }
 
 // ---- MODE 0 fast path: 2 horizontally adjacent pixels per thread -----------------------------------------
@@ -670,9 +726,16 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
                    const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
-                   cudaStream_t stream) {
+                   cudaStream_t stream, const unsigned char* kinds) {
     const int grid = tiles_x * tiles_y;
     const bool ztest = zt.scene != nullptr;   // (bgs_render_aux frames never carry a depth buffer)
+    if (mode >= 3) {
+        auto* kernel = mode == 3 ? (ztest ? raster_mixed_kernel<3, true> : raster_mixed_kernel<3, false>)
+                                 : (ztest ? raster_mixed_kernel<4, true> : raster_mixed_kernel<4, false>);
+        kernel<<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, truncated,
+                                                zt.splat_d, zt.scene, zt.pitch, kinds);
+        return;
+    }
     // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
     // pixels (more of its lanes then idle at the tile's splat boundaries)
     if (aux == nullptr && mode == 0 && large_footprints) {

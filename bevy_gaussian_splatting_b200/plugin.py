@@ -258,6 +258,37 @@ def check_scene_entities_4d(entities) -> CloudSettings:
     return dataclasses.replace(first, gaussian_mode=mode)
 
 
+# CloudSettings fields a bgs_render_entities call takes for the whole frame: the one depth sort and its flags
+ENTITIES_FRAME_FIELDS = ("radix_sort_depth_bits", "sort_mode", "sort_all", "binning_rounds")
+
+
+def check_entities(entities) -> CloudSettings:
+    """`entities`: a sequence of (handle, CloudSettings, transform or None), one bgs_render_entities call's clouds, each
+    drawn with its own settings.  Returns the settings the frame-wide values (ENTITIES_FRAME_FIELDS) come from, the first
+    entity's; raises ValueError when there are none, too many, or two entities disagree on a frame-wide field."""
+    entities = list(entities)
+    if not entities:
+        raise ValueError("render_entities: no entities")
+    if len(entities) > abi.BGS_SCENE_MAX_CLOUDS:
+        raise ValueError(f"render_entities: {len(entities)} entities, at most {abi.BGS_SCENE_MAX_CLOUDS}")
+    first = entities[0][1]
+    for j, (_, st, _) in enumerate(entities[1:], 1):
+        for name in ENTITIES_FRAME_FIELDS:
+            a, b = getattr(first, name), getattr(st, name)
+            if a != b:
+                raise ValueError(f"render_entities: entity {j} has {name} = {b!r}, entity 0 {a!r}: the frame has one depth sort")
+    return first
+
+
+def entity_settings(settings: CloudSettings) -> abi.bgs_entity_settings:
+    """One entity's bgs_entity_settings."""
+    s = settings.to_abi()
+    return abi.bgs_entity_settings(gaussian_mode=s.gaussian_mode, rasterize_mode=s.rasterize_mode, aabb=s.aabb,
+                                   opacity_adaptive_radius=s.opacity_adaptive_radius, draw_mode=s.draw_mode,
+                                   num_classes=int(settings.num_classes),
+                                   window=abi.bgs_time_window(float(settings.time_start), float(settings.time_stop)))
+
+
 class GaussianSplattingPlugin:
     """Owns one `bgs_context` (one GPU).  `render_view` = run_radix_sort + DrawGaussians for one view."""
 
@@ -375,6 +406,38 @@ class GaussianSplattingPlugin:
             return out
         self._check(self._lib.bgs_render_scene(self._ctx, clouds, unis, k, C.byref(v), C.byref(s), None if ex is None else C.byref(ex),
                                                None if zd is None else C.byref(zd), _ptr(out), code, 0))
+        return out
+
+    def render_entities(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None, previous_view: View | None = None,
+                        delta_time: float | None = None, asynchronous: bool = False, premultiplied: bool = False,
+                        blend_over: bool = False, out: np.ndarray | None = None) -> np.ndarray:
+        """`render_scene` with each entity drawn with its own CloudSettings (`bgs_render_entities`): gaussian_mode,
+        rasterize_mode, aabb, opacity_adaptive_radius, draw_mode, num_classes and the 4D window are per entity, so a
+        highlighted selection, a Classification object or a 2DGS surface drawn with aabb share one depth-sorted frame
+        with the scan around them.  radix_sort_depth_bits (and the other sort fields) are the frame's and must agree
+        (`check_entities`, ValueError before any call).  The other arguments are `render_scene`'s."""
+        entities = list(entities)
+        first = check_entities(entities)
+        code, dtype, ch = self.FORMATS[fmt]
+        v = view.to_abi()
+        s = first.to_abi()
+        s.flags |= ((abi.BGS_FLAG_ASYNC if asynchronous else 0) | (abi.BGS_FLAG_PREMULTIPLIED_OUT if premultiplied else 0)
+                    | (abi.BGS_FLAG_BLEND_OVER_TARGET if blend_over else 0))
+        ex = None
+        if previous_view is not None:
+            ex = abi.bgs_render_extras(num_classes=1, delta_time=float(delta_time) if delta_time is not None else 0.0)
+            ex.previous_clip_from_world[:] = previous_view.to_abi().clip_from_world[:]
+        k = len(entities)
+        clouds = (C.c_void_p * k)(*[h._h.value for h, _, _ in entities])
+        unis = (abi.bgs_cloud_uniform * k)(*[self.cloud_uniform(st, tr, h.aabb) for h, st, tr in entities])
+        ents = (abi.bgs_entity_settings * k)(*[entity_settings(st) for _, st, _ in entities])
+        if out is None:
+            out = np.empty((view.height, view.width, ch), dtype)
+        assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
+        zd = self._scene_depth(scene_depth, view)
+        self._check(self._lib.bgs_render_entities(self._ctx, clouds, unis, ents, k, C.byref(v), C.byref(s),
+                                                  None if ex is None else C.byref(ex), None if zd is None else C.byref(zd),
+                                                  _ptr(out), code, 0))
         return out
 
     def _render_4d(self, handle, v, u, s, ex, zd, settings, target, code, is_device):

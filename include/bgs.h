@@ -645,6 +645,49 @@ bgs_status bgs_render_scene_4d(bgs_context* ctx, const bgs_cloud* const* clouds,
                                const bgs_view* view, const bgs_settings* settings, const bgs_render_extras* extras,
                                const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
 
+/* bgs_render_scene_4d with each entity's own CloudSettings: an editor highlights one object's selection inside a room
+ * drawn in full, a labelled object is drawn in Classification inside a scan drawn in Color, a 3DGS object or a 4D
+ * performer stands on a 2DGS surface drawn with aabb -- all in one depth-sorted frame.
+ *
+ * The rule, exactly:
+ *   Everything that is not below stays bgs_render_scene_4d's: index space, keys, the stable sort over (key, g), binning,
+ *     the depth test, output modes, ASYNC, the pair-overflow re-render, ordering against queued writes, debug hooks.
+ *   Frame-wide values.  frame->radix_sort_depth_bits and frame->flags (BGS_FLAG_SORT_ALL refused, as in scenes); the
+ *     OpticalFlow previous view and delta_time of `extras` (its num_classes is not read); the depth buffer and the output.
+ *   Per-entity values.  entities[j] carries entity j's gaussian_mode, rasterize_mode, aabb, opacity_adaptive_radius,
+ *     draw_mode, num_classes and (Gaussian4d clouds only) time window; uniforms[j] its uniform.
+ *   Records.  The record of g = o_j + i is, bit for bit, the record the single-cloud call (bgs_render_depth_test, or
+ *     bgs_render_4d for a 4D cloud) writes for gaussian i with cloud j, uniforms[j] and entity j's settings as the frame's;
+ *     so are the 2DGS aabb surfel record and the splat depth under a depth buffer.  A non-4D entity in Velocity gives an
+ *     undrawn record, as bgs_render_scene_4d rules.
+ *   Depth colour range.  bgs_render_scene's: sorted[1] / sorted[N-1] of the joint list over every entry, computed when
+ *     some entity is in Depth mode.  (A deliberate difference: the reference takes each entity's range from its own sort.)
+ *   Coverage.  Each (pixel, splat) decision is the one that splat's own blend makes -- quad-uv (OBB: 3DGS, 2DGS and 4D),
+ *     conic (3DGS and 4D with aabb) or surfel (2DGS with aabb) -- bit for bit, and the splats blend in joint order.
+ *     Frames whose entities use more than one of the three run one blend that tests each splat by its own kind; like
+ *     aabb frames, they are never split into chunked rounds (BGS_FLAG_CHUNKS is ignored).
+ *   Identity.  When all k entities agree (every setting above, num_classes in Classification, and the non-4D entities'
+ *     gaussian_mode), the call is bgs_render_scene_4d with those settings, byte for byte: pixels, sorted entries, tile
+ *     ranges and slices, records, stats and launch count.
+ * Launches: one projection per (layout and SH degree, plain or Classification / OpticalFlow / Velocity colour kernel)
+ *   among the non-4D entities and one for the 4D ones; a frame of mixed blend kinds adds one launch that tags each
+ *   visible splat with its kind.
+ * Refused with BGS_EINVAL, nothing enqueued or written: every refusal of bgs_render_scene_4d that still applies; any
+ *   refusal of the single-cloud call for an entity with its settings (num_classes == 0 in Classification, a 4D cloud
+ *   whose entity is not BGS_GAUSSIAN_4D, BGS_GAUSSIAN_4D on a 3D cloud, Normal on a 4D entity, an invalid window, ...);
+ *   entities == NULL.  BGS_GAUSSIAN_2D with aabb beside a 4D cloud is accepted.  NULL clouds, uniforms, entities, view
+ *   or frame -> BGS_NOT_READY. */
+typedef struct {
+    uint32_t gaussian_mode, rasterize_mode, aabb, opacity_adaptive_radius, draw_mode;   /* bgs_settings' */
+    uint32_t num_classes;        /* Classification entities: > 0 */
+    bgs_time_window window;      /* Gaussian4d entities only */
+} bgs_entity_settings;
+bgs_status bgs_render_entities(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                               const bgs_entity_settings* entities, uint32_t k, const bgs_view* view,
+                               const bgs_settings* frame /* radix_sort_depth_bits and flags only */,
+                               const bgs_render_extras* extras /* previous view and delta_time; num_classes unused */,
+                               const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target

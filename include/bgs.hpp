@@ -424,6 +424,41 @@ public:
         check(st);
         return true;
     }
+    // render_scene with each entity drawn with its own settings (bgs_render_entities): gaussian_mode, rasterize_mode, aabb,
+    // opacity_adaptive_radius, draw_mode, num_classes and [time_start, time_stop] are the entity's; the sort settings and
+    // `extra_flags` are the frame's, taken from entities[0].  The arguments are render_scene's.
+    bool render_entities(const std::vector<SceneEntity>& entities, const bgs_view& view, void* out_rgba,
+                         uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr, float delta_time = 0.0f,
+                         const float* depth = nullptr, uint64_t pitch_bytes = 0, bool out_is_device = false,
+                         uint32_t extra_flags = 0) {
+        if (entities.empty()) check(BGS_EINVAL);
+        std::vector<const bgs_cloud*> clouds;
+        std::vector<bgs_cloud_uniform> unis;
+        std::vector<bgs_entity_settings> ents;
+        for (const SceneEntity& e : entities) {
+            bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
+            std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
+            clouds.push_back(e.cloud->get());
+            unis.push_back(u);
+            const bgs_settings s = e.settings.to_abi();
+            ents.push_back({s.gaussian_mode, s.rasterize_mode, s.aabb, s.opacity_adaptive_radius, s.draw_mode,
+                            e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
+        }
+        const bgs_settings s = entities[0].settings.to_abi(extra_flags);
+        bgs_render_extras ex{};
+        ex.num_classes = 1;
+        if (previous_view) {
+            std::memcpy(ex.previous_clip_from_world, previous_view->clip_from_world, 64);
+            ex.delta_time = delta_time;
+        }
+        const bgs_scene_depth zd{depth, pitch_bytes};
+        const bgs_status st = bgs_render_entities(ctx_, clouds.data(), unis.data(), ents.data(), (uint32_t)clouds.size(), &view, &s,
+                                                  previous_view ? &ex : nullptr, depth ? &zd : nullptr, out_rgba, format,
+                                                  out_is_device ? 1 : 0);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
     // Colour + depth + normal frames of one view in one pass (BASELINE.json config 4; bgs_render_aux).
     bool render_view_aux(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view, void* out_rgba,
                          void* out_depth, void* out_normal, uint32_t format = BGS_FORMAT_RGBA8_SRGB, bool out_is_device = false) {
