@@ -137,6 +137,7 @@ struct FramePlan {
     int raster_mode;        // 0 = quad-uv falloff (USE_OBB, 3DGS and 2DGS), 1 = 3DGS conic (USE_AABB), 2 = 2DGS ray-splat (USE_AABB)
     int rounds;             // binning rounds: 1, or MAX_CHUNKS on a chunked frame
     bool large_fp;          // blend variant for large footprints (results are identical)
+    bool box;               // the bounding-box overlay (BGS_FLAG_VISUALIZE_BOUNDING_BOX): one round, raster_body's blend
     bool by_slot;           // compact mode: records at recs[slot] (else SORT_ALL: by front-to-back rank)
     bool depth_range;       // Depth colouring / aux frames: the projection needs sorted[1] / sorted[N-1]
     bool overlap;           // the projection runs on the second stream beside the depth sort
@@ -155,8 +156,9 @@ FramePlan plan_frame(const bgs_context* c, const bgs_settings* st, bool want_aux
     // saturation-aware chunking: frames whose splats cover many tiles each (last frame: >= 32 pairs per visible splat
     // and >= 2^24 pairs: below that, one round is cheaper than the extra launches) run binning / tile sort /
     // blend in front-to-back rank rounds; the rounds after every tile has saturated emit nothing.
-    // Quad-uv records only; BGS_FLAG_CHUNKS / _NO_CHUNKS force it.
-    bool chunked = p.raster_mode == 0 && !want_aux && num_tiles <= CHUNK_MAX_TILES && !(st->flags & BGS_FLAG_NO_CHUNKS);
+    // Quad-uv records only, and not on overlay frames (like aux frames); BGS_FLAG_CHUNKS / _NO_CHUNKS force it.
+    p.box = (st->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0;
+    bool chunked = p.raster_mode == 0 && !want_aux && !p.box && num_tiles <= CHUNK_MAX_TILES && !(st->flags & BGS_FLAG_NO_CHUNKS);
     if (chunked && !(st->flags & BGS_FLAG_CHUNKS))
         chunked = c->n_vis_hint > 0 && c->n_pairs_hint >= (c->last.rounds > 1 ? 3u << 22 : 1u << 24) &&
                   (uint64_t)c->n_pairs_hint >= (c->last.rounds > 1 ? 24ull : 32ull) * c->n_vis_hint;   // (hysteresis)
@@ -611,7 +613,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
             launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
                           fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal, &c->ctr->truncated,
-                          zt, c->stream_r, c->kinds.p);
+                          zt, c->stream_r, c->kinds.p, p.box);
             CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
             CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
         } else
@@ -689,7 +691,10 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
                   out_depth, out_normal, &o));
     for (int attempt = 0; attempt < 4; ++attempt) {
         FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
-        if (scene && scene->entities) p.raster_mode = scene->raster_mode;   // (st plans it as an aabb frame: one round)
+        if (scene && scene->entities) {   // (st plans it as an aabb frame or an overlay one: one round)
+            p.raster_mode = scene->raster_mode;
+            p.box = scene->box;
+        }
         if (p.raster_mode == 2 || p.raster_mode == 4) TRY(c->extra.grow(c, (size_t)c->cap_n * 64, false));
         if (p.raster_mode >= 3) TRY(c->kinds.grow(c, (size_t)c->cap_n, false));
         if (want_aux) TRY(c->aux.grow(c, (size_t)c->cap_n * 32, false));
@@ -828,18 +833,26 @@ bgs_status bgs_render_scene_4d(bgs_context* c, const bgs_cloud* const* clouds, c
 // the blend kind of an entity's records (raster.cu): 0 = quad-uv, 1 = conic (3DGS and 4D with aabb), 2 = surfel
 static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.gaussian_mode == BGS_GAUSSIAN_2D ? 2 : 1); }
 
-bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
-                               const bgs_entity_settings* ents, uint32_t k, const bgs_view* view, const bgs_settings* frame,
-                               const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
-                               int out_is_device_ptr) {
+bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                  const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
+                                  const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
     const char* call = "render_entities";
     if (!c) return BGS_EINVAL;
     if (!clouds || !unis || !ents || !view || !frame)
         return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/entities/view/settings not ready", call);
     if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "%s: k = %u is not in 1..%d", call, k, BGS_SCENE_MAX_CLOUDS);
     if (frame->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
-    for (uint32_t j = 0; j < k; ++j)
+    for (uint32_t j = 0; j < k; ++j) {
         if (!clouds[j]) return fail(c, BGS_EINVAL, "%s: clouds[%u] is NULL", call, j);
+        if (entity_flags && (entity_flags[j] & ~(uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX))
+            return fail(c, BGS_EINVAL, "%s: entity_flags[%u] = 0x%x has an unknown bit", call, j, entity_flags[j]);
+    }
+    // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
+    auto box_of = [&](uint32_t j) {
+        return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
+               (entity_flags && (entity_flags[j] & BGS_ENTITY_VISUALIZE_BOUNDING_BOX) != 0);
+    };
     // entity j as its single-cloud call: its settings with the frame's sort bits and flags, its num_classes and window
     std::vector<bgs_settings> st(k);
     std::vector<bgs_render_extras> exs(k);
@@ -867,7 +880,7 @@ bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, c
         agree = agree && e.rasterize_mode == e0.rasterize_mode && e.aabb == e0.aabb &&
                 e.opacity_adaptive_radius == e0.opacity_adaptive_radius && e.draw_mode == e0.draw_mode &&
                 (e.rasterize_mode != BGS_RASTERIZE_CLASSIFICATION || e.num_classes == e0.num_classes) &&
-                blend_kind(e) == blend_kind(e0) && (is4 || !any_3d || e.gaussian_mode == gm3);
+                blend_kind(e) == blend_kind(e0) && box_of(j) == box_of(0) && (is4 || !any_3d || e.gaussian_mode == gm3);
         if (!is4) { any_3d = true; gm3 = e.gaussian_mode; }
         any_depth = any_depth || e.rasterize_mode == BGS_RASTERIZE_DEPTH;
         kinds |= 1u << blend_kind(e);
@@ -876,6 +889,7 @@ bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, c
     if (agree) {   // one frame's settings: exactly bgs_render_scene_4d
         bgs_settings s = st[0];
         s.gaussian_mode = any_3d ? gm3 : (uint32_t)BGS_GAUSSIAN_4D;
+        if (box_of(0)) s.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
         const bool need_ex = ex || ents[0].rasterize_mode == BGS_RASTERIZE_CLASSIFICATION;
         return render_scene_impl(c, call, true, clouds, unis, windows.data(), k, view, &s, need_ex ? &exs[0] : nullptr, depth,
                                  out_rgba, out_format, out_is_device_ptr);
@@ -891,6 +905,7 @@ bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, c
     tab.n_total = (uint32_t)total;
     scene->kinds.k = k;
     uint32_t offset = 0;
+    bool box_all = true;
     for (uint32_t j = 0; j < k; ++j) {
         const bgs_cloud* cl = clouds[j];
         const uint32_t rm = st[j].rasterize_mode;
@@ -910,12 +925,15 @@ bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, c
         if (sh) scene->need_sh[gi] = 1u;
         scene->classes.n[j] = ents[j].num_classes;
         scene->kinds.offset[j] = offset;
-        scene->kinds.kind[j] = (uint32_t)blend_kind(ents[j]);
+        scene->kinds.kind[j] = (uint32_t)blend_kind(ents[j]) | (box_of(j) ? BOX_KIND : 0u);
+        scene->box = scene->box || box_of(j);
+        box_all = box_all && box_of(j);
         offset += cl->n;
         scene->clouds.push_back(cl);
     }
-    // one kind: its own blend; several: the mixed one (with the surfel records when some entity has them)
-    scene->raster_mode = __builtin_popcount(kinds) > 1 ? ((kinds & 4u) ? 4 : 3) : __builtin_ctz(kinds);
+    // one kind: its own blend; several, or entities with and without the overlay: the mixed one (with the surfel records
+    // when some entity has them)
+    scene->raster_mode = __builtin_popcount(kinds) > 1 || box_all != scene->box ? ((kinds & 4u) ? 4 : 3) : __builtin_ctz(kinds);
     // the frame as render_impl plans it: its flags and sort bits, the Depth range when some entity is in Depth mode, and
     // the blend kind (an aabb frame when it is not quad-uv: one round)
     bgs_settings sf = *frame;
@@ -923,8 +941,17 @@ bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, c
     sf.aabb = scene->raster_mode != 0;
     sf.gaussian_mode = scene->raster_mode == 2 ? BGS_GAUSSIAN_2D : BGS_GAUSSIAN_3D;
     sf.draw_mode = BGS_DRAW_ALL;
+    if (scene->box) sf.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
     return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr,
                        depth, nullptr, scene);
+}
+
+bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                               const bgs_entity_settings* ents, uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                               const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
+                               int out_is_device_ptr) {
+    return bgs_render_entities_ex(c, clouds, unis, ents, nullptr, k, view, frame, ex, depth, out_rgba, out_format,
+                                  out_is_device_ptr);
 }
 
 bgs_status bgs_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,

@@ -100,6 +100,8 @@ struct SceneClasses {
 
 // The blend kind of each segment of a mixed-geometry frame (bgs_render_entities): 0 = quad-uv (OBB), 1 = conic (3DGS / 4D
 // with aabb), 2 = surfel (2DGS with aabb); raster.cu's class launch tags each compact slot with its segment's kind.
+// Bit 2 of a kind (BOX_KIND) is the segment's bounding-box overlay, read only by the overlay's mixed blend.
+constexpr uint32_t BOX_KIND = 4u;
 struct SegmentKinds {
     uint32_t k;
     uint32_t offset[BGS_SCENE_MAX_CLOUDS];

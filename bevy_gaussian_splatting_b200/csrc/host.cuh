@@ -73,12 +73,14 @@ struct SceneFacts {
     // bgs_render_entities frames whose entities disagree: each group's launch (project_group, plus ENTITY_MODES for the
     // Classification / OpticalFlow / Velocity colour kernel) with whether one of its segments reads the SH coefficients,
     // the segments' num_classes, and the blend (raster.cu's mode: 0..2 when every splat has one kind, else 3 / 4 with
-    // `kinds`)
+    // `kinds`), and whether some entity draws its bounding boxes (kinds' BOX_KIND bits say which, on mixed frames; on the
+    // others every entity does)
     bool entities = false;
     std::vector<uint32_t> need_sh;   // per entry of groups
     SceneClasses classes = {};
     int raster_mode = 0;
     SegmentKinds kinds = {};
+    bool box = false;
 };
 
 // What the host knows of a frame it has enqueued: the context keeps the last one enqueued (`pend`) and, once its

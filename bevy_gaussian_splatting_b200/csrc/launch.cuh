@@ -81,11 +81,12 @@ struct ZTestArgs {
     size_t pitch = 0;
 };
 // mode 0..2: one blend kind for every splat; 3 / 4 (bgs_render_entities): mixed kinds, read from `kinds` (one byte per
-// record), 4 when some splat is a surfel
+// record), 4 when some splat is a surfel.  box: the bounding-box overlay (BGS_FLAG_VISUALIZE_BOUNDING_BOX) on every
+// splat, or on a mixed frame on those whose kinds byte has bit 2 set; large_footprints is then not read.
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
                    const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
-                   cudaStream_t stream, const unsigned char* kinds = nullptr);
+                   cudaStream_t stream, const unsigned char* kinds = nullptr, bool box = false);
 // a mixed-geometry frame's blend kind of each compact slot (records n_vis of ctr), from its segment's
 void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
                           uint32_t n_hint, int sm_count, cudaStream_t stream);

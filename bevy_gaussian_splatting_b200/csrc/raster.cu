@@ -216,6 +216,15 @@ __device__ __forceinline__ float warp_min_depth(float z) {
 }
 __device__ __forceinline__ float lds_f32(uint32_t a) { float r; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(a)); return r; }
 
+// BOX (BGS_FLAG_VISUALIZE_BOUNDING_BOX, gaussian.wgsl:486-495): the pair lies on its quad's edge band when s = uv / 2 + 1/2
+// is within 0.08 of 0 or 1 on either axis (a NaN component is not an edge).  uv is the quad uv of a quad-uv splat and
+// m / R of a conic or surfel one.
+constexpr float BOX_EDGE = 0.08f;
+__device__ __forceinline__ bool box_edge(float u, float v) {
+    const float sx = __fadd_rn(__fmul_rn(u, 0.5f), 0.5f), sy = __fadd_rn(__fmul_rn(v, 0.5f), 0.5f);
+    return sx < BOX_EDGE || sx > 1.0f - BOX_EDGE || sy < BOX_EDGE || sy > 1.0f - BOX_EDGE;
+}
+
 // Each warp compacts the chunk's `cnt` staged splats to those `hit(j)` keeps, in order, into its u16 list as
 // `rec0 + j * 16` (the q0 record's address relative to rec0); returns the list's length.
 template <class Hit>
@@ -243,7 +252,11 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // MODE 3 / 4 (bgs_render_entities): mixed kinds, each splat tested by its own: kinds[r] (raster_kinds_kernel) is record r's
 // 0 = quad-uv, 1 = conic, 2 = surfel; MODE 4 when some splat is a surfel (the only one that stages the surfel records).
 // Warp candidates: bbox for every kind, and the separating-axis test of MODE 0 for the quad-uv splats.
-template <int MODE, bool AUX, bool ZTEST>
+// BOX (raster_box_kernel, raster_mixed_box_kernel): the bounding-box overlay.  A covered pair (after the aabb discard and
+// the depth test) on its quad's edge band (box_edge) blends (0.3, 1, 0.1) at alpha 1 into every frame it writes, which
+// stops the pixel; other pairs blend as without it.  Mixed frames read the overlay bit of each splat from bit 2 of its
+// kinds byte (its entity's), the others draw every splat's box.  MODE 0 takes the generic loop, not the inline-asm one.
+template <int MODE, bool AUX, bool ZTEST, bool BOX = false>
 __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
                                             const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
                                             int H, int tiles_x, void* __restrict__ out, uint32_t format,
@@ -319,8 +332,9 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
             s_q0[t] = p0;
             s_uv[t] = p1;
             s_q2[t] = __ldg(rp + 2);
-            const int kind = MIXED ? (int)__ldg(kinds + r) : MODE;
-            if (MIXED) s_kind[t] = (unsigned char)kind;
+            const int kb = MIXED ? (int)__ldg(kinds + r) : MODE;   // BOX: kind | overlay << 2
+            if (MIXED) s_kind[t] = (unsigned char)kb;
+            const int kind = BOX ? (kb & 3) : kb;
             if (kind == 0) {
                 // thresholds of the per-warp separating-axis cull below, once per splat: the quad |u| <= 1, |v| <= 1
                 // misses a warp rectangle (pixel centres within +-3.5 x +-1.5 of its centre) when |u(centre)| exceeds
@@ -352,7 +366,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
             // (`|`, not `||`: the four compares are one predicated test, not a chain of branches)
             bool hit = !((int)(bx >> 16) < wx0 | (int)(bx & 0xFFFFu) > wx0 + 7 | (int)(by >> 16) < wy0 |
                          (int)(by & 0xFFFFu) > wy0 + 3);
-            if ((MODE == 0 || (MIXED && s_kind[j] == 0)) && hit) {
+            if ((MODE == 0 || (MIXED && (BOX ? (s_kind[j] & 3) : s_kind[j]) == 0)) && hit) {
                 // separating-axis test of the splat's quad against this warp's pixel centres
                 // [wx0 + .5, wx0 + 7.5] x [wy0 + .5, wy0 + 3.5] (thresholds staged per splat above): the bbox
                 // of a slanted quad passes many warps none of whose pixels it covers
@@ -364,7 +378,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
             if (ZTEST && hit) hit = !(reinterpret_cast<const float*>(s_mem + REC_D)[4 * j] < zmin);
             return hit;
         });
-        if (MODE == 0 && !AUX) {
+        if (MODE == 0 && !AUX && !BOX) {
             // four candidates per iteration, so loop control is paid once per four; each list entry is its own 16-bit
             // load (cheaper than unpacking a 32-bit pair); blending stays strictly in list order.
             // The blend is PREDICATED, not branched: 15 SASS instructions per candidate instead of a divergent block
@@ -440,10 +454,14 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                 auto depth_ok = [&]() { return !ZTEST || lds_f32(a_rec + REC_D) >= zs; };
                 float e;
                 float4 q2;
-                const int kind = MIXED ? (int)s_kind[(a_rec - a_base) >> 4] : MODE;
+                const int kb = MIXED ? (int)s_kind[(a_rec - a_base) >> 4] : MODE;
+                const int kind = BOX ? (kb & 3) : kb;
+                const bool box = BOX && (!MIXED || (kb >> 2) != 0);   // this splat's overlay
+                bool edge = false;                                     // BOX: the pair is on its quad's edge band
                 if (kind == 0) {
                     const float2 uv = quad_uv(fx, fy, q0, q1);
                     if (!(fabsf(uv.x) <= 1.0f && fabsf(uv.y) <= 1.0f && depth_ok())) continue;
+                    if (BOX) edge = box && box_edge(uv.x, uv.y);
                     const float qd = __fmaf_rn(uv.y, uv.y, __fmul_rn(uv.x, uv.x));
                     q2 = lds4(a_rec + REC_Q2);
                     // exp(-4.5 qd) = 2^(qd * -4.5 log2 e); qd <= 2 so the argument stays >= -13 (no range fix-up)
@@ -453,7 +471,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                     const float dx = __fsub_rn(fx, q0.x), dy = __fsub_rn(fy, q0.y);
                     const float mx = __fadd_rn(dx, dx), my = -__fadd_rn(dy, dy);
                     const float Rq = q1.y;   // MODE 1: quad half-side in half-pixels
-                    float power;
+                    float power, R = Rq;     // R: the half-side the coverage test compares |m| against
                     if (kind == 1 || !SURF) {
                         if (!(fabsf(mx) <= Rq && fabsf(my) <= Rq && depth_ok())) continue;
                         // q0.z, q0.w, q1.x = conic x, y, z;  d = -m  (gaussian.wgsl:459-462)
@@ -463,6 +481,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                     } else {
                         const float4 e0 = lds4(a_rec + SM_EXTRA);
                         if (!(fabsf(mx) <= e0.x && fabsf(my) <= e0.x && depth_ok())) continue;
+                        if (BOX) R = e0.x;
                         const float4 e1 = lds4(a_rec + SM_EXTRA + RT_CHUNK * 16);
                         const float4 e2 = lds4(a_rec + SM_EXTRA + 2 * RT_CHUNK * 16);
                         const float4 e3 = lds4(a_rec + SM_EXTRA + 3 * RT_CHUNK * 16);
@@ -483,8 +502,18 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                         power = -__fmul_rn(0.5f, fminf(s3, s2));
                     }
                     if (power > 0.0f) continue;                      // gaussian.wgsl:468-470
+                    if (BOX) edge = box && box_edge(__fdiv_rn(mx, R), __fdiv_rn(my, R));
                     q2 = lds4(a_rec + REC_Q2);
                     e = __expf(power);
+                }
+                if (BOX && edge) {   // the overlay colour at alpha exactly 1 (w = T) into every frame; T = 0 stops the pixel
+                    cr = fmaf(T, 0.3f, cr); cg = fmaf(T, 1.0f, cg); cb = fmaf(T, 0.1f, cb);
+                    if (AUX) {
+                        dr = fmaf(T, 0.3f, dr); dg = fmaf(T, 1.0f, dg); db = fmaf(T, 0.1f, db);
+                        nr = fmaf(T, 0.3f, nr); ng = fmaf(T, 1.0f, ng); nb = fmaf(T, 0.1f, nb);
+                    }
+                    T = 0.0f;
+                    break;
                 }
                 const float a = fminf(e * q2.w, 0.999f);
                 const float w = a * T;
@@ -531,7 +560,31 @@ raster_mixed_kernel(const SplatRec* __restrict__ recs, const float4* __restrict_
                                     truncated, splat_d, scene, pitch, kinds);
 }
 
-// the kind of each compact slot r < n_vis: its global index's segment's
+// The bounding-box overlay's blends (raster_body's BOX): raster_kernel's and raster_mixed_kernel's, with their launch
+// bounds.  Kernels of their own, so the frames without the overlay keep the very kernels they had.
+template <int MODE, bool AUX, bool ZTEST>
+__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : 5)
+raster_box_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
+                  const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
+                  const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
+                  const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
+                  size_t pitch) {
+    raster_body<MODE, AUX, ZTEST, true>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth,
+                                        out_normal, truncated, splat_d, scene, pitch, nullptr);
+}
+
+template <int MODE, bool ZTEST>
+__global__ void __launch_bounds__(RT_THREADS, ZTEST ? 4 : 5)
+raster_mixed_box_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
+                        const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W, int H, int tiles_x,
+                        void* __restrict__ out, uint32_t format, const uint32_t* __restrict__ truncated,
+                        const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
+                        const unsigned char* __restrict__ kinds) {
+    raster_body<MODE, false, ZTEST, true>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr,
+                                          nullptr, truncated, splat_d, scene, pitch, kinds);
+}
+
+// the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
 __global__ void raster_kinds_kernel(SegmentKinds sk, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
                                     unsigned char* __restrict__ out) {
     const uint32_t n_vis = ctr->n_vis;
@@ -726,9 +779,28 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
 void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
                    const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
                    const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
-                   cudaStream_t stream, const unsigned char* kinds) {
+                   cudaStream_t stream, const unsigned char* kinds, bool box) {
     const int grid = tiles_x * tiles_y;
     const bool ztest = zt.scene != nullptr;   // (bgs_render_aux frames never carry a depth buffer)
+    if (box) {   // the bounding-box overlay: raster_body's generic loop for every mode, never raster2_kernel
+        if (mode >= 3) {
+            auto* kernel = mode == 3 ? (ztest ? raster_mixed_box_kernel<3, true> : raster_mixed_box_kernel<3, false>)
+                                     : (ztest ? raster_mixed_box_kernel<4, true> : raster_mixed_box_kernel<4, false>);
+            kernel<<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, truncated,
+                                                    zt.splat_d, zt.scene, zt.pitch, kinds);
+            return;
+        }
+        static void (*const box_kernels[3][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int,
+                                               void*, uint32_t, const float4*, void*, void*, const uint32_t*, const float*,
+                                               const float*, size_t) = {
+            {raster_box_kernel<0, false, false>, raster_box_kernel<1, false, false>, raster_box_kernel<2, false, false>},
+            {raster_box_kernel<0, true, false>, raster_box_kernel<1, true, false>, raster_box_kernel<2, true, false>},
+            {raster_box_kernel<0, false, true>, raster_box_kernel<1, false, true>, raster_box_kernel<2, false, true>}};
+        box_kernels[ztest ? 2 : aux != nullptr][mode]<<<grid, RT_THREADS, 0, stream>>>(
+            recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated, zt.splat_d,
+            zt.scene, zt.pitch);
+        return;
+    }
     if (mode >= 3) {
         auto* kernel = mode == 3 ? (ztest ? raster_mixed_kernel<3, true> : raster_mixed_kernel<3, false>)
                                  : (ztest ? raster_mixed_kernel<4, true> : raster_mixed_kernel<4, false>);

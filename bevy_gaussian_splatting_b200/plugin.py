@@ -414,13 +414,15 @@ class GaussianSplattingPlugin:
         """`render_scene` with each entity drawn with its own CloudSettings (`bgs_render_entities`): gaussian_mode,
         rasterize_mode, aabb, opacity_adaptive_radius, draw_mode, num_classes and the 4D window are per entity, so a
         highlighted selection, a Classification object or a 2DGS surface drawn with aabb share one depth-sorted frame
-        with the scan around them.  radix_sort_depth_bits (and the other sort fields) are the frame's and must agree
-        (`check_entities`, ValueError before any call).  The other arguments are `render_scene`'s."""
+        with the scan around them.  visualize_bounding_box is per entity too (`bgs_render_entities_ex`'s entity flags).
+        radix_sort_depth_bits (and the other sort fields) are the frame's and must agree (`check_entities`, ValueError
+        before any call).  The other arguments are `render_scene`'s."""
         entities = list(entities)
         first = check_entities(entities)
         code, dtype, ch = self.FORMATS[fmt]
         v = view.to_abi()
         s = first.to_abi()
+        s.flags &= ~abi.BGS_FLAG_VISUALIZE_BOUNDING_BOX   # (each entity's own, below)
         s.flags |= ((abi.BGS_FLAG_ASYNC if asynchronous else 0) | (abi.BGS_FLAG_PREMULTIPLIED_OUT if premultiplied else 0)
                     | (abi.BGS_FLAG_BLEND_OVER_TARGET if blend_over else 0))
         ex = None
@@ -428,6 +430,8 @@ class GaussianSplattingPlugin:
             ex = abi.bgs_render_extras(num_classes=1, delta_time=float(delta_time) if delta_time is not None else 0.0)
             ex.previous_clip_from_world[:] = previous_view.to_abi().clip_from_world[:]
         k = len(entities)
+        eflags = (C.c_uint32 * k)(*[abi.BGS_ENTITY_VISUALIZE_BOUNDING_BOX if st.visualize_bounding_box else 0
+                                    for _, st, _ in entities])
         clouds = (C.c_void_p * k)(*[h._h.value for h, _, _ in entities])
         unis = (abi.bgs_cloud_uniform * k)(*[self.cloud_uniform(st, tr, h.aabb) for h, st, tr in entities])
         ents = (abi.bgs_entity_settings * k)(*[entity_settings(st) for _, st, _ in entities])
@@ -435,9 +439,9 @@ class GaussianSplattingPlugin:
             out = np.empty((view.height, view.width, ch), dtype)
         assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
         zd = self._scene_depth(scene_depth, view)
-        self._check(self._lib.bgs_render_entities(self._ctx, clouds, unis, ents, k, C.byref(v), C.byref(s),
-                                                  None if ex is None else C.byref(ex), None if zd is None else C.byref(zd),
-                                                  _ptr(out), code, 0))
+        self._check(self._lib.bgs_render_entities_ex(self._ctx, clouds, unis, ents, eflags, k, C.byref(v), C.byref(s),
+                                                     None if ex is None else C.byref(ex), None if zd is None else C.byref(zd),
+                                                     _ptr(out), code, 0))
         return out
 
     def _render_4d(self, handle, v, u, s, ex, zd, settings, target, code, is_device):

@@ -126,9 +126,6 @@ class CloudSettings:
     playback_mode: PlaybackMode = PlaybackMode.Still
 
     def to_abi(self) -> abi.bgs_settings:
-        if self.visualize_bounding_box:
-            # VISUALIZE_BOUNDING_BOX (gaussian.wgsl:486-495) is a debug overlay outside the hot path (SURVEY.md §8)
-            raise NotImplementedError("CloudSettings.visualize_bounding_box is not supported by the C ABI")
         return abi.bgs_settings(
             gaussian_mode=int(self.gaussian_mode),
             rasterize_mode=int(self.rasterize_mode),
@@ -137,7 +134,8 @@ class CloudSettings:
             draw_mode=int(self.draw_mode),
             radix_sort_depth_bits=int(self.radix_sort_depth_bits),
             flags=(abi.BGS_FLAG_SORT_ALL if self.sort_all else 0)
-            | (0 if self.binning_rounds is None else (abi.BGS_FLAG_CHUNKS if self.binning_rounds else abi.BGS_FLAG_NO_CHUNKS)),
+            | (0 if self.binning_rounds is None else (abi.BGS_FLAG_CHUNKS if self.binning_rounds else abi.BGS_FLAG_NO_CHUNKS))
+            | (abi.BGS_FLAG_VISUALIZE_BOUNDING_BOX if self.visualize_bounding_box else 0),
             reserved=0,
         )
 

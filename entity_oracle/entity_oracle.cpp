@@ -5,12 +5,48 @@
 
 #include "entity_oracle.h"
 
+namespace {
+
+// VISUALIZE_BOUNDING_BOX (gaussian.wgsl:486-495) for a covered pair's decision: uv = (u, v) of a quad-uv splat, m / R of a
+// conic or surfel one; s = uv * 0.5 + 0.5 (the multiply exact, one rounding); an edge within 0.08 of 0 or 1 on either axis
+bool box_edge(const Decision& d, const orc_settings& s, float* sx_out = nullptr, float* sy_out = nullptr) {
+    const float ux = s.aabb ? d.mx / d.Rq : d.u, uy = s.aabb ? d.my / d.Rq : d.v;
+    const float sx = ux * 0.5f + 0.5f, sy = uy * 0.5f + 0.5f;
+    if (sx_out) { *sx_out = sx; *sy_out = sy; }
+    const float w = 0.08f;
+    return sx < w || sx > 1.0f - w || sy < w || sy > 1.0f - w;
+}
+
+}  // namespace
+
 extern "C" {
+
+int eo_edge_probe(uint32_t count, const orc_splat* splats, const orc_settings* s, const float* pixel_xy, uint32_t* covered,
+                  uint32_t* edge, float* s_xy) {
+    if (!s) return 2;
+    for (uint32_t j = 0; j < count; ++j) {
+        const Decision d = decide(splats[j], *s, pixel_xy[2 * j], pixel_xy[2 * j + 1]);
+        float sx = 0.0f, sy = 0.0f;
+        const bool e = d.covered && box_edge(d, *s, &sx, &sy);
+        covered[j] = d.covered ? 1u : 0u;
+        edge[j] = e ? 1u : 0u;
+        if (s_xy) { s_xy[2 * j] = d.covered ? sx : 0.0f; s_xy[2 * j + 1] = d.covered ? sy : 0.0f; }
+    }
+    return 0;
+}
 
 int eo_frame(uint32_t k, const s4o_cloud* cl, const orc_view* view, const orc_settings* es, const uint32_t* nc,
              const tor_temporal* ex, const float* scene, uint64_t pitch_bytes, uint32_t* n_vis, uint64_t* n_pairs, uint32_t* sorted,
              float* records, uint32_t* rank_to_id, float* depths, uint32_t* tile_ranges, uint32_t* tile_entries, uint64_t cap,
              float* image, int threads) {
+    return eo_frame_ex(k, cl, view, es, nc, nullptr, ex, scene, pitch_bytes, n_vis, n_pairs, sorted, records, rank_to_id,
+                       depths, tile_ranges, tile_entries, cap, image, nullptr, threads);
+}
+
+int eo_frame_ex(uint32_t k, const s4o_cloud* cl, const orc_view* view, const orc_settings* es, const uint32_t* nc,
+                const uint32_t* entity_flags, const tor_temporal* ex, const float* scene, uint64_t pitch_bytes, uint32_t* n_vis,
+                uint64_t* n_pairs, uint32_t* sorted, float* records, uint32_t* rank_to_id, float* depths, uint32_t* tile_ranges,
+                uint32_t* tile_entries, uint64_t cap, float* image, uint8_t* edge_mask, int threads) {
     if (k == 0 || !cl || !view || !es || !nc || !ex) return 2;
 #ifdef _OPENMP
     if (threads > 0) omp_set_num_threads(threads);
@@ -131,14 +167,24 @@ int eo_frame(uint32_t k, const s4o_cloud* cl, const orc_view* view, const orc_se
             const int x = tx * TILE + lx, y = ty * TILE + ly;
             if (x >= W || y >= H) continue;
             float T = 1.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f;
+            bool edged = false;
             for (uint64_t e = count[t]; e < count[t + 1]; ++e) {
                 const orc_splat& sp = F.splats[entries[e]];
-                float a;
-                if (!eval_alpha(sp, sb[seg_of[entries[e]]], (float)x + 0.5f, (float)y + 0.5f, &a)) continue;
+                const uint32_t j = seg_of[entries[e]];
+                const Decision d = decide(sp, sb[j], (float)x + 0.5f, (float)y + 0.5f);
+                if (!d.covered) continue;
                 if (scene) {
                     const float zs = *reinterpret_cast<const float*>(reinterpret_cast<const char*>(scene) + (uint64_t)y * pitch_bytes + 4u * (uint64_t)x);
                     if (!(dz[entries[e]] >= zs)) continue;
                 }
+                // the entity's bounding-box overlay: an edge pair blends (0.3, 1, 0.1) at alpha 1, which stops the pixel
+                if (entity_flags && (entity_flags[j] & 1u) && box_edge(d, sb[j])) {
+                    cr += T * 0.3f; cg += T * 1.0f; cb += T * 0.1f;
+                    T = 0.0f;
+                    edged = true;
+                    break;
+                }
+                const float a = alpha_of(sp, d.power);
                 const float w = a * T;
                 cr += w * sp.r; cg += w * sp.g; cb += w * sp.b;
                 T = T * (1.0f - a);
@@ -146,6 +192,7 @@ int eo_frame(uint32_t k, const s4o_cloud* cl, const orc_view* view, const orc_se
             }
             float* px = image + 4 * ((size_t)y * W + x);
             px[0] = cr; px[1] = cg; px[2] = cb; px[3] = 1.0f;
+            if (edge_mask) edge_mask[(size_t)y * W + x] = edged ? 1u : 0u;
         }
     }
     return 0;

@@ -26,6 +26,22 @@ int eo_frame(uint32_t k, const s4o_cloud* clouds, const orc_view* view, const or
              float* records, uint32_t* rank_to_id, float* depths, uint32_t* tile_ranges, uint32_t* tile_entries, uint64_t cap,
              float* image, int threads);
 
+/* eo_frame with each entity's flags (bgs_render_entities_ex): entity_flags[j] bit 0 (BGS_ENTITY_VISUALIZE_BOUNDING_BOX)
+ * draws entity j's bounding boxes (include/bgs.h's BGS_FLAG_VISUALIZE_BOUNDING_BOX rule: a covered, depth-passing pair on
+ * its quad's edge band blends (0.3, 1, 0.1) at alpha 1 and stops the pixel); entity_flags == NULL is eo_frame.  edge_mask
+ * (W*H bytes, optional): 1 where an edge pair blended. */
+int eo_frame_ex(uint32_t k, const s4o_cloud* clouds, const orc_view* view, const orc_settings* settings, const uint32_t* num_classes,
+                const uint32_t* entity_flags, const tor_temporal* ex, const float* scene, uint64_t pitch_bytes, uint32_t* n_vis,
+                uint64_t* n_pairs, uint32_t* sorted, float* records, uint32_t* rank_to_id, float* depths, uint32_t* tile_ranges,
+                uint32_t* tile_entries, uint64_t cap, float* image, uint8_t* edge_mask, int threads);
+
+/* The overlay's edge decision per pair: splat record splats[j] (orc_splat, the oracle's own) at the pixel centre
+ * (pixel_xy[2j], pixel_xy[2j+1]) under settings s (aabb, gaussian_mode as the blend reads them: 1 = conic, 0 = surfel).
+ * covered[j]: the coverage decision (oracle/bgs_oracle.cpp's decide()); edge[j]: covered and on the edge band; s_xy
+ * (optional, 2 per pair): s = uv * 0.5 + 0.5 of covered pairs. */
+int eo_edge_probe(uint32_t count, const orc_splat* splats, const orc_settings* s, const float* pixel_xy, uint32_t* covered,
+                  uint32_t* edge, float* s_xy);
+
 #ifdef __cplusplus
 }
 #endif

@@ -86,12 +86,38 @@ enum {
                                a synchronous call renders such a frame again by itself and composites it once; after a
                                queued one, bgs_sync's BGS_NOT_READY means the overflowed frames did not touch their
                                targets, so rendering them again composites each once. */
-    BGS_FLAG_CHUNKS = 8u    /* bin / tile-sort / blend in front-to-back rank rounds that stop emitting (splat, tile)
+    BGS_FLAG_CHUNKS = 8u,   /* bin / tile-sort / blend in front-to-back rank rounds that stop emitting (splat, tile)
                                pairs once every tile has saturated.  Same pixels, bit for bit.  Only USE_OBB frames from
-                               bgs_render (not USE_AABB ones, not bgs_render_aux) of at most 65536 tiles are ever split
+                               bgs_render (not USE_AABB ones, not bgs_render_aux, not BGS_FLAG_VISUALIZE_BOUNDING_BOX
+                               ones) of at most 65536 tiles are ever split
                                into rounds; other frames ignore the flag and run one round.  Without either flag the
                                library picks rounds for such frames when the previous frame had >= 32 (splat, tile)
                                pairs per visible splat and >= 2^24 pairs. */
+    BGS_FLAG_VISUALIZE_BOUNDING_BOX = 64u /* CloudSettings.visualize_bounding_box (the reference's VISUALIZE_BOUNDING_BOX
+                               shader def, gaussian.wgsl:486-495): draw a band around each splat's quad, opaque green.
+                               Honoured by bgs_render, _ex, _depth_test, _aux, _4d, _scene and _scene_4d (every listed
+                               cloud) and bgs_render_entities (every entity).  The rule, exactly:
+                               - For a (pixel, splat) pair whose coverage decision holds (after the aabb power > 0
+                                 discard) and, under a depth buffer, whose depth test holds, take uv: the quad uv of the
+                                 coverage test |u|, |v| <= 1 for quad-uv splats (USE_OBB: 3DGS, 2DGS, 4D); (mx / R, my / R)
+                                 for conic (3DGS / 4D with aabb) and surfel (2DGS with aabb) splats, m the quad-space
+                                 offset in half-pixels (y up) and R the half-side the coverage test compares |m| against,
+                                 IEEE division.
+                               - s = uv * 0.5f + 0.5f per component in f32 (the multiply is exact: one rounding).  The
+                                 pair is an edge iff s.x < 0.08f || s.x > 1.0f - 0.08f || s.y < 0.08f || s.y > 1.0f - 0.08f
+                                 (the subtraction in f32; a NaN component is not an edge).
+                               - An edge pair blends (0.3f, 1.0f, 0.1f) at alpha exactly 1: C += T * colour, T := 0, so
+                                 the pixel stops.  Any other covered pair blends as without the flag.  The test comes
+                                 before the opacity, so boxes are drawn whatever the splat's opacity or colour (opacity
+                                 0, global_opacity 0, Velocity's zeroed splats); a splat with no quad (culled, unselected
+                                 under BGS_DRAW_SELECTED, time-masked 4D) has none.
+                               - bgs_render_aux: the depth and normal frames get the same edges, in the same colour.
+                               - Unchanged: key-gen, both sorts, records, binning, tile ranges and slices, splat depths
+                                 and every debug hook.  An overlay frame runs in one round (BGS_FLAG_CHUNKS is ignored),
+                                 so bgs_frame_stats is that of the same frame with BGS_FLAG_NO_CHUNKS.
+                               - Unpinned: the reference interpolates uv across the quad in fixed function; whether that
+                                 equals this uv (or its negation on one axis) is unpinned to the last ulp, so decisions
+                                 within an ulp of a band edge may differ from the reference's. */
 };
 typedef struct {
     uint32_t gaussian_mode;           /* BGS_GAUSSIAN_* */
@@ -687,6 +713,19 @@ bgs_status bgs_render_entities(bgs_context* ctx, const bgs_cloud* const* clouds,
                                const bgs_settings* frame /* radix_sort_depth_bits and flags only */,
                                const bgs_render_extras* extras /* previous view and delta_time; num_classes unused */,
                                const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr);
+
+/* bgs_render_entities with each entity's own flags (the reference's per-entity pipeline key): entity_flags[j] (k words;
+ * NULL = none) is a set of BGS_ENTITY_* bits.  BGS_ENTITY_VISUALIZE_BOUNDING_BOX draws entity j's bounding boxes
+ * (BGS_FLAG_VISUALIZE_BOUNDING_BOX's rule, for its splats only); the frame's BGS_FLAG_VISUALIZE_BOUNDING_BOX draws every
+ * entity's.  Entities agree only when their overlays also agree; entities that differ in nothing else still blend in the
+ * mixed blend.  bgs_render_entities is this call with entity_flags = NULL.  Refused with BGS_EINVAL, nothing enqueued or
+ * written: an unknown bit in some entity_flags[j], and every refusal of bgs_render_entities. */
+enum { BGS_ENTITY_VISUALIZE_BOUNDING_BOX = 1u };
+bgs_status bgs_render_entities_ex(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                                  const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */,
+                                  uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                                  const bgs_render_extras* extras, const bgs_scene_depth* depth, void* out_rgba,
+                                  uint32_t out_format, int out_is_device_ptr);
 
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a

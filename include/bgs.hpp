@@ -36,6 +36,7 @@ struct CloudSettings {   // src/gaussian/settings.rs:110-133 (defaults)
     float global_opacity = 1.0f;
     float global_scale = 1.0f;
     bool opacity_adaptive_radius = true;
+    bool visualize_bounding_box = false;   // the band around each splat's quad (BGS_FLAG_VISUALIZE_BOUNDING_BOX)
     RadixSortDepthBits radix_sort_depth_bits = RadixSortDepthBits::Bits32;
     DrawMode draw_mode = DrawMode::All;
     GaussianMode gaussian_mode = GaussianMode::Gaussian3d;
@@ -51,6 +52,7 @@ struct CloudSettings {   // src/gaussian/settings.rs:110-133 (defaults)
 
     bgs_settings to_abi(uint32_t flags = 0) const {
         if (binning_rounds >= 0) flags |= binning_rounds ? BGS_FLAG_CHUNKS : BGS_FLAG_NO_CHUNKS;
+        if (visualize_bounding_box) flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
         bgs_settings s{};
         s.gaussian_mode = (uint32_t)gaussian_mode; s.rasterize_mode = (uint32_t)rasterize_mode;
         s.aabb = aabb; s.opacity_adaptive_radius = opacity_adaptive_radius; s.draw_mode = (uint32_t)draw_mode;
@@ -424,9 +426,9 @@ public:
         check(st);
         return true;
     }
-    // render_scene with each entity drawn with its own settings (bgs_render_entities): gaussian_mode, rasterize_mode, aabb,
-    // opacity_adaptive_radius, draw_mode, num_classes and [time_start, time_stop] are the entity's; the sort settings and
-    // `extra_flags` are the frame's, taken from entities[0].  The arguments are render_scene's.
+    // render_scene with each entity drawn with its own settings (bgs_render_entities_ex): gaussian_mode, rasterize_mode, aabb,
+    // opacity_adaptive_radius, draw_mode, num_classes, visualize_bounding_box and [time_start, time_stop] are the entity's;
+    // the sort settings and `extra_flags` are the frame's, taken from entities[0].  The arguments are render_scene's.
     bool render_entities(const std::vector<SceneEntity>& entities, const bgs_view& view, void* out_rgba,
                          uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr, float delta_time = 0.0f,
                          const float* depth = nullptr, uint64_t pitch_bytes = 0, bool out_is_device = false,
@@ -435,6 +437,7 @@ public:
         std::vector<const bgs_cloud*> clouds;
         std::vector<bgs_cloud_uniform> unis;
         std::vector<bgs_entity_settings> ents;
+        std::vector<uint32_t> eflags;
         for (const SceneEntity& e : entities) {
             bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
             std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
@@ -443,8 +446,10 @@ public:
             const bgs_settings s = e.settings.to_abi();
             ents.push_back({s.gaussian_mode, s.rasterize_mode, s.aabb, s.opacity_adaptive_radius, s.draw_mode,
                             e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
+            eflags.push_back(e.settings.visualize_bounding_box ? (uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX : 0u);
         }
-        const bgs_settings s = entities[0].settings.to_abi(extra_flags);
+        bgs_settings s = entities[0].settings.to_abi(extra_flags);
+        if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
         bgs_render_extras ex{};
         ex.num_classes = 1;
         if (previous_view) {
@@ -452,9 +457,9 @@ public:
             ex.delta_time = delta_time;
         }
         const bgs_scene_depth zd{depth, pitch_bytes};
-        const bgs_status st = bgs_render_entities(ctx_, clouds.data(), unis.data(), ents.data(), (uint32_t)clouds.size(), &view, &s,
-                                                  previous_view ? &ex : nullptr, depth ? &zd : nullptr, out_rgba, format,
-                                                  out_is_device ? 1 : 0);
+        const bgs_status st = bgs_render_entities_ex(ctx_, clouds.data(), unis.data(), ents.data(), eflags.data(),
+                                                     (uint32_t)clouds.size(), &view, &s, previous_view ? &ex : nullptr,
+                                                     depth ? &zd : nullptr, out_rgba, format, out_is_device ? 1 : 0);
         if (st == BGS_NOT_READY) return false;
         check(st);
         return true;
