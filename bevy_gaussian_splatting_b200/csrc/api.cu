@@ -454,7 +454,7 @@ static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, co
 }
 
 // Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.  A scene frame
-// (bgs_render_scene) runs key-gen, the depth range, the projection and the splat depths over its segment table; `cloud`
+// (render_entities_impl) runs key-gen, the depth range, the projection and the splat depths over its segment table; `cloud`
 // is then its first cloud and fc its first segment's.
 static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const ModeConsts* modes,
                                 const TemporalConsts* tc, const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd,
@@ -475,15 +475,18 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     // ---- stage 1: key-gen (+ stable compaction of the visible set)
     // compact mode: keys[0][slot], slot_ids[slot] = gaussian index, vals[0][slot] = slot (sort payload)
     // SORT_ALL    : keys[0][i], vals[0][i] = i (payload is the gaussian index itself)
-    if (scene && scene->entities && p.depth_range && scene->tab.seg[0].fc.rasterize_mode != BGS_RASTERIZE_DEPTH) {
-        // (key-gen gathers the culled ends for the Depth range when segment 0 is in Depth mode: some other entity is)
-        SceneTable kt = scene->tab;
-        kt.seg[0].fc.rasterize_mode = BGS_RASTERIZE_DEPTH;
-        CU(c, launch_keygen_scene(kt, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt, c->ctr, c->hist,
-                                  p.depth_passes, std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
-    } else if (scene) {   // (scenes are compact frames)
-        CU(c, launch_keygen_scene(scene->tab, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt, c->ctr,
-                                  c->hist, p.depth_passes, std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
+    if (scene) {   // (scenes are compact frames)
+        // key-gen gathers the culled ends for the Depth range when segment 0 is in Depth mode: when only some other
+        // entity is, it reads a copy of the table whose segment 0 is
+        SceneTable kt;
+        const bool depth0 = p.depth_range && scene->tab.seg[0].fc.rasterize_mode != BGS_RASTERIZE_DEPTH;
+        if (depth0) {
+            kt = scene->tab;
+            kt.seg[0].fc.rasterize_mode = BGS_RASTERIZE_DEPTH;
+        }
+        CU(c, launch_keygen_scene(depth0 ? kt : scene->tab, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p,
+                                  c->kg_block_cnt, c->ctr, c->hist, p.depth_passes,
+                                  std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
     } else if (p.by_slot) {
         // the cooperative key-gen also produces the depth sort's digit histograms
         // (keys[1] = visibility-mask scratch until the sort's first pass overwrites it)
@@ -516,29 +519,16 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     }
     CU(c, cudaEventRecord(c->ev_p0, ps));
     bool scene_3d = false;   // a scene lists a non-4D cloud (whose splat depths splat_depth_scene writes)
-    if (scene && scene->entities) {   // entities that disagree: each segment with its own settings and num_classes
-        const ModeConsts mc = modes ? *modes : ModeConsts{};
+    if (scene) {   // one launch per projection group: each segment with its own settings and num_classes
         for (size_t i = 0; i < scene->groups.size(); ++i) {
             const uint32_t g = scene->groups[i];
-            if (g == PROJECT_GROUP_4D) {
-                launch_project_4d_entities(scene->tab, scene->times, scene->classes, mc, c->slot_ids.p, c->ctr, c->recs.p,
-                                           zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
-            } else {
-                launch_project_entities(scene->tab, g, scene->need_sh[i] != 0, scene->classes, mc, c->slot_ids.p, c->ctr,
-                                        c->recs.p, (p.raster_mode == 2 || p.raster_mode == 4) ? c->extra.p : nullptr, p.n_hint,
-                                        c->sm_count, c->cutoff_tab, ps);
-                scene_3d = true;
-            }
-            ++launches;
-        }
-    } else if (scene) {   // one launch per projection kernel the scene's clouds need
-        for (const uint32_t g : scene->groups) {
             if (g == PROJECT_GROUP_4D) {   // (also writes the 4D segments' splat depths, from the moved positions)
-                launch_project_4d_scene(scene->tab, scene->times, c->slot_ids.p, c->ctr, modes ? *modes : ModeConsts{}, c->recs.p,
+                launch_project_4d_scene(scene->tab, scene->times, scene->classes, *modes, c->slot_ids.p, c->ctr, c->recs.p,
                                         zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
             } else {
-                launch_project_scene(scene->tab, g, c->slot_ids.p, c->ctr, c->recs.p, p.raster_mode == 2 ? c->extra.p : nullptr,
-                                     p.n_hint, c->sm_count, c->cutoff_tab, modes, ps);
+                launch_project_scene(scene->tab, g, scene->need_sh[i] != 0, scene->classes, *modes, c->slot_ids.p, c->ctr,
+                                     c->recs.p, (p.raster_mode == 2 || p.raster_mode == 4) ? c->extra.p : nullptr, p.n_hint,
+                                     c->sm_count, c->cutoff_tab, ps);
                 scene_3d = true;
             }
             ++launches;
@@ -555,15 +545,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaEventRecord(c->ev_p1, ps));
     // depth-tested frames: the splat depths, indexed like the records (the projection's index list)
     ZTestArgs zt;
-    if (zd && scene_3d && scene->entities) {
-        // (the splat-depth launch covers the 3D groups 0 .. 7: an entity frame's Classification / OpticalFlow /
-        // Velocity segments, groups 16 .. 23, are read as the plain group of their layout)
-        SceneTable dt = scene->tab;
-        for (uint32_t j = 0; j < dt.k; ++j)
-            if (dt.seg[j].group != PROJECT_GROUP_4D) dt.seg[j].group &= ~ENTITY_MODES;
-        launch_splat_depth_scene(dt, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
-        ++launches;
-    } else if (zd && scene_3d) {
+    if (zd && scene_3d) {
         launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
     } else if (zd && !tc && !scene) {
@@ -678,11 +660,11 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         TRY(bgs_sync(c));
     }
     const FrameConsts fc = scene ? scene->tab.seg[0].fc : frame_consts(cloud, view, uni, st, want_aux);
-    // Classification / OpticalFlow: project_modes_kernel with the extras (NULL extras: num_classes = 1)
+    // Classification / OpticalFlow, and every scene frame: the projection takes the extras (NULL extras: num_classes = 1)
     ModeConsts mc = {};
     mc.num_classes = ex ? ex->num_classes : 1u;
     if (ex) { memcpy(mc.prev_clip_from_world, ex->previous_clip_from_world, 64); mc.delta_time = ex->delta_time; }
-    const ModeConsts* modes = st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION || (scene && scene->entities) ? &mc : nullptr;
+    const ModeConsts* modes = st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION || scene ? &mc : nullptr;
     const uint32_t n = scene ? scene->tab.n_total : cloud->n, num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
@@ -691,7 +673,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
                   out_depth, out_normal, &o));
     for (int attempt = 0; attempt < 4; ++attempt) {
         FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
-        if (scene && scene->entities) {   // (st plans it as an aabb frame or an overlay one: one round)
+        if (scene) {   // (st plans it as an aabb frame or an overlay one: one round)
             p.raster_mode = scene->raster_mode;
             p.box = scene->box;
         }
@@ -754,100 +736,27 @@ bgs_status bgs_render_4d(bgs_context* c, const bgs_cloud* cloud, const bgs_view*
     return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth, &tc);
 }
 
-// bgs_render_scene, and bgs_render_scene_4d (with_4d: Gaussian4d clouds are projected at uniforms[j].time in windows[j];
-// with none listed the two calls are one and windows is not read)
-static bgs_status render_scene_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
-                                    const bgs_cloud_uniform* unis, const bgs_time_window* windows, uint32_t k,
-                                    const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex,
-                                    const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
-    if (!c) return BGS_EINVAL;
-    if (!clouds || !unis || !view || !st) return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/view/settings not ready", call);
+// the refusals every scene call makes of its list before reading it: k, SORT_ALL and NULL clouds
+static bgs_status check_scene_list(bgs_context* c, const char* call, const bgs_cloud* const* clouds, uint32_t k,
+                                   const bgs_settings* frame) {
     if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "%s: k = %u is not in 1..%d", call, k, BGS_SCENE_MAX_CLOUDS);
-    if (st->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
-    bool any_4d = false;
-    for (uint32_t j = 0; j < k; ++j) {
+    if (frame->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
+    for (uint32_t j = 0; j < k; ++j)
         if (!clouds[j]) return fail(c, BGS_EINVAL, "%s: clouds[%u] is NULL", call, j);
-        any_4d = any_4d || (with_4d && is_4d(clouds[j]->layout));
-    }
-    // a scene with 4D clouds: those are checked as bgs_render_4d frames (gaussian_mode read as Gaussian4d), the others
-    // against the frame's settings, a Velocity frame's as a Color one (they are drawn as nothing, include/bgs.h)
-    bgs_settings s4 = *st, s3 = *st;
-    if (any_4d) {
-        if (!windows) return fail(c, BGS_EINVAL, "%s: windows is NULL with a Gaussian4d cloud listed", call);
-        if (st->gaussian_mode == BGS_GAUSSIAN_2D && st->aabb)
-            return fail(c, BGS_EINVAL, "%s: BGS_GAUSSIAN_2D with aabb = 1 takes no Gaussian4d cloud (its blend reads a surfel record for every splat)", call);
-        s4.gaussian_mode = BGS_GAUSSIAN_4D;
-        if (s3.rasterize_mode == BGS_RASTERIZE_VELOCITY) s3.rasterize_mode = BGS_RASTERIZE_COLOR;
-    }
-    auto scene = std::make_shared<SceneFacts>();
-    uint64_t total = 0;
-    for (uint32_t j = 0; j < k; ++j) {
-        const bool is4 = any_4d && is_4d(clouds[j]->layout);
-        if (any_4d && !is4 && st->gaussian_mode == BGS_GAUSSIAN_4D)
-            return fail(c, BGS_EINVAL, "%s: gaussian_mode BGS_GAUSSIAN_4D with clouds[%u], which is not a Gaussian4d cloud", call, j);
-        // (without 4D clouds: bgs_render_depth_test's check, which refuses 4D clouds and other devices)
-        TRY(check_render(c, clouds[j], view, &unis[j], is4 ? &s4 : &s3, ex, out_format, false, is4));
-        if (is4) TRY(temporal_consts(c, call, unis[j].time, windows[j].time_start, windows[j].time_stop, scene->times.t[j]));
-        total += clouds[j]->n;
-    }
-    if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "%s: N = %llu gaussians, must be < 2^30", call, (unsigned long long)total);
-    if (depth) TRY(check_scene_depth(c, depth, view));
-    SceneTable& tab = scene->tab;
-    memset(&tab, 0, sizeof(tab));
-    tab.k = k;
-    tab.n_total = (uint32_t)total;
-    uint32_t offset = 0;
-    for (uint32_t j = 0; j < k; ++j) {
-        const bgs_cloud* cl = clouds[j];
-        SceneSeg& sg = tab.seg[j];
-        sg.fc = frame_consts(cl, view, &unis[j], any_4d && is_4d(cl->layout) ? &s4 : st, false);
-        sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
-        sg.pos = cl->pos;
-        sg.blocks = cl->blocks;
-        sg.offset = offset;
-        sg.n = cl->n;
-        sg.group = project_group(cl->layout, cl->sh_degree);
-        offset += cl->n;
-        scene->clouds.push_back(cl);
-        if (std::find(scene->groups.begin(), scene->groups.end(), sg.group) == scene->groups.end()) scene->groups.push_back(sg.group);
-    }
-    return render_impl(c, clouds[0], view, &unis[0], st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth,
-                       nullptr, scene);
-}
-
-bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis, uint32_t k,
-                            const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
-                            void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
-    return render_scene_impl(c, "render_scene", false, clouds, unis, nullptr, k, view, st, ex, depth, out_rgba, out_format,
-                             out_is_device_ptr);
-}
-
-bgs_status bgs_render_scene_4d(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
-                               const bgs_time_window* windows, uint32_t k, const bgs_view* view, const bgs_settings* st,
-                               const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
-                               int out_is_device_ptr) {
-    return render_scene_impl(c, "render_scene_4d", true, clouds, unis, windows, k, view, st, ex, depth, out_rgba, out_format,
-                             out_is_device_ptr);
+    return BGS_OK;
 }
 
 // the blend kind of an entity's records (raster.cu): 0 = quad-uv, 1 = conic (3DGS and 4D with aabb), 2 = surfel
 static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.gaussian_mode == BGS_GAUSSIAN_2D ? 2 : 1); }
 
-bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
-                                  const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
-                                  const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
-                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
-    const char* call = "render_entities";
-    if (!c) return BGS_EINVAL;
-    if (!clouds || !unis || !ents || !view || !frame)
-        return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/entities/view/settings not ready", call);
-    if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "%s: k = %u is not in 1..%d", call, k, BGS_SCENE_MAX_CLOUDS);
-    if (frame->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
-    for (uint32_t j = 0; j < k; ++j) {
-        if (!clouds[j]) return fail(c, BGS_EINVAL, "%s: clouds[%u] is NULL", call, j);
-        if (entity_flags && (entity_flags[j] & ~(uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX))
-            return fail(c, BGS_EINVAL, "%s: entity_flags[%u] = 0x%x has an unknown bit", call, j, entity_flags[j]);
-    }
+// Every scene frame: k entities, each checked as its single-cloud call (bgs_render_depth_test, or bgs_render_4d for a
+// Gaussian4d cloud when with_4d) with its own settings, num_classes and window, drawn into one depth-sorted frame.
+// entity_flags: each entity's BGS_ENTITY_* bits (NULL: none).  The list has passed check_scene_list.
+static bgs_status render_entities_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
+                                       const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
+                                       const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
+                                       const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                                       void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
         return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
@@ -855,50 +764,36 @@ bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds
     };
     // entity j as its single-cloud call: its settings with the frame's sort bits and flags, its num_classes and window
     std::vector<bgs_settings> st(k);
-    std::vector<bgs_render_extras> exs(k);
-    std::vector<bgs_time_window> windows(k);
-    SceneTimes times = {};
-    bool agree = true, any_3d = false, any_depth = false;
-    uint32_t gm3 = 0, kinds = 0;
+    auto scene = std::make_shared<SceneFacts>();
+    bool any_depth = false, undrawn = true;
+    uint32_t kinds = 0;
     uint64_t total = 0;
     for (uint32_t j = 0; j < k; ++j) {
         const bgs_entity_settings& e = ents[j];
-        const bool is4 = is_4d(clouds[j]->layout);
+        const bool is4 = with_4d && is_4d(clouds[j]->layout);
         bgs_settings& s = st[j];
         s = *frame;
         s.gaussian_mode = e.gaussian_mode; s.rasterize_mode = e.rasterize_mode; s.aabb = e.aabb;
         s.opacity_adaptive_radius = e.opacity_adaptive_radius; s.draw_mode = e.draw_mode;
-        exs[j] = ex ? *ex : bgs_render_extras{};
-        exs[j].num_classes = e.num_classes;
-        windows[j] = e.window;
-        bgs_settings chk = s;   // (a non-4D entity in Velocity is undrawn, and checked as a Color one, as in scenes)
+        bgs_render_extras ej = ex ? *ex : bgs_render_extras{};
+        ej.num_classes = e.num_classes;
+        bgs_settings chk = s;   // (a non-4D entity in Velocity is undrawn, and checked as a Color one)
         if (!is4 && chk.rasterize_mode == BGS_RASTERIZE_VELOCITY) chk.rasterize_mode = BGS_RASTERIZE_COLOR;
-        TRY(check_render(c, clouds[j], view, &unis[j], &chk, ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &exs[j] : nullptr,
+        TRY(check_render(c, clouds[j], view, &unis[j], &chk, ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr,
                          out_format, false, is4));
-        if (is4) TRY(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, times.t[j]));
+        if (is4) TRY(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, scene->times.t[j]));
         const bgs_entity_settings& e0 = ents[0];
-        agree = agree && e.rasterize_mode == e0.rasterize_mode && e.aabb == e0.aabb &&
-                e.opacity_adaptive_radius == e0.opacity_adaptive_radius && e.draw_mode == e0.draw_mode &&
-                (e.rasterize_mode != BGS_RASTERIZE_CLASSIFICATION || e.num_classes == e0.num_classes) &&
-                blend_kind(e) == blend_kind(e0) && box_of(j) == box_of(0) && (is4 || !any_3d || e.gaussian_mode == gm3);
-        if (!is4) { any_3d = true; gm3 = e.gaussian_mode; }
+        undrawn = undrawn && !is4 && e.rasterize_mode == BGS_RASTERIZE_VELOCITY && e.gaussian_mode == e0.gaussian_mode &&
+                  e.aabb == e0.aabb && e.opacity_adaptive_radius == e0.opacity_adaptive_radius && e.draw_mode == e0.draw_mode &&
+                  box_of(j) == box_of(0);
         any_depth = any_depth || e.rasterize_mode == BGS_RASTERIZE_DEPTH;
         kinds |= 1u << blend_kind(e);
         total += clouds[j]->n;
     }
-    if (agree) {   // one frame's settings: exactly bgs_render_scene_4d
-        bgs_settings s = st[0];
-        s.gaussian_mode = any_3d ? gm3 : (uint32_t)BGS_GAUSSIAN_4D;
-        if (box_of(0)) s.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
-        const bool need_ex = ex || ents[0].rasterize_mode == BGS_RASTERIZE_CLASSIFICATION;
-        return render_scene_impl(c, call, true, clouds, unis, windows.data(), k, view, &s, need_ex ? &exs[0] : nullptr, depth,
-                                 out_rgba, out_format, out_is_device_ptr);
-    }
+    // (one Velocity frame without a Gaussian4d cloud: nothing has a colour source, as in bgs_render_depth_test)
+    if (undrawn) return fail(c, BGS_EINVAL, "%s: a Velocity frame with no Gaussian4d cloud listed", call);
     if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "%s: N = %llu gaussians, must be < 2^30", call, (unsigned long long)total);
     if (depth) TRY(check_scene_depth(c, depth, view));
-    auto scene = std::make_shared<SceneFacts>();
-    scene->entities = true;
-    scene->times = times;
     SceneTable& tab = scene->tab;
     memset(&tab, 0, sizeof(tab));
     tab.k = k;
@@ -944,6 +839,74 @@ bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds
     if (scene->box) sf.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
     return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr,
                        depth, nullptr, scene);
+}
+
+// bgs_render_scene, and bgs_render_scene_4d (with_4d: Gaussian4d clouds are projected at uniforms[j].time in windows[j];
+// with none listed the two calls are one and windows is not read): the scene's own refusals, then every cloud an entity
+// with the frame's settings
+static bgs_status render_scene_as_entities(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
+                                           const bgs_cloud_uniform* unis, const bgs_time_window* windows, uint32_t k,
+                                           const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex,
+                                           const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
+                                           int out_is_device_ptr) {
+    if (!c) return BGS_EINVAL;
+    if (!clouds || !unis || !view || !st) return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/view/settings not ready", call);
+    TRY(check_scene_list(c, call, clouds, k, st));
+    bool any_4d = false;
+    for (uint32_t j = 0; j < k; ++j) any_4d = any_4d || (with_4d && is_4d(clouds[j]->layout));
+    if (any_4d) {
+        if (!windows) return fail(c, BGS_EINVAL, "%s: windows is NULL with a Gaussian4d cloud listed", call);
+        if (st->gaussian_mode == BGS_GAUSSIAN_2D && st->aabb)
+            return fail(c, BGS_EINVAL, "%s: BGS_GAUSSIAN_2D with aabb = 1 takes no Gaussian4d cloud (its blend reads a surfel record for every splat)", call);
+    }
+    // a scene with 4D clouds: those are drawn as bgs_render_4d frames (gaussian_mode read as Gaussian4d), the others with
+    // the frame's settings (a Velocity frame's are drawn as nothing, include/bgs.h)
+    std::vector<bgs_entity_settings> ents(k);
+    for (uint32_t j = 0; j < k; ++j) {
+        const bool is4 = any_4d && is_4d(clouds[j]->layout);
+        if (any_4d && !is4 && st->gaussian_mode == BGS_GAUSSIAN_4D)
+            return fail(c, BGS_EINVAL, "%s: gaussian_mode BGS_GAUSSIAN_4D with clouds[%u], which is not a Gaussian4d cloud", call, j);
+        bgs_entity_settings& e = ents[j];
+        e.gaussian_mode = is4 ? (uint32_t)BGS_GAUSSIAN_4D : st->gaussian_mode;
+        e.rasterize_mode = st->rasterize_mode; e.aabb = st->aabb;
+        e.opacity_adaptive_radius = st->opacity_adaptive_radius; e.draw_mode = st->draw_mode;
+        e.num_classes = ex ? ex->num_classes : 1u;
+        e.window = is4 ? windows[j] : bgs_time_window{};
+    }
+    return render_entities_impl(c, call, with_4d, clouds, unis, ents.data(), nullptr, k, view, st, ex, depth, out_rgba,
+                                out_format, out_is_device_ptr);
+}
+
+bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis, uint32_t k,
+                            const bgs_view* view, const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                            void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    return render_scene_as_entities(c, "render_scene", false, clouds, unis, nullptr, k, view, st, ex, depth, out_rgba, out_format,
+                                    out_is_device_ptr);
+}
+
+bgs_status bgs_render_scene_4d(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                               const bgs_time_window* windows, uint32_t k, const bgs_view* view, const bgs_settings* st,
+                               const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
+                               int out_is_device_ptr) {
+    return render_scene_as_entities(c, "render_scene_4d", true, clouds, unis, windows, k, view, st, ex, depth, out_rgba,
+                                    out_format, out_is_device_ptr);
+}
+
+bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                  const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
+                                  const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    const char* call = "render_entities";
+    if (!c) return BGS_EINVAL;
+    if (!clouds || !unis || !ents || !view || !frame)
+        return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/entities/view/settings not ready", call);
+    TRY(check_scene_list(c, call, clouds, k, frame));
+    if (entity_flags)
+        for (uint32_t j = 0; j < k; ++j)
+            if (entity_flags[j] & ~(uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX)
+                return fail(c, BGS_EINVAL, "%s: entity_flags[%u] = 0x%x has an unknown bit", call, j, entity_flags[j]);
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
+                                out_is_device_ptr);
 }
 
 bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,

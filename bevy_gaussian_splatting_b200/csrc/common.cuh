@@ -33,8 +33,9 @@ struct FrameConsts {
     uint32_t aux;               // bgs_render_aux: the projection also emits the Depth and Normal colour sources
 };
 
-// bgs_render_scene's segment table.  Segment j holds cloud j's gaussians at global indices [offset, offset + n); its
-// FrameConsts carry the frame-wide values and cloud j's uniform and layout (n_cloud is the scene's N).  The scene
+// A scene frame's segment table (bgs_render_scene, _scene_4d, _entities).  Segment j holds cloud j's gaussians at global
+// indices [offset, offset + n); its FrameConsts carry the frame-wide values and entity j's settings, uniform and layout
+// (n_cloud is the scene's N).  The scene
 // kernels take it by value: 64 segments are ~22 KB of kernel parameters (CUDA >= 12.1 allows 32 KB on sm_90), so a
 // queued frame's table lives in its own launches and no later frame can overwrite it.
 struct SceneSeg {
@@ -64,15 +65,15 @@ struct SceneTable {
     }
 };
 
-// The projection group of Gaussian4d segments (bgs_render_scene_4d): project_group gives the 3D layouts 0 .. 7 (f16 bit,
-// SH degree << 1), so 4D segments never fall into a 3D launch, and splat_depth_scene leaves their depths to the 4D
-// projection, which takes them from the moved positions.
+// The projection group of Gaussian4d segments: project_group gives the 3D layouts 0 .. 7 (f16 bit, SH degree << 1), so
+// 4D segments never fall into a 3D launch, and splat_depth_scene leaves their depths to the 4D projection, which takes
+// them from the moved positions.
 constexpr uint32_t PROJECT_GROUP_4D = 8u;
-// bgs_render_entities: a 3D group's bit for the Classification / OpticalFlow / Velocity colour kernel (groups 16 .. 23)
+// a 3D group's bit for the Classification / OpticalFlow / Velocity colour kernel (groups 16 .. 23)
 constexpr uint32_t ENTITY_MODES = 16u;
 
-// bgs_render_extras as the Classification / OpticalFlow projection reads it.  Only project_modes_kernel takes it (as an
-// argument of its own), so the arguments and code of every other kernel stay what they were.
+// bgs_render_extras as the Classification / OpticalFlow projection reads it: an argument of project_modes_kernel, the
+// Gaussian4d kernels and the scene kernels, so project_kernel's arguments and code stay what they were.
 struct ModeConsts {
     float prev_clip_from_world[16];   // the view's clip_from_world of the previous frame (column-major)
     float delta_time;                 // > 0, finite
@@ -86,14 +87,14 @@ struct TemporalConsts {
     float duration;      // time_stop - time_start (finite, non-zero): the time terms' theta = dt / duration
 };
 
-// bgs_render_scene_4d's per-segment times (t[j] is segment j's; only 4D segments read theirs).  An argument of
-// project_4d_scene_kernel alone (768 B beside the ~22 KB segment table), so the other scene kernels keep theirs.
+// A scene's per-segment times (t[j] is segment j's; only 4D segments read theirs).  An argument of project_4d_scene_kernel
+// alone (768 B beside the ~22 KB segment table).
 struct SceneTimes {
     TemporalConsts t[BGS_SCENE_MAX_CLOUDS];
 };
 
-// bgs_render_entities' per-segment num_classes (n[j] is segment j's).  An argument of the entity projection kernels alone,
-// as SceneTimes is, so FrameConsts -- and the parameters of every single-cloud kernel -- stay as they are.
+// A scene's per-segment num_classes (n[j] is segment j's).  An argument of the scene projection kernels, as SceneTimes
+// is, so FrameConsts -- and the parameters of every single-cloud kernel -- stay as they are.
 struct SceneClasses {
     uint32_t n[BGS_SCENE_MAX_CLOUDS];
 };

@@ -62,20 +62,17 @@ struct bgs_particles {
     cudaEvent_t ev_write = nullptr;   // the last step of these behaviours (recorded on the stepping context's stream)
 };
 
-// A bgs_render_scene frame: its segment table (what its kernels and the culled-flags hook read), the clouds it lists
-// (clouds[j] is segment j's; a cloud may be listed more than once) and its distinct projection groups.  A
-// bgs_render_scene_4d frame also carries its 4D segments' times (PROJECT_GROUP_4D among the groups).
+// A scene frame (bgs_render_scene, _scene_4d, _entities): its segment table (what its kernels and the culled-flags hook
+// read), its 4D segments' times, the clouds it lists (clouds[j] is segment j's; a cloud may be listed more than once),
+// its distinct projection groups (project_group, plus ENTITY_MODES for the Classification / OpticalFlow / Velocity colour
+// kernel, or PROJECT_GROUP_4D) with whether one of each group's segments reads the SH coefficients, the segments'
+// num_classes, the blend (raster.cu's mode: 0..2 when every splat has one kind, else 3 / 4 with `kinds`), and whether
+// some entity draws its bounding boxes (kinds' BOX_KIND bits say which, on mixed frames; on the others every entity does)
 struct SceneFacts {
     SceneTable tab;
     SceneTimes times = {};
     std::vector<const bgs_cloud*> clouds;
     std::vector<uint32_t> groups;
-    // bgs_render_entities frames whose entities disagree: each group's launch (project_group, plus ENTITY_MODES for the
-    // Classification / OpticalFlow / Velocity colour kernel) with whether one of its segments reads the SH coefficients,
-    // the segments' num_classes, and the blend (raster.cu's mode: 0..2 when every splat has one kind, else 3 / 4 with
-    // `kinds`), and whether some entity draws its bounding boxes (kinds' BOX_KIND bits say which, on mixed frames; on the
-    // others every entity does)
-    bool entities = false;
     std::vector<uint32_t> need_sh;   // per entry of groups
     SceneClasses classes = {};
     int raster_mode = 0;

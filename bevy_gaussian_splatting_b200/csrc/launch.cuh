@@ -35,11 +35,8 @@ void launch_project(CloudLayout layout, uint32_t sh_degree, const void* blocks, 
                     const float* cutoff_tab, float4* aux, const ModeConsts* modes /* null: project_kernel */,
                     cudaStream_t stream);
 void launch_cutoff_table(float* tab, cudaStream_t stream);
-// bgs_render_scene: the projection of the segments whose project_group is `group` (one launch), and the depth range
+// scene frames (bgs_render_scene, _scene_4d, _entities): the projection group of a cloud's segments, and the depth range
 uint32_t project_group(CloudLayout layout, uint32_t sh_degree);
-void launch_project_scene(const SceneTable& tab, uint32_t group, const uint32_t* slot_ids, const FrameCounters* ctr,
-                          SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
-                          const ModeConsts* modes /* null: project_scene_kernel */, cudaStream_t stream);
 void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payload, const uint32_t* slot_ids, FrameCounters* ctr,
                               cudaStream_t stream);
 // Gaussian4d clouds (bgs_render_4d): records as launch_project's, and the splat depths of depth-tested frames (depths
@@ -47,20 +44,16 @@ void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payl
 void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                        const FrameConsts& fc, const ModeConsts& mc, const TemporalConsts& tc, SplatRec* recs, float* depths,
                        uint32_t n_hint, int sm_count, cudaStream_t stream);
-// bgs_render_scene_4d: the projection of every segment in PROJECT_GROUP_4D (one launch), each at its own times, and their
-// splat depths from the moved positions (depths non-null)
-void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const uint32_t* slot_ids, const FrameCounters* ctr,
-                             const ModeConsts& mc, SplatRec* recs, float* depths, uint32_t n_hint, int sm_count,
-                             cudaStream_t stream);
-// bgs_render_entities frames whose entities disagree: the projection of the segments of one group (project_group, |
-// ENTITY_MODES for the Classification / OpticalFlow / Velocity kernel), each with its own settings and num_classes;
-// need_sh: some segment of the group reads the SH coefficients.  And the 4D segments' (PROJECT_GROUP_4D).
-void launch_project_entities(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
+// scene frames: the projection of the segments of one group (project_group, | ENTITY_MODES for the Classification /
+// OpticalFlow / Velocity kernel; one launch), each with its own settings and num_classes; need_sh: some segment of the
+// group reads the SH coefficients.  And the Gaussian4d segments' (PROJECT_GROUP_4D), each at its own times, with their
+// splat depths from the moved positions (depths non-null).
+void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
+                          const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
+                          float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream);
+void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
                              const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
-                             float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream);
-void launch_project_4d_entities(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
-                                const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
-                                float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
+                             float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
 // bin.cu
 int bin_coop_blocks_per_sm();
 cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,

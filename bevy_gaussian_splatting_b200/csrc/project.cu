@@ -759,35 +759,7 @@ project_modes_kernel(const void* __restrict__ blocks, const uint32_t* __restrict
                  ctr, mc);
 }
 
-// ---- bgs_render_scene: the projection over a segment table (common.cuh).  Record r is compact slot r, whose global
-// index slot_ids[r] lies in segment j: its block is gaussian slot_ids[r] - offset of cloud j's blocks, and project_one
-// runs with segment j's FrameConsts, so the record is the one a frame of cloud j alone would write.  One launch per
-// kernel instantiation (`group`): its warps stride over every slot and project those whose cloud is in the group.
-
-// (the f32 blocks of degree 2 and 3 hold 48 SH floats in registers beside the segment's constants: 3 CTAs per SM keeps
-// them from spilling)
-template <bool F16, uint32_t D>
-constexpr int scene_min_ctas() { return !F16 && D >= 2 ? 3 : PROJ_MIN_CTAS; }
-
-template <bool F16, uint32_t D>
-__global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
-project_scene_kernel(SceneTable tab, uint32_t group, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
-                     SplatRec* __restrict__ recs, float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
-    project_loop(SceneSrc{tab, 1u << group, slot_ids},
-                 Geo3d<F16, D, false>{ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_COLOR, recs, extra, cutoff_tab, nullptr},
-                 ctr, ModeConsts{});
-}
-template <bool F16, uint32_t D>
-__global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
-project_modes_scene_kernel(SceneTable tab, uint32_t group, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
-                           const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs, float4* __restrict__ extra,
-                           const float* __restrict__ cutoff_tab) {
-    project_loop(SceneSrc{tab, 1u << group, slot_ids},
-                 Geo3d<F16, D, true>{ctr, tab.seg[0].fc.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION, recs, extra, cutoff_tab,
-                                     nullptr},
-                 ctr, mc);
-}
-
+// ---- scene frames (the segment table, common.cuh): the depth range, and the projection group of a cloud's segments
 void launch_depth_range_scene(const SceneTable& tab, const uint32_t* sorted_payload, const uint32_t* slot_ids, FrameCounters* ctr,
                               cudaStream_t stream) {
     depth_range_scene_kernel<<<1, 32, 0, stream>>>(tab, sorted_payload, slot_ids, ctr);
@@ -798,23 +770,6 @@ uint32_t project_group(CloudLayout layout, uint32_t sh_degree) {
     return (is_f16(layout) ? 1u : 0u) | sh_degree << 1;
 }
 
-void launch_project_scene(const SceneTable& tab, uint32_t group, const uint32_t* slot_ids, const FrameCounters* ctr,
-                          SplatRec* recs, float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
-                          const ModeConsts* modes, cudaStream_t stream) {
-    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
-    with_layout_degree(group & 1u ? CloudLayout::F16 : CloudLayout::F32, group >> 1, [&](auto L, auto Dt) {
-        constexpr CloudLayout Lv = decltype(L)::value;
-        constexpr uint32_t D = decltype(Dt)::value;
-        if constexpr (!is_4d(Lv)) {
-            if (modes)
-                project_modes_scene_kernel<is_f16(Lv), D><<<grid, PROJ_THREADS, 0, stream>>>(tab, group, *modes, slot_ids, ctr, recs,
-                                                                                            extra, cutoff_tab);
-            else
-                project_scene_kernel<is_f16(Lv), D><<<grid, PROJ_THREADS, 0, stream>>>(tab, group, slot_ids, ctr, recs, extra,
-                                                                                      cutoff_tab);
-        }
-    });
-}
 // ---- Gaussian4d (bgs_render_4d; the rule is include/bgs.h's).  Matrices [col][row], as WGSL indexes them.
 
 // gaussian_4d.wgsl:37-130: Sigma of the 4D gaussian conditioned on time t
@@ -1015,32 +970,22 @@ void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_sl
                                                          recs, depths);
 }
 
-// ---- bgs_render_scene_4d: project_4d_kernel over a segment table.  Record r is compact slot r; its global index lies in
-// segment j, and only the segments of PROJECT_GROUP_4D are this launch's (the 3D ones are launch_project_scene's).  Each
-// lane stages its own entry's first 128 B line from its own cloud's blocks, then project_one_4d runs with segment j's
-// FrameConsts and times, so the record and splat depth are those bgs_render_4d writes for that cloud.
-__global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
-project_4d_scene_kernel(SceneTable tab, SceneTimes times, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
-                        const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs,
-                        float* __restrict__ depths /* depth-tested frames only */) {
-    project_loop(SceneSrc{tab, 1u << PROJECT_GROUP_4D, slot_ids, &times}, Geo4d{ctr, recs, depths}, ctr, mc);
-}
-// sm_90 takes up to 32764 B of kernel parameters (CUDA >= 12.1): the table (~22 KB), the times (768 B), the extras and
-// four pointers
-static_assert(sizeof(SceneTable) + sizeof(SceneTimes) + sizeof(ModeConsts) + 4 * sizeof(void*) + 16 <= 32764,
-              "project_4d_scene_kernel's parameters exceed the sm_90 limit");
+// ---- Scene frames (bgs_render_scene, _scene_4d and _entities): the projection over a segment table (common.cuh).
+// Record r is compact slot r, whose global index slot_ids[r] lies in segment j: its block is gaussian slot_ids[r] -
+// offset of cloud j's blocks, and project_one / project_one_4d run with segment j's FrameConsts (its entity's settings),
+// times and num_classes, so the record is the one a frame of cloud j alone would write.  One launch per group
+// (project_group, | ENTITY_MODES for the Classification / OpticalFlow / Velocity kernel, or PROJECT_GROUP_4D): its warps
+// stride over every slot and project those whose segment is in the group; need_sh says whether one of the group's
+// segments reads the SH coefficients.
 
-void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const uint32_t* slot_ids, const FrameCounters* ctr,
-                             const ModeConsts& mc, SplatRec* recs, float* depths, uint32_t n_hint, int sm_count,
-                             cudaStream_t stream) {
-    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
-    project_4d_scene_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, times, mc, slot_ids, ctr, recs, depths);
-}
-// ---- bgs_render_entities frames whose entities disagree.  The scene kernels above take the colour kernel's SH need and
-// num_classes from the frame; here each segment's FrameConsts carries its own entity's settings, the launch is told
-// whether any of its segments reads the SH coefficients, and project_one sees its segment's num_classes.
+// (the f32 blocks of degree 2 and 3 hold 48 SH floats in registers beside the segment's constants: 3 CTAs per SM keeps
+// them from spilling)
+template <bool F16, uint32_t D>
+constexpr int scene_min_ctas() { return !F16 && D >= 2 ? 3 : PROJ_MIN_CTAS; }
+
+// G's projection with segment j's num_classes
 template <class G>
-struct EntityGeo : G {
+struct SceneGeo : G {
     const SceneClasses& classes;
     template <class Src>
     __device__ __forceinline__ void project(const Src& src, uint32_t j, uint32_t e, uint32_t r, float4 p4, const float q[4],
@@ -1053,44 +998,46 @@ struct EntityGeo : G {
 
 template <bool F16, uint32_t D, bool MODES2>
 __global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
-project_entities_kernel(SceneTable tab, uint32_t group, uint32_t need_sh, SceneClasses classes, ModeConsts mc,
-                        const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs,
-                        float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
+project_scene_kernel(SceneTable tab, uint32_t group, uint32_t need_sh, SceneClasses classes, ModeConsts mc,
+                     const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs,
+                     float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
     project_loop(SceneSrc{tab, 1u << group, slot_ids},
-                 EntityGeo<Geo3d<F16, D, MODES2>>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, nullptr}, classes}, ctr, mc);
+                 SceneGeo<Geo3d<F16, D, MODES2>>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, nullptr}, classes}, ctr, mc);
 }
 
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
-project_4d_entities_kernel(SceneTable tab, SceneTimes times, SceneClasses classes, ModeConsts mc,
-                           const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
-                           SplatRec* __restrict__ recs, float* __restrict__ depths /* depth-tested frames only */) {
-    project_loop(SceneSrc{tab, 1u << PROJECT_GROUP_4D, slot_ids, &times}, EntityGeo<Geo4d>{{ctr, recs, depths}, classes}, ctr, mc);
+project_4d_scene_kernel(SceneTable tab, SceneTimes times, SceneClasses classes, ModeConsts mc,
+                        const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                        SplatRec* __restrict__ recs, float* __restrict__ depths /* depth-tested frames only */) {
+    project_loop(SceneSrc{tab, 1u << PROJECT_GROUP_4D, slot_ids, &times}, SceneGeo<Geo4d>{{ctr, recs, depths}, classes}, ctr, mc);
 }
+// sm_90 takes up to 32764 B of kernel parameters (CUDA >= 12.1): the table (~22 KB), the times (768 B), the classes
+// (256 B), the extras and four pointers
 static_assert(sizeof(SceneTable) + sizeof(SceneTimes) + sizeof(SceneClasses) + sizeof(ModeConsts) + 4 * sizeof(void*) + 16 <= 32764,
-              "project_4d_entities_kernel's parameters exceed the sm_90 limit");
+              "project_4d_scene_kernel's parameters exceed the sm_90 limit");
 
-void launch_project_entities(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
-                             const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
-                             float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream) {
+void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
+                          const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
+                          float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream) {
     const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     const uint32_t g = group & ~ENTITY_MODES;
     with_layout_degree(g & 1u ? CloudLayout::F16 : CloudLayout::F32, g >> 1, [&](auto L, auto Dt) {
         constexpr CloudLayout Lv = decltype(L)::value;
         constexpr uint32_t D = decltype(Dt)::value;
         if constexpr (!is_4d(Lv)) {
-            auto* kernel = (group & ENTITY_MODES) ? project_entities_kernel<is_f16(Lv), D, true>
-                                                  : project_entities_kernel<is_f16(Lv), D, false>;
+            auto* kernel = (group & ENTITY_MODES) ? project_scene_kernel<is_f16(Lv), D, true>
+                                                  : project_scene_kernel<is_f16(Lv), D, false>;
             kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, group, need_sh ? 1u : 0u, classes, mc, slot_ids, ctr, recs, extra,
                                                       cutoff_tab);
         }
     });
 }
 
-void launch_project_4d_entities(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
-                                const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
-                                float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream) {
+void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
+                             const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
+                             float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream) {
     const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
-    project_4d_entities_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, times, classes, mc, slot_ids, ctr, recs, depths);
+    project_4d_scene_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, times, classes, mc, slot_ids, ctr, recs, depths);
 }
 
 void launch_depth_range(const float4* pos, uint32_t n, const uint32_t* sorted_payload, const uint32_t* slot_ids,

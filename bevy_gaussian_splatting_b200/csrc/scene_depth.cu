@@ -33,12 +33,13 @@ splat_depth_kernel(const float4* __restrict__ pos, const uint32_t* __restrict__ 
     splat_depth_body(OneCloud{pos, fc, nullptr, index_list, by_slot}, ctr, depths);
 }
 
-// bgs_render_scene: record r is compact slot r.  Gaussian4d segments (bgs_render_scene_4d) are not this launch's: their
-// projection writes their depths from the moved positions.
+// Scene frames: record r is compact slot r.  Every 3D group is this launch's, with either colour kernel (groups 0 .. 7
+// and 16 .. 23, ENTITY_MODES); Gaussian4d segments are not: their projection writes their depths from the moved positions.
 __global__ void __launch_bounds__(SD_THREADS)
 splat_depth_scene_kernel(SceneTable tab, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
                          float* __restrict__ depths) {
-    splat_depth_body(SceneSrc{tab, (1u << PROJECT_GROUP_4D) - 1u, slot_ids}, ctr, depths);
+    constexpr uint32_t groups_3d = ((1u << PROJECT_GROUP_4D) - 1u) * (1u | 1u << ENTITY_MODES);   // 0x00FF00FF
+    splat_depth_body(SceneSrc{tab, groups_3d, slot_ids}, ctr, depths);
 }
 
 void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,

@@ -6,11 +6,12 @@ cloud (6 M seeded gaussians, f16, global_scale 0.02) at 1920x1080, rendered
   (c) the same K subsets as K bgs_render calls, far first, each after the first with BGS_FLAG_BLEND_OVER_TARGET (the
       reference's per-entity order).
 
-    python scripts/scene_probe.py [--frames N] [--out FILE]
+    python scripts/scene_probe.py [--frames N] [--mode Color|...|Classification] [--ks 2,8,64] [--out FILE]
 
 Each frame is synchronous into a device target; p50 and p90 of N frames after 5 of warm-up (host clock around a call
-that ends in a device synchronise), and the frame's launch count.  Also checks that (b)'s frame is byte-identical to
-(a)'s.  Prints one JSON line with the card's name and power limit beside the numbers.
+that ends in a device synchronise), the p50 of the projection stage (bgs_stage_times_us()[2], device events) and the
+frame's launch count.  --mode draws every frame in that RasterizeMode (default Color).  Also checks that (b)'s frame is
+byte-identical to (a)'s.  Prints one JSON line with the card's name and power limit beside the numbers.
 """
 from __future__ import annotations
 
@@ -39,30 +40,38 @@ def card():
     return q.stdout.strip()
 
 
-def timed(fn, frames):
+def timed(fn, frames, plugin=None):
+    """p50 / p90 of `frames` calls of fn; with `plugin`, also the p50 of its last frame's projection stage."""
     for _ in range(5):
         fn()
     torch.cuda.synchronize()
-    ts = []
+    ts, proj = [], []
     for _ in range(frames):
         t0 = time.perf_counter()
         fn()
         torch.cuda.synchronize()
         ts.append((time.perf_counter() - t0) * 1e3)
-    return {"p50_ms": round(float(np.percentile(ts, 50)), 4), "p90_ms": round(float(np.percentile(ts, 90)), 4)}
+        if plugin is not None:
+            proj.append(float(plugin.stage_times_us()[2]))
+    r = {"p50_ms": round(float(np.percentile(ts, 50)), 4), "p90_ms": round(float(np.percentile(ts, 90)), 4)}
+    if plugin is not None:
+        r["proj_us_p50"] = round(float(np.percentile(proj, 50)), 2)
+    return r
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=50)
+    ap.add_argument("--mode", default="Color", choices=[m.name for m in B.RasterizeMode if m <= B.RasterizeMode.Classification])
+    ap.add_argument("--ks", default=",".join(map(str, KS)))
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    res = {"card": card(), "n": N, "viewport": [W, H], "layout": "f16", "frames": a.frames}
+    res = {"card": card(), "n": N, "viewport": [W, H], "layout": "f16", "frames": a.frames, "mode": a.mode}
     p = B.GaussianSplattingPlugin(0)
     lib, ctx = p._lib, p._ctx
     view = B.headless_view(W, H)
     v = view.to_abi()
-    st = B.CloudSettings(global_scale=SCALE)
+    st = B.CloudSettings(global_scale=SCALE, rasterize_mode=B.RasterizeMode[a.mode])
     s = st.to_abi()
     s_over = st.to_abi()
     s_over.flags |= abi.BGS_FLAG_BLEND_OVER_TARGET
@@ -79,10 +88,10 @@ def main():
     def whole():
         check(lib.bgs_render(ctx, h._h, C.byref(v), C.byref(u), C.byref(s), out.data_ptr(), code, 1))
 
-    res["a_whole"] = timed(whole, a.frames) | {"launches": p.last_launch_count}
+    res["a_whole"] = timed(whole, a.frames, p) | {"launches": p.last_launch_count}
     ref = out.clone()
     cam = np.asarray(view.to_abi().world_position[:3], np.float32)
-    for k in KS:
+    for k in map(int, a.ks.split(",")):
         cuts = np.linspace(0, N, k + 1).astype(np.int64)
         parts = [p.subset(h, np.arange(cuts[j], cuts[j + 1])) for j in range(k)]
         clouds = (C.c_void_p * k)(*[q._h.value for q in parts])
@@ -97,7 +106,7 @@ def main():
             for i, j in enumerate(far_first):
                 check(lib.bgs_render(ctx, parts[j]._h, C.byref(v), C.byref(u), C.byref(s_over if i else s), out.data_ptr(), code, 1))
 
-        r = {"b_scene": timed(scene, a.frames) | {"launches": p.last_launch_count}}
+        r = {"b_scene": timed(scene, a.frames, p) | {"launches": p.last_launch_count}}
         r["b_identical_to_a"] = bool(torch.equal(out, ref))
         r["c_chain"] = timed(chain, a.frames)
         r["b_over_a"] = round(r["b_scene"]["p50_ms"] / res["a_whole"]["p50_ms"], 4)
