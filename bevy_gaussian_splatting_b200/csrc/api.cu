@@ -528,7 +528,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             } else {
                 launch_project_scene(scene->tab, g, scene->need_sh[i] != 0, scene->classes, *modes, c->slot_ids.p, c->ctr,
                                      c->recs.p, (p.raster_mode == 2 || p.raster_mode == 4) ? c->extra.p : nullptr, p.n_hint,
-                                     c->sm_count, c->cutoff_tab, ps);
+                                     c->sm_count, c->cutoff_tab, fc.aux ? c->aux.p : nullptr, ps);
                 scene_3d = true;
             }
             ++launches;
@@ -751,12 +751,14 @@ static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.ga
 
 // Every scene frame: k entities, each checked as its single-cloud call (bgs_render_depth_test, or bgs_render_4d for a
 // Gaussian4d cloud when with_4d) with its own settings, num_classes and window, drawn into one depth-sorted frame.
-// entity_flags: each entity's BGS_ENTITY_* bits (NULL: none).  The list has passed check_scene_list.
+// entity_flags: each entity's BGS_ENTITY_* bits (NULL: none).  The list has passed check_scene_list.  want_aux
+// (bgs_render_entities_aux): every segment also projects its Depth and Normal colours, blended into out_depth / out_normal.
 static bgs_status render_entities_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
                                        const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                        const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
                                        const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
-                                       void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+                                       void* out_rgba, uint32_t out_format, int out_is_device_ptr, bool want_aux = false,
+                                       void* out_depth = nullptr, void* out_normal = nullptr) {
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
         return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
@@ -805,7 +807,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
         const bgs_cloud* cl = clouds[j];
         const uint32_t rm = st[j].rasterize_mode;
         SceneSeg& sg = tab.seg[j];
-        sg.fc = frame_consts(cl, view, &unis[j], &st[j], false);
+        sg.fc = frame_consts(cl, view, &unis[j], &st[j], want_aux);
         sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
         sg.pos = cl->pos;
         sg.blocks = cl->blocks;
@@ -837,8 +839,8 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     sf.gaussian_mode = scene->raster_mode == 2 ? BGS_GAUSSIAN_2D : BGS_GAUSSIAN_3D;
     sf.draw_mode = BGS_DRAW_ALL;
     if (scene->box) sf.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
-    return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr,
-                       depth, nullptr, scene);
+    return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, want_aux, out_depth,
+                       out_normal, depth, nullptr, scene);
 }
 
 // bgs_render_scene, and bgs_render_scene_4d (with_4d: Gaussian4d clouds are projected at uniforms[j].time in windows[j];
@@ -892,12 +894,10 @@ bgs_status bgs_render_scene_4d(bgs_context* c, const bgs_cloud* const* clouds, c
                                     out_format, out_is_device_ptr);
 }
 
-bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
-                                  const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
-                                  const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
-                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
-    const char* call = "render_entities";
-    if (!c) return BGS_EINVAL;
+// bgs_render_entities_ex's refusals of its arguments before the entities are read as single-cloud calls
+static bgs_status check_entities_call(bgs_context* c, const char* call, const bgs_cloud* const* clouds,
+                                      const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
+                                      const uint32_t* entity_flags, uint32_t k, const bgs_view* view, const bgs_settings* frame) {
     if (!clouds || !unis || !ents || !view || !frame)
         return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/entities/view/settings not ready", call);
     TRY(check_scene_list(c, call, clouds, k, frame));
@@ -905,8 +905,42 @@ bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds
         for (uint32_t j = 0; j < k; ++j)
             if (entity_flags[j] & ~(uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX)
                 return fail(c, BGS_EINVAL, "%s: entity_flags[%u] = 0x%x has an unknown bit", call, j, entity_flags[j]);
+    return BGS_OK;
+}
+
+bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                  const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
+                                  const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    const char* call = "render_entities";
+    if (!c) return BGS_EINVAL;
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
     return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
                                 out_is_device_ptr);
+}
+
+// bgs_render_entities_ex's frame and, in the same pass, its Depth and Normal frames (include/bgs.h): the refusals of
+// bgs_render_entities_ex, then those of the aux frames
+bgs_status bgs_render_entities_aux(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                   const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k,
+                                   const bgs_view* view, const bgs_settings* frame, const bgs_render_extras* ex,
+                                   const bgs_scene_depth* depth, void* out_rgba, void* out_depth, void* out_normal,
+                                   uint32_t out_format, int out_is_device_ptr) {
+    const char* call = "render_entities_aux";
+    if (!c) return BGS_EINVAL;
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
+    if (!out_rgba || !out_depth || !out_normal) return fail(c, BGS_EINVAL, "%s: the three output frames are required", call);
+    if (frame->flags & BGS_FLAG_ASYNC) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
+    for (uint32_t j = 0; j < k; ++j) {
+        // (a 4D cloud has no Normal colour; a covariance cloud no rotation; Velocity changes which splats draw, and how)
+        if (is_4d(clouds[j]->layout)) return fail(c, BGS_EINVAL, "%s: clouds[%u] is a Gaussian4d cloud", call, j);
+        if (clouds[j]->layout == CloudLayout::F16Cov)
+            return fail(c, BGS_EINVAL, "%s: clouds[%u] is a precomputed-covariance cloud (no rotation for the normal)", call, j);
+        if (ents[j].rasterize_mode == BGS_RASTERIZE_VELOCITY)
+            return fail(c, BGS_EINVAL, "%s: entities[%u] is in Velocity mode", call, j);
+    }
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
+                                out_is_device_ptr, true, out_depth, out_normal);
 }
 
 bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,

@@ -50,7 +50,9 @@ void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_sl
 // splat depths from the moved positions (depths non-null).
 void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
                           const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
-                          float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream);
+                          float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
+                          float4* aux /* bgs_render_entities_aux: each segment's depth / normal colours; else null */,
+                          cudaStream_t stream);
 void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
                              const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
                              float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);

@@ -585,10 +585,12 @@ __device__ __forceinline__ void store_rec(SplatRec* __restrict__ dst, const Spla
 
 // One entry of the index list -> the 48 B record at recs[r] (+ the 2DGS extra record and the aux colours).  An
 // undrawn gaussian (outside the frustum, or unselected under DrawMode::Selected) gets an empty bbox and no colour.
-// MODES2: the Classification / OpticalFlow colour sources (project_modes_kernel) instead of the four others.
+// MODES2: the Classification / OpticalFlow colour sources (project_modes_kernel) instead of the four others.  SCENE (the
+// scene kernels): a MODES2 segment also computes the aux colours when fc.aux is set (bgs_render_entities_aux); a
+// template flag, so project_modes_kernel stays as it is.
 // no_source: the frame has no colour source for this gaussian (a 3D or 2D one in a bgs_render_scene_4d Velocity frame:
 // the reference builds no pipeline for it), so it stays undrawn.  Only the scene kernels pass it.
-template <bool F16, uint32_t D, bool MODES2>
+template <bool F16, uint32_t D, bool MODES2, bool SCENE = false>
 __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCounters* __restrict__ ctr, uint32_t r,
                                             float4 p4, const float q[4], const float so[4], const float* sh,
                                             const float* __restrict__ cutoff_tab, uint32_t op_bits,
@@ -640,6 +642,12 @@ __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCo
                 flow_colour(fc, mc, pw, rgb);
             }
             rec.r = rgb[0]; rec.g = rgb[1]; rec.b = rgb[2];
+            if constexpr (SCENE) {
+                if (fc.aux) {
+                    depth_colour(fc, ctr, pw, drgb);
+                    normal_colour(fc, A, Rm, sc, nrgb);
+                }
+            }
         } else {
             if (mode == BGS_RASTERIZE_COLOR) sh_colour<D>(fc, A, pw, sh, rgb);
             if (mode == BGS_RASTERIZE_POSITION) position_colour(fc, pw, rgb);
@@ -730,7 +738,7 @@ struct Geo3d {
     __device__ __forceinline__ void project(const Src& src, uint32_t j, uint32_t, uint32_t r, float4 p4, const float q[4],
                                             const float so[4], const float* sh, uint32_t op_bits, const ModeConsts& mc) const {
         const FrameConsts& fc = src.fc(j);
-        project_one<F16, D, MODES2>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc,
+        project_one<F16, D, MODES2, Src::SEGMENTED>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc,
                                     MODES2 && Src::SEGMENTED && fc.rasterize_mode == BGS_RASTERIZE_VELOCITY);
     }
 };
@@ -1000,9 +1008,10 @@ template <bool F16, uint32_t D, bool MODES2>
 __global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
 project_scene_kernel(SceneTable tab, uint32_t group, uint32_t need_sh, SceneClasses classes, ModeConsts mc,
                      const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs,
-                     float4* __restrict__ extra, const float* __restrict__ cutoff_tab) {
+                     float4* __restrict__ extra, const float* __restrict__ cutoff_tab,
+                     float4* __restrict__ aux /* bgs_render_entities_aux only */) {
     project_loop(SceneSrc{tab, 1u << group, slot_ids},
-                 SceneGeo<Geo3d<F16, D, MODES2>>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, nullptr}, classes}, ctr, mc);
+                 SceneGeo<Geo3d<F16, D, MODES2>>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, aux}, classes}, ctr, mc);
 }
 
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
@@ -1018,7 +1027,8 @@ static_assert(sizeof(SceneTable) + sizeof(SceneTimes) + sizeof(SceneClasses) + s
 
 void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
                           const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
-                          float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream) {
+                          float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, float4* aux,
+                          cudaStream_t stream) {
     const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     const uint32_t g = group & ~ENTITY_MODES;
     with_layout_degree(g & 1u ? CloudLayout::F16 : CloudLayout::F32, g >> 1, [&](auto L, auto Dt) {
@@ -1028,7 +1038,7 @@ void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, c
             auto* kernel = (group & ENTITY_MODES) ? project_scene_kernel<is_f16(Lv), D, true>
                                                   : project_scene_kernel<is_f16(Lv), D, false>;
             kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, group, need_sh ? 1u : 0u, classes, mc, slot_ids, ctr, recs, extra,
-                                                      cutoff_tab);
+                                                      cutoff_tab, aux);
         }
     });
 }

@@ -177,7 +177,9 @@ constexpr uint32_t SM_BYTES_2D = SM_EXTRA + 4 * RT_CHUNK * 16;
 // AUX (bgs_render_aux): 2 x float4 [256] after the mode's own arrays: depth rgb, normal rgb of the staged splats
 // ZTEST (bgs_render_depth_test): float [256] at a 16 B stride after the mode's own arrays: the staged splats' depths d,
 // at the same offset from a splat's q0 record for every splat (what the candidate lists hold), so the blend loops reach
-// d with one load from the record address
+// d with one load from the record address.  AUX + ZTEST (bgs_render_entities_aux with a depth buffer): d rides in the
+// unused w lane of the staged depth colour instead, so MODE 4's arrays (40 KB) and the CTA's other shared arrays stay
+// within the 48 KB static limit
 constexpr uint32_t ZT_BYTES = RT_CHUNK * 16;
 
 // a staged splat's uv and q2 records, as offsets from the shared address of its q0 record (what the candidate lists hold)
@@ -246,8 +248,9 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // MODE 1: 3DGS USE_AABB conic falloff                              gaussian.wgsl:459-471
 // MODE 2: 2DGS USE_AABB ray-splat intersection                     gaussian.wgsl:441-458, gaussian_2d.wgsl:134-156
 // AUX: the same pass also blends the splats' Depth and Normal colour sources (aux records, 2 x float4 per splat) into two
-// more frames with the very same alphas: config C4's colour + depth + normal outputs cost one pass, not three.
-// ZTEST (MODE 0, 1, 2 without AUX): bgs_render_depth_test.  A pair blends only where its coverage decision holds and
+// more frames with the very same alphas: config C4's colour + depth + normal outputs cost one pass, not three.  Every
+// mode takes it (bgs_render_aux: MODE 0, 1, 2; bgs_render_entities_aux: any MODE, with or without ZTEST and BOX).
+// ZTEST: bgs_render_depth_test.  A pair blends only where its coverage decision holds and
 // d >= the pixel's scene depth; the warp's candidates leave out the splats below the scene everywhere in its rectangle.
 // MODE 3 / 4 (bgs_render_entities): mixed kinds, each splat tested by its own: kinds[r] (raster_kinds_kernel) is record r's
 // 0 = quad-uv, 1 = conic, 2 = surfel; MODE 4 when some splat is a surfel (the only one that stages the surfel records).
@@ -264,13 +267,12 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                                             void* __restrict__ out_normal, const uint32_t* __restrict__ truncated,
                                             const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
                                             const unsigned char* __restrict__ kinds) {
-    static_assert(!(AUX && ZTEST), "bgs_render_aux takes no depth buffer");
     constexpr bool MIXED = MODE >= 3, SURF = MODE == 2 || MODE == 4;
-    static_assert(!(AUX && MIXED), "bgs_render_aux renders one cloud");
     __shared__ __align__(16) unsigned char s_mem[(SURF ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0) +
-                                                 (ZTEST ? ZT_BYTES : 0)];
+                                                 (ZTEST && !AUX ? ZT_BYTES : 0)];
     constexpr uint32_t SM_AUX = SURF ? SM_BYTES_2D : SM_BYTES;
-    constexpr uint32_t REC_D = SM_AUX;   // ZTEST: d of the splat whose q0 record is at a, at a + REC_D
+    // ZTEST: d of the splat whose q0 record is at a, at a + REC_D (AUX: the w lane of its staged depth colour)
+    constexpr uint32_t REC_D = AUX ? SM_AUX + 12 : SM_AUX;
     __shared__ __align__(16) uint32_t s_ent[2][ENT_WORDS];    // TMA destination: the tile's pair-list chunks
     __shared__ __align__(8) unsigned long long s_bar[2];
     // MODE 0 and mixed: per staged splat cull thresholds (u, v) (quad-uv splats only)
@@ -353,10 +355,12 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
             }
             if (AUX) {
                 float4* s_ax = reinterpret_cast<float4*>(s_mem + SM_AUX);
-                s_ax[t] = __ldg(aux + (size_t)r * 2);
+                float4 ad = __ldg(aux + (size_t)r * 2);
+                if (ZTEST) ad.w = __ldg(splat_d + r);   // (REC_D; the blend reads the colour's x, y, z only)
+                s_ax[t] = ad;
                 s_ax[RT_CHUNK + t] = __ldg(aux + (size_t)r * 2 + 1);
             }
-            if (ZTEST) reinterpret_cast<float*>(s_mem + REC_D)[4 * t] = __ldg(splat_d + r);
+            if (ZTEST && !AUX) reinterpret_cast<float*>(s_mem + REC_D)[4 * t] = __ldg(splat_d + r);
         }
         __syncthreads();
         // each warp's candidates: the splats whose bbox touches its 8x4 pixels, listed by shared address of q0[j]
@@ -537,8 +541,9 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
     }
 }
 
+// (MODE 2 with AUX and ZTEST spills at 5 CTAs per SM: 4 leave it 64 registers)
 template <int MODE, bool AUX, bool ZTEST = false>
-__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : 5)
+__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : (MODE == 2 && AUX && ZTEST ? 4 : 5))
 raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
               const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
               const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
@@ -563,7 +568,7 @@ raster_mixed_kernel(const SplatRec* __restrict__ recs, const float4* __restrict_
 // The bounding-box overlay's blends (raster_body's BOX): raster_kernel's and raster_mixed_kernel's, with their launch
 // bounds.  Kernels of their own, so the frames without the overlay keep the very kernels they had.
 template <int MODE, bool AUX, bool ZTEST>
-__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : 5)
+__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : (MODE == 2 && AUX && ZTEST ? 4 : 5))
 raster_box_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
                   const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
                   const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
@@ -582,6 +587,21 @@ raster_mixed_box_kernel(const SplatRec* __restrict__ recs, const float4* __restr
                         const unsigned char* __restrict__ kinds) {
     raster_body<MODE, false, ZTEST, true>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr,
                                           nullptr, truncated, splat_d, scene, pitch, kinds);
+}
+
+// bgs_render_entities_aux's blends of mixed kinds: raster_mixed_kernel's (BOX: raster_mixed_box_kernel's) with the depth
+// and normal frames.  Kernels of their own, so the mixed frames without aux keep the very kernels they had.  (MODE 4, or
+// ZTEST, spills at 5 CTAs per SM.)
+template <int MODE, bool ZTEST, bool BOX>
+__global__ void __launch_bounds__(RT_THREADS, MODE == 4 || ZTEST ? 4 : 5)
+raster_mixed_aux_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
+                        const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W, int H, int tiles_x,
+                        void* __restrict__ out, uint32_t format, const float4* __restrict__ aux, void* __restrict__ out_depth,
+                        void* __restrict__ out_normal, const uint32_t* __restrict__ truncated,
+                        const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
+                        const unsigned char* __restrict__ kinds) {
+    raster_body<MODE, true, ZTEST, BOX>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth,
+                                        out_normal, truncated, splat_d, scene, pitch, kinds);
 }
 
 // the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
@@ -781,7 +801,22 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
                    const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
                    cudaStream_t stream, const unsigned char* kinds, bool box) {
     const int grid = tiles_x * tiles_y;
-    const bool ztest = zt.scene != nullptr;   // (bgs_render_aux frames never carry a depth buffer)
+    const bool ztest = zt.scene != nullptr;
+    // the kernel tables' rows: plain, AUX, ZTEST, AUX + ZTEST
+    const int row = (ztest ? 2 : 0) + (aux != nullptr ? 1 : 0);
+    if (mode >= 3 && aux != nullptr) {   // bgs_render_entities_aux of mixed kinds
+        static void (*const mixed_aux[2][2][2])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int,
+                                                void*, uint32_t, const float4*, void*, void*, const uint32_t*, const float*,
+                                                const float*, size_t, const unsigned char*) = {
+            {{raster_mixed_aux_kernel<3, false, false>, raster_mixed_aux_kernel<3, false, true>},
+             {raster_mixed_aux_kernel<3, true, false>, raster_mixed_aux_kernel<3, true, true>}},
+            {{raster_mixed_aux_kernel<4, false, false>, raster_mixed_aux_kernel<4, false, true>},
+             {raster_mixed_aux_kernel<4, true, false>, raster_mixed_aux_kernel<4, true, true>}}};
+        mixed_aux[mode - 3][ztest][box]<<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out,
+                                                                         format, aux, out_depth, out_normal, truncated,
+                                                                         zt.splat_d, zt.scene, zt.pitch, kinds);
+        return;
+    }
     if (box) {   // the bounding-box overlay: raster_body's generic loop for every mode, never raster2_kernel
         if (mode >= 3) {
             auto* kernel = mode == 3 ? (ztest ? raster_mixed_box_kernel<3, true> : raster_mixed_box_kernel<3, false>)
@@ -790,13 +825,14 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
                                                     zt.splat_d, zt.scene, zt.pitch, kinds);
             return;
         }
-        static void (*const box_kernels[3][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int,
+        static void (*const box_kernels[4][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int,
                                                void*, uint32_t, const float4*, void*, void*, const uint32_t*, const float*,
                                                const float*, size_t) = {
             {raster_box_kernel<0, false, false>, raster_box_kernel<1, false, false>, raster_box_kernel<2, false, false>},
             {raster_box_kernel<0, true, false>, raster_box_kernel<1, true, false>, raster_box_kernel<2, true, false>},
-            {raster_box_kernel<0, false, true>, raster_box_kernel<1, false, true>, raster_box_kernel<2, false, true>}};
-        box_kernels[ztest ? 2 : aux != nullptr][mode]<<<grid, RT_THREADS, 0, stream>>>(
+            {raster_box_kernel<0, false, true>, raster_box_kernel<1, false, true>, raster_box_kernel<2, false, true>},
+            {raster_box_kernel<0, true, true>, raster_box_kernel<1, true, true>, raster_box_kernel<2, true, true>}};
+        box_kernels[row][mode]<<<grid, RT_THREADS, 0, stream>>>(
             recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated, zt.splat_d,
             zt.scene, zt.pitch);
         return;
@@ -816,14 +852,15 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
             zt.scene, zt.pitch);
         return;
     }
-    // aux != nullptr: colour + depth + normal in one pass (bgs_render_aux)
-    static void (*const kernels[3][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*,
+    // aux != nullptr: colour + depth + normal in one pass (bgs_render_aux, bgs_render_entities_aux)
+    static void (*const kernels[4][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*,
                                        uint32_t, const float4*, void*, void*, const uint32_t*, const float*, const float*,
                                        size_t) = {
         {raster_kernel<0, false>, raster_kernel<1, false>, raster_kernel<2, false>},
         {raster_kernel<0, true>, raster_kernel<1, true>, raster_kernel<2, true>},
-        {raster_kernel<0, false, true>, raster_kernel<1, false, true>, raster_kernel<2, false, true>}};
-    kernels[ztest ? 2 : aux != nullptr][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
+        {raster_kernel<0, false, true>, raster_kernel<1, false, true>, raster_kernel<2, false, true>},
+        {raster_kernel<0, true, true>, raster_kernel<1, true, true>, raster_kernel<2, true, true>}};
+    kernels[row][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
         recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated, zt.splat_d,
         zt.scene, zt.pitch);
 }

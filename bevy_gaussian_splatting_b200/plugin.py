@@ -21,7 +21,7 @@ from . import abi
 from .camera import GaussianCamera, View
 from .gaussian import SH_WIDTHS, PlanarGaussian3d, PlanarGaussian4d, compute_aabb
 from .particles import PARTICLE_BEHAVIOR_DTYPE, as_particle_behaviors
-from .settings import CloudSettings, GaussianMode, SparseSelect
+from .settings import CloudSettings, GaussianMode, RasterizeMode, SparseSelect
 
 
 def _ptr(a: np.ndarray):
@@ -280,6 +280,22 @@ def check_entities(entities) -> CloudSettings:
     return first
 
 
+def check_entities_aux(entities) -> CloudSettings:
+    """`check_entities` for one bgs_render_entities_aux call, which also raises ValueError for a Gaussian4d cloud (its
+    layout has no Normal colour), a precomputed-covariance cloud (no rotation) and an entity in Velocity mode (it changes
+    which splats draw, so the three frames would not share their alphas)."""
+    entities = list(entities)
+    first = check_entities(entities)
+    for j, (h, st, _) in enumerate(entities):
+        if is_4d_handle(h):
+            raise ValueError(f"render_entities_aux: entity {j} is a Gaussian4d cloud")
+        if getattr(h, "precompute_covariance", False):
+            raise ValueError(f"render_entities_aux: entity {j} is a precomputed-covariance cloud")
+        if RasterizeMode(st.rasterize_mode) == RasterizeMode.Velocity:
+            raise ValueError(f"render_entities_aux: entity {j} is in Velocity mode")
+    return first
+
+
 def entity_settings(settings: CloudSettings) -> abi.bgs_entity_settings:
     """One entity's bgs_entity_settings."""
     s = settings.to_abi()
@@ -420,6 +436,35 @@ class GaussianSplattingPlugin:
         entities = list(entities)
         first = check_entities(entities)
         code, dtype, ch = self.FORMATS[fmt]
+        if out is None:
+            out = np.empty((view.height, view.width, ch), dtype)
+        assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
+        args = self._entities_args(entities, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over)
+        zd = self._scene_depth(scene_depth, view)
+        self._check(self._lib.bgs_render_entities_ex(self._ctx, *args, None if zd is None else C.byref(zd), _ptr(out), code, 0))
+        return out
+
+    def render_entities_aux(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None,
+                            previous_view: View | None = None, delta_time: float | None = None, premultiplied: bool = False,
+                            blend_over: bool = False) -> list[np.ndarray]:
+        """`render_entities`' frame and its depth and normal frames in ONE pass (`bgs_render_entities_aux`): returns
+        [rgba, depth, normal], the depth and normal frames being `render_entities`' with every entity's rasterize_mode
+        replaced by Depth and by Normal.  Validates like `render_entities` (`check_entities_aux`: also ValueError, before
+        any call, for a Gaussian4d or precomputed-covariance cloud and a Velocity entity).  Synchronous only.
+        `blend_over`: each frame over the context's previous frame of its kind (rgba: the last frame; depth / normal: the
+        last aux frame's)."""
+        entities = list(entities)
+        first = check_entities_aux(entities)
+        code, dtype, ch = self.FORMATS[fmt]
+        outs = [np.empty((view.height, view.width, ch), dtype) for _ in range(3)]
+        args = self._entities_args(entities, first, view, previous_view, delta_time, False, premultiplied, blend_over)
+        zd = self._scene_depth(scene_depth, view)
+        self._check(self._lib.bgs_render_entities_aux(self._ctx, *args, None if zd is None else C.byref(zd), *(_ptr(o) for o in outs),
+                                                      code, 0))
+        return outs
+
+    def _entities_args(self, entities, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over):
+        """(clouds, uniforms, entities, entity flags, k, view, frame, extras) of a bgs_render_entities_ex or _aux call."""
         v = view.to_abi()
         s = first.to_abi()
         s.flags &= ~abi.BGS_FLAG_VISUALIZE_BOUNDING_BOX   # (each entity's own, below)
@@ -435,14 +480,7 @@ class GaussianSplattingPlugin:
         clouds = (C.c_void_p * k)(*[h._h.value for h, _, _ in entities])
         unis = (abi.bgs_cloud_uniform * k)(*[self.cloud_uniform(st, tr, h.aabb) for h, st, tr in entities])
         ents = (abi.bgs_entity_settings * k)(*[entity_settings(st) for _, st, _ in entities])
-        if out is None:
-            out = np.empty((view.height, view.width, ch), dtype)
-        assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
-        zd = self._scene_depth(scene_depth, view)
-        self._check(self._lib.bgs_render_entities_ex(self._ctx, clouds, unis, ents, eflags, k, C.byref(v), C.byref(s),
-                                                     None if ex is None else C.byref(ex), None if zd is None else C.byref(zd),
-                                                     _ptr(out), code, 0))
-        return out
+        return clouds, unis, ents, eflags, k, C.byref(v), C.byref(s), None if ex is None else C.byref(ex)
 
     def _render_4d(self, handle, v, u, s, ex, zd, settings, target, code, is_device):
         return self._lib.bgs_render_4d(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), None if ex is None else C.byref(ex),
@@ -487,15 +525,23 @@ class GaussianSplattingPlugin:
         return self._us_cache[1], self._us_cache[2], self._us_cache[3]
 
     def render_view_aux(self, handle: PlanarGaussian3dHandle, settings: CloudSettings, view: View,
-                        transform: CloudTransform | None = None, fmt: str = "rgba32f"):
-        """Colour, depth and normal frames of one view in ONE pass (`bgs_render_aux`, BASELINE.json config 4)."""
+                        transform: CloudTransform | None = None, fmt: str = "rgba32f", scene_depth=None):
+        """Colour, depth and normal frames of one view in ONE pass (`bgs_render_aux`, BASELINE.json config 4).
+        `scene_depth` (as in `render_view`): the three frames depth-tested against it, through `bgs_render_entities_aux`
+        with this one entity (the same frames `bgs_render_aux` draws, with the depth test)."""
         code, dtype, ch = self.FORMATS[fmt]
         v = view.to_abi()
         u = self.cloud_uniform(settings, transform, handle.aabb)
         s = settings.to_abi()
         outs = [np.empty((view.height, view.width, ch), dtype) for _ in range(3)]
-        st = self._lib.bgs_render_aux(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), _ptr(outs[0]), _ptr(outs[1]),
-                                      _ptr(outs[2]), code, 0)
+        if scene_depth is None:
+            st = self._lib.bgs_render_aux(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), _ptr(outs[0]), _ptr(outs[1]),
+                                          _ptr(outs[2]), code, 0)
+        else:
+            zd = self._scene_depth(scene_depth, view)
+            e = entity_settings(settings)
+            st = self._lib.bgs_render_entities_aux(self._ctx, (C.c_void_p * 1)(handle._h.value), C.byref(u), C.byref(e), None, 1,
+                                                   C.byref(v), C.byref(s), None, C.byref(zd), *(_ptr(o) for o in outs), code, 0)
         self._check(st)
         return outs
 

@@ -727,6 +727,43 @@ bgs_status bgs_render_entities_ex(bgs_context* ctx, const bgs_cloud* const* clou
                                   const bgs_render_extras* extras, const bgs_scene_depth* depth, void* out_rgba,
                                   uint32_t out_format, int out_is_device_ptr);
 
+/* bgs_render_entities_ex's frame and its depth and normal frames in ONE pass: bgs_render_aux for a scene, with or without
+ * a depth buffer.  A 2DGS room scan with a 3DGS object in it gets the G-buffer an app needs for relighting, SSAO or
+ * mesh compositing from one key-gen, sort, projection, binning and blend, with the splats of both clouds in joint order.
+ *
+ * The rule, exactly:
+ *   out_rgba.  Byte for byte the frame bgs_render_entities_ex produces with the same arguments; every colour mode a
+ *     non-4D entity takes, Classification and OpticalFlow included (extras as there).
+ *   out_depth / out_normal.  Byte for byte the frames bgs_render_entities_ex produces when every entity's rasterize_mode is
+ *     replaced by Depth / by Normal and everything else is kept: draw modes, each entity's bounding-box overlay (its edges
+ *     in all three frames, as bgs_render_aux draws them), the depth test, BGS_FLAG_PREMULTIPLIED_OUT and
+ *     BGS_FLAG_BLEND_OVER_TARGET.  The Depth colour range is the scenes' joint sorted[1] / sorted[N-1] rule.
+ *   Targets.  All three share out_format and the host/device kind of the pointers.  Blend-over: a device target is blended
+ *     over what it holds, each of the three over its own pixels.  Host targets: out_rgba over the context's last frame
+ *     (as bgs_render_entities_ex), out_depth / out_normal over the depth / normal frames of the last aux frame
+ *     (bgs_render_aux or this call) this context delivered to host memory -- transparent black before the first, and
+ *     whenever this frame is larger than every aux frame before it (the library's aux buffers grow, zeroed).
+ *   k == 1.  With depth == NULL and a Color, Depth, Position or Normal entity the call is bgs_render_aux with that
+ *     entity's settings as the frame's, byte for byte in all three frames; with a depth buffer it is that frame with the
+ *     depth test.  (bgs_render_aux itself takes no depth buffer.)
+ *   Hooks and stats.  Sorted entries, tile ranges and slices, records (bgs_debug_projected: the rgba frame's colours; the
+ *     aux colours are not part of the records), splat depths and bgs_frame_stats are those of the rgba frame's
+ *     bgs_render_entities_ex call rendered in one round: like bgs_render_aux, the call is never split into chunked rounds
+ *     (BGS_FLAG_CHUNKS is ignored).
+ *   Synchronous only.
+ * Launches: bgs_render_entities_ex's, plus the Depth range's when no entity is in Depth mode.
+ * Refused with BGS_EINVAL, nothing enqueued or written and the previous frame's debug hooks kept: every refusal of
+ *   bgs_render_entities_ex; a NULL target (any of the three); a device target not aligned to its pixel (each of the
+ *   three); BGS_FLAG_ASYNC; a Gaussian4d cloud (its layout has no Normal colour); a precomputed-covariance cloud (no
+ *   rotation); an entity in Velocity mode (it changes opacity and which splats draw, so the three frames would no
+ *   longer share their alphas).  NULL clouds, uniforms, entities, view or frame -> BGS_NOT_READY. */
+bgs_status bgs_render_entities_aux(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                                   const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */,
+                                   uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                                   const bgs_render_extras* extras, const bgs_scene_depth* depth /* may be NULL */,
+                                   void* out_rgba, void* out_depth, void* out_normal, uint32_t out_format,
+                                   int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target
