@@ -194,6 +194,11 @@ struct FrameOut {
     void* host_rgba = nullptr;          // host frames the result is copied to
     void* host_depth = nullptr;
     void* host_normal = nullptr;
+    // a views frame: view i's device target, host frame (host targets; else NULL) and bytes
+    uint32_t views = 0;
+    void* view_rgba[MAX_VIEWS] = {};
+    void* view_host[MAX_VIEWS] = {};
+    size_t view_bytes[MAX_VIEWS] = {};
 };
 
 // the caller's device frames, or the library's own (grown on demand)
@@ -234,6 +239,26 @@ bgs_status frame_out(bgs_context* c, const bgs_settings* st, uint32_t format, si
     for (int k = 0; k < 2; ++k) TRY(c->frame_aux[k].grow(c, bytes, true));
     o->depth = c->frame_aux[0].p; o->normal = c->frame_aux[1].p;
     o->host_depth = out_depth; o->host_normal = out_normal;
+    return BGS_OK;
+}
+
+// a views frame's targets: the caller's device frames, or the library's frames holding every view, one after another
+// (the targets have passed bgs_render_views' checks)
+bgs_status frame_out_views(bgs_context* c, const bgs_settings* st, uint32_t format, const ViewTable& vt, void* const* targets,
+                           int out_is_device_ptr, FrameOut* o) {
+    const size_t bpp = format_bpp(format);
+    size_t total = 0;
+    for (uint32_t i = 0; i < vt.v; ++i) total += (size_t)vt.W[i] * vt.H[i] * bpp;
+    TRY(frame_out(c, st, format, out_is_device_ptr ? (size_t)vt.W[0] * vt.H[0] * bpp : total,
+                  out_is_device_ptr ? targets[0] : nullptr, out_is_device_ptr, false, nullptr, nullptr, o));
+    o->views = vt.v;
+    size_t at = 0;
+    for (uint32_t i = 0; i < vt.v; ++i) {
+        o->view_bytes[i] = (size_t)vt.W[i] * vt.H[i] * bpp;
+        o->view_rgba[i] = out_is_device_ptr ? targets[i] : static_cast<char*>(o->rgba) + at;
+        o->view_host[i] = out_is_device_ptr ? nullptr : targets[i];
+        at += o->view_bytes[i];
+    }
     return BGS_OK;
 }
 
@@ -458,9 +483,10 @@ static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, co
 // is then its first cloud and fc its first segment's.
 static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const ModeConsts* modes,
                                 const TemporalConsts* tc, const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd,
-                                const std::shared_ptr<const SceneFacts>& scene) {
+                                const std::shared_ptr<const SceneFacts>& scene, const ViewTable* views) {
     const uint32_t n = scene ? scene->tab.n_total : cloud->n;
-    const uint32_t num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
+    // (a views frame: every view's tiles, one global tile id space)
+    const uint32_t num_tiles = views ? views->tile0[views->v] : (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     cudaStream_t q = c->stream;
     uint32_t launches = 0;
     if (scene) {
@@ -573,7 +599,11 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
         uint2* rng = c->ranges + (size_t)r * num_tiles;
         uint32_t* hist_r = c->hist + (size_t)(4 + 4 * r) * 256;
         // the depth sort's spare ping-pong buffers (N words each) hold the large-footprint queue
-        CU(c, launch_bin_emit_coop(c->recs.p, p.by_slot ? c->vals[cur].p : nullptr, c->ctr, cc, fa, fb, num_tiles,
+        if (views)   // (one round)
+            CU(c, launch_bin_emit_views(c->recs.p, c->vals[cur].p, c->ctr, cc, num_tiles, c->bin_block_cnt, c->cap_pairs,
+                                        c->pkeys[0].p, c->pvals[0].p, c->keys[cur ^ 1].p, c->vals[cur ^ 1].p, c->cap_n,
+                                        p.bin_grid, c->d_sticky, c->slot_ids.p, *views, c->sm_count, q));
+        else CU(c, launch_bin_emit_coop(c->recs.p, p.by_slot ? c->vals[cur].p : nullptr, c->ctr, cc, fa, fb, num_tiles,
                                    c->bin_block_cnt, fc.tiles_x, c->cap_pairs, c->pkeys[0].p, c->pvals[0].p,
                                    c->keys[cur ^ 1].p, c->vals[cur ^ 1].p, c->cap_n, p.bin_grid, c->d_sticky, q));
         ++launches;
@@ -593,9 +623,13 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             // the blend runs on the LOW-priority stream; the render stream resumes once it is done
             CU(c, cudaEventRecord(c->ev_front, q));
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
-            launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
-                          fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal, &c->ctr->truncated,
-                          zt, c->stream_r, c->kinds.p, p.box);
+            if (views)
+                launch_raster_views(p.raster_mode, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, o.raster_format,
+                                    &c->ctr->truncated, zt.splat_d, c->kinds.p, p.box, *views, c->stream_r);
+            else
+                launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
+                              fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal,
+                              &c->ctr->truncated, zt, c->stream_r, c->kinds.p, p.box);
             CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
             CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
         } else
@@ -610,11 +644,21 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, q));
     CU(c, cudaMemcpyAsync(c->h_sticky, c->d_sticky, 4, cudaMemcpyDeviceToHost, q));
     if (o.slot >= 0) CU(c, cudaEventRecord(c->ev_raster[o.slot], q));
-    if (o.slot >= 0 && o.host_rgba) {
+    // a views frame to host memory: each view's frame to its own host target
+    auto copy_views = [&](cudaStream_t s) -> bgs_status {
+        for (uint32_t i = 0; i < o.views; ++i)
+            CU(c, cudaMemcpyAsync(o.view_host[i], o.view_rgba[i], o.view_bytes[i], cudaMemcpyDeviceToHost, s));
+        return BGS_OK;
+    };
+    const bool views_to_host = o.views > 0 && o.view_host[0] != nullptr;
+    if (o.slot >= 0 && (o.host_rgba || views_to_host)) {
         CU(c, cudaStreamWaitEvent(c->stream_copy, c->ev_raster[o.slot], 0));
-        CU(c, cudaMemcpyAsync(o.host_rgba, o.rgba, o.bytes, cudaMemcpyDeviceToHost, c->stream_copy));
+        if (views_to_host) TRY(copy_views(c->stream_copy));
+        else CU(c, cudaMemcpyAsync(o.host_rgba, o.rgba, o.bytes, cudaMemcpyDeviceToHost, c->stream_copy));
         CU(c, cudaEventRecord(c->ev_copied[o.slot], c->stream_copy));
         c->copy_pending[o.slot] = true;
+    } else if (views_to_host) {
+        TRY(copy_views(q));
     } else if (o.host_rgba) {
         CU(c, cudaMemcpyAsync(o.host_rgba, o.rgba, o.bytes, cudaMemcpyDeviceToHost, q));
         if (o.host_depth) {
@@ -622,7 +666,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaMemcpyAsync(o.host_normal, o.normal, o.bytes, cudaMemcpyDeviceToHost, q));
         }
     }
-    c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, fc.tiles_x, fc.tiles_y, fc.Wi, fc.Hi, o.rgba, zd != nullptr, scene};
+    c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, views ? (int)num_tiles : fc.tiles_x, views ? 1 : fc.tiles_y, fc.Wi,
+               fc.Hi, o.rgba, zd != nullptr, scene};
     c->launches = launches;
     return BGS_OK;
 }
@@ -650,7 +695,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
                               const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
                               int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal,
                               const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr,
-                              const std::shared_ptr<const SceneFacts>& scene = nullptr) {
+                              const std::shared_ptr<const SceneFacts>& scene = nullptr, void* const* view_targets = nullptr) {
     if (!c) return BGS_EINVAL;
     if (!scene) TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));   // (scenes: per cloud, before)
     if (zd) TRY(check_scene_depth(c, zd, view));
@@ -665,12 +710,21 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     mc.num_classes = ex ? ex->num_classes : 1u;
     if (ex) { memcpy(mc.prev_clip_from_world, ex->previous_clip_from_world, 64); mc.delta_time = ex->delta_time; }
     const ModeConsts* modes = st->rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION || scene ? &mc : nullptr;
-    const uint32_t n = scene ? scene->tab.n_total : cloud->n, num_tiles = (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
+    // a views frame (scene->views.v > 1): every view's tiles and targets
+    const bool views = scene && scene->views.v > 1;
+    const uint32_t n = scene ? scene->tab.n_total : cloud->n;
+    const uint32_t num_tiles = views ? scene->views.tile0[scene->views.v] : (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
     FrameOut o;
-    TRY(frame_out(c, st, out_format, (size_t)fc.Wi * fc.Hi * format_bpp(out_format), out_rgba, out_is_device_ptr, want_aux,
-                  out_depth, out_normal, &o));
+    if (views) TRY(frame_out_views(c, st, out_format, scene->views, view_targets, out_is_device_ptr, &o));
+    else TRY(frame_out(c, st, out_format, (size_t)fc.Wi * fc.Hi * format_bpp(out_format), out_rgba, out_is_device_ptr, want_aux,
+                       out_depth, out_normal, &o));
+    ViewTable vt = {};
+    if (views) {
+        vt = scene->views;
+        for (uint32_t i = 0; i < vt.v; ++i) vt.out[i] = o.view_rgba[i];
+    }
     for (int attempt = 0; attempt < 4; ++attempt) {
         FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
         if (scene) {   // (st plans it as an aabb frame or an overlay one: one round)
@@ -685,7 +739,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         TRY(ensure_arena(c, num_tiles));
         TRY(ensure_status(c, c->status_depth, c->status_n, n));
         TRY(ensure_status(c, c->status_pairs, c->status_np, c->cap_pairs));
-        TRY(enqueue_frame(c, cloud, fc, modes, tc, p, o, zd, scene));
+        TRY(enqueue_frame(c, cloud, fc, modes, tc, p, o, zd, scene, views ? &vt : nullptr));
         if (st->flags & BGS_FLAG_ASYNC) {
             c->async_pending = true;
             c->have_frame = false;     // hooks need bgs_sync() first
@@ -753,12 +807,15 @@ static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.ga
 // Gaussian4d cloud when with_4d) with its own settings, num_classes and window, drawn into one depth-sorted frame.
 // entity_flags: each entity's BGS_ENTITY_* bits (NULL: none).  The list has passed check_scene_list.  want_aux
 // (bgs_render_entities_aux): every segment also projects its Depth and Normal colours, blended into out_depth / out_normal.
+// nv > 1 (bgs_render_views, which has checked nv, the targets and the entities' modes): the k entities seen from each of
+// the nv views (depth: nv buffers, or NULL), segment i k + j entity j from view i, view i's frame into view_targets[i].
 static bgs_status render_entities_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
                                        const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                        const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
                                        const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
                                        void* out_rgba, uint32_t out_format, int out_is_device_ptr, bool want_aux = false,
-                                       void* out_depth = nullptr, void* out_normal = nullptr) {
+                                       void* out_depth = nullptr, void* out_normal = nullptr, uint32_t nv = 1,
+                                       void* const* view_targets = nullptr) {
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
         return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
@@ -781,8 +838,9 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
         ej.num_classes = e.num_classes;
         bgs_settings chk = s;   // (a non-4D entity in Velocity is undrawn, and checked as a Color one)
         if (!is4 && chk.rasterize_mode == BGS_RASTERIZE_VELOCITY) chk.rasterize_mode = BGS_RASTERIZE_COLOR;
-        TRY(check_render(c, clouds[j], view, &unis[j], &chk, ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr,
-                         out_format, false, is4));
+        for (uint32_t i = 0; i < nv; ++i)   // (as the single-view call of each view)
+            TRY(check_render(c, clouds[j], &view[i], &unis[j], &chk,
+                             ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr, out_format, false, is4));
         if (is4) TRY(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, scene->times.t[j]));
         const bgs_entity_settings& e0 = ents[0];
         undrawn = undrawn && !is4 && e.rasterize_mode == BGS_RASTERIZE_VELOCITY && e.gaussian_mode == e0.gaussian_mode &&
@@ -794,39 +852,56 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     }
     // (one Velocity frame without a Gaussian4d cloud: nothing has a colour source, as in bgs_render_depth_test)
     if (undrawn) return fail(c, BGS_EINVAL, "%s: a Velocity frame with no Gaussian4d cloud listed", call);
+    const uint64_t n_view = total;   // (every view lists the k entities: N = nv x n_view)
+    total *= nv;
     if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "%s: N = %llu gaussians, must be < 2^30", call, (unsigned long long)total);
-    if (depth) TRY(check_scene_depth(c, depth, view));
+    if (depth)
+        for (uint32_t i = 0; i < nv; ++i) TRY(check_scene_depth(c, &depth[i], &view[i]));
     SceneTable& tab = scene->tab;
     memset(&tab, 0, sizeof(tab));
-    tab.k = k;
+    tab.k = k * nv;
     tab.n_total = (uint32_t)total;
-    scene->kinds.k = k;
+    scene->kinds.k = k * nv;
     uint32_t offset = 0;
     bool box_all = true;
-    for (uint32_t j = 0; j < k; ++j) {
-        const bgs_cloud* cl = clouds[j];
-        const uint32_t rm = st[j].rasterize_mode;
-        SceneSeg& sg = tab.seg[j];
-        sg.fc = frame_consts(cl, view, &unis[j], &st[j], want_aux);
-        sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
-        sg.pos = cl->pos;
-        sg.blocks = cl->blocks;
-        sg.offset = offset;
-        sg.n = cl->n;
-        // the plain colour kernel, or the Classification / OpticalFlow one (which leaves a 3D Velocity record undrawn)
-        sg.group = project_group(cl->layout, cl->sh_degree);
-        if (sg.group != PROJECT_GROUP_4D && rm >= BGS_RASTERIZE_CLASSIFICATION) sg.group |= ENTITY_MODES;
-        const bool sh = rm == ((sg.group & ENTITY_MODES) ? BGS_RASTERIZE_CLASSIFICATION : BGS_RASTERIZE_COLOR);
-        const size_t gi = std::find(scene->groups.begin(), scene->groups.end(), sg.group) - scene->groups.begin();
-        if (gi == scene->groups.size()) { scene->groups.push_back(sg.group); scene->need_sh.push_back(0u); }
-        if (sh) scene->need_sh[gi] = 1u;
-        scene->classes.n[j] = ents[j].num_classes;
-        scene->kinds.offset[j] = offset;
-        scene->kinds.kind[j] = (uint32_t)blend_kind(ents[j]) | (box_of(j) ? BOX_KIND : 0u);
-        scene->box = scene->box || box_of(j);
-        box_all = box_all && box_of(j);
-        offset += cl->n;
-        scene->clouds.push_back(cl);
+    for (uint32_t i = 0; i < nv; ++i)
+        for (uint32_t j = 0; j < k; ++j) {
+            const uint32_t sj = i * k + j;   // entity j seen from view i
+            const bgs_cloud* cl = clouds[j];
+            const uint32_t rm = st[j].rasterize_mode;
+            SceneSeg& sg = tab.seg[sj];
+            sg.fc = frame_consts(cl, &view[i], &unis[j], &st[j], want_aux);
+            sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
+            sg.pos = cl->pos;
+            sg.blocks = cl->blocks;
+            sg.offset = offset;
+            sg.n = cl->n;
+            // the plain colour kernel, or the Classification / OpticalFlow one (which leaves a 3D Velocity record undrawn)
+            sg.group = project_group(cl->layout, cl->sh_degree);
+            if (sg.group != PROJECT_GROUP_4D && rm >= BGS_RASTERIZE_CLASSIFICATION) sg.group |= ENTITY_MODES;
+            const bool sh = rm == ((sg.group & ENTITY_MODES) ? BGS_RASTERIZE_CLASSIFICATION : BGS_RASTERIZE_COLOR);
+            const size_t gi = std::find(scene->groups.begin(), scene->groups.end(), sg.group) - scene->groups.begin();
+            if (gi == scene->groups.size()) { scene->groups.push_back(sg.group); scene->need_sh.push_back(0u); }
+            if (sh) scene->need_sh[gi] = 1u;
+            scene->times.t[sj] = scene->times.t[j];
+            scene->classes.n[sj] = ents[j].num_classes;
+            scene->kinds.offset[sj] = offset;
+            scene->kinds.kind[sj] = (uint32_t)blend_kind(ents[j]) | (box_of(j) ? BOX_KIND : 0u);
+            scene->box = scene->box || box_of(j);
+            box_all = box_all && box_of(j);
+            offset += cl->n;
+            scene->clouds.push_back(cl);
+        }
+    if (nv > 1) {   // each view's tiles after the earlier views', its depth buffer
+        ViewTable& vt = scene->views;
+        vt.v = nv;
+        vt.n_view = (uint32_t)n_view;
+        for (uint32_t i = 0; i < nv; ++i) {
+            const FrameConsts& f = tab.seg[i * k].fc;
+            vt.W[i] = f.Wi; vt.H[i] = f.Hi; vt.tiles_x[i] = f.tiles_x; vt.tiles_y[i] = f.tiles_y;
+            vt.tile0[i + 1] = vt.tile0[i] + (uint32_t)f.tiles_x * (uint32_t)f.tiles_y;
+            if (depth) { vt.scene[i] = depth[i].depth; vt.pitch[i] = (size_t)depth[i].pitch_bytes; }
+        }
     }
     // one kind: its own blend; several, or entities with and without the overlay: the mixed one (with the surfel records
     // when some entity has them)
@@ -839,8 +914,9 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     sf.gaussian_mode = scene->raster_mode == 2 ? BGS_GAUSSIAN_2D : BGS_GAUSSIAN_3D;
     sf.draw_mode = BGS_DRAW_ALL;
     if (scene->box) sf.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
+    if (nv > 1) sf.flags = (sf.flags & ~(uint32_t)BGS_FLAG_CHUNKS) | BGS_FLAG_NO_CHUNKS;   // (one round)
     return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, want_aux, out_depth,
-                       out_normal, depth, nullptr, scene);
+                       out_normal, depth, nullptr, scene, view_targets);
 }
 
 // bgs_render_scene, and bgs_render_scene_4d (with_4d: Gaussian4d clouds are projected at uniforms[j].time in windows[j];
@@ -941,6 +1017,41 @@ bgs_status bgs_render_entities_aux(bgs_context* c, const bgs_cloud* const* cloud
     }
     return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
                                 out_is_device_ptr, true, out_depth, out_normal);
+}
+
+// bgs_render_entities_ex of each of v views in one frame (include/bgs.h): the refusals of bgs_render_entities_ex (each view
+// checked as its own call), then those of the views frame; one view is bgs_render_entities_ex itself
+bgs_status bgs_render_views(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                            const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* views,
+                            uint32_t v, const bgs_settings* frame, const bgs_scene_depth* depths, void* const* out_rgba,
+                            uint32_t out_format, int out_is_device_ptr) {
+    const char* call = "render_views";
+    if (!c) return BGS_EINVAL;
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, views, frame));
+    if (v == 0) return fail(c, BGS_EINVAL, "%s: v = 0 views", call);
+    if ((uint64_t)v * k > BGS_SCENE_MAX_CLOUDS)
+        return fail(c, BGS_EINVAL, "%s: v x k = %u x %u segments, at most %d", call, v, k, BGS_SCENE_MAX_CLOUDS);
+    if (!out_rgba) return fail(c, BGS_EINVAL, "%s: out_rgba is NULL", call);
+    const size_t bpp = format_bpp(out_format);
+    for (uint32_t i = 0; i < v; ++i) {
+        if (!out_rgba[i]) return fail(c, BGS_EINVAL, "%s: out_rgba[%u] is NULL", call, i);
+        if (out_is_device_ptr && reinterpret_cast<uintptr_t>(out_rgba[i]) % bpp != 0)
+            return fail(c, BGS_EINVAL, "%s: device target out_rgba[%u] = %p is not aligned to its %zu-byte pixels", call, i,
+                        out_rgba[i], bpp);
+    }
+    for (uint32_t j = 0; j < k; ++j) {
+        // (a Depth entity's colour range is the frame's sorted list; OpticalFlow has one previous view per frame)
+        if (ents[j].rasterize_mode == BGS_RASTERIZE_DEPTH) return fail(c, BGS_EINVAL, "%s: entities[%u] is in Depth mode", call, j);
+        if (ents[j].rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW)
+            return fail(c, BGS_EINVAL, "%s: entities[%u] is in OpticalFlow mode", call, j);
+    }
+    if ((frame->flags & BGS_FLAG_BLEND_OVER_TARGET) && !out_is_device_ptr)
+        return fail(c, BGS_EINVAL, "%s: BGS_FLAG_BLEND_OVER_TARGET takes device targets", call);
+    if (v == 1)
+        return bgs_render_entities_ex(c, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, out_rgba[0], out_format,
+                                      out_is_device_ptr);
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, nullptr,
+                                out_format, out_is_device_ptr, false, nullptr, nullptr, v, out_rgba);
 }
 
 bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,

@@ -44,12 +44,25 @@ __device__ __forceinline__ void block_sum_prefix3(const uint32_t* cnt3, uint32_t
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(BIN_THREADS)
-bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ perm, FrameCounters* __restrict__ ctr,
-                     ChunkCounters* __restrict__ cc, uint32_t frac_a, uint32_t frac_b, uint32_t num_tiles_total,
-                     uint32_t* __restrict__ block_cnt /* [grid][3] */, int tiles_x, uint32_t capacity, uint32_t* __restrict__ pair_keys,
-                     uint32_t* __restrict__ pair_vals, uint32_t* __restrict__ q_rank, uint32_t* __restrict__ q_off,
-                     uint32_t q_cap, uint32_t* __restrict__ sticky_need) {
+// VIEWS (bgs_render_views): a splat's tile ids are its view's, tile0[i] + ty tiles_x(i) + tx; its view is its global
+// index's (slot_ids[record index] / n_view), looked up where the pairs are written: by the owning thread, and for the
+// medium and large queues by the warp that drains the entry.  (A one-view frame has tile0 = 0 and tiles_x.)
+template <bool VIEWS>
+__device__ __forceinline__ void bin_emit_body(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ perm,
+                                              FrameCounters* __restrict__ ctr, ChunkCounters* __restrict__ cc, uint32_t frac_a,
+                                              uint32_t frac_b, uint32_t num_tiles_total, uint32_t* __restrict__ block_cnt,
+                                              int tiles_x, uint32_t capacity, uint32_t* __restrict__ pair_keys,
+                                              uint32_t* __restrict__ pair_vals, uint32_t* __restrict__ q_rank,
+                                              uint32_t* __restrict__ q_off, uint32_t q_cap, uint32_t* __restrict__ sticky_need,
+                                              const uint32_t* __restrict__ slot_ids, const ViewTable* vt) {
+    // record index r's first tile id and row length
+    auto tile_base = [&](uint32_t r, uint32_t& base, uint32_t& row) {
+        base = 0u; row = (uint32_t)tiles_x;
+        if constexpr (VIEWS) {
+            const uint32_t i = vt->view_of(__ldg(slot_ids + r));
+            base = vt->tile0[i]; row = (uint32_t)vt->tiles_x[i];
+        }
+    };
     __shared__ uint32_t s_wtot[3][BIN_THREADS / 32];
     __shared__ unsigned long long s_red64[3 * 8];
     __shared__ uint32_t s_tot[3];
@@ -181,11 +194,12 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
             } else {
                 const uint32_t txlo = (bx[j] & 0xFFFFu) >> 4, txhi = (bx[j] >> 16) >> 4;
                 const uint32_t tylo = (by[j] & 0xFFFFu) >> 4, tyhi = (by[j] >> 16) >> 4;
-                uint32_t o = off;
+                uint32_t o = off, kb, kx;
+                tile_base(ri[j], kb, kx);
                 for (uint32_t ty = tylo; ty <= tyhi; ++ty)
                     for (uint32_t tx = txlo; tx <= txhi; ++tx) {
                         if (o < capacity) {
-                            pair_keys[o] = ty * (uint32_t)tiles_x + tx;
+                            pair_keys[o] = kb + ty * kx + tx;
                             pair_vals[o] = ri[j];
                         }
                         ++o;
@@ -220,11 +234,13 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
             const uint32_t r = __shfl_sync(0xffffffffu, m_ri, sI), off = __shfl_sync(0xffffffffu, m_off, sI);
             const uint32_t txlo = __shfl_sync(0xffffffffu, m_txlo, sI), tylo = __shfl_sync(0xffffffffu, m_tylo, sI);
             const uint32_t w = __shfl_sync(0xffffffffu, m_w, sI);
+            uint32_t kb, kx;
+            tile_base(r, kb, kx);
             for (uint32_t k = lane; k < total; k += 32) {
                 const uint32_t o = off + k;
                 if (o < capacity) {
                     const uint32_t qy = k / w;
-                    pair_keys[o] = (tylo + qy) * (uint32_t)tiles_x + (txlo + (k - qy * w));
+                    pair_keys[o] = kb + (tylo + qy) * kx + (txlo + (k - qy * w));
                     pair_vals[o] = r;
                 }
             }
@@ -253,16 +269,40 @@ bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restri
         const uint32_t total = min(total_all, i0 + per);
         uint32_t ty = tylo + (i0 + (uint32_t)lane) / w, tx = txlo + (i0 + (uint32_t)lane) % w;
         const uint32_t dy = 32u / w, dxr = 32u % w;
+        uint32_t kb, kx;
+        tile_base(r, kb, kx);
         for (uint32_t i = i0 + lane; i < total; i += 32) {
             const uint32_t o = off + i;
             if (o < capacity) {
-                pair_keys[o] = ty * (uint32_t)tiles_x + tx;
+                pair_keys[o] = kb + ty * kx + tx;
                 pair_vals[o] = r;
             }
             ty += dy; tx += dxr;
             if (tx > txhi) { tx -= w; ++ty; }
         }
     }
+}
+
+__global__ void __launch_bounds__(BIN_THREADS)
+bin_emit_coop_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ perm, FrameCounters* __restrict__ ctr,
+                     ChunkCounters* __restrict__ cc, uint32_t frac_a, uint32_t frac_b, uint32_t num_tiles_total,
+                     uint32_t* __restrict__ block_cnt /* [grid][3] */, int tiles_x, uint32_t capacity, uint32_t* __restrict__ pair_keys,
+                     uint32_t* __restrict__ pair_vals, uint32_t* __restrict__ q_rank, uint32_t* __restrict__ q_off,
+                     uint32_t q_cap, uint32_t* __restrict__ sticky_need) {
+    bin_emit_body<false>(recs, perm, ctr, cc, frac_a, frac_b, num_tiles_total, block_cnt, tiles_x, capacity, pair_keys, pair_vals,
+                         q_rank, q_off, q_cap, sticky_need, nullptr, nullptr);
+}
+
+// bgs_render_views' binning: one round over every view's splats, each into its own view's tiles
+__global__ void __launch_bounds__(BIN_THREADS)
+bin_emit_views_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ perm, FrameCounters* __restrict__ ctr,
+                      ChunkCounters* __restrict__ cc, uint32_t num_tiles_total, uint32_t* __restrict__ block_cnt,
+                      uint32_t capacity, uint32_t* __restrict__ pair_keys, uint32_t* __restrict__ pair_vals,
+                      uint32_t* __restrict__ q_rank, uint32_t* __restrict__ q_off, uint32_t q_cap,
+                      uint32_t* __restrict__ sticky_need, const uint32_t* __restrict__ slot_ids,
+                      const __grid_constant__ ViewTable vt) {
+    bin_emit_body<true>(recs, perm, ctr, cc, 0u, 65536u, num_tiles_total, block_cnt, 0, capacity, pair_keys, pair_vals, q_rank,
+                        q_off, q_cap, sticky_need, slot_ids, &vt);
 }
 
 int bin_coop_blocks_per_sm() {
@@ -278,6 +318,23 @@ cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, Fra
                     (void*)&block_cnt, (void*)&tiles_x, (void*)&capacity, (void*)&pair_keys,
                     (void*)&pair_vals, (void*)&q_rank, (void*)&q_off, (void*)&q_cap, (void*)&sticky_need};
     return cudaLaunchCooperativeKernel((const void*)bin_emit_coop_kernel, dim3(grid), dim3(BIN_THREADS), args, 0, stream);
+}
+cudaError_t launch_bin_emit_views(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
+                                  uint32_t num_tiles_total, uint32_t* block_cnt, uint32_t capacity, uint32_t* pair_keys,
+                                  uint32_t* pair_vals, uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, uint32_t grid,
+                                  uint32_t* sticky_need, const uint32_t* slot_ids, const ViewTable& vt, int sm_count,
+                                  cudaStream_t stream) {
+    // (the grid is planned for bin_emit_coop_kernel: no larger than this kernel's co-resident CTAs)
+    static const int per_sm = [] {
+        int b = 0;
+        return cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, bin_emit_views_kernel, BIN_THREADS, 0) == cudaSuccess ? b : 0;
+    }();
+    if (per_sm == 0) return cudaErrorNotSupported;
+    grid = grid < (uint32_t)(per_sm * sm_count) ? grid : (uint32_t)(per_sm * sm_count);
+    void* args[] = {(void*)&recs, (void*)&perm, (void*)&ctr, (void*)&cc, (void*)&num_tiles_total, (void*)&block_cnt,
+                    (void*)&capacity, (void*)&pair_keys, (void*)&pair_vals, (void*)&q_rank, (void*)&q_off, (void*)&q_cap,
+                    (void*)&sticky_need, (void*)&slot_ids, (void*)&vt};
+    return cudaLaunchCooperativeKernel((const void*)bin_emit_views_kernel, dim3(grid), dim3(BIN_THREADS), args, 0, stream);
 }
 
 }  // namespace bgs

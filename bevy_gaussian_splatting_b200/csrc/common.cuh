@@ -109,6 +109,32 @@ struct SegmentKinds {
     uint32_t kind[BGS_SCENE_MAX_CLOUDS];
 };
 
+// A views frame (bgs_render_views): v views of one entity list.  View i owns segments i k .. i k + k - 1 and the global
+// indices [i n_view, (i + 1) n_view), and the global tile ids [tile0[i], tile0[i + 1]), row-major in its own
+// tiles_x x tiles_y grid.  Binning reads the tile geometry; the blend also the view's size, target and depth buffer (scene
+// NULL: no depth test).  Taken by value (__grid_constant__, ~2.8 KB of kernel parameters) like the segment table.
+constexpr uint32_t MAX_VIEWS = BGS_SCENE_MAX_CLOUDS;
+struct ViewTable {
+    uint32_t v;                 // views, 2 .. MAX_VIEWS (0: not a views frame)
+    uint32_t n_view;            // global indices per view (the entity list's N)
+    uint32_t tile0[MAX_VIEWS + 1];   // tile0[v] = every view's tiles
+    int W[MAX_VIEWS], H[MAX_VIEWS], tiles_x[MAX_VIEWS], tiles_y[MAX_VIEWS];
+    void* out[MAX_VIEWS];
+    const float* scene[MAX_VIEWS];
+    size_t pitch[MAX_VIEWS];
+    // the view of global index g < v n_view
+    __device__ __forceinline__ uint32_t view_of(uint32_t g) const { return g / n_view; }
+    // the view of global tile b < tile0[v]: the last i with tile0[i] <= b
+    __device__ __forceinline__ uint32_t view_of_tile(uint32_t b) const {
+        uint32_t lo = 0u, hi = v;
+        while (hi - lo > 1u) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (tile0[mid] <= b) lo = mid; else hi = mid;
+        }
+        return lo;
+    }
+};
+
 // Projected splat record, 48 B, stored by front-to-back rank.
 struct __align__(16) SplatRec {
     float cx, cy, ux, uy;       // centre (px), first row of the pixel-offset -> uv map

@@ -78,6 +78,9 @@ struct SceneFacts {
     int raster_mode = 0;
     SegmentKinds kinds = {};
     bool box = false;
+    // a views frame (bgs_render_views, views.v > 1): the table has views.v x k segments, segment i k + j entity j seen from
+    // view i; the views' tile geometry and depth buffers (their targets are the frame's, filled in when it is enqueued)
+    ViewTable views = {};
 };
 
 // What the host knows of a frame it has enqueued: the context keeps the last one enqueued (`pend`) and, once its
@@ -89,7 +92,7 @@ struct FrameFacts {
     bool sort_all = false;
     bool by_slot = false;               // records indexed by compact slot (else by front-to-back rank)
     int rounds = 1;                     // binning rounds
-    int tiles_x = 0, tiles_y = 0, W = 0, H = 0;
+    int tiles_x = 0, tiles_y = 0, W = 0, H = 0;   // (a views frame: every view's tiles x 1, view 0's W x H)
     const void* target = nullptr;       // the device frame the blend wrote
     bool depth_tested = false;          // bgs_render_depth_test with a depth buffer: splat_depth holds the splats' d
     std::shared_ptr<const SceneFacts> scene;   // bgs_render_scene frames only (nulled with `cloud`)

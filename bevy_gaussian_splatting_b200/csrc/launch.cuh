@@ -63,6 +63,12 @@ cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, Fra
                                  int tiles_x, uint32_t capacity, uint32_t* pair_keys, uint32_t* pair_vals,
                                  uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, uint32_t grid,
                                  uint32_t* sticky_need, cudaStream_t stream);
+// bgs_render_views: one round, each splat into its view's tiles (slot_ids: compact slot -> global index)
+cudaError_t launch_bin_emit_views(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
+                                  uint32_t num_tiles_total, uint32_t* block_cnt, uint32_t capacity, uint32_t* pair_keys,
+                                  uint32_t* pair_vals, uint32_t* q_rank, uint32_t* q_off, uint32_t q_cap, uint32_t grid,
+                                  uint32_t* sticky_need, const uint32_t* slot_ids, const ViewTable& vt, int sm_count,
+                                  cudaStream_t stream);
 // scene_depth.cu
 void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                         const FrameConsts& fc, float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
@@ -85,6 +91,11 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
 // a mixed-geometry frame's blend kind of each compact slot (records n_vis of ctr), from its segment's
 void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
                           uint32_t n_hint, int sm_count, cudaStream_t stream);
+// bgs_render_views' blend: one CTA per global tile of every view (vt.tile0[vt.v]), each into its view's target; mode and box
+// as launch_raster's; splat_d non-null and vt.scene[i]: the depth test against view i's buffer
+void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
+                         uint32_t format, const uint32_t* truncated, const float* splat_d, const unsigned char* kinds, bool box,
+                         const ViewTable& vt, cudaStream_t stream);
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
                          uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,

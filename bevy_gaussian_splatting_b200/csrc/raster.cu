@@ -259,14 +259,17 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // the depth test) on its quad's edge band (box_edge) blends (0.3, 1, 0.1) at alpha 1 into every frame it writes, which
 // stops the pixel; other pairs blend as without it.  Mixed frames read the overlay bit of each splat from bit 2 of its
 // kinds byte (its entity's), the others draw every splat's box.  MODE 0 takes the generic loop, not the inline-asm one.
-template <int MODE, bool AUX, bool ZTEST, bool BOX = false>
+// VIEWS (raster_views_kernel, bgs_render_views): the CTA's global tile blockIdx.x lies in view i = vt->view_of_tile; W, H,
+// tiles_x, out, scene and pitch are then view i's, the CTA takes the local tile blockIdx.x - tile0[i] in centre_out_tile's
+// order within the view, and reads the global tile's range.
+template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false>
 __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
                                             const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
                                             int H, int tiles_x, void* __restrict__ out, uint32_t format,
                                             const float4* __restrict__ aux, void* __restrict__ out_depth,
                                             void* __restrict__ out_normal, const uint32_t* __restrict__ truncated,
                                             const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
-                                            const unsigned char* __restrict__ kinds) {
+                                            const unsigned char* __restrict__ kinds, const ViewTable* vt = nullptr) {
     constexpr bool MIXED = MODE >= 3, SURF = MODE == 2 || MODE == 4;
     __shared__ __align__(16) unsigned char s_mem[(SURF ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0) +
                                                  (ZTEST && !AUX ? ZT_BYTES : 0)];
@@ -285,9 +288,17 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
     unsigned short* s_list = reinterpret_cast<unsigned short*>(s_mem + SM_LIST) + warp * RT_CHUNK;
     const uint32_t a_base = (uint32_t)__cvta_generic_to_shared(s_mem);
     const uint32_t a_list = a_base + SM_LIST + (uint32_t)warp * RT_CHUNK * 2u;
-    int tile_x, tile_y;
-    centre_out_tile((int)blockIdx.x, tiles_x, (int)gridDim.x / tiles_x, tile_x, tile_y);
-    const int tile = tile_y * tiles_x + tile_x;
+    int tile_x, tile_y, tile;
+    if constexpr (VIEWS) {
+        const uint32_t i = vt->view_of_tile(blockIdx.x);
+        W = vt->W[i]; H = vt->H[i]; tiles_x = vt->tiles_x[i]; out = vt->out[i];
+        if (ZTEST) { scene = vt->scene[i]; pitch = vt->pitch[i]; }
+        centre_out_tile((int)(blockIdx.x - vt->tile0[i]), tiles_x, vt->tiles_y[i], tile_x, tile_y);
+        tile = (int)vt->tile0[i] + tile_y * tiles_x + tile_x;
+    } else {
+        centre_out_tile((int)blockIdx.x, tiles_x, (int)gridDim.x / tiles_x, tile_x, tile_y);
+        tile = tile_y * tiles_x + tile_x;
+    }
     // warp w covers the 8x4 rectangle at ((w & 1) * 8, (w >> 1) * 4) of the tile
     const int wx0 = tile_x * TILE_PX + (warp & 1) * 8, wy0 = tile_y * TILE_PX + (warp >> 1) * 4;
     const int px = wx0 + (lane & 7), py = wy0 + (lane >> 3);
@@ -604,6 +615,18 @@ raster_mixed_aux_kernel(const SplatRec* __restrict__ recs, const float4* __restr
                                         out_normal, truncated, splat_d, scene, pitch, kinds);
 }
 
+// bgs_render_views' blends: raster_kernel's (MODE 0..2), raster_mixed_kernel's (3, 4) and their BOX kernels', each CTA on
+// its view's tile (raster_body's VIEWS).  (MODE 0 spills at 6 CTAs per SM; the mixed depth-tested blends, the depth-tested
+// overlay and MODE 4's overlay at 5.)
+template <int MODE, bool ZTEST, bool BOX>
+__global__ void __launch_bounds__(RT_THREADS, (ZTEST && (MODE >= 3 || BOX)) || (BOX && MODE == 4) ? 4 : 5)
+raster_views_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
+                    const uint2* __restrict__ ranges, uint32_t format, const uint32_t* __restrict__ truncated,
+                    const float* __restrict__ splat_d, const unsigned char* __restrict__ kinds, const __grid_constant__ ViewTable vt) {
+    raster_body<MODE, false, ZTEST, BOX, true>(recs, extra, tile_entries, ranges, 0, 0, 0, nullptr, format, nullptr, nullptr,
+                                               nullptr, truncated, splat_d, nullptr, 0, kinds, &vt);
+}
+
 // the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
 __global__ void raster_kinds_kernel(SegmentKinds sk, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
                                     unsigned char* __restrict__ out) {
@@ -863,6 +886,20 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
     kernels[row][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
         recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated, zt.splat_d,
         zt.scene, zt.pitch);
+}
+
+void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
+                         uint32_t format, const uint32_t* truncated, const float* splat_d, const unsigned char* kinds, bool box,
+                         const ViewTable& vt, cudaStream_t stream) {
+    using Kernel = void (*)(const SplatRec*, const float4*, const uint32_t*, const uint2*, uint32_t, const uint32_t*,
+                            const float*, const unsigned char*, const ViewTable);
+#define VIEWS_ROW_(Z, B) {raster_views_kernel<0, Z, B>, raster_views_kernel<1, Z, B>, raster_views_kernel<2, Z, B>, \
+                          raster_views_kernel<3, Z, B>, raster_views_kernel<4, Z, B>}
+    static const Kernel kernels[2][2][5] = {{VIEWS_ROW_(false, false), VIEWS_ROW_(false, true)},
+                                            {VIEWS_ROW_(true, false), VIEWS_ROW_(true, true)}};
+#undef VIEWS_ROW_
+    kernels[splat_d != nullptr][box][mode]<<<vt.tile0[vt.v], RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, format,
+                                                                                     truncated, splat_d, kinds, vt);
 }
 
 // One front-to-back round of a chunked frame (quad-uv records only); see raster2_kernel.

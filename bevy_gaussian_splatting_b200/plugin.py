@@ -296,6 +296,23 @@ def check_entities_aux(entities) -> CloudSettings:
     return first
 
 
+def check_views(entities, views) -> CloudSettings:
+    """`check_entities` for one bgs_render_views call of `views` (a sequence of View), which also raises ValueError when
+    there are no views, when views x entities exceeds abi.BGS_SCENE_MAX_CLOUDS segments, and for an entity in Depth mode
+    (its colour range would be per view) or OpticalFlow mode (one previous view per frame)."""
+    entities, views = list(entities), list(views)
+    first = check_entities(entities)
+    if not views:
+        raise ValueError("render_views: no views")
+    if len(views) * len(entities) > abi.BGS_SCENE_MAX_CLOUDS:
+        raise ValueError(f"render_views: {len(views)} views x {len(entities)} entities, at most {abi.BGS_SCENE_MAX_CLOUDS} segments")
+    for j, (_, st, _) in enumerate(entities):
+        mode = RasterizeMode(st.rasterize_mode)
+        if mode in (RasterizeMode.Depth, RasterizeMode.OpticalFlow):
+            raise ValueError(f"render_views: entity {j} is in {mode.name} mode")
+    return first
+
+
 def entity_settings(settings: CloudSettings) -> abi.bgs_entity_settings:
     """One entity's bgs_entity_settings."""
     s = settings.to_abi()
@@ -461,6 +478,34 @@ class GaussianSplattingPlugin:
         zd = self._scene_depth(scene_depth, view)
         self._check(self._lib.bgs_render_entities_aux(self._ctx, *args, None if zd is None else C.byref(zd), *(_ptr(o) for o in outs),
                                                       code, 0))
+        return outs
+
+    def render_views(self, entities, views, fmt: str = "rgba32f", scene_depths=None, asynchronous: bool = False,
+                     premultiplied: bool = False, outs=None) -> list[np.ndarray]:
+        """`render_entities` of every view in `views` (a sequence of View) in ONE frame (`bgs_render_views`): returns one
+        (H_i, W_i, 4) host frame per view, each byte for byte `render_entities`' frame of that view.  Stereo eyes, cube-map
+        faces or split-screen cameras share one key-gen, sort, projection, binning and blend.  `scene_depths`: one depth
+        buffer per view (as `render_view`'s `scene_depth`), or None.  `outs`: the host frames to fill (one per view).
+        `asynchronous`: only enqueue the frame; the frames are filled once `sync()` returns.  Validates with `check_views`
+        (ValueError before any call)."""
+        entities, views = list(entities), list(views)
+        first = check_views(entities, views)
+        code, dtype, ch = self.FORMATS[fmt]
+        if outs is None:
+            outs = [np.empty((v.height, v.width, ch), dtype) for v in views]
+        assert len(outs) == len(views)
+        for o, v in zip(outs, views):
+            assert o.dtype == dtype and o.size == v.height * v.width * ch and o.flags.c_contiguous
+        clouds, unis, ents, eflags, k, _, s, _ = self._entities_args(entities, first, views[0], None, None, asynchronous,
+                                                                     premultiplied, False)
+        n = len(views)
+        vs = (abi.bgs_view * n)(*[v.to_abi() for v in views])
+        zds = None
+        if scene_depths is not None:
+            assert len(scene_depths) == n
+            zds = (abi.bgs_scene_depth * n)(*[self._scene_depth(d, v) for d, v in zip(scene_depths, views)])
+        targets = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        self._check(self._lib.bgs_render_views(self._ctx, clouds, unis, ents, eflags, k, vs, n, s, zds, targets, code, 0))
         return outs
 
     def _entities_args(self, entities, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over):

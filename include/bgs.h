@@ -764,6 +764,44 @@ bgs_status bgs_render_entities_aux(bgs_context* ctx, const bgs_cloud* const* clo
                                    void* out_rgba, void* out_depth, void* out_normal, uint32_t out_format,
                                    int out_is_device_ptr);
 
+/* bgs_render_entities_ex of several views of one scene in ONE frame: stereo eyes, the six faces of a cube map, split-screen
+ * and picture-in-picture cameras, or many cameras of a dataset share one key-gen, depth sort, projection, binning,
+ * tile-id sort and blend launch instead of one set of launches per view (the reference renders every GaussianCamera).
+ *
+ * The rule, exactly:
+ *   Per-view identity.  out_rgba[i] is byte for byte the frame bgs_render_entities_ex(clouds, uniforms, entities,
+ *     entity_flags, k, &views[i], frame, NULL, depths ? &depths[i] : NULL, out_rgba[i], out_format, out_is_device_ptr)
+ *     produces: in all three formats, with BGS_FLAG_PREMULTIPLIED_OUT, per-entity and frame-wide bounding-box overlays,
+ *     and under each view's own depth buffer.  With BGS_FLAG_BLEND_OVER_TARGET each device target is blended over its own
+ *     pixels.  Views may differ in size, and a view's size need not be a multiple of the tile size.
+ *   Index space.  Segment i k + j is cloud j with uniforms[j] and entities[j], seen from view i; global indices run view
+ *     after view (view i's are [i n, (i + 1) n), n = sum of the clouds' counts).  N = v n must be below 2^30, and
+ *     v k <= BGS_SCENE_MAX_CLOUDS.
+ *   Sort.  One stable depth sort over (key, g) of every view's entries; restricted to view i it is view i's own order.
+ *   Tiles.  View i's tiles are the global tile ids [T_i, T_i + tiles_x(i) tiles_y(i)), T_i the sum over the earlier
+ *     views, each view's in row-major order.  The tile-id sort runs over the global id, with pair_passes(total tiles)
+ *     digit places.
+ *   One round.  A views frame is never split into chunked rounds (BGS_FLAG_CHUNKS is ignored; chunked pixels are
+ *     bit-identical anyway).
+ *   Hooks and stats.  Sorted entries, records (bgs_debug_projected), splat depths and tile entries are in the global index
+ *     and rank space; bgs_debug_tile_ranges writes every view's ranges, view after view.  bgs_frame_stats: n = N, n_visible
+ *     and n_pairs over the whole frame, rounds = 1, tiles_x = every view's tiles and tiles_y = 1 (so a hook buffer sized
+ *     tiles_x x tiles_y holds the ranges), width and height view 0's.
+ *   BGS_FLAG_ASYNC is allowed, with bgs_render_entities_ex's pair-overflow rule.  Host targets: the library's frames hold
+ *     all v frames, and each view is copied out to its out_rgba[i].
+ *   v == 1.  The call is bgs_render_entities_ex: pixels, hooks, stats and launch count.
+ * Launches: those of one bgs_render_entities_ex frame of the same entities, whatever v is.
+ * Refused with BGS_EINVAL, nothing enqueued or written and the previous frame's debug hooks kept: every refusal
+ *   bgs_render_entities_ex makes for some view; v == 0, v k > BGS_SCENE_MAX_CLOUDS or N >= 2^30; a NULL out_rgba or
+ *   out_rgba[i]; a device target not aligned to its pixel; an entity in Depth mode (its colour range would be per
+ *   view); an entity in OpticalFlow mode (one previous view per frame); BGS_FLAG_BLEND_OVER_TARGET with host targets
+ *   (the context's last frame is not v frames).  NULL clouds, uniforms, entities, views or frame -> BGS_NOT_READY. */
+bgs_status bgs_render_views(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                            const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */, uint32_t k,
+                            const bgs_view* views, uint32_t v, const bgs_settings* frame,
+                            const bgs_scene_depth* depths /* v, or NULL */, void* const* out_rgba /* v */,
+                            uint32_t out_format, int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target

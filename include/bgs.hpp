@@ -464,6 +464,40 @@ public:
         check(st);
         return true;
     }
+    // render_entities of each of `views` in one frame (bgs_render_views): out_rgba[i] receives views[i]'s frame, byte for
+    // byte render_entities' frame of that view.  depths: one buffer per view (pitches[i] its row pitch), or empty.  No
+    // extras: Depth and OpticalFlow entities are refused.
+    bool render_views(const std::vector<SceneEntity>& entities, const std::vector<bgs_view>& views,
+                      const std::vector<void*>& out_rgba, uint32_t format = BGS_FORMAT_RGBA8_SRGB,
+                      const std::vector<const float*>& depths = {}, const std::vector<uint64_t>& pitches = {},
+                      bool out_is_device = false, uint32_t extra_flags = 0) {
+        if (entities.empty() || views.empty() || out_rgba.size() != views.size()) check(BGS_EINVAL);
+        if (!depths.empty() && (depths.size() != views.size() || pitches.size() != views.size())) check(BGS_EINVAL);
+        std::vector<const bgs_cloud*> clouds;
+        std::vector<bgs_cloud_uniform> unis;
+        std::vector<bgs_entity_settings> ents;
+        std::vector<uint32_t> eflags;
+        for (const SceneEntity& e : entities) {
+            bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
+            std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
+            clouds.push_back(e.cloud->get());
+            unis.push_back(u);
+            const bgs_settings s = e.settings.to_abi();
+            ents.push_back({s.gaussian_mode, s.rasterize_mode, s.aabb, s.opacity_adaptive_radius, s.draw_mode,
+                            e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
+            eflags.push_back(e.settings.visualize_bounding_box ? (uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX : 0u);
+        }
+        bgs_settings s = entities[0].settings.to_abi(extra_flags);
+        if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
+        std::vector<bgs_scene_depth> zd;
+        for (size_t i = 0; i < depths.size(); ++i) zd.push_back({depths[i], pitches[i]});
+        const bgs_status st = bgs_render_views(ctx_, clouds.data(), unis.data(), ents.data(), eflags.data(),
+                                               (uint32_t)clouds.size(), views.data(), (uint32_t)views.size(), &s,
+                                               zd.empty() ? nullptr : zd.data(), out_rgba.data(), format, out_is_device ? 1 : 0);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
     // Colour + depth + normal frames of one view in one pass (BASELINE.json config 4; bgs_render_aux).
     bool render_view_aux(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view, void* out_rgba,
                          void* out_depth, void* out_normal, uint32_t format = BGS_FORMAT_RGBA8_SRGB, bool out_is_device = false) {
