@@ -124,6 +124,31 @@ class bgs_particle_behavior(C.Structure):
     ]
 
 
+class bgs_khr_accessor(C.Structure):
+    """One KHR_gaussian_splatting attribute's accessor as bgs_cloud_upload_khr reads it (glTF component codes)."""
+    _fields_ = [
+        ("data", C.c_void_p),
+        ("byte_stride", C.c_uint32),
+        ("component_type", C.c_uint32),
+        ("normalized", C.c_uint32),
+        ("components", C.c_uint32),
+    ]
+
+
+class bgs_khr_primitive(C.Structure):
+    """A KHR_gaussian_splatting primitive's accessors; sh[d*d + c] is coefficient c of degree d."""
+    _fields_ = [
+        ("n", C.c_uint32),
+        ("position", bgs_khr_accessor),
+        ("rotation", bgs_khr_accessor),
+        ("scale", bgs_khr_accessor),
+        ("opacity", bgs_khr_accessor),
+        ("color_0", bgs_khr_accessor),
+        ("sh", bgs_khr_accessor * 16),
+        ("sh_degree", C.c_uint32),
+    ]
+
+
 # every symbol include/bgs.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = [
@@ -138,6 +163,7 @@ SYMBOLS = [
     ("bgs_cloud_download_f32_sh", C.c_int, [_P, _P, _P, _P, _P, _P]),
     ("bgs_cloud_download_f16_sh", C.c_int, [_P, _P, _P, _P, _P]),
     ("bgs_cloud_sh_degree", C.c_int, [_P, C.POINTER(C.c_uint32)]),
+    ("bgs_cloud_upload_khr", C.c_int, [_P, C.POINTER(bgs_khr_primitive), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(_P)]),
     ("bgs_cloud_destroy", None, [_P]),
     ("bgs_cloud_select_sparse", C.c_int, [_P, _P, C.c_float, C.c_uint32, C.POINTER(C.c_uint32)]),
     ("bgs_cloud_visibility_get", C.c_int, [_P, _P, _P]),

@@ -67,6 +67,68 @@ cudaError_t copy_rows(void* dst, size_t dst_pitch, const void* src, size_t src_p
     return cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, width, n, kind, q);
 }
 
+// The rest of a new cloud's upload: its staged planes (the position plane is the cloud's own; the others go to device
+// scratch, the SH plane at whole chunks per gaussian) are written by stage(d), repacked into the gaussian-major blocks the
+// projection gathers, and freed again.  stage returns BGS_OK, or a status it has reported; on any failure the cloud is
+// released and *out stays NULL.
+template <class Stage>
+bgs_status stage_and_repack(bgs_context* ctx, const char* call, bgs_cloud* cl, Stage stage, bgs_cloud** out) {
+    const CloudLayout layout = cl->layout;
+    const uint32_t n = cl->n, sh_degree = cl->sh_degree;
+    void* d[PLANES] = {cl->pos, nullptr, nullptr, nullptr, nullptr};
+    cudaError_t e = cudaSuccess;
+    for (int p = PLANE_SH; p < PLANES && e == cudaSuccess; ++p)
+        if (plane_bytes(layout, sh_degree, p)) e = cudaMalloc(&d[p], (size_t)n * staged_bytes(layout, sh_degree, p));
+    bgs_status st = BGS_OK;
+    if (e == cudaSuccess) st = stage(d);
+    if (e == cudaSuccess && st == BGS_OK) {
+        launch_repack(layout, sh_degree, d[PLANE_SH], d[PLANE_ROT], d[PLANE_SO], d[PLANE_TT], n, cl->view(), ctx->stream);
+        e = cudaStreamSynchronize(ctx->stream);
+    }
+    for (int p = PLANE_SH; p < PLANES; ++p) cudaFree(d[p]);
+    if (e != cudaSuccess) return drop_cloud(ctx, call, cl, e);
+    if (st != BGS_OK) {
+        bgs_cloud_destroy(cl);
+        return st;
+    }
+    *out = cl;
+    return BGS_OK;
+}
+
+struct KhrSlot {
+    const char* name;
+    const bgs_khr_accessor* a;
+};
+
+uint32_t khr_component_bytes(uint32_t type) {
+    return type == KHR_I8 || type == KHR_U8 ? 1u : type == KHR_I16 || type == KHR_U16 ? 2u : type == KHR_F32 ? 4u : 0u;
+}
+
+// the (components, component type, normalised) combinations each slot accepts (scene.rs:1590-1960); sh: the SH slots
+bool khr_accepted(const KhrSlot& s, bool sh) {
+    const bgs_khr_accessor& a = *s.a;
+    const uint32_t t = a.component_type, c = a.components;
+    const bool f32 = t == KHR_F32, norm = a.normalized != 0;
+    if (sh || !strcmp(s.name, "POSITION")) return c == 3 && f32;
+    if (!strcmp(s.name, "ROTATION")) return c == 4 && (f32 || ((t == KHR_I8 || t == KHR_I16) && norm));
+    if (!strcmp(s.name, "SCALE")) return c == 3 && (f32 || t == KHR_I8 || t == KHR_I16);
+    if (!strcmp(s.name, "OPACITY")) return c == 1 && (f32 || ((t == KHR_U8 || t == KHR_U16) && norm));
+    return (c == 3 || c == 4) && (f32 || t == KHR_U8 || t == KHR_U16);   // COLOR_0
+}
+
+bgs_status khr_check(bgs_context* c, const KhrSlot& s, bool sh) {
+    const bgs_khr_accessor& a = *s.a;
+    if (!a.data) return fail(c, BGS_EINVAL, "upload_khr: %s has no data", s.name);
+    if (!khr_accepted(s, sh))
+        return fail(c, BGS_EINVAL, "upload_khr: %s does not accept %u components of component type %u (normalized %u)", s.name,
+                    a.components, a.component_type, a.normalized);
+    const uint32_t cb = khr_component_bytes(a.component_type);
+    if (a.byte_stride < cb * a.components || a.byte_stride % cb)
+        return fail(c, BGS_EINVAL, "upload_khr: %s byte_stride %u is below its element size %u or not a multiple of %u", s.name,
+                    a.byte_stride, cb * a.components, cb);
+    return BGS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -83,26 +145,17 @@ static bgs_status upload_common(bgs_context* ctx, uint32_t n, CloudLayout layout
     CU(ctx, cudaSetDevice(ctx->device));
     bgs_cloud* cl = nullptr;
     TRY(new_cloud(ctx, "cloud upload", n, layout, sh_degree, &cl));
-    // the position plane is the cloud's own; the other planes go to device scratch (the SH plane at whole chunks per
-    // gaussian, the rest of each last chunk zero), are repacked into the gaussian-major blocks the projection gathers,
-    // and are freed again
-    void* d[PLANES] = {cl->pos, nullptr, nullptr, nullptr, nullptr};
-    cudaError_t e = cudaSuccess;
-    for (int p = 0; p < PLANES && e == cudaSuccess; ++p) {
-        const size_t width = plane_bytes(layout, sh_degree, p), staged = staged_bytes(layout, sh_degree, p);
-        if (width == 0) continue;
-        if (p != PLANE_POS) e = cudaMalloc(&d[p], (size_t)n * staged);
-        if (e == cudaSuccess && staged != width) e = cudaMemsetAsync(d[p], 0, (size_t)n * staged, ctx->stream);
-        if (e == cudaSuccess) e = copy_rows(d[p], staged, src[p], width, width, n, cudaMemcpyHostToDevice, ctx->stream);
-    }
-    if (e == cudaSuccess) {
-        launch_repack(layout, sh_degree, d[PLANE_SH], d[PLANE_ROT], d[PLANE_SO], d[PLANE_TT], n, cl->view(), ctx->stream);
-        e = cudaStreamSynchronize(ctx->stream);
-    }
-    for (int p = PLANE_SH; p < PLANES; ++p) cudaFree(d[p]);
-    if (e != cudaSuccess) return drop_cloud(ctx, "cloud upload", cl, e);
-    *out = cl;
-    return BGS_OK;
+    // the caller's planes, each staged SH row's last chunk zero past the plane's width
+    return stage_and_repack(ctx, "cloud upload", cl, [&](void* const* d) {
+        cudaError_t e = cudaSuccess;
+        for (int p = 0; p < PLANES && e == cudaSuccess; ++p) {
+            const size_t width = plane_bytes(layout, sh_degree, p), staged = staged_bytes(layout, sh_degree, p);
+            if (width == 0) continue;
+            if (staged != width) e = cudaMemsetAsync(d[p], 0, (size_t)n * staged, ctx->stream);
+            if (e == cudaSuccess) e = copy_rows(d[p], staged, src[p], width, width, n, cudaMemcpyHostToDevice, ctx->stream);
+        }
+        return e == cudaSuccess ? BGS_OK : fail(ctx, status_of(e), "cloud upload: %s", cudaGetErrorString(e));
+    }, out);
 }
 
 bgs_status bgs_cloud_upload_f32(bgs_context* ctx, uint32_t n, const float* pos_vis, const float* sh,
@@ -139,6 +192,79 @@ bgs_status bgs_cloud_upload_4d(bgs_context* ctx, uint32_t n, const float* pos_vi
                                const float* scale_opacity, const float* timestamp_timescale, bgs_cloud** out) {
     return upload_common(ctx, n, CloudLayout::F32x4D, SH_DEGREE_MAX, pos_vis, sh, rotations, scale_opacity, timestamp_timescale,
                          out);
+}
+
+// ---- KHR_gaussian_splatting primitives (khr.cu; the rule: include/bgs.h)
+
+bgs_status bgs_cloud_upload_khr(bgs_context* ctx, const bgs_khr_primitive* prim, uint32_t f16, uint32_t* out_zero_quats,
+                                bgs_cloud** out) {
+    if (!ctx || !out) return BGS_EINVAL;
+    *out = nullptr;
+    if (!prim) return fail(ctx, BGS_EINVAL, "upload_khr: null primitive");
+    const uint32_t n = prim->n, d = prim->sh_degree;
+    if (n == 0 || n >= (1u << 30)) return fail(ctx, BGS_EINVAL, "upload_khr: n must be in [1, 2^30)");
+    if (d > SH_DEGREE_MAX) return fail(ctx, BGS_EINVAL, "upload_khr: sh_degree %u is not in [0, 3]", d);
+    static const char* const kSh[16] = {"SH_DEGREE_0_COEF_0", "SH_DEGREE_1_COEF_0", "SH_DEGREE_1_COEF_1", "SH_DEGREE_1_COEF_2",
+                                        "SH_DEGREE_2_COEF_0", "SH_DEGREE_2_COEF_1", "SH_DEGREE_2_COEF_2", "SH_DEGREE_2_COEF_3",
+                                        "SH_DEGREE_2_COEF_4", "SH_DEGREE_3_COEF_0", "SH_DEGREE_3_COEF_1", "SH_DEGREE_3_COEF_2",
+                                        "SH_DEGREE_3_COEF_3", "SH_DEGREE_3_COEF_4", "SH_DEGREE_3_COEF_5", "SH_DEGREE_3_COEF_6"};
+    // slots 0..3 the required attributes, then COLOR_0 (without SH) or the SH coefficients
+    const bool has_sh = d > 0 || prim->sh[0].data;
+    const uint32_t bands = has_sh ? sh_bands(d) : 0u;
+    std::vector<KhrSlot> slots = {{"POSITION", &prim->position}, {"ROTATION", &prim->rotation}, {"SCALE", &prim->scale},
+                                  {"OPACITY", &prim->opacity}};
+    const bool has_color = !has_sh && prim->color_0.data;
+    if (has_color) slots.push_back({"COLOR_0", &prim->color_0});
+    for (uint32_t k = 0; k < bands; ++k) slots.push_back({kSh[k], &prim->sh[k]});
+    for (size_t s = 0; s < slots.size(); ++s) TRY(khr_check(ctx, slots[s], s >= 4 && has_sh));
+    CU(ctx, cudaSetDevice(ctx->device));
+
+    // one device copy of each accessor's span, each at a 256 B boundary, then the two result words
+    Layout l;
+    std::vector<size_t> off(slots.size()), span(slots.size());
+    for (size_t s = 0; s < slots.size(); ++s) {
+        const bgs_khr_accessor& a = *slots[s].a;
+        span[s] = (size_t)(n - 1) * a.byte_stride + (size_t)khr_component_bytes(a.component_type) * a.components;
+        off[s] = l.add(span[s]);
+    }
+    const size_t o_words = l.add(8);
+    const CloudLayout layout = f16 ? CloudLayout::F16 : CloudLayout::F32;
+    bgs_cloud* cl = nullptr;
+    TRY(new_cloud(ctx, "upload_khr", n, layout, bands ? d : 0u, &cl));
+    StreamScratch scratch(ctx->stream);
+    uint32_t zero_quats = 0;
+    TRY(stage_and_repack(ctx, "upload_khr", cl, [&](void* const* dp) {
+        cudaError_t e = scratch.alloc(l.end);
+        uint8_t* base = static_cast<uint8_t*>(scratch.p);
+        KhrDecode k{};
+        KhrSrc* src[5 + 16] = {&k.position, &k.rotation, &k.scale, &k.opacity, has_color ? &k.color : &k.sh[0]};
+        for (uint32_t j = 1; j < bands; ++j) src[4 + j] = &k.sh[j];
+        for (size_t s = 0; s < slots.size() && e == cudaSuccess; ++s) {
+            const bgs_khr_accessor& a = *slots[s].a;
+            *src[s] = KhrSrc{base + off[s], a.byte_stride, a.component_type, a.normalized};
+            e = cudaMemcpyAsync(base + off[s], a.data, span[s], cudaMemcpyHostToDevice, ctx->stream);
+        }
+        uint32_t words[2] = {0, 0};
+        uint32_t* d_words = reinterpret_cast<uint32_t*>(base + o_words);
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_words, 0, 8, ctx->stream);
+        if (e == cudaSuccess) {
+            k.n = n; k.bands = bands; k.sh_units = (uint32_t)(staged_bytes(layout, cl->sh_degree, PLANE_SH) / 16);
+            launch_khr_decode(k, f16 != 0, cl->pos, dp[PLANE_SH], dp[PLANE_ROT], dp[PLANE_SO], d_words, ctx->stream);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(words, d_words, 8, cudaMemcpyDeviceToHost, ctx->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        if (e != cudaSuccess) return fail(ctx, status_of(e), "upload_khr: %s", cudaGetErrorString(e));
+        static const char* const kRule[6] = {"POSITION contains non-finite values", "ROTATION is non-finite after normalising",
+                                             "SCALE gives a non-finite exp(scale)", "OPACITY is NaN or outside [0, 1]",
+                                             "an SH coefficient is non-finite", "COLOR_0 contains non-finite values"};
+        for (int b = 0; b < 6; ++b)
+            if (words[0] & (1u << b)) return fail(ctx, BGS_EINVAL, "upload_khr: %s", kRule[b]);
+        zero_quats = words[1];
+        return BGS_OK;
+    }, out));
+    if (out_zero_quats) *out_zero_quats = zero_quats;
+    return BGS_OK;
 }
 
 bgs_status bgs_cloud_sh_degree(const bgs_cloud* cl, uint32_t* out) {

@@ -136,4 +136,19 @@ void launch_unpack(CloudLayout layout, uint32_t sh_degree, CloudView cloud, uint
                    void* tt /* 4D only */, cudaStream_t stream);
 // interpolate.cu
 void launch_interpolate(CloudLayout layout, uint32_t sh_degree, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream);
+// khr.cu: glTF component codes, the decode's rule bits (words[0]; words[1] counts zero-length quaternions), one accessor
+// as the kernel reads it (its span's device copy), and a primitive's accessors (bands: SH coefficients per channel, 0
+// for none; sh_units: 16 B units of the staged SH plane per gaussian)
+enum : uint32_t { KHR_I8 = 5120, KHR_U8 = 5121, KHR_I16 = 5122, KHR_U16 = 5123, KHR_F32 = 5126 };
+enum : uint32_t { KHR_BAD_POSITION = 1, KHR_BAD_ROTATION = 2, KHR_BAD_SCALE = 4, KHR_BAD_OPACITY = 8, KHR_BAD_SH = 16, KHR_BAD_COLOR = 32 };
+struct KhrSrc {
+    const uint8_t* data;
+    uint32_t stride, type, normalized;
+};
+struct KhrDecode {
+    KhrSrc position, rotation, scale, opacity, color, sh[16];
+    uint32_t n, bands, sh_units;
+};
+// the staged planes of an f32 (so non-null) or f16 (rot: the packed second record) cloud
+void launch_khr_decode(const KhrDecode& k, bool f16, float4* pos, void* sh, void* rot, void* so, uint32_t* words, cudaStream_t stream);
 }  // namespace bgs

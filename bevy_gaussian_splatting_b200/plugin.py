@@ -14,6 +14,7 @@ from __future__ import annotations
 import ctypes as C
 import dataclasses
 import os
+import warnings
 
 import numpy as np
 
@@ -114,9 +115,9 @@ class PlanarGaussian3dHandle:
 
     @classmethod
     def _adopt(cls, plugin: "GaussianSplattingPlugin", h: C.c_void_p, n: int, f16: bool,
-               precompute_covariance: bool) -> "PlanarGaussian3dHandle":
-        """A handle owning a `bgs_cloud*` the library made (bgs_cloud_subset); its Aabb is computed from the positions,
-        as `calculate_bounds` would compute it for the cloud once saved and loaded."""
+               precompute_covariance: bool, aabb=None) -> "PlanarGaussian3dHandle":
+        """A handle owning a `bgs_cloud*` the library made (bgs_cloud_subset, _upload_khr); its Aabb is `aabb`, or computed
+        from the positions read back, as `calculate_bounds` would compute it for the cloud once saved and loaded."""
         self = cls.__new__(cls)
         PlanarGaussian3dHandle._next_serial += 1
         self.serial = PlanarGaussian3dHandle._next_serial
@@ -126,7 +127,7 @@ class PlanarGaussian3dHandle:
         d = C.c_uint32()
         plugin._check(plugin._lib.bgs_cloud_sh_degree(h, C.byref(d)))
         self.sh_degree = int(d.value)
-        self.aabb = compute_aabb(plugin.positions(self))
+        self.aabb = compute_aabb(plugin.positions(self)) if aabb is None else aabb
         return self
 
     def destroy(self):
@@ -185,6 +186,25 @@ class ParticleBehaviorsHandle:
             self.destroy()
         except Exception:
             pass
+
+
+@dataclasses.dataclass
+class SceneHandles:
+    """A KHR_gaussian_splatting scene resident on one GPU (`GaussianSplattingPlugin.add_scene`): one handle per primitive,
+    shared by every node that places it, the scene's bundles and how many zero-length rotations each primitive had."""
+
+    handles: list
+    bundles: list
+    zero_quats: list
+
+    def entities(self) -> list:
+        """(handle, settings, transform) per bundle: the entity list `render_entities`, `render_entities_aux` and
+        `render_views` take."""
+        return [(self.handles[b.primitive], b.settings, b.transform) for b in self.bundles]
+
+    def destroy(self):
+        for h in self.handles:
+            h.destroy()
 
 
 # CloudSettings fields a bgs_render_scene call takes from each entity (into its bgs_cloud_uniform); every other field is
@@ -345,6 +365,48 @@ class GaussianSplattingPlugin:
                 raise ValueError("add_cloud: a Gaussian4d cloud is stored in f32 only")
             return PlanarGaussian4dHandle(self, cloud)
         return PlanarGaussian3dHandle(self, cloud, f16, precompute_covariance)
+
+    def add_scene(self, scene, f16: bool = False) -> SceneHandles:
+        """A loaded KHR_gaussian_splatting scene (`B.load_scene`) made resident: each primitive is decoded on the GPU
+        (`bgs_cloud_upload_khr`) into one cloud at its SH degree, f32 or f16, which every node placing it shares (a mesh
+        placed by k nodes is one cloud and k entities).  Each handle's Aabb comes from the primitive's POSITION values.
+        Zero-length rotations become the identity with a warning, as in the reference; a value the reference refuses
+        raises BgsError (BGS_EINVAL) and leaves no cloud behind."""
+        handles, zero_quats = [], []
+        try:
+            for prim in scene.primitives:
+                h, zq, p = C.c_void_p(), C.c_uint32(), prim.to_abi()
+                self._check(self._lib.bgs_cloud_upload_khr(self._ctx, C.byref(p), int(f16), C.byref(zq), C.byref(h)))
+                handles.append(PlanarGaussian3dHandle._adopt(self, h, prim.n, f16, False,
+                                                             aabb=compute_aabb(prim.position.array())))
+                zero_quats.append(int(zq.value))
+                if zq.value:
+                    warnings.warn(f"mesh {prim.mesh} primitive {prim.primitive}: attribute 'KHR_gaussian_splatting:ROTATION' "
+                                  f"contained {zq.value} zero-length quaternions; replacing them with identity rotations")
+        except Exception:
+            for h in handles:
+                h.destroy()
+            raise
+        return SceneHandles(handles, list(scene.bundles), zero_quats)
+
+    def save_scene(self, path, entities, cameras=(), names=None, metadata=None) -> None:
+        """The reference's "G to save" for clouds resident here: `entities` (handle, settings, transform) -- e.g.
+        `SceneHandles.entities()` after a selection edit, a subset or a particle step -- written by `B.write_scene` with
+        `cameras` (SceneCamera), each distinct handle downloaded once.  `names` / `metadata`: per entity (default
+        "cloud{j}" / the default extension values).  Gaussian4d and precomputed-covariance clouds raise ValueError."""
+        from .khr import SceneExportCloud, write_scene
+
+        entities = list(entities)
+        clouds = {}
+        for h, _, _ in entities:
+            if is_4d_handle(h) or getattr(h, "precompute_covariance", False):
+                raise ValueError("save_scene: Gaussian4d and precomputed-covariance clouds have no KHR_gaussian_splatting form")
+            if h.serial not in clouds:
+                clouds[h.serial] = self.download(h)
+        names = names or [f"cloud{j}" for j in range(len(entities))]
+        metadata = metadata or [None] * len(entities)
+        write_scene(path, [SceneExportCloud(clouds[h.serial], nm, st, tr, md)
+                           for (h, st, tr), nm, md in zip(entities, names, metadata)], cameras)
 
     def _check(self, st: int):
         if st != abi.BGS_OK:

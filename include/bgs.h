@@ -205,6 +205,49 @@ bgs_status bgs_cloud_download_f16_sh(bgs_context* ctx, const bgs_cloud* cloud, f
                                      uint32_t* sh_packed /* n * S_d / 2 */, uint32_t* second_plane /* n*4 */);
 bgs_status bgs_cloud_sh_degree(const bgs_cloud* cloud, uint32_t* out);
 
+/* A KHR_gaussian_splatting glTF primitive decoded into a resident cloud on the GPU (the reference's scene loader,
+ * src/io/scene.rs).  The caller parses the glTF and describes each attribute's accessor; the call copies each
+ * accessor's span, (n - 1) * byte_stride + element size bytes from `data`, once to the device, decodes it there and
+ * repacks it as bgs_cloud_upload_f32_sh / _f16_sh (f16 != 0) would from the decoded planes, at sh_degree.
+ *
+ * bgs_khr_accessor: `data` is the host address of element 0, byte_stride the distance between elements (the
+ * bufferView's byteStride, or the element size when tightly packed), component_type the glTF code (5120 i8, 5121 u8,
+ * 5122 i16, 5123 u16, 5126 f32), components 1 (SCALAR), 3 (VEC3) or 4 (VEC4).  Accepted, as the reference accepts them:
+ *   POSITION  VEC3 f32;
+ *   ROTATION  VEC4 f32, or normalised i8 / i16;
+ *   SCALE     VEC3 f32, i8 or i16, normalised or not (a log scale);
+ *   OPACITY   SCALAR f32, or normalised u8 / u16;
+ *   COLOR_0   VEC3 / VEC4 f32, u8 or u16 (u8 / u16 read as normalised whatever `normalized` says; alpha dropped);
+ *   sh[k]     VEC3 f32, coefficient k = d*d + c of degree d, present for every k < (sh_degree + 1)^2.
+ * With sh_degree 0 and sh[0].data NULL the primitive has no SH: the DC coefficients are COLOR_0 / 0.282095 when COLOR_0
+ * is present (its data non-NULL), else 0.  COLOR_0 is ignored when SH are present; sh[k] beyond the degree are ignored.
+ * The decode, every f32 operation round-to-nearest without FMA: a normalised value is max(v / 127, -1), max(v / 32767,
+ * -1), v / 255 or v / 65535; the quaternion, in its stored order, becomes q * (1 / sqrt(((q0 q0 + q1 q1) + q2 q2) +
+ * q3 q3)), or (1, 0, 0, 0) when that sum is <= FLT_EPSILON (such quaternions are counted in *out_zero_quats, which may
+ * be NULL); scale = exp(raw) evaluated in f64 and rounded once to f32; position w = 1; f16 clouds round each value to
+ * nearest even.  The rotation plane holds the four stored lanes in order (the reference reads (1, 0, 0, 0) as identity).
+ * Refused with BGS_EINVAL, naming the attribute, before anything reaches the device: a NULL required accessor, an
+ * unaccepted (components, component_type, normalized), byte_stride below the element size or not a multiple of the
+ * component size, n outside [1, 2^30), sh_degree > 3.  Refused with BGS_EINVAL after the decode, the cloud released and
+ * *out left NULL: a non-finite position, rotation (after normalising), exp(scale), SH coefficient or COLOR_0 value, and
+ * an opacity that is NaN or outside [0, 1].  Synchronous; the context stays usable after any refusal. */
+typedef struct {
+    const void* data;
+    uint32_t byte_stride;
+    uint32_t component_type;
+    uint32_t normalized;
+    uint32_t components;
+} bgs_khr_accessor;
+typedef struct {
+    uint32_t n;
+    bgs_khr_accessor position, rotation, scale, opacity;
+    bgs_khr_accessor color_0; /* optional: data NULL when absent */
+    bgs_khr_accessor sh[16];
+    uint32_t sh_degree;
+} bgs_khr_primitive;
+bgs_status bgs_cloud_upload_khr(bgs_context* ctx, const bgs_khr_primitive* primitive, uint32_t f16, uint32_t* out_zero_quats,
+                                bgs_cloud** out);
+
 /* Selection edits of a resident cloud: the visibility lane (pos_vis[4i + 3]) that DrawMode::Selected and
  * HighlightSelected read, changed in place without a re-upload.  All three calls are synchronous.
  *

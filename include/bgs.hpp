@@ -572,6 +572,17 @@ public:
         }
         return h;
     }
+    // A KHR_gaussian_splatting primitive whose accessors the caller has described (bgs_cloud_upload_khr; this header parses
+    // no glTF), as an f32 cloud.  *zero_quats (optional): how many zero-length rotations became the identity.
+    PlanarGaussian3dHandle upload_khr(const bgs_khr_primitive& primitive, uint32_t* zero_quats = nullptr) {
+        PlanarGaussian3dHandle h;
+        check(bgs_cloud_upload_khr(ctx_, &primitive, 0, zero_quats, &h.h_));
+        h.n_ = primitive.n;
+        PlanarGaussian3d p;
+        p.position_visibility = positions(h);
+        p.compute_aabb(h.aabb_min_, h.aabb_max_);
+        return h;
+    }
     // The cloud's four planes at its SH degree (bgs_cloud_download_f32_sh: this host uploads f32 clouds only).
     PlanarGaussian3d download(const PlanarGaussian3dHandle& cloud) {
         const size_t n = cloud.len();
