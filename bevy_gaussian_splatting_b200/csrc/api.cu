@@ -108,6 +108,7 @@ bgs_status ensure_arena(bgs_context* c, uint32_t tiles) {
     tiles = std::max(tiles, c->arena_tiles);
     Layout l;
     const size_t o_ctr = l.add(sizeof(FrameCounters));
+    const size_t o_vr = l.add(sizeof(ViewRanges));
     const size_t o_hist = l.add((8 + 4 * MAX_CHUNKS) * 256 * 4);
     // (the queued-frame grids are never larger than the synchronous ones)
     const size_t o_kgc = l.add((size_t)c->kg_grid * 4);
@@ -120,6 +121,7 @@ bgs_status ensure_arena(bgs_context* c, uint32_t tiles) {
     const size_t o_done = l.add(chunk_tiles);
     TRY(c->arena.grow(c, l.padded(), false));
     c->ctr = reinterpret_cast<FrameCounters*>(c->arena.p + o_ctr);
+    c->view_ranges = reinterpret_cast<ViewRanges*>(c->arena.p + o_vr);
     c->hist = reinterpret_cast<uint32_t*>(c->arena.p + o_hist);
     c->kg_block_cnt = reinterpret_cast<uint32_t*>(c->arena.p + o_kgc);
     c->bin_block_cnt = reinterpret_cast<uint32_t*>(c->arena.p + o_binc);
@@ -194,11 +196,24 @@ struct FrameOut {
     void* host_rgba = nullptr;          // host frames the result is copied to
     void* host_depth = nullptr;
     void* host_normal = nullptr;
-    // a views frame: view i's device target, host frame (host targets; else NULL) and bytes
+    // a views frame: view i's device targets, host frames (host targets; else NULL) and bytes (of one frame); the depth and
+    // normal ones on aux frames
     uint32_t views = 0;
     void* view_rgba[MAX_VIEWS] = {};
     void* view_host[MAX_VIEWS] = {};
+    void* view_depth[MAX_VIEWS] = {};
+    void* view_normal[MAX_VIEWS] = {};
+    void* view_host_depth[MAX_VIEWS] = {};
+    void* view_host_normal[MAX_VIEWS] = {};
     size_t view_bytes[MAX_VIEWS] = {};
+};
+
+// A views frame's targets: view i's frame into rgba[i] and, on aux frames, its depth and normal frames into depth[i] and
+// normal[i] (NULL arrays otherwise)
+struct ViewTargets {
+    void* const* rgba;
+    void* const* depth;
+    void* const* normal;
 };
 
 // the caller's device frames, or the library's own (grown on demand)
@@ -243,20 +258,30 @@ bgs_status frame_out(bgs_context* c, const bgs_settings* st, uint32_t format, si
 }
 
 // a views frame's targets: the caller's device frames, or the library's frames holding every view, one after another
-// (the targets have passed bgs_render_views' checks)
-bgs_status frame_out_views(bgs_context* c, const bgs_settings* st, uint32_t format, const ViewTable& vt, void* const* targets,
+// (aux frames: frame_aux[0] every view's depth frame, frame_aux[1] every normal frame) (the targets have passed
+// bgs_render_views' or bgs_render_views_aux's checks)
+bgs_status frame_out_views(bgs_context* c, const bgs_settings* st, uint32_t format, const ViewTable& vt, const ViewTargets& t,
                            int out_is_device_ptr, FrameOut* o) {
     const size_t bpp = format_bpp(format);
+    const bool aux = t.depth != nullptr;
     size_t total = 0;
     for (uint32_t i = 0; i < vt.v; ++i) total += (size_t)vt.W[i] * vt.H[i] * bpp;
     TRY(frame_out(c, st, format, out_is_device_ptr ? (size_t)vt.W[0] * vt.H[0] * bpp : total,
-                  out_is_device_ptr ? targets[0] : nullptr, out_is_device_ptr, false, nullptr, nullptr, o));
+                  out_is_device_ptr ? t.rgba[0] : nullptr, out_is_device_ptr, false, nullptr, nullptr, o));
+    if (aux && !out_is_device_ptr)
+        for (int k = 0; k < 2; ++k) TRY(c->frame_aux[k].grow(c, total, true));
     o->views = vt.v;
     size_t at = 0;
     for (uint32_t i = 0; i < vt.v; ++i) {
         o->view_bytes[i] = (size_t)vt.W[i] * vt.H[i] * bpp;
-        o->view_rgba[i] = out_is_device_ptr ? targets[i] : static_cast<char*>(o->rgba) + at;
-        o->view_host[i] = out_is_device_ptr ? nullptr : targets[i];
+        o->view_rgba[i] = out_is_device_ptr ? t.rgba[i] : static_cast<char*>(o->rgba) + at;
+        o->view_host[i] = out_is_device_ptr ? nullptr : t.rgba[i];
+        if (aux) {
+            o->view_depth[i] = out_is_device_ptr ? t.depth[i] : static_cast<char*>(c->frame_aux[0].p) + at;
+            o->view_normal[i] = out_is_device_ptr ? t.normal[i] : static_cast<char*>(c->frame_aux[1].p) + at;
+            o->view_host_depth[i] = out_is_device_ptr ? nullptr : t.depth[i];
+            o->view_host_normal[i] = out_is_device_ptr ? nullptr : t.normal[i];
+        }
         at += o->view_bytes[i];
     }
     return BGS_OK;
@@ -538,8 +563,12 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     //      rank), or Depth colouring / aux frames (by slot), which need the depth range of the sorted set first
     const cudaStream_t ps = p.overlap ? c->stream2 : q;
     if (p.overlap) CU(c, cudaStreamWaitEvent(c->stream2, c->ev_fork, 0));
+    // (a views aux frame: each view's range from its own entries, which its projection reads)
+    const bool view_ranges = views && fc.aux;
     if (p.depth_range) {
-        if (scene) launch_depth_range_scene(scene->tab, c->vals[cur].p, c->slot_ids.p, c->ctr, q);
+        if (view_ranges) launch_depth_range_views(scene->tab, views->v, views->n_view, c->vals[cur].p, c->slot_ids.p, c->ctr,
+                                                  c->view_ranges, p.n_hint, c->sm_count, q);
+        else if (scene) launch_depth_range_scene(scene->tab, c->vals[cur].p, c->slot_ids.p, c->ctr, q);
         else launch_depth_range(cloud->pos, n, c->vals[cur].p, p.by_slot ? c->slot_ids.p : nullptr, c->ctr, fc, q);
         ++launches;
     }
@@ -554,7 +583,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             } else {
                 launch_project_scene(scene->tab, g, scene->need_sh[i] != 0, scene->classes, *modes, c->slot_ids.p, c->ctr,
                                      c->recs.p, (p.raster_mode == 2 || p.raster_mode == 4) ? c->extra.p : nullptr, p.n_hint,
-                                     c->sm_count, c->cutoff_tab, fc.aux ? c->aux.p : nullptr, ps);
+                                     c->sm_count, c->cutoff_tab, fc.aux ? c->aux.p : nullptr, ps,
+                                     view_ranges ? c->view_ranges : nullptr, view_ranges ? scene->tab.k / views->v : 0u);
                 scene_3d = true;
             }
             ++launches;
@@ -625,7 +655,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
             if (views)
                 launch_raster_views(p.raster_mode, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, o.raster_format,
-                                    &c->ctr->truncated, zt.splat_d, c->kinds.p, p.box, *views, c->stream_r);
+                                    &c->ctr->truncated, zt.splat_d, c->kinds.p, p.box, *views, c->stream_r,
+                                    fc.aux ? c->aux.p : nullptr);
             else
                 launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
                               fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal,
@@ -644,10 +675,15 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, q));
     CU(c, cudaMemcpyAsync(c->h_sticky, c->d_sticky, 4, cudaMemcpyDeviceToHost, q));
     if (o.slot >= 0) CU(c, cudaEventRecord(c->ev_raster[o.slot], q));
-    // a views frame to host memory: each view's frame to its own host target
+    // a views frame to host memory: each view's frames to its own host targets
     auto copy_views = [&](cudaStream_t s) -> bgs_status {
-        for (uint32_t i = 0; i < o.views; ++i)
+        for (uint32_t i = 0; i < o.views; ++i) {
             CU(c, cudaMemcpyAsync(o.view_host[i], o.view_rgba[i], o.view_bytes[i], cudaMemcpyDeviceToHost, s));
+            if (o.view_host_depth[i]) {
+                CU(c, cudaMemcpyAsync(o.view_host_depth[i], o.view_depth[i], o.view_bytes[i], cudaMemcpyDeviceToHost, s));
+                CU(c, cudaMemcpyAsync(o.view_host_normal[i], o.view_normal[i], o.view_bytes[i], cudaMemcpyDeviceToHost, s));
+            }
+        }
         return BGS_OK;
     };
     const bool views_to_host = o.views > 0 && o.view_host[0] != nullptr;
@@ -695,7 +731,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
                               const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
                               int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal,
                               const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr,
-                              const std::shared_ptr<const SceneFacts>& scene = nullptr, void* const* view_targets = nullptr) {
+                              const std::shared_ptr<const SceneFacts>& scene = nullptr, const ViewTargets* view_targets = nullptr) {
     if (!c) return BGS_EINVAL;
     if (!scene) TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));   // (scenes: per cloud, before)
     if (zd) TRY(check_scene_depth(c, zd, view));
@@ -717,13 +753,17 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
     FrameOut o;
-    if (views) TRY(frame_out_views(c, st, out_format, scene->views, view_targets, out_is_device_ptr, &o));
+    if (views) TRY(frame_out_views(c, st, out_format, scene->views, *view_targets, out_is_device_ptr, &o));
     else TRY(frame_out(c, st, out_format, (size_t)fc.Wi * fc.Hi * format_bpp(out_format), out_rgba, out_is_device_ptr, want_aux,
                        out_depth, out_normal, &o));
     ViewTable vt = {};
     if (views) {
         vt = scene->views;
-        for (uint32_t i = 0; i < vt.v; ++i) vt.out[i] = o.view_rgba[i];
+        for (uint32_t i = 0; i < vt.v; ++i) {
+            vt.out[i] = o.view_rgba[i];
+            vt.out_depth[i] = o.view_depth[i];
+            vt.out_normal[i] = o.view_normal[i];
+        }
     }
     for (int attempt = 0; attempt < 4; ++attempt) {
         FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
@@ -807,15 +847,16 @@ static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.ga
 // Gaussian4d cloud when with_4d) with its own settings, num_classes and window, drawn into one depth-sorted frame.
 // entity_flags: each entity's BGS_ENTITY_* bits (NULL: none).  The list has passed check_scene_list.  want_aux
 // (bgs_render_entities_aux): every segment also projects its Depth and Normal colours, blended into out_depth / out_normal.
-// nv > 1 (bgs_render_views, which has checked nv, the targets and the entities' modes): the k entities seen from each of
-// the nv views (depth: nv buffers, or NULL), segment i k + j entity j from view i, view i's frame into view_targets[i].
+// nv > 1 (bgs_render_views or, with want_aux, bgs_render_views_aux, which have checked nv, the targets and the entities'
+// modes): the k entities seen from each of the nv views (depth: nv buffers, or NULL), segment i k + j entity j from view i,
+// view i's frames into view_targets' entries i.
 static bgs_status render_entities_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
                                        const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                        const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
                                        const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
                                        void* out_rgba, uint32_t out_format, int out_is_device_ptr, bool want_aux = false,
                                        void* out_depth = nullptr, void* out_normal = nullptr, uint32_t nv = 1,
-                                       void* const* view_targets = nullptr) {
+                                       const ViewTargets* view_targets = nullptr) {
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
         return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
@@ -871,7 +912,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
             const uint32_t rm = st[j].rasterize_mode;
             SceneSeg& sg = tab.seg[sj];
             sg.fc = frame_consts(cl, &view[i], &unis[j], &st[j], want_aux);
-            sg.fc.n_cloud = tab.n_total;   // (Depth colouring reads the joint sorted list of N entries)
+            sg.fc.n_cloud = (uint32_t)n_view;   // (Depth colouring reads its view's sorted list of n_view entries)
             sg.pos = cl->pos;
             sg.blocks = cl->blocks;
             sg.offset = offset;
@@ -1050,8 +1091,54 @@ bgs_status bgs_render_views(bgs_context* c, const bgs_cloud* const* clouds, cons
     if (v == 1)
         return bgs_render_entities_ex(c, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, out_rgba[0], out_format,
                                       out_is_device_ptr);
+    const ViewTargets targets{out_rgba, nullptr, nullptr};
     return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, nullptr,
-                                out_format, out_is_device_ptr, false, nullptr, nullptr, v, out_rgba);
+                                out_format, out_is_device_ptr, false, nullptr, nullptr, v, &targets);
+}
+
+// bgs_render_entities_aux of each of v views in one frame (include/bgs.h): the refusals of bgs_render_entities_aux and of
+// bgs_render_views but the Depth one, then those of its three target arrays; one view is bgs_render_entities_aux itself
+bgs_status bgs_render_views_aux(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* views,
+                                uint32_t v, const bgs_settings* frame, const bgs_scene_depth* depths, void* const* out_rgba,
+                                void* const* out_depth, void* const* out_normal, uint32_t out_format, int out_is_device_ptr) {
+    const char* call = "render_views_aux";
+    if (!c) return BGS_EINVAL;
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, views, frame));
+    if (v == 0) return fail(c, BGS_EINVAL, "%s: v = 0 views", call);
+    if ((uint64_t)v * k > BGS_SCENE_MAX_CLOUDS)
+        return fail(c, BGS_EINVAL, "%s: v x k = %u x %u segments, at most %d", call, v, k, BGS_SCENE_MAX_CLOUDS);
+    const size_t bpp = format_bpp(out_format);
+    const char* names[3] = {"out_rgba", "out_depth", "out_normal"};
+    void* const* arrays[3] = {out_rgba, out_depth, out_normal};
+    for (int a = 0; a < 3; ++a) {
+        if (!arrays[a]) return fail(c, BGS_EINVAL, "%s: %s is NULL", call, names[a]);
+        for (uint32_t i = 0; i < v; ++i) {
+            if (!arrays[a][i]) return fail(c, BGS_EINVAL, "%s: %s[%u] is NULL", call, names[a], i);
+            if (out_is_device_ptr && reinterpret_cast<uintptr_t>(arrays[a][i]) % bpp != 0)
+                return fail(c, BGS_EINVAL, "%s: device target %s[%u] = %p is not aligned to its %zu-byte pixels", call, names[a],
+                            i, arrays[a][i], bpp);
+        }
+    }
+    if (frame->flags & BGS_FLAG_ASYNC) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
+    for (uint32_t j = 0; j < k; ++j) {
+        // (bgs_render_entities_aux's refusals; OpticalFlow has one previous view per frame)
+        if (is_4d(clouds[j]->layout)) return fail(c, BGS_EINVAL, "%s: clouds[%u] is a Gaussian4d cloud", call, j);
+        if (clouds[j]->layout == CloudLayout::F16Cov)
+            return fail(c, BGS_EINVAL, "%s: clouds[%u] is a precomputed-covariance cloud (no rotation for the normal)", call, j);
+        if (ents[j].rasterize_mode == BGS_RASTERIZE_VELOCITY)
+            return fail(c, BGS_EINVAL, "%s: entities[%u] is in Velocity mode", call, j);
+        if (ents[j].rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW)
+            return fail(c, BGS_EINVAL, "%s: entities[%u] is in OpticalFlow mode", call, j);
+    }
+    if ((frame->flags & BGS_FLAG_BLEND_OVER_TARGET) && !out_is_device_ptr)
+        return fail(c, BGS_EINVAL, "%s: BGS_FLAG_BLEND_OVER_TARGET takes device targets", call);
+    if (v == 1)
+        return bgs_render_entities_aux(c, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, out_rgba[0],
+                                       out_depth[0], out_normal[0], out_format, out_is_device_ptr);
+    const ViewTargets targets{out_rgba, out_depth, out_normal};
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, nullptr,
+                                out_format, out_is_device_ptr, true, nullptr, nullptr, v, &targets);
 }
 
 bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,

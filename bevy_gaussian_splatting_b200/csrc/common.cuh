@@ -112,7 +112,8 @@ struct SegmentKinds {
 // A views frame (bgs_render_views): v views of one entity list.  View i owns segments i k .. i k + k - 1 and the global
 // indices [i n_view, (i + 1) n_view), and the global tile ids [tile0[i], tile0[i + 1]), row-major in its own
 // tiles_x x tiles_y grid.  Binning reads the tile geometry; the blend also the view's size, target and depth buffer (scene
-// NULL: no depth test).  Taken by value (__grid_constant__, ~2.8 KB of kernel parameters) like the segment table.
+// NULL: no depth test), and on aux frames (bgs_render_views_aux) its depth and normal targets.  Taken by value
+// (__grid_constant__, ~3.8 KB of kernel parameters) like the segment table.
 constexpr uint32_t MAX_VIEWS = BGS_SCENE_MAX_CLOUDS;
 struct ViewTable {
     uint32_t v;                 // views, 2 .. MAX_VIEWS (0: not a views frame)
@@ -122,6 +123,8 @@ struct ViewTable {
     void* out[MAX_VIEWS];
     const float* scene[MAX_VIEWS];
     size_t pitch[MAX_VIEWS];
+    void* out_depth[MAX_VIEWS];      // aux frames only
+    void* out_normal[MAX_VIEWS];
     // the view of global index g < v n_view
     __device__ __forceinline__ uint32_t view_of(uint32_t g) const { return g / n_view; }
     // the view of global tile b < tile0[v]: the last i with tile0[i] <= b
@@ -133,6 +136,22 @@ struct ViewTable {
         }
         return lo;
     }
+};
+// sm_90 takes up to 32764 B of kernel parameters (CUDA >= 12.1): the kernels that take the view table (binning and the
+// views blends) pass it with fewer than 256 B of other parameters
+static_assert(sizeof(ViewTable) + 256 <= 32764, "a kernel taking the view table exceeds the sm_90 parameter limit");
+
+// bgs_render_views_aux's Depth range of each view (depth_range_views_kernel), in the frame arena (cleared with it).
+// View i's list is its visible entries in sort order, then its culled entries in ascending index; range[i] is
+// (distance of its sorted[n - 1], distance of its sorted[1]), as FrameCounters' depth_min / depth_max are the
+// single-view frame's.  The other fields are the pass's: positions p in the sorted payload are kept as ~p, so the
+// cleared arena reads as "none yet" and a larger word is an earlier position.
+struct ViewRanges {
+    float2 range[MAX_VIEWS];
+    unsigned long long first2[MAX_VIEWS];   // (~p0) << 32 | ~p1: the view's first two visible positions p0 < p1
+    uint32_t last_p1[MAX_VIEWS];            // its last visible position + 1 (0: none)
+    uint32_t n_vis[MAX_VIEWS];              // its visible entries
+    uint32_t done;                          // CTAs past the pass (the last one computes the ranges)
 };
 
 // Projected splat record, 48 B, stored by front-to-back rank.

@@ -78,8 +78,9 @@ struct SceneFacts {
     int raster_mode = 0;
     SegmentKinds kinds = {};
     bool box = false;
-    // a views frame (bgs_render_views, views.v > 1): the table has views.v x k segments, segment i k + j entity j seen from
-    // view i; the views' tile geometry and depth buffers (their targets are the frame's, filled in when it is enqueued)
+    // a views frame (bgs_render_views, _views_aux, views.v > 1): the table has views.v x k segments, segment i k + j entity j
+    // seen from view i; the views' tile geometry and depth buffers (their targets are the frame's, filled in when it is
+    // enqueued)
     ViewTable views = {};
 };
 
@@ -142,12 +143,12 @@ struct bgs_context {
     DevBuf<float4> aux;               // 2 x float4 per record: depth / normal colour sources (bgs_render_aux only)
     DevBuf<float> splat_depth;        // 1 float per record: the splat depths d of depth-tested frames (allocated on first use)
     DevBuf<unsigned char> kinds;      // 1 byte per record: the blend kind of a mixed-geometry frame's splats (first use)
-    DevBuf<void> frame_aux[2];        // depth / normal frames when bgs_render_aux delivers to host memory
+    DevBuf<void> frame_aux[2];        // depth / normal frames when an aux frame delivers to host memory (views: every view's)
     // scratch sized by the pair capacity (grow-only; cap_pairs pairs)
     uint32_t cap_pairs = 0;
     DevBuf<uint32_t> pkeys[2], pvals[2];
     DevBuf<float4> state;             // per-pixel blend state between rounds (tile-major), tiles * 256 * 16 B
-    // zeroed-per-frame arena: counters | hist | keygen CTA counts | bin CTA counts | ranges | done bytes
+    // zeroed-per-frame arena: counters | view ranges | hist | keygen CTA counts | bin CTA counts | ranges | done bytes
     DevBuf<uint8_t> arena;
     uint32_t arena_tiles = 0;
     // look-back status rows of the two sorts (64-bit epoch-tagged words, cleared once at allocation)
@@ -171,6 +172,7 @@ struct bgs_context {
     uint32_t* kg_block_cnt = nullptr;  // [kg_grid]: keygen_coop's per-CTA visible counts
     uint32_t* bin_block_cnt = nullptr; // [bin_grid][3]: bin_emit_coop's per-CTA pair / medium / large counts
     uint2* ranges = nullptr;           // per tile (~start, end) into the sorted pair list (0, 0 = empty)
+    ViewRanges* view_ranges = nullptr; // bgs_render_views_aux: each view's Depth range
     unsigned char* tile_done = nullptr;   // per tile: saturated (chunked frames)
     // async frames delivered to host memory alternate the two frames so frame k's D2H copy (copy stream) overlaps
     // frame k+1's kernels

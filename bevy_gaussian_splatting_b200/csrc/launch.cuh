@@ -47,12 +47,18 @@ void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_sl
 // scene frames: the projection of the segments of one group (project_group, | ENTITY_MODES for the Classification /
 // OpticalFlow / Velocity kernel; one launch), each with its own settings and num_classes; need_sh: some segment of the
 // group reads the SH coefficients.  And the Gaussian4d segments' (PROJECT_GROUP_4D), each at its own times, with their
-// splat depths from the moved positions (depths non-null).
+// splat depths from the moved positions (depths non-null).  view_ranges non-null (bgs_render_views_aux, k segments per
+// view): each segment's Depth colours over its view's range.
 void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
                           const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
                           float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab,
                           float4* aux /* bgs_render_entities_aux: each segment's depth / normal colours; else null */,
-                          cudaStream_t stream);
+                          cudaStream_t stream, const ViewRanges* view_ranges = nullptr, uint32_t k = 0);
+// bgs_render_views_aux: the Depth range of each of v views of n_view global indices (ViewRanges::range; the arena clear
+// resets the rest), in place of launch_depth_range_scene
+void launch_depth_range_views(const SceneTable& tab, uint32_t v, uint32_t n_view, const uint32_t* sorted_payload,
+                              const uint32_t* slot_ids, const FrameCounters* ctr, ViewRanges* view_ranges, uint32_t n_hint,
+                              int sm_count, cudaStream_t stream);
 void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
                              const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
                              float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
@@ -92,10 +98,11 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
 void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
                           uint32_t n_hint, int sm_count, cudaStream_t stream);
 // bgs_render_views' blend: one CTA per global tile of every view (vt.tile0[vt.v]), each into its view's target; mode and box
-// as launch_raster's; splat_d non-null and vt.scene[i]: the depth test against view i's buffer
+// as launch_raster's; splat_d non-null and vt.scene[i]: the depth test against view i's buffer; aux non-null
+// (bgs_render_views_aux): also the depth and normal frames, into vt.out_depth[i] / vt.out_normal[i]
 void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
                          uint32_t format, const uint32_t* truncated, const float* splat_d, const unsigned char* kinds, bool box,
-                         const ViewTable& vt, cudaStream_t stream);
+                         const ViewTable& vt, cudaStream_t stream, const float4* aux = nullptr);
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
                          uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,

@@ -462,12 +462,13 @@ __device__ __forceinline__ void sh_colour(const FrameConsts& fc, const float A[3
     }
 }
 
-// RasterizeMode::Depth: material/depth.wgsl:3-11 over depth_range_kernel's [depth_min, depth_max]
-__device__ __forceinline__ void depth_colour(const FrameConsts& fc, const FrameCounters* __restrict__ ctr,
-                                             const float pw[3], float rgb[3]) {
+// RasterizeMode::Depth: material/depth.wgsl:3-11 over the range (depth_min, depth_max) that range() reads
+template <class Range>
+__device__ __forceinline__ void depth_colour_over(const FrameConsts& fc, Range range, const float pw[3], float rgb[3]) {
     if (fc.n_cloud < 2u) return;   // the reference reads sorted[1]: undefined for a 1-gaussian cloud (oracle: black)
     const float depth = sqrtf(cam_dist2(fc, pw));
-    const float dmin = ctr->depth_min, dmax = ctr->depth_max;
+    const float2 dr = range();
+    const float dmin = dr.x, dmax = dr.y;
     float nd = (depth - dmin) / (dmax - dmin);
     nd = fminf(fmaxf(nd, 0.0f), 1.0f);   // fmin/fmax ignore a NaN operand, like the oracle's
     float t1 = (nd - 0.5f) / (1.0f - 0.5f); t1 = fminf(fmaxf(t1, 0.0f), 1.0f);
@@ -475,6 +476,11 @@ __device__ __forceinline__ void depth_colour(const FrameConsts& fc, const FrameC
     rgb[0] = t1 * t1 * (3.0f - 2.0f * t1);
     rgb[1] = 1.0f - fabsf(nd - 0.5f) * 2.0f;
     rgb[2] = 1.0f - t2 * t2 * (3.0f - 2.0f * t2);
+}
+// ... over depth_range_kernel's [depth_min, depth_max]
+__device__ __forceinline__ void depth_colour(const FrameConsts& fc, const FrameCounters* __restrict__ ctr,
+                                             const float pw[3], float rgb[3]) {
+    depth_colour_over(fc, [&] { return make_float2(ctr->depth_min, ctr->depth_max); }, pw, rgb);
 }
 
 // RasterizeMode::Normal: gaussian.wgsl:350-368, the view-space direction of the splat's third scaled axis
@@ -590,12 +596,19 @@ __device__ __forceinline__ void store_rec(SplatRec* __restrict__ dst, const Spla
 // template flag, so project_modes_kernel stays as it is.
 // no_source: the frame has no colour source for this gaussian (a 3D or 2D one in a bgs_render_scene_4d Velocity frame:
 // the reference builds no pipeline for it), so it stays undrawn.  Only the scene kernels pass it.
-template <bool F16, uint32_t D, bool MODES2, bool SCENE = false>
+// VIEWS (project_views_aux_kernel, bgs_render_views_aux): the Depth colours are over *view_range, the segment's view's
+// range, instead of the frame's.
+template <bool F16, uint32_t D, bool MODES2, bool SCENE = false, bool VIEWS = false>
 __device__ __forceinline__ void project_one(const FrameConsts& fc, const FrameCounters* __restrict__ ctr, uint32_t r,
                                             float4 p4, const float q[4], const float so[4], const float* sh,
                                             const float* __restrict__ cutoff_tab, uint32_t op_bits,
                                             SplatRec* __restrict__ recs, float4* __restrict__ extra,
-                                            float4* __restrict__ aux, const ModeConsts& mc, bool no_source = false) {
+                                            float4* __restrict__ aux, const ModeConsts& mc, bool no_source = false,
+                                            const float2* __restrict__ view_range = nullptr) {
+    auto depth_colour = [&](const FrameConsts& f, const FrameCounters* c, const float p[3], float rgb[3]) {
+        if constexpr (VIEWS) depth_colour_over(f, [&] { return *view_range; }, p, rgb);
+        else bgs::depth_colour(f, c, p, rgb);
+    };
     SplatRec rec;
     rec.ux = 0.f; rec.uy = 0.f; rec.vx = 0.f; rec.vy = 0.f;
     rec.bx = BBOX_EMPTY; rec.by = BBOX_EMPTY;
@@ -720,7 +733,8 @@ __device__ __forceinline__ void project_loop(const Src& src, const Geo& geo, con
 }
 
 // The 3D and 2D splats: Attr<F16, D>'s blocks and project_one's record.  MODES2: project_modes_kernel's colour sources.
-template <bool F16, uint32_t D, bool MODES2>
+// VIEWS: segment j's Depth colours are over view_range[j / k] (project_views_aux_kernel).
+template <bool F16, uint32_t D, bool MODES2, bool VIEWS = false>
 struct Geo3d {
     using A = Attr<F16, D>;
     static constexpr int SCH = A::CH, BCH = A::CH, GEO = A::GEO, EXT = sh_floats(D);
@@ -730,6 +744,8 @@ struct Geo3d {
     float4* extra;
     const float* cutoff_tab;
     float4* aux;
+    const float2* view_range = nullptr;
+    uint32_t k = 0u;   // segments per view
 
     __device__ __forceinline__ float4 read(const uint4* stage, int lane, float* sh, float q[4], float so[4], uint32_t& op_bits) const {
         return A::load(stage, lane, sh, q, so, need_sh, op_bits);
@@ -738,8 +754,9 @@ struct Geo3d {
     __device__ __forceinline__ void project(const Src& src, uint32_t j, uint32_t, uint32_t r, float4 p4, const float q[4],
                                             const float so[4], const float* sh, uint32_t op_bits, const ModeConsts& mc) const {
         const FrameConsts& fc = src.fc(j);
-        project_one<F16, D, MODES2, Src::SEGMENTED>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc,
-                                    MODES2 && Src::SEGMENTED && fc.rasterize_mode == BGS_RASTERIZE_VELOCITY);
+        project_one<F16, D, MODES2, Src::SEGMENTED, VIEWS>(fc, ctr, r, p4, q, so, sh, cutoff_tab, op_bits, recs, extra, aux, mc,
+                                                           MODES2 && Src::SEGMENTED && fc.rasterize_mode == BGS_RASTERIZE_VELOCITY,
+                                                           VIEWS ? view_range + j / k : nullptr);
     }
 };
 
@@ -1014,6 +1031,131 @@ project_scene_kernel(SceneTable tab, uint32_t group, uint32_t need_sh, SceneClas
                  SceneGeo<Geo3d<F16, D, MODES2>>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, aux}, classes}, ctr, mc);
 }
 
+// bgs_render_views_aux's projection: project_scene_kernel's, with each segment's Depth colours (its colour source and its
+// aux depth colour) over its view's range, vr->range[j / k].  A kernel of its own, so the other scene frames keep
+// project_scene_kernel as it is.
+template <bool F16, uint32_t D, bool MODES2>
+__global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
+project_views_aux_kernel(SceneTable tab, uint32_t group, uint32_t need_sh, SceneClasses classes, ModeConsts mc,
+                         const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                         SplatRec* __restrict__ recs, float4* __restrict__ extra, const float* __restrict__ cutoff_tab,
+                         float4* __restrict__ aux, const ViewRanges* __restrict__ vr, uint32_t k) {
+    project_loop(SceneSrc{tab, 1u << group, slot_ids},
+                 SceneGeo<Geo3d<F16, D, MODES2, true>>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, aux, vr->range, k}, classes},
+                 ctr, mc);
+}
+
+// ---- bgs_render_views_aux: each view's Depth range (ViewRanges) from one pass over the n_vis sorted visible entries.
+// The joint sort is stable and view i's global indices are [i n, (i + 1) n), so view i's entries keep, in the joint
+// sorted list, the order of its own frame's sort.  Its list's sorted[1] is then its second visible entry (with fewer than
+// two visible: its first culled index), and its sorted[n - 1] its last culled index (with none culled: its last visible
+// entry).  The culled ends come from slot_ids: the stable compaction keeps a view's visible global indices as one
+// ascending run, so its first culled index is where that run first departs from i n, i n + 1, ..., and its last culled
+// index where the run, read backwards, first departs from (i + 1) n - 1, (i + 1) n - 2, ...
+constexpr int DRV_THREADS = 256, DRV_CTAS_PER_SM = 4;
+
+// sorted position p into a ViewRanges::first2 word (shared or global): kept when it is among the two smallest so far
+__device__ __forceinline__ void first2_insert(unsigned long long* w, uint32_t p) {
+    const unsigned long long x = 0xFFFFFFFFu - p;
+    unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(w);
+    for (;;) {
+        const unsigned long long a = cur >> 32, b = cur & 0xFFFFFFFFull;
+        unsigned long long next;
+        if (x > a) next = x << 32 | a;
+        else if (x > b) next = a << 32 | x;
+        else return;
+        const unsigned long long prev = atomicCAS(w, cur, next);
+        if (prev == cur) return;
+        cur = prev;
+    }
+}
+
+// the smallest t in [0, len) with miss(t), len if none, for a miss() that stays true once true: a 32-way search, the
+// whole warp calling it (miss is read only below len)
+template <class Miss>
+__device__ __forceinline__ uint32_t warp_first_miss(uint32_t len, Miss miss) {
+    const uint32_t lane = threadIdx.x & 31u;
+    uint32_t lo = 0u, hi = len;   // the answer lies in [lo, hi]
+    while (lo < hi) {
+        const uint32_t step = (hi - lo + 31u) / 32u, t = lo + lane * step;
+        const uint32_t m = __ballot_sync(0xFFFFFFFFu, t >= hi || miss(t));
+        if (m == 0u) {
+            lo += 31u * step + 1u;
+        } else {
+            const uint32_t f = (uint32_t)__ffs(m) - 1u;
+            hi = min(hi, lo + f * step);
+            if (f > 0u) lo += (f - 1u) * step + 1u;
+        }
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(DRV_THREADS)
+depth_range_views_kernel(SceneTable tab, uint32_t v, uint32_t n_view, const uint32_t* __restrict__ sorted_payload,
+                         const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                         ViewRanges* __restrict__ vr) {
+    __shared__ unsigned long long s_first2[MAX_VIEWS];
+    __shared__ uint32_t s_last_p1[MAX_VIEWS], s_cnt[MAX_VIEWS];
+    __shared__ bool s_final;
+    const uint32_t t = threadIdx.x, lane = t & 31u;
+    if (t < MAX_VIEWS) { s_first2[t] = 0ull; s_last_p1[t] = 0u; s_cnt[t] = 0u; }
+    __syncthreads();
+    // the pass: each warp's lanes hold consecutive positions, so a view's lowest two lanes in the warp are its warp's
+    // first two positions and its highest lane its last
+    const uint32_t n_vis = ctr->n_vis;
+    for (uint32_t p0 = blockIdx.x * DRV_THREADS; p0 < n_vis; p0 += gridDim.x * DRV_THREADS) {
+        const uint32_t p = p0 + t;
+        const uint32_t view = p < n_vis ? __ldg(slot_ids + __ldg(sorted_payload + p)) / n_view : 0xFFFFFFFFu;
+        const uint32_t peers = __match_any_sync(0xFFFFFFFFu, view);
+        if (view != 0xFFFFFFFFu) {
+            const uint32_t rank = __popc(peers & lanemask_lt());
+            if (rank == 0u) atomicAdd(&s_cnt[view], (uint32_t)__popc(peers));
+            if (rank < 2u) first2_insert(&s_first2[view], p);
+            if ((peers >> lane) == 1u) atomicMax(&s_last_p1[view], p + 1u);
+        }
+    }
+    __syncthreads();
+    if (t < v) {
+        const unsigned long long f = s_first2[t];
+        if (f >> 32) first2_insert(&vr->first2[t], 0xFFFFFFFFu - (uint32_t)(f >> 32));
+        if (f & 0xFFFFFFFFull) first2_insert(&vr->first2[t], 0xFFFFFFFFu - (uint32_t)f);
+        if (s_last_p1[t]) atomicMax(&vr->last_p1[t], s_last_p1[t]);
+        if (s_cnt[t]) atomicAdd(&vr->n_vis[t], s_cnt[t]);
+    }
+    __threadfence();
+    __syncthreads();
+    if (t == 0) s_final = atomicAdd(&vr->done, 1u) == gridDim.x - 1u;
+    __syncthreads();
+    // the last CTA past the pass: every view's range, one warp per view
+    if (!s_final || n_view < 2u) return;   // (n < 2: the range stays (0, 0) and depth_colour draws black, as one view's)
+    __threadfence();
+    const volatile ViewRanges* w = vr;
+    const SceneSrc src{tab};
+    auto dist = [&](uint32_t id) {   // depth_range_body's
+        const uint32_t j = src.seg(id);
+        const FrameConsts& fc = src.fc(j);
+        const float4 p = *src.pos_at(j, id);
+        float pw[4];
+        mat4_point(fc.model, p.x, p.y, p.z, pw);
+        return sqrtf(cam_dist2(fc, pw));
+    };
+    auto id_at = [&](uint32_t pos) { return __ldg(slot_ids + __ldg(sorted_payload + pos)); };
+    for (uint32_t i = t >> 5; i < v; i += DRV_THREADS / 32) {
+        const uint32_t cnt = w->n_vis[i], last_p1 = w->last_p1[i];
+        const unsigned long long f = w->first2[i];
+        uint32_t run0 = 0u;   // the view's first compact slot
+        for (uint32_t e = 0; e < i; ++e) run0 += w->n_vis[e];
+        const uint32_t base = i * n_view;
+        const uint32_t lo = warp_first_miss(cnt, [&](uint32_t x) { return __ldg(slot_ids + run0 + x) != base + x; });
+        const uint32_t hi = warp_first_miss(cnt, [&](uint32_t x) {
+            return __ldg(slot_ids + run0 + cnt - 1u - x) != base + n_view - 1u - x;
+        });
+        const uint32_t first = cnt >= 2u ? id_at(0xFFFFFFFFu - (uint32_t)(f & 0xFFFFFFFFull)) : base + lo;
+        const uint32_t last = cnt < n_view ? base + n_view - 1u - hi : id_at(last_p1 - 1u);
+        if (lane == 0u) vr->range[i] = make_float2(dist(last), dist(first));
+    }
+}
+
 __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_4d_scene_kernel(SceneTable tab, SceneTimes times, SceneClasses classes, ModeConsts mc,
                         const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
@@ -1024,23 +1166,40 @@ project_4d_scene_kernel(SceneTable tab, SceneTimes times, SceneClasses classes, 
 // (256 B), the extras and four pointers
 static_assert(sizeof(SceneTable) + sizeof(SceneTimes) + sizeof(SceneClasses) + sizeof(ModeConsts) + 4 * sizeof(void*) + 16 <= 32764,
               "project_4d_scene_kernel's parameters exceed the sm_90 limit");
+// (project_views_aux_kernel: the table, the classes, the extras, seven pointers and three words)
+static_assert(sizeof(SceneTable) + sizeof(SceneClasses) + sizeof(ModeConsts) + 7 * sizeof(void*) + 16 <= 32764,
+              "project_views_aux_kernel's parameters exceed the sm_90 limit");
 
 void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, const SceneClasses& classes,
                           const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
                           float4* extra, uint32_t n_hint, int sm_count, const float* cutoff_tab, float4* aux,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, const ViewRanges* view_ranges, uint32_t k) {
     const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
     const uint32_t g = group & ~ENTITY_MODES;
     with_layout_degree(g & 1u ? CloudLayout::F16 : CloudLayout::F32, g >> 1, [&](auto L, auto Dt) {
         constexpr CloudLayout Lv = decltype(L)::value;
         constexpr uint32_t D = decltype(Dt)::value;
         if constexpr (!is_4d(Lv)) {
+            if (view_ranges) {
+                auto* kernel = (group & ENTITY_MODES) ? project_views_aux_kernel<is_f16(Lv), D, true>
+                                                      : project_views_aux_kernel<is_f16(Lv), D, false>;
+                kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, group, need_sh ? 1u : 0u, classes, mc, slot_ids, ctr, recs, extra,
+                                                          cutoff_tab, aux, view_ranges, k);
+                return;
+            }
             auto* kernel = (group & ENTITY_MODES) ? project_scene_kernel<is_f16(Lv), D, true>
                                                   : project_scene_kernel<is_f16(Lv), D, false>;
             kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, group, need_sh ? 1u : 0u, classes, mc, slot_ids, ctr, recs, extra,
                                                       cutoff_tab, aux);
         }
     });
+}
+
+void launch_depth_range_views(const SceneTable& tab, uint32_t v, uint32_t n_view, const uint32_t* sorted_payload,
+                              const uint32_t* slot_ids, const FrameCounters* ctr, ViewRanges* view_ranges, uint32_t n_hint,
+                              int sm_count, cudaStream_t stream) {
+    const uint32_t grid = persistent_grid(n_hint, DRV_THREADS, DRV_CTAS_PER_SM, sm_count);
+    depth_range_views_kernel<<<grid, DRV_THREADS, 0, stream>>>(tab, v, n_view, sorted_payload, slot_ids, ctr, view_ranges);
 }
 
 void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,

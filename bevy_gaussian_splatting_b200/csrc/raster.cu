@@ -261,7 +261,8 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // kinds byte (its entity's), the others draw every splat's box.  MODE 0 takes the generic loop, not the inline-asm one.
 // VIEWS (raster_views_kernel, bgs_render_views): the CTA's global tile blockIdx.x lies in view i = vt->view_of_tile; W, H,
 // tiles_x, out, scene and pitch are then view i's, the CTA takes the local tile blockIdx.x - tile0[i] in centre_out_tile's
-// order within the view, and reads the global tile's range.
+// order within the view, and reads the global tile's range.  With AUX (raster_views_aux_kernel, bgs_render_views_aux)
+// out_depth and out_normal are view i's too.
 template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false>
 __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
                                             const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
@@ -293,6 +294,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
         const uint32_t i = vt->view_of_tile(blockIdx.x);
         W = vt->W[i]; H = vt->H[i]; tiles_x = vt->tiles_x[i]; out = vt->out[i];
         if (ZTEST) { scene = vt->scene[i]; pitch = vt->pitch[i]; }
+        if (AUX) { out_depth = vt->out_depth[i]; out_normal = vt->out_normal[i]; }
         centre_out_tile((int)(blockIdx.x - vt->tile0[i]), tiles_x, vt->tiles_y[i], tile_x, tile_y);
         tile = (int)vt->tile0[i] + tile_y * tiles_x + tile_x;
     } else {
@@ -627,6 +629,20 @@ raster_views_kernel(const SplatRec* __restrict__ recs, const float4* __restrict_
                                                nullptr, truncated, splat_d, nullptr, 0, kinds, &vt);
 }
 
+// bgs_render_views_aux's blends: raster_views_kernel's with the depth and normal frames (MODE 3 and 4: raster_mixed_aux's
+// body).  Kernels of their own, so bgs_render_views keeps the very kernels it has.  Launch bounds from the ptxas report:
+// MODE 2 with ZTEST spills at 4 CTAs per SM (3 leave it 85 registers); MODE 4, and MODE 2 and 3 with ZTEST or BOX, at 5.
+template <int MODE, bool ZTEST, bool BOX>
+__global__ void __launch_bounds__(RT_THREADS, MODE == 2 && ZTEST ? 3 : (MODE == 4 || ((ZTEST || BOX) && MODE >= 2) ? 4 : 5))
+raster_views_aux_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
+                        const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, uint32_t format,
+                        const float4* __restrict__ aux, const uint32_t* __restrict__ truncated,
+                        const float* __restrict__ splat_d, const unsigned char* __restrict__ kinds,
+                        const __grid_constant__ ViewTable vt) {
+    raster_body<MODE, true, ZTEST, BOX, true>(recs, extra, tile_entries, ranges, 0, 0, 0, nullptr, format, aux, nullptr,
+                                              nullptr, truncated, splat_d, nullptr, 0, kinds, &vt);
+}
+
 // the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
 __global__ void raster_kinds_kernel(SegmentKinds sk, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
                                     unsigned char* __restrict__ out) {
@@ -890,7 +906,19 @@ void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const 
 
 void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
                          uint32_t format, const uint32_t* truncated, const float* splat_d, const unsigned char* kinds, bool box,
-                         const ViewTable& vt, cudaStream_t stream) {
+                         const ViewTable& vt, cudaStream_t stream, const float4* aux) {
+    if (aux) {
+        using AuxKernel = void (*)(const SplatRec*, const float4*, const uint32_t*, const uint2*, uint32_t, const float4*,
+                                   const uint32_t*, const float*, const unsigned char*, const ViewTable);
+#define VIEWS_AUX_ROW_(Z, B) {raster_views_aux_kernel<0, Z, B>, raster_views_aux_kernel<1, Z, B>, raster_views_aux_kernel<2, Z, B>, \
+                              raster_views_aux_kernel<3, Z, B>, raster_views_aux_kernel<4, Z, B>}
+        static const AuxKernel kernels[2][2][5] = {{VIEWS_AUX_ROW_(false, false), VIEWS_AUX_ROW_(false, true)},
+                                                   {VIEWS_AUX_ROW_(true, false), VIEWS_AUX_ROW_(true, true)}};
+#undef VIEWS_AUX_ROW_
+        kernels[splat_d != nullptr][box][mode]<<<vt.tile0[vt.v], RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges,
+                                                                                         format, aux, truncated, splat_d, kinds, vt);
+        return;
+    }
     using Kernel = void (*)(const SplatRec*, const float4*, const uint32_t*, const uint2*, uint32_t, const uint32_t*,
                             const float*, const unsigned char*, const ViewTable);
 #define VIEWS_ROW_(Z, B) {raster_views_kernel<0, Z, B>, raster_views_kernel<1, Z, B>, raster_views_kernel<2, Z, B>, \

@@ -333,6 +333,28 @@ def check_views(entities, views) -> CloudSettings:
     return first
 
 
+def check_views_aux(entities, views) -> CloudSettings:
+    """`check_entities_aux` and `check_views` for one bgs_render_views_aux call of `views` (a sequence of View): ValueError
+    for no views, views x entities over abi.BGS_SCENE_MAX_CLOUDS segments, a Gaussian4d or precomputed-covariance cloud,
+    and an entity in Velocity or OpticalFlow mode.  Depth entities are accepted: each view's Depth colours are over its own
+    range."""
+    entities, views = list(entities), list(views)
+    first = check_entities(entities)
+    if not views:
+        raise ValueError("render_views_aux: no views")
+    if len(views) * len(entities) > abi.BGS_SCENE_MAX_CLOUDS:
+        raise ValueError(f"render_views_aux: {len(views)} views x {len(entities)} entities, at most {abi.BGS_SCENE_MAX_CLOUDS} segments")
+    for j, (h, st, _) in enumerate(entities):
+        if is_4d_handle(h):
+            raise ValueError(f"render_views_aux: entity {j} is a Gaussian4d cloud")
+        if getattr(h, "precompute_covariance", False):
+            raise ValueError(f"render_views_aux: entity {j} is a precomputed-covariance cloud")
+        mode = RasterizeMode(st.rasterize_mode)
+        if mode in (RasterizeMode.Velocity, RasterizeMode.OpticalFlow):
+            raise ValueError(f"render_views_aux: entity {j} is in {mode.name} mode")
+    return first
+
+
 def entity_settings(settings: CloudSettings) -> abi.bgs_entity_settings:
     """One entity's bgs_entity_settings."""
     s = settings.to_abi()
@@ -568,6 +590,35 @@ class GaussianSplattingPlugin:
             zds = (abi.bgs_scene_depth * n)(*[self._scene_depth(d, v) for d, v in zip(scene_depths, views)])
         targets = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
         self._check(self._lib.bgs_render_views(self._ctx, clouds, unis, ents, eflags, k, vs, n, s, zds, targets, code, 0))
+        return outs
+
+    def render_views_aux(self, entities, views, fmt: str = "rgba32f", scene_depths=None, premultiplied: bool = False,
+                         outs=None) -> list[list[np.ndarray]]:
+        """`render_entities_aux` of every view in `views` in ONE frame (`bgs_render_views_aux`): returns [rgba, depth,
+        normal] per view, each byte for byte `render_entities_aux`' frames of that view.  Entities in Depth mode are drawn
+        over each view's own depth range.  `scene_depths`: one depth buffer per view, or None.  `outs`: the host frames to
+        fill, [[rgba, depth, normal] per view].  Synchronous only.  Validates with `check_views_aux` (ValueError before any
+        call)."""
+        entities, views = list(entities), list(views)
+        first = check_views_aux(entities, views)
+        code, dtype, ch = self.FORMATS[fmt]
+        if outs is None:
+            outs = [[np.empty((v.height, v.width, ch), dtype) for _ in range(3)] for v in views]
+        assert len(outs) == len(views)
+        for trio, v in zip(outs, views):
+            assert len(trio) == 3
+            for o in trio:
+                assert o.dtype == dtype and o.size == v.height * v.width * ch and o.flags.c_contiguous
+        clouds, unis, ents, eflags, k, _, s, _ = self._entities_args(entities, first, views[0], None, None, False,
+                                                                     premultiplied, False)
+        n = len(views)
+        vs = (abi.bgs_view * n)(*[v.to_abi() for v in views])
+        zds = None
+        if scene_depths is not None:
+            assert len(scene_depths) == n
+            zds = (abi.bgs_scene_depth * n)(*[self._scene_depth(d, v) for d, v in zip(scene_depths, views)])
+        targets = [(C.c_void_p * n)(*[trio[f].ctypes.data for trio in outs]) for f in range(3)]
+        self._check(self._lib.bgs_render_views_aux(self._ctx, clouds, unis, ents, eflags, k, vs, n, s, zds, *targets, code, 0))
         return outs
 
     def _entities_args(self, entities, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over):

@@ -845,6 +845,41 @@ bgs_status bgs_render_views(bgs_context* ctx, const bgs_cloud* const* clouds, co
                             const bgs_scene_depth* depths /* v, or NULL */, void* const* out_rgba /* v */,
                             uint32_t out_format, int out_is_device_ptr);
 
+/* bgs_render_entities_aux of several views of one scene in ONE frame: the colour, depth and normal frames of every view --
+ * a stereo headset's eyes for reprojection, the six faces of a cube map for relighting, a glTF scene's cameras, or a 2DGS
+ * surfel scene seen from many dataset cameras -- from one key-gen, depth sort, projection, binning, tile-id sort and
+ * blend launch instead of one set of launches per view.  Entities in Depth mode are drawn, each view over its own range.
+ *
+ * The rule, exactly:
+ *   Per-view identity.  out_rgba[i], out_depth[i] and out_normal[i] are byte for byte the three frames
+ *     bgs_render_entities_aux(clouds, uniforms, entities, entity_flags, k, &views[i], frame, NULL,
+ *     depths ? &depths[i] : NULL, out_rgba[i], out_depth[i], out_normal[i], out_format, out_is_device_ptr) produces: in
+ *     all three formats, with BGS_FLAG_PREMULTIPLIED_OUT, per-entity and frame-wide bounding-box overlays, and under each
+ *     view's own depth buffer.  With BGS_FLAG_BLEND_OVER_TARGET each device target is blended over its own pixels.
+ *   Per-view Depth range.  View i's list is its visible entries in sort order, then its culled entries in ascending
+ *     index; its Depth colours (a Depth entity's rgba, every entity's out_depth) are over the distances of that list's
+ *     sorted[n-1] / sorted[1], n the entity list's count -- bgs_render_entities_aux's rule for view i alone, including a
+ *     view with 0 or 1 visible gaussians, a view with none culled, and black Depth colours when n < 2.
+ *   Index space, sort, tiles, one round, hooks and stats: bgs_render_views' (segment i k + j, view i's global indices
+ *     [i n, (i + 1) n), N = v n below 2^30, one stable sort, view after view of tiles, BGS_FLAG_CHUNKS ignored).  Host
+ *     targets: the library's frames hold all v frames of each kind, and each view's three are copied out to its targets.
+ *   v == 1.  The call is bgs_render_entities_aux: all three frames, hooks, stats and launch count.
+ *   Synchronous only.
+ * Launches: those of one bgs_render_entities_aux frame of the same entities, whatever v is (v >= 2: the per-view Depth
+ *   range in place of the frame's, as one launch).
+ * Refused with BGS_EINVAL, nothing enqueued or written and the previous frame's debug hooks kept: every refusal
+ *   bgs_render_entities_aux makes for some view; v == 0, v k > BGS_SCENE_MAX_CLOUDS or N >= 2^30; a NULL out_rgba,
+ *   out_depth or out_normal, or a NULL entry of one; a device target not aligned to its pixel (each of the 3 v);
+ *   BGS_FLAG_ASYNC; a Gaussian4d cloud, a precomputed-covariance cloud, an entity in Velocity mode (as
+ *   bgs_render_entities_aux); an entity in OpticalFlow mode (one previous view per frame); BGS_FLAG_BLEND_OVER_TARGET with
+ *   host targets.  NULL clouds, uniforms, entities, views or frame -> BGS_NOT_READY. */
+bgs_status bgs_render_views_aux(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                                const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */,
+                                uint32_t k, const bgs_view* views, uint32_t v, const bgs_settings* frame,
+                                const bgs_scene_depth* depths /* v, or NULL */, void* const* out_rgba /* v */,
+                                void* const* out_depth /* v */, void* const* out_normal /* v */,
+                                uint32_t out_format, int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target

@@ -471,32 +471,29 @@ public:
                       const std::vector<void*>& out_rgba, uint32_t format = BGS_FORMAT_RGBA8_SRGB,
                       const std::vector<const float*>& depths = {}, const std::vector<uint64_t>& pitches = {},
                       bool out_is_device = false, uint32_t extra_flags = 0) {
-        if (entities.empty() || views.empty() || out_rgba.size() != views.size()) check(BGS_EINVAL);
-        if (!depths.empty() && (depths.size() != views.size() || pitches.size() != views.size())) check(BGS_EINVAL);
-        std::vector<const bgs_cloud*> clouds;
-        std::vector<bgs_cloud_uniform> unis;
-        std::vector<bgs_entity_settings> ents;
-        std::vector<uint32_t> eflags;
-        for (const SceneEntity& e : entities) {
-            bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
-            std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
-            clouds.push_back(e.cloud->get());
-            unis.push_back(u);
-            const bgs_settings s = e.settings.to_abi();
-            ents.push_back({s.gaussian_mode, s.rasterize_mode, s.aabb, s.opacity_adaptive_radius, s.draw_mode,
-                            e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
-            eflags.push_back(e.settings.visualize_bounding_box ? (uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX : 0u);
-        }
-        bgs_settings s = entities[0].settings.to_abi(extra_flags);
-        if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
-        std::vector<bgs_scene_depth> zd;
-        for (size_t i = 0; i < depths.size(); ++i) zd.push_back({depths[i], pitches[i]});
-        const bgs_status st = bgs_render_views(ctx_, clouds.data(), unis.data(), ents.data(), eflags.data(),
-                                               (uint32_t)clouds.size(), views.data(), (uint32_t)views.size(), &s,
-                                               zd.empty() ? nullptr : zd.data(), out_rgba.data(), format, out_is_device ? 1 : 0);
-        if (st == BGS_NOT_READY) return false;
-        check(st);
-        return true;
+        if (out_rgba.size() != views.size()) check(BGS_EINVAL);
+        return views_call(entities, views, depths, pitches, extra_flags, [&](const ViewsArgs& a) {
+            return bgs_render_views(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(), (uint32_t)a.clouds.size(),
+                                    views.data(), (uint32_t)views.size(), &a.s, a.zd.empty() ? nullptr : a.zd.data(),
+                                    out_rgba.data(), format, out_is_device ? 1 : 0);
+        });
+    }
+    // render_views' frames and each view's depth and normal frames in one pass (bgs_render_views_aux): out_rgba[i],
+    // out_depth[i] and out_normal[i] receive views[i]'s three frames, byte for byte bgs_render_entities_aux's of that view.
+    // Depth entities are drawn over each view's own range; OpticalFlow entities are refused.  Synchronous only.
+    bool render_views_aux(const std::vector<SceneEntity>& entities, const std::vector<bgs_view>& views,
+                          const std::vector<void*>& out_rgba, const std::vector<void*>& out_depth,
+                          const std::vector<void*>& out_normal, uint32_t format = BGS_FORMAT_RGBA8_SRGB,
+                          const std::vector<const float*>& depths = {}, const std::vector<uint64_t>& pitches = {},
+                          bool out_is_device = false, uint32_t extra_flags = 0) {
+        if (out_rgba.size() != views.size() || out_depth.size() != views.size() || out_normal.size() != views.size())
+            check(BGS_EINVAL);
+        return views_call(entities, views, depths, pitches, extra_flags, [&](const ViewsArgs& a) {
+            return bgs_render_views_aux(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(),
+                                        (uint32_t)a.clouds.size(), views.data(), (uint32_t)views.size(), &a.s,
+                                        a.zd.empty() ? nullptr : a.zd.data(), out_rgba.data(), out_depth.data(),
+                                        out_normal.data(), format, out_is_device ? 1 : 0);
+        });
     }
     // Colour + depth + normal frames of one view in one pass (BASELINE.json config 4; bgs_render_aux).
     bool render_view_aux(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view, void* out_rgba,
@@ -636,6 +633,40 @@ public:
 
 private:
     void check(bgs_status st) { if (st != BGS_OK) throw Error(st, bgs_last_error(ctx_)); }
+    // the entity arrays of a render_views / render_views_aux call, and the call made with them (false: BGS_NOT_READY)
+    struct ViewsArgs {
+        std::vector<const bgs_cloud*> clouds;
+        std::vector<bgs_cloud_uniform> unis;
+        std::vector<bgs_entity_settings> ents;
+        std::vector<uint32_t> eflags;
+        bgs_settings s;
+        std::vector<bgs_scene_depth> zd;
+    };
+    template <class Call>
+    bool views_call(const std::vector<SceneEntity>& entities, const std::vector<bgs_view>& views,
+                    const std::vector<const float*>& depths, const std::vector<uint64_t>& pitches, uint32_t extra_flags,
+                    Call call) {
+        if (entities.empty() || views.empty()) check(BGS_EINVAL);
+        if (!depths.empty() && (depths.size() != views.size() || pitches.size() != views.size())) check(BGS_EINVAL);
+        ViewsArgs a;
+        for (const SceneEntity& e : entities) {
+            bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
+            std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
+            a.clouds.push_back(e.cloud->get());
+            a.unis.push_back(u);
+            const bgs_settings s = e.settings.to_abi();
+            a.ents.push_back({s.gaussian_mode, s.rasterize_mode, s.aabb, s.opacity_adaptive_radius, s.draw_mode,
+                              e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
+            a.eflags.push_back(e.settings.visualize_bounding_box ? (uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX : 0u);
+        }
+        a.s = entities[0].settings.to_abi(extra_flags);
+        if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) a.s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
+        for (size_t i = 0; i < depths.size(); ++i) a.zd.push_back({depths[i], pitches[i]});
+        const bgs_status st = call(a);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
     bgs_context* ctx_ = nullptr;
 };
 
