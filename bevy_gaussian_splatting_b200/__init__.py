@@ -4,7 +4,7 @@ Product = `csrc/` (hand-written sm_90a kernels + the C ABI of include/bgs.h, bui
 The Python modules here are the host-side mirror of the reference interface for this path
 (same names as mosure/bevy_gaussian_splatting: src/lib.rs:7-29 re-exports) used by tests and bench.
 """
-from .abi import BgsError  # noqa: F401
+from .abi import PICK_DTYPE, BgsError  # noqa: F401
 from .camera import GaussianCamera, View, headless_view, orbit_view, perspective_view  # noqa: F401
 from .gaussian import (PlanarGaussian3d, PlanarGaussian4d, random_gaussians_3d, random_gaussians_3d_seeded,  # noqa: F401
                        random_gaussians_4d_seeded, SH_COEFF_COUNT, SH_4D_COEFF_COUNT, SH_WIDTHS)

@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libbgs.so")
 
@@ -26,6 +28,7 @@ BGS_FLAG_VISUALIZE_BOUNDING_BOX = 64
 BGS_ENTITY_VISUALIZE_BOUNDING_BOX = 1
 BGS_SCENE_MAX_CLOUDS = 64
 BGS_SELECT_REPLACE, BGS_SELECT_ADD = 0, 1
+BGS_PICK_NONE = 0xFFFFFFFF
 
 
 class bgs_view(C.Structure):
@@ -149,6 +152,14 @@ class bgs_khr_primitive(C.Structure):
     ]
 
 
+class bgs_pick(C.Structure):
+    """One pixel of a pick frame (bgs_render_entities_pick), 16 B; the numpy twin is PICK_DTYPE."""
+    _fields_ = [("entity", C.c_uint32), ("index", C.c_uint32), ("weight", C.c_float), ("depth", C.c_float)]
+
+
+PICK_DTYPE = np.dtype([("entity", "<u4"), ("index", "<u4"), ("weight", "<f4"), ("depth", "<f4")])
+
+
 # every symbol include/bgs.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = [
@@ -169,6 +180,8 @@ SYMBOLS = [
     ("bgs_cloud_visibility_get", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_visibility_set", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_select_in_mesh", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32, _P, C.c_uint32, C.POINTER(C.c_uint32)]),
+    ("bgs_cloud_select_in_view", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_view), _P, C.c_int, C.c_uint32,
+                                           C.POINTER(C.c_uint32)]),
     ("bgs_cloud_subset", C.c_int, [_P, _P, _P, C.c_uint32, C.POINTER(_P), C.POINTER(C.c_uint32)]),
     ("bgs_cloud_download_f32", C.c_int, [_P, _P, _P, _P, _P, _P]),
     ("bgs_cloud_download_f16", C.c_int, [_P, _P, _P, _P, _P]),
@@ -204,6 +217,10 @@ SYMBOLS = [
                                           C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
                                           C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, _P, _P, C.c_uint32,
                                           C.c_int]),
+    ("bgs_render_entities_pick", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P,
+                                           C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
+                                           C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int,
+                                           _P]),
     ("bgs_render_views", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P, C.c_uint32,
                                    C.POINTER(bgs_view), C.c_uint32, C.POINTER(bgs_settings), C.POINTER(bgs_scene_depth), _P,
                                    C.c_uint32, C.c_int]),

@@ -206,6 +206,9 @@ struct FrameOut {
     void* view_host_depth[MAX_VIEWS] = {};
     void* view_host_normal[MAX_VIEWS] = {};
     size_t view_bytes[MAX_VIEWS] = {};
+    // a pick frame (bgs_render_entities_pick): its device records, the host target they are copied to (else NULL)
+    uint4* pick = nullptr;
+    void* host_pick = nullptr;
 };
 
 // A views frame's targets: view i's frame into rgba[i] and, on aux frames, its depth and normal frames into depth[i] and
@@ -288,6 +291,35 @@ bgs_status frame_out_views(bgs_context* c, const bgs_settings* st, uint32_t form
 }
 
 }  // namespace
+
+namespace bgs {
+
+FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                                const bgs_settings* st, bool want_aux) {
+    const int W = (int)view->viewport[2], H = (int)view->viewport[3];
+    FrameConsts fc;
+    memcpy(fc.model, uni->transform, 64);
+    memcpy(fc.view_from_world, view->view_from_world, 64);
+    memcpy(fc.clip_from_world, view->clip_from_world, 64);
+    memcpy(fc.cam, view->world_position, 12);
+    fc.W = view->viewport[2]; fc.H = view->viewport[3];
+    fc.p00 = view->clip_from_view[0]; fc.p11 = view->clip_from_view[5];
+    fc.global_opacity = uni->global_opacity; fc.global_scale = uni->global_scale;
+    fc.color_space = uni->color_space;
+    fc.key_shift = 32u - st->radix_sort_depth_bits;
+    fc.gaussian_mode = st->gaussian_mode; fc.rasterize_mode = st->rasterize_mode; fc.aabb = st->aabb;
+    fc.adaptive = st->opacity_adaptive_radius; fc.draw_mode = st->draw_mode;
+    fc.Wi = W; fc.Hi = H; fc.tiles_x = (W + TILE_PX - 1) / TILE_PX; fc.tiles_y = (H + TILE_PX - 1) / TILE_PX;
+    fc.n_cloud = cloud->n;
+    fc.aux = want_aux ? 1u : 0u;
+    fc.cov_pre = cloud->layout == CloudLayout::F16Cov ? 1u : 0u;
+    memcpy(fc.aabb_min, uni->aabb_min, 12); memcpy(fc.aabb_max, uni->aabb_max, 12);
+    static const float kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    fc.model_identity = memcmp(uni->transform, kIdentity, 64) == 0 ? 1u : 0u;   // (-0.0 entries take the general path)
+    return fc;
+}
+
+}  // namespace bgs
 
 extern "C" {
 
@@ -478,30 +510,6 @@ static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs
     return BGS_OK;
 }
 
-static FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                                const bgs_settings* st, bool want_aux) {
-    const int W = (int)view->viewport[2], H = (int)view->viewport[3];
-    FrameConsts fc;
-    memcpy(fc.model, uni->transform, 64);
-    memcpy(fc.view_from_world, view->view_from_world, 64);
-    memcpy(fc.clip_from_world, view->clip_from_world, 64);
-    memcpy(fc.cam, view->world_position, 12);
-    fc.W = view->viewport[2]; fc.H = view->viewport[3];
-    fc.p00 = view->clip_from_view[0]; fc.p11 = view->clip_from_view[5];
-    fc.global_opacity = uni->global_opacity; fc.global_scale = uni->global_scale;
-    fc.color_space = uni->color_space;
-    fc.key_shift = 32u - st->radix_sort_depth_bits;
-    fc.gaussian_mode = st->gaussian_mode; fc.rasterize_mode = st->rasterize_mode; fc.aabb = st->aabb;
-    fc.adaptive = st->opacity_adaptive_radius; fc.draw_mode = st->draw_mode;
-    fc.Wi = W; fc.Hi = H; fc.tiles_x = (W + TILE_PX - 1) / TILE_PX; fc.tiles_y = (H + TILE_PX - 1) / TILE_PX;
-    fc.n_cloud = cloud->n;
-    fc.aux = want_aux ? 1u : 0u;
-    fc.cov_pre = cloud->layout == CloudLayout::F16Cov ? 1u : 0u;
-    memcpy(fc.aabb_min, uni->aabb_min, 12); memcpy(fc.aabb_max, uni->aabb_max, 12);
-    static const float kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    fc.model_identity = memcmp(uni->transform, kIdentity, 64) == 0 ? 1u : 0u;   // (-0.0 entries take the general path)
-    return fc;
-}
 
 // Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.  A scene frame
 // (render_entities_impl) runs key-gen, the depth range, the projection and the splat depths over its segment table; `cloud`
@@ -579,7 +587,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             const uint32_t g = scene->groups[i];
             if (g == PROJECT_GROUP_4D) {   // (also writes the 4D segments' splat depths, from the moved positions)
                 launch_project_4d_scene(scene->tab, scene->times, scene->classes, *modes, c->slot_ids.p, c->ctr, c->recs.p,
-                                        zd ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
+                                        zd || o.pick ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
             } else {
                 launch_project_scene(scene->tab, g, scene->need_sh[i] != 0, scene->classes, *modes, c->slot_ids.p, c->ctr,
                                      c->recs.p, (p.raster_mode == 2 || p.raster_mode == 4) ? c->extra.p : nullptr, p.n_hint,
@@ -599,9 +607,9 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     }
     if (!scene) ++launches;
     CU(c, cudaEventRecord(c->ev_p1, ps));
-    // depth-tested frames: the splat depths, indexed like the records (the projection's index list)
+    // depth-tested and pick frames: the splat depths, indexed like the records (the projection's index list)
     ZTestArgs zt;
-    if (zd && scene_3d) {
+    if ((zd || o.pick) && scene_3d) {
         launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
     } else if (zd && !tc && !scene) {
@@ -610,6 +618,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
         ++launches;
     }
     if (zd) { zt.splat_d = c->splat_depth.p; zt.scene = zd->depth; zt.pitch = (size_t)zd->pitch_bytes; }
+    if (o.pick) zt.splat_d = c->splat_depth.p;
     if (p.overlap) {
         CU(c, cudaEventRecord(c->ev_join, c->stream2));
         CU(c, cudaStreamWaitEvent(q, c->ev_join, 0));
@@ -653,7 +662,11 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             // the blend runs on the LOW-priority stream; the render stream resumes once it is done
             CU(c, cudaEventRecord(c->ev_front, q));
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
-            if (views)
+            if (o.pick)
+                launch_raster_pick(p.raster_mode, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
+                                   fc.tiles_y, o.rgba, o.raster_format, &c->ctr->truncated, zt, c->kinds.p, p.box,
+                                   PickArgs{o.pick, c->slot_ids.p, scene->kinds}, c->stream_r);
+            else if (views)
                 launch_raster_views(p.raster_mode, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, o.raster_format,
                                     &c->ctr->truncated, zt.splat_d, c->kinds.p, p.box, *views, c->stream_r,
                                     fc.aux ? c->aux.p : nullptr);
@@ -701,9 +714,11 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaMemcpyAsync(o.host_depth, o.depth, o.bytes, cudaMemcpyDeviceToHost, q));
             CU(c, cudaMemcpyAsync(o.host_normal, o.normal, o.bytes, cudaMemcpyDeviceToHost, q));
         }
+        if (o.host_pick)
+            CU(c, cudaMemcpyAsync(o.host_pick, o.pick, (size_t)fc.Wi * fc.Hi * sizeof(bgs_pick), cudaMemcpyDeviceToHost, q));
     }
     c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, views ? (int)num_tiles : fc.tiles_x, views ? 1 : fc.tiles_y, fc.Wi,
-               fc.Hi, o.rgba, zd != nullptr, scene};
+               fc.Hi, o.rgba, zd != nullptr || o.pick != nullptr, scene};
     c->launches = launches;
     return BGS_OK;
 }
@@ -731,7 +746,8 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
                               const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
                               int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal,
                               const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr,
-                              const std::shared_ptr<const SceneFacts>& scene = nullptr, const ViewTargets* view_targets = nullptr) {
+                              const std::shared_ptr<const SceneFacts>& scene = nullptr, const ViewTargets* view_targets = nullptr,
+                              void* out_pick = nullptr) {
     if (!c) return BGS_EINVAL;
     if (!scene) TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));   // (scenes: per cloud, before)
     if (zd) TRY(check_scene_depth(c, zd, view));
@@ -756,6 +772,13 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     if (views) TRY(frame_out_views(c, st, out_format, scene->views, *view_targets, out_is_device_ptr, &o));
     else TRY(frame_out(c, st, out_format, (size_t)fc.Wi * fc.Hi * format_bpp(out_format), out_rgba, out_is_device_ptr, want_aux,
                        out_depth, out_normal, &o));
+    if (out_pick && out_is_device_ptr) {
+        o.pick = static_cast<uint4*>(out_pick);
+    } else if (out_pick) {
+        TRY(c->pick_frame.grow(c, (size_t)fc.Wi * fc.Hi * sizeof(bgs_pick), false));
+        o.pick = c->pick_frame.p;
+        o.host_pick = out_pick;
+    }
     ViewTable vt = {};
     if (views) {
         vt = scene->views;
@@ -774,7 +797,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         if (p.raster_mode == 2 || p.raster_mode == 4) TRY(c->extra.grow(c, (size_t)c->cap_n * 64, false));
         if (p.raster_mode >= 3) TRY(c->kinds.grow(c, (size_t)c->cap_n, false));
         if (want_aux) TRY(c->aux.grow(c, (size_t)c->cap_n * 32, false));
-        if (zd) TRY(c->splat_depth.grow(c, (size_t)c->cap_n * 4, false));
+        if (zd || o.pick) TRY(c->splat_depth.grow(c, (size_t)c->cap_n * 4, false));
         if (p.rounds > 1) TRY(c->state.grow(c, (size_t)num_tiles * 256 * sizeof(float4), false));
         TRY(ensure_arena(c, num_tiles));
         TRY(ensure_status(c, c->status_depth, c->status_n, n));
@@ -856,7 +879,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
                                        const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
                                        void* out_rgba, uint32_t out_format, int out_is_device_ptr, bool want_aux = false,
                                        void* out_depth = nullptr, void* out_normal = nullptr, uint32_t nv = 1,
-                                       const ViewTargets* view_targets = nullptr) {
+                                       const ViewTargets* view_targets = nullptr, void* out_pick = nullptr) {
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
         return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
@@ -955,9 +978,9 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     sf.gaussian_mode = scene->raster_mode == 2 ? BGS_GAUSSIAN_2D : BGS_GAUSSIAN_3D;
     sf.draw_mode = BGS_DRAW_ALL;
     if (scene->box) sf.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
-    if (nv > 1) sf.flags = (sf.flags & ~(uint32_t)BGS_FLAG_CHUNKS) | BGS_FLAG_NO_CHUNKS;   // (one round)
+    if (nv > 1 || out_pick) sf.flags = (sf.flags & ~(uint32_t)BGS_FLAG_CHUNKS) | BGS_FLAG_NO_CHUNKS;   // (one round)
     return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, want_aux, out_depth,
-                       out_normal, depth, nullptr, scene, view_targets);
+                       out_normal, depth, nullptr, scene, view_targets, out_pick);
 }
 
 // bgs_render_scene, and bgs_render_scene_4d (with_4d: Gaussian4d clouds are projected at uniforms[j].time in windows[j];
@@ -1058,6 +1081,24 @@ bgs_status bgs_render_entities_aux(bgs_context* c, const bgs_cloud* const* cloud
     }
     return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
                                 out_is_device_ptr, true, out_depth, out_normal);
+}
+
+// bgs_render_entities_ex's frame and, from the same blend, its pick frame (include/bgs.h): the refusals of
+// bgs_render_entities_ex, then those of the pick target
+bgs_status bgs_render_entities_pick(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                    const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k,
+                                    const bgs_view* view, const bgs_settings* frame, const bgs_render_extras* ex,
+                                    const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format, int out_is_device_ptr,
+                                    void* out_pick) {
+    const char* call = "render_entities_pick";
+    if (!c) return BGS_EINVAL;
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
+    if (!out_pick) return fail(c, BGS_EINVAL, "%s: out_pick is NULL", call);
+    if (out_is_device_ptr && reinterpret_cast<uintptr_t>(out_pick) % sizeof(bgs_pick) != 0)
+        return fail(c, BGS_EINVAL, "%s: device pick target %p is not aligned to its 16-byte records", call, out_pick);
+    if (frame->flags & BGS_FLAG_ASYNC) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
+                                out_is_device_ptr, false, nullptr, nullptr, 1, nullptr, out_pick);
 }
 
 // bgs_render_entities_ex of each of v views in one frame (include/bgs.h): the refusals of bgs_render_entities_ex (each view

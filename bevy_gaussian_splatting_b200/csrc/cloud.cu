@@ -451,6 +451,46 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* c, bgs_cloud* cl, const float* 
     return BGS_OK;
 }
 
+bgs_status bgs_cloud_select_in_view(bgs_context* c, bgs_cloud* cl, const bgs_cloud_uniform* uni, const bgs_view* view,
+                                    const uint8_t* mask, int mask_is_device_ptr, uint32_t mode, uint32_t* out_inside) {
+    if (!c) return BGS_EINVAL;
+    if (!cl || !uni || !view || !mask) return fail(c, BGS_EINVAL, "select_in_view: null cloud, uniform, view or mask");
+    if (mode != BGS_SELECT_REPLACE && mode != BGS_SELECT_ADD) return fail(c, BGS_EINVAL, "select_in_view: unknown mode %u", mode);
+    TRY(enter_call(c, "select_in_view", cl->device));
+    if (is_4d(cl->layout))
+        return fail(c, BGS_EINVAL, "select_in_view: a Gaussian4d cloud (its drawn position depends on time: use bgs_render_entities_pick)");
+    const int W = (int)view->viewport[2], H = (int)view->viewport[3];
+    if (W <= 0 || H <= 0 || W > 65535 || H > 65535) return fail(c, BGS_EINVAL, "select_in_view: viewport %dx%d out of range", W, H);
+    if (mask_is_device_ptr) {
+        cudaPointerAttributes a = {};
+        const cudaError_t e = cudaPointerGetAttributes(&a, mask);
+        if (e != cudaSuccess) cudaGetLastError();   // (an unknown pointer: clear the error, refuse below)
+        if (e != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != c->device)
+            return fail(c, BGS_EINVAL, "select_in_view: mask %p is not device memory of device %d", (const void*)mask, c->device);
+    }
+    // the render calls' frame constants: only the model, the clip matrix and the viewport are read
+    bgs_settings st = {};
+    st.radix_sort_depth_bits = 32;
+    const FrameConsts fc = frame_consts(cl, view, uni, &st, false);
+    TRY(before_cloud_write(c, cl));
+    cudaStream_t q = c->stream;
+    const size_t mask_bytes = (size_t)W * H;
+    TRY(c->view_select.grow(c, 256 + (mask_is_device_ptr ? 0 : mask_bytes), false));
+    uint32_t* word = reinterpret_cast<uint32_t*>(c->view_select.p);
+    const uint8_t* dmask = mask;
+    if (!mask_is_device_ptr) {
+        CU(c, cudaMemcpyAsync(c->view_select.p + 256, mask, mask_bytes, cudaMemcpyHostToDevice, q));
+        dmask = c->view_select.p + 256;
+    }
+    CU(c, cudaMemsetAsync(word, 0, 4, q));
+    launch_view_select(cl->view(), cl->n, fc, dmask, mode, word, q);
+    CU(c, cudaGetLastError());
+    uint32_t inside = 0;
+    TRY(read_word(c, word, &inside));
+    if (out_inside) *out_inside = inside;
+    return BGS_OK;
+}
+
 // ---- particle behaviours (particles.cu).  The step is a queued write (host.cuh: queue_cloud_write), never drained;
 // it also orders itself after the behaviours' earlier steps and marks itself on them.
 

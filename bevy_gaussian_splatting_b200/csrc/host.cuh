@@ -95,7 +95,7 @@ struct FrameFacts {
     int rounds = 1;                     // binning rounds
     int tiles_x = 0, tiles_y = 0, W = 0, H = 0;   // (a views frame: every view's tiles x 1, view 0's W x H)
     const void* target = nullptr;       // the device frame the blend wrote
-    bool depth_tested = false;          // bgs_render_depth_test with a depth buffer: splat_depth holds the splats' d
+    bool depth_tested = false;          // a depth buffer or a pick frame (bgs_render_entities_pick): splat_depth holds the splats' d
     std::shared_ptr<const SceneFacts> scene;   // bgs_render_scene frames only (nulled with `cloud`)
     bool reads(const bgs_cloud* cl) const {
         if (cloud == cl) return true;
@@ -144,6 +144,7 @@ struct bgs_context {
     DevBuf<float> splat_depth;        // 1 float per record: the splat depths d of depth-tested frames (allocated on first use)
     DevBuf<unsigned char> kinds;      // 1 byte per record: the blend kind of a mixed-geometry frame's splats (first use)
     DevBuf<void> frame_aux[2];        // depth / normal frames when an aux frame delivers to host memory (views: every view's)
+    DevBuf<uint4> pick_frame;         // the pick frame when bgs_render_entities_pick delivers to host memory
     // scratch sized by the pair capacity (grow-only; cap_pairs pairs)
     uint32_t cap_pairs = 0;
     DevBuf<uint32_t> pkeys[2], pvals[2];
@@ -161,6 +162,8 @@ struct bgs_context {
     // bgs_cloud_select_in_mesh's own scratch (never the frame's): words | vertices | indices | binned records | binned
     // boxes | global records, and the pair side: digit histograms | per-cell ranges | pair keys / values x 2
     DevBuf<uint8_t> mesh_tri, mesh_pairs;
+    // bgs_cloud_select_in_view's own scratch: its count word | a host mask's device copy
+    DevBuf<uint8_t> view_select;
     bool async_pending = false;        // a BGS_FLAG_ASYNC frame has been enqueued and not yet completed
     bool step_pending = false;         // a particle step has been enqueued since the last bgs_sync
     // an interpolation (a queued write that reads other clouds) has been enqueued since the last bgs_sync: ev_done
@@ -312,6 +315,11 @@ bgs_status queue_cloud_write_reading(bgs_context* c, bgs_cloud* cl, const bgs_cl
         return BGS_OK;
     });
 }
+
+// the frame constants the render calls build for a cloud, uniform, view and settings (api.cu); bgs_cloud_select_in_view
+// builds its own with them
+FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni, const bgs_settings* st,
+                         bool want_aux);
 
 // ---- frame scratch (api.cu) that the selections borrow
 int pair_passes(uint32_t num_tiles);

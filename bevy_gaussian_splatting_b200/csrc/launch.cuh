@@ -103,6 +103,19 @@ void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, c
 void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
                          uint32_t format, const uint32_t* truncated, const float* splat_d, const unsigned char* kinds, bool box,
                          const ViewTable& vt, cudaStream_t stream, const float4* aux = nullptr);
+// bgs_render_entities_pick: launch_raster's frame (mode and box as there, never raster2_kernel) and, per pixel, the pick
+// record (include/bgs.h's bgs_pick) into `out`, from the record's global index (slot_ids) and segment (seg: offsets and
+// k) and its depth zt.splat_d[record] (a pick frame's splat depths, written with or without a depth buffer; zt.scene
+// NULL: no depth test)
+struct PickArgs {
+    uint4* out;
+    const uint32_t* slot_ids;
+    SegmentKinds seg;
+};
+static_assert(sizeof(bgs_pick) == sizeof(uint4), "a pick record is stored as one uint4");
+void launch_raster_pick(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
+                        int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format, const uint32_t* truncated,
+                        const ZTestArgs& zt, const unsigned char* kinds, bool box, const PickArgs& pk, cudaStream_t stream);
 void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
                          int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
                          uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,
@@ -131,6 +144,10 @@ uint32_t mesh_words_n_bin(const void* words_host);
 void launch_mesh_count(CloudView cloud, uint32_t n, const float* mesh_from_cloud, const void* bin_rec, const void* glob_rec,
                        const uint32_t* cell_tri, const uint2* ranges, const void* words_host, int level, uint32_t mode, void* words,
                        cudaStream_t stream);
+// view_select.cu: bgs_cloud_select_in_view's pass (fc: the frame constants of the cloud, uniform and view; mask Hi x Wi
+// bytes on the device; mode as the mesh selection's; *inside += the gaussians inside)
+void launch_view_select(CloudView cloud, uint32_t n, const FrameConsts& fc, const uint8_t* mask, uint32_t mode,
+                        uint32_t* inside, cudaStream_t stream);
 // particles.cu
 void launch_particle_step(void* behaviors, uint32_t count, float dt, CloudView cloud, cudaStream_t stream);
 // subset.cu

@@ -263,14 +263,19 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // tiles_x, out, scene and pitch are then view i's, the CTA takes the local tile blockIdx.x - tile0[i] in centre_out_tile's
 // order within the view, and reads the global tile's range.  With AUX (raster_views_aux_kernel, bgs_render_views_aux)
 // out_depth and out_normal are view i's too.
-template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false>
+// PICK (raster_pick_kernel, bgs_render_entities_pick): beside its colour each pixel keeps the largest weight w = a T of the
+// pairs it blends (an overlay edge pair: w = T) and that pair's record; a later pair replaces it only when its w is strictly
+// larger.  Every pixel of pk->out is written: (entity, index, w, d) of that pair, or BGS_PICK_NONE where nothing blends.
+// Pick frames take the generic loop in every mode, never the inline-asm one.
+template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false, bool PICK = false>
 __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
                                             const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
                                             int H, int tiles_x, void* __restrict__ out, uint32_t format,
                                             const float4* __restrict__ aux, void* __restrict__ out_depth,
                                             void* __restrict__ out_normal, const uint32_t* __restrict__ truncated,
                                             const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
-                                            const unsigned char* __restrict__ kinds, const ViewTable* vt = nullptr) {
+                                            const unsigned char* __restrict__ kinds, const ViewTable* vt = nullptr,
+                                            const PickArgs* pk = nullptr) {
     constexpr bool MIXED = MODE >= 3, SURF = MODE == 2 || MODE == 4;
     __shared__ __align__(16) unsigned char s_mem[(SURF ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0) +
                                                  (ZTEST && !AUX ? ZT_BYTES : 0)];
@@ -317,6 +322,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
 
     if (range.x >= range.y) {            // empty tile: nothing to stage (uniform across the CTA)
         // (blend-over mode leaves the target's pixels as they are)
+        if (PICK && inside) pk->out[(size_t)py * W + px] = make_uint4(BGS_PICK_NONE, BGS_PICK_NONE, 0u, 0u);
         if (inside && !((format >> 8) & OUT_OVER)) {
             write_pixel(out, format, (size_t)py * W + px, 0.f, 0.f, 0.f, 1.0f);
             if (AUX) {
@@ -336,6 +342,8 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
 
     float T = inside ? 1.0f : 0.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f;   // T < T_STOP <=> this pixel is done
     float dr = 0.0f, dg = 0.0f, db = 0.0f, nr = 0.0f, ng = 0.0f, nb = 0.0f;   // AUX: depth / normal frames
+    float best_w = -1.0f;               // PICK: the largest w so far (-1: none), and its record
+    uint32_t best_r = BGS_PICK_NONE;
     for (uint32_t base = range.x; base < range.y; base += RT_CHUNK, ++ps.chunk) {
         if (__syncthreads_count(T < T_STOP ? 0 : 1) == 0) break;   // also fences reuse of the staging buffers
         const uint32_t cnt = min((uint32_t)RT_CHUNK, range.y - base);
@@ -395,7 +403,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
             if (ZTEST && hit) hit = !(reinterpret_cast<const float*>(s_mem + REC_D)[4 * j] < zmin);
             return hit;
         });
-        if (MODE == 0 && !AUX && !BOX) {
+        if (MODE == 0 && !AUX && !BOX && !PICK) {
             // four candidates per iteration, so loop control is paid once per four; each list entry is its own 16-bit
             // load (cheaper than unpacking a 32-bit pair); blending stays strictly in list order.
             // The blend is PREDICATED, not branched: 15 SASS instructions per candidate instead of a divergent block
@@ -524,6 +532,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                     e = __expf(power);
                 }
                 if (BOX && edge) {   // the overlay colour at alpha exactly 1 (w = T) into every frame; T = 0 stops the pixel
+                    if (PICK && T > best_w) { best_w = T; best_r = ps.entry(base, (a_rec - a_base) >> 4); }
                     cr = fmaf(T, 0.3f, cr); cg = fmaf(T, 1.0f, cg); cb = fmaf(T, 0.1f, cb);
                     if (AUX) {
                         dr = fmaf(T, 0.3f, dr); dg = fmaf(T, 1.0f, dg); db = fmaf(T, 0.1f, db);
@@ -534,6 +543,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                 }
                 const float a = fminf(e * q2.w, 0.999f);
                 const float w = a * T;
+                if (PICK && w > best_w) { best_w = w; best_r = ps.entry(base, (a_rec - a_base) >> 4); }
                 cr = fmaf(w, q2.x, cr); cg = fmaf(w, q2.y, cg); cb = fmaf(w, q2.z, cb);
                 if (AUX) {
                     const float4 ad = lds4(a_rec + SM_AUX), an = lds4(a_rec + SM_AUX + RT_CHUNK * 16);
@@ -548,6 +558,19 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
     ps.finish();
     if (!inside) return;
     write_pixel(out, format, (size_t)py * W + px, cr, cg, cb, T);
+    if constexpr (PICK) {   // record -> global index (compact slot) -> (entity, index within its cloud), and its d
+        uint4 rec = make_uint4(BGS_PICK_NONE, BGS_PICK_NONE, 0u, 0u);
+        if (best_r != BGS_PICK_NONE) {
+            const uint32_t g = __ldg(pk->slot_ids + best_r);
+            uint32_t lo = 0u, hi = pk->seg.k;   // the last j with offset <= g (SceneTable::find)
+            while (hi - lo > 1u) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (pk->seg.offset[mid] <= g) lo = mid; else hi = mid;
+            }
+            rec = make_uint4(lo, g - pk->seg.offset[lo], __float_as_uint(best_w), __float_as_uint(__ldg(splat_d + best_r)));
+        }
+        pk->out[(size_t)py * W + px] = rec;
+    }
     if (AUX) {
         write_pixel(out_depth, format, (size_t)py * W + px, dr, dg, db, T);
         write_pixel(out_normal, format, (size_t)py * W + px, nr, ng, nb, T);
@@ -641,6 +664,19 @@ raster_views_aux_kernel(const SplatRec* __restrict__ recs, const float4* __restr
                         const __grid_constant__ ViewTable vt) {
     raster_body<MODE, true, ZTEST, BOX, true>(recs, extra, tile_entries, ranges, 0, 0, 0, nullptr, format, aux, nullptr,
                                               nullptr, truncated, splat_d, nullptr, 0, kinds, &vt);
+}
+
+// bgs_render_entities_pick's blends: raster_kernel's (MODE 0..2), raster_mixed_kernel's (3, 4) and their BOX kernels', with
+// the pick frame (raster_body's PICK).  Kernels of their own, so every other frame keeps the very kernels it had.  (At 5
+// CTAs per SM MODE 1 and 2 spill even without the depth test or the overlay: 4 leave every variant 64 registers.)
+template <int MODE, bool ZTEST, bool BOX>
+__global__ void __launch_bounds__(RT_THREADS, 4)
+raster_pick_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
+                   const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
+                   const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
+                   size_t pitch, const unsigned char* __restrict__ kinds, const __grid_constant__ PickArgs pk) {
+    raster_body<MODE, false, ZTEST, BOX, false, true>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr,
+                                                      nullptr, nullptr, truncated, splat_d, scene, pitch, kinds, nullptr, &pk);
 }
 
 // the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
@@ -928,6 +964,20 @@ void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, co
 #undef VIEWS_ROW_
     kernels[splat_d != nullptr][box][mode]<<<vt.tile0[vt.v], RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, format,
                                                                                      truncated, splat_d, kinds, vt);
+}
+
+void launch_raster_pick(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
+                        int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format, const uint32_t* truncated,
+                        const ZTestArgs& zt, const unsigned char* kinds, bool box, const PickArgs& pk, cudaStream_t stream) {
+    using Kernel = void (*)(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*, uint32_t,
+                            const uint32_t*, const float*, const float*, size_t, const unsigned char*, const PickArgs);
+#define PICK_ROW_(Z, B) {raster_pick_kernel<0, Z, B>, raster_pick_kernel<1, Z, B>, raster_pick_kernel<2, Z, B>, \
+                         raster_pick_kernel<3, Z, B>, raster_pick_kernel<4, Z, B>}
+    static const Kernel kernels[2][2][5] = {{PICK_ROW_(false, false), PICK_ROW_(false, true)},
+                                            {PICK_ROW_(true, false), PICK_ROW_(true, true)}};
+#undef PICK_ROW_
+    kernels[zt.scene != nullptr][box][mode]<<<tiles_x * tiles_y, RT_THREADS, 0, stream>>>(
+        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, truncated, zt.splat_d, zt.scene, zt.pitch, kinds, pk);
 }
 
 // One front-to-back round of a chunked frame (quad-uv records only); see raster2_kernel.

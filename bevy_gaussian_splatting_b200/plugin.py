@@ -564,6 +564,25 @@ class GaussianSplattingPlugin:
                                                       code, 0))
         return outs
 
+    def render_entities_pick(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None,
+                             previous_view: View | None = None, delta_time: float | None = None, premultiplied: bool = False,
+                             blend_over: bool = False) -> tuple[np.ndarray, np.ndarray]:
+        """`render_entities`' frame and, from the same pass, its pick frame (`bgs_render_entities_pick`): returns (rgba,
+        pick), pick an (h, w) array of abi.PICK_DTYPE -- per pixel the entity and gaussian index of the pair with the
+        largest blend weight w = a T, that w and the splat's depth d (BGS_PICK_NONE, 0, 0 where nothing blends).  rgba is
+        byte for byte `render_entities`' frame.  Validates like `render_entities` (`check_entities`, ValueError before any
+        call).  Synchronous only; `blend_over` applies to rgba only."""
+        entities = list(entities)
+        first = check_entities(entities)
+        code, dtype, ch = self.FORMATS[fmt]
+        out = np.empty((view.height, view.width, ch), dtype)
+        pick = np.empty((view.height, view.width), abi.PICK_DTYPE)
+        args = self._entities_args(entities, first, view, previous_view, delta_time, False, premultiplied, blend_over)
+        zd = self._scene_depth(scene_depth, view)
+        self._check(self._lib.bgs_render_entities_pick(self._ctx, *args, None if zd is None else C.byref(zd), _ptr(out), code, 0,
+                                                       _ptr(pick)))
+        return out, pick
+
     def render_views(self, entities, views, fmt: str = "rgba32f", scene_depths=None, asynchronous: bool = False,
                      premultiplied: bool = False, outs=None) -> list[np.ndarray]:
         """`render_entities` of every view in `views` (a sequence of View) in ONE frame (`bgs_render_views`): returns one
@@ -772,6 +791,81 @@ class GaussianSplattingPlugin:
         self._check(self._lib.bgs_cloud_select_in_mesh(self._ctx, handle._h, _ptr(v), len(v), _ptr(i), len(i),
                                                        None if m is None else _ptr(m), modes[mode], C.byref(inside)))
         return int(inside.value)
+
+    def select_in_view(self, handle: PlanarGaussian3dHandle, view: View, mask, transform: CloudTransform | None = None,
+                       mode: str = "replace") -> int:
+        """Rectangle, lasso and brush selection through the volume (`bgs_cloud_select_in_view`): a gaussian is inside when
+        the projection with `transform` and `view` finds it in the frustum and the mask pixel under its centre is set (the
+        exact rule: include/bgs.h).  `mask`: an (h, w) bool / uint8 numpy array, or an object with
+        `__cuda_array_interface__` of that shape and type in device memory (read after its producer stream's work, as
+        `scene_depth` is).  mode "replace": visibility 1 inside, 0 elsewhere; "add": 1 inside, the rest untouched.
+        Returns how many are inside."""
+        modes = {"replace": abi.BGS_SELECT_REPLACE, "add": abi.BGS_SELECT_ADD}
+        if mode not in modes:
+            raise ValueError(f"mode must be one of {sorted(modes)}")
+        shape = (view.height, view.width)
+        cai = getattr(mask, "__cuda_array_interface__", None)
+        if cai is not None:
+            if np.dtype(cai["typestr"]) not in (np.dtype(np.uint8), np.dtype(np.bool_)):
+                raise TypeError(f"mask must be bool or uint8, not {cai['typestr']}")
+            if tuple(cai["shape"]) != shape:
+                raise ValueError(f"mask must have shape {shape}, not {tuple(cai['shape'])}")
+            strides = cai.get("strides")
+            if strides is not None and tuple(strides) != (view.width, 1):
+                raise ValueError("mask must be C-contiguous")
+            if cai.get("stream") is not None:
+                _stream_wait(self.stream_ptr, int(cai["stream"]))
+            ptr, is_device, keep = C.c_void_p(int(cai["data"][0])), 1, mask
+        else:
+            m = np.asarray(mask)
+            if m.dtype not in (np.dtype(np.uint8), np.dtype(np.bool_)):
+                raise TypeError(f"mask must be bool or uint8, not {m.dtype}")
+            if m.shape != shape:
+                raise ValueError(f"mask must have shape {shape}, not {m.shape}")
+            keep = np.ascontiguousarray(m).view(np.uint8)
+            ptr, is_device = _ptr(keep), 0
+        u = self.cloud_uniform(CloudSettings(), transform, handle.aabb)
+        v = view.to_abi()
+        inside = C.c_uint32()
+        self._check(self._lib.bgs_cloud_select_in_view(self._ctx, handle._h, C.byref(u), C.byref(v), ptr, is_device, modes[mode],
+                                                       C.byref(inside)))
+        del keep
+        return int(inside.value)
+
+    def select_picked(self, entities, pick: np.ndarray, mask=None, min_weight: float = 0.0, mode: str = "replace") -> int:
+        """Select what a pick frame shows (host-side, over `set_visibility`): for each distinct handle among `entities`
+        (the list `render_entities_pick` rendered), the gaussians picked at the pixels where `mask` ((h, w) bool; None:
+        every pixel) is set, with weight >= min_weight.  Instances of one cloud select into that one cloud.  mode
+        "replace": each handle's visibility 1 at its picked gaussians, 0 elsewhere; "add": 1 there, the rest untouched.
+        Returns how many distinct (cloud, gaussian) pairs were picked."""
+        if mode not in ("replace", "add"):
+            raise ValueError("mode must be one of ['add', 'replace']")
+        entities = list(entities)
+        pick = np.asarray(pick)
+        if pick.dtype != abi.PICK_DTYPE or pick.ndim != 2:
+            raise ValueError("pick must be an (h, w) array of PICK_DTYPE")
+        sel = (pick["entity"] != abi.BGS_PICK_NONE) & (pick["weight"] >= np.float32(min_weight))
+        if mask is not None:
+            mask = np.asarray(mask, bool)
+            if mask.shape != pick.shape:
+                raise ValueError(f"mask must have shape {pick.shape}, not {mask.shape}")
+            sel &= mask
+        ent, idx = pick["entity"][sel], pick["index"][sel]
+        if ent.size and int(ent.max()) >= len(entities):
+            raise ValueError(f"pick names entity {int(ent.max())}, but {len(entities)} entities were given")
+        handles = []
+        for h, _, _ in entities:
+            if not any(h is o for o in handles):
+                handles.append(h)
+        total = 0
+        for h in handles:
+            js = [j for j, (e, _, _) in enumerate(entities) if e is h]
+            mine = np.unique(idx[np.isin(ent, js)])
+            total += mine.size
+            vis = np.zeros(h.n, np.float32) if mode == "replace" else self.visibility(h)
+            vis[mine] = 1.0
+            self.set_visibility(h, vis)
+        return total
 
     def visibility(self, handle: PlanarGaussian3dHandle) -> np.ndarray:
         """The visibility lane of every gaussian, (n,) float32."""

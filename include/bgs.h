@@ -317,6 +317,26 @@ bgs_status bgs_cloud_select_in_mesh(bgs_context* ctx, bgs_cloud* cloud, const fl
                                     const float* mesh_from_cloud /* 16, column-major, may be NULL */, uint32_t mode,
                                     uint32_t* out_inside /* may be NULL */);
 
+/* bgs_cloud_select_in_view: selection through a screen-space mask -- rectangle, lasso and brush selection "through" the
+ * volume, whatever is occluded (the host rasterises the shape into the mask).  mode as bgs_cloud_select_in_mesh's:
+ * BGS_SELECT_REPLACE: visibility := inside ? 1.0 : 0.0; BGS_SELECT_ADD: 1.0 where inside, left untouched elsewhere.
+ * *out_inside (may be NULL) = how many gaussians are inside.  The rule, exactly:
+ *   - gaussian i is inside iff the projection, with this uniform's transform and this view, finds it in the frustum
+ *     (key-gen's in_frustum decision); its record centre (cx, cy) -- bit for bit what bgs_debug_projected reports for it --
+ *     satisfies 0 <= cx < w and 0 <= cy < h; and mask[floor(cy) * w + floor(cx)] != 0, with w = (int)viewport[2] and
+ *     h = (int)viewport[3].  A NaN centre is never inside;
+ *   - every gaussian takes part, whatever its visibility lane, draw mode or opacity; only the uniform's transform is read.
+ *   mask: h * w bytes, row-major, in host memory or (mask_is_device_ptr) device memory of the context's GPU.
+ *   Cost: one streaming pass over the position plane.  Synchronous; the quiesce rules of the writers above.  It uses its
+ *   own scratch, not the frame's: the bgs_debug_* hooks, bgs_frame_stats_get and bgs_stage_times_us keep reporting the
+ *   last frame, and the next frame's plan does not change.
+ *   A Gaussian4d cloud (its drawn position depends on time; bgs_render_entities_pick covers 4D); a NULL ctx, cloud,
+ *   uniform, view or mask; a viewport outside 1..65535; an unknown mode; a device mask that is not device memory of the
+ *   context's GPU; or a cloud on another device -> BGS_EINVAL.  A refused call changes nothing. */
+bgs_status bgs_cloud_select_in_view(bgs_context* ctx, bgs_cloud* cloud, const bgs_cloud_uniform* uniform, const bgs_view* view,
+                                    const uint8_t* mask /* h * w, row-major */, int mask_is_device_ptr, uint32_t mode,
+                                    uint32_t* out_inside /* may be NULL */);
+
 /* Keeping a selection as its own cloud, and reading a cloud back (the reference's save_selection,
  * src/query/select.rs:156-176: cloud.subset(indices), then write_to_file).
  *
@@ -806,6 +826,51 @@ bgs_status bgs_render_entities_aux(bgs_context* ctx, const bgs_cloud* const* clo
                                    const bgs_render_extras* extras, const bgs_scene_depth* depth /* may be NULL */,
                                    void* out_rgba, void* out_depth, void* out_normal, uint32_t out_format,
                                    int out_is_device_ptr);
+
+/* bgs_render_entities_ex's frame and, from the same pass, a pick frame: which gaussian the viewer sees at each pixel, for
+ * click-to-select, brush and rectangle tools, hover highlights, and "place at cursor" or "measure" (the depth under the
+ * cursor).  Per pixel, one 16 B bgs_pick record.
+ *
+ * The rule, exactly:
+ *   out_rgba.  Byte for byte the frame bgs_render_entities_ex produces with the same arguments: in all three formats, with
+ *     BGS_FLAG_PREMULTIPLIED_OUT and BGS_FLAG_BLEND_OVER_TARGET, per-entity and frame-wide bounding-box overlays, and under
+ *     a depth buffer.
+ *   Pairs.  The pairs a pixel's pick considers are exactly those that blend into its colour: each passes its splat's own
+ *     coverage decision (quad-uv, conic or surfel), the depth test when a buffer is given, and arrives while the pixel is
+ *     still alive (T >= T_STOP).
+ *   Weight.  A pair's weight is w = a * T, the f32 product the blend multiplies the splat's colour by (an overlay edge
+ *     pair has a = 1: w = T).
+ *   Pick.  The pair with the largest w.  On a tie the pair earlier in blend order wins: a later pair replaces the current
+ *     pick only when its w is strictly greater (a NaN w is never picked).
+ *   Record.  entity: the entity j of the picked splat.  index: its gaussian index i within cloud j, as uploaded (the
+ *     instances of one cloud differ in entity only).  weight: w.  depth: the splat depth d bgs_render_depth_test compares,
+ *     clip z / w of the splat's world position (a 4D entity's moved position).
+ *   Empty pixels.  A pixel where nothing blends gets {BGS_PICK_NONE, BGS_PICK_NONE, 0.0f, 0.0f} (0 is the reverse-Z far
+ *     value, a Depth32Float clear).
+ *   Targets.  out_pick (w * h records, row-major) shares out_is_device_ptr with out_rgba.  Every pixel of out_pick is
+ *     written: blend-over applies to out_rgba only.
+ *   Hooks and stats.  Sorted entries, tile ranges and slices, records and bgs_frame_stats are those of the same
+ *     bgs_render_entities_ex frame rendered in one round: a pick frame is never chunked (BGS_FLAG_CHUNKS is ignored).
+ *     After a pick frame bgs_debug_splat_depths reports every rank's d, whether or not a depth buffer was given.
+ *   Synchronous only.
+ * Launches: bgs_render_entities_ex's, plus the splat depths' when no depth buffer is given and a non-4D cloud is listed
+ *   (the blend itself writes the pick records).
+ * Refused with BGS_EINVAL, nothing enqueued or written and the previous frame's debug hooks kept: every refusal of
+ *   bgs_render_entities_ex; a NULL out_pick; a device out_pick not aligned to 16 B; BGS_FLAG_ASYNC.  NULL clouds,
+ *   uniforms, entities, view or frame -> BGS_NOT_READY. */
+typedef struct {
+    uint32_t entity;   /* entity j, or BGS_PICK_NONE */
+    uint32_t index;    /* gaussian index within cloud j, or BGS_PICK_NONE */
+    float weight;      /* w = a * T of the picked pair; 0 where nothing blends */
+    float depth;       /* its splat depth d; 0 where nothing blends */
+} bgs_pick;            /* 16 B */
+#define BGS_PICK_NONE 0xFFFFFFFFu   /* (a macro: C99 enumerators are ints) */
+bgs_status bgs_render_entities_pick(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                                    const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */,
+                                    uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                                    const bgs_render_extras* extras, const bgs_scene_depth* depth /* may be NULL */,
+                                    void* out_rgba, uint32_t out_format, int out_is_device_ptr,
+                                    void* out_pick /* w * h bgs_pick */);
 
 /* bgs_render_entities_ex of several views of one scene in ONE frame: stereo eyes, the six faces of a cube map, split-screen
  * and picture-in-picture cameras, or many cameras of a dataset share one key-gen, depth sort, projection, binning,

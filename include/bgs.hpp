@@ -134,6 +134,8 @@ inline PlanarGaussian3d random_gaussians_3d_seeded(size_t n, uint64_t seed) {
 // random_particle_behaviors (particle.rs:374-410): behaviour i moves gaussian i; velocity U(-1, 1), acceleration
 // U(-0.01, 0.01), jerk U(-1e-4, 1e-4) in all four lanes.  The same splitmix64 stream as above, seeded.
 using ParticleBehaviors = std::vector<bgs_particle_behavior>;
+// one pixel of a pick frame (bgs_render_entities_pick): entity, gaussian index, blend weight, splat depth
+using Pick = bgs_pick;
 inline ParticleBehaviors random_particle_behaviors(size_t n, uint64_t seed) {
     ParticleBehaviors b(n);
     uint64_t ctr = seed * 0x9E3779B97F4A7C15ull + 0x7654321ull;
@@ -433,36 +435,27 @@ public:
                          uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr, float delta_time = 0.0f,
                          const float* depth = nullptr, uint64_t pitch_bytes = 0, bool out_is_device = false,
                          uint32_t extra_flags = 0) {
-        if (entities.empty()) check(BGS_EINVAL);
-        std::vector<const bgs_cloud*> clouds;
-        std::vector<bgs_cloud_uniform> unis;
-        std::vector<bgs_entity_settings> ents;
-        std::vector<uint32_t> eflags;
-        for (const SceneEntity& e : entities) {
-            bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
-            std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
-            clouds.push_back(e.cloud->get());
-            unis.push_back(u);
-            const bgs_settings s = e.settings.to_abi();
-            ents.push_back({s.gaussian_mode, s.rasterize_mode, s.aabb, s.opacity_adaptive_radius, s.draw_mode,
-                            e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
-            eflags.push_back(e.settings.visualize_bounding_box ? (uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX : 0u);
-        }
-        bgs_settings s = entities[0].settings.to_abi(extra_flags);
-        if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
-        bgs_render_extras ex{};
-        ex.num_classes = 1;
-        if (previous_view) {
-            std::memcpy(ex.previous_clip_from_world, previous_view->clip_from_world, 64);
-            ex.delta_time = delta_time;
-        }
-        const bgs_scene_depth zd{depth, pitch_bytes};
-        const bgs_status st = bgs_render_entities_ex(ctx_, clouds.data(), unis.data(), ents.data(), eflags.data(),
-                                                     (uint32_t)clouds.size(), &view, &s, previous_view ? &ex : nullptr,
-                                                     depth ? &zd : nullptr, out_rgba, format, out_is_device ? 1 : 0);
-        if (st == BGS_NOT_READY) return false;
-        check(st);
-        return true;
+        return entities_call(entities, previous_view, delta_time, extra_flags, [&](const EntitiesArgs& a) {
+            const bgs_scene_depth zd{depth, pitch_bytes};
+            return bgs_render_entities_ex(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(),
+                                          (uint32_t)a.clouds.size(), &view, &a.s, a.ex, depth ? &zd : nullptr, out_rgba, format,
+                                          out_is_device ? 1 : 0);
+        });
+    }
+    // render_entities' frame and, from the same pass, its pick frame (bgs_render_entities_pick): out_pick receives w x h
+    // Pick records -- per pixel the entity and gaussian index of the pair with the largest blend weight, that weight and
+    // the splat's depth, or BGS_PICK_NONE.  out_pick shares out_is_device with out_rgba (a device one 16 B aligned).
+    // Synchronous only; the other arguments are render_entities'.
+    void render_entities_pick(const std::vector<SceneEntity>& entities, const bgs_view& view, void* out_rgba, void* out_pick,
+                              uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr,
+                              float delta_time = 0.0f, const float* depth = nullptr, uint64_t pitch_bytes = 0,
+                              bool out_is_device = false, uint32_t extra_flags = 0) {
+        entities_call(entities, previous_view, delta_time, extra_flags, [&](const EntitiesArgs& a) {
+            const bgs_scene_depth zd{depth, pitch_bytes};
+            return bgs_render_entities_pick(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(),
+                                            (uint32_t)a.clouds.size(), &view, &a.s, a.ex, depth ? &zd : nullptr, out_rgba, format,
+                                            out_is_device ? 1 : 0, out_pick);
+        });
     }
     // render_entities of each of `views` in one frame (bgs_render_views): out_rgba[i] receives views[i]'s frame, byte for
     // byte render_entities' frame of that view.  depths: one buffer per view (pitches[i] its row pitch), or empty.  No
@@ -521,6 +514,16 @@ public:
         uint32_t inside = 0;
         check(bgs_cloud_select_in_mesh(ctx_, cloud.get(), vertices.data(), (uint32_t)(vertices.size() / 3), indices.data(),
                                        (uint32_t)(indices.size() / 3), mesh_from_cloud, mode, &inside));
+        return inside;
+    }
+    // select_in_view: rectangle, lasso and brush selection through the volume (bgs_cloud_select_in_view): a gaussian is
+    // inside when the projection with `transform` and `view` finds it in the frustum and mask[floor(cy) w + floor(cx)] is
+    // set; mask h x w bytes, host or (mask_is_device) device memory; mode as select_in_mesh's; returns how many are inside.
+    uint32_t select_in_view(PlanarGaussian3dHandle& cloud, const bgs_view& view, const uint8_t* mask, bool mask_is_device = false,
+                            const Mat4& transform = Mat4::identity(), uint32_t mode = BGS_SELECT_REPLACE) {
+        const bgs_cloud_uniform u = cloud_uniform(CloudSettings{}, transform);
+        uint32_t inside = 0;
+        check(bgs_cloud_select_in_view(ctx_, cloud.get(), &u, &view, mask, mask_is_device ? 1 : 0, mode, &inside));
         return inside;
     }
     std::vector<float> visibility(const PlanarGaussian3dHandle& cloud) {
@@ -634,6 +637,45 @@ public:
 private:
     void check(bgs_status st) { if (st != BGS_OK) throw Error(st, bgs_last_error(ctx_)); }
     // the entity arrays of a render_views / render_views_aux call, and the call made with them (false: BGS_NOT_READY)
+    // the arguments of a bgs_render_entities_ex / _pick call of `entities`
+    struct EntitiesArgs {
+        std::vector<const bgs_cloud*> clouds;
+        std::vector<bgs_cloud_uniform> unis;
+        std::vector<bgs_entity_settings> ents;
+        std::vector<uint32_t> eflags;
+        bgs_settings s;
+        bgs_render_extras extras;
+        const bgs_render_extras* ex;
+    };
+    template <class Call>
+    bool entities_call(const std::vector<SceneEntity>& entities, const bgs_view* previous_view, float delta_time,
+                       uint32_t extra_flags, Call call) {
+        if (entities.empty()) check(BGS_EINVAL);
+        EntitiesArgs a;
+        for (const SceneEntity& e : entities) {
+            bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
+            std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
+            a.clouds.push_back(e.cloud->get());
+            a.unis.push_back(u);
+            const bgs_settings s = e.settings.to_abi();
+            a.ents.push_back({s.gaussian_mode, s.rasterize_mode, s.aabb, s.opacity_adaptive_radius, s.draw_mode,
+                              e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
+            a.eflags.push_back(e.settings.visualize_bounding_box ? (uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX : 0u);
+        }
+        a.s = entities[0].settings.to_abi(extra_flags);
+        if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) a.s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
+        a.extras = bgs_render_extras{};
+        a.extras.num_classes = 1;
+        if (previous_view) {
+            std::memcpy(a.extras.previous_clip_from_world, previous_view->clip_from_world, 64);
+            a.extras.delta_time = delta_time;
+        }
+        a.ex = previous_view ? &a.extras : nullptr;
+        const bgs_status st = call(a);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
     struct ViewsArgs {
         std::vector<const bgs_cloud*> clouds;
         std::vector<bgs_cloud_uniform> unis;
