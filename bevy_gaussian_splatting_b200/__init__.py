@@ -15,6 +15,6 @@ from .gcloud import decode_gcloud, encode_gcloud, read_gcloud, write_gcloud  # n
 from .particles import (PARTICLE_BEHAVIOR_DTYPE, PARTICLE_INACTIVE, ParticleBehaviors,  # noqa: F401
                         random_particle_behaviors)
 from .plugin import (CloudTransform, GaussianSplattingPlugin, ParticleBehaviorsHandle, PlanarGaussian3dHandle,  # noqa: F401
-                     PlanarGaussian4dHandle, SceneHandles)
+                     PlanarGaussian4dHandle, SceneHandles, similarity_transform)
 from .settings import (CloudSettings, DrawMode, GaussianColorSpace, GaussianMode, PlaybackMode,  # noqa: F401
                        RadixSortDepthBits, RasterizeMode, ShaderDefines, SortMode, SparseSelect, playback_update)

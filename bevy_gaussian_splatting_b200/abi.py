@@ -28,6 +28,7 @@ BGS_FLAG_VISUALIZE_BOUNDING_BOX = 64
 BGS_ENTITY_VISUALIZE_BOUNDING_BOX = 1
 BGS_SCENE_MAX_CLOUDS = 64
 BGS_SELECT_REPLACE, BGS_SELECT_ADD = 0, 1
+BGS_TRANSFORM_ALL, BGS_TRANSFORM_SELECTED = 0, 1
 BGS_PICK_NONE = 0xFFFFFFFF
 
 
@@ -193,6 +194,8 @@ SYMBOLS = [
     ("bgs_cloud_particles_step", C.c_int, [_P, _P, _P, C.c_float]),
     ("bgs_cloud_positions_get", C.c_int, [_P, _P, _P]),
     ("bgs_cloud_interpolate", C.c_int, [_P, _P, _P, _P, C.c_float, C.c_float, C.c_float]),
+    ("bgs_cloud_transform", C.c_int, [_P, _P, _P, C.c_uint32]),
+    ("bgs_cloud_bounds", C.c_int, [_P, _P, C.c_uint32, _P, _P, C.POINTER(C.c_uint32)]),
     ("bgs_render", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P,
                              C.c_uint32, C.c_int]),
     ("bgs_render_ex", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings),

@@ -129,6 +129,129 @@ bgs_status khr_check(bgs_context* c, const KhrSlot& s, bool sh) {
     return BGS_OK;
 }
 
+// ---- bgs_cloud_transform's host half (the rule: include/bgs.h), in f64
+
+// the renderer's SH band l (1..3) at the direction d: project.cu's sh_basis polynomials times its c_shc constants (here
+// at f64, the decimal values spherical_harmonics.wgsl gives)
+void sh_band_basis(int l, const double d[3], double* y) {
+    const double x = d[0], yy_ = d[1], z = d[2];
+    const double xx = x * x, yy = yy_ * yy_, zz = z * z;
+    if (l == 1) {
+        y[0] = -0.4886025119029199 * yy_; y[1] = 0.4886025119029199 * z; y[2] = -0.4886025119029199 * x;
+    } else if (l == 2) {
+        y[0] = 1.0925484305920792 * (x * yy_); y[1] = -1.0925484305920792 * (yy_ * z);
+        y[2] = 0.31539156525252005 * ((2.0 * zz - xx) - yy); y[3] = -1.0925484305920792 * (x * z);
+        y[4] = 0.5462742152960396 * (xx - yy);
+    } else {
+        y[0] = -0.5900435899266435 * (yy_ * (3.0 * xx - yy)); y[1] = 2.890611442640554 * ((x * yy_) * z);
+        y[2] = -0.4570457994644658 * (yy_ * ((4.0 * zz - xx) - yy)); y[3] = 0.3731763325901154 * (z * ((2.0 * zz - 3.0 * xx) - 3.0 * yy));
+        y[4] = -0.4570457994644658 * (x * ((4.0 * zz - xx) - yy)); y[5] = 1.445305721320277 * (z * (xx - yy));
+        y[6] = -0.5900435899266435 * (x * (xx - 3.0 * yy));
+    }
+}
+
+// E_l = D_l^T (row-major), D_l defined by Y_l(R^T d) = D_l Y_l(d): the least-squares solution of Y E = Z over 64 fixed
+// directions d_k (a Fibonacci sphere), Y's rows Y_l(d_k) and Z's Y_l(R^T d_k), through the normal equations and
+// Gauss-Jordan elimination with partial pivoting.  Entries below 2^-40 in magnitude are exactly 0.
+void sh_rotation(const double R[3][3], int l, double* E) {
+    const int m = 2 * l + 1;
+    constexpr int N = 64;
+    double G[7][14] = {};   // [Y^T Y | Y^T Z]
+    for (int k = 0; k < N; ++k) {
+        const double z = 1.0 - (2.0 * k + 1.0) / N, r = std::sqrt(1.0 - z * z), phi = k * 2.399963229728653;
+        const double d[3] = {r * std::cos(phi), r * std::sin(phi), z};
+        const double rd[3] = {R[0][0] * d[0] + R[1][0] * d[1] + R[2][0] * d[2], R[0][1] * d[0] + R[1][1] * d[1] + R[2][1] * d[2],
+                              R[0][2] * d[0] + R[1][2] * d[1] + R[2][2] * d[2]};
+        double y[7], yr[7];
+        sh_band_basis(l, d, y);
+        sh_band_basis(l, rd, yr);
+        for (int i = 0; i < m; ++i)
+            for (int j = 0; j < m; ++j) { G[i][j] += y[i] * y[j]; G[i][m + j] += y[i] * yr[j]; }
+    }
+    for (int c = 0; c < m; ++c) {
+        int p = c;
+        for (int r = c + 1; r < m; ++r)
+            if (std::fabs(G[r][c]) > std::fabs(G[p][c])) p = r;
+        for (int j = 0; j < 2 * m; ++j) std::swap(G[c][j], G[p][j]);
+        const double inv = 1.0 / G[c][c];
+        for (int j = 0; j < 2 * m; ++j) G[c][j] *= inv;
+        for (int r = 0; r < m; ++r)
+            if (r != c) {
+                const double f = G[r][c];
+                for (int j = 0; j < 2 * m; ++j) G[r][j] -= f * G[c][j];
+            }
+    }
+    for (int i = 0; i < m; ++i)
+        for (int j = 0; j < m; ++j) {
+            const double e = G[i][m + j];
+            E[i * m + j] = std::fabs(e) < 0x1p-40 ? 0.0 : e;
+        }
+}
+
+// The matrix's check and the kernel's constants; false (with the reason in `why`) for a matrix the call refuses
+bool transform_params(const float* M, TransformParams* P, const char** why) {
+    for (int k = 0; k < 16; ++k)
+        if (!std::isfinite(M[k])) { *why = "an entry is not finite"; return false; }
+    if (M[3] != 0.0f || M[7] != 0.0f || M[11] != 0.0f || M[15] != 1.0f) { *why = "the bottom row is not (0, 0, 0, 1)"; return false; }
+    double A[3][3];   // A[row][col]
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) A[i][j] = M[4 * j + i];
+    auto dot = [&](int a, int b) { return (A[0][a] * A[0][b] + A[1][a] * A[1][b]) + A[2][a] * A[2][b]; };
+    const double s2 = ((dot(0, 0) + dot(1, 1)) + dot(2, 2)) / 3.0;
+    if (!(s2 > 0.0)) { *why = "the 3x3 block is zero"; return false; }
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j)
+            if (!(std::fabs(dot(i, j) - (i == j ? s2 : 0.0)) <= 1e-5 * s2)) {
+                *why = "the 3x3 block is not a rotation times a uniform scale (shear or non-uniform scale)";
+                return false;
+            }
+    const double det = (A[0][0] * (A[1][1] * A[2][2] - A[1][2] * A[2][1]) - A[0][1] * (A[1][0] * A[2][2] - A[1][2] * A[2][0])) +
+                       A[0][2] * (A[1][0] * A[2][1] - A[1][1] * A[2][0]);
+    if (!(det > 0.0)) { *why = "the 3x3 block is a reflection"; return false; }
+    const double s = std::sqrt(s2);
+    double R[3][3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) R[i][j] = A[i][j] / s;
+    // Shepperd: the largest of tr, R00, R11, R22 (the first on a tie) picks the component taken from a square root
+    const double tr = (R[0][0] + R[1][1]) + R[2][2];
+    double q[4];   // w, x, y, z
+    int b = 0;
+    const double cand[4] = {tr, R[0][0], R[1][1], R[2][2]};
+    for (int k = 1; k < 4; ++k)
+        if (cand[k] > cand[b]) b = k;
+    if (b == 0) {
+        const double t = 0.5 * std::sqrt(1.0 + tr), f = 0.25 / t;
+        q[0] = t; q[1] = (R[2][1] - R[1][2]) * f; q[2] = (R[0][2] - R[2][0]) * f; q[3] = (R[1][0] - R[0][1]) * f;
+    } else if (b == 1) {
+        const double t = 0.5 * std::sqrt(((1.0 + R[0][0]) - R[1][1]) - R[2][2]), f = 0.25 / t;
+        q[0] = (R[2][1] - R[1][2]) * f; q[1] = t; q[2] = (R[0][1] + R[1][0]) * f; q[3] = (R[0][2] + R[2][0]) * f;
+    } else if (b == 2) {
+        const double t = 0.5 * std::sqrt(((1.0 - R[0][0]) + R[1][1]) - R[2][2]), f = 0.25 / t;
+        q[0] = (R[0][2] - R[2][0]) * f; q[1] = (R[0][1] + R[1][0]) * f; q[2] = t; q[3] = (R[1][2] + R[2][1]) * f;
+    } else {
+        const double t = 0.5 * std::sqrt(((1.0 - R[0][0]) - R[1][1]) + R[2][2]), f = 0.25 / t;
+        q[0] = (R[1][0] - R[0][1]) * f; q[1] = (R[0][2] + R[2][0]) * f; q[2] = (R[1][2] + R[2][1]) * f; q[3] = t;
+    }
+    const double qn = std::sqrt(((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3]);
+    const double sg = q[0] < 0.0 ? -1.0 : 1.0;
+    for (double& v : q) v = sg * v / qn;
+    // the SH follow the rotation of the unit quaternion (in f64, before rounding): R_q = R_std(q)
+    const double w = q[0], x = q[1], y = q[2], z = q[3];
+    const double Rq[3][3] = {{1.0 - 2.0 * (y * y + z * z), 2.0 * (x * y - w * z), 2.0 * (x * z + w * y)},
+                             {2.0 * (x * y + w * z), 1.0 - 2.0 * (x * x + z * z), 2.0 * (y * z - w * x)},
+                             {2.0 * (x * z - w * y), 2.0 * (y * z + w * x), 1.0 - 2.0 * (x * x + y * y)}};
+    for (int k = 0; k < 16; ++k) P->m[k] = M[k];
+    for (int k = 0; k < 4; ++k) P->q[k] = (float)q[k];
+    P->s = (float)s;
+    float* const bands[3] = {P->sh1, P->sh2, P->sh3};
+    for (int l = 1; l <= 3; ++l) {
+        double E[49];
+        sh_rotation(Rq, l, E);
+        for (int k = 0; k < (2 * l + 1) * (2 * l + 1); ++k) bands[l - 1][k] = (float)E[k];
+    }
+    return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -609,6 +732,56 @@ bgs_status bgs_cloud_interpolate(bgs_context* c, bgs_cloud* out, const bgs_cloud
         CU(c, cudaGetLastError());
         return BGS_OK;
     });
+}
+
+// ---- transform and bounds (transform.cu).  The transform is a queued write (host.cuh: queue_cloud_write), never
+// drained, as the particle step is; the bounds only read the cloud (before_cloud_read), into their own words.
+
+bgs_status bgs_cloud_transform(bgs_context* c, bgs_cloud* cl, const float* local_from_local, uint32_t mode) {
+    if (!cl || !local_from_local) return fail(c, BGS_EINVAL, "transform: null cloud or matrix");
+    if (mode != BGS_TRANSFORM_ALL && mode != BGS_TRANSFORM_SELECTED) return fail(c, BGS_EINVAL, "transform: unknown mode %u", mode);
+    TRY(enter_call(c, "transform", cl->device));
+    if (is_4d(cl->layout)) return fail(c, BGS_EINVAL, "transform: Gaussian4d clouds are not transformed");
+    TransformParams P;
+    const char* why = "";
+    if (!transform_params(local_from_local, &P, &why)) return fail(c, BGS_EINVAL, "transform: %s", why);
+    TRY(queue_cloud_write(c, cl, [&](cudaStream_t q) {
+        launch_transform(cl->layout, cl->sh_degree, cl->view(), cl->n, P, mode == BGS_TRANSFORM_SELECTED, q);
+        CU(c, cudaGetLastError());
+        return BGS_OK;
+    }));
+    c->step_pending = true;
+    return BGS_OK;
+}
+
+bgs_status bgs_cloud_bounds(bgs_context* c, const bgs_cloud* cl, uint32_t mode, float out_min[3], float out_max[3],
+                            uint32_t* out_count) {
+    if (!cl || !out_min || !out_max) return fail(c, BGS_EINVAL, "bounds: null cloud or output");
+    if (mode != BGS_TRANSFORM_ALL && mode != BGS_TRANSFORM_SELECTED) return fail(c, BGS_EINVAL, "bounds: unknown mode %u", mode);
+    TRY(enter_call(c, "bounds", cl->device));
+    TRY(before_cloud_read(c, cl));
+    cudaStream_t q = c->stream;
+    TRY(c->bounds_words.grow(c, 7 * 4, false));
+    uint32_t* words = c->bounds_words.p;
+    CU(c, cudaMemsetAsync(words, 0xFF, 3 * 4, q));
+    CU(c, cudaMemsetAsync(words + 3, 0, 4 * 4, q));
+    launch_bounds(cl->pos, cl->n, mode == BGS_TRANSFORM_SELECTED, words, c->sm_count, q);
+    CU(c, cudaGetLastError());
+    uint32_t h[7];
+    CU(c, cudaMemcpyAsync(h, words, sizeof h, cudaMemcpyDeviceToHost, q));
+    CU(c, cudaStreamSynchronize(q));
+    auto decode = [](uint32_t k) {
+        const uint32_t u = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
+        float f;
+        memcpy(&f, &u, 4);
+        return f;
+    };
+    for (int k = 0; k < 3; ++k) {
+        out_min[k] = h[6] ? decode(h[k]) : INFINITY;
+        out_max[k] = h[6] ? decode(h[3 + k]) : -INFINITY;
+    }
+    if (out_count) *out_count = h[6];
+    return BGS_OK;
 }
 
 // ---- subset and download (subset.cu).  Both only read the source cloud (before_cloud_read), so neither drains another

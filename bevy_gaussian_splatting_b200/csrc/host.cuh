@@ -164,6 +164,8 @@ struct bgs_context {
     DevBuf<uint8_t> mesh_tri, mesh_pairs;
     // bgs_cloud_select_in_view's own scratch: its count word | a host mask's device copy
     DevBuf<uint8_t> view_select;
+    // bgs_cloud_bounds' own words (transform.cu: launch_bounds)
+    DevBuf<uint32_t> bounds_words;
     bool async_pending = false;        // a BGS_FLAG_ASYNC frame has been enqueued and not yet completed
     bool step_pending = false;         // a particle step has been enqueued since the last bgs_sync
     // an interpolation (a queued write that reads other clouds) has been enqueued since the last bgs_sync: ev_done

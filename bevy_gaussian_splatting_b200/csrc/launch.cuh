@@ -158,6 +158,19 @@ void launch_subset_scatter(CloudLayout layout, uint32_t sh_degree, CloudView src
 void launch_subset_gather(CloudLayout layout, uint32_t sh_degree, CloudView src, const uint32_t* idx, uint32_t k, CloudView dst, cudaStream_t stream);
 void launch_unpack(CloudLayout layout, uint32_t sh_degree, CloudView cloud, uint32_t lo, uint32_t m, void* sh, void* rot, void* so,
                    void* tt /* 4D only */, cudaStream_t stream);
+// transform.cu: bgs_cloud_transform's constants (cloud.cu: transform_params; the rule: include/bgs.h) -- the column-major
+// matrix, q_R (w, x, y, z), s, and E_l = D_l^T row-major for the SH bands 1..3 -- and its pass; bgs_cloud_bounds' pass
+// (words: min keys x, y, z, preset to 0xFFFFFFFF | max keys x, y, z, preset to 0 | count, preset to 0; a key is the f32's
+// bits with the sign bit flipped when clear and every bit flipped when set)
+struct TransformParams {
+    float m[16];
+    float q[4];
+    float s;
+    float sh1[9], sh2[25], sh3[49];
+};
+void launch_transform(CloudLayout layout, uint32_t sh_degree, CloudView cloud, uint32_t n, const TransformParams& p,
+                      uint32_t selected_only, cudaStream_t stream);
+void launch_bounds(const float4* pos, uint32_t n, uint32_t selected_only, uint32_t* words, int sm_count, cudaStream_t stream);
 // interpolate.cu
 void launch_interpolate(CloudLayout layout, uint32_t sh_degree, CloudView lhs, CloudView rhs, uint32_t n, float t, CloudView out, cudaStream_t stream);
 // khr.cu: glTF component codes, the decode's rule bits (words[0]; words[1] counts zero-length quaternions), one accessor

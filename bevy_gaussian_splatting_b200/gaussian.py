@@ -162,10 +162,18 @@ class PlanarGaussian3d:
 def compute_aabb(position_visibility: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
     """`PlanarGaussian3d.compute_aabb` of an (n, 4) position plane."""
     p = np.asarray(position_visibility, np.float32)[:, :3]
+    if not len(p):
+        return aabb_of_extent(np.full(3, np.inf, np.float32), np.full(3, -np.inf, np.float32))
+    return aabb_of_extent(p.min(0), p.max(0))
+
+
+def aabb_of_extent(pmin, pmax) -> tuple[np.ndarray, np.ndarray]:
+    """`compute_aabb`'s steps from the per-axis min and max of the positions (+inf / -inf for none): the extent -+ 0.1,
+    then centre and half extents, in f32."""
     off = np.float32(0.1)
     # (min over (p - 0.1) == min(p) - 0.1: f32 subtraction of a constant is monotone)
-    lo = (p.min(0) - off).astype(np.float32) if len(p) else np.full(3, np.inf, np.float32)
-    hi = (p.max(0) + off).astype(np.float32) if len(p) else np.full(3, -np.inf, np.float32)
+    lo = (np.asarray(pmin, np.float32) - off).astype(np.float32)
+    hi = (np.asarray(pmax, np.float32) + off).astype(np.float32)
     two = np.float32(2.0)
     center = ((lo + hi).astype(np.float32) / two).astype(np.float32)
     half = ((hi - lo).astype(np.float32) / two).astype(np.float32)

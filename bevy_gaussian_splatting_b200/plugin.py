@@ -20,7 +20,7 @@ import numpy as np
 
 from . import abi
 from .camera import GaussianCamera, View
-from .gaussian import SH_WIDTHS, PlanarGaussian3d, PlanarGaussian4d, compute_aabb
+from .gaussian import SH_WIDTHS, PlanarGaussian3d, PlanarGaussian4d, aabb_of_extent, compute_aabb
 from .particles import PARTICLE_BEHAVIOR_DTYPE, as_particle_behaviors
 from .settings import CloudSettings, GaussianMode, RasterizeMode, SparseSelect
 
@@ -78,6 +78,23 @@ class CloudTransform:
     """GlobalTransform of the cloud entity -> CloudUniform.transform (render/mod.rs:1056-1072)."""
 
     matrix: np.ndarray = dataclasses.field(default_factory=lambda: np.eye(4, dtype=np.float32))
+
+
+def similarity_transform(translation=(0.0, 0.0, 0.0), rotation_wxyz=(1.0, 0.0, 0.0, 0.0), scale: float = 1.0,
+                         pivot=(0.0, 0.0, 0.0)) -> np.ndarray:
+    """The 4x4 f32 matrix (CloudTransform.matrix's convention; `transform` passes it column-major) that scales by
+    `scale` and rotates by the quaternion `rotation_wxyz` (normalised here) about `pivot`, then translates by
+    `translation`: T(pivot + translation) R S T(-pivot), built in f64.  A gizmo rotates a selection about its centre."""
+    q = np.asarray(rotation_wxyz, np.float64)
+    w, x, y, z = q / np.linalg.norm(q)
+    R = np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+                  [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+                  [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]])
+    p = np.asarray(pivot, np.float64)
+    m = np.eye(4)
+    m[:3, :3] = float(scale) * R
+    m[:3, 3] = p + np.asarray(translation, np.float64) - m[:3, :3] @ p
+    return m.astype(np.float32)
 
 
 class PlanarGaussian3dHandle:
@@ -988,6 +1005,37 @@ class GaussianSplattingPlugin:
         `subset(lhs, np.arange(lhs.n))`.  `sync()` completes it."""
         self._check(self._lib.bgs_cloud_interpolate(self._ctx, out._h, lhs._h, rhs._h, C.c_float(settings.time),
                                                     C.c_float(settings.time_start), C.c_float(settings.time_stop)))
+
+    # -- transforms and bounds: a gizmo drag baked into the cloud, and its Aabb refreshed (the rule: include/bgs.h)
+    def transform(self, handle: PlanarGaussian3dHandle, matrix, selected: bool = False) -> None:
+        """Bake the similarity transform `matrix` (a 4x4 in CloudTransform.matrix's convention, or a CloudTransform),
+        in the cloud's own frame, into every gaussian or, `selected`, the selected ones (visibility !(v < 0.5)):
+        positions, rotations, scales or covariances, and SH bands 1-3.  Enqueued like `step_particles`: frames rendered
+        before it (on any context) see the old cloud, everything after it the new one.  A world-space delta W of an
+        entity with model matrix `model` is `inv(model) @ W @ model` here.  Shear, non-uniform scale, reflections and
+        Gaussian4d clouds raise BgsError (BGS_EINVAL).  handle.aabb is not updated: call `update_aabb`."""
+        m = matrix.matrix if isinstance(matrix, CloudTransform) else matrix
+        m = np.asarray(m, np.float32)
+        if m.shape != (4, 4):
+            raise ValueError(f"transform: the matrix must be 4x4, not {m.shape}")
+        cm = np.ascontiguousarray(m.T.reshape(16))
+        mode = abi.BGS_TRANSFORM_SELECTED if selected else abi.BGS_TRANSFORM_ALL
+        self._check(self._lib.bgs_cloud_transform(self._ctx, handle._h, _ptr(cm), mode))
+
+    def bounds(self, handle: PlanarGaussian3dHandle, selected: bool = False) -> tuple[np.ndarray, np.ndarray, int]:
+        """(min (3,) f32, max (3,) f32, count) of the positions of every gaussian, or of the selected ones, whose x, y
+        and z are finite, after every write queued on the cloud; (+inf, -inf, 0) for none."""
+        lo, hi, n = np.empty(3, np.float32), np.empty(3, np.float32), C.c_uint32()
+        mode = abi.BGS_TRANSFORM_SELECTED if selected else abi.BGS_TRANSFORM_ALL
+        self._check(self._lib.bgs_cloud_bounds(self._ctx, handle._h, mode, _ptr(lo), _ptr(hi), C.byref(n)))
+        return lo, hi, int(n.value)
+
+    def update_aabb(self, handle: PlanarGaussian3dHandle) -> tuple[np.ndarray, np.ndarray]:
+        """handle.aabb := the entity's Aabb from the GPU bounds of every finite position, through compute_aabb's f32
+        steps (for finite positions, bit for bit compute_aabb(positions(handle))).  Returns it."""
+        lo, hi, _ = self.bounds(handle)
+        handle.aabb = aabb_of_extent(lo, hi)
+        return handle.aabb
 
     # -- parity / measurement hooks
     def frame_stats(self) -> abi.bgs_frame_stats:

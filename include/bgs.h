@@ -491,6 +491,65 @@ bgs_status bgs_cloud_positions_get(bgs_context* ctx, const bgs_cloud* cloud, flo
 bgs_status bgs_cloud_interpolate(bgs_context* ctx, bgs_cloud* out, const bgs_cloud* lhs, const bgs_cloud* rhs, float time,
                                  float time_start, float time_stop);
 
+/* Transforms and bounds: move, rotate or scale a resident cloud or its selection in place (an editor's gizmo drag, the
+ * alignment of one scan to another, a node transform baked in before saving), and measure its positions' bounds.
+ * bgs_cloud_transform bakes a similarity transform M -- a rotation R, a uniform scale s > 0 and a translation, given
+ * column-major in the cloud's own frame (a world-space delta W becomes model^-1 W model) -- into the stored gaussians.
+ * The rule, exactly:
+ *   - which gaussians: BGS_TRANSFORM_ALL every one; BGS_TRANSFORM_SELECTED those whose visibility v has !(v < 0.5f)
+ *     (DrawMode::Selected's and bgs_cloud_subset's predicate: NaN and +inf are selected, -0 and -inf are not), read as
+ *     the visibility lane is when the transform runs.  Every byte of a gaussian it leaves alone stays as it was, in both
+ *     device copies;
+ *   - the matrix, checked on the host in f64: every entry finite; the bottom row exactly (0, 0, 0, 1); with c_i the
+ *     columns of the 3x3 block A, |c|^2 = (x*x + y*y) + z*z and s^2 = ((|c0|^2 + |c1|^2) + |c2|^2) / 3 > 0;
+ *     |c_i . c_j - s^2 delta_ij| <= 1e-5 s^2 for every i, j; det A > 0 (a reflection has no quaternion with positive
+ *     scales).  s = sqrt(s^2), R = A / s, and q_R is R's quaternion by Shepperd's method (the largest of trace, R00, R11,
+ *     R22 picks the root, the first on a tie), normalised in f64, taken with w >= 0 and rounded to f32; s is rounded
+ *     to f32 likewise;
+ *   - position: p' = M (x, y, z, 1), each row ((m_r0 x + m_r1 y) + m_r2 z) + m_r3 -- the projection's model multiply,
+ *     so the baked position is, bit for bit, the world position a frame with uniform.transform = M computes.  Both
+ *     copies are written; the visibility lane keeps its bits;
+ *   - rotation: q' = q_R (x) q, the Hamilton product in storage order (w, x, y, z), not normalised:
+ *       w' = ((aw bw - ax bx) - ay by) - az bz        x' = ((aw bx + ax bw) + ay bz) - az by
+ *       y' = ((aw by - ax bz) + ay bw) + az bx        z' = ((aw bz + ax by) - ay bx) + az bw    (a = q_R, b = q).
+ *     The renderer's rotation rows are R_std(q)^T, so a splat's covariance is R_std S^2 R_std^T and R_std(q') =
+ *     R R_std(q).  That identity holds for unit quaternions only, as the renderer's formula is one for unit ones;
+ *   - scale: scale' = s * scale per axis; opacity keeps its bits;
+ *   - precomputed-covariance layout: Sigma' = A Sigma A^T (= s^2 R Sigma R^T), with X = A Sigma then X A^T, each entry
+ *     (a0 b0 + a1 b1) + a2 b2 -- the projection's T Sigma T^t order; the opacity word keeps its bits;
+ *   - SH: for each channel and band l in 1..3 up to the cloud's degree, c'_l = D_l^T c_l, where D_l is defined by
+ *     Y_l(R^T d) = D_l Y_l(d) with Y_l the renderer's own band-l basis (its polynomials times its constants), so the
+ *     baked colour seen along a direction equals the original's seen along the rotated one.  D_l is computed once per
+ *     call on the host in f64, from q_R's rotation before rounding (least squares over 64 fixed directions; entries
+ *     below 2^-40 are 0), and rounded to f32.  (D_l^T composes as the rotations do: D(R1 R2)^T = D(R1)^T D(R2)^T.)  The
+ *     kernel sums c'_i = E_i0 c_0 + E_i1 c_1 + ... over j ascending, E = D_l^T.  Band 0 and the padding lanes are never
+ *     touched: a degree-0 cloud's SH stays bit for bit;
+ *   - every operation f32 round-to-nearest-even without FMA, subnormals kept; non-finite values propagate as that
+ *     arithmetic gives them.  f16 layouts: each half is widened exactly, transformed in f32 and narrowed
+ *     round-to-nearest-even (past 65504: +-inf), in the upload's lane map; the opacity half, and the zero words of the
+ *     last SH chunk, keep their stored bits.
+ * Ordering: a queued write of the cloud, exactly as bgs_cloud_particles_step: one kernel enqueued on the context's render
+ *   stream, no host synchronisation.  Frames and calls enqueued before it, on any context, see the old cloud; every
+ *   call after it the new one.  bgs_sync(ctx) completes it, bgs_cloud_destroy waits for it.  A context that never
+ *   transforms issues the same launches as before.  The entity's Aabb is not updated, as after a particle step:
+ *   bgs_cloud_bounds is how the caller refreshes it.
+ * A null argument, a cloud on another device than the context's, an unknown mode, a matrix that fails the check, or a
+ * Gaussian4d cloud (its two rotations and spherindrical coefficients are not rotated here) -> BGS_EINVAL; a refused call
+ * changes and enqueues nothing.
+ * bgs_cloud_bounds: per axis, the min and max of the position plane (cloud-local, after every write queued on the
+ * cloud) over the gaussians `mode` selects (the transform's predicate) whose x, y and z are all finite; *out_count (may
+ * be NULL) is how many took part.  With none: min = +inf, max = -inf, count 0.  -0 and +0 compare equal: which zero
+ * comes back when both occur on an axis is unpinned.  Synchronous: it waits on the device only for the writes queued on
+ * this cloud, never for other contexts' frames; one streaming pass over the position plane (16 B per gaussian) into the
+ * call's own words, then one read-back, so the debug hooks and the next frame's plan are untouched.  A Gaussian4d
+ * cloud's base positions are measured.  A null argument, a cloud on another device or an unknown mode -> BGS_EINVAL.
+ * An entity's Aabb (positions -+ 0.1) follows from the bounds as the host's compute_aabb computes it. */
+enum { BGS_TRANSFORM_ALL = 0u, BGS_TRANSFORM_SELECTED = 1u };
+bgs_status bgs_cloud_transform(bgs_context* ctx, bgs_cloud* cloud, const float* local_from_local /* 16, column-major */,
+                               uint32_t mode);
+bgs_status bgs_cloud_bounds(bgs_context* ctx, const bgs_cloud* cloud, uint32_t mode /* BGS_TRANSFORM_* */, float out_min[3],
+                            float out_max[3], uint32_t* out_count /* may be NULL */);
+
 /* One view of one cloud: key-gen -> depth radix sort -> projection + SH colour -> tile
  * binning -> per-tile front-to-back blend.  out_rgba is caller-owned (host pointer, or a
  * device pointer when out_is_device_ptr != 0); may be NULL to keep the frame on the device.

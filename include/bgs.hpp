@@ -620,6 +620,34 @@ public:
                      const CloudSettings& settings) {
         check(bgs_cloud_interpolate(ctx_, out.get(), lhs.get(), rhs.get(), settings.time, settings.time_start, settings.time_stop));
     }
+    // Transforms (the rule and its ordering: bgs.h): bake the similarity transform m (column-major, in the cloud's own
+    // frame: a world-space delta W of an entity with model matrix `model` is model^-1 W model) into every gaussian, or
+    // with selected_only into the selected ones, enqueued like a particle step.  The entity's Aabb is not updated:
+    // refresh it from bounds().
+    void transform(PlanarGaussian3dHandle& cloud, const Mat4& m, bool selected_only = false) {
+        check(bgs_cloud_transform(ctx_, cloud.get(), m.m, selected_only ? BGS_TRANSFORM_SELECTED : BGS_TRANSFORM_ALL));
+    }
+    // bounds: per axis, the min and max of the finite positions of every (or every selected) gaussian, after every write
+    // queued on the cloud; count 0 (min +inf, max -inf) when there are none.
+    struct Bounds {
+        float min[3], max[3];
+        uint32_t count;
+    };
+    Bounds bounds(const PlanarGaussian3dHandle& cloud, bool selected_only = false) {
+        Bounds b{};
+        check(bgs_cloud_bounds(ctx_, cloud.get(), selected_only ? BGS_TRANSFORM_SELECTED : BGS_TRANSFORM_ALL, b.min, b.max,
+                               &b.count));
+        return b;
+    }
+    // update_aabb: the handle's Aabb from the GPU bounds, through compute_aabb's f32 steps (+-0.1, centre, half extents)
+    void update_aabb(PlanarGaussian3dHandle& cloud) {
+        const Bounds b = bounds(cloud);
+        for (int k = 0; k < 3; ++k) {
+            const float lo = b.min[k] - 0.1f, hi = b.max[k] + 0.1f;
+            const float center = (lo + hi) / 2.0f, half = (hi - lo) / 2.0f;
+            cloud.aabb_min_[k] = center - half; cloud.aabb_max_[k] = center + half;
+        }
+    }
     std::vector<float> positions(const PlanarGaussian3dHandle& cloud) {   // n * 4: x, y, z, visibility
         std::vector<float> v((size_t)cloud.len() * 4);
         check(bgs_cloud_positions_get(ctx_, cloud.get(), v.data()));
