@@ -185,59 +185,66 @@ FramePlan plan_frame(const bgs_context* c, const bgs_settings* st, bool want_aux
     return p;
 }
 
+// What a frame writes, and where: each of v views' colour frame rgba[i] and, on aux frames, its depth and normal frames
+// depth[i] and normal[i], and on pick frames (bgs_render_entities_pick) the pick frame `pick` (else NULL), in `format`, in
+// device memory (`device`) or host memory.  A single-view frame is view 0.
+struct Targets {
+    uint32_t format;
+    int device;
+    uint32_t v;
+    bool aux;
+    void* const* rgba;
+    void* const* depth;
+    void* const* normal;
+    void* pick;
+};
+// a single-view frame's colour frame alone
+Targets colour_target(void* const* rgba, uint32_t format, int device) {
+    return {format, device, 1, false, rgba, nullptr, nullptr, nullptr};
+}
+
 // Where a frame's pixels go.
 struct FrameOut {
-    void* rgba = nullptr;               // the blend's target (device): the caller's frame or one of the library's
-    void* depth = nullptr;              // bgs_render_aux's depth / normal targets (device)
-    void* normal = nullptr;
     uint32_t raster_format = 0;         // output mode of the blend kernels: format | mode << 8 (raster.cu)
-    size_t bytes = 0;                   // of one frame
     int slot = -1;                      // a queued frame in the library's own frames: which of the two (else -1)
-    void* host_rgba = nullptr;          // host frames the result is copied to
-    void* host_depth = nullptr;
-    void* host_normal = nullptr;
-    // a views frame: view i's device targets, host frames (host targets; else NULL) and bytes (of one frame); the depth and
-    // normal ones on aux frames
-    uint32_t views = 0;
-    void* view_rgba[MAX_VIEWS] = {};
-    void* view_host[MAX_VIEWS] = {};
-    void* view_depth[MAX_VIEWS] = {};
-    void* view_normal[MAX_VIEWS] = {};
-    void* view_host_depth[MAX_VIEWS] = {};
-    void* view_host_normal[MAX_VIEWS] = {};
-    size_t view_bytes[MAX_VIEWS] = {};
+    // view i's bytes (of one frame), its device targets (the caller's frames or the library's), and the host frames they
+    // are copied to (host targets; else NULL); the depth and normal ones on aux frames
+    uint32_t v = 1;
+    size_t bytes[MAX_VIEWS] = {};
+    void* rgba[MAX_VIEWS] = {};
+    void* depth[MAX_VIEWS] = {};
+    void* normal[MAX_VIEWS] = {};
+    void* host_rgba[MAX_VIEWS] = {};
+    void* host_depth[MAX_VIEWS] = {};
+    void* host_normal[MAX_VIEWS] = {};
     // a pick frame (bgs_render_entities_pick): its device records, the host target they are copied to (else NULL)
     uint4* pick = nullptr;
     void* host_pick = nullptr;
 };
 
-// A views frame's targets: view i's frame into rgba[i] and, on aux frames, its depth and normal frames into depth[i] and
-// normal[i] (NULL arrays otherwise)
-struct ViewTargets {
-    void* const* rgba;
-    void* const* depth;
-    void* const* normal;
-};
-
-// the caller's device frames, or the library's own (grown on demand)
-bgs_status frame_out(bgs_context* c, const bgs_settings* st, uint32_t format, size_t bytes, void* out_rgba,
-                     int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal, FrameOut* o) {
+// A frame's targets, view i W[i] x H[i] pixels: the caller's device frames, or the library's own (grown on demand), which
+// hold every view's frame one after another (aux frames: frame_aux[0] every view's depth frame, frame_aux[1] every normal
+// frame) and are copied to the caller's host frames
+bgs_status frame_out(bgs_context* c, const bgs_settings* st, const Targets& t, const int* W, const int* H, FrameOut* o) {
     const bool blend_over = (st->flags & BGS_FLAG_BLEND_OVER_TARGET) != 0;
-    o->raster_format = format | ((blend_over ? 2u : ((st->flags & BGS_FLAG_PREMULTIPLIED_OUT) ? 1u : 0u)) << 8);
-    o->bytes = bytes;
+    o->raster_format = t.format | ((blend_over ? 2u : ((st->flags & BGS_FLAG_PREMULTIPLIED_OUT) ? 1u : 0u)) << 8);
+    const size_t bpp = format_bpp(t.format);
+    o->v = t.v;
+    size_t total = 0;
+    for (uint32_t i = 0; i < t.v; ++i) total += o->bytes[i] = (size_t)W[i] * H[i] * bpp;
     // device targets are written with pixel-sized vector stores (and read so in blend-over mode): each must be aligned to
     // one pixel, 4 / 8 / 16 bytes
-    const size_t bpp = format_bpp(format);
-    if (out_is_device_ptr)
-        for (const void* t : {out_rgba, want_aux ? out_depth : nullptr, want_aux ? out_normal : nullptr})
-            if (reinterpret_cast<uintptr_t>(t) % bpp != 0)
-                return fail(c, BGS_EINVAL, "render: device target %p is not aligned to its %zu-byte pixels", t, bpp);
-    if (out_rgba && out_is_device_ptr) {
-        o->rgba = out_rgba;
+    if (t.device)
+        for (uint32_t i = 0; i < t.v; ++i)
+            for (const void* p : {t.rgba[i], t.aux ? t.depth[i] : nullptr, t.aux ? t.normal[i] : nullptr})
+                if (reinterpret_cast<uintptr_t>(p) % bpp != 0)
+                    return fail(c, BGS_EINVAL, "render: device target %p is not aligned to its %zu-byte pixels", p, bpp);
+    if (t.device && t.rgba[0]) {
+        for (uint32_t i = 0; i < t.v; ++i) o->rgba[i] = t.rgba[i];
     } else {
         for (int k = 0; k < 2; ++k) {
-            if (bytes <= c->frames[k].bytes) continue;
-            TRY(c->frames[k].grow(c, bytes, true));      // (BGS_FLAG_BLEND_OVER_TARGET reads the target)
+            if (total <= c->frames[k].bytes) continue;
+            TRY(c->frames[k].grow(c, total, true));      // (BGS_FLAG_BLEND_OVER_TARGET reads the target)
             c->copy_pending[k] = false;
         }
         // async frames rendered into the library's own buffers alternate two device frames, so whatever consumes
@@ -249,43 +256,30 @@ bgs_status frame_out(bgs_context* c, const bgs_settings* st, uint32_t format, si
         else if (st->flags & BGS_FLAG_ASYNC) { k = c->frame_toggle; c->frame_toggle ^= 1; }
         c->frame_last = k;
         if (st->flags & BGS_FLAG_ASYNC) o->slot = k;
-        o->rgba = c->frames[k].p;
-        o->host_rgba = out_rgba;
-    }
-    if (!want_aux) return BGS_OK;
-    if (out_is_device_ptr) { o->depth = out_depth; o->normal = out_normal; return BGS_OK; }
-    for (int k = 0; k < 2; ++k) TRY(c->frame_aux[k].grow(c, bytes, true));
-    o->depth = c->frame_aux[0].p; o->normal = c->frame_aux[1].p;
-    o->host_depth = out_depth; o->host_normal = out_normal;
-    return BGS_OK;
-}
-
-// a views frame's targets: the caller's device frames, or the library's frames holding every view, one after another
-// (aux frames: frame_aux[0] every view's depth frame, frame_aux[1] every normal frame) (the targets have passed
-// bgs_render_views' or bgs_render_views_aux's checks)
-bgs_status frame_out_views(bgs_context* c, const bgs_settings* st, uint32_t format, const ViewTable& vt, const ViewTargets& t,
-                           int out_is_device_ptr, FrameOut* o) {
-    const size_t bpp = format_bpp(format);
-    const bool aux = t.depth != nullptr;
-    size_t total = 0;
-    for (uint32_t i = 0; i < vt.v; ++i) total += (size_t)vt.W[i] * vt.H[i] * bpp;
-    TRY(frame_out(c, st, format, out_is_device_ptr ? (size_t)vt.W[0] * vt.H[0] * bpp : total,
-                  out_is_device_ptr ? t.rgba[0] : nullptr, out_is_device_ptr, false, nullptr, nullptr, o));
-    if (aux && !out_is_device_ptr)
-        for (int k = 0; k < 2; ++k) TRY(c->frame_aux[k].grow(c, total, true));
-    o->views = vt.v;
-    size_t at = 0;
-    for (uint32_t i = 0; i < vt.v; ++i) {
-        o->view_bytes[i] = (size_t)vt.W[i] * vt.H[i] * bpp;
-        o->view_rgba[i] = out_is_device_ptr ? t.rgba[i] : static_cast<char*>(o->rgba) + at;
-        o->view_host[i] = out_is_device_ptr ? nullptr : t.rgba[i];
-        if (aux) {
-            o->view_depth[i] = out_is_device_ptr ? t.depth[i] : static_cast<char*>(c->frame_aux[0].p) + at;
-            o->view_normal[i] = out_is_device_ptr ? t.normal[i] : static_cast<char*>(c->frame_aux[1].p) + at;
-            o->view_host_depth[i] = out_is_device_ptr ? nullptr : t.depth[i];
-            o->view_host_normal[i] = out_is_device_ptr ? nullptr : t.normal[i];
+        size_t at = 0;
+        for (uint32_t i = 0; i < t.v; at += o->bytes[i++]) {
+            o->rgba[i] = static_cast<char*>(c->frames[k].p) + at;
+            o->host_rgba[i] = t.rgba[i];
         }
-        at += o->view_bytes[i];
+    }
+    if (t.aux && t.device) {
+        for (uint32_t i = 0; i < t.v; ++i) { o->depth[i] = t.depth[i]; o->normal[i] = t.normal[i]; }
+    } else if (t.aux) {
+        for (int k = 0; k < 2; ++k) TRY(c->frame_aux[k].grow(c, total, true));
+        size_t at = 0;
+        for (uint32_t i = 0; i < t.v; at += o->bytes[i++]) {
+            o->depth[i] = static_cast<char*>(c->frame_aux[0].p) + at;
+            o->normal[i] = static_cast<char*>(c->frame_aux[1].p) + at;
+            o->host_depth[i] = t.depth[i];
+            o->host_normal[i] = t.normal[i];
+        }
+    }
+    if (t.pick && t.device) {
+        o->pick = static_cast<uint4*>(t.pick);
+    } else if (t.pick) {
+        TRY(c->pick_frame.grow(c, (size_t)W[0] * H[0] * sizeof(bgs_pick), false));
+        o->pick = c->pick_frame.p;
+        o->host_pick = t.pick;
     }
     return BGS_OK;
 }
@@ -608,7 +602,6 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     if (!scene) ++launches;
     CU(c, cudaEventRecord(c->ev_p1, ps));
     // depth-tested and pick frames: the splat depths, indexed like the records (the projection's index list)
-    ZTestArgs zt;
     if ((zd || o.pick) && scene_3d) {
         launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
@@ -617,8 +610,29 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
                            c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
     }
-    if (zd) { zt.splat_d = c->splat_depth.p; zt.scene = zd->depth; zt.pitch = (size_t)zd->pitch_bytes; }
-    if (o.pick) zt.splat_d = c->splat_depth.p;
+    // the blend's inputs (each round: its pair list and ranges) and targets
+    BlendArgs b;
+    b.mode = p.raster_mode;
+    b.box = p.box;
+    b.large_footprints = p.large_fp;
+    b.recs = c->recs.p;
+    b.extra = c->extra.p;
+    b.W = fc.Wi; b.H = fc.Hi; b.tiles_x = fc.tiles_x; b.tiles_y = fc.tiles_y;
+    b.out = o.rgba[0];
+    b.format = o.raster_format;
+    b.aux = fc.aux ? c->aux.p : nullptr;
+    b.out_depth = o.depth[0];
+    b.out_normal = o.normal[0];
+    b.truncated = &c->ctr->truncated;
+    if (zd || o.pick) b.splat_d = c->splat_depth.p;
+    if (zd) { b.scene = zd->depth; b.pitch = (size_t)zd->pitch_bytes; }
+    b.kinds = c->kinds.p;
+    b.views = views;
+    PickArgs pk = {};
+    if (o.pick) {
+        pk = PickArgs{o.pick, c->slot_ids.p, scene->kinds};
+        b.pick = &pk;
+    }
     if (p.overlap) {
         CU(c, cudaEventRecord(c->ev_join, c->stream2));
         CU(c, cudaStreamWaitEvent(q, c->ev_join, 0));
@@ -653,6 +667,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
                                 next_epoch(c), &cc->sort_barrier, p.tile_passes, 0, rng, c->sm_count, p.pair_sort_per_sm, q));
         ++launches;
         pcur = p.tile_passes & 1;
+        b.tile_entries = c->pvals[pcur].p;
+        b.ranges = rng;
         if (r + 1 == p.rounds) {
             // (chunked frames: the earlier rounds' blends are accounted to stage 4)
             CU(c, cudaEventRecord(c->ev[4], q));
@@ -662,24 +678,11 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             // the blend runs on the LOW-priority stream; the render stream resumes once it is done
             CU(c, cudaEventRecord(c->ev_front, q));
             CU(c, cudaStreamWaitEvent(c->stream_r, c->ev_front, 0));
-            if (o.pick)
-                launch_raster_pick(p.raster_mode, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
-                                   fc.tiles_y, o.rgba, o.raster_format, &c->ctr->truncated, zt, c->kinds.p, p.box,
-                                   PickArgs{o.pick, c->slot_ids.p, scene->kinds}, c->stream_r);
-            else if (views)
-                launch_raster_views(p.raster_mode, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, o.raster_format,
-                                    &c->ctr->truncated, zt.splat_d, c->kinds.p, p.box, *views, c->stream_r,
-                                    fc.aux ? c->aux.p : nullptr);
-            else
-                launch_raster(p.raster_mode, p.large_fp, c->recs.p, c->extra.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x,
-                              fc.tiles_y, o.rgba, o.raster_format, fc.aux ? c->aux.p : nullptr, o.depth, o.normal,
-                              &c->ctr->truncated, zt, c->stream_r, c->kinds.p, p.box);
+            launch_raster(b, c->stream_r);
             CU(c, cudaEventRecord(c->ev_rdone, c->stream_r));
             CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
         } else
-            launch_raster_round(c->recs.p, c->pvals[pcur].p, rng, fc.Wi, fc.Hi, fc.tiles_x, fc.tiles_y, o.rgba, o.raster_format,
-                                c->state.p, c->tile_done, &c->ctr->tiles_done, &c->ctr->truncated, r == 0, r + 1 == p.rounds, zt,
-                                q);
+            launch_raster_round(b, c->state.p, c->tile_done, &c->ctr->tiles_done, r == 0, r + 1 == p.rounds, q);
         ++launches;
     }
     c->pair_result = pcur;
@@ -688,37 +691,29 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, q));
     CU(c, cudaMemcpyAsync(c->h_sticky, c->d_sticky, 4, cudaMemcpyDeviceToHost, q));
     if (o.slot >= 0) CU(c, cudaEventRecord(c->ev_raster[o.slot], q));
-    // a views frame to host memory: each view's frames to its own host targets
-    auto copy_views = [&](cudaStream_t s) -> bgs_status {
-        for (uint32_t i = 0; i < o.views; ++i) {
-            CU(c, cudaMemcpyAsync(o.view_host[i], o.view_rgba[i], o.view_bytes[i], cudaMemcpyDeviceToHost, s));
-            if (o.view_host_depth[i]) {
-                CU(c, cudaMemcpyAsync(o.view_host_depth[i], o.view_depth[i], o.view_bytes[i], cudaMemcpyDeviceToHost, s));
-                CU(c, cudaMemcpyAsync(o.view_host_normal[i], o.view_normal[i], o.view_bytes[i], cudaMemcpyDeviceToHost, s));
+    // host targets: each view's frames, then the pick frame, copied out; a queued frame's on the copy stream, after its blend
+    if (o.host_rgba[0]) {
+        cudaStream_t s = q;
+        if (o.slot >= 0) {
+            CU(c, cudaStreamWaitEvent(c->stream_copy, c->ev_raster[o.slot], 0));
+            s = c->stream_copy;
+        }
+        for (uint32_t i = 0; i < o.v; ++i) {
+            CU(c, cudaMemcpyAsync(o.host_rgba[i], o.rgba[i], o.bytes[i], cudaMemcpyDeviceToHost, s));
+            if (o.host_depth[i]) {
+                CU(c, cudaMemcpyAsync(o.host_depth[i], o.depth[i], o.bytes[i], cudaMemcpyDeviceToHost, s));
+                CU(c, cudaMemcpyAsync(o.host_normal[i], o.normal[i], o.bytes[i], cudaMemcpyDeviceToHost, s));
             }
         }
-        return BGS_OK;
-    };
-    const bool views_to_host = o.views > 0 && o.view_host[0] != nullptr;
-    if (o.slot >= 0 && (o.host_rgba || views_to_host)) {
-        CU(c, cudaStreamWaitEvent(c->stream_copy, c->ev_raster[o.slot], 0));
-        if (views_to_host) TRY(copy_views(c->stream_copy));
-        else CU(c, cudaMemcpyAsync(o.host_rgba, o.rgba, o.bytes, cudaMemcpyDeviceToHost, c->stream_copy));
-        CU(c, cudaEventRecord(c->ev_copied[o.slot], c->stream_copy));
-        c->copy_pending[o.slot] = true;
-    } else if (views_to_host) {
-        TRY(copy_views(q));
-    } else if (o.host_rgba) {
-        CU(c, cudaMemcpyAsync(o.host_rgba, o.rgba, o.bytes, cudaMemcpyDeviceToHost, q));
-        if (o.host_depth) {
-            CU(c, cudaMemcpyAsync(o.host_depth, o.depth, o.bytes, cudaMemcpyDeviceToHost, q));
-            CU(c, cudaMemcpyAsync(o.host_normal, o.normal, o.bytes, cudaMemcpyDeviceToHost, q));
-        }
         if (o.host_pick)
-            CU(c, cudaMemcpyAsync(o.host_pick, o.pick, (size_t)fc.Wi * fc.Hi * sizeof(bgs_pick), cudaMemcpyDeviceToHost, q));
+            CU(c, cudaMemcpyAsync(o.host_pick, o.pick, (size_t)fc.Wi * fc.Hi * sizeof(bgs_pick), cudaMemcpyDeviceToHost, s));
+        if (o.slot >= 0) {
+            CU(c, cudaEventRecord(c->ev_copied[o.slot], c->stream_copy));
+            c->copy_pending[o.slot] = true;
+        }
     }
     c->pend = {cloud, n, fc, !p.by_slot, p.by_slot, p.rounds, views ? (int)num_tiles : fc.tiles_x, views ? 1 : fc.tiles_y, fc.Wi,
-               fc.Hi, o.rgba, zd != nullptr || o.pick != nullptr, scene};
+               fc.Hi, o.rgba[0], zd != nullptr || o.pick != nullptr, scene};
     c->launches = launches;
     return BGS_OK;
 }
@@ -743,20 +738,17 @@ static bgs_status check_scene_depth(bgs_context* c, const bgs_scene_depth* zd, c
 }
 
 static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                              const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
-                              int out_is_device_ptr, bool want_aux, void* out_depth, void* out_normal,
-                              const bgs_scene_depth* zd = nullptr, const TemporalConsts* tc = nullptr,
-                              const std::shared_ptr<const SceneFacts>& scene = nullptr, const ViewTargets* view_targets = nullptr,
-                              void* out_pick = nullptr) {
+                              const bgs_settings* st, const bgs_render_extras* ex, const Targets& t, const bgs_scene_depth* zd,
+                              const TemporalConsts* tc, const std::shared_ptr<const SceneFacts>& scene) {
     if (!c) return BGS_EINVAL;
-    if (!scene) TRY(check_render(c, cloud, view, uni, st, ex, out_format, want_aux, tc != nullptr));   // (scenes: per cloud, before)
+    if (!scene) TRY(check_render(c, cloud, view, uni, st, ex, t.format, t.aux, tc != nullptr));   // (scenes: per cloud, before)
     if (zd) TRY(check_scene_depth(c, zd, view));
     if (c->async_pending && !(st->flags & BGS_FLAG_ASYNC)) {
         // a synchronous render after queued frames completes them first; their failure (including an overflowed
         // pair list = BGS_NOT_READY) is the caller's to see, so this frame is not rendered on top of it
         TRY(bgs_sync(c));
     }
-    const FrameConsts fc = scene ? scene->tab.seg[0].fc : frame_consts(cloud, view, uni, st, want_aux);
+    const FrameConsts fc = scene ? scene->tab.seg[0].fc : frame_consts(cloud, view, uni, st, t.aux);
     // Classification / OpticalFlow, and every scene frame: the projection takes the extras (NULL extras: num_classes = 1)
     ModeConsts mc = {};
     mc.num_classes = ex ? ex->num_classes : 1u;
@@ -769,34 +761,25 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
     FrameOut o;
-    if (views) TRY(frame_out_views(c, st, out_format, scene->views, *view_targets, out_is_device_ptr, &o));
-    else TRY(frame_out(c, st, out_format, (size_t)fc.Wi * fc.Hi * format_bpp(out_format), out_rgba, out_is_device_ptr, want_aux,
-                       out_depth, out_normal, &o));
-    if (out_pick && out_is_device_ptr) {
-        o.pick = static_cast<uint4*>(out_pick);
-    } else if (out_pick) {
-        TRY(c->pick_frame.grow(c, (size_t)fc.Wi * fc.Hi * sizeof(bgs_pick), false));
-        o.pick = c->pick_frame.p;
-        o.host_pick = out_pick;
-    }
+    TRY(frame_out(c, st, t, views ? scene->views.W : &fc.Wi, views ? scene->views.H : &fc.Hi, &o));
     ViewTable vt = {};
     if (views) {
         vt = scene->views;
         for (uint32_t i = 0; i < vt.v; ++i) {
-            vt.out[i] = o.view_rgba[i];
-            vt.out_depth[i] = o.view_depth[i];
-            vt.out_normal[i] = o.view_normal[i];
+            vt.out[i] = o.rgba[i];
+            vt.out_depth[i] = o.depth[i];
+            vt.out_normal[i] = o.normal[i];
         }
     }
     for (int attempt = 0; attempt < 4; ++attempt) {
-        FramePlan p = plan_frame(c, st, want_aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
+        FramePlan p = plan_frame(c, st, t.aux, num_tiles, n);   // (each attempt: the pair hints read cap_pairs)
         if (scene) {   // (st plans it as an aabb frame or an overlay one: one round)
             p.raster_mode = scene->raster_mode;
             p.box = scene->box;
         }
         if (p.raster_mode == 2 || p.raster_mode == 4) TRY(c->extra.grow(c, (size_t)c->cap_n * 64, false));
         if (p.raster_mode >= 3) TRY(c->kinds.grow(c, (size_t)c->cap_n, false));
-        if (want_aux) TRY(c->aux.grow(c, (size_t)c->cap_n * 32, false));
+        if (t.aux) TRY(c->aux.grow(c, (size_t)c->cap_n * 32, false));
         if (zd || o.pick) TRY(c->splat_depth.grow(c, (size_t)c->cap_n * 4, false));
         if (p.rounds > 1) TRY(c->state.grow(c, (size_t)num_tiles * 256 * sizeof(float4), false));
         TRY(ensure_arena(c, num_tiles));
@@ -821,13 +804,13 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
 bgs_status bgs_render_ex(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                          const bgs_settings* st, const bgs_render_extras* ex, void* out_rgba, uint32_t out_format,
                          int out_is_device_ptr) {
-    return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr);
+    return render_impl(c, cloud, view, uni, st, ex, colour_target(&out_rgba, out_format, out_is_device_ptr), nullptr, nullptr, nullptr);
 }
 
 bgs_status bgs_render_depth_test(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                                  const bgs_settings* st, const bgs_render_extras* ex, const bgs_scene_depth* depth,
                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
-    return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth);
+    return render_impl(c, cloud, view, uni, st, ex, colour_target(&out_rgba, out_format, out_is_device_ptr), depth, nullptr, nullptr);
 }
 
 // bgs_render_4d's time refusals (include/bgs.h): time and window finite, time_stop != time_start, and a window length
@@ -850,7 +833,7 @@ bgs_status bgs_render_4d(bgs_context* c, const bgs_cloud* cloud, const bgs_view*
     if (!c) return BGS_EINVAL;
     TemporalConsts tc = {};
     if (uni) TRY(temporal_consts(c, "render_4d", uni->time, time_start, time_stop, tc));
-    return render_impl(c, cloud, view, uni, st, ex, out_rgba, out_format, out_is_device_ptr, false, nullptr, nullptr, depth, &tc);
+    return render_impl(c, cloud, view, uni, st, ex, colour_target(&out_rgba, out_format, out_is_device_ptr), depth, &tc, nullptr);
 }
 
 // the refusals every scene call makes of its list before reading it: k, SORT_ALL and NULL clouds
@@ -868,18 +851,17 @@ static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.ga
 
 // Every scene frame: k entities, each checked as its single-cloud call (bgs_render_depth_test, or bgs_render_4d for a
 // Gaussian4d cloud when with_4d) with its own settings, num_classes and window, drawn into one depth-sorted frame.
-// entity_flags: each entity's BGS_ENTITY_* bits (NULL: none).  The list has passed check_scene_list.  want_aux
-// (bgs_render_entities_aux): every segment also projects its Depth and Normal colours, blended into out_depth / out_normal.
-// nv > 1 (bgs_render_views or, with want_aux, bgs_render_views_aux, which have checked nv, the targets and the entities'
-// modes): the k entities seen from each of the nv views (depth: nv buffers, or NULL), segment i k + j entity j from view i,
-// view i's frames into view_targets' entries i.
+// entity_flags: each entity's BGS_ENTITY_* bits (NULL: none).  The list has passed check_scene_list.  Aux targets
+// (bgs_render_entities_aux): every segment also projects its Depth and Normal colours, blended into the depth and normal
+// frames.  t.v = nv > 1 views (bgs_render_views or, with aux targets, bgs_render_views_aux, which have checked nv, the
+// targets and the entities' modes): the k entities seen from each of the nv views (depth: nv buffers, or NULL), segment
+// i k + j entity j from view i, view i's frames into its targets.
 static bgs_status render_entities_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
                                        const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                        const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
                                        const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
-                                       void* out_rgba, uint32_t out_format, int out_is_device_ptr, bool want_aux = false,
-                                       void* out_depth = nullptr, void* out_normal = nullptr, uint32_t nv = 1,
-                                       const ViewTargets* view_targets = nullptr, void* out_pick = nullptr) {
+                                       const Targets& t) {
+    const uint32_t nv = t.v;
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
         return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
@@ -904,7 +886,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
         if (!is4 && chk.rasterize_mode == BGS_RASTERIZE_VELOCITY) chk.rasterize_mode = BGS_RASTERIZE_COLOR;
         for (uint32_t i = 0; i < nv; ++i)   // (as the single-view call of each view)
             TRY(check_render(c, clouds[j], &view[i], &unis[j], &chk,
-                             ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr, out_format, false, is4));
+                             ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr, t.format, false, is4));
         if (is4) TRY(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, scene->times.t[j]));
         const bgs_entity_settings& e0 = ents[0];
         undrawn = undrawn && !is4 && e.rasterize_mode == BGS_RASTERIZE_VELOCITY && e.gaussian_mode == e0.gaussian_mode &&
@@ -934,7 +916,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
             const bgs_cloud* cl = clouds[j];
             const uint32_t rm = st[j].rasterize_mode;
             SceneSeg& sg = tab.seg[sj];
-            sg.fc = frame_consts(cl, &view[i], &unis[j], &st[j], want_aux);
+            sg.fc = frame_consts(cl, &view[i], &unis[j], &st[j], t.aux);
             sg.fc.n_cloud = (uint32_t)n_view;   // (Depth colouring reads its view's sorted list of n_view entries)
             sg.pos = cl->pos;
             sg.blocks = cl->blocks;
@@ -978,9 +960,8 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     sf.gaussian_mode = scene->raster_mode == 2 ? BGS_GAUSSIAN_2D : BGS_GAUSSIAN_3D;
     sf.draw_mode = BGS_DRAW_ALL;
     if (scene->box) sf.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
-    if (nv > 1 || out_pick) sf.flags = (sf.flags & ~(uint32_t)BGS_FLAG_CHUNKS) | BGS_FLAG_NO_CHUNKS;   // (one round)
-    return render_impl(c, clouds[0], view, &unis[0], &sf, ex, out_rgba, out_format, out_is_device_ptr, want_aux, out_depth,
-                       out_normal, depth, nullptr, scene, view_targets, out_pick);
+    if (nv > 1 || t.pick) sf.flags = (sf.flags & ~(uint32_t)BGS_FLAG_CHUNKS) | BGS_FLAG_NO_CHUNKS;   // (one round)
+    return render_impl(c, clouds[0], view, &unis[0], &sf, ex, t, depth, nullptr, scene);
 }
 
 // bgs_render_scene, and bgs_render_scene_4d (with_4d: Gaussian4d clouds are projected at uniforms[j].time in windows[j];
@@ -1015,8 +996,8 @@ static bgs_status render_scene_as_entities(bgs_context* c, const char* call, boo
         e.num_classes = ex ? ex->num_classes : 1u;
         e.window = is4 ? windows[j] : bgs_time_window{};
     }
-    return render_entities_impl(c, call, with_4d, clouds, unis, ents.data(), nullptr, k, view, st, ex, depth, out_rgba,
-                                out_format, out_is_device_ptr);
+    return render_entities_impl(c, call, with_4d, clouds, unis, ents.data(), nullptr, k, view, st, ex, depth,
+                                colour_target(&out_rgba, out_format, out_is_device_ptr));
 }
 
 bgs_status bgs_render_scene(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis, uint32_t k,
@@ -1055,12 +1036,63 @@ bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds
     const char* call = "render_entities";
     if (!c) return BGS_EINVAL;
     TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
-    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
-                                out_is_device_ptr);
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth,
+                                colour_target(&out_rgba, out_format, out_is_device_ptr));
 }
 
-// bgs_render_entities_ex's frame and, in the same pass, its Depth and Normal frames (include/bgs.h): the refusals of
-// bgs_render_entities_ex, then those of the aux frames
+// The refusals of bgs_render_entities_aux, _pick, bgs_render_views and _views_aux (include/bgs.h), in this order, each
+// made by the calls it names: bgs_render_entities_ex's of the list; v and v x k (views calls); the targets; BGS_FLAG_ASYNC
+// (aux and pick calls); each entity's: Gaussian4d, covariance and Velocity (aux calls), Depth (views without aux),
+// OpticalFlow (views calls); blend-over (views calls: device targets only).
+static bgs_status check_targets_call(bgs_context* c, const char* call, const bgs_cloud* const* clouds,
+                                     const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
+                                     const uint32_t* entity_flags, uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                                     const Targets& t, bool views, bool pick) {
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
+    if (views) {
+        if (t.v == 0) return fail(c, BGS_EINVAL, "%s: v = 0 views", call);
+        if ((uint64_t)t.v * k > BGS_SCENE_MAX_CLOUDS)
+            return fail(c, BGS_EINVAL, "%s: v x k = %u x %u segments, at most %d", call, t.v, k, BGS_SCENE_MAX_CLOUDS);
+        const size_t bpp = format_bpp(t.format);
+        const char* names[3] = {"out_rgba", "out_depth", "out_normal"};
+        void* const* arrays[3] = {t.rgba, t.depth, t.normal};
+        for (int a = 0; a < (t.aux ? 3 : 1); ++a) {
+            if (!arrays[a]) return fail(c, BGS_EINVAL, "%s: %s is NULL", call, names[a]);
+            for (uint32_t i = 0; i < t.v; ++i) {
+                if (!arrays[a][i]) return fail(c, BGS_EINVAL, "%s: %s[%u] is NULL", call, names[a], i);
+                if (t.device && reinterpret_cast<uintptr_t>(arrays[a][i]) % bpp != 0)
+                    return fail(c, BGS_EINVAL, "%s: device target %s[%u] = %p is not aligned to its %zu-byte pixels", call,
+                                names[a], i, arrays[a][i], bpp);
+            }
+        }
+    } else if (t.aux && (!t.rgba[0] || !t.depth[0] || !t.normal[0])) {
+        return fail(c, BGS_EINVAL, "%s: the three output frames are required", call);
+    }
+    if (pick) {
+        if (!t.pick) return fail(c, BGS_EINVAL, "%s: out_pick is NULL", call);
+        if (t.device && reinterpret_cast<uintptr_t>(t.pick) % sizeof(bgs_pick) != 0)
+            return fail(c, BGS_EINVAL, "%s: device pick target %p is not aligned to its 16-byte records", call, t.pick);
+    }
+    if ((t.aux || pick) && (frame->flags & BGS_FLAG_ASYNC)) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
+    for (uint32_t j = 0; j < k; ++j) {
+        // (a 4D cloud has no Normal colour; a covariance cloud no rotation; Velocity changes which splats draw, and how; a
+        // views frame's Depth entity would take its colour range from every view's sorted list; OpticalFlow has one previous
+        // view per frame)
+        const uint32_t rm = ents[j].rasterize_mode;
+        if (t.aux && is_4d(clouds[j]->layout)) return fail(c, BGS_EINVAL, "%s: clouds[%u] is a Gaussian4d cloud", call, j);
+        if (t.aux && clouds[j]->layout == CloudLayout::F16Cov)
+            return fail(c, BGS_EINVAL, "%s: clouds[%u] is a precomputed-covariance cloud (no rotation for the normal)", call, j);
+        if (t.aux && rm == BGS_RASTERIZE_VELOCITY) return fail(c, BGS_EINVAL, "%s: entities[%u] is in Velocity mode", call, j);
+        if (views && !t.aux && rm == BGS_RASTERIZE_DEPTH) return fail(c, BGS_EINVAL, "%s: entities[%u] is in Depth mode", call, j);
+        if (views && rm == BGS_RASTERIZE_OPTICAL_FLOW)
+            return fail(c, BGS_EINVAL, "%s: entities[%u] is in OpticalFlow mode", call, j);
+    }
+    if (views && (frame->flags & BGS_FLAG_BLEND_OVER_TARGET) && !t.device)
+        return fail(c, BGS_EINVAL, "%s: BGS_FLAG_BLEND_OVER_TARGET takes device targets", call);
+    return BGS_OK;
+}
+
+// bgs_render_entities_ex's frame and, in the same pass, its Depth and Normal frames (include/bgs.h)
 bgs_status bgs_render_entities_aux(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
                                    const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k,
                                    const bgs_view* view, const bgs_settings* frame, const bgs_render_extras* ex,
@@ -1068,23 +1100,12 @@ bgs_status bgs_render_entities_aux(bgs_context* c, const bgs_cloud* const* cloud
                                    uint32_t out_format, int out_is_device_ptr) {
     const char* call = "render_entities_aux";
     if (!c) return BGS_EINVAL;
-    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
-    if (!out_rgba || !out_depth || !out_normal) return fail(c, BGS_EINVAL, "%s: the three output frames are required", call);
-    if (frame->flags & BGS_FLAG_ASYNC) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
-    for (uint32_t j = 0; j < k; ++j) {
-        // (a 4D cloud has no Normal colour; a covariance cloud no rotation; Velocity changes which splats draw, and how)
-        if (is_4d(clouds[j]->layout)) return fail(c, BGS_EINVAL, "%s: clouds[%u] is a Gaussian4d cloud", call, j);
-        if (clouds[j]->layout == CloudLayout::F16Cov)
-            return fail(c, BGS_EINVAL, "%s: clouds[%u] is a precomputed-covariance cloud (no rotation for the normal)", call, j);
-        if (ents[j].rasterize_mode == BGS_RASTERIZE_VELOCITY)
-            return fail(c, BGS_EINVAL, "%s: entities[%u] is in Velocity mode", call, j);
-    }
-    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
-                                out_is_device_ptr, true, out_depth, out_normal);
+    const Targets t{out_format, out_is_device_ptr, 1, true, &out_rgba, &out_depth, &out_normal, nullptr};
+    TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, view, frame, t, false, false));
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, t);
 }
 
-// bgs_render_entities_ex's frame and, from the same blend, its pick frame (include/bgs.h): the refusals of
-// bgs_render_entities_ex, then those of the pick target
+// bgs_render_entities_ex's frame and, from the same blend, its pick frame (include/bgs.h)
 bgs_status bgs_render_entities_pick(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
                                     const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k,
                                     const bgs_view* view, const bgs_settings* frame, const bgs_render_extras* ex,
@@ -1092,94 +1113,39 @@ bgs_status bgs_render_entities_pick(bgs_context* c, const bgs_cloud* const* clou
                                     void* out_pick) {
     const char* call = "render_entities_pick";
     if (!c) return BGS_EINVAL;
-    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
-    if (!out_pick) return fail(c, BGS_EINVAL, "%s: out_pick is NULL", call);
-    if (out_is_device_ptr && reinterpret_cast<uintptr_t>(out_pick) % sizeof(bgs_pick) != 0)
-        return fail(c, BGS_EINVAL, "%s: device pick target %p is not aligned to its 16-byte records", call, out_pick);
-    if (frame->flags & BGS_FLAG_ASYNC) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
-    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, out_rgba, out_format,
-                                out_is_device_ptr, false, nullptr, nullptr, 1, nullptr, out_pick);
+    const Targets t{out_format, out_is_device_ptr, 1, false, &out_rgba, nullptr, nullptr, out_pick};
+    TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, view, frame, t, false, true));
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, t);
 }
 
-// bgs_render_entities_ex of each of v views in one frame (include/bgs.h): the refusals of bgs_render_entities_ex (each view
-// checked as its own call), then those of the views frame; one view is bgs_render_entities_ex itself
+// bgs_render_entities_ex of each of v views in one frame (include/bgs.h); one view is bgs_render_entities_ex itself
 bgs_status bgs_render_views(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
                             const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* views,
                             uint32_t v, const bgs_settings* frame, const bgs_scene_depth* depths, void* const* out_rgba,
                             uint32_t out_format, int out_is_device_ptr) {
     const char* call = "render_views";
     if (!c) return BGS_EINVAL;
-    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, views, frame));
-    if (v == 0) return fail(c, BGS_EINVAL, "%s: v = 0 views", call);
-    if ((uint64_t)v * k > BGS_SCENE_MAX_CLOUDS)
-        return fail(c, BGS_EINVAL, "%s: v x k = %u x %u segments, at most %d", call, v, k, BGS_SCENE_MAX_CLOUDS);
-    if (!out_rgba) return fail(c, BGS_EINVAL, "%s: out_rgba is NULL", call);
-    const size_t bpp = format_bpp(out_format);
-    for (uint32_t i = 0; i < v; ++i) {
-        if (!out_rgba[i]) return fail(c, BGS_EINVAL, "%s: out_rgba[%u] is NULL", call, i);
-        if (out_is_device_ptr && reinterpret_cast<uintptr_t>(out_rgba[i]) % bpp != 0)
-            return fail(c, BGS_EINVAL, "%s: device target out_rgba[%u] = %p is not aligned to its %zu-byte pixels", call, i,
-                        out_rgba[i], bpp);
-    }
-    for (uint32_t j = 0; j < k; ++j) {
-        // (a Depth entity's colour range is the frame's sorted list; OpticalFlow has one previous view per frame)
-        if (ents[j].rasterize_mode == BGS_RASTERIZE_DEPTH) return fail(c, BGS_EINVAL, "%s: entities[%u] is in Depth mode", call, j);
-        if (ents[j].rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW)
-            return fail(c, BGS_EINVAL, "%s: entities[%u] is in OpticalFlow mode", call, j);
-    }
-    if ((frame->flags & BGS_FLAG_BLEND_OVER_TARGET) && !out_is_device_ptr)
-        return fail(c, BGS_EINVAL, "%s: BGS_FLAG_BLEND_OVER_TARGET takes device targets", call);
+    const Targets t{out_format, out_is_device_ptr, v, false, out_rgba, nullptr, nullptr, nullptr};
+    TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, views, frame, t, true, false));
     if (v == 1)
         return bgs_render_entities_ex(c, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, out_rgba[0], out_format,
                                       out_is_device_ptr);
-    const ViewTargets targets{out_rgba, nullptr, nullptr};
-    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, nullptr,
-                                out_format, out_is_device_ptr, false, nullptr, nullptr, v, &targets);
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, t);
 }
 
-// bgs_render_entities_aux of each of v views in one frame (include/bgs.h): the refusals of bgs_render_entities_aux and of
-// bgs_render_views but the Depth one, then those of its three target arrays; one view is bgs_render_entities_aux itself
+// bgs_render_entities_aux of each of v views in one frame (include/bgs.h); one view is bgs_render_entities_aux itself
 bgs_status bgs_render_views_aux(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
                                 const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* views,
                                 uint32_t v, const bgs_settings* frame, const bgs_scene_depth* depths, void* const* out_rgba,
                                 void* const* out_depth, void* const* out_normal, uint32_t out_format, int out_is_device_ptr) {
     const char* call = "render_views_aux";
     if (!c) return BGS_EINVAL;
-    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, views, frame));
-    if (v == 0) return fail(c, BGS_EINVAL, "%s: v = 0 views", call);
-    if ((uint64_t)v * k > BGS_SCENE_MAX_CLOUDS)
-        return fail(c, BGS_EINVAL, "%s: v x k = %u x %u segments, at most %d", call, v, k, BGS_SCENE_MAX_CLOUDS);
-    const size_t bpp = format_bpp(out_format);
-    const char* names[3] = {"out_rgba", "out_depth", "out_normal"};
-    void* const* arrays[3] = {out_rgba, out_depth, out_normal};
-    for (int a = 0; a < 3; ++a) {
-        if (!arrays[a]) return fail(c, BGS_EINVAL, "%s: %s is NULL", call, names[a]);
-        for (uint32_t i = 0; i < v; ++i) {
-            if (!arrays[a][i]) return fail(c, BGS_EINVAL, "%s: %s[%u] is NULL", call, names[a], i);
-            if (out_is_device_ptr && reinterpret_cast<uintptr_t>(arrays[a][i]) % bpp != 0)
-                return fail(c, BGS_EINVAL, "%s: device target %s[%u] = %p is not aligned to its %zu-byte pixels", call, names[a],
-                            i, arrays[a][i], bpp);
-        }
-    }
-    if (frame->flags & BGS_FLAG_ASYNC) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
-    for (uint32_t j = 0; j < k; ++j) {
-        // (bgs_render_entities_aux's refusals; OpticalFlow has one previous view per frame)
-        if (is_4d(clouds[j]->layout)) return fail(c, BGS_EINVAL, "%s: clouds[%u] is a Gaussian4d cloud", call, j);
-        if (clouds[j]->layout == CloudLayout::F16Cov)
-            return fail(c, BGS_EINVAL, "%s: clouds[%u] is a precomputed-covariance cloud (no rotation for the normal)", call, j);
-        if (ents[j].rasterize_mode == BGS_RASTERIZE_VELOCITY)
-            return fail(c, BGS_EINVAL, "%s: entities[%u] is in Velocity mode", call, j);
-        if (ents[j].rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW)
-            return fail(c, BGS_EINVAL, "%s: entities[%u] is in OpticalFlow mode", call, j);
-    }
-    if ((frame->flags & BGS_FLAG_BLEND_OVER_TARGET) && !out_is_device_ptr)
-        return fail(c, BGS_EINVAL, "%s: BGS_FLAG_BLEND_OVER_TARGET takes device targets", call);
+    const Targets t{out_format, out_is_device_ptr, v, true, out_rgba, out_depth, out_normal, nullptr};
+    TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, views, frame, t, true, false));
     if (v == 1)
         return bgs_render_entities_aux(c, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, out_rgba[0],
                                        out_depth[0], out_normal[0], out_format, out_is_device_ptr);
-    const ViewTargets targets{out_rgba, out_depth, out_normal};
-    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, nullptr,
-                                out_format, out_is_device_ptr, true, nullptr, nullptr, v, &targets);
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, t);
 }
 
 bgs_status bgs_render_entities(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
@@ -1200,7 +1166,8 @@ bgs_status bgs_render_aux(bgs_context* c, const bgs_cloud* cloud, const bgs_view
                           int out_is_device_ptr) {
     if (c && (!out_rgba || !out_depth || !out_normal)) return fail(c, BGS_EINVAL, "render_aux: the three output frames are required");
     if (c && st && (st->flags & BGS_FLAG_ASYNC)) return fail(c, BGS_EINVAL, "render_aux: BGS_FLAG_ASYNC is not supported");
-    return render_impl(c, cloud, view, uni, st, nullptr, out_rgba, out_format, out_is_device_ptr, true, out_depth, out_normal);
+    const Targets t{out_format, out_is_device_ptr, 1, true, &out_rgba, &out_depth, &out_normal, nullptr};
+    return render_impl(c, cloud, view, uni, st, nullptr, t, nullptr, nullptr, nullptr);
 }
 
 bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {

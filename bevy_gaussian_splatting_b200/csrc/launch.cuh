@@ -80,46 +80,53 @@ void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_sl
                         const FrameConsts& fc, float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
 void launch_splat_depth_scene(const SceneTable& tab, const uint32_t* slot_ids, const FrameCounters* ctr, float* depths,
                               uint32_t n_hint, int sm_count, cudaStream_t stream);
-// raster.cu.  ZTestArgs: a depth-tested frame's splat depths (indexed like the records) and the scene's depth buffer
-// (bgs_scene_depth); scene == nullptr blends without the test.
-struct ZTestArgs {
-    const float* splat_d = nullptr;
-    const float* scene = nullptr;
-    size_t pitch = 0;
-};
-// mode 0..2: one blend kind for every splat; 3 / 4 (bgs_render_entities): mixed kinds, read from `kinds` (one byte per
-// record), 4 when some splat is a surfel.  box: the bounding-box overlay (BGS_FLAG_VISUALIZE_BOUNDING_BOX) on every
-// splat, or on a mixed frame on those whose kinds byte has bit 2 set; large_footprints is then not read.
-void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
-                   const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
-                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
-                   cudaStream_t stream, const unsigned char* kinds = nullptr, bool box = false);
-// a mixed-geometry frame's blend kind of each compact slot (records n_vis of ctr), from its segment's
-void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
-                          uint32_t n_hint, int sm_count, cudaStream_t stream);
-// bgs_render_views' blend: one CTA per global tile of every view (vt.tile0[vt.v]), each into its view's target; mode and box
-// as launch_raster's; splat_d non-null and vt.scene[i]: the depth test against view i's buffer; aux non-null
-// (bgs_render_views_aux): also the depth and normal frames, into vt.out_depth[i] / vt.out_normal[i]
-void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
-                         uint32_t format, const uint32_t* truncated, const float* splat_d, const unsigned char* kinds, bool box,
-                         const ViewTable& vt, cudaStream_t stream, const float4* aux = nullptr);
-// bgs_render_entities_pick: launch_raster's frame (mode and box as there, never raster2_kernel) and, per pixel, the pick
-// record (include/bgs.h's bgs_pick) into `out`, from the record's global index (slot_ids) and segment (seg: offsets and
-// k) and its depth zt.splat_d[record] (a pick frame's splat depths, written with or without a depth buffer; zt.scene
-// NULL: no depth test)
+// raster.cu.  A one-round frame's blend of the sorted pairs `tile_entries` (per tile: `ranges`) into `out`, W x H in
+// tiles_x x tiles_y tiles, in `format` (BGS_FORMAT_* | output mode << 8).  mode 0..2: one blend kind for every splat;
+// 3 / 4 (bgs_render_entities): mixed kinds, read from `kinds` (one byte per record), 4 when some splat is a surfel.  box:
+// the bounding-box overlay (BGS_FLAG_VISUALIZE_BOUNDING_BOX) on every splat, or on a mixed frame on those whose kinds byte
+// has bit 2 set.  large_footprints: the quad-uv blend of a plain single-view frame takes raster2_kernel.  aux non-null
+// (bgs_render_aux, _entities_aux, _views_aux): also the depth and normal frames, into out_depth / out_normal.  scene
+// non-null (bgs_scene_depth): the depth test of the splat depths splat_d (indexed like the records) against that buffer.
+// views non-null (bgs_render_views, _views_aux): one CTA per global tile of every view (views->tile0[views->v]), each into
+// its view's targets and depth buffer (scene is then view 0's).  pick non-null (bgs_render_entities_pick): also, per pixel,
+// the pick record (include/bgs.h's bgs_pick) into pick->out, from the record's global index (slot_ids) and segment (seg:
+// offsets and k) and its depth splat_d[record] (written with or without a depth buffer).
 struct PickArgs {
     uint4* out;
     const uint32_t* slot_ids;
     SegmentKinds seg;
 };
 static_assert(sizeof(bgs_pick) == sizeof(uint4), "a pick record is stored as one uint4");
-void launch_raster_pick(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
-                        int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format, const uint32_t* truncated,
-                        const ZTestArgs& zt, const unsigned char* kinds, bool box, const PickArgs& pk, cudaStream_t stream);
-void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
-                         int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
-                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,
+struct BlendArgs {
+    int mode = 0;
+    bool box = false;
+    bool large_footprints = false;
+    const SplatRec* recs = nullptr;
+    const float4* extra = nullptr;
+    const uint32_t* tile_entries = nullptr;
+    const uint2* ranges = nullptr;
+    int W = 0, H = 0, tiles_x = 0, tiles_y = 0;
+    void* out = nullptr;
+    uint32_t format = 0;
+    const float4* aux = nullptr;
+    void* out_depth = nullptr;
+    void* out_normal = nullptr;
+    const uint32_t* truncated = nullptr;
+    const float* splat_d = nullptr;
+    const float* scene = nullptr;
+    size_t pitch = 0;
+    const unsigned char* kinds = nullptr;
+    const ViewTable* views = nullptr;
+    const PickArgs* pick = nullptr;
+};
+void launch_raster(const BlendArgs& a, cudaStream_t stream);
+// one front-to-back round of a chunked frame (a's single-view quad-uv blend, depth test included): each pixel's blend state
+// in `state` between rounds, tile_done / tiles_done the tiles saturated so far
+void launch_raster_round(const BlendArgs& a, float4* state, unsigned char* tile_done, uint32_t* tiles_done, int first, int last,
                          cudaStream_t stream);
+// a mixed-geometry frame's blend kind of each compact slot (records n_vis of ctr), from its segment's
+void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
+                          uint32_t n_hint, int sm_count, cudaStream_t stream);
 // select.cu
 uint32_t select_num_buckets(uint32_t n);
 int select_sort_passes(uint32_t n_buckets);

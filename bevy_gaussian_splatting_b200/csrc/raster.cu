@@ -14,6 +14,9 @@
 // Coverage maths (quad_uv) uses explicit __fmul_rn/__fmaf_rn so u,v are bit-identical to the oracle.
 #include <cuda_fp16.h>
 
+#include <type_traits>
+#include <utility>
+
 #include "common.cuh"
 #include "launch.cuh"
 
@@ -255,18 +258,18 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // MODE 3 / 4 (bgs_render_entities): mixed kinds, each splat tested by its own: kinds[r] (raster_kinds_kernel) is record r's
 // 0 = quad-uv, 1 = conic, 2 = surfel; MODE 4 when some splat is a surfel (the only one that stages the surfel records).
 // Warp candidates: bbox for every kind, and the separating-axis test of MODE 0 for the quad-uv splats.
-// BOX (raster_box_kernel, raster_mixed_box_kernel): the bounding-box overlay.  A covered pair (after the aabb discard and
-// the depth test) on its quad's edge band (box_edge) blends (0.3, 1, 0.1) at alpha 1 into every frame it writes, which
-// stops the pixel; other pairs blend as without it.  Mixed frames read the overlay bit of each splat from bit 2 of its
-// kinds byte (its entity's), the others draw every splat's box.  MODE 0 takes the generic loop, not the inline-asm one.
-// VIEWS (raster_views_kernel, bgs_render_views): the CTA's global tile blockIdx.x lies in view i = vt->view_of_tile; W, H,
-// tiles_x, out, scene and pitch are then view i's, the CTA takes the local tile blockIdx.x - tile0[i] in centre_out_tile's
-// order within the view, and reads the global tile's range.  With AUX (raster_views_aux_kernel, bgs_render_views_aux)
-// out_depth and out_normal are view i's too.
-// PICK (raster_pick_kernel, bgs_render_entities_pick): beside its colour each pixel keeps the largest weight w = a T of the
-// pairs it blends (an overlay edge pair: w = T) and that pair's record; a later pair replaces it only when its w is strictly
-// larger.  Every pixel of pk->out is written: (entity, index, w, d) of that pair, or BGS_PICK_NONE where nothing blends.
-// Pick frames take the generic loop in every mode, never the inline-asm one.
+// BOX (BGS_FLAG_VISUALIZE_BOUNDING_BOX): the bounding-box overlay.  A covered pair (after the aabb discard and the depth
+// test) on its quad's edge band (box_edge) blends (0.3, 1, 0.1) at alpha 1 into every frame it writes, which stops the
+// pixel; other pairs blend as without it.  Mixed frames read the overlay bit of each splat from bit 2 of its kinds byte
+// (its entity's), the others draw every splat's box.  MODE 0 takes the generic loop, not the inline-asm one.
+// VIEWS (raster_kernel's ViewTable variants, bgs_render_views): the CTA's global tile blockIdx.x lies in view
+// i = vt->view_of_tile; W, H, tiles_x, out, scene and pitch are then view i's, the CTA takes the local tile
+// blockIdx.x - tile0[i] in centre_out_tile's order within the view, and reads the global tile's range.  With AUX
+// (bgs_render_views_aux) out_depth and out_normal are view i's too.
+// PICK (raster_kernel's PickArgs variants, bgs_render_entities_pick): beside its colour each pixel keeps the largest
+// weight w = a T of the pairs it blends (an overlay edge pair: w = T) and that pair's record; a later pair replaces it only
+// when its w is strictly larger.  Every pixel of pk->out is written: (entity, index, w, d) of that pair, or BGS_PICK_NONE
+// where nothing blends.  Pick frames take the generic loop in every mode, never the inline-asm one.
 template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false, bool PICK = false>
 __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
                                             const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
@@ -577,106 +580,51 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
     }
 }
 
-// (MODE 2 with AUX and ZTEST spills at 5 CTAs per SM: 4 leave it 64 registers)
-template <int MODE, bool AUX, bool ZTEST = false>
-__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : (MODE == 2 && AUX && ZTEST ? 4 : 5))
+// The blend kernels: raster_body of one (MODE, AUX, ZTEST, BOX) and one frame kind, picked by the trailing parameter's type
+// Tail: OneView (a single-view frame), ViewTable (a views frame: raster_body's VIEWS) or PickArgs (a pick frame: its PICK).
+// Every variant takes the same scalar parameters; raster_body sees null for those its variant never reads, so a variant's
+// code does not depend on them.
+struct OneView {};
+template <class Tail> constexpr bool IS_VIEWS = std::is_same<Tail, ViewTable>::value;
+template <class Tail> constexpr bool IS_PICK = std::is_same<Tail, PickArgs>::value;
+
+// Minimum CTAs per SM of each variant: the most that leave it without spills (ptxas report), and for MODE 0 without aux
+// the 6 its register budget was written for.
+//   single view, MODE 0..2: MODE 2 with AUX and ZTEST spills at 5 (4 leave it 64 registers).
+//   single view, mixed (MODE 3 / 4): ZTEST spills at 5; with AUX, MODE 4 too.
+//   views: MODE 0 spills at 6; the mixed depth-tested blends, the depth-tested overlay and MODE 4's overlay at 5.  With
+//     AUX: MODE 2 with ZTEST spills at 4 (3 leave it 85 registers); MODE 4, and MODE 2 and 3 with ZTEST or BOX, at 5.
+//   pick: MODE 1 and 2 spill at 5 even without the depth test or the overlay; 4 leave every variant 64 registers.
+template <int MODE, bool AUX, bool ZTEST, bool BOX, class Tail>
+constexpr int raster_min_ctas() {
+    if (IS_PICK<Tail>) return 4;
+    if (IS_VIEWS<Tail> && AUX) return MODE == 2 && ZTEST ? 3 : (MODE == 4 || ((ZTEST || BOX) && MODE >= 2) ? 4 : 5);
+    if (IS_VIEWS<Tail>) return (ZTEST && (MODE >= 3 || BOX)) || (BOX && MODE == 4) ? 4 : 5;
+    if (MODE >= 3 && AUX) return MODE == 4 || ZTEST ? 4 : 5;
+    if (MODE >= 3) return ZTEST ? 4 : 5;
+    return MODE == 0 && !AUX ? 6 : (MODE == 2 && AUX && ZTEST ? 4 : 5);
+}
+
+// &tail as a T*, or null when the tail is not a T
+template <class T, class Tail>
+__device__ __forceinline__ const T* tail_as(const Tail& tail) {
+    if constexpr (std::is_same<T, Tail>::value) return &tail;
+    else return nullptr;
+}
+
+template <int MODE, bool AUX, bool ZTEST, bool BOX, class Tail>
+__global__ void __launch_bounds__(RT_THREADS, raster_min_ctas<MODE, AUX, ZTEST, BOX, Tail>())
 raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
               const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
               const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
               const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
-              size_t pitch) {
-    raster_body<MODE, AUX, ZTEST>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal,
-                                  truncated, splat_d, scene, pitch, nullptr);
-}
-
-// bgs_render_entities' blend of mixed kinds (MODE 3, or 4 with surfels).  (At 5 CTAs per SM the depth-tested variant
-// spills: 4 leave it 64 registers.)
-template <int MODE, bool ZTEST>
-__global__ void __launch_bounds__(RT_THREADS, ZTEST ? 4 : 5)
-raster_mixed_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
-                    const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
-                    const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
-                    size_t pitch, const unsigned char* __restrict__ kinds) {
-    raster_body<MODE, false, ZTEST>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr,
-                                    truncated, splat_d, scene, pitch, kinds);
-}
-
-// The bounding-box overlay's blends (raster_body's BOX): raster_kernel's and raster_mixed_kernel's, with their launch
-// bounds.  Kernels of their own, so the frames without the overlay keep the very kernels they had.
-template <int MODE, bool AUX, bool ZTEST>
-__global__ void __launch_bounds__(RT_THREADS, (MODE == 0 && !AUX) ? 6 : (MODE == 2 && AUX && ZTEST ? 4 : 5))
-raster_box_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
-                  const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
-                  const float4* __restrict__ aux, void* __restrict__ out_depth, void* __restrict__ out_normal,
-                  const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
-                  size_t pitch) {
-    raster_body<MODE, AUX, ZTEST, true>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth,
-                                        out_normal, truncated, splat_d, scene, pitch, nullptr);
-}
-
-template <int MODE, bool ZTEST>
-__global__ void __launch_bounds__(RT_THREADS, ZTEST ? 4 : 5)
-raster_mixed_box_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
-                        const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W, int H, int tiles_x,
-                        void* __restrict__ out, uint32_t format, const uint32_t* __restrict__ truncated,
-                        const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
-                        const unsigned char* __restrict__ kinds) {
-    raster_body<MODE, false, ZTEST, true>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr,
-                                          nullptr, truncated, splat_d, scene, pitch, kinds);
-}
-
-// bgs_render_entities_aux's blends of mixed kinds: raster_mixed_kernel's (BOX: raster_mixed_box_kernel's) with the depth
-// and normal frames.  Kernels of their own, so the mixed frames without aux keep the very kernels they had.  (MODE 4, or
-// ZTEST, spills at 5 CTAs per SM.)
-template <int MODE, bool ZTEST, bool BOX>
-__global__ void __launch_bounds__(RT_THREADS, MODE == 4 || ZTEST ? 4 : 5)
-raster_mixed_aux_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
-                        const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W, int H, int tiles_x,
-                        void* __restrict__ out, uint32_t format, const float4* __restrict__ aux, void* __restrict__ out_depth,
-                        void* __restrict__ out_normal, const uint32_t* __restrict__ truncated,
-                        const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
-                        const unsigned char* __restrict__ kinds) {
-    raster_body<MODE, true, ZTEST, BOX>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth,
-                                        out_normal, truncated, splat_d, scene, pitch, kinds);
-}
-
-// bgs_render_views' blends: raster_kernel's (MODE 0..2), raster_mixed_kernel's (3, 4) and their BOX kernels', each CTA on
-// its view's tile (raster_body's VIEWS).  (MODE 0 spills at 6 CTAs per SM; the mixed depth-tested blends, the depth-tested
-// overlay and MODE 4's overlay at 5.)
-template <int MODE, bool ZTEST, bool BOX>
-__global__ void __launch_bounds__(RT_THREADS, (ZTEST && (MODE >= 3 || BOX)) || (BOX && MODE == 4) ? 4 : 5)
-raster_views_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
-                    const uint2* __restrict__ ranges, uint32_t format, const uint32_t* __restrict__ truncated,
-                    const float* __restrict__ splat_d, const unsigned char* __restrict__ kinds, const __grid_constant__ ViewTable vt) {
-    raster_body<MODE, false, ZTEST, BOX, true>(recs, extra, tile_entries, ranges, 0, 0, 0, nullptr, format, nullptr, nullptr,
-                                               nullptr, truncated, splat_d, nullptr, 0, kinds, &vt);
-}
-
-// bgs_render_views_aux's blends: raster_views_kernel's with the depth and normal frames (MODE 3 and 4: raster_mixed_aux's
-// body).  Kernels of their own, so bgs_render_views keeps the very kernels it has.  Launch bounds from the ptxas report:
-// MODE 2 with ZTEST spills at 4 CTAs per SM (3 leave it 85 registers); MODE 4, and MODE 2 and 3 with ZTEST or BOX, at 5.
-template <int MODE, bool ZTEST, bool BOX>
-__global__ void __launch_bounds__(RT_THREADS, MODE == 2 && ZTEST ? 3 : (MODE == 4 || ((ZTEST || BOX) && MODE >= 2) ? 4 : 5))
-raster_views_aux_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
-                        const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, uint32_t format,
-                        const float4* __restrict__ aux, const uint32_t* __restrict__ truncated,
-                        const float* __restrict__ splat_d, const unsigned char* __restrict__ kinds,
-                        const __grid_constant__ ViewTable vt) {
-    raster_body<MODE, true, ZTEST, BOX, true>(recs, extra, tile_entries, ranges, 0, 0, 0, nullptr, format, aux, nullptr,
-                                              nullptr, truncated, splat_d, nullptr, 0, kinds, &vt);
-}
-
-// bgs_render_entities_pick's blends: raster_kernel's (MODE 0..2), raster_mixed_kernel's (3, 4) and their BOX kernels', with
-// the pick frame (raster_body's PICK).  Kernels of their own, so every other frame keeps the very kernels it had.  (At 5
-// CTAs per SM MODE 1 and 2 spill even without the depth test or the overlay: 4 leave every variant 64 registers.)
-template <int MODE, bool ZTEST, bool BOX>
-__global__ void __launch_bounds__(RT_THREADS, 4)
-raster_pick_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extra, const uint32_t* __restrict__ tile_entries,
-                   const uint2* __restrict__ ranges, int W, int H, int tiles_x, void* __restrict__ out, uint32_t format,
-                   const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
-                   size_t pitch, const unsigned char* __restrict__ kinds, const __grid_constant__ PickArgs pk) {
-    raster_body<MODE, false, ZTEST, BOX, false, true>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, nullptr,
-                                                      nullptr, nullptr, truncated, splat_d, scene, pitch, kinds, nullptr, &pk);
+              size_t pitch, const unsigned char* __restrict__ kinds, const __grid_constant__ Tail tail) {
+    constexpr bool VIEWS = IS_VIEWS<Tail>;   // (a views frame's size, targets and depth buffers are its view's)
+    raster_body<MODE, AUX, ZTEST, BOX, VIEWS, IS_PICK<Tail>>(
+        recs, extra, tile_entries, ranges, VIEWS ? 0 : W, VIEWS ? 0 : H, VIEWS ? 0 : tiles_x, VIEWS ? nullptr : out, format,
+        AUX ? aux : nullptr, AUX && !VIEWS ? out_depth : nullptr, AUX && !VIEWS ? out_normal : nullptr, truncated, splat_d,
+        VIEWS ? nullptr : scene, VIEWS ? 0 : pitch, MODE >= 3 ? kinds : nullptr, tail_as<ViewTable>(tail),
+        tail_as<PickArgs>(tail));
 }
 
 // the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
@@ -871,123 +819,48 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
     store_pixel2(out, format, (size_t)py * W + px0, in0, in1, r0, g0, b0, r1, g1, b1, T0, T1);
 }
 
-void launch_raster(int mode, bool large_footprints, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries,
-                   const uint2* ranges, int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format,
-                   const float4* aux, void* out_depth, void* out_normal, const uint32_t* truncated, const ZTestArgs& zt,
-                   cudaStream_t stream, const unsigned char* kinds, bool box) {
-    const int grid = tiles_x * tiles_y;
-    const bool ztest = zt.scene != nullptr;
-    // the kernel tables' rows: plain, AUX, ZTEST, AUX + ZTEST
-    const int row = (ztest ? 2 : 0) + (aux != nullptr ? 1 : 0);
-    if (mode >= 3 && aux != nullptr) {   // bgs_render_entities_aux of mixed kinds
-        static void (*const mixed_aux[2][2][2])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int,
-                                                void*, uint32_t, const float4*, void*, void*, const uint32_t*, const float*,
-                                                const float*, size_t, const unsigned char*) = {
-            {{raster_mixed_aux_kernel<3, false, false>, raster_mixed_aux_kernel<3, false, true>},
-             {raster_mixed_aux_kernel<3, true, false>, raster_mixed_aux_kernel<3, true, true>}},
-            {{raster_mixed_aux_kernel<4, false, false>, raster_mixed_aux_kernel<4, false, true>},
-             {raster_mixed_aux_kernel<4, true, false>, raster_mixed_aux_kernel<4, true, true>}}};
-        mixed_aux[mode - 3][ztest][box]<<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out,
-                                                                         format, aux, out_depth, out_normal, truncated,
-                                                                         zt.splat_d, zt.scene, zt.pitch, kinds);
-        return;
-    }
-    if (box) {   // the bounding-box overlay: raster_body's generic loop for every mode, never raster2_kernel
-        if (mode >= 3) {
-            auto* kernel = mode == 3 ? (ztest ? raster_mixed_box_kernel<3, true> : raster_mixed_box_kernel<3, false>)
-                                     : (ztest ? raster_mixed_box_kernel<4, true> : raster_mixed_box_kernel<4, false>);
-            kernel<<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, truncated,
-                                                    zt.splat_d, zt.scene, zt.pitch, kinds);
-            return;
-        }
-        static void (*const box_kernels[4][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int,
-                                               void*, uint32_t, const float4*, void*, void*, const uint32_t*, const float*,
-                                               const float*, size_t) = {
-            {raster_box_kernel<0, false, false>, raster_box_kernel<1, false, false>, raster_box_kernel<2, false, false>},
-            {raster_box_kernel<0, true, false>, raster_box_kernel<1, true, false>, raster_box_kernel<2, true, false>},
-            {raster_box_kernel<0, false, true>, raster_box_kernel<1, false, true>, raster_box_kernel<2, false, true>},
-            {raster_box_kernel<0, true, true>, raster_box_kernel<1, true, true>, raster_box_kernel<2, true, true>}};
-        box_kernels[row][mode]<<<grid, RT_THREADS, 0, stream>>>(
-            recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated, zt.splat_d,
-            zt.scene, zt.pitch);
-        return;
-    }
-    if (mode >= 3) {
-        auto* kernel = mode == 3 ? (ztest ? raster_mixed_kernel<3, true> : raster_mixed_kernel<3, false>)
-                                 : (ztest ? raster_mixed_kernel<4, true> : raster_mixed_kernel<4, false>);
-        kernel<<<grid, RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, truncated,
-                                                zt.splat_d, zt.scene, zt.pitch, kinds);
-        return;
-    }
-    // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
-    // pixels (more of its lanes then idle at the tile's splat boundaries)
-    if (aux == nullptr && mode == 0 && large_footprints) {
-        (ztest ? raster2_kernel<false, true> : raster2_kernel<false, false>)<<<grid, R2_THREADS, 0, stream>>>(
-            recs, tile_entries, ranges, W, H, tiles_x, out, format, nullptr, nullptr, nullptr, truncated, 1, 1, zt.splat_d,
-            zt.scene, zt.pitch);
-        return;
-    }
-    // aux != nullptr: colour + depth + normal in one pass (bgs_render_aux, bgs_render_entities_aux)
-    static void (*const kernels[4][3])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*,
-                                       uint32_t, const float4*, void*, void*, const uint32_t*, const float*, const float*,
-                                       size_t) = {
-        {raster_kernel<0, false>, raster_kernel<1, false>, raster_kernel<2, false>},
-        {raster_kernel<0, true>, raster_kernel<1, true>, raster_kernel<2, true>},
-        {raster_kernel<0, false, true>, raster_kernel<1, false, true>, raster_kernel<2, false, true>},
-        {raster_kernel<0, true, true>, raster_kernel<1, true, true>, raster_kernel<2, true, true>}};
-    kernels[row][mode == 0 ? 0 : mode == 1 ? 1 : 2]<<<grid, RT_THREADS, 0, stream>>>(
-        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, aux, out_depth, out_normal, truncated, zt.splat_d,
-        zt.scene, zt.pitch);
+// The blend kernels of one Tail, indexed mode + 5 (box + 2 (ztest + 2 aux)) (pick frames have no aux variants)
+template <class Tail, int... I>
+const auto* blend_kernels(std::integer_sequence<int, I...>) {
+    static void (*const table[])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*, uint32_t,
+                                 const float4*, void*, void*, const uint32_t*, const float*, const float*, size_t,
+                                 const unsigned char*, const Tail) = {
+        raster_kernel<I % 5, I >= 20, (I / 10) % 2 != 0, (I / 5) % 2 != 0, Tail>...};
+    return table;
 }
 
-void launch_raster_views(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
-                         uint32_t format, const uint32_t* truncated, const float* splat_d, const unsigned char* kinds, bool box,
-                         const ViewTable& vt, cudaStream_t stream, const float4* aux) {
-    if (aux) {
-        using AuxKernel = void (*)(const SplatRec*, const float4*, const uint32_t*, const uint2*, uint32_t, const float4*,
-                                   const uint32_t*, const float*, const unsigned char*, const ViewTable);
-#define VIEWS_AUX_ROW_(Z, B) {raster_views_aux_kernel<0, Z, B>, raster_views_aux_kernel<1, Z, B>, raster_views_aux_kernel<2, Z, B>, \
-                              raster_views_aux_kernel<3, Z, B>, raster_views_aux_kernel<4, Z, B>}
-        static const AuxKernel kernels[2][2][5] = {{VIEWS_AUX_ROW_(false, false), VIEWS_AUX_ROW_(false, true)},
-                                                   {VIEWS_AUX_ROW_(true, false), VIEWS_AUX_ROW_(true, true)}};
-#undef VIEWS_AUX_ROW_
-        kernels[splat_d != nullptr][box][mode]<<<vt.tile0[vt.v], RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges,
-                                                                                         format, aux, truncated, splat_d, kinds, vt);
-        return;
-    }
-    using Kernel = void (*)(const SplatRec*, const float4*, const uint32_t*, const uint2*, uint32_t, const uint32_t*,
-                            const float*, const unsigned char*, const ViewTable);
-#define VIEWS_ROW_(Z, B) {raster_views_kernel<0, Z, B>, raster_views_kernel<1, Z, B>, raster_views_kernel<2, Z, B>, \
-                          raster_views_kernel<3, Z, B>, raster_views_kernel<4, Z, B>}
-    static const Kernel kernels[2][2][5] = {{VIEWS_ROW_(false, false), VIEWS_ROW_(false, true)},
-                                            {VIEWS_ROW_(true, false), VIEWS_ROW_(true, true)}};
-#undef VIEWS_ROW_
-    kernels[splat_d != nullptr][box][mode]<<<vt.tile0[vt.v], RT_THREADS, 0, stream>>>(recs, extra, tile_entries, ranges, format,
-                                                                                     truncated, splat_d, kinds, vt);
+template <class Tail>
+void launch_blend(const BlendArgs& a, uint32_t grid, const Tail& tail, cudaStream_t stream) {
+    static const auto* const kernels = blend_kernels<Tail>(std::make_integer_sequence<int, IS_PICK<Tail> ? 20 : 40>());
+    const int i = a.mode + 5 * ((a.box ? 1 : 0) + 2 * ((a.scene ? 1 : 0) + 2 * (a.aux ? 1 : 0)));
+    kernels[i]<<<grid, RT_THREADS, 0, stream>>>(
+        a.recs, a.extra, a.tile_entries, a.ranges, a.W, a.H, a.tiles_x, a.out, a.format, a.aux, a.out_depth, a.out_normal,
+        a.truncated, a.splat_d, a.scene, a.pitch, a.kinds, tail);
 }
 
-void launch_raster_pick(int mode, const SplatRec* recs, const float4* extra, const uint32_t* tile_entries, const uint2* ranges,
-                        int W, int H, int tiles_x, int tiles_y, void* out, uint32_t format, const uint32_t* truncated,
-                        const ZTestArgs& zt, const unsigned char* kinds, bool box, const PickArgs& pk, cudaStream_t stream) {
-    using Kernel = void (*)(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*, uint32_t,
-                            const uint32_t*, const float*, const float*, size_t, const unsigned char*, const PickArgs);
-#define PICK_ROW_(Z, B) {raster_pick_kernel<0, Z, B>, raster_pick_kernel<1, Z, B>, raster_pick_kernel<2, Z, B>, \
-                         raster_pick_kernel<3, Z, B>, raster_pick_kernel<4, Z, B>}
-    static const Kernel kernels[2][2][5] = {{PICK_ROW_(false, false), PICK_ROW_(false, true)},
-                                            {PICK_ROW_(true, false), PICK_ROW_(true, true)}};
-#undef PICK_ROW_
-    kernels[zt.scene != nullptr][box][mode]<<<tiles_x * tiles_y, RT_THREADS, 0, stream>>>(
-        recs, extra, tile_entries, ranges, W, H, tiles_x, out, format, truncated, zt.splat_d, zt.scene, zt.pitch, kinds, pk);
+void launch_raster(const BlendArgs& a, cudaStream_t stream) {
+    if (a.views) {
+        launch_blend(a, a.views->tile0[a.views->v], *a.views, stream);
+    } else if (a.pick) {
+        launch_blend(a, (uint32_t)(a.tiles_x * a.tiles_y), *a.pick, stream);
+    } else if (a.mode == 0 && !a.aux && !a.box && a.large_footprints) {
+        // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
+        // pixels (more of its lanes then idle at the tile's splat boundaries)
+        auto* kernel = a.scene ? raster2_kernel<false, true> : raster2_kernel<false, false>;
+        kernel<<<a.tiles_x * a.tiles_y, R2_THREADS, 0, stream>>>(
+            a.recs, a.tile_entries, a.ranges, a.W, a.H, a.tiles_x, a.out, a.format, nullptr, nullptr, nullptr, a.truncated, 1, 1,
+            a.splat_d, a.scene, a.pitch);
+    } else {
+        launch_blend(a, (uint32_t)(a.tiles_x * a.tiles_y), OneView{}, stream);
+    }
 }
 
 // One front-to-back round of a chunked frame (quad-uv records only); see raster2_kernel.
-void launch_raster_round(const SplatRec* recs, const uint32_t* tile_entries, const uint2* ranges, int W, int H, int tiles_x,
-                         int tiles_y, void* out, uint32_t format, float4* state, unsigned char* tile_done,
-                         uint32_t* tiles_done, const uint32_t* truncated, int first, int last, const ZTestArgs& zt,
+void launch_raster_round(const BlendArgs& a, float4* state, unsigned char* tile_done, uint32_t* tiles_done, int first, int last,
                          cudaStream_t stream) {
-    (zt.scene ? raster2_kernel<true, true> : raster2_kernel<true, false>)<<<tiles_x * tiles_y, R2_THREADS, 0, stream>>>(
-        recs, tile_entries, ranges, W, H, tiles_x, out, format, state, tile_done, tiles_done, truncated, first, last,
-        zt.splat_d, zt.scene, zt.pitch);
+    (a.scene ? raster2_kernel<true, true> : raster2_kernel<true, false>)<<<a.tiles_x * a.tiles_y, R2_THREADS, 0, stream>>>(
+        a.recs, a.tile_entries, a.ranges, a.W, a.H, a.tiles_x, a.out, a.format, state, tile_done, tiles_done, a.truncated, first,
+        last, a.splat_d, a.scene, a.pitch);
 }
 
 }  // namespace bgs

@@ -17,11 +17,11 @@ Classes of (splat, pixel) pairs a frame reaches (`pair_classes`):
   K0 / K+ / K-   the deciding quantity is exactly the threshold / one ulp above (not covered) / one ulp below
   KF             the decision differs when u, v are a rounded multiply plus a rounded add instead of the fma
   KS             the pixel is a corner pixel of its warp's 8x4 rectangle, the splat's centre lies outside that
-                 rectangle diagonally and the decision is within 4 ulps: the separating-axis cull of raster_kernel<0>
-                 decides on its slack
+                 rectangle diagonally and the decision is within 4 ulps: the separating-axis cull of MODE 0's
+                 raster_kernel decides on its slack
   KCH0 / KCH1    the pair sits in chunk 0 / chunk >= 1 of a tile with more than 256 entries (the TMA double buffer)
-  KPOS_EVEN / KPOS_ODD / KPOS_TAIL   raster_kernel<0, false>: the splat's position in its warp's candidate list
-                 (first or second of a pair, or the last of an odd-length list)
+  KPOS_EVEN / KPOS_ODD / KPOS_TAIL   raster_kernel<0, false, false, false, OneView>: the splat's position in its warp's
+                 candidate list (first or second of a pair, or the last of an odd-length list)
   KF_EVEN / KF_ODD / KF_TAIL   KF pairs at each of those positions (each has its own copy of the u, v arithmetic)
   KPX0 / KPX1    raster2_kernel: the pixel is its lane's first / second pixel
 
@@ -175,7 +175,7 @@ def knife_case(oracle, geom: str, saturated: bool, n_knife: int = 96, w: int = 3
     front of their knife splat (away from its pixel) so that its pair lands in the tile's second chunk; behind them a
     background of splats (`heavy`: big ones, so that the frame has >= 8 pairs per visible splat).  Unless `heavy`, the
     background keeps out of the warp rectangles of every fourth knife splat with 0 or 2 front dots: there the knife
-    splat ends an odd-length candidate list (raster_kernel<0, false>'s odd tail), and it takes a fused/unfused split
+    splat ends an odd-length candidate list (MODE 0's raster_kernel's odd tail), and it takes a fused/unfused split
     where its scale walk meets one."""
     gm, aabb = GEOMETRIES[geom]
     s = settings_for(geom, saturated)
@@ -319,7 +319,7 @@ def round_of(rank, n_vis):
 
 
 def warp_candidates_r0(rec, tile_slice, chunk, wx0, wy0):
-    """numpy replica of raster_kernel<0>'s per-warp candidate list for one chunk of a tile slice: bbox test, then the
+    """numpy replica of MODE 0's raster_kernel's per-warp candidate list for one chunk of a tile slice: bbox test, then the
     separating-axis test in f32 (same operations and order).  -> (list of ranks, ambiguous): `ambiguous` marks the
     ranks whose SAT value lies within 1e-4 relative of its threshold, where contraction by the compiler may decide."""
     f = np.float32

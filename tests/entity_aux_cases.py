@@ -4,16 +4,16 @@ its covariance cloud (an aux frame refuses it), its first cloud listed a second 
 
 The cases reach every blend instantiation an aux frame can take; with the depth buffer on or off (the tests' other
 parameter) they launch each kernel below once as given and once with ZTEST:
-  quad          raster_kernel<0, true, Z>               every entity quad-uv (3DGS and 2DGS without aabb)
-  quad_box      raster_box_kernel<0, true, Z>           the same, every entity with its overlay
-  conic         raster_kernel<1, true, Z>               every entity 3DGS with aabb
-  conic_box     raster_box_kernel<1, true, Z>
-  surfel        raster_kernel<2, true, Z>               every entity 2DGS with aabb
-  surfel_box    raster_box_kernel<2, true, Z>
-  mixed         raster_mixed_aux_kernel<3, Z, false>    quad-uv and conic entities
-  mixed_box     raster_mixed_aux_kernel<3, Z, true>     the same, two entities with their overlay
-  mixed_surfel      raster_mixed_aux_kernel<4, Z, false>  quad-uv, conic and surfel entities
-  mixed_surfel_box  raster_mixed_aux_kernel<4, Z, true>   the same, the surfel entity with its overlay
+  quad              raster_kernel<0, true, Z, false, OneView>  every entity quad-uv (3DGS and 2DGS without aabb)
+  quad_box          raster_kernel<0, true, Z, true, OneView>   the same, every entity with its overlay
+  conic             raster_kernel<1, true, Z, false, OneView>  every entity 3DGS with aabb
+  conic_box         raster_kernel<1, true, Z, true, OneView>
+  surfel            raster_kernel<2, true, Z, false, OneView>  every entity 2DGS with aabb
+  surfel_box        raster_kernel<2, true, Z, true, OneView>
+  mixed             raster_kernel<3, true, Z, false, OneView>  quad-uv and conic entities
+  mixed_box         raster_kernel<3, true, Z, true, OneView>   the same, two entities with their overlay
+  mixed_surfel      raster_kernel<4, true, Z, false, OneView>  quad-uv, conic and surfel entities
+  mixed_surfel_box  raster_kernel<4, true, Z, true, OneView>   the same, the surfel entity with its overlay
 Colour sources differ per entity (Color, Depth, Normal, Position, Classification, OpticalFlow) and so do draw modes, so
 the rgba frame and its Depth / Normal substitutes all differ."""
 from __future__ import annotations

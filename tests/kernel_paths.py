@@ -184,7 +184,7 @@ def footprint_rect(xlo: int, xhi: int, ylo: int, yhi: int) -> tuple[int, int, in
 
 
 def large_footprint_raster(n_vis_hint: int, n_pairs_hint: int) -> bool:
-    """api.cu plan_frame (large_fp): raster2_kernel<false> instead of raster_kernel<0> (USE_OBB frames only)."""
+    """api.cu plan_frame (large_fp): raster2_kernel<false> instead of MODE 0's raster_kernel (USE_OBB frames only)."""
     return n_vis_hint > 0 and n_pairs_hint >= 8 * n_vis_hint
 
 

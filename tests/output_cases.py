@@ -245,8 +245,9 @@ def same_bytes(a, b, allow_negzero=True):
 
 W, H = 331, 207                    # odd * odd pixels (odd RGBA8 slot offsets), partial edge tiles, >= 65536 pixels
 PATHS = ("r0", "r0aux", "aabb3d", "aabb3d-aux", "aabb2d", "aabb2d-aux", "r2", "rounds")
-KERNEL = {"r0": "raster_kernel<0, false>", "r0aux": "raster_kernel<0, true>", "aabb3d": "raster_kernel<1, false>",
-          "aabb3d-aux": "raster_kernel<1, true>", "aabb2d": "raster_kernel<2, false>", "aabb2d-aux": "raster_kernel<2, true>",
+KERNEL = {"r0": "raster_kernel<0, false, false, false, OneView>", "r0aux": "raster_kernel<0, true, false, false, OneView>",
+          "aabb3d": "raster_kernel<1, false, false, false, OneView>", "aabb3d-aux": "raster_kernel<1, true, false, false, OneView>",
+          "aabb2d": "raster_kernel<2, false, false, false, OneView>", "aabb2d-aux": "raster_kernel<2, true, false, false, OneView>",
           "r2": "raster2_kernel<false>", "rounds": "raster2_kernel<true>"}
 GEOM = {"r0": "obb3d", "r0aux": "obb3d", "aabb3d": "aabb3d", "aabb3d-aux": "aabb3d", "aabb2d": "aabb2d",
         "aabb2d-aux": "aabb2d", "r2": "obb3d", "rounds": "obb3d"}

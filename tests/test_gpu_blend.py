@@ -1,13 +1,13 @@
 """Every blend kernel's coverage decisions bit for bit, and its pixel values against per-pixel error bounds.
 
 Each variant of csrc/raster.cu is reached through the selection rules restated in `kernel_paths`:
-  r0      raster_kernel<0, false>   USE_OBB first frame of a fresh context (no hints: not large_footprint_raster)
-  r0aux   raster_kernel<0, true>    the same frame through render_view_aux
-  r2      raster2_kernel<false>     the hinted second frame of a heavy frame, once large_footprint_raster holds
-  rounds  raster2_kernel<true>      binning_rounds=True, the knife pairs in a round after the first
-  aabb3d  raster_kernel<1, *>       3DGS USE_AABB (colour, and aux)
-  aabb2d  raster_kernel<2, *>       2DGS USE_AABB (colour, and aux)
-  obb2d   raster_kernel<0, false>   2DGS USE_OBB surfel records (uy = vx = 0)
+  r0      raster_kernel<0, false, false, false, OneView>  USE_OBB first frame of a fresh context (no hints: not large_footprint_raster)
+  r0aux   raster_kernel<0, true, false, false, OneView>   the same frame through render_view_aux
+  r2      raster2_kernel<false>                           the hinted second frame of a heavy frame, once large_footprint_raster holds
+  rounds  raster2_kernel<true>                            binning_rounds=True, the knife pairs in a round after the first
+  aabb3d  raster_kernel<1, *, false, false, OneView>      3DGS USE_AABB (colour, and aux)
+  aabb2d  raster_kernel<2, *, false, false, OneView>      2DGS USE_AABB (colour, and aux)
+  obb2d   raster_kernel<0, false, false, false, OneView>  2DGS USE_OBB surfel records (uy = vx = 0)
 and rendered in three output modes: over an opaque clear, premultiplied (C, 1 - T), and blended over a seeded RGBA32F
 target (C + T dst.rgb, (1 - T) + T dst.a).
 
@@ -209,7 +209,7 @@ def run_path(p, h, s, view, variant, out_mode, fmt="rgba32f", dst=None):
         assert fs.rounds > 1
     else:
         assert fs.rounds == 1
-    if variant in ("r0", "obb2d"):   # the next frame (quantised formats) stays on raster_kernel<0> too
+    if variant in ("r0", "obb2d"):   # the next frame (quantised formats) stays on MODE 0's raster_kernel too
         assert not KP.large_footprint_raster(fs.n_visible, fs.n_pairs)
     return img
 

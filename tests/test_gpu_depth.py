@@ -2,7 +2,7 @@
 
 1. bgs_debug_splat_depths is bit-exact against the oracle's d: compact and SORT_ALL frames, 32-, 24- and 16-bit keys,
    the three cloud layouts, 2DGS and 3DGS.
-2. A zero depth buffer gives the bytes of bgs_render_ex on every blend kernel (raster_kernel<0|1|2>, raster2_kernel<false>,
+2. A zero depth buffer gives the bytes of bgs_render_ex on every blend kernel (MODE 0..2's raster_kernel, raster2_kernel<false>,
    chunked raster2_kernel<true>), in each format and output mode, synchronous and queued, with the same sorted entries,
    tile ranges, tile entries and frame stats.
 3. Saturated frames with knife buffers at, one ulp above and one ulp below the deciding splat's d, and occluder buffers

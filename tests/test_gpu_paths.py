@@ -519,17 +519,17 @@ def test_raster_edge_cases_have_their_shape(oracle):
 @gpu
 @pytest.mark.parametrize("k,lead,op", RASTER_CASES)
 def test_raster_chunk_edges_and_variants(oracle, k, lead, op):
-    """The oracle bar on raster_kernel<0>, then byte identity of every other blend of the same frame: binning rounds
+    """The oracle bar on MODE 0's raster_kernel, then byte identity of every other blend of the same frame: binning rounds
     (raster2_kernel<true>), raster2_kernel<false> (picked after a frame of large footprints), and the colour frame of
-    bgs_render_aux (raster_kernel<0, true>), in all three formats and with premultiplied output.  USE_AABB frames
-    (raster_kernel<1>, <2>) are checked against the oracle."""
+    bgs_render_aux (MODE 0's aux raster_kernel), in all three formats and with premultiplied output.  USE_AABB frames
+    (MODE 1 and 2) are checked against the oracle."""
     import dataclasses
 
     cloud, view = raster_edge_cloud(k, lead, RASTER_OPACITY[op])
     s = B.CloudSettings(binning_rounds=False, **RASTER_SETTINGS)
     p = B.GaussianSplattingPlugin(0)
     try:
-        img, til = check_against_oracle(p, oracle, cloud, s, view)      # fresh context: raster_kernel<0>, hinted frame too
+        img, til = check_against_oracle(p, oracle, cloud, s, view)      # fresh context: MODE 0's raster_kernel, hinted frame too
         assert til["tile_ranges"][1, 1] - til["tile_ranges"][1, 0] == k
         h = p.add_cloud(cloud)
         heavy = p.add_cloud(B.random_gaussians_3d_seeded(200, 3))
@@ -539,7 +539,7 @@ def test_raster_chunk_edges_and_variants(oracle, k, lead, op):
                 for premul in (False, True):
                     base = p.render_view(h, s, view, fmt=fmt, premultiplied=premul)
                     fs = p.frame_stats()
-                    assert not KP.large_footprint_raster(fs.n_visible, fs.n_pairs)     # next frame: raster_kernel<0> again
+                    assert not KP.large_footprint_raster(fs.n_visible, fs.n_pairs)     # next frame: MODE 0's raster_kernel again
                     again = p.render_view(h, s, view, fmt=fmt, premultiplied=premul)
                     rounds = p.render_view(h, dataclasses.replace(s, binning_rounds=True), view, fmt=fmt, premultiplied=premul)
                     assert p.frame_stats().rounds == 5

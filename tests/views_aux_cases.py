@@ -4,16 +4,16 @@ cloud whose views cover the Depth range's edge cases.
 
 Each mix reaches one blend kernel of bgs_render_views_aux; with the per-view depth buffers on or off (the tests' other
 parameter) it launches it once as given and once with ZTEST:
-  quad              raster_views_aux_kernel<0, Z, false>   every entity quad-uv; a Depth entity
-  quad_box          raster_views_aux_kernel<0, Z, true>    the same, every entity with its overlay
-  conic             raster_views_aux_kernel<1, Z, false>   every entity 3DGS with aabb; a Depth entity
-  conic_box         raster_views_aux_kernel<1, Z, true>
-  surfel            raster_views_aux_kernel<2, Z, false>   every entity 2DGS with aabb
-  surfel_box        raster_views_aux_kernel<2, Z, true>
-  mixed             raster_views_aux_kernel<3, Z, false>   quad-uv and conic entities; a Depth entity
-  mixed_box         raster_views_aux_kernel<3, Z, true>    the same, two entities with their overlay
-  mixed_surfel      raster_views_aux_kernel<4, Z, false>   quad-uv, conic and surfel entities; a Depth entity
-  mixed_surfel_box  raster_views_aux_kernel<4, Z, true>    the same, the surfel entity with its overlay
+  quad              raster_kernel<0, true, Z, false, ViewTable>  every entity quad-uv; a Depth entity
+  quad_box          raster_kernel<0, true, Z, true, ViewTable>   the same, every entity with its overlay
+  conic             raster_kernel<1, true, Z, false, ViewTable>  every entity 3DGS with aabb; a Depth entity
+  conic_box         raster_kernel<1, true, Z, true, ViewTable>
+  surfel            raster_kernel<2, true, Z, false, ViewTable>  every entity 2DGS with aabb
+  surfel_box        raster_kernel<2, true, Z, true, ViewTable>
+  mixed             raster_kernel<3, true, Z, false, ViewTable>  quad-uv and conic entities; a Depth entity
+  mixed_box         raster_kernel<3, true, Z, true, ViewTable>   the same, two entities with their overlay
+  mixed_surfel      raster_kernel<4, true, Z, false, ViewTable>  quad-uv, conic and surfel entities; a Depth entity
+  mixed_surfel_box  raster_kernel<4, true, Z, true, ViewTable>   the same, the surfel entity with its overlay
 Every mix's depth frames are over each view's own range, whether or not an entity is in Depth mode."""
 from __future__ import annotations
 

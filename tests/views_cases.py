@@ -1,13 +1,13 @@
 """Inputs of bgs_render_views' tests (tests/test_gpu_views.py): view sets (a stereo pair, three views of different sizes
 that the 16-pixel tile does not divide, six cube faces) around scene4d_cases' room, and entity mixes from entity_cases'
 room and performer that reach each blend kernel a views frame launches:
-  quad        raster_views_kernel<0, Z, false>   quad-uv entities: HighlightSelected, Classification, Position, 4D
-  quad_box    raster_views_kernel<0, Z, true>    the same, every entity's overlay (the frame-wide flag)
-  conic       raster_views_kernel<1, Z, false>   every entity 3DGS or 4D with aabb
-  surfel      raster_views_kernel<2, Z, false>   every entity 2DGS with aabb (the room's f32 / f16 clouds)
-  mixed       raster_views_kernel<4, Z, false>   entity_cases' "kinds": quad-uv, conic, surfel and 4D entities
-  mixed_box   raster_views_kernel<4, Z, true>    the same, some entities with their overlay
-  mixed_conic raster_views_kernel<3, Z, false>   quad-uv and conic entities, Classification among them
+  quad         raster_kernel<0, false, Z, false, ViewTable>  quad-uv entities: HighlightSelected, Classification, Position, 4D
+  quad_box     raster_kernel<0, false, Z, true, ViewTable>   the same, every entity's overlay (the frame-wide flag)
+  conic        raster_kernel<1, false, Z, false, ViewTable>  every entity 3DGS or 4D with aabb
+  surfel       raster_kernel<2, false, Z, false, ViewTable>  every entity 2DGS with aabb (the room's f32 / f16 clouds)
+  mixed        raster_kernel<4, false, Z, false, ViewTable>  entity_cases' "kinds": quad-uv, conic, surfel and 4D entities
+  mixed_box    raster_kernel<4, false, Z, true, ViewTable>   the same, some entities with their overlay
+  mixed_conic  raster_kernel<3, false, Z, false, ViewTable>  quad-uv and conic entities, Classification among them
 (Z: with a depth buffer per view, or without.)  No entity is in Depth or OpticalFlow mode, which a views frame refuses."""
 from __future__ import annotations
 
