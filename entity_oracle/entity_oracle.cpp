@@ -40,13 +40,13 @@ int eo_frame(uint32_t k, const s4o_cloud* cl, const orc_view* view, const orc_se
              float* records, uint32_t* rank_to_id, float* depths, uint32_t* tile_ranges, uint32_t* tile_entries, uint64_t cap,
              float* image, int threads) {
     return eo_frame_ex(k, cl, view, es, nc, nullptr, ex, scene, pitch_bytes, n_vis, n_pairs, sorted, records, rank_to_id,
-                       depths, tile_ranges, tile_entries, cap, image, nullptr, threads);
+                       depths, tile_ranges, tile_entries, cap, image, nullptr, nullptr, threads);
 }
 
 int eo_frame_ex(uint32_t k, const s4o_cloud* cl, const orc_view* view, const orc_settings* es, const uint32_t* nc,
                 const uint32_t* entity_flags, const tor_temporal* ex, const float* scene, uint64_t pitch_bytes, uint32_t* n_vis,
                 uint64_t* n_pairs, uint32_t* sorted, float* records, uint32_t* rank_to_id, float* depths, uint32_t* tile_ranges,
-                uint32_t* tile_entries, uint64_t cap, float* image, uint8_t* edge_mask, int threads) {
+                uint32_t* tile_entries, uint64_t cap, float* image, uint8_t* edge_mask, float* surfel_extra, int threads) {
     if (k == 0 || !cl || !view || !es || !nc || !ex) return 2;
 #ifdef _OPENMP
     if (threads > 0) omp_set_num_threads(threads);
@@ -146,6 +146,16 @@ int eo_frame_ex(uint32_t k, const s4o_cloud* cl, const orc_view* view, const orc
         if (records) to_record(F.splats[r], st[seg_of[r]].aabb != 0u, records + 12 * (size_t)r);
         if (rank_to_id) rank_to_id[r] = F.rank_to_id[r];
         if (depths) depths[r] = dz[r];
+        if (surfel_extra) {   // the surfel's four staged float4s (raster.cu's e0..e3), zeros for the other kinds
+            float* e = surfel_extra + 16 * (size_t)r;
+            std::fill(e, e + 16, 0.0f);
+            if (sb[seg_of[r]].aabb && sb[seg_of[r]].gaussian_mode == 0u) {
+                const float* x = F.splats[r].extra;
+                for (int c = 0; c < 4; ++c) e[c] = x[3 + c];   // Rq, mean x, mean y, W / H
+                for (int q = 0; q < 3; ++q)
+                    for (int c = 0; c < 3; ++c) e[4 * (q + 1) + c] = x[7 + 3 * q + c];   // T0, T1, T2
+            }
+        }
     }
     const int W = ctx[0].Wi, H = ctx[0].Hi;
     const int TX = (W + TILE - 1) / TILE, TY = (H + TILE - 1) / TILE, NT = TX * TY;

@@ -29,11 +29,13 @@ int eo_frame(uint32_t k, const s4o_cloud* clouds, const orc_view* view, const or
 /* eo_frame with each entity's flags (bgs_render_entities_ex): entity_flags[j] bit 0 (BGS_ENTITY_VISUALIZE_BOUNDING_BOX)
  * draws entity j's bounding boxes (include/bgs.h's BGS_FLAG_VISUALIZE_BOUNDING_BOX rule: a covered, depth-passing pair on
  * its quad's edge band blends (0.3, 1, 0.1) at alpha 1 and stops the pixel); entity_flags == NULL is eo_frame.  edge_mask
- * (W*H bytes, optional): 1 where an edge pair blended. */
+ * (W*H bytes, optional): 1 where an edge pair blended.  surfel_extra (16 floats per rank, optional): a 2DGS aabb rank's
+ * surfel extras as the blend kernels stage them, e0 = (Rq, mean x, mean y, W / H), e1, e2, e3 = (T0, 0), (T1, 0),
+ * (T2, 0) (gaussian_2d.wgsl's homography rows); zeros for the other ranks. */
 int eo_frame_ex(uint32_t k, const s4o_cloud* clouds, const orc_view* view, const orc_settings* settings, const uint32_t* num_classes,
                 const uint32_t* entity_flags, const tor_temporal* ex, const float* scene, uint64_t pitch_bytes, uint32_t* n_vis,
                 uint64_t* n_pairs, uint32_t* sorted, float* records, uint32_t* rank_to_id, float* depths, uint32_t* tile_ranges,
-                uint32_t* tile_entries, uint64_t cap, float* image, uint8_t* edge_mask, int threads);
+                uint32_t* tile_entries, uint64_t cap, float* image, uint8_t* edge_mask, float* surfel_extra, int threads);
 
 /* The overlay's edge decision per pair: splat record splats[j] (orc_splat, the oracle's own) at the pixel centre
  * (pixel_xy[2j], pixel_xy[2j+1]) under settings s (aabb, gaussian_mode as the blend reads them: 1 = conic, 0 = surfel).

@@ -43,7 +43,8 @@ def frame(clouds, view, settings, num_classes=None, extras=None, scene=None, wan
           entity_flags=None) -> dict:
     """-> s4o_frame's dict (sorted, records, rank_to_id, depths, tile_ranges, tile_entries, n_vis, n_pairs, image).
     `entity_flags` (one word per cloud, bit 0 = the bounding-box overlay; None = none): eo_frame_ex, whose dict adds
-    edge_mask (H x W bool, where an edge pair blended)."""
+    edge_mask (H x W bool, where an edge pair blended) and surfel_extra ((n_vis, 16) float32: each 2DGS aabb rank's surfel
+    extras e0..e3 as the blend kernels stage them, zeros for the other ranks)."""
     arr, keep = S4O._clouds(clouds)
     k = len(clouds)
     sa = (O.orc_settings * k)(*[O._conv(s, O.orc_settings) for s in settings])
@@ -80,16 +81,17 @@ def _frame_ex(k, arr, v, sa, nc, ef, ex, scene, pitch, n, W, H, nt, want_image, 
     nv, npairs = C.c_uint32(), C.c_uint64()
     head = [C.c_uint32(k), arr, C.byref(v), sa, _p(nc), _p(ef), C.byref(ex), _p(scene), C.c_uint64(pitch), C.byref(nv),
             C.byref(npairs)]
-    rc = load().eo_frame_ex(*head, *([None] * 6), C.c_uint64(0), None, None, C.c_int(threads))
+    rc = load().eo_frame_ex(*head, *([None] * 6), C.c_uint64(0), None, None, None, C.c_int(threads))
     assert rc == 0, rc
     out = dict(sorted=np.empty((n, 2), np.uint32), records=np.empty((nv.value, 12), np.float32),
                rank_to_id=np.empty(nv.value, np.uint32), depths=np.empty(nv.value, np.float32),
                tile_ranges=np.empty((nt, 2), np.uint32), tile_entries=np.empty(npairs.value, np.uint32),
                image=np.empty((H, W, 4), np.float32) if want_image else None,
-               edge_mask=np.empty((H, W), np.uint8) if want_image else None)
+               edge_mask=np.empty((H, W), np.uint8) if want_image else None,
+               surfel_extra=np.empty((nv.value, 16), np.float32))
     assert load().eo_frame_ex(*head, _p(out["sorted"]), _p(out["records"]), _p(out["rank_to_id"]), _p(out["depths"]),
                               _p(out["tile_ranges"]), _p(out["tile_entries"]), C.c_uint64(npairs.value), _p(out["image"]),
-                              _p(out["edge_mask"]), C.c_int(threads)) == 0
+                              _p(out["edge_mask"]), _p(out["surfel_extra"]), C.c_int(threads)) == 0
     out["n_vis"], out["n_pairs"] = nv.value, npairs.value
     if want_image:
         out["edge_mask"] = out["edge_mask"].astype(bool)

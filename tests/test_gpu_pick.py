@@ -1,8 +1,8 @@
 """bgs_render_entities_pick and bgs_cloud_select_in_view on the H100.  The pick call's colour frame is bgs_render_entities_ex's
 byte for byte in every format and output mode, with and without a depth buffer and the overlays, on mixed-kind scenes with
 a 4D performer, and its hooks are the one-round frame's; its pick frame matches pick_oracle's pairs under blend_cases'
-bounds, with depths bit for bit the splat depths; the view selection is the set the entity oracle's records give; and
-the refusals change nothing."""
+bounds (quad-uv, conic and surfel pairs), with depths bit for bit the splat depths; the view selection is the set the
+entity oracle's records give; and the refusals change nothing."""
 import ctypes as C
 import dataclasses
 
@@ -25,87 +25,28 @@ pytestmark = pytest.mark.gpu
 
 W, H = 200, 120   # (not tile multiples)
 VIEW = B.headless_view(W, H)
-FORMATS = {"f32": (np.float32, torch.float32, abi.BGS_FORMAT_RGBA32F), "f16": (np.float16, torch.float16, abi.BGS_FORMAT_RGBA16F),
-           "u8": (np.uint8, torch.uint8, abi.BGS_FORMAT_RGBA8_SRGB)}
-
-
-def _ok(p, rc):
-    assert rc == abi.BGS_OK, p._lib.bgs_last_error(p._ctx)
+FORMATS = PK.FORMATS
+_ok, _addr, _bytes, _hooks = PK.ok, PK.addr, PK.as_bytes, PK.hooks
 
 
 def _depth(seed):
     return torch.rand((H, W), generator=torch.Generator(device="cuda").manual_seed(seed), device="cuda") * 0.04
 
 
-class Scene:
-    def __init__(self, p, listed, flags):
-        self.p, self.flags = p, flags
-        up = {}
-        self.handles, self.unis, self.sts, self.counts, self.oracle = [], [], [], [], []
-        for cloud, layout, tr, st in listed:
-            if id(cloud) not in up:
-                up[id(cloud)] = p.add_cloud(cloud, f16=layout in ("f16", "cov"), precompute_covariance=layout == "cov")
-            h = up[id(cloud)]
-            self.handles.append(h)
-            self.unis.append(p.cloud_uniform(st, tr, h.aabb))
-            self.sts.append(st)
-            self.counts.append(len(cloud.position_visibility))
-            self.oracle.append(E.oracle_entry(cloud, layout, self.unis[-1], st))
-
-    def call(self, name, out, fmt, frame_flags=0, depth=None, device=False, pick=None):
-        k = len(self.handles)
-        s = self.sts[0].to_abi()
-        s.flags = (s.flags & ~abi.BGS_FLAG_VISUALIZE_BOUNDING_BOX) | frame_flags
-        zd = None if depth is None else abi.bgs_scene_depth(depth=depth.data_ptr(), pitch_bytes=4 * W)
-        args = [self.p._ctx, (C.c_void_p * k)(*[h._h.value for h in self.handles]), (abi.bgs_cloud_uniform * k)(*self.unis),
-                (abi.bgs_entity_settings * k)(*[entity_settings(st) for st in self.sts]), (C.c_uint32 * k)(*self.flags), k,
-                C.byref(VIEW.to_abi()), C.byref(s), None, None if zd is None else C.byref(zd), _addr(out), FORMATS[fmt][2],
-                int(device)]
-        if name == "pick":
-            args.append(_addr(pick))
-        return getattr(self.p._lib, "bgs_render_entities_" + name)(*args)
-
-
-def _addr(t):
-    if t is None:
-        return None
-    return t.data_ptr() if isinstance(t, torch.Tensor) else t.ctypes.data
+def Scene(p, listed, flags):
+    return PK.Scene(p, listed, flags, VIEW)
 
 
 def _target(fmt, device, fill=None):
-    npd, tod, _ = FORMATS[fmt]
-    if device:
-        t = torch.zeros((H, W, 4), dtype=tod, device="cuda")
-        if fill is not None:
-            t.copy_(torch.from_numpy(fill))
-        return t
-    return np.zeros((H, W, 4), npd) if fill is None else fill.copy()
+    return PK.target(VIEW, fmt, device, fill)
 
 
 def _pick_target(device):
-    if device:
-        return torch.full((H, W, 4), 0x7F7F7F7F, dtype=torch.int32, device="cuda")
-    return np.full((H, W), 0x7F, np.uint8).repeat(16, axis=1).view(abi.PICK_DTYPE).reshape(H, W)
+    return PK.pick_target(VIEW, device)
 
 
 def _pick_host(t):
-    if isinstance(t, torch.Tensor):
-        torch.cuda.synchronize()
-        return t.cpu().numpy().view(np.uint8).reshape(H, W, 16).view(abi.PICK_DTYPE).reshape(H, W)
-    return t
-
-
-def _bytes(t):
-    if isinstance(t, torch.Tensor):
-        torch.cuda.synchronize()
-        return t.cpu().numpy().tobytes()
-    return t.tobytes()
-
-
-def _hooks(p):
-    rec, ids = p.projected()
-    return dict(stats=bytes(p.frame_stats()), sorted=p.sorted_entries().tobytes(), records=rec.tobytes(), ids=ids.tobytes(),
-                ranges=p.tile_ranges().tobytes(), entries=p.tile_entries().tobytes())
+    return PK.pick_host(t, VIEW)
 
 
 OVERLAYS = {"none": (0, None), "frame": (abi.BGS_FLAG_VISUALIZE_BOUNDING_BOX, None), "entity": (0, (1, 0, 0, 1, 0, 1))}
@@ -197,6 +138,61 @@ def test_pick_matches_the_pick_oracle(with_depth, overlay, saturated):
             zs = depth.cpu().numpy()
             assert (pick["depth"][some] >= zs[some]).all()
         if overlay == "entity":   # edge pixels of an entity with its overlay: w = T
+            assert want["edge_mask"].any()
+    finally:
+        p.destroy()
+
+
+def _surfel_scene(name):
+    """2DGS aabb surfels alone, beside quad-uv and conic entities, and entity_cases' surfel_4d case."""
+    if name == "surfel_4d":
+        return E.entities("surfel_4d")
+    room = S4.room()
+    surf = dict(gaussian_mode=B.GaussianMode.Gaussian2d, aabb=True)
+    (c0, l0, _, tr0, kw0), (c1, l1, _, tr1, kw1), (c2, l2, _, tr2, kw2), (c3, l3, _, tr3, kw3) = room
+    if name == "surfels":
+        return [(c0, l0, tr0, B.CloudSettings(**kw0, **surf)), (c1, l1, tr1, B.CloudSettings(**kw1, **surf)),
+                (c3, l3, tr3, B.CloudSettings(**kw3, **surf)),
+                (c0, l0, SC.transform((0.5, 0.2, -0.6), 0.9, 0.4), B.CloudSettings(global_opacity=0.7, **surf))]
+    return [(c0, l0, tr0, B.CloudSettings(**kw0, **surf)), (c1, l1, tr1, B.CloudSettings(**kw1)),
+            (c2, l2, tr2, B.CloudSettings(**kw2, aabb=True)), (c3, l3, tr3, B.CloudSettings(**kw3, **surf))]
+
+
+@pytest.mark.parametrize("with_depth", [False, True])
+@pytest.mark.parametrize("overlay", ["none", "entity"])
+@pytest.mark.parametrize("scene", ["surfels", "surfel_quad_conic", "surfel_4d"])
+def test_pick_matches_the_pick_oracle_on_surfels(scene, with_depth, overlay):
+    """Surfel pairs held to pick_oracle's restatement of the surfel branch (surfel alphas come from __expf, as conic
+    ones do: alpha_error_coefs(True)), beside quad-uv and conic ones and in the surfel_4d entity case."""
+    listed = _surfel_scene(scene)
+    flags = [(j + 1) % 2 if overlay == "entity" else 0 for j in range(len(listed))]
+    depth = _depth(13) if with_depth else None
+    zs = None if depth is None else depth.cpu().numpy()
+    p = B.GaussianSplattingPlugin(0)
+    try:
+        sc = Scene(p, listed, flags)
+        out, pick = _target("f32", False), _pick_target(False)
+        _ok(p, sc.call("pick", out, "f32", 0, depth, False, pick))
+        want = EO.frame(sc.oracle, VIEW.to_abi(), [st.to_abi() for st in sc.sts], [1] * len(sc.sts), scene=zs,
+                        entity_flags=flags)
+        _, ids = p.projected()
+        assert np.array_equal(ids, want["rank_to_id"])
+        kinds = PK.rank_kinds(want["rank_to_id"], sc.counts, sc.sts, flags)
+        assert ((kinds & 3) == 2).sum() > 1000
+        pairs = PO.pairs(want, kinds, W, H, BC.alpha_error_coefs(True), scene=zs)
+        if scene != "surfels":   # quad-uv pairs: the larger of the two bounds
+            pairs_obb = PO.pairs(want, kinds, W, H, BC.alpha_error_coefs(False), scene=zs)
+            pairs["bound"] = np.maximum(pairs["bound"], pairs_obb["bound"])
+        rank = PK.to_rank(pick, ids, sc.counts)
+        picked, strict = PK.check_pick(pick, rank, pairs)
+        assert picked > 0.1 * W * H and strict > 0.3 * picked, (picked, strict)
+        # surfels are picked, and strictly decided somewhere
+        some = rank >= 0
+        assert ((kinds[rank[some]] & 3) == 2).sum() > 0.05 * W * H
+        assert np.array_equal(pick["depth"][some].view(np.uint32), want["depths"][rank[some]].view(np.uint32))
+        if with_depth:
+            assert (pick["depth"][some] >= zs[some]).all()
+        if overlay == "entity":
             assert want["edge_mask"].any()
     finally:
         p.destroy()

@@ -138,6 +138,6 @@ def test_pick_oracle_picks_the_hand_computed_pair():
     pr = PO.pairs(_frame(many), np.zeros(6, np.uint8), 16, 16, BC.alpha_error_coefs(False))
     pix = 8 * 16 + 8
     assert int(pr["offsets"][pix + 1] - pr["offsets"][pix]) == 4
-    # surfels are not restated
+    # a surfel rank needs the frame's surfel extras
     with pytest.raises(ValueError):
         PO.pairs(_frame(recs), np.array([0, 0, 2], np.uint8), 16, 16, BC.alpha_error_coefs(False))
