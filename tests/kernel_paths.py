@@ -269,6 +269,59 @@ def keygen_cta_tiles(n: int, grid: int) -> list[tuple[int, int]]:
     return [(b * tiles // grid, (b + 1) * tiles // grid) for b in range(grid)]
 
 
+BIN_VIEWS_CTAS_PER_SM_FIT = 3    # bin.cu:328-331: bin_emit_views_kernel's own occupancy (80 registers x 256 threads)
+DRV_THREADS, DRV_CTAS_PER_SM = 256, 4   # project.cu:1055: depth_range_views_kernel's CTA size and its cap per SM
+
+
+def views_tiles(sizes) -> list[int]:
+    """api.cu:945-950 (render_entities_impl, vt.tile0): each view's tile0, then the total (tile0[v]); `sizes` are the
+    views' (width, height)."""
+    out = [0]
+    for w, h in sizes:
+        out.append(out[-1] + num_tiles(w, h))
+    return out
+
+
+def views_bin_grid(sm_count: int, queued: bool, views_per_sm: int = BIN_VIEWS_CTAS_PER_SM_FIT) -> int:
+    """bin.cu:327-333 (launch_bin_emit_views): the binning grid planned for bin_emit_coop_kernel, capped by the views
+    kernel's own co-resident CTAs."""
+    return min(bin_grid(sm_count, queued), views_per_sm * sm_count)
+
+
+def depth_range_views_grid(n_hint: int, sm_count: int = H100_SMS) -> int:
+    """project.cu:1198-1202 (launch_depth_range_views) through entry_src.cuh:114-119 (persistent_grid): ceil(n_hint / 256)
+    CTAs, at most 4 per SM, at least 1."""
+    return max(1, min(-(-n_hint // DRV_THREADS), DRV_CTAS_PER_SM * sm_count))
+
+
+def depth_range_views_passes(n_vis: int, grid: int) -> int:
+    """project.cu:1106 (depth_range_views_kernel's pass): grid-stride passes of CTA 0 (the most any CTA takes)."""
+    return -(-n_vis // (grid * DRV_THREADS))
+
+
+def depth_range_views_cta(p: int, grid: int) -> int:
+    """project.cu:1106: the CTA whose pass reads sorted position p."""
+    return (p // DRV_THREADS) % grid
+
+
+def warp_first_miss_rounds(length: int, first: int) -> int:
+    """project.cu:1076-1091 (warp_first_miss): the rounds of the 32-way search over [0, length) whose first miss is at
+    `first` (length when there is none)."""
+    lo, hi, rounds = 0, length, 0
+    while lo < hi:
+        rounds += 1
+        step = (hi - lo + 31) // 32
+        f = next((lane for lane in range(32) if lo + lane * step >= hi or lo + lane * step >= first), None)
+        if f is None:
+            lo += 31 * step + 1
+        else:
+            hi = min(hi, lo + f * step)
+            if f > 0:
+                lo += (f - 1) * step + 1
+    assert lo == first
+    return rounds
+
+
 def device_sm_count(device: int = 0) -> int:
     import torch
 

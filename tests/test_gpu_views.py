@@ -13,6 +13,7 @@ import torch
 import bevy_gaussian_splatting_b200 as B
 import entity_cases as E
 import views_cases as V
+import views_scale_cases as VS
 from bevy_gaussian_splatting_b200 import abi
 from bevy_gaussian_splatting_b200.plugin import entity_settings
 from entity_oracle import entity_oracle as EO
@@ -161,36 +162,11 @@ def test_hooks_restricted_to_a_view_are_its_own(mix, views):
         sc = Scene(p, mix)
         _ok(p, sc.views(vs, [_target(v, "f32", False) for v in vs], "f32", 0, depths))
         got = _hooks(p, True)
-        n = got["stats"].n // len(vs)
-        assert got["stats"].n == n * len(vs) and got["stats"].rounds == 1 and got["stats"].tiles_y == 1
-        assert (got["stats"].width, got["stats"].height) == (vs[0].width, vs[0].height)
-        tile0 = 0
-        n_vis = n_pairs = 0
+        wants = []
         for i, v in enumerate(vs):
             _ok(p, sc.ex(v, _target(v, "f32", False), "f32", abi.BGS_FLAG_NO_CHUNKS, depths[i]))
-            want = _hooks(p, True)
-            n_vis += want["stats"].n_visible
-            n_pairs += want["stats"].n_pairs
-            srt = got["sorted"]
-            mine = (srt[:, 1] >= i * n) & (srt[:, 1] < (i + 1) * n)
-            sub = srt[mine].copy()
-            sub[:, 1] -= i * n
-            assert np.array_equal(sub, want["sorted"]), ("sorted", i)
-            rmine = (got["ids"] >= i * n) & (got["ids"] < (i + 1) * n)
-            assert got["records"][rmine].tobytes() == want["records"].tobytes(), ("records", i)
-            assert np.array_equal(got["ids"][rmine] - i * n, want["ids"]), ("ids", i)
-            assert got["splat_depths"][rmine].tobytes() == want["splat_depths"].tobytes(), ("splat depths", i)
-            tiles = ((v.width + 15) // 16) * ((v.height + 15) // 16)
-            block = got["ranges"][tile0:tile0 + tiles].astype(np.int64)
-            wr = want["ranges"].astype(np.int64)
-            assert np.array_equal(block[:, 1] - block[:, 0], wr[:, 1] - wr[:, 0]), ("ranges", i)
-            for t in range(tiles):
-                g = got["ids"][got["entries"][block[t, 0]:block[t, 1]]] - i * n
-                w = want["ids"][want["entries"][wr[t, 0]:wr[t, 1]]]
-                assert np.array_equal(g, w), ("tile entries", i, t)
-            tile0 += tiles
-        assert tile0 == got["stats"].tiles_x
-        assert (got["stats"].n_visible, got["stats"].n_pairs) == (n_vis, n_pairs)
+            wants.append(_hooks(p, True))
+        VS.check_restricted(got, wants, vs)
     finally:
         p.destroy()
 
