@@ -27,6 +27,7 @@ BGS_FLAG_BLEND_OVER_TARGET = 32
 BGS_FLAG_VISUALIZE_BOUNDING_BOX = 64
 BGS_ENTITY_VISUALIZE_BOUNDING_BOX = 1
 BGS_SCENE_MAX_CLOUDS = 64
+BGS_ENTITIES_MANY_MAX = 65536
 BGS_SELECT_REPLACE, BGS_SELECT_ADD = 0, 1
 BGS_TRANSFORM_ALL, BGS_TRANSFORM_SELECTED = 0, 1
 BGS_PICK_NONE = 0xFFFFFFFF
@@ -224,6 +225,13 @@ SYMBOLS = [
                                            C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
                                            C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int,
                                            _P]),
+    ("bgs_render_entities_many", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P,
+                                           C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
+                                           C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
+    ("bgs_render_entities_pick_many", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P,
+                                                C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
+                                                C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32,
+                                                C.c_int, _P]),
     ("bgs_render_views", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P, C.c_uint32,
                                    C.POINTER(bgs_view), C.c_uint32, C.POINTER(bgs_settings), C.POINTER(bgs_scene_depth), _P,
                                    C.c_uint32, C.c_int]),

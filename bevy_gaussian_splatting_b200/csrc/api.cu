@@ -352,7 +352,8 @@ bgs_status bgs_context_create(int cuda_device, bgs_context** out) {
         c->bin_grid_async = (uint32_t)(c->sm_count * std::min(bb, COOP_CTAS_PER_SM_ASYNC));
         c->rs_per_sm = radix_coop_blocks_per_sm(16);
         c->kg_scene_per_sm = (uint32_t)keygen_scene_blocks_per_sm();
-        if (c->kg_grid == 0 || c->bin_grid == 0 || c->rs_per_sm == 0 || c->kg_scene_per_sm == 0) coop = 0;
+        c->kg_many_per_sm = (uint32_t)keygen_many_blocks_per_sm();
+        if (c->kg_grid == 0 || c->bin_grid == 0 || c->rs_per_sm == 0 || c->kg_scene_per_sm == 0 || c->kg_many_per_sm == 0) coop = 0;
     }
     if (e == cudaSuccess && !coop) {
         snprintf(c->err, sizeof(c->err), "device %d cannot co-schedule the cooperative kernels (an sm_90a GPU such as the H100 is required)", cuda_device);
@@ -387,6 +388,8 @@ void bgs_context_destroy(bgs_context* c) {
     if (c->h_sticky) cudaFreeHost(c->h_sticky);
     if (c->h_word) cudaFreeHost(c->h_word);
     if (c->h_bounce) cudaFreeHost(c->h_bounce);
+    for (auto& m : c->many)
+        if (m.host) cudaFreeHost(m.host);
     cudaFree(c->d_sticky);
     cudaFree(c->cutoff_tab);
     delete c;   // (releases every DevBuf)
@@ -464,10 +467,13 @@ bgs_status bgs_sync(bgs_context* c) {
 
 static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                                const bgs_settings* st, const bgs_render_extras* ex, uint32_t out_format, bool want_aux,
-                               bool temporal) {
+                               bool temporal, bool set_device = true) {
     // not-ready inputs map to the reference's silent skip-frame (radix.rs:645-658, mod.rs:1533-1539)
     if (!cloud || !view || !uni || !st) return fail(c, BGS_NOT_READY, "render: cloud/view/uniform/settings not ready");
-    TRY(enter_call(c, "render", cloud->device));   // (contexts of one GPU may share clouds)
+    // (contexts of one GPU may share clouds; a scene's entities after its first only check the device, which the first
+    // made current)
+    if (set_device) TRY(enter_call(c, "render", cloud->device));
+    else if (cloud->device != c->device) return fail(c, BGS_EINVAL, "render: cloud lives on another device");
     if (out_format > BGS_FORMAT_RGBA32F) return fail(c, BGS_EINVAL, "render: unknown out_format %u", out_format);
     if (st->radix_sort_depth_bits != 16 && st->radix_sort_depth_bits != 24 && st->radix_sort_depth_bits != 32)
         return fail(c, BGS_EINVAL, "render: radix_sort_depth_bits must be 16, 24 or 32");
@@ -517,12 +523,13 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     cudaStream_t q = c->stream;
     uint32_t launches = 0;
     if (scene) {
-        const std::vector<const bgs_cloud*>& cl = scene->clouds;
-        for (size_t j = 0; j < cl.size(); ++j)
-            if (std::find(cl.begin(), cl.begin() + j, cl[j]) == cl.begin() + j) TRY(before_cloud_read(c, cl[j]));
+        for (const bgs_cloud* cl : scene->distinct) TRY(before_cloud_read(c, cl));
     } else {
         TRY(before_cloud_read(c, cloud));
     }
+    const bool many = scene && scene->many;   // (bgs_render_entities_many: the segment table in device memory)
+    const SceneTableDev* dt = many ? &scene->dtab : nullptr;
+    if (many) CU(c, cudaMemcpyAsync(c->many[scene->slot].dev.p, scene->h_tab, scene->tab_bytes, cudaMemcpyHostToDevice, q));
     CU(c, cudaMemsetAsync(c->arena.p, 0, c->arena.bytes, q));   // counters, histograms, ranges: ~0.4 MB
     CU(c, cudaEventRecord(c->ev[0], q));
     // ---- stage 1: key-gen (+ stable compaction of the visible set)
@@ -531,15 +538,22 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     if (scene) {   // (scenes are compact frames)
         // key-gen gathers the culled ends for the Depth range when segment 0 is in Depth mode: when only some other
         // entity is, it reads a copy of the table whose segment 0 is
-        SceneTable kt;
         const bool depth0 = p.depth_range && scene->tab.seg[0].fc.rasterize_mode != BGS_RASTERIZE_DEPTH;
-        if (depth0) {
-            kt = scene->tab;
-            kt.seg[0].fc.rasterize_mode = BGS_RASTERIZE_DEPTH;
+        if (many) {   // (the frame-wide values are an argument of their own)
+            FrameConsts f0 = scene->tab.seg[0].fc;
+            if (depth0) f0.rasterize_mode = BGS_RASTERIZE_DEPTH;
+            CU(c, launch_keygen_many(*dt, f0, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p, c->kg_block_cnt, c->ctr,
+                                     c->hist, p.depth_passes, std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_many_per_sm), q));
+        } else {
+            SceneTable kt;
+            if (depth0) {
+                kt = scene->tab;
+                kt.seg[0].fc.rasterize_mode = BGS_RASTERIZE_DEPTH;
+            }
+            CU(c, launch_keygen_scene(depth0 ? kt : scene->tab, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p,
+                                      c->kg_block_cnt, c->ctr, c->hist, p.depth_passes,
+                                      std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
         }
-        CU(c, launch_keygen_scene(depth0 ? kt : scene->tab, c->keys[1].p, c->keys[0].p, c->slot_ids.p, c->vals[0].p,
-                                  c->kg_block_cnt, c->ctr, c->hist, p.depth_passes,
-                                  std::min(p.kg_grid, (uint32_t)c->sm_count * c->kg_scene_per_sm), q));
     } else if (p.by_slot) {
         // the cooperative key-gen also produces the depth sort's digit histograms
         // (keys[1] = visibility-mask scratch until the sort's first pass overwrites it)
@@ -570,6 +584,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     if (p.depth_range) {
         if (view_ranges) launch_depth_range_views(scene->tab, views->v, views->n_view, c->vals[cur].p, c->slot_ids.p, c->ctr,
                                                   c->view_ranges, p.n_hint, c->sm_count, q);
+        else if (many) launch_depth_range_many(*dt, c->vals[cur].p, c->slot_ids.p, c->ctr, q);
         else if (scene) launch_depth_range_scene(scene->tab, c->vals[cur].p, c->slot_ids.p, c->ctr, q);
         else launch_depth_range(cloud->pos, n, c->vals[cur].p, p.by_slot ? c->slot_ids.p : nullptr, c->ctr, fc, q);
         ++launches;
@@ -579,7 +594,12 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     if (scene) {   // one launch per projection group: each segment with its own settings and num_classes
         for (size_t i = 0; i < scene->groups.size(); ++i) {
             const uint32_t g = scene->groups[i];
-            if (g == PROJECT_GROUP_4D) {   // (also writes the 4D segments' splat depths, from the moved positions)
+            if (many) {
+                launch_project_many(*dt, g, scene->need_sh[i] != 0, *modes, c->slot_ids.p, c->ctr, c->recs.p,
+                                    (p.raster_mode == 2 || p.raster_mode == 4) ? c->extra.p : nullptr,
+                                    zd || o.pick ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, c->cutoff_tab, ps);
+                scene_3d = scene_3d || g != PROJECT_GROUP_4D;
+            } else if (g == PROJECT_GROUP_4D) {   // (also writes the 4D segments' splat depths, from the moved positions)
                 launch_project_4d_scene(scene->tab, scene->times, scene->classes, *modes, c->slot_ids.p, c->ctr, c->recs.p,
                                         zd || o.pick ? c->splat_depth.p : nullptr, p.n_hint, c->sm_count, ps);
             } else {
@@ -603,7 +623,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     CU(c, cudaEventRecord(c->ev_p1, ps));
     // depth-tested and pick frames: the splat depths, indexed like the records (the projection's index list)
     if ((zd || o.pick) && scene_3d) {
-        launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
+        if (many) launch_splat_depth_many(*dt, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
+        else launch_splat_depth_scene(scene->tab, c->slot_ids.p, c->ctr, c->splat_depth.p, p.n_hint, c->sm_count, ps);
         ++launches;
     } else if (zd && !tc && !scene) {
         launch_splat_depth(cloud->pos, p.by_slot ? c->slot_ids.p : c->vals[cur].p, p.by_slot ? 1 : 0, c->ctr, fc,
@@ -629,7 +650,11 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     b.kinds = c->kinds.p;
     b.views = views;
     PickArgs pk = {};
-    if (o.pick) {
+    PickArgsDev pkd = {};
+    if (o.pick && many) {
+        pkd = PickArgsDev{o.pick, c->slot_ids.p, *dt};
+        b.pick_dev = &pkd;
+    } else if (o.pick) {
         pk = PickArgs{o.pick, c->slot_ids.p, scene->kinds};
         b.pick = &pk;
     }
@@ -639,7 +664,8 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     }
     CU(c, cudaEventRecord(c->ev[3], q));
     if (p.raster_mode >= 3) {   // a mixed-geometry frame: each record's blend kind, for the blend
-        launch_segment_kinds(scene->kinds, c->slot_ids.p, c->ctr, c->kinds.p, p.n_hint, c->sm_count, q);
+        if (many) launch_segment_kinds_many(*dt, c->slot_ids.p, c->ctr, c->kinds.p, p.n_hint, c->sm_count, q);
+        else launch_segment_kinds(scene->kinds, c->slot_ids.p, c->ctr, c->kinds.p, p.n_hint, c->sm_count, q);
         ++launches;
     }
     // ---- stage 4: tile binning -> stable tile-id sort -> ranges; stage 5: per-tile front-to-back blend.
@@ -688,6 +714,11 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     c->pair_result = pcur;
     CU(c, cudaEventRecord(c->ev[5], q));
     CU(c, cudaEventRecord(c->ev_done, q));
+    if (many) {   // (the table's last reader is the blend, which the render stream has joined)
+        CU(c, cudaEventRecord(c->many[scene->slot].ev, q));
+        c->many[scene->slot].used = true;
+        c->many_last = scene->slot;
+    }
     CU(c, cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(FrameCounters), cudaMemcpyDeviceToHost, q));
     CU(c, cudaMemcpyAsync(c->h_sticky, c->d_sticky, 4, cudaMemcpyDeviceToHost, q));
     if (o.slot >= 0) CU(c, cudaEventRecord(c->ev_raster[o.slot], q));
@@ -837,9 +868,10 @@ bgs_status bgs_render_4d(bgs_context* c, const bgs_cloud* cloud, const bgs_view*
 }
 
 // the refusals every scene call makes of its list before reading it: k, SORT_ALL and NULL clouds
+// (at most max_k entities: BGS_SCENE_MAX_CLOUDS, or BGS_ENTITIES_MANY_MAX for bgs_render_entities_many)
 static bgs_status check_scene_list(bgs_context* c, const char* call, const bgs_cloud* const* clouds, uint32_t k,
-                                   const bgs_settings* frame) {
-    if (k == 0 || k > BGS_SCENE_MAX_CLOUDS) return fail(c, BGS_EINVAL, "%s: k = %u is not in 1..%d", call, k, BGS_SCENE_MAX_CLOUDS);
+                                   const bgs_settings* frame, uint32_t max_k = BGS_SCENE_MAX_CLOUDS) {
+    if (k == 0 || k > max_k) return fail(c, BGS_EINVAL, "%s: k = %u is not in 1..%u", call, k, max_k);
     if (frame->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
     for (uint32_t j = 0; j < k; ++j)
         if (!clouds[j]) return fail(c, BGS_EINVAL, "%s: clouds[%u] is NULL", call, j);
@@ -848,6 +880,46 @@ static bgs_status check_scene_list(bgs_context* c, const char* call, const bgs_c
 
 // the blend kind of an entity's records (raster.cu): 0 = quad-uv, 1 = conic (3DGS and 4D with aabb), 2 = surfel
 static int blend_kind(const bgs_entity_settings& e) { return !e.aabb ? 0 : (e.gaussian_mode == BGS_GAUSSIAN_2D ? 2 : 1); }
+
+// a refusal s of entity j's checks, its message led by the entity's index (bgs_render_entities_many: among thousands of
+// entities, the message says which)
+static bgs_status entity_refusal(bgs_context* c, bgs_status s, const char* call, uint32_t j) {
+    char msg[sizeof(c->err)];
+    memcpy(msg, c->err, sizeof(msg));
+    return fail(c, s, "%s: entities[%u]: %s", call, j, msg);
+}
+
+// bgs_render_entities_many's table of k segments in the staging of its slot (bgs_context::many): the slot the last
+// frame enqueued with a table did not take, once the frame that last read it has completed; its regions (Layout) as
+// SceneTableDev's pointers, in device memory of the context's GPU.  Called once the list has passed every refusal, so a
+// refused call neither waits nor allocates.
+static bgs_status many_table(bgs_context* c, uint32_t k, SceneFacts* scene) {
+    CU(c, cudaSetDevice(c->device));   // (the device copy is the context's GPU's, whatever the thread had current)
+    const int slot = c->many_last ^ 1;
+    bgs_context::ManySlot& m = c->many[slot];
+    if (m.used) CU(c, cudaEventSynchronize(m.ev));
+    Layout l;
+    const size_t o_seg = l.add((size_t)k * sizeof(SceneSeg)), o_off = l.add((size_t)k * 4);
+    const size_t o_times = l.add((size_t)k * sizeof(TemporalConsts)), o_cls = l.add((size_t)k * 4), o_kind = l.add((size_t)k * 4);
+    const size_t bytes = l.padded();
+    if (bytes > m.host_bytes) {
+        if (m.host) cudaFreeHost(m.host);
+        m.host = nullptr;
+        m.host_bytes = 0;
+        CU(c, cudaMallocHost(&m.host, bytes));
+        m.host_bytes = bytes;
+    }
+    TRY(m.dev.grow(c, bytes, false));
+    uint8_t* d = m.dev.p;
+    scene->many = true;
+    scene->slot = slot;
+    scene->h_tab = m.host;
+    scene->tab_bytes = bytes;
+    scene->dtab = SceneTableDev{k, 0u, reinterpret_cast<const SceneSeg*>(d + o_seg), reinterpret_cast<const uint32_t*>(d + o_off),
+                                reinterpret_cast<const TemporalConsts*>(d + o_times),
+                                reinterpret_cast<const uint32_t*>(d + o_cls), reinterpret_cast<const uint32_t*>(d + o_kind)};
+    return BGS_OK;
+}
 
 // Every scene frame: k entities, each checked as its single-cloud call (bgs_render_depth_test, or bgs_render_4d for a
 // Gaussian4d cloud when with_4d) with its own settings, num_classes and window, drawn into one depth-sorted frame.
@@ -860,7 +932,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
                                        const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                        const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
                                        const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
-                                       const Targets& t) {
+                                       const Targets& t, bool many = false) {
     const uint32_t nv = t.v;
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
@@ -869,7 +941,10 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     };
     // entity j as its single-cloud call: its settings with the frame's sort bits and flags, its num_classes and window
     std::vector<bgs_settings> st(k);
+    std::vector<TemporalConsts> tcs(k);   // (entity j's times, Gaussian4d entities only)
     auto scene = std::make_shared<SceneFacts>();
+    // (many: a refusal names the entity)
+    auto checked = [&](bgs_status s, uint32_t j) { return s == BGS_OK || !many ? s : entity_refusal(c, s, call, j); };
     bool any_depth = false, undrawn = true;
     uint32_t kinds = 0;
     uint64_t total = 0;
@@ -885,9 +960,11 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
         bgs_settings chk = s;   // (a non-4D entity in Velocity is undrawn, and checked as a Color one)
         if (!is4 && chk.rasterize_mode == BGS_RASTERIZE_VELOCITY) chk.rasterize_mode = BGS_RASTERIZE_COLOR;
         for (uint32_t i = 0; i < nv; ++i)   // (as the single-view call of each view)
-            TRY(check_render(c, clouds[j], &view[i], &unis[j], &chk,
-                             ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr, t.format, false, is4));
-        if (is4) TRY(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, scene->times.t[j]));
+            TRY(checked(check_render(c, clouds[j], &view[i], &unis[j], &chk,
+                                     ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr, t.format, false, is4,
+                                     j == 0 && i == 0),
+                        j));
+        if (is4) TRY(checked(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, tcs[j]), j));
         const bgs_entity_settings& e0 = ents[0];
         undrawn = undrawn && !is4 && e.rasterize_mode == BGS_RASTERIZE_VELOCITY && e.gaussian_mode == e0.gaussian_mode &&
                   e.aabb == e0.aabb && e.opacity_adaptive_radius == e0.opacity_adaptive_radius && e.draw_mode == e0.draw_mode &&
@@ -903,11 +980,29 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     if (total >= (1ull << 30)) return fail(c, BGS_EINVAL, "%s: N = %llu gaussians, must be < 2^30", call, (unsigned long long)total);
     if (depth)
         for (uint32_t i = 0; i < nv; ++i) TRY(check_scene_depth(c, &depth[i], &view[i]));
+    // where the table goes: the SceneFacts' own arrays, or (many) the staging of a device table
+    SceneSeg* segs = scene->tab.seg;
+    uint32_t* offsets = scene->kinds.offset;
+    TemporalConsts* times = scene->times.t;
+    uint32_t* classes = scene->classes.n;
+    uint32_t* seg_kinds = scene->kinds.kind;
+    if (many) {
+        TRY(many_table(c, k, scene.get()));
+        uint8_t* h = static_cast<uint8_t*>(const_cast<void*>(scene->h_tab));
+        const SceneTableDev& d = scene->dtab;
+        const uint8_t* d0 = reinterpret_cast<const uint8_t*>(d.seg);
+        segs = reinterpret_cast<SceneSeg*>(h);
+        offsets = reinterpret_cast<uint32_t*>(h + (reinterpret_cast<const uint8_t*>(d.offset) - d0));
+        times = reinterpret_cast<TemporalConsts*>(h + (reinterpret_cast<const uint8_t*>(d.times) - d0));
+        classes = reinterpret_cast<uint32_t*>(h + (reinterpret_cast<const uint8_t*>(d.classes) - d0));
+        seg_kinds = reinterpret_cast<uint32_t*>(h + (reinterpret_cast<const uint8_t*>(d.kinds) - d0));
+    }
     SceneTable& tab = scene->tab;
     memset(&tab, 0, sizeof(tab));
-    tab.k = k * nv;
+    tab.k = many ? 1u : k * nv;   // (many: tab holds segment 0 alone, the frame's first)
     tab.n_total = (uint32_t)total;
-    scene->kinds.k = k * nv;
+    scene->kinds.k = many ? 0u : k * nv;
+    scene->dtab.n_total = (uint32_t)total;
     uint32_t offset = 0;
     bool box_all = true;
     for (uint32_t i = 0; i < nv; ++i)
@@ -915,7 +1010,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
             const uint32_t sj = i * k + j;   // entity j seen from view i
             const bgs_cloud* cl = clouds[j];
             const uint32_t rm = st[j].rasterize_mode;
-            SceneSeg& sg = tab.seg[sj];
+            SceneSeg& sg = segs[sj];
             sg.fc = frame_consts(cl, &view[i], &unis[j], &st[j], t.aux);
             sg.fc.n_cloud = (uint32_t)n_view;   // (Depth colouring reads its view's sorted list of n_view entries)
             sg.pos = cl->pos;
@@ -929,15 +1024,19 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
             const size_t gi = std::find(scene->groups.begin(), scene->groups.end(), sg.group) - scene->groups.begin();
             if (gi == scene->groups.size()) { scene->groups.push_back(sg.group); scene->need_sh.push_back(0u); }
             if (sh) scene->need_sh[gi] = 1u;
-            scene->times.t[sj] = scene->times.t[j];
-            scene->classes.n[sj] = ents[j].num_classes;
-            scene->kinds.offset[sj] = offset;
-            scene->kinds.kind[sj] = (uint32_t)blend_kind(ents[j]) | (box_of(j) ? BOX_KIND : 0u);
+            times[sj] = tcs[j];
+            classes[sj] = ents[j].num_classes;
+            offsets[sj] = offset;
+            seg_kinds[sj] = (uint32_t)blend_kind(ents[j]) | (box_of(j) ? BOX_KIND : 0u);
             scene->box = scene->box || box_of(j);
             box_all = box_all && box_of(j);
             offset += cl->n;
             scene->clouds.push_back(cl);
         }
+    if (many) tab.seg[0] = segs[0];
+    scene->distinct = scene->clouds;
+    std::sort(scene->distinct.begin(), scene->distinct.end());
+    scene->distinct.erase(std::unique(scene->distinct.begin(), scene->distinct.end()), scene->distinct.end());
     if (nv > 1) {   // each view's tiles after the earlier views', its depth buffer
         ViewTable& vt = scene->views;
         vt.v = nv;
@@ -1018,10 +1117,11 @@ bgs_status bgs_render_scene_4d(bgs_context* c, const bgs_cloud* const* clouds, c
 // bgs_render_entities_ex's refusals of its arguments before the entities are read as single-cloud calls
 static bgs_status check_entities_call(bgs_context* c, const char* call, const bgs_cloud* const* clouds,
                                       const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
-                                      const uint32_t* entity_flags, uint32_t k, const bgs_view* view, const bgs_settings* frame) {
+                                      const uint32_t* entity_flags, uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                                      uint32_t max_k = BGS_SCENE_MAX_CLOUDS) {
     if (!clouds || !unis || !ents || !view || !frame)
         return fail(c, BGS_NOT_READY, "%s: clouds/uniforms/entities/view/settings not ready", call);
-    TRY(check_scene_list(c, call, clouds, k, frame));
+    TRY(check_scene_list(c, call, clouds, k, frame, max_k));
     if (entity_flags)
         for (uint32_t j = 0; j < k; ++j)
             if (entity_flags[j] & ~(uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX)
@@ -1047,8 +1147,8 @@ bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds
 static bgs_status check_targets_call(bgs_context* c, const char* call, const bgs_cloud* const* clouds,
                                      const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                      const uint32_t* entity_flags, uint32_t k, const bgs_view* view, const bgs_settings* frame,
-                                     const Targets& t, bool views, bool pick) {
-    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame));
+                                     const Targets& t, bool views, bool pick, uint32_t max_k = BGS_SCENE_MAX_CLOUDS) {
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame, max_k));
     if (views) {
         if (t.v == 0) return fail(c, BGS_EINVAL, "%s: v = 0 views", call);
         if ((uint64_t)t.v * k > BGS_SCENE_MAX_CLOUDS)
@@ -1116,6 +1216,33 @@ bgs_status bgs_render_entities_pick(bgs_context* c, const bgs_cloud* const* clou
     const Targets t{out_format, out_is_device_ptr, 1, false, &out_rgba, nullptr, nullptr, out_pick};
     TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, view, frame, t, false, true));
     return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, t);
+}
+
+// bgs_render_entities_ex and _pick for any number of entities (include/bgs.h): the segment table in device memory
+bgs_status bgs_render_entities_many(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                    const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
+                                    const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                                    void* out_rgba, uint32_t out_format, int out_is_device_ptr) {
+    const char* call = "render_entities_many";
+    if (!c) return BGS_EINVAL;
+    TRY(check_entities_call(c, call, clouds, unis, ents, entity_flags, k, view, frame, BGS_ENTITIES_MANY_MAX));
+    // (frame_out's refusal, made here so that a refused call has not built the table)
+    if (out_is_device_ptr && reinterpret_cast<uintptr_t>(out_rgba) % format_bpp(out_format) != 0)
+        return fail(c, BGS_EINVAL, "render: device target %p is not aligned to its %zu-byte pixels", out_rgba, format_bpp(out_format));
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth,
+                                colour_target(&out_rgba, out_format, out_is_device_ptr), true);
+}
+
+bgs_status bgs_render_entities_pick_many(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                         const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k,
+                                         const bgs_view* view, const bgs_settings* frame, const bgs_render_extras* ex,
+                                         const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
+                                         int out_is_device_ptr, void* out_pick) {
+    const char* call = "render_entities_pick_many";
+    if (!c) return BGS_EINVAL;
+    const Targets t{out_format, out_is_device_ptr, 1, false, &out_rgba, nullptr, nullptr, out_pick};
+    TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, view, frame, t, false, true, BGS_ENTITIES_MANY_MAX));
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, t, true);
 }
 
 // bgs_render_entities_ex of each of v views in one frame (include/bgs.h); one view is bgs_render_entities_ex itself
@@ -1189,7 +1316,8 @@ bgs_status bgs_debug_sorted_entries(bgs_context* c, uint32_t* out) {
         // culled tail: key = all-ones >> shift, indices ascending (what a stable sort leaves there)
         uint32_t* flags = nullptr;
         CU(c, cudaMalloc(&flags, (size_t)n * 4));
-        if (c->last.scene) launch_culled_flags_scene(c->last.scene->tab, flags, c->stream);
+        if (c->last.scene && c->last.scene->many) launch_culled_flags_many(c->last.scene->dtab, flags, c->stream);
+        else if (c->last.scene) launch_culled_flags_scene(c->last.scene->tab, flags, c->stream);
         else launch_culled_flags(c->last.cloud->pos, n, c->last.fc, flags, c->stream);
         std::vector<uint32_t> f(n);
         cudaError_t e = cudaMemcpyAsync(f.data(), flags, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream);

@@ -65,6 +65,33 @@ struct SceneTable {
     }
 };
 
+// bgs_render_entities_many's segment table, which lives in device memory (one copy per frame from the host) so that k is
+// not bounded by the kernel-parameter limit: k segments seg[0 .. k) as SceneTable's, and beside them their offsets (what
+// find and advance read: one word per step instead of a SceneSeg), times, num_classes and blend kinds.  Its kernels take
+// this handle by value.
+struct TemporalConsts;
+struct SceneTableDev {
+    uint32_t k;                 // segments, 1 .. BGS_ENTITIES_MANY_MAX
+    uint32_t n_total;           // N = sum of n
+    const SceneSeg* seg;
+    const uint32_t* offset;     // seg[j].offset
+    const TemporalConsts* times;
+    const uint32_t* classes;    // num_classes of each segment
+    const uint32_t* kinds;      // SegmentKinds::kind of each segment
+    __device__ __forceinline__ uint32_t find(uint32_t g) const {
+        uint32_t lo = 0u, hi = k;
+        while (hi - lo > 1u) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (__ldg(offset + mid) <= g) lo = mid; else hi = mid;
+        }
+        return lo;
+    }
+    __device__ __forceinline__ uint32_t advance(uint32_t j, uint32_t g) const {
+        while (j + 1u < k && __ldg(offset + j + 1u) <= g) ++j;
+        return j;
+    }
+};
+
 // The projection group of Gaussian4d segments: project_group gives the 3D layouts 0 .. 7 (f16 bit, SH degree << 1), so
 // 4D segments never fall into a 3D launch, and splat_depth_scene leaves their depths to the 4D projection, which takes
 // them from the moved positions.

@@ -67,14 +67,17 @@ struct OneCloud {
     }
 };
 
-// bgs_render_scene's table.  `groups` has bit b set for the segments of project_group b this launch covers; `times` are
-// bgs_render_scene_4d's per-segment times.  seg / advance give the segment of an index (seg clamps one past the end to
-// the last gaussian's segment; advance walks forward from j for an index that only grows within a thread).
-struct SceneSrc {
-    const SceneTable& t;
+// A segment table: bgs_render_scene's (SceneTable, a kernel parameter; SceneSrc) or bgs_render_entities_many's
+// (SceneTableDev, in device memory; SceneSrcDev).  `groups` has bit b set for the segments of project_group b this launch
+// covers; `times` are the per-segment times of Gaussian4d segments.  seg / advance give the segment of an index (seg clamps
+// one past the end to the last gaussian's segment; advance walks forward from j for an index that only grows within a
+// thread).
+template <class Table>
+struct SegmentSrc {
+    const Table& t;
     uint32_t groups = ~0u;
     const uint32_t* slot_ids = nullptr;   // compact slot -> global index
-    const SceneTimes* times = nullptr;
+    const TemporalConsts* times = nullptr;
     static constexpr bool SEGMENTED = true;
     static constexpr uint32_t NONE = 0xFFFFFFFFu;
 
@@ -82,7 +85,7 @@ struct SceneSrc {
     __device__ __forceinline__ uint32_t advance(uint32_t j, uint32_t i) const { return t.advance(j, i); }
     __device__ __forceinline__ bool mine(uint32_t j) const { return (groups >> t.seg[j].group) & 1u; }
     __device__ __forceinline__ const FrameConsts& fc(uint32_t j) const { return t.seg[j].fc; }
-    __device__ __forceinline__ const TemporalConsts& tc(uint32_t j) const { return times->t[j]; }
+    __device__ __forceinline__ const TemporalConsts& tc(uint32_t j) const { return times[j]; }
     __device__ __forceinline__ const float4* pos_at(uint32_t j, uint32_t i) const { return t.seg[j].pos + (i - t.seg[j].offset); }
     template <int BCH>
     __device__ __forceinline__ const uint4* block_at(uint32_t j, uint32_t i) const {
@@ -108,6 +111,8 @@ struct SceneSrc {
         }
     }
 };
+using SceneSrc = SegmentSrc<SceneTable>;
+using SceneSrcDev = SegmentSrc<SceneTableDev>;
 
 // The grid of a persistent grid-stride kernel over entries whose count only the device knows: ceil(n_hint / threads)
 // CTAs, at most ctas_per_sm per SM, at least one.

@@ -2,6 +2,7 @@
 // (the calls on a resident cloud).  The objects behind include/bgs.h's handles, error reporting, the context registry,
 // the order of a cloud's accesses, and the frame scratch that the selections borrow.
 #pragma once
+#include <algorithm>
 #include <atomic>
 #include <memory>
 #include <mutex>
@@ -72,6 +73,7 @@ struct SceneFacts {
     SceneTable tab;
     SceneTimes times = {};
     std::vector<const bgs_cloud*> clouds;
+    std::vector<const bgs_cloud*> distinct;   // the clouds listed, each once (sorted by address)
     std::vector<uint32_t> groups;
     std::vector<uint32_t> need_sh;   // per entry of groups
     SceneClasses classes = {};
@@ -82,6 +84,14 @@ struct SceneFacts {
     // seen from view i; the views' tile geometry and depth buffers (their targets are the frame's, filled in when it is
     // enqueued)
     ViewTable views = {};
+    // a bgs_render_entities_many frame: the segments, times, num_classes and kinds are in the device table dtab (tab holds
+    // N and segment 0 alone), which enqueue_frame copies from the pinned staging h_tab (tab_bytes) of the context's table
+    // slot `slot` (bgs_context::many)
+    bool many = false;
+    SceneTableDev dtab = {};
+    const void* h_tab = nullptr;
+    size_t tab_bytes = 0;
+    int slot = 0;
 };
 
 // What the host knows of a frame it has enqueued: the context keeps the last one enqueued (`pend`) and, once its
@@ -99,10 +109,7 @@ struct FrameFacts {
     std::shared_ptr<const SceneFacts> scene;   // bgs_render_scene frames only (nulled with `cloud`)
     bool reads(const bgs_cloud* cl) const {
         if (cloud == cl) return true;
-        if (scene)
-            for (const bgs_cloud* s : scene->clouds)
-                if (s == cl) return true;
-        return false;
+        return scene && std::binary_search(scene->distinct.begin(), scene->distinct.end(), cl);
     }
     void forget() { cloud = nullptr; scene.reset(); }
 };
@@ -116,6 +123,7 @@ struct bgs_context {
                                           // a smaller grid leaves that room to the other frames' issue-bound blend
     int rs_per_sm = 0;                    // co-resident radix-sort CTAs per SM (radix.cu)
     uint32_t kg_scene_per_sm = 0;         // co-resident CTAs per SM of bgs_render_scene's key-gen (keygen.cu)
+    uint32_t kg_many_per_sm = 0;          // ... of bgs_render_entities_many's
     uint32_t sort_epoch = 0;              // look-back status epoch: +1 per sort launch (status words never need clearing)
     cudaStream_t stream = nullptr;    // render stream (high priority): everything but the projection
     cudaStream_t stream2 = nullptr;   // projection runs here, beside the depth sort
@@ -196,6 +204,20 @@ struct bgs_context {
     // context goes): one chunk's planes each, so the host's copy of one chunk overlaps the device-to-host copy of the next
     uint8_t* h_bounce = nullptr;
 
+    // bgs_render_entities_many's segment tables: two slots, each a pinned staging buffer, its device copy (both grow-only)
+    // and the event recorded after the last frame that read it.  A frame takes the slot the last one enqueued did not
+    // (many_last), once that slot's frame has completed, so neither a queued frame's table nor the one the debug hooks of
+    // the last frame read is overwritten.
+    struct ManySlot {
+        uint8_t* host = nullptr;
+        size_t host_bytes = 0;
+        DevBuf<uint8_t> dev;
+        cudaEvent_t ev = nullptr;
+        bool used = false;
+    };
+    ManySlot many[2];
+    int many_last = 1;
+
     FrameFacts pend, last;
     bool have_frame = false;           // `last` is valid (for the debug hooks)
     int depth_result = 0, pair_result = 0;   // which ping-pong buffer holds the sorted result
@@ -211,7 +233,7 @@ struct bgs_context {
         for (cudaEvent_t& e : ev) f(e, true);
         f(ev_p0, true); f(ev_p1, true);
         for (cudaEvent_t* e : {&ev_front, &ev_rdone, &ev_fork, &ev_join, &ev_done, &ev_raster[0], &ev_raster[1],
-                               &ev_copied[0], &ev_copied[1]})
+                               &ev_copied[0], &ev_copied[1], &many[0].ev, &many[1].ev})
             f(*e, false);
     }
 };

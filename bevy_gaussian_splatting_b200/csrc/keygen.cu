@@ -212,6 +212,15 @@ keygen_scene_kernel(SceneTable tab, uint32_t* __restrict__ masks, uint32_t* __re
                      hist_passes);
 }
 
+// bgs_render_entities_many: the same over a segment table in device memory.  fc carries the frame-wide values (its
+// rasterize_mode and aux), as segment 0's do for keygen_scene_kernel.
+__global__ void __launch_bounds__(KG_THREADS)
+keygen_many_kernel(SceneTableDev tab, FrameConsts fc, uint32_t* __restrict__ masks, uint32_t* __restrict__ keys_out,
+                   uint32_t* __restrict__ ids_out, uint32_t* __restrict__ slots_out, uint32_t* __restrict__ block_cnt,
+                   FrameCounters* __restrict__ ctr, uint32_t* __restrict__ hist, int hist_passes) {
+    keygen_coop_body(SceneSrcDev{tab}, tab.n_total, fc, masks, keys_out, ids_out, slots_out, block_cnt, ctr, hist, hist_passes);
+}
+
 // Debug hook: rebuild the reference's full sorted_entry_buffer (sort/mod.rs:323-329) from the
 // compacted result: [0, n_vis) = sorted visible entries, then every culled index ascending
 // with key 0xFFFFFFFF >> shift.  Single block per call chunk; not on the hot path.
@@ -234,6 +243,10 @@ __global__ void culled_flags_kernel(const float4* __restrict__ pos, uint32_t n, 
 
 __global__ void culled_flags_scene_kernel(SceneTable tab, uint32_t* __restrict__ flags) {
     culled_flags_body(SceneSrc{tab}, tab.n_total, flags);
+}
+
+__global__ void culled_flags_many_kernel(SceneTableDev tab, uint32_t* __restrict__ flags) {
+    culled_flags_body(SceneSrcDev{tab}, tab.n_total, flags);
 }
 
 void launch_keygen_all(const float4* pos, uint32_t n, const FrameConsts& fc, uint32_t* keys_out, uint32_t* ids_out,
@@ -274,6 +287,25 @@ cudaError_t launch_keygen_scene(const SceneTable& tab, uint32_t* masks, uint32_t
 
 void launch_culled_flags_scene(const SceneTable& tab, uint32_t* flags, cudaStream_t stream) {
     culled_flags_scene_kernel<<<(tab.n_total + 255) / 256, 256, 0, stream>>>(tab, flags);
+}
+
+int keygen_many_blocks_per_sm() {
+    int b = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, keygen_many_kernel, KG_THREADS, 0) != cudaSuccess) return 0;
+    return b;
+}
+cudaError_t launch_keygen_many(const SceneTableDev& tab, const FrameConsts& fc, uint32_t* masks, uint32_t* keys_out,
+                               uint32_t* ids_out, uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr, uint32_t* hist,
+                               int hist_passes, uint32_t grid, cudaStream_t stream) {
+    SceneTableDev t = tab;
+    FrameConsts f = fc;
+    void* args[] = {(void*)&t, (void*)&f, (void*)&masks, (void*)&keys_out, (void*)&ids_out, (void*)&slots_out,
+                    (void*)&block_cnt, (void*)&ctr, (void*)&hist, (void*)&hist_passes};
+    return cudaLaunchCooperativeKernel((const void*)keygen_many_kernel, dim3(grid), dim3(KG_THREADS), args, 0, stream);
+}
+
+void launch_culled_flags_many(const SceneTableDev& tab, uint32_t* flags, cudaStream_t stream) {
+    culled_flags_many_kernel<<<(tab.n_total + 255) / 256, 256, 0, stream>>>(tab, flags);
 }
 
 }  // namespace bgs

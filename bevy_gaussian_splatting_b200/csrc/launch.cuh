@@ -18,6 +18,12 @@ cudaError_t launch_keygen_scene(const SceneTable& tab, uint32_t* masks, uint32_t
                                 uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr, uint32_t* hist, int hist_passes,
                                 uint32_t grid, cudaStream_t stream);
 void launch_culled_flags_scene(const SceneTable& tab, uint32_t* flags, cudaStream_t stream);
+// bgs_render_entities_many's: the same over a segment table in device memory (fc: the frame-wide values)
+int keygen_many_blocks_per_sm();
+cudaError_t launch_keygen_many(const SceneTableDev& tab, const FrameConsts& fc, uint32_t* masks, uint32_t* keys_out,
+                               uint32_t* ids_out, uint32_t* slots_out, uint32_t* block_cnt, FrameCounters* ctr, uint32_t* hist,
+                               int hist_passes, uint32_t grid, cudaStream_t stream);
+void launch_culled_flags_many(const SceneTableDev& tab, uint32_t* flags, cudaStream_t stream);
 // radix.cu
 uint32_t radix_num_tiles(uint32_t capacity);
 int radix_coop_blocks_per_sm(int items);
@@ -62,6 +68,13 @@ void launch_depth_range_views(const SceneTable& tab, uint32_t v, uint32_t n_view
 void launch_project_4d_scene(const SceneTable& tab, const SceneTimes& times, const SceneClasses& classes,
                              const ModeConsts& mc, const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs,
                              float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
+// bgs_render_entities_many: the same over a segment table in device memory (its times and num_classes beside it); one
+// launch_project_many per group, the 4D group included (depths: its splat depths)
+void launch_depth_range_many(const SceneTableDev& tab, const uint32_t* sorted_payload, const uint32_t* slot_ids,
+                             FrameCounters* ctr, cudaStream_t stream);
+void launch_project_many(const SceneTableDev& tab, uint32_t group, bool need_sh, const ModeConsts& mc,
+                         const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs, float4* extra,
+                         float* depths, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream);
 // bin.cu
 int bin_coop_blocks_per_sm();
 cudaError_t launch_bin_emit_coop(const SplatRec* recs, const uint32_t* perm, FrameCounters* ctr, ChunkCounters* cc,
@@ -80,6 +93,8 @@ void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_sl
                         const FrameConsts& fc, float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream);
 void launch_splat_depth_scene(const SceneTable& tab, const uint32_t* slot_ids, const FrameCounters* ctr, float* depths,
                               uint32_t n_hint, int sm_count, cudaStream_t stream);
+void launch_splat_depth_many(const SceneTableDev& tab, const uint32_t* slot_ids, const FrameCounters* ctr, float* depths,
+                             uint32_t n_hint, int sm_count, cudaStream_t stream);
 // raster.cu.  A one-round frame's blend of the sorted pairs `tile_entries` (per tile: `ranges`) into `out`, W x H in
 // tiles_x x tiles_y tiles, in `format` (BGS_FORMAT_* | output mode << 8).  mode 0..2: one blend kind for every splat;
 // 3 / 4 (bgs_render_entities): mixed kinds, read from `kinds` (one byte per record), 4 when some splat is a surfel.  box:
@@ -95,6 +110,25 @@ struct PickArgs {
     uint4* out;
     const uint32_t* slot_ids;
     SegmentKinds seg;
+    // global index g as (segment, index within it): the last j with offset <= g (SceneTable::find)
+    __device__ __forceinline__ uint2 locate(uint32_t g) const {
+        uint32_t lo = 0u, hi = seg.k;
+        while (hi - lo > 1u) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (seg.offset[mid] <= g) lo = mid; else hi = mid;
+        }
+        return make_uint2(lo, g - seg.offset[lo]);
+    }
+};
+// bgs_render_entities_many's pick frame: the segments are the device table's
+struct PickArgsDev {
+    uint4* out;
+    const uint32_t* slot_ids;
+    SceneTableDev tab;
+    __device__ __forceinline__ uint2 locate(uint32_t g) const {
+        const uint32_t j = tab.find(g);
+        return make_uint2(j, g - __ldg(tab.offset + j));
+    }
 };
 static_assert(sizeof(bgs_pick) == sizeof(uint4), "a pick record is stored as one uint4");
 struct BlendArgs {
@@ -118,6 +152,7 @@ struct BlendArgs {
     const unsigned char* kinds = nullptr;
     const ViewTable* views = nullptr;
     const PickArgs* pick = nullptr;
+    const PickArgsDev* pick_dev = nullptr;   // (bgs_render_entities_pick_many: in place of pick)
 };
 void launch_raster(const BlendArgs& a, cudaStream_t stream);
 // one front-to-back round of a chunked frame (a's single-view quad-uv blend, depth test included): each pixel's blend state
@@ -127,6 +162,8 @@ void launch_raster_round(const BlendArgs& a, float4* state, unsigned char* tile_
 // a mixed-geometry frame's blend kind of each compact slot (records n_vis of ctr), from its segment's
 void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
                           uint32_t n_hint, int sm_count, cudaStream_t stream);
+void launch_segment_kinds_many(const SceneTableDev& tab, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
+                               uint32_t n_hint, int sm_count, cudaStream_t stream);
 // select.cu
 uint32_t select_num_buckets(uint32_t n);
 int select_sort_passes(uint32_t n_buckets);

@@ -1008,10 +1008,13 @@ void launch_project_4d(const void* blocks, const uint32_t* index_list, int by_sl
 template <bool F16, uint32_t D>
 constexpr int scene_min_ctas() { return !F16 && D >= 2 ? 3 : PROJ_MIN_CTAS; }
 
-// G's projection with segment j's num_classes
-template <class G>
+// G's projection with segment j's num_classes (classes.n[j]: a SceneClasses, or a SceneTableDev's array)
+struct ClassesDev {
+    const uint32_t* n;
+};
+template <class G, class Classes = SceneClasses>
 struct SceneGeo : G {
-    const SceneClasses& classes;
+    const Classes& classes;
     template <class Src>
     __device__ __forceinline__ void project(const Src& src, uint32_t j, uint32_t e, uint32_t r, float4 p4, const float q[4],
                                             const float so[4], const float* ext, uint32_t op_bits, const ModeConsts& mc) const {
@@ -1160,7 +1163,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, PROJ_MIN_CTAS)
 project_4d_scene_kernel(SceneTable tab, SceneTimes times, SceneClasses classes, ModeConsts mc,
                         const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
                         SplatRec* __restrict__ recs, float* __restrict__ depths /* depth-tested frames only */) {
-    project_loop(SceneSrc{tab, 1u << PROJECT_GROUP_4D, slot_ids, &times}, SceneGeo<Geo4d>{{ctr, recs, depths}, classes}, ctr, mc);
+    project_loop(SceneSrc{tab, 1u << PROJECT_GROUP_4D, slot_ids, times.t}, SceneGeo<Geo4d>{{ctr, recs, depths}, classes}, ctr, mc);
 }
 // sm_90 takes up to 32764 B of kernel parameters (CUDA >= 12.1): the table (~22 KB), the times (768 B), the classes
 // (256 B), the extras and four pointers
@@ -1191,6 +1194,60 @@ void launch_project_scene(const SceneTable& tab, uint32_t group, bool need_sh, c
                                                   : project_scene_kernel<is_f16(Lv), D, false>;
             kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, group, need_sh ? 1u : 0u, classes, mc, slot_ids, ctr, recs, extra,
                                                       cutoff_tab, aux);
+        }
+    });
+}
+
+// ---- bgs_render_entities_many: the scene kernels over a segment table in device memory (SceneSrcDev), their bodies
+// the scene frames' own
+__global__ void depth_range_many_kernel(SceneTableDev tab, const uint32_t* __restrict__ sorted_payload,
+                                        const uint32_t* __restrict__ slot_ids, FrameCounters* __restrict__ ctr) {
+    depth_range_body(SceneSrcDev{tab}, tab.n_total, sorted_payload, slot_ids, ctr);
+}
+
+template <bool F16, uint32_t D, bool MODES2>
+__global__ void __launch_bounds__(PROJ_THREADS, scene_min_ctas<F16, D>())
+project_many_kernel(SceneTableDev tab, uint32_t group, uint32_t need_sh, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
+                    const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs, float4* __restrict__ extra,
+                    const float* __restrict__ cutoff_tab) {
+    project_loop(SceneSrcDev{tab, 1u << group, slot_ids},
+                 SceneGeo<Geo3d<F16, D, MODES2>, ClassesDev>{{ctr, need_sh != 0u, recs, extra, cutoff_tab, nullptr},
+                                                             ClassesDev{tab.classes}},
+                 ctr, mc);
+}
+
+// (the segment's constants come from global memory: at PROJ_MIN_CTAS per SM its 128 registers spill 4 B; at 3, 168
+// registers and no spill)
+constexpr int PROJ_4D_MANY_CTAS = 3;
+__global__ void __launch_bounds__(PROJ_THREADS, PROJ_4D_MANY_CTAS)
+project_4d_many_kernel(SceneTableDev tab, ModeConsts mc, const uint32_t* __restrict__ slot_ids,
+                       const FrameCounters* __restrict__ ctr, SplatRec* __restrict__ recs, float* __restrict__ depths) {
+    project_loop(SceneSrcDev{tab, 1u << PROJECT_GROUP_4D, slot_ids, tab.times},
+                 SceneGeo<Geo4d, ClassesDev>{{ctr, recs, depths}, ClassesDev{tab.classes}}, ctr, mc);
+}
+
+void launch_depth_range_many(const SceneTableDev& tab, const uint32_t* sorted_payload, const uint32_t* slot_ids,
+                             FrameCounters* ctr, cudaStream_t stream) {
+    depth_range_many_kernel<<<1, 32, 0, stream>>>(tab, sorted_payload, slot_ids, ctr);
+}
+
+void launch_project_many(const SceneTableDev& tab, uint32_t group, bool need_sh, const ModeConsts& mc,
+                         const uint32_t* slot_ids, const FrameCounters* ctr, SplatRec* recs, float4* extra,
+                         float* depths, uint32_t n_hint, int sm_count, const float* cutoff_tab, cudaStream_t stream) {
+    if (group == PROJECT_GROUP_4D) {
+        const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_4D_MANY_CTAS, sm_count);
+        project_4d_many_kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, mc, slot_ids, ctr, recs, depths);
+        return;
+    }
+    const uint32_t grid = persistent_grid(n_hint, PROJ_THREADS, PROJ_MIN_CTAS, sm_count);
+    const uint32_t g = group & ~ENTITY_MODES;
+    with_layout_degree(g & 1u ? CloudLayout::F16 : CloudLayout::F32, g >> 1, [&](auto L, auto Dt) {
+        constexpr CloudLayout Lv = decltype(L)::value;
+        constexpr uint32_t D = decltype(Dt)::value;
+        if constexpr (!is_4d(Lv)) {
+            auto* kernel = (group & ENTITY_MODES) ? project_many_kernel<is_f16(Lv), D, true>
+                                                  : project_many_kernel<is_f16(Lv), D, false>;
+            kernel<<<grid, PROJ_THREADS, 0, stream>>>(tab, group, need_sh ? 1u : 0u, mc, slot_ids, ctr, recs, extra, cutoff_tab);
         }
     });
 }

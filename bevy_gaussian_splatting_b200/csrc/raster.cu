@@ -270,7 +270,7 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // weight w = a T of the pairs it blends (an overlay edge pair: w = T) and that pair's record; a later pair replaces it only
 // when its w is strictly larger.  Every pixel of pk->out is written: (entity, index, w, d) of that pair, or BGS_PICK_NONE
 // where nothing blends.  Pick frames take the generic loop in every mode, never the inline-asm one.
-template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false, bool PICK = false>
+template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false, bool PICK = false, class Pick = PickArgs>
 __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
                                             const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
                                             int H, int tiles_x, void* __restrict__ out, uint32_t format,
@@ -278,7 +278,7 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
                                             void* __restrict__ out_normal, const uint32_t* __restrict__ truncated,
                                             const float* __restrict__ splat_d, const float* __restrict__ scene, size_t pitch,
                                             const unsigned char* __restrict__ kinds, const ViewTable* vt = nullptr,
-                                            const PickArgs* pk = nullptr) {
+                                            const Pick* pk = nullptr) {
     constexpr bool MIXED = MODE >= 3, SURF = MODE == 2 || MODE == 4;
     __shared__ __align__(16) unsigned char s_mem[(SURF ? SM_BYTES_2D : SM_BYTES) + (AUX ? 2 * RT_CHUNK * 16 : 0) +
                                                  (ZTEST && !AUX ? ZT_BYTES : 0)];
@@ -564,13 +564,8 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
     if constexpr (PICK) {   // record -> global index (compact slot) -> (entity, index within its cloud), and its d
         uint4 rec = make_uint4(BGS_PICK_NONE, BGS_PICK_NONE, 0u, 0u);
         if (best_r != BGS_PICK_NONE) {
-            const uint32_t g = __ldg(pk->slot_ids + best_r);
-            uint32_t lo = 0u, hi = pk->seg.k;   // the last j with offset <= g (SceneTable::find)
-            while (hi - lo > 1u) {
-                const uint32_t mid = (lo + hi) >> 1;
-                if (pk->seg.offset[mid] <= g) lo = mid; else hi = mid;
-            }
-            rec = make_uint4(lo, g - pk->seg.offset[lo], __float_as_uint(best_w), __float_as_uint(__ldg(splat_d + best_r)));
+            const uint2 at = pk->locate(__ldg(pk->slot_ids + best_r));
+            rec = make_uint4(at.x, at.y, __float_as_uint(best_w), __float_as_uint(__ldg(splat_d + best_r)));
         }
         pk->out[(size_t)py * W + px] = rec;
     }
@@ -581,12 +576,13 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
 }
 
 // The blend kernels: raster_body of one (MODE, AUX, ZTEST, BOX) and one frame kind, picked by the trailing parameter's type
-// Tail: OneView (a single-view frame), ViewTable (a views frame: raster_body's VIEWS) or PickArgs (a pick frame: its PICK).
+// Tail: OneView (a single-view frame), ViewTable (a views frame: raster_body's VIEWS) or PickArgs / PickArgsDev (a pick
+// frame: its PICK, the segments a kernel parameter or bgs_render_entities_many's device table).
 // Every variant takes the same scalar parameters; raster_body sees null for those its variant never reads, so a variant's
 // code does not depend on them.
 struct OneView {};
 template <class Tail> constexpr bool IS_VIEWS = std::is_same<Tail, ViewTable>::value;
-template <class Tail> constexpr bool IS_PICK = std::is_same<Tail, PickArgs>::value;
+template <class Tail> constexpr bool IS_PICK = std::is_same<Tail, PickArgs>::value || std::is_same<Tail, PickArgsDev>::value;
 
 // Minimum CTAs per SM of each variant: the most that leave it without spills (ptxas report), and for MODE 0 without aux
 // the 6 its register budget was written for.
@@ -620,11 +616,12 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
               const uint32_t* __restrict__ truncated, const float* __restrict__ splat_d, const float* __restrict__ scene,
               size_t pitch, const unsigned char* __restrict__ kinds, const __grid_constant__ Tail tail) {
     constexpr bool VIEWS = IS_VIEWS<Tail>;   // (a views frame's size, targets and depth buffers are its view's)
-    raster_body<MODE, AUX, ZTEST, BOX, VIEWS, IS_PICK<Tail>>(
+    using Pick = typename std::conditional<std::is_same<Tail, PickArgsDev>::value, PickArgsDev, PickArgs>::type;
+    raster_body<MODE, AUX, ZTEST, BOX, VIEWS, IS_PICK<Tail>, Pick>(
         recs, extra, tile_entries, ranges, VIEWS ? 0 : W, VIEWS ? 0 : H, VIEWS ? 0 : tiles_x, VIEWS ? nullptr : out, format,
         AUX ? aux : nullptr, AUX && !VIEWS ? out_depth : nullptr, AUX && !VIEWS ? out_normal : nullptr, truncated, splat_d,
         VIEWS ? nullptr : scene, VIEWS ? 0 : pitch, MODE >= 3 ? kinds : nullptr, tail_as<ViewTable>(tail),
-        tail_as<PickArgs>(tail));
+        tail_as<Pick>(tail));
 }
 
 // the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
@@ -642,11 +639,27 @@ __global__ void raster_kinds_kernel(SegmentKinds sk, const uint32_t* __restrict_
     }
 }
 
+// bgs_render_entities_many's: the segments are the device table's
+__global__ void raster_kinds_many_kernel(SceneTableDev tab, const uint32_t* __restrict__ slot_ids,
+                                         const FrameCounters* __restrict__ ctr, unsigned char* __restrict__ out) {
+    const uint32_t n_vis = ctr->n_vis;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n_vis; r += gridDim.x * blockDim.x)
+        out[r] = (unsigned char)__ldg(tab.kinds + tab.find(__ldg(slot_ids + r)));
+}
+
+static uint32_t kinds_grid(uint32_t n_hint, int sm_count) {
+    const uint32_t grid = (n_hint + 255) / 256;
+    return grid < 1u ? 1u : (grid > (uint32_t)(8 * sm_count) ? (uint32_t)(8 * sm_count) : grid);
+}
+
+void launch_segment_kinds_many(const SceneTableDev& tab, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
+                               uint32_t n_hint, int sm_count, cudaStream_t stream) {
+    raster_kinds_many_kernel<<<kinds_grid(n_hint, sm_count), 256, 0, stream>>>(tab, slot_ids, ctr, out);
+}
+
 void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
                           uint32_t n_hint, int sm_count, cudaStream_t stream) {
-    uint32_t grid = (n_hint + 255) / 256;
-    grid = grid < 1u ? 1u : (grid > (uint32_t)(8 * sm_count) ? (uint32_t)(8 * sm_count) : grid);
-    raster_kinds_kernel<<<grid, 256, 0, stream>>>(kinds, slot_ids, ctr, out);
+    raster_kinds_kernel<<<kinds_grid(n_hint, sm_count), 256, 0, stream>>>(kinds, slot_ids, ctr, out);
 }
 
 // ---- MODE 0 fast path: 2 horizontally adjacent pixels per thread -----------------------------------------
@@ -843,6 +856,8 @@ void launch_raster(const BlendArgs& a, cudaStream_t stream) {
         launch_blend(a, a.views->tile0[a.views->v], *a.views, stream);
     } else if (a.pick) {
         launch_blend(a, (uint32_t)(a.tiles_x * a.tiles_y), *a.pick, stream);
+    } else if (a.pick_dev) {
+        launch_blend(a, (uint32_t)(a.tiles_x * a.tiles_y), *a.pick_dev, stream);
     } else if (a.mode == 0 && !a.aux && !a.box && a.large_footprints) {
         // the 2-pixels-per-thread variant wins when splats cover many tiles each and loses when most splats are a few
         // pixels (more of its lanes then idle at the tile's splat boundaries)

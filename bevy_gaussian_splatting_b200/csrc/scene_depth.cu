@@ -42,6 +42,14 @@ splat_depth_scene_kernel(SceneTable tab, const uint32_t* __restrict__ slot_ids, 
     splat_depth_body(SceneSrc{tab, groups_3d, slot_ids}, ctr, depths);
 }
 
+// bgs_render_entities_many: the same over a segment table in device memory
+__global__ void __launch_bounds__(SD_THREADS)
+splat_depth_many_kernel(SceneTableDev tab, const uint32_t* __restrict__ slot_ids, const FrameCounters* __restrict__ ctr,
+                        float* __restrict__ depths) {
+    constexpr uint32_t groups_3d = ((1u << PROJECT_GROUP_4D) - 1u) * (1u | 1u << ENTITY_MODES);
+    splat_depth_body(SceneSrcDev{tab, groups_3d, slot_ids}, ctr, depths);
+}
+
 void launch_splat_depth(const float4* pos, const uint32_t* index_list, int by_slot, const FrameCounters* ctr,
                         const FrameConsts& fc, float* depths, uint32_t n_hint, int sm_count, cudaStream_t stream) {
     const uint32_t grid = persistent_grid(n_hint, SD_THREADS, SD_CTAS_PER_SM, sm_count);
@@ -52,6 +60,12 @@ void launch_splat_depth_scene(const SceneTable& tab, const uint32_t* slot_ids, c
                               uint32_t n_hint, int sm_count, cudaStream_t stream) {
     const uint32_t grid = persistent_grid(n_hint, SD_THREADS, SD_CTAS_PER_SM, sm_count);
     splat_depth_scene_kernel<<<grid, SD_THREADS, 0, stream>>>(tab, slot_ids, ctr, depths);
+}
+
+void launch_splat_depth_many(const SceneTableDev& tab, const uint32_t* slot_ids, const FrameCounters* ctr, float* depths,
+                             uint32_t n_hint, int sm_count, cudaStream_t stream) {
+    const uint32_t grid = persistent_grid(n_hint, SD_THREADS, SD_CTAS_PER_SM, sm_count);
+    splat_depth_many_kernel<<<grid, SD_THREADS, 0, stream>>>(tab, slot_ids, ctr, depths);
 }
 
 }  // namespace bgs

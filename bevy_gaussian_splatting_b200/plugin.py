@@ -299,22 +299,29 @@ def check_scene_entities_4d(entities) -> CloudSettings:
 ENTITIES_FRAME_FIELDS = ("radix_sort_depth_bits", "sort_mode", "sort_all", "binning_rounds")
 
 
-def check_entities(entities) -> CloudSettings:
+def check_entities(entities, max_entities: int = abi.BGS_SCENE_MAX_CLOUDS, call: str = "render_entities") -> CloudSettings:
     """`entities`: a sequence of (handle, CloudSettings, transform or None), one bgs_render_entities call's clouds, each
     drawn with its own settings.  Returns the settings the frame-wide values (ENTITIES_FRAME_FIELDS) come from, the first
-    entity's; raises ValueError when there are none, too many, or two entities disagree on a frame-wide field."""
+    entity's; raises ValueError when there are none, more than `max_entities`, or two entities disagree on a frame-wide
+    field (`call` names the call in the message)."""
     entities = list(entities)
     if not entities:
-        raise ValueError("render_entities: no entities")
-    if len(entities) > abi.BGS_SCENE_MAX_CLOUDS:
-        raise ValueError(f"render_entities: {len(entities)} entities, at most {abi.BGS_SCENE_MAX_CLOUDS}")
+        raise ValueError(f"{call}: no entities")
+    if len(entities) > max_entities:
+        raise ValueError(f"{call}: {len(entities)} entities, at most {max_entities}")
     first = entities[0][1]
     for j, (_, st, _) in enumerate(entities[1:], 1):
         for name in ENTITIES_FRAME_FIELDS:
             a, b = getattr(first, name), getattr(st, name)
             if a != b:
-                raise ValueError(f"render_entities: entity {j} has {name} = {b!r}, entity 0 {a!r}: the frame has one depth sort")
+                raise ValueError(f"{call}: entity {j} has {name} = {b!r}, entity 0 {a!r}: the frame has one depth sort")
     return first
+
+
+def check_entities_many(entities, call: str = "render_entities_many") -> CloudSettings:
+    """`check_entities` for one bgs_render_entities_many or _pick_many call (`call` names it in the message): up to
+    abi.BGS_ENTITIES_MANY_MAX entities."""
+    return check_entities(entities, abi.BGS_ENTITIES_MANY_MAX, call)
 
 
 def check_entities_aux(entities) -> CloudSettings:
@@ -551,15 +558,30 @@ class GaussianSplattingPlugin:
         with the scan around them.  visualize_bounding_box is per entity too (`bgs_render_entities_ex`'s entity flags).
         radix_sort_depth_bits (and the other sort fields) are the frame's and must agree (`check_entities`, ValueError
         before any call).  The other arguments are `render_scene`'s."""
+        return self._render_entities("bgs_render_entities_ex", check_entities, entities, view, fmt, scene_depth,
+                                     previous_view, delta_time, asynchronous, premultiplied, blend_over, out)
+
+    def render_entities_many(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None,
+                             previous_view: View | None = None, delta_time: float | None = None, asynchronous: bool = False,
+                             premultiplied: bool = False, blend_over: bool = False, out: np.ndarray | None = None) -> np.ndarray:
+        """`render_entities` for any number of entities up to abi.BGS_ENTITIES_MANY_MAX (`bgs_render_entities_many`):
+        byte for byte the frame `render_entities` defines, for instanced clouds (one handle listed many times under
+        different transforms), glTF scenes with many node placements (`SceneHandles.entities()`) or editor scenes of many
+        objects.  Validates with `check_entities_many` (ValueError before any call)."""
+        return self._render_entities("bgs_render_entities_many", check_entities_many, entities, view, fmt, scene_depth,
+                                     previous_view, delta_time, asynchronous, premultiplied, blend_over, out)
+
+    def _render_entities(self, fn: str, check, entities, view, fmt, scene_depth, previous_view, delta_time, asynchronous,
+                         premultiplied, blend_over, out):
         entities = list(entities)
-        first = check_entities(entities)
+        first = check(entities)
         code, dtype, ch = self.FORMATS[fmt]
         if out is None:
             out = np.empty((view.height, view.width, ch), dtype)
         assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
         args = self._entities_args(entities, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over)
         zd = self._scene_depth(scene_depth, view)
-        self._check(self._lib.bgs_render_entities_ex(self._ctx, *args, None if zd is None else C.byref(zd), _ptr(out), code, 0))
+        self._check(getattr(self._lib, fn)(self._ctx, *args, None if zd is None else C.byref(zd), _ptr(out), code, 0))
         return out
 
     def render_entities_aux(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None,
@@ -589,15 +611,29 @@ class GaussianSplattingPlugin:
         largest blend weight w = a T, that w and the splat's depth d (BGS_PICK_NONE, 0, 0 where nothing blends).  rgba is
         byte for byte `render_entities`' frame.  Validates like `render_entities` (`check_entities`, ValueError before any
         call).  Synchronous only; `blend_over` applies to rgba only."""
+        return self._render_entities_pick("bgs_render_entities_pick", check_entities, entities, view, fmt, scene_depth,
+                                          previous_view, delta_time, premultiplied, blend_over)
+
+    def render_entities_pick_many(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None,
+                                  previous_view: View | None = None, delta_time: float | None = None,
+                                  premultiplied: bool = False, blend_over: bool = False) -> tuple[np.ndarray, np.ndarray]:
+        """`render_entities_pick` for any number of entities up to abi.BGS_ENTITIES_MANY_MAX
+        (`bgs_render_entities_pick_many`): a pick record's entity may exceed 63.  Validates with `check_entities_many`."""
+        return self._render_entities_pick("bgs_render_entities_pick_many",
+                                          lambda e: check_entities_many(e, "render_entities_pick_many"), entities, view, fmt,
+                                          scene_depth, previous_view, delta_time, premultiplied, blend_over)
+
+    def _render_entities_pick(self, fn: str, check, entities, view, fmt, scene_depth, previous_view, delta_time, premultiplied,
+                              blend_over):
         entities = list(entities)
-        first = check_entities(entities)
+        first = check(entities)
         code, dtype, ch = self.FORMATS[fmt]
         out = np.empty((view.height, view.width, ch), dtype)
         pick = np.empty((view.height, view.width), abi.PICK_DTYPE)
         args = self._entities_args(entities, first, view, previous_view, delta_time, False, premultiplied, blend_over)
         zd = self._scene_depth(scene_depth, view)
-        self._check(self._lib.bgs_render_entities_pick(self._ctx, *args, None if zd is None else C.byref(zd), _ptr(out), code, 0,
-                                                       _ptr(pick)))
+        self._check(getattr(self._lib, fn)(self._ctx, *args, None if zd is None else C.byref(zd), _ptr(out), code, 0,
+                                              _ptr(pick)))
         return out, pick
 
     def render_views(self, entities, views, fmt: str = "rgba32f", scene_depths=None, asynchronous: bool = False,

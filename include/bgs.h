@@ -931,6 +931,44 @@ bgs_status bgs_render_entities_pick(bgs_context* ctx, const bgs_cloud* const* cl
                                     void* out_rgba, uint32_t out_format, int out_is_device_ptr,
                                     void* out_pick /* w * h bgs_pick */);
 
+/* bgs_render_entities_ex and bgs_render_entities_pick for scenes of any number of entities: instanced vegetation, crowds
+ * and props (one resident cloud listed thousands of times under different transforms), glTF scenes whose meshes are placed
+ * by many nodes, and editor scenes of many objects, each drawn in ONE depth-sorted frame.  The capped calls pass the
+ * segment table as a kernel parameter (BGS_SCENE_MAX_CLOUDS segments fill most of it); these two keep it in device memory,
+ * copied there from pinned host staging once per frame.
+ *
+ * The rule, exactly:
+ *   Identity.  For every k in 1 .. BGS_ENTITIES_MANY_MAX, bgs_render_entities_many gives byte for byte the frame the rule
+ *     of bgs_render_entities_ex defines for the same arguments: pixels in all three formats and output modes, sorted
+ *     entries, tile ranges and slices, records, splat depths, bgs_frame_stats, chunked rounds, overlays, 4D entities at
+ *     their own times, mixed blend kinds, the depth test, and BGS_FLAG_ASYNC with its pair-overflow rule.
+ *     bgs_render_entities_pick_many is the same for bgs_render_entities_pick, its pick records included.  For k <=
+ *     BGS_SCENE_MAX_CLOUDS each equals the capped call, launch count included: the table's copy is a memory copy, not a
+ *     launch.
+ *   Index space.  Entity j's gaussians sit at global indices o_j + i (o_j: the gaussians of entities 0 .. j - 1), and
+ *     N < 2^30.  A pick record's entity is j, which may exceed 63.
+ *   Ordering.  Each distinct listed cloud is read after every write queued on it, as in scenes.  The context keeps two
+ *     tables, each reused and grown on demand: a call takes the one the last call with a table did not, after the frame
+ *     that last read it has completed (so at most two such frames are in flight; a third call waits on the host for the
+ *     first).  Neither a queued frame's table nor the one the debug hooks of the last frame read is ever overwritten.
+ *     A refused call takes no table: it neither waits nor allocates.
+ * Refused with BGS_EINVAL, nothing enqueued or written and the previous frame's debug hooks kept: k == 0 or k >
+ *   BGS_ENTITIES_MANY_MAX; N >= 2^30; BGS_FLAG_SORT_ALL; a NULL clouds[j]; every refusal bgs_render_entities_ex /
+ *   bgs_render_entities_pick makes for some entity, its message naming the entity ("entities[j]: ...").  NULL clouds,
+ *   uniforms, entities, view or frame -> BGS_NOT_READY. */
+#define BGS_ENTITIES_MANY_MAX 65536u
+bgs_status bgs_render_entities_many(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                                    const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */,
+                                    uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                                    const bgs_render_extras* extras, const bgs_scene_depth* depth /* may be NULL */,
+                                    void* out_rgba, uint32_t out_format, int out_is_device_ptr);
+bgs_status bgs_render_entities_pick_many(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                                         const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */,
+                                         uint32_t k, const bgs_view* view, const bgs_settings* frame,
+                                         const bgs_render_extras* extras, const bgs_scene_depth* depth /* may be NULL */,
+                                         void* out_rgba, uint32_t out_format, int out_is_device_ptr,
+                                         void* out_pick /* w * h bgs_pick */);
+
 /* bgs_render_entities_ex of several views of one scene in ONE frame: stereo eyes, the six faces of a cube map, split-screen
  * and picture-in-picture cameras, or many cameras of a dataset share one key-gen, depth sort, projection, binning,
  * tile-id sort and blend launch instead of one set of launches per view (the reference renders every GaussianCamera).

@@ -457,6 +457,31 @@ public:
                                             out_is_device ? 1 : 0, out_pick);
         });
     }
+    // render_entities and render_entities_pick for any number of entities up to BGS_ENTITIES_MANY_MAX
+    // (bgs_render_entities_many, _pick_many): the same frames, for instanced clouds, glTF scenes with many node placements or
+    // editor scenes of many objects.  The arguments are theirs.
+    bool render_entities_many(const std::vector<SceneEntity>& entities, const bgs_view& view, void* out_rgba,
+                              uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr,
+                              float delta_time = 0.0f, const float* depth = nullptr, uint64_t pitch_bytes = 0,
+                              bool out_is_device = false, uint32_t extra_flags = 0) {
+        return entities_call(entities, previous_view, delta_time, extra_flags, [&](const EntitiesArgs& a) {
+            const bgs_scene_depth zd{depth, pitch_bytes};
+            return bgs_render_entities_many(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(),
+                                            (uint32_t)a.clouds.size(), &view, &a.s, a.ex, depth ? &zd : nullptr, out_rgba, format,
+                                            out_is_device ? 1 : 0);
+        });
+    }
+    void render_entities_pick_many(const std::vector<SceneEntity>& entities, const bgs_view& view, void* out_rgba, void* out_pick,
+                                   uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr,
+                                   float delta_time = 0.0f, const float* depth = nullptr, uint64_t pitch_bytes = 0,
+                                   bool out_is_device = false, uint32_t extra_flags = 0) {
+        entities_call(entities, previous_view, delta_time, extra_flags, [&](const EntitiesArgs& a) {
+            const bgs_scene_depth zd{depth, pitch_bytes};
+            return bgs_render_entities_pick_many(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(),
+                                                 (uint32_t)a.clouds.size(), &view, &a.s, a.ex, depth ? &zd : nullptr, out_rgba,
+                                                 format, out_is_device ? 1 : 0, out_pick);
+        });
+    }
     // render_entities of each of `views` in one frame (bgs_render_views): out_rgba[i] receives views[i]'s frame, byte for
     // byte render_entities' frame of that view.  depths: one buffer per view (pitches[i] its row pitch), or empty.  No
     // extras: Depth and OpticalFlow entities are refused.
