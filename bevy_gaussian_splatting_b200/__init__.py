@@ -14,7 +14,7 @@ from .khr import (GaussianScene, KhrAccessor, KhrPrimitive, KhrSpec, SceneBundle
 from .gcloud import decode_gcloud, encode_gcloud, read_gcloud, write_gcloud  # noqa: F401
 from .particles import (PARTICLE_BEHAVIOR_DTYPE, PARTICLE_INACTIVE, ParticleBehaviors,  # noqa: F401
                         random_particle_behaviors)
-from .plugin import (CloudTransform, GaussianSplattingPlugin, ParticleBehaviorsHandle, PlanarGaussian3dHandle,  # noqa: F401
-                     PlanarGaussian4dHandle, SceneHandles, similarity_transform)
+from .plugin import (CloudTransform, EntityList, GaussianSplattingPlugin, ParticleBehaviorsHandle,  # noqa: F401
+                     PlanarGaussian3dHandle, PlanarGaussian4dHandle, SceneHandles, similarity_transform)
 from .settings import (CloudSettings, DrawMode, GaussianColorSpace, GaussianMode, PlaybackMode,  # noqa: F401
                        RadixSortDepthBits, RasterizeMode, ShaderDefines, SortMode, SparseSelect, playback_update)

@@ -28,6 +28,7 @@ BGS_FLAG_VISUALIZE_BOUNDING_BOX = 64
 BGS_ENTITY_VISUALIZE_BOUNDING_BOX = 1
 BGS_SCENE_MAX_CLOUDS = 64
 BGS_ENTITIES_MANY_MAX = 65536
+BGS_MATRIX_COLUMN_MAJOR, BGS_MATRIX_ROW_MAJOR = 0, 1
 BGS_SELECT_REPLACE, BGS_SELECT_ADD = 0, 1
 BGS_TRANSFORM_ALL, BGS_TRANSFORM_SELECTED = 0, 1
 BGS_PICK_NONE = 0xFFFFFFFF
@@ -232,6 +233,18 @@ SYMBOLS = [
                                                 C.c_uint32, C.POINTER(bgs_view), C.POINTER(bgs_settings),
                                                 C.POINTER(bgs_render_extras), C.POINTER(bgs_scene_depth), _P, C.c_uint32,
                                                 C.c_int, _P]),
+    ("bgs_entity_list_create", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P, C.c_uint32,
+                                         C.POINTER(_P)]),
+    ("bgs_entity_list_set", C.c_int, [_P, _P, C.c_uint32, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P]),
+    ("bgs_entity_list_append", C.c_int, [_P, C.c_uint32, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P]),
+    ("bgs_entity_list_truncate", C.c_int, [_P, C.c_uint32]),
+    ("bgs_entity_list_set_transforms", C.c_int, [_P, C.c_uint32, C.c_uint32, _P, C.c_uint32, C.c_int]),
+    ("bgs_entity_list_size", C.c_uint32, [_P]),
+    ("bgs_entity_list_destroy", None, [_P]),
+    ("bgs_render_entity_list", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_settings), C.POINTER(bgs_render_extras),
+                                         C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int]),
+    ("bgs_render_entity_list_pick", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_settings), C.POINTER(bgs_render_extras),
+                                              C.POINTER(bgs_scene_depth), _P, C.c_uint32, C.c_int, _P]),
     ("bgs_render_views", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P, C.c_uint32,
                                    C.POINTER(bgs_view), C.c_uint32, C.POINTER(bgs_settings), C.POINTER(bgs_scene_depth), _P,
                                    C.c_uint32, C.c_int]),

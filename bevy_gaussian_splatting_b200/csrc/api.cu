@@ -16,6 +16,7 @@ namespace bgs {
 
 std::mutex g_registry_mu;
 std::vector<bgs_context*> g_contexts;
+std::vector<bgs_entity_list*> g_lists;
 
 bgs_status fail(bgs_context* ctx, bgs_status st, const char* fmt, ...) {
     if (ctx) {
@@ -55,6 +56,16 @@ bgs_status ensure_status(bgs_context* c, DevBuf<void>& rows, uint32_t& rows_capa
     TRY(rows.grow(c, (size_t)4 * radix_num_tiles(capacity) * 256 * 8, true));
     rows_capacity = capacity;
     return BGS_OK;
+}
+
+void detach_listed_cloud(const bgs_cloud* cl) {
+    for (bgs_entity_list* l : g_lists) {
+        const auto it = l->clouds.find(cl);
+        if (it == l->clouds.end()) continue;
+        l->clouds.erase(it);
+        for (ListEntity& x : l->ent)
+            if (x.cloud == cl) { x.cloud = nullptr; ++l->detached; }
+    }
 }
 
 uint32_t next_epoch(bgs_context* c) {
@@ -290,27 +301,9 @@ namespace bgs {
 
 FrameConsts frame_consts(const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
                                 const bgs_settings* st, bool want_aux) {
-    const int W = (int)view->viewport[2], H = (int)view->viewport[3];
-    FrameConsts fc;
-    memcpy(fc.model, uni->transform, 64);
-    memcpy(fc.view_from_world, view->view_from_world, 64);
-    memcpy(fc.clip_from_world, view->clip_from_world, 64);
-    memcpy(fc.cam, view->world_position, 12);
-    fc.W = view->viewport[2]; fc.H = view->viewport[3];
-    fc.p00 = view->clip_from_view[0]; fc.p11 = view->clip_from_view[5];
-    fc.global_opacity = uni->global_opacity; fc.global_scale = uni->global_scale;
-    fc.color_space = uni->color_space;
-    fc.key_shift = 32u - st->radix_sort_depth_bits;
-    fc.gaussian_mode = st->gaussian_mode; fc.rasterize_mode = st->rasterize_mode; fc.aabb = st->aabb;
-    fc.adaptive = st->opacity_adaptive_radius; fc.draw_mode = st->draw_mode;
-    fc.Wi = W; fc.Hi = H; fc.tiles_x = (W + TILE_PX - 1) / TILE_PX; fc.tiles_y = (H + TILE_PX - 1) / TILE_PX;
-    fc.n_cloud = cloud->n;
-    fc.aux = want_aux ? 1u : 0u;
-    fc.cov_pre = cloud->layout == CloudLayout::F16Cov ? 1u : 0u;
-    memcpy(fc.aabb_min, uni->aabb_min, 12); memcpy(fc.aabb_max, uni->aabb_max, 12);
-    static const float kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    fc.model_identity = memcmp(uni->transform, kIdentity, 64) == 0 ? 1u : 0u;   // (-0.0 entries take the general path)
-    return fc;
+    return make_frame_consts(*view, *uni, st->radix_sort_depth_bits, st->gaussian_mode, st->rasterize_mode, st->aabb,
+                             st->opacity_adaptive_radius, st->draw_mode, cloud->n,
+                             cloud->layout == CloudLayout::F16Cov ? 1u : 0u, want_aux ? 1u : 0u);
 }
 
 }  // namespace bgs
@@ -376,12 +369,26 @@ bgs_status bgs_context_create(int cuda_device, bgs_context** out) {
 
 void bgs_context_destroy(bgs_context* c) {
     if (!c) return;
+    // its lists refuse every later call; their device arrays go once the context's streams are drained
+    std::vector<std::shared_ptr<ListTable>> tables;
+    std::vector<void*> uploads;
     {
         std::lock_guard<std::mutex> lk(g_registry_mu);
         g_contexts.erase(std::remove(g_contexts.begin(), g_contexts.end(), c), g_contexts.end());
+        for (bgs_entity_list* l : g_lists)
+            if (l->ctx == c) {
+                tables.push_back(std::move(l->cur));
+                tables.push_back(std::move(l->spare));
+                uploads.push_back(l->upload.p);
+                l->upload.p = nullptr;
+                l->upload.bytes = 0;
+                l->ctx = nullptr;
+            }
     }
     cudaSetDevice(c->device);
     c->each_stream([](cudaStream_t& s, int) { if (s) cudaStreamSynchronize(s); });
+    tables.clear();
+    for (void* u : uploads) cudaFree(u);
     c->each_event([](cudaEvent_t& ev, bool) { if (ev) cudaEventDestroy(ev); });
     c->each_stream([](cudaStream_t& s, int) { if (s) cudaStreamDestroy(s); });
     if (c->h_ctr) cudaFreeHost(c->h_ctr);
@@ -465,18 +472,37 @@ bgs_status bgs_sync(bgs_context* c) {
     return gs;
 }
 
-static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
-                               const bgs_settings* st, const bgs_render_extras* ex, uint32_t out_format, bool want_aux,
-                               bool temporal, bool set_device = true) {
-    // not-ready inputs map to the reference's silent skip-frame (radix.rs:645-658, mod.rs:1533-1539)
-    if (!cloud || !view || !uni || !st) return fail(c, BGS_NOT_READY, "render: cloud/view/uniform/settings not ready");
-    // (contexts of one GPU may share clouds; a scene's entities after its first only check the device, which the first
-    // made current)
-    if (set_device) TRY(enter_call(c, "render", cloud->device));
-    else if (cloud->device != c->device) return fail(c, BGS_EINVAL, "render: cloud lives on another device");
+// check_render's refusals of the frame's format and sort bits
+static bgs_status check_frame_bits(bgs_context* c, const bgs_settings* st, uint32_t out_format) {
     if (out_format > BGS_FORMAT_RGBA32F) return fail(c, BGS_EINVAL, "render: unknown out_format %u", out_format);
     if (st->radix_sort_depth_bits != 16 && st->radix_sort_depth_bits != 24 && st->radix_sort_depth_bits != 32)
         return fail(c, BGS_EINVAL, "render: radix_sort_depth_bits must be 16, 24 or 32");
+    return BGS_OK;
+}
+
+// ... of an OpticalFlow frame's extras
+static bgs_status check_flow_extras(bgs_context* c, const bgs_render_extras* ex) {
+    if (!ex) return fail(c, BGS_EINVAL, "render: OpticalFlow needs the previous view (bgs_render_ex extras)");
+    if (!(std::isfinite(ex->delta_time) && ex->delta_time > 0.0f))
+        return fail(c, BGS_EINVAL, "render: OpticalFlow delta_time %g is not finite and > 0", (double)ex->delta_time);
+    for (int i = 0; i < 16; ++i)
+        if (!std::isfinite(ex->previous_clip_from_world[i]))
+            return fail(c, BGS_EINVAL, "render: previous_clip_from_world[%d] is not finite", i);
+    return BGS_OK;
+}
+
+// ... of the view
+static bgs_status check_viewport(bgs_context* c, const bgs_view* view) {
+    const int W = (int)view->viewport[2], H = (int)view->viewport[3];
+    if (W <= 0 || H <= 0 || W > 65535 || H > 65535) return fail(c, BGS_EINVAL, "render: viewport %dx%d out of range", W, H);
+    return BGS_OK;
+}
+
+// ... of the cloud's layout and the settings (ex: the extras as the call reads them, NULL for none), which depend on
+// nothing else but the OpticalFlow extras, checked only with `flow` (bgs_entity_list checks an entity's settings at the
+// edit, and the frame's extras when it renders)
+static bgs_status check_settings(bgs_context* c, const bgs_cloud* cloud, const bgs_settings* st, const bgs_render_extras* ex,
+                                 bool want_aux, bool temporal, bool flow) {
     if (temporal) {
         if (!is_4d(cloud->layout)) return fail(c, BGS_EINVAL, "render_4d: the cloud is not a Gaussian4d cloud (bgs_cloud_upload_4d)");
         if (st->gaussian_mode != BGS_GAUSSIAN_4D)
@@ -494,20 +520,25 @@ static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs
         return fail(c, BGS_EINVAL, "render_aux: Classification and OpticalFlow frames take extras: use bgs_render_ex");
     if (st->rasterize_mode == BGS_RASTERIZE_CLASSIFICATION && ex && ex->num_classes == 0)
         return fail(c, BGS_EINVAL, "render: Classification with num_classes = 0");
-    if (st->rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW) {
-        if (!ex) return fail(c, BGS_EINVAL, "render: OpticalFlow needs the previous view (bgs_render_ex extras)");
-        if (!(std::isfinite(ex->delta_time) && ex->delta_time > 0.0f))
-            return fail(c, BGS_EINVAL, "render: OpticalFlow delta_time %g is not finite and > 0", (double)ex->delta_time);
-        for (int i = 0; i < 16; ++i)
-            if (!std::isfinite(ex->previous_clip_from_world[i]))
-                return fail(c, BGS_EINVAL, "render: previous_clip_from_world[%d] is not finite", i);
-    }
+    if (flow && st->rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW) TRY(check_flow_extras(c, ex));
     if (st->draw_mode > BGS_DRAW_HIGHLIGHT_SELECTED) return fail(c, BGS_EINVAL, "render: bad draw_mode");
     if (cloud->layout == CloudLayout::F16Cov && (st->gaussian_mode != BGS_GAUSSIAN_3D || st->rasterize_mode == BGS_RASTERIZE_NORMAL || want_aux))
         return fail(c, BGS_EINVAL, "render: a precomputed-covariance cloud has no rotation / scale: Gaussian3d with Color, Depth or Position only");
-    const int W = (int)view->viewport[2], H = (int)view->viewport[3];
-    if (W <= 0 || H <= 0 || W > 65535 || H > 65535) return fail(c, BGS_EINVAL, "render: viewport %dx%d out of range", W, H);
     return BGS_OK;
+}
+
+static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs_view* view, const bgs_cloud_uniform* uni,
+                               const bgs_settings* st, const bgs_render_extras* ex, uint32_t out_format, bool want_aux,
+                               bool temporal, bool set_device = true) {
+    // not-ready inputs map to the reference's silent skip-frame (radix.rs:645-658, mod.rs:1533-1539)
+    if (!cloud || !view || !uni || !st) return fail(c, BGS_NOT_READY, "render: cloud/view/uniform/settings not ready");
+    // (contexts of one GPU may share clouds; a scene's entities after its first only check the device, which the first
+    // made current)
+    if (set_device) TRY(enter_call(c, "render", cloud->device));
+    else if (cloud->device != c->device) return fail(c, BGS_EINVAL, "render: cloud lives on another device");
+    TRY(check_frame_bits(c, st, out_format));
+    TRY(check_settings(c, cloud, st, ex, want_aux, temporal, true));
+    return check_viewport(c, view);
 }
 
 
@@ -529,7 +560,14 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     }
     const bool many = scene && scene->many;   // (bgs_render_entities_many: the segment table in device memory)
     const SceneTableDev* dt = many ? &scene->dtab : nullptr;
-    if (many) CU(c, cudaMemcpyAsync(c->many[scene->slot].dev.p, scene->h_tab, scene->tab_bytes, cudaMemcpyHostToDevice, q));
+    if (many && scene->list_tab) {   // (bgs_render_entity_list: the segments from the list's records and the view)
+        const ListTable& lt = *scene->list_tab;
+        CU(c, launch_entity_list_expand(lt.a.recs, lt.a.offset, dt->k, scene->list_view, scene->list_depth_bits, dt->n_total,
+                                        lt.seg, q));
+        ++launches;
+    } else if (many) {
+        CU(c, cudaMemcpyAsync(c->many[scene->slot].dev.p, scene->h_tab, scene->tab_bytes, cudaMemcpyHostToDevice, q));
+    }
     CU(c, cudaMemsetAsync(c->arena.p, 0, c->arena.bytes, q));   // counters, histograms, ranges: ~0.4 MB
     CU(c, cudaEventRecord(c->ev[0], q));
     // ---- stage 1: key-gen (+ stable compaction of the visible set)
@@ -714,7 +752,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     c->pair_result = pcur;
     CU(c, cudaEventRecord(c->ev[5], q));
     CU(c, cudaEventRecord(c->ev_done, q));
-    if (many) {   // (the table's last reader is the blend, which the render stream has joined)
+    if (many && !scene->list_tab) {   // (the table's last reader is the blend, which the render stream has joined)
         CU(c, cudaEventRecord(c->many[scene->slot].ev, q));
         c->many[scene->slot].used = true;
         c->many_last = scene->slot;
@@ -1243,6 +1281,388 @@ bgs_status bgs_render_entities_pick_many(bgs_context* c, const bgs_cloud* const*
     const Targets t{out_format, out_is_device_ptr, 1, false, &out_rgba, nullptr, nullptr, out_pick};
     TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, view, frame, t, false, true, BGS_ENTITIES_MANY_MAX));
     return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, view, frame, ex, depth, t, true);
+}
+
+// ---- bgs_entity_list (include/bgs.h): a resident entity list, edited in place, rendered as bgs_render_entities_many
+
+// entity j of an edit as bgs_render_entities_many checks it, in so far as the check depends on the entity alone (the frame's
+// format, sort bits, view and OpticalFlow extras are the render call's); x and r its host facts and device record
+static bgs_status list_entity(bgs_context* c, const char* call, uint32_t j, const bgs_cloud* cl, const bgs_cloud_uniform& u,
+                              const bgs_entity_settings& e, uint32_t flags, ListEntity& x, EntityRec& r, TemporalConsts& tc) {
+    if (!cl) return fail(c, BGS_EINVAL, "%s: entities[%u]: the cloud is NULL", call, j);
+    if (flags & ~(uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX)
+        return fail(c, BGS_EINVAL, "%s: entities[%u]: entity flags 0x%x have an unknown bit", call, j, flags);
+    if (cl->device != c->device) return entity_refusal(c, fail(c, BGS_EINVAL, "render: cloud lives on another device"), call, j);
+    const bool is4 = is_4d(cl->layout);
+    bgs_settings chk = {};   // (a non-4D entity in Velocity is undrawn, and checked as a Color one)
+    chk.gaussian_mode = e.gaussian_mode; chk.aabb = e.aabb; chk.opacity_adaptive_radius = e.opacity_adaptive_radius;
+    chk.draw_mode = e.draw_mode;
+    chk.rasterize_mode = !is4 && e.rasterize_mode == BGS_RASTERIZE_VELOCITY ? (uint32_t)BGS_RASTERIZE_COLOR : e.rasterize_mode;
+    bgs_render_extras ej = {};
+    ej.num_classes = e.num_classes;
+    const bgs_status s = check_settings(c, cl, &chk, &ej, false, is4, false);
+    if (s != BGS_OK) return entity_refusal(c, s, call, j);
+    tc = {};
+    if (is4) {
+        const bgs_status st = temporal_consts(c, call, u.time, e.window.time_start, e.window.time_stop, tc);
+        if (st != BGS_OK) return entity_refusal(c, st, call, j);
+    }
+    uint32_t group = project_group(cl->layout, cl->sh_degree);
+    if (group != PROJECT_GROUP_4D && e.rasterize_mode >= BGS_RASTERIZE_CLASSIFICATION) group |= ENTITY_MODES;
+    const bool sh = e.rasterize_mode == ((group & ENTITY_MODES) ? BGS_RASTERIZE_CLASSIFICATION : BGS_RASTERIZE_COLOR);
+    x = ListEntity{cl, u, e, flags, cl->n, group, 0u, sh, is4};
+    r = EntityRec{u, e.gaussian_mode, e.rasterize_mode, e.aabb, e.opacity_adaptive_radius, e.draw_mode, cl->n, group,
+                  cl->layout == CloudLayout::F16Cov ? 1u : 0u, cl->pos, cl->blocks};
+    return BGS_OK;
+}
+
+// the key render_entities_impl's Velocity refusal compares entities by (box: the entity's overlay bit as the frame sees it)
+static std::array<uint32_t, 5> velocity_key(const ListEntity& x, bool box) {
+    return {x.e.gaussian_mode, x.e.aabb, x.e.opacity_adaptive_radius, x.e.draw_mode, box ? 1u : 0u};
+}
+
+// adds (d = +1) or removes (d = -1) entity x's share of the list's counters
+static void list_count(bgs_entity_list* l, const ListEntity& x, int d) {
+    auto bump = [d](uint32_t& v) { v = (uint32_t)((int64_t)v + d); };
+    if (x.cloud) {
+        if ((l->clouds[x.cloud] += (uint32_t)d) == 0) l->clouds.erase(x.cloud);
+    } else {
+        bump(l->detached);
+    }
+    std::array<uint32_t, 2>& g = l->groups[x.group];
+    bump(g[0]);
+    if (x.sh) bump(g[1]);
+    if (g[0] == 0) l->groups.erase(x.group);
+    bump(l->kinds[blend_kind(x.e)]);
+    const bool boxed = (x.flags & BGS_ENTITY_VISUALIZE_BOUNDING_BOX) != 0;
+    if (boxed) bump(l->boxed);
+    if (x.e.rasterize_mode == BGS_RASTERIZE_DEPTH) bump(l->depth);
+    if (x.e.rasterize_mode == BGS_RASTERIZE_OPTICAL_FLOW) bump(l->flow);
+    if (!x.is4 && x.e.rasterize_mode == BGS_RASTERIZE_VELOCITY)
+        for (int b = 0; b < 2; ++b) {
+            const auto key = velocity_key(x, b ? true : boxed);
+            if ((l->velocity[b][key] += (uint32_t)d) == 0) l->velocity[b].erase(key);
+        }
+    l->total = (uint64_t)((int64_t)l->total + d * (int64_t)x.n);
+}
+
+// the list's current generation, writable for entities [0, need): written in place when no frame holds it; else (or when
+// it is too small) the list moves to a generation no frame holds, a held one kept as the spare, with [0, size) copied
+// over on the context's stream (after every frame that read the generation it moves to)
+static bgs_status list_writable(bgs_entity_list* l, uint32_t need) {
+    bgs_context* c = l->ctx;
+    std::shared_ptr<ListTable>& cur = l->cur;
+    if (cur && cur.use_count() == 1 && cur->cap >= need) return BGS_OK;
+    std::shared_ptr<ListTable> next;
+    if (l->spare && l->spare.use_count() == 1 && l->spare->cap >= need) {
+        next = l->spare;
+    } else {
+        const uint32_t cap = std::max({need, 64u, cur ? std::min(2u * cur->cap, BGS_ENTITIES_MANY_MAX) : 0u});
+        next = std::make_shared<ListTable>();
+        Layout lay;
+        const size_t o_rec = lay.add((size_t)cap * sizeof(EntityRec)), o_off = lay.add((size_t)cap * 4);
+        const size_t o_t = lay.add((size_t)cap * sizeof(TemporalConsts)), o_cls = lay.add((size_t)cap * 4);
+        const size_t o_k = lay.add((size_t)cap * 4), o_kb = lay.add((size_t)cap * 4), o_seg = lay.add((size_t)cap * sizeof(SceneSeg));
+        TRY(next->mem.grow(c, lay.padded(), false));
+        uint8_t* m = next->mem.p;
+        next->cap = cap;
+        next->a = EntityListArrays{reinterpret_cast<EntityRec*>(m + o_rec), reinterpret_cast<uint32_t*>(m + o_off),
+                                   reinterpret_cast<TemporalConsts*>(m + o_t), reinterpret_cast<uint32_t*>(m + o_cls),
+                                   reinterpret_cast<uint32_t*>(m + o_k), reinterpret_cast<uint32_t*>(m + o_kb)};
+        next->seg = reinterpret_cast<SceneSeg*>(m + o_seg);
+    }
+    const size_t k = l->ent.size();
+    if (cur && k) {
+        const EntityListArrays &f = cur->a, &t = next->a;
+        cudaStream_t q = c->stream;
+        CU(c, cudaMemcpyAsync(t.recs, f.recs, k * sizeof(EntityRec), cudaMemcpyDeviceToDevice, q));
+        CU(c, cudaMemcpyAsync(t.offset, f.offset, k * 4, cudaMemcpyDeviceToDevice, q));
+        CU(c, cudaMemcpyAsync(t.times, f.times, k * sizeof(TemporalConsts), cudaMemcpyDeviceToDevice, q));
+        CU(c, cudaMemcpyAsync(t.classes, f.classes, k * 4, cudaMemcpyDeviceToDevice, q));
+        CU(c, cudaMemcpyAsync(t.kinds, f.kinds, k * 4, cudaMemcpyDeviceToDevice, q));
+        CU(c, cudaMemcpyAsync(t.kinds_box, f.kinds_box, k * 4, cudaMemcpyDeviceToDevice, q));
+    }
+    l->spare = cur && cur.use_count() > 1 ? cur : (next == l->spare ? nullptr : l->spare);
+    cur = next;
+    return BGS_OK;
+}
+
+// the edit of entities idx[0 .. count) (each < the size, distinct; idx == NULL: an append after the last entity) to the
+// given ones: every entity checked before anything changes, then the counters, the host facts and, in one upload and one
+// scatter, the device arrays; the offsets after the first entity whose gaussian count changed are rewritten (O(k))
+static bgs_status list_edit(bgs_entity_list* l, const char* call, const uint32_t* idx, uint32_t count,
+                            const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
+                            const uint32_t* entity_flags) {
+    if (!l || !l->ctx) return BGS_EINVAL;
+    bgs_context* c = l->ctx;
+    const uint32_t k = (uint32_t)l->ent.size();
+    if (!idx && (uint64_t)k + count > BGS_ENTITIES_MANY_MAX)
+        return fail(c, BGS_EINVAL, "%s: k = %llu entities, at most %u", call, (unsigned long long)k + count, BGS_ENTITIES_MANY_MAX);
+    if (count == 0) return BGS_OK;
+    if (!clouds || !unis || !ents) return fail(c, BGS_EINVAL, "%s: clouds/uniforms/entities is NULL", call);
+    CU(c, cudaSetDevice(c->device));
+    if (idx) {
+        std::vector<uint32_t> sorted(idx, idx + count);
+        std::sort(sorted.begin(), sorted.end());
+        if (sorted.back() >= k) return fail(c, BGS_EINVAL, "%s: index %u is not below k = %u", call, sorted.back(), k);
+        if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+            return fail(c, BGS_EINVAL, "%s: index %u is given twice", call, *std::adjacent_find(sorted.begin(), sorted.end()));
+    }
+    // the upload: idx | records | offsets | times | num_classes | kinds
+    Layout lay;
+    const size_t o_idx = lay.add((size_t)count * 4), o_rec = lay.add((size_t)count * sizeof(EntityRec));
+    const size_t o_off = lay.add((size_t)count * 4), o_t = lay.add((size_t)count * sizeof(TemporalConsts));
+    const size_t o_cls = lay.add((size_t)count * 4), o_k = lay.add((size_t)count * 4);
+    std::vector<uint8_t> up(lay.padded());
+    uint32_t* u_idx = reinterpret_cast<uint32_t*>(up.data() + o_idx);
+    EntityRec* u_rec = reinterpret_cast<EntityRec*>(up.data() + o_rec);
+    uint32_t* u_off = reinterpret_cast<uint32_t*>(up.data() + o_off);
+    TemporalConsts* u_t = reinterpret_cast<TemporalConsts*>(up.data() + o_t);
+    uint32_t* u_cls = reinterpret_cast<uint32_t*>(up.data() + o_cls);
+    uint32_t* u_k = reinterpret_cast<uint32_t*>(up.data() + o_k);
+    std::vector<ListEntity> xs(count);
+    int64_t total = (int64_t)l->total;
+    for (uint32_t i = 0; i < count; ++i) {
+        const uint32_t j = idx ? idx[i] : k + i;
+        const uint32_t f = entity_flags ? entity_flags[i] : 0u;
+        TRY(list_entity(c, call, j, clouds[i], unis[i], ents[i], f, xs[i], u_rec[i], u_t[i]));
+        u_idx[i] = j;
+        u_cls[i] = ents[i].num_classes;
+        u_k[i] = (uint32_t)blend_kind(ents[i]) | ((f & BGS_ENTITY_VISUALIZE_BOUNDING_BOX) ? BOX_KIND : 0u);
+        total += (int64_t)xs[i].n - (idx ? (int64_t)l->ent[j].n : 0);
+    }
+    if (total >= (1ll << 30)) return fail(c, BGS_EINVAL, "%s: N = %lld gaussians, must be < 2^30", call, (long long)total);
+    TRY(list_writable(l, k + (idx ? 0u : count)));
+    TRY(l->upload.grow(c, up.size(), false));
+    std::lock_guard<std::mutex> lk(g_registry_mu);   // (bgs_cloud_destroy detaches entities under it)
+    uint32_t moved = k;   // the first entity whose gaussian count changed
+    if (!idx) l->ent.resize(k + count);
+    for (uint32_t i = 0; i < count; ++i) {
+        const uint32_t j = u_idx[i];
+        if (idx) {
+            if (l->ent[j].n != xs[i].n) moved = std::min(moved, j);
+            list_count(l, l->ent[j], -1);
+        }
+        xs[i].offset = idx ? l->ent[j].offset : (uint32_t)(j ? l->ent[j - 1].offset + l->ent[j - 1].n : 0u);
+        l->ent[j] = xs[i];
+        list_count(l, xs[i], +1);
+    }
+    std::vector<uint32_t> offsets;
+    if (moved < k) {
+        for (uint32_t j = moved; j < (uint32_t)l->ent.size(); ++j) {
+            l->ent[j].offset = j ? l->ent[j - 1].offset + l->ent[j - 1].n : 0u;
+            offsets.push_back(l->ent[j].offset);
+        }
+    }
+    for (uint32_t i = 0; i < count; ++i) u_off[i] = l->ent[u_idx[i]].offset;
+    cudaStream_t q = c->stream;
+    // (pageable sources: each copy has taken its bytes when it returns, so the vectors may go)
+    CU(c, cudaMemcpyAsync(l->upload.p, up.data(), up.size(), cudaMemcpyHostToDevice, q));
+    const uint8_t* d = l->upload.p;
+    const EntityListUpload u{reinterpret_cast<const uint32_t*>(d + o_idx), reinterpret_cast<const EntityRec*>(d + o_rec),
+                             reinterpret_cast<const uint32_t*>(d + o_off), reinterpret_cast<const TemporalConsts*>(d + o_t),
+                             reinterpret_cast<const uint32_t*>(d + o_cls), reinterpret_cast<const uint32_t*>(d + o_k)};
+    CU(c, launch_entity_list_scatter(u, count, l->cur->a, q));
+    if (!offsets.empty())
+        CU(c, cudaMemcpyAsync(l->cur->a.offset + moved, offsets.data(), offsets.size() * 4, cudaMemcpyHostToDevice, q));
+    return BGS_OK;
+}
+
+bgs_status bgs_entity_list_create(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                                  const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k,
+                                  bgs_entity_list** out) {
+    if (!c || !out) return BGS_EINVAL;
+    *out = nullptr;
+    bgs_entity_list* l = new (std::nothrow) bgs_entity_list();
+    if (!l) return fail(c, BGS_ENOMEM, "entity_list_create: out of host memory");
+    l->ctx = c;
+    const bgs_status s = list_edit(l, "entity_list_create", nullptr, k, clouds, unis, ents, entity_flags);
+    if (s != BGS_OK) {
+        delete l;
+        return s;
+    }
+    std::lock_guard<std::mutex> lk(g_registry_mu);
+    g_lists.push_back(l);
+    *out = l;
+    return BGS_OK;
+}
+
+bgs_status bgs_entity_list_set(bgs_entity_list* l, const uint32_t* indices, uint32_t count, const bgs_cloud* const* clouds,
+                               const bgs_cloud_uniform* unis, const bgs_entity_settings* ents, const uint32_t* entity_flags) {
+    if (!l || !l->ctx) return BGS_EINVAL;
+    if (count && !indices) return fail(l->ctx, BGS_EINVAL, "entity_list_set: indices is NULL");
+    return list_edit(l, "entity_list_set", count ? indices : nullptr, count, clouds, unis, ents, entity_flags);
+}
+
+bgs_status bgs_entity_list_append(bgs_entity_list* l, uint32_t count, const bgs_cloud* const* clouds,
+                                  const bgs_cloud_uniform* unis, const bgs_entity_settings* ents, const uint32_t* entity_flags) {
+    return list_edit(l, "entity_list_append", nullptr, count, clouds, unis, ents, entity_flags);
+}
+
+bgs_status bgs_entity_list_truncate(bgs_entity_list* l, uint32_t k) {
+    if (!l || !l->ctx) return BGS_EINVAL;
+    if (k > l->ent.size()) return fail(l->ctx, BGS_EINVAL, "entity_list_truncate: k = %u is above the size %zu", k, l->ent.size());
+    std::lock_guard<std::mutex> lk(g_registry_mu);
+    for (size_t j = k; j < l->ent.size(); ++j) list_count(l, l->ent[j], -1);
+    l->ent.resize(k);   // (the device arrays past k are not read)
+    return BGS_OK;
+}
+
+bgs_status bgs_entity_list_set_transforms(bgs_entity_list* l, uint32_t first, uint32_t count, const float* m, uint32_t layout,
+                                          int is_device_ptr) {
+    const char* call = "entity_list_set_transforms";
+    if (!l || !l->ctx) return BGS_EINVAL;
+    bgs_context* c = l->ctx;
+    if ((uint64_t)first + count > l->ent.size())
+        return fail(c, BGS_EINVAL, "%s: [%u, %llu) is beyond the size %zu", call, first, (unsigned long long)first + count, l->ent.size());
+    if (layout != BGS_MATRIX_COLUMN_MAJOR && layout != BGS_MATRIX_ROW_MAJOR) return fail(c, BGS_EINVAL, "%s: unknown layout %u", call, layout);
+    if (count == 0) return BGS_OK;
+    if (!m) return fail(c, BGS_EINVAL, "%s: m is NULL", call);
+    CU(c, cudaSetDevice(c->device));
+    if (is_device_ptr) {
+        cudaPointerAttributes a = {};
+        const cudaError_t e = cudaPointerGetAttributes(&a, m);
+        if (e != cudaSuccess) cudaGetLastError();   // (an unknown pointer: clear the error, refuse below)
+        if (e != cudaSuccess || a.type != cudaMemoryTypeDevice || a.device != c->device)
+            return fail(c, BGS_EINVAL, "%s: m = %p is not device memory of device %d", call, (const void*)m, c->device);
+    }
+    TRY(list_writable(l, (uint32_t)l->ent.size()));
+    cudaStream_t q = c->stream;
+    const size_t bytes = (size_t)count * 64;
+    const float* src = m;
+    if (!is_device_ptr) {
+        // host matrices go through the upload buffer from a copy of the library's own, so the caller's array (pageable or
+        // pinned) may be reused once the call returns
+        TRY(l->upload.grow(c, bytes, false));
+        const std::vector<float> staged(m, m + (size_t)count * 16);
+        CU(c, cudaMemcpyAsync(l->upload.p, staged.data(), bytes, cudaMemcpyHostToDevice, q));   // (pageable: taken on return)
+        src = reinterpret_cast<const float*>(l->upload.p);
+    }
+    EntityRec* dst = l->cur->a.recs + first;
+    if (layout == BGS_MATRIX_ROW_MAJOR) CU(c, launch_entity_list_transforms(src, count, dst, q));
+    else CU(c, cudaMemcpy2DAsync(dst->uni.transform, sizeof(EntityRec), src, 64, 64, count, cudaMemcpyDeviceToDevice, q));
+    if (!is_device_ptr)   // (once nothing can fail)
+        for (uint32_t i = 0; i < count; ++i)
+            for (int e = 0; e < 16; ++e)
+                l->ent[first + i].uni.transform[e] = layout == BGS_MATRIX_ROW_MAJOR ? m[i * 16 + (e & 3) * 4 + (e >> 2)] : m[i * 16 + e];
+    return BGS_OK;
+}
+
+uint32_t bgs_entity_list_size(const bgs_entity_list* l) { return l ? (uint32_t)l->ent.size() : 0u; }
+
+void bgs_entity_list_destroy(bgs_entity_list* l) {
+    if (!l) return;
+    {
+        std::lock_guard<std::mutex> lk(g_registry_mu);
+        g_lists.erase(std::remove(g_lists.begin(), g_lists.end(), l), g_lists.end());
+        if (bgs_context* c = l->ctx) {
+            cudaSetDevice(c->device);
+            if (c->async_pending) c->each_stream([](cudaStream_t& s, int) { cudaStreamSynchronize(s); });
+            for (FrameFacts* f : {&c->pend, &c->last})
+                if (f->scene && f->scene->list == l) {
+                    if (f == &c->last) c->have_frame = false;
+                    f->forget();
+                    f->n = 0;
+                }
+        }
+    }
+    delete l;   // (its generations go once no frame holds them)
+}
+
+// bgs_render_entity_list and _pick: the refusals bgs_render_entities_many / _pick_many would make of the list that depend
+// on the frame, then the frame's facts from the list's counters and its expansion over the list's current generation
+static bgs_status render_list_impl(bgs_context* c, const char* call, const bgs_entity_list* l, const bgs_view* view,
+                                   const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
+                                   const Targets& t) {
+    if (!c || !l) return BGS_EINVAL;
+    if (l->ctx != c) return fail(c, BGS_EINVAL, "%s: the list belongs to another context", call);
+    if (!view || !frame) return fail(c, BGS_NOT_READY, "%s: view/settings not ready", call);
+    const uint32_t k = (uint32_t)l->ent.size();
+    if (k == 0) return fail(c, BGS_EINVAL, "%s: k = 0 is not in 1..%u", call, BGS_ENTITIES_MANY_MAX);
+    if (frame->flags & BGS_FLAG_SORT_ALL) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_SORT_ALL is not supported", call);
+    CU(c, cudaSetDevice(c->device));
+    auto scene = std::make_shared<SceneFacts>();
+    const bool box_frame = (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0;
+    bool undrawn;
+    {
+        std::lock_guard<std::mutex> lk(g_registry_mu);   // (the counters, against a detaching bgs_cloud_destroy)
+        if (l->detached) {
+            uint32_t j = 0;
+            while (l->ent[j].cloud) ++j;
+            return fail(c, BGS_EINVAL, "%s: entities[%u]: its cloud was destroyed (bgs_entity_list_set replaces it)", call, j);
+        }
+        const ListEntity& x0 = l->ent[0];
+        undrawn = !x0.is4 && x0.e.rasterize_mode == BGS_RASTERIZE_VELOCITY;
+        if (undrawn) {
+            const auto& counts = l->velocity[box_frame ? 1 : 0];
+            const auto it = counts.find(velocity_key(x0, box_frame || (x0.flags & BGS_ENTITY_VISUALIZE_BOUNDING_BOX)));
+            undrawn = it != counts.end() && it->second == k;
+        }
+        for (const auto& cl : l->clouds) scene->distinct.push_back(cl.first);
+        for (const auto& g : l->groups) {
+            scene->groups.push_back(g.first);
+            scene->need_sh.push_back(g.second[1] ? 1u : 0u);
+        }
+        scene->box = box_frame || l->boxed > 0;
+        const bool box_all = box_frame || l->boxed == k;
+        const uint32_t kinds = (l->kinds[0] ? 1u : 0u) | (l->kinds[1] ? 2u : 0u) | (l->kinds[2] ? 4u : 0u);
+        scene->raster_mode = __builtin_popcount(kinds) > 1 || box_all != scene->box ? ((kinds & 4u) ? 4 : 3) : __builtin_ctz(kinds);
+        // segment 0 as the host keeps it: render_impl and enqueue_frame read only its frame-wide fields (view, tiles, sort
+        // bits, aux) and its rasterize_mode, never the transform, which may have been set from device memory since
+        SceneSeg& s0 = scene->tab.seg[0];
+        bgs_settings st0 = *frame;
+        st0.gaussian_mode = x0.e.gaussian_mode; st0.rasterize_mode = x0.e.rasterize_mode; st0.aabb = x0.e.aabb;
+        st0.opacity_adaptive_radius = x0.e.opacity_adaptive_radius; st0.draw_mode = x0.e.draw_mode;
+        TRY(check_frame_bits(c, frame, t.format));
+        TRY(check_viewport(c, view));
+        s0.fc = frame_consts(x0.cloud, view, &x0.uni, &st0, false);
+        s0.fc.n_cloud = (uint32_t)l->total;
+        s0.pos = x0.cloud->pos; s0.blocks = x0.cloud->blocks; s0.offset = 0; s0.n = x0.n; s0.group = x0.group;
+        scene->tab.k = 1;
+        scene->tab.n_total = (uint32_t)l->total;
+        scene->many = true;
+        scene->list = l;
+        scene->list_tab = l->cur;
+        scene->list_view = *view;
+        scene->list_depth_bits = frame->radix_sort_depth_bits;
+        const ListTable& lt = *l->cur;
+        scene->dtab = SceneTableDev{k, (uint32_t)l->total, lt.seg, lt.a.offset, lt.a.times, lt.a.classes,
+                                    box_frame ? lt.a.kinds_box : lt.a.kinds};
+        if (l->flow) TRY(check_flow_extras(c, ex));
+    }
+    if (undrawn) return fail(c, BGS_EINVAL, "%s: a Velocity frame with no Gaussian4d cloud listed", call);
+    if (depth) TRY(check_scene_depth(c, depth, view));
+    if (t.device && reinterpret_cast<uintptr_t>(t.rgba[0]) % format_bpp(t.format) != 0)
+        return fail(c, BGS_EINVAL, "render: device target %p is not aligned to its %zu-byte pixels", t.rgba[0], format_bpp(t.format));
+    if (t.pick) {
+        if (t.device && reinterpret_cast<uintptr_t>(t.pick) % sizeof(bgs_pick) != 0)
+            return fail(c, BGS_EINVAL, "%s: device pick target %p is not aligned to its 16-byte records", call, t.pick);
+        if (frame->flags & BGS_FLAG_ASYNC) return fail(c, BGS_EINVAL, "%s: BGS_FLAG_ASYNC is not supported", call);
+    }
+    // the frame as render_entities_impl plans it
+    bgs_settings sf = *frame;
+    sf.rasterize_mode = l->depth ? BGS_RASTERIZE_DEPTH : BGS_RASTERIZE_COLOR;
+    sf.aabb = scene->raster_mode != 0;
+    sf.gaussian_mode = scene->raster_mode == 2 ? BGS_GAUSSIAN_2D : BGS_GAUSSIAN_3D;
+    sf.draw_mode = BGS_DRAW_ALL;
+    if (scene->box) sf.flags |= BGS_FLAG_VISUALIZE_BOUNDING_BOX;
+    if (t.pick) sf.flags = (sf.flags & ~(uint32_t)BGS_FLAG_CHUNKS) | BGS_FLAG_NO_CHUNKS;   // (one round)
+    return render_impl(c, l->ent[0].cloud, view, &l->ent[0].uni, &sf, ex, t, depth, nullptr, scene);
+}
+
+bgs_status bgs_render_entity_list(bgs_context* c, const bgs_entity_list* l, const bgs_view* view, const bgs_settings* frame,
+                                  const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba, uint32_t out_format,
+                                  int out_is_device_ptr) {
+    return render_list_impl(c, "render_entity_list", l, view, frame, ex, depth, colour_target(&out_rgba, out_format, out_is_device_ptr));
+}
+
+bgs_status bgs_render_entity_list_pick(bgs_context* c, const bgs_entity_list* l, const bgs_view* view, const bgs_settings* frame,
+                                       const bgs_render_extras* ex, const bgs_scene_depth* depth, void* out_rgba,
+                                       uint32_t out_format, int out_is_device_ptr, void* out_pick) {
+    const char* call = "render_entity_list_pick";
+    if (c && !out_pick) return fail(c, BGS_EINVAL, "%s: out_pick is NULL", call);
+    const Targets t{out_format, out_is_device_ptr, 1, false, &out_rgba, nullptr, nullptr, out_pick};
+    return render_list_impl(c, call, l, view, frame, ex, depth, t);
 }
 
 // bgs_render_entities_ex of each of v views in one frame (include/bgs.h); one view is bgs_render_entities_ex itself

@@ -413,6 +413,7 @@ void bgs_cloud_destroy(bgs_cloud* cl) {
                 if (c->last.reads(cl)) { c->last.forget(); c->have_frame = false; }
             }
         }
+        detach_listed_cloud(cl);   // (entity lists: their frames are drained above; rendering them is refused until repaired)
     }
     if (cl->ev_write) {   // particle steps still queued on any context write the planes
         cudaEventSynchronize(cl->ev_write);

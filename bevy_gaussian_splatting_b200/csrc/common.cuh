@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/bgs.h"
 
@@ -32,6 +33,42 @@ struct FrameConsts {
     uint32_t cov_pre;           // the cloud carries Covariance3dOpacityPacked128 records (f16.rs:131-170) instead of rotation + scale
     uint32_t aux;               // bgs_render_aux: the projection also emits the Depth and Normal colour sources
 };
+
+// The FrameConsts of one cloud (n_cloud gaussians, cov_pre its layout) under a uniform, a view and its settings: the one
+// construction both the host (frame_consts, api.cu) and bgs_entity_list's expansion kernel (entity_list.cu) use, so a
+// segment built on the device is bit for bit the one the host builds.  model_identity is a bitwise test, as memcmp
+// is: -0.0 and NaN entries take the general path.
+__host__ __device__ inline FrameConsts make_frame_consts(const bgs_view& view, const bgs_cloud_uniform& uni,
+                                                         uint32_t radix_sort_depth_bits, uint32_t gaussian_mode,
+                                                         uint32_t rasterize_mode, uint32_t aabb, uint32_t adaptive,
+                                                         uint32_t draw_mode, uint32_t n_cloud, uint32_t cov_pre, uint32_t aux) {
+    const int W = (int)view.viewport[2], H = (int)view.viewport[3];
+    FrameConsts fc;
+    memcpy(fc.model, uni.transform, 64);
+    memcpy(fc.view_from_world, view.view_from_world, 64);
+    memcpy(fc.clip_from_world, view.clip_from_world, 64);
+    memcpy(fc.cam, view.world_position, 12);
+    fc.W = view.viewport[2]; fc.H = view.viewport[3];
+    fc.p00 = view.clip_from_view[0]; fc.p11 = view.clip_from_view[5];
+    fc.global_opacity = uni.global_opacity; fc.global_scale = uni.global_scale;
+    fc.color_space = uni.color_space;
+    fc.key_shift = 32u - radix_sort_depth_bits;
+    fc.gaussian_mode = gaussian_mode; fc.rasterize_mode = rasterize_mode; fc.aabb = aabb;
+    fc.adaptive = adaptive; fc.draw_mode = draw_mode;
+    fc.Wi = W; fc.Hi = H; fc.tiles_x = (W + TILE_PX - 1) / TILE_PX; fc.tiles_y = (H + TILE_PX - 1) / TILE_PX;
+    fc.n_cloud = n_cloud;
+    fc.aux = aux;
+    fc.cov_pre = cov_pre;
+    memcpy(fc.aabb_min, uni.aabb_min, 12); memcpy(fc.aabb_max, uni.aabb_max, 12);
+    uint32_t identity = 1u;
+    for (int i = 0; i < 16; ++i) {
+        uint32_t bits;
+        memcpy(&bits, &uni.transform[i], 4);
+        if (bits != (i % 5 == 0 ? 0x3f800000u : 0u)) identity = 0u;
+    }
+    fc.model_identity = identity;
+    return fc;
+}
 
 // A scene frame's segment table (bgs_render_scene, _scene_4d, _entities).  Segment j holds cloud j's gaussians at global
 // indices [offset, offset + n); its FrameConsts carry the frame-wide values and entity j's settings, uniform and layout
@@ -91,6 +128,20 @@ struct SceneTableDev {
         return j;
     }
 };
+
+// bgs_entity_list's compact record of one entity (device memory, 160 B): what its segment takes from the entity alone.
+// entity_list.cu expands it with the frame's view into the segment; its offset, times, num_classes and kind live in the
+// table's own arrays beside it.
+struct EntityRec {
+    bgs_cloud_uniform uni;      // transform column-major
+    uint32_t gaussian_mode, rasterize_mode, aabb, adaptive, draw_mode;   // bgs_entity_settings'
+    uint32_t n;                 // the cloud's gaussians
+    uint32_t group;             // SceneSeg::group
+    uint32_t cov_pre;           // FrameConsts::cov_pre
+    const float4* pos;
+    const void* blocks;
+};
+static_assert(sizeof(EntityRec) == 160, "EntityRec is 160 bytes");
 
 // The projection group of Gaussian4d segments: project_group gives the 3D layouts 0 .. 7 (f16 bit, SH degree << 1), so
 // 4D segments never fall into a 3D launch, and splat_depth_scene leaves their depths to the 4D projection, which takes

@@ -3,7 +3,9 @@
 // the order of a cloud's accesses, and the frame scratch that the selections borrow.
 #pragma once
 #include <algorithm>
+#include <array>
 #include <atomic>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <vector>
@@ -63,6 +65,17 @@ struct bgs_particles {
     cudaEvent_t ev_write = nullptr;   // the last step of these behaviours (recorded on the stepping context's stream)
 };
 
+// One generation of a bgs_entity_list's device arrays, cap entities each: the compact records, the segment table's
+// offset, time, num_classes and kind arrays (kinds_box: the kinds with BOX_KIND set, for frames with the frame-wide
+// overlay), and the segments the expansion writes once per frame.  A frame holds the generation it reads (SceneFacts), so
+// an edit writes the list's current generation in place only when no frame holds it (api.cu: list_writable).
+struct ListTable {
+    uint32_t cap = 0;
+    DevBuf<uint8_t> mem;
+    EntityListArrays a = {};
+    SceneSeg* seg = nullptr;
+};
+
 // A scene frame (bgs_render_scene, _scene_4d, _entities): its segment table (what its kernels and the culled-flags hook
 // read), its 4D segments' times, the clouds it lists (clouds[j] is segment j's; a cloud may be listed more than once),
 // its distinct projection groups (project_group, plus ENTITY_MODES for the Classification / OpticalFlow / Velocity colour
@@ -92,6 +105,12 @@ struct SceneFacts {
     const void* h_tab = nullptr;
     size_t tab_bytes = 0;
     int slot = 0;
+    // a bgs_render_entity_list frame: dtab is generation `list_tab` of the list, whose segments the frame's first launch
+    // expands from its records and the view (radix_sort_depth_bits: the frame's)
+    const bgs_entity_list* list = nullptr;
+    std::shared_ptr<ListTable> list_tab;
+    bgs_view list_view = {};
+    uint32_t list_depth_bits = 0;
 };
 
 // What the host knows of a frame it has enqueued: the context keeps the last one enqueued (`pend`) and, once its
@@ -238,12 +257,40 @@ struct bgs_context {
     }
 };
 
+// An entity list resident on one context (bgs_entity_list): per entity what the host needs of it (x), and counters over
+// the entities, kept by every edit, from which a frame takes its facts without a pass over the list.
+struct ListEntity {
+    const bgs_cloud* cloud;      // NULL once the cloud is destroyed (the entity is detached)
+    bgs_cloud_uniform uni;       // as last given by the host (a transform set from device memory is not read back)
+    bgs_entity_settings e;
+    uint32_t flags;              // BGS_ENTITY_*
+    uint32_t n, group, offset;   // the cloud's gaussians, the projection group, the first global index
+    bool sh, is4;                // the group's launch reads SH coefficients for it; a Gaussian4d cloud
+};
+struct bgs_entity_list {
+    bgs_context* ctx;            // NULL once the context is destroyed
+    std::vector<ListEntity> ent;
+    uint64_t total = 0;          // N
+    std::map<const bgs_cloud*, uint32_t> clouds;   // entities per listed cloud (detached ones not counted)
+    std::map<uint32_t, std::array<uint32_t, 2>> groups;   // entities per projection group, and of those reading SH
+    uint32_t kinds[3] = {0, 0, 0};   // entities per blend kind
+    uint32_t boxed = 0, depth = 0, flow = 0, detached = 0;   // entities with the overlay bit, in Depth, in OpticalFlow, detached
+    // non-4D Velocity entities per (gaussian_mode, aabb, opacity_adaptive_radius, draw_mode, overlay bit): [0] with the
+    // entity's own overlay bit, [1] with the bit set (frames with the frame-wide overlay)
+    std::map<std::array<uint32_t, 5>, uint32_t> velocity[2];
+    std::shared_ptr<ListTable> cur, spare;   // the generation edits and frames use; one a frame held, for reuse
+    DevBuf<uint8_t> upload;      // the edits' records on their way to the scatter
+};
+
 namespace bgs {
 
 // live contexts: clouds may be shared by the contexts of one GPU, so destroying a cloud must clear every context's
 // references to it, and a write to a cloud must wait for every context's frames that may read it
 extern std::mutex g_registry_mu;
 extern std::vector<bgs_context*> g_contexts;
+// live entity lists (bgs_entity_list): destroying a cloud detaches the entities that list it (api.cu), under the registry lock
+extern std::vector<bgs_entity_list*> g_lists;
+void detach_listed_cloud(const bgs_cloud* cl);
 
 // Sets the context's last-error text (when there is a context) and returns `st`.
 bgs_status fail(bgs_context* ctx, bgs_status st, const char* fmt, ...);

@@ -232,4 +232,26 @@ struct KhrDecode {
 };
 // the staged planes of an f32 (so non-null) or f16 (rot: the packed second record) cloud
 void launch_khr_decode(const KhrDecode& k, bool f16, float4* pos, void* sh, void* rot, void* so, uint32_t* words, cudaStream_t stream);
+// entity_list.cu: bgs_entity_list's expansion of k records into segments (one launch per frame), and its edits' scatter
+// of records (count entities, at the distinct indices idx) and of row-major transforms into records dst[0 .. count)
+struct EntityListUpload {
+    const uint32_t* idx;
+    const EntityRec* recs;
+    const uint32_t* offset;
+    const TemporalConsts* times;
+    const uint32_t* classes;
+    const uint32_t* kinds;      // SegmentKinds::kind without the frame's overlay flag
+};
+struct EntityListArrays {
+    EntityRec* recs;
+    uint32_t* offset;
+    TemporalConsts* times;
+    uint32_t* classes;
+    uint32_t* kinds;            // ... and kinds_box with BOX_KIND set on every entity (frames with the frame-wide overlay)
+    uint32_t* kinds_box;
+};
+cudaError_t launch_entity_list_expand(const EntityRec* recs, const uint32_t* offset, uint32_t k, const bgs_view& view,
+                                      uint32_t radix_sort_depth_bits, uint32_t n_total, SceneSeg* seg, cudaStream_t stream);
+cudaError_t launch_entity_list_scatter(const EntityListUpload& u, uint32_t count, const EntityListArrays& a, cudaStream_t stream);
+cudaError_t launch_entity_list_transforms(const float* m, uint32_t count, EntityRec* dst, cudaStream_t stream);
 }  // namespace bgs

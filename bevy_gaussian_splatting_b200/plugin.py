@@ -388,6 +388,135 @@ def entity_settings(settings: CloudSettings) -> abi.bgs_entity_settings:
                                    window=abi.bgs_time_window(float(settings.time_start), float(settings.time_stop)))
 
 
+def matrices_arg(matrices) -> tuple[int, int, int, bool, int | None, object]:
+    """(address, count, layout, is_device, producer stream, the object to keep alive) of `EntityList.set_transforms`'
+    matrices: a host (count, 4, 4) array (read as float32, row-major), or any `__cuda_array_interface__` object of that
+    shape and float32, row-major (C-contiguous) or column-major (each 4x4 block transposed: a torch `.mT` of a contiguous
+    tensor) from its strides.  The producer stream is the interface's (v3) "stream" entry, None when it names none.
+    Raises ValueError for another shape or a non-contiguous device array, TypeError for another dtype."""
+    cai = getattr(matrices, "__cuda_array_interface__", None)
+    if cai is None:
+        a = np.ascontiguousarray(matrices, np.float32)
+        if a.ndim != 3 or a.shape[1:] != (4, 4):
+            raise ValueError(f"set_transforms: matrices must have shape (count, 4, 4), not {a.shape}")
+        return a.ctypes.data, a.shape[0], abi.BGS_MATRIX_ROW_MAJOR, False, None, a
+    if np.dtype(cai["typestr"]) != np.dtype("<f4"):
+        raise TypeError(f"set_transforms: matrices must be float32, not {cai['typestr']}")
+    shape = tuple(cai["shape"])
+    if len(shape) != 3 or shape[1:] != (4, 4):
+        raise ValueError(f"set_transforms: matrices must have shape (count, 4, 4), not {shape}")
+    strides = cai.get("strides")
+    if strides is None or tuple(strides) == (64, 16, 4) or shape[0] == 0:
+        layout = abi.BGS_MATRIX_ROW_MAJOR
+    elif tuple(strides) == (64, 4, 16):
+        layout = abi.BGS_MATRIX_COLUMN_MAJOR
+    else:
+        raise ValueError(f"set_transforms: strides {tuple(strides)} are neither contiguous row-major (64, 16, 4) nor "
+                         "column-major (64, 4, 16) 4x4 f32 matrices")
+    return int(cai["data"][0]), shape[0], layout, True, cai.get("stream"), matrices
+
+
+class EntityList:
+    """A scene's entity list resident on the GPU (`bgs_entity_list`), owned by one plugin's context: created from entities
+    given as `render_entities_many` takes them, then edited in place -- `set`, `append`, `truncate`, `set_transforms` --
+    and drawn by `plugin.render_entity_list`.  An engine sends only the entities that changed; a GPU simulation writes the
+    transforms from device memory.  Every edit validates with `check_entities_many`'s rules (ValueError before any call):
+    the frame-wide fields (ENTITIES_FRAME_FIELDS) of every entity agree.  The list holds the handles it lists, so the
+    garbage collector cannot destroy a listed cloud."""
+
+    def __init__(self, plugin: "GaussianSplattingPlugin", entities=()):
+        entities = list(entities)
+        self._plugin, self._lib = plugin, plugin._lib
+        self._h = C.c_void_p()
+        self._handles, self._settings = [], []
+        self._checked(entities, len(entities))
+        plugin._check(self._lib.bgs_entity_list_create(plugin._ctx, *plugin._entity_arrays(entities), len(entities),
+                                                       C.byref(self._h)))
+        self._handles = [h for h, _, _ in entities]
+        self._settings = [st for _, st, _ in entities]
+
+    def _checked(self, entities, size: int, indices=None):
+        """check_entities_many's rules for `entities` becoming list entities `indices` (default: appended after the last),
+        the list then `size` long: each agrees with the list's first entity (or, in an empty list, the first given) on
+        every frame-wide field, messages naming the list index."""
+        if size > abi.BGS_ENTITIES_MANY_MAX:
+            raise ValueError(f"entity_list: {size} entities, at most {abi.BGS_ENTITIES_MANY_MAX}")
+        if not entities:
+            return
+        indices = indices if indices is not None else range(len(self), len(self) + len(entities))
+        ref, at = (self._settings[0], 0) if self._settings else (entities[0][1], indices[0])
+        for j, (_, st, _) in zip(indices, entities):
+            for name in ENTITIES_FRAME_FIELDS:
+                a, b = getattr(ref, name), getattr(st, name)
+                if a != b:
+                    raise ValueError(f"entity_list: entity {j} has {name} = {b!r}, entity {at} {a!r}: the frame has one depth sort")
+
+    def _frame(self, call: str):
+        if not self._settings:
+            raise ValueError(f"{call}: no entities")
+        return self._settings[0]
+
+    def __len__(self) -> int:
+        return len(self._handles)
+
+    def set(self, indices, entities):
+        """Entities `indices` (distinct, each < len(self)) become `entities`: cloud, settings and transform may all change."""
+        indices, entities = [int(i) for i in indices], list(entities)
+        if len(indices) != len(entities):
+            raise ValueError(f"entity_list: {len(indices)} indices for {len(entities)} entities")
+        if any(not 0 <= i < len(self) for i in indices) or len(set(indices)) != len(indices):
+            raise ValueError(f"entity_list: indices must be distinct and in 0..{len(self) - 1}")
+        self._checked(entities, len(self), indices)
+        idx = (C.c_uint32 * len(indices))(*indices)
+        self._plugin._check(self._lib.bgs_entity_list_set(self._h, idx, len(indices), *self._plugin._entity_arrays(entities)))
+        for i, (h, st, _) in zip(indices, entities):
+            self._handles[i], self._settings[i] = h, st
+
+    def append(self, entities):
+        entities = list(entities)
+        self._checked(entities, len(self) + len(entities))
+        self._plugin._check(self._lib.bgs_entity_list_append(self._h, len(entities), *self._plugin._entity_arrays(entities)))
+        self._handles += [h for h, _, _ in entities]
+        self._settings += [st for _, st, _ in entities]
+
+    def truncate(self, k: int):
+        """Keeps the first k entities.  To remove entity j: set j to the last entity, then truncate by one."""
+        if not 0 <= k <= len(self):
+            raise ValueError(f"entity_list: truncate to {k}, not in 0..{len(self)}")
+        self._plugin._check(self._lib.bgs_entity_list_truncate(self._h, k))
+        del self._handles[k:], self._settings[k:]
+
+    def set_transforms(self, first: int, matrices):
+        """The transforms of entities [first, first + count) from `matrices` (see `matrices_arg`).  A host array may be
+        reused once the call returns.  A device array is read on the context's stream after the work queued so far on its
+        producer's stream: the stream its interface names (v3), or for a torch tensor torch's current stream on its device.
+        Any other device array must be complete when the call is made (the context's streams do not wait for the legacy
+        default stream).  It must stay unchanged until the context's stream has passed the call."""
+        ptr, count, layout, device, producer, keep = matrices_arg(matrices)
+        if not (0 <= first and first + count <= len(self)):
+            raise ValueError(f"entity_list: transforms [{first}, {first + count}) beyond {len(self)} entities")
+        if device and producer is None and type(matrices).__module__.startswith("torch"):
+            # (torch's interface names no stream: its producer is torch's current stream, 0 being the legacy default one)
+            import torch
+
+            producer = torch.cuda.current_stream(matrices.device).cuda_stream or 1
+        if producer is not None:
+            _stream_wait(self._plugin.stream_ptr, int(producer))
+        self._plugin._check(self._lib.bgs_entity_list_set_transforms(self._h, first, count, C.c_void_p(ptr), layout, int(device)))
+        del keep
+
+    def close(self):
+        if self._h:
+            self._lib.bgs_entity_list_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class GaussianSplattingPlugin:
     """Owns one `bgs_context` (one GPU).  `render_view` = run_radix_sort + DrawGaussians for one view."""
 
@@ -584,6 +713,42 @@ class GaussianSplattingPlugin:
         self._check(getattr(self._lib, fn)(self._ctx, *args, None if zd is None else C.byref(zd), _ptr(out), code, 0))
         return out
 
+    def entity_list(self, entities=()) -> "EntityList":
+        """A resident entity list (`bgs_entity_list`) of `entities`, given as `render_entities_many` takes them, edited in
+        place between frames and drawn by `render_entity_list`."""
+        return EntityList(self, entities)
+
+    def render_entity_list(self, lst: "EntityList", view: View, fmt: str = "rgba32f", scene_depth=None,
+                           previous_view: View | None = None, delta_time: float | None = None, asynchronous: bool = False,
+                           premultiplied: bool = False, blend_over: bool = False, out: np.ndarray | None = None) -> np.ndarray:
+        """`render_entities_many` of the list as it stands (`bgs_render_entity_list`): byte for byte its frame, with no
+        per-entity work on the host.  The frame-wide settings are the list's first entity's.  ValueError for an empty list."""
+        code, dtype, ch = self.FORMATS[fmt]
+        if out is None:
+            out = np.empty((view.height, view.width, ch), dtype)
+        assert out.dtype == dtype and out.size == view.height * view.width * ch and out.flags.c_contiguous
+        v, s, ex = self._frame_args(lst._frame("render_entity_list"), view, previous_view, delta_time, asynchronous, premultiplied,
+                                    blend_over)
+        zd = self._scene_depth(scene_depth, view)
+        self._check(self._lib.bgs_render_entity_list(self._ctx, lst._h, C.byref(v), C.byref(s), None if ex is None else C.byref(ex),
+                                                     None if zd is None else C.byref(zd), _ptr(out), code, 0))
+        return out
+
+    def render_entity_list_pick(self, lst: "EntityList", view: View, fmt: str = "rgba32f", scene_depth=None,
+                                previous_view: View | None = None, delta_time: float | None = None, premultiplied: bool = False,
+                                blend_over: bool = False) -> tuple[np.ndarray, np.ndarray]:
+        """`render_entities_pick_many` of the list as it stands (`bgs_render_entity_list_pick`): (rgba, pick)."""
+        code, dtype, ch = self.FORMATS[fmt]
+        out = np.empty((view.height, view.width, ch), dtype)
+        pick = np.empty((view.height, view.width), abi.PICK_DTYPE)
+        v, s, ex = self._frame_args(lst._frame("render_entity_list_pick"), view, previous_view, delta_time, False,
+                                    premultiplied, blend_over)
+        zd = self._scene_depth(scene_depth, view)
+        self._check(self._lib.bgs_render_entity_list_pick(self._ctx, lst._h, C.byref(v), C.byref(s),
+                                                          None if ex is None else C.byref(ex),
+                                                          None if zd is None else C.byref(zd), _ptr(out), code, 0, _ptr(pick)))
+        return out, pick
+
     def render_entities_aux(self, entities, view: View, fmt: str = "rgba32f", scene_depth=None,
                             previous_view: View | None = None, delta_time: float | None = None, premultiplied: bool = False,
                             blend_over: bool = False) -> list[np.ndarray]:
@@ -695,22 +860,31 @@ class GaussianSplattingPlugin:
 
     def _entities_args(self, entities, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over):
         """(clouds, uniforms, entities, entity flags, k, view, frame, extras) of a bgs_render_entities_ex or _aux call."""
+        v, s, ex = self._frame_args(first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over)
+        return (*self._entity_arrays(entities), len(entities), C.byref(v), C.byref(s), None if ex is None else C.byref(ex))
+
+    def _frame_args(self, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over):
+        """(view, frame, extras or None) of an entity frame whose frame-wide settings are `first`'s."""
         v = view.to_abi()
         s = first.to_abi()
-        s.flags &= ~abi.BGS_FLAG_VISUALIZE_BOUNDING_BOX   # (each entity's own, below)
+        s.flags &= ~abi.BGS_FLAG_VISUALIZE_BOUNDING_BOX   # (each entity's own: _entity_arrays)
         s.flags |= ((abi.BGS_FLAG_ASYNC if asynchronous else 0) | (abi.BGS_FLAG_PREMULTIPLIED_OUT if premultiplied else 0)
                     | (abi.BGS_FLAG_BLEND_OVER_TARGET if blend_over else 0))
         ex = None
         if previous_view is not None:
             ex = abi.bgs_render_extras(num_classes=1, delta_time=float(delta_time) if delta_time is not None else 0.0)
             ex.previous_clip_from_world[:] = previous_view.to_abi().clip_from_world[:]
+        return v, s, ex
+
+    def _entity_arrays(self, entities):
+        """(clouds, uniforms, entities, entity flags) of an entity list."""
         k = len(entities)
         eflags = (C.c_uint32 * k)(*[abi.BGS_ENTITY_VISUALIZE_BOUNDING_BOX if st.visualize_bounding_box else 0
                                     for _, st, _ in entities])
         clouds = (C.c_void_p * k)(*[h._h.value for h, _, _ in entities])
         unis = (abi.bgs_cloud_uniform * k)(*[self.cloud_uniform(st, tr, h.aabb) for h, st, tr in entities])
         ents = (abi.bgs_entity_settings * k)(*[entity_settings(st) for _, st, _ in entities])
-        return clouds, unis, ents, eflags, k, C.byref(v), C.byref(s), None if ex is None else C.byref(ex)
+        return clouds, unis, ents, eflags
 
     def _render_4d(self, handle, v, u, s, ex, zd, settings, target, code, is_device):
         return self._lib.bgs_render_4d(self._ctx, handle._h, C.byref(v), C.byref(u), C.byref(s), None if ex is None else C.byref(ex),

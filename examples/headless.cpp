@@ -4,7 +4,7 @@
 //   headless [count=100000] [width=1920] [height=1080] [global_scale=1.0] [out=headless_output/0.ppm]
 //            [--dump-cloud file] [--raw file] [--remove-floaters radius]
 //            [--particles N --steps K --dt S [--dump-particles file]] [--interpolate SEED --time T]
-//            [--rasterize classification|optical-flow] [--num-classes K] [--prev-view dx,dy,dz]
+//            [--rasterize classification|optical-flow] [--num-classes K] [--prev-view dx,dy,dz] [--instances N]
 // --dump-cloud writes the four f32 planes (n, then pos_vis, sh, rot, scale_opacity) so another host can
 // render the identical cloud; --raw writes the RGBA8 frame bytes.  --remove-floaters selects the sparse gaussians
 // (SparseSelect with that radius), inverts the selection and draws only the rest (DrawMode::Selected), the
@@ -15,6 +15,8 @@
 // --interpolate blends the cloud (lhs) with random_gaussians_3d_seeded(count, SEED) (rhs) at time T of the window
 // [0, 1] into a third cloud, made as the subset of every gaussian of lhs, and draws that one (the reference's
 // GaussianInterpolate { lhs, rhs }); --dump-cloud then writes rhs's four planes after lhs's.
+// --instances N draws the cloud instanced N times on a grid through a resident entity list (bgs_entity_list), the
+// instances then moved by one set_transforms from a row-major host array.
 // --rasterize picks RasterizeMode::Classification (labels: gaussian i gets visibility 2 + i % K, --num-classes K, default
 // 3) or OpticalFlow (the previous frame's camera is the headless camera moved by --prev-view, default 0.05,0,0, at
 // 1/60 s); the previous view's clip_from_world is printed as 16 hex words ("prev_clip: ...").
@@ -38,6 +40,7 @@ int main(int argc, char** argv) {
     std::string dump_particles;
     long interp_seed = -1; float interp_time = 0.0f;
     std::string rasterize = "color"; uint32_t num_classes = 3; float prev_off[3] = {0.05f, 0.0f, 0.0f};
+    uint32_t instances = 0;      // --instances N: the cloud instanced N times on a grid through an entity list
     float depth_plane = -1.0f;   // --depth-plane Z: render depth-tested against a half-frame plane at reverse-Z depth Z
     int pos = 0;
     for (int i = 1; i < argc; ++i) {
@@ -53,6 +56,7 @@ int main(int argc, char** argv) {
         if (a == "--time" && i + 1 < argc) { interp_time = (float)std::atof(argv[++i]); continue; }
         if (a == "--rasterize" && i + 1 < argc) { rasterize = argv[++i]; continue; }
         if (a == "--depth-plane" && i + 1 < argc) { depth_plane = (float)std::atof(argv[++i]); continue; }
+        if (a == "--instances" && i + 1 < argc) { instances = (uint32_t)std::strtoul(argv[++i], nullptr, 10); continue; }
         if (a == "--num-classes" && i + 1 < argc) { num_classes = (uint32_t)std::strtoul(argv[++i], nullptr, 10); continue; }
         if (a == "--prev-view" && i + 1 < argc) {
             if (std::sscanf(argv[++i], "%f,%f,%f", &prev_off[0], &prev_off[1], &prev_off[2]) != 3) return 1;
@@ -163,7 +167,28 @@ int main(int argc, char** argv) {
                                                       frame.data(), BGS_FORMAT_RGBA8_SRGB);
             mem_free(d);
         }
-        for (int f = 0; f < 3 && depth_plane < 0.0f; ++f)
+        std::unique_ptr<bgs::EntityList> list;   // (kept to the end: destroying it drops the frame the stats describe)
+        if (instances > 0) {
+            // instance j at ((j % 32) / 4 - 4, 1.5 + (j / 32 % 32) / 8 - 2, -2 - (j / 1024) / 2) (exact in f32), listed once;
+            // then every instance moved by +0.5 in x through one row-major set_transforms, and three frames of the list
+            std::vector<bgs::GaussianSplattingPlugin::SceneEntity> ents(instances);
+            std::vector<float> rows((size_t)instances * 16, 0.0f);
+            for (uint32_t j = 0; j < instances; ++j) {
+                const float t[3] = {(float)(j % 32) * 0.25f - 4.0f, 1.5f + (float)(j / 32 % 32) * 0.125f - 2.0f,
+                                    -2.0f - (float)(j / 1024) * 0.5f};
+                ents[j].cloud = &drawn_cloud;
+                ents[j].settings = settings;
+                for (int k = 0; k < 3; ++k) ents[j].transform.m[12 + k] = t[k];
+                float* r = &rows[(size_t)j * 16];
+                r[0] = r[5] = r[10] = r[15] = 1.0f;
+                r[3] = t[0] + 0.5f; r[7] = t[1]; r[11] = t[2];
+            }
+            list.reset(new bgs::EntityList(plugin.entity_list(ents)));
+            list->set_transforms(0, instances, rows.data(), true);
+            for (int f = 0; f < 3; ++f) drawn = plugin.render_entity_list(*list, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);
+            std::printf("instances: %u through an entity list\n", list->size());
+        }
+        for (int f = 0; f < 3 && depth_plane < 0.0f && instances == 0; ++f)
             drawn = settings.rasterize_mode == bgs::RasterizeMode::OpticalFlow
                         ? plugin.render_view(drawn_cloud, settings, view, prev_view, 1.0f / 60.0f, frame.data(), BGS_FORMAT_RGBA8_SRGB)
                         : plugin.render_view(drawn_cloud, settings, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);

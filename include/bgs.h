@@ -974,6 +974,78 @@ bgs_status bgs_render_entities_pick_many(bgs_context* ctx, const bgs_cloud* cons
                                          void* out_rgba, uint32_t out_format, int out_is_device_ptr,
                                          void* out_pick /* w * h bgs_pick */);
 
+/* A scene's entity list kept resident on the GPU and edited in place, for bgs_render_entities_many's frames without
+ * rebuilding the scene on the host every frame: an engine sends only the entities that were added, changed or removed,
+ * and a GPU simulation (a crowd, a flock, physics props) writes the transforms from device memory.  Each entity is what
+ * bgs_render_entities_many takes: a cloud, a bgs_cloud_uniform, a bgs_entity_settings and BGS_ENTITY_* flags.
+ *
+ * bgs_entity_list_create: a list of k entities (0 <= k <= BGS_ENTITIES_MANY_MAX) owned by ctx; entity_flags may be NULL.
+ * bgs_entity_list_set: entities indices[0 .. count) (distinct, each < k) become the given ones; the cloud, settings,
+ *   uniform and flags may all change.
+ * bgs_entity_list_append: count entities after the last.  bgs_entity_list_truncate: keeps the first k (k <= the size).
+ *   To remove entity j, set j to the last entity and truncate by one.
+ * bgs_entity_list_set_transforms: uniforms[j].transform for j in [first, first + count) from count contiguous 4x4 f32
+ *   matrices at m, in BGS_MATRIX_COLUMN_MAJOR (the uniform's own layout) or BGS_MATRIX_ROW_MAJOR (a (count, 4, 4) torch
+ *   tensor).  A host array (pageable or pinned) is read before the call returns and may be reused at once.  A device array
+ *   (is_device_ptr) is read on the context's stream (bgs_context_stream): the caller orders that stream after the
+ *   array's producer (the context's streams are non-blocking: they do not wait for the legacy default stream), and may
+ *   reuse the array once the stream has passed the call.
+ * bgs_entity_list_size: the number of entities (0 for NULL).
+ * bgs_entity_list_destroy: drains the context's queued frames, and the debug hooks drop a frame that read the list, as
+ *   bgs_cloud_destroy does for a cloud.  Destroy a context's lists before the context; a list whose context is gone
+ *   refuses every call.
+ * bgs_render_entity_list / _pick: bgs_render_entities_many / _pick_many of the list as it stands.
+ *
+ * The rule, exactly:
+ *   Identity.  A list frame is byte for byte the frame bgs_render_entities_many (bgs_render_entities_pick_many) gives for
+ *     the list's entities with the same view, frame, extras, depth and target: pixels in all three formats and output
+ *     modes, sorted entries, tile ranges and slices, records, splat depths, bgs_frame_stats, chunked rounds, overlays, 4D
+ *     entities, mixed blend kinds, the depth test, BGS_FLAG_ASYNC with its pair-overflow rule, and pick records.  This
+ *     holds for transforms set from device memory, which the host never sees.
+ *   Launches.  bgs_render_entities_many's, plus one: the expansion of the list's records into the frame's segment table.
+ *   Ordering.  Edits are ordered with frames on the context's stream: a frame enqueued before an edit renders the list as
+ *     it was, a frame enqueued after it the list as edited.  An edit never rewrites what a queued frame, or the frame the
+ *     debug hooks describe, reads.  Each distinct listed cloud is read after every write queued on it, as in scenes.
+ *   Validation at the edit.  create, set and append make every refusal bgs_render_entities_many makes of an entity that
+ *     depends on the entity alone (its settings, its cloud's device, the 4D window, num_classes in Classification, a
+ *     covariance cloud with Normal, unknown flag bits, a NULL cloud), their messages naming the entity
+ *     ("entities[j]: ..."), and refuse an edit that would take N to 2^30 or more; a refused edit changes nothing.  The
+ *     render calls make the rest, each with the status bgs_render_entities_many returns for the same list: the view, the
+ *     frame's bits and flags, BGS_FLAG_SORT_ALL, the format, OpticalFlow entities without extras, a Velocity frame with
+ *     no Gaussian4d cloud, k == 0, the depth buffer and the targets.
+ *   Cloud lifetime.  bgs_cloud_destroy of a cloud a live list holds (on any context of its GPU) detaches the entities
+ *     that list it: rendering the list is then refused with BGS_EINVAL naming such an entity, until bgs_entity_list_set
+ *     replaces it.  Nothing dangling is read.
+ *   Host cost.  A render call does no work proportional to k: only to the list's distinct clouds and projection groups.
+ *     An edit of count entities costs O(count) on the host, O(k) when it changes an entity's gaussian count (the offsets
+ *     are recomputed).
+ * Refused with BGS_EINVAL: a NULL list, context or out; a list of another context; indices out of range or repeated;
+ *   first + count beyond the size; a NULL array with count > 0; an unknown layout; a device array that is not device
+ *   memory of the context's GPU.  NULL view or frame -> BGS_NOT_READY. */
+typedef struct bgs_entity_list bgs_entity_list;   /* opaque, library-owned */
+enum { BGS_MATRIX_COLUMN_MAJOR = 0, BGS_MATRIX_ROW_MAJOR = 1 };
+bgs_status bgs_entity_list_create(bgs_context* ctx, const bgs_cloud* const* clouds, const bgs_cloud_uniform* uniforms,
+                                  const bgs_entity_settings* entities, const uint32_t* entity_flags /* k, or NULL */,
+                                  uint32_t k, bgs_entity_list** out);
+bgs_status bgs_entity_list_set(bgs_entity_list* list, const uint32_t* indices, uint32_t count, const bgs_cloud* const* clouds,
+                               const bgs_cloud_uniform* uniforms, const bgs_entity_settings* entities,
+                               const uint32_t* entity_flags /* count, or NULL */);
+bgs_status bgs_entity_list_append(bgs_entity_list* list, uint32_t count, const bgs_cloud* const* clouds,
+                                  const bgs_cloud_uniform* uniforms, const bgs_entity_settings* entities,
+                                  const uint32_t* entity_flags /* count, or NULL */);
+bgs_status bgs_entity_list_truncate(bgs_entity_list* list, uint32_t k);
+bgs_status bgs_entity_list_set_transforms(bgs_entity_list* list, uint32_t first, uint32_t count, const float* m,
+                                          uint32_t layout /* BGS_MATRIX_* */, int is_device_ptr);
+uint32_t bgs_entity_list_size(const bgs_entity_list* list);
+void bgs_entity_list_destroy(bgs_entity_list* list);
+bgs_status bgs_render_entity_list(bgs_context* ctx, const bgs_entity_list* list, const bgs_view* view, const bgs_settings* frame,
+                                  const bgs_render_extras* extras, const bgs_scene_depth* depth /* may be NULL */,
+                                  void* out_rgba, uint32_t out_format, int out_is_device_ptr);
+bgs_status bgs_render_entity_list_pick(bgs_context* ctx, const bgs_entity_list* list, const bgs_view* view,
+                                       const bgs_settings* frame, const bgs_render_extras* extras,
+                                       const bgs_scene_depth* depth /* may be NULL */, void* out_rgba, uint32_t out_format,
+                                       int out_is_device_ptr, void* out_pick /* w * h bgs_pick */);
+
 /* bgs_render_entities_ex of several views of one scene in ONE frame: stereo eyes, the six faces of a cube map, split-screen
  * and picture-in-picture cameras, or many cameras of a dataset share one key-gen, depth sort, projection, binning,
  * tile-id sort and blend launch instead of one set of launches per view (the reference renders every GaussianCamera).

@@ -205,6 +205,7 @@ public:
 };
 
 class GaussianSplattingPlugin;
+class EntityList;
 
 class PlanarGaussian3dHandle {   // a cloud resident in HBM
 public:
@@ -687,24 +688,28 @@ public:
     bgs_frame_stats frame_stats() { bgs_frame_stats fs{}; check(bgs_frame_stats_get(ctx_, &fs)); return fs; }
     bgs_context* context() const { return ctx_; }
 
-private:
-    void check(bgs_status st) { if (st != BGS_OK) throw Error(st, bgs_last_error(ctx_)); }
-    // the entity arrays of a render_views / render_views_aux call, and the call made with them (false: BGS_NOT_READY)
-    // the arguments of a bgs_render_entities_ex / _pick call of `entities`
-    struct EntitiesArgs {
+    // A resident entity list (bgs_entity_list) of `entities`, edited in place and drawn by render_entity_list
+    inline EntityList entity_list(const std::vector<SceneEntity>& entities);
+    // render_entities_many / render_entities_pick_many of the list as it stands (bgs_render_entity_list, _pick): the same
+    // frames, with no per-entity work on the host.  The frame's settings are the list's first entity's; the other
+    // arguments are render_entities_many's.
+    inline bool render_entity_list(const EntityList& list, const bgs_view& view, void* out_rgba,
+                                   uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr,
+                                   float delta_time = 0.0f, const float* depth = nullptr, uint64_t pitch_bytes = 0,
+                                   bool out_is_device = false, uint32_t extra_flags = 0);
+    inline void render_entity_list_pick(const EntityList& list, const bgs_view& view, void* out_rgba, void* out_pick,
+                                        uint32_t format = BGS_FORMAT_RGBA8_SRGB, const bgs_view* previous_view = nullptr,
+                                        float delta_time = 0.0f, const float* depth = nullptr, uint64_t pitch_bytes = 0,
+                                        bool out_is_device = false, uint32_t extra_flags = 0);
+    // the per-entity arrays of a bgs_render_entities_ex call (or a bgs_entity_list edit) of `entities`
+    struct EntityArrays {
         std::vector<const bgs_cloud*> clouds;
         std::vector<bgs_cloud_uniform> unis;
         std::vector<bgs_entity_settings> ents;
         std::vector<uint32_t> eflags;
-        bgs_settings s;
-        bgs_render_extras extras;
-        const bgs_render_extras* ex;
     };
-    template <class Call>
-    bool entities_call(const std::vector<SceneEntity>& entities, const bgs_view* previous_view, float delta_time,
-                       uint32_t extra_flags, Call call) {
-        if (entities.empty()) check(BGS_EINVAL);
-        EntitiesArgs a;
+    static EntityArrays entity_arrays(const std::vector<SceneEntity>& entities) {
+        EntityArrays a;
         for (const SceneEntity& e : entities) {
             bgs_cloud_uniform u = cloud_uniform(e.settings, e.transform);
             std::memcpy(u.aabb_min, e.cloud->aabb_min(), 12); std::memcpy(u.aabb_max, e.cloud->aabb_max(), 12);
@@ -715,7 +720,21 @@ private:
                               e.settings.num_classes, {e.settings.time_start, e.settings.time_stop}});
             a.eflags.push_back(e.settings.visualize_bounding_box ? (uint32_t)BGS_ENTITY_VISUALIZE_BOUNDING_BOX : 0u);
         }
-        a.s = entities[0].settings.to_abi(extra_flags);
+        return a;
+    }
+private:
+    void check(bgs_status st) { if (st != BGS_OK) throw Error(st, bgs_last_error(ctx_)); }
+    // the entity arrays of a render_views / render_views_aux call, and the call made with them (false: BGS_NOT_READY)
+    // the arguments of a bgs_render_entities_ex / _pick call of `entities`
+    struct EntitiesArgs : EntityArrays {
+        bgs_settings s;
+        bgs_render_extras extras;
+        const bgs_render_extras* ex;
+    };
+    // the frame's settings (`first`'s, with extra_flags) and extras of an entity frame
+    static void frame_args(const CloudSettings& first, const bgs_view* previous_view, float delta_time, uint32_t extra_flags,
+                           EntitiesArgs& a) {
+        a.s = first.to_abi(extra_flags);
         if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) a.s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
         a.extras = bgs_render_extras{};
         a.extras.num_classes = 1;
@@ -724,6 +743,14 @@ private:
             a.extras.delta_time = delta_time;
         }
         a.ex = previous_view ? &a.extras : nullptr;
+    }
+    template <class Call>
+    bool entities_call(const std::vector<SceneEntity>& entities, const bgs_view* previous_view, float delta_time,
+                       uint32_t extra_flags, Call call) {
+        if (entities.empty()) check(BGS_EINVAL);
+        EntitiesArgs a;
+        static_cast<EntityArrays&>(a) = entity_arrays(entities);
+        frame_args(entities[0].settings, previous_view, delta_time, extra_flags, a);
         const bgs_status st = call(a);
         if (st == BGS_NOT_READY) return false;
         check(st);
@@ -764,6 +791,92 @@ private:
     }
     bgs_context* ctx_ = nullptr;
 };
+
+
+// A scene's entity list resident on the GPU (bgs_entity_list, include/bgs.h): created by
+// GaussianSplattingPlugin::entity_list, edited in place, drawn by render_entity_list; destroyed with the object (before its
+// plugin).  Every edit throws Error on a refusal, which changes nothing.
+class EntityList {
+public:
+    using SceneEntity = GaussianSplattingPlugin::SceneEntity;
+    EntityList(const EntityList&) = delete;
+    EntityList& operator=(const EntityList&) = delete;
+    EntityList(EntityList&& o) noexcept : ctx_(o.ctx_), h_(o.h_), settings_(std::move(o.settings_)) { o.h_ = nullptr; }
+    ~EntityList() { bgs_entity_list_destroy(h_); }
+    // entities indices[i] (distinct, each < size()) become entities[i]: cloud, settings and transform may all change
+    void set(const std::vector<uint32_t>& indices, const std::vector<SceneEntity>& entities) {
+        if (indices.size() != entities.size()) throw Error(BGS_EINVAL, "EntityList::set: one entity per index");
+        const auto a = GaussianSplattingPlugin::entity_arrays(entities);
+        check(bgs_entity_list_set(h_, indices.data(), (uint32_t)indices.size(), a.clouds.data(), a.unis.data(), a.ents.data(),
+                                  a.eflags.data()));
+        for (size_t i = 0; i < indices.size(); ++i) settings_[indices[i]] = entities[i].settings;
+    }
+    void append(const std::vector<SceneEntity>& entities) {
+        const auto a = GaussianSplattingPlugin::entity_arrays(entities);
+        check(bgs_entity_list_append(h_, (uint32_t)entities.size(), a.clouds.data(), a.unis.data(), a.ents.data(),
+                                     a.eflags.data()));
+        for (const SceneEntity& e : entities) settings_.push_back(e.settings);
+    }
+    // keeps the first k entities; to remove entity j, set j to the last entity and truncate by one
+    void truncate(uint32_t k) {
+        check(bgs_entity_list_truncate(h_, k));
+        settings_.resize(k);
+    }
+    // the transforms of entities [first, first + count) from count 4x4 f32 matrices at m: column-major (Mat4's layout) or
+    // row_major; device memory (read on the context's stream, which the caller orders after the matrices' producer)
+    void set_transforms(uint32_t first, uint32_t count, const float* m, bool row_major = false, bool device = false) {
+        check(bgs_entity_list_set_transforms(h_, first, count, m, row_major ? BGS_MATRIX_ROW_MAJOR : BGS_MATRIX_COLUMN_MAJOR,
+                                             device ? 1 : 0));
+    }
+    uint32_t size() const { return bgs_entity_list_size(h_); }
+    bgs_entity_list* get() const { return h_; }
+
+private:
+    friend class GaussianSplattingPlugin;
+    EntityList(bgs_context* ctx, bgs_entity_list* h, std::vector<CloudSettings> settings)
+        : ctx_(ctx), h_(h), settings_(std::move(settings)) {}
+    void check(bgs_status st) { if (st != BGS_OK) throw Error(st, bgs_last_error(ctx_)); }
+    bgs_context* ctx_;
+    bgs_entity_list* h_;
+    std::vector<CloudSettings> settings_;   // (the frame's settings are the first entity's)
+};
+
+inline EntityList GaussianSplattingPlugin::entity_list(const std::vector<SceneEntity>& entities) {
+    const EntityArrays a = entity_arrays(entities);
+    bgs_entity_list* h = nullptr;
+    check(bgs_entity_list_create(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(), (uint32_t)entities.size(),
+                                 &h));
+    std::vector<CloudSettings> settings;
+    for (const SceneEntity& e : entities) settings.push_back(e.settings);
+    return EntityList(ctx_, h, std::move(settings));
+}
+
+inline bool GaussianSplattingPlugin::render_entity_list(const EntityList& list, const bgs_view& view, void* out_rgba,
+                                                        uint32_t format, const bgs_view* previous_view, float delta_time,
+                                                        const float* depth, uint64_t pitch_bytes, bool out_is_device,
+                                                        uint32_t extra_flags) {
+    if (list.settings_.empty()) check(BGS_EINVAL);
+    EntitiesArgs a;
+    frame_args(list.settings_[0], previous_view, delta_time, extra_flags, a);
+    const bgs_scene_depth zd{depth, pitch_bytes};
+    const bgs_status st = bgs_render_entity_list(ctx_, list.get(), &view, &a.s, a.ex, depth ? &zd : nullptr, out_rgba, format,
+                                                 out_is_device ? 1 : 0);
+    if (st == BGS_NOT_READY) return false;
+    check(st);
+    return true;
+}
+
+inline void GaussianSplattingPlugin::render_entity_list_pick(const EntityList& list, const bgs_view& view, void* out_rgba,
+                                                             void* out_pick, uint32_t format, const bgs_view* previous_view,
+                                                             float delta_time, const float* depth, uint64_t pitch_bytes,
+                                                             bool out_is_device, uint32_t extra_flags) {
+    if (list.settings_.empty()) check(BGS_EINVAL);
+    EntitiesArgs a;
+    frame_args(list.settings_[0], previous_view, delta_time, extra_flags, a);
+    const bgs_scene_depth zd{depth, pitch_bytes};
+    check(bgs_render_entity_list_pick(ctx_, list.get(), &view, &a.s, a.ex, depth ? &zd : nullptr, out_rgba, format,
+                                      out_is_device ? 1 : 0, out_pick));
+}
 
 }  // namespace bgs
 
