@@ -5,7 +5,8 @@ The Python modules here are the host-side mirror of the reference interface for 
 (same names as mosure/bevy_gaussian_splatting: src/lib.rs:7-29 re-exports) used by tests and bench.
 """
 from .abi import PICK_DTYPE, BgsError  # noqa: F401
-from .camera import GaussianCamera, View, headless_view, orbit_view, perspective_view  # noqa: F401
+from .camera import (GaussianCamera, View, headless_view, interpolate_view, orbit_view, perspective_view,  # noqa: F401
+                     shutter_times)
 from .gaussian import (PlanarGaussian3d, PlanarGaussian4d, random_gaussians_3d, random_gaussians_3d_seeded,  # noqa: F401
                        random_gaussians_4d_seeded, SH_COEFF_COUNT, SH_4D_COEFF_COUNT, SH_WIDTHS)
 from .io import load_cloud, parse_ply_3d, parse_ply_4d, write_ply_4d  # noqa: F401

@@ -251,6 +251,9 @@ SYMBOLS = [
     ("bgs_render_views_aux", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P, C.c_uint32,
                                        C.POINTER(bgs_view), C.c_uint32, C.POINTER(bgs_settings), C.POINTER(bgs_scene_depth), _P,
                                        _P, _P, C.c_uint32, C.c_int]),
+    ("bgs_render_shutter", C.c_int, [_P, _P, C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_entity_settings), _P, C.c_uint32,
+                                     C.POINTER(bgs_view), C.c_uint32, C.POINTER(bgs_settings), C.POINTER(bgs_scene_depth), _P,
+                                     C.c_uint32, C.c_int]),
     ("bgs_render_aux", C.c_int, [_P, _P, C.POINTER(bgs_view), C.POINTER(bgs_cloud_uniform), C.POINTER(bgs_settings), _P, _P, _P,
                                  C.c_uint32, C.c_int]),
     ("bgs_sync", C.c_int, [_P]),

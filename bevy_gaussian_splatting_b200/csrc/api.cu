@@ -198,7 +198,8 @@ FramePlan plan_frame(const bgs_context* c, const bgs_settings* st, bool want_aux
 
 // What a frame writes, and where: each of v views' colour frame rgba[i] and, on aux frames, its depth and normal frames
 // depth[i] and normal[i], and on pick frames (bgs_render_entities_pick) the pick frame `pick` (else NULL), in `format`, in
-// device memory (`device`) or host memory.  A single-view frame is view 0.
+// device memory (`device`) or host memory.  A single-view frame is view 0.  A shutter frame (bgs_render_shutter): the v
+// views are its samples, whose blends go to the context's sub-frames, and rgba[0] is its one frame.
 struct Targets {
     uint32_t format;
     int device;
@@ -208,6 +209,7 @@ struct Targets {
     void* const* depth;
     void* const* normal;
     void* pick;
+    bool shutter = false;
 };
 // a single-view frame's colour frame alone
 Targets colour_target(void* const* rgba, uint32_t format, int device) {
@@ -544,10 +546,12 @@ static bgs_status check_render(bgs_context* c, const bgs_cloud* cloud, const bgs
 
 // Enqueues one attempt at a frame: every launch of the plan, the counters' read-back and the copy-out.  A scene frame
 // (render_entities_impl) runs key-gen, the depth range, the projection and the splat depths over its segment table; `cloud`
-// is then its first cloud and fc its first segment's.
+// is then its first cloud and fc its first segment's.  sub_frames non-null (a shutter frame, with views): the views blend
+// stores each view's raw (C, T) at views->out[i], slices of sub_frames, and the resolve writes the frame o.rgba[0].
 static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const FrameConsts& fc, const ModeConsts* modes,
                                 const TemporalConsts* tc, const FramePlan& p, const FrameOut& o, const bgs_scene_depth* zd,
-                                const std::shared_ptr<const SceneFacts>& scene, const ViewTable* views) {
+                                const std::shared_ptr<const SceneFacts>& scene, const ViewTable* views,
+                                const float4* sub_frames) {
     const uint32_t n = scene ? scene->tab.n_total : cloud->n;
     // (a views frame: every view's tiles, one global tile id space)
     const uint32_t num_tiles = views ? views->tile0[views->v] : (uint32_t)fc.tiles_x * (uint32_t)fc.tiles_y;
@@ -687,6 +691,7 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
     if (zd) { b.scene = zd->depth; b.pitch = (size_t)zd->pitch_bytes; }
     b.kinds = c->kinds.p;
     b.views = views;
+    b.raw = sub_frames != nullptr;
     PickArgs pk = {};
     PickArgsDev pkd = {};
     if (o.pick && many) {
@@ -747,6 +752,11 @@ static bgs_status enqueue_frame(bgs_context* c, const bgs_cloud* cloud, const Fr
             CU(c, cudaStreamWaitEvent(q, c->ev_rdone, 0));
         } else
             launch_raster_round(b, c->state.p, c->tile_done, &c->ctr->tiles_done, r == 0, r + 1 == p.rounds, q);
+        ++launches;
+    }
+    if (sub_frames) {   // (after the blend, which the render stream has joined)
+        launch_shutter_resolve(sub_frames, views->v, (uint32_t)fc.Wi * (uint32_t)fc.Hi, o.rgba[0], o.raster_format,
+                               &c->ctr->truncated, q);
         ++launches;
     }
     c->pair_result = pcur;
@@ -830,12 +840,17 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
     TRY(ensure_cloud_scratch(c, n));
     if (c->cap_pairs == 0) TRY(ensure_pair_scratch(c, std::max(n, 1u << 20)));   // first guess; grows on demand
     FrameOut o;
-    TRY(frame_out(c, st, t, views ? scene->views.W : &fc.Wi, views ? scene->views.H : &fc.Hi, &o));
+    Targets to = t;
+    if (t.shutter) to.v = 1;   // (one frame, of view 0's size, which every sample has)
+    TRY(frame_out(c, st, to, views ? scene->views.W : &fc.Wi, views ? scene->views.H : &fc.Hi, &o));
+    // a shutter frame: sample i's blend into its W x H slice of the sub-frames
+    const size_t wh = (size_t)fc.Wi * fc.Hi;
+    if (t.shutter) TRY(c->sub_frames.grow(c, t.v * wh * sizeof(float4), false));
     ViewTable vt = {};
     if (views) {
         vt = scene->views;
         for (uint32_t i = 0; i < vt.v; ++i) {
-            vt.out[i] = o.rgba[i];
+            vt.out[i] = t.shutter ? static_cast<void*>(c->sub_frames.p + i * wh) : o.rgba[i];
             vt.out_depth[i] = o.depth[i];
             vt.out_normal[i] = o.normal[i];
         }
@@ -854,7 +869,7 @@ static bgs_status render_impl(bgs_context* c, const bgs_cloud* cloud, const bgs_
         TRY(ensure_arena(c, num_tiles));
         TRY(ensure_status(c, c->status_depth, c->status_n, n));
         TRY(ensure_status(c, c->status_pairs, c->status_np, c->cap_pairs));
-        TRY(enqueue_frame(c, cloud, fc, modes, tc, p, o, zd, scene, views ? &vt : nullptr));
+        TRY(enqueue_frame(c, cloud, fc, modes, tc, p, o, zd, scene, views ? &vt : nullptr, t.shutter ? c->sub_frames.p : nullptr));
         if (st->flags & BGS_FLAG_ASYNC) {
             c->async_pending = true;
             c->have_frame = false;     // hooks need bgs_sync() first
@@ -965,13 +980,17 @@ static bgs_status many_table(bgs_context* c, uint32_t k, SceneFacts* scene) {
 // (bgs_render_entities_aux): every segment also projects its Depth and Normal colours, blended into the depth and normal
 // frames.  t.v = nv > 1 views (bgs_render_views or, with aux targets, bgs_render_views_aux, which have checked nv, the
 // targets and the entities' modes): the k entities seen from each of the nv views (depth: nv buffers, or NULL), segment
-// i k + j entity j from view i, view i's frames into its targets.
+// i k + j entity j from view i, view i's frames into its targets.  A shutter frame (t.shutter, bgs_render_shutter, which has
+// checked the same): view i is sample i, whose segment i k + j takes uniforms[i k + j] (a views frame's views all take
+// uniforms[j]).
 static bgs_status render_entities_impl(bgs_context* c, const char* call, bool with_4d, const bgs_cloud* const* clouds,
                                        const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                        const uint32_t* entity_flags, uint32_t k, const bgs_view* view,
                                        const bgs_settings* frame, const bgs_render_extras* ex, const bgs_scene_depth* depth,
                                        const Targets& t, bool many = false) {
     const uint32_t nv = t.v;
+    // view i's entity j reads unis[i stride + j]; nu sets of uniforms
+    const uint32_t stride = t.shutter ? k : 0u, nu = t.shutter ? nv : 1u;
     // each entity's bounding-box overlay: its own bit, or the frame's flag for every entity
     auto box_of = [&](uint32_t j) {
         return (frame->flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX) != 0 ||
@@ -979,7 +998,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
     };
     // entity j as its single-cloud call: its settings with the frame's sort bits and flags, its num_classes and window
     std::vector<bgs_settings> st(k);
-    std::vector<TemporalConsts> tcs(k);   // (entity j's times, Gaussian4d entities only)
+    std::vector<TemporalConsts> tcs((size_t)nu * k);   // (entity j's times with uniforms i: tcs[i k + j], Gaussian4d entities only)
     auto scene = std::make_shared<SceneFacts>();
     // (many: a refusal names the entity)
     auto checked = [&](bgs_status s, uint32_t j) { return s == BGS_OK || !many ? s : entity_refusal(c, s, call, j); };
@@ -998,11 +1017,12 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
         bgs_settings chk = s;   // (a non-4D entity in Velocity is undrawn, and checked as a Color one)
         if (!is4 && chk.rasterize_mode == BGS_RASTERIZE_VELOCITY) chk.rasterize_mode = BGS_RASTERIZE_COLOR;
         for (uint32_t i = 0; i < nv; ++i)   // (as the single-view call of each view)
-            TRY(checked(check_render(c, clouds[j], &view[i], &unis[j], &chk,
+            TRY(checked(check_render(c, clouds[j], &view[i], &unis[i * stride + j], &chk,
                                      ex || e.rasterize_mode == BGS_RASTERIZE_CLASSIFICATION ? &ej : nullptr, t.format, false, is4,
                                      j == 0 && i == 0),
                         j));
-        if (is4) TRY(checked(temporal_consts(c, call, unis[j].time, e.window.time_start, e.window.time_stop, tcs[j]), j));
+        for (uint32_t i = 0; is4 && i < nu; ++i)
+            TRY(checked(temporal_consts(c, call, unis[i * stride + j].time, e.window.time_start, e.window.time_stop, tcs[i * k + j]), j));
         const bgs_entity_settings& e0 = ents[0];
         undrawn = undrawn && !is4 && e.rasterize_mode == BGS_RASTERIZE_VELOCITY && e.gaussian_mode == e0.gaussian_mode &&
                   e.aabb == e0.aabb && e.opacity_adaptive_radius == e0.opacity_adaptive_radius && e.draw_mode == e0.draw_mode &&
@@ -1049,7 +1069,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
             const bgs_cloud* cl = clouds[j];
             const uint32_t rm = st[j].rasterize_mode;
             SceneSeg& sg = segs[sj];
-            sg.fc = frame_consts(cl, &view[i], &unis[j], &st[j], t.aux);
+            sg.fc = frame_consts(cl, &view[i], &unis[i * stride + j], &st[j], t.aux);
             sg.fc.n_cloud = (uint32_t)n_view;   // (Depth colouring reads its view's sorted list of n_view entries)
             sg.pos = cl->pos;
             sg.blocks = cl->blocks;
@@ -1062,7 +1082,7 @@ static bgs_status render_entities_impl(bgs_context* c, const char* call, bool wi
             const size_t gi = std::find(scene->groups.begin(), scene->groups.end(), sg.group) - scene->groups.begin();
             if (gi == scene->groups.size()) { scene->groups.push_back(sg.group); scene->need_sh.push_back(0u); }
             if (sh) scene->need_sh[gi] = 1u;
-            times[sj] = tcs[j];
+            times[sj] = tcs[(size_t)(stride ? i : 0u) * k + j];
             classes[sj] = ents[j].num_classes;
             offsets[sj] = offset;
             seg_kinds[sj] = (uint32_t)blend_kind(ents[j]) | (box_of(j) ? BOX_KIND : 0u);
@@ -1181,7 +1201,8 @@ bgs_status bgs_render_entities_ex(bgs_context* c, const bgs_cloud* const* clouds
 // The refusals of bgs_render_entities_aux, _pick, bgs_render_views and _views_aux (include/bgs.h), in this order, each
 // made by the calls it names: bgs_render_entities_ex's of the list; v and v x k (views calls); the targets; BGS_FLAG_ASYNC
 // (aux and pick calls); each entity's: Gaussian4d, covariance and Velocity (aux calls), Depth (views without aux),
-// OpticalFlow (views calls); blend-over (views calls: device targets only).
+// OpticalFlow (views calls); blend-over (views calls: device targets only).  A shutter call (bgs_render_shutter, t.shutter)
+// makes the views calls' refusals of its v samples, of its one target, and takes blend-over into host targets.
 static bgs_status check_targets_call(bgs_context* c, const char* call, const bgs_cloud* const* clouds,
                                      const bgs_cloud_uniform* unis, const bgs_entity_settings* ents,
                                      const uint32_t* entity_flags, uint32_t k, const bgs_view* view, const bgs_settings* frame,
@@ -1196,7 +1217,7 @@ static bgs_status check_targets_call(bgs_context* c, const char* call, const bgs
         void* const* arrays[3] = {t.rgba, t.depth, t.normal};
         for (int a = 0; a < (t.aux ? 3 : 1); ++a) {
             if (!arrays[a]) return fail(c, BGS_EINVAL, "%s: %s is NULL", call, names[a]);
-            for (uint32_t i = 0; i < t.v; ++i) {
+            for (uint32_t i = 0; i < (t.shutter ? 1u : t.v); ++i) {
                 if (!arrays[a][i]) return fail(c, BGS_EINVAL, "%s: %s[%u] is NULL", call, names[a], i);
                 if (t.device && reinterpret_cast<uintptr_t>(arrays[a][i]) % bpp != 0)
                     return fail(c, BGS_EINVAL, "%s: device target %s[%u] = %p is not aligned to its %zu-byte pixels", call,
@@ -1225,7 +1246,7 @@ static bgs_status check_targets_call(bgs_context* c, const char* call, const bgs
         if (views && rm == BGS_RASTERIZE_OPTICAL_FLOW)
             return fail(c, BGS_EINVAL, "%s: entities[%u] is in OpticalFlow mode", call, j);
     }
-    if (views && (frame->flags & BGS_FLAG_BLEND_OVER_TARGET) && !t.device)
+    if (views && !t.shutter && (frame->flags & BGS_FLAG_BLEND_OVER_TARGET) && !t.device)
         return fail(c, BGS_EINVAL, "%s: BGS_FLAG_BLEND_OVER_TARGET takes device targets", call);
     return BGS_OK;
 }
@@ -1692,6 +1713,28 @@ bgs_status bgs_render_views_aux(bgs_context* c, const bgs_cloud* const* clouds, 
     if (v == 1)
         return bgs_render_entities_aux(c, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, out_rgba[0],
                                        out_depth[0], out_normal[0], out_format, out_is_device_ptr);
+    return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, t);
+}
+
+// The mean of s sub-frames of bgs_render_entities_ex, each with its own view and uniforms, in one frame (include/bgs.h);
+// one sample is bgs_render_entities_ex itself
+bgs_status bgs_render_shutter(bgs_context* c, const bgs_cloud* const* clouds, const bgs_cloud_uniform* unis,
+                              const bgs_entity_settings* ents, const uint32_t* entity_flags, uint32_t k, const bgs_view* views,
+                              uint32_t s, const bgs_settings* frame, const bgs_scene_depth* depths, void* out_rgba,
+                              uint32_t out_format, int out_is_device_ptr) {
+    const char* call = "render_shutter";
+    if (!c) return BGS_EINVAL;
+    Targets t = colour_target(&out_rgba, out_format, out_is_device_ptr);
+    t.v = s;
+    t.shutter = true;
+    TRY(check_targets_call(c, call, clouds, unis, ents, entity_flags, k, views, frame, t, true, false));
+    for (uint32_t i = 1; i < s; ++i)
+        if ((int)views[i].viewport[2] != (int)views[0].viewport[2] || (int)views[i].viewport[3] != (int)views[0].viewport[3])
+            return fail(c, BGS_EINVAL, "%s: views[%u] is %dx%d, views[0] %dx%d: every sample is one frame's size", call, i,
+                        (int)views[i].viewport[2], (int)views[i].viewport[3], (int)views[0].viewport[2], (int)views[0].viewport[3]);
+    if (s == 1)
+        return bgs_render_entities_ex(c, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, out_rgba, out_format,
+                                      out_is_device_ptr);
     return render_entities_impl(c, call, true, clouds, unis, ents, entity_flags, k, views, frame, nullptr, depths, t);
 }
 

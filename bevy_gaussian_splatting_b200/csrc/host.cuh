@@ -172,6 +172,7 @@ struct bgs_context {
     DevBuf<unsigned char> kinds;      // 1 byte per record: the blend kind of a mixed-geometry frame's splats (first use)
     DevBuf<void> frame_aux[2];        // depth / normal frames when an aux frame delivers to host memory (views: every view's)
     DevBuf<uint4> pick_frame;         // the pick frame when bgs_render_entities_pick delivers to host memory
+    DevBuf<float4> sub_frames;        // bgs_render_shutter: each sample's raw (C, T) per pixel, s x W x H (grow-only)
     // scratch sized by the pair capacity (grow-only; cap_pairs pairs)
     uint32_t cap_pairs = 0;
     DevBuf<uint32_t> pkeys[2], pvals[2];

@@ -151,6 +151,7 @@ struct BlendArgs {
     size_t pitch = 0;
     const unsigned char* kinds = nullptr;
     const ViewTable* views = nullptr;
+    bool raw = false;   // (bgs_render_shutter, with views: each view's pixels' raw (C, T) as float4 into its out, no format)
     const PickArgs* pick = nullptr;
     const PickArgsDev* pick_dev = nullptr;   // (bgs_render_entities_pick_many: in place of pick)
 };
@@ -164,6 +165,12 @@ void launch_segment_kinds(const SegmentKinds& kinds, const uint32_t* slot_ids, c
                           uint32_t n_hint, int sm_count, cudaStream_t stream);
 void launch_segment_kinds_many(const SceneTableDev& tab, const uint32_t* slot_ids, const FrameCounters* ctr, unsigned char* out,
                                uint32_t n_hint, int sm_count, cudaStream_t stream);
+// shutter.cu: bgs_render_shutter's resolve.  sub: s sub-frames of wh pixels each, pixel p of sub-frame i at sub[i wh + p],
+// its raw (C, T) as the blend stored it; out: the frame, in `format` (raster.cu's: BGS_FORMAT_* | output mode << 8), pixel p
+// the pixel write of the pairwise mean (include/bgs.h).  Writes nothing when *truncated is set (the frame is rendered again).
+// s in 2 .. MAX_VIEWS.
+void launch_shutter_resolve(const float4* sub, uint32_t s, uint32_t wh, void* out, uint32_t format, const uint32_t* truncated,
+                            cudaStream_t stream);
 // select.cu
 uint32_t select_num_buckets(uint32_t n);
 int select_sort_passes(uint32_t n_buckets);

@@ -19,6 +19,7 @@
 
 #include "common.cuh"
 #include "launch.cuh"
+#include "pixel.cuh"
 
 namespace bgs {
 
@@ -108,65 +109,6 @@ __device__ __forceinline__ void centre_out_tile(int b, int tiles_x, int tiles_y,
     const int k = b / tiles_x, mid = tiles_y / 2;
     tile_x = b - k * tiles_x;
     tile_y = (k & 1) ? mid - (k + 1) / 2 : mid + k / 2;
-}
-
-__device__ __forceinline__ float linear_to_srgb(float c) {
-    c = fminf(fmaxf(c, 0.0f), 1.0f);
-    // __powf = ex2.approx(lg2.approx(c) / 2.4): ~1e-6 relative, far below the 8-bit quantisation step (the full
-    // powf was 7 % of the kernel's instructions)
-    return c <= 0.0031308f ? 12.92f * c : 1.055f * __powf(c, 1.0f / 2.4f) - 0.055f;
-}
-
-// ---- frame output.  `format` = BGS_FORMAT_* | output mode << 8:
-//   mode 0: the splat layer over an opaque black clear (examples/headless.rs:70): (C, 1)
-//   mode 1 (BGS_FLAG_PREMULTIPLIED_OUT): the layer alone, premultiplied: (C, 1 - T)
-//   mode 2 (BGS_FLAG_BLEND_OVER_TARGET): blended over what the target holds, dst = src + (1 - src.a) dst on all four
-//           channels (PREMULTIPLIED_ALPHA_BLENDING, render/mod.rs:944-948): (C + T dst.rgb, (1 - T) + T dst.a)
-constexpr uint32_t OUT_PREMUL = 1u, OUT_OVER = 2u;
-__device__ __forceinline__ float srgb_decode(float c) {
-    return c <= 0.04045f ? c * (1.0f / 12.92f) : __powf((c + 0.055f) * (1.0f / 1.055f), 2.4f);
-}
-__device__ __forceinline__ float4 read_pixel(const void* out, uint32_t fmt, size_t pix) {
-    if (fmt == BGS_FORMAT_RGBA32F) return reinterpret_cast<const float4*>(out)[pix];
-    if (fmt == BGS_FORMAT_RGBA16F) {
-        const uint2 v = reinterpret_cast<const uint2*>(out)[pix];
-        const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v.x)), hi = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-        return make_float4(lo.x, lo.y, hi.x, hi.y);
-    }
-    const uint32_t v = reinterpret_cast<const uint32_t*>(out)[pix];
-    return make_float4(srgb_decode((float)(v & 255u) * (1.0f / 255.0f)), srgb_decode((float)((v >> 8) & 255u) * (1.0f / 255.0f)),
-                       srgb_decode((float)((v >> 16) & 255u) * (1.0f / 255.0f)), (float)(v >> 24) * (1.0f / 255.0f));
-}
-// pixel encoders: RGBA16F, and sRGB8 with a linear alpha byte (or 255 when !with_alpha)
-__device__ __forceinline__ uint2 pack_rgba16f(float r, float g, float b, float a) {
-    const __half2 lo = __floats2half2_rn(r, g), hi = __floats2half2_rn(b, a);
-    return make_uint2(*reinterpret_cast<const uint32_t*>(&lo), *reinterpret_cast<const uint32_t*>(&hi));
-}
-__device__ __forceinline__ uint32_t pack_srgb8(float r, float g, float b, float a, bool with_alpha) {
-    const uint32_t r8 = (uint32_t)(linear_to_srgb(r) * 255.0f + 0.5f);
-    const uint32_t g8 = (uint32_t)(linear_to_srgb(g) * 255.0f + 0.5f);
-    const uint32_t b8 = (uint32_t)(linear_to_srgb(b) * 255.0f + 0.5f);
-    const uint32_t a8 = with_alpha ? (uint32_t)(fminf(fmaxf(a, 0.0f), 1.0f) * 255.0f + 0.5f) : 255u;
-    return r8 | (g8 << 8) | (b8 << 16) | (a8 << 24);
-}
-// one pixel's accumulated premultiplied colour (r, g, b) and remaining transmittance T -> the frame
-__device__ __forceinline__ void write_pixel(void* out, uint32_t format, size_t pix, float r, float g, float b, float T) {
-    const uint32_t fmt = format & 0xFFu, mode = format >> 8;
-    float a = 1.0f;
-    if (mode & OUT_OVER) {
-        const float4 d = read_pixel(out, fmt, pix);
-        r = fmaf(T, d.x, r); g = fmaf(T, d.y, g); b = fmaf(T, d.z, b);
-        a = fmaf(T, d.w, 1.0f - T);
-    } else if (mode & OUT_PREMUL) {
-        a = 1.0f - T;
-    }
-    if (fmt == BGS_FORMAT_RGBA32F) {
-        reinterpret_cast<float4*>(out)[pix] = make_float4(r, g, b, a);
-    } else if (fmt == BGS_FORMAT_RGBA16F) {
-        reinterpret_cast<uint2*>(out)[pix] = pack_rgba16f(r, g, b, a);
-    } else {
-        reinterpret_cast<uint32_t*>(out)[pix] = pack_srgb8(r, g, b, a, mode != 0);
-    }
 }
 
 // shared-memory layout (byte offsets from one base so the hot loop needs a single address register)
@@ -270,7 +212,11 @@ __device__ __forceinline__ uint32_t compact_candidates(uint32_t cnt, unsigned sh
 // weight w = a T of the pairs it blends (an overlay edge pair: w = T) and that pair's record; a later pair replaces it only
 // when its w is strictly larger.  Every pixel of pk->out is written: (entity, index, w, d) of that pair, or BGS_PICK_NONE
 // where nothing blends.  Pick frames take the generic loop in every mode, never the inline-asm one.
-template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false, bool PICK = false, class Pick = PickArgs>
+// RAW (raster_kernel's SubFrames variants, bgs_render_shutter; with VIEWS): each pixel stores its raw blended state
+// (C, T) as a float4 into its view's out, before any output mode, and an empty tile stores (0, 0, 0, 1); format is not
+// read.  The resolve (shutter.cu) encodes the frame from those states.
+template <int MODE, bool AUX, bool ZTEST, bool BOX = false, bool VIEWS = false, bool PICK = false, class Pick = PickArgs,
+          bool RAW = false>
 __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, const float4* __restrict__ extra,
                                             const uint32_t* __restrict__ tile_entries, const uint2* __restrict__ ranges, int W,
                                             int H, int tiles_x, void* __restrict__ out, uint32_t format,
@@ -326,7 +272,8 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
     if (range.x >= range.y) {            // empty tile: nothing to stage (uniform across the CTA)
         // (blend-over mode leaves the target's pixels as they are)
         if (PICK && inside) pk->out[(size_t)py * W + px] = make_uint4(BGS_PICK_NONE, BGS_PICK_NONE, 0u, 0u);
-        if (inside && !((format >> 8) & OUT_OVER)) {
+        if (RAW && inside) reinterpret_cast<float4*>(out)[(size_t)py * W + px] = make_float4(0.f, 0.f, 0.f, 1.0f);
+        if (!RAW && inside && !((format >> 8) & OUT_OVER)) {
             write_pixel(out, format, (size_t)py * W + px, 0.f, 0.f, 0.f, 1.0f);
             if (AUX) {
                 write_pixel(out_depth, format, (size_t)py * W + px, 0.f, 0.f, 0.f, 1.0f);
@@ -560,7 +507,8 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
     }
     ps.finish();
     if (!inside) return;
-    write_pixel(out, format, (size_t)py * W + px, cr, cg, cb, T);
+    if (RAW) reinterpret_cast<float4*>(out)[(size_t)py * W + px] = make_float4(cr, cg, cb, T);
+    else write_pixel(out, format, (size_t)py * W + px, cr, cg, cb, T);
     if constexpr (PICK) {   // record -> global index (compact slot) -> (entity, index within its cloud), and its d
         uint4 rec = make_uint4(BGS_PICK_NONE, BGS_PICK_NONE, 0u, 0u);
         if (best_r != BGS_PICK_NONE) {
@@ -577,11 +525,16 @@ __device__ __forceinline__ void raster_body(const SplatRec* __restrict__ recs, c
 
 // The blend kernels: raster_body of one (MODE, AUX, ZTEST, BOX) and one frame kind, picked by the trailing parameter's type
 // Tail: OneView (a single-view frame), ViewTable (a views frame: raster_body's VIEWS) or PickArgs / PickArgsDev (a pick
-// frame: its PICK, the segments a kernel parameter or bgs_render_entities_many's device table).
+// frame: its PICK, the segments a kernel parameter or bgs_render_entities_many's device table), or SubFrames (a shutter
+// frame's sub-frames: VIEWS and RAW, view i's out its slice of the sub-frame scratch).
 // Every variant takes the same scalar parameters; raster_body sees null for those its variant never reads, so a variant's
 // code does not depend on them.
 struct OneView {};
-template <class Tail> constexpr bool IS_VIEWS = std::is_same<Tail, ViewTable>::value;
+struct SubFrames {
+    ViewTable vt;
+};
+template <class Tail> constexpr bool IS_RAW = std::is_same<Tail, SubFrames>::value;
+template <class Tail> constexpr bool IS_VIEWS = std::is_same<Tail, ViewTable>::value || IS_RAW<Tail>;
 template <class Tail> constexpr bool IS_PICK = std::is_same<Tail, PickArgs>::value || std::is_same<Tail, PickArgsDev>::value;
 
 // Minimum CTAs per SM of each variant: the most that leave it without spills (ptxas report), and for MODE 0 without aux
@@ -607,6 +560,12 @@ __device__ __forceinline__ const T* tail_as(const Tail& tail) {
     if constexpr (std::is_same<T, Tail>::value) return &tail;
     else return nullptr;
 }
+// the view table of a views or shutter frame's tail, else null
+template <class Tail>
+__device__ __forceinline__ const ViewTable* view_table(const Tail& tail) {
+    if constexpr (IS_RAW<Tail>) return &tail.vt;
+    else return tail_as<ViewTable>(tail);
+}
 
 template <int MODE, bool AUX, bool ZTEST, bool BOX, class Tail>
 __global__ void __launch_bounds__(RT_THREADS, raster_min_ctas<MODE, AUX, ZTEST, BOX, Tail>())
@@ -617,11 +576,10 @@ raster_kernel(const SplatRec* __restrict__ recs, const float4* __restrict__ extr
               size_t pitch, const unsigned char* __restrict__ kinds, const __grid_constant__ Tail tail) {
     constexpr bool VIEWS = IS_VIEWS<Tail>;   // (a views frame's size, targets and depth buffers are its view's)
     using Pick = typename std::conditional<std::is_same<Tail, PickArgsDev>::value, PickArgsDev, PickArgs>::type;
-    raster_body<MODE, AUX, ZTEST, BOX, VIEWS, IS_PICK<Tail>, Pick>(
+    raster_body<MODE, AUX, ZTEST, BOX, VIEWS, IS_PICK<Tail>, Pick, IS_RAW<Tail>>(
         recs, extra, tile_entries, ranges, VIEWS ? 0 : W, VIEWS ? 0 : H, VIEWS ? 0 : tiles_x, VIEWS ? nullptr : out, format,
         AUX ? aux : nullptr, AUX && !VIEWS ? out_depth : nullptr, AUX && !VIEWS ? out_normal : nullptr, truncated, splat_d,
-        VIEWS ? nullptr : scene, VIEWS ? 0 : pitch, MODE >= 3 ? kinds : nullptr, tail_as<ViewTable>(tail),
-        tail_as<Pick>(tail));
+        VIEWS ? nullptr : scene, VIEWS ? 0 : pitch, MODE >= 3 ? kinds : nullptr, view_table(tail), tail_as<Pick>(tail));
 }
 
 // the kind of each compact slot r < n_vis: its global index's segment's (overlay frames: kind | overlay << 2)
@@ -832,7 +790,7 @@ raster2_kernel(const SplatRec* __restrict__ recs, const uint32_t* __restrict__ t
     store_pixel2(out, format, (size_t)py * W + px0, in0, in1, r0, g0, b0, r1, g1, b1, T0, T1);
 }
 
-// The blend kernels of one Tail, indexed mode + 5 (box + 2 (ztest + 2 aux)) (pick frames have no aux variants)
+// The blend kernels of one Tail, indexed mode + 5 (box + 2 (ztest + 2 aux)) (pick and shutter frames have no aux variants)
 template <class Tail, int... I>
 const auto* blend_kernels(std::integer_sequence<int, I...>) {
     static void (*const table[])(const SplatRec*, const float4*, const uint32_t*, const uint2*, int, int, int, void*, uint32_t,
@@ -844,7 +802,7 @@ const auto* blend_kernels(std::integer_sequence<int, I...>) {
 
 template <class Tail>
 void launch_blend(const BlendArgs& a, uint32_t grid, const Tail& tail, cudaStream_t stream) {
-    static const auto* const kernels = blend_kernels<Tail>(std::make_integer_sequence<int, IS_PICK<Tail> ? 20 : 40>());
+    static const auto* const kernels = blend_kernels<Tail>(std::make_integer_sequence<int, IS_PICK<Tail> || IS_RAW<Tail> ? 20 : 40>());
     const int i = a.mode + 5 * ((a.box ? 1 : 0) + 2 * ((a.scene ? 1 : 0) + 2 * (a.aux ? 1 : 0)));
     kernels[i]<<<grid, RT_THREADS, 0, stream>>>(
         a.recs, a.extra, a.tile_entries, a.ranges, a.W, a.H, a.tiles_x, a.out, a.format, a.aux, a.out_depth, a.out_normal,
@@ -852,7 +810,9 @@ void launch_blend(const BlendArgs& a, uint32_t grid, const Tail& tail, cudaStrea
 }
 
 void launch_raster(const BlendArgs& a, cudaStream_t stream) {
-    if (a.views) {
+    if (a.views && a.raw) {
+        launch_blend(a, a.views->tile0[a.views->v], SubFrames{*a.views}, stream);
+    } else if (a.views) {
         launch_blend(a, a.views->tile0[a.views->v], *a.views, stream);
     } else if (a.pick) {
         launch_blend(a, (uint32_t)(a.tiles_x * a.tiles_y), *a.pick, stream);

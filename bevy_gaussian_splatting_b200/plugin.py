@@ -379,6 +379,46 @@ def check_views_aux(entities, views) -> CloudSettings:
     return first
 
 
+# CloudSettings fields a bgs_render_shutter call takes from each sample (into its uniforms); the others are every sample's
+SHUTTER_PER_SAMPLE_FIELDS = frozenset({"time", "global_opacity", "global_scale"})
+
+
+def check_shutter(samples, views) -> CloudSettings:
+    """`samples`: s entity lists [(handle, CloudSettings, transform or None), ...], one per sub-frame of one
+    bgs_render_shutter call, and `views` its s views.  Each sample passes `check_views` as a one-view frame.  Raises
+    ValueError when there are no samples, the views are not one per sample or not all of one size, s x k exceeds
+    abi.BGS_SCENE_MAX_CLOUDS segments, or two samples differ in their entity count, an entity's handle or any settings field
+    but time, global_opacity and global_scale (SHUTTER_PER_SAMPLE_FIELDS; the transform may differ too).  Returns the
+    frame's settings (sample 0's first entity's)."""
+    samples, views = [list(e) for e in samples], list(views)
+    if not samples:
+        raise ValueError("render_shutter: no samples")
+    if len(views) != len(samples):
+        raise ValueError(f"render_shutter: {len(views)} views for {len(samples)} samples: one view per sample")
+    first = check_views(samples[0], views[:1])
+    k = len(samples[0])
+    if len(samples) * k > abi.BGS_SCENE_MAX_CLOUDS:
+        raise ValueError(f"render_shutter: {len(samples)} samples x {k} entities, at most {abi.BGS_SCENE_MAX_CLOUDS} segments")
+    for i, v in enumerate(views):
+        if (v.width, v.height) != (views[0].width, views[0].height):
+            raise ValueError(f"render_shutter: view {i} is {v.width}x{v.height}, view 0 {views[0].width}x{views[0].height}: "
+                             "every sample is one frame's size")
+    for i, ents in enumerate(samples[1:], 1):
+        if len(ents) != k:
+            raise ValueError(f"render_shutter: sample {i} has {len(ents)} entities, sample 0 {k}")
+        for j, ((h0, st0, _), (h, st, _)) in enumerate(zip(samples[0], ents)):
+            if h is not h0:
+                raise ValueError(f"render_shutter: sample {i} entity {j} is another cloud than sample 0's")
+            for f in dataclasses.fields(st0):
+                if f.name in SHUTTER_PER_SAMPLE_FIELDS:
+                    continue
+                a, b = getattr(st0, f.name), getattr(st, f.name)
+                if a != b:
+                    raise ValueError(f"render_shutter: sample {i} entity {j} has {f.name} = {b!r}, sample 0 {a!r}: "
+                                     "only time, global_opacity, global_scale and the transform are per sample")
+    return first
+
+
 def entity_settings(settings: CloudSettings) -> abi.bgs_entity_settings:
     """One entity's bgs_entity_settings."""
     s = settings.to_abi()
@@ -857,6 +897,35 @@ class GaussianSplattingPlugin:
         targets = [(C.c_void_p * n)(*[trio[f].ctypes.data for trio in outs]) for f in range(3)]
         self._check(self._lib.bgs_render_views_aux(self._ctx, clouds, unis, ents, eflags, k, vs, n, s, zds, *targets, code, 0))
         return outs
+
+    def render_shutter(self, samples, views, fmt: str = "rgba32f", scene_depths=None, premultiplied: bool = False,
+                       asynchronous: bool = False, out: np.ndarray | None = None) -> np.ndarray:
+        """A motion-blurred frame (`bgs_render_shutter`): the mean of s sub-frames, sample i being `render_entities` of
+        samples[i] from views[i], averaged before the output encoding.  `samples` is s entity lists
+        [(handle, CloudSettings, transform or None), ...]; handles and settings must agree position by position, except
+        time, global_opacity, global_scale and the transform (`check_shutter`, ValueError before any call): a camera move
+        (`interpolate_view`), moving objects and a Gaussian4d performer at the shutter's times (`shutter_times`).
+        `scene_depths`: None, one depth buffer for every sample, or one per sample.  `asynchronous`: only enqueue the
+        frame; `out` is filled once `sync()` returns.  Returns the (H, W, 4) host frame."""
+        samples, views = [list(e) for e in samples], list(views)
+        first = check_shutter(samples, views)
+        code, dtype, ch = self.FORMATS[fmt]
+        if out is None:
+            out = np.empty((views[0].height, views[0].width, ch), dtype)
+        assert out.dtype == dtype and out.size == views[0].height * views[0].width * ch and out.flags.c_contiguous
+        clouds, _, ents, eflags, k, _, s, _ = self._entities_args(samples[0], first, views[0], None, None, asynchronous,
+                                                                  premultiplied, False)
+        n = len(samples)
+        unis = (abi.bgs_cloud_uniform * (n * k))(*[self.cloud_uniform(st, tr, h.aabb) for ents_i in samples for h, st, tr in ents_i])
+        vs = (abi.bgs_view * n)(*[v.to_abi() for v in views])
+        zds = None
+        if scene_depths is not None:
+            if not isinstance(scene_depths, (list, tuple)):
+                scene_depths = [scene_depths] * n
+            assert len(scene_depths) == n
+            zds = (abi.bgs_scene_depth * n)(*[self._scene_depth(d, v) for d, v in zip(scene_depths, views)])
+        self._check(self._lib.bgs_render_shutter(self._ctx, clouds, unis, ents, eflags, k, vs, n, s, zds, _ptr(out), code, 0))
+        return out
 
     def _entities_args(self, entities, first, view, previous_view, delta_time, asynchronous, premultiplied, blend_over):
         """(clouds, uniforms, entities, entity flags, k, view, frame, extras) of a bgs_render_entities_ex or _aux call."""

@@ -5,6 +5,7 @@
 //            [--dump-cloud file] [--raw file] [--remove-floaters radius]
 //            [--particles N --steps K --dt S [--dump-particles file]] [--interpolate SEED --time T]
 //            [--rasterize classification|optical-flow] [--num-classes K] [--prev-view dx,dy,dz] [--instances N]
+//            [--shutter S]
 // --dump-cloud writes the four f32 planes (n, then pos_vis, sh, rot, scale_opacity) so another host can
 // render the identical cloud; --raw writes the RGBA8 frame bytes.  --remove-floaters selects the sparse gaussians
 // (SparseSelect with that radius), inverts the selection and draws only the rest (DrawMode::Selected), the
@@ -17,6 +18,7 @@
 // GaussianInterpolate { lhs, rhs }); --dump-cloud then writes rhs's four planes after lhs's.
 // --instances N draws the cloud instanced N times on a grid through a resident entity list (bgs_entity_list), the
 // instances then moved by one set_transforms from a row-major host array.
+// --shutter S draws the cloud as one motion-blurred frame of S samples (bgs_render_shutter), sample i moved by 0.25 i in x.
 // --rasterize picks RasterizeMode::Classification (labels: gaussian i gets visibility 2 + i % K, --num-classes K, default
 // 3) or OpticalFlow (the previous frame's camera is the headless camera moved by --prev-view, default 0.05,0,0, at
 // 1/60 s); the previous view's clip_from_world is printed as 16 hex words ("prev_clip: ...").
@@ -41,6 +43,7 @@ int main(int argc, char** argv) {
     long interp_seed = -1; float interp_time = 0.0f;
     std::string rasterize = "color"; uint32_t num_classes = 3; float prev_off[3] = {0.05f, 0.0f, 0.0f};
     uint32_t instances = 0;      // --instances N: the cloud instanced N times on a grid through an entity list
+    uint32_t shutter = 0;        // --shutter S: a motion-blurred frame of S samples
     float depth_plane = -1.0f;   // --depth-plane Z: render depth-tested against a half-frame plane at reverse-Z depth Z
     int pos = 0;
     for (int i = 1; i < argc; ++i) {
@@ -57,6 +60,7 @@ int main(int argc, char** argv) {
         if (a == "--rasterize" && i + 1 < argc) { rasterize = argv[++i]; continue; }
         if (a == "--depth-plane" && i + 1 < argc) { depth_plane = (float)std::atof(argv[++i]); continue; }
         if (a == "--instances" && i + 1 < argc) { instances = (uint32_t)std::strtoul(argv[++i], nullptr, 10); continue; }
+        if (a == "--shutter" && i + 1 < argc) { shutter = (uint32_t)std::strtoul(argv[++i], nullptr, 10); continue; }
         if (a == "--num-classes" && i + 1 < argc) { num_classes = (uint32_t)std::strtoul(argv[++i], nullptr, 10); continue; }
         if (a == "--prev-view" && i + 1 < argc) {
             if (std::sscanf(argv[++i], "%f,%f,%f", &prev_off[0], &prev_off[1], &prev_off[2]) != 3) return 1;
@@ -188,7 +192,20 @@ int main(int argc, char** argv) {
             for (int f = 0; f < 3; ++f) drawn = plugin.render_entity_list(*list, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);
             std::printf("instances: %u through an entity list\n", list->size());
         }
-        for (int f = 0; f < 3 && depth_plane < 0.0f && instances == 0; ++f)
+        if (shutter > 0) {
+            std::vector<std::vector<bgs::GaussianSplattingPlugin::SceneEntity>> samples(shutter);
+            for (uint32_t i = 0; i < shutter; ++i) {
+                bgs::GaussianSplattingPlugin::SceneEntity e;
+                e.cloud = &drawn_cloud;
+                e.settings = settings;
+                e.transform.m[12] = 0.25f * (float)i;
+                samples[i].push_back(e);
+            }
+            const std::vector<bgs_view> views(shutter, view);
+            for (int f = 0; f < 3; ++f) drawn = plugin.render_shutter(samples, views, frame.data(), BGS_FORMAT_RGBA8_SRGB);
+            std::printf("shutter: %u samples\n", shutter);
+        }
+        for (int f = 0; f < 3 && depth_plane < 0.0f && instances == 0 && shutter == 0; ++f)
             drawn = settings.rasterize_mode == bgs::RasterizeMode::OpticalFlow
                         ? plugin.render_view(drawn_cloud, settings, view, prev_view, 1.0f / 60.0f, frame.data(), BGS_FORMAT_RGBA8_SRGB)
                         : plugin.render_view(drawn_cloud, settings, view, frame.data(), BGS_FORMAT_RGBA8_SRGB);

@@ -1119,6 +1119,45 @@ bgs_status bgs_render_views_aux(bgs_context* ctx, const bgs_cloud* const* clouds
                                 void* const* out_depth /* v */, void* const* out_normal /* v */,
                                 uint32_t out_format, int out_is_device_ptr);
 
+/* A motion-blurred frame in ONE pass: the box-filtered mean of s sub-frames of one scene, each with its own camera, entity
+ * transforms and Gaussian4d times -- a shutter interval of a video export, a fast camera move, an instanced object or a
+ * gizmo drag in motion, or synthetic blurred frames for training deblurring models.  The s sub-frames share one key-gen,
+ * depth sort, projection, binning, tile-id sort and blend launch (bgs_render_views' machinery, sample i as view i), and one
+ * resolve launch averages them before any output encoding, so the mean is of linear premultiplied values, not of encoded
+ * pixels.
+ *
+ * The rule, exactly:
+ *   Sample i.  Sample i is the blended state -- C_i, the premultiplied rgb, and T_i, the transmittance -- that
+ *     bgs_render_entities_ex(clouds, &uniforms[i k], entities, entity_flags, k, &views[i], frame, NULL,
+ *     depths ? &depths[i] : NULL, ...) passes to its pixel write.  Everything a bgs_cloud_uniform carries may differ
+ *     between samples: the transform (object motion), time (a Gaussian4d entity is conditioned at uniforms[i k + j].time in
+ *     its own window), global opacity and scale.  The clouds, entities' settings and entity flags are every sample's.
+ *   The mean.  C = sum(0, s) / s and T = sum(0, s) / s of the samples' C_i and T_i, in f32 with IEEE round-to-nearest
+ *     division, where sum(a, b) is x_a when b - a == 1 and otherwise sum(a, m) + sum(m, b), m = a + (b - a + 1) / 2 in
+ *     integer division.  (This fixed pairwise order makes the mean of 2^m equal samples that sample exactly; s = 3 is
+ *     ((x0 + x1) + x2) / 3.)
+ *   The output.  out_rgba is one frame of the views' common size: the pixel write of (C, T), as bgs_render_entities_ex
+ *     writes a pixel -- in all three formats, opaque or with BGS_FLAG_PREMULTIPLIED_OUT, and with
+ *     BGS_FLAG_BLEND_OVER_TARGET the averaged layer over the target, once.  Host and device targets follow
+ *     bgs_render_entities_ex's rules for one frame (host targets: blend-over is over the context's last frame).
+ *   s == 1.  The call is bgs_render_entities_ex: pixels, hooks, stats and launch count.
+ *   s >= 2.  Index space, the stable sort, tiles, one round (BGS_FLAG_CHUNKS ignored), hooks and stats, BGS_FLAG_ASYNC and
+ *     the pair-overflow re-render are bgs_render_views', with sample i as view i: segment i k + j is entity j with
+ *     uniforms[i k + j] seen from views[i], and sample i's global indices are [i n, (i + 1) n).  The sub-frames live in a
+ *     grow-only context scratch of s w h 16 bytes.
+ * Launches: those of the bgs_render_views frame of the same entities, plus one (the resolve), whatever s is.
+ * Refused with BGS_EINVAL, nothing enqueued or written and the previous frame's debug hooks kept: s == 0,
+ *   s k > BGS_SCENE_MAX_CLOUDS or N = s n >= 2^30; views of different widths or heights; every refusal bgs_render_views
+ *   makes, with each sample's own uniforms (an entity in Depth or OpticalFlow mode, a non-finite time of a Gaussian4d
+ *   entity in any sample, ...); a NULL out_rgba or a device target not aligned to its pixel.  NULL clouds, uniforms,
+ *   entities, views or frame -> BGS_NOT_READY. */
+bgs_status bgs_render_shutter(bgs_context* ctx, const bgs_cloud* const* clouds,
+                              const bgs_cloud_uniform* uniforms /* s * k: sample i's entity j at i * k + j */,
+                              const bgs_entity_settings* entities /* k */, const uint32_t* entity_flags /* k, or NULL */,
+                              uint32_t k, const bgs_view* views /* s, all of one width and height */, uint32_t s,
+                              const bgs_settings* frame, const bgs_scene_depth* depths /* s, or NULL */, void* out_rgba,
+                              uint32_t out_format, int out_is_device_ptr);
+
 /* Wait for every frame enqueued with BGS_FLAG_ASYNC.  BGS_OK: the last frame is complete and valid.
  * BGS_NOT_READY: a frame's (splat, tile) pair list outgrew its buffer (scene/camera changed a
  * lot); the buffer has been grown -- render that frame again.  An overflowed frame leaves its target

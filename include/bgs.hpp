@@ -514,6 +514,37 @@ public:
                                         out_normal.data(), format, out_is_device ? 1 : 0);
         });
     }
+    // A motion-blurred frame (bgs_render_shutter): out_rgba receives the mean of samples.size() sub-frames, sample i being
+    // render_entities of samples[i] from views[i] (all of one size), averaged before the output encoding.  The samples
+    // list the same clouds with the same settings, entity by entity; their transforms and settings.time, global_opacity
+    // and global_scale may differ (a sample that differs otherwise: BGS_EINVAL).  depths: one buffer for every sample
+    // (pitches[0] its row pitch), one per sample, or empty.  The other arguments are render_views'.
+    bool render_shutter(const std::vector<std::vector<SceneEntity>>& samples, const std::vector<bgs_view>& views, void* out_rgba,
+                        uint32_t format = BGS_FORMAT_RGBA8_SRGB, const std::vector<const float*>& depths = {},
+                        const std::vector<uint64_t>& pitches = {}, bool out_is_device = false, uint32_t extra_flags = 0) {
+        if (samples.empty() || samples[0].empty() || samples.size() != views.size()) check(BGS_EINVAL);
+        if (!depths.empty() && (pitches.size() != depths.size() || (depths.size() != 1 && depths.size() != views.size())))
+            check(BGS_EINVAL);
+        EntityArrays a = entity_arrays(samples[0]);   // (a.unis: sample i's k uniforms at i k)
+        for (size_t i = 1; i < samples.size(); ++i) {
+            const EntityArrays b = entity_arrays(samples[i]);
+            if (b.clouds != a.clouds || b.eflags != a.eflags ||
+                std::memcmp(b.ents.data(), a.ents.data(), a.ents.size() * sizeof(bgs_entity_settings)) != 0)
+                check(BGS_EINVAL);
+            a.unis.insert(a.unis.end(), b.unis.begin(), b.unis.end());
+        }
+        std::vector<bgs_scene_depth> zd;
+        for (size_t i = 0; !depths.empty() && i < views.size(); ++i)
+            zd.push_back({depths[depths.size() == 1 ? 0 : i], pitches[depths.size() == 1 ? 0 : i]});
+        bgs_settings s = samples[0][0].settings.to_abi(extra_flags);
+        if (!(extra_flags & BGS_FLAG_VISUALIZE_BOUNDING_BOX)) s.flags &= ~(uint32_t)BGS_FLAG_VISUALIZE_BOUNDING_BOX;   // (per entity)
+        const bgs_status st = bgs_render_shutter(ctx_, a.clouds.data(), a.unis.data(), a.ents.data(), a.eflags.data(),
+                                                 (uint32_t)a.clouds.size(), views.data(), (uint32_t)views.size(), &s,
+                                                 zd.empty() ? nullptr : zd.data(), out_rgba, format, out_is_device ? 1 : 0);
+        if (st == BGS_NOT_READY) return false;
+        check(st);
+        return true;
+    }
     // Colour + depth + normal frames of one view in one pass (BASELINE.json config 4; bgs_render_aux).
     bool render_view_aux(const PlanarGaussian3dHandle& cloud, const CloudSettings& settings, const bgs_view& view, void* out_rgba,
                          void* out_depth, void* out_normal, uint32_t format = BGS_FORMAT_RGBA8_SRGB, bool out_is_device = false) {
